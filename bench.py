@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """bench.py -- headline benchmark of the query -> top-k hot path (BASELINE.json metric):
 
-    queries/sec @ top-k=100 on a 100M x 768 IVF-PQ index (nlist=16384, M=64, nbits=8, nprobe=32), 1/2/4/8 B200,
-    plus the list-scan kernel's achieved HBM GB/s against the measured peak.
+    queries/sec @ top-k=100 on a 100M x 768 IVF-PQ index (nlist=16384, M=64, nbits=8, nprobe=32), 1/2/4/8 H100,
+    plus the list-scan kernel's achieved HBM GB/s against the HBM peak.
 
 One "step" = one pass of the hot path (coarse scan -> LUT -> ADC list scan -> top-k [-> all-gather + merge])
 over one batch of `--nq` synthetic queries.  `value` = queries/s with the queries already resident in HBM;
@@ -85,11 +85,13 @@ def parse():
     ap.add_argument("--partition", default="list", choices=["list", "vector"],
                     help="static datastore partition across GPUs: whole inverted lists per GPU, or 1/G of every list")
     ap.add_argument("--cpu-seconds", type=float, default=15.0, help="CPU-baseline time budget")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the result of the last timed step (ids.npy as float64, scores.npy as float32) to DIR")
     return ap.parse_args()
 
 
 # ----------------------------------------------------------------------------------------------------------
-# clocks sampling (B200_PROFILING.md recipe)
+# clocks sampling
 # ----------------------------------------------------------------------------------------------------------
 class ClockSampler:
     FIELDS = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
@@ -411,13 +413,15 @@ def encoder_bench(args, device, steps=3, warmup=2):
         out[f"batch_{bs}"] = {"queries": args.nq, "tokens": total_tokens, "ms": ms, "queries_per_s": args.nq / ms * 1e3,
                               "gemm_tflops": flops / ms / 1e9, "launches": model.launches * len(batches), "clocks": clocks}
     peaks = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    sustained = 1469.3
+    sustained, source = 989.0, "H100 SXM data sheet, dense fp16 at 700 W (not measured)"
     if os.path.exists(peaks):
         sustained = json.load(open(peaks)).get("bf16_tflops_sustained", sustained)
+        source = "measured (MEASURED_PEAKS.json bf16_tflops_sustained)"
     for v in out.values():
-        v["frac_of_measured_bf16_sustained"] = v["gemm_tflops"] / sustained
+        v["frac_of_peak"] = v["gemm_tflops"] / sustained
     out["peak_tflops"] = sustained
-    out["note"] = ("fp16 tcgen05 GEMMs (72 per forward), un-padded token stream, 169.9 MFLOP/token counted (Linear layers "
+    out["peak_source"] = source
+    out["note"] = ("fp16 wgmma GEMMs (72 per forward), un-padded token stream, 169.9 MFLOP/token counted (Linear layers "
                    "only), seeded random-init BERT-base weights, token counts of examples/nq_open.jsonl")
     return out
 
@@ -629,7 +633,7 @@ def measured_peak_gbs():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback: H100 SXM data sheet 3.35 TB/s (not measured)"
 
 
 def scan_source_hash() -> str:
@@ -656,6 +660,31 @@ def scan_source_hash() -> str:
     return h.hexdigest()[:16]
 
 
+DUMP_MAX_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir: str, I: torch.Tensor, D: torch.Tensor) -> dict:
+    """What a caller of the timed search receives -- ids [nq, k] and scores [nq, k] -- as DIR/ids.npy (float64: exact for
+    every id) and DIR/scores.npy (float32).  Above 64 MB in all, a fixed seeded sample of query rows is written instead,
+    with the row numbers in DIR/rows.npy.  The corpus and the queries are seeded and the index build is deterministic,
+    so two builds run with the same arguments can be compared file by file."""
+    ids, scores = I.cpu().numpy(), D.cpu().numpy()
+    nq, k = ids.shape
+    rows = None
+    per_row = k * (8 + 4)
+    if nq * per_row > DUMP_MAX_BYTES:
+        nsel = max(1, (DUMP_MAX_BYTES - 8 * nq) // per_row)
+        rows = np.sort(np.random.default_rng(0).choice(nq, size=min(nq, nsel), replace=False))
+        ids, scores = ids[rows], scores[rows]
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "ids.npy"), ids.astype(np.float64))
+    np.save(os.path.join(out_dir, "scores.npy"), scores.astype(np.float32))
+    if rows is not None:
+        np.save(os.path.join(out_dir, "rows.npy"), rows.astype(np.float64))
+    return {"dir": out_dir, "files": ["ids.npy", "scores.npy"] + (["rows.npy"] if rows is not None else []),
+            "rows": int(ids.shape[0]), "k": int(k)}
+
+
 def workload_name(args):
     return (f"IVF-PQ nlist={args.nlist} M={args.m} nbits=8 nprobe={args.nprobe}, {args.n}x{args.d} synthetic gmm, "
             f"top-k={args.k}, batch of {args.nq} queries")
@@ -667,7 +696,7 @@ def make_config(args, world):
             "M": args.m, "nbits": 8, "nprobe": args.nprobe, "k": args.k, "nq_per_step": args.nq, "n_gpus": world,
             "sharding": (f"datastore statically partitioned over {world} GPU(s) by {args.partition}; coarse scan sharded "
                          f"by query; per-shard top-k combined over NVLink"),
-            "l2": "index (>= 6.4 GB of PQ codes at 100M) is far larger than the 126 MB L2; every step re-reads it"}
+            "l2": "index (>= 6.4 GB of PQ codes at 100M) is far larger than the 50 MB L2; every step re-reads it"}
 
 
 # ----------------------------------------------------------------------------------------------------------
@@ -725,8 +754,8 @@ def main():
     run_env = {}
     if world > 1:
         t_init = time.time()
-        # NVLS (in-switch multicast) set-up took ~140 s at 8 ranks on this pool and buys nothing for the few-MB
-        # gathers of this path; communicator creation takes ~4 s without it.  Override with NCCL_NVLS_ENABLE=1.
+        # NVLS (in-switch multicast) set-up is slow and buys nothing for the few-MB gathers of this path.  Override
+        # with NCCL_NVLS_ENABLE=1.
         os.environ.setdefault("NCCL_NVLS_ENABLE", "0")
         run_env["NCCL_NVLS_ENABLE"] = os.environ["NCCL_NVLS_ENABLE"]
         torch.distributed.init_process_group("nccl", device_id=device)
@@ -796,6 +825,7 @@ def main():
                    }[searcher.gather_mode]
     prof = {kk: vv / args.steps for kk, vv in prof_acc.items()}
     I_keep, D_keep = I.clone(), D.clone()        # result of the last timed step: what the parity block checks
+    dumped = dump_outputs(args.dump_outputs, I_keep, D_keep) if (args.dump_outputs and rank == 0) else None
 
     # ---- end-to-end arm: pinned host queries in, host (ids, scores) out, copies inside the timed region
     sliced = world > 1 and args.e2e_transfer == "sliced"
@@ -876,9 +906,9 @@ def main():
                 "unit": "GB/s", "frac": (scan_gbs / peak) if scan_gbs else None, "traffic": None,
                 "peak_source": peak_src, "bytes_per_launch": prof.get("scan_bytes"),
                 "ms_per_launch": prof.get("scan_ms"),
-                "note": "algorithmic pair-bytes (sum over probed (query, list) pairs of len x M) against the measured HBM "
-                        "peak; batched queries share lists through L2, so DRAM traffic is lower, and ncu shows the "
-                        "kernel's binding resource is the L1/shared-memory data pipe, see profiles/"}
+                "note": "algorithmic pair-bytes (sum over probed (query, list) pairs of len x M) against the HBM peak "
+                        "(peak_source); batched queries share lists through L2, so DRAM traffic is lower; every code byte costs "
+                        "one shared-memory table look-up (DESIGN.md section 4.1)"}
     # DRAM traffic of the scan kernel comes from an `ncu --set full` capture of this exact configuration AND this
     # exact kernel source (a number printed under the profiler is never a bench value, so it is read from the
     # committed summary, not measured here; a summary of another kernel version is refused)
@@ -984,7 +1014,9 @@ def main():
                                                 else "2 NCCL all_gather_into_tensor")} if world > 1 else None),
                "build": build_info,
                "run_env": {**run_env, "torch_allow_tf32": bool(torch.backends.cuda.matmul.allow_tf32),
-                           "build_gemms": "librsb (3xTF32 tcgen05 + exact fp32 re-score); no cuBLAS in build or search"}}
+                           "build_gemms": "librsb (3xTF32 wgmma + exact fp32 re-score); no cuBLAS in build or search"}}
+        if dumped is not None:
+            out["dumped_outputs"] = dumped
         if ranks_out is not None:
             out["per_rank"] = ranks_out
         out.update(extra)

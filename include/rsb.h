@@ -1,5 +1,5 @@
 /*
- * rsb.h -- C-ABI of librsb (retrieval-scaling on B200): the drop-in boundary for the reference's
+ * rsb.h -- C-ABI of librsb (retrieval-scaling on H100): the drop-in boundary for the reference's
  * query -> top-k retrieval path.  Plain C types only: device pointers, sizes and a cudaStream_t passed
  * as void*.  No torch / C++ types cross this boundary.
  *
@@ -180,7 +180,7 @@ int rsb_pq_accumulate(const float* r_dev, int64_t n, int d, int M, const uint8_t
 
 /* ---- options -------------------------------------------------------------------------------------------- */
 enum {
-    RSB_OPT_COARSE_TENSOR = 0 /* 1 (default): coarse quantizer scores by 3xTF32 on tcgen05 tensor cores (fp32-equivalent
+    RSB_OPT_COARSE_TENSOR = 0 /* 1 (default): coarse quantizer scores by 3xTF32 on wgmma tensor cores (fp32-equivalent
                                  accuracy); 0: CUDA-core fp32 FMA tiles */
 };
 int rsb_set_option(rsb_index_t* h, int option, int64_t value);
@@ -202,7 +202,7 @@ int rsb_set_profiling(rsb_index_t* h, int enable);
 /* synchronises the events of the last search; out[RSB_PROF_COUNT] doubles */
 int rsb_get_profile(rsb_index_t* h, double* out, int n);
 
-/* ---- query encoder: BERT-base forward in fp16 on tcgen05 tensor cores ------------------------------------
+/* ---- query encoder: BERT-base forward in fp16 on wgmma tensor cores ------------------------------------
  * Replaces `model(**encoded_batch)` (src/search.py:92) for `Contriever(BertModel)` (contriever/src/contriever.py:
  * 11-55) and plain HF BERT checkpoints with CLS pooling (src/search.py:93-94).  Token streams are un-padded:
  * input_ids / token_type_ids are [T] int32 (padding removed), cu_seqlens [B+1] int32 prefix sums. */

@@ -1,4 +1,4 @@
-"""retrieval_scaling_b200 -- B200-native (sm_100a) implementation of the query -> top-k dense-retrieval hot
+"""retrieval_scaling_b200 -- H100-native (sm_90a) implementation of the query -> top-k dense-retrieval hot
 path of RulinShao/retrieval-scaling: Contriever/BERT query encoding and Flat / IVF-Flat / IVF-PQ
 inner-product search behind the reference's `Indexer(cfg).search(query_embs, k)` surface.
 

@@ -224,7 +224,7 @@ static KnnPlan knn_plan(int nq, int64_t n, int k) {
     chunk = std::min(chunk, n4);
     p.chunk = (int)chunk;
     p.nchunks = (int)std::max<int64_t>(1, (n + chunk - 1) / chunk);
-    int want = (2 * 148 + p.qb - 1) / p.qb;
+    int want = (2 * device_num_sms() + p.qb - 1) / p.qb;
     p.nsplit = std::max(1, std::min(want, std::max(1, p.chunk / 4096)));
     p.items = p.nchunks * p.nsplit;
     size_t o = 0;
@@ -288,7 +288,7 @@ static int knn_ip_device(rsb_index* h, const float* q, int nq, const float* x, i
                     }
                 }
             }
-            if (tc)  // 3xTF32 on tcgen05 (fp32-equivalent accuracy); CUDA-core fp32 tiles otherwise
+            if (tc)  // 3xTF32 on wgmma (fp32-equivalent accuracy); CUDA-core fp32 tiles otherwise
                 on_tensor = launch_gemm_tf32x3(tc->qh, tc->ql, nb, tc->xh + (size_t)c0 * d, tc->xl + (size_t)c0 * d, cols, d,
                                                S, p.chunk, st);
             if (!on_tensor) launch_sgemm_nt(q + (size_t)q0 * d, nb, x + (size_t)c0 * d, cols, d, S, p.chunk, st);
@@ -807,7 +807,7 @@ static int search_impl(rsb_index_t* h, const float* q, int nq, int k, int nprobe
         if (h->prof) CU(cudaEventRecord(h->ev[0], st));
         const FlatPlan fp = flat_plan(h, nq, k);
         if (fp.tensor && h->ntotal > 0) {
-            // tensor-core candidates (k + 8 per query, 3xTF32 on tcgen05), then exact fp32 re-score -> top-k
+            // tensor-core candidates (k + 8 per query, 3xTF32 on wgmma), then exact fp32 re-score -> top-k
             if (ws_bytes < fp.total) return fail(RSB_ERR_OOM, "workspace too small: need %zu bytes, got %zu", fp.total, ws_bytes);
             unsigned char* w = static_cast<unsigned char*>(ws);
             TensorOperands tc;
@@ -873,14 +873,13 @@ static int search_impl(rsb_index_t* h, const float* q, int nq, int k, int nprobe
         const float* cD = reinterpret_cast<const float*>(w + p.off_cD);
         // Large batches visit the lists in id order; when a persistent block only gets a few dozen items (small
         // batches, the full-sweep micro-benchmark) the lists are visited longest-first so that the blocks finish on
-        // short items (measured r01: full sweep +6 %, but 1.4 % slower on the 10k-query batch, hence the threshold).
+        // short items (longest-first helps the full sweep but slows large batches, hence the threshold).
         // RSB_LIST_ORDER_LPT=1 forces longest-first.
         static const bool lpt_env = getenv("RSB_LIST_ORDER_LPT") != nullptr;
         const bool lpt_order = lpt_env || ((long)nb * p.nprobe < 64L * 3 * device_num_sms());
         // Thresholds shared between GPUs: ONE lead pair per query job-wide -- only the GPU that holds the query's rank-0 list
-        // leads it, the others get their first bound for that query over NVLink (see pair_bin).  Fewer cold top-k selections
-        // per GPU: 2 GPUs 821-824 -> 830 k queries/s (end to end 817-822 -> 828 k), 8 GPUs 2.75 -> 2.85 M
-        // (profiles/r02_multi_gpu_runs.txt).  RSB_LOCAL_LEADS=1: a lead pair per query on every GPU (its best-ranked list that is
+        // leads it, the others get their first bound for that query over NVLink (see pair_bin): fewer cold top-k
+        // selections per GPU.  RSB_LOCAL_LEADS=1: a lead pair per query on every GPU (its best-ranked list that is
         // non-empty there), the single-GPU rule.
         static const bool local_leads = getenv("RSB_LOCAL_LEADS") != nullptr;
         const int lead_mode = (shared && shared->local && shared->npeers > 1 && !local_leads) ? 1 : 0;
@@ -959,7 +958,8 @@ extern "C" int rsb_search_preassigned_shared(rsb_index_t* h, const float* q, int
 extern "C" int rsb_kmeans_accumulate(const float* x, int64_t n, int d, const int32_t* assign, int k, float* sums,
                                      float* counts, rsb_stream_t stream) {
     if (!x || !assign || !sums || !counts || n < 0 || d <= 0 || k <= 0) return fail(RSB_ERR_INVALID, "bad argument");
-    launch_kmeans_accumulate(x, n, d, assign, k, sums, counts, (cudaStream_t)stream);
+    const cudaError_t e = launch_kmeans_accumulate(x, n, d, assign, k, sums, counts, (cudaStream_t)stream);
+    if (e != cudaSuccess) return fail(e == cudaErrorMemoryAllocation ? RSB_ERR_OOM : RSB_ERR_CUDA, "%s", cudaGetErrorString(e));
     CHECK_LAUNCH();
     return RSB_OK;
 }
@@ -973,7 +973,8 @@ extern "C" int rsb_pq_assign(const float* r, int64_t n, int d, int M, const floa
 extern "C" int rsb_pq_accumulate(const float* r, int64_t n, int d, int M, const uint8_t* codes, float* sums, float* counts,
                                  rsb_stream_t stream) {
     if (!r || !codes || !sums || !counts || n < 0 || d <= 0 || M <= 0 || d % M) return fail(RSB_ERR_INVALID, "bad argument");
-    launch_pq_accumulate(r, n, d, M, codes, sums, counts, (cudaStream_t)stream);
+    const cudaError_t e = launch_pq_accumulate(r, n, d, M, codes, sums, counts, (cudaStream_t)stream);
+    if (e != cudaSuccess) return fail(e == cudaErrorMemoryAllocation ? RSB_ERR_OOM : RSB_ERR_CUDA, "%s", cudaGetErrorString(e));
     CHECK_LAUNCH();
     return RSB_OK;
 }

@@ -2,11 +2,10 @@
 // called from src/search.py:83-96 with the model in fp16) on variable-length (un-padded) token streams.
 //
 //   embed_ln_kernel      word + position + token-type gather, LayerNorm(eps)                    -> H  [T,768]  f16
-//   gemm_tn_pair_kernel  Y = X . W^T (+bias [+GELU | +residual]) on 5th-gen tensor cores, CTA pairs (tcgen05
-//                        cta_group::2): TMA (cp.async.bulk.tensor, 128B swizzle) -> shared-memory ring -> tcgen05.mma
-//                        kind::f16 (fp32 accumulate in double-buffered TMEM) -> tcgen05.ld epilogue.  One elected
-//                        thread of the leader CTA issues the MMAs; warp-specialised producer / issuer / epilogue roles
-//                        synchronised with mbarriers.  gemm_tn_kernel: 128 x 128 tiles, one per CTA, for N % 256 != 0.
+//   gemm_tn_kernel       Y = X . W^T (+bias [+GELU | +residual]) on the Hopper tensor cores: TMA (cp.async.bulk.tensor,
+//                        128B swizzle) -> shared-memory ring -> wgmma.mma_async f16 (fp32 accumulate in registers) ->
+//                        epilogue from the registers.  Warp-specialised producer / consumer warpgroups synchronised
+//                        with mbarriers.
 //   attention_mma32_kernel / attention_flash_kernel   softmax(QK^T / sqrt(64)) V per (sequence, head) on mma.sync:
 //                        one warp per (sequence, head) up to 32 tokens, flash-style blocks of 128 queries beyond
 //                        (collect_long_kernel lists those sequences once per forward)
@@ -32,38 +31,26 @@ namespace {
 using namespace rsbtc;
 
 // ---------------------------------------------------------------------------------------------------------
-// GEMM  C[M,N] = A[M,K] . B[N,K]^T  (A = activations, B = nn.Linear weight: both K-major), f16 in, f32 accumulate.
-// CTA tile 128 x 128, K step 64 (= one 128-byte swizzle row), 3-stage TMA ring (2 CTAs / SM co-resident so one CTA's
-// epilogue overlaps the other's main loop).  192 threads: warp 0 = TMA producer, warp 1 = TMEM owner + MMA issuer,
-// warps 2-5 = epilogue (warp w reads TMEM lanes 32*(w%4)..+31).
+// GEMM  C[M,N] = A[M,K] . B[N,K]^T  (A = activations, B = nn.Linear weight: both K-major), f16 in, f32 accumulate, on
+// the Hopper tensor cores.  CTA tile 128 x 128, K step 64 (= one 128-byte swizzle row), 4-stage ring of TMA loads
+// (cp.async.bulk.tensor, 128B swizzle) signalled through mbarriers.  384 threads: warpgroup 0 = producer (one thread
+// issues the TMA loads), warpgroups 1-2 = consumers: each issues wgmma.m64n128k16 on its 64 rows of the tile and
+// applies the epilogue (+bias [+GELU | +residual]) straight from its accumulator registers.
 // ---------------------------------------------------------------------------------------------------------
-constexpr int G_BM = 128, G_BN = 128, G_BK = 64, G_STAGES = 3, G_THREADS = 192;
-constexpr int G_STAGE_BYTES = (G_BM + G_BN) * G_BK * 2;                 // 32 KB
+constexpr int G_BM = 128, G_BN = 128, G_BK = 64, G_STAGES = 4, G_THREADS = 384;
+constexpr int G_TILE_BYTES = 128 * G_BK * 2;                            // 16 KB
+constexpr int G_STAGE_BYTES = 2 * G_TILE_BYTES;                         // A and B tiles
 constexpr int G_SMEM = G_STAGES * G_STAGE_BYTES + 1024 /*align*/ + 256; // ring + barriers
 
 enum { EPI_BIAS = 0, EPI_BIAS_GELU = 1, EPI_BIAS_RESIDUAL = 2 };
 
-// HF BERT's "gelu": 0.5 x (1 + erf(x / sqrt 2)).  erf by Abramowitz-Stegun 7.1.26 with the hardware reciprocal /
-// exp2: |error| <= 5e-7 absolute -- below fp16 resolution of the output everywhere except the ~1e-6-sized negative
-// tail -- at about half the instructions of CUDA's erff.  The FFN1 epilogue is bound by its instruction issue rate
-// (ncu: 64 % issue-active at 33 % tensor-active with erff, profiles/r02_encoder_epilogue.md).  -DRSB_EXACT_ERF: erff.
-__device__ __forceinline__ float gelu_erf(float x) {
-#ifndef RSB_EXACT_ERF
-    const float z = fabsf(x) * 0.70710678118654752f;
-    const float t = __fdividef(1.f, fmaf(0.3275911f, z, 1.f));
-    float p = fmaf(1.061405429f, t, -1.453152027f);
-    p = fmaf(p, t, 1.421413741f);
-    p = fmaf(p, t, -0.284496736f);
-    p = fmaf(p, t, 0.254829592f);
-    const float e = 1.f - p * t * __expf(-z * z);
-    return 0.5f * x * (1.f + copysignf(e, x));
-#else
-    return 0.5f * x * (1.f + erff(x * 0.70710678118654752f));
+#ifdef RSB_EXACT_ERF
+// HF BERT's "gelu" with CUDA's erff (-DRSB_EXACT_ERF; the default is the restatement gelu_erf_pair below)
+__device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
 #endif
-}
 
-// sm_100's packed fp32 pair instructions (FFMA2 / FMUL2 / FADD2: one issue slot per two lanes of work), used by the
-// GELU / bias epilogue of the pair GEMM below.
+// fp32 pairs packed in 64-bit registers.  Hopper has no packed fp32 arithmetic: each pair operation is two scalar
+// round-to-nearest operations (never contracted), the same rounding as a packed instruction.
 __device__ __forceinline__ unsigned long long f2pack(float lo, float hi) {
     unsigned long long r;
     asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
@@ -73,176 +60,21 @@ __device__ __forceinline__ void f2unpack(unsigned long long v, float& lo, float&
     asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
 __device__ __forceinline__ unsigned long long f2fma(unsigned long long a, unsigned long long b, unsigned long long c) {
-    unsigned long long d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-    return d;
+    float a0, a1, b0, b1, c0, c1;
+    f2unpack(a, a0, a1); f2unpack(b, b0, b1); f2unpack(c, c0, c1);
+    return f2pack(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 __device__ __forceinline__ unsigned long long f2mul(unsigned long long a, unsigned long long b) {
-    unsigned long long d;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    return d;
-}
-template <int EPI>
-__global__ __launch_bounds__(G_THREADS)
-void gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                    __half* __restrict__ C, const __half* __restrict__ bias, const __half* __restrict__ residual,
-                    int M, int N, int K) {
-    extern __shared__ unsigned char smem_dyn[];
-    // 1024-byte alignment required by the 128B swizzle atom
-    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + G_STAGES * G_STAGE_BYTES);
-    uint64_t* empty = full + G_STAGES;
-    uint64_t* tmem_full = empty + G_STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full + 1);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int m0 = blockIdx.y * G_BM, n0 = blockIdx.x * G_BN;
-    const int nk = K / G_BK;
-
-    if (threadIdx.x == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmB)) : "memory");
-        for (int s = 0; s < G_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        mbar_init(tmem_full, 1);
-        fence_barrier_init();
-    }
-    if (warp == 1) tmem_alloc(tmem_slot, G_BN);   // 128 fp32 accumulator columns
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        if (lane == 0) {
-            for (int kb = 0; kb < nk; ++kb) {
-                const int s = kb % G_STAGES;
-                if (kb >= G_STAGES) mbar_wait(&empty[s], ((kb / G_STAGES) - 1) & 1);
-                unsigned char* a_dst = smem + s * G_STAGE_BYTES;
-                unsigned char* b_dst = a_dst + G_BM * G_BK * 2;
-                mbar_expect_tx(&full[s], G_STAGE_BYTES);
-                tma_load_2d(a_dst, &tmA, &full[s], kb * G_BK, m0);
-                tma_load_2d(b_dst, &tmB, &full[s], kb * G_BK, n0);
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // InstrDescriptor: c_format F32 (1<<4) | a,b F16 (0) | K-major both | N>>3 at [17,23) | M>>4 at [24,29)
-            const uint32_t idesc = (1u << 4) | ((uint32_t)(G_BN >> 3) << 17) | ((uint32_t)(G_BM >> 4) << 24);
-            for (int kb = 0; kb < nk; ++kb) {
-                const int s = kb % G_STAGES;
-                mbar_wait(&full[s], (kb / G_STAGES) & 1);
-                tc_fence_after();
-                const uint32_t a_addr = smem_u32(smem + s * G_STAGE_BYTES);
-                const uint32_t b_addr = a_addr + G_BM * G_BK * 2;
-                const uint64_t adesc = make_sw128_kmajor_desc(a_addr);
-                const uint64_t bdesc = make_sw128_kmajor_desc(b_addr);
-#pragma unroll
-                for (int k4 = 0; k4 < G_BK / 16; ++k4) {
-                    // advance 16 K-elements = 32 bytes inside the swizzle row: +2 in the (addr >> 4) field
-                    umma_f16(tmem_base, adesc + (uint64_t)(k4 * 2), bdesc + (uint64_t)(k4 * 2), idesc, (kb | k4) ? 1u : 0u);
-                }
-                umma_commit(&empty[s]);                 // frees the smem stage when these MMAs retire
-                if (kb == nk - 1) umma_commit(tmem_full);  // accumulator complete
-            }
-        }
-    } else {
-        // ===== epilogue: TMEM -> registers -> (+bias, GELU | residual) -> f16 -> global
-        const int q = warp & 3;                 // TMEM lane quarter this warp may access
-        const int row = m0 + q * 32 + lane;
-        mbar_wait(tmem_full, 0);
-        tc_fence_after();
-#pragma unroll 1
-        for (int c = 0; c < G_BN; c += 32) {
-            uint32_t r[32];
-            tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c, r);
-            if (row < M) {
-                const int col0 = n0 + c;
-                __half* dst = C + (size_t)row * N + col0;
-                const __half* res = EPI == EPI_BIAS_RESIDUAL ? residual + (size_t)row * N + col0 : nullptr;
-#pragma unroll
-                for (int v = 0; v < 4; ++v) {   // 4 x (8 halves = 16 bytes)
-                    const uint4 bv = *reinterpret_cast<const uint4*>(bias + col0 + v * 8);
-                    const __half2* b2 = reinterpret_cast<const __half2*>(&bv);
-                    uint4 rv = make_uint4(0, 0, 0, 0);
-                    if (EPI == EPI_BIAS_RESIDUAL) rv = *reinterpret_cast<const uint4*>(res + v * 8);
-                    const __half2* r2 = reinterpret_cast<const __half2*>(&rv);
-                    uint4 ov;
-                    __half2* o2 = reinterpret_cast<__half2*>(&ov);
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        float x0 = __uint_as_float(r[v * 8 + e * 2]) + __low2float(b2[e]);
-                        float x1 = __uint_as_float(r[v * 8 + e * 2 + 1]) + __high2float(b2[e]);
-                        if (EPI == EPI_BIAS_GELU) {
-                            x0 = gelu_erf(x0);
-                            x1 = gelu_erf(x1);
-                        }
-                        if (EPI == EPI_BIAS_RESIDUAL) { x0 += __low2float(r2[e]); x1 += __high2float(r2[e]); }
-                        o2[e] = __floats2half2_rn(x0, x1);
-                    }
-                    *reinterpret_cast<uint4*>(dst + v * 8) = ov;
-                }
-            }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, G_BN);
-}
-
-// ---------------------------------------------------------------------------------------------------------
-// Epilogue of the persistent kernels.  After tcgen05.ld every lane holds 32 fp32 accumulators of ONE row; a lane
-// writes them as two 256-bit stores (sm_100 STG.256: whole 32-byte sectors, measured 52.8 -> 46.4 ms per 10k queries
-// against 128-bit stores, profiles/r02_ab_round1_leftovers.txt).  A shared-memory transpose that makes each store
-// instruction cover 8 rows x 64 contiguous bytes was measured SLOWER (51.3 ms, profiles/r02_encoder_epilogue.md): the
-// epilogue is bound by its instruction count and the latency of its loads, not by L2 write transactions.  So the
-// residual of chunk i+1 is requested before chunk i is processed (its ~1 us L2 round trip used to sit in front of every
-// chunk of the attention-output GEMM), and the TMEM load of a chunk is issued before those requests and waited on after.
-// ---------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void ldg256(uint32_t (&v)[8], const void* p) {
-    asm volatile("ld.global.v8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-                 : "l"(p));
-}
-__device__ __forceinline__ void stg256(void* p, const uint32_t (&v)[8]) {
-    asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "r"(v[0]), "r"(v[1]), "r"(v[2]),
-                 "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_ld32_issue(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ---------------------------------------------------------------------------------------------------------
-// Epilogue of the pair GEMM (the first form -- residual prefetched one chunk ahead, fp16 bias, GELU with copysign -- and a
-// 16-warp variant were measured against it and removed: profiles/r02_encoder_epilogue.md):
-//  * the whole residual row segment of a warp (its 64 or 128 columns) is requested BEFORE the warp waits for the
-//    accumulator, so the L2 round trip overlaps the tile's MMA phase instead of the first chunks of the epilogue;
-//  * tcgen05.ld of chunk i+1 is in flight while chunk i is processed (two register buffers);
-//  * the accumulator stage is handed back to the MMA warp as soon as the last tcgen05.ld has landed, before the last
-//    chunk is processed and stored;
-//  * bias as fp32 in shared memory, added with packed pair adds; residual added in half precision after rounding the
-//    dense output to half, which is also the order of HF BertSelfOutput / BertOutput (dense -> fp16, then + input);
-//  * GELU restated as relu(x) + 0.5|x| (erf(|x|/sqrt 2) - 1): one packed multiply-add onto max(x, 0) instead of
-//    1 - p, copysign and 0.5 x (1 + e); with z' = |x| sqrt(log2(e)/2) the exponent is just -z'^2 (negation folded into
-//    the MUFU operand) and every scale factor is folded into the polynomial's coefficients: 16 instead of 18
-//    instructions per pair, and no cancellation for x < 0 (numpy restatement: max 1 fp16 ulp from the fp64 erf form).
-// ---------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ unsigned long long f2add(unsigned long long a, unsigned long long b) {
-    unsigned long long d;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    return d;
+    float a0, a1, b0, b1;
+    f2unpack(a, a0, a1); f2unpack(b, b0, b1);
+    return f2pack(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 __device__ __forceinline__ unsigned long long f2splat(float v) { return f2pack(v, v); }
 
+// GELU restated as relu(x) + 0.5|x| (erf(|x|/sqrt 2) - 1): one multiply-add onto max(x, 0) instead of 1 - p, copysign
+// and 0.5 x (1 + e); with z' = |x| sqrt(log2(e)/2) the exponent is just -z'^2 (negation folded into the MUFU operand)
+// and every scale factor is folded into the polynomial's coefficients, with no cancellation for x < 0 (numpy
+// restatement: max 1 fp16 ulp from the fp64 erf form, tests/test_gelu_restatement.py).
 __device__ __forceinline__ unsigned long long gelu_erf_pair(unsigned long long X) {
     float x0, x1;
     f2unpack(X, x0, x1);
@@ -271,255 +103,93 @@ __device__ __forceinline__ unsigned long long gelu_erf_pair(unsigned long long X
 #endif
 }
 
-// one row (this lane's) x 32 columns; bias_c: fp32 in shared memory (same address in every lane: broadcast)
 template <int EPI>
-__device__ __forceinline__ void epilogue_store_chunk(const uint32_t (&r)[32], const uint32_t (&rr)[2][8], __half* dst,
-                                                        uint32_t bias_c /* shared-window address */) {
-#pragma unroll
-    for (int w = 0; w < 2; ++w) {
-        uint32_t o[8];
-#pragma unroll
-        for (int v = 0; v < 4; ++v) {
-            float4 b;                                     // explicit ld.shared: the generic pointer would compile to LD
-            asm("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(b.x), "=f"(b.y), "=f"(b.z), "=f"(b.w)
-                : "r"(bias_c + (uint32_t)((w * 16 + v * 4) * 4)));
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-                const int j = w * 16 + v * 4 + e * 2;
-                unsigned long long X = f2add(f2pack(__uint_as_float(r[j]), __uint_as_float(r[j + 1])),
-                                             e ? f2pack(b.z, b.w) : f2pack(b.x, b.y));
-                if (EPI == EPI_BIAS_GELU) X = gelu_erf_pair(X);
-                float x0, x1;
-                f2unpack(X, x0, x1);
-                __half2 h = __floats2half2_rn(x0, x1);
-                if (EPI == EPI_BIAS_RESIDUAL) h = __hadd2(h, *reinterpret_cast<const __half2*>(&rr[w][v * 2 + e]));
-                o[v * 2 + e] = *reinterpret_cast<const uint32_t*>(&h);
-            }
-        }
-        stg256(dst + w * 16, o);
-    }
-}
-
-// all NCH chunks of one tile for this warp.  `release()` hands the accumulator stage back (called by every lane).
-template <int EPI, int NCH, class Release>
-__device__ __forceinline__ void epilogue_tile(uint32_t tmem_row_base, int acc_col0, int c_lo, int row, int M, int N, int n0,
-                                                 __half* __restrict__ C, const float* __restrict__ bias_f,
-                                                 const __half* __restrict__ residual, uint64_t* full_bar, uint32_t parity,
-                                                 Release release) {
-    const bool live = row < M;
-    const __half* res_row = residual + (size_t)(live ? row : 0) * N + n0 + c_lo;
-    __half* dst_row = C + (size_t)(live ? row : 0) * N + n0 + c_lo;
-    const uint32_t bias_sa = smem_u32(bias_f + n0 + c_lo);
-    uint32_t rr[NCH][2][8];
-    if (EPI == EPI_BIAS_RESIDUAL && live) {
-#pragma unroll
-        for (int i = 0; i < NCH; ++i) { ldg256(rr[i][0], res_row + i * 32); ldg256(rr[i][1], res_row + i * 32 + 16); }
-    }
-    mbar_wait(full_bar, parity);
-    tc_fence_after();
-    uint32_t r[2][32];
-    tmem_ld32_issue(tmem_row_base + (uint32_t)(acc_col0 + c_lo), r[0]);
-    tmem_ld_wait();
-#pragma unroll
-    for (int j = 0; j < 32; ++j) asm volatile("" : "+r"(r[0][j]));
-#pragma unroll
-    for (int i = 0; i < NCH; ++i) {
-        if (i + 1 < NCH) tmem_ld32_issue(tmem_row_base + (uint32_t)(acc_col0 + c_lo + (i + 1) * 32), r[(i + 1) & 1]);
-        else release();                                   // every tcgen05.ld of this warp has completed
-        if (live) epilogue_store_chunk<EPI>(r[i & 1], rr[i], dst_row + i * 32, bias_sa + (uint32_t)(i * 32 * 4));
-        if (i + 1 < NCH) {
-            tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 32; ++j) asm volatile("" : "+r"(r[(i + 1) & 1][j]));
-        }
-    }
-}
-
-// ---------------------------------------------------------------------------------------------------------
-// Tile constants of the pair GEMM below.  (Round 2 also had a "v2": one CTA per 128 x 256 tile, persistent, double-buffered
-// TMEM -- 62-64 % of the MMA rate at best because an SM then receives 48 KB of operands per k-block; removed in favour of
-// the pair kernel, measurements in profiles/r02_encoder_epilogue.md.)
-// ---------------------------------------------------------------------------------------------------------
-constexpr int H_BM = 128, H_BN = 256, H_BK = 64;
-constexpr int H_EPI_WARPS = 8;                       // 2 warps per TMEM lane quarter, 128 accumulator columns each
-constexpr int H_THREADS = 64 + 32 * H_EPI_WARPS;     // warp 0 TMA, warp 1 MMA, warps 2.. epilogue
-constexpr int H_BIAS_MAX = 4096;                     // bias vector staged in shared memory as fp32 (N <= 4096)
-
-// ---------------------------------------------------------------------------------------------------------
-// cluster helpers (pair GEMM below).  Round 2 also measured a "v3": v2 plus 2-CTA clusters whose CTAs each fetched half
-// of the shared weight tile and multicast it (tcgen05 cta_group::1): +-1 % (profiles/r02_ab_round1_leftovers.txt,
-// r02_encoder_epilogue.md) -- multicast does not reduce what each SM receives -- and was removed in favour of the pair kernel.
-// ---------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ uint32_t cluster_id_x() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ uint32_t num_clusters_x() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%nclusterid.x;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
-// ---------------------------------------------------------------------------------------------------------
-// Pair GEMM: CTA PAIRS (tcgen05 cta_group::2).  Why: the single-CTA 128x256 kernel pulls 48 KB of operands into its SM per
-// 512-cycle k-block = 96 B/clk, the SM's L2 port delivers ~64 B/clk, and the K = 768 / K = 3072 GEMMs sat at 62-64 % of
-// the MMA rate whatever the epilogue did (profiles/r02_encoder_epilogue.md); multicasting the weight tile (v3) does not
-// change what each SM has to RECEIVE, which is why it measured +-1 %.  A pair of CTAs computes one 256 x 256 tile with
-// 2-SM MMAs: each CTA stages only its 128 activation rows and HALF of the weight tile (32 KB per k-block = 64 B/clk), the
-// tensor cores of both SMs read the two halves of B from both shared memories, and each CTA ends up with its 128 x 256
-// accumulator in its own TMEM.  The leader CTA (cluster rank 0) issues every MMA; both CTAs' TMA loads signal the
-// leader's "full" barrier (2CTA form, peer bit of the barrier address cleared), the leader's commits are multicast to
-// both CTAs' "empty" / "accumulator full" barriers, and both CTAs' epilogue warps release the accumulator on the
-// leader's barrier (remote arrive).  6-stage ring of 32 KB.
-// ---------------------------------------------------------------------------------------------------------
-constexpr int P_STAGES = 6;
-constexpr int P_A_BYTES = 128 * H_BK * 2, P_B_BYTES = 128 * H_BK * 2;     // 16 KB + 16 KB
-constexpr int P_STAGE_BYTES = P_A_BYTES + P_B_BYTES;
-constexpr int P_SMEM = P_STAGES * P_STAGE_BYTES + 1024 + 256 + H_BIAS_MAX * 4;    // fp32 bias (second epilogue form)
-
-__device__ __forceinline__ void tma_load_2d_2cta(void* smem_dst, const CUtensorMap* map, uint32_t leader_bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
-            smem_u32(smem_dst)),
-        "l"(reinterpret_cast<uint64_t>(map)), "r"(leader_bar), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ void umma_f16_2cta(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit_2cta(uint64_t* bar, uint16_t cta_mask) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                     smem_u32(bar)),
-                 "h"(cta_mask)
-                 : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* local_bar, uint32_t cta_rank) {
-    uint32_t remote;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(local_bar)), "r"(cta_rank));
-    // default semantics (as CUTLASS' ClusterBarrier::arrive): the ".release.cluster" form compiles to MEMBAR.ALL.GPU +
-    // ERRBAR in front of the arrive, i.e. every epilogue warp waited for its global stores of the tile to drain before it
-    // could hand the accumulator back (ncu: "membar" = 18-24 % of the stall samples of the K = 768 GEMMs).  What the
-    // barrier orders here are tcgen05.ld completions, which tcgen05.wait::ld + tcgen05.fence::before_thread_sync cover.
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
-}
-
-template <int EPI>
-__global__ __cluster_dims__(2, 1, 1) __launch_bounds__(H_THREADS, 1)
-void gemm_tn_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB128,
-                         __half* __restrict__ C, const __half* __restrict__ bias, const __half* __restrict__ residual,
-                         int M, int N, int K, int m_rev) {
+__global__ __launch_bounds__(G_THREADS, 1)
+void gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                    __half* __restrict__ C, const __half* __restrict__ bias, const __half* __restrict__ residual,
+                    int M, int N, int K, int m_rev) {
     extern __shared__ unsigned char smem_dyn[];
+    // 1024-byte alignment required by the 128B swizzle atom
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + P_STAGES * P_STAGE_BYTES);
-    uint64_t* empty = full + P_STAGES;
-    uint64_t* tmem_full = empty + P_STAGES;      // [2]
-    uint64_t* tmem_empty = tmem_full + 2;        // [2]  (the leader's collects both CTAs' epilogue warps)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + G_STAGES * G_STAGE_BYTES);
+    uint64_t* empty = full + G_STAGES;
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int rank = (int)cluster_ctarank();                 // 0 = leader: rows 0-127 of the pair's tile, columns 0-127 of B
-    const int tiles_n = N / H_BN;
-    const int pairs_m = ((M + H_BM - 1) / H_BM + 1) / 2;
-    const int npairs = pairs_m * tiles_n;
-    const int nk = K / H_BK;
-    const int pair0 = (int)cluster_id_x(), pair_step = (int)num_clusters_x();
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
+    const int tm = m_rev ? (int)(gridDim.y - 1 - blockIdx.y) : (int)blockIdx.y;
+    const int m0 = tm * G_BM, n0 = blockIdx.x * G_BN;
+    const int nk = K / G_BK;
 
     if (threadIdx.x == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmB128)) : "memory");
-        for (int s = 0; s < P_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(&tmem_full[a], 1); mbar_init(&tmem_empty[a], 2 * H_EPI_WARPS); }
+        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmB)) : "memory");
+        for (int s = 0; s < G_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }   // 8 consumer warps
         fence_barrier_init();
     }
-    if (warp == 1) {                                          // one warp of EACH CTA of the pair
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::);
-    }
-    float* bias_f = reinterpret_cast<float*>(smem + P_STAGES * P_STAGE_BYTES + 256);
-    for (int i = threadIdx.x; i < N; i += H_THREADS) bias_f[i] = __half2float(bias[i]);
-    tc_fence_before();
     __syncthreads();
-    cluster_sync_all();                                       // both CTAs' barriers and TMEM exist before anything remote arrives
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
-        if (lane == 0) {
-            int it = 0;
-            for (int pair = pair0; pair < npairs; pair += pair_step) {
-                const int m0 = ((m_rev ? pairs_m - 1 - pair / tiles_n : pair / tiles_n) * 2 + rank) * H_BM, n0 = (pair % tiles_n) * H_BN + rank * 128;
-                for (int kb = 0; kb < nk; ++kb, ++it) {
-                    const int s = it % P_STAGES;
-                    mbar_wait(&empty[s], ((it / P_STAGES) & 1) ^ 1);   // the leader's MMAs have consumed this slot in BOTH CTAs
-                    unsigned char* a_dst = smem + s * P_STAGE_BYTES;
-                    const uint32_t leader_bar = smem_u32(&full[s]) & 0xFEFFFFFFu;   // same offset in the rank-0 CTA
-                    if (rank == 0) mbar_expect_tx(&full[s], 2 * P_STAGE_BYTES);     // this CTA's 32 KB + the peer's 32 KB
-                    tma_load_2d_2cta(a_dst, &tmA, leader_bar, kb * H_BK, m0);      // rows past M are zero-filled by TMA
-                    tma_load_2d_2cta(a_dst + P_A_BYTES, &tmB128, leader_bar, kb * H_BK, n0);
-                }
+    if (wg == 0) {
+        if (threadIdx.x == 0) {
+            for (int kb = 0; kb < nk; ++kb) {
+                const int s = kb % G_STAGES;
+                mbar_wait(&empty[s], ((kb / G_STAGES) & 1) ^ 1);   // the first pass over the ring falls through
+                unsigned char* a_dst = smem + s * G_STAGE_BYTES;
+                mbar_expect_tx(&full[s], G_STAGE_BYTES);
+                tma_load_2d(a_dst, &tmA, &full[s], kb * G_BK, m0);                 // rows past M are zero-filled by TMA
+                tma_load_2d(a_dst + G_TILE_BYTES, &tmB, &full[s], kb * G_BK, n0);
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0 && rank == 0) {
-            // c_format F32 | a,b F16 | K-major | N = 256 | M = 256 (the pair's rows)
-            const uint32_t idesc = (1u << 4) | ((uint32_t)(H_BN >> 3) << 17) | ((uint32_t)((2 * H_BM) >> 4) << 24);
-            int it = 0, lt = 0;
-            for (int pair = pair0; pair < npairs; pair += pair_step, ++lt) {
-                const int acc = lt & 1;
-                mbar_wait(&tmem_empty[acc], ((lt >> 1) & 1) ^ 1);      // both CTAs' epilogues have drained this accumulator
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(acc * H_BN);
-                for (int kb = 0; kb < nk; ++kb, ++it) {
-                    const int s = it % P_STAGES;
-                    mbar_wait(&full[s], (it / P_STAGES) & 1);          // both CTAs' tiles of this k-block have landed
-                    tc_fence_after();
-                    const uint32_t a_addr = smem_u32(smem + s * P_STAGE_BYTES);
-                    const uint64_t adesc = make_sw128_kmajor_desc(a_addr);
-                    const uint64_t bdesc = make_sw128_kmajor_desc(a_addr + P_A_BYTES);
+        return;
+    }
+
+    const int cw = wg - 1;                                    // consumer warpgroup: tile rows 64 cw .. 64 cw + 63
+    float acc[64];
 #pragma unroll
-                    for (int k4 = 0; k4 < H_BK / 16; ++k4)
-                        umma_f16_2cta(d_tmem, adesc + (uint64_t)(k4 * 2), bdesc + (uint64_t)(k4 * 2), idesc, (kb | k4) ? 1u : 0u);
-                    umma_commit_2cta(&empty[s], (uint16_t)0x3);       // frees the slot in both CTAs
-                }
-                umma_commit_2cta(&tmem_full[acc], (uint16_t)0x3);     // both CTAs' epilogues may read their halves
-            }
-        }
-    } else {
-        const int q = warp & 3;
-        constexpr int COLS = H_BN / (H_EPI_WARPS / 4);       // this warp's share of the columns: 128
-        const int c_lo = ((warp - 2) >> 2) * COLS;
-        int lt = 0;
-        for (int pair = pair0; pair < npairs; pair += pair_step, ++lt) {
-            const int acc = lt & 1;
-            const int m0 = ((m_rev ? pairs_m - 1 - pair / tiles_n : pair / tiles_n) * 2 + rank) * H_BM, n0 = (pair % tiles_n) * H_BN;
-            epilogue_tile<EPI, COLS / 32>(tmem_base + ((uint32_t)(q * 32) << 16), acc * H_BN, c_lo, m0 + q * 32 + lane, M, N, n0, C,
-                                          bias_f, residual, &tmem_full[acc], (uint32_t)((lt >> 1) & 1), [&]() {
-                                              tc_fence_before();
-                                              __syncwarp();
-                                              if (lane == 0) mbar_arrive_cluster(&tmem_empty[acc], 0u);   // the leader's barrier counts both CTAs' warps
-                                          });
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    for (int kb = 0; kb < nk; ++kb) {
+        const int s = kb % G_STAGES;
+        mbar_wait(&full[s], (kb / G_STAGES) & 1);
+        const uint32_t a_addr = smem_u32(smem + s * G_STAGE_BYTES);
+        const uint64_t adesc = make_sw128_kmajor_desc(a_addr + cw * 64 * 128);
+        const uint64_t bdesc = make_sw128_kmajor_desc(a_addr + G_TILE_BYTES);
+        acc_fence(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int k4 = 0; k4 < G_BK / 16; ++k4)   // advance 16 K-elements = 32 bytes inside the swizzle row: +2 in the (addr >> 4) field
+            wgmma_f16_n128(acc, adesc + (uint64_t)(k4 * 2), bdesc + (uint64_t)(k4 * 2));
+        wgmma_commit();
+        acc_fence(acc);
+        wgmma_wait<1>();                                      // the previous k-block's MMAs have retired: free its stage
+        if (kb > 0) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[(kb - 1) % G_STAGES]);
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();                                       // no CTA leaves (or frees TMEM) while its peer may still use it
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512));
+    wgmma_wait<0>();
+    acc_fence(acc);
+
+    // epilogue: acc[4 j + 2 h + c] is row r_lo + 8 h, column 8 j + 2 (lane % 4) + c of this warpgroup's 64 x 128 block.
+    // Bias added in fp32, GELU on the fp32 sum, rounded to half; the residual is added in half precision after the
+    // rounding, which is also the order of HF BertSelfOutput / BertOutput (dense -> fp16, then + input).
+    const int r_lo = m0 + cw * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int c_lo = n0 + 2 * (lane & 3);
+    float2 bj[16];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) bj[j] = __half22float2(*reinterpret_cast<const __half2*>(bias + c_lo + 8 * j));
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int row = r_lo + 8 * h;
+        if (row >= M) continue;
+        __half* dst = C + (size_t)row * N + c_lo;
+        const __half* res = residual + (size_t)row * N + c_lo;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            float x0 = __fadd_rn(acc[4 * j + 2 * h], bj[j].x), x1 = __fadd_rn(acc[4 * j + 2 * h + 1], bj[j].y);
+            if (EPI == EPI_BIAS_GELU) f2unpack(gelu_erf_pair(f2pack(x0, x1)), x0, x1);
+            __half2 o = __floats2half2_rn(x0, x1);
+            if (EPI == EPI_BIAS_RESIDUAL) o = __hadd2(o, *reinterpret_cast<const __half2*>(res + 8 * j));
+            *reinterpret_cast<__half2*>(dst + 8 * j) = o;
+        }
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -608,10 +278,9 @@ __global__ void layernorm_kernel(const __half* __restrict__ in, int T, const __h
 }
 
 // Persistent form for the two LayerNorms of a layer: a warp walks rows gw, gw + nw, ... with the raw 1.5 KB of its NEXT
-// row already requested while it reduces and stores the current one.  Inside a forward
-// the one-row-per-warp kernel ran 28-31 us against 21.5 us in isolation (RSB_BERT_PROFILE): after a GEMM the SM clock
-// sits at ~1.45 GHz under the power cap, and a warp that loads, reduces and stores one row and exits is bound by its own
-// latency chain, not by HBM.  Same arithmetic, same order of operations per row (RSB_LN_V1=1: the first form, A/B).
+// row already requested while it reduces and stores the current one.  Inside a forward (clock lowered by the power
+// cap after a GEMM) a warp that loads, reduces and stores one row and exits is bound by its own latency chain, not by
+// HBM; the one-row-per-warp kernel was slower there than in isolation (RSB_BERT_PROFILE).  Same arithmetic, same order of operations per row (RSB_LN_V1=1: the first form, A/B).
 __global__ __launch_bounds__(256, 3)
 void layernorm_rows_kernel(const __half* __restrict__ in, int T, const __half* __restrict__ gamma,
                            const __half* __restrict__ beta, float eps, __half* __restrict__ out) {
@@ -675,7 +344,7 @@ constexpr int ATT_HD = 64, ATT_PADH = 72, ATT_MAXS = 512;
 
 // ---------------------------------------------------------------------------------------------------------
 // attention for query-length sequences (S <= 32): ONE WARP per (sequence, head), QK^T and PV on the tensor cores
-// with mma.sync.m16n8k16 (a 32x32x64 problem is far too small for a tcgen05 tile), softmax on the accumulator
+// with mma.sync.m16n8k16 (a 32x32x64 problem is far too small for a wgmma tile), softmax on the accumulator
 // fragments in registers.  Q and K fragments are read straight from global memory as 32-bit words (row-major
 // [token, 64] slices are exactly the A / "col" B fragment layouts); V is staged per warp in shared memory and
 // read with ldmatrix.trans.  ~64 MMAs per (sequence, head) instead of ~10k scalar instructions.
@@ -711,12 +380,11 @@ void attention_mma32_kernel(const __half* __restrict__ qkv, const int* __restric
     Tile Qs = reinterpret_cast<Tile>(att32_smem + wib * ATT32_WARP_BYTES);
     Tile Ks = Qs + 32, Vs = Qs + 64;
 
-    // (A persistent variant that prefetched the next item's tiles with cp.async into a second buffer was measured and
-    // dropped: 81 vs 74 us per layer -- the double buffer halves the resident warps and the kernel is bound by the
-    // dependent-instruction latency of each warp, profiles/r02_ncu_summary_scan_attention.md.)
+    // (A persistent variant that prefetched the next item's tiles with cp.async into a second buffer was slower: the
+    // double buffer halves the resident warps and the kernel is bound by the dependent-instruction latency of each warp.)
     // stage Q, K, V (rows >= S zero-filled): 8 lanes cover one 128-byte row, a warp instruction covers 4 whole rows --
-    // every sector that is fetched is used (the 32-bit fragment loads straight from global memory of the first version
-    // touched 32 sectors per instruction for 128 useful bytes; the kernel ran at half of the HBM rate)
+    // every sector that is fetched is used (32-bit fragment loads straight from global memory would touch 32 sectors per
+    // instruction for 128 useful bytes)
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
         const int idx = lane + 32 * i, j = idx >> 3, c = idx & 7;
@@ -882,8 +550,8 @@ void attention_flash_kernel(const __half* __restrict__ qkv, const int* __restric
     __shared__ __align__(16) __half Vs[32][ATT_PADH];
     // work items (long sequence, head, block of 128 queries) in a grid-stride loop over the list that collect_long_kernel
     // wrote once for this forward.  A batch of queries holds one or two sequences beyond 32 tokens: walking all
-    // B x heads x nqb candidates every layer kept the side stream busy for 36 us and slowed the short-sequence kernel it
-    // overlaps with (attention 74 -> 120 us per layer inside a forward, RSB_BERT_PROFILE).
+    // B x heads x nqb candidates every layer would keep the side stream busy and slow the short-sequence kernel it
+    // overlaps with.
     const int n_items = *long_count * heads * nqb;
     for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
     const int qblk = item % nqb, h = (item / nqb) % heads, b = long_list[item / (nqb * heads)];
@@ -1072,8 +740,8 @@ struct Linear {
     __half* w = nullptr;   // [N, K]
     __half* b = nullptr;   // [N]
     int N = 0, K = 0;
-    CUtensorMap map;       // box 128 rows (v1 tiles)
-    bool map_ok = false, pair_ok = false;   // pair_ok: N a multiple of 256 and the fp32 bias fits its shared-memory slot
+    CUtensorMap map;       // box 128 rows
+    bool map_ok = false;
 };
 
 struct Layer {
@@ -1106,7 +774,6 @@ int alloc_linear(Linear& l, int N, int K) {
     cudaMemset(l.w, 0, (size_t)N * K * 2);
     cudaMemset(l.b, 0, (size_t)N * 2);
     l.map_ok = make_map(&l.map, l.w, N, K, G_BN);
-    l.pair_ok = (N % H_BN == 0) && N <= H_BIAS_MAX;
     return l.map_ok ? RSB_OK : RSB_ERR_CUDA;
 }
 void free_linear(Linear& l) { cudaFree(l.w); cudaFree(l.b); }
@@ -1116,24 +783,13 @@ void free_linear(Linear& l) { cudaFree(l.w); cudaFree(l.b); }
 template <int EPI>
 int launch_gemm(const __half* A, int M, const Linear& lin, __half* C, const __half* residual, cudaStream_t st, bool m_rev = false) {
     CUtensorMap tmA;
-    if (!make_map(&tmA, A, (uint64_t)M, (uint64_t)lin.K, G_BM)) return RSB_ERR_CUDA;
+    if (!lin.map_ok || !make_map(&tmA, A, (uint64_t)M, (uint64_t)lin.K, G_BM)) return RSB_ERR_CUDA;
     static rsb::PerDeviceFlag configured;                    // attributes are per (function, device)
-    if (configured.first()) {
-        cudaFuncSetAttribute(gemm_tn_kernel<EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, G_SMEM);
-        cudaFuncSetAttribute(gemm_tn_pair_kernel<EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, P_SMEM);
-    }
-    const int sms = rsb::device_num_sms();
-    static const bool v1 = getenv("RSB_GEMM_V1") != nullptr;       // A/B: 128 x 128 tiles, one tile per CTA
-    if (!v1 && lin.pair_ok && lin.map_ok) {                      // CTA pairs, 2-SM MMAs (N a multiple of 256)
-        const int npairs = (lin.N / H_BN) * (((M + H_BM - 1) / H_BM + 1) / 2);
-        const int clusters = std::max(1, std::min(npairs, sms / 2));
-        static const bool no_snake = getenv("RSB_NO_SNAKE") != nullptr;
-        gemm_tn_pair_kernel<EPI><<<2 * clusters, H_THREADS, P_SMEM, st>>>(tmA, lin.map, C, lin.b, residual, M, lin.N, lin.K,
-                                                                          (m_rev && !no_snake) ? 1 : 0);
-        return RSB_OK;
-    }
-    dim3 grid(lin.N / G_BN, (M + G_BM - 1) / G_BM);                // N not a multiple of 256 (or forced): 128 x 128 tiles
-    gemm_tn_kernel<EPI><<<grid, G_THREADS, G_SMEM, st>>>(tmA, lin.map, C, lin.b, residual, M, lin.N, lin.K);
+    if (configured.first()) cudaFuncSetAttribute(gemm_tn_kernel<EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, G_SMEM);
+    static const bool no_snake = getenv("RSB_NO_SNAKE") != nullptr;
+    dim3 grid(lin.N / G_BN, (M + G_BM - 1) / G_BM);              // consecutive CTAs share one row tile of A
+    gemm_tn_kernel<EPI><<<grid, G_THREADS, G_SMEM, st>>>(tmA, lin.map, C, lin.b, residual, M, lin.N, lin.K,
+                                                         (m_rev && !no_snake) ? 1 : 0);
     return RSB_OK;
 }
 
@@ -1385,8 +1041,8 @@ extern "C" int rsb_gemm_f16(const void* A, const void* W, const void* bias, cons
     if (epilogue == EPI_BIAS_RESIDUAL && !residual) return bfail(RSB_ERR_INVALID, "residual is NULL");
     Linear lin;
     lin.w = (__half*)W; lin.b = (__half*)bias; lin.N = N; lin.K = K;
-    if (!make_map(&lin.map, W, N, K, G_BN)) return bfail(RSB_ERR_CUDA, "tensor map encode failed");
-    lin.pair_ok = (N % H_BN == 0) && N <= H_BIAS_MAX;
+    lin.map_ok = make_map(&lin.map, W, N, K, G_BN);
+    if (!lin.map_ok) return bfail(RSB_ERR_CUDA, "tensor map encode failed");
     cudaStream_t st = (cudaStream_t)stream;
     int rc;
     if (epilogue == EPI_BIAS) rc = launch_gemm<EPI_BIAS>((const __half*)A, M, lin, (__half*)C, nullptr, st);

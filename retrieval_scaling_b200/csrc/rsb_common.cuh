@@ -118,10 +118,9 @@ __device__ __forceinline__ void block_sort_desc_regs(u64* keys, int P) {
 // Block-wide bitonic sort of keys[0..P) (P a power of two), DESCENDING.  All threads of the block call it.
 __device__ __forceinline__ void block_sort_desc(u64* keys, int P) {
     const int tid = threadIdx.x, nt = blockDim.x;
-    // Measured on B200 (BASELINE config, scripts/gpu_ab.sh): the register variant wins for P <= blockDim (one key
-    // per thread: coarse select -0.1 ms) but loses for 2..8 keys per thread (scan +0.24 ms, merge +0.06 ms: its
-    // shuffles run on the same LSU pipe the look-ups saturate and it executes ~1.7x the instructions), so larger
-    // sorts stay on the shared-memory network unless RSB_SORT_REGS_ALL is defined.
+    // The register variant is used for P <= blockDim (one key per thread); for 2..8 keys per thread its shuffles run
+    // on the same LSU pipe the look-ups saturate and it executes ~1.7x the instructions, so larger sorts stay on the
+    // shared-memory network unless RSB_SORT_REGS_ALL is defined.
 #ifndef RSB_SORT_CLASSIC
     if ((nt & (nt - 1)) == 0 && nt >= 32) {                // block-uniform dispatch
         if (P <= nt) { block_sort_desc_regs<1>(keys, P); return; }

@@ -4,7 +4,7 @@
 //
 //   sgemm_nt_kernel      S[nq, n] = Q[nq, d] . X[n, d]^T   fp32 FMA tiles on the CUDA cores (used when d % 32 != 0, for
 //                        rsb_add's list assignment, or when RSB_OPT_COARSE_TENSOR = 0; the default scorer is the
-//                        3xTF32 tcgen05 GEMM of rsb_tf32.cu followed by refine_exact_kernel below)
+//                        3xTF32 wgmma GEMM of rsb_tf32.cu followed by refine_exact_kernel below)
 //   select_rows_kernel   per (row, column-split): thread-maxima prefilter + threshold-filtered candidate buffer
 //                        -> top-k keys
 //   merge_items_kernel   per query: merge the per-item key lists -> D (f32), I (i64)
@@ -149,8 +149,8 @@ void select_rows_kernel(const float* __restrict__ S, int ncols, int ld, unsigned
     u64* mx = keys + cap;   // 256-entry scratch behind the candidate buffer
     for (int tile = c0; tile < c1; tile += SEL_TILE) {
         float4 v[SEL_ROUNDS];
-        // All sixteen 128-bit loads are issued before anything consumes them (ncu: with load and use interleaved
-        // the in-order issue left ONE load in flight per warp and the kernel sat at 1 TB/s, 36% long-scoreboard).
+        // All sixteen 128-bit loads are issued before anything consumes them: with load and use interleaved the
+        // in-order issue leaves ONE load in flight per warp.
         // No guards on the loads: c, c0 and ld are multiples of 4 and a row owns ld >= c1 floats, so a float4 at
         // min(c, ld - 4) is always inside the row; lanes past c1 read don't-care values that every use below
         // masks with (c + j < c1).
@@ -424,8 +424,7 @@ void merge_items_kernel(const u64* __restrict__ keys_in, const int* __restrict__
     }
 }
 
-// Default form (round 2, measured on B200 at the BASELINE configuration: 0.165 -> 0.091 ms per 10k queries,
-// profiles/r02_ab_round1_leftovers.txt).  Same result as merge_items_kernel, but the per-item loop -- one dependent
+// Default form.  Same result as merge_items_kernel, but the per-item loop -- one dependent
 // count load, one key load and one barrier per item, 32 times per query: latency-bound -- is replaced by a prefix sum
 // over the item counts and rounds over the flattened candidate range (cap - k_out candidates per round, usually two
 // rounds), each thread locating its item by a binary search in shared memory.  On a list-partitioned multi-GPU shard
@@ -554,7 +553,7 @@ void merge_shards_kernel(const float* __restrict__ D_all, const int64_t* __restr
 // =============================================================================================================
 // Exact fp32 re-score of tensor-core (3xTF32) candidates: for each query, recompute <q, x[id]> with FFMA for the
 // k_in candidate rows, sort (score desc, id asc) and keep k_out.  Makes the coarse quantizer's output independent
-// of the tensor-core accumulation order (ids/scores as from the CUDA-core path) at ~0.1 ms per 10k queries.
+// of the tensor-core accumulation order (ids/scores as from the CUDA-core path).
 // =============================================================================================================
 __global__ __launch_bounds__(256)
 void refine_exact_kernel(const float* __restrict__ Q, const float* __restrict__ X, int d, const int64_t* __restrict__ I_in,

@@ -43,7 +43,7 @@ inline int device_num_sms() {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        if (n <= 0) n = 148;
+        if (n <= 0) n = 132;
     }
     return n;
 }
@@ -64,7 +64,7 @@ int launch_merge_shards_peers_scatter(const float* const* D_ptrs, const int64_t*
                                       int nq_slice, int k, int k_out, float* const* D_outs, int64_t* const* I_outs,
                                       int nout, cudaStream_t st);
 
-// ---- rsb_tf32.cu (tensor-core fp32-accurate scores: 3xTF32 on tcgen05) ---------------------------------
+// ---- rsb_tf32.cu (tensor-core fp32-accurate scores: 3xTF32 on wgmma) ---------------------------------
 bool tf32_path_available();
 void launch_split_tf32(const float* x, size_t n, float* hi, float* lo, cudaStream_t st);
 bool launch_gemm_tf32x3(const float* Ah, const float* Al, int M, const float* Bh, const float* Bl, int N, int K,
@@ -142,9 +142,9 @@ void launch_codebook_transpose(const float* cb, int M, int dsub, float* cbT, cud
 void launch_pq_encode(const float* x, int64_t n, int d, const int32_t* list, const float* centroids,
                       const float* codebook, int M, uint8_t* codes, cudaStream_t st);
 // k-means update steps of index.train(): member sums / counts (float atomics)
-void launch_kmeans_accumulate(const float* x, int64_t n, int d, const int32_t* assign, int k, float* sums, float* counts,
+cudaError_t launch_kmeans_accumulate(const float* x, int64_t n, int d, const int32_t* assign, int k, float* sums, float* counts,
                               cudaStream_t st);
-void launch_pq_accumulate(const float* r, int64_t n, int d, int M, const uint8_t* codes, float* sums, float* counts,
+cudaError_t launch_pq_accumulate(const float* r, int64_t n, int d, int M, const uint8_t* codes, float* sums, float* counts,
                           cudaStream_t st);
 // natural codes -> interleaved blocks (see rsb_layout.h).  src_row[i] = row in `codes_nat` of the i-th vector in
 // list-sorted order; rank/list via list_of_sorted + list_nat_off.

@@ -7,6 +7,8 @@
 #include "rsb_layout.h"
 #include "rsb_tc.cuh"
 
+#include <cub/device/device_radix_sort.cuh>
+
 #include <float.h>
 #include <stdlib.h>
 #include <algorithm>
@@ -352,12 +354,11 @@ void pq_lut_kernel(const float* __restrict__ queries, int nq, int d, int M, cons
 // M = 64, dsub = 12 (the BASELINE configuration): codebook-stationary variant.  A block owns 8 code values j for all
 // 64 sub-quantizers: every thread keeps the two 12-float codebook entries (j, m), (j+4, m) in registers for its
 // whole life and streams queries through shared memory (16 at a time, 48 KB), so the inner loop is 3 conflict-free
-// LDS.128 + 24 FMA + 2 coalesced stores per query with no global-memory latency in it.  ncu on the query-stationary
-// kernel above showed nothing saturated (issue 38%, 16 warps/SM, L2 12%): it was latency-bound on the codebook
-// loads; this one is bound by the 64 KB/query table write.
+// LDS.128 + 24 FMA + 2 coalesced stores per query with no global-memory latency in it.  The query-stationary kernel
+// above is latency-bound on the codebook loads; this one is bound by the 64 KB/query table write.
 constexpr int L64_QS = 16;
 
-// JT = code values per thread (rows j0 + 4*i of the transposed codebook): 2 in round 1; 4 halves the shared-memory reads
+// JT = code values per thread (rows j0 + 4*i of the transposed codebook): 4 instead of 2 halves the shared-memory reads
 // of the query sub-vectors per table entry (the kernel's binding pipe) at 48 codebook registers per thread.
 template <int JT>
 __global__ __launch_bounds__(256, JT == 2 ? 4 : 3)
@@ -596,8 +597,8 @@ __device__ __forceinline__ unsigned pq_scan_list(const unsigned char* lutb, cons
     // capacity check (one barrier); a compaction that found k candidates tightens the bound for every block
     // working on this query
     // The other blocks' bound for this query is read from global memory at the START of a check interval and merged in
-    // at its end: ncu's source view had 8 % of the kernel's stall samples on the max that consumed a load issued right
-    // in front of it.  A bound that is one interval old is still a valid bound.
+    // at its end, so the load is not consumed right after it is issued.  A bound that is one interval old is still a
+    // valid bound.
 #define RSB_PQ_CHECKPOINT()                                                                                \
     {                                                                                                      \
         const unsigned tau_new = block_maybe_compact(keys, s_count, k, cap, PQ_SLACK, tau);                \
@@ -996,48 +997,99 @@ void launch_pq_encode(const float* x, int64_t n, int d, const int32_t* list, con
 // PQ codebooks; reference call sites src/indicies/ivf_flat.py:166, ivf_pq.py:170).  The assignment steps are the
 // coarse quantizer itself (tensor-core scorer + exact re-score) and pq_encode_kernel; these accumulate the member sums.
 // =============================================================================================================
-// sums[k, d] += x[row] for row's cluster, counts[k] += 1.  One warp per row, float4 atomics spread over d.
-__global__ void kmeans_accumulate_kernel(const float* __restrict__ x, int64_t n, int d, const int32_t* __restrict__ assign,
-                                         int k, float* __restrict__ sums, float* __restrict__ counts) {
-    const int lane = threadIdx.x & 31;
-    const int64_t wid = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const int64_t nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
-    for (int64_t i = wid; i < n; i += nw) {
-        const int a = assign[i];
-        if (a < 0 || a >= k) continue;
-        const float* src = x + (size_t)i * d;
-        float* dst = sums + (size_t)a * d;
-        for (int c = lane; c < d; c += 32) atomicAdd(dst + c, src[c]);
-        if (lane == 0) atomicAdd(counts + a, 1.f);
+// Member sums in a fixed order, so that training gives the same centroids / codebooks on every run: the members are
+// grouped by cluster with a stable radix sort (ties keep ascending row order), then one warp per cluster adds its
+// members' rows in ascending row order.  An "item" is one row (k-means: key = its cluster, its vector = x[item]) or one
+// (row, sub-quantizer) pair (PQ: key = m * 256 + code, its vector = the m-th sub-vector of the row).
+__global__ void accumulate_keys_kernel(int64_t nitems, int M, const int32_t* __restrict__ assign, int k,
+                                       const uint8_t* __restrict__ codes, int32_t* __restrict__ keys, int64_t* __restrict__ items) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nitems; i += (int64_t)gridDim.x * blockDim.x) {
+        int key;
+        if (codes) key = (int)(i % M) * 256 + codes[i];
+        else key = (assign[i] >= 0 && assign[i] < k) ? assign[i] : k;      // out-of-range assignments: ignored
+        keys[i] = key;
+        items[i] = i;
     }
 }
-void launch_kmeans_accumulate(const float* x, int64_t n, int d, const int32_t* assign, int k, float* sums, float* counts,
-                              cudaStream_t st) {
-    if (n <= 0) return;
-    const int blocks = (int)std::min<int64_t>(8 * (int64_t)num_sms(), (n * 32 + 255) / 256);
-    kmeans_accumulate_kernel<<<blocks, 256, 0, st>>>(x, n, d, assign, k, sums, counts);
+__global__ void accumulate_bounds_kernel(const int32_t* __restrict__ keys, int64_t nitems, int nkeys,
+                                         int64_t* __restrict__ begin, int64_t* __restrict__ end) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nitems; i += (int64_t)gridDim.x * blockDim.x) {
+        const int key = keys[i];
+        if (key >= nkeys) continue;
+        if (i == 0 || keys[i - 1] != key) begin[key] = i;
+        if (i == nitems - 1 || keys[i + 1] != key) end[key] = i + 1;
+    }
+}
+// sums[key, 0:w] += sum of the item vectors of `key` in ascending item order, counts[key] += their number
+__global__ void accumulate_sums_kernel(const float* __restrict__ x, int d, int M, int w, const int64_t* __restrict__ items,
+                                       const int64_t* __restrict__ begin, const int64_t* __restrict__ end, int nkeys,
+                                       float* __restrict__ sums, float* __restrict__ counts) {
+    const int lane = threadIdx.x & 31;
+    const int key = (int)(((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+    if (key >= nkeys) return;
+    const int64_t b = begin[key], e = end[key];
+    for (int c0 = 0; c0 < w; c0 += 32) {
+        const int c = c0 + lane;
+        float acc = 0.f;
+        for (int64_t j = b; j < e; ++j) {
+            const int64_t it = items[j];
+            if (c < w) acc += x[(it / M) * d + (it % M) * w + c];
+        }
+        if (c < w && e > b) sums[(size_t)key * w + c] += acc;
+    }
+    if (lane == 0 && e > b) counts[key] += (float)(e - b);
 }
 
-// PQ: sums[m, code, :] += r[row, m*dsub : (m+1)*dsub], counts[m, code] += 1.  One thread per (row, m).
-__global__ void pq_accumulate_kernel(const float* __restrict__ r, int64_t n, int d, int M, const uint8_t* __restrict__ codes,
-                                     float* __restrict__ sums, float* __restrict__ counts) {
-    const int dsub = d / M;
-    const int64_t total = n * M;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-        const int64_t row = i / M;
-        const int m = (int)(i % M);
-        const int j = codes[i];
-        const float* src = r + (size_t)row * d + m * dsub;
-        float* dst = sums + ((size_t)m * 256 + j) * dsub;
-        for (int t = 0; t < dsub; ++t) atomicAdd(dst + t, src[t]);
-        atomicAdd(counts + m * 256 + j, 1.f);
+static cudaError_t accumulate_sorted(const float* x, int64_t n, int d, int M, const int32_t* assign, int k,
+                                     const uint8_t* codes, int nkeys, float* sums, float* counts, cudaStream_t st) {
+    const int64_t nitems = n * M;
+    int bits = 1;
+    while ((1 << bits) <= nkeys) ++bits;                                   // key nkeys (ignored items) must fit
+    int32_t *keys = nullptr, *keys_sorted = nullptr;
+    int64_t *items = nullptr, *items_sorted = nullptr, *bounds = nullptr;
+    void* tmp = nullptr;
+    size_t tmp_bytes = 0;
+    cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys, keys_sorted, items, items_sorted, nitems, 0, bits, st);
+    if (e == cudaSuccess) e = cudaMallocAsync(&keys, (size_t)nitems * 4, st);
+    if (e == cudaSuccess) e = cudaMallocAsync(&keys_sorted, (size_t)nitems * 4, st);
+    if (e == cudaSuccess) e = cudaMallocAsync(&items, (size_t)nitems * 8, st);
+    if (e == cudaSuccess) e = cudaMallocAsync(&items_sorted, (size_t)nitems * 8, st);
+    if (e == cudaSuccess) e = cudaMallocAsync(&bounds, (size_t)nkeys * 2 * 8, st);
+    if (e == cudaSuccess) e = cudaMallocAsync(&tmp, tmp_bytes, st);
+    if (e == cudaSuccess) {
+        const int blocks = (int)std::min<int64_t>(8 * (int64_t)num_sms(), (nitems + 255) / 256);
+        accumulate_keys_kernel<<<blocks, 256, 0, st>>>(nitems, M, assign, k, codes, keys, items);
+        e = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, keys_sorted, items, items_sorted, nitems, 0, bits, st);
     }
+    if (e == cudaSuccess) e = cudaMemsetAsync(bounds, 0, (size_t)nkeys * 2 * 8, st);
+    if (e == cudaSuccess) {
+        const int blocks = (int)std::min<int64_t>(8 * (int64_t)num_sms(), (nitems + 255) / 256);
+        accumulate_bounds_kernel<<<blocks, 256, 0, st>>>(keys_sorted, nitems, nkeys, bounds, bounds + nkeys);
+        accumulate_sums_kernel<<<(nkeys + 7) / 8, 256, 0, st>>>(x, d, M, d / M, items_sorted, bounds, bounds + nkeys, nkeys,
+                                                              sums, counts);
+        e = cudaGetLastError();
+    }
+    cudaFreeAsync(tmp, st);
+    cudaFreeAsync(bounds, st);
+    cudaFreeAsync(items_sorted, st);
+    cudaFreeAsync(items, st);
+    cudaFreeAsync(keys_sorted, st);
+    cudaFreeAsync(keys, st);
+    return e;
 }
-void launch_pq_accumulate(const float* r, int64_t n, int d, int M, const uint8_t* codes, float* sums, float* counts,
-                          cudaStream_t st) {
-    if (n <= 0) return;
-    const int blocks = (int)std::min<int64_t>(8 * (int64_t)num_sms(), (n * M + 255) / 256);
-    pq_accumulate_kernel<<<blocks, 256, 0, st>>>(r, n, d, M, codes, sums, counts);
+
+// sums[k, d] += x[row] for row's cluster, counts[k] += 1
+cudaError_t launch_kmeans_accumulate(const float* x, int64_t n, int d, const int32_t* assign, int k, float* sums, float* counts,
+                                     cudaStream_t st) {
+    if (n <= 0) return cudaSuccess;
+    return accumulate_sorted(x, n, d, 1, assign, k, nullptr, k, sums, counts, st);
+}
+
+// PQ: sums[m, code, :] += r[row, m*dsub : (m+1)*dsub], counts[m, code] += 1
+cudaError_t launch_pq_accumulate(const float* r, int64_t n, int d, int M, const uint8_t* codes, float* sums, float* counts,
+                                 cudaStream_t st) {
+    if (n <= 0) return cudaSuccess;
+    return accumulate_sorted(r, n, d, M, nullptr, 0, codes, M * 256, sums, counts, st);
 }
 
 // =============================================================================================================

@@ -1,13 +1,13 @@
-// rsb_tf32.cu -- fp32-accurate inner-product scores on the 5th-gen tensor cores: S[M,N] = A[M,K] . B[N,K]^T with
+// rsb_tf32.cu -- fp32-accurate inner-product scores on the Hopper tensor cores: S[M,N] = A[M,K] . B[N,K]^T with
 // A, B fp32, computed as the error-compensated 3xTF32 product
 //        A.B ~= Ah.Bh + Ah.Bl + Al.Bh        (x = xh + xl, xh = tf32(x), xl = tf32(x - xh); the dropped Al.Bl term
-// is ~2^-22 relative) accumulated in fp32 in TMEM.  Used for the IVF coarse quantizer (the IndexFlatIP the reference
-// builds at src/indicies/ivf_flat.py:142, ivf_pq.py:145), where the CUDA-core fp32 GEMM was 14 % of a search step.
+// is ~2^-22 relative) accumulated in fp32 registers.  Used for the IVF coarse quantizer (the IndexFlatIP the reference
+// builds at src/indicies/ivf_flat.py:142, ivf_pq.py:145).
 //
-// Same pipeline as the encoder GEMM (rsb_bert.cu): TMA tensor loads (128B swizzle, 32 fp32 = one swizzle row per
-// K step) -> 3-stage shared-memory ring of {Ah, Al, Bh, Bl} tiles -> one elected thread issues 12
-// tcgen05.mma.kind::tf32 per stage (4 K-slices x 3 products) -> tcgen05.commit -> epilogue warps tcgen05.ld the
-// 128x128 fp32 tile and store it with 128-bit writes.
+// Same pipeline as the encoder GEMM (rsb_bert.cu): 128 x 128 output tile per CTA, TMA tensor loads (128B swizzle,
+// 32 fp32 = one swizzle row per K step) -> 3-stage shared-memory ring of {Ah, Al, Bh, Bl} tiles filled by one
+// producer thread -> two consumer warpgroups, each issuing 12 wgmma.m64n128k8.tf32 per stage (4 K-slices x 3
+// products) on its 64 rows -> epilogue from the accumulator registers.
 #include "rsb_common.cuh"
 #include "rsb_internal.h"
 #include "rsb_tc.cuh"
@@ -19,10 +19,13 @@ namespace rsb {
 
 using namespace rsbtc;
 
-constexpr int T_BM = 128, T_BN = 128, T_BK = 32, T_STAGES = 3, T_THREADS = 192;
-constexpr int T_TILE_BYTES = 128 * T_BK * 4;                 // 16 KB
-constexpr int T_STAGE_BYTES = 4 * T_TILE_BYTES;              // Ah, Al, Bh, Bl
+constexpr int T_BM = 128, T_BN = 128, T_BK = 32, T_STAGES = 3;
+constexpr int T_THREADS = 384;                                // warpgroup 0: TMA producer, warpgroups 1-2: MMA + epilogue
+constexpr int T_TILE_BYTES = 128 * T_BK * 4;                  // 16 KB
+constexpr int T_STAGE_BYTES = 4 * T_TILE_BYTES;               // Ah, Al, Bh, Bl
 constexpr int T_SMEM = T_STAGES * T_STAGE_BYTES + 1024 + 256;
+constexpr int T_LDS = T_BN + 1;                               // row stride of the fused epilogue's staged tile (floats)
+static_assert(T_BM * T_LDS * 4 + T_BM * 9 * 8 <= T_STAGES * T_STAGE_BYTES, "staged tile must fit in the ring");
 
 __global__ void split_tf32_kernel(const float* __restrict__ x, size_t n, float* __restrict__ hi, float* __restrict__ lo) {
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
@@ -42,297 +45,209 @@ void launch_split_tf32(const float* x, size_t n, float* hi, float* lo, cudaStrea
     split_tf32_kernel<<<blocks, 256, 0, st>>>(x, n, hi, lo);
 }
 
-__global__ __launch_bounds__(T_THREADS)
+// FUSED = false: the 128 x 128 score tile goes to C.  FUSED = true: the score tile never goes to HBM.  Every row of
+// the tile keeps its 9 largest scores (sorted insertion in column order, strict comparisons => ties keep the lower
+// column); the top 8 are emitted as candidates (64 B per row per 128-column tile) together with the 9th as a bound:
+// an element the filter dropped is <= the 9th largest of its tile, so if the kc-th best CANDIDATE of a row is
+// strictly greater than the maximum of these bounds over the row, no dropped element can belong to the row's top kc
+// -- select_cands_kernel checks exactly that and flags the (rare) rows for which it fails; those are re-done
+// exhaustively in fp32 by exact_rows_kernel.  The result is therefore the exact top-kc of the 3xTF32 scores without
+// writing and re-reading nq x nlist x 4 bytes.
+template <bool FUSED>
+__global__ __launch_bounds__(T_THREADS, 1)
 void gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
                         const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl,
-                        float* __restrict__ C, int ldc, int M, int N, int K) {
+                        float* __restrict__ C, int ldc, u64* __restrict__ cand, unsigned* __restrict__ xbound,
+                        int M, int N, int K, unsigned col_base, int m_fastest) {
     extern __shared__ unsigned char smem_dyn[];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + T_STAGES * T_STAGE_BYTES);
     uint64_t* empty = full + T_STAGES;
-    uint64_t* tmem_full = empty + T_STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full + 1);
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int m0 = blockIdx.y * T_BM, n0 = blockIdx.x * T_BN;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
+    int tm = blockIdx.y, tn = blockIdx.x;
+    const int nhalf = 2 * ((N + 255) / 256);                  // 128-column candidate items per row (FUSED)
+    if (FUSED) {
+        // tile order: m fastest = consecutive tiles share one B (centroid) tile and sweep the query tiles, which stay
+        // L2-resident -- n fastest re-reads the whole centroid matrix per query tile
+        const int tiles_m = (M + T_BM - 1) / T_BM;
+        tm = m_fastest ? (int)blockIdx.x % tiles_m : (int)blockIdx.x / nhalf;
+        tn = m_fastest ? (int)blockIdx.x / tiles_m : (int)blockIdx.x % nhalf;
+    }
+    const int m0 = tm * T_BM, n0 = tn * T_BN;
     const int nk = K / T_BK;
+    if (FUSED && n0 >= N) {                                   // the empty second half of a 256-column group: no candidates
+        const int row = m0 + (int)threadIdx.x;
+        if (threadIdx.x < T_BM && row < M) {
+            const size_t item = (size_t)row * nhalf + (size_t)tn;
+            ulonglong2* dst = reinterpret_cast<ulonglong2*>(cand + item * 8);
+#pragma unroll
+            for (int i = 0; i < 4; ++i) dst[i] = make_ulonglong2(0ull, 0ull);
+            xbound[item] = 0u;
+        }
+        return;
+    }
 
     if (threadIdx.x == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmAh)) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmAl)) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmBh)) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmBl)) : "memory");
-        for (int s = 0; s < T_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        mbar_init(tmem_full, 1);
+        for (int s = 0; s < T_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }   // 8 consumer warps
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, T_BN);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (wg == 0) {
+        if (threadIdx.x == 0) {
             for (int kb = 0; kb < nk; ++kb) {
                 const int s = kb % T_STAGES;
-                if (kb >= T_STAGES) mbar_wait(&empty[s], ((kb / T_STAGES) - 1) & 1);
+                mbar_wait(&empty[s], ((kb / T_STAGES) & 1) ^ 1);   // the first pass over the ring falls through
                 unsigned char* base = smem + s * T_STAGE_BYTES;
                 mbar_expect_tx(&full[s], T_STAGE_BYTES);
-                tma_load_2d(base + 0 * T_TILE_BYTES, &tmAh, &full[s], kb * T_BK, m0);
+                tma_load_2d(base + 0 * T_TILE_BYTES, &tmAh, &full[s], kb * T_BK, m0);   // rows past M / N read as zero
                 tma_load_2d(base + 1 * T_TILE_BYTES, &tmAl, &full[s], kb * T_BK, m0);
                 tma_load_2d(base + 2 * T_TILE_BYTES, &tmBh, &full[s], kb * T_BK, n0);
                 tma_load_2d(base + 3 * T_TILE_BYTES, &tmBl, &full[s], kb * T_BK, n0);
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // c_format F32 (1<<4) | a_format TF32 (2<<7) | b_format TF32 (2<<10) | K-major | N>>3 | M>>4
-            const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(T_BN >> 3) << 17) | ((uint32_t)(T_BM >> 4) << 24);
-            for (int kb = 0; kb < nk; ++kb) {
-                const int s = kb % T_STAGES;
-                mbar_wait(&full[s], (kb / T_STAGES) & 1);
-                tc_fence_after();
-                const uint32_t base = smem_u32(smem + s * T_STAGE_BYTES);
-                const uint64_t ah = make_sw128_kmajor_desc(base + 0 * T_TILE_BYTES);
-                const uint64_t al = make_sw128_kmajor_desc(base + 1 * T_TILE_BYTES);
-                const uint64_t bh = make_sw128_kmajor_desc(base + 2 * T_TILE_BYTES);
-                const uint64_t bl = make_sw128_kmajor_desc(base + 3 * T_TILE_BYTES);
-#pragma unroll
-                for (int k4 = 0; k4 < T_BK / 8; ++k4) {   // UMMA_K = 8 tf32 = 32 bytes: +2 in the (addr >> 4) field
-                    const uint64_t o = (uint64_t)(k4 * 2);
-                    // small terms first, the dominant Ah.Bh product last
-                    umma_tf32(tmem_base, al + o, bh + o, idesc, (kb | k4) ? 1u : 0u);
-                    umma_tf32(tmem_base, ah + o, bl + o, idesc, 1u);
-                    umma_tf32(tmem_base, ah + o, bh + o, idesc, 1u);
-                }
-                umma_commit(&empty[s]);
-                if (kb == nk - 1) umma_commit(tmem_full);
-            }
-        }
-    } else {
-        const int q = warp & 3;
-        const int row = m0 + q * 32 + lane;
-        mbar_wait(tmem_full, 0);
-        tc_fence_after();
-#pragma unroll 1
-        for (int c = 0; c < T_BN; c += 32) {
-            uint32_t r[32];
-            tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c, r);
-            if (row < M) {
-                const int col0 = n0 + c;
-                float* dst = C + (size_t)row * ldc + col0;
-                if (col0 + 31 < N) {
-#pragma unroll
-                    for (int v = 0; v < 8; ++v)
-                        *reinterpret_cast<float4*>(dst + v * 4) =
-                            make_float4(__uint_as_float(r[v * 4]), __uint_as_float(r[v * 4 + 1]),
-                                        __uint_as_float(r[v * 4 + 2]), __uint_as_float(r[v * 4 + 3]));
-                } else {
-#pragma unroll
-                    for (int e = 0; e < 32; ++e)
-                        if (col0 + e < N) dst[e] = __uint_as_float(r[e]);
-                }
-            }
-        }
+        return;
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, T_BN);
-}
 
-
-// =============================================================================================================
-// Fused scorer + candidate filter (round 2): the same 3xTF32 product, but persistent 128 x 256 tiles with a
-// double-buffered TMEM accumulator (2 x 256 columns), and the score matrix never goes to HBM.  Every epilogue
-// lane owns one query row of a 128-column half tile and keeps its 9 largest scores in registers (sorted insertion,
-// strict comparisons => ties keep the lower column); the top 8 are emitted as candidates (64 B per row per half
-// tile) together with the 9th as a bound:  an element the filter dropped is <= the 9th largest of its half tile, so
-// if the kc-th best CANDIDATE of a row is strictly greater than the maximum of these bounds over the row, no
-// dropped element can belong to the row's top kc -- select_cands_kernel checks exactly that and flags the (rare)
-// rows for which it fails; those are re-done exhaustively in fp32 by exact_rows_kernel.  The result is therefore
-// the exact top-kc of the 3xTF32 scores, as before, without writing and re-reading nq x nlist x 4 bytes
-// (653 MB per 10k-query batch at the BASELINE configuration).
-//
-// warp 0: TMA producer, warp 1: MMA issuer (12 tcgen05.mma.kind::tf32 per 32-wide k-block), warps 2-9: epilogue
-// (warp % 4 = TMEM lane quarter, (warp - 2) / 4 = column half).
-// =============================================================================================================
-constexpr int F_BM = 128, F_BN = 256, F_BK = 32, F_STAGES = 2, F_EPI_WARPS = 8;
-constexpr int F_THREADS = 64 + 32 * F_EPI_WARPS;
-constexpr int F_A_BYTES = F_BM * F_BK * 4;                        // 16 KB (hi or lo)
-constexpr int F_B_BYTES = F_BN * F_BK * 4;                        // 32 KB
-constexpr int F_STAGE_BYTES = 2 * (F_A_BYTES + F_B_BYTES);        // 96 KB
-constexpr int F_SMEM = F_STAGES * F_STAGE_BYTES + 1024 + 256;
-
-__device__ __forceinline__ void f_mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-__global__ __launch_bounds__(F_THREADS, 1)
-void gemm_tf32x3_topt_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
-                             const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl,
-                             u64* __restrict__ cand, unsigned* __restrict__ xbound, int M, int N, int K,
-                             unsigned col_base, int m_fastest) {
-    extern __shared__ unsigned char smem_dyn[];
-    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + F_STAGES * F_STAGE_BYTES);
-    uint64_t* empty = full + F_STAGES;
-    uint64_t* tmem_full = empty + F_STAGES;      // [2]
-    uint64_t* tmem_empty = tmem_full + 2;        // [2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int tiles_n = (N + F_BN - 1) / F_BN;
-    const int tiles_m = (M + F_BM - 1) / F_BM;
-    const int ntiles = tiles_m * tiles_n;
-    const int nhalf = 2 * tiles_n;
-    const int nk = K / F_BK;
-
-    if (threadIdx.x == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmAh)) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmAl)) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmBh)) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmBl)) : "memory");
-        for (int s = 0; s < F_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(&tmem_full[a], 1); mbar_init(&tmem_empty[a], F_EPI_WARPS); }
-        fence_barrier_init();
-    }
-    if (warp == 1) tmem_alloc(tmem_slot, 512);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        if (lane == 0) {
-            int it = 0;
-            for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-                // tile order: m fastest = consecutive tiles share one B (centroid) tile and sweep the query tiles, which
-                // stay L2-resident (61 MB at 10k queries) -- n fastest re-reads the whole centroid matrix per query tile
-                const int tm = m_fastest ? tile % tiles_m : tile / tiles_n, tn = m_fastest ? tile / tiles_m : tile % tiles_n;
-                const int m0 = tm * F_BM, n0 = tn * F_BN;
-                for (int kb = 0; kb < nk; ++kb, ++it) {
-                    const int s = it % F_STAGES;
-                    mbar_wait(&empty[s], ((it / F_STAGES) & 1) ^ 1);   // first pass over the ring falls through
-                    unsigned char* base = smem + s * F_STAGE_BYTES;
-                    mbar_expect_tx(&full[s], F_STAGE_BYTES);
-                    tma_load_2d(base, &tmAh, &full[s], kb * F_BK, m0);
-                    tma_load_2d(base + F_A_BYTES, &tmAl, &full[s], kb * F_BK, m0);
-                    tma_load_2d(base + 2 * F_A_BYTES, &tmBh, &full[s], kb * F_BK, n0);
-                    tma_load_2d(base + 2 * F_A_BYTES + F_B_BYTES, &tmBl, &full[s], kb * F_BK, n0);
-                }
-            }
+    const int cw = wg - 1;                                    // consumer warpgroup: tile rows 64 cw .. 64 cw + 63
+    float acc[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    for (int kb = 0; kb < nk; ++kb) {
+        const int s = kb % T_STAGES;
+        mbar_wait(&full[s], (kb / T_STAGES) & 1);
+        const uint32_t base = smem_u32(smem + s * T_STAGE_BYTES);
+        const uint64_t ah = make_sw128_kmajor_desc(base + cw * 64 * 128);
+        const uint64_t al = make_sw128_kmajor_desc(base + T_TILE_BYTES + cw * 64 * 128);
+        const uint64_t bh = make_sw128_kmajor_desc(base + 2 * T_TILE_BYTES);
+        const uint64_t bl = make_sw128_kmajor_desc(base + 3 * T_TILE_BYTES);
+        acc_fence(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int k4 = 0; k4 < T_BK / 8; ++k4) {               // K = 8 tf32 = 32 bytes: +2 in the (addr >> 4) field
+            const uint64_t o = (uint64_t)(k4 * 2);
+            wgmma_tf32_n128(acc, al + o, bh + o);             // small terms first, the dominant Ah.Bh product last
+            wgmma_tf32_n128(acc, ah + o, bl + o);
+            wgmma_tf32_n128(acc, ah + o, bh + o);
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(F_BN >> 3) << 17) | ((uint32_t)(F_BM >> 4) << 24);
-            int it = 0, lt = 0;
-            for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++lt) {
-                const int acc = lt & 1;
-                mbar_wait(&tmem_empty[acc], ((lt >> 1) & 1) ^ 1);      // the epilogue has drained this accumulator
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(acc * F_BN);
-                for (int kb = 0; kb < nk; ++kb, ++it) {
-                    const int s = it % F_STAGES;
-                    mbar_wait(&full[s], (it / F_STAGES) & 1);
-                    tc_fence_after();
-                    const uint32_t base = smem_u32(smem + s * F_STAGE_BYTES);
-                    const uint64_t ah = make_sw128_kmajor_desc(base);
-                    const uint64_t al = make_sw128_kmajor_desc(base + F_A_BYTES);
-                    const uint64_t bh = make_sw128_kmajor_desc(base + 2 * F_A_BYTES);
-                    const uint64_t bl = make_sw128_kmajor_desc(base + 2 * F_A_BYTES + F_B_BYTES);
-#pragma unroll
-                    for (int k4 = 0; k4 < F_BK / 8; ++k4) {
-                        const uint64_t o = (uint64_t)(k4 * 2);
-                        umma_tf32(d_tmem, al + o, bh + o, idesc, (kb | k4) ? 1u : 0u);   // small terms first
-                        umma_tf32(d_tmem, ah + o, bl + o, idesc, 1u);
-                        umma_tf32(d_tmem, ah + o, bh + o, idesc, 1u);
-                    }
-                    umma_commit(&empty[s]);
-                }
-                umma_commit(&tmem_full[acc]);
-            }
-        }
-    } else {
-        const int q = warp & 3;                        // TMEM lane quarter (hardware: warp id mod 4)
-        const int half = (warp - 2) >> 2;              // which 128 columns of the tile
-        int lt = 0;
-        for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++lt) {
-            const int acc = lt & 1;
-            const int tm = m_fastest ? tile % tiles_m : tile / tiles_n, tn = m_fastest ? tile / tiles_m : tile % tiles_n;
-            const int m0 = tm * F_BM, n0 = tn * F_BN + half * 128;
-            const int row = m0 + q * 32 + lane;
-            float v[9];
-            int c[9];
-#pragma unroll
-            for (int i = 0; i < 9; ++i) { v[i] = -INFINITY; c[i] = -1; }
-            mbar_wait(&tmem_full[acc], (lt >> 1) & 1);
-            tc_fence_after();
-#pragma unroll 1
-            for (int cc = 0; cc < 128; cc += 32) {
-                uint32_t r[32];
-                tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * F_BN + half * 128 + cc), r);
-                const int colb = n0 + cc;
-#pragma unroll
-                for (int e = 0; e < 32; ++e) {
-                    const float x = __uint_as_float(r[e]);
-                    if (colb + e < N && x > v[8]) {
-                        v[8] = x; c[8] = colb + e;
-#pragma unroll
-                        for (int i = 8; i > 0; --i) {
-                            if (v[i] > v[i - 1]) {
-                                const float tv = v[i]; v[i] = v[i - 1]; v[i - 1] = tv;
-                                const int tc = c[i]; c[i] = c[i - 1]; c[i - 1] = tc;
-                            }
-                        }
-                    }
-                }
-            }
-            // every TMEM read of this warp is complete (tcgen05.wait::ld inside tmem_ld32): release the accumulator
-            tc_fence_before();
+        wgmma_commit();
+        acc_fence(acc);
+        wgmma_wait<1>();                                      // the previous k-block's MMAs have retired: free its stage
+        if (kb > 0) {
             __syncwarp();
-            if (lane == 0) f_mbar_arrive(&tmem_empty[acc]);
-            if (row < M) {
-                const size_t item = (size_t)row * nhalf + (size_t)(tn * 2 + half);
-                u64 keys[8];
-#pragma unroll
-                for (int i = 0; i < 8; ++i)
-                    keys[i] = c[i] >= 0 ? ((static_cast<u64>(ord_f32(v[i])) << 32) |
-                                           static_cast<u64>(0xFFFFFFFFu - (col_base + (unsigned)c[i])))
-                                        : 0ull;
-                ulonglong2* dst = reinterpret_cast<ulonglong2*>(cand + item * 8);
-#pragma unroll
-                for (int i = 0; i < 4; ++i) dst[i] = make_ulonglong2(keys[2 * i], keys[2 * i + 1]);
-                xbound[item] = c[8] >= 0 ? ord_f32(v[8]) : 0u;
-            }
+            if (lane == 0) mbar_arrive(&empty[(kb - 1) % T_STAGES]);
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, 512);
+    wgmma_wait<0>();
+    acc_fence(acc);
+
+    const int r_lo = cw * 64 + (warp & 3) * 16 + (lane >> 2);   // tile row of acc[4 j + c]; acc[4 j + 2 + c]: r_lo + 8
+    const int c_lo = 2 * (lane & 3);                            // tile column of acc[4 j]: 8 j + c_lo
+    if (!FUSED) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = m0 + r_lo + 8 * h;
+            if (row >= M) continue;
+            float* dst = C + (size_t)row * ldc + n0;
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+                const int col = 8 * j + c_lo;
+                if (n0 + col + 1 < N) *reinterpret_cast<float2*>(dst + col) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+                else if (n0 + col < N) dst[col] = acc[4 * j + 2 * h];
+            }
+        }
+        return;
+    }
+
+    // fused epilogue: both consumer warpgroups are done with the ring -> stage the 128 x 128 tile there.  Every row is
+    // split between the warpgroups: each selects the 9 largest scores of its 64 columns in column order, then the
+    // second half's list (sorted, ties in column order) goes through the same strict-comparison insertion into the
+    // first half's -- the result is exactly that of one sequential pass over the 128 columns.
+    named_sync(1, 256);
+    float* S = reinterpret_cast<float*>(smem);
+#pragma unroll
+    for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            S[(r_lo + 8 * h) * T_LDS + 8 * j + c_lo] = acc[4 * j + 2 * h];
+            S[(r_lo + 8 * h) * T_LDS + 8 * j + c_lo + 1] = acc[4 * j + 2 * h + 1];
+        }
+    named_sync(1, 256);
+    const int r = (int)threadIdx.x & 127;                     // tile row
+    const int half = cw;                                      // columns 64 half .. 64 half + 63
+    const int row = m0 + r;
+    float v[9];
+    int c[9];
+#pragma unroll
+    for (int i = 0; i < 9; ++i) { v[i] = -INFINITY; c[i] = -1; }
+    auto insert = [&](float x, int col) {
+        if (x > v[8]) {
+            v[8] = x; c[8] = col;
+#pragma unroll
+            for (int i = 8; i > 0; --i) {
+                if (v[i] > v[i - 1]) {
+                    const float tv = v[i]; v[i] = v[i - 1]; v[i - 1] = tv;
+                    const int tc = c[i]; c[i] = c[i - 1]; c[i - 1] = tc;
+                }
+            }
+        }
+    };
+    const float* srow = S + r * T_LDS;
+    const int ncol = N - n0 < T_BN ? N - n0 : T_BN;
+    const int e1 = ncol < 64 * (half + 1) ? ncol : 64 * (half + 1);
+#pragma unroll 4
+    for (int e = 64 * half; e < e1; ++e) insert(srow[e], n0 + e);
+    float* hv = S + T_BM * T_LDS;                             // second half's lists: [128][9] scores, [128][9] columns
+    int* hc = reinterpret_cast<int*>(hv + T_BM * 9);
+    if (half == 1) {
+#pragma unroll
+        for (int i = 0; i < 9; ++i) { hv[r * 9 + i] = v[i]; hc[r * 9 + i] = c[i]; }
+    }
+    named_sync(1, 256);
+    if (half == 1 || row >= M) return;
+#pragma unroll
+    for (int i = 0; i < 9; ++i) insert(hv[r * 9 + i], hc[r * 9 + i]);
+    const size_t item = (size_t)row * nhalf + (size_t)tn;
+    u64 keys[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+        keys[i] = c[i] >= 0 ? ((static_cast<u64>(ord_f32(v[i])) << 32) | static_cast<u64>(0xFFFFFFFFu - (col_base + (unsigned)c[i])))
+                            : 0ull;
+    ulonglong2* dst = reinterpret_cast<ulonglong2*>(cand + item * 8);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) dst[i] = make_ulonglong2(keys[2 * i], keys[2 * i + 1]);
+    xbound[item] = c[8] >= 0 ? ord_f32(v[8]) : 0u;
 }
 
-// candidates kept per row per call: 8 per 128-column half tile
-size_t fused_cand_per_row(int N) { return (size_t)((N + F_BN - 1) / F_BN) * 2 * 8; }
+static bool make_maps(CUtensorMap (&m)[4], const float* Ah, const float* Al, int M, const float* Bh, const float* Bl, int N, int K) {
+    return make_map_2d(&m[0], Ah, (uint64_t)M, (uint64_t)K, T_BM, 4) && make_map_2d(&m[1], Al, (uint64_t)M, (uint64_t)K, T_BM, 4) &&
+           make_map_2d(&m[2], Bh, (uint64_t)N, (uint64_t)K, T_BN, 4) && make_map_2d(&m[3], Bl, (uint64_t)N, (uint64_t)K, T_BN, 4);
+}
+
+// candidates kept per row per call: 8 per 128-column tile, counted in pairs of tiles (256 columns)
+size_t fused_cand_per_row(int N) { return (size_t)((N + 255) / 256) * 2 * 8; }
 
 // Ah/Al [M,K], Bh/Bl [N,K] fp32 (already split).  cand [M, fused_cand_per_row(N)] u64 keys (score order high word,
 // 0xFFFFFFFF - (col_base + column) low word, 0 = empty), xbound [M, fused_cand_per_row(N) / 8] (ordered score of the
-// best dropped element of each half tile, 0 = none).  Returns false if the path cannot run (caller falls back).
+// best dropped element of each 128-column tile, 0 = none).  Returns false if the path cannot run (caller falls back).
 bool launch_gemm_tf32x3_topt(const float* Ah, const float* Al, int M, const float* Bh, const float* Bl, int N, int K,
                              unsigned col_base, u64* cand, unsigned* xbound, cudaStream_t st) {
     if (M <= 0 || N <= 0) return true;
-    if (K % F_BK) return false;
-    CUtensorMap mAh, mAl, mBh, mBl;
-    if (!make_map_2d(&mAh, Ah, (uint64_t)M, (uint64_t)K, F_BM, 4) || !make_map_2d(&mAl, Al, (uint64_t)M, (uint64_t)K, F_BM, 4) ||
-        !make_map_2d(&mBh, Bh, (uint64_t)N, (uint64_t)K, F_BN, 4) || !make_map_2d(&mBl, Bl, (uint64_t)N, (uint64_t)K, F_BN, 4))
-        return false;
+    if (K % T_BK) return false;
+    CUtensorMap m[4];
+    if (!make_maps(m, Ah, Al, M, Bh, Bl, N, K)) return false;
     static PerDeviceSize configured;
-    if (configured.raise(F_SMEM))
-        cudaFuncSetAttribute(gemm_tf32x3_topt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, F_SMEM);
-    const int ntiles = ((M + F_BM - 1) / F_BM) * ((N + F_BN - 1) / F_BN);
-    const int grid = ntiles < device_num_sms() ? ntiles : device_num_sms();
+    if (configured.raise(T_SMEM))
+        cudaFuncSetAttribute(gemm_tf32x3_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, T_SMEM);
+    const int ntiles = ((M + T_BM - 1) / T_BM) * (int)(fused_cand_per_row(N) / 8);
     static const int m_fastest = getenv("RSB_COARSE_N_FASTEST") ? 0 : 1;
-    gemm_tf32x3_topt_kernel<<<grid, F_THREADS, F_SMEM, st>>>(mAh, mAl, mBh, mBl, cand, xbound, M, N, K, col_base, m_fastest);
+    gemm_tf32x3_kernel<true><<<ntiles, T_THREADS, T_SMEM, st>>>(m[0], m[1], m[2], m[3], nullptr, 0, cand, xbound, M, N, K,
+                                                                 col_base, m_fastest);
     return true;
 }
 
@@ -344,15 +259,13 @@ bool launch_gemm_tf32x3(const float* Ah, const float* Al, int M, const float* Bh
                         float* C, int ldc, cudaStream_t st) {
     if (M <= 0 || N <= 0) return true;
     if (K % T_BK) return false;
-    CUtensorMap mAh, mAl, mBh, mBl;
-    if (!make_map_2d(&mAh, Ah, (uint64_t)M, (uint64_t)K, T_BM, 4) || !make_map_2d(&mAl, Al, (uint64_t)M, (uint64_t)K, T_BM, 4) ||
-        !make_map_2d(&mBh, Bh, (uint64_t)N, (uint64_t)K, T_BN, 4) || !make_map_2d(&mBl, Bl, (uint64_t)N, (uint64_t)K, T_BN, 4))
-        return false;
+    CUtensorMap m[4];
+    if (!make_maps(m, Ah, Al, M, Bh, Bl, N, K)) return false;
     static PerDeviceSize configured;
     if (configured.raise(T_SMEM))
-        cudaFuncSetAttribute(gemm_tf32x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, T_SMEM);
+        cudaFuncSetAttribute(gemm_tf32x3_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, T_SMEM);
     dim3 grid((N + T_BN - 1) / T_BN, (M + T_BM - 1) / T_BM);
-    gemm_tf32x3_kernel<<<grid, T_THREADS, T_SMEM, st>>>(mAh, mAl, mBh, mBl, C, ldc, M, N, K);
+    gemm_tf32x3_kernel<false><<<grid, T_THREADS, T_SMEM, st>>>(m[0], m[1], m[2], m[3], C, ldc, nullptr, nullptr, M, N, K, 0u, 0);
     return true;
 }
 

@@ -43,7 +43,7 @@ def embed_passages(args, passages: Iterable[dict], model, tokenizer) -> Tuple[li
     CLS row (reference :66-79)."""
     name = str(args.model_name_or_path)
     if any(t in name for t in _UNSUPPORTED):
-        raise AttributeError(f"{name}: this encoder family is out of scope of the B200 hot path "
+        raise AttributeError(f"{name}: this encoder family is out of scope of the GPU hot path "
                              f"(BERT-architecture Contriever / dragon checkpoints only)")
     from . import search as _search                      # device is resolved there (tests patch it)
     bs = int(args.per_gpu_batch_size)
@@ -110,7 +110,7 @@ def load_passage_shard(args, shard_id: int) -> List[dict]:
     if not os.path.exists(path):
         raise NotImplementedError(
             f"{path} not found: chunking raw text into passages (src/data.py::fast_load_jsonl_shard) is CPU text "
-            f"processing outside the B200 hot path; produce the passage shards with the reference, then embed here")
+            f"processing outside the GPU hot path; produce the passage shards with the reference, then embed here")
     with open(path, "r", encoding="utf-8") as f:
         return [json.loads(line) for line in f if line.strip()]
 

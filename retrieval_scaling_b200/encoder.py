@@ -1,10 +1,10 @@
-"""B200 query encoder with the reference's call protocol (`src/search.py:239-258,83-96`):
+"""GPU query encoder with the reference's call protocol (`src/search.py:239-258,83-96`):
 
     model, tokenizer, _ = load_retriever(name)            # contriever/src/contriever.py:103-138
     model.eval().to(device).half()                        # no-ops here: the CUDA path is always fp16 / inference
     emb = model(input_ids=..., attention_mask=..., token_type_ids=...)   # -> Tensor[B, 768] fp16
 
-The forward pass is librsb's `rsb_bert_forward` (tcgen05 tensor-core GEMMs fed by TMA with fused bias / GELU /
+The forward pass is librsb's `rsb_bert_forward` (wgmma tensor-core GEMMs fed by TMA with fused bias / GELU /
 residual epilogues, fused embedding+LayerNorm, shared-memory attention, mean / CLS pooling) on the un-padded
 token stream.  No CPU / eager-PyTorch fallback: constructing the model without CUDA raises.
 """
@@ -48,7 +48,7 @@ class B200Contriever:
 
     def __init__(self, config=None, pooling: str = "average", device=None):
         if not torch.cuda.is_available():
-            raise RuntimeError("B200Contriever needs a CUDA device (sm_100a): there is no CPU path")
+            raise RuntimeError("B200Contriever needs a CUDA device (sm_90a): there is no CPU path")
         if pooling not in ("average", "cls"):
             raise ValueError(f"unknown pooling {pooling!r}")
         self.L = _lib.lib()
@@ -249,7 +249,7 @@ def read_retriever_files(model_path: str, tokenizer_name: Optional[str] = None):
         hf = load_hf(transformers.AutoModel, model_path)
         sd = strip_wrapper_prefix(hf.state_dict())
     if getattr(cfg, "model_type", "bert") != "bert":
-        raise AttributeError(f"{model_path}: only BERT-architecture encoders run on the B200 path")
+        raise AttributeError(f"{model_path}: only BERT-architecture encoders run on the GPU path")
     return sd, cfg, tokenizer, model_id
 
 
@@ -264,7 +264,7 @@ def load_retriever(model_path: str, tokenizer_name: Optional[str] = None, poolin
     sd, cfg, tokenizer, model_id = read_retriever_files(model_path, tokenizer_name)
     if not fp16:
         import warnings
-        warnings.warn("no_fp16 / fp16=False was requested, but the B200 encoder computes in fp16 with fp32 accumulation "
+        warnings.warn("no_fp16 / fp16=False was requested, but the encoder computes in fp16 with fp32 accumulation "
                       "only (the reference's default path, src/search.py:257-258); continuing in fp16")
     model = B200Contriever(cfg, pooling)
     model.load_state_dict(sd, strict=False)

@@ -1,11 +1,11 @@
-"""B200 index objects exposing the faiss object protocol the reference's wrappers use
+"""GPU index objects exposing the faiss object protocol the reference's wrappers use
 (`src/indicies/flat.py:42,58,139`, `ivf_flat.py:73,143-149,166,171,180,225`, `ivf_pq.py:76,146-154,170,185,230`):
 
     index.train(x) / index.add(x) / index.search(x, k) -> (D float32 [nq,k], I int64 [nq,k])
     index.nprobe, index.ntotal, index.is_trained, index.d
     write_index(index, path) / read_index(path)
 
-All numerics run in librsb.so (hand-written sm_100a CUDA, C-ABI `include/rsb.h`); torch is used for device
+All numerics run in librsb.so (hand-written sm_90a CUDA, C-ABI `include/rsb.h`); torch is used for device
 memory and streams only.  No CPU fallback: constructing an index without a CUDA device raises.
 
 Inputs may be numpy arrays (any float dtype; upcast to fp32 like `query_embs.astype(np.float32)` in
@@ -30,7 +30,7 @@ NEG = float(np.finfo(np.float32).min)
 
 def _require_cuda():
     if not torch.cuda.is_available():
-        raise RuntimeError("retrieval_scaling_b200 needs a CUDA device (B200, sm_100a): there is no CPU path")
+        raise RuntimeError("retrieval_scaling_b200 needs a CUDA device (H100, sm_90a): there is no CPU path")
 
 
 def _dev_f32(x, device) -> torch.Tensor:

@@ -43,15 +43,15 @@ def embed_queries(args, queries, model, tokenizer, model_name_or_path):
     `question_maxlength`; Contriever models mean-pool inside the model, other HF BERT checkpoints (dragon*)
     take the CLS row (`output.last_hidden_state[:, 0, :]`, reference :93-94)."""
     if any(t in model_name_or_path for t in ("sentence-transformers", "e5", "Qwen3", "drama", "ReasonIR", "GRIT")):
-        raise AttributeError(f"{model_name_or_path}: this encoder family is out of scope of the B200 hot path "
+        raise AttributeError(f"{model_name_or_path}: this encoder family is out of scope of the GPU hot path "
                              f"(BERT-architecture Contriever / dragon checkpoints only)")
     if hasattr(model, "eval"):
         model.eval()
     embeddings, batch = [], []
     bs = int(args.per_gpu_batch_size)
-    # The B200 encoder works on the un-padded token stream, so a sequence's embedding does not depend on what else
+    # The encoder works on the un-padded token stream, so a sequence's embedding does not depend on what else
     # is in its batch: several reference-sized batches (default 64) are encoded in one forward (`encode_group`,
-    # 2048 sequences: 3.5x the throughput of batch 64, see profiles/) and nothing is copied to the host until the end.
+    # 2048 sequences, see bench.py's encoder block) and nothing is copied to the host until the end.
     group = max(bs, int(getattr(model, "encode_group", bs)) // bs * bs)
     lowercase = bool(args.get("lowercase", False)) if hasattr(args, "get") else False
     normalize = bool(args.get("normalize_text", False)) if hasattr(args, "get") else False
@@ -412,5 +412,5 @@ def post_hoc_merge_topk(cfg):
 
 def search_topk(cfg):
     if cfg.model.get("sparse_retriever", None):
-        raise NotImplementedError("BM25 / pyserini search is outside the B200 hot path (SURVEY §2 #10)")
+        raise NotImplementedError("BM25 / pyserini search is outside the GPU hot path (SURVEY §2 #10)")
     search_dense_topk(cfg)

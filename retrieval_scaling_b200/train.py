@@ -8,7 +8,7 @@ product through the IndexFlatIP quantizer); PQ sub-quantizers: L2 k-means, ksub=
 most 256*ksub points.  Parity is defined *given* the trained centroids / codebooks (SURVEY §8a row a10).
 
 The Lloyd iterations are driven from here; the arithmetic of every step runs in librsb (`LibrsbOps`):
-  assignment (coarse)  : the coarse quantizer itself -- fused 3xTF32 tcgen05 scorer + exact fp32 re-score (rsb_coarse on a
+  assignment (coarse)  : the coarse quantizer itself -- fused 3xTF32 wgmma scorer + exact fp32 re-score (rsb_coarse on a
                          scratch handle holding the current centroids) -> fp32-exact argmax
   assignment (PQ)      : rsb_pq_assign (the residual-encoding kernel without the residual step)
   update               : rsb_kmeans_accumulate / rsb_pq_accumulate (member sums and counts)
@@ -35,7 +35,7 @@ class LibrsbOps:
 
     def __init__(self):
         if not torch.cuda.is_available():
-            raise RuntimeError("index training runs on librsb's CUDA kernels: a CUDA device (B200, sm_100a) is required")
+            raise RuntimeError("index training runs on librsb's CUDA kernels: a CUDA device (H100, sm_90a) is required")
         self._scratch = {}
 
     @staticmethod

@@ -6,7 +6,7 @@
 Hydra / OmegaConf are replaced by `retrieval_scaling_b200.config` (same YAML files, same dotted overrides).
 Task switches: tasks.datastore.embedding (already-chunked passage shards -> embedding pickles, SURVEY §8f-4),
 tasks.datastore.index (build or load the index), tasks.eval.search (query -> top-k, the hot path).
-tasks.eval.merge_search and tasks.eval.inference belong to subsystems that are out of scope of the B200 hot path
+tasks.eval.merge_search and tasks.eval.inference belong to subsystems that are out of scope of the GPU hot path
 (SURVEY.md §2) and raise NotImplementedError.
 """
 import logging

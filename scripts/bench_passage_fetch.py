@@ -2,7 +2,7 @@
 """SURVEY §8f-2 on the host: materialising nq x k passages.  Times the reference's per-passage way (`_id2psg`,
 src/indicies/ivf_pq.py:209-214: open(), seek(), readline(), json.loads() for every (query, rank)) restated here against
 `index_utils.fetch_passages` (group by file, sort by offset, one open() per file) on synthetic passage shards.
-    python scripts/bench_passage_fetch.py > profiles/r02_passage_fetch.txt"""
+    python scripts/bench_passage_fetch.py"""
 import json
 import os
 import sys

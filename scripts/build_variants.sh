@@ -6,7 +6,7 @@ set -e
 cd "$(dirname "$0")/.."
 OUT=retrieval_scaling_b200/_variants
 mkdir -p "$OUT"
-FLAGS="-O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -lineinfo -Xcompiler -fPIC --expt-relaxed-constexpr"
+FLAGS="-O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -lineinfo -Xcompiler -fPIC --expt-relaxed-constexpr"
 while [ $# -ge 2 ]; do
   NAME=$1; DEFS=$2; shift 2
   TMP=$(mktemp -d)

@@ -1,8 +1,8 @@
 """Generates tests/golden/encoder_*.npz by running the REFERENCE's own class
-(`contriever.src.contriever.Contriever`, /root/reference/contriever/src/contriever.py:11-55) on seeded weights and
-fixed token batches.  Run in the build container only (needs /root/reference):
+(`contriever.src.contriever.Contriever`, contriever/src/contriever.py:11-55 of the reference checkout) on seeded weights
+and fixed token batches.  Needs a checkout of the reference project, named by REFERENCE_ROOT:
 
-    PYTHONPATH=/root/reference:/root/repo python tests/golden/make_encoder_golden.py
+    REFERENCE_ROOT=<reference checkout> python tests/golden/make_encoder_golden.py
 """
 import os
 import sys
@@ -10,7 +10,7 @@ import sys
 import numpy as np
 import torch
 
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, os.environ["REFERENCE_ROOT"])
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 
 from transformers import BertConfig  # noqa: E402

@@ -1,20 +1,20 @@
 """Generates tests/golden/normalize_text_golden.json from the reference's own function
-(`/root/reference/contriever/src/normalize_text.py::normalize`).  Run in the build container only (the reference
-tree does not exist on the GPU box); the fixture it writes is what the tests read.
+(`contriever/src/normalize_text.py::normalize` of the reference checkout named by REFERENCE_ROOT); the fixture it
+writes is what the tests read, so the tests need no reference checkout.
 
-  python tests/golden/make_normalize_golden.py
+  REFERENCE_ROOT=<reference checkout> python tests/golden/make_normalize_golden.py
 """
 import importlib.util
 import json
 import os
 import random
 
-REF = "/root/reference/contriever/src/normalize_text.py"
+REL = "contriever/src/normalize_text.py"
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 def main():
-    spec = importlib.util.spec_from_file_location("ref_normalize_text", REF)
+    spec = importlib.util.spec_from_file_location("ref_normalize_text", os.path.join(os.environ["REFERENCE_ROOT"], REL))
     mod = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(mod)
     # (1) every code point the reference changes, as {codepoint: replacement}
@@ -35,7 +35,7 @@ def main():
         strings.append("".join(rng.choice(pool) for _ in range(rng.randint(1, 40))))
     cases = [[s, mod.normalize(s)] for s in strings]
     with open(os.path.join(HERE, "normalize_text_golden.json"), "w", encoding="utf-8") as f:
-        json.dump({"source": REF, "changed_codepoints": changed, "cases": cases}, f, ensure_ascii=True, indent=0)
+        json.dump({"source": REL, "changed_codepoints": changed, "cases": cases}, f, ensure_ascii=True, indent=0)
     print(f"{len(changed)} changed code points, {len(cases)} string cases")
 
 

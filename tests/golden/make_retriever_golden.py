@@ -1,8 +1,9 @@
 """Generates tests/golden/retriever_ckpt.npz with the REFERENCE's own loader and model
-(`contriever.src.contriever.load_retriever`, /root/reference/contriever/src/contriever.py:103-138) on the deterministic
-checkpoint directory of retriever_fixture.py.  Run in the build container only (needs /root/reference):
+(`contriever.src.contriever.load_retriever`, contriever/src/contriever.py:103-138 of the reference checkout) on the
+deterministic checkpoint directory of retriever_fixture.py.  Needs a checkout of the reference project, named by
+REFERENCE_ROOT:
 
-    PYTHONPATH=/root/reference:/root/repo python tests/golden/make_retriever_golden.py
+    REFERENCE_ROOT=<reference checkout> python tests/golden/make_retriever_golden.py
 """
 import os
 import sys
@@ -11,7 +12,7 @@ import tempfile
 import numpy as np
 import torch
 
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, os.environ["REFERENCE_ROOT"])
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))

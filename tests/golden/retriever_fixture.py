@@ -8,7 +8,7 @@
 
 Weights come from `oracle.bert_oracle.seeded_state_dict` (CPU generator: identical on every machine), so the golden
 embeddings committed in tests/golden/retriever_ckpt.npz -- produced by the REFERENCE's `load_retriever` on exactly
-this directory (make_retriever_golden.py) -- are valid on the GPU box, where /root/reference does not exist."""
+this directory (make_retriever_golden.py) -- hold on any machine, without a reference checkout."""
 import argparse
 import json
 import os

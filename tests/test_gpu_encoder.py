@@ -1,4 +1,5 @@
-"""GPU parity of the query encoder: tcgen05/TMA GEMM against torch.matmul, and the full BERT forward against
+"""GPU parity of the query encoder: the tensor-core (wgmma/TMA) GEMM against torch.matmul (the test keeps the name of
+the tcgen05 kernel it was written for), and the full BERT forward against
 (a) golden outputs of the reference's own Contriever class and (b) the torch oracle run in fp16 on the GPU
 (the like-for-like of `query_encoder.half()`, src/search.py:257-258).  Tolerances: cosine >= 0.9999 and
 max |err| within fp16 noise (SURVEY.md App. C.4)."""

@@ -132,7 +132,7 @@ class _HashTokenizer:
 
 
 def test_datastore_api_encode_and_search(tmp_path):
-    """text -> B200 encoder -> Indexer.search through the reference's DatastoreAPI surface (api/api_index.py:21-67)."""
+    """text -> GPU encoder -> Indexer.search through the reference's DatastoreAPI surface (api/api_index.py:21-67)."""
     import torch
     from oracle import bert_oracle as BO
     from retrieval_scaling_b200.api_index import DatastoreAPI

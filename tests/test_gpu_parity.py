@@ -239,7 +239,7 @@ def test_ivfpq_matches_oracle(d, M, nlist, nprobe, k, n, nq):
 
 
 def test_tensor_core_coarse_matches_cuda_core_coarse():
-    """3xTF32 (tcgen05) coarse quantizer == fp32 CUDA-core coarse quantizer == oracle, on a C3-shaped problem."""
+    """3xTF32 (wgmma) coarse quantizer == fp32 CUDA-core coarse quantizer == oracle, on a C3-shaped problem."""
     r = _rsb()
     rng = np.random.default_rng(29)
     d, nlist, nq, nprobe = 768, 1000, 300, 32
@@ -493,3 +493,43 @@ def test_host_pipeline_overlapped_transfers_return_the_same_rows():
     for qh, (Ih, Dh) in zip(batches, outs):
         I, D = index.search_ids(qh.cuda(), k)
         assert torch.equal(Ih, I.cpu()) and torch.equal(Dh, D.cpu())
+
+
+# ------------------------------------------------------------------------------------------------------------
+# training: member sums are reproducible (fixed summation order), so index.train gives the same index every run
+# ------------------------------------------------------------------------------------------------------------
+def test_training_sums_match_float64_and_are_reproducible():
+    from retrieval_scaling_b200 import train
+    ops = train.default_ops()
+    g = torch.Generator(device="cuda").manual_seed(11)
+    n, d, k, M = 20000, 96, 300, 8
+    x = torch.randn(n, d, generator=g, device="cuda")
+    a = torch.randint(-1, k + 1, (n,), generator=g, device="cuda")          # -1 and k: out of range, ignored
+    sums, counts = ops.accumulate(x, a, k)
+    an, xn = a.cpu().numpy(), x.cpu().numpy().astype(np.float64)
+    ok = (an >= 0) & (an < k)
+    ref = np.zeros((k, d))
+    np.add.at(ref, an[ok], xn[ok])
+    assert np.array_equal(counts.cpu().numpy(), np.bincount(an[ok], minlength=k).astype(np.float32))
+    assert np.abs(sums.cpu().numpy() - ref).max() < 1e-4
+    for _ in range(3):
+        s2, c2 = ops.accumulate(x, a, k)
+        assert torch.equal(s2, sums) and torch.equal(c2, counts)
+
+    codes = torch.randint(0, 256, (n, M), generator=g, device="cuda", dtype=torch.uint8)
+    psums, pcounts = ops.pq_accumulate(x, codes, M, 256)
+    cn = codes.cpu().numpy().astype(np.int64)
+    dsub = d // M
+    pref = np.zeros((M, 256, dsub))
+    for m in range(M):
+        np.add.at(pref[m], cn[:, m], xn[:, m * dsub:(m + 1) * dsub])
+        assert np.array_equal(pcounts[m].cpu().numpy(), np.bincount(cn[:, m], minlength=256).astype(np.float32))
+    assert np.abs(psums.cpu().numpy() - pref).max() < 1e-4
+    s2, c2 = ops.pq_accumulate(x, codes, M, 256)
+    assert torch.equal(s2, psums) and torch.equal(c2, pcounts)
+
+    xs = torch.nn.functional.normalize(x, dim=1)
+    c1 = train.kmeans(xs, 64, niter=5, metric="ip", spherical=True, seed=3)
+    assert torch.equal(c1, train.kmeans(xs, 64, niter=5, metric="ip", spherical=True, seed=3))
+    cb1 = train.train_pq(x, M, 256, niter=4, seed=3)
+    assert torch.equal(cb1, train.train_pq(x, M, 256, niter=4, seed=3))
