@@ -138,6 +138,25 @@ int rsb_peer_broadcast(const void* src_dev, size_t bytes, void* const* dst_ptrs_
 int rsb_coarse(rsb_index_t* h, const float* q_dev, int nq, int nprobe, int64_t* list_dev, float* score_dev,
                void* ws_dev, size_t ws_bytes, rsb_stream_t stream);
 
+/* ---- exact re-ranking (faiss IndexRefine / IndexRefineFlat::search; the reference's unused re-score path
+ *      src/indicies/ivf_pq.py:119-123 `get_knn_scores` against `self.embeds`) ------------------------------------
+ * The re-rank store is caller-owned device memory [ntotal, d], row i = the vector of index id i, in fp32 or fp16
+ * (16-byte aligned, d % 8 == 0).  Scores are <q, x_id> accumulated in fp32 from the decoded elements, in the same
+ * order for both types (an fp16 store and an fp32 store of the same fp16-representable values agree bit for bit).  Rows are sorted by score descending, ties by ascending id; fewer than k valid candidates are
+ * padded with id -1 / score -FLT_MAX; candidate ids -1 (and ids outside [0, ntotal)) are skipped.
+ * k_base = k * k_factor <= 4096 (the scan's k limit); larger returns RSB_ERR_UNSUPPORTED.  ntotal <= 2^31. */
+enum { RSB_DTYPE_F32 = 0, RSB_DTYPE_F16 = 1 };
+size_t rsb_refine_workspace_bytes(int nq, int k_base, int k);
+/* re-rank given candidates cand_dev [nq, k_base] int64 (e.g. a search result at k_base) -> D_dev/I_dev [nq, k] */
+int rsb_refine(const float* q_dev, int nq, const void* store_dev, int store_dtype, int d, int64_t ntotal,
+               const int64_t* cand_dev, int k_base, int k, float* D_dev, int64_t* I_dev, void* ws_dev, size_t ws_bytes,
+               rsb_stream_t stream);
+/* IndexRefine::search on an IVFPQ handle: rsb_search at k_base = k * k_factor into the workspace, then rsb_refine */
+size_t rsb_search_refine_workspace_bytes(rsb_index_t* h, int nq, int k, int k_factor, int nprobe);
+int rsb_search_refine(rsb_index_t* h, const float* q_dev, int nq, int k, int k_factor, int nprobe, const void* store_dev,
+                      int store_dtype, int64_t ntotal, float* D_dev, int64_t* I_dev, void* ws_dev, size_t ws_bytes,
+                      rsb_stream_t stream);
+
 /* ---- shard merge (src/search.py:357-367; api/serve_main_node.py:130-163) ---------------------------- */
 /* D_all_dev/I_all_dev [nshards, nq, k]: concat per query, sort by score desc (ties: lower shard, then lower
  * rank, i.e. Python's stable sort over shard order), keep k_out.  Entries with id < 0 are ignored. */

@@ -954,6 +954,97 @@ extern "C" int rsb_search_preassigned_shared(rsb_index_t* h, const float* q, int
     return search_impl(h, q, nq, k, nprobe, list_dev, coarse_dis_dev, D, I, ws, ws_bytes, stream, &sh);
 }
 
+// ---- exact re-ranking (faiss IndexRefine::search) -----------------------------------------------------------
+static int refine_check(const void* store, int store_dtype, int d, int64_t ntotal, int k_base, int k) {
+    if (store_dtype != RSB_DTYPE_F32 && store_dtype != RSB_DTYPE_F16)
+        return fail(RSB_ERR_INVALID, "store_dtype must be RSB_DTYPE_F32 or RSB_DTYPE_F16, got %d", store_dtype);
+    if (k <= 0 || k_base < k) return fail(RSB_ERR_INVALID, "need 0 < k <= k_base, got k = %d, k_base = %d", k, k_base);
+    if (k_base > 4096) return fail(RSB_ERR_UNSUPPORTED, "k_base = k * k_factor = %d > 4096 is not supported", k_base);
+    if (ntotal < 0 || ntotal > ((int64_t)1 << 31)) return fail(RSB_ERR_INVALID, "store rows must be in [0, 2^31], got %lld", (long long)ntotal);
+    if (d <= 0 || d % 8) return fail(RSB_ERR_INVALID, "d = %d must be a positive multiple of 8 for the re-rank store", d);
+    if (ntotal > 0 && (!store || (reinterpret_cast<uintptr_t>(store) & 15)))
+        return fail(RSB_ERR_INVALID, "the re-rank store must be a 16-byte aligned device pointer");
+    return RSB_OK;
+}
+
+static int refine_impl(const float* q, int nq, const void* store, int store_dtype, int d, int64_t ntotal, const int64_t* cand,
+                       int k_base, int k, float* D, int64_t* I, void* ws, size_t ws_bytes, cudaStream_t st) {
+    const RefinePlan p = refine_plan(nq, k_base, k);
+    if (ws_bytes < p.ws_bytes) return fail(RSB_ERR_OOM, "workspace too small: need %zu bytes, got %zu", p.ws_bytes, ws_bytes);
+    if (launch_refine_rows(p, q, nq, store, store_dtype == RSB_DTYPE_F16 ? 2 : 4, d, ntotal, cand, k_base, k, D, I, ws, st) != 0)
+        return fail(RSB_ERR_UNSUPPORTED, "d = %d with k_base = %d needs more shared memory than the re-rank kernel has", d, k_base);
+    CHECK_LAUNCH();
+    return RSB_OK;
+}
+
+extern "C" size_t rsb_refine_workspace_bytes(int nq, int k_base, int k) {
+    if (nq <= 0 || k <= 0 || k_base < k) return 0;
+    return refine_plan(nq, k_base, k).ws_bytes;
+}
+
+extern "C" int rsb_refine(const float* q, int nq, const void* store, int store_dtype, int d, int64_t ntotal,
+                          const int64_t* cand, int k_base, int k, float* D, int64_t* I, void* ws, size_t ws_bytes,
+                          rsb_stream_t stream) {
+    RSB_TRY(refine_check(store, store_dtype, d, ntotal, k_base, k));
+    if (nq < 0) return fail(RSB_ERR_INVALID, "bad nq = %d", nq);
+    if (nq == 0) return RSB_OK;
+    if (!q || !cand || !D || !I) return fail(RSB_ERR_INVALID, "null argument");
+    return refine_impl(q, nq, store, store_dtype, d, ntotal, cand, k_base, k, D, I, ws, ws_bytes, (cudaStream_t)stream);
+}
+
+// Queries are processed in batches of qb: base search at k_base into [qb, k_base] candidate buffers, then the re-rank.
+struct SearchRefinePlan {
+    int qb;
+    size_t search_ws, off_D, off_I, off_ref, total;
+};
+static SearchRefinePlan search_refine_plan(rsb_index* h, int nq, int k, int k_base, int nprobe) {
+    SearchRefinePlan p;
+    nq = std::max(nq, 1);
+    p.qb = std::min(nq, 16384);
+    const int last = nq % p.qb ? nq % p.qb : p.qb;     // the last batch may split its queries into more chunks
+    p.search_ws = align_up(rsb_workspace_bytes(h, p.qb, k_base, nprobe));
+    p.off_D = p.search_ws;
+    p.off_I = p.off_D + align_up((size_t)p.qb * k_base * 4);
+    p.off_ref = p.off_I + align_up((size_t)p.qb * k_base * 8);
+    p.total = p.off_ref + align_up(std::max(refine_plan(p.qb, k_base, k).ws_bytes, refine_plan(last, k_base, k).ws_bytes));
+    return p;
+}
+
+extern "C" size_t rsb_search_refine_workspace_bytes(rsb_index_t* h, int nq, int k, int k_factor, int nprobe) {
+    if (!h || k <= 0 || k_factor <= 0) return 0;
+    return search_refine_plan(h, nq, k, k * k_factor, nprobe).total;
+}
+
+extern "C" int rsb_search_refine(rsb_index_t* h, const float* q, int nq, int k, int k_factor, int nprobe, const void* store,
+                                 int store_dtype, int64_t ntotal, float* D, int64_t* I, void* ws, size_t ws_bytes,
+                                 rsb_stream_t stream) {
+    if (!h) return fail(RSB_ERR_INVALID, "null handle");
+    if (h->kind != RSB_IVFPQ) return fail(RSB_ERR_INVALID, "re-ranking is for IVFPQ indexes: Flat / IVFFlat scores are already exact");
+    if (k <= 0 || k_factor <= 0) return fail(RSB_ERR_INVALID, "bad k = %d / k_factor = %d", k, k_factor);
+    if ((int64_t)k * k_factor > 4096) return fail(RSB_ERR_UNSUPPORTED, "k * k_factor = %lld > 4096 is not supported", (long long)k * k_factor);
+    const int k_base = k * k_factor;
+    RSB_TRY(refine_check(store, store_dtype, h->d, ntotal, k_base, k));
+    if (ntotal != h->ntotal + h->n_staged)
+        return fail(RSB_ERR_INVALID, "the re-rank store has %lld rows, the index holds %lld vectors", (long long)ntotal,
+                    (long long)(h->ntotal + h->n_staged));
+    if (nq < 0) return fail(RSB_ERR_INVALID, "bad nq = %d", nq);
+    if (nq == 0) return RSB_OK;
+    if (!q || !D || !I) return fail(RSB_ERR_INVALID, "null argument");
+    const SearchRefinePlan p = search_refine_plan(h, nq, k, k_base, nprobe);
+    if (ws_bytes < p.total) return fail(RSB_ERR_OOM, "workspace too small: need %zu bytes, got %zu", p.total, ws_bytes);
+    unsigned char* w = static_cast<unsigned char*>(ws);
+    float* Db = reinterpret_cast<float*>(w + p.off_D);
+    int64_t* Ib = reinterpret_cast<int64_t*>(w + p.off_I);
+    for (int q0 = 0; q0 < nq; q0 += p.qb) {
+        const int nb = std::min(p.qb, nq - q0);
+        const float* qb = q + (size_t)q0 * h->d;
+        RSB_TRY(rsb_search(h, qb, nb, k_base, nprobe, Db, Ib, w, p.search_ws, stream));
+        RSB_TRY(refine_impl(qb, nb, store, store_dtype, h->d, ntotal, Ib, k_base, k, D + (size_t)q0 * k, I + (size_t)q0 * k,
+                            w + p.off_ref, p.total - p.off_ref, (cudaStream_t)stream));
+    }
+    return RSB_OK;
+}
+
 // ---- training steps (index.train) ---------------------------------------------------------------------------
 extern "C" int rsb_kmeans_accumulate(const float* x, int64_t n, int d, const int32_t* assign, int k, float* sums,
                                      float* counts, rsb_stream_t stream) {

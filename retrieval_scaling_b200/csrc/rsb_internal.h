@@ -64,6 +64,21 @@ int launch_merge_shards_peers_scatter(const float* const* D_ptrs, const int64_t*
                                       int nq_slice, int k, int k_out, float* const* D_outs, int64_t* const* I_outs,
                                       int nout, cudaStream_t st);
 
+// ---- rsb_refine.cu (exact re-ranking of candidates against a re-rank store) -------------------------------
+struct RefinePlan {
+    int nchunks;          // CTAs per query
+    int chunk;            // candidates per CTA
+    int P;                // sort width (power of two >= chunk)
+    int k_item;           // keys a CTA hands to the merge (nchunks > 1)
+    size_t ws_bytes;      // partial keys + counts (0 when nchunks == 1)
+};
+RefinePlan refine_plan(int nq, int k_base, int k);
+// X: store [ntotal, d], elem_bytes 2 (fp16) or 4 (fp32); cand [nq, k_base] ids (-1 = skip); returns <0 if the shared
+// memory the kernel needs (P * 8 + d * 4 bytes) exceeds 200 KB
+int launch_refine_rows(const RefinePlan& p, const float* Q, int nq, const void* X, int elem_bytes, int d,
+                       int64_t ntotal, const int64_t* cand, int k_base, int k, float* D, int64_t* I, void* ws,
+                       cudaStream_t st);
+
 // ---- rsb_tf32.cu (tensor-core fp32-accurate scores: 3xTF32 on wgmma) ---------------------------------
 bool tf32_path_available();
 void launch_split_tf32(const float* x, size_t n, float* hi, float* lo, cudaStream_t st);

@@ -170,6 +170,11 @@ class ShardedSearcher:
                  search_fn: Optional[Callable] = None, merge_fn: Optional[Callable] = None,
                  shard_coarse: bool = True, fused_gather: bool = True, sliced_merge: bool = True,
                  share_tau: bool = True, peer_coarse: bool = True):
+        from .index import IndexRefine
+        if isinstance(index, IndexRefine) and int(world) > 1:
+            raise NotImplementedError("ShardedSearcher partitions one index over the GPUs; re-ranking would need the "
+                                      "candidates' store rows from peer GPUs, which is not implemented.  Re-rank per "
+                                      "shard group instead (search.GroupSearcher) or search on one GPU")
         self.sliced_merge = bool(sliced_merge)
         # with the fused (symmetric-memory) gather: exchange the running top-k thresholds between the GPUs during the
         # scan, and publish the sharded coarse tables with P2P stores instead of NCCL all-gathers

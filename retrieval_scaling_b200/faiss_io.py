@@ -3,6 +3,7 @@ persists with `faiss.write_index` / loads with `faiss.read_index` (`src/indicies
 `ivf_flat.py:71,167,185`, `ivf_pq.py:75,171,190`):
 
     "IxFI"  IndexFlatIP            "IwFl"  IndexIVFFlat (quantizer IndexFlatIP)      "IwPQ"  IndexIVFPQ (by_residual)
+    "IxRF"  IndexRefineFlat (IVF-PQ base + exact re-rank vectors; faiss IndexRefine with an IndexFlat refine index)
 
 [FAISS-ext] faiss is not installable in this image, so this module restates the on-disk layout of faiss 1.8.0
 (`faiss/impl/index_write.cpp`, `index_read.cpp`) from the published source and is pinned only by byte-level
@@ -17,6 +18,8 @@ faiss build.  Layout (little endian):
   IwPQ           : ivf header | by_residual u8 | code_size u64 | PQ: d u64 | M u64 | nbits u64 | (u64 n | float32[n]) | inverted lists
   inverted lists : "ilar" | nlist u64 | code_size u64 | "full" (u64 n | u64 sizes[n])  or  "sprs" (u64 n | u64 (list, size) pairs)
                    then, for every list in order: codes u8[size * code_size] | ids i64[size]
+  IxRF           : header | <base index> | <refine index, here IxFI> | k_factor f32
+                   (index_write.cpp: IndexRefine branch; index_read.cpp turns a flat refine index into IndexRefineFlat)
 """
 from __future__ import annotations
 
@@ -164,7 +167,17 @@ def read_faiss(f) -> Dict:
             raise ValueError("IVFPQ code_size mismatch")
         return {"kind": "IVFPQ", **h, "by_residual": by_residual, "M": M, "nbits": nbits,
                 "codebook": cent.reshape(M, ksub, pd // M), "offsets": offsets, "codes": codes, "ids": ids}
-    raise NotImplementedError(f"faiss index type {tag!r} is not supported (Flat / IVFFlat / IVFPQ only)")
+    if tag == "IxRF":
+        hdr = _read_header(f)
+        base = read_faiss(f)
+        refine = read_faiss(f)
+        k_factor = _rd(f, "f")
+        if refine["kind"] != "Flat":
+            raise NotImplementedError("only a flat refine index (IndexRefineFlat) is supported, not IxSQ / PQ refinement")
+        if base["d"] != hdr["d"] or refine["d"] != hdr["d"] or refine["ntotal"] != base["ntotal"]:
+            raise ValueError("IndexRefine: base and refine index disagree on d or ntotal")
+        return {"kind": "Refine", **hdr, "base": base, "xb": refine["xb"], "k_factor": k_factor}
+    raise NotImplementedError(f"faiss index type {tag!r} is not supported (Flat / IVFFlat / IVFPQ / RefineFlat only)")
 
 
 # ----------------------------------------------------------------------------------------------------------
@@ -250,6 +263,12 @@ def write_faiss(f, parts: Dict) -> None:
         _wr(f, "Q", cb.size)
         f.write(cb.tobytes())
         _write_invlists(f, parts["centroids"].shape[0], code_size, parts["offsets"], parts["codes"], parts["ids"])
+    elif kind == "Refine":
+        xb = parts["xb"]
+        _write_header(f, "IxRF", xb.shape[1], xb.shape[0], True, METRIC_INNER_PRODUCT)
+        write_faiss(f, parts["base"])
+        _write_flat(f, xb, METRIC_INNER_PRODUCT)
+        _wr(f, "f", float(parts.get("k_factor", 1.0)))
     else:
         raise NotImplementedError(kind)
 
@@ -260,4 +279,4 @@ def is_faiss_file(path: str) -> bool:
             tag = f.read(4).decode("ascii", "replace")
     except OSError:
         return False
-    return tag in ("IxFI", "IxF2", "IxFl", "IwFl", "IwPQ")
+    return tag in ("IxFI", "IxF2", "IxFl", "IwFl", "IwPQ", "IxRF")

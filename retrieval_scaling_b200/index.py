@@ -328,6 +328,132 @@ class IndexIVFPQ(_IVFBase):
             torch.cuda.current_stream().synchronize()
 
 
+_STORE_DTYPES = {"float16": (torch.float16, _lib.RSB_DTYPE_F16), "float32": (torch.float32, _lib.RSB_DTYPE_F32)}
+
+
+class IndexRefine:
+    """faiss.IndexRefineFlat(base) / IndexRefine(base, IndexFlatIP(d)): the base IVF-PQ search returns k * k_factor
+    candidates, which are re-scored exactly against a re-rank store of the original vectors (row = index id), and the
+    best k are kept (rsb_search_refine).  Only IVF-PQ bases are accepted: Flat / IVF-Flat scores are already exact.
+
+    The store is a device tensor [ntotal, d] in float16 or float32.  The embedding task writes fp16 embeddings, so an
+    fp16 store of them is lossless; an fp16 store of fp32 vectors rounds them (faiss `Refine(SQfp16)`).
+    Results are sorted by exact score descending, ties by ascending id, padded with (-FLT_MAX, -1)."""
+
+    def __init__(self, base, store_dtype: str = "float16", k_factor: int = 1):
+        if not isinstance(base, IndexIVFPQ):
+            raise ValueError(f"IndexRefine re-ranks IVF-PQ results; a {type(base).__name__} base already returns exact scores")
+        if store_dtype not in _STORE_DTYPES:
+            raise ValueError(f"store_dtype must be float16 or float32, got {store_dtype!r}")
+        self.base, self.store_dtype = base, store_dtype
+        self.k_factor = int(k_factor)
+        self.L, self.d, self.device = base.L, base.d, base.device
+        self._store = torch.empty((0, self.d), dtype=_STORE_DTYPES[store_dtype][0], device=self.device)
+        self._n = 0                                     # rows of the store in use (capacity = self._store.shape[0])
+
+    # -- faiss protocol ------------------------------------------------------------------------------------------
+    @property
+    def ntotal(self) -> int:
+        return self.base.ntotal
+
+    @property
+    def is_trained(self) -> bool:
+        return self.base.is_trained
+
+    @property
+    def nprobe(self) -> int:
+        return self.base.nprobe
+
+    @nprobe.setter
+    def nprobe(self, v: int) -> None:
+        self.base.nprobe = int(v)
+
+    @property
+    def store(self) -> torch.Tensor:
+        """The re-rank store [ntotal, d] (a view; row i = the vector of index id i)."""
+        return self._store[: self._n]
+
+    def train(self, x) -> None:
+        self.base.train(x)
+
+    def add(self, x, ids=None) -> None:
+        """Adds to the base and appends to the store.  The store is addressed by index id, so ids are the base's
+        sequential ids (as faiss IndexRefine requires)."""
+        if ids is not None:
+            raise ValueError("IndexRefine addresses its store by index id: add() takes no custom ids")
+        if self._n != self.base.ntotal:
+            raise ValueError(f"the store holds {self._n} rows but the base index {self.base.ntotal} vectors")
+        self.base.add(x)
+        self.add_store(x)
+
+    def reserve(self, n: int) -> None:
+        """Allocates store capacity for n rows, after checking that it fits in free device memory."""
+        if n <= self._store.shape[0]:
+            return
+        need = int(n) * self.d * self._store.element_size()
+        free, _ = torch.cuda.mem_get_info(self.device)
+        if need > free:
+            raise MemoryError(f"the re-rank store needs {need} bytes ({n} x {self.d} {self.store_dtype}); "
+                              f"{free} bytes are free on {self.device}")
+        grown = torch.empty((int(n), self.d), dtype=self._store.dtype, device=self.device)
+        grown[: self._n].copy_(self._store[: self._n])
+        self._store = grown
+
+    def add_store(self, x) -> None:
+        """Appends rows to the store only (for a base that already holds these vectors, e.g. one read from disk)."""
+        if isinstance(x, np.ndarray):
+            x = torch.from_numpy(np.ascontiguousarray(x))
+        x = torch.as_tensor(x)
+        if x.dim() != 2 or x.shape[1] != self.d:
+            raise ValueError(f"expected [n, {self.d}] vectors, got {tuple(x.shape)}")
+        n = x.shape[0]
+        if self._n + n > self._store.shape[0]:
+            self.reserve(max(self._n + n, int(1.25 * self._store.shape[0])))
+        self._store[self._n: self._n + n].copy_(x.to(device=self.device, dtype=self._store.dtype))
+        self._n += n
+        torch.cuda.current_stream(self.device).synchronize()     # x may be a temporary
+
+    def search_ids(self, q, k: int, nprobe: Optional[int] = None, k_factor: Optional[int] = None):
+        """q [nq, d] -> (ids int64 [nq,k], scores float32 [nq,k]) CUDA tensors, enqueued on the current stream."""
+        with torch.cuda.device(self.device):
+            q = _dev_f32(q, self.device)
+            if q.dim() != 2 or q.shape[1] != self.d:
+                raise ValueError(f"expected [nq, {self.d}] queries, got {tuple(q.shape)}")
+            nq, k = q.shape[0], int(k)
+            kf = int(self.k_factor if k_factor is None else k_factor)
+            npb = int(self.nprobe if nprobe is None else nprobe)
+            D = torch.empty((nq, k), dtype=torch.float32, device=self.device)
+            I = torch.empty((nq, k), dtype=torch.int64, device=self.device)
+            if nq == 0:
+                return I, D
+            ws = self.base._workspace(self.L.rsb_search_refine_workspace_bytes(self.base._h, nq, k, kf, npb))
+            _lib.check(self.L.rsb_search_refine(self.base._h, _ptr(q), nq, k, kf, npb, _ptr(self._store),
+                                                _STORE_DTYPES[self.store_dtype][1], self._n, _ptr(D), _ptr(I), _ptr(ws),
+                                                ws.numel(), _stream()))
+            return I, D
+
+    def search(self, x, k: int):
+        """faiss protocol: returns (D, I).  numpy in -> numpy out; torch in -> CUDA tensors out."""
+        I, D = self.search_ids(x, k)
+        if isinstance(x, np.ndarray) or not isinstance(x, torch.Tensor):
+            return D.cpu().numpy(), I.cpu().numpy()
+        return D, I
+
+    def rerank(self, q: torch.Tensor, cand: torch.Tensor, k: int):
+        """The re-rank step alone (rsb_refine): candidates cand [nq, k_base] int64 (-1 = none) -> (ids, scores) [nq, k]."""
+        with torch.cuda.device(self.device):
+            q = _dev_f32(q, self.device)
+            cand = cand.to(device=self.device, dtype=torch.int64).contiguous()
+            nq, k_base = cand.shape
+            D = torch.empty((nq, int(k)), dtype=torch.float32, device=self.device)
+            I = torch.empty((nq, int(k)), dtype=torch.int64, device=self.device)
+            ws = self.base._workspace(self.L.rsb_refine_workspace_bytes(nq, k_base, int(k)))
+            _lib.check(self.L.rsb_refine(_ptr(q), nq, _ptr(self._store), _STORE_DTYPES[self.store_dtype][1], self.d,
+                                         self._n, _ptr(cand), k_base, int(k), _ptr(D), _ptr(I), _ptr(ws), ws.numel(),
+                                         _stream()))
+            return I, D
+
+
 # ------------------------------------------------------------------------------------------------------------
 # persistence: same call sites as faiss.write_index / faiss.read_index (flat.py:39,63; ivf_flat.py:71,167,185;
 # ivf_pq.py:75,171,190).  Files are written in faiss' binary layout (faiss_io.py: IxFI / IwFl / IwPQ), because the
@@ -341,6 +467,10 @@ MAGIC = "RSB1"
 
 
 def _to_faiss_parts(index: _IndexBase) -> dict:
+    if isinstance(index, IndexRefine):
+        # faiss IndexRefineFlat: an fp16 store is written upcast to fp32 (exact)
+        return {"kind": "Refine", "d": index.d, "ntotal": index.ntotal, "base": _to_faiss_parts(index.base),
+                "xb": index.store.float().cpu().numpy(), "k_factor": float(index.k_factor)}
     off, payload, ids = index.export_lists()
     off, payload, ids = off.cpu().numpy(), payload.cpu().numpy(), ids.cpu().numpy()
     if index.kind == _lib.RSB_FLAT:
@@ -353,9 +483,26 @@ def _to_faiss_parts(index: _IndexBase) -> dict:
     return {"kind": "IVFPQ", "codes": payload, "codebook": index.get_codebook().cpu().numpy(), **parts}
 
 
-def _from_faiss_parts(p: dict, device=None) -> _IndexBase:
+def _from_faiss_parts(p: dict, device=None, refine_dtype: Optional[str] = None) -> _IndexBase:
     if p.get("metric", 0) != 0 or p.get("quantizer_metric", 0) != 0:
         raise NotImplementedError("only METRIC_INNER_PRODUCT indexes are supported (the reference builds IP indexes only)")
+    if p["kind"] == "Refine":
+        kf = float(p["k_factor"])
+        if kf != int(kf) or kf < 1:
+            raise NotImplementedError(f"k_factor = {kf}: only whole k_factor >= 1 is supported")
+        xb = p["xb"]
+        dtype = refine_dtype or "float32"
+        if dtype == "float16":
+            xh = xb.astype(np.float16)
+            if not np.array_equal(xh.astype(np.float32), xb):
+                raise ValueError("the refine vectors are not all representable in float16; read with refine_dtype='float32'")
+            xb = xh
+        index = IndexRefine(_from_faiss_parts(p["base"], device), store_dtype=dtype, k_factor=int(kf))
+        if index.ntotal != xb.shape[0]:
+            raise ValueError(f"refine index holds {xb.shape[0]} vectors, its base {index.ntotal}")
+        index.reserve(xb.shape[0])
+        index.add_store(xb)
+        return index
     if p["kind"] == "Flat":
         index = IndexFlatIP(p["d"], device)
         if p["ntotal"]:
@@ -386,6 +533,8 @@ def write_index(index: _IndexBase, path: str, fmt: Optional[str] = None) -> None
     fmt = (fmt or os.environ.get("RSB_INDEX_FORMAT", "faiss")).lower()
     if fmt not in ("faiss", "rsb1"):
         raise ValueError(f"unknown index file format {fmt!r} (faiss | rsb1)")
+    if isinstance(index, IndexRefine) and fmt != "faiss":
+        raise ValueError("an IndexRefine is written in faiss' IndexRefineFlat layout only (fmt='faiss')")
     if fmt == "faiss":
         from . import faiss_io
         try:
@@ -423,11 +572,13 @@ def write_index(index: _IndexBase, path: str, fmt: Optional[str] = None) -> None
     os.replace(tmp, path)
 
 
-def read_index(path: str, device=None) -> _IndexBase:
-    """Loads an RSB1 container or a faiss binary index file (auto-detected by its fourcc)."""
+def read_index(path: str, device=None, refine_dtype: Optional[str] = None) -> _IndexBase:
+    """Loads an RSB1 container or a faiss binary index file (auto-detected by its fourcc).  For an IndexRefineFlat
+    file (IxRF) `refine_dtype` picks the store: "float32" (default) or "float16", which is accepted only when every
+    stored value round-trips through fp16 (ValueError otherwise)."""
     from . import faiss_io
     if faiss_io.is_faiss_file(path):
-        return _from_faiss_parts(faiss_io.read_faiss(path), device)
+        return _from_faiss_parts(faiss_io.read_faiss(path), device, refine_dtype)
     with open(path, "rb") as f:
         blob = pickle.load(f)
     if not isinstance(blob, dict) or blob.get("magic") != MAGIC:

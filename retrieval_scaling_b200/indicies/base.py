@@ -30,10 +30,26 @@ class Indexer(object):
         return dict(index_dir=index_dir, embed_paths=embedding_paths, index_path=index_path, meta_file=index_path + ".meta",
                     pos_map_save_path=os.path.join(index_dir, "passage_pos_id_map.pkl"))
 
+    @staticmethod
+    def refine_options(index_cfg):
+        """Optional keys `refine_k_factor` (absent or 0: no re-ranking) and `refine_dtype` (float16 | float32; absent:
+        the embedding pickles' dtype) -> (k_factor, dtype).  Re-ranking applies to IVFPQ only."""
+        k_factor = int(index_cfg.get("refine_k_factor", 0) or 0)
+        dtype = index_cfg.get("refine_dtype", None)
+        if k_factor < 0:
+            raise ValueError(f"datastore.index.refine_k_factor must be >= 0, got {k_factor}")
+        if k_factor and index_cfg.index_type != "IVFPQ":
+            raise ValueError(f"datastore.index.refine_k_factor re-ranks IVFPQ results; {index_cfg.index_type} scores "
+                             f"are already exact")
+        if dtype not in (None, "float16", "float32"):
+            raise ValueError(f"datastore.index.refine_dtype must be float16 or float32, got {dtype!r}")
+        return k_factor, dtype
+
     def __init__(self, cfg, index_shard_ids=None):
         self.cfg = cfg
         self.args = cfg.datastore.index
         self.index_type = self.args.index_type
+        self.refine_options(self.args)
 
         passage_dir = self.cfg.datastore.embedding.passages_dir
         paths = self.artefact_paths(cfg, index_shard_ids)
@@ -54,9 +70,11 @@ class Indexer(object):
             self.datastore = IVFFlatIndexer(trained_index_path=index_path + ".trained", sample_train_size=a.sample_train_size,
                                             prev_index_path=None, ncentroids=a.ncentroids, probe=a.probe, **common)
         elif self.index_type == "IVFPQ":
+            k_factor, refine_dtype = self.refine_options(a)
             self.datastore = IVFPQIndexer(trained_index_path=index_path + ".trained", sample_train_size=a.sample_train_size,
                                           prev_index_path=None, ncentroids=a.ncentroids, probe=a.probe,
-                                          n_subquantizers=a.n_subquantizers, code_size=a.n_bits, **common)
+                                          n_subquantizers=a.n_subquantizers, code_size=a.n_bits,
+                                          refine_k_factor=k_factor, refine_dtype=refine_dtype, **common)
         else:
             raise NotImplementedError
 

@@ -57,12 +57,13 @@ def shard_id_of_embedding_path(path: str) -> int:
     return int(m.group(1))
 
 
-def load_embedding_shard(path: str) -> np.ndarray:
-    """(ids, embeddings) pickle -> float32 [n, d]; the ids inside the pickle are ignored, row order defines
-    chunk_id (reference `flat.py:59,86`)."""
+def load_embedding_shard(path: str, dtype=np.float32) -> np.ndarray:
+    """(ids, embeddings) pickle -> [n, d] in `dtype` (None: as stored, fp16 when the embedding task wrote it); the
+    ids inside the pickle are ignored, row order defines chunk_id (reference `flat.py:59,86`)."""
     with open(path, "rb") as f:
         _ids, emb = pickle.load(f)
-    return np.ascontiguousarray(np.asarray(emb), dtype=np.float32)
+    emb = np.asarray(emb)
+    return np.ascontiguousarray(emb, dtype=emb.dtype if dtype is None else dtype)
 
 
 def convert_pkl_to_jsonl(passage_dir: str) -> None:

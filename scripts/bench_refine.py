@@ -1,0 +1,184 @@
+#!/usr/bin/env python
+"""Exact re-ranking (index.IndexRefine, DESIGN §4.4) on the benchmark's IVF-PQ index: prints one JSON line.
+
+    python scripts/bench_refine.py --n 20000000 --k-factor 8 [--steps 5 --warmup 2]
+
+The index, corpus, queries and exact ground truth are bench.py's (same builder, same seeds, same defaults for nlist / M
+/ nprobe / k / nq).  The synthetic corpus is fp32; the re-rank store holds it in fp16, as the embedding task would have
+written it.  Reported:
+  * unrefined and refined QPS over the same queries (CUDA events around --steps searches each);
+  * the two stages on their own, CUDA events between them: base search at k' = k * k_factor, then the re-rank kernel
+    (rsb_refine); gathered bytes = valid candidates x d x 2 (every candidate row is read once per query), achieved
+    bytes/s against the HBM peak;
+  * recall@k, exact top-1 / top-10 inside the returned k, refined and unrefined, against bench.py's fp32 ground truth;
+  * parity: the re-rank of the first --parity-queries queries equals oracle/refine_oracle.py (faiss IndexRefine::search)
+    on the same candidates, every returned pair re-scored in float64 from the store;
+  * the card's name and power limit.
+The fp16 store (n x d x 2 bytes: 154 GB at 100M) must fit in device memory next to the index; sizes that do not are
+refused before anything is built."""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+import numpy as np
+import torch
+
+import bench as B
+
+
+def parse():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--k-factor", type=int, default=8)
+    ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--n", type=int, default=20_000_000)
+    ap.add_argument("--nq", type=int, default=10_000)
+    ap.add_argument("--nlist", type=int, default=16384)
+    ap.add_argument("--m", type=int, default=64)
+    ap.add_argument("--nprobe", type=int, default=32)
+    ap.add_argument("--k", type=int, default=100)
+    ap.add_argument("--d", type=int, default=768)
+    ap.add_argument("--train-per-centroid", type=int, default=64)
+    ap.add_argument("--recall-queries", type=int, default=1000)
+    ap.add_argument("--parity-queries", type=int, default=256)
+    a = ap.parse_args()
+    a.partition = "list"
+    return a
+
+
+def store_bytes(args) -> int:
+    return args.n * args.d * 2
+
+
+def gpu_identity(device) -> dict:
+    out = {"gpu": torch.cuda.get_device_name(device), "power_limit_w": None}
+    try:
+        r = subprocess.run(["nvidia-smi", f"--id={device.index or 0}", "--query-gpu=power.limit",
+                            "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=20)
+        out["power_limit_w"] = float(r.stdout.strip().splitlines()[0])
+    except Exception:
+        pass
+    return out
+
+
+def timed(fn, steps, warmup):
+    for _ in range(warmup):
+        fn()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(steps):
+        out = fn()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / steps, out
+
+
+def parity(ref, xq, Ib, Ir, Dr, k, npq):
+    """The re-rank result is the exact top-k of the base's k' candidates: oracle on the same candidates, float64."""
+    from oracle import parity as P
+    from oracle import refine_oracle as R
+    kb = Ib.shape[1]
+    Ib_h = Ib[:npq].cpu().numpy()
+    rows = ref.store[Ib[:npq].clamp_min(0)].cpu().numpy()                          # [npq, k', d] fp16
+    xq_h = xq[:npq].cpu().numpy()
+    Dref = np.full((npq, k), np.finfo(np.float32).min, np.float32)
+    Iref = np.full((npq, k), -1, np.int64)
+    exact = {}
+    for i in range(npq):
+        loc = np.where(Ib_h[i] >= 0, np.arange(kb), -1)
+        Dl, Il = R.refine_candidates(xq_h[i:i + 1], rows[i], loc[None], k, dtype=np.float64)
+        Dref[i], Iref[i] = Dl[0], np.where(Il[0] >= 0, Ib_h[i][Il[0].clip(0)], -1)
+        s64 = rows[i].astype(np.float64) @ xq_h[i].astype(np.float64)
+        exact.update({(i, int(c)): float(s64[j]) for j, c in enumerate(Ib_h[i]) if c >= 0})
+    Dg, Ig = Dr[:npq].cpu().numpy(), Ir[:npq].cpu().numpy()
+    par = P.topk_parity(Dg, Ig, Dref, Iref, rtol=1e-5, atol=1e-5,
+                        score_of=lambda qs, ids: [exact.get((int(a), int(b)), np.nan) for a, b in zip(qs, ids)])
+    pairs = [(i, int(c), float(Dg[i, r])) for i in range(npq) for r, c in enumerate(Ig[i]) if c >= 0]
+    bad = sum(1 for i, c, s in pairs if (i, c) not in exact or abs(exact[(i, c)] - s) > 1e-5 + 1e-5 * abs(exact[(i, c)]))
+    par.update({"queries": f"the first {npq} queries", "rescored_pairs": len(pairs), "rescore_out_of_tol": bad,
+                "oracle": "oracle/refine_oracle.py (faiss IndexRefine::search) on the GPU's base candidates, float64"})
+    par["ok"] = bool(par["non_tie_mismatches"] == 0 and par["scores_out_of_tol"] == 0 and par["padding_mismatches"] == 0
+                     and bad == 0)
+    return par
+
+
+def main():
+    args = parse()
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_refine.py needs a CUDA device: the product path has no CPU fallback")
+    device = torch.device("cuda", 0)
+    torch.cuda.set_device(device)
+    need = store_bytes(args) + args.n * (args.m + 8)                   # store + PQ codes + ids
+    free, _ = torch.cuda.mem_get_info(device)
+    if need > 0.9 * free:
+        raise SystemExit(f"the fp16 store of {args.n} x {args.d} ({store_bytes(args)} bytes) and the index need ~{need} "
+                         f"bytes, {free} are free on {device}; use a smaller --n")
+    import retrieval_scaling_b200 as rsb
+    from retrieval_scaling_b200 import synth
+    k, kf = args.k, args.k_factor
+    kb = k * kf
+    probe = synth.Corpus(d=args.d, mode="gmm", n_centres=max(16, args.nlist // 4), device=device)
+    xq = probe.queries(args.nq)
+    del probe
+    n_gt = min(args.recall_queries, args.nq)
+    index, corpus, _, gt_I, build = B.build_index(args, 0, 1, device, gt_queries=xq[:n_gt].contiguous())
+
+    t0 = time.time()
+    ref = rsb.IndexRefine(index, "float16", kf)
+    ref.reserve(args.n)
+    for c in range((args.n + B.CHUNK_ROWS - 1) // B.CHUNK_ROWS):
+        ref.add_store(corpus.chunk(c, B.CHUNK_ROWS)[: min(B.CHUNK_ROWS, args.n - c * B.CHUNK_ROWS)])
+    store_s = time.time() - t0
+
+    ms_base_k, (Iu, _) = timed(lambda: index.search_ids(xq, k), args.steps, args.warmup)
+    ms_ref, (I, D) = timed(lambda: ref.search_ids(xq, k), args.steps, args.warmup)
+    # the stages on their own: base search at k' -> re-rank kernel, events between them
+    for _ in range(args.warmup):
+        Ib, _ = index.search_ids(xq, kb)
+        ref.rerank(xq, Ib, k)
+    torch.cuda.synchronize()
+    evs = []
+    for _ in range(args.steps):
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
+        ev[0].record()
+        Ib, _ = index.search_ids(xq, kb)
+        ev[1].record()
+        Ir, Dr = ref.rerank(xq, Ib, k)
+        ev[2].record()
+        evs.append(ev)
+    torch.cuda.synchronize()
+    base_ms = float(np.mean([a.elapsed_time(b) for a, b, _ in evs]))
+    refine_ms = float(np.mean([b.elapsed_time(c) for _, b, c in evs]))
+    valid = int((Ib >= 0).sum().item())
+    gathered = valid * args.d * 2
+    peak, peak_src = B.measured_peak_gbs()
+    gbs = gathered / refine_ms / 1e6
+    strip = lambda r: {kk: vv for kk, vv in r.items() if kk != "ground_truth"}   # noqa: E731
+    out = {"metric": f"queries/sec @ top-k={k} with exact re-ranking of k x {kf} candidates, "
+                     f"{args.n // 1_000_000}M x {args.d} IVF-PQ, fp16 store",
+           "config": {**B.make_config(args, 1), "k_factor": kf, "k_base": kb},
+           "qps_refined": args.nq / (ms_ref / 1e3), "qps_unrefined": args.nq / (ms_base_k / 1e3),
+           "ms_per_step_refined": ms_ref, "ms_per_step_unrefined": ms_base_k,
+           "base_search_ms": base_ms, "refine_kernel_ms": refine_ms,
+           "store": {"dtype": "float16", "bytes": store_bytes(args), "build_s": store_s},
+           "gathered_bytes": gathered, "gathered_bytes_shape": args.nq * kb * args.d * 2,
+           "valid_candidate_frac": valid / (args.nq * kb), "achieved_gbs": gbs, "peak_gbs": peak,
+           "peak_source": peak_src, "frac_of_peak": gbs / peak, **gpu_identity(device),
+           "same_result_as_two_stage": bool(torch.equal(I, Ir) and torch.equal(D, Dr)),
+           "recall": strip(B.recall_block(I[:n_gt], gt_I, k)), "recall_unrefined": strip(B.recall_block(Iu[:n_gt], gt_I, k)),
+           "recall_ground_truth": "bench.py's exact fp32 inner-product search over the same corpus",
+           "parity": parity(ref, xq, Ib, Ir, Dr, k, min(args.parity_queries, args.nq)),
+           "build": build, "steps": args.steps, "warmup": args.warmup}
+    print(json.dumps(out), flush=True)
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())
