@@ -62,6 +62,19 @@ int rsb_ivfflat_create(int d, int nlist, rsb_index_t** out);
  * RESTRICTION (narrower than faiss): nbits must be 8 (tables of 256 entries, one byte per code); nbits = 4 / 10 / 12 /
  * 16 and other M return RSB_ERR_UNSUPPORTED (-> NotImplementedError in Python). */
 int rsb_ivfpq_create(int d, int nlist, int M, int nbits, rsb_index_t** out);
+/* Storage dtype of the vectors (enum RSB_DTYPE_* below): RSB_DTYPE_F32 is rsb_flat_create / rsb_ivfflat_create;
+ * RSB_DTYPE_F16 keeps every row as fp16 -- the embedding task writes fp16 passage embeddings (src/embed.py:137-138)
+ * and the reference upcasts them only on load (src/indicies/flat.py:86), so fp16 storage of them is lossless at half
+ * the bytes.  faiss equivalent: IndexScalarQuantizer / IndexIVFScalarQuantizer(QT_fp16, METRIC_INNER_PRODUCT, no
+ * residual).  Stored values are the fp16 rounding (to nearest even) of what is added; scores are exact fp32 inner
+ * products of the fp32 query with the decoded rows.  d % 8 == 0 (16-byte rows), else RSB_ERR_INVALID.
+ *   Flat (<- src/indicies/flat.py:42, ric/conf/default.yaml `index_type: Flat`): scored on wgmma tensor cores from the
+ *     fp16 rows themselves (scaled fp16 hi/lo query split, then an exact fp32 re-score), needs d % 64 == 0, else
+ *     RSB_ERR_UNSUPPORTED.  Final scores equal the fp32 index's wherever both return the same id.
+ *   IVF-Flat (<- src/indicies/ivf_flat.py:143-149, api/conf/ivf_flat.yaml): the list scan reads 2 bytes per element and
+ *     adds in the fp32 scan's order: ids and scores are bit-identical to an fp32 index holding the same values. */
+int rsb_flat_create_dtype(int d, int dtype, rsb_index_t** out);
+int rsb_ivfflat_create_dtype(int d, int nlist, int dtype, rsb_index_t** out);
 int rsb_free(rsb_index_t* h);
 
 /* ---- trained state (what index.train() produces; ivf_flat.py:166, ivf_pq.py:170) ------------------ */
@@ -81,6 +94,15 @@ int rsb_add(rsb_index_t* h, const float* x_dev, int64_t n, const int64_t* ids_de
 /* as rsb_add but the coarse assignment is supplied by the caller (int32 list id per row) */
 int rsb_add_preassigned(rsb_index_t* h, const float* x_dev, int64_t n, const int64_t* ids_dev,
                         const int32_t* list_dev, rsb_stream_t stream);
+/* rsb_add / rsb_add_preassigned with rows x_dev [n, d] in x_dtype (RSB_DTYPE_F32 or RSB_DTYPE_F16): the embedding
+ * pickles' fp16 rows (src/indicies/flat.py:58-59, ivf_flat.py:180) cross PCIe once at 2 bytes per element and are
+ * converted on the device to the index's storage dtype.  IVF list assignment of fp16 rows runs the fp32 coarse
+ * quantizer on the upcast (exact) values, so the lists are those an fp32 index assigns.  IVFPQ takes RSB_DTYPE_F32
+ * only (RSB_ERR_UNSUPPORTED otherwise). */
+int rsb_add_typed(rsb_index_t* h, const void* x_dev, int x_dtype, int64_t n, const int64_t* ids_dev, void* ws_dev,
+                  size_t ws_bytes, rsb_stream_t stream);
+int rsb_add_preassigned_typed(rsb_index_t* h, const void* x_dev, int x_dtype, int64_t n, const int64_t* ids_dev,
+                              const int32_t* list_dev, rsb_stream_t stream);
 /* IVFPQ only: rows are already PQ codes [n, M] uint8 (e.g. read from an existing index file) */
 int rsb_add_codes(rsb_index_t* h, const uint8_t* codes_dev, int64_t n, const int64_t* ids_dev,
                   const int32_t* list_dev, rsb_stream_t stream);
@@ -94,18 +116,21 @@ enum {
     RSB_INFO_NTOTAL = 5,       /* index.ntotal     */
     RSB_INFO_IS_TRAINED = 6,   /* index.is_trained */
     RSB_INFO_MAX_LIST_LEN = 7,
-    RSB_INFO_INDEX_BYTES = 8   /* device bytes held by the searchable layout */
+    RSB_INFO_INDEX_BYTES = 8,  /* device bytes held by the searchable layout */
+    RSB_INFO_DTYPE = 9         /* storage dtype of the vectors: RSB_DTYPE_F32 / RSB_DTYPE_F16 (IVFPQ: RSB_DTYPE_F32) */
 };
 int rsb_info(rsb_index_t* h, int what, int64_t* out);
 /* list sizes [nlist] int64 to a device buffer */
 int rsb_list_sizes(rsb_index_t* h, int64_t* sizes_dev, rsb_stream_t stream);
 /* Export the inverted lists in natural CSR order (insertion order inside each list), as the oracle and a
  * faiss file writer want them: offsets_dev [nlist+1] int64, payload_dev = uint8 codes [ntotal, M] (IVFPQ)
- * or float32 vectors [ntotal, d] (IVFFLAT / FLAT), ids_dev [ntotal] int64.  Any pointer may be NULL. */
+ * or vectors [ntotal, d] in the storage dtype, float32 or fp16 (IVFFLAT / FLAT), ids_dev [ntotal] int64.  Any pointer
+ * may be NULL. */
 int rsb_export_lists(rsb_index_t* h, int64_t* offsets_dev, void* payload_dev, int64_t* ids_dev,
                      rsb_stream_t stream);
 
 /* ---- search (index.search(x, k) + index.nprobe: flat.py:139, ivf_flat.py:73,225, ivf_pq.py:76,230) --- */
+/* covers the fp16 Flat index's scaled query split (2 x [nq, d] fp16 + [nq] fp32 per query batch) */
 size_t rsb_workspace_bytes(rsb_index_t* h, int nq, int k, int nprobe);
 /* q_dev [nq, d] float32; D_dev [nq, k] float32; I_dev [nq, k] int64.  nprobe ignored for FLAT. */
 int rsb_search(rsb_index_t* h, const float* q_dev, int nq, int k, int nprobe,
@@ -200,7 +225,8 @@ int rsb_pq_accumulate(const float* r_dev, int64_t n, int d, int M, const uint8_t
 /* ---- options -------------------------------------------------------------------------------------------- */
 enum {
     RSB_OPT_COARSE_TENSOR = 0 /* 1 (default): coarse quantizer scores by 3xTF32 on wgmma tensor cores (fp32-equivalent
-                                 accuracy); 0: CUDA-core fp32 FMA tiles */
+                                 accuracy); 0: CUDA-core fp32 FMA tiles.  0 on an fp16 Flat index returns
+                                 RSB_ERR_UNSUPPORTED: its rows are scored on tensor cores only */
 };
 int rsb_set_option(rsb_index_t* h, int option, int64_t value);
 
@@ -211,7 +237,8 @@ enum {
     RSB_PROF_LUT_MS = 2,    /* PQ look-up-table build                   */
     RSB_PROF_SCAN_MS = 3,   /* inverted-list scan kernel (the hot one)  */
     RSB_PROF_MERGE_MS = 4,  /* per-query top-k merge                    */
-    RSB_PROF_SCAN_BYTES = 5,/* algorithmic bytes of the scan: sum over probed (q,list) pairs of len*row_bytes */
+    RSB_PROF_SCAN_BYTES = 5,/* algorithmic bytes of the scan: sum over probed (q,list) pairs of len*row_bytes
+                               (IVF-Flat row_bytes = d * 4, or d * 2 with fp16 storage) */
     RSB_PROF_PAIRS = 6,     /* number of valid (q,list) pairs            */
     RSB_PROF_LAUNCHES = 7,  /* kernels launched by the last search       */
     RSB_PROF_SCAN_PATH = 8, /* IVFPQ scan: 1 = literal-offset shared-memory look-ups, 2 = generic addressing */

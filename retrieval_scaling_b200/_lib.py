@@ -15,7 +15,7 @@ RSB_ERR_INVALID, RSB_ERR_CUDA, RSB_ERR_STATE, RSB_ERR_UNSUPPORTED, RSB_ERR_OOM =
 RSB_FLAT, RSB_IVFFLAT, RSB_IVFPQ = 0, 1, 2
 RSB_DTYPE_F32, RSB_DTYPE_F16 = 0, 1
 (INFO_KIND, INFO_D, INFO_NLIST, INFO_M, INFO_NBITS, INFO_NTOTAL, INFO_IS_TRAINED, INFO_MAX_LIST_LEN,
- INFO_INDEX_BYTES) = range(9)
+ INFO_INDEX_BYTES, INFO_DTYPE) = range(10)
 PROF_NAMES = ("coarse_ms", "setup_ms", "lut_ms", "scan_ms", "merge_ms", "scan_bytes", "pairs", "launches", "scan_path")
 
 # every symbol include/rsb.h declares: (name, restype, argtypes)
@@ -26,6 +26,8 @@ SIGNATURES = [
     ("rsb_flat_create", c_int, [c_int, POINTER(_H)]),
     ("rsb_ivfflat_create", c_int, [c_int, c_int, POINTER(_H)]),
     ("rsb_ivfpq_create", c_int, [c_int, c_int, c_int, c_int, POINTER(_H)]),
+    ("rsb_flat_create_dtype", c_int, [c_int, c_int, POINTER(_H)]),
+    ("rsb_ivfflat_create_dtype", c_int, [c_int, c_int, c_int, POINTER(_H)]),
     ("rsb_free", c_int, [_H]),
     ("rsb_set_centroids", c_int, [_H, c_void_p, c_void_p]),
     ("rsb_set_pq_codebook", c_int, [_H, c_void_p, c_void_p]),
@@ -34,6 +36,8 @@ SIGNATURES = [
     ("rsb_add_workspace_bytes", c_size_t, [_H, c_int64]),
     ("rsb_add", c_int, [_H, c_void_p, c_int64, c_void_p, c_void_p, c_size_t, c_void_p]),
     ("rsb_add_preassigned", c_int, [_H, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
+    ("rsb_add_typed", c_int, [_H, c_void_p, c_int, c_int64, c_void_p, c_void_p, c_size_t, c_void_p]),
+    ("rsb_add_preassigned_typed", c_int, [_H, c_void_p, c_int, c_int64, c_void_p, c_void_p, c_void_p]),
     ("rsb_add_codes", c_int, [_H, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
     ("rsb_finalize", c_int, [_H, c_void_p]),
     ("rsb_info", c_int, [_H, c_int, POINTER(c_int64)]),

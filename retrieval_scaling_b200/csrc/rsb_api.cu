@@ -50,7 +50,7 @@ static inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a
 // handle
 // ---------------------------------------------------------------------------------------------------------
 struct Segment {
-    void* payload = nullptr;   // float [n, d] (FLAT / IVFFLAT) or uint8 [n, M] (IVFPQ)
+    void* payload = nullptr;   // [n, d] in the storage dtype (FLAT / IVFFLAT) or uint8 [n, M] (IVFPQ)
     int64_t* ids = nullptr;    // [n]
     int32_t* list = nullptr;   // [n] (IVF only)
     int64_t n = 0;
@@ -58,6 +58,7 @@ struct Segment {
 
 struct rsb_index {
     int kind = 0, d = 0, nlist = 0, M = 0, nbits = 0, dsub = 0;
+    int dtype = RSB_DTYPE_F32;   // storage of FLAT / IVFFLAT rows: RSB_DTYPE_F32 or RSB_DTYPE_F16
     float* centroids = nullptr;
     float* codebook = nullptr;
     float* codebook_t = nullptr;
@@ -93,7 +94,8 @@ struct rsb_index {
     int ev_done = 0;
     unsigned long long* prof_dev = nullptr;  // [3]: scan elements, pairs, scan path flag
     long launches = 0;
-    size_t row_bytes() const { return kind == RSB_IVFPQ ? (size_t)M : (size_t)d * 4; }
+    int elem_bytes() const { return dtype == RSB_DTYPE_F16 ? 2 : 4; }
+    size_t row_bytes() const { return kind == RSB_IVFPQ ? (size_t)M : (size_t)d * elem_bytes(); }
 };
 
 static void free_segment(Segment& s) {
@@ -113,10 +115,17 @@ static void free_layout(rsb_index* h) {
 extern "C" int rsb_version(void) { return RSB_VERSION; }
 extern "C" const char* rsb_last_error(void) { return g_err.c_str(); }
 
-static int create_common(int kind, int d, int nlist, int M, int nbits, rsb_index_t** out) {
+static int create_common(int kind, int d, int nlist, int M, int nbits, rsb_index_t** out, int dtype = RSB_DTYPE_F32) {
     if (!out) return fail(RSB_ERR_INVALID, "out is NULL");
     *out = nullptr;
     if (d <= 0 || (d & 3)) return fail(RSB_ERR_INVALID, "dimension must be a positive multiple of 4, got %d", d);
+    if (dtype != RSB_DTYPE_F32 && dtype != RSB_DTYPE_F16)
+        return fail(RSB_ERR_INVALID, "dtype must be RSB_DTYPE_F32 or RSB_DTYPE_F16, got %d", dtype);
+    if (dtype == RSB_DTYPE_F16) {
+        if (d % 8) return fail(RSB_ERR_INVALID, "fp16 storage needs 16-byte rows: d = %d is not a multiple of 8", d);
+        if (kind == RSB_FLAT && d % 64)
+            return fail(RSB_ERR_UNSUPPORTED, "the fp16 Flat scorer (wgmma, 64 fp16 per K step) needs d %% 64 == 0, got %d", d);
+    }
     if (kind != RSB_FLAT && nlist <= 0) return fail(RSB_ERR_INVALID, "nlist must be > 0, got %d", nlist);
     if (kind == RSB_IVFPQ) {
         if (nbits != 8) return fail(RSB_ERR_UNSUPPORTED, "only nbits = 8 is implemented, got %d", nbits);
@@ -125,7 +134,7 @@ static int create_common(int kind, int d, int nlist, int M, int nbits, rsb_index
             return fail(RSB_ERR_UNSUPPORTED, "n_subquantizers must be 16, 32, 64 (tuned path) or a multiple of 4 up to 128 (got %d)", M);
     }
     rsb_index* h = new rsb_index();
-    h->kind = kind; h->d = d; h->nlist = kind == RSB_FLAT ? 1 : nlist; h->M = M; h->nbits = nbits;
+    h->kind = kind; h->d = d; h->nlist = kind == RSB_FLAT ? 1 : nlist; h->M = M; h->nbits = nbits; h->dtype = dtype;
     h->dsub = M ? d / M : 0;
     for (auto& set : h->evs) for (auto& e : set) cudaEventCreate(&e);
     if (cudaMalloc(&h->prof_dev, 32) != cudaSuccess) { delete h; return fail(RSB_ERR_OOM, "cudaMalloc failed"); }
@@ -136,6 +145,12 @@ static int create_common(int kind, int d, int nlist, int M, int nbits, rsb_index
 extern "C" int rsb_flat_create(int d, rsb_index_t** out) { return create_common(RSB_FLAT, d, 1, 0, 0, out); }
 extern "C" int rsb_ivfflat_create(int d, int nlist, rsb_index_t** out) {
     return create_common(RSB_IVFFLAT, d, nlist, 0, 0, out);
+}
+extern "C" int rsb_flat_create_dtype(int d, int dtype, rsb_index_t** out) {
+    return create_common(RSB_FLAT, d, 1, 0, 0, out, dtype);
+}
+extern "C" int rsb_ivfflat_create_dtype(int d, int nlist, int dtype, rsb_index_t** out) {
+    return create_common(RSB_IVFFLAT, d, nlist, 0, 0, out, dtype);
 }
 extern "C" int rsb_ivfpq_create(int d, int nlist, int M, int nbits, rsb_index_t** out) {
     return create_common(RSB_IVFPQ, d, nlist, M, nbits, out);
@@ -235,15 +250,20 @@ static KnnPlan knn_plan(int nq, int64_t n, int k) {
     return p;
 }
 
-// optional tensor-core operands: database rows pre-split into tf32 hi/lo parts + scratch for the split queries
+// optional tensor-core operands: database rows pre-split into tf32 hi/lo parts + scratch for the split queries.
+// f16: the database rows x are fp16 and are the B operand themselves (xh / xl unused); qh / ql hold the scaled fp16
+// query split and qinv [min(nq, qb)] the inverse scales (launch_split_f16).
 struct TensorOperands {
     const float* xh;
     const float* xl;
     float* qh;   // [min(nq, qb), d]
     float* ql;
+    bool f16 = false;
+    float* qinv = nullptr;
 };
 
-static int knn_ip_device(rsb_index* h, const float* q, int nq, const float* x, int64_t n, int d, int k,
+// x: [n, d] fp32 rows, or fp16 rows when tc->f16
+static int knn_ip_device(rsb_index* h, const float* q, int nq, const void* x, int64_t n, int d, int k,
                          const int64_t* ids, int64_t id_offset, float* D, int64_t* I, void* ws, size_t ws_bytes,
                          cudaStream_t st, const TensorOperands* tc = nullptr) {
     if (nq <= 0) return RSB_OK;
@@ -254,13 +274,17 @@ static int knn_ip_device(rsb_index* h, const float* q, int nq, const float* x, i
     float* S = reinterpret_cast<float*>(w + p.off_S);
     u64* keys = reinterpret_cast<u64*>(w + p.off_keys);
     int* cnt = reinterpret_cast<int*>(w + p.off_cnt);
+    const bool f16 = tc && tc->f16;
+    const int eb = f16 ? 2 : 4;
+    const unsigned char* xb8 = static_cast<const unsigned char*>(x);
     for (int q0 = 0; q0 < nq; q0 += p.qb) {
         const int nb = std::min(p.qb, nq - q0);
         if (n == 0) {
             CU(cudaMemsetAsync(cnt, 0, (size_t)nb * p.items * 4, st));
         }
         if (tc && n > 0) {
-            launch_split_tf32(q + (size_t)q0 * d, (size_t)nb * d, tc->qh, tc->ql, st);
+            if (f16) launch_split_f16(q + (size_t)q0 * d, nb, d, tc->qh, tc->ql, tc->qinv, st);
+            else launch_split_tf32(q + (size_t)q0 * d, (size_t)nb * d, tc->qh, tc->ql, st);
             if (h) h->launches += 1;
         }
         for (int c = 0; c < p.nchunks && n > 0; ++c) {
@@ -278,20 +302,27 @@ static int knn_ip_device(rsb_index* h, const float* q, int nq, const float* x, i
                     u64* cand = reinterpret_cast<u64*>(w + p.off_S);
                     unsigned* xb = reinterpret_cast<unsigned*>(w + p.off_S + align_up((size_t)nb * ncand * 8));
                     unsigned char* flags = w + p.off_S + align_up((size_t)nb * ncand * 8) + align_up((size_t)nb * nx * 4);
-                    if (launch_gemm_tf32x3_topt(tc->qh, tc->ql, nb, tc->xh + (size_t)c0 * d, tc->xl + (size_t)c0 * d, cols, d,
-                                                (unsigned)c0, cand, xb, st) &&
-                        launch_select_cands(cand, nb, (int)ncand, xb, (int)nx, k, keys, cnt, p.items, c, flags, st) == 0) {
-                        launch_exact_rows(q + (size_t)q0 * d, nb, x + (size_t)c0 * d, cols, d, (unsigned)c0, flags, k, keys, cnt,
-                                          p.items, c, st);
+                    const bool scored =
+                        f16 ? launch_gemm_f16x2_topt(tc->qh, tc->ql, tc->qinv, nb, xb8 + (size_t)c0 * d * eb, cols, d, (unsigned)c0,
+                                                     cand, xb, st)
+                            : launch_gemm_tf32x3_topt(tc->qh, tc->ql, nb, tc->xh + (size_t)c0 * d, tc->xl + (size_t)c0 * d, cols,
+                                                      d, (unsigned)c0, cand, xb, st);
+                    if (scored && launch_select_cands(cand, nb, (int)ncand, xb, (int)nx, k, keys, cnt, p.items, c, flags, st) == 0) {
+                        launch_exact_rows(q + (size_t)q0 * d, nb, xb8 + (size_t)c0 * d * eb, eb, cols, d, (unsigned)c0, flags, k,
+                                          keys, cnt, p.items, c, st);
                         if (h) h->launches += 3;
                         continue;
                     }
                 }
             }
-            if (tc)  // 3xTF32 on wgmma (fp32-equivalent accuracy); CUDA-core fp32 tiles otherwise
+            if (f16)  // fp16 rows: hi/lo query split on wgmma; there is no CUDA-core fp16 path
+                on_tensor = launch_gemm_f16x2(tc->qh, tc->ql, tc->qinv, nb, xb8 + (size_t)c0 * d * eb, cols, d, S, p.chunk, st);
+            else if (tc)  // 3xTF32 on wgmma (fp32-equivalent accuracy); CUDA-core fp32 tiles otherwise
                 on_tensor = launch_gemm_tf32x3(tc->qh, tc->ql, nb, tc->xh + (size_t)c0 * d, tc->xl + (size_t)c0 * d, cols, d,
                                                S, p.chunk, st);
-            if (!on_tensor) launch_sgemm_nt(q + (size_t)q0 * d, nb, x + (size_t)c0 * d, cols, d, S, p.chunk, st);
+            if (f16 && !on_tensor) return fail(RSB_ERR_CUDA, "the fp16 tensor-core scorer could not be set up (tensor map encoding failed)");
+            if (!on_tensor)
+                launch_sgemm_nt(q + (size_t)q0 * d, nb, static_cast<const float*>(x) + (size_t)c0 * d, cols, d, S, p.chunk, st);
             launch_select_rows(S, nb, cols, p.chunk, (unsigned)c0, k, p.nsplit, keys, cnt, p.items, c * p.nsplit, st);
             if (h) h->launches += 2;
         }
@@ -320,7 +351,8 @@ static const int kAssignRows = 16384;  // rows per coarse-assignment batch insid
 // list = argmax_c <x, c> for `n` rows through the index's coarse quantizer (tensor-core candidates + exact fp32
 // re-score, or CUDA-core fp32 tiles: coarse_impl below); defined after the search plan
 static size_t assign_workspace_bytes(const rsb_index* h, int64_t n);
-static int assign_lists(rsb_index* h, const float* x, int64_t n, int32_t* list_out, void* ws, size_t ws_bytes, cudaStream_t st);
+static int assign_lists(rsb_index* h, const float* x, int64_t n, int32_t* list_out, void* ws, size_t ws_bytes, cudaStream_t st,
+                        int64_t r_begin = 0);
 
 extern "C" size_t rsb_add_workspace_bytes(rsb_index_t* h, int64_t n) {
     if (!h || h->kind == RSB_FLAT) return 256;
@@ -336,9 +368,15 @@ static int stage_common(rsb_index* h, Segment& seg, const int64_t* ids, int64_t 
     return RSB_OK;
 }
 
-static int add_impl(rsb_index* h, const float* x, const uint8_t* codes_in, int64_t n, const int64_t* ids,
+// x: [n, d] in x_dtype (RSB_DTYPE_F32 / RSB_DTYPE_F16); stored in the handle's dtype (fp32 -> fp16 rounds to nearest
+// even, fp16 -> fp32 is exact).  IVF list assignment runs on fp32 values (fp16 input is upcast 16384 rows at a time).
+static int add_impl(rsb_index* h, const void* x, int x_dtype, const uint8_t* codes_in, int64_t n, const int64_t* ids,
                     const int32_t* list_in, void* ws, size_t ws_bytes, cudaStream_t st) {
     if (!h) return fail(RSB_ERR_INVALID, "null handle");
+    if (x_dtype != RSB_DTYPE_F32 && x_dtype != RSB_DTYPE_F16)
+        return fail(RSB_ERR_INVALID, "x_dtype must be RSB_DTYPE_F32 or RSB_DTYPE_F16, got %d", x_dtype);
+    if (x_dtype == RSB_DTYPE_F16 && h->kind == RSB_IVFPQ)
+        return fail(RSB_ERR_UNSUPPORTED, "IVFPQ encodes fp32 rows: pass x as RSB_DTYPE_F32");
     if (n < 0) return fail(RSB_ERR_INVALID, "n < 0");
     if (n == 0) return RSB_OK;
     if (!x && !codes_in) return fail(RSB_ERR_INVALID, "null data pointer");
@@ -355,19 +393,39 @@ static int add_impl(rsb_index* h, const float* x, const uint8_t* codes_in, int64
         CUB_(cudaMalloc(&seg.list, (size_t)n * 4));
         if (list_in) {
             CUB_(cudaMemcpyAsync(seg.list, list_in, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
-        } else {
+        } else if (x_dtype == RSB_DTYPE_F32) {
             // list = argmax_c <x, c>  (fp32-exact, IndexFlatIP quantizer semantics)
-            rc = assign_lists(h, x, n, seg.list, ws, ws_bytes, st);
+            rc = assign_lists(h, static_cast<const float*>(x), n, seg.list, ws, ws_bytes, st);
+            if (rc != RSB_OK) return bail(rc);
+        } else {
+            // fp16 rows: the same quantizer on the upcast values (exact), so the lists are those of the fp32 rows
+            const int64_t rows = std::min<int64_t>(n, kAssignRows);
+            float* up = nullptr;
+            CUB_(cudaMalloc(&up, (size_t)rows * h->d * 4));
+            for (int64_t r0 = 0; r0 < n && rc == RSB_OK; r0 += rows) {
+                const int64_t nb = std::min<int64_t>(rows, n - r0);
+                launch_f16_to_f32(static_cast<const uint16_t*>(x) + (size_t)r0 * h->d, (size_t)nb * h->d, up, st);
+                rc = assign_lists(h, up, nb, seg.list, ws, ws_bytes, st, r0);
+            }
+            cudaStreamSynchronize(st);
+            cudaFree(up);
             if (rc != RSB_OK) return bail(rc);
         }
     }
     if (h->kind == RSB_IVFPQ) {
         CUB_(cudaMalloc(&seg.payload, (size_t)n * h->M));
         if (codes_in) CUB_(cudaMemcpyAsync(seg.payload, codes_in, (size_t)n * h->M, cudaMemcpyDeviceToDevice, st));
-        else launch_pq_encode(x, n, h->d, seg.list, h->centroids, h->codebook, h->M, static_cast<uint8_t*>(seg.payload), st);
+        else launch_pq_encode(static_cast<const float*>(x), n, h->d, seg.list, h->centroids, h->codebook, h->M,
+                              static_cast<uint8_t*>(seg.payload), st);
     } else {
-        CUB_(cudaMalloc(&seg.payload, (size_t)n * h->d * 4));
-        CUB_(cudaMemcpyAsync(seg.payload, x, (size_t)n * h->d * 4, cudaMemcpyDeviceToDevice, st));
+        const size_t elems = (size_t)n * h->d;
+        CUB_(cudaMalloc(&seg.payload, elems * h->elem_bytes()));
+        if (x_dtype == h->dtype)
+            CUB_(cudaMemcpyAsync(seg.payload, x, elems * h->elem_bytes(), cudaMemcpyDeviceToDevice, st));
+        else if (h->dtype == RSB_DTYPE_F16)
+            launch_f32_to_f16(static_cast<const float*>(x), elems, seg.payload, st);
+        else
+            launch_f16_to_f32(x, elems, static_cast<float*>(seg.payload), st);
     }
     CUB_(cudaPeekAtLastError());
 #undef CUB_
@@ -378,19 +436,27 @@ static int add_impl(rsb_index* h, const float* x, const uint8_t* codes_in, int64
 
 extern "C" int rsb_add(rsb_index_t* h, const float* x, int64_t n, const int64_t* ids, void* ws, size_t ws_bytes,
                        rsb_stream_t stream) {
-    return add_impl(h, x, nullptr, n, ids, nullptr, ws, ws_bytes, (cudaStream_t)stream);
+    return add_impl(h, x, RSB_DTYPE_F32, nullptr, n, ids, nullptr, ws, ws_bytes, (cudaStream_t)stream);
+}
+extern "C" int rsb_add_typed(rsb_index_t* h, const void* x, int x_dtype, int64_t n, const int64_t* ids, void* ws,
+                             size_t ws_bytes, rsb_stream_t stream) {
+    return add_impl(h, x, x_dtype, nullptr, n, ids, nullptr, ws, ws_bytes, (cudaStream_t)stream);
 }
 extern "C" int rsb_add_preassigned(rsb_index_t* h, const float* x, int64_t n, const int64_t* ids,
                                    const int32_t* list, rsb_stream_t stream) {
+    return rsb_add_preassigned_typed(h, x, RSB_DTYPE_F32, n, ids, list, stream);
+}
+extern "C" int rsb_add_preassigned_typed(rsb_index_t* h, const void* x, int x_dtype, int64_t n, const int64_t* ids,
+                                         const int32_t* list, rsb_stream_t stream) {
     if (h && h->kind == RSB_FLAT) return fail(RSB_ERR_INVALID, "a Flat index has no lists");
     if (!list) return fail(RSB_ERR_INVALID, "list_dev is NULL");
-    return add_impl(h, x, nullptr, n, ids, list, nullptr, 0, (cudaStream_t)stream);
+    return add_impl(h, x, x_dtype, nullptr, n, ids, list, nullptr, 0, (cudaStream_t)stream);
 }
 extern "C" int rsb_add_codes(rsb_index_t* h, const uint8_t* codes, int64_t n, const int64_t* ids,
                              const int32_t* list, rsb_stream_t stream) {
     if (!h || h->kind != RSB_IVFPQ) return fail(RSB_ERR_INVALID, "rsb_add_codes needs an IVFPQ index");
     if (!list || !codes) return fail(RSB_ERR_INVALID, "null argument");
-    return add_impl(h, nullptr, codes, n, ids, list, nullptr, 0, (cudaStream_t)stream);
+    return add_impl(h, nullptr, RSB_DTYPE_F32, codes, n, ids, list, nullptr, 0, (cudaStream_t)stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -462,8 +528,9 @@ extern "C" int rsb_finalize(rsb_index_t* h, rsb_stream_t stream) {
         h->staging.clear(); h->n_staged = 0;
         h->payload = payload; h->payload_bytes = (size_t)n * rb; h->ids_slots = ids;
         h->ntotal = n; h->nslots = n; h->max_list_len = (int)std::min<int64_t>(n, 0x7fffffff);
-        // tensor-core scoring needs the rows split into tf32 hi/lo parts (2x the fp32 footprint): only below 8 GB
-        if (h->flat_tensor && (h->d % 32 == 0) && n > 0 && (size_t)n * rb <= ((size_t)8 << 30) && tf32_path_available()) {
+        // tensor-core scoring needs the rows split into tf32 hi/lo parts (2x the fp32 footprint): only below 8 GB.
+        // fp16 rows are the tensor-core operand as stored: no split copy at any size.
+        if (h->dtype == RSB_DTYPE_F32 && h->flat_tensor && (h->d % 32 == 0) && n > 0 && (size_t)n * rb <= ((size_t)8 << 30) && tf32_path_available()) {
             if (cudaMalloc(&h->flat_hi, (size_t)n * rb) == cudaSuccess && cudaMalloc(&h->flat_lo, (size_t)n * rb) == cudaSuccess) {
                 launch_split_tf32(reinterpret_cast<const float*>(payload), (size_t)n * h->d, h->flat_hi, h->flat_lo, st);
                 CU(cudaStreamSynchronize(st));
@@ -592,6 +659,7 @@ extern "C" int rsb_info(rsb_index_t* h, int what, int64_t* out) {
         case RSB_INFO_IS_TRAINED: *out = is_trained(h) ? 1 : 0; break;
         case RSB_INFO_MAX_LIST_LEN: *out = h->max_list_len; break;
         case RSB_INFO_INDEX_BYTES: *out = (int64_t)(h->payload_bytes + (size_t)h->nslots * 8); break;
+        case RSB_INFO_DTYPE: *out = h->dtype; break;
         default: return fail(RSB_ERR_INVALID, "unknown info key %d", what);
     }
     return RSB_OK;
@@ -694,9 +762,15 @@ struct FlatPlan {
 static FlatPlan flat_plan(const rsb_index* h, int nq, int k) {
     FlatPlan p;
     const int64_t n = std::max<int64_t>(h->ntotal + h->n_staged, 1);
-    p.tensor = h->flat_tensor && h->flat_hi && h->flat_lo && h->n_staged == 0 && (h->d % 32 == 0) && k + 8 <= 4096 &&
-               tf32_path_available();
-    p.kc = p.tensor ? (int)std::min<int64_t>(n, (int64_t)k + 8) : k;
+    if (h->dtype == RSB_DTYPE_F16) {
+        // always the tensor-core scorer; k + 8 candidates, at most 4096 (the select / re-score limit)
+        p.tensor = true;
+        p.kc = (int)std::min<int64_t>(n, std::min(k + 8, 4096));
+    } else {
+        p.tensor = h->flat_tensor && h->flat_hi && h->flat_lo && h->n_staged == 0 && (h->d % 32 == 0) && k + 8 <= 4096 &&
+                   tf32_path_available();
+        p.kc = p.tensor ? (int)std::min<int64_t>(n, (int64_t)k + 8) : k;
+    }
     p.knn = knn_plan(nq, n, p.kc);
     size_t o = align_up(p.knn.total);
     p.off_qsplit = o; o += p.tensor ? align_up((size_t)2 * p.knn.qb * h->d * 4) : 0;
@@ -739,7 +813,7 @@ static int coarse_impl(rsb_index* h, const float* q, int nq, const SearchPlan& p
     int64_t* cI2 = reinterpret_cast<int64_t*>(w + p.off_cI2);
     RSB_TRY(knn_ip_device(h, q, nq, h->centroids, h->nlist, h->d, p.kc, nullptr, 0, cD2, cI2, w + p.off_coarse_ws,
                           p.coarse.total, st, &tc));
-    if (launch_refine_exact(q, nq, h->centroids, h->d, cI2, p.kc, p.nprobe, cD, cI, nullptr, st) != 0)
+    if (launch_refine_exact(q, nq, h->centroids, 4, h->d, cI2, p.kc, p.nprobe, cD, cI, nullptr, st) != 0)
         return fail(RSB_ERR_UNSUPPORTED, "nprobe = %d is too large for the coarse re-score kernel", p.nprobe);
     h->launches += 1;
     CHECK_LAUNCH();
@@ -750,7 +824,9 @@ static size_t assign_workspace_bytes(const rsb_index* h, int64_t n) {
     const int rows = (int)std::min<int64_t>(std::max<int64_t>(n, 1), kAssignRows);
     return search_plan(h, rows, 1, 1).total + 256;
 }
-static int assign_lists(rsb_index* h, const float* x, int64_t n, int32_t* list_out, void* ws, size_t ws_bytes, cudaStream_t st) {
+// rows x[0, n) get lists list_out[r_begin + i]
+static int assign_lists(rsb_index* h, const float* x, int64_t n, int32_t* list_out, void* ws, size_t ws_bytes, cudaStream_t st,
+                        int64_t r_begin) {
     const int rows = (int)std::min<int64_t>(std::max<int64_t>(n, 1), kAssignRows);
     const SearchPlan p = search_plan(h, rows, 1, 1);
     if (ws_bytes < p.total) return fail(RSB_ERR_OOM, "add workspace too small: need %zu, got %zu", p.total, ws_bytes);
@@ -758,7 +834,7 @@ static int assign_lists(rsb_index* h, const float* x, int64_t n, int32_t* list_o
     for (int64_t r0 = 0; r0 < n; r0 += p.qb) {
         const int nb = (int)std::min<int64_t>(p.qb, n - r0);
         RSB_TRY(coarse_impl(h, x + (size_t)r0 * h->d, nb, p, w, st));
-        launch_i64_to_i32(reinterpret_cast<const int64_t*>(w + p.off_cI), nb, list_out + r0, st);
+        launch_i64_to_i32(reinterpret_cast<const int64_t*>(w + p.off_cI), nb, list_out + r_begin + r0, st);
     }
     CHECK_LAUNCH();
     return RSB_OK;
@@ -807,28 +883,34 @@ static int search_impl(rsb_index_t* h, const float* q, int nq, int k, int nprobe
         if (h->prof) CU(cudaEventRecord(h->ev[0], st));
         const FlatPlan fp = flat_plan(h, nq, k);
         if (fp.tensor && h->ntotal > 0) {
-            // tensor-core candidates (k + 8 per query, 3xTF32 on wgmma), then exact fp32 re-score -> top-k
+            // tensor-core candidates (k + 8 per query; 3xTF32 on wgmma, or the scaled fp16 query split against fp16
+            // rows), then exact fp32 re-score -> top-k
             if (ws_bytes < fp.total) return fail(RSB_ERR_OOM, "workspace too small: need %zu bytes, got %zu", fp.total, ws_bytes);
             unsigned char* w = static_cast<unsigned char*>(ws);
             TensorOperands tc;
             tc.xh = h->flat_hi; tc.xl = h->flat_lo;
             tc.qh = reinterpret_cast<float*>(w + fp.off_qsplit);
             tc.ql = tc.qh + (size_t)fp.knn.qb * h->d;
+            if (h->dtype == RSB_DTYPE_F16) {   // [qb, d] fp16 hi, [qb, d] fp16 lo, [qb] fp32 inverse scales
+                tc.f16 = true;
+                tc.ql = reinterpret_cast<float*>(reinterpret_cast<uint16_t*>(tc.qh) + (size_t)fp.knn.qb * h->d);
+                tc.qinv = reinterpret_cast<float*>(reinterpret_cast<uint16_t*>(tc.qh) + (size_t)2 * fp.knn.qb * h->d);
+            }
             float* D2 = reinterpret_cast<float*>(w + fp.off_D2);
             int64_t* I2 = reinterpret_cast<int64_t*>(w + fp.off_I2);
             for (int q0 = 0; q0 < nq; q0 += fp.knn.qb) {
                 const int nb = std::min(fp.knn.qb, nq - q0);
                 const float* qb = q + (size_t)q0 * h->d;
-                RSB_TRY(knn_ip_device(h, qb, nb, reinterpret_cast<const float*>(h->payload), h->ntotal, h->d, fp.kc, nullptr, 0,
-                                      D2, I2, w, fp.knn.total, st, &tc));
-                if (launch_refine_exact(qb, nb, reinterpret_cast<const float*>(h->payload), h->d, I2, fp.kc, k, D + (size_t)q0 * k,
+                RSB_TRY(knn_ip_device(h, qb, nb, h->payload, h->ntotal, h->d, fp.kc, nullptr, 0, D2, I2, w, fp.knn.total, st, &tc));
+                if (launch_refine_exact(qb, nb, h->payload, h->elem_bytes(), h->d, I2, fp.kc, k, D + (size_t)q0 * k,
                                         I + (size_t)q0 * k, h->ids_slots, st) != 0)
                     return fail(RSB_ERR_UNSUPPORTED, "k = %d is too large for the re-score kernel", k);
                 h->launches += 1;
             }
             CHECK_LAUNCH();
         } else {
-            RSB_TRY(knn_ip_device(h, q, nq, reinterpret_cast<const float*>(h->payload), h->ntotal, h->d, k, h->ids_slots, 0,
+            // fp32 rows on CUDA cores (or an empty index of either dtype: all padding, no row is read)
+            RSB_TRY(knn_ip_device(h, q, nq, h->payload, h->ntotal, h->d, k, h->ids_slots, 0,
                                   D, I, ws, ws_bytes, st));
         }
         if (h->prof) {
@@ -912,7 +994,7 @@ static int search_impl(rsb_index_t* h, const float* q, int nq, int k, int nprobe
                 return fail(RSB_ERR_UNSUPPORTED, "no scan kernel for M = %d", h->M);
         } else {
             if (prof) CU(cudaEventRecord(h->ev[3], st));
-            launch_ivfflat_scan(a, qb, reinterpret_cast<const float*>(h->payload), h->d, nb, st);
+            launch_ivfflat_scan(a, qb, h->payload, h->elem_bytes(), h->d, nb, st);
         }
         h->launches += 1;
         if (prof) CU(cudaEventRecord(h->ev[4], st));
@@ -1121,7 +1203,10 @@ extern "C" int rsb_merge_topk_peers_scatter(const float* const* D_ptrs_dev, cons
 extern "C" int rsb_set_option(rsb_index_t* h, int option, int64_t value) {
     if (!h) return fail(RSB_ERR_INVALID, "null handle");
     switch (option) {
-        case RSB_OPT_COARSE_TENSOR: h->coarse_tensor = value != 0; h->flat_tensor = value != 0; return RSB_OK;
+        case RSB_OPT_COARSE_TENSOR:
+            if (value == 0 && h->kind == RSB_FLAT && h->dtype == RSB_DTYPE_F16)
+                return fail(RSB_ERR_UNSUPPORTED, "an fp16 Flat index scores on tensor cores only (no CUDA-core fp16 path)");
+            h->coarse_tensor = value != 0; h->flat_tensor = value != 0; return RSB_OK;
         default: return fail(RSB_ERR_INVALID, "unknown option %d", option);
     }
 }

@@ -3,12 +3,25 @@
 #ifndef RSB_COMMON_CUH_
 #define RSB_COMMON_CUH_
 
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 namespace rsb {
 
 typedef unsigned long long u64;
+
+// ---- stored rows: elements c .. c+3 of a row (c % 4 == 0) as fp32 ------------------------------------------
+// fp32 rows: one 16-byte load; fp16 rows: one 8-byte load of 4 halves (exact conversion).  The kernels that score
+// rows are templated on the row type and run the same fmaf sequence on these values, so an fp16 row and an fp32
+// row holding the same (fp16-representable) values give bit-identical scores.
+__device__ __forceinline__ float4 load_row4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
+__device__ __forceinline__ float4 load_row4(const __half* p) {
+    const uint2 u = __ldg(reinterpret_cast<const uint2*>(p));
+    const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&u.x));
+    const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&u.y));
+    return make_float4(a.x, a.y, b.x, b.y);
+}
 
 // ---- order-preserving float <-> uint mapping (larger float => larger uint) -------------------------------
 __device__ __forceinline__ unsigned ord_f32(float f) {

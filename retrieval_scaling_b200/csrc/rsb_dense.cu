@@ -321,10 +321,12 @@ int launch_select_cands(const u64* cand, int nrows, int ncand, const unsigned* x
 
 // Exhaustive fp32 re-do of the flagged rows: one block per row (unflagged rows exit at once), a warp scores one column
 // per step (128-bit coalesced loads, query in shared memory), threshold-filtered candidate buffer as in the list scans.
+// T = __half: fp16 database rows (Flat with fp16 storage), 8-byte loads, the same lane mapping and fmaf order.
 constexpr int XR_THREADS = 256, XR_WARPS = XR_THREADS / 32, XR_CHECK = 16, XR_SLACK = XR_CHECK * XR_WARPS;
 
+template <typename T>
 __global__ __launch_bounds__(XR_THREADS)
-void exact_rows_kernel(const float* __restrict__ Q, const float* __restrict__ X, int ncols, int d, unsigned col_base,
+void exact_rows_kernel(const float* __restrict__ Q, const T* __restrict__ X, int ncols, int d, unsigned col_base,
                        const unsigned char* __restrict__ flags, int kc, int cap, u64* __restrict__ out_keys,
                        int* __restrict__ out_cnt, int items_per_row, int item_idx) {
     const int row = blockIdx.x;
@@ -343,10 +345,10 @@ void exact_rows_kernel(const float* __restrict__ Q, const float* __restrict__ X,
     for (int it = 0; it < n_iter; ++it) {
         const int col = it * XR_WARPS + warp;
         const bool ok = col < ncols;
-        const float* p = X + (size_t)(ok ? col : 0) * d;
+        const T* p = X + (size_t)(ok ? col : 0) * d;
         float acc = 0.f;
         for (int c = lane * 4; c < d; c += 128) {
-            const float4 xv = __ldg(reinterpret_cast<const float4*>(p + c));
+            const float4 xv = load_row4(p + c);
             const float4 qv = *reinterpret_cast<const float4*>(qs + c);
             acc = fmaf(xv.x, qv.x, acc); acc = fmaf(xv.y, qv.y, acc); acc = fmaf(xv.z, qv.z, acc); acc = fmaf(xv.w, qv.w, acc);
         }
@@ -362,17 +364,29 @@ void exact_rows_kernel(const float* __restrict__ Q, const float* __restrict__ X,
     if (threadIdx.x == 0) out_cnt[item] = n;
 }
 
-void launch_exact_rows(const float* Q, int nrows, const float* X, int ncols, int d, unsigned col_base,
-                       const unsigned char* flags, int kc, u64* out_keys, int* out_cnt, int items_per_row, int item,
-                       cudaStream_t st) {
-    if (nrows <= 0 || ncols <= 0) return;
+template <typename T>
+static void launch_exact_rows_t(const float* Q, int nrows, const T* X, int ncols, int d, unsigned col_base,
+                                const unsigned char* flags, int kc, u64* out_keys, int* out_cnt, int items_per_row,
+                                int item, cudaStream_t st) {
     const int cap = cand_capacity(kc, XR_SLACK);
     const size_t smem = (((size_t)d * 4 + 15) & ~(size_t)15) + (size_t)cap * 8;
     static PerDeviceSize configured;
     if (smem > 48 * 1024 && configured.raise(smem))
-        cudaFuncSetAttribute(exact_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    exact_rows_kernel<<<nrows, XR_THREADS, smem, st>>>(Q, X, ncols, d, col_base, flags, kc, cap, out_keys, out_cnt,
-                                                      items_per_row, item);
+        cudaFuncSetAttribute(exact_rows_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    exact_rows_kernel<T><<<nrows, XR_THREADS, smem, st>>>(Q, X, ncols, d, col_base, flags, kc, cap, out_keys, out_cnt,
+                                                         items_per_row, item);
+}
+
+void launch_exact_rows(const float* Q, int nrows, const void* X, int elem_bytes, int ncols, int d, unsigned col_base,
+                       const unsigned char* flags, int kc, u64* out_keys, int* out_cnt, int items_per_row, int item,
+                       cudaStream_t st) {
+    if (nrows <= 0 || ncols <= 0) return;
+    if (elem_bytes == 2)
+        launch_exact_rows_t(Q, nrows, static_cast<const __half*>(X), ncols, d, col_base, flags, kc, out_keys, out_cnt,
+                            items_per_row, item, st);
+    else
+        launch_exact_rows_t(Q, nrows, static_cast<const float*>(X), ncols, d, col_base, flags, kc, out_keys, out_cnt,
+                            items_per_row, item, st);
 }
 
 // =============================================================================================================
@@ -553,10 +567,12 @@ void merge_shards_kernel(const float* __restrict__ D_all, const int64_t* __restr
 // =============================================================================================================
 // Exact fp32 re-score of tensor-core (3xTF32) candidates: for each query, recompute <q, x[id]> with FFMA for the
 // k_in candidate rows, sort (score desc, id asc) and keep k_out.  Makes the coarse quantizer's output independent
-// of the tensor-core accumulation order (ids/scores as from the CUDA-core path).
+// of the tensor-core accumulation order (ids/scores as from the CUDA-core path).  T = __half: fp16 rows, same lane
+// mapping and fmaf order (scores bit-equal to those of fp32 rows holding the same values).
 // =============================================================================================================
+template <typename T>
 __global__ __launch_bounds__(256)
-void refine_exact_kernel(const float* __restrict__ Q, const float* __restrict__ X, int d, const int64_t* __restrict__ I_in,
+void refine_exact_kernel(const float* __restrict__ Q, const T* __restrict__ X, int d, const int64_t* __restrict__ I_in,
                          int k_in, int k_out, int P, float* __restrict__ D, int64_t* __restrict__ I,
                          const int64_t* __restrict__ id_map) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -571,9 +587,9 @@ void refine_exact_kernel(const float* __restrict__ Q, const float* __restrict__ 
         const int64_t id = I_in[(size_t)q * k_in + j];
         float acc = 0.f;
         if (id >= 0) {
-            const float* x = X + (size_t)id * d;
+            const T* x = X + (size_t)id * d;
             for (int c = lane * 4; c < d; c += 128) {
-                const float4 xv = __ldg(reinterpret_cast<const float4*>(x + c));
+                const float4 xv = load_row4(x + c);
                 const float4 qv = *reinterpret_cast<const float4*>(qs + c);
                 acc = fmaf(xv.x, qv.x, acc); acc = fmaf(xv.y, qv.y, acc);
                 acc = fmaf(xv.z, qv.z, acc); acc = fmaf(xv.w, qv.w, acc);
@@ -596,16 +612,25 @@ void refine_exact_kernel(const float* __restrict__ Q, const float* __restrict__ 
     }
 }
 
-int launch_refine_exact(const float* Q, int nq, const float* X, int d, const int64_t* I_in, int k_in, int k_out,
-                        float* D, int64_t* I, const int64_t* id_map, cudaStream_t st) {
+template <typename T>
+static void launch_refine_exact_t(const float* Q, int nq, const T* X, int d, const int64_t* I_in, int k_in, int k_out,
+                                  int P, size_t smem, float* D, int64_t* I, const int64_t* id_map, cudaStream_t st) {
+    static PerDeviceSize configured;
+    if (smem > 48 * 1024 && configured.raise(smem))
+        cudaFuncSetAttribute(refine_exact_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    refine_exact_kernel<T><<<nq, 256, smem, st>>>(Q, X, d, I_in, k_in, k_out, P, D, I, id_map);
+}
+
+int launch_refine_exact(const float* Q, int nq, const void* X, int elem_bytes, int d, const int64_t* I_in, int k_in,
+                        int k_out, float* D, int64_t* I, const int64_t* id_map, cudaStream_t st) {
     if (nq <= 0) return 0;
     const int P = next_pow2(max(2, k_in));
     const size_t smem = (size_t)P * 8 + (size_t)d * 4;
     if (smem > 200 * 1024) return -1;
-    static PerDeviceSize configured;
-    if (smem > 48 * 1024 && configured.raise(smem))
-        cudaFuncSetAttribute(refine_exact_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    refine_exact_kernel<<<nq, 256, smem, st>>>(Q, X, d, I_in, k_in, k_out, P, D, I, id_map);
+    if (elem_bytes == 2)
+        launch_refine_exact_t(Q, nq, static_cast<const __half*>(X), d, I_in, k_in, k_out, P, smem, D, I, id_map, st);
+    else
+        launch_refine_exact_t(Q, nq, static_cast<const float*>(X), d, I_in, k_in, k_out, P, smem, D, I, id_map, st);
     return 0;
 }
 

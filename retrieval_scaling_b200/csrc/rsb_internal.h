@@ -54,8 +54,9 @@ void launch_select_rows(const float* S, int nrows, int ncols, int ld, unsigned c
                         u64* out_keys, int* out_cnt, int items_per_row, int item_base, cudaStream_t st);
 void launch_merge_items(const u64* keys, const int* cnt, int nq, int nitems, int k_item, int k_out,
                         const int64_t* ids, int64_t id_offset, float* D, int64_t* I, cudaStream_t st);
-int launch_refine_exact(const float* Q, int nq, const float* X, int d, const int64_t* I_in, int k_in, int k_out,
-                        float* D, int64_t* I, const int64_t* id_map, cudaStream_t st);
+// X [*, d] rows of elem_bytes 4 (fp32) or 2 (fp16)
+int launch_refine_exact(const float* Q, int nq, const void* X, int elem_bytes, int d, const int64_t* I_in, int k_in,
+                        int k_out, float* D, int64_t* I, const int64_t* id_map, cudaStream_t st);
 int launch_merge_shards(const float* D_all, const int64_t* I_all, int nshards, int nq, int k, int k_out, float* D,
                         int64_t* I, cudaStream_t st);
 int launch_merge_shards_peers(const float* const* D_ptrs, const int64_t* const* I_ptrs, int nshards, int nq, int k,
@@ -92,9 +93,19 @@ bool launch_gemm_tf32x3_topt(const float* Ah, const float* Al, int M, const floa
 // rsb_dense.cu: top-kc of a row's candidates + exactness check (flag) ; exhaustive fp32 re-do of flagged rows
 int launch_select_cands(const u64* cand, int nrows, int ncand, const unsigned* xbound, int nx, int kc, u64* out_keys,
                         int* out_cnt, int items_per_row, int item, unsigned char* flags, cudaStream_t st);
-void launch_exact_rows(const float* Q, int nrows, const float* X, int ncols, int d, unsigned col_base,
+void launch_exact_rows(const float* Q, int nrows, const void* X, int elem_bytes, int ncols, int d, unsigned col_base,
                        const unsigned char* flags, int kc, u64* out_keys, int* out_cnt, int items_per_row, int item,
                        cudaStream_t st);
+
+// ---- rsb_tf32.cu, fp16 form (Flat with fp16 storage): the database rows are the fp16 B operand as stored ------
+// queries [M, K] fp32 -> per row a power-of-two scale s (largest |element| * s in [2^14, 2^15)), hi = fp16(q s),
+// lo = fp16(q s - hi), inv = 1 / s
+void launch_split_f16(const float* q, int M, int K, void* hi, void* lo, float* inv, cudaStream_t st);
+// as launch_gemm_tf32x3 / _topt with S = (hi + lo) . B^T * inv[row]; B [N, K] fp16; K % 64 == 0
+bool launch_gemm_f16x2(const void* Ah, const void* Al, const float* inv, int M, const void* B, int N, int K, float* C,
+                       int ldc, cudaStream_t st);
+bool launch_gemm_f16x2_topt(const void* Ah, const void* Al, const float* inv, int M, const void* B, int N, int K,
+                            unsigned col_base, u64* cand, unsigned* xbound, cudaStream_t st);
 
 // ---- rsb_ivf.cu -----------------------------------------------------------------------------------------
 // (query, list) work list, sorted by list so that concurrently running blocks share inverted lists in L2.
@@ -136,8 +147,8 @@ struct ScanArgs {
     unsigned* dbg_flag;           // nullable: 1 = literal-offset LDS path ran, 2 = generic path
 };
 
-// IVF-Flat: vecs [nslots, d] float32 in CSR order, queries [nq, d]
-void launch_ivfflat_scan(const ScanArgs& a, const float* queries, const float* vecs, int d, int nq,
+// IVF-Flat: vecs [nslots, d] in CSR order, fp32 (elem_bytes 4) or fp16 (elem_bytes 2); queries [nq, d] fp32
+void launch_ivfflat_scan(const ScanArgs& a, const float* queries, const void* vecs, int elem_bytes, int d, int nq,
                          cudaStream_t st);
 
 // IVF-PQ
@@ -182,6 +193,8 @@ void launch_slot_of_sorted(const int32_t* sorted_list, int64_t n, const int64_t*
 void launch_fill_i64(int64_t* p, int64_t n, int64_t v, cudaStream_t st);
 void launch_iota_i64(int64_t* p, int64_t n, int64_t start, cudaStream_t st);
 void launch_i64_to_i32(const int64_t* src, int64_t n, int32_t* dst, cudaStream_t st);
+void launch_f32_to_f16(const float* src, size_t n, void* dst, cudaStream_t st);   // round to nearest even
+void launch_f16_to_f32(const void* src, size_t n, float* dst, cudaStream_t st);
 // copy `bytes` (multiple of 16) from src to dst_ptrs[p] + dst_offset for every p < npeers (peer-mapped destinations)
 void launch_peer_broadcast(const void* src, size_t bytes, void* const* dst_ptrs, int npeers, size_t dst_offset,
                            cudaStream_t st);

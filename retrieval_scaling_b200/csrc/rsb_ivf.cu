@@ -161,15 +161,18 @@ __device__ __forceinline__ void raise_tau(const ScanArgs& a, int q, unsigned v) 
 // IVF-Flat list scan.  One block per (query, list) item (persistent blocks, dynamic scheduler).  A warp scores
 // two stored vectors per step: 128-bit coalesced loads of the vectors, the query staged in shared memory,
 // fp32 FMA, a 5-shuffle transposing reduction; scores above the running threshold go to the block's candidate
-// buffer.  HBM/L2-bandwidth bound: 4*d bytes per scored vector.
+// buffer.  HBM/L2-bandwidth bound: 4*d bytes per scored vector (fp32 rows) or 2*d (fp16 rows: lane l loads the
+// 4 halves of elements 4l + 128j .. +3 with one 8-byte load and runs the fp32 kernel's fmaf sequence on them, so
+// scores are bit-identical to those of fp32 rows holding the same values).
 // =============================================================================================================
 constexpr int FS_THREADS = 256;
 constexpr int FS_WARPS = FS_THREADS / 32;
 constexpr int FS_CHECK = 16;                             // iterations between capacity checks
 constexpr int FS_SLACK = FS_CHECK * FS_WARPS * 2;        // candidates appended between checks (256)
 
+template <typename T>
 __global__ __launch_bounds__(FS_THREADS)
-void ivfflat_scan_kernel(ScanArgs a, const float* __restrict__ queries, const float* __restrict__ vecs, int d,
+void ivfflat_scan_kernel(ScanArgs a, const float* __restrict__ queries, const T* __restrict__ vecs, int d,
                          int cap) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float* qs = reinterpret_cast<float*>(smem_raw);
@@ -200,13 +203,13 @@ void ivfflat_scan_kernel(ScanArgs a, const float* __restrict__ queries, const fl
         for (int it = 0; it < n_iter; ++it) {
             const int v0 = (it * FS_WARPS + warp) * 2, v1 = v0 + 1;
             const bool ok0 = v0 < len, ok1 = v1 < len;
-            const float* p0 = vecs + (size_t)(base + (ok0 ? v0 : 0)) * d;
-            const float* p1 = vecs + (size_t)(base + (ok1 ? v1 : 0)) * d;
+            const T* p0 = vecs + (size_t)(base + (ok0 ? v0 : 0)) * d;
+            const T* p1 = vecs + (size_t)(base + (ok1 ? v1 : 0)) * d;
             float a0 = 0.f, a1 = 0.f;
 #pragma unroll 6
             for (int c = lane * 4; c < d; c += 128) {
-                const float4 x0 = __ldg(reinterpret_cast<const float4*>(p0 + c));
-                const float4 x1 = __ldg(reinterpret_cast<const float4*>(p1 + c));
+                const float4 x0 = load_row4(p0 + c);
+                const float4 x1 = load_row4(p1 + c);
                 const float4 qv = *reinterpret_cast<const float4*>(qs + c);
                 a0 = fmaf(x0.x, qv.x, a0); a0 = fmaf(x0.y, qv.y, a0); a0 = fmaf(x0.z, qv.z, a0); a0 = fmaf(x0.w, qv.w, a0);
                 a1 = fmaf(x1.x, qv.x, a1); a1 = fmaf(x1.y, qv.y, a1); a1 = fmaf(x1.z, qv.z, a1); a1 = fmaf(x1.w, qv.w, a1);
@@ -241,20 +244,27 @@ void ivfflat_scan_kernel(ScanArgs a, const float* __restrict__ queries, const fl
 
 static int num_sms() { return device_num_sms(); }
 
-void launch_ivfflat_scan(const ScanArgs& a, const float* queries, const float* vecs, int d, int nq,
+template <typename T>
+static void launch_ivfflat_scan_t(const ScanArgs& a, const float* queries, const T* vecs, int d, int npairs,
+                                  cudaStream_t st) {
+    const int cap = cand_capacity(a.k, FS_SLACK);
+    const size_t smem = (((size_t)d * 4 + 15) & ~(size_t)15) + (size_t)cap * 8;
+    cudaFuncSetAttribute(ivfflat_scan_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    int occ = 1;
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, ivfflat_scan_kernel<T>, FS_THREADS, smem);
+    if (occ < 1) occ = 1;
+    const int grid = min(npairs, num_sms() * occ);
+    ivfflat_scan_kernel<T><<<grid, FS_THREADS, smem, st>>>(a, queries, vecs, d, cap);
+}
+
+void launch_ivfflat_scan(const ScanArgs& a, const float* queries, const void* vecs, int elem_bytes, int d, int nq,
                          cudaStream_t st) {
     const int npairs = nq * a.nprobe;
     if (!a.tau_external) cudaMemsetAsync(a.tau, 0, (size_t)nq * 4, st);
     cudaMemsetAsync(a.out_cnt, 0, (size_t)npairs * 4, st);
     if (npairs == 0) return;
-    const int cap = cand_capacity(a.k, FS_SLACK);
-    const size_t smem = (((size_t)d * 4 + 15) & ~(size_t)15) + (size_t)cap * 8;
-    cudaFuncSetAttribute(ivfflat_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    int occ = 1;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, ivfflat_scan_kernel, FS_THREADS, smem);
-    if (occ < 1) occ = 1;
-    const int grid = min(npairs, num_sms() * occ);
-    ivfflat_scan_kernel<<<grid, FS_THREADS, smem, st>>>(a, queries, vecs, d, cap);
+    if (elem_bytes == 2) launch_ivfflat_scan_t(a, queries, static_cast<const __half*>(vecs), d, npairs, st);
+    else launch_ivfflat_scan_t(a, queries, static_cast<const float*>(vecs), d, npairs, st);
 }
 
 // =============================================================================================================
@@ -1261,6 +1271,24 @@ void launch_fill_i64(int64_t* p, int64_t n, int64_t v, cudaStream_t st) {
 void launch_iota_i64(int64_t* p, int64_t n, int64_t start, cudaStream_t st) {
     if (n <= 0) return;
     fill_i64_kernel<<<(int)std::min<int64_t>(4096, (n + 255) / 256), 256, 0, st>>>(p, n, start, 1);
+}
+
+// storage conversions of rsb_add: fp32 -> fp16 rounds to nearest even; fp16 -> fp32 is exact
+__global__ void f32_to_f16_kernel(const float* __restrict__ src, size_t n, __half* __restrict__ dst) {
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+        dst[i] = __float2half_rn(src[i]);
+}
+__global__ void f16_to_f32_kernel(const __half* __restrict__ src, size_t n, float* __restrict__ dst) {
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+        dst[i] = __half2float(src[i]);
+}
+void launch_f32_to_f16(const float* src, size_t n, void* dst, cudaStream_t st) {
+    if (n == 0) return;
+    f32_to_f16_kernel<<<(int)std::min<size_t>(8192, (n + 255) / 256), 256, 0, st>>>(src, n, static_cast<__half*>(dst));
+}
+void launch_f16_to_f32(const void* src, size_t n, float* dst, cudaStream_t st) {
+    if (n == 0) return;
+    f16_to_f32_kernel<<<(int)std::min<size_t>(8192, (n + 255) / 256), 256, 0, st>>>(static_cast<const __half*>(src), n, dst);
 }
 
 __global__ void i64_to_i32_kernel(const int64_t* __restrict__ src, int64_t n, int32_t* __restrict__ dst) {

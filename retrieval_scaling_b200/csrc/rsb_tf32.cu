@@ -8,6 +8,13 @@
 // 32 fp32 = one swizzle row per K step) -> 3-stage shared-memory ring of {Ah, Al, Bh, Bl} tiles filled by one
 // producer thread -> two consumer warpgroups, each issuing 12 wgmma.m64n128k8.tf32 per stage (4 K-slices x 3
 // products) on its 64 rows -> epilogue from the accumulator registers.
+//
+// fp16 form (F16 = true; Flat indexes with fp16 storage): B is the database as stored (fp16 rows, exact), so no split
+// copy of it exists.  Each query row is scaled by a power of two s that puts its largest |element| in [2^14, 2^15)
+// (exact), and split into fp16 hi = fp16(q s), lo = fp16(q s - hi): 22 significant bits, as many as the 3xTF32 query
+// split; there is no lo.lo term because B is exact.  Per stage two wgmma.m64n128k16.f16 per 16-wide K-slice (lo.B,
+// then hi.B) share the B tile, 64 fp16 = one swizzle row per K step; the epilogue multiplies by 1 / s.  Both forms
+// share the mainloop ring and the epilogues below (score tile, or the fused top-8 candidate + bound filter).
 #include "rsb_common.cuh"
 #include "rsb_internal.h"
 #include "rsb_tc.cuh"
@@ -19,10 +26,10 @@ namespace rsb {
 
 using namespace rsbtc;
 
-constexpr int T_BM = 128, T_BN = 128, T_BK = 32, T_STAGES = 3;
+constexpr int T_BM = 128, T_BN = 128, T_BK = 32, T_BK16 = 64, T_STAGES = 3;
 constexpr int T_THREADS = 384;                                // warpgroup 0: TMA producer, warpgroups 1-2: MMA + epilogue
 constexpr int T_TILE_BYTES = 128 * T_BK * 4;                  // 16 KB
-constexpr int T_STAGE_BYTES = 4 * T_TILE_BYTES;               // Ah, Al, Bh, Bl
+constexpr int T_STAGE_BYTES = 4 * T_TILE_BYTES;               // Ah, Al, Bh, Bl (fp16 form: Ah, Al, B)
 constexpr int T_SMEM = T_STAGES * T_STAGE_BYTES + 1024 + 256;
 constexpr int T_LDS = T_BN + 1;                               // row stride of the fused epilogue's staged tile (floats)
 static_assert(T_BM * T_LDS * 4 + T_BM * 9 * 8 <= T_STAGES * T_STAGE_BYTES, "staged tile must fit in the ring");
@@ -45,6 +52,36 @@ void launch_split_tf32(const float* x, size_t n, float* hi, float* lo, cudaStrea
     split_tf32_kernel<<<blocks, 256, 0, st>>>(x, n, hi, lo);
 }
 
+// one block of 128 threads per query row: scale to the top of the fp16 range, split into hi + lo
+__global__ __launch_bounds__(128)
+void split_f16_kernel(const float* __restrict__ q, int K, __half* __restrict__ hi, __half* __restrict__ lo,
+                      float* __restrict__ inv) {
+    __shared__ float s_max[4];
+    const float* row = q + (size_t)blockIdx.x * K;
+    float m = 0.f;
+    for (int c = threadIdx.x; c < K; c += 128) m = fmaxf(m, fabsf(row[c]));
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((threadIdx.x & 31) == 0) s_max[threadIdx.x >> 5] = m;
+    __syncthreads();
+    m = fmaxf(fmaxf(s_max[0], s_max[1]), fmaxf(s_max[2], s_max[3]));
+    int e = 0;
+    frexpf(m, &e);                                            // m = f 2^e, f in [0.5, 1)
+    const int sh = m > 0.f && isfinite(m) ? min(126, max(-126, 15 - e)) : 0;
+    const float s = ldexpf(1.f, sh);
+    for (int c = threadIdx.x; c < K; c += 128) {
+        const float v = row[c] * s;
+        const __half h = __float2half_rn(v);
+        hi[(size_t)blockIdx.x * K + c] = h;
+        lo[(size_t)blockIdx.x * K + c] = __float2half_rn(v - __half2float(h));   // v - h is exact in fp32
+    }
+    if (threadIdx.x == 0) inv[blockIdx.x] = ldexpf(1.f, -sh);
+}
+
+void launch_split_f16(const float* q, int M, int K, void* hi, void* lo, float* inv, cudaStream_t st) {
+    if (M <= 0) return;
+    split_f16_kernel<<<M, 128, 0, st>>>(q, K, static_cast<__half*>(hi), static_cast<__half*>(lo), inv);
+}
+
 // FUSED = false: the 128 x 128 score tile goes to C.  FUSED = true: the score tile never goes to HBM.  Every row of
 // the tile keeps its 9 largest scores (sorted insertion in column order, strict comparisons => ties keep the lower
 // column); the top 8 are emitted as candidates (64 B per row per 128-column tile) together with the 9th as a bound:
@@ -53,12 +90,15 @@ void launch_split_tf32(const float* x, size_t n, float* hi, float* lo, cudaStrea
 // -- select_cands_kernel checks exactly that and flags the (rare) rows for which it fails; those are re-done
 // exhaustively in fp32 by exact_rows_kernel.  The result is therefore the exact top-kc of the 3xTF32 scores without
 // writing and re-reading nq x nlist x 4 bytes.
-template <bool FUSED>
+// F16: fp16 operands (tmBl unused), scores multiplied by inv[row] before either epilogue.
+template <bool F16, bool FUSED>
 __global__ __launch_bounds__(T_THREADS, 1)
-void gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
-                        const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl,
-                        float* __restrict__ C, int ldc, u64* __restrict__ cand, unsigned* __restrict__ xbound,
-                        int M, int N, int K, unsigned col_base, int m_fastest) {
+void gemm_ip_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
+                       const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl,
+                       const float* __restrict__ inv, float* __restrict__ C, int ldc, u64* __restrict__ cand,
+                       unsigned* __restrict__ xbound, int M, int N, int K, unsigned col_base, int m_fastest) {
+    constexpr int BK = F16 ? T_BK16 : T_BK;                   // K elements per stage: one 128-byte swizzle row
+    constexpr int STAGE_TX = (F16 ? 3 : 4) * T_TILE_BYTES;
     extern __shared__ unsigned char smem_dyn[];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + T_STAGES * T_STAGE_BYTES);
@@ -75,7 +115,7 @@ void gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_c
         tn = m_fastest ? (int)blockIdx.x / tiles_m : (int)blockIdx.x % nhalf;
     }
     const int m0 = tm * T_BM, n0 = tn * T_BN;
-    const int nk = K / T_BK;
+    const int nk = K / BK;
     if (FUSED && n0 >= N) {                                   // the empty second half of a 256-column group: no candidates
         const int row = m0 + (int)threadIdx.x;
         if (threadIdx.x < T_BM && row < M) {
@@ -92,7 +132,7 @@ void gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_c
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmAh)) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmAl)) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmBh)) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmBl)) : "memory");
+        if (!F16) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmBl)) : "memory");
         for (int s = 0; s < T_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }   // 8 consumer warps
         fence_barrier_init();
     }
@@ -104,11 +144,11 @@ void gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_c
                 const int s = kb % T_STAGES;
                 mbar_wait(&empty[s], ((kb / T_STAGES) & 1) ^ 1);   // the first pass over the ring falls through
                 unsigned char* base = smem + s * T_STAGE_BYTES;
-                mbar_expect_tx(&full[s], T_STAGE_BYTES);
-                tma_load_2d(base + 0 * T_TILE_BYTES, &tmAh, &full[s], kb * T_BK, m0);   // rows past M / N read as zero
-                tma_load_2d(base + 1 * T_TILE_BYTES, &tmAl, &full[s], kb * T_BK, m0);
-                tma_load_2d(base + 2 * T_TILE_BYTES, &tmBh, &full[s], kb * T_BK, n0);
-                tma_load_2d(base + 3 * T_TILE_BYTES, &tmBl, &full[s], kb * T_BK, n0);
+                mbar_expect_tx(&full[s], STAGE_TX);
+                tma_load_2d(base + 0 * T_TILE_BYTES, &tmAh, &full[s], kb * BK, m0);   // rows past M / N read as zero
+                tma_load_2d(base + 1 * T_TILE_BYTES, &tmAl, &full[s], kb * BK, m0);
+                tma_load_2d(base + 2 * T_TILE_BYTES, &tmBh, &full[s], kb * BK, n0);
+                if (!F16) tma_load_2d(base + 3 * T_TILE_BYTES, &tmBl, &full[s], kb * BK, n0);
             }
         }
         return;
@@ -128,12 +168,21 @@ void gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_c
         const uint64_t bl = make_sw128_kmajor_desc(base + 3 * T_TILE_BYTES);
         acc_fence(acc);
         wgmma_fence();
+        if (F16) {
 #pragma unroll
-        for (int k4 = 0; k4 < T_BK / 8; ++k4) {               // K = 8 tf32 = 32 bytes: +2 in the (addr >> 4) field
-            const uint64_t o = (uint64_t)(k4 * 2);
-            wgmma_tf32_n128(acc, al + o, bh + o);             // small terms first, the dominant Ah.Bh product last
-            wgmma_tf32_n128(acc, ah + o, bl + o);
-            wgmma_tf32_n128(acc, ah + o, bh + o);
+            for (int k4 = 0; k4 < T_BK16 / 16; ++k4) {        // K = 16 fp16 = 32 bytes: +2 in the (addr >> 4) field
+                const uint64_t o = (uint64_t)(k4 * 2);
+                wgmma_f16_n128(acc, al + o, bh + o);          // the small term first, then the dominant hi.B product
+                wgmma_f16_n128(acc, ah + o, bh + o);
+            }
+        } else {
+#pragma unroll
+            for (int k4 = 0; k4 < T_BK / 8; ++k4) {           // K = 8 tf32 = 32 bytes: +2 in the (addr >> 4) field
+                const uint64_t o = (uint64_t)(k4 * 2);
+                wgmma_tf32_n128(acc, al + o, bh + o);         // small terms first, the dominant Ah.Bh product last
+                wgmma_tf32_n128(acc, ah + o, bl + o);
+                wgmma_tf32_n128(acc, ah + o, bh + o);
+            }
         }
         wgmma_commit();
         acc_fence(acc);
@@ -148,6 +197,15 @@ void gemm_tf32x3_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_c
 
     const int r_lo = cw * 64 + (warp & 3) * 16 + (lane >> 2);   // tile row of acc[4 j + c]; acc[4 j + 2 + c]: r_lo + 8
     const int c_lo = 2 * (lane & 3);                            // tile column of acc[4 j]: 8 j + c_lo
+    if (F16) {                                                  // undo the per-row query scale (a power of two: exact)
+        const float s0 = m0 + r_lo < M ? inv[m0 + r_lo] : 0.f;
+        const float s1 = m0 + r_lo + 8 < M ? inv[m0 + r_lo + 8] : 0.f;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            acc[4 * j] *= s0; acc[4 * j + 1] *= s0;
+            acc[4 * j + 2] *= s1; acc[4 * j + 3] *= s1;
+        }
+    }
     if (!FUSED) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -232,6 +290,29 @@ static bool make_maps(CUtensorMap (&m)[4], const float* Ah, const float* Al, int
 // candidates kept per row per call: 8 per 128-column tile, counted in pairs of tiles (256 columns)
 size_t fused_cand_per_row(int N) { return (size_t)((N + 255) / 256) * 2 * 8; }
 
+template <bool F16>
+static void launch_gemm_topt(const CUtensorMap (&m)[4], const float* inv, int M, int N, int K, unsigned col_base, u64* cand,
+                             unsigned* xbound, cudaStream_t st) {
+    static PerDeviceSize configured;
+    if (configured.raise(T_SMEM))
+        cudaFuncSetAttribute(gemm_ip_tc_kernel<F16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, T_SMEM);
+    const int ntiles = ((M + T_BM - 1) / T_BM) * (int)(fused_cand_per_row(N) / 8);
+    static const int m_fastest = getenv("RSB_COARSE_N_FASTEST") ? 0 : 1;
+    gemm_ip_tc_kernel<F16, true><<<ntiles, T_THREADS, T_SMEM, st>>>(m[0], m[1], m[2], m[3], inv, nullptr, 0, cand, xbound,
+                                                                    M, N, K, col_base, m_fastest);
+}
+
+template <bool F16>
+static void launch_gemm_scores(const CUtensorMap (&m)[4], const float* inv, int M, int N, int K, float* C, int ldc,
+                               cudaStream_t st) {
+    static PerDeviceSize configured;
+    if (configured.raise(T_SMEM))
+        cudaFuncSetAttribute(gemm_ip_tc_kernel<F16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, T_SMEM);
+    dim3 grid((N + T_BN - 1) / T_BN, (M + T_BM - 1) / T_BM);
+    gemm_ip_tc_kernel<F16, false><<<grid, T_THREADS, T_SMEM, st>>>(m[0], m[1], m[2], m[3], inv, C, ldc, nullptr, nullptr,
+                                                                   M, N, K, 0u, 0);
+}
+
 // Ah/Al [M,K], Bh/Bl [N,K] fp32 (already split).  cand [M, fused_cand_per_row(N)] u64 keys (score order high word,
 // 0xFFFFFFFF - (col_base + column) low word, 0 = empty), xbound [M, fused_cand_per_row(N) / 8] (ordered score of the
 // best dropped element of each 128-column tile, 0 = none).  Returns false if the path cannot run (caller falls back).
@@ -241,13 +322,7 @@ bool launch_gemm_tf32x3_topt(const float* Ah, const float* Al, int M, const floa
     if (K % T_BK) return false;
     CUtensorMap m[4];
     if (!make_maps(m, Ah, Al, M, Bh, Bl, N, K)) return false;
-    static PerDeviceSize configured;
-    if (configured.raise(T_SMEM))
-        cudaFuncSetAttribute(gemm_tf32x3_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, T_SMEM);
-    const int ntiles = ((M + T_BM - 1) / T_BM) * (int)(fused_cand_per_row(N) / 8);
-    static const int m_fastest = getenv("RSB_COARSE_N_FASTEST") ? 0 : 1;
-    gemm_tf32x3_kernel<true><<<ntiles, T_THREADS, T_SMEM, st>>>(m[0], m[1], m[2], m[3], nullptr, 0, cand, xbound, M, N, K,
-                                                                 col_base, m_fastest);
+    launch_gemm_topt<false>(m, nullptr, M, N, K, col_base, cand, xbound, st);
     return true;
 }
 
@@ -261,11 +336,37 @@ bool launch_gemm_tf32x3(const float* Ah, const float* Al, int M, const float* Bh
     if (K % T_BK) return false;
     CUtensorMap m[4];
     if (!make_maps(m, Ah, Al, M, Bh, Bl, N, K)) return false;
-    static PerDeviceSize configured;
-    if (configured.raise(T_SMEM))
-        cudaFuncSetAttribute(gemm_tf32x3_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, T_SMEM);
-    dim3 grid((N + T_BN - 1) / T_BN, (M + T_BM - 1) / T_BM);
-    gemm_tf32x3_kernel<false><<<grid, T_THREADS, T_SMEM, st>>>(m[0], m[1], m[2], m[3], C, ldc, nullptr, nullptr, M, N, K, 0u, 0);
+    launch_gemm_scores<false>(m, nullptr, M, N, K, C, ldc, st);
+    return true;
+}
+
+// Ah/Al [M,K] fp16 (launch_split_f16), inv [M], B [N,K] fp16 rows as stored.  K % 64 == 0.  Returns false if the
+// tensor maps cannot be encoded; there is no CUDA-core fp16 path to fall back to (the caller reports an error).
+static bool make_maps_f16(CUtensorMap (&m)[4], const void* Ah, const void* Al, int M, const void* B, int N, int K) {
+    if (!(make_map_2d(&m[0], Ah, (uint64_t)M, (uint64_t)K, T_BM, 2) && make_map_2d(&m[1], Al, (uint64_t)M, (uint64_t)K, T_BM, 2) &&
+          make_map_2d(&m[2], B, (uint64_t)N, (uint64_t)K, T_BN, 2)))
+        return false;
+    m[3] = m[2];                                              // unused by the fp16 kernel
+    return true;
+}
+
+bool launch_gemm_f16x2(const void* Ah, const void* Al, const float* inv, int M, const void* B, int N, int K, float* C,
+                       int ldc, cudaStream_t st) {
+    if (M <= 0 || N <= 0) return true;
+    if (K % T_BK16) return false;
+    CUtensorMap m[4];
+    if (!make_maps_f16(m, Ah, Al, M, B, N, K)) return false;
+    launch_gemm_scores<true>(m, inv, M, N, K, C, ldc, st);
+    return true;
+}
+
+bool launch_gemm_f16x2_topt(const void* Ah, const void* Al, const float* inv, int M, const void* B, int N, int K,
+                            unsigned col_base, u64* cand, unsigned* xbound, cudaStream_t st) {
+    if (M <= 0 || N <= 0) return true;
+    if (K % T_BK16) return false;
+    CUtensorMap m[4];
+    if (!make_maps_f16(m, Ah, Al, M, B, N, K)) return false;
+    launch_gemm_topt<true>(m, inv, M, N, K, col_base, cand, xbound, st);
     return true;
 }
 

@@ -41,6 +41,37 @@ def _dev_f32(x, device) -> torch.Tensor:
     return x.to(device=device, dtype=torch.float32, non_blocking=True).contiguous()
 
 
+def _dev_rows(x, device) -> torch.Tensor:
+    """Vectors to add: fp16 tensors / arrays stay fp16 (they cross PCIe at 2 bytes per element; rsb_add_typed converts
+    them on the device), anything else becomes fp32 as in _dev_f32."""
+    if isinstance(x, np.ndarray):
+        x = torch.from_numpy(np.ascontiguousarray(x))
+    if not isinstance(x, torch.Tensor):
+        x = torch.as_tensor(x)
+    dtype = torch.float16 if x.dtype == torch.float16 else torch.float32
+    return x.to(device=device, dtype=dtype, non_blocking=True).contiguous()
+
+
+# storage dtypes of Flat / IVF-Flat vectors (rsb_*_create_dtype) and of IndexRefine's store
+_STORE_DTYPES = {"float16": (torch.float16, _lib.RSB_DTYPE_F16), "float32": (torch.float32, _lib.RSB_DTYPE_F32)}
+
+
+def _check_dtype(dtype: str, what: str = "dtype") -> str:
+    if dtype not in _STORE_DTYPES:
+        raise ValueError(f"{what} must be float16 or float32, got {dtype!r}")
+    return dtype
+
+
+def _as_storage(x: np.ndarray, dtype: str, what: str) -> np.ndarray:
+    """Host vectors for an index that stores `dtype`: an fp16 index accepts only values that round-trip through fp16."""
+    if dtype != "float16" or x.dtype == np.float16:
+        return x
+    xh = x.astype(np.float16)
+    if not np.array_equal(xh.astype(x.dtype), x):
+        raise ValueError(f"{what}: not every value is representable in float16; use float32 storage")
+    return xh
+
+
 def _ptr(t: Optional[torch.Tensor]):
     return ctypes.c_void_p(t.data_ptr()) if t is not None and t.numel() > 0 else ctypes.c_void_p(0)
 
@@ -51,6 +82,7 @@ def _stream():
 
 class _IndexBase:
     kind = None
+    dtype = "float32"      # storage dtype of the vectors (Flat / IVF-Flat may hold float16)
 
     def __init__(self, d: int, device=None):
         _require_cuda()
@@ -101,7 +133,7 @@ class _IndexBase:
 
     def add(self, x, ids=None) -> None:
         with torch.cuda.device(self.device):
-            x = _dev_f32(x, self.device)
+            x = _dev_f32(x, self.device) if self.kind == _lib.RSB_IVFPQ else _dev_rows(x, self.device)
             if x.dim() != 2 or x.shape[1] != self.d:
                 raise ValueError(f"expected [n, {self.d}] vectors, got {tuple(x.shape)}")
             n = x.shape[0]
@@ -111,7 +143,11 @@ class _IndexBase:
                 if idt.numel() != n:
                     raise ValueError("ids and x disagree on n")
             ws = self._workspace(self.L.rsb_add_workspace_bytes(self._h, n))
-            _lib.check(self.L.rsb_add(self._h, _ptr(x), n, _ptr(idt), _ptr(ws), ws.numel(), _stream()))
+            if x.dtype == torch.float16:
+                _lib.check(self.L.rsb_add_typed(self._h, _ptr(x), _lib.RSB_DTYPE_F16, n, _ptr(idt), _ptr(ws), ws.numel(),
+                                                _stream()))
+            else:
+                _lib.check(self.L.rsb_add(self._h, _ptr(x), n, _ptr(idt), _ptr(ws), ws.numel(), _stream()))
             torch.cuda.current_stream().synchronize()  # x / idt may be temporaries
 
     def finalize(self) -> None:
@@ -170,7 +206,7 @@ class _IndexBase:
             if self.kind == _lib.RSB_IVFPQ:
                 payload = torch.empty((n, self._info(_lib.INFO_M)), dtype=torch.uint8, device=self.device)
             else:
-                payload = torch.empty((n, self.d), dtype=torch.float32, device=self.device)
+                payload = torch.empty((n, self.d), dtype=_STORE_DTYPES[self.dtype][0], device=self.device)
             ids = torch.empty(n, dtype=torch.int64, device=self.device)
             _lib.check(self.L.rsb_export_lists(self._h, _ptr(off), _ptr(payload), _ptr(ids), _stream()))
             torch.cuda.current_stream().synchronize()
@@ -178,13 +214,21 @@ class _IndexBase:
 
 
 class IndexFlatIP(_IndexBase):
-    """faiss.IndexFlatIP(d)  (reference: src/indicies/flat.py:42)."""
+    """faiss.IndexFlatIP(d)  (reference: src/indicies/flat.py:42).
+
+    dtype="float16" stores the vectors as fp16 (faiss IndexScalarQuantizer(QT_fp16, METRIC_INNER_PRODUCT)): half the
+    bytes, scored on tensor cores from the fp16 rows at any size that fits (d % 64 == 0, else NotImplementedError),
+    with exact fp32 final scores.  Lossless for the fp16 embeddings the embedding task writes."""
     kind = _lib.RSB_FLAT
 
-    def __init__(self, d: int, device=None):
+    def __init__(self, d: int, device=None, dtype: str = "float32"):
         super().__init__(d, device)
+        self.dtype = _check_dtype(dtype)
         with torch.cuda.device(self.device):
-            _lib.check(self.L.rsb_flat_create(self.d, ctypes.byref(self._h)))
+            if self.dtype == "float32":
+                _lib.check(self.L.rsb_flat_create(self.d, ctypes.byref(self._h)))
+            else:
+                _lib.check(self.L.rsb_flat_create_dtype(self.d, _STORE_DTYPES[self.dtype][1], ctypes.byref(self._h)))
 
 
 class _IVFBase(_IndexBase):
@@ -250,11 +294,15 @@ class _IVFBase(_IndexBase):
 
     def add_preassigned(self, x, lists, ids=None) -> None:
         with torch.cuda.device(self.device):
-            x = _dev_f32(x, self.device)
+            x = _dev_f32(x, self.device) if self.kind == _lib.RSB_IVFPQ else _dev_rows(x, self.device)
             n = x.shape[0]
             lt = torch.as_tensor(lists).to(device=self.device, dtype=torch.int32).contiguous()
             idt = None if ids is None else torch.as_tensor(ids).to(device=self.device, dtype=torch.int64).contiguous()
-            _lib.check(self.L.rsb_add_preassigned(self._h, _ptr(x), n, _ptr(idt), _ptr(lt), _stream()))
+            if x.dtype == torch.float16:
+                _lib.check(self.L.rsb_add_preassigned_typed(self._h, _ptr(x), _lib.RSB_DTYPE_F16, n, _ptr(idt), _ptr(lt),
+                                                            _stream()))
+            else:
+                _lib.check(self.L.rsb_add_preassigned(self._h, _ptr(x), n, _ptr(idt), _ptr(lt), _stream()))
             torch.cuda.current_stream().synchronize()
 
     def list_sizes(self) -> torch.Tensor:
@@ -270,13 +318,21 @@ class _IVFBase(_IndexBase):
 
 
 class IndexIVFFlat(_IVFBase):
-    """faiss.IndexIVFFlat(IndexFlatIP(d), d, nlist, METRIC_INNER_PRODUCT)  (src/indicies/ivf_flat.py:143-149)."""
+    """faiss.IndexIVFFlat(IndexFlatIP(d), d, nlist, METRIC_INNER_PRODUCT)  (src/indicies/ivf_flat.py:143-149).
+
+    dtype="float16" stores the vectors as fp16 (faiss IndexIVFScalarQuantizer(QT_fp16, by_residual=False)): the list
+    scan reads half the bytes, and ids and scores are bit-identical to an fp32 index holding the same values."""
     kind = _lib.RSB_IVFFLAT
 
-    def __init__(self, d: int, nlist: int, device=None):
+    def __init__(self, d: int, nlist: int, device=None, dtype: str = "float32"):
         super().__init__(d, nlist, device)
+        self.dtype = _check_dtype(dtype)
         with torch.cuda.device(self.device):
-            _lib.check(self.L.rsb_ivfflat_create(self.d, self.nlist, ctypes.byref(self._h)))
+            if self.dtype == "float32":
+                _lib.check(self.L.rsb_ivfflat_create(self.d, self.nlist, ctypes.byref(self._h)))
+            else:
+                _lib.check(self.L.rsb_ivfflat_create_dtype(self.d, self.nlist, _STORE_DTYPES[self.dtype][1],
+                                                           ctypes.byref(self._h)))
 
     def train(self, x) -> None:
         with torch.cuda.device(self.device):
@@ -326,9 +382,6 @@ class IndexIVFPQ(_IVFBase):
             idt = None if ids is None else torch.as_tensor(ids).to(device=self.device, dtype=torch.int64).contiguous()
             _lib.check(self.L.rsb_add_codes(self._h, _ptr(ct), n, _ptr(idt), _ptr(lt), _stream()))
             torch.cuda.current_stream().synchronize()
-
-
-_STORE_DTYPES = {"float16": (torch.float16, _lib.RSB_DTYPE_F16), "float32": (torch.float32, _lib.RSB_DTYPE_F32)}
 
 
 class IndexRefine:
@@ -473,6 +526,8 @@ def _to_faiss_parts(index: _IndexBase) -> dict:
                 "xb": index.store.float().cpu().numpy(), "k_factor": float(index.k_factor)}
     off, payload, ids = index.export_lists()
     off, payload, ids = off.cpu().numpy(), payload.cpu().numpy(), ids.cpu().numpy()
+    # fp16 storage is written upcast to fp32 (exact): the file is the one the fp32 index of the same values writes
+    payload = payload.astype(np.float32) if payload.dtype == np.float16 else payload
     if index.kind == _lib.RSB_FLAT:
         if not np.array_equal(ids, np.arange(len(ids))):
             raise ValueError("faiss IndexFlatIP has no id map: only sequential ids can be written in faiss format")
@@ -483,9 +538,14 @@ def _to_faiss_parts(index: _IndexBase) -> dict:
     return {"kind": "IVFPQ", "codes": payload, "codebook": index.get_codebook().cpu().numpy(), **parts}
 
 
-def _from_faiss_parts(p: dict, device=None, refine_dtype: Optional[str] = None) -> _IndexBase:
+def _from_faiss_parts(p: dict, device=None, refine_dtype: Optional[str] = None,
+                      storage_dtype: Optional[str] = None) -> _IndexBase:
     if p.get("metric", 0) != 0 or p.get("quantizer_metric", 0) != 0:
         raise NotImplementedError("only METRIC_INNER_PRODUCT indexes are supported (the reference builds IP indexes only)")
+    if storage_dtype is not None:
+        _check_dtype(storage_dtype, "storage_dtype")
+        if p["kind"] not in ("Flat", "IVFFlat"):
+            raise ValueError(f"storage_dtype applies to Flat and IVFFlat indexes, not {p['kind']}")
     if p["kind"] == "Refine":
         kf = float(p["k_factor"])
         if kf != int(kf) or kf < 1:
@@ -503,18 +563,21 @@ def _from_faiss_parts(p: dict, device=None, refine_dtype: Optional[str] = None) 
         index.reserve(xb.shape[0])
         index.add_store(xb)
         return index
+    dtype = storage_dtype or "float32"
     if p["kind"] == "Flat":
-        index = IndexFlatIP(p["d"], device)
+        xb = _as_storage(p["xb"], dtype, "the Flat index's vectors") if p["ntotal"] else None
+        index = IndexFlatIP(p["d"], device, dtype=dtype)
         if p["ntotal"]:
-            index.add(p["xb"])
+            index.add(xb)
         return index
     nlist = p["nlist"]
     lists = np.repeat(np.arange(nlist, dtype=np.int32), np.diff(p["offsets"]))
     if p["kind"] == "IVFFlat":
-        index = IndexIVFFlat(p["d"], nlist, device)
+        xb = _as_storage(p["vectors"], dtype, "the IVFFlat index's vectors") if len(p["ids"]) else None
+        index = IndexIVFFlat(p["d"], nlist, device, dtype=dtype)
         index.set_centroids(p["centroids"])
         if len(p["ids"]):
-            index.add_preassigned(p["vectors"], lists, p["ids"])
+            index.add_preassigned(xb, lists, p["ids"])
     else:
         if not p.get("by_residual", True):
             raise NotImplementedError("IVFPQ without by_residual")
@@ -549,6 +612,8 @@ def write_index(index: _IndexBase, path: str, fmt: Optional[str] = None) -> None
             os.replace(tmp, path)
             return
     blob = {"magic": MAGIC, "kind": int(index.kind), "d": index.d, "nprobe": int(index.nprobe)}
+    if index.dtype != "float32":
+        blob["dtype"] = index.dtype                      # the payload below is kept as stored
     if isinstance(index, _IVFBase):
         blob["nlist"] = index.nlist
         try:
@@ -572,22 +637,31 @@ def write_index(index: _IndexBase, path: str, fmt: Optional[str] = None) -> None
     os.replace(tmp, path)
 
 
-def read_index(path: str, device=None, refine_dtype: Optional[str] = None) -> _IndexBase:
+def read_index(path: str, device=None, refine_dtype: Optional[str] = None,
+               storage_dtype: Optional[str] = None) -> _IndexBase:
     """Loads an RSB1 container or a faiss binary index file (auto-detected by its fourcc).  For an IndexRefineFlat
     file (IxRF) `refine_dtype` picks the store: "float32" (default) or "float16", which is accepted only when every
-    stored value round-trips through fp16 (ValueError otherwise)."""
+    stored value round-trips through fp16 (ValueError otherwise).  `storage_dtype` does the same for the vectors of a
+    Flat / IVFFlat index (IxFI / IwFl / RSB1); None keeps the file's dtype (fp32 for faiss files)."""
     from . import faiss_io
     if faiss_io.is_faiss_file(path):
-        return _from_faiss_parts(faiss_io.read_faiss(path), device, refine_dtype)
+        return _from_faiss_parts(faiss_io.read_faiss(path), device, refine_dtype, storage_dtype)
     with open(path, "rb") as f:
         blob = pickle.load(f)
     if not isinstance(blob, dict) or blob.get("magic") != MAGIC:
         raise ValueError(f"{path} is not an RSB1 index file")
     kind = blob["kind"]
+    if storage_dtype is not None:
+        _check_dtype(storage_dtype, "storage_dtype")
+        if kind not in (_lib.RSB_FLAT, _lib.RSB_IVFFLAT):
+            raise ValueError("storage_dtype applies to Flat and IVFFlat indexes only")
+    dtype = storage_dtype or blob.get("dtype", "float32")
+    if "payload" in blob and kind != _lib.RSB_IVFPQ:
+        blob["payload"] = _as_storage(blob["payload"], dtype, f"{path}: the index vectors")
     if kind == _lib.RSB_FLAT:
-        index = IndexFlatIP(blob["d"], device)
+        index = IndexFlatIP(blob["d"], device, dtype=dtype)
     elif kind == _lib.RSB_IVFFLAT:
-        index = IndexIVFFlat(blob["d"], blob["nlist"], device)
+        index = IndexIVFFlat(blob["d"], blob["nlist"], device, dtype=dtype)
     elif kind == _lib.RSB_IVFPQ:
         index = IndexIVFPQ(blob["d"], blob["nlist"], blob["M"], blob["nbits"], device)
     else:

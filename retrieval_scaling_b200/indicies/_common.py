@@ -77,24 +77,26 @@ class BaseIndexer:
     index_kind = "Flat"
 
     def __init__(self, embed_paths, index_path, meta_file, passage_dir=None, pos_map_save_path=None,
-                 dimension=768, trained_index_path=None, sample_train_size=1000000, probe=1):
+                 dimension=768, trained_index_path=None, sample_train_size=1000000, probe=1, storage_dtype=None):
         self.embed_paths = list(embed_paths) if embed_paths is not None else []
         self.index_path, self.meta_file = index_path, meta_file
         self.trained_index_path = trained_index_path
         self.passage_dir, self.pos_map_save_path = passage_dir, pos_map_save_path
         self.dimension, self.sample_size, self.probe = int(dimension), int(sample_train_size), int(probe)
         self.cuda = True   # informational: unlike the reference (`self.cuda = False`), search runs on the GPU
+        # datastore.index.storage_dtype (Flat / IVFFlat): None = fp32 vectors, the reference's upcast-on-load path
+        self.storage_dtype = storage_dtype
 
         if os.path.exists(index_path) and os.path.exists(meta_file):
             print("Loading index...")
-            self.index = rsb_index.read_index(index_path)
+            self.index = rsb_index.read_index(index_path, storage_dtype=storage_dtype)
             self.index_id_to_db_id = DbIdMap.load(meta_file)
         else:
             self.index_id_to_db_id = DbIdMap()
             self.index = self._new_index()
             if not self.index.is_trained:
                 if trained_index_path and os.path.exists(trained_index_path):
-                    self.index = rsb_index.read_index(trained_index_path)
+                    self.index = rsb_index.read_index(trained_index_path, storage_dtype=storage_dtype)
                 else:
                     print("Training index...")
                     self._sample_and_train_index()
@@ -129,7 +131,7 @@ class BaseIndexer:
         t0 = time.time()
         for i, p in enumerate(self.embed_paths):
             shard_id = iu.shard_id_of_embedding_path(p)
-            emb = iu.load_embedding_shard(p)
+            emb = self._load_shard_for_add(p)
             self.index.add(emb)
             self.index_id_to_db_id.extend_shard(shard_id, emb.shape[0])
             print("Added %d / %d shards, (%d min)" % (i + 1, len(self.embed_paths), (time.time() - t0) / 60))
@@ -138,6 +140,19 @@ class BaseIndexer:
         rsb_index.write_index(self.index, self.index_path)
         self.index_id_to_db_id.dump(self.meta_file)
         print(f"Total data indexed {len(self.index_id_to_db_id)}")
+
+    def _load_shard_for_add(self, path: str) -> np.ndarray:
+        """fp32 rows (the reference's upcast on load), or, with storage_dtype set, the rows as the embedding task
+        stored them: fp16 pickles go to the GPU as fp16.  An fp16 index refuses an fp32 shard whose values do not
+        round-trip through fp16, since its results would no longer be the reference's."""
+        if self.storage_dtype is None:
+            return iu.load_embedding_shard(path)
+        emb = iu.load_embedding_shard(path, dtype=None)
+        if emb.dtype not in (np.float16, np.float32):
+            emb = emb.astype(np.float32)
+        if self.storage_dtype == "float16":
+            emb = rsb_index._as_storage(emb, "float16", f"embedding shard {path}")
+        return emb
 
     # -- passages --------------------------------------------------------------------------------------------
     def load_psg_pos_id_map(self):

@@ -45,11 +45,26 @@ class Indexer(object):
             raise ValueError(f"datastore.index.refine_dtype must be float16 or float32, got {dtype!r}")
         return k_factor, dtype
 
+    @staticmethod
+    def storage_dtype(index_cfg):
+        """Optional key `storage_dtype` (float32 | float16; absent: None, today's fp32 path) -> the dtype Flat and IVFFlat
+        indexes store their vectors in.  IVFPQ stores codes, so the key is refused there."""
+        dtype = index_cfg.get("storage_dtype", None)
+        if dtype is None:
+            return None
+        if dtype not in ("float16", "float32"):
+            raise ValueError(f"datastore.index.storage_dtype must be float16 or float32, got {dtype!r}")
+        if index_cfg.index_type not in ("Flat", "IVFFlat"):
+            raise ValueError(f"datastore.index.storage_dtype applies to Flat and IVFFlat indexes; {index_cfg.index_type} "
+                             f"stores PQ codes")
+        return dtype
+
     def __init__(self, cfg, index_shard_ids=None):
         self.cfg = cfg
         self.args = cfg.datastore.index
         self.index_type = self.args.index_type
         self.refine_options(self.args)
+        storage_dtype = self.storage_dtype(self.args)
 
         passage_dir = self.cfg.datastore.embedding.passages_dir
         paths = self.artefact_paths(cfg, index_shard_ids)
@@ -65,10 +80,11 @@ class Indexer(object):
                 if os.path.exists(p):
                     os.remove(p)
         if self.index_type == "Flat":
-            self.datastore = FlatIndexer(**common)
+            self.datastore = FlatIndexer(storage_dtype=storage_dtype, **common)
         elif self.index_type == "IVFFlat":
             self.datastore = IVFFlatIndexer(trained_index_path=index_path + ".trained", sample_train_size=a.sample_train_size,
-                                            prev_index_path=None, ncentroids=a.ncentroids, probe=a.probe, **common)
+                                            prev_index_path=None, ncentroids=a.ncentroids, probe=a.probe,
+                                            storage_dtype=storage_dtype, **common)
         elif self.index_type == "IVFPQ":
             k_factor, refine_dtype = self.refine_options(a)
             self.datastore = IVFPQIndexer(trained_index_path=index_path + ".trained", sample_train_size=a.sample_train_size,

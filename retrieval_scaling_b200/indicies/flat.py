@@ -9,8 +9,9 @@ class FlatIndexer(BaseIndexer):
     index_kind = "Flat"
 
     def __init__(self, embed_paths=None, index_path=None, meta_file=None, passage_dir=None,
-                 pos_map_save_path=None, dimension=768):
-        super().__init__(embed_paths, index_path, meta_file, passage_dir, pos_map_save_path, dimension)
+                 pos_map_save_path=None, dimension=768, storage_dtype=None):
+        super().__init__(embed_paths, index_path, meta_file, passage_dir, pos_map_save_path, dimension,
+                         storage_dtype=storage_dtype)
 
     def _new_index(self):
-        return rsb_index.IndexFlatIP(self.dimension)
+        return rsb_index.IndexFlatIP(self.dimension, dtype=self.storage_dtype or "float32")

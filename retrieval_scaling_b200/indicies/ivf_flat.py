@@ -13,13 +13,13 @@ class IVFFlatIndexer(BaseIndexer):
     def __init__(self, embed_paths, index_path, meta_file, trained_index_path, passage_dir=None,
                  pos_map_save_path=None, sample_train_size=1000000, prev_index_path=None, dimension=768,
                  dtype=None, ncentroids=4096, probe=2048, num_keys_to_add_at_a_time=1000000,
-                 DSTORE_SIZE_BATCH=51200000):
+                 DSTORE_SIZE_BATCH=51200000, storage_dtype=None):
         self.ncentroids = int(ncentroids)
         self.prev_index_path = prev_index_path
         self.num_keys_to_add_at_a_time = num_keys_to_add_at_a_time
         super().__init__(embed_paths, index_path, meta_file, passage_dir, pos_map_save_path, dimension,
                          trained_index_path=prev_index_path or trained_index_path,
-                         sample_train_size=sample_train_size, probe=probe)
+                         sample_train_size=sample_train_size, probe=probe, storage_dtype=storage_dtype)
 
     def _new_index(self):
-        return rsb_index.IndexIVFFlat(self.dimension, self.ncentroids)
+        return rsb_index.IndexIVFFlat(self.dimension, self.ncentroids, dtype=self.storage_dtype or "float32")
