@@ -242,7 +242,8 @@ enum {
     RSB_PROF_PAIRS = 6,     /* number of valid (q,list) pairs            */
     RSB_PROF_LAUNCHES = 7,  /* kernels launched by the last search       */
     RSB_PROF_SCAN_PATH = 8, /* IVFPQ scan: 1 = literal-offset shared-memory look-ups, 2 = generic addressing */
-    RSB_PROF_COUNT = 9
+    RSB_PROF_RESCORED = 9,  /* IVFPQ paired scan: vectors re-scored exactly after the quantised-table filter */
+    RSB_PROF_COUNT = 10
 };
 int rsb_set_profiling(rsb_index_t* h, int enable);
 /* synchronises the events of the last search; out[RSB_PROF_COUNT] doubles */

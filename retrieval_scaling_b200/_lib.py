@@ -16,7 +16,8 @@ RSB_FLAT, RSB_IVFFLAT, RSB_IVFPQ = 0, 1, 2
 RSB_DTYPE_F32, RSB_DTYPE_F16 = 0, 1
 (INFO_KIND, INFO_D, INFO_NLIST, INFO_M, INFO_NBITS, INFO_NTOTAL, INFO_IS_TRAINED, INFO_MAX_LIST_LEN,
  INFO_INDEX_BYTES, INFO_DTYPE) = range(10)
-PROF_NAMES = ("coarse_ms", "setup_ms", "lut_ms", "scan_ms", "merge_ms", "scan_bytes", "pairs", "launches", "scan_path")
+PROF_NAMES = ("coarse_ms", "setup_ms", "lut_ms", "scan_ms", "merge_ms", "scan_bytes", "pairs", "launches", "scan_path",
+              "rescored")
 
 # every symbol include/rsb.h declares: (name, restype, argtypes)
 _H = c_void_p

@@ -92,7 +92,7 @@ struct rsb_index {
     cudaEvent_t evs[kProfSets][6] = {};
     cudaEvent_t* ev = evs[0];
     int ev_done = 0;
-    unsigned long long* prof_dev = nullptr;  // [3]: scan elements, pairs, scan path flag
+    unsigned long long* prof_dev = nullptr;  // [4]: scan elements, pairs, scan path flag, re-scored vectors
     long launches = 0;
     int elem_bytes() const { return dtype == RSB_DTYPE_F16 ? 2 : 4; }
     size_t row_bytes() const { return kind == RSB_IVFPQ ? (size_t)M : (size_t)d * elem_bytes(); }
@@ -720,11 +720,19 @@ extern "C" int rsb_export_lists(rsb_index_t* h, int64_t* offsets, void* payload,
 // ---------------------------------------------------------------------------------------------------------
 // search
 // ---------------------------------------------------------------------------------------------------------
+// IVF-PQ with the interleaved layout scans two queries of a list per item (rsb_ivf.cu).  RSB_PQ_SINGLE_ITEMS=1
+// (read once) scans every (query, list) pair on its own: the reference the tests compare the paired scan against.
+static bool pq_paired_scan(const rsb_index* h) {
+    static const bool single = getenv("RSB_PQ_SINGLE_ITEMS") != nullptr;
+    return h->kind == RSB_IVFPQ && pq_interleaved_layout(h->M) && !single;
+}
+
 struct SearchPlan {
     int qb, nprobe;          // queries per batch, effective nprobe
     int kc;                  // candidates taken from the tensor-core coarse scan before the exact re-score
     KnnPlan coarse;
-    size_t off_coarse_ws, off_cD, off_cI, off_pair, off_lut, off_keys, off_cnt, off_tau, off_qsplit, off_cD2, off_cI2, total;
+    size_t off_coarse_ws, off_cD, off_cI, off_pair, off_lut, off_qlut, off_quant, off_keys, off_cnt, off_tau, off_qsplit,
+        off_cD2, off_cI2, total;
 };
 static SearchPlan search_plan(const rsb_index* h, int nq, int k, int nprobe) {
     SearchPlan p;
@@ -743,6 +751,9 @@ static SearchPlan search_plan(const rsb_index* h, int nq, int k, int nprobe) {
     p.off_pair = o;      o += align_up(pair_work_bytes(qb, p.nprobe, h->nlist));
     const size_t lut_words = pq_interleaved_layout(h->M) ? (size_t)kLutWords : (size_t)h->M * 256;
     p.off_lut = o;       o += h->kind == RSB_IVFPQ ? align_up((size_t)qb * lut_words * 4) : 0;
+    const bool paired = pq_paired_scan(h);
+    p.off_qlut = o;      o += paired ? align_up((size_t)qb * kLutWords * 2) : 0;
+    p.off_quant = o;     o += paired ? align_up((size_t)qb * sizeof(PQQuant)) : 0;
     p.off_keys = o;      o += align_up((size_t)qb * p.nprobe * k * 8);
     p.off_cnt = o;       o += align_up((size_t)qb * p.nprobe * 4);
     p.off_tau = o;       o += align_up((size_t)qb * 4);
@@ -965,8 +976,10 @@ static int search_impl(rsb_index_t* h, const float* q, int nq, int k, int nprobe
         // non-empty there), the single-GPU rule.
         static const bool local_leads = getenv("RSB_LOCAL_LEADS") != nullptr;
         const int lead_mode = (shared && shared->local && shared->npeers > 1 && !local_leads) ? 1 : 0;
-        launch_pair_setup(cI, nb, p.nprobe, h->nlist, h->list_len, lpt_order ? h->list_rank : nullptr, pw, st, lead_mode);
-        h->launches += 3;
+        const bool paired = pq_paired_scan(h) && nb > 1;          // one query: no list is probed twice
+        launch_pair_setup(cI, nb, p.nprobe, h->nlist, h->list_len, lpt_order ? h->list_rank : nullptr, pw, st, lead_mode,
+                          paired);
+        h->launches += paired ? 5 : 3;
         if (prof) CU(cudaEventRecord(h->ev[2], st));
 
         ScanArgs a;
@@ -983,12 +996,23 @@ static int search_impl(rsb_index_t* h, const float* q, int nq, int k, int nprobe
         a.out_keys = reinterpret_cast<u64*>(w + p.off_keys);
         a.out_cnt = reinterpret_cast<int*>(w + p.off_cnt);
         a.dbg_flag = reinterpret_cast<unsigned*>(h->prof_dev + 2);
+        a.items = paired ? pw.items : nullptr;
+        a.n_pairs = pw.n_pairs;
+        a.qlut = paired ? reinterpret_cast<const unsigned short*>(w + p.off_qlut) : nullptr;
+        a.quant = paired ? reinterpret_cast<const PQQuant*>(w + p.off_quant) : nullptr;
+        a.rescored = prof ? h->prof_dev + 3 : nullptr;
+        if (prof) CU(cudaMemsetAsync(h->prof_dev + 3, 0, 8, st));
 
         if (h->kind == RSB_IVFPQ) {
             float* lut = reinterpret_cast<float*>(w + p.off_lut);
             if (pq_interleaved_layout(h->M)) launch_pq_lut(qb, nb, h->d, h->M, h->codebook_t, lut, st);
             else launch_pq_lut_generic(qb, nb, h->d, h->M, h->codebook, lut, st);
             h->launches += 1;
+            if (paired) {
+                launch_pq_lut_quant(lut, nb, h->M, reinterpret_cast<unsigned short*>(w + p.off_qlut),
+                                    reinterpret_cast<PQQuant*>(w + p.off_quant), st);
+                h->launches += 1;
+            }
             if (prof) CU(cudaEventRecord(h->ev[3], st));
             if (launch_ivfpq_scan(a, lut, h->payload, h->M, nb, st) != 0)
                 return fail(RSB_ERR_UNSUPPORTED, "no scan kernel for M = %d", h->M);
@@ -996,7 +1020,7 @@ static int search_impl(rsb_index_t* h, const float* q, int nq, int k, int nprobe
             if (prof) CU(cudaEventRecord(h->ev[3], st));
             launch_ivfflat_scan(a, qb, h->payload, h->elem_bytes(), h->d, nb, st);
         }
-        h->launches += 1;
+        h->launches += paired ? 2 : 1;                 // paired work list: both scan variants, one returns at once
         if (prof) CU(cudaEventRecord(h->ev[4], st));
         launch_merge_items(a.out_keys, a.out_cnt, nb, p.nprobe, k, k, h->ids_slots, 0, D + (size_t)q0 * k,
                            I + (size_t)q0 * k, st);
@@ -1004,7 +1028,7 @@ static int search_impl(rsb_index_t* h, const float* q, int nq, int k, int nprobe
         if (prof) {
             CU(cudaEventRecord(h->ev[5], st));
             CU(cudaMemcpyAsync(h->prof_dev, pw.scan_bytes, 8, cudaMemcpyDeviceToDevice, st));
-            CU(cudaMemcpyAsync(h->prof_dev + 1, pw.n_items, 4, cudaMemcpyDeviceToDevice, st));
+            CU(cudaMemcpyAsync(h->prof_dev + 1, pw.n_pairs, 4, cudaMemcpyDeviceToDevice, st));
             h->ev_done++;
         }
         CHECK_LAUNCH();
@@ -1232,12 +1256,13 @@ extern "C" int rsb_get_profile(rsb_index_t* h, double* out, int n) {
         }
     }
     h->ev_done = 0;
-    unsigned long long host[3] = {0, 0, 0};
-    CU(cudaMemcpy(host, h->prof_dev, 24, cudaMemcpyDeviceToHost));
+    unsigned long long host[4] = {0, 0, 0, 0};
+    CU(cudaMemcpy(host, h->prof_dev, 32, cudaMemcpyDeviceToHost));
     out[RSB_PROF_SCAN_BYTES] = (double)host[0] * (double)h->row_bytes();
     out[RSB_PROF_PAIRS] = (double)(unsigned)(host[1] & 0xffffffffull);
     out[RSB_PROF_LAUNCHES] = (double)h->launches;
     out[RSB_PROF_SCAN_PATH] = (double)(unsigned)(host[2] & 0xffffffffull);
+    out[RSB_PROF_RESCORED] = (double)host[3];
     return RSB_OK;
 }
 

@@ -110,10 +110,13 @@ bool launch_gemm_f16x2_topt(const void* Ah, const void* Al, const float* inv, in
 // ---- rsb_ivf.cu -----------------------------------------------------------------------------------------
 // (query, list) work list, sorted by list so that concurrently running blocks share inverted lists in L2.
 struct PairWork {
-    int* hist;            // [nlist + 1] scratch (zeroed by the launcher)
-    int* cursor;          // [nlist] scratch
+    int* hist;            // [2 * nlist + 1] scratch (zeroed by the launcher)
+    int* cursor;          // [2 * nlist] scratch
+    int* icursor;         // [2 * nlist] scratch (paired items)
     int* order;           // [nq * nprobe] out: pair index (q * nprobe + j), list-major
-    int* n_items;         // [1] out: number of valid pairs
+    int2* items;          // [nq * nprobe] out (paired items): (pair a, pair b or -1), list-major
+    int* n_items;         // [1] out: number of scan items (= n_pairs unless paired)
+    int* n_pairs;         // [1] out: number of valid pairs
     int* item_counter;    // [1] zeroed: dynamic scheduler of the scan kernel
     u64* scan_bytes;      // [1] out: sum over valid pairs of list_len (elements; caller scales by row bytes)
 };
@@ -121,8 +124,18 @@ size_t pair_work_bytes(int nq, int nprobe, int nlist);
 PairWork carve_pair_work(void* base, int nq, int nprobe, int nlist);
 // list_rank[l] = position of list l in the order the lists should be visited (may be null: list id order)
 // lead_mode 0: a query's lead pair = its best-ranked list that is non-empty HERE; 1: its probe-rank-0 list only
+// paired: also build `items`, where two non-lead pairs of the same list form one item (IVF-PQ paired scan)
 void launch_pair_setup(const int64_t* coarse_ids, int nq, int nprobe, int nlist, const int* list_len,
-                       const int* list_rank, PairWork w, cudaStream_t st, int lead_mode = 0);
+                       const int* list_rank, PairWork w, cudaStream_t st, int lead_mode = 0, bool paired = false);
+
+// Per-query constants of the 10-bit quantised table Q (IVF-PQ paired scan).  For every look-up-table entry T of
+// sub-quantizer m:  T = lo_m + delta * Q + e,  |e| <= resid_m.
+struct PQQuant {
+    double base;          // sum_m lo_m
+    double delta;         // quantisation step (fp32 value)
+    double err;           // sum_m max_j resid_m (evaluated in fp64)
+    double amax;          // sum_m max_j |T[m][j]|
+};
 
 struct ScanArgs {
     const int64_t* coarse_ids;    // [nq * nprobe]
@@ -145,6 +158,12 @@ struct ScanArgs {
     u64* out_keys;                // [nq * nprobe, k]
     int* out_cnt;                 // [nq * nprobe]
     unsigned* dbg_flag;           // nullable: 1 = literal-offset LDS path ran, 2 = generic path
+    // IVF-PQ paired scan (null: every item is one pair, a.order[item])
+    const int2* items;            // [n_items] (pair a, pair b or -1)
+    const int* n_pairs;           // [1] valid pairs (n_items < n_pairs iff some item is paired)
+    const unsigned short* qlut;   // [nq][256][64] 10-bit quantised tables
+    const PQQuant* quant;         // [nq]
+    u64* rescored;                // nullable: += vectors re-scored exactly after the quantised filter
 };
 
 // IVF-Flat: vecs [nslots, d] in CSR order, fp32 (elem_bytes 4) or fp16 (elem_bytes 2); queries [nq, d] fp32
@@ -154,6 +173,8 @@ void launch_ivfflat_scan(const ScanArgs& a, const float* queries, const void* ve
 // IVF-PQ
 void launch_pq_lut(const float* queries, int nq, int d, int M, const float* codebook_t, float* lut,
                    cudaStream_t st);                                 // lut [nq, 256, 64]
+// lut [nq, 256, 64] -> qlut [nq, 256, 64] u16 and quant [nq] (tables for the paired scan)
+void launch_pq_lut_quant(const float* lut, int nq, int M, unsigned short* qlut, PQQuant* quant, cudaStream_t st);
 int launch_ivfpq_scan(const ScanArgs& a, const float* lut, const uint8_t* codes, int M, int nq,
                       cudaStream_t st);                              // returns <0 if M unsupported
 // generic-M path (M not in {16, 32, 64}): table [nq][M][256], codes in natural [slot][M] order

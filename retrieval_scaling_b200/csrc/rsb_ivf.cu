@@ -12,6 +12,7 @@
 #include <float.h>
 #include <stdlib.h>
 #include <algorithm>
+#include <type_traits>
 
 namespace rsb {
 
@@ -25,8 +26,10 @@ size_t pair_work_bytes(int nq, int nprobe, int nlist) {
     size_t b = 0;
     b += ((size_t)(2 * nlist + 1) * 4 + 255) & ~(size_t)255;   // hist
     b += ((size_t)2 * nlist * 4 + 255) & ~(size_t)255;         // cursor
+    b += ((size_t)2 * nlist * 4 + 255) & ~(size_t)255;         // icursor
     b += ((size_t)nq * nprobe * 4 + 255) & ~(size_t)255;       // order
-    b += 256;                                                  // n_items, item_counter, scan_bytes
+    b += ((size_t)nq * nprobe * 8 + 255) & ~(size_t)255;       // items
+    b += 256;                                                  // n_items, item_counter, scan_bytes, n_pairs
     return b;
 }
 
@@ -35,10 +38,13 @@ PairWork carve_pair_work(void* base, int nq, int nprobe, int nlist) {
     PairWork w;
     w.hist = reinterpret_cast<int*>(p);      p += ((size_t)(2 * nlist + 1) * 4 + 255) & ~(size_t)255;
     w.cursor = reinterpret_cast<int*>(p);    p += ((size_t)2 * nlist * 4 + 255) & ~(size_t)255;
+    w.icursor = reinterpret_cast<int*>(p);   p += ((size_t)2 * nlist * 4 + 255) & ~(size_t)255;
     w.order = reinterpret_cast<int*>(p);     p += ((size_t)nq * nprobe * 4 + 255) & ~(size_t)255;
+    w.items = reinterpret_cast<int2*>(p);    p += ((size_t)nq * nprobe * 8 + 255) & ~(size_t)255;
     w.n_items = reinterpret_cast<int*>(p);
     w.item_counter = reinterpret_cast<int*>(p + 16);
     w.scan_bytes = reinterpret_cast<u64*>(p + 32);
+    w.n_pairs = reinterpret_cast<int*>(p + 48);
     return w;
 }
 
@@ -83,8 +89,10 @@ __global__ void pair_hist_kernel(const int64_t* __restrict__ coarse_ids, int npa
     if ((threadIdx.x & 31) == 0 && local) atomicAdd(scan_elems, local);
 }
 
-// single-block exclusive scan: cursor[l] = sum_{i<l} hist[i]; *total = sum
-__global__ void pair_scan_kernel(const int* __restrict__ hist, int nlist, int* cursor, int* total) {
+// single-block exclusive scan: cursor[l] = sum_{i<l} c(i); *total = sum, where c(i) = hist[i] for i < half and
+// ceil(hist[i] / 2) (the number of paired items of a bin) from `half` on
+__global__ void pair_scan_kernel(const int* __restrict__ hist, int nlist, int* cursor, int* total, int* total2,
+                                 int half) {
     __shared__ int warp_sums[32];
     __shared__ int carry_s;
     if (threadIdx.x == 0) carry_s = 0;
@@ -92,7 +100,7 @@ __global__ void pair_scan_kernel(const int* __restrict__ hist, int nlist, int* c
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
     for (int base = 0; base < nlist; base += blockDim.x) {
         const int i = base + threadIdx.x;
-        const int v = i < nlist ? hist[i] : 0;
+        const int v = i < nlist ? (i < half ? hist[i] : (hist[i] + 1) >> 1) : 0;
         int x = v;
         for (int o = 1; o < 32; o <<= 1) {
             const int y = __shfl_up_sync(0xffffffffu, x, o);
@@ -116,7 +124,10 @@ __global__ void pair_scan_kernel(const int* __restrict__ hist, int nlist, int* c
         if (threadIdx.x == 0) carry_s = carry + warp_sums[nw - 1];
         __syncthreads();
     }
-    if (threadIdx.x == 0) *total = carry_s;
+    if (threadIdx.x == 0) {
+        *total = carry_s;
+        if (total2) *total2 = carry_s;
+    }
 }
 
 __global__ void pair_scatter_kernel(const int64_t* __restrict__ coarse_ids, int npairs, int nprobe, int nlist,
@@ -129,18 +140,42 @@ __global__ void pair_scatter_kernel(const int64_t* __restrict__ coarse_ids, int 
     }
 }
 
+// Paired items: the c pairs of a non-lead bin (one list, c different queries) become ceil(c / 2) items of two pairs
+// (the last one single when c is odd); lead pairs stay single items.  Bin order -- and so the lead-first, by-list
+// order of the work list -- is kept.  After the scatter, cursor[b] is the END of bin b in `order`.
+__global__ void pair_items_kernel(const int* __restrict__ hist, const int* __restrict__ cursor,
+                                  const int* __restrict__ icursor, const int* __restrict__ order, int nlist,
+                                  int2* __restrict__ items) {
+    for (int b = blockIdx.x * blockDim.x + threadIdx.x; b < 2 * nlist; b += gridDim.x * blockDim.x) {
+        const int c = hist[b];
+        const int* src = order + (cursor[b] - c);
+        int2* dst = items + icursor[b];
+        if (b < nlist) {
+            for (int i = 0; i < c; ++i) dst[i] = make_int2(src[i], -1);
+        } else {
+            for (int i = 0; 2 * i < c; ++i) dst[i] = make_int2(src[2 * i], 2 * i + 1 < c ? src[2 * i + 1] : -1);
+        }
+    }
+}
+
 void launch_pair_setup(const int64_t* coarse_ids, int nq, int nprobe, int nlist, const int* list_len,
-                       const int* list_rank, PairWork w, cudaStream_t st, int lead_mode) {
+                       const int* list_rank, PairWork w, cudaStream_t st, int lead_mode, bool paired) {
     const int npairs = nq * nprobe;
     cudaMemsetAsync(w.hist, 0, (size_t)(2 * nlist + 1) * 4, st);
-    cudaMemsetAsync(w.n_items, 0, 256, st);  // n_items, item_counter, scan_bytes
+    cudaMemsetAsync(w.n_items, 0, 256, st);  // n_items, item_counter, scan_bytes, n_pairs
     if (npairs == 0) return;
     const int blocks = min(1024, (npairs + 255) / 256);
     pair_hist_kernel<<<blocks, 256, 0, st>>>(coarse_ids, npairs, nprobe, nlist, list_len, list_rank, w.hist,
                                              w.scan_bytes, lead_mode);
-    pair_scan_kernel<<<1, 1024, 0, st>>>(w.hist, 2 * nlist, w.cursor, w.n_items);
+    pair_scan_kernel<<<1, 1024, 0, st>>>(w.hist, 2 * nlist, w.cursor, w.n_pairs, paired ? nullptr : w.n_items,
+                                         2 * nlist);
     pair_scatter_kernel<<<blocks, 256, 0, st>>>(coarse_ids, npairs, nprobe, nlist, list_len, list_rank, w.cursor,
                                                 w.order, lead_mode);
+    if (paired) {
+        pair_scan_kernel<<<1, 1024, 0, st>>>(w.hist, 2 * nlist, w.icursor, w.n_items, nullptr, nlist);
+        pair_items_kernel<<<(2 * nlist + 255) / 256, 256, 0, st>>>(w.hist, w.cursor, w.icursor, w.order, nlist,
+                                                                   w.items);
+    }
 }
 
 // Raise the running threshold of query q to v: locally with atomicMax and, when the thresholds are shared between
@@ -474,10 +509,66 @@ void launch_pq_lut(const float* queries, int nq, int d, int M, const float* code
     launch_pq_lut_t(best, queries, nq, d, M, codebook_t, lut, st);
 }
 
+// 10-bit quantisation of a query's fp32 table for the paired scan (one block per query, in the table's
+// [code value j][64 words] layout; word w holds sub-quantizer w % M).  Q = rint((T - lo_m) / delta) with
+// delta = max_m (max_j T - lo_m) / 1023, so a sum of M <= 64 entries fits in 16 bits.  The residual
+// T - (lo_m + delta * Q) is measured in fp64 rather than assumed to be delta / 2: the fp32 quotient may round
+// across a half-way point.
+__global__ __launch_bounds__(256)
+void pq_lut_quant_kernel(const float* __restrict__ lut, int M, unsigned short* __restrict__ qlut,
+                         PQQuant* __restrict__ quant) {
+    __shared__ float s_lo[4][64], s_hi[4][64], s_abs[4][64];
+    __shared__ double s_res[4][64];
+    const int q = blockIdx.x, w = threadIdx.x & 63, jr = threadIdx.x >> 6;
+    const float* t = lut + (size_t)q * kLutWords;
+    float lo = FLT_MAX, hi = -FLT_MAX, am = 0.f;
+    for (int j = jr; j < 256; j += 4) {
+        const float x = t[j * kLutRowWords + w];
+        lo = fminf(lo, x); hi = fmaxf(hi, x); am = fmaxf(am, fabsf(x));
+    }
+    s_lo[jr][w] = lo; s_hi[jr][w] = hi; s_abs[jr][w] = am;
+    __syncthreads();
+#pragma unroll
+    for (int i = 0; i < 4; ++i) { lo = fminf(lo, s_lo[i][w]); hi = fmaxf(hi, s_hi[i][w]); am = fmaxf(am, s_abs[i][w]); }
+    float range = 0.f;
+    for (int m = 0; m < M; ++m) {
+        float l = s_lo[0][m], h = s_hi[0][m];
+#pragma unroll
+        for (int i = 1; i < 4; ++i) { l = fminf(l, s_lo[i][m]); h = fmaxf(h, s_hi[i][m]); }
+        range = fmaxf(range, h - l);
+    }
+    const float delta = range > 0.f ? range / 1023.f : 1.f;
+    double res = 0.0;
+    for (int j = jr; j < 256; j += 4) {
+        const float x = t[j * kLutRowWords + w];
+        const float qv = fminf(fmaxf(rintf((x - lo) / delta), 0.f), 1023.f);
+        qlut[(size_t)q * kLutWords + j * kLutRowWords + w] = (unsigned short)qv;
+        res = fmax(res, fabs((double)x - ((double)lo + (double)delta * (double)qv)));
+    }
+    __syncthreads();                                   // every thread has read s_lo / s_hi / s_abs
+    if (jr == 0) { s_lo[0][w] = lo; s_abs[0][w] = am; }
+    s_res[jr][w] = res;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        PQQuant r{0.0, (double)delta, 0.0, 0.0};
+        for (int m = 0; m < M; ++m) {
+            r.base += (double)s_lo[0][m];
+            r.err += fmax(fmax(s_res[0][m], s_res[1][m]), fmax(s_res[2][m], s_res[3][m]));
+            r.amax += (double)s_abs[0][m];
+        }
+        quant[q] = r;
+    }
+}
+
+void launch_pq_lut_quant(const float* lut, int nq, int M, unsigned short* qlut, PQQuant* quant, cudaStream_t st) {
+    if (nq <= 0) return;
+    pq_lut_quant_kernel<<<nq, 256, 0, st>>>(lut, M, qlut, quant);
+}
+
 // =============================================================================================================
 // IVF-PQ ADC list scan -- the hot kernel.  score(code) = dis0 + sum_m T[m][code[m]].
 //
-// One block (256 threads, 8 warps) per (query, list) item; persistent blocks pull items (sorted by list, so
+// One block (256 threads, 8 warps) per item; persistent blocks pull items (sorted by list, so
 // concurrent blocks share a list in L2) from an atomic counter.  The query's 64 KB fp32 table sits in shared
 // memory laid out [code value j][64 words]; K = M/16 lanes cooperate on one vector and every look-up address is
 // produced by ONE PRMT:  addr = (code_byte << 8) | lane_word_offset  (rsb_layout.h proves the 32 lanes of a warp
@@ -487,6 +578,17 @@ void launch_pq_lut(const float* queries, int nq, int d, int M, const float* code
 // block's candidate buffer (warp-aggregated shared atomics), which is compacted by a bitonic sort only when it
 // fills.  The per-query threshold is shared between blocks through global memory (atomicMax) so later lists of
 // a query are filtered by what earlier lists already found.
+//
+// PAIRED items (two queries probing the same list, see pair_items_kernel) score both queries with one look-up: the
+// block packs the two queries' 10-bit quantised tables (pq_lut_quant_kernel) into one 64 KB table of u32 words,
+// query a in the low 16 bits and query b in the high 16, and accumulates with integer adds -- a sum of M <= 64
+// entries is at most 64 * 1023 < 2^16, so the lanes never carry into each other.  For the integer sum S of a vector:
+//     s <= dis0 + base + delta * S + err + gamma * (|dis0| + amax)
+// where s is the fp32 score the single-item path computes, err bounds the table's quantisation residuals and the
+// gamma term bounds the fp32 rounding of the ~66-term sum (gamma = 70 * 2^-24).  A vector is re-scored exactly
+// (pq_vector_score, from the fp32 table in global memory, in pq_block_score's summation order) iff S >= S_min, the
+// smallest S that could reach the running threshold, and is appended iff its exact score passes today's test: the
+// candidate sets, and so the results, are those of the single-item path.
 // =============================================================================================================
 constexpr int PQ_THREADS = 256;
 constexpr int PQ_WARPS = PQ_THREADS / 32;
@@ -496,6 +598,10 @@ constexpr int PQ_WARPS = PQ_THREADS / 32;
 constexpr int PQ_CHECK = RSB_PQ_CHECK;                       // code blocks per warp between capacity checks (2 or 3)
 static_assert(PQ_CHECK == 2 || PQ_CHECK == 3, "the scan loop is written for 2 or 3 blocks per check");
 constexpr int PQ_SLACK = PQ_CHECK * PQ_WARPS * 32;           // 512 / 768 candidates between checks
+// Paired items check capacity after every code block per warp: the two candidate buffers then need
+// cand_capacity(k, 256) entries each, which for k <= 256 fit in the single-item buffer's cand_capacity(k, 512) entries,
+// so paired and single items share one block shape (3 blocks of 256 threads per SM) and shared-memory footprint.
+constexpr int PQ_PAIR_SLACK = PQ_WARPS * 32;                 // 256 candidates per buffer between checks
 // Shared-window address at which this kernel's dynamic shared memory is expected to start (the kernel declares
 // no static shared memory; sm_90+ reserve the first 1 KB of the window).  When the runtime address matches, the
 // table base is folded into the LDS immediate ("FAST" path: PRMT -> LDS [R + 0x400] -> FADD); otherwise the
@@ -504,64 +610,101 @@ constexpr unsigned PQ_LUT_SADDR = 1024;
 
 __device__ __forceinline__ unsigned smem_addr_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
 
-template <bool FAST>
-__device__ __forceinline__ float lut_at(const unsigned char* lutb, unsigned codes, unsigned off, unsigned sel) {
+// T = float: the fp32 table; T = unsigned: the packed 2 x 16-bit table of a paired item (same word layout)
+template <bool FAST, typename T>
+__device__ __forceinline__ T lut_at(const unsigned char* lutb, unsigned codes, unsigned off, unsigned sel) {
     // result byte0 = off (lane word offset, < 256), byte1 = selected code byte, bytes 2,3 = 0
     const unsigned a = __byte_perm(codes, off, sel);
     if (FAST) {
-        float v;
-        asm volatile("ld.shared.f32 %0, [%1+%2];" : "=f"(v) : "r"(a), "n"(PQ_LUT_SADDR));
+        T v;
+        if constexpr (std::is_same<T, float>::value)
+            asm volatile("ld.shared.f32 %0, [%1+%2];" : "=f"(v) : "r"(a), "n"(PQ_LUT_SADDR));
+        else
+            asm volatile("ld.shared.u32 %0, [%1+%2];" : "=r"(v) : "r"(a), "n"(PQ_LUT_SADDR));
         return v;
     }
-    return *reinterpret_cast<const float*>(lutb + a);
+    return *reinterpret_cast<const T*>(lutb + a);
 }
 
-template <bool FAST>
-__device__ __forceinline__ float pq_pass(const unsigned char* lutb, const uint4 c, const unsigned (&off)[16]) {
-    float s0, s1;
-    s0 = lut_at<FAST>(lutb, c.x, off[0], 0x5504);
-    s1 = lut_at<FAST>(lutb, c.x, off[1], 0x5514);
-    s0 += lut_at<FAST>(lutb, c.x, off[2], 0x5524);
-    s1 += lut_at<FAST>(lutb, c.x, off[3], 0x5534);
-    s0 += lut_at<FAST>(lutb, c.y, off[4], 0x5504);
-    s1 += lut_at<FAST>(lutb, c.y, off[5], 0x5514);
-    s0 += lut_at<FAST>(lutb, c.y, off[6], 0x5524);
-    s1 += lut_at<FAST>(lutb, c.y, off[7], 0x5534);
-    s0 += lut_at<FAST>(lutb, c.z, off[8], 0x5504);
-    s1 += lut_at<FAST>(lutb, c.z, off[9], 0x5514);
-    s0 += lut_at<FAST>(lutb, c.z, off[10], 0x5524);
-    s1 += lut_at<FAST>(lutb, c.z, off[11], 0x5534);
-    s0 += lut_at<FAST>(lutb, c.w, off[12], 0x5504);
-    s1 += lut_at<FAST>(lutb, c.w, off[13], 0x5514);
-    s0 += lut_at<FAST>(lutb, c.w, off[14], 0x5524);
-    s1 += lut_at<FAST>(lutb, c.w, off[15], 0x5534);
+// 16 look-ups of one pass; `at(codes, off, sel)` returns the table entry (shared-memory table, or the fp32 table in
+// global memory for the exact re-score of a paired item)
+template <typename T, typename At>
+__device__ __forceinline__ T pq_pass(At at, const uint4 c, const unsigned (&off)[16]) {
+    T s0, s1;
+    s0 = at(c.x, off[0], 0x5504);
+    s1 = at(c.x, off[1], 0x5514);
+    s0 += at(c.x, off[2], 0x5524);
+    s1 += at(c.x, off[3], 0x5534);
+    s0 += at(c.y, off[4], 0x5504);
+    s1 += at(c.y, off[5], 0x5514);
+    s0 += at(c.y, off[6], 0x5524);
+    s1 += at(c.y, off[7], 0x5534);
+    s0 += at(c.z, off[8], 0x5504);
+    s1 += at(c.z, off[9], 0x5514);
+    s0 += at(c.z, off[10], 0x5524);
+    s1 += at(c.z, off[11], 0x5534);
+    s0 += at(c.w, off[12], 0x5504);
+    s1 += at(c.w, off[13], 0x5514);
+    s0 += at(c.w, off[14], 0x5524);
+    s1 += at(c.w, off[15], 0x5534);
     return s0 + s1;
 }
 
-// score of block-local vector `lane` from the K code chunks of one 32-vector block
-template <int K, bool FAST>
-__device__ __forceinline__ float pq_block_score(const unsigned char* lutb, const uint4 (&c)[K],
-                                                const unsigned (&off)[16], int r) {
-    float p[K];
+// score of block-local vector `lane` from the K code chunks of one 32-vector block (T = unsigned: the two packed
+// 16-bit sums of a paired item)
+template <int K, bool FAST, typename T = float>
+__device__ __forceinline__ T pq_block_score(const unsigned char* lutb, const uint4 (&c)[K],
+                                            const unsigned (&off)[16], int r) {
+    const auto at = [lutb](unsigned w, unsigned o, unsigned sel) { return lut_at<FAST, T>(lutb, w, o, sel); };
+    T p[K];
 #pragma unroll
-    for (int t = 0; t < K; ++t) p[t] = pq_pass<FAST>(lutb, c[t], off);
+    for (int t = 0; t < K; ++t) p[t] = pq_pass<T>(at, c[t], off);
     if (K == 4) {
         // lane rank r holds partials of the group's vectors t = 0..3; route vector t to lane rank t
-        float k0 = (r & 2) ? p[2] : p[0];
-        float k1 = (r & 2) ? p[K - 1] : p[1];
-        const float s0 = (r & 2) ? p[0] : p[2];
-        const float s1 = (r & 2) ? p[1] : p[K - 1];
+        T k0 = (r & 2) ? p[2] : p[0];
+        T k1 = (r & 2) ? p[K - 1] : p[1];
+        const T s0 = (r & 2) ? p[0] : p[2];
+        const T s1 = (r & 2) ? p[1] : p[K - 1];
         k0 += __shfl_xor_sync(0xffffffffu, s0, 2);
         k1 += __shfl_xor_sync(0xffffffffu, s1, 2);
-        const float keep = (r & 1) ? k1 : k0;
-        const float send = (r & 1) ? k0 : k1;
+        const T keep = (r & 1) ? k1 : k0;
+        const T send = (r & 1) ? k0 : k1;
         return keep + __shfl_xor_sync(0xffffffffu, send, 1);
     } else if (K == 2) {
-        const float keep = r ? p[K - 1] : p[0];
-        const float send = r ? p[0] : p[K - 1];
+        const T keep = r ? p[K - 1] : p[0];
+        const T send = r ? p[0] : p[K - 1];
         return keep + __shfl_xor_sync(0xffffffffu, send, 1);
     }
     return p[0];
+}
+
+// Exact fp32 score (without dis0) of this lane's block-local vector, for the lanes with `need` set (the others get
+// 0); all 32 lanes must call it.  Equal bit for bit to pq_block_score<K, FAST, float>: vector t of group g is
+// lane (g, t)'s vector, and lane (g, r) holds its pass-t chunk in c[t].  Every lane of the group runs pass t
+// (pq_pass, same entries, same order) on the fp32 table, giving partials p_0 .. p_{K-1} (index = lane rank).  The
+// shuffle tree of pq_block_score leaves lane t with, for K = 4, (p_t + p_{t^2}) + (p_{t^1} + p_{t^3}): step one adds
+// the partner at distance 2 to the kept partial, step two the partner at distance 1.  The two xor-shuffle
+// additions below compute exactly that in lane t (fp32 addition is commutative); K = 2 gives p_t + p_{t^1}, K = 1 p_0.
+template <int K>
+__device__ __forceinline__ float pq_vector_score(const float* __restrict__ lutq, const uint4 (&c)[K],
+                                                 const unsigned (&off)[16], int r, bool need) {
+    const unsigned char* tb = reinterpret_cast<const unsigned char*>(lutq);
+    const auto at = [tb](unsigned w, unsigned o, unsigned sel) {
+        return __ldg(reinterpret_cast<const float*>(tb + __byte_perm(w, o, sel)));
+    };
+    const int lane = threadIdx.x & 31;
+    float score = 0.f;
+#pragma unroll
+    for (int t = 0; t < K; ++t) {
+        const unsigned owners = __ballot_sync(0xffffffffu, need && r == t);
+        if (owners == 0u) continue;                                    // warp-uniform
+        float p = 0.f;
+        if ((owners >> (lane - r + t)) & 1u) p = pq_pass<float>(at, c[t], off);
+        if (K == 4) p += __shfl_xor_sync(0xffffffffu, p, 2);
+        if (K >= 2) p += __shfl_xor_sync(0xffffffffu, p, 1);
+        if (r == t) score = p;
+    }
+    return score;
 }
 
 // Predicated 128-bit loads: past the end of the list the registers simply keep their old contents (the scores of
@@ -643,17 +786,147 @@ __device__ __forceinline__ unsigned pq_scan_list(const unsigned char* lutb, cons
     return tau;
 }
 
+// S_min: the smallest integer sum that can still give an fp32 score above the threshold tau, for
+// c0 = dis0 + base + err + gamma * (|dis0| + amax) and inv_delta = 1 / delta (rounded down, less one for the fp64
+// evaluation, whose relative error is ~1e-16 on a value < 2^17); 0 = re-score all.
+__device__ __forceinline__ int pq_smin(unsigned tau, double c0, double inv_delta) {
+    if (tau == 0u) return 0;
+    const float t = unord_f32(tau);
+    if (!isfinite(t)) return 0;
+    const double x = floor(((double)t - c0) * inv_delta) - 1.0;
+    return x > 0.0 ? (x < 65536.0 ? (int)x : 65536) : 0;
+}
+
+// Shared-memory state of a paired item; h = 0 / 1 for query a / b.
+struct PQPairState {
+    double thr[2][2];     // {c0, inv_delta} of pq_smin
+    int q[2];
+    float dis0[2];
+    int count[2];         // candidate counts
+};
+
+// Exact re-score of the flagged vectors of one block for query h of a paired item, appended under the usual rule
+// (exact ordered score > the query's threshold).  The threshold is the query's global one, which every block's
+// compactions raise: a valid bound like the register copy the single-item path keeps.  Not inlined: it runs for a
+// small fraction of the blocks, and its 16 outstanding table loads per pass would otherwise compete for registers
+// with the scan loop (spills); the call keeps them out of the loop's allocation.
 template <int K>
+__device__ __noinline__ void pq_rescore_append(const unsigned* tau_g, const float* lut_g, PQPairState* st, int h,
+                                               u64* keys, uint4 c0, uint4 c1, uint4 c2, uint4 c3, bool need,
+                                               unsigned slot) {
+    const int lane = threadIdx.x & 31, g = lane / K, r = lane % K;
+    unsigned off[16];
+#pragma unroll
+    for (int s = 0; s < 16; ++s) off[s] = 4u * (unsigned)pq_pos(16 * K, K, g, r, s);
+    uint4 c[K];
+    c[0] = c0;
+    if (K > 1) c[1] = c1;
+    if (K > 2) { c[2] = c2; c[K - 1] = c3; }
+    const int q = st->q[h];
+    const unsigned tau = *reinterpret_cast<const volatile unsigned*>(tau_g + q);
+    const float score = st->dis0[h] + pq_vector_score<K>(lut_g + (size_t)q * kLutWords, c, off, r, need);
+    const unsigned o = ord_f32(score);
+    warp_append(keys, &st->count[h], need && o > tau, make_key(o, slot));
+}
+
+// scan one inverted list for the two queries of a paired item (packed 2 x 16-bit table in shared memory)
+template <int K, bool FAST>
+__device__ __forceinline__ void pq_scan_pair(const unsigned char* lutb, const uint4* cbase, int nblk, int len,
+                                             unsigned slot0, const unsigned (&off)[16], int r, u64* keys_a,
+                                             u64* keys_b, PQPairState* st, const float* __restrict__ lut_g, int k,
+                                             int cap2, const ScanArgs& a, int lane, int warp) {
+    const int n_iter = (nblk + PQ_WARPS - 1) / PQ_WARPS;
+    const int lim = cap2 - PQ_PAIR_SLACK;
+    unsigned tau_a = *reinterpret_cast<const volatile unsigned*>(a.tau + st->q[0]);
+    unsigned tau_b = *reinterpret_cast<const volatile unsigned*>(a.tau + st->q[1]);
+    int smin_a = pq_smin(tau_a, st->thr[0][0], st->thr[0][1]), smin_b = pq_smin(tau_b, st->thr[1][0], st->thr[1][1]);
+    uint4 A[K], B[K];
+#pragma unroll
+    for (int t = 0; t < K; ++t) A[t] = B[t] = make_uint4(0, 0, 0, 0);
+    pq_load_block<K>(A, cbase, warp, nblk, lane);
+    pq_load_block<K>(B, cbase, warp + PQ_WARPS, nblk, lane);
+    // integer sums of both queries in one look-up; the few vectors whose sum reaches S_min are re-scored exactly
+#define RSB_PQ_STEP2(X, b)                                                                                 \
+    {                                                                                                      \
+        const int b_ = (b);                                                                                \
+        if (b_ < nblk) {                                                                                   \
+            const unsigned sum = pq_block_score<K, FAST, unsigned>(lutb, X, off, r);                       \
+            const int vi = b_ * 32 + lane;                                                                 \
+            const bool na = vi < len && (int)(sum & 0xffffu) >= smin_a;                                    \
+            const bool nb = vi < len && (int)(sum >> 16) >= smin_b;                                        \
+            if (__any_sync(0xffffffffu, na || nb)) {                                                       \
+                pq_rescore_append<K>(a.tau, lut_g, st, 0, keys_a, X[0], X[K > 1 ? 1 : 0], X[K > 2 ? 2 : 0],   \
+                                     X[K - 1], na, slot0 + (unsigned)vi);                                  \
+                pq_rescore_append<K>(a.tau, lut_g, st, 1, keys_b, X[0], X[K > 1 ? 1 : 0], X[K > 2 ? 2 : 0],   \
+                                     X[K - 1], nb, slot0 + (unsigned)vi);                                  \
+                if (a.rescored) {                                                                          \
+                    const int n = __popc(__ballot_sync(0xffffffffu, na)) +                                 \
+                                  __popc(__ballot_sync(0xffffffffu, nb));                                  \
+                    if (lane == 0) atomicAdd(a.rescored, (u64)n);                                          \
+                }                                                                                          \
+            }                                                                                              \
+        }                                                                                                  \
+        pq_load_block<K>(X, cbase, b_ + 2 * PQ_WARPS, nblk, lane);                                         \
+    }
+    // One barrier checks both buffers.  A compaction that found k candidates raises the query's global threshold;
+    // S_min is recomputed whenever a threshold moved, by this block's compaction or by the global value.
+#define RSB_PQ_CHECKPOINT2()                                                                               \
+    {                                                                                                      \
+        const unsigned ta0 = tau_a, tb0 = tau_b;                                                           \
+        if (__syncthreads_or(*reinterpret_cast<volatile int*>(&st->count[0]) > lim ||                      \
+                             *reinterpret_cast<volatile int*>(&st->count[1]) > lim)) {                     \
+            if (st->count[0] > lim) {                                                                      \
+                const unsigned t_ = block_compact(keys_a, &st->count[0], k, cap2, tau_a);                    \
+                if (t_ > tau_a && threadIdx.x == 0) raise_tau(a, st->q[0], t_);                            \
+                tau_a = t_;                                                                                \
+            }                                                                                              \
+            if (st->count[1] > lim) {                                                                      \
+                const unsigned t_ = block_compact(keys_b, &st->count[1], k, cap2, tau_b);                    \
+                if (t_ > tau_b && threadIdx.x == 0) raise_tau(a, st->q[1], t_);                            \
+                tau_b = t_;                                                                                \
+            }                                                                                              \
+        }                                                                                                  \
+        const unsigned ga = *reinterpret_cast<const volatile unsigned*>(a.tau + st->q[0]);                 \
+        const unsigned gb = *reinterpret_cast<const volatile unsigned*>(a.tau + st->q[1]);                 \
+        tau_a = ga > tau_a ? ga : tau_a;                                                                   \
+        tau_b = gb > tau_b ? gb : tau_b;                                                                   \
+        if (tau_a != ta0) smin_a = pq_smin(tau_a, st->thr[0][0], st->thr[0][1]);                           \
+        if (tau_b != tb0) smin_b = pq_smin(tau_b, st->thr[1][0], st->thr[1][1]);                           \
+    }
+    for (int it = 0; it < n_iter; it += 2) {
+        const int b0 = it * PQ_WARPS + warp;
+        RSB_PQ_STEP2(A, b0);
+        RSB_PQ_CHECKPOINT2();
+        RSB_PQ_STEP2(B, b0 + PQ_WARPS);
+        RSB_PQ_CHECKPOINT2();
+    }
+#undef RSB_PQ_STEP2
+#undef RSB_PQ_CHECKPOINT2
+}
+
+// PAIRED = false compiles the single-item path alone, so it keeps its own register allocation (the paired branch needs
+// more registers than the single-item loop and would make the single-item loop spill).  It runs every search without
+// a paired work list (one query, RSB_PQ_SINGLE_ITEMS) and every paired work list in which no two pairs share a list
+// (n_items == n_pairs, e.g. the full sweep): both variants are launched and each returns at once unless it is the one
+// the work list needs.
+template <int K, bool PAIRED>
 __global__ __launch_bounds__(PQ_THREADS, 3)
-void ivfpq_scan_kernel(ScanArgs a, const float* __restrict__ lut_g, const uint8_t* __restrict__ codes, int cap) {
+void ivfpq_scan_kernel(ScanArgs a, const float* __restrict__ lut_g, const uint8_t* __restrict__ codes, int cap,
+                       int cap2) {
     constexpr int M = 16 * K;
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    const unsigned char* lutb = smem_raw;                              // 64 KB table
-    u64* keys = reinterpret_cast<u64*>(smem_raw + kLutWords * 4);      // candidate buffer
-    int* s_ctrl = reinterpret_cast<int*>(smem_raw + kLutWords * 4 + (size_t)cap * 8);
-    int* s_count = s_ctrl;
-    int* s_item = s_ctrl + 4;                                          // two slots (current / next item)
+    unsigned char* lutb = smem_raw;                                    // 64 KB table (fp32, or packed 2 x u16)
+    // candidate buffers: one of `cap` entries (single items) or two of `cap2` (paired items), in one region
+    u64* keys_a = reinterpret_cast<u64*>(smem_raw + kLutWords * 4);
+    u64* keys_b = keys_a + cap2;
+    PQPairState* st = reinterpret_cast<PQPairState*>(keys_a + max(cap, 2 * cap2));
+    int* s_count = st->count;                                          // [0]: single items and query a
+    int* s_ctrl = reinterpret_cast<int*>(st + 1);
+    uint64_t* lut_bar = reinterpret_cast<uint64_t*>(s_ctrl);          // 8-byte aligned
+    int* s_item = s_ctrl + 2;                                          // two slots (current / next item)
+    int* s_work = s_ctrl + 4;                                          // the item's pairs, see below
 
+    if (a.items && PAIRED != (*a.n_items != *a.n_pairs)) return;      // the other variant scans this work list
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int g = lane / K, r = lane % K;
     unsigned off[16];
@@ -663,13 +936,29 @@ void ivfpq_scan_kernel(ScanArgs a, const float* __restrict__ lut_g, const uint8_
     const bool fast = smem_addr_u32(smem_raw) == PQ_LUT_SADDR;         // block-uniform
     if (a.dbg_flag && blockIdx.x == 0 && tid == 0) *a.dbg_flag = fast ? 1u : 2u;
 
-    uint64_t* lut_bar = reinterpret_cast<uint64_t*>(s_ctrl + 2);      // 8-byte aligned (cap * 8 + 64 KB + 8)
     unsigned lut_phase = 0u;
     if (tid == 0) {
         rsbtc::mbar_init(lut_bar, 1);
         rsbtc::fence_barrier_init();
         s_item[0] = atomicAdd(a.item_counter, 1);
     }
+
+    // Emit a pair's candidates.  They only need sorting (and trimming to k) when more than k survived; the
+    // per-query merge kernel treats every item as an unordered set.
+    const auto emit = [&](int pair, int q, u64* keys, int* count, int capacity, unsigned tau) {
+        int n = *count;
+        bool sorted = false;
+        if (n > a.k) {                                                 // block-uniform
+            block_compact(keys, count, a.k, capacity, tau);
+            n = a.k;
+            sorted = true;
+        }
+        for (int i = tid; i < n; i += PQ_THREADS) a.out_keys[(size_t)pair * a.k + i] = keys[i];
+        if (tid == 0) {
+            a.out_cnt[pair] = n;
+            if (sorted) raise_tau(a, q, key_ord(keys[a.k - 1]));
+        }
+    };
 
     const int n_items = *a.n_items;
     int cur_q = -1, par = 0;
@@ -680,59 +969,104 @@ void ivfpq_scan_kernel(ScanArgs a, const float* __restrict__ lut_g, const uint8_
         // thread 0 reserves the block's NEXT item now and publishes it at the end of this one, so the atomic's
         // round trip is hidden behind the scan
         int next_item = 0;
-        if (tid == 0) { *s_count = 0; next_item = atomicAdd(a.item_counter, 1); }
-        const int pair = a.order[item];
-        const int q = pair / a.nprobe;
-        const int list = (int)a.coarse_ids[pair];
-        const float dis0 = a.coarse_scores[pair];
-        if (q != cur_q) {                                          // block-uniform
-            // 64 KB table: one bulk copy by the TMA engine (global -> shared, no register staging, no trip through
-            // the LSU data pipe that the look-ups saturate), completion signalled on an mbarrier.  All generic-proxy
-            // reads of the previous table finished before barrier (B) above; the proxy fence orders them before
-            // the async-proxy writes.
-            if (tid == 0) {
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                rsbtc::mbar_expect_tx(lut_bar, kLutWords * 4);
-                asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                             ::"r"(smem_addr_u32(smem_raw)),
-                               "l"(reinterpret_cast<unsigned long long>(lut_g + (size_t)q * kLutWords)), "r"(kLutWords * 4),
-                               "r"(smem_addr_u32(lut_bar))
-                             : "memory");
+        if (tid == 0) {
+            next_item = atomicAdd(a.item_counter, 1);
+            const int2 it = PAIRED ? a.items[item] : make_int2(a.order[item], -1);
+            // A paired item whose queries do not both have a bound yet (thresholds that come from another GPU) is
+            // scanned as two single items: without a bound every vector would need the exact re-score.
+            bool pair = it.y >= 0;
+            if (pair) {
+                const unsigned ta = *reinterpret_cast<volatile unsigned*>(a.tau + it.x / a.nprobe);
+                const unsigned tb = *reinterpret_cast<volatile unsigned*>(a.tau + it.y / a.nprobe);
+                pair = ta != 0u && tb != 0u;
             }
-            rsbtc::mbar_wait(lut_bar, lut_phase);
-            lut_phase ^= 1u;
-            cur_q = q;
+            s_work[0] = it.x;                                      // single item, or query a of a paired item
+            s_work[1] = pair ? it.y : -1;                          // query b of a paired item
+            s_work[2] = pair ? -1 : it.y;                          // second single item of a split pair
         }
-        unsigned tau = *reinterpret_cast<volatile unsigned*>(a.tau + q);
         __syncthreads();
-
+        const int w0 = s_work[0], w1 = s_work[1], w2 = s_work[2];
+        const int list = (int)a.coarse_ids[w0];
         const int len = a.list_len[list];
         const int64_t slot0 = a.list_off[list];                       // multiple of 32
         const int nblk = (len + 31) >> 5;
         const uint4* cbase = reinterpret_cast<const uint4*>(codes + (size_t)slot0 * M);  // K*32 uint4 per block
-        if (fast)
-            tau = pq_scan_list<K, true>(lutb, cbase, nblk, len, (unsigned)slot0, dis0, off, r, keys, s_count, tau, a.k,
-                                        cap, a, q, lane, warp);
-        else
-            tau = pq_scan_list<K, false>(lutb, cbase, nblk, len, (unsigned)slot0, dis0, off, r, keys, s_count, tau, a.k,
-                                         cap, a, q, lane, warp);
 
-        // Emit the block's candidates.  They only need sorting (and trimming to k) when more than k survived;
-        // the per-query merge kernel treats every item as an unordered set.
-        __syncthreads();
-        int n = *s_count;
-        bool sorted = false;
-        if (n > a.k) {                                                // block-uniform
-            block_compact(keys, s_count, a.k, cap, tau);
-            n = a.k;
-            sorted = true;
+        if (PAIRED && w1 >= 0) {
+            // ---- paired item: pack the two quantised tables (query a low half, query b high half)
+            const int qa = w0 / a.nprobe, qb = w1 / a.nprobe;
+            const uint4* ta = reinterpret_cast<const uint4*>(a.qlut + (size_t)qa * kLutWords);
+            const uint4* tb = reinterpret_cast<const uint4*>(a.qlut + (size_t)qb * kLutWords);
+            uint4* dst = reinterpret_cast<uint4*>(lutb);
+            for (int i = tid; i < kLutWords / 8; i += PQ_THREADS) {
+                const uint4 x = __ldg(ta + i), y = __ldg(tb + i);
+                dst[2 * i] = make_uint4(__byte_perm(x.x, y.x, 0x5410), __byte_perm(x.x, y.x, 0x7632),
+                                        __byte_perm(x.y, y.y, 0x5410), __byte_perm(x.y, y.y, 0x7632));
+                dst[2 * i + 1] = make_uint4(__byte_perm(x.z, y.z, 0x5410), __byte_perm(x.z, y.z, 0x7632),
+                                            __byte_perm(x.w, y.w, 0x5410), __byte_perm(x.w, y.w, 0x7632));
+            }
+            cur_q = -1;
+            if (tid < 2) {
+                constexpr double gamma = 70.0 / 16777216.0;
+                const int pair = tid ? w1 : w0, q = tid ? qb : qa;
+                const float dis0 = a.coarse_scores[pair];
+                const PQQuant qq = a.quant[q];
+                st->thr[tid][0] = (double)dis0 + qq.base + qq.err + gamma * (fabs((double)dis0) + qq.amax);
+                st->thr[tid][1] = 1.0 / qq.delta;
+                st->q[tid] = q;
+                st->dis0[tid] = dis0;
+                st->count[tid] = 0;
+            }
+            __syncthreads();
+            if (fast)
+                pq_scan_pair<K, true>(lutb, cbase, nblk, len, (unsigned)slot0, off, r, keys_a, keys_b, st, lut_g, a.k,
+                                      cap2, a, lane, warp);
+            else
+                pq_scan_pair<K, false>(lutb, cbase, nblk, len, (unsigned)slot0, off, r, keys_a, keys_b, st, lut_g, a.k,
+                                       cap2, a, lane, warp);
+            __syncthreads();
+            emit(w0, qa, keys_a, &st->count[0], cap2, 0u);
+            emit(w1, qb, keys_b, &st->count[1], cap2, 0u);
+        } else {
+            // ---- single item(s): the query's fp32 table
+            for (int h = 0; h < 2; ++h) {
+                const int pair = h ? w2 : w0;
+                if (pair < 0) break;                                   // block-uniform
+                if (h) __syncthreads();                                // the first item's emit is done
+                const int q = pair / a.nprobe;
+                const float dis0 = a.coarse_scores[pair];
+                if (tid == 0) s_count[0] = 0;
+                if (q != cur_q) {                                      // block-uniform
+                    // 64 KB table: one bulk copy by the TMA engine (global -> shared, no register staging, no trip
+                    // through the LSU data pipe that the look-ups saturate), completion signalled on an mbarrier.
+                    // All generic-proxy accesses of the previous table finished before the last barrier; the proxy
+                    // fence orders them before the async-proxy writes.
+                    if (tid == 0) {
+                        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                        rsbtc::mbar_expect_tx(lut_bar, kLutWords * 4);
+                        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                                     ::"r"(smem_addr_u32(smem_raw)),
+                                       "l"(reinterpret_cast<unsigned long long>(lut_g + (size_t)q * kLutWords)),
+                                       "r"(kLutWords * 4), "r"(smem_addr_u32(lut_bar))
+                                     : "memory");
+                    }
+                    rsbtc::mbar_wait(lut_bar, lut_phase);
+                    lut_phase ^= 1u;
+                    cur_q = q;
+                }
+                unsigned tau = *reinterpret_cast<volatile unsigned*>(a.tau + q);
+                __syncthreads();
+                if (fast)
+                    tau = pq_scan_list<K, true>(lutb, cbase, nblk, len, (unsigned)slot0, dis0, off, r, keys_a, s_count,
+                                                tau, a.k, cap, a, q, lane, warp);
+                else
+                    tau = pq_scan_list<K, false>(lutb, cbase, nblk, len, (unsigned)slot0, dis0, off, r, keys_a,
+                                                 s_count, tau, a.k, cap, a, q, lane, warp);
+                __syncthreads();
+                emit(pair, q, keys_a, s_count, cap, tau);
+            }
         }
-        for (int i = tid; i < n; i += PQ_THREADS) a.out_keys[(size_t)pair * a.k + i] = keys[i];
-        if (tid == 0) {
-            a.out_cnt[pair] = n;
-            if (sorted) raise_tau(a, q, key_ord(keys[a.k - 1]));
-            s_item[par ^ 1] = next_item;
-        }
+        if (tid == 0) s_item[par ^ 1] = next_item;
         par ^= 1;
     }
 }
@@ -870,13 +1204,18 @@ template <int K>
 static void launch_ivfpq_scan_t(const ScanArgs& a, const float* lut, const uint8_t* codes, int npairs,
                                 cudaStream_t st) {
     const int cap = cand_capacity(a.k, PQ_SLACK);
-    const size_t smem = (size_t)kLutWords * 4 + (size_t)cap * 8 + 32;   // + count, LUT mbarrier, two item slots
-    cudaFuncSetAttribute(ivfpq_scan_kernel<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    int occ = 1;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, ivfpq_scan_kernel<K>, PQ_THREADS, smem);
-    if (occ < 1) occ = 1;
-    const int grid = min(npairs, num_sms() * occ);
-    ivfpq_scan_kernel<K><<<grid, PQ_THREADS, smem, st>>>(a, lut, codes, cap);
+    const auto launch = [&](auto kernel, int cap2) {
+        // table + candidate buffer region + PQPairState, LUT mbarrier, item slots, the item's pairs
+        const size_t smem = (size_t)kLutWords * 4 + (size_t)std::max(cap, 2 * cap2) * 8 + sizeof(PQPairState) + 32;
+        cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        int occ = 1;
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, PQ_THREADS, smem);
+        if (occ < 1) occ = 1;
+        const int grid = min(npairs, num_sms() * occ);
+        kernel<<<grid, PQ_THREADS, smem, st>>>(a, lut, codes, cap, cap2);
+    };
+    if (a.items) launch(ivfpq_scan_kernel<K, true>, cand_capacity(a.k, PQ_PAIR_SLACK));
+    launch(ivfpq_scan_kernel<K, false>, 0);
 }
 
 

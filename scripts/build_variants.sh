@@ -10,8 +10,9 @@ FLAGS="-O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -lineinfo -Xcompiler
 while [ $# -ge 2 ]; do
   NAME=$1; DEFS=$2; shift 2
   TMP=$(mktemp -d)
-  for s in rsb_dense rsb_ivf rsb_api rsb_bert rsb_tf32; do
-    nvcc $FLAGS $DEFS -c retrieval_scaling_b200/csrc/$s.cu -o $TMP/$s.o &
+  # the library's source list (retrieval_scaling_b200/_build.py), so a variant links every object librsb.so has
+  for s in $(python3 -c "import sys; sys.path.insert(0, 'retrieval_scaling_b200'); import _build; print(' '.join(_build.SOURCES))"); do
+    nvcc $FLAGS $DEFS -c retrieval_scaling_b200/csrc/$s -o $TMP/${s%.cu}.o &
   done
   wait
   nvcc -shared -o $OUT/librsb_$NAME.so $TMP/*.o -lcudart
