@@ -585,10 +585,11 @@ void launch_pq_lut_quant(const float* lut, int nq, int M, unsigned short* qlut, 
 // entries is at most 64 * 1023 < 2^16, so the lanes never carry into each other.  For the integer sum S of a vector:
 //     s <= dis0 + base + delta * S + err + gamma * (|dis0| + amax)
 // where s is the fp32 score the single-item path computes, err bounds the table's quantisation residuals and the
-// gamma term bounds the fp32 rounding of the ~66-term sum (gamma = 70 * 2^-24).  A vector is re-scored exactly
-// (pq_vector_score, from the fp32 table in global memory, in pq_block_score's summation order) iff S >= S_min, the
-// smallest S that could reach the running threshold, and is appended iff its exact score passes today's test: the
-// candidate sets, and so the results, are those of the single-item path.
+// gamma term bounds the fp32 rounding of the ~66-term sum (gamma = 70 * 2^-24).  A vector whose S >= S_min, the
+// smallest S that could reach the running threshold, is appended as a pending entry; pending entries are re-scored
+// exactly by the whole block (pq_resolve / pq_slot_score, from the fp32 table in global memory, in pq_block_score's
+// summation order) before any compaction and before the item's candidates are emitted, and kept iff the exact score
+// passes today's test: the candidate sets, and so the results, are those of the single-item path.
 // =============================================================================================================
 constexpr int PQ_THREADS = 256;
 constexpr int PQ_WARPS = PQ_THREADS / 32;
@@ -678,33 +679,35 @@ __device__ __forceinline__ T pq_block_score(const unsigned char* lutb, const uin
     return p[0];
 }
 
-// Exact fp32 score (without dis0) of this lane's block-local vector, for the lanes with `need` set (the others get
-// 0); all 32 lanes must call it.  Equal bit for bit to pq_block_score<K, FAST, float>: vector t of group g is
-// lane (g, t)'s vector, and lane (g, r) holds its pass-t chunk in c[t].  Every lane of the group runs pass t
-// (pq_pass, same entries, same order) on the fp32 table, giving partials p_0 .. p_{K-1} (index = lane rank).  The
-// shuffle tree of pq_block_score leaves lane t with, for K = 4, (p_t + p_{t^2}) + (p_{t^1} + p_{t^3}): step one adds
-// the partner at distance 2 to the kept partial, step two the partner at distance 1.  The two xor-shuffle
-// additions below compute exactly that in lane t (fp32 addition is commutative); K = 2 gives p_t + p_{t^1}, K = 1 p_0.
+// Exact fp32 score (without dis0) of the vector at `slot`, computed by one thread from the fp32 table in global
+// memory.  Equal bit for bit to pq_block_score<K, FAST, float>: block-local vector v = g*K + t is lane (g, t)'s
+// vector, and lane (g, r) holds its pass-t chunk, read here from the interleaved layout (rsb_layout.h) with lane
+// (g, r)'s look-up offsets.  Each pass runs pq_pass (same entries, same order), giving partials p_0 .. p_{K-1}
+// (index = lane rank).  The shuffle tree of pq_block_score leaves lane t with, for K = 4,
+// (p_t + p_{t^2}) + (p_{t^1} + p_{t^3}): step one adds the partner at distance 2 to the kept partial, step two the
+// partner at distance 1.  fp32 addition is commutative, so for every t that is (p_0 + p_2) + (p_1 + p_3); K = 2
+// gives p_0 + p_1, K = 1 p_0.  The passes run one at a time (16 table loads in flight), so the re-score fits in the
+// scan loop's register allocation.
 template <int K>
-__device__ __forceinline__ float pq_vector_score(const float* __restrict__ lutq, const uint4 (&c)[K],
-                                                 const unsigned (&off)[16], int r, bool need) {
+__device__ __forceinline__ float pq_slot_score(const float* __restrict__ lutq, const uint4* __restrict__ codes4,
+                                               unsigned slot) {
     const unsigned char* tb = reinterpret_cast<const unsigned char*>(lutq);
     const auto at = [tb](unsigned w, unsigned o, unsigned sel) {
         return __ldg(reinterpret_cast<const float*>(tb + __byte_perm(w, o, sel)));
     };
-    const int lane = threadIdx.x & 31;
-    float score = 0.f;
+    const int v = (int)(slot & 31u), g = v / K, t = v % K;
+    const uint4* chunk = codes4 + (size_t)(slot >> 5) * (K * 32) + t * 32 + g * K;   // + r: lane (g, r)'s chunk
+    float even = 0.f, odd = 0.f;                                     // p_0 (+ p_2), p_1 (+ p_3)
+#pragma unroll 1
+    for (int r = 0; r < K; ++r) {
+        unsigned off[16];
 #pragma unroll
-    for (int t = 0; t < K; ++t) {
-        const unsigned owners = __ballot_sync(0xffffffffu, need && r == t);
-        if (owners == 0u) continue;                                    // warp-uniform
-        float p = 0.f;
-        if ((owners >> (lane - r + t)) & 1u) p = pq_pass<float>(at, c[t], off);
-        if (K == 4) p += __shfl_xor_sync(0xffffffffu, p, 2);
-        if (K >= 2) p += __shfl_xor_sync(0xffffffffu, p, 1);
-        if (r == t) score = p;
+        for (int s = 0; s < 16; ++s) off[s] = 4u * (unsigned)pq_pos(16 * K, K, g, r, s);
+        const float p = pq_pass<float>(at, __ldg(chunk + r), off);
+        if (r & 1) odd = r < 2 ? p : odd + p;
+        else even = r < 2 ? p : even + p;
     }
-    return score;
+    return K == 1 ? even : even + odd;
 }
 
 // Predicated 128-bit loads: past the end of the list the registers simply keep their old contents (the scores of
@@ -805,36 +808,52 @@ struct PQPairState {
     int count[2];         // candidate counts
 };
 
-// Exact re-score of the flagged vectors of one block for query h of a paired item, appended under the usual rule
-// (exact ordered score > the query's threshold).  The threshold is the query's global one, which every block's
-// compactions raise: a valid bound like the register copy the single-item path keeps.  Not inlined: it runs for a
-// small fraction of the blocks, and its 16 outstanding table loads per pass would otherwise compete for registers
-// with the scan loop (spills); the call keeps them out of the loop's allocation.
+// Resolve the PENDING entries of query h's candidate buffer of a paired item.  The look-up loop appends a vector
+// whose integer sum reaches S_min as the key make_key(0, slot): no scored key has ordered score 0, because a scored
+// key is appended only when its ordered score exceeds a threshold >= 0.  Here each pending vector is re-scored
+// exactly (pq_slot_score) and kept iff its ordered score beats `tau`, a valid bound for the query like the register
+// copy the single-item path keeps; scored entries are kept as they are.  All threads call it at a block-uniform
+// point; afterwards the buffer holds scored keys only (in no particular order), so a compaction derives its
+// threshold from exact scores.  The buffer is rewritten in place, 256 entries per round: a round's survivors land
+// below the next round's entries.
 template <int K>
-__device__ __noinline__ void pq_rescore_append(const unsigned* tau_g, const float* lut_g, PQPairState* st, int h,
-                                               u64* keys, uint4 c0, uint4 c1, uint4 c2, uint4 c3, bool need,
-                                               unsigned slot) {
-    const int lane = threadIdx.x & 31, g = lane / K, r = lane % K;
-    unsigned off[16];
-#pragma unroll
-    for (int s = 0; s < 16; ++s) off[s] = 4u * (unsigned)pq_pos(16 * K, K, g, r, s);
-    uint4 c[K];
-    c[0] = c0;
-    if (K > 1) c[1] = c1;
-    if (K > 2) { c[2] = c2; c[K - 1] = c3; }
-    const int q = st->q[h];
-    const unsigned tau = *reinterpret_cast<const volatile unsigned*>(tau_g + q);
-    const float score = st->dis0[h] + pq_vector_score<K>(lut_g + (size_t)q * kLutWords, c, off, r, need);
-    const unsigned o = ord_f32(score);
-    warp_append(keys, &st->count[h], need && o > tau, make_key(o, slot));
+__device__ __forceinline__ void pq_resolve(u64* keys, PQPairState* st, int h, const float* __restrict__ lut_g,
+                                           const uint4* __restrict__ codes4, unsigned tau, u64* rescored) {
+    int* count = &st->count[h];
+    __syncthreads();                                                   // every append is done
+    const int n = *count;
+    __syncthreads();                                                   // every thread has read n
+    if (threadIdx.x == 0) *count = 0;
+    const float* lutq = lut_g + (size_t)st->q[h] * kLutWords;
+    const float dis0 = st->dis0[h];
+    for (int i0 = 0; i0 < n; i0 += PQ_THREADS) {
+        const int i = i0 + threadIdx.x;
+        u64 key = i < n ? keys[i] : 0ull;
+        const bool pending = i < n && key_ord(key) == 0u;
+        __syncthreads();                                               // this round's entries have been read
+        bool keep = i < n;
+        if (pending) {
+            const unsigned slot = key_slot(key);
+            const unsigned o = ord_f32(dis0 + pq_slot_score<K>(lutq, codes4, slot));
+            key = make_key(o, slot);
+            keep = o > tau;
+        }
+        if (rescored) {
+            const unsigned m = __ballot_sync(0xffffffffu, pending);
+            if (m && (threadIdx.x & 31) == 0) atomicAdd(rescored, (u64)__popc(m));
+        }
+        warp_append(keys, count, keep, key);
+    }
+    __syncthreads();
 }
 
 // scan one inverted list for the two queries of a paired item (packed 2 x 16-bit table in shared memory)
 template <int K, bool FAST>
 __device__ __forceinline__ void pq_scan_pair(const unsigned char* lutb, const uint4* cbase, int nblk, int len,
                                              unsigned slot0, const unsigned (&off)[16], int r, u64* keys_a,
-                                             u64* keys_b, PQPairState* st, const float* __restrict__ lut_g, int k,
-                                             int cap2, const ScanArgs& a, int lane, int warp) {
+                                             u64* keys_b, PQPairState* st, const float* __restrict__ lut_g,
+                                             const uint4* __restrict__ codes4, int k, int cap2, const ScanArgs& a,
+                                             int lane, int warp) {
     const int n_iter = (nblk + PQ_WARPS - 1) / PQ_WARPS;
     const int lim = cap2 - PQ_PAIR_SLACK;
     unsigned tau_a = *reinterpret_cast<const volatile unsigned*>(a.tau + st->q[0]);
@@ -845,63 +864,66 @@ __device__ __forceinline__ void pq_scan_pair(const unsigned char* lutb, const ui
     for (int t = 0; t < K; ++t) A[t] = B[t] = make_uint4(0, 0, 0, 0);
     pq_load_block<K>(A, cbase, warp, nblk, lane);
     pq_load_block<K>(B, cbase, warp + PQ_WARPS, nblk, lane);
-    // integer sums of both queries in one look-up; the few vectors whose sum reaches S_min are re-scored exactly
+    // integer sums of both queries in one look-up; a vector whose sum reaches S_min is appended as pending
 #define RSB_PQ_STEP2(X, b)                                                                                 \
     {                                                                                                      \
         const int b_ = (b);                                                                                \
         if (b_ < nblk) {                                                                                   \
             const unsigned sum = pq_block_score<K, FAST, unsigned>(lutb, X, off, r);                       \
             const int vi = b_ * 32 + lane;                                                                 \
-            const bool na = vi < len && (int)(sum & 0xffffu) >= smin_a;                                    \
-            const bool nb = vi < len && (int)(sum >> 16) >= smin_b;                                        \
-            if (__any_sync(0xffffffffu, na || nb)) {                                                       \
-                pq_rescore_append<K>(a.tau, lut_g, st, 0, keys_a, X[0], X[K > 1 ? 1 : 0], X[K > 2 ? 2 : 0],   \
-                                     X[K - 1], na, slot0 + (unsigned)vi);                                  \
-                pq_rescore_append<K>(a.tau, lut_g, st, 1, keys_b, X[0], X[K > 1 ? 1 : 0], X[K > 2 ? 2 : 0],   \
-                                     X[K - 1], nb, slot0 + (unsigned)vi);                                  \
-                if (a.rescored) {                                                                          \
-                    const int n = __popc(__ballot_sync(0xffffffffu, na)) +                                 \
-                                  __popc(__ballot_sync(0xffffffffu, nb));                                  \
-                    if (lane == 0) atomicAdd(a.rescored, (u64)n);                                          \
-                }                                                                                          \
-            }                                                                                              \
+            const u64 pend = make_key(0u, slot0 + (unsigned)vi);                                           \
+            warp_append(keys_a, &st->count[0], vi < len && (int)(sum & 0xffffu) >= smin_a, pend);          \
+            warp_append(keys_b, &st->count[1], vi < len && (int)(sum >> 16) >= smin_b, pend);              \
         }                                                                                                  \
         pq_load_block<K>(X, cbase, b_ + 2 * PQ_WARPS, nblk, lane);                                         \
     }
-    // One barrier checks both buffers.  A compaction that found k candidates raises the query's global threshold;
-    // S_min is recomputed whenever a threshold moved, by this block's compaction or by the global value.
-#define RSB_PQ_CHECKPOINT2()                                                                               \
+    // One barrier checks both buffers.  A buffer over its limit has its pending entries resolved, then is compacted;
+    // a compaction that found k candidates raises the query's global threshold.  The global thresholds (ga, gb) are
+    // read at the START of the code block and merged in here, so their loads are not waited for (a bound one block
+    // old is still a valid bound).  S_min is recomputed whenever a threshold moved.  The over-limit branch gives the
+    // two code register sets up to the re-score and loads their blocks (next X = bx, Y = by) again afterwards, so the
+    // re-score does not add to the loop's register allocation.
+#define RSB_PQ_CHECKPOINT2(X, bx, Y, by)                                                                   \
     {                                                                                                      \
         const unsigned ta0 = tau_a, tb0 = tau_b;                                                           \
+        tau_a = ga > tau_a ? ga : tau_a;                                                                   \
+        tau_b = gb > tau_b ? gb : tau_b;                                                                   \
         if (__syncthreads_or(*reinterpret_cast<volatile int*>(&st->count[0]) > lim ||                      \
                              *reinterpret_cast<volatile int*>(&st->count[1]) > lim)) {                     \
             if (st->count[0] > lim) {                                                                      \
-                const unsigned t_ = block_compact(keys_a, &st->count[0], k, cap2, tau_a);                    \
+                pq_resolve<K>(keys_a, st, 0, lut_g, codes4, tau_a, a.rescored);                            \
+                const unsigned t_ = block_compact(keys_a, &st->count[0], k, cap2, tau_a);                  \
                 if (t_ > tau_a && threadIdx.x == 0) raise_tau(a, st->q[0], t_);                            \
                 tau_a = t_;                                                                                \
             }                                                                                              \
             if (st->count[1] > lim) {                                                                      \
-                const unsigned t_ = block_compact(keys_b, &st->count[1], k, cap2, tau_b);                    \
+                pq_resolve<K>(keys_b, st, 1, lut_g, codes4, tau_b, a.rescored);                            \
+                const unsigned t_ = block_compact(keys_b, &st->count[1], k, cap2, tau_b);                  \
                 if (t_ > tau_b && threadIdx.x == 0) raise_tau(a, st->q[1], t_);                            \
                 tau_b = t_;                                                                                \
             }                                                                                              \
+            for (int t = 0; t < K; ++t) X[t] = Y[t] = make_uint4(0, 0, 0, 0);                              \
+            pq_load_block<K>(X, cbase, bx, nblk, lane);                                                    \
+            pq_load_block<K>(Y, cbase, by, nblk, lane);                                                    \
         }                                                                                                  \
-        const unsigned ga = *reinterpret_cast<const volatile unsigned*>(a.tau + st->q[0]);                 \
-        const unsigned gb = *reinterpret_cast<const volatile unsigned*>(a.tau + st->q[1]);                 \
-        tau_a = ga > tau_a ? ga : tau_a;                                                                   \
-        tau_b = gb > tau_b ? gb : tau_b;                                                                   \
         if (tau_a != ta0) smin_a = pq_smin(tau_a, st->thr[0][0], st->thr[0][1]);                           \
         if (tau_b != tb0) smin_b = pq_smin(tau_b, st->thr[1][0], st->thr[1][1]);                           \
     }
     for (int it = 0; it < n_iter; it += 2) {
         const int b0 = it * PQ_WARPS + warp;
+        unsigned ga = *reinterpret_cast<const volatile unsigned*>(a.tau + st->q[0]);
+        unsigned gb = *reinterpret_cast<const volatile unsigned*>(a.tau + st->q[1]);
         RSB_PQ_STEP2(A, b0);
-        RSB_PQ_CHECKPOINT2();
+        RSB_PQ_CHECKPOINT2(B, b0 + PQ_WARPS, A, b0 + 2 * PQ_WARPS);
+        ga = *reinterpret_cast<const volatile unsigned*>(a.tau + st->q[0]);
+        gb = *reinterpret_cast<const volatile unsigned*>(a.tau + st->q[1]);
         RSB_PQ_STEP2(B, b0 + PQ_WARPS);
-        RSB_PQ_CHECKPOINT2();
+        RSB_PQ_CHECKPOINT2(A, b0 + 2 * PQ_WARPS, B, b0 + 3 * PQ_WARPS);
     }
 #undef RSB_PQ_STEP2
 #undef RSB_PQ_CHECKPOINT2
+    pq_resolve<K>(keys_a, st, 0, lut_g, codes4, tau_a, a.rescored);     // emit sees scored keys only
+    pq_resolve<K>(keys_b, st, 1, lut_g, codes4, tau_b, a.rescored);
 }
 
 // PAIRED = false compiles the single-item path alone, so it keeps its own register allocation (the paired branch needs
@@ -998,6 +1020,7 @@ void ivfpq_scan_kernel(ScanArgs a, const float* __restrict__ lut_g, const uint8_
             const uint4* ta = reinterpret_cast<const uint4*>(a.qlut + (size_t)qa * kLutWords);
             const uint4* tb = reinterpret_cast<const uint4*>(a.qlut + (size_t)qb * kLutWords);
             uint4* dst = reinterpret_cast<uint4*>(lutb);
+#pragma unroll 2
             for (int i = tid; i < kLutWords / 8; i += PQ_THREADS) {
                 const uint4 x = __ldg(ta + i), y = __ldg(tb + i);
                 dst[2 * i] = make_uint4(__byte_perm(x.x, y.x, 0x5410), __byte_perm(x.x, y.x, 0x7632),
@@ -1018,12 +1041,13 @@ void ivfpq_scan_kernel(ScanArgs a, const float* __restrict__ lut_g, const uint8_
                 st->count[tid] = 0;
             }
             __syncthreads();
+            const uint4* codes4 = reinterpret_cast<const uint4*>(codes);
             if (fast)
-                pq_scan_pair<K, true>(lutb, cbase, nblk, len, (unsigned)slot0, off, r, keys_a, keys_b, st, lut_g, a.k,
-                                      cap2, a, lane, warp);
+                pq_scan_pair<K, true>(lutb, cbase, nblk, len, (unsigned)slot0, off, r, keys_a, keys_b, st, lut_g,
+                                      codes4, a.k, cap2, a, lane, warp);
             else
-                pq_scan_pair<K, false>(lutb, cbase, nblk, len, (unsigned)slot0, off, r, keys_a, keys_b, st, lut_g, a.k,
-                                       cap2, a, lane, warp);
+                pq_scan_pair<K, false>(lutb, cbase, nblk, len, (unsigned)slot0, off, r, keys_a, keys_b, st, lut_g,
+                                       codes4, a.k, cap2, a, lane, warp);
             __syncthreads();
             emit(w0, qa, keys_a, &st->count[0], cap2, 0u);
             emit(w1, qb, keys_b, &st->count[1], cap2, 0u);
