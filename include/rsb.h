@@ -182,6 +182,37 @@ int rsb_search_refine(rsb_index_t* h, const float* q_dev, int nq, int k, int k_f
                       int store_dtype, int64_t ntotal, float* D_dev, int64_t* I_dev, void* ws_dev, size_t ws_bytes,
                       rsb_stream_t stream);
 
+/* ---- tiered re-rank store: one logical [ntotal, d] store whose rows [0, n_dev) are device memory (store_dev) and
+ *      rows [n_dev, ntotal) page-locked host memory mapped into the device address space (store_host points at row
+ *      n_dev, not row 0).  n_dev = ntotal is the all-device store above; n_dev = 0 keeps every row on the host.
+ * Results are bit-identical to rsb_refine / rsb_search_refine on an all-device store holding the same values.
+ * Queries are processed in chunks of floor(staging_bytes / (k_base * d * elem_bytes)) (staging_bytes must hold at
+ * least one query's worst case).  Within a chunk the host-tier candidates are de-duplicated on the device (radix sort
+ * by id), every distinct host row crosses PCIe once into a staging buffer inside the workspace, and the re-rank reads
+ * it from there; device-tier rows never cross PCIe.  Nothing synchronises the host.
+ * host_rows_dev (device int64, may be NULL) is incremented by the number of distinct host rows gathered.
+ * Every argument is checked before any launch: a host tier that is not page-locked and mapped (pageable memory, a
+ * device pointer) returns RSB_ERR_INVALID. */
+int rsb_host_alloc(size_t bytes, void** out);   /* cudaHostAlloc(portable | mapped): exactly `bytes`, unlike torch's
+                                                   pinned allocator, which rounds blocks up to a power of two */
+int rsb_host_free(void* p);
+size_t rsb_refine_tiered_workspace_bytes(int nq, int k_base, int k, int d, int store_dtype, size_t staging_bytes);
+int rsb_refine_tiered(const float* q_dev, int nq, const void* store_dev, int64_t n_dev, const void* store_host,
+                      int store_dtype, int d, int64_t ntotal, const int64_t* cand_dev, int k_base, int k, float* D_dev,
+                      int64_t* I_dev, void* ws_dev, size_t ws_bytes, size_t staging_bytes, int64_t* host_rows_dev,
+                      rsb_stream_t stream);
+/* workspace for either store dtype */
+size_t rsb_search_refine_tiered_workspace_bytes(rsb_index_t* h, int nq, int k, int k_factor, int nprobe,
+                                                size_t staging_bytes);
+int rsb_search_refine_tiered(rsb_index_t* h, const float* q_dev, int nq, int k, int k_factor, int nprobe,
+                             const void* store_dev, int64_t n_dev, const void* store_host, int store_dtype, int64_t ntotal,
+                             float* D_dev, int64_t* I_dev, void* ws_dev, size_t ws_bytes, size_t staging_bytes,
+                             int64_t* host_rows_dev, rsb_stream_t stream);
+/* enable != 0: time the sort / gather / score stages of every later tiered chunk with CUDA events, on the device
+ * current at the call (this waits for each chunk on the host: for measurement only).  ms_out (may be NULL) receives
+ * the [3] milliseconds accumulated since the previous call, which resets them. */
+int rsb_refine_tiered_profile(int enable, double* ms_out);
+
 /* ---- shard merge (src/search.py:357-367; api/serve_main_node.py:130-163) ---------------------------- */
 /* D_all_dev/I_all_dev [nshards, nq, k]: concat per query, sort by score desc (ties: lower shard, then lower
  * rank, i.e. Python's stable sort over shard order), keep k_out.  Entries with id < 0 are ignored. */

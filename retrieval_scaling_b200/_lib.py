@@ -61,6 +61,15 @@ SIGNATURES = [
     ("rsb_search_refine_workspace_bytes", c_size_t, [_H, c_int, c_int, c_int, c_int]),
     ("rsb_search_refine", c_int, [_H, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int64, c_void_p, c_void_p,
                                   c_void_p, c_size_t, c_void_p]),
+    ("rsb_host_alloc", c_int, [c_size_t, POINTER(c_void_p)]),
+    ("rsb_host_free", c_int, [c_void_p]),
+    ("rsb_refine_tiered_workspace_bytes", c_size_t, [c_int, c_int, c_int, c_int, c_int, c_size_t]),
+    ("rsb_refine_tiered", c_int, [c_void_p, c_int, c_void_p, c_int64, c_void_p, c_int, c_int, c_int64, c_void_p, c_int,
+                                  c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_void_p, c_void_p]),
+    ("rsb_search_refine_tiered_workspace_bytes", c_size_t, [_H, c_int, c_int, c_int, c_int, c_size_t]),
+    ("rsb_search_refine_tiered", c_int, [_H, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_int,
+                                         c_int64, c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_void_p, c_void_p]),
+    ("rsb_refine_tiered_profile", c_int, [c_int, POINTER(c_double)]),
     ("rsb_merge_topk", c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     ("rsb_merge_topk_peers", c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     ("rsb_merge_topk_peers_scatter", c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,

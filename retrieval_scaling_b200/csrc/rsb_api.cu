@@ -1061,14 +1061,15 @@ extern "C" int rsb_search_preassigned_shared(rsb_index_t* h, const float* q, int
 }
 
 // ---- exact re-ranking (faiss IndexRefine::search) -----------------------------------------------------------
-static int refine_check(const void* store, int store_dtype, int d, int64_t ntotal, int k_base, int k) {
+// store_rows: rows behind `store` (-1: all ntotal); a tiered store's device tier holds n_dev of them
+static int refine_check(const void* store, int store_dtype, int d, int64_t ntotal, int k_base, int k, int64_t store_rows = -1) {
     if (store_dtype != RSB_DTYPE_F32 && store_dtype != RSB_DTYPE_F16)
         return fail(RSB_ERR_INVALID, "store_dtype must be RSB_DTYPE_F32 or RSB_DTYPE_F16, got %d", store_dtype);
     if (k <= 0 || k_base < k) return fail(RSB_ERR_INVALID, "need 0 < k <= k_base, got k = %d, k_base = %d", k, k_base);
     if (k_base > 4096) return fail(RSB_ERR_UNSUPPORTED, "k_base = k * k_factor = %d > 4096 is not supported", k_base);
     if (ntotal < 0 || ntotal > ((int64_t)1 << 31)) return fail(RSB_ERR_INVALID, "store rows must be in [0, 2^31], got %lld", (long long)ntotal);
     if (d <= 0 || d % 8) return fail(RSB_ERR_INVALID, "d = %d must be a positive multiple of 8 for the re-rank store", d);
-    if (ntotal > 0 && (!store || (reinterpret_cast<uintptr_t>(store) & 15)))
+    if ((store_rows < 0 ? ntotal : store_rows) > 0 && (!store || (reinterpret_cast<uintptr_t>(store) & 15)))
         return fail(RSB_ERR_INVALID, "the re-rank store must be a 16-byte aligned device pointer");
     return RSB_OK;
 }
@@ -1148,6 +1149,160 @@ extern "C" int rsb_search_refine(rsb_index_t* h, const float* q, int nq, int k, 
         RSB_TRY(refine_impl(qb, nb, store, store_dtype, h->d, ntotal, Ib, k_base, k, D + (size_t)q0 * k, I + (size_t)q0 * k,
                             w + p.off_ref, p.total - p.off_ref, (cudaStream_t)stream));
     }
+    return RSB_OK;
+}
+
+// ---- tiered re-rank store: rows [0, n_dev) in device memory, rows [n_dev, ntotal) in mapped page-locked host memory
+extern "C" int rsb_host_alloc(size_t bytes, void** out) {
+    if (!out) return fail(RSB_ERR_INVALID, "out is NULL");
+    *out = nullptr;
+    if (bytes == 0) return RSB_OK;
+    CU(cudaHostAlloc(out, bytes, cudaHostAllocPortable | cudaHostAllocMapped));
+    return RSB_OK;
+}
+
+extern "C" int rsb_host_free(void* p) {
+    if (p) CU(cudaFreeHost(p));
+    return RSB_OK;
+}
+
+// Argument checks that need no CUDA call.
+static int tiered_check(const void* store_dev, int64_t n_dev, const void* store_host, int store_dtype, int d,
+                        int64_t ntotal, int k_base, int k, size_t staging_bytes) {
+    if (n_dev < 0 || n_dev > ntotal)
+        return fail(RSB_ERR_INVALID, "n_dev = %lld must be in [0, ntotal = %lld]", (long long)n_dev, (long long)ntotal);
+    RSB_TRY(refine_check(store_dev, store_dtype, d, ntotal, k_base, k, n_dev));
+    const size_t per_q = (size_t)k_base * d * (store_dtype == RSB_DTYPE_F16 ? 2 : 4);
+    if (staging_bytes < per_q)
+        return fail(RSB_ERR_INVALID, "staging_bytes = %zu is below one query's worst case (k_base * d * elem = %zu)",
+                    staging_bytes, per_q);
+    if (n_dev < ntotal && (!store_host || (reinterpret_cast<uintptr_t>(store_host) & 15)))
+        return fail(RSB_ERR_INVALID, "the host tier must be a 16-byte aligned page-locked host pointer");
+    return RSB_OK;
+}
+
+// The host tier [first, first + bytes) must be page-locked and mapped: both ends are checked, and the kernels read it
+// through the device alias returned in *alias.  Pageable memory and device memory are refused.
+static int host_tier_alias(const void* first, size_t bytes, const void** alias) {
+    const unsigned char* p[2] = {static_cast<const unsigned char*>(first), static_cast<const unsigned char*>(first) + bytes - 1};
+    void* dp[2] = {nullptr, nullptr};
+    for (int i = 0; i < 2; ++i) {
+        cudaPointerAttributes a{};
+        if (cudaPointerGetAttributes(&a, p[i]) != cudaSuccess || a.type != cudaMemoryTypeHost) {
+            cudaGetLastError();
+            return fail(RSB_ERR_INVALID, "the host tier is not page-locked host memory (rsb_host_alloc / cudaHostAlloc)");
+        }
+        if (cudaHostGetDevicePointer(&dp[i], const_cast<unsigned char*>(p[i]), 0) != cudaSuccess) {
+            cudaGetLastError();
+            return fail(RSB_ERR_INVALID, "the host tier is not mapped into the device address space (cudaHostAllocMapped)");
+        }
+    }
+    if (static_cast<unsigned char*>(dp[1]) != static_cast<unsigned char*>(dp[0]) + bytes - 1)
+        return fail(RSB_ERR_INVALID, "the host tier is not one mapped allocation");
+    *alias = dp[0];
+    return RSB_OK;
+}
+
+// Both the workspace query and the call size the workspace for the larger of the fp16 and fp32 plans, so one query
+// serves either store dtype.
+static size_t tiered_ws(int nq, int k_base, int k, int d, size_t staging_bytes) {
+    const TieredPlan a = tiered_plan(nq, k_base, k, d, 2, staging_bytes), b = tiered_plan(nq, k_base, k, d, 4, staging_bytes);
+    return std::max(a.qc ? a.total : 0, b.qc ? b.total : 0);
+}
+
+// Validated: the tiered re-rank of nq queries (all device rows: the plain kernel; no staging, no host rows).
+static int refine_tiered_impl(const float* q, int nq, const void* store_dev, int64_t n_dev, const void* host_alias,
+                              int store_dtype, int d, int64_t ntotal, const int64_t* cand, int k_base, int k, float* D,
+                              int64_t* I, void* ws, size_t ws_bytes, size_t staging_bytes, int64_t* host_rows,
+                              cudaStream_t st) {
+    const int eb = store_dtype == RSB_DTYPE_F16 ? 2 : 4;
+    if (n_dev == ntotal) return refine_impl(q, nq, store_dev, store_dtype, d, ntotal, cand, k_base, k, D, I, ws, ws_bytes, st);
+    const TieredPlan p = tiered_plan(nq, k_base, k, d, eb, staging_bytes);
+    if (!p.qc) return fail(RSB_ERR_CUDA, "could not size the tiered re-rank workspace: %s", cudaGetErrorString(cudaGetLastError()));
+    if (!p.smem_ok)
+        return fail(RSB_ERR_UNSUPPORTED, "d = %d with k_base = %d needs more shared memory than the re-rank kernel has", d, k_base);
+    if (ws_bytes < p.total) return fail(RSB_ERR_OOM, "workspace too small: need %zu bytes, got %zu", p.total, ws_bytes);
+    const cudaError_t e = launch_refine_tiered(p, q, nq, store_dev, n_dev, host_alias, eb, d, ntotal, cand, k_base, k, D, I,
+                                               ws, reinterpret_cast<long long*>(host_rows), st);
+    if (e != cudaSuccess) return fail(RSB_ERR_CUDA, "tiered re-rank: %s", cudaGetErrorString(e));
+    return RSB_OK;
+}
+
+extern "C" size_t rsb_refine_tiered_workspace_bytes(int nq, int k_base, int k, int d, int store_dtype, size_t staging_bytes) {
+    if (nq <= 0 || k <= 0 || k_base < k || k_base > 4096 || d <= 0 || d % 8) return 0;
+    if (store_dtype != RSB_DTYPE_F32 && store_dtype != RSB_DTYPE_F16) return 0;
+    return std::max(refine_plan(nq, k_base, k).ws_bytes, tiered_ws(nq, k_base, k, d, staging_bytes));
+}
+
+extern "C" int rsb_refine_tiered(const float* q, int nq, const void* store_dev, int64_t n_dev, const void* store_host,
+                                 int store_dtype, int d, int64_t ntotal, const int64_t* cand, int k_base, int k, float* D,
+                                 int64_t* I, void* ws, size_t ws_bytes, size_t staging_bytes, int64_t* host_rows,
+                                 rsb_stream_t stream) {
+    RSB_TRY(tiered_check(store_dev, n_dev, store_host, store_dtype, d, ntotal, k_base, k, staging_bytes));
+    if (nq < 0) return fail(RSB_ERR_INVALID, "bad nq = %d", nq);
+    if (nq == 0) return RSB_OK;
+    if (!q || !cand || !D || !I) return fail(RSB_ERR_INVALID, "null argument");
+    const void* alias = nullptr;
+    if (n_dev < ntotal)
+        RSB_TRY(host_tier_alias(store_host, (size_t)(ntotal - n_dev) * d * (store_dtype == RSB_DTYPE_F16 ? 2 : 4), &alias));
+    return refine_tiered_impl(q, nq, store_dev, n_dev, alias, store_dtype, d, ntotal, cand, k_base, k, D, I, ws, ws_bytes,
+                              staging_bytes, host_rows, (cudaStream_t)stream);
+}
+
+static size_t search_refine_tiered_ws(rsb_index* h, int nq, int k, int k_base, int nprobe, size_t staging_bytes,
+                                      size_t* off_ref) {
+    const SearchRefinePlan p = search_refine_plan(h, nq, k, k_base, nprobe);
+    const int n = std::max(nq, 1), last = n % p.qb ? n % p.qb : p.qb;
+    *off_ref = p.off_ref;
+    return p.total + std::max(tiered_ws(p.qb, k_base, k, h->d, staging_bytes), tiered_ws(last, k_base, k, h->d, staging_bytes));
+}
+
+extern "C" size_t rsb_search_refine_tiered_workspace_bytes(rsb_index_t* h, int nq, int k, int k_factor, int nprobe,
+                                                          size_t staging_bytes) {
+    if (!h || k <= 0 || k_factor <= 0 || (int64_t)k * k_factor > 4096) return 0;
+    size_t off_ref = 0;
+    return search_refine_tiered_ws(h, nq, k, k * k_factor, nprobe, staging_bytes, &off_ref);
+}
+
+extern "C" int rsb_search_refine_tiered(rsb_index_t* h, const float* q, int nq, int k, int k_factor, int nprobe,
+                                        const void* store_dev, int64_t n_dev, const void* store_host, int store_dtype,
+                                        int64_t ntotal, float* D, int64_t* I, void* ws, size_t ws_bytes,
+                                        size_t staging_bytes, int64_t* host_rows, rsb_stream_t stream) {
+    if (!h) return fail(RSB_ERR_INVALID, "null handle");
+    if (h->kind != RSB_IVFPQ) return fail(RSB_ERR_INVALID, "re-ranking is for IVFPQ indexes: Flat / IVFFlat scores are already exact");
+    if (k <= 0 || k_factor <= 0) return fail(RSB_ERR_INVALID, "bad k = %d / k_factor = %d", k, k_factor);
+    if ((int64_t)k * k_factor > 4096) return fail(RSB_ERR_UNSUPPORTED, "k * k_factor = %lld > 4096 is not supported", (long long)k * k_factor);
+    const int k_base = k * k_factor;
+    RSB_TRY(tiered_check(store_dev, n_dev, store_host, store_dtype, h->d, ntotal, k_base, k, staging_bytes));
+    if (ntotal != h->ntotal + h->n_staged)
+        return fail(RSB_ERR_INVALID, "the re-rank store has %lld rows, the index holds %lld vectors", (long long)ntotal,
+                    (long long)(h->ntotal + h->n_staged));
+    if (nq < 0) return fail(RSB_ERR_INVALID, "bad nq = %d", nq);
+    if (nq == 0) return RSB_OK;
+    if (!q || !D || !I) return fail(RSB_ERR_INVALID, "null argument");
+    const void* alias = nullptr;
+    if (n_dev < ntotal)
+        RSB_TRY(host_tier_alias(store_host, (size_t)(ntotal - n_dev) * h->d * (store_dtype == RSB_DTYPE_F16 ? 2 : 4), &alias));
+    size_t off_ref = 0;
+    const size_t total = search_refine_tiered_ws(h, nq, k, k_base, nprobe, staging_bytes, &off_ref);
+    if (ws_bytes < total) return fail(RSB_ERR_OOM, "workspace too small: need %zu bytes, got %zu", total, ws_bytes);
+    const SearchRefinePlan p = search_refine_plan(h, nq, k, k_base, nprobe);
+    unsigned char* w = static_cast<unsigned char*>(ws);
+    float* Db = reinterpret_cast<float*>(w + p.off_D);
+    int64_t* Ib = reinterpret_cast<int64_t*>(w + p.off_I);
+    for (int q0 = 0; q0 < nq; q0 += p.qb) {
+        const int nb = std::min(p.qb, nq - q0);
+        const float* qb = q + (size_t)q0 * h->d;
+        RSB_TRY(rsb_search(h, qb, nb, k_base, nprobe, Db, Ib, w, p.search_ws, stream));
+        RSB_TRY(refine_tiered_impl(qb, nb, store_dev, n_dev, alias, store_dtype, h->d, ntotal, Ib, k_base, k,
+                                   D + (size_t)q0 * k, I + (size_t)q0 * k, w + off_ref, ws_bytes - off_ref, staging_bytes,
+                                   host_rows, (cudaStream_t)stream));
+    }
+    return RSB_OK;
+}
+
+extern "C" int rsb_refine_tiered_profile(int enable, double* ms_out) {
+    if (tiered_profile(enable, ms_out) != 0) return fail(RSB_ERR_CUDA, "cudaEventCreate failed");
     return RSB_OK;
 }
 

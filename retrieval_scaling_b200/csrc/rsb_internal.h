@@ -74,11 +74,37 @@ struct RefinePlan {
     size_t ws_bytes;      // partial keys + counts (0 when nchunks == 1)
 };
 RefinePlan refine_plan(int nq, int k_base, int k);
+bool refine_smem_fits(const RefinePlan& p, int d);    // P * 8 + d * 4 bytes of shared memory <= 200 KB
+// tiered store: rows id >= n_dev are read from staging + slot[q * k_base + j] * d
+struct TierArgs {
+    int64_t n_dev;
+    const void* staging;
+    const int* slot;      // [nq, k_base]
+};
 // X: store [ntotal, d], elem_bytes 2 (fp16) or 4 (fp32); cand [nq, k_base] ids (-1 = skip); returns <0 if the shared
-// memory the kernel needs (P * 8 + d * 4 bytes) exceeds 200 KB
+// memory the kernel needs does not fit (refine_smem_fits)
 int launch_refine_rows(const RefinePlan& p, const float* Q, int nq, const void* X, int elem_bytes, int d,
                        int64_t ntotal, const int64_t* cand, int k_base, int k, float* D, int64_t* I, void* ws,
-                       cudaStream_t st);
+                       cudaStream_t st, const TierArgs* tier = nullptr);
+// Workspace of a tiered re-rank of nq queries: queries are processed qc at a time, qc = the queries whose worst case
+// (k_base * d * elem_bytes each) fits staging_bytes.  qc = 0: staging_bytes is below one query's worst case, or the
+// CUB temporary sizes could not be queried.
+struct TieredPlan {
+    int qc;
+    bool smem_ok;
+    size_t cub_bytes, ref_bytes;
+    size_t off_keys, off_keys2, off_vals, off_vals2, off_slot, off_uniq, off_count, off_cub, off_ref, off_stage, total;
+};
+TieredPlan tiered_plan(int nq, int k_base, int k, int d, int elem_bytes, size_t staging_bytes);
+// X_dev: rows [0, n_dev); X_host: device alias of the mapped host tier, rows [n_dev, ntotal) (n_dev < ntotal).
+// host_rows (nullable) += distinct host rows gathered.
+cudaError_t launch_refine_tiered(const TieredPlan& p, const float* Q, int nq, const void* X_dev, int64_t n_dev,
+                                 const void* X_host, int elem_bytes, int d, int64_t ntotal, const int64_t* cand,
+                                 int k_base, int k, float* D, int64_t* I, void* ws, long long* host_rows,
+                                 cudaStream_t st);
+// enable != 0: time every later tiered chunk's sort / gather / score with events (synchronises per chunk).
+// ms3 (nullable) <- the milliseconds accumulated since the previous call, which resets them.
+int tiered_profile(int enable, double* ms3);
 
 // ---- rsb_tf32.cu (tensor-core fp32-accurate scores: 3xTF32 on wgmma) ---------------------------------
 bool tf32_path_available();

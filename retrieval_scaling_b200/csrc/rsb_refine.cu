@@ -8,11 +8,22 @@
 // The kernel is bound by gather bandwidth: every candidate row is read once per query (nq * k' * d * elem_bytes bytes
 // per batch) and used for one dot product.  A warp scores RF_ROWS rows at a time and issues all of their 16-byte loads
 // before it consumes any of them, so each warp keeps several rows in flight; the query lives in shared memory.
+//
+// Tiered store (rows [0, n_dev) in device memory, rows [n_dev, ntotal) in mapped page-locked host memory), per chunk
+// of queries whose worst case fits the staging buffer:
+//   tier_keys_kernel -> cub radix sort of (host row, candidate position) -> tier_flag_kernel -> cub inclusive scan
+//   -> tier_scatter_kernel   every distinct host row of the chunk gets one staging slot; slot[q, j] per candidate
+//   gather_host_rows_kernel<T>   copies the distinct host rows over PCIe into the staging buffer, once each
+//   refine_rows_kernel<T, true>  as above, reading host-tier rows from the staging buffer
+// The distinct-row count stays on the device (the gather grid covers the worst case), so nothing synchronises the host.
 #include "rsb_common.cuh"
 #include "rsb_internal.h"
 
+#include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
 #include <cuda_fp16.h>
 #include <float.h>
+#include <limits.h>
 
 #include <algorithm>
 
@@ -53,12 +64,15 @@ __device__ __forceinline__ float dot8(const uint4 (&v)[1], const float* qs, floa
 // direct = 0: writes the chunk's best min(k_item, valid) keys to out_keys[(q * nchunks + c) * k_item ...] and their
 // number to out_cnt[q * nchunks + c], for merge_items_flat_kernel.
 // Four CTAs per SM (64 registers): without the bound ptxas picks 48 registers for the fp32 form and spills.
-template <typename T>
+// TIERED: ids >= n_dev are read from staging + slot[q * k_base + j] * d instead of X + id * d (the key keeps the id);
+// the lane mapping and the fmaf order are the same, so a row scores bit-identically from either place.
+template <typename T, bool TIERED>
 __global__ __launch_bounds__(RF_THREADS, 4)
 void refine_rows_kernel(const float* __restrict__ Q, const T* __restrict__ X, int d, int64_t ntotal,
                         const int64_t* __restrict__ cand, int k_base, int chunk, int P, int k_out, int direct,
                         float* __restrict__ D, int64_t* __restrict__ I, u64* __restrict__ out_keys,
-                        int* __restrict__ out_cnt) {
+                        int* __restrict__ out_cnt, int64_t n_dev, const T* __restrict__ staging,
+                        const int* __restrict__ slot) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     u64* keys = reinterpret_cast<u64*>(smem_raw);                     // [P]
     float* qs = reinterpret_cast<float*>(smem_raw + (size_t)P * 8);   // [d]
@@ -81,7 +95,9 @@ void refine_rows_kernel(const float* __restrict__ Q, const T* __restrict__ X, in
         for (int r = 0; r < RF_ROWS; ++r) {
             id[r] = r0 + r < n ? ids[r0 + r] : -1;
             ok[r] = id[r] >= 0 && id[r] < ntotal;                     // warp-uniform
-            row[r] = reinterpret_cast<const uint4*>(X + (size_t)(ok[r] ? id[r] : 0) * d);
+            const T* src = X + (size_t)(ok[r] ? id[r] : 0) * d;
+            if (TIERED && ok[r] && id[r] >= n_dev) src = staging + (size_t)slot[(size_t)q * k_base + j0 + r0 + r] * d;
+            row[r] = reinterpret_cast<const uint4*>(src);
             acc[r] = 0.f;
         }
         for (int e = lane * RF_E; e < d; e += 32 * RF_E) {
@@ -140,31 +156,234 @@ RefinePlan refine_plan(int nq, int k_base, int k) {
     return p;
 }
 
+bool refine_smem_fits(const RefinePlan& p, int d) { return (size_t)p.P * 8 + (size_t)d * 4 <= 200 * 1024; }
+
+template <typename T, bool TIERED>
+static void launch_rows(const RefinePlan& p, dim3 grid, size_t smem, const float* Q, const void* X, int d, int64_t ntotal,
+                        const int64_t* cand, int k_base, int k, int direct, float* D, int64_t* I, u64* keys, int* cnt,
+                        const TierArgs* tier, cudaStream_t st) {
+    static PerDeviceSize configured;
+    if (smem > 48 * 1024 && configured.raise(smem))
+        cudaFuncSetAttribute(refine_rows_kernel<T, TIERED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    refine_rows_kernel<T, TIERED><<<grid, RF_THREADS, smem, st>>>(
+        Q, static_cast<const T*>(X), d, ntotal, cand, k_base, p.chunk, p.P, k, direct, D, I, keys, cnt,
+        TIERED ? tier->n_dev : ntotal, TIERED ? static_cast<const T*>(tier->staging) : nullptr,
+        TIERED ? tier->slot : nullptr);
+}
+
 int launch_refine_rows(const RefinePlan& p, const float* Q, int nq, const void* X, int elem_bytes, int d,
                        int64_t ntotal, const int64_t* cand, int k_base, int k, float* D, int64_t* I, void* ws,
-                       cudaStream_t st) {
+                       cudaStream_t st, const TierArgs* tier) {
     if (nq <= 0) return 0;
     const size_t smem = (size_t)p.P * 8 + (size_t)d * 4;
-    if (smem > 200 * 1024) return -1;
+    if (!refine_smem_fits(p, d)) return -1;
     const int direct = p.nchunks == 1;
     u64* keys = direct ? nullptr : static_cast<u64*>(ws);
     int* cnt = direct ? nullptr : reinterpret_cast<int*>(static_cast<unsigned char*>(ws) + (size_t)nq * p.nchunks * p.k_item * 8);
     dim3 grid(nq, p.nchunks);
     if (elem_bytes == 2) {
-        static PerDeviceSize configured;
-        if (smem > 48 * 1024 && configured.raise(smem))
-            cudaFuncSetAttribute(refine_rows_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        refine_rows_kernel<__half><<<grid, RF_THREADS, smem, st>>>(Q, static_cast<const __half*>(X), d, ntotal, cand, k_base,
-                                                                   p.chunk, p.P, k, direct, D, I, keys, cnt);
+        if (tier) launch_rows<__half, true>(p, grid, smem, Q, X, d, ntotal, cand, k_base, k, direct, D, I, keys, cnt, tier, st);
+        else launch_rows<__half, false>(p, grid, smem, Q, X, d, ntotal, cand, k_base, k, direct, D, I, keys, cnt, tier, st);
     } else {
-        static PerDeviceSize configured;
-        if (smem > 48 * 1024 && configured.raise(smem))
-            cudaFuncSetAttribute(refine_rows_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        refine_rows_kernel<float><<<grid, RF_THREADS, smem, st>>>(Q, static_cast<const float*>(X), d, ntotal, cand, k_base,
-                                                                  p.chunk, p.P, k, direct, D, I, keys, cnt);
+        if (tier) launch_rows<float, true>(p, grid, smem, Q, X, d, ntotal, cand, k_base, k, direct, D, I, keys, cnt, tier, st);
+        else launch_rows<float, false>(p, grid, smem, Q, X, d, ntotal, cand, k_base, k, direct, D, I, keys, cnt, tier, st);
     }
     if (!direct) launch_merge_items(keys, cnt, nq, p.nchunks, p.k_item, k, nullptr, 0, D, I, st);
     return 0;
+}
+
+// ---- tiered store: de-duplication of host-tier candidates, staged gather ------------------------------------------
+constexpr int TK_THREADS = 256;
+constexpr int GH_THREADS = 256, GH_U = 8;     // gather: 8 independent 16-byte loads per thread, all issued before any store
+
+// key = host row (id - n_dev) for a host-tier candidate, n_host (sorts last) for anything else; value = position.
+__global__ void tier_keys_kernel(const int64_t* __restrict__ cand, int L, int64_t n_dev, int64_t ntotal, unsigned n_host,
+                                 unsigned* __restrict__ keys, int* __restrict__ vals, int* __restrict__ slot) {
+    const int i = blockIdx.x * TK_THREADS + threadIdx.x;
+    if (i >= L) return;
+    const int64_t id = cand[i];
+    keys[i] = id >= n_dev && id < ntotal ? (unsigned)(id - n_dev) : n_host;
+    vals[i] = i;
+    slot[i] = -1;
+}
+
+// flag[i] = 1 on the first element of each run of equal host rows (sorted keys)
+__global__ void tier_flag_kernel(const unsigned* __restrict__ keys, int L, unsigned n_host, int* __restrict__ flag) {
+    const int i = blockIdx.x * TK_THREADS + threadIdx.x;
+    if (i >= L) return;
+    const unsigned key = keys[i];
+    flag[i] = key < n_host && (i == 0 || keys[i - 1] != key);
+}
+
+// inc = inclusive scan of flag: the run of element i owns staging slot inc[i] - 1
+__global__ void tier_scatter_kernel(const unsigned* __restrict__ keys, const int* __restrict__ vals,
+                                    const int* __restrict__ flag, const int* __restrict__ inc, int L, unsigned n_host,
+                                    int* __restrict__ slot, unsigned* __restrict__ uniq, int* __restrict__ count,
+                                    long long* __restrict__ host_rows) {
+    const int i = blockIdx.x * TK_THREADS + threadIdx.x;
+    if (i >= L) return;
+    const unsigned key = keys[i];
+    if (key < n_host) {
+        slot[vals[i]] = inc[i] - 1;
+        if (flag[i]) uniq[inc[i] - 1] = key;
+    }
+    if (i == L - 1) {
+        *count = inc[i];
+        if (host_rows) *host_rows += inc[i];
+    }
+}
+
+// staging[s] = host[uniq[s]] for s < *count.  The grid covers the worst case (every candidate distinct); blocks past
+// the device-side count return at once.  host is the device alias of the mapped host tier (row 0 = store row n_dev).
+template <typename T>
+__global__ __launch_bounds__(GH_THREADS)
+void gather_host_rows_kernel(const uint4* __restrict__ host, const unsigned* __restrict__ uniq,
+                             const int* __restrict__ count, int d, uint4* __restrict__ staging) {
+    const int row16 = d * (int)sizeof(T) / 16;
+    const size_t total = (size_t)*count * row16;
+    const size_t b0 = (size_t)blockIdx.x * GH_THREADS * GH_U + threadIdx.x;
+    if (b0 - threadIdx.x >= total) return;
+    uint4 v[GH_U];
+#pragma unroll
+    for (int u = 0; u < GH_U; ++u) {
+        const size_t e = b0 + (size_t)u * GH_THREADS;
+        if (e < total) {
+            const size_t r = e / row16;
+            v[u] = host[(size_t)uniq[r] * row16 + (e - r * row16)];
+        }
+    }
+#pragma unroll
+    for (int u = 0; u < GH_U; ++u) {
+        const size_t e = b0 + (size_t)u * GH_THREADS;
+        if (e < total) staging[e] = v[u];
+    }
+}
+
+static size_t al(size_t x) { return (x + 255) / 256 * 256; }
+
+TieredPlan tiered_plan(int nq, int k_base, int k, int d, int elem_bytes, size_t staging_bytes) {
+    TieredPlan p{};
+    nq = std::max(nq, 1);
+    const size_t per_q = (size_t)k_base * d * elem_bytes;
+    if (per_q == 0 || staging_bytes < per_q) return p;
+    size_t qc = std::min<size_t>(staging_bytes / per_q, (size_t)nq);
+    qc = std::min<size_t>(qc, (size_t)(INT_MAX / k_base));
+    p.qc = (int)qc;
+    const int last = nq % p.qc ? nq % p.qc : p.qc;
+    const int L = p.qc * k_base;
+    size_t sort_bytes = 0, scan_bytes = 0;
+    if (cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const unsigned*)nullptr, (unsigned*)nullptr,
+                                        (const int*)nullptr, (int*)nullptr, L, 0, 32) != cudaSuccess ||
+        cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, (const int*)nullptr, (int*)nullptr, L) != cudaSuccess) {
+        cudaGetLastError();
+        p.qc = 0;
+        return p;
+    }
+    p.cub_bytes = std::max(sort_bytes, scan_bytes);
+    p.ref_bytes = std::max(refine_plan(p.qc, k_base, k).ws_bytes, refine_plan(last, k_base, k).ws_bytes);
+    p.smem_ok = refine_smem_fits(refine_plan(p.qc, k_base, k), d) && refine_smem_fits(refine_plan(last, k_base, k), d);
+    const size_t a4 = al((size_t)L * 4);
+    p.off_keys = 0;                      // tier keys, then the run flags
+    p.off_keys2 = p.off_keys + a4;       // sorted keys
+    p.off_vals = p.off_keys2 + a4;       // positions, then the inclusive scan
+    p.off_vals2 = p.off_vals + a4;       // sorted positions
+    p.off_slot = p.off_vals2 + a4;
+    p.off_uniq = p.off_slot + a4;
+    p.off_count = p.off_uniq + a4;
+    p.off_cub = p.off_count + 256;
+    p.off_ref = p.off_cub + al(p.cub_bytes);
+    p.off_stage = p.off_ref + al(p.ref_bytes);
+    p.total = p.off_stage + al(qc * per_q);
+    return p;
+}
+
+struct TierProfile {
+    bool on = false;
+    cudaEvent_t ev[4] = {};
+    double ms[3] = {0, 0, 0};
+};
+static TierProfile g_tier_prof;
+
+int tiered_profile(int enable, double* ms3) {
+    TierProfile& t = g_tier_prof;
+    if (ms3)
+        for (int i = 0; i < 3; ++i) ms3[i] = t.ms[i];
+    for (double& m : t.ms) m = 0;
+    if (enable && !t.on) {
+        for (auto& e : t.ev)
+            if (cudaEventCreate(&e) != cudaSuccess) return -1;
+    } else if (!enable && t.on) {
+        for (auto& e : t.ev) cudaEventDestroy(e);
+    }
+    t.on = enable != 0;
+    return 0;
+}
+
+cudaError_t launch_refine_tiered(const TieredPlan& p, const float* Q, int nq, const void* X_dev, int64_t n_dev,
+                                 const void* X_host, int elem_bytes, int d, int64_t ntotal, const int64_t* cand,
+                                 int k_base, int k, float* D, int64_t* I, void* ws, long long* host_rows,
+                                 cudaStream_t st) {
+    unsigned char* w = static_cast<unsigned char*>(ws);
+    unsigned* keys = reinterpret_cast<unsigned*>(w + p.off_keys);
+    unsigned* keys2 = reinterpret_cast<unsigned*>(w + p.off_keys2);
+    int* flag = reinterpret_cast<int*>(w + p.off_keys);
+    int* vals = reinterpret_cast<int*>(w + p.off_vals);
+    int* inc = reinterpret_cast<int*>(w + p.off_vals);
+    int* vals2 = reinterpret_cast<int*>(w + p.off_vals2);
+    int* slot = reinterpret_cast<int*>(w + p.off_slot);
+    unsigned* uniq = reinterpret_cast<unsigned*>(w + p.off_uniq);
+    int* count = reinterpret_cast<int*>(w + p.off_count);
+    void* cub_tmp = w + p.off_cub;
+    const unsigned n_host = (unsigned)(ntotal - n_dev);
+    int bits = 1;
+    while (bits < 32 && ((uint64_t)1 << bits) <= n_host) ++bits;     // n_host itself (the "not host" key) must fit
+    uint4* staging = reinterpret_cast<uint4*>(w + p.off_stage);
+    TierArgs tier;
+    tier.n_dev = n_dev;
+    tier.staging = staging;
+    tier.slot = slot;
+    TierProfile& prof = g_tier_prof;
+    const size_t row_bytes = (size_t)d * elem_bytes;
+    for (int q0 = 0; q0 < nq; q0 += p.qc) {
+        const int nc = std::min(p.qc, nq - q0);
+        const int L = nc * k_base;
+        const int tb = (L + TK_THREADS - 1) / TK_THREADS;
+        const int64_t* cq = cand + (size_t)q0 * k_base;
+        if (prof.on) cudaEventRecord(prof.ev[0], st);
+        tier_keys_kernel<<<tb, TK_THREADS, 0, st>>>(cq, L, n_dev, ntotal, n_host, keys, vals, slot);
+        size_t tmp = p.cub_bytes;
+        cudaError_t e = cub::DeviceRadixSort::SortPairs(cub_tmp, tmp, keys, keys2, vals, vals2, L, 0, bits, st);
+        if (e != cudaSuccess) return e;
+        tier_flag_kernel<<<tb, TK_THREADS, 0, st>>>(keys2, L, n_host, flag);
+        tmp = p.cub_bytes;
+        e = cub::DeviceScan::InclusiveSum(cub_tmp, tmp, flag, inc, L, st);
+        if (e != cudaSuccess) return e;
+        tier_scatter_kernel<<<tb, TK_THREADS, 0, st>>>(keys2, vals2, flag, inc, L, n_host, slot, uniq, count, host_rows);
+        if (prof.on) cudaEventRecord(prof.ev[1], st);
+        const size_t words = (size_t)L * row_bytes / 16;
+        const unsigned gb = (unsigned)((words + GH_THREADS * GH_U - 1) / (GH_THREADS * GH_U));
+        if (elem_bytes == 2)
+            gather_host_rows_kernel<__half><<<gb, GH_THREADS, 0, st>>>(static_cast<const uint4*>(X_host), uniq, count, d, staging);
+        else
+            gather_host_rows_kernel<float><<<gb, GH_THREADS, 0, st>>>(static_cast<const uint4*>(X_host), uniq, count, d, staging);
+        if (prof.on) cudaEventRecord(prof.ev[2], st);
+        if (launch_refine_rows(refine_plan(nc, k_base, k), Q + (size_t)q0 * d, nc, X_dev, elem_bytes, d, ntotal, cq,
+                               k_base, k, D + (size_t)q0 * k, I + (size_t)q0 * k, w + p.off_ref, st, &tier) != 0)
+            return cudaErrorInvalidConfiguration;       // not reached: the caller checked p.smem_ok
+        if (prof.on) {                                  // profiling only: waits for the chunk to read its events
+            cudaEventRecord(prof.ev[3], st);
+            e = cudaEventSynchronize(prof.ev[3]);
+            if (e != cudaSuccess) return e;
+            for (int i = 0; i < 3; ++i) {
+                float ms = 0.f;
+                cudaEventElapsedTime(&ms, prof.ev[i], prof.ev[i + 1]);
+                prof.ms[i] += ms;
+            }
+        }
+        e = cudaPeekAtLastError();
+        if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
 }
 
 }  // namespace rsb

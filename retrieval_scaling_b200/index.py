@@ -384,6 +384,42 @@ class IndexIVFPQ(_IVFBase):
             torch.cuda.current_stream().synchronize()
 
 
+class _PinnedOwner:
+    """Frees an rsb_host_alloc buffer once nothing references it (the ctypes array the CPU tensor is built on holds
+    this object)."""
+
+    def __init__(self, L, ptr: int, device):
+        self.L, self.ptr, self.device = L, ptr, device
+
+    def __del__(self):
+        try:
+            torch.cuda.current_stream(self.device).synchronize()     # no search in flight may still read it
+            self.L.rsb_host_free(ctypes.c_void_p(self.ptr))
+        except Exception:
+            pass
+
+
+def _pinned_rows(L, rows: int, d: int, dtype: torch.dtype, device) -> torch.Tensor:
+    """A CPU tensor [rows, d] over page-locked, device-mapped host memory of exactly rows * d elements (rsb_host_alloc;
+    torch's pinned allocator would round the block up to a power of two)."""
+    nbytes = int(rows) * d * torch.empty((), dtype=dtype).element_size()
+    if nbytes == 0:
+        return torch.empty((0, d), dtype=dtype)
+    p = ctypes.c_void_p(0)
+    _lib.check(L.rsb_host_alloc(nbytes, ctypes.byref(p)))
+    buf = (ctypes.c_char * nbytes).from_address(p.value)
+    buf._owner = _PinnedOwner(L, p.value, device)
+    return torch.frombuffer(buf, dtype=dtype).view(int(rows), d)
+
+
+def _check_device_rows(device_rows) -> Optional[int]:
+    if device_rows is None:
+        return None
+    if isinstance(device_rows, (bool, np.bool_)) or not isinstance(device_rows, (int, np.integer)) or device_rows < 0:
+        raise ValueError(f"device_rows must be None or an integer >= 0, got {device_rows!r}")
+    return int(device_rows)
+
+
 class IndexRefine:
     """faiss.IndexRefineFlat(base) / IndexRefine(base, IndexFlatIP(d)): the base IVF-PQ search returns k * k_factor
     candidates, which are re-scored exactly against a re-rank store of the original vectors (row = index id), and the
@@ -391,18 +427,60 @@ class IndexRefine:
 
     The store is a device tensor [ntotal, d] in float16 or float32.  The embedding task writes fp16 embeddings, so an
     fp16 store of them is lossless; an fp16 store of fp32 vectors rounds them (faiss `Refine(SQfp16)`).
-    Results are sorted by exact score descending, ties by ascending id, padded with (-FLT_MAX, -1)."""
+    Results are sorted by exact score descending, ties by ascending id, padded with (-FLT_MAX, -1).
 
-    def __init__(self, base, store_dtype: str = "float16", k_factor: int = 1):
+    device_rows = n (an integer) makes the store tiered, for stores larger than device memory: rows [0, n) stay in
+    device memory and rows from n on go to page-locked, device-mapped host memory (rsb_search_refine_tiered).  Each
+    search gathers the distinct host rows its candidates need over PCIe, `staging_bytes` of queries' worst case at a
+    time; the results are bit-identical to an all-device store of the same values.  device_rows = None (default)
+    keeps every row on the device."""
+
+    staging_bytes = 512 << 20           # tiered store: device staging buffer for the host rows of a chunk of queries
+
+    def __init__(self, base, store_dtype: str = "float16", k_factor: int = 1, device_rows: Optional[int] = None):
         if not isinstance(base, IndexIVFPQ):
             raise ValueError(f"IndexRefine re-ranks IVF-PQ results; a {type(base).__name__} base already returns exact scores")
         if store_dtype not in _STORE_DTYPES:
             raise ValueError(f"store_dtype must be float16 or float32, got {store_dtype!r}")
         self.base, self.store_dtype = base, store_dtype
         self.k_factor = int(k_factor)
+        self.device_rows = _check_device_rows(device_rows)
         self.L, self.d, self.device = base.L, base.d, base.device
         self._store = torch.empty((0, self.d), dtype=_STORE_DTYPES[store_dtype][0], device=self.device)
+        self._host = torch.empty((0, self.d), dtype=self._store.dtype)      # host tier (tiered store only)
         self._n = 0                                     # rows of the store in use (capacity = self._store.shape[0])
+
+    @property
+    def tiered(self) -> bool:
+        return self.device_rows is not None
+
+    @property
+    def n_dev(self) -> int:
+        """Rows of the store in device memory."""
+        return min(self.device_rows, self._n) if self.tiered else self._n
+
+    @property
+    def device_store(self) -> torch.Tensor:
+        """Rows [0, n_dev) (a device tensor view)."""
+        return self._store[: self.n_dev]
+
+    @property
+    def host_store(self) -> torch.Tensor:
+        """Rows [n_dev, ntotal) of a tiered store (a CPU tensor view over the pinned host tier)."""
+        return self._host[: self._n - self.n_dev]
+
+    def store_rows(self, ids) -> torch.Tensor:
+        """The store rows of the given index ids [n] -> [n, d] device tensor, read from whichever tier holds them."""
+        ids = torch.as_tensor(ids).to(device="cpu", dtype=torch.int64).reshape(-1)
+        if ids.numel() and (int(ids.min()) < 0 or int(ids.max()) >= self._n):
+            raise IndexError(f"store ids must be in [0, {self._n})")
+        if not self.tiered:
+            return self._store[ids.to(self.device)]
+        out = torch.empty((ids.numel(), self.d), dtype=self._store.dtype, device=self.device)
+        on_dev = ids < self.n_dev
+        out[on_dev.to(self.device)] = self._store[ids[on_dev].to(self.device)]
+        out[(~on_dev).to(self.device)] = self._host[ids[~on_dev] - self.n_dev].to(self.device)
+        return out
 
     # -- faiss protocol ------------------------------------------------------------------------------------------
     @property
@@ -424,6 +502,8 @@ class IndexRefine:
     @property
     def store(self) -> torch.Tensor:
         """The re-rank store [ntotal, d] (a view; row i = the vector of index id i)."""
+        if self.tiered:
+            raise ValueError("a tiered store is not one tensor: use device_store, host_store or store_rows")
         return self._store[: self._n]
 
     def train(self, x) -> None:
@@ -440,34 +520,58 @@ class IndexRefine:
         self.add_store(x)
 
     def reserve(self, n: int) -> None:
-        """Allocates store capacity for n rows, after checking that it fits in free device memory."""
-        if n <= self._store.shape[0]:
-            return
-        need = int(n) * self.d * self._store.element_size()
-        free, _ = torch.cuda.mem_get_info(self.device)
-        if need > free:
-            raise MemoryError(f"the re-rank store needs {need} bytes ({n} x {self.d} {self.store_dtype}); "
-                              f"{free} bytes are free on {self.device}")
-        grown = torch.empty((int(n), self.d), dtype=self._store.dtype, device=self.device)
-        grown[: self._n].copy_(self._store[: self._n])
-        self._store = grown
+        """Allocates store capacity for n rows, after checking that the device rows fit in free device memory (a tiered
+        store puts rows past device_rows in pinned host memory)."""
+        n_dev = int(n) if not self.tiered else min(int(n), self.device_rows)
+        if n_dev > self._store.shape[0]:
+            need = n_dev * self.d * self._store.element_size()
+            free, _ = torch.cuda.mem_get_info(self.device)
+            if need > free:
+                raise MemoryError(f"the re-rank store needs {need} bytes ({n_dev} x {self.d} {self.store_dtype}); "
+                                  f"{free} bytes are free on {self.device}")
+            grown = torch.empty((n_dev, self.d), dtype=self._store.dtype, device=self.device)
+            grown[: self.n_dev].copy_(self._store[: self.n_dev])
+            self._store = grown
+        n_host = int(n) - n_dev
+        if n_host > self._host.shape[0]:
+            grown = _pinned_rows(self.L, n_host, self.d, self._store.dtype, self.device)
+            used = self._n - self.n_dev
+            torch.cuda.current_stream(self.device).synchronize()    # a search in flight may read the old host tier
+            grown[:used].copy_(self._host[:used])
+            self._host = grown
+
+    def _capacity(self) -> int:
+        return self._store.shape[0] + self._host.shape[0]
 
     def add_store(self, x) -> None:
-        """Appends rows to the store only (for a base that already holds these vectors, e.g. one read from disk)."""
+        """Appends rows to the store only (for a base that already holds these vectors, e.g. one read from disk).
+        Rows bound for the host tier are copied there directly: host input never crosses PCIe for them."""
         if isinstance(x, np.ndarray):
             x = torch.from_numpy(np.ascontiguousarray(x))
         x = torch.as_tensor(x)
         if x.dim() != 2 or x.shape[1] != self.d:
             raise ValueError(f"expected [n, {self.d}] vectors, got {tuple(x.shape)}")
         n = x.shape[0]
-        if self._n + n > self._store.shape[0]:
-            self.reserve(max(self._n + n, int(1.25 * self._store.shape[0])))
-        self._store[self._n: self._n + n].copy_(x.to(device=self.device, dtype=self._store.dtype))
+        if self._n + n > self._capacity():
+            self.reserve(max(self._n + n, int(1.25 * self._capacity())))
+        n_to_dev = n if not self.tiered else max(0, min(n, self.device_rows - self._n))
+        if n_to_dev:
+            self._store[self._n: self._n + n_to_dev].copy_(x[:n_to_dev].to(device=self.device, dtype=self._store.dtype))
+        if n_to_dev < n:
+            h0 = self._n + n_to_dev - self.device_rows
+            torch.cuda.current_stream(self.device).synchronize()    # a search in flight may be reading the host tier
+            self._host[h0: h0 + n - n_to_dev].copy_(x[n_to_dev:].to(dtype=self._store.dtype))
         self._n += n
         torch.cuda.current_stream(self.device).synchronize()     # x may be a temporary
 
-    def search_ids(self, q, k: int, nprobe: Optional[int] = None, k_factor: Optional[int] = None):
-        """q [nq, d] -> (ids int64 [nq,k], scores float32 [nq,k]) CUDA tensors, enqueued on the current stream."""
+    def _tier_args(self):
+        """(device tier, n_dev, host tier pointer) of rsb_*_tiered."""
+        return _ptr(self._store), self.n_dev, _ptr(self.host_store)
+
+    def search_ids(self, q, k: int, nprobe: Optional[int] = None, k_factor: Optional[int] = None,
+                   host_rows: Optional[torch.Tensor] = None):
+        """q [nq, d] -> (ids int64 [nq,k], scores float32 [nq,k]) CUDA tensors, enqueued on the current stream.
+        host_rows (tiered store; a 1-element int64 CUDA tensor) is incremented by the distinct host rows gathered."""
         with torch.cuda.device(self.device):
             q = _dev_f32(q, self.device)
             if q.dim() != 2 or q.shape[1] != self.d:
@@ -478,6 +582,13 @@ class IndexRefine:
             D = torch.empty((nq, k), dtype=torch.float32, device=self.device)
             I = torch.empty((nq, k), dtype=torch.int64, device=self.device)
             if nq == 0:
+                return I, D
+            if self.tiered:
+                sb = int(self.staging_bytes)
+                ws = self.base._workspace(self.L.rsb_search_refine_tiered_workspace_bytes(self.base._h, nq, k, kf, npb, sb))
+                _lib.check(self.L.rsb_search_refine_tiered(
+                    self.base._h, _ptr(q), nq, k, kf, npb, *self._tier_args(), _STORE_DTYPES[self.store_dtype][1],
+                    self._n, _ptr(D), _ptr(I), _ptr(ws), ws.numel(), sb, _ptr(host_rows), _stream()))
                 return I, D
             ws = self.base._workspace(self.L.rsb_search_refine_workspace_bytes(self.base._h, nq, k, kf, npb))
             _lib.check(self.L.rsb_search_refine(self.base._h, _ptr(q), nq, k, kf, npb, _ptr(self._store),
@@ -492,14 +603,24 @@ class IndexRefine:
             return D.cpu().numpy(), I.cpu().numpy()
         return D, I
 
-    def rerank(self, q: torch.Tensor, cand: torch.Tensor, k: int):
-        """The re-rank step alone (rsb_refine): candidates cand [nq, k_base] int64 (-1 = none) -> (ids, scores) [nq, k]."""
+    def rerank(self, q: torch.Tensor, cand: torch.Tensor, k: int, staging_bytes: Optional[int] = None,
+               host_rows: Optional[torch.Tensor] = None):
+        """The re-rank step alone (rsb_refine / rsb_refine_tiered): candidates cand [nq, k_base] int64 (-1 = none) ->
+        (ids, scores) [nq, k].  staging_bytes and host_rows apply to a tiered store (see search_ids)."""
         with torch.cuda.device(self.device):
             q = _dev_f32(q, self.device)
             cand = cand.to(device=self.device, dtype=torch.int64).contiguous()
             nq, k_base = cand.shape
             D = torch.empty((nq, int(k)), dtype=torch.float32, device=self.device)
             I = torch.empty((nq, int(k)), dtype=torch.int64, device=self.device)
+            if self.tiered:
+                sb = int(self.staging_bytes if staging_bytes is None else staging_bytes)
+                dt = _STORE_DTYPES[self.store_dtype][1]
+                ws = self.base._workspace(self.L.rsb_refine_tiered_workspace_bytes(nq, k_base, int(k), self.d, dt, sb))
+                _lib.check(self.L.rsb_refine_tiered(_ptr(q), nq, *self._tier_args(), dt, self.d, self._n, _ptr(cand),
+                                                    k_base, int(k), _ptr(D), _ptr(I), _ptr(ws), ws.numel(), sb,
+                                                    _ptr(host_rows), _stream()))
+                return I, D
             ws = self.base._workspace(self.L.rsb_refine_workspace_bytes(nq, k_base, int(k)))
             _lib.check(self.L.rsb_refine(_ptr(q), nq, _ptr(self._store), _STORE_DTYPES[self.store_dtype][1], self.d,
                                          self._n, _ptr(cand), k_base, int(k), _ptr(D), _ptr(I), _ptr(ws), ws.numel(),
@@ -522,8 +643,9 @@ MAGIC = "RSB1"
 def _to_faiss_parts(index: _IndexBase) -> dict:
     if isinstance(index, IndexRefine):
         # faiss IndexRefineFlat: an fp16 store is written upcast to fp32 (exact)
+        xb = torch.cat([index.device_store.float().cpu(), index.host_store.float()]) if index.tiered else index.store.float().cpu()
         return {"kind": "Refine", "d": index.d, "ntotal": index.ntotal, "base": _to_faiss_parts(index.base),
-                "xb": index.store.float().cpu().numpy(), "k_factor": float(index.k_factor)}
+                "xb": xb.numpy(), "k_factor": float(index.k_factor)}
     off, payload, ids = index.export_lists()
     off, payload, ids = off.cpu().numpy(), payload.cpu().numpy(), ids.cpu().numpy()
     # fp16 storage is written upcast to fp32 (exact): the file is the one the fp32 index of the same values writes

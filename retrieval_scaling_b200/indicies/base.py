@@ -43,7 +43,21 @@ class Indexer(object):
                              f"are already exact")
         if dtype not in (None, "float16", "float32"):
             raise ValueError(f"datastore.index.refine_dtype must be float16 or float32, got {dtype!r}")
+        Indexer.refine_device_rows(index_cfg)
         return k_factor, dtype
+
+    @staticmethod
+    def refine_device_rows(index_cfg):
+        """Optional key `refine_device_rows` (absent: None, every store row in device memory): an integer >= 0; store rows
+        from that id on are kept in pinned host memory (index.IndexRefine(device_rows=...)).  Needs refine_k_factor > 0."""
+        rows = index_cfg.get("refine_device_rows", None)
+        if rows is None:
+            return None
+        if isinstance(rows, bool) or not isinstance(rows, int) or rows < 0:
+            raise ValueError(f"datastore.index.refine_device_rows must be an integer >= 0, got {rows!r}")
+        if not int(index_cfg.get("refine_k_factor", 0) or 0) > 0:
+            raise ValueError("datastore.index.refine_device_rows splits the re-rank store: it needs refine_k_factor > 0")
+        return rows
 
     @staticmethod
     def storage_dtype(index_cfg):
@@ -90,7 +104,8 @@ class Indexer(object):
             self.datastore = IVFPQIndexer(trained_index_path=index_path + ".trained", sample_train_size=a.sample_train_size,
                                           prev_index_path=None, ncentroids=a.ncentroids, probe=a.probe,
                                           n_subquantizers=a.n_subquantizers, code_size=a.n_bits,
-                                          refine_k_factor=k_factor, refine_dtype=refine_dtype, **common)
+                                          refine_k_factor=k_factor, refine_dtype=refine_dtype,
+                                          refine_device_rows=self.refine_device_rows(a), **common)
         else:
             raise NotImplementedError
 

@@ -4,7 +4,8 @@ METRIC_INNER_PRODUCT); note the reference passes `n_bits` as `code_size` = bits 
 
 With `refine_k_factor` > 0 the search re-ranks k * refine_k_factor IVF-PQ candidates exactly against the passage
 embeddings (index.IndexRefine; the reference's unused `get_knn_scores` path, `ivf_pq.py:119-123`).  The store is
-built from the embedding pickles on the GPU; the `.faiss` file stays the plain IVF-PQ index."""
+built from the embedding pickles on the GPU, or, with `refine_device_rows`, split between device memory (rows below it)
+and pinned host memory (the rest); the `.faiss` file stays the plain IVF-PQ index."""
 from __future__ import annotations
 
 import numpy as np
@@ -20,7 +21,8 @@ class IVFPQIndexer(BaseIndexer):
     def __init__(self, embed_paths, index_path, meta_file, trained_index_path, passage_dir=None,
                  pos_map_save_path=None, sample_train_size=1000000, prev_index_path=None, dimension=768,
                  dtype=None, ncentroids=4096, probe=2048, num_keys_to_add_at_a_time=1000000,
-                 DSTORE_SIZE_BATCH=51200000, n_subquantizers=16, code_size=8, refine_k_factor=0, refine_dtype=None):
+                 DSTORE_SIZE_BATCH=51200000, n_subquantizers=16, code_size=8, refine_k_factor=0, refine_dtype=None,
+                 refine_device_rows=None):
         self.ncentroids = int(ncentroids)
         self.n_subquantizers, self.code_size = int(n_subquantizers), int(code_size)
         self.prev_index_path = prev_index_path
@@ -28,14 +30,15 @@ class IVFPQIndexer(BaseIndexer):
                          trained_index_path=prev_index_path or trained_index_path,
                          sample_train_size=sample_train_size, probe=probe)
         if refine_k_factor:
-            self.index = self._build_refine(int(refine_k_factor), refine_dtype)
+            self.index = self._build_refine(int(refine_k_factor), refine_dtype, refine_device_rows)
 
     def _new_index(self):
         return rsb_index.IndexIVFPQ(self.dimension, self.ncentroids, self.n_subquantizers, self.code_size)
 
-    def _build_refine(self, k_factor: int, refine_dtype):
+    def _build_refine(self, k_factor: int, refine_dtype, device_rows=None):
         """Re-rank store from the embedding pickles in the order `_add_keys` added them (the `.meta` order, so row =
-        index id), uploaded one shard at a time."""
+        index id), copied one shard at a time: rows below device_rows (None: all) are uploaded, the rest are copied
+        into the pinned host tier without crossing PCIe."""
         base, meta = self.index, self.index_id_to_db_id
         if len(meta) != base.ntotal:
             raise ValueError(f"{self.meta_file} maps {len(meta)} ids but the index holds {base.ntotal} vectors")
@@ -50,7 +53,7 @@ class IVFPQIndexer(BaseIndexer):
                                  f"must follow the index's id order")
             if refine is None:
                 dtype = refine_dtype or ("float16" if emb.dtype == np.float16 else "float32")
-                refine = rsb_index.IndexRefine(base, store_dtype=dtype, k_factor=k_factor)
+                refine = rsb_index.IndexRefine(base, store_dtype=dtype, k_factor=k_factor, device_rows=device_rows)
                 refine.reserve(base.ntotal)                 # MemoryError (with the byte count) before any upload
             refine.add_store(emb)
             row += n

@@ -15,7 +15,21 @@ written it.  Reported:
     on the same candidates, every returned pair re-scored in float64 from the store;
   * the card's name and power limit.
 The fp16 store (n x d x 2 bytes: 154 GB at 100M) must fit in device memory next to the index; sizes that do not are
-refused before anything is built."""
+refused before anything is built.
+
+    python scripts/bench_refine.py --n 20000000 --device-rows 0 [--staging-gb 1] [--compare-device]
+
+--device-rows R makes the store tiered (rows [0, R) in device memory, the rest in pinned host memory) and reports, at
+every --tiered-nq batch size (k = --k, k_factor = --k-factor):
+  * refined and unrefined QPS, and the re-rank alone;
+  * the re-rank's sort / gather / score milliseconds (CUDA events per query chunk, rsb_refine_tiered_profile);
+  * distinct host rows gathered per re-rank and their fraction of the host-tier candidates; gathered GB/s against a
+    plain pinned -> device cudaMemcpy measured in the same run (the achievable PCIe reference);
+  * with R = 0, the zero-copy baseline: the all-device kernel (rsb_refine) handed the mapped host pointer directly;
+  * with --compare-device, the all-device store in the same run: byte-identical results required;
+  * recall@k refined and unrefined and the parity block, at the largest batch;
+  * the card's name and power limit, the PCIe link generation and width, the host's MemAvailable.
+The host tier is capped at half of MemAvailable (larger sizes are refused before anything is built) and freed at exit."""
 import argparse
 import json
 import os
@@ -47,6 +61,10 @@ def parse():
     ap.add_argument("--train-per-centroid", type=int, default=64)
     ap.add_argument("--recall-queries", type=int, default=1000)
     ap.add_argument("--parity-queries", type=int, default=256)
+    ap.add_argument("--device-rows", type=int, default=None, help="tiered store: rows kept in device memory")
+    ap.add_argument("--staging-gb", type=float, default=1.0, help="tiered store: staging buffer (GiB)")
+    ap.add_argument("--tiered-nq", default="1,64,10000", help="tiered store: batch sizes to report")
+    ap.add_argument("--compare-device", action="store_true", help="tiered store: also build the all-device store")
     a = ap.parse_args()
     a.partition = "list"
     return a
@@ -86,7 +104,7 @@ def parity(ref, xq, Ib, Ir, Dr, k, npq):
     from oracle import refine_oracle as R
     kb = Ib.shape[1]
     Ib_h = Ib[:npq].cpu().numpy()
-    rows = ref.store[Ib[:npq].clamp_min(0)].cpu().numpy()                          # [npq, k', d] fp16
+    rows = ref.store_rows(Ib[:npq].clamp_min(0).reshape(-1)).reshape(npq, kb, -1).cpu().numpy()   # [npq, k', d] fp16
     xq_h = xq[:npq].cpu().numpy()
     Dref = np.full((npq, k), np.finfo(np.float32).min, np.float32)
     Iref = np.full((npq, k), -1, np.int64)
@@ -109,12 +127,177 @@ def parity(ref, xq, Ib, Ir, Dr, k, npq):
     return par
 
 
+def host_identity(device) -> dict:
+    """PCIe link (read-only nvidia-smi query) and the host's MemAvailable."""
+    out = {"host_mem_available_bytes": mem_available()}
+    for key, field in (("pcie_link_gen", "pcie.link.gen.current"), ("pcie_link_width", "pcie.link.width.current"),
+                       ("pcie_link_gen_max", "pcie.link.gen.max"), ("pcie_link_width_max", "pcie.link.width.max")):
+        out[key] = None
+        try:
+            r = subprocess.run(["nvidia-smi", f"--id={device.index or 0}", f"--query-gpu={field}",
+                                "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=20)
+            v = (r.stdout.strip() or r.stderr.strip()).splitlines()[0].strip()
+            out[key] = int(v) if v.isdigit() else v
+        except Exception:
+            pass
+    return out
+
+
+def mem_available() -> int:
+    with open("/proc/meminfo") as f:
+        for line in f:
+            if line.startswith("MemAvailable:"):
+                return int(line.split()[1]) * 1024
+    raise SystemExit("MemAvailable not found in /proc/meminfo")
+
+
+def pinned_copy_gbs(device, nbytes=1 << 30, reps=10) -> float:
+    """Plain pinned host -> device copy bandwidth (cudaMemcpyAsync of a page-locked buffer): the PCIe reference."""
+    from retrieval_scaling_b200 import _lib
+    from retrieval_scaling_b200.index import _pinned_rows
+    src = _pinned_rows(_lib.lib(), nbytes // 16, 16, torch.uint8, device)
+    dst = torch.empty_like(src, device=device)
+    dst.copy_(src, non_blocking=True)
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(reps):
+        dst.copy_(src, non_blocking=True)
+    e1.record()
+    torch.cuda.synchronize()
+    return nbytes * reps / (e0.elapsed_time(e1) / 1e3) / 1e9
+
+
+def tiered_profile(L, enable):
+    import ctypes
+    ms = (ctypes.c_double * 3)()
+    from retrieval_scaling_b200 import _lib
+    _lib.check(L.rsb_refine_tiered_profile(int(enable), ms))
+    return list(ms)
+
+
+def zero_copy_rerank(ref, q, Ib, k):
+    """The all-device kernel (rsb_refine) handed the mapped host tier directly (n_dev = 0): every candidate row crosses
+    PCIe once per query, no de-duplication, no staging."""
+    from retrieval_scaling_b200 import _lib
+    from retrieval_scaling_b200.index import _ptr, _stream
+    nq, kb = Ib.shape
+    D = torch.empty((nq, k), dtype=torch.float32, device=ref.device)
+    I = torch.empty((nq, k), dtype=torch.int64, device=ref.device)
+    ws = ref.base._workspace(ref.L.rsb_refine_workspace_bytes(nq, kb, k))
+    _lib.check(ref.L.rsb_refine(_ptr(q), nq, _ptr(ref.host_store), _lib.RSB_DTYPE_F16, ref.d, ref.ntotal, _ptr(Ib), kb, k,
+                                _ptr(D), _ptr(I), _ptr(ws), ws.numel(), _stream()))
+    return I, D
+
+
+def tiered_main(args, device):
+    import retrieval_scaling_b200 as rsb
+    from retrieval_scaling_b200 import synth
+    k, kf = args.k, args.k_factor
+    kb = k * kf
+    n_dev = min(args.device_rows, args.n)
+    host_bytes = (args.n - n_dev) * args.d * 2
+    avail = mem_available()
+    if host_bytes > avail // 2:
+        raise SystemExit(f"the host tier of {args.n - n_dev} x {args.d} fp16 needs {host_bytes} bytes of pinned memory; "
+                         f"the cap is half of MemAvailable = {avail // 2} bytes: use a larger --device-rows or a smaller --n")
+    free, _ = torch.cuda.mem_get_info(device)
+    dev_bytes = n_dev * args.d * 2 + (store_bytes(args) if args.compare_device else 0)
+    # + the corpus generator's fp32 chunk and its temporary while the store is filled
+    need = dev_bytes + args.n * (args.m + 8) + int(args.staging_gb * (1 << 30)) + 2 * B.CHUNK_ROWS * args.d * 4
+    if need > 0.9 * free:
+        raise SystemExit(f"the device tier, the index and the staging buffer need ~{need} bytes, {free} are free on "
+                         f"{device}: use a smaller --device-rows or drop --compare-device")
+    info = {**gpu_identity(device), **host_identity(device), "pinned_to_device_memcpy_gbs": pinned_copy_gbs(device)}
+    probe = synth.Corpus(d=args.d, mode="gmm", n_centres=max(16, args.nlist // 4), device=device)
+    xq_all = probe.queries(args.nq)
+    del probe
+    n_gt = min(args.recall_queries, args.nq)
+    index, corpus, _, gt_I, build = B.build_index(args, 0, 1, device, gt_queries=xq_all[:n_gt].contiguous())
+
+    t0 = time.time()
+    stores = {"tiered": rsb.IndexRefine(index, "float16", kf, device_rows=n_dev)}
+    if args.compare_device:
+        stores["device"] = rsb.IndexRefine(index, "float16", kf)
+    for ref in stores.values():
+        ref.staging_bytes = int(args.staging_gb * (1 << 30))
+        ref.reserve(args.n)
+    for c in range((args.n + B.CHUNK_ROWS - 1) // B.CHUNK_ROWS):
+        x = corpus.chunk(c, B.CHUNK_ROWS)[: min(B.CHUNK_ROWS, args.n - c * B.CHUNK_ROWS)]
+        for ref in stores.values():
+            ref.add_store(x)
+    store_s = time.time() - t0
+    ref = stores["tiered"]
+    L = ref.L
+
+    per_nq = []
+    for nq in [int(v) for v in args.tiered_nq.split(",")]:
+        nq = min(nq, args.nq)
+        xq = xq_all[:nq].contiguous()
+        ms_unref, (Iu, _) = timed(lambda: index.search_ids(xq, k), args.steps, args.warmup)
+        ms_ref, (I, D) = timed(lambda: ref.search_ids(xq, k), args.steps, args.warmup)
+        Ib, _ = index.search_ids(xq, kb)
+        ms_rerank, (Ir, Dr) = timed(lambda: ref.rerank(xq, Ib, k), args.steps, args.warmup)
+        rows = torch.zeros(1, dtype=torch.int64, device=device)
+        tiered_profile(L, 1)
+        for _ in range(args.steps):
+            ref.rerank(xq, Ib, k, host_rows=rows)
+        split = [v / args.steps for v in tiered_profile(L, 0)]
+        uniq = int(rows.item()) / args.steps
+        host_cand = int(((Ib >= n_dev) & (Ib < args.n)).sum().item())
+        row = {"nq": nq, "qps_refined": nq / (ms_ref / 1e3), "qps_unrefined": nq / (ms_unref / 1e3),
+               "ms_per_step_refined": ms_ref, "ms_per_step_unrefined": ms_unref, "rerank_ms": ms_rerank,
+               "sort_ms": split[0], "gather_ms": split[1], "score_ms": split[2],
+               "host_tier_candidates": host_cand, "unique_host_rows": uniq,
+               "unique_frac_of_host_candidates": uniq / host_cand if host_cand else None,
+               "gathered_bytes": uniq * args.d * 2,
+               "gathered_gbs": uniq * args.d * 2 / (split[1] / 1e3) / 1e9 if split[1] > 0 else None}
+        row["gathered_frac_of_memcpy"] = (row["gathered_gbs"] / info["pinned_to_device_memcpy_gbs"]
+                                          if row["gathered_gbs"] else None)
+        row["same_result_as_two_stage"] = bool(torch.equal(I, Ir) and torch.equal(D, Dr))
+        if n_dev == 0:
+            ms_zc, (Iz, Dz) = timed(lambda: zero_copy_rerank(ref, xq, Ib, k), args.steps, args.warmup)
+            row["zero_copy_rerank_ms"] = ms_zc
+            row["zero_copy_same_result"] = bool(torch.equal(Iz, Ir) and torch.equal(Dz, Dr))
+        else:
+            row["zero_copy_rerank_ms"] = "not measured (needs --device-rows 0: rsb_refine reads one contiguous store)"
+        if "device" in stores:
+            full = stores["device"]
+            ms_dev, (Id, Dd) = timed(lambda: full.search_ids(xq, k), args.steps, args.warmup)
+            ms_dev_rr, (Idr, Ddr) = timed(lambda: full.rerank(xq, Ib, k), args.steps, args.warmup)
+            row.update({"device_store_qps_refined": nq / (ms_dev / 1e3), "device_store_rerank_ms": ms_dev_rr,
+                        "identical_to_device_store": bool(torch.equal(I, Id) and torch.equal(D, Dd)
+                                                          and torch.equal(Ir, Idr) and torch.equal(Dr, Ddr))})
+        per_nq.append(row)
+        last = (xq, I, Iu, Ib, Ir, Dr, nq)
+
+    xq, I, Iu, Ib, Ir, Dr, nq = last
+    strip = lambda r: {kk: vv for kk, vv in r.items() if kk != "ground_truth"}   # noqa: E731
+    ng = min(n_gt, nq)
+    out = {"metric": f"exact re-ranking of k x {kf} candidates from a tiered fp16 store ({n_dev} device rows, "
+                     f"{args.n - n_dev} pinned host rows), {args.n // 1_000_000}M x {args.d} IVF-PQ",
+           "config": {**B.make_config(args, 1), "k_factor": kf, "k_base": kb, "device_rows": n_dev,
+                      "host_rows": args.n - n_dev, "staging_bytes": ref.staging_bytes},
+           "per_nq": per_nq, **info,
+           "store": {"dtype": "float16", "device_bytes": n_dev * args.d * 2, "host_bytes": host_bytes, "build_s": store_s},
+           "recall_nq": ng, "recall": strip(B.recall_block(I[:ng], gt_I[:ng], k)),
+           "recall_unrefined": strip(B.recall_block(Iu[:ng], gt_I[:ng], k)),
+           "recall_ground_truth": "bench.py's exact fp32 inner-product search over the same corpus",
+           "parity": parity(ref, xq, Ib, Ir, Dr, k, min(args.parity_queries, nq)),
+           "build": build, "steps": args.steps, "warmup": args.warmup}
+    del stores, ref
+    print(json.dumps(out), flush=True)
+    return 0
+
+
 def main():
     args = parse()
     if not torch.cuda.is_available():
         raise SystemExit("bench_refine.py needs a CUDA device: the product path has no CPU fallback")
     device = torch.device("cuda", 0)
     torch.cuda.set_device(device)
+    if args.device_rows is not None:
+        return tiered_main(args, device)
     need = store_bytes(args) + args.n * (args.m + 8)                   # store + PQ codes + ids
     free, _ = torch.cuda.mem_get_info(device)
     if need > 0.9 * free:
