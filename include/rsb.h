@@ -170,7 +170,7 @@ int rsb_coarse(rsb_index_t* h, const float* q_dev, int nq, int nprobe, int64_t* 
  * order for both types (an fp16 store and an fp32 store of the same fp16-representable values agree bit for bit).  Rows are sorted by score descending, ties by ascending id; fewer than k valid candidates are
  * padded with id -1 / score -FLT_MAX; candidate ids -1 (and ids outside [0, ntotal)) are skipped.
  * k_base = k * k_factor <= 4096 (the scan's k limit); larger returns RSB_ERR_UNSUPPORTED.  ntotal <= 2^31. */
-enum { RSB_DTYPE_F32 = 0, RSB_DTYPE_F16 = 1 };
+enum { RSB_DTYPE_F32 = 0, RSB_DTYPE_F16 = 1, RSB_DTYPE_SQ8 = 2 /* re-rank store only: rsb_refine_sq8 below */ };
 size_t rsb_refine_workspace_bytes(int nq, int k_base, int k);
 /* re-rank given candidates cand_dev [nq, k_base] int64 (e.g. a search result at k_base) -> D_dev/I_dev [nq, k] */
 int rsb_refine(const float* q_dev, int nq, const void* store_dev, int store_dtype, int d, int64_t ntotal,
@@ -212,6 +212,37 @@ int rsb_search_refine_tiered(rsb_index_t* h, const float* q_dev, int nq, int k, 
  * current at the call (this waits for each chunk on the host: for measurement only).  ms_out (may be NULL) receives
  * the [3] milliseconds accumulated since the previous call, which resets them. */
 int rsb_refine_tiered_profile(int enable, double* ms_out);
+
+/* ---- SQ8 re-rank store: faiss IndexRefine(base, IndexScalarQuantizer(d, QT_8bit)), factory string "...,Refine(SQ8)" --
+ *      (the same re-score path, src/indicies/ivf_pq.py:119-123 `get_knn_scores`, from one byte per element)
+ * Scalar quantizer QT_8bit, RS_minmax, one range per dimension; sq_dev is [2, d] float32: vmin [d], then vdiff [d]
+ * (faiss' `sq.trained` layout).  Every operation below is a separately rounded fp32 operation:
+ *   train   vmin[j] = min over the rows of x[:, j], vdiff[j] = max - vmin[j]
+ *   encode  xi = vdiff != 0 ? (x - vmin) / vdiff : 0, clamped to [0, 1]; code = (int)(255.f * xi)  (rows outside the
+ *           trained range clamp; fp16 input is encoded from its exact fp32 value)
+ *   decode  x = vmin + ((code + 0.5f) / 255.f) * vdiff
+ * The re-rank decodes every element and scores it as the fp32 store does (same lane order, same fmaf sequence), so ids
+ * and scores are bit-identical to rsb_refine / rsb_search_refine on an fp32 store holding the decoded rows.
+ * x_dev [n, d] in x_dtype (RSB_DTYPE_F32 / RSB_DTYPE_F16); codes_dev [n, d] uint8.  rsb_sq8_train needs n >= 1. */
+int rsb_sq8_train(const void* x_dev, int x_dtype, int64_t n, int d, float* sq_dev, rsb_stream_t stream);
+int rsb_sq8_encode(const void* x_dev, int x_dtype, int64_t n, int d, const float* sq_dev, uint8_t* codes_dev,
+                   rsb_stream_t stream);
+/* rsb_refine_tiered / rsb_search_refine_tiered for an SQ8 store of codes: the store dtype is implied and sq_dev
+ * (16-byte aligned) takes its place.  n_dev = ntotal is the all-device store (store_host unused); n_dev < ntotal keeps
+ * rows [n_dev, ntotal) in mapped page-locked host memory, gathered as above at d bytes per row.  d % 16 == 0 (whole
+ * 16-byte rows), else RSB_ERR_INVALID.  rsb_refine / rsb_search_refine / rsb_refine_tiered / rsb_search_refine_tiered
+ * refuse RSB_DTYPE_SQ8 with RSB_ERR_INVALID: they have no trained range. */
+size_t rsb_refine_sq8_workspace_bytes(int nq, int k_base, int k, int d, size_t staging_bytes);
+int rsb_refine_sq8(const float* q_dev, int nq, const void* store_dev, int64_t n_dev, const void* store_host,
+                   const float* sq_dev, int d, int64_t ntotal, const int64_t* cand_dev, int k_base, int k, float* D_dev,
+                   int64_t* I_dev, void* ws_dev, size_t ws_bytes, size_t staging_bytes, int64_t* host_rows_dev,
+                   rsb_stream_t stream);
+size_t rsb_search_refine_sq8_workspace_bytes(rsb_index_t* h, int nq, int k, int k_factor, int nprobe,
+                                             size_t staging_bytes);
+int rsb_search_refine_sq8(rsb_index_t* h, const float* q_dev, int nq, int k, int k_factor, int nprobe,
+                          const void* store_dev, int64_t n_dev, const void* store_host, const float* sq_dev,
+                          int64_t ntotal, float* D_dev, int64_t* I_dev, void* ws_dev, size_t ws_bytes,
+                          size_t staging_bytes, int64_t* host_rows_dev, rsb_stream_t stream);
 
 /* ---- shard merge (src/search.py:357-367; api/serve_main_node.py:130-163) ---------------------------- */
 /* D_all_dev/I_all_dev [nshards, nq, k]: concat per query, sort by score desc (ties: lower shard, then lower

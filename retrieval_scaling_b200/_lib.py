@@ -13,7 +13,7 @@ LIB_PATH = os.environ.get("RSB_LIBRARY") or os.path.join(_HERE, "librsb.so")
 RSB_OK = 0
 RSB_ERR_INVALID, RSB_ERR_CUDA, RSB_ERR_STATE, RSB_ERR_UNSUPPORTED, RSB_ERR_OOM = -1, -2, -3, -4, -5
 RSB_FLAT, RSB_IVFFLAT, RSB_IVFPQ = 0, 1, 2
-RSB_DTYPE_F32, RSB_DTYPE_F16 = 0, 1
+RSB_DTYPE_F32, RSB_DTYPE_F16, RSB_DTYPE_SQ8 = 0, 1, 2
 (INFO_KIND, INFO_D, INFO_NLIST, INFO_M, INFO_NBITS, INFO_NTOTAL, INFO_IS_TRAINED, INFO_MAX_LIST_LEN,
  INFO_INDEX_BYTES, INFO_DTYPE) = range(10)
 PROF_NAMES = ("coarse_ms", "setup_ms", "lut_ms", "scan_ms", "merge_ms", "scan_bytes", "pairs", "launches", "scan_path",
@@ -70,6 +70,14 @@ SIGNATURES = [
     ("rsb_search_refine_tiered", c_int, [_H, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_int,
                                          c_int64, c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_void_p, c_void_p]),
     ("rsb_refine_tiered_profile", c_int, [c_int, POINTER(c_double)]),
+    ("rsb_sq8_train", c_int, [c_void_p, c_int, c_int64, c_int, c_void_p, c_void_p]),
+    ("rsb_sq8_encode", c_int, [c_void_p, c_int, c_int64, c_int, c_void_p, c_void_p, c_void_p]),
+    ("rsb_refine_sq8_workspace_bytes", c_size_t, [c_int, c_int, c_int, c_int, c_size_t]),
+    ("rsb_refine_sq8", c_int, [c_void_p, c_int, c_void_p, c_int64, c_void_p, c_void_p, c_int, c_int64, c_void_p, c_int,
+                               c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_void_p, c_void_p]),
+    ("rsb_search_refine_sq8_workspace_bytes", c_size_t, [_H, c_int, c_int, c_int, c_int, c_size_t]),
+    ("rsb_search_refine_sq8", c_int, [_H, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p,
+                                      c_int64, c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_void_p, c_void_p]),
     ("rsb_merge_topk", c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     ("rsb_merge_topk_peers", c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     ("rsb_merge_topk_peers_scatter", c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,

@@ -1061,24 +1061,35 @@ extern "C" int rsb_search_preassigned_shared(rsb_index_t* h, const float* q, int
 }
 
 // ---- exact re-ranking (faiss IndexRefine::search) -----------------------------------------------------------
-// store_rows: rows behind `store` (-1: all ntotal); a tiered store's device tier holds n_dev of them
-static int refine_check(const void* store, int store_dtype, int d, int64_t ntotal, int k_base, int k, int64_t store_rows = -1) {
-    if (store_dtype != RSB_DTYPE_F32 && store_dtype != RSB_DTYPE_F16)
+static int store_elem_bytes(int store_dtype) { return store_dtype == RSB_DTYPE_SQ8 ? 1 : store_dtype == RSB_DTYPE_F16 ? 2 : 4; }
+
+// store_rows: rows behind `store` (-1: all ntotal); a tiered store's device tier holds n_dev of them.
+// store_dtype RSB_DTYPE_SQ8 is accepted only from the SQ8 entry points (sq8 = true), which carry the trained range.
+static int refine_check(const void* store, int store_dtype, int d, int64_t ntotal, int k_base, int k, int64_t store_rows = -1,
+                        bool sq8 = false) {
+    if (store_dtype == RSB_DTYPE_SQ8 && !sq8)
+        return fail(RSB_ERR_INVALID, "an RSB_DTYPE_SQ8 store is decoded with its trained range: use rsb_refine_sq8 / "
+                                     "rsb_search_refine_sq8");
+    if (store_dtype != RSB_DTYPE_F32 && store_dtype != RSB_DTYPE_F16 && !sq8)
         return fail(RSB_ERR_INVALID, "store_dtype must be RSB_DTYPE_F32 or RSB_DTYPE_F16, got %d", store_dtype);
     if (k <= 0 || k_base < k) return fail(RSB_ERR_INVALID, "need 0 < k <= k_base, got k = %d, k_base = %d", k, k_base);
     if (k_base > 4096) return fail(RSB_ERR_UNSUPPORTED, "k_base = k * k_factor = %d > 4096 is not supported", k_base);
     if (ntotal < 0 || ntotal > ((int64_t)1 << 31)) return fail(RSB_ERR_INVALID, "store rows must be in [0, 2^31], got %lld", (long long)ntotal);
     if (d <= 0 || d % 8) return fail(RSB_ERR_INVALID, "d = %d must be a positive multiple of 8 for the re-rank store", d);
+    if (sq8 && d % 16) return fail(RSB_ERR_INVALID, "d = %d must be a multiple of 16 for an SQ8 store (whole 16-byte rows)", d);
     if ((store_rows < 0 ? ntotal : store_rows) > 0 && (!store || (reinterpret_cast<uintptr_t>(store) & 15)))
         return fail(RSB_ERR_INVALID, "the re-rank store must be a 16-byte aligned device pointer");
     return RSB_OK;
 }
 
+// sq: the SQ8 store's [2, d] (vmin, vdiff); null for fp16 / fp32
 static int refine_impl(const float* q, int nq, const void* store, int store_dtype, int d, int64_t ntotal, const int64_t* cand,
-                       int k_base, int k, float* D, int64_t* I, void* ws, size_t ws_bytes, cudaStream_t st) {
+                       int k_base, int k, float* D, int64_t* I, void* ws, size_t ws_bytes, cudaStream_t st,
+                       const float* sq = nullptr) {
     const RefinePlan p = refine_plan(nq, k_base, k);
     if (ws_bytes < p.ws_bytes) return fail(RSB_ERR_OOM, "workspace too small: need %zu bytes, got %zu", p.ws_bytes, ws_bytes);
-    if (launch_refine_rows(p, q, nq, store, store_dtype == RSB_DTYPE_F16 ? 2 : 4, d, ntotal, cand, k_base, k, D, I, ws, st) != 0)
+    if (launch_refine_rows(p, q, nq, store, store_elem_bytes(store_dtype), d, ntotal, cand, k_base, k, D, I, ws, st,
+                           nullptr, sq) != 0)
         return fail(RSB_ERR_UNSUPPORTED, "d = %d with k_base = %d needs more shared memory than the re-rank kernel has", d, k_base);
     CHECK_LAUNCH();
     return RSB_OK;
@@ -1168,16 +1179,22 @@ extern "C" int rsb_host_free(void* p) {
 
 // Argument checks that need no CUDA call.
 static int tiered_check(const void* store_dev, int64_t n_dev, const void* store_host, int store_dtype, int d,
-                        int64_t ntotal, int k_base, int k, size_t staging_bytes) {
+                        int64_t ntotal, int k_base, int k, size_t staging_bytes, bool sq8 = false) {
     if (n_dev < 0 || n_dev > ntotal)
         return fail(RSB_ERR_INVALID, "n_dev = %lld must be in [0, ntotal = %lld]", (long long)n_dev, (long long)ntotal);
-    RSB_TRY(refine_check(store_dev, store_dtype, d, ntotal, k_base, k, n_dev));
-    const size_t per_q = (size_t)k_base * d * (store_dtype == RSB_DTYPE_F16 ? 2 : 4);
+    RSB_TRY(refine_check(store_dev, store_dtype, d, ntotal, k_base, k, n_dev, sq8));
+    const size_t per_q = (size_t)k_base * d * store_elem_bytes(store_dtype);
     if (staging_bytes < per_q)
         return fail(RSB_ERR_INVALID, "staging_bytes = %zu is below one query's worst case (k_base * d * elem = %zu)",
                     staging_bytes, per_q);
     if (n_dev < ntotal && (!store_host || (reinterpret_cast<uintptr_t>(store_host) & 15)))
         return fail(RSB_ERR_INVALID, "the host tier must be a 16-byte aligned page-locked host pointer");
+    return RSB_OK;
+}
+
+static int sq_check(const float* sq) {
+    if (!sq || (reinterpret_cast<uintptr_t>(sq) & 15))
+        return fail(RSB_ERR_INVALID, "the SQ8 range sq_dev [2, d] must be a 16-byte aligned device pointer");
     return RSB_OK;
 }
 
@@ -1204,8 +1221,12 @@ static int host_tier_alias(const void* first, size_t bytes, const void** alias) 
 }
 
 // Both the workspace query and the call size the workspace for the larger of the fp16 and fp32 plans, so one query
-// serves either store dtype.
-static size_t tiered_ws(int nq, int k_base, int k, int d, size_t staging_bytes) {
+// serves either store dtype.  sq8: the SQ8 plan (1-byte elements) alone, for the SQ8 entry points.
+static size_t tiered_ws(int nq, int k_base, int k, int d, size_t staging_bytes, bool sq8 = false) {
+    if (sq8) {
+        const TieredPlan p = tiered_plan(nq, k_base, k, d, 1, staging_bytes);
+        return p.qc ? p.total : 0;
+    }
     const TieredPlan a = tiered_plan(nq, k_base, k, d, 2, staging_bytes), b = tiered_plan(nq, k_base, k, d, 4, staging_bytes);
     return std::max(a.qc ? a.total : 0, b.qc ? b.total : 0);
 }
@@ -1214,16 +1235,16 @@ static size_t tiered_ws(int nq, int k_base, int k, int d, size_t staging_bytes) 
 static int refine_tiered_impl(const float* q, int nq, const void* store_dev, int64_t n_dev, const void* host_alias,
                               int store_dtype, int d, int64_t ntotal, const int64_t* cand, int k_base, int k, float* D,
                               int64_t* I, void* ws, size_t ws_bytes, size_t staging_bytes, int64_t* host_rows,
-                              cudaStream_t st) {
-    const int eb = store_dtype == RSB_DTYPE_F16 ? 2 : 4;
-    if (n_dev == ntotal) return refine_impl(q, nq, store_dev, store_dtype, d, ntotal, cand, k_base, k, D, I, ws, ws_bytes, st);
+                              cudaStream_t st, const float* sq = nullptr) {
+    const int eb = store_elem_bytes(store_dtype);
+    if (n_dev == ntotal) return refine_impl(q, nq, store_dev, store_dtype, d, ntotal, cand, k_base, k, D, I, ws, ws_bytes, st, sq);
     const TieredPlan p = tiered_plan(nq, k_base, k, d, eb, staging_bytes);
     if (!p.qc) return fail(RSB_ERR_CUDA, "could not size the tiered re-rank workspace: %s", cudaGetErrorString(cudaGetLastError()));
     if (!p.smem_ok)
         return fail(RSB_ERR_UNSUPPORTED, "d = %d with k_base = %d needs more shared memory than the re-rank kernel has", d, k_base);
     if (ws_bytes < p.total) return fail(RSB_ERR_OOM, "workspace too small: need %zu bytes, got %zu", p.total, ws_bytes);
     const cudaError_t e = launch_refine_tiered(p, q, nq, store_dev, n_dev, host_alias, eb, d, ntotal, cand, k_base, k, D, I,
-                                               ws, reinterpret_cast<long long*>(host_rows), st);
+                                               ws, reinterpret_cast<long long*>(host_rows), st, sq);
     if (e != cudaSuccess) return fail(RSB_ERR_CUDA, "tiered re-rank: %s", cudaGetErrorString(e));
     return RSB_OK;
 }
@@ -1234,27 +1255,38 @@ extern "C" size_t rsb_refine_tiered_workspace_bytes(int nq, int k_base, int k, i
     return std::max(refine_plan(nq, k_base, k).ws_bytes, tiered_ws(nq, k_base, k, d, staging_bytes));
 }
 
-extern "C" int rsb_refine_tiered(const float* q, int nq, const void* store_dev, int64_t n_dev, const void* store_host,
-                                 int store_dtype, int d, int64_t ntotal, const int64_t* cand, int k_base, int k, float* D,
-                                 int64_t* I, void* ws, size_t ws_bytes, size_t staging_bytes, int64_t* host_rows,
-                                 rsb_stream_t stream) {
-    RSB_TRY(tiered_check(store_dev, n_dev, store_host, store_dtype, d, ntotal, k_base, k, staging_bytes));
+// rsb_refine_tiered and rsb_refine_sq8 (sq8 = true: store_dtype RSB_DTYPE_SQ8 with its range sq)
+static int refine_tiered_entry(const float* q, int nq, const void* store_dev, int64_t n_dev, const void* store_host,
+                               int store_dtype, int d, int64_t ntotal, const int64_t* cand, int k_base, int k, float* D,
+                               int64_t* I, void* ws, size_t ws_bytes, size_t staging_bytes, int64_t* host_rows,
+                               cudaStream_t stream, const float* sq, bool sq8) {
+    RSB_TRY(tiered_check(store_dev, n_dev, store_host, store_dtype, d, ntotal, k_base, k, staging_bytes, sq8));
+    if (sq8) RSB_TRY(sq_check(sq));
     if (nq < 0) return fail(RSB_ERR_INVALID, "bad nq = %d", nq);
     if (nq == 0) return RSB_OK;
     if (!q || !cand || !D || !I) return fail(RSB_ERR_INVALID, "null argument");
     const void* alias = nullptr;
     if (n_dev < ntotal)
-        RSB_TRY(host_tier_alias(store_host, (size_t)(ntotal - n_dev) * d * (store_dtype == RSB_DTYPE_F16 ? 2 : 4), &alias));
+        RSB_TRY(host_tier_alias(store_host, (size_t)(ntotal - n_dev) * d * store_elem_bytes(store_dtype), &alias));
     return refine_tiered_impl(q, nq, store_dev, n_dev, alias, store_dtype, d, ntotal, cand, k_base, k, D, I, ws, ws_bytes,
-                              staging_bytes, host_rows, (cudaStream_t)stream);
+                              staging_bytes, host_rows, stream, sq);
+}
+
+extern "C" int rsb_refine_tiered(const float* q, int nq, const void* store_dev, int64_t n_dev, const void* store_host,
+                                 int store_dtype, int d, int64_t ntotal, const int64_t* cand, int k_base, int k, float* D,
+                                 int64_t* I, void* ws, size_t ws_bytes, size_t staging_bytes, int64_t* host_rows,
+                                 rsb_stream_t stream) {
+    return refine_tiered_entry(q, nq, store_dev, n_dev, store_host, store_dtype, d, ntotal, cand, k_base, k, D, I, ws,
+                               ws_bytes, staging_bytes, host_rows, (cudaStream_t)stream, nullptr, false);
 }
 
 static size_t search_refine_tiered_ws(rsb_index* h, int nq, int k, int k_base, int nprobe, size_t staging_bytes,
-                                      size_t* off_ref) {
+                                      size_t* off_ref, bool sq8 = false) {
     const SearchRefinePlan p = search_refine_plan(h, nq, k, k_base, nprobe);
     const int n = std::max(nq, 1), last = n % p.qb ? n % p.qb : p.qb;
     *off_ref = p.off_ref;
-    return p.total + std::max(tiered_ws(p.qb, k_base, k, h->d, staging_bytes), tiered_ws(last, k_base, k, h->d, staging_bytes));
+    return p.total + std::max(tiered_ws(p.qb, k_base, k, h->d, staging_bytes, sq8),
+                              tiered_ws(last, k_base, k, h->d, staging_bytes, sq8));
 }
 
 extern "C" size_t rsb_search_refine_tiered_workspace_bytes(rsb_index_t* h, int nq, int k, int k_factor, int nprobe,
@@ -1264,16 +1296,19 @@ extern "C" size_t rsb_search_refine_tiered_workspace_bytes(rsb_index_t* h, int n
     return search_refine_tiered_ws(h, nq, k, k * k_factor, nprobe, staging_bytes, &off_ref);
 }
 
-extern "C" int rsb_search_refine_tiered(rsb_index_t* h, const float* q, int nq, int k, int k_factor, int nprobe,
-                                        const void* store_dev, int64_t n_dev, const void* store_host, int store_dtype,
-                                        int64_t ntotal, float* D, int64_t* I, void* ws, size_t ws_bytes,
-                                        size_t staging_bytes, int64_t* host_rows, rsb_stream_t stream) {
+// rsb_search_refine_tiered and rsb_search_refine_sq8 (sq8 = true: store_dtype RSB_DTYPE_SQ8 with its range sq)
+static int search_refine_tiered_entry(rsb_index_t* h, const float* q, int nq, int k, int k_factor, int nprobe,
+                                      const void* store_dev, int64_t n_dev, const void* store_host, int store_dtype,
+                                      int64_t ntotal, float* D, int64_t* I, void* ws, size_t ws_bytes,
+                                      size_t staging_bytes, int64_t* host_rows, rsb_stream_t stream, const float* sq,
+                                      bool sq8) {
     if (!h) return fail(RSB_ERR_INVALID, "null handle");
     if (h->kind != RSB_IVFPQ) return fail(RSB_ERR_INVALID, "re-ranking is for IVFPQ indexes: Flat / IVFFlat scores are already exact");
     if (k <= 0 || k_factor <= 0) return fail(RSB_ERR_INVALID, "bad k = %d / k_factor = %d", k, k_factor);
     if ((int64_t)k * k_factor > 4096) return fail(RSB_ERR_UNSUPPORTED, "k * k_factor = %lld > 4096 is not supported", (long long)k * k_factor);
     const int k_base = k * k_factor;
-    RSB_TRY(tiered_check(store_dev, n_dev, store_host, store_dtype, h->d, ntotal, k_base, k, staging_bytes));
+    RSB_TRY(tiered_check(store_dev, n_dev, store_host, store_dtype, h->d, ntotal, k_base, k, staging_bytes, sq8));
+    if (sq8) RSB_TRY(sq_check(sq));
     if (ntotal != h->ntotal + h->n_staged)
         return fail(RSB_ERR_INVALID, "the re-rank store has %lld rows, the index holds %lld vectors", (long long)ntotal,
                     (long long)(h->ntotal + h->n_staged));
@@ -1282,9 +1317,9 @@ extern "C" int rsb_search_refine_tiered(rsb_index_t* h, const float* q, int nq, 
     if (!q || !D || !I) return fail(RSB_ERR_INVALID, "null argument");
     const void* alias = nullptr;
     if (n_dev < ntotal)
-        RSB_TRY(host_tier_alias(store_host, (size_t)(ntotal - n_dev) * h->d * (store_dtype == RSB_DTYPE_F16 ? 2 : 4), &alias));
+        RSB_TRY(host_tier_alias(store_host, (size_t)(ntotal - n_dev) * h->d * store_elem_bytes(store_dtype), &alias));
     size_t off_ref = 0;
-    const size_t total = search_refine_tiered_ws(h, nq, k, k_base, nprobe, staging_bytes, &off_ref);
+    const size_t total = search_refine_tiered_ws(h, nq, k, k_base, nprobe, staging_bytes, &off_ref, sq8);
     if (ws_bytes < total) return fail(RSB_ERR_OOM, "workspace too small: need %zu bytes, got %zu", total, ws_bytes);
     const SearchRefinePlan p = search_refine_plan(h, nq, k, k_base, nprobe);
     unsigned char* w = static_cast<unsigned char*>(ws);
@@ -1296,14 +1331,77 @@ extern "C" int rsb_search_refine_tiered(rsb_index_t* h, const float* q, int nq, 
         RSB_TRY(rsb_search(h, qb, nb, k_base, nprobe, Db, Ib, w, p.search_ws, stream));
         RSB_TRY(refine_tiered_impl(qb, nb, store_dev, n_dev, alias, store_dtype, h->d, ntotal, Ib, k_base, k,
                                    D + (size_t)q0 * k, I + (size_t)q0 * k, w + off_ref, ws_bytes - off_ref, staging_bytes,
-                                   host_rows, (cudaStream_t)stream));
+                                   host_rows, (cudaStream_t)stream, sq));
     }
     return RSB_OK;
+}
+
+extern "C" int rsb_search_refine_tiered(rsb_index_t* h, const float* q, int nq, int k, int k_factor, int nprobe,
+                                        const void* store_dev, int64_t n_dev, const void* store_host, int store_dtype,
+                                        int64_t ntotal, float* D, int64_t* I, void* ws, size_t ws_bytes,
+                                        size_t staging_bytes, int64_t* host_rows, rsb_stream_t stream) {
+    return search_refine_tiered_entry(h, q, nq, k, k_factor, nprobe, store_dev, n_dev, store_host, store_dtype, ntotal, D,
+                                      I, ws, ws_bytes, staging_bytes, host_rows, stream, nullptr, false);
 }
 
 extern "C" int rsb_refine_tiered_profile(int enable, double* ms_out) {
     if (tiered_profile(enable, ms_out) != 0) return fail(RSB_ERR_CUDA, "cudaEventCreate failed");
     return RSB_OK;
+}
+
+// ---- SQ8 re-rank store (faiss IndexRefine(base, IndexScalarQuantizer(d, QT_8bit))): uint8 codes + [2, d] (vmin, vdiff)
+static int sq8_input_check(const void* x, int x_dtype, int64_t n, int d, const float* sq) {
+    if (x_dtype != RSB_DTYPE_F32 && x_dtype != RSB_DTYPE_F16)
+        return fail(RSB_ERR_INVALID, "x_dtype must be RSB_DTYPE_F32 or RSB_DTYPE_F16, got %d", x_dtype);
+    if (n < 0 || d <= 0) return fail(RSB_ERR_INVALID, "bad n = %lld / d = %d", (long long)n, d);
+    if ((n > 0 && !x) || !sq) return fail(RSB_ERR_INVALID, "null argument");
+    return RSB_OK;
+}
+
+extern "C" int rsb_sq8_train(const void* x, int x_dtype, int64_t n, int d, float* sq, rsb_stream_t stream) {
+    RSB_TRY(sq8_input_check(x, x_dtype, n, d, sq));
+    if (n == 0) return fail(RSB_ERR_INVALID, "the scalar quantizer needs at least one training row");
+    const cudaError_t e = launch_sq8_train(x, x_dtype == RSB_DTYPE_F16, n, d, sq, (cudaStream_t)stream);
+    if (e != cudaSuccess) return fail(RSB_ERR_CUDA, "sq8 train: %s", cudaGetErrorString(e));
+    return RSB_OK;
+}
+
+extern "C" int rsb_sq8_encode(const void* x, int x_dtype, int64_t n, int d, const float* sq, uint8_t* codes,
+                              rsb_stream_t stream) {
+    RSB_TRY(sq8_input_check(x, x_dtype, n, d, sq));
+    if (n == 0) return RSB_OK;
+    if (!codes) return fail(RSB_ERR_INVALID, "null argument");
+    const cudaError_t e = launch_sq8_encode(x, x_dtype == RSB_DTYPE_F16, n, d, sq, codes, (cudaStream_t)stream);
+    if (e != cudaSuccess) return fail(RSB_ERR_CUDA, "sq8 encode: %s", cudaGetErrorString(e));
+    return RSB_OK;
+}
+
+extern "C" size_t rsb_refine_sq8_workspace_bytes(int nq, int k_base, int k, int d, size_t staging_bytes) {
+    if (nq <= 0 || k <= 0 || k_base < k || k_base > 4096 || d <= 0 || d % 16) return 0;
+    return std::max(refine_plan(nq, k_base, k).ws_bytes, tiered_ws(nq, k_base, k, d, staging_bytes, true));
+}
+
+extern "C" int rsb_refine_sq8(const float* q, int nq, const void* store_dev, int64_t n_dev, const void* store_host,
+                              const float* sq, int d, int64_t ntotal, const int64_t* cand, int k_base, int k, float* D,
+                              int64_t* I, void* ws, size_t ws_bytes, size_t staging_bytes, int64_t* host_rows,
+                              rsb_stream_t stream) {
+    return refine_tiered_entry(q, nq, store_dev, n_dev, store_host, RSB_DTYPE_SQ8, d, ntotal, cand, k_base, k, D, I, ws,
+                               ws_bytes, staging_bytes, host_rows, (cudaStream_t)stream, sq, true);
+}
+
+extern "C" size_t rsb_search_refine_sq8_workspace_bytes(rsb_index_t* h, int nq, int k, int k_factor, int nprobe,
+                                                       size_t staging_bytes) {
+    if (!h || k <= 0 || k_factor <= 0 || (int64_t)k * k_factor > 4096 || h->d % 16) return 0;
+    size_t off_ref = 0;
+    return search_refine_tiered_ws(h, nq, k, k * k_factor, nprobe, staging_bytes, &off_ref, true);
+}
+
+extern "C" int rsb_search_refine_sq8(rsb_index_t* h, const float* q, int nq, int k, int k_factor, int nprobe,
+                                     const void* store_dev, int64_t n_dev, const void* store_host, const float* sq,
+                                     int64_t ntotal, float* D, int64_t* I, void* ws, size_t ws_bytes, size_t staging_bytes,
+                                     int64_t* host_rows, rsb_stream_t stream) {
+    return search_refine_tiered_entry(h, q, nq, k, k_factor, nprobe, store_dev, n_dev, store_host, RSB_DTYPE_SQ8, ntotal, D,
+                                      I, ws, ws_bytes, staging_bytes, host_rows, stream, sq, true);
 }
 
 // ---- training steps (index.train) ---------------------------------------------------------------------------

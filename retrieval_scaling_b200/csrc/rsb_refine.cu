@@ -1,8 +1,8 @@
 // rsb_refine.cu -- exact re-ranking of IVF-PQ candidates against a caller-owned re-rank store (faiss IndexRefine /
 // IndexRefineFlat::search, reference call site src/indicies/ivf_pq.py:119-123 `get_knn_scores`).
 //
-//   refine_rows_kernel<T>  per (query, candidate chunk): gather the candidates' rows of the store (T = fp16 or fp32),
-//                          score <q, x_id> in fp32, sort the chunk's keys (score desc, id asc) and either write the
+//   refine_rows_kernel<T>  per (query, candidate chunk): gather the candidates' rows of the store (T = fp16, fp32 or
+//                          uint8 SQ8 codes, decoded per element), score <q, x_id> in fp32, sort the chunk's keys (score desc, id asc) and either write the
 //                          final (D, I) row (one chunk per query) or the chunk's top-k keys for merge_items_flat_kernel.
 //
 // The kernel is bound by gather bandwidth: every candidate row is read once per query (nq * k' * d * elem_bytes bytes
@@ -32,12 +32,16 @@ namespace rsb {
 constexpr int RF_THREADS = 256, RF_WARPS = RF_THREADS / 32, RF_ROWS = 4;
 constexpr int RF_MIN_CHUNK = 256;     // candidates per CTA below which splitting a query stops paying
 
-// A lane takes 8 consecutive elements per step (one 16-byte load of fp16, two of fp32) and adds them in element
-// order, so both store types sum in the same order: equal decoded values give bit-identical scores.
+// A lane takes 8 consecutive elements per step (one 16-byte load of fp16, two of fp32, one 8-byte load of SQ8 codes)
+// and adds them in element order, so every store type sums in the same order: equal decoded values give
+// bit-identical scores.
 constexpr int RF_E = 8;
-template <typename T> struct Loads { static constexpr int n = RF_E * (int)sizeof(T) / 16; };
+template <typename T> struct Loads { using V = uint4; static constexpr int n = RF_E * (int)sizeof(T) / 16; };
+template <> struct Loads<uint8_t> { using V = uint2; static constexpr int n = 1; };
 
-__device__ __forceinline__ float dot8(const uint4 (&v)[2], const float* qs, float acc, float) {
+// dot8(v, qs, acc, T(), sq): acc += <q[e .. e+8), x[e .. e+8)> by fmaf in element order.  sq (SQ8 only) points at
+// vmin[e] in shared memory, with vdiff[e] d floats further on (sq_d).
+__device__ __forceinline__ float dot8(const uint4 (&v)[2], const float* qs, float acc, float, const float*, int) {
 #pragma unroll
     for (int j = 0; j < 2; ++j) {
         const float4 a = *reinterpret_cast<const float4*>(qs + 4 * j);
@@ -46,7 +50,7 @@ __device__ __forceinline__ float dot8(const uint4 (&v)[2], const float* qs, floa
     }
     return acc;
 }
-__device__ __forceinline__ float dot8(const uint4 (&v)[1], const float* qs, float acc, __half) {
+__device__ __forceinline__ float dot8(const uint4 (&v)[1], const float* qs, float acc, __half, const float*, int) {
     const float4 a = *reinterpret_cast<const float4*>(qs);
     const float4 b = *reinterpret_cast<const float4*>(qs + 4);
     const float2 x0 = __half22float2(*reinterpret_cast<const __half2*>(&v[0].x));
@@ -58,38 +62,72 @@ __device__ __forceinline__ float dot8(const uint4 (&v)[1], const float* qs, floa
     return acc;
 }
 
+// SQ8 decode (faiss ScalarQuantizer QT_8bit, non-uniform): x = vmin + ((c + 0.5f) / 255.f) * vdiff, every operation a
+// separately rounded fp32 op.  c + 0.5 is exact from the bits of 2^23 + c; the quotient comes from a reciprocal
+// multiply and one fma correction, which gives the correctly rounded (c + 0.5f) / 255.f for each of the 256 codes
+// (a plain reciprocal multiply differs for 191 of them).  __fmul_rn / __fadd_rn keep nvcc from contracting the decode.
+__device__ __forceinline__ float sq8_decode(unsigned w, unsigned byte, float vmin, float vdiff) {
+    constexpr float inv = 1.f / 255.f;
+    const float a = __fadd_rn(__uint_as_float(__byte_perm(w, 0x4B000000u, 0x7440u | byte)), -8388607.5f);
+    const float t = __fmul_rn(a, inv);
+    const float u = __fmaf_rn(__fmaf_rn(-t, 255.f, a), inv, t);
+    return __fadd_rn(vmin, __fmul_rn(u, vdiff));
+}
+
+__device__ __forceinline__ float dot8(const uint2 (&v)[1], const float* qs, float acc, uint8_t, const float* sq,
+                                      int sq_d) {
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+        const unsigned w = j ? v[0].y : v[0].x;
+        const float4 a = *reinterpret_cast<const float4*>(qs + 4 * j);
+        const float4 lo = *reinterpret_cast<const float4*>(sq + 4 * j);
+        const float4 df = *reinterpret_cast<const float4*>(sq + sq_d + 4 * j);
+        acc = fmaf(sq8_decode(w, 0, lo.x, df.x), a.x, acc); acc = fmaf(sq8_decode(w, 1, lo.y, df.y), a.y, acc);
+        acc = fmaf(sq8_decode(w, 2, lo.z, df.z), a.z, acc); acc = fmaf(sq8_decode(w, 3, lo.w, df.w), a.w, acc);
+    }
+    return acc;
+}
+
 // grid = (nq, nchunks).  Block (q, c) scores candidates [c * chunk, min(k_base, (c + 1) * chunk)) of query q.
 // Candidates with id < 0 (the base search's padding) or id >= ntotal are skipped.
 // direct = 1 (nchunks == 1): writes D/I [nq, k_out], padded with (-FLT_MAX, -1).
 // direct = 0: writes the chunk's best min(k_item, valid) keys to out_keys[(q * nchunks + c) * k_item ...] and their
 // number to out_cnt[q * nchunks + c], for merge_items_flat_kernel.
-// Four CTAs per SM (64 registers): without the bound ptxas picks 48 registers for the fp32 form and spills.
+// Four CTAs per SM (64 registers): without the bound ptxas picks 48 registers for the fp32 form and spills.  The SQ8
+// form (decode arithmetic, vmin / vdiff operands) spills at 64 registers and runs three CTAs per SM (80 registers).
 // TIERED: ids >= n_dev are read from staging + slot[q * k_base + j] * d instead of X + id * d (the key keeps the id);
 // the lane mapping and the fmaf order are the same, so a row scores bit-identically from either place.
+// T = uint8_t (SQ8 codes): sq [2, d] fp32 (vmin, vdiff) is copied to shared memory after the query, and every element
+// is decoded before its fmaf, so the scores are those of an fp32 store holding the decoded rows.
 template <typename T, bool TIERED>
-__global__ __launch_bounds__(RF_THREADS, 4)
+__global__ __launch_bounds__(RF_THREADS, sizeof(T) == 1 ? 3 : 4)
 void refine_rows_kernel(const float* __restrict__ Q, const T* __restrict__ X, int d, int64_t ntotal,
                         const int64_t* __restrict__ cand, int k_base, int chunk, int P, int k_out, int direct,
                         float* __restrict__ D, int64_t* __restrict__ I, u64* __restrict__ out_keys,
                         int* __restrict__ out_cnt, int64_t n_dev, const T* __restrict__ staging,
-                        const int* __restrict__ slot) {
+                        const int* __restrict__ slot, const float* __restrict__ sq) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     u64* keys = reinterpret_cast<u64*>(smem_raw);                     // [P]
-    float* qs = reinterpret_cast<float*>(smem_raw + (size_t)P * 8);   // [d]
-    constexpr int NL = Loads<T>::n;                                   // 16-byte loads per lane and step
+    float* qs = reinterpret_cast<float*>(smem_raw + (size_t)P * 8);   // [d], then (SQ8) vmin [d], vdiff [d]
+    using V = typename Loads<T>::V;
+    constexpr int NL = Loads<T>::n;                                   // loads of V per lane and step
+    constexpr bool SQ8 = sizeof(T) == 1;
     const int q = blockIdx.x, c = blockIdx.y, nchunks = gridDim.y;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int j0 = c * chunk;
     const int n = min(chunk, k_base - j0);
     for (int e = tid * 4; e < d; e += RF_THREADS * 4)
         *reinterpret_cast<float4*>(qs + e) = *reinterpret_cast<const float4*>(Q + (size_t)q * d + e);
+    if (SQ8)
+        for (int e = tid * 4; e < 2 * d; e += RF_THREADS * 4)
+            *reinterpret_cast<float4*>(qs + d + e) = *reinterpret_cast<const float4*>(sq + e);
     for (int i = tid; i < P; i += RF_THREADS) keys[i] = 0ull;
     __syncthreads();
     const int64_t* ids = cand + (size_t)q * k_base + j0;
     for (int r0 = warp * RF_ROWS; r0 < n; r0 += RF_WARPS * RF_ROWS) {
         int64_t id[RF_ROWS];
         bool ok[RF_ROWS];
-        const uint4* row[RF_ROWS];
+        const V* row[RF_ROWS];
         float acc[RF_ROWS];
 #pragma unroll
         for (int r = 0; r < RF_ROWS; ++r) {
@@ -97,18 +135,18 @@ void refine_rows_kernel(const float* __restrict__ Q, const T* __restrict__ X, in
             ok[r] = id[r] >= 0 && id[r] < ntotal;                     // warp-uniform
             const T* src = X + (size_t)(ok[r] ? id[r] : 0) * d;
             if (TIERED && ok[r] && id[r] >= n_dev) src = staging + (size_t)slot[(size_t)q * k_base + j0 + r0 + r] * d;
-            row[r] = reinterpret_cast<const uint4*>(src);
+            row[r] = reinterpret_cast<const V*>(src);
             acc[r] = 0.f;
         }
         for (int e = lane * RF_E; e < d; e += 32 * RF_E) {
-            uint4 v[RF_ROWS][NL];
+            V v[RF_ROWS][NL];
 #pragma unroll
             for (int r = 0; r < RF_ROWS; ++r)
 #pragma unroll
                 for (int j = 0; j < NL; ++j)
-                    v[r][j] = ok[r] ? __ldg(row[r] + e / RF_E * NL + j) : make_uint4(0u, 0u, 0u, 0u);
+                    v[r][j] = ok[r] ? __ldg(row[r] + e / RF_E * NL + j) : V{};
 #pragma unroll
-            for (int r = 0; r < RF_ROWS; ++r) acc[r] = dot8(v[r], qs + e, acc[r], T());
+            for (int r = 0; r < RF_ROWS; ++r) acc[r] = dot8(v[r], qs + e, acc[r], T(), qs + d + e, d);
         }
 #pragma unroll
         for (int r = 0; r < RF_ROWS; ++r) {
@@ -156,38 +194,48 @@ RefinePlan refine_plan(int nq, int k_base, int k) {
     return p;
 }
 
-bool refine_smem_fits(const RefinePlan& p, int d) { return (size_t)p.P * 8 + (size_t)d * 4 <= 200 * 1024; }
+static size_t refine_smem(const RefinePlan& p, int d, int elem_bytes) {
+    return (size_t)p.P * 8 + (size_t)d * 4 * (elem_bytes == 1 ? 3 : 1);
+}
+bool refine_smem_fits(const RefinePlan& p, int d, int elem_bytes) { return refine_smem(p, d, elem_bytes) <= 200 * 1024; }
 
 template <typename T, bool TIERED>
 static void launch_rows(const RefinePlan& p, dim3 grid, size_t smem, const float* Q, const void* X, int d, int64_t ntotal,
                         const int64_t* cand, int k_base, int k, int direct, float* D, int64_t* I, u64* keys, int* cnt,
-                        const TierArgs* tier, cudaStream_t st) {
+                        const TierArgs* tier, const float* sq, cudaStream_t st) {
     static PerDeviceSize configured;
     if (smem > 48 * 1024 && configured.raise(smem))
         cudaFuncSetAttribute(refine_rows_kernel<T, TIERED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     refine_rows_kernel<T, TIERED><<<grid, RF_THREADS, smem, st>>>(
         Q, static_cast<const T*>(X), d, ntotal, cand, k_base, p.chunk, p.P, k, direct, D, I, keys, cnt,
         TIERED ? tier->n_dev : ntotal, TIERED ? static_cast<const T*>(tier->staging) : nullptr,
-        TIERED ? tier->slot : nullptr);
+        TIERED ? tier->slot : nullptr, sq);
+}
+
+template <typename T>
+static void launch_rows(const RefinePlan& p, dim3 grid, size_t smem, const float* Q, const void* X, int d, int64_t ntotal,
+                        const int64_t* cand, int k_base, int k, int direct, float* D, int64_t* I, u64* keys, int* cnt,
+                        const TierArgs* tier, const float* sq, cudaStream_t st) {
+    if (tier) launch_rows<T, true>(p, grid, smem, Q, X, d, ntotal, cand, k_base, k, direct, D, I, keys, cnt, tier, sq, st);
+    else launch_rows<T, false>(p, grid, smem, Q, X, d, ntotal, cand, k_base, k, direct, D, I, keys, cnt, tier, sq, st);
 }
 
 int launch_refine_rows(const RefinePlan& p, const float* Q, int nq, const void* X, int elem_bytes, int d,
                        int64_t ntotal, const int64_t* cand, int k_base, int k, float* D, int64_t* I, void* ws,
-                       cudaStream_t st, const TierArgs* tier) {
+                       cudaStream_t st, const TierArgs* tier, const float* sq) {
     if (nq <= 0) return 0;
-    const size_t smem = (size_t)p.P * 8 + (size_t)d * 4;
-    if (!refine_smem_fits(p, d)) return -1;
+    const size_t smem = refine_smem(p, d, elem_bytes);
+    if (!refine_smem_fits(p, d, elem_bytes)) return -1;
     const int direct = p.nchunks == 1;
     u64* keys = direct ? nullptr : static_cast<u64*>(ws);
     int* cnt = direct ? nullptr : reinterpret_cast<int*>(static_cast<unsigned char*>(ws) + (size_t)nq * p.nchunks * p.k_item * 8);
     dim3 grid(nq, p.nchunks);
-    if (elem_bytes == 2) {
-        if (tier) launch_rows<__half, true>(p, grid, smem, Q, X, d, ntotal, cand, k_base, k, direct, D, I, keys, cnt, tier, st);
-        else launch_rows<__half, false>(p, grid, smem, Q, X, d, ntotal, cand, k_base, k, direct, D, I, keys, cnt, tier, st);
-    } else {
-        if (tier) launch_rows<float, true>(p, grid, smem, Q, X, d, ntotal, cand, k_base, k, direct, D, I, keys, cnt, tier, st);
-        else launch_rows<float, false>(p, grid, smem, Q, X, d, ntotal, cand, k_base, k, direct, D, I, keys, cnt, tier, st);
-    }
+    if (elem_bytes == 1)
+        launch_rows<uint8_t>(p, grid, smem, Q, X, d, ntotal, cand, k_base, k, direct, D, I, keys, cnt, tier, sq, st);
+    else if (elem_bytes == 2)
+        launch_rows<__half>(p, grid, smem, Q, X, d, ntotal, cand, k_base, k, direct, D, I, keys, cnt, tier, sq, st);
+    else
+        launch_rows<float>(p, grid, smem, Q, X, d, ntotal, cand, k_base, k, direct, D, I, keys, cnt, tier, sq, st);
     if (!direct) launch_merge_items(keys, cnt, nq, p.nchunks, p.k_item, k, nullptr, 0, D, I, st);
     return 0;
 }
@@ -281,7 +329,8 @@ TieredPlan tiered_plan(int nq, int k_base, int k, int d, int elem_bytes, size_t 
     }
     p.cub_bytes = std::max(sort_bytes, scan_bytes);
     p.ref_bytes = std::max(refine_plan(p.qc, k_base, k).ws_bytes, refine_plan(last, k_base, k).ws_bytes);
-    p.smem_ok = refine_smem_fits(refine_plan(p.qc, k_base, k), d) && refine_smem_fits(refine_plan(last, k_base, k), d);
+    p.smem_ok = refine_smem_fits(refine_plan(p.qc, k_base, k), d, elem_bytes) &&
+                refine_smem_fits(refine_plan(last, k_base, k), d, elem_bytes);
     const size_t a4 = al((size_t)L * 4);
     p.off_keys = 0;                      // tier keys, then the run flags
     p.off_keys2 = p.off_keys + a4;       // sorted keys
@@ -322,7 +371,7 @@ int tiered_profile(int enable, double* ms3) {
 cudaError_t launch_refine_tiered(const TieredPlan& p, const float* Q, int nq, const void* X_dev, int64_t n_dev,
                                  const void* X_host, int elem_bytes, int d, int64_t ntotal, const int64_t* cand,
                                  int k_base, int k, float* D, int64_t* I, void* ws, long long* host_rows,
-                                 cudaStream_t st) {
+                                 cudaStream_t st, const float* sq) {
     unsigned char* w = static_cast<unsigned char*>(ws);
     unsigned* keys = reinterpret_cast<unsigned*>(w + p.off_keys);
     unsigned* keys2 = reinterpret_cast<unsigned*>(w + p.off_keys2);
@@ -362,13 +411,15 @@ cudaError_t launch_refine_tiered(const TieredPlan& p, const float* Q, int nq, co
         if (prof.on) cudaEventRecord(prof.ev[1], st);
         const size_t words = (size_t)L * row_bytes / 16;
         const unsigned gb = (unsigned)((words + GH_THREADS * GH_U - 1) / (GH_THREADS * GH_U));
-        if (elem_bytes == 2)
+        if (elem_bytes == 1)
+            gather_host_rows_kernel<uint8_t><<<gb, GH_THREADS, 0, st>>>(static_cast<const uint4*>(X_host), uniq, count, d, staging);
+        else if (elem_bytes == 2)
             gather_host_rows_kernel<__half><<<gb, GH_THREADS, 0, st>>>(static_cast<const uint4*>(X_host), uniq, count, d, staging);
         else
             gather_host_rows_kernel<float><<<gb, GH_THREADS, 0, st>>>(static_cast<const uint4*>(X_host), uniq, count, d, staging);
         if (prof.on) cudaEventRecord(prof.ev[2], st);
         if (launch_refine_rows(refine_plan(nc, k_base, k), Q + (size_t)q0 * d, nc, X_dev, elem_bytes, d, ntotal, cq,
-                               k_base, k, D + (size_t)q0 * k, I + (size_t)q0 * k, w + p.off_ref, st, &tier) != 0)
+                               k_base, k, D + (size_t)q0 * k, I + (size_t)q0 * k, w + p.off_ref, st, &tier, sq) != 0)
             return cudaErrorInvalidConfiguration;       // not reached: the caller checked p.smem_ok
         if (prof.on) {                                  // profiling only: waits for the chunk to read its events
             cudaEventRecord(prof.ev[3], st);
@@ -384,6 +435,78 @@ cudaError_t launch_refine_tiered(const TieredPlan& p, const float* Q, int nq, co
         if (e != cudaSuccess) return e;
     }
     return cudaSuccess;
+}
+
+// ---- SQ8 store: training (per-dimension min / max) and encoding (faiss ScalarQuantizer QT_8bit, RS_minmax) ---------
+constexpr int SQ_THREADS = 256, SQ_SLABS = 1024;
+
+__device__ __forceinline__ float to_f32(float x) { return x; }
+__device__ __forceinline__ float to_f32(__half x) { return __half2float(x); }
+
+// while training, sq holds order-preserving keys: ord(min) in [0, d), ord(max) in [d, 2d)
+__global__ void sq8_init_kernel(unsigned* __restrict__ sq, int d) {
+    const int j = blockIdx.x * SQ_THREADS + threadIdx.x;
+    if (j < d) { sq[j] = 0xFFFFFFFFu; sq[d + j] = 0u; }
+}
+
+// block (column tile, slab): rows slab, slab + gridDim.y, ... of columns [tile * SQ_THREADS, ...)
+template <typename T>
+__global__ __launch_bounds__(SQ_THREADS)
+void sq8_train_kernel(const T* __restrict__ x, int64_t n, int d, unsigned* __restrict__ sq) {
+    const int j = blockIdx.x * SQ_THREADS + threadIdx.x;
+    if (j >= d) return;
+    float lo = INFINITY, hi = -INFINITY;
+    for (int64_t r = blockIdx.y; r < n; r += gridDim.y) {
+        const float v = to_f32(x[(size_t)r * d + j]);
+        lo = fminf(lo, v);
+        hi = fmaxf(hi, v);
+    }
+    atomicMin(sq + j, ord_f32(lo));
+    atomicMax(sq + d + j, ord_f32(hi));
+}
+
+// keys -> vmin [d], vdiff = vmax - vmin [d] (fp32)
+__global__ void sq8_finish_kernel(float* __restrict__ sq, int d) {
+    const int j = blockIdx.x * SQ_THREADS + threadIdx.x;
+    if (j >= d) return;
+    unsigned* u = reinterpret_cast<unsigned*>(sq);
+    const float vmin = unord_f32(u[j]), vmax = unord_f32(u[d + j]);
+    sq[j] = vmin;
+    sq[d + j] = __fsub_rn(vmax, vmin);
+}
+
+// code = (int)(255.f * clamp((x - vmin) / vdiff, 0, 1)), 0 where vdiff == 0; separately rounded fp32 ops
+template <typename T>
+__global__ __launch_bounds__(SQ_THREADS)
+void sq8_encode_kernel(const T* __restrict__ x, size_t total, int d, const float* __restrict__ sq,
+                       uint8_t* __restrict__ codes) {
+    for (size_t i = (size_t)blockIdx.x * SQ_THREADS + threadIdx.x; i < total; i += (size_t)gridDim.x * SQ_THREADS) {
+        const int j = (int)(i % d);
+        const float vmin = sq[j], vdiff = sq[d + j];
+        float xi = vdiff != 0.f ? __fdiv_rn(__fsub_rn(to_f32(x[i]), vmin), vdiff) : 0.f;
+        xi = xi < 0.f ? 0.f : (xi > 1.f ? 1.f : xi);
+        codes[i] = (uint8_t)(int)__fmul_rn(255.f, xi);
+    }
+}
+
+cudaError_t launch_sq8_train(const void* x, int x_f16, int64_t n, int d, float* sq, cudaStream_t st) {
+    unsigned* u = reinterpret_cast<unsigned*>(sq);
+    const unsigned tiles = (unsigned)((d + SQ_THREADS - 1) / SQ_THREADS);
+    sq8_init_kernel<<<tiles, SQ_THREADS, 0, st>>>(u, d);
+    const dim3 grid(tiles, (unsigned)std::min<int64_t>(n, SQ_SLABS));
+    if (x_f16) sq8_train_kernel<__half><<<grid, SQ_THREADS, 0, st>>>(static_cast<const __half*>(x), n, d, u);
+    else sq8_train_kernel<float><<<grid, SQ_THREADS, 0, st>>>(static_cast<const float*>(x), n, d, u);
+    sq8_finish_kernel<<<tiles, SQ_THREADS, 0, st>>>(sq, d);
+    return cudaPeekAtLastError();
+}
+
+cudaError_t launch_sq8_encode(const void* x, int x_f16, int64_t n, int d, const float* sq, uint8_t* codes,
+                              cudaStream_t st) {
+    const size_t total = (size_t)n * d;
+    const unsigned blocks = (unsigned)std::min<size_t>((total + SQ_THREADS - 1) / SQ_THREADS, 132 * 64);
+    if (x_f16) sq8_encode_kernel<__half><<<blocks, SQ_THREADS, 0, st>>>(static_cast<const __half*>(x), total, d, sq, codes);
+    else sq8_encode_kernel<float><<<blocks, SQ_THREADS, 0, st>>>(static_cast<const float*>(x), total, d, sq, codes);
+    return cudaPeekAtLastError();
 }
 
 }  // namespace rsb

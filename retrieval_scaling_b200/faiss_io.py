@@ -3,7 +3,8 @@ persists with `faiss.write_index` / loads with `faiss.read_index` (`src/indicies
 `ivf_flat.py:71,167,185`, `ivf_pq.py:75,171,190`):
 
     "IxFI"  IndexFlatIP            "IwFl"  IndexIVFFlat (quantizer IndexFlatIP)      "IwPQ"  IndexIVFPQ (by_residual)
-    "IxRF"  IndexRefineFlat (IVF-PQ base + exact re-rank vectors; faiss IndexRefine with an IndexFlat refine index)
+    "IxRF"  IndexRefineFlat (IVF-PQ base + exact re-rank vectors; faiss IndexRefine with an IndexFlat refine index), or
+            IndexRefine with an "IxSQ" IndexScalarQuantizer refine index of qtype QT_8bit (`Refine(SQ8)`)
 
 [FAISS-ext] faiss is not installable in this image, so this module restates the on-disk layout of faiss 1.8.0
 (`faiss/impl/index_write.cpp`, `index_read.cpp`) from the published source and is pinned only by byte-level
@@ -18,8 +19,13 @@ faiss build.  Layout (little endian):
   IwPQ           : ivf header | by_residual u8 | code_size u64 | PQ: d u64 | M u64 | nbits u64 | (u64 n | float32[n]) | inverted lists
   inverted lists : "ilar" | nlist u64 | code_size u64 | "full" (u64 n | u64 sizes[n])  or  "sprs" (u64 n | u64 (list, size) pairs)
                    then, for every list in order: codes u8[size * code_size] | ids i64[size]
-  IxRF           : header | <base index> | <refine index, here IxFI> | k_factor f32
+  IxRF           : header | <base index> | <refine index, IxFI or IxSQ> | k_factor f32
                    (index_write.cpp: IndexRefine branch; index_read.cpp turns a flat refine index into IndexRefineFlat)
+  IxSQ           : header | qtype i32 | rangestat i32 | rangestat_arg f32 | d u64 | code_size u64
+                   | trained (u64 n | float32[n]) | codes (u64 n | u8[n])
+                   (write_ScalarQuantizer + the codes vector; only qtype QT_8bit = 0 is supported, whose trained vector
+                   is [2, d] = vmin then vdiff and code_size = d; rangestat only steers training and is written as
+                   RS_minmax = 0)
 """
 from __future__ import annotations
 
@@ -29,6 +35,7 @@ from typing import BinaryIO, Dict
 import numpy as np
 
 METRIC_INNER_PRODUCT, METRIC_L2 = 0, 1
+QT_8BIT, RS_MINMAX = 0, 0
 
 
 def fourcc(s: str) -> int:
@@ -76,6 +83,19 @@ def _read_flat(f: BinaryIO, hdr: Dict) -> Dict:
     if n != hdr["ntotal"] * hdr["d"]:
         raise ValueError(f"flat index payload has {n} floats, expected {hdr['ntotal']} x {hdr['d']}")
     return {"kind": "Flat", **hdr, "xb": xb.reshape(hdr["ntotal"], hdr["d"])}
+
+
+def _read_sq(f: BinaryIO, hdr: Dict) -> Dict:
+    qtype, rangestat, rangestat_arg = _rd(f, "i"), _rd(f, "i"), _rd(f, "f")
+    d, code_size = _rd(f, "Q"), _rd(f, "Q")
+    trained = _rd_array(f, np.float32, _rd(f, "Q"))
+    codes = _rd_array(f, np.uint8, _rd(f, "Q"))
+    if qtype != QT_8BIT:
+        raise NotImplementedError(f"IndexScalarQuantizer qtype {qtype}: only QT_8bit (0) is supported")
+    if d != hdr["d"] or code_size != d or trained.size != 2 * d or codes.size != hdr["ntotal"] * d:
+        raise ValueError("IndexScalarQuantizer: d, code_size, trained or codes disagree with the header")
+    return {"kind": "SQ", **hdr, "rangestat": rangestat, "rangestat_arg": rangestat_arg,
+            "sq": trained.reshape(2, d), "codes": codes.reshape(hdr["ntotal"], d)}
 
 
 def _read_invlists(f: BinaryIO, nlist_expected: int, tag_bytes: bytes = None):
@@ -138,6 +158,8 @@ def read_faiss(f) -> Dict:
     tag = _fourcc_str(_rd(f, "I"))
     if tag in ("IxFI", "IxF2", "IxFl"):
         return _read_flat(f, _read_header(f))
+    if tag == "IxSQ":
+        return _read_sq(f, _read_header(f))
     if tag == "IwFl":
         h = _read_ivf_header(f)
         # faiss does not store code_size for IwFl (index_read.cpp sets it to d * sizeof(float)).  Files written by the
@@ -172,10 +194,12 @@ def read_faiss(f) -> Dict:
         base = read_faiss(f)
         refine = read_faiss(f)
         k_factor = _rd(f, "f")
-        if refine["kind"] != "Flat":
-            raise NotImplementedError("only a flat refine index (IndexRefineFlat) is supported, not IxSQ / PQ refinement")
+        if refine["kind"] not in ("Flat", "SQ"):
+            raise NotImplementedError("only a flat (IxFI) or QT_8bit scalar-quantizer (IxSQ) refine index is supported")
         if base["d"] != hdr["d"] or refine["d"] != hdr["d"] or refine["ntotal"] != base["ntotal"]:
             raise ValueError("IndexRefine: base and refine index disagree on d or ntotal")
+        if refine["kind"] == "SQ":          # SQ8 store: codes [ntotal, d] uint8 + sq [2, d] (vmin, vdiff), no "xb"
+            return {"kind": "Refine", **hdr, "base": base, "sq": refine["sq"], "codes": refine["codes"], "k_factor": k_factor}
         return {"kind": "Refine", **hdr, "base": base, "xb": refine["xb"], "k_factor": k_factor}
     raise NotImplementedError(f"faiss index type {tag!r} is not supported (Flat / IVFFlat / IVFPQ / RefineFlat only)")
 
@@ -202,6 +226,22 @@ def _write_flat(f: BinaryIO, xb: np.ndarray, metric: int = METRIC_INNER_PRODUCT)
     _write_header(f, "IxFI" if metric == METRIC_INNER_PRODUCT else "IxF2", xb.shape[1], xb.shape[0], True, metric)
     _wr(f, "Q", xb.size)
     f.write(xb.tobytes())
+
+
+def _write_sq(f: BinaryIO, sq: np.ndarray, codes: np.ndarray):
+    sq = np.ascontiguousarray(sq, dtype=np.float32)
+    codes = np.ascontiguousarray(codes, dtype=np.uint8)
+    d = sq.shape[1]
+    _write_header(f, "IxSQ", d, codes.shape[0], True, METRIC_INNER_PRODUCT)
+    _wr(f, "i", QT_8BIT)
+    _wr(f, "i", RS_MINMAX)
+    _wr(f, "f", 0.0)
+    _wr(f, "Q", d)
+    _wr(f, "Q", d)                            # code_size: one byte per element
+    _wr(f, "Q", sq.size)
+    f.write(sq.tobytes())
+    _wr(f, "Q", codes.size)
+    f.write(codes.tobytes())
 
 
 def _write_invlists(f: BinaryIO, nlist: int, code_size: int, offsets: np.ndarray, codes: np.ndarray, ids: np.ndarray):
@@ -264,10 +304,13 @@ def write_faiss(f, parts: Dict) -> None:
         f.write(cb.tobytes())
         _write_invlists(f, parts["centroids"].shape[0], code_size, parts["offsets"], parts["codes"], parts["ids"])
     elif kind == "Refine":
-        xb = parts["xb"]
-        _write_header(f, "IxRF", xb.shape[1], xb.shape[0], True, METRIC_INNER_PRODUCT)
+        rows = parts["codes"] if "codes" in parts else parts["xb"]
+        _write_header(f, "IxRF", rows.shape[1], rows.shape[0], True, METRIC_INNER_PRODUCT)
         write_faiss(f, parts["base"])
-        _write_flat(f, xb, METRIC_INNER_PRODUCT)
+        if "codes" in parts:
+            _write_sq(f, parts["sq"], parts["codes"])
+        else:
+            _write_flat(f, rows, METRIC_INNER_PRODUCT)
         _wr(f, "f", float(parts.get("k_factor", 1.0)))
     else:
         raise NotImplementedError(kind)

@@ -56,6 +56,14 @@ def _dev_rows(x, device) -> torch.Tensor:
 _STORE_DTYPES = {"float16": (torch.float16, _lib.RSB_DTYPE_F16), "float32": (torch.float32, _lib.RSB_DTYPE_F32)}
 
 
+# IndexRefine's store: the storage dtypes, plus "sq8" (uint8 codes of a trained scalar quantizer)
+_REFINE_DTYPES = {**_STORE_DTYPES, "sq8": (torch.uint8, _lib.RSB_DTYPE_SQ8)}
+
+
+def _dtype_code(x: torch.Tensor) -> int:
+    return _lib.RSB_DTYPE_F16 if x.dtype == torch.float16 else _lib.RSB_DTYPE_F32
+
+
 def _check_dtype(dtype: str, what: str = "dtype") -> str:
     if dtype not in _STORE_DTYPES:
         raise ValueError(f"{what} must be float16 or float32, got {dtype!r}")
@@ -429,6 +437,12 @@ class IndexRefine:
     fp16 store of them is lossless; an fp16 store of fp32 vectors rounds them (faiss `Refine(SQfp16)`).
     Results are sorted by exact score descending, ties by ascending id, padded with (-FLT_MAX, -1).
 
+    store_dtype = "sq8" keeps one uint8 code per element (faiss IndexRefine(base, IndexScalarQuantizer(d, QT_8bit)),
+    `Refine(SQ8)`): half the bytes of fp16.  Its per-dimension range (vmin, vdiff) is trained by train(x) (base and
+    quantizer, as faiss IndexRefine::train) or train_store(x) (quantizer only); add_store encodes fp16 / fp32 rows on the
+    device.  Scores are exact fp32 inner products with the decoded rows vmin + ((c + 0.5f) / 255.f) * vdiff, bit-identical
+    to a float32 store holding those rows.  d % 16 == 0.
+
     device_rows = n (an integer) makes the store tiered, for stores larger than device memory: rows [0, n) stay in
     device memory and rows from n on go to page-locked, device-mapped host memory (rsb_search_refine_tiered).  Each
     search gathers the distinct host rows its candidates need over PCIe, `staging_bytes` of queries' worst case at a
@@ -440,15 +454,18 @@ class IndexRefine:
     def __init__(self, base, store_dtype: str = "float16", k_factor: int = 1, device_rows: Optional[int] = None):
         if not isinstance(base, IndexIVFPQ):
             raise ValueError(f"IndexRefine re-ranks IVF-PQ results; a {type(base).__name__} base already returns exact scores")
-        if store_dtype not in _STORE_DTYPES:
-            raise ValueError(f"store_dtype must be float16 or float32, got {store_dtype!r}")
+        if store_dtype not in _REFINE_DTYPES:
+            raise ValueError(f"store_dtype must be float16, float32 or sq8, got {store_dtype!r}")
+        if store_dtype == "sq8" and base.d % 16:
+            raise ValueError(f"an sq8 store needs d % 16 == 0 (whole 16-byte rows), got d = {base.d}")
         self.base, self.store_dtype = base, store_dtype
         self.k_factor = int(k_factor)
         self.device_rows = _check_device_rows(device_rows)
         self.L, self.d, self.device = base.L, base.d, base.device
-        self._store = torch.empty((0, self.d), dtype=_STORE_DTYPES[store_dtype][0], device=self.device)
+        self._store = torch.empty((0, self.d), dtype=_REFINE_DTYPES[store_dtype][0], device=self.device)
         self._host = torch.empty((0, self.d), dtype=self._store.dtype)      # host tier (tiered store only)
         self._n = 0                                     # rows of the store in use (capacity = self._store.shape[0])
+        self._sq: Optional[torch.Tensor] = None         # sq8: trained [2, d] float32 (vmin, vdiff) on the device
 
     @property
     def tiered(self) -> bool:
@@ -507,7 +524,33 @@ class IndexRefine:
         return self._store[: self._n]
 
     def train(self, x) -> None:
+        """Trains the base; an sq8 store also trains its quantizer on the same rows (faiss IndexRefine::train)."""
         self.base.train(x)
+        if self.store_dtype == "sq8":
+            self.train_store(x)
+
+    def train_store(self, x) -> None:
+        """sq8 only: trains the store's quantizer (per-dimension min and max of the rows x [n, d], fp16 or fp32), for a
+        base that is already trained or read from disk.  Rows already in the store keep their codes."""
+        if self.store_dtype != "sq8":
+            raise ValueError(f"a {self.store_dtype} store has no quantizer to train")
+        with torch.cuda.device(self.device):
+            x = _dev_rows(x, self.device)
+            if x.dim() != 2 or x.shape[1] != self.d or x.shape[0] == 0:
+                raise ValueError(f"expected [n >= 1, {self.d}] training vectors, got {tuple(x.shape)}")
+            sq = torch.empty((2, self.d), dtype=torch.float32, device=self.device)
+            _lib.check(self.L.rsb_sq8_train(_ptr(x), _dtype_code(x), x.shape[0], self.d, _ptr(sq), _stream()))
+            torch.cuda.current_stream(self.device).synchronize()     # x may be a temporary
+            self._sq = sq
+
+    @property
+    def sq_params(self) -> Tuple[torch.Tensor, torch.Tensor]:
+        """sq8 only: the trained (vmin [d], vdiff [d]) float32 device tensors."""
+        if self.store_dtype != "sq8":
+            raise ValueError(f"a {self.store_dtype} store has no quantizer")
+        if self._sq is None:
+            raise ValueError("the sq8 quantizer is not trained: call train() or train_store() first")
+        return self._sq[0], self._sq[1]
 
     def add(self, x, ids=None) -> None:
         """Adds to the base and appends to the store.  The store is addressed by index id, so ids are the base's
@@ -545,12 +588,28 @@ class IndexRefine:
 
     def add_store(self, x) -> None:
         """Appends rows to the store only (for a base that already holds these vectors, e.g. one read from disk).
-        Rows bound for the host tier are copied there directly: host input never crosses PCIe for them."""
+        Rows bound for the host tier are copied there directly: host input never crosses PCIe for them.  An sq8 store
+        encodes every row on the device (fp16 rows cross PCIe as fp16) and copies the host tier's codes into it."""
         if isinstance(x, np.ndarray):
             x = torch.from_numpy(np.ascontiguousarray(x))
         x = torch.as_tensor(x)
         if x.dim() != 2 or x.shape[1] != self.d:
             raise ValueError(f"expected [n, {self.d}] vectors, got {tuple(x.shape)}")
+        if self.store_dtype != "sq8":
+            self._append(x)
+            return
+        self.sq_params                                              # ValueError before anything is stored
+        step = max(1, (256 << 20) // (4 * self.d))
+        with torch.cuda.device(self.device):
+            for a in range(0, x.shape[0], step):
+                xc = _dev_rows(x[a:a + step], self.device)
+                codes = torch.empty(xc.shape, dtype=torch.uint8, device=self.device)
+                _lib.check(self.L.rsb_sq8_encode(_ptr(xc), _dtype_code(xc), xc.shape[0], self.d, _ptr(self._sq),
+                                                 _ptr(codes), _stream()))
+                self._append(codes)
+
+    def _append(self, x: torch.Tensor) -> None:
+        """Appends rows already in the store's element type (or, for fp16 / fp32, convertible to it) to the tiers."""
         n = x.shape[0]
         if self._n + n > self._capacity():
             self.reserve(max(self._n + n, int(1.25 * self._capacity())))
@@ -568,6 +627,10 @@ class IndexRefine:
         """(device tier, n_dev, host tier pointer) of rsb_*_tiered."""
         return _ptr(self._store), self.n_dev, _ptr(self.host_store)
 
+    def _sq_ptr(self):
+        self.sq_params                                              # ValueError if the quantizer is untrained
+        return _ptr(self._sq)
+
     def search_ids(self, q, k: int, nprobe: Optional[int] = None, k_factor: Optional[int] = None,
                    host_rows: Optional[torch.Tensor] = None):
         """q [nq, d] -> (ids int64 [nq,k], scores float32 [nq,k]) CUDA tensors, enqueued on the current stream.
@@ -582,6 +645,13 @@ class IndexRefine:
             D = torch.empty((nq, k), dtype=torch.float32, device=self.device)
             I = torch.empty((nq, k), dtype=torch.int64, device=self.device)
             if nq == 0:
+                return I, D
+            if self.store_dtype == "sq8":                   # all-device (n_dev = ntotal) or tiered: one entry point
+                sb = int(self.staging_bytes)
+                ws = self.base._workspace(self.L.rsb_search_refine_sq8_workspace_bytes(self.base._h, nq, k, kf, npb, sb))
+                _lib.check(self.L.rsb_search_refine_sq8(
+                    self.base._h, _ptr(q), nq, k, kf, npb, *self._tier_args(), self._sq_ptr(), self._n, _ptr(D), _ptr(I),
+                    _ptr(ws), ws.numel(), sb, _ptr(host_rows), _stream()))
                 return I, D
             if self.tiered:
                 sb = int(self.staging_bytes)
@@ -613,6 +683,13 @@ class IndexRefine:
             nq, k_base = cand.shape
             D = torch.empty((nq, int(k)), dtype=torch.float32, device=self.device)
             I = torch.empty((nq, int(k)), dtype=torch.int64, device=self.device)
+            if self.store_dtype == "sq8":
+                sb = int(self.staging_bytes if staging_bytes is None else staging_bytes)
+                ws = self.base._workspace(self.L.rsb_refine_sq8_workspace_bytes(nq, k_base, int(k), self.d, sb))
+                _lib.check(self.L.rsb_refine_sq8(_ptr(q), nq, *self._tier_args(), self._sq_ptr(), self.d, self._n,
+                                                 _ptr(cand), k_base, int(k), _ptr(D), _ptr(I), _ptr(ws), ws.numel(), sb,
+                                                 _ptr(host_rows), _stream()))
+                return I, D
             if self.tiered:
                 sb = int(self.staging_bytes if staging_bytes is None else staging_bytes)
                 dt = _STORE_DTYPES[self.store_dtype][1]
@@ -642,6 +719,11 @@ MAGIC = "RSB1"
 
 def _to_faiss_parts(index: _IndexBase) -> dict:
     if isinstance(index, IndexRefine):
+        if index.store_dtype == "sq8":      # faiss IndexRefine with an IndexScalarQuantizer(QT_8bit) refine index
+            codes = torch.cat([index.device_store.cpu(), index.host_store]) if index.tiered else index.store.cpu()
+            return {"kind": "Refine", "d": index.d, "ntotal": index.ntotal, "base": _to_faiss_parts(index.base),
+                    "sq": torch.stack(index.sq_params).cpu().numpy(), "codes": codes.numpy(),
+                    "k_factor": float(index.k_factor)}
         # faiss IndexRefineFlat: an fp16 store is written upcast to fp32 (exact)
         xb = torch.cat([index.device_store.float().cpu(), index.host_store.float()]) if index.tiered else index.store.float().cpu()
         return {"kind": "Refine", "d": index.d, "ntotal": index.ntotal, "base": _to_faiss_parts(index.base),
@@ -672,6 +754,18 @@ def _from_faiss_parts(p: dict, device=None, refine_dtype: Optional[str] = None,
         kf = float(p["k_factor"])
         if kf != int(kf) or kf < 1:
             raise NotImplementedError(f"k_factor = {kf}: only whole k_factor >= 1 is supported")
+        if "codes" in p:                   # IxSQ QT_8bit refine index: the codes and the trained range load as they are
+            if refine_dtype not in (None, "sq8"):
+                raise ValueError(f"the refine index is an 8-bit scalar quantizer (IxSQ): its store is sq8, not {refine_dtype}")
+            index = IndexRefine(_from_faiss_parts(p["base"], device), store_dtype="sq8", k_factor=int(kf))
+            if index.ntotal != p["codes"].shape[0]:
+                raise ValueError(f"refine index holds {p['codes'].shape[0]} vectors, its base {index.ntotal}")
+            index._sq = torch.from_numpy(np.ascontiguousarray(p["sq"], dtype=np.float32)).to(index.device)
+            index.reserve(p["codes"].shape[0])
+            index._append(torch.from_numpy(np.ascontiguousarray(p["codes"])))
+            return index
+        if refine_dtype == "sq8":
+            raise ValueError("the refine index holds float vectors (IxFI): read it with refine_dtype float32 or float16")
         xb = p["xb"]
         dtype = refine_dtype or "float32"
         if dtype == "float16":
@@ -763,7 +857,8 @@ def read_index(path: str, device=None, refine_dtype: Optional[str] = None,
                storage_dtype: Optional[str] = None) -> _IndexBase:
     """Loads an RSB1 container or a faiss binary index file (auto-detected by its fourcc).  For an IndexRefineFlat
     file (IxRF) `refine_dtype` picks the store: "float32" (default) or "float16", which is accepted only when every
-    stored value round-trips through fp16 (ValueError otherwise).  `storage_dtype` does the same for the vectors of a
+    stored value round-trips through fp16 (ValueError otherwise).  An IxRF file whose refine index is an 8-bit scalar
+    quantizer (IxSQ, QT_8bit) loads as an sq8 store (refine_dtype None or "sq8"; float16 / float32 raise ValueError).  `storage_dtype` does the same for the vectors of a
     Flat / IVFFlat index (IxFI / IwFl / RSB1); None keeps the file's dtype (fp32 for faiss files)."""
     from . import faiss_io
     if faiss_io.is_faiss_file(path):

@@ -32,7 +32,7 @@ class Indexer(object):
 
     @staticmethod
     def refine_options(index_cfg):
-        """Optional keys `refine_k_factor` (absent or 0: no re-ranking) and `refine_dtype` (float16 | float32; absent:
+        """Optional keys `refine_k_factor` (absent or 0: no re-ranking) and `refine_dtype` (float16 | float32 | sq8; absent:
         the embedding pickles' dtype) -> (k_factor, dtype).  Re-ranking applies to IVFPQ only."""
         k_factor = int(index_cfg.get("refine_k_factor", 0) or 0)
         dtype = index_cfg.get("refine_dtype", None)
@@ -41,8 +41,8 @@ class Indexer(object):
         if k_factor and index_cfg.index_type != "IVFPQ":
             raise ValueError(f"datastore.index.refine_k_factor re-ranks IVFPQ results; {index_cfg.index_type} scores "
                              f"are already exact")
-        if dtype not in (None, "float16", "float32"):
-            raise ValueError(f"datastore.index.refine_dtype must be float16 or float32, got {dtype!r}")
+        if dtype not in (None, "float16", "float32", "sq8"):
+            raise ValueError(f"datastore.index.refine_dtype must be float16, float32 or sq8, got {dtype!r}")
         Indexer.refine_device_rows(index_cfg)
         return k_factor, dtype
 

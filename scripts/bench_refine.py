@@ -29,7 +29,17 @@ every --tiered-nq batch size (k = --k, k_factor = --k-factor):
   * with --compare-device, the all-device store in the same run: byte-identical results required;
   * recall@k refined and unrefined and the parity block, at the largest batch;
   * the card's name and power limit, the PCIe link generation and width, the host's MemAvailable.
-The host tier is capped at half of MemAvailable (larger sizes are refused before anything is built) and freed at exit."""
+The host tier is capped at half of MemAvailable (larger sizes are refused before anything is built) and freed at exit.
+
+    python scripts/bench_refine.py --n 20000000 --k-factor 8 --store-dtype sq8 --compare-store float16
+
+--store-dtype picks the store: float16 (default), float32, or sq8 (8-bit scalar-quantizer codes, faiss Refine(SQ8),
+trained on the first --sq-train-rows corpus rows).  --compare-store builds a second store of another dtype on the same
+index in the same run.  With either set to something other than a lone float16 store, the line holds one block per store
+under "stores": dtype, device / host bytes, build seconds, and per --store-nq batch size the refined QPS, the re-rank
+kernel milliseconds and gathered GB/s (nq x k' x d x element bytes over the kernel time), with recall@k, exact
+top-1 / top-10 and parity at the largest batch.  With --device-rows the same options apply to the tiered store (the
+comparison store is then all-device and must be byte-identical for sq8 vs sq8 only)."""
 import argparse
 import json
 import os
@@ -65,13 +75,61 @@ def parse():
     ap.add_argument("--staging-gb", type=float, default=1.0, help="tiered store: staging buffer (GiB)")
     ap.add_argument("--tiered-nq", default="1,64,10000", help="tiered store: batch sizes to report")
     ap.add_argument("--compare-device", action="store_true", help="tiered store: also build the all-device store")
+    ap.add_argument("--store-dtype", default="float16", choices=("float16", "float32", "sq8"))
+    ap.add_argument("--compare-store", default=None, choices=("float16", "float32", "sq8"),
+                    help="all-device runs: also build a store of this dtype on the same index")
+    ap.add_argument("--store-nq", default="10000,64,1", help="batch sizes reported per store (--store-dtype / --compare-store)")
+    ap.add_argument("--sq-train-rows", type=int, default=1_000_000, help="sq8: corpus rows the quantizer is trained on")
     a = ap.parse_args()
     a.partition = "list"
     return a
 
 
-def store_bytes(args) -> int:
-    return args.n * args.d * 2
+ELEM_BYTES = {"float16": 2, "float32": 4, "sq8": 1}
+
+
+def store_bytes(args, dtype="float16") -> int:
+    return args.n * args.d * ELEM_BYTES[dtype]
+
+
+def train_sq8(refs, corpus, args):
+    """Trains every sq8 store in refs on the first min(n, --sq-train-rows) corpus rows."""
+    refs = [r for r in refs if r.store_dtype == "sq8"]
+    if not refs:
+        return
+    n = min(args.n, args.sq_train_rows)
+    x = torch.cat([corpus.chunk(c, B.CHUNK_ROWS) for c in range((n + B.CHUNK_ROWS - 1) // B.CHUNK_ROWS)])[:n]
+    for r in refs:
+        r.train_store(x)
+    del x
+
+
+def fill_stores(stores, corpus, args):
+    """Trains the sq8 stores, then adds every corpus chunk to every store; returns the build seconds per store."""
+    secs = {}
+    for name, ref in stores.items():
+        t0 = time.time()
+        train_sq8([ref], corpus, args)
+        ref.reserve(args.n)
+        secs[name] = time.time() - t0
+    for c in range((args.n + B.CHUNK_ROWS - 1) // B.CHUNK_ROWS):
+        x = corpus.chunk(c, B.CHUNK_ROWS)[: min(B.CHUNK_ROWS, args.n - c * B.CHUNK_ROWS)]
+        for name, ref in stores.items():
+            torch.cuda.synchronize()
+            t0 = time.time()
+            ref.add_store(x)
+            torch.cuda.synchronize()
+            secs[name] += time.time() - t0
+    return secs
+
+
+def decoded_rows(ref, rows: torch.Tensor) -> np.ndarray:
+    """Store rows as the re-rank scores them: sq8 codes decoded by the oracle's rule, others upcast."""
+    if ref.store_dtype != "sq8":
+        return rows.cpu().numpy()
+    from oracle import sq8_oracle as S
+    sq = torch.stack(ref.sq_params).cpu().numpy()
+    return S.sq8_decode(rows.cpu().numpy().reshape(-1, ref.d), sq).reshape(rows.shape)
 
 
 def gpu_identity(device) -> dict:
@@ -104,7 +162,7 @@ def parity(ref, xq, Ib, Ir, Dr, k, npq):
     from oracle import refine_oracle as R
     kb = Ib.shape[1]
     Ib_h = Ib[:npq].cpu().numpy()
-    rows = ref.store_rows(Ib[:npq].clamp_min(0).reshape(-1)).reshape(npq, kb, -1).cpu().numpy()   # [npq, k', d] fp16
+    rows = decoded_rows(ref, ref.store_rows(Ib[:npq].clamp_min(0).reshape(-1)).reshape(npq, kb, -1))   # [npq, k', d]
     xq_h = xq[:npq].cpu().numpy()
     Dref = np.full((npq, k), np.finfo(np.float32).min, np.float32)
     Iref = np.full((npq, k), -1, np.int64)
@@ -185,7 +243,8 @@ def zero_copy_rerank(ref, q, Ib, k):
     D = torch.empty((nq, k), dtype=torch.float32, device=ref.device)
     I = torch.empty((nq, k), dtype=torch.int64, device=ref.device)
     ws = ref.base._workspace(ref.L.rsb_refine_workspace_bytes(nq, kb, k))
-    _lib.check(ref.L.rsb_refine(_ptr(q), nq, _ptr(ref.host_store), _lib.RSB_DTYPE_F16, ref.d, ref.ntotal, _ptr(Ib), kb, k,
+    dt = _lib.RSB_DTYPE_F16 if ref.store_dtype == "float16" else _lib.RSB_DTYPE_F32
+    _lib.check(ref.L.rsb_refine(_ptr(q), nq, _ptr(ref.host_store), dt, ref.d, ref.ntotal, _ptr(Ib), kb, k,
                                 _ptr(D), _ptr(I), _ptr(ws), ws.numel(), _stream()))
     return I, D
 
@@ -196,13 +255,14 @@ def tiered_main(args, device):
     k, kf = args.k, args.k_factor
     kb = k * kf
     n_dev = min(args.device_rows, args.n)
-    host_bytes = (args.n - n_dev) * args.d * 2
+    dtype, eb = args.store_dtype, ELEM_BYTES[args.store_dtype]
+    host_bytes = (args.n - n_dev) * args.d * eb
     avail = mem_available()
     if host_bytes > avail // 2:
-        raise SystemExit(f"the host tier of {args.n - n_dev} x {args.d} fp16 needs {host_bytes} bytes of pinned memory; "
+        raise SystemExit(f"the host tier of {args.n - n_dev} x {args.d} {dtype} needs {host_bytes} bytes of pinned memory; "
                          f"the cap is half of MemAvailable = {avail // 2} bytes: use a larger --device-rows or a smaller --n")
     free, _ = torch.cuda.mem_get_info(device)
-    dev_bytes = n_dev * args.d * 2 + (store_bytes(args) if args.compare_device else 0)
+    dev_bytes = n_dev * args.d * eb + (store_bytes(args, dtype) if args.compare_device else 0)
     # + the corpus generator's fp32 chunk and its temporary while the store is filled
     need = dev_bytes + args.n * (args.m + 8) + int(args.staging_gb * (1 << 30)) + 2 * B.CHUNK_ROWS * args.d * 4
     if need > 0.9 * free:
@@ -215,18 +275,12 @@ def tiered_main(args, device):
     n_gt = min(args.recall_queries, args.nq)
     index, corpus, _, gt_I, build = B.build_index(args, 0, 1, device, gt_queries=xq_all[:n_gt].contiguous())
 
-    t0 = time.time()
-    stores = {"tiered": rsb.IndexRefine(index, "float16", kf, device_rows=n_dev)}
+    stores = {"tiered": rsb.IndexRefine(index, dtype, kf, device_rows=n_dev)}
     if args.compare_device:
-        stores["device"] = rsb.IndexRefine(index, "float16", kf)
+        stores["device"] = rsb.IndexRefine(index, dtype, kf)
     for ref in stores.values():
         ref.staging_bytes = int(args.staging_gb * (1 << 30))
-        ref.reserve(args.n)
-    for c in range((args.n + B.CHUNK_ROWS - 1) // B.CHUNK_ROWS):
-        x = corpus.chunk(c, B.CHUNK_ROWS)[: min(B.CHUNK_ROWS, args.n - c * B.CHUNK_ROWS)]
-        for ref in stores.values():
-            ref.add_store(x)
-    store_s = time.time() - t0
+    store_s = fill_stores(stores, corpus, args)["tiered"]
     ref = stores["tiered"]
     L = ref.L
 
@@ -250,17 +304,18 @@ def tiered_main(args, device):
                "sort_ms": split[0], "gather_ms": split[1], "score_ms": split[2],
                "host_tier_candidates": host_cand, "unique_host_rows": uniq,
                "unique_frac_of_host_candidates": uniq / host_cand if host_cand else None,
-               "gathered_bytes": uniq * args.d * 2,
-               "gathered_gbs": uniq * args.d * 2 / (split[1] / 1e3) / 1e9 if split[1] > 0 else None}
+               "gathered_bytes": uniq * args.d * eb,
+               "gathered_gbs": uniq * args.d * eb / (split[1] / 1e3) / 1e9 if split[1] > 0 else None}
         row["gathered_frac_of_memcpy"] = (row["gathered_gbs"] / info["pinned_to_device_memcpy_gbs"]
                                           if row["gathered_gbs"] else None)
         row["same_result_as_two_stage"] = bool(torch.equal(I, Ir) and torch.equal(D, Dr))
-        if n_dev == 0:
+        if n_dev == 0 and dtype != "sq8":
             ms_zc, (Iz, Dz) = timed(lambda: zero_copy_rerank(ref, xq, Ib, k), args.steps, args.warmup)
             row["zero_copy_rerank_ms"] = ms_zc
             row["zero_copy_same_result"] = bool(torch.equal(Iz, Ir) and torch.equal(Dz, Dr))
         else:
-            row["zero_copy_rerank_ms"] = "not measured (needs --device-rows 0: rsb_refine reads one contiguous store)"
+            row["zero_copy_rerank_ms"] = ("not measured (needs --device-rows 0: rsb_refine reads one contiguous store)"
+                                          if dtype != "sq8" else "not measured (rsb_refine has no sq8 form)")
         if "device" in stores:
             full = stores["device"]
             ms_dev, (Id, Dd) = timed(lambda: full.search_ids(xq, k), args.steps, args.warmup)
@@ -274,18 +329,77 @@ def tiered_main(args, device):
     xq, I, Iu, Ib, Ir, Dr, nq = last
     strip = lambda r: {kk: vv for kk, vv in r.items() if kk != "ground_truth"}   # noqa: E731
     ng = min(n_gt, nq)
-    out = {"metric": f"exact re-ranking of k x {kf} candidates from a tiered fp16 store ({n_dev} device rows, "
+    out = {"metric": f"exact re-ranking of k x {kf} candidates from a tiered {dtype} store ({n_dev} device rows, "
                      f"{args.n - n_dev} pinned host rows), {args.n // 1_000_000}M x {args.d} IVF-PQ",
            "config": {**B.make_config(args, 1), "k_factor": kf, "k_base": kb, "device_rows": n_dev,
                       "host_rows": args.n - n_dev, "staging_bytes": ref.staging_bytes},
            "per_nq": per_nq, **info,
-           "store": {"dtype": "float16", "device_bytes": n_dev * args.d * 2, "host_bytes": host_bytes, "build_s": store_s},
+           "store": {"dtype": dtype, "device_bytes": n_dev * args.d * eb, "host_bytes": host_bytes, "build_s": store_s},
            "recall_nq": ng, "recall": strip(B.recall_block(I[:ng], gt_I[:ng], k)),
            "recall_unrefined": strip(B.recall_block(Iu[:ng], gt_I[:ng], k)),
            "recall_ground_truth": "bench.py's exact fp32 inner-product search over the same corpus",
            "parity": parity(ref, xq, Ib, Ir, Dr, k, min(args.parity_queries, nq)),
            "build": build, "steps": args.steps, "warmup": args.warmup}
     del stores, ref
+    print(json.dumps(out), flush=True)
+    return 0
+
+
+def stores_main(args, device):
+    """All-device stores of --store-dtype and --compare-store on one index, measured one after the other."""
+    import retrieval_scaling_b200 as rsb
+    from retrieval_scaling_b200 import synth
+    dtypes = [args.store_dtype] + [t for t in [args.compare_store] if t and t != args.store_dtype]
+    need = sum(store_bytes(args, t) for t in dtypes) + args.n * (args.m + 8) + 2 * B.CHUNK_ROWS * args.d * 4
+    free, _ = torch.cuda.mem_get_info(device)
+    if need > 0.9 * free:
+        raise SystemExit(f"the {' + '.join(dtypes)} stores of {args.n} x {args.d} and the index need ~{need} bytes, "
+                         f"{free} are free on {device}; use a smaller --n or drop --compare-store")
+    k, kf = args.k, args.k_factor
+    kb = k * kf
+    probe = synth.Corpus(d=args.d, mode="gmm", n_centres=max(16, args.nlist // 4), device=device)
+    xq_all = probe.queries(args.nq)
+    del probe
+    n_gt = min(args.recall_queries, args.nq)
+    index, corpus, _, gt_I, build = B.build_index(args, 0, 1, device, gt_queries=xq_all[:n_gt].contiguous())
+    stores = {t: rsb.IndexRefine(index, t, kf) for t in dtypes}
+    secs = fill_stores(stores, corpus, args)
+    info = gpu_identity(device)
+    peak, peak_src = B.measured_peak_gbs()
+    strip = lambda r: {kk: vv for kk, vv in r.items() if kk != "ground_truth"}   # noqa: E731
+    nqs = sorted({min(int(v), args.nq) for v in args.store_nq.split(",")}, reverse=True)
+    blocks = {}
+    for t, ref in stores.items():
+        eb = ELEM_BYTES[t]
+        per_nq = []
+        for nq in nqs:
+            xq = xq_all[:nq].contiguous()
+            ms_unref, (Iu, _) = timed(lambda: index.search_ids(xq, k), args.steps, args.warmup)
+            ms_ref, (I, D) = timed(lambda: ref.search_ids(xq, k), args.steps, args.warmup)
+            Ib, _ = index.search_ids(xq, kb)
+            ms_rr, (Ir, Dr) = timed(lambda: ref.rerank(xq, Ib, k), args.steps, args.warmup)
+            gathered = nq * kb * args.d * eb
+            per_nq.append({"nq": nq, "qps_refined": nq / (ms_ref / 1e3), "qps_unrefined": nq / (ms_unref / 1e3),
+                           "ms_per_step_refined": ms_ref, "ms_per_step_unrefined": ms_unref, "rerank_kernel_ms": ms_rr,
+                           "gathered_bytes": gathered, "gathered_gbs": gathered / (ms_rr / 1e3) / 1e9,
+                           "valid_candidate_frac": int((Ib >= 0).sum().item()) / (nq * kb),
+                           "same_result_as_two_stage": bool(torch.equal(I, Ir) and torch.equal(D, Dr))})
+            if nq == nqs[0]:
+                ng = min(n_gt, nq)
+                top = {"recall": strip(B.recall_block(I[:ng], gt_I[:ng], k)),
+                       "recall_unrefined": strip(B.recall_block(Iu[:ng], gt_I[:ng], k)), "recall_nq": ng,
+                       "parity": parity(ref, xq, Ib, Ir, Dr, k, min(args.parity_queries, nq))}
+        blocks[t] = {"dtype": t, "device_bytes": store_bytes(args, t), "host_bytes": 0, "build_s": secs[t],
+                     "per_nq": per_nq, **top}
+        if t == "sq8":
+            blocks[t]["sq8_train_rows"] = min(args.n, args.sq_train_rows)
+    out = {"metric": f"exact re-ranking of k x {kf} candidates, {args.n // 1_000_000}M x {args.d} IVF-PQ, "
+                     f"{' vs '.join(dtypes)} store",
+           "config": {**B.make_config(args, 1), "k_factor": kf, "k_base": kb}, "stores": blocks, **info,
+           "peak_gbs": peak, "peak_source": peak_src,
+           "gathered_bytes_rule": "nq x k' x d x element bytes (every candidate row read once per query)",
+           "recall_ground_truth": "bench.py's exact fp32 inner-product search over the same corpus",
+           "build": build, "steps": args.steps, "warmup": args.warmup}
     print(json.dumps(out), flush=True)
     return 0
 
@@ -298,6 +412,8 @@ def main():
     torch.cuda.set_device(device)
     if args.device_rows is not None:
         return tiered_main(args, device)
+    if args.store_dtype != "float16" or args.compare_store is not None:
+        return stores_main(args, device)
     need = store_bytes(args) + args.n * (args.m + 8)                   # store + PQ codes + ids
     free, _ = torch.cuda.mem_get_info(device)
     if need > 0.9 * free:
