@@ -59,9 +59,18 @@ int rsb_ivfflat_create(int d, int nlist, rsb_index_t** out);
  * a bank-conflict-free look-up layout that exists for K in {1, 2, 4}: csrc/rsb_layout.h); any other multiple of 4 up to
  * 128 dividing d (e.g. 24 / 48 / 96 on d = 768, which faiss and the reference's n_subquantizers key accept) runs a
  * functionally complete generic path (natural code order, [m][256] tables, one thread per vector) -- correct, not tuned.
- * RESTRICTION (narrower than faiss): nbits must be 8 (tables of 256 entries, one byte per code); nbits = 4 / 10 / 12 /
- * 16 and other M return RSB_ERR_UNSUPPORTED (-> NotImplementedError in Python). */
+ * rsb_ivfpq_create takes nbits = 8 only (tables of 256 entries, one byte per code); any other nbits returns
+ * RSB_ERR_UNSUPPORTED (-> NotImplementedError in Python), as do other M. */
 int rsb_ivfpq_create(int d, int nlist, int M, int nbits, rsb_index_t** out);
+/* As rsb_ivfpq_create, with nbits = 8 (identical to it) or nbits = 4.  4-bit codes are packed two per byte in faiss'
+ * order (PQEncoderGeneric, LSB first: byte b = c[2b] | c[2b+1] << 4), so a vector holds Mb = M / 2 code bytes, and the
+ * index is scanned as an 8-bit index of Mb byte sub-quantizers with the pair tables T'[b][j] = T[2b][j & 15] +
+ * T[2b+1][j >> 4]: M = 32 / 64 / 128 run the tuned scan (Mb = 16 / 32 / 64), any other M with M % 8 == 0, M / 2 <= 128
+ * and d % M == 0 the generic one.  Scores differ from faiss' sequential sum over m by fp32 rounding only.
+ * nbits other than 4 / 8 (codes crossing bytes, tables beyond shared memory) -> RSB_ERR_UNSUPPORTED; a 4-bit M outside
+ * those shapes -> RSB_ERR_INVALID.  With nbits = 4 the codebook (rsb_set_pq_codebook / rsb_get_pq_codebook) is
+ * [M, 16, d/M], and codes (rsb_add_codes, rsb_export_lists) are [n, M / 2] packed bytes. */
+int rsb_ivfpq_create_nbits(int d, int nlist, int M, int nbits, rsb_index_t** out);
 /* Storage dtype of the vectors (enum RSB_DTYPE_* below): RSB_DTYPE_F32 is rsb_flat_create / rsb_ivfflat_create;
  * RSB_DTYPE_F16 keeps every row as fp16 -- the embedding task writes fp16 passage embeddings (src/embed.py:137-138)
  * and the reference upcasts them only on load (src/indicies/flat.py:86), so fp16 storage of them is lossless at half
@@ -80,7 +89,7 @@ int rsb_free(rsb_index_t* h);
 /* ---- trained state (what index.train() produces; ivf_flat.py:166, ivf_pq.py:170) ------------------ */
 /* coarse centroids [nlist, d] float32, copied */
 int rsb_set_centroids(rsb_index_t* h, const float* centroids_dev, rsb_stream_t stream);
-/* PQ codebook [M, 256, d/M] float32, copied */
+/* PQ codebook [M, 2^nbits, d/M] float32, copied */
 int rsb_set_pq_codebook(rsb_index_t* h, const float* codebook_dev, rsb_stream_t stream);
 int rsb_get_centroids(rsb_index_t* h, float* out_dev, rsb_stream_t stream);
 int rsb_get_pq_codebook(rsb_index_t* h, float* out_dev, rsb_stream_t stream);
@@ -103,7 +112,7 @@ int rsb_add_typed(rsb_index_t* h, const void* x_dev, int x_dtype, int64_t n, con
                   size_t ws_bytes, rsb_stream_t stream);
 int rsb_add_preassigned_typed(rsb_index_t* h, const void* x_dev, int x_dtype, int64_t n, const int64_t* ids_dev,
                               const int32_t* list_dev, rsb_stream_t stream);
-/* IVFPQ only: rows are already PQ codes [n, M] uint8 (e.g. read from an existing index file) */
+/* IVFPQ only: rows are already PQ codes [n, M * nbits / 8] uint8 (e.g. read from an existing index file) */
 int rsb_add_codes(rsb_index_t* h, const uint8_t* codes_dev, int64_t n, const int64_t* ids_dev,
                   const int32_t* list_dev, rsb_stream_t stream);
 /* Build the searchable layout (CSR inverted lists; PQ codes interleaved per 32 vectors).  Synchronises
@@ -123,7 +132,7 @@ int rsb_info(rsb_index_t* h, int what, int64_t* out);
 /* list sizes [nlist] int64 to a device buffer */
 int rsb_list_sizes(rsb_index_t* h, int64_t* sizes_dev, rsb_stream_t stream);
 /* Export the inverted lists in natural CSR order (insertion order inside each list), as the oracle and a
- * faiss file writer want them: offsets_dev [nlist+1] int64, payload_dev = uint8 codes [ntotal, M] (IVFPQ)
+ * faiss file writer want them: offsets_dev [nlist+1] int64, payload_dev = uint8 codes [ntotal, M * nbits / 8] (IVFPQ)
  * or vectors [ntotal, d] in the storage dtype, float32 or fp16 (IVFFLAT / FLAT), ids_dev [ntotal] int64.  Any pointer
  * may be NULL. */
 int rsb_export_lists(rsb_index_t* h, int64_t* offsets_dev, void* payload_dev, int64_t* ids_dev,
@@ -283,6 +292,14 @@ int rsb_pq_assign(const float* r_dev, int64_t n, int d, int M, const float* code
 /* PQ k-means update step: sums_dev [M, 256, d/M] += slices, counts_dev [M, 256] (float) += 1 */
 int rsb_pq_accumulate(const float* r_dev, int64_t n, int d, int M, const uint8_t* codes_dev, float* sums_dev,
                       float* counts_dev, rsb_stream_t stream);
+/* The same two steps for ksub = 256 (nbits = 8: rsb_pq_assign / rsb_pq_accumulate) or ksub = 16 (nbits = 4); other
+ * ksub -> RSB_ERR_UNSUPPORTED.  codebook_dev [M, ksub, d/M]; codes_dev [n, M], one code per byte (not packed), the
+ * nearest entry by L2 with the lowest index winning exact ties; sums_dev [M, ksub, d/M], counts_dev [M, ksub].  Member
+ * sums are added in a fixed order, so training gives the same codebook on every run. */
+int rsb_pq_assign_ksub(const float* r_dev, int64_t n, int d, int M, int ksub, const float* codebook_dev,
+                       uint8_t* codes_dev, rsb_stream_t stream);
+int rsb_pq_accumulate_ksub(const float* r_dev, int64_t n, int d, int M, int ksub, const uint8_t* codes_dev,
+                           float* sums_dev, float* counts_dev, rsb_stream_t stream);
 
 /* ---- options -------------------------------------------------------------------------------------------- */
 enum {
@@ -335,8 +352,15 @@ int rsb_gemm_f16(const void* A_dev, const void* W_dev, const void* bias_dev, con
 
 /* diagnostic: shared-window address at which dynamic shared memory starts (the scan kernel folds it into LDS) */
 int rsb_debug_smem_base(void);
+/* diagnostic: the fp32 look-up tables an IVFPQ search builds for queries q_dev [nq, d], as the scan reads them:
+ * lut_dev [nq, rsb_pq_lut_floats(h)], entry (j, b) of byte sub-quantizer b at rsb_pq_lut_index(Mb, j, b) (Mb = M * nbits
+ * / 8; with nbits = 4 the entry is the pair sum T[2b][j & 15] + T[2b+1][j >> 4]).  rsb_pq_lut_floats: -1 if h is not
+ * IVFPQ. */
+int rsb_pq_lut_floats(rsb_index_t* h);
+int rsb_pq_tables(rsb_index_t* h, const float* q_dev, int nq, float* lut_dev, rsb_stream_t stream);
 
 /* ---- layout self-description (lets host-side tests pin the interleaved PQ layout without a GPU) ------- */
+/* M here counts code bytes per vector (M * nbits / 8; with 4-bit codes, byte b holds sub-quantizers 2b and 2b+1) */
 /* byte offset, inside a 32-vector block of M*32 bytes, of sub-quantizer m of block-local vector v */
 int rsb_pq_layout_offset(int M, int v, int m);
 /* float index, inside one 256x64 look-up-table row block, where entry (j, m) lives (first replica) */

@@ -27,6 +27,7 @@ SIGNATURES = [
     ("rsb_flat_create", c_int, [c_int, POINTER(_H)]),
     ("rsb_ivfflat_create", c_int, [c_int, c_int, POINTER(_H)]),
     ("rsb_ivfpq_create", c_int, [c_int, c_int, c_int, c_int, POINTER(_H)]),
+    ("rsb_ivfpq_create_nbits", c_int, [c_int, c_int, c_int, c_int, POINTER(_H)]),
     ("rsb_flat_create_dtype", c_int, [c_int, c_int, POINTER(_H)]),
     ("rsb_ivfflat_create_dtype", c_int, [c_int, c_int, c_int, POINTER(_H)]),
     ("rsb_free", c_int, [_H]),
@@ -53,6 +54,8 @@ SIGNATURES = [
     ("rsb_kmeans_accumulate", c_int, [c_void_p, c_int64, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     ("rsb_pq_assign", c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     ("rsb_pq_accumulate", c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    ("rsb_pq_assign_ksub", c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    ("rsb_pq_accumulate_ksub", c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     ("rsb_peer_broadcast", c_int, [c_void_p, c_size_t, c_void_p, c_int, c_size_t, c_void_p]),
     ("rsb_coarse", c_int, [_H, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     ("rsb_refine_workspace_bytes", c_size_t, [c_int, c_int, c_int]),
@@ -98,6 +101,8 @@ SIGNATURES = [
     ("rsb_bert_launches", c_int64, [_H]),
     ("rsb_gemm_f16", c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     ("rsb_debug_smem_base", c_int, []),
+    ("rsb_pq_lut_floats", c_int, [_H]),
+    ("rsb_pq_tables", c_int, [_H, c_void_p, c_int, c_void_p, c_void_p]),
     ("rsb_pq_layout_offset", c_int, [c_int, c_int, c_int]),
     ("rsb_pq_lut_index", c_int, [c_int, c_int, c_int]),
 ]

@@ -57,7 +57,10 @@ struct Segment {
 };
 
 struct rsb_index {
-    int kind = 0, d = 0, nlist = 0, M = 0, nbits = 0, dsub = 0;
+    // IVFPQ: M sub-quantizers of nbits bits each (faiss' values: codebook, encoding, training, rsb_info) and
+    // Mb = M * nbits / 8 code bytes per vector (layout, interleave, tables, scan, export).  nbits = 4 packs two codes
+    // per byte and is scanned as an 8-bit index of Mb byte sub-quantizers (rsb_ivf.cu, pq_lut4_kernel).
+    int kind = 0, d = 0, nlist = 0, M = 0, nbits = 0, dsub = 0, Mb = 0;
     int dtype = RSB_DTYPE_F32;   // storage of FLAT / IVFFLAT rows: RSB_DTYPE_F32 or RSB_DTYPE_F16
     float* centroids = nullptr;
     float* codebook = nullptr;
@@ -95,7 +98,8 @@ struct rsb_index {
     unsigned long long* prof_dev = nullptr;  // [4]: scan elements, pairs, scan path flag, re-scored vectors
     long launches = 0;
     int elem_bytes() const { return dtype == RSB_DTYPE_F16 ? 2 : 4; }
-    size_t row_bytes() const { return kind == RSB_IVFPQ ? (size_t)M : (size_t)d * elem_bytes(); }
+    size_t row_bytes() const { return kind == RSB_IVFPQ ? (size_t)Mb : (size_t)d * elem_bytes(); }
+    int ksub() const { return 1 << nbits; }
 };
 
 static void free_segment(Segment& s) {
@@ -128,14 +132,17 @@ static int create_common(int kind, int d, int nlist, int M, int nbits, rsb_index
     }
     if (kind != RSB_FLAT && nlist <= 0) return fail(RSB_ERR_INVALID, "nlist must be > 0, got %d", nlist);
     if (kind == RSB_IVFPQ) {
-        if (nbits != 8) return fail(RSB_ERR_UNSUPPORTED, "only nbits = 8 is implemented, got %d", nbits);
+        if (nbits != 8 && nbits != 4) return fail(RSB_ERR_UNSUPPORTED, "nbits must be 8 or 4, got %d", nbits);
         if (M <= 0 || d % M) return fail(RSB_ERR_INVALID, "d = %d is not divisible by M = %d", d, M);
-        if (!pq_interleaved_layout(M) && ((M & 3) || M > 128))
+        if (nbits == 8 && !pq_interleaved_layout(M) && ((M & 3) || M > 128))
             return fail(RSB_ERR_UNSUPPORTED, "n_subquantizers must be 16, 32, 64 (tuned path) or a multiple of 4 up to 128 (got %d)", M);
+        if (nbits == 4 && ((M & 7) || M / 2 > 128))
+            return fail(RSB_ERR_INVALID, "4-bit codes need M %% 8 == 0 and M / 2 <= 128 code bytes (got M = %d)", M);
     }
     rsb_index* h = new rsb_index();
     h->kind = kind; h->d = d; h->nlist = kind == RSB_FLAT ? 1 : nlist; h->M = M; h->nbits = nbits; h->dtype = dtype;
     h->dsub = M ? d / M : 0;
+    h->Mb = M * nbits / 8;
     for (auto& set : h->evs) for (auto& e : set) cudaEventCreate(&e);
     if (cudaMalloc(&h->prof_dev, 32) != cudaSuccess) { delete h; return fail(RSB_ERR_OOM, "cudaMalloc failed"); }
     cudaMemset(h->prof_dev, 0, 32);
@@ -153,6 +160,12 @@ extern "C" int rsb_ivfflat_create_dtype(int d, int nlist, int dtype, rsb_index_t
     return create_common(RSB_IVFFLAT, d, nlist, 0, 0, out, dtype);
 }
 extern "C" int rsb_ivfpq_create(int d, int nlist, int M, int nbits, rsb_index_t** out) {
+    if (out) *out = nullptr;
+    if (nbits != 8)
+        return fail(RSB_ERR_UNSUPPORTED, "rsb_ivfpq_create takes nbits = 8 only, got %d (4-bit codes: rsb_ivfpq_create_nbits)", nbits);
+    return create_common(RSB_IVFPQ, d, nlist, M, nbits, out);
+}
+extern "C" int rsb_ivfpq_create_nbits(int d, int nlist, int M, int nbits, rsb_index_t** out) {
     return create_common(RSB_IVFPQ, d, nlist, M, nbits, out);
 }
 extern "C" int rsb_free(rsb_index_t* h) {
@@ -189,12 +202,14 @@ extern "C" int rsb_set_pq_codebook(rsb_index_t* h, const float* cb, rsb_stream_t
     if (h->kind != RSB_IVFPQ) return fail(RSB_ERR_INVALID, "not an IVFPQ index");
     if (h->ntotal || h->n_staged) return fail(RSB_ERR_STATE, "cannot change the codebook of a populated index");
     cudaStream_t st = (cudaStream_t)stream;
-    const size_t bytes = (size_t)h->M * 256 * h->dsub * 4;
+    const size_t bytes = (size_t)h->M * h->ksub() * h->dsub * 4;
     if (!h->codebook) CU(cudaMalloc(&h->codebook, bytes));
-    if (!h->codebook_t) CU(cudaMalloc(&h->codebook_t, bytes));
     CU(cudaMemcpyAsync(h->codebook, cb, bytes, cudaMemcpyDeviceToDevice, st));
-    launch_codebook_transpose(h->codebook, h->M, h->dsub, h->codebook_t, st);
-    CHECK_LAUNCH();
+    if (h->nbits == 8) {   // the 8-bit table kernels read the codebook transposed; pq_lut4_kernel reads it as stored
+        if (!h->codebook_t) CU(cudaMalloc(&h->codebook_t, bytes));
+        launch_codebook_transpose(h->codebook, h->M, h->dsub, h->codebook_t, st);
+        CHECK_LAUNCH();
+    }
     h->has_codebook = true;
     return RSB_OK;
 }
@@ -207,7 +222,7 @@ extern "C" int rsb_get_centroids(rsb_index_t* h, float* out, rsb_stream_t stream
 extern "C" int rsb_get_pq_codebook(rsb_index_t* h, float* out, rsb_stream_t stream) {
     if (!h || !out) return fail(RSB_ERR_INVALID, "null argument");
     if (!h->has_codebook) return fail(RSB_ERR_STATE, "index has no PQ codebook");
-    CU(cudaMemcpyAsync(out, h->codebook, (size_t)h->M * 256 * h->dsub * 4, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+    CU(cudaMemcpyAsync(out, h->codebook, (size_t)h->M * h->ksub() * h->dsub * 4, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
     return RSB_OK;
 }
 
@@ -413,8 +428,11 @@ static int add_impl(rsb_index* h, const void* x, int x_dtype, const uint8_t* cod
         }
     }
     if (h->kind == RSB_IVFPQ) {
-        CUB_(cudaMalloc(&seg.payload, (size_t)n * h->M));
-        if (codes_in) CUB_(cudaMemcpyAsync(seg.payload, codes_in, (size_t)n * h->M, cudaMemcpyDeviceToDevice, st));
+        CUB_(cudaMalloc(&seg.payload, (size_t)n * h->Mb));
+        if (codes_in) CUB_(cudaMemcpyAsync(seg.payload, codes_in, (size_t)n * h->Mb, cudaMemcpyDeviceToDevice, st));
+        else if (h->nbits == 4)
+            launch_pq_encode4(static_cast<const float*>(x), n, h->d, seg.list, h->centroids, h->codebook, h->M, true,
+                              static_cast<uint8_t*>(seg.payload), st);
         else launch_pq_encode(static_cast<const float*>(x), n, h->d, seg.list, h->centroids, h->codebook, h->M,
                               static_cast<uint8_t*>(seg.payload), st);
     } else {
@@ -624,10 +642,10 @@ extern "C" int rsb_finalize(rsb_index_t* h, rsb_stream_t stream) {
     if (pq) {
         CUF(cudaMalloc(&dst_row, (size_t)n * 8));
         launch_slot_of_sorted(sorted_list, n, h->list_nat_off, h->list_slot_off, dst_row, st);
-        if (pq_interleaved_layout(h->M))
+        if (pq_interleaved_layout(h->Mb))
             launch_pq_interleave(seg_payload_dev, seg_starts_dev, nseg, sorted_src, sorted_list, n, h->list_nat_off,
-                                 h->list_slot_off, h->M, h->payload, st);
-        else   // generic M: natural [slot][M] rows
+                                 h->list_slot_off, h->Mb, h->payload, st);
+        else   // generic M: natural [slot][Mb] rows
             launch_gather_rows(seg_payload_dev, seg_starts_dev, nseg, sorted_src, dst_row, n, (int)rb, h->payload, st);
         launch_gather_ids(seg_ids_dev, seg_starts_dev, nseg, sorted_src, dst_row, n, h->ids_slots, st);
     } else {
@@ -698,10 +716,10 @@ static int export_impl(rsb_index* h, int64_t* offsets, void* payload, int64_t* i
     if (offsets) CU(cudaMemcpyAsync(offsets, h->list_nat_off, (size_t)(h->nlist + 1) * 8, cudaMemcpyDeviceToDevice, st));
     if (h->ntotal == 0) return RSB_OK;
     if (h->kind == RSB_IVFPQ) {
-        if (payload && pq_interleaved_layout(h->M))
-            launch_pq_deinterleave(h->payload, h->list_nat_off, h->list_slot_off, h->list_len, h->nlist, h->M, static_cast<uint8_t*>(payload), st);
+        if (payload && pq_interleaved_layout(h->Mb))
+            launch_pq_deinterleave(h->payload, h->list_nat_off, h->list_slot_off, h->list_len, h->nlist, h->Mb, static_cast<uint8_t*>(payload), st);
         else if (payload)
-            launch_compact_slots_rows(h->payload, h->list_nat_off, h->list_slot_off, h->nlist, h->M, static_cast<uint8_t*>(payload), st);
+            launch_compact_slots_rows(h->payload, h->list_nat_off, h->list_slot_off, h->nlist, h->Mb, static_cast<uint8_t*>(payload), st);
         if (ids) launch_compact_slots_i64(h->ids_slots, h->list_nat_off, h->list_slot_off, h->list_len, h->nlist, ids, st);
         CHECK_LAUNCH();
     } else {
@@ -724,7 +742,7 @@ extern "C" int rsb_export_lists(rsb_index_t* h, int64_t* offsets, void* payload,
 // (read once) scans every (query, list) pair on its own: the reference the tests compare the paired scan against.
 static bool pq_paired_scan(const rsb_index* h) {
     static const bool single = getenv("RSB_PQ_SINGLE_ITEMS") != nullptr;
-    return h->kind == RSB_IVFPQ && pq_interleaved_layout(h->M) && !single;
+    return h->kind == RSB_IVFPQ && pq_interleaved_layout(h->Mb) && !single;
 }
 
 struct SearchPlan {
@@ -749,7 +767,7 @@ static SearchPlan search_plan(const rsb_index* h, int nq, int k, int nprobe) {
     p.off_cD = o;        o += align_up((size_t)qb * p.nprobe * 4);
     p.off_cI = o;        o += align_up((size_t)qb * p.nprobe * 8);
     p.off_pair = o;      o += align_up(pair_work_bytes(qb, p.nprobe, h->nlist));
-    const size_t lut_words = pq_interleaved_layout(h->M) ? (size_t)kLutWords : (size_t)h->M * 256;
+    const size_t lut_words = pq_interleaved_layout(h->Mb) ? (size_t)kLutWords : (size_t)h->Mb * 256;
     p.off_lut = o;       o += h->kind == RSB_IVFPQ ? align_up((size_t)qb * lut_words * 4) : 0;
     const bool paired = pq_paired_scan(h);
     p.off_qlut = o;      o += paired ? align_up((size_t)qb * kLutWords * 2) : 0;
@@ -1005,17 +1023,19 @@ static int search_impl(rsb_index_t* h, const float* q, int nq, int k, int nprobe
 
         if (h->kind == RSB_IVFPQ) {
             float* lut = reinterpret_cast<float*>(w + p.off_lut);
-            if (pq_interleaved_layout(h->M)) launch_pq_lut(qb, nb, h->d, h->M, h->codebook_t, lut, st);
+            // from here on the index is scanned as Mb byte sub-quantizers (Mb = M for 8-bit codes)
+            if (h->nbits == 4) launch_pq_lut4(qb, nb, h->d, h->M, h->codebook, lut, st);
+            else if (pq_interleaved_layout(h->M)) launch_pq_lut(qb, nb, h->d, h->M, h->codebook_t, lut, st);
             else launch_pq_lut_generic(qb, nb, h->d, h->M, h->codebook, lut, st);
             h->launches += 1;
             if (paired) {
-                launch_pq_lut_quant(lut, nb, h->M, reinterpret_cast<unsigned short*>(w + p.off_qlut),
+                launch_pq_lut_quant(lut, nb, h->Mb, reinterpret_cast<unsigned short*>(w + p.off_qlut),
                                     reinterpret_cast<PQQuant*>(w + p.off_quant), st);
                 h->launches += 1;
             }
             if (prof) CU(cudaEventRecord(h->ev[3], st));
-            if (launch_ivfpq_scan(a, lut, h->payload, h->M, nb, st) != 0)
-                return fail(RSB_ERR_UNSUPPORTED, "no scan kernel for M = %d", h->M);
+            if (launch_ivfpq_scan(a, lut, h->payload, h->Mb, nb, st) != 0)
+                return fail(RSB_ERR_UNSUPPORTED, "no scan kernel for %d code bytes per vector", h->Mb);
         } else {
             if (prof) CU(cudaEventRecord(h->ev[3], st));
             launch_ivfflat_scan(a, qb, h->payload, h->elem_bytes(), h->d, nb, st);
@@ -1415,15 +1435,26 @@ extern "C" int rsb_kmeans_accumulate(const float* x, int64_t n, int d, const int
 }
 extern "C" int rsb_pq_assign(const float* r, int64_t n, int d, int M, const float* codebook, uint8_t* codes,
                              rsb_stream_t stream) {
-    if (!r || !codebook || !codes || n < 0 || d <= 0 || M <= 0 || d % M) return fail(RSB_ERR_INVALID, "bad argument");
-    launch_pq_encode(r, n, d, nullptr, nullptr, codebook, M, codes, (cudaStream_t)stream);
-    CHECK_LAUNCH();
-    return RSB_OK;
+    return rsb_pq_assign_ksub(r, n, d, M, 256, codebook, codes, stream);
 }
 extern "C" int rsb_pq_accumulate(const float* r, int64_t n, int d, int M, const uint8_t* codes, float* sums, float* counts,
                                  rsb_stream_t stream) {
+    return rsb_pq_accumulate_ksub(r, n, d, M, 256, codes, sums, counts, stream);
+}
+extern "C" int rsb_pq_assign_ksub(const float* r, int64_t n, int d, int M, int ksub, const float* codebook, uint8_t* codes,
+                                  rsb_stream_t stream) {
+    if (!r || !codebook || !codes || n < 0 || d <= 0 || M <= 0 || d % M) return fail(RSB_ERR_INVALID, "bad argument");
+    if (ksub != 256 && ksub != 16) return fail(RSB_ERR_UNSUPPORTED, "ksub must be 256 or 16 (nbits 8 or 4), got %d", ksub);
+    if (ksub == 16) launch_pq_encode4(r, n, d, nullptr, nullptr, codebook, M, false, codes, (cudaStream_t)stream);
+    else launch_pq_encode(r, n, d, nullptr, nullptr, codebook, M, codes, (cudaStream_t)stream);
+    CHECK_LAUNCH();
+    return RSB_OK;
+}
+extern "C" int rsb_pq_accumulate_ksub(const float* r, int64_t n, int d, int M, int ksub, const uint8_t* codes, float* sums,
+                                      float* counts, rsb_stream_t stream) {
     if (!r || !codes || !sums || !counts || n < 0 || d <= 0 || M <= 0 || d % M) return fail(RSB_ERR_INVALID, "bad argument");
-    const cudaError_t e = launch_pq_accumulate(r, n, d, M, codes, sums, counts, (cudaStream_t)stream);
+    if (ksub != 256 && ksub != 16) return fail(RSB_ERR_UNSUPPORTED, "ksub must be 256 or 16 (nbits 8 or 4), got %d", ksub);
+    const cudaError_t e = launch_pq_accumulate(r, n, d, M, ksub, codes, sums, counts, (cudaStream_t)stream);
     if (e != cudaSuccess) return fail(e == cudaErrorMemoryAllocation ? RSB_ERR_OOM : RSB_ERR_CUDA, "%s", cudaGetErrorString(e));
     CHECK_LAUNCH();
     return RSB_OK;
@@ -1520,6 +1551,22 @@ extern "C" int rsb_get_profile(rsb_index_t* h, double* out, int n) {
 }
 
 extern "C" int rsb_debug_smem_base(void) { return (int)probe_dynamic_smem_base(0); }
+
+extern "C" int rsb_pq_lut_floats(rsb_index_t* h) {
+    if (!h || h->kind != RSB_IVFPQ) return -1;
+    return pq_interleaved_layout(h->Mb) ? kLutWords : h->Mb * 256;
+}
+extern "C" int rsb_pq_tables(rsb_index_t* h, const float* q, int nq, float* lut, rsb_stream_t stream) {
+    if (!h || h->kind != RSB_IVFPQ) return fail(RSB_ERR_INVALID, "rsb_pq_tables needs an IVFPQ index");
+    if (nq < 0 || (nq > 0 && (!q || !lut))) return fail(RSB_ERR_INVALID, "null argument");
+    if (!h->has_codebook) return fail(RSB_ERR_STATE, "index has no PQ codebook");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (h->nbits == 4) launch_pq_lut4(q, nq, h->d, h->M, h->codebook, lut, st);
+    else if (pq_interleaved_layout(h->M)) launch_pq_lut(q, nq, h->d, h->M, h->codebook_t, lut, st);
+    else launch_pq_lut_generic(q, nq, h->d, h->M, h->codebook, lut, st);
+    CHECK_LAUNCH();
+    return RSB_OK;
+}
 
 extern "C" int rsb_pq_layout_offset(int M, int v, int m) {
     if (v < 0 || v >= 32 || m < 0 || m >= M) return -1;

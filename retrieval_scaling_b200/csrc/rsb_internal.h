@@ -221,11 +221,20 @@ void launch_codebook_transpose(const float* cb, int M, int dsub, float* cbT, cud
 // residual PQ encoding: codes[n, M] = argmin_j || (x - centroid[list])_m - cb[m][j] ||^2
 void launch_pq_encode(const float* x, int64_t n, int d, const int32_t* list, const float* centroids,
                       const float* codebook, int M, uint8_t* codes, cudaStream_t st);
+// 4-bit sub-quantizers (nbits = 4, M_b = M / 2 code bytes per vector), codebook [M, 16, dsub] as stored.
+// Table of the byte sub-quantizers T'[b][j] = T[2b][j & 15] + T[2b+1][j >> 4], written in the layout the scan of M_b
+// bytes reads: [nq, 256, 64] when pq_interleaved_layout(M_b), else [nq][M_b][256].
+void launch_pq_lut4(const float* queries, int nq, int d, int M, const float* codebook, float* lut, cudaStream_t st);
+// nearest of the 16 entries per sub-quantizer (x - centroid[list]; list null: x is the residual).  packed: codes
+// [n, M/2] with byte b = c[2b] | c[2b+1] << 4 (faiss PQEncoderGeneric order); else codes [n, M], one code per byte.
+void launch_pq_encode4(const float* x, int64_t n, int d, const int32_t* list, const float* centroids,
+                       const float* codebook, int M, bool packed, uint8_t* codes, cudaStream_t st);
 // k-means update steps of index.train(): member sums / counts (float atomics)
 cudaError_t launch_kmeans_accumulate(const float* x, int64_t n, int d, const int32_t* assign, int k, float* sums, float* counts,
                               cudaStream_t st);
-cudaError_t launch_pq_accumulate(const float* r, int64_t n, int d, int M, const uint8_t* codes, float* sums, float* counts,
-                          cudaStream_t st);
+// codes [n, M] one code per byte (< ksub; larger codes are skipped); sums [M, ksub, d/M], counts [M, ksub]
+cudaError_t launch_pq_accumulate(const float* r, int64_t n, int d, int M, int ksub, const uint8_t* codes, float* sums,
+                                 float* counts, cudaStream_t st);
 // natural codes -> interleaved blocks (see rsb_layout.h).  src_row[i] = row in `codes_nat` of the i-th vector in
 // list-sorted order; rank/list via list_of_sorted + list_nat_off.
 void launch_pq_interleave(const uint8_t* const* seg_ptrs, const int64_t* seg_starts, int nseg,

@@ -566,6 +566,70 @@ void launch_pq_lut_quant(const float* lut, int nq, int M, unsigned short* qlut, 
 }
 
 // =============================================================================================================
+// 4-bit sub-quantizers (faiss nbits = 4).  Codes are packed two per byte, LSB first (faiss PQEncoderGeneric): byte b
+// of a code is c[2b] | c[2b+1] << 4.  Grouping the M sub-quantizers in pairs gives one 256-entry table per code byte,
+//        T'[b][j] = T[2b][j & 15] + T[2b+1][j >> 4]          (one fp32 rounding per entry)
+// and score = dis0 + sum_b T'[b][byte_b]: an 8-bit table over M_b = M / 2 "byte sub-quantizers".  A 4-bit index is
+// therefore stored, interleaved, quantised (pq_lut_quant_kernel) and scanned exactly like an 8-bit index of M_b
+// sub-quantizers; only the table build below and the encoder are specific to it.
+// =============================================================================================================
+// One block per query.  Phase 1: the M x 16 sub-products <q_m, cb[m][c]> (sequential fmaf over dsub, the order of the
+// 8-bit table kernels), kept in shared memory split by parity of m -- E[c][b] = T[2b][c], O[c][b] = T[2b+1][c] -- so
+// that in phase 2 consecutive lanes (consecutive b) read consecutive banks.  Phase 2 writes T' straight into the
+// scan's table layout: IL = the interleaved [j][64 words] rows (word w holds byte sub-quantizer w % M_b, replicated
+// when M_b < 64), else the generic [b][256] table.
+template <bool IL>
+__global__ __launch_bounds__(256)
+void pq_lut4_kernel(const float* __restrict__ queries, int d, int M, const float* __restrict__ codebook,
+                    float* __restrict__ lut) {
+    extern __shared__ __align__(16) float s_lut4[];          // query [d] | E [16][M/2] | O [16][M/2]
+    const int q = blockIdx.x, dsub = d / M, Mb = M >> 1;
+    float* qs = s_lut4;
+    float* E = s_lut4 + d;
+    float* O = E + 16 * Mb;
+    for (int c = threadIdx.x; c < d; c += blockDim.x) qs[c] = queries[(size_t)q * d + c];
+    __syncthreads();
+    for (int i = threadIdx.x; i < M * 16; i += blockDim.x) {
+        const int m = i >> 4, c = i & 15;
+        const float* cb = codebook + (size_t)i * dsub;          // cb[m][c] of [M, 16, dsub]
+        const float* x = qs + m * dsub;
+        float s = 0.f;
+        for (int t = 0; t < dsub; ++t) s = fmaf(x[t], __ldg(cb + t), s);
+        ((m & 1) ? O : E)[c * Mb + (m >> 1)] = s;
+    }
+    __syncthreads();
+    if (IL) {
+        float* out = lut + (size_t)q * kLutWords;
+        for (int i = threadIdx.x; i < kLutWords; i += blockDim.x) {
+            const int j = i / kLutRowWords, b = (i % kLutRowWords) % Mb;
+            out[i] = E[(j & 15) * Mb + b] + O[(j >> 4) * Mb + b];
+        }
+    } else {
+        float* out = lut + (size_t)q * Mb * 256;
+        for (int i = threadIdx.x; i < Mb * 256; i += blockDim.x) {
+            const int b = i >> 8, j = i & 255;
+            out[i] = E[(j & 15) * Mb + b] + O[(j >> 4) * Mb + b];
+        }
+    }
+}
+
+void launch_pq_lut4(const float* queries, int nq, int d, int M, const float* codebook, float* lut, cudaStream_t st) {
+    if (nq <= 0) return;
+    const size_t smem = ((size_t)d + 16 * (size_t)M) * 4;
+    if (pq_interleaved_layout(M / 2)) {
+        static PerDeviceSize configured;
+        if (smem > 48 * 1024 && configured.raise(smem))
+            cudaFuncSetAttribute(pq_lut4_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        pq_lut4_kernel<true><<<nq, 256, smem, st>>>(queries, d, M, codebook, lut);
+    } else {
+        static PerDeviceSize configured;
+        if (smem > 48 * 1024 && configured.raise(smem))
+            cudaFuncSetAttribute(pq_lut4_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        pq_lut4_kernel<false><<<nq, 256, smem, st>>>(queries, d, M, codebook, lut);
+    }
+}
+
+// =============================================================================================================
 // IVF-PQ ADC list scan -- the hot kernel.  score(code) = dis0 + sum_m T[m][code[m]].
 //
 // One block (256 threads, 8 warps) per item; persistent blocks pull items (sorted by list, so
@@ -1365,6 +1429,52 @@ void launch_pq_encode(const float* x, int64_t n, int d, const int32_t* list, con
     }
 }
 
+// 4-bit residual encoding: nearest of the 16 entries of each sub-quantizer (L2, the arithmetic and the first-minimum
+// tie rule of pq_encode_kernel).  grid (row tiles of 128, M / 2 when packed, else M); a block stages the 16 x dsub
+// codebooks of the sub-quantizers it encodes.  packed: codes [n, M/2], byte b = c[2b] | c[2b+1] << 4 (faiss order);
+// unpacked (PQ training's assignment step): codes [n, M], one code per byte.
+__global__ __launch_bounds__(128)
+void pq_encode4_kernel(const float* __restrict__ x, int64_t n, int d, const int32_t* __restrict__ list,
+                       const float* __restrict__ centroids, const float* __restrict__ codebook, int M, int packed,
+                       uint8_t* __restrict__ codes) {
+    extern __shared__ __align__(16) float cb4_s[];           // [per][16][dsub]
+    const int dsub = d / M, per = packed ? 2 : 1, m0 = blockIdx.y * per;
+    for (int i = threadIdx.x; i < per * 16 * dsub; i += blockDim.x) cb4_s[i] = codebook[(size_t)m0 * 16 * dsub + i];
+    __syncthreads();
+    const int64_t row = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (row >= n) return;
+    unsigned byte = 0;
+    for (int h = 0; h < per; ++h) {
+        const int m = m0 + h;
+        const float* xr = x + (size_t)row * d + m * dsub;
+        const float* cr = list ? centroids + (size_t)list[row] * d + m * dsub : nullptr;
+        float best = FLT_MAX;
+        int bj = 0;
+        for (int j = 0; j < 16; ++j) {
+            float dist = 0.f;
+            for (int t = 0; t < dsub; ++t) {
+                const float r = cr ? xr[t] - __ldg(cr + t) : xr[t];
+                const float df = r - cb4_s[(h * 16 + j) * dsub + t];
+                dist = fmaf(df, df, dist);
+            }
+            if (dist < best) { best = dist; bj = j; }
+        }
+        byte |= (unsigned)bj << (4 * h);
+    }
+    codes[(size_t)row * (M / per) + blockIdx.y] = (uint8_t)byte;
+}
+
+void launch_pq_encode4(const float* x, int64_t n, int d, const int32_t* list, const float* centroids,
+                       const float* codebook, int M, bool packed, uint8_t* codes, cudaStream_t st) {
+    if (n <= 0) return;
+    const size_t smem = (size_t)(packed ? 2 : 1) * 16 * (d / M) * 4;
+    static PerDeviceSize configured;
+    if (smem > 48 * 1024 && configured.raise(smem))
+        cudaFuncSetAttribute(pq_encode4_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    dim3 grid((unsigned)((n + 127) / 128), packed ? M / 2 : M);
+    pq_encode4_kernel<<<grid, 128, smem, st>>>(x, n, d, list, centroids, codebook, M, packed ? 1 : 0, codes);
+}
+
 // =============================================================================================================
 // k-means update steps (index.train(): faiss Clustering for the coarse quantizer, ProductQuantizer::train for the
 // PQ codebooks; reference call sites src/indicies/ivf_flat.py:166, ivf_pq.py:170).  The assignment steps are the
@@ -1373,12 +1483,13 @@ void launch_pq_encode(const float* x, int64_t n, int d, const int32_t* list, con
 // Member sums in a fixed order, so that training gives the same centroids / codebooks on every run: the members are
 // grouped by cluster with a stable radix sort (ties keep ascending row order), then one warp per cluster adds its
 // members' rows in ascending row order.  An "item" is one row (k-means: key = its cluster, its vector = x[item]) or one
-// (row, sub-quantizer) pair (PQ: key = m * 256 + code, its vector = the m-th sub-vector of the row).
+// (row, sub-quantizer) pair (PQ: key = m * ksub + code, its vector = the m-th sub-vector of the row).
 __global__ void accumulate_keys_kernel(int64_t nitems, int M, const int32_t* __restrict__ assign, int k,
-                                       const uint8_t* __restrict__ codes, int32_t* __restrict__ keys, int64_t* __restrict__ items) {
+                                       const uint8_t* __restrict__ codes, int ksub, int32_t* __restrict__ keys,
+                                       int64_t* __restrict__ items) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nitems; i += (int64_t)gridDim.x * blockDim.x) {
         int key;
-        if (codes) key = (int)(i % M) * 256 + codes[i];
+        if (codes) key = codes[i] < ksub ? (int)(i % M) * ksub + codes[i] : M * ksub;   // codes >= ksub: ignored
         else key = (assign[i] >= 0 && assign[i] < k) ? assign[i] : k;      // out-of-range assignments: ignored
         keys[i] = key;
         items[i] = i;
@@ -1431,7 +1542,7 @@ static cudaError_t accumulate_sorted(const float* x, int64_t n, int d, int M, co
     if (e == cudaSuccess) e = cudaMallocAsync(&tmp, tmp_bytes, st);
     if (e == cudaSuccess) {
         const int blocks = (int)std::min<int64_t>(8 * (int64_t)num_sms(), (nitems + 255) / 256);
-        accumulate_keys_kernel<<<blocks, 256, 0, st>>>(nitems, M, assign, k, codes, keys, items);
+        accumulate_keys_kernel<<<blocks, 256, 0, st>>>(nitems, M, assign, k, codes, nkeys / M, keys, items);
         e = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, keys_sorted, items, items_sorted, nitems, 0, bits, st);
     }
     if (e == cudaSuccess) e = cudaMemsetAsync(bounds, 0, (size_t)nkeys * 2 * 8, st);
@@ -1458,11 +1569,11 @@ cudaError_t launch_kmeans_accumulate(const float* x, int64_t n, int d, const int
     return accumulate_sorted(x, n, d, 1, assign, k, nullptr, k, sums, counts, st);
 }
 
-// PQ: sums[m, code, :] += r[row, m*dsub : (m+1)*dsub], counts[m, code] += 1
-cudaError_t launch_pq_accumulate(const float* r, int64_t n, int d, int M, const uint8_t* codes, float* sums, float* counts,
-                                 cudaStream_t st) {
+// PQ: sums[m, code, :] += r[row, m*dsub : (m+1)*dsub], counts[m, code] += 1  (sums [M, ksub, dsub], counts [M, ksub])
+cudaError_t launch_pq_accumulate(const float* r, int64_t n, int d, int M, int ksub, const uint8_t* codes, float* sums,
+                                 float* counts, cudaStream_t st) {
     if (n <= 0) return cudaSuccess;
-    return accumulate_sorted(r, n, d, M, nullptr, 0, codes, M * 256, sums, counts, st);
+    return accumulate_sorted(r, n, d, M, nullptr, 0, codes, M * ksub, sums, counts, st);
 }
 
 // =============================================================================================================

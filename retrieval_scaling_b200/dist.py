@@ -175,6 +175,10 @@ class ShardedSearcher:
             raise NotImplementedError("ShardedSearcher partitions one index over the GPUs; re-ranking would need the "
                                       "candidates' store rows from peer GPUs, which is not implemented.  Re-rank per "
                                       "shard group instead (search.GroupSearcher) or search on one GPU")
+        if int(world) > 1 and getattr(index, "nbits", 8) != 8:
+            raise NotImplementedError(f"ShardedSearcher over several GPUs is implemented for nbits = 8 IVF-PQ indexes; this "
+                                      f"index has nbits = {index.nbits}.  Search it per shard group (search.GroupSearcher) "
+                                      f"or on one GPU")
         self.sliced_merge = bool(sliced_merge)
         # with the fused (symmetric-memory) gather: exchange the running top-k thresholds between the GPUs during the
         # scan, and publish the sharded coarse tables with P2P stores instead of NCCL all-gathers

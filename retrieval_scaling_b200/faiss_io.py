@@ -151,7 +151,8 @@ def _read_ivf_header(f: BinaryIO) -> Dict:
 
 def read_faiss(f) -> Dict:
     """Parses a faiss index file (path or binary stream) into plain numpy parts:
-    Flat: xb [n,d];  IVFFlat: centroids, offsets, vectors [n,d], ids;  IVFPQ: + codebook [M,256,dsub], codes [n,M]."""
+    Flat: xb [n,d];  IVFFlat: centroids, offsets, vectors [n,d], ids;  IVFPQ: + codebook [M,2^nbits,dsub], codes
+    [n, code_size] as stored (code_size = M * nbits / 8: 4-bit codes stay packed two per byte, faiss' order)."""
     if isinstance(f, (str, bytes)):
         with open(f, "rb") as fh:
             return read_faiss(fh)

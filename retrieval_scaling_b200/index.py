@@ -212,7 +212,8 @@ class _IndexBase:
             nlist = max(1, self._info(_lib.INFO_NLIST))
             off = torch.zeros(nlist + 1, dtype=torch.int64, device=self.device)
             if self.kind == _lib.RSB_IVFPQ:
-                payload = torch.empty((n, self._info(_lib.INFO_M)), dtype=torch.uint8, device=self.device)
+                code_size = self._info(_lib.INFO_M) * self._info(_lib.INFO_NBITS) // 8
+                payload = torch.empty((n, code_size), dtype=torch.uint8, device=self.device)
             else:
                 payload = torch.empty((n, self.d), dtype=_STORE_DTYPES[self.dtype][0], device=self.device)
             ids = torch.empty(n, dtype=torch.int64, device=self.device)
@@ -348,14 +349,21 @@ class IndexIVFFlat(_IVFBase):
 
 
 class IndexIVFPQ(_IVFBase):
-    """faiss.IndexIVFPQ(IndexFlatIP(d), d, nlist, M, nbits, METRIC_INNER_PRODUCT)  (src/indicies/ivf_pq.py:146-152)."""
+    """faiss.IndexIVFPQ(IndexFlatIP(d), d, nlist, M, nbits, METRIC_INNER_PRODUCT)  (src/indicies/ivf_pq.py:146-152).
+
+    nbits 8 or 4.  4-bit codes are packed two per byte in faiss' order (byte b = c[2b] | c[2b+1] << 4), so `code_size`
+    = M * nbits / 8 bytes per vector: codes taken by `add_codes` and returned by `export_lists` are [n, code_size]."""
     kind = _lib.RSB_IVFPQ
 
     def __init__(self, d: int, nlist: int, M: int, nbits: int = 8, device=None):
         super().__init__(d, nlist, device)
         self.M, self.nbits = int(M), int(nbits)
         with torch.cuda.device(self.device):
-            _lib.check(self.L.rsb_ivfpq_create(self.d, self.nlist, self.M, self.nbits, ctypes.byref(self._h)))
+            _lib.check(self.L.rsb_ivfpq_create_nbits(self.d, self.nlist, self.M, self.nbits, ctypes.byref(self._h)))
+
+    @property
+    def code_size(self) -> int:
+        return self.M * self.nbits // 8
 
     def set_codebook(self, cb) -> None:
         with torch.cuda.device(self.device):
@@ -386,6 +394,9 @@ class IndexIVFPQ(_IVFBase):
         with torch.cuda.device(self.device):
             ct = torch.as_tensor(codes).to(device=self.device, dtype=torch.uint8).contiguous()
             n = ct.shape[0]
+            if ct.dim() != 2 or ct.shape[1] != self.code_size:
+                raise ValueError(f"codes must be [n, {self.code_size}] uint8 (M * nbits / 8 bytes per vector), "
+                                 f"got {tuple(ct.shape)}")
             lt = torch.as_tensor(lists).to(device=self.device, dtype=torch.int32).contiguous()
             idt = None if ids is None else torch.as_tensor(ids).to(device=self.device, dtype=torch.int64).contiguous()
             _lib.check(self.L.rsb_add_codes(self._h, _ptr(ct), n, _ptr(idt), _ptr(lt), _stream()))

@@ -4,14 +4,14 @@ Restates what `index.train(x)` does in the reference's call sites (`src/indicies
 `src/indicies/ivf_pq.py:170`) with faiss 1.8.0 defaults: Level-1 clustering niter=10, at most 256 training
 points per centroid, seed 1234, *spherical* because the metric is inner product (the IndexIVF constructor sets
 `cp.spherical = true` for METRIC_INNER_PRODUCT: centroids L2-normalised every iteration, assignment by max inner
-product through the IndexFlatIP quantizer); PQ sub-quantizers: L2 k-means, ksub=256, niter=25, on residuals of at
-most 256*ksub points.  Parity is defined *given* the trained centroids / codebooks (SURVEY §8a row a10).
+product through the IndexFlatIP quantizer); PQ sub-quantizers: L2 k-means, ksub=256 (or 16 for 4-bit codes), niter=25,
+on residuals of at most 256*ksub points.  Parity is defined *given* the trained centroids / codebooks (SURVEY §8a row a10).
 
 The Lloyd iterations are driven from here; the arithmetic of every step runs in librsb (`LibrsbOps`):
   assignment (coarse)  : the coarse quantizer itself -- fused 3xTF32 wgmma scorer + exact fp32 re-score (rsb_coarse on a
                          scratch handle holding the current centroids) -> fp32-exact argmax
-  assignment (PQ)      : rsb_pq_assign (the residual-encoding kernel without the residual step)
-  update               : rsb_kmeans_accumulate / rsb_pq_accumulate (member sums and counts)
+  assignment (PQ)      : rsb_pq_assign_ksub (the residual-encoding kernel without the residual step)
+  update               : rsb_kmeans_accumulate / rsb_pq_accumulate_ksub (member sums and counts)
 torch only divides sums by counts, normalises and re-seeds empty clusters (O(k d) element-wise work) and draws the
 random subsets.  There is no CPU path: `LibrsbOps` raises without CUDA; the CPU unit tests of the host logic pass
 their own numpy stand-in for the three operations (tests/test_train_cpu.py).
@@ -66,14 +66,16 @@ class LibrsbOps:
         return sums, counts
 
     def pq_assign(self, r: torch.Tensor, cb: torch.Tensor) -> torch.Tensor:
-        """codes uint8 [n, M]: nearest (L2) codebook entry of every sub-vector; cb [M, 256, dsub]."""
+        """codes uint8 [n, M] (one code per byte): nearest (L2) codebook entry of every sub-vector; cb [M, ksub, dsub],
+        ksub 256 or 16."""
         from . import _lib
         n, d = r.shape
-        M = cb.shape[0]
+        M, ksub = cb.shape[0], cb.shape[1]
         codes = torch.empty(n, M, dtype=torch.uint8, device=r.device)
         with torch.cuda.device(r.device):
-            _lib.check(_lib.lib().rsb_pq_assign(ctypes.c_void_p(r.data_ptr()), n, d, M, ctypes.c_void_p(cb.contiguous().data_ptr()),
-                                                ctypes.c_void_p(codes.data_ptr()), self._st()))
+            _lib.check(_lib.lib().rsb_pq_assign_ksub(ctypes.c_void_p(r.data_ptr()), n, d, M, ksub,
+                                                     ctypes.c_void_p(cb.contiguous().data_ptr()),
+                                                     ctypes.c_void_p(codes.data_ptr()), self._st()))
         return codes
 
     def pq_accumulate(self, r: torch.Tensor, codes: torch.Tensor, M: int, ksub: int):
@@ -82,8 +84,9 @@ class LibrsbOps:
         sums = torch.zeros(M, ksub, d // M, dtype=torch.float32, device=r.device)
         counts = torch.zeros(M, ksub, dtype=torch.float32, device=r.device)
         with torch.cuda.device(r.device):
-            _lib.check(_lib.lib().rsb_pq_accumulate(ctypes.c_void_p(r.data_ptr()), n, d, M, ctypes.c_void_p(codes.data_ptr()),
-                                                    ctypes.c_void_p(sums.data_ptr()), ctypes.c_void_p(counts.data_ptr()), self._st()))
+            _lib.check(_lib.lib().rsb_pq_accumulate_ksub(ctypes.c_void_p(r.data_ptr()), n, d, M, ksub,
+                                                         ctypes.c_void_p(codes.data_ptr()), ctypes.c_void_p(sums.data_ptr()),
+                                                         ctypes.c_void_p(counts.data_ptr()), self._st()))
         return sums, counts
 
 
@@ -145,9 +148,9 @@ def kmeans(x: torch.Tensor, k: int, niter: int = 10, metric: str = "ip", spheric
 
 
 def train_pq(residuals: torch.Tensor, M: int, ksub: int = 256, niter: int = 25, seed: int = 1234, ops=None) -> torch.Tensor:
-    """residuals [n, d] -> codebook [M, ksub, d/M]; M independent L2 k-means."""
-    if ksub != 256:
-        raise NotImplementedError("only 8-bit sub-quantizers (ksub = 256) are implemented")
+    """residuals [n, d] -> codebook [M, ksub, d/M]; M independent L2 k-means.  ksub 256 (nbits 8) or 16 (nbits 4)."""
+    if ksub not in (256, 16):
+        raise NotImplementedError(f"ksub = {ksub}: only 8-bit (256) and 4-bit (16) sub-quantizers are implemented")
     ops = ops or default_ops()
     r = residuals.float()
     n, d = r.shape

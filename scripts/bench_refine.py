@@ -39,7 +39,18 @@ index in the same run.  With either set to something other than a lone float16 s
 under "stores": dtype, device / host bytes, build seconds, and per --store-nq batch size the refined QPS, the re-rank
 kernel milliseconds and gathered GB/s (nq x k' x d x element bytes over the kernel time), with recall@k, exact
 top-1 / top-10 and parity at the largest batch.  With --device-rows the same options apply to the tiered store (the
-comparison store is then all-device and must be byte-identical for sq8 vs sq8 only)."""
+comparison store is then all-device and must be byte-identical for sq8 vs sq8 only).
+
+    python scripts/bench_refine.py --n 20000000 --k-factor 8 --pq-arms 64x8,64x4,128x4
+
+--pq-arms builds one IVF-PQ index per arm MxNBITS (4-bit codes: two per byte, faiss' packing) on the same corpus and
+coarse centroids, and one fp16 and one sq8 re-rank store shared by all arms (the re-rank depends on the candidates only).
+Per --store-nq batch size the arms are measured one after the other (alternated), each unrefined and refined from both
+stores (base search at k' = k * k_factor, then the re-rank kernel: rsb_search_refine gives the same result in one call).
+Per arm: QPS, the LUT and scan milliseconds of the base search (RSB_PROF), recall@k / top-1 / top-10 at the largest batch,
+build seconds, and the parity block (the re-rank against oracle/refine_oracle.py as above, plus every pair of the
+unrefined result re-scored in float64 from the exported codes, oracle/pq4_oracle.py).  --nbits applies to the other
+modes' single index (default 8: bench.py's index)."""
 import argparse
 import json
 import os
@@ -80,6 +91,8 @@ def parse():
                     help="all-device runs: also build a store of this dtype on the same index")
     ap.add_argument("--store-nq", default="10000,64,1", help="batch sizes reported per store (--store-dtype / --compare-store)")
     ap.add_argument("--sq-train-rows", type=int, default=1_000_000, help="sq8: corpus rows the quantizer is trained on")
+    ap.add_argument("--nbits", type=int, default=8, choices=(8, 4), help="bits per sub-quantizer of the single index")
+    ap.add_argument("--pq-arms", default=None, help="compare IVF-PQ arms MxNBITS, e.g. 64x8,64x4,128x4")
     a = ap.parse_args()
     a.partition = "list"
     return a
@@ -141,6 +154,153 @@ def gpu_identity(device) -> dict:
     except Exception:
         pass
     return out
+
+
+def build_arms(args, device, arms, gt_queries):
+    """IVF-PQ indexes (M, nbits) for every arm on bench.py's corpus, with bench.build_index's rules: coarse k-means on
+    the same training sample, each PQ codebook trained on the residuals of its first 256 * 256 rows (the sample bench.py
+    uses), rows added chunk by chunk with ids = row numbers.  The coarse assignment of a chunk and the exact top-k ground
+    truth are computed once for all arms.  The 8-bit arm is the index bench.py builds.  Returns (indexes, corpus,
+    gt_I, build seconds per arm)."""
+    import retrieval_scaling_b200 as rsb
+    from retrieval_scaling_b200 import synth, train
+    t0 = time.time()
+    corpus = synth.Corpus(d=args.d, mode="gmm", n_centres=max(16, args.nlist // 4), device=device)
+    xt = corpus.train_sample(min(args.n, args.nlist * args.train_per_centroid))
+    cent = train.kmeans(xt, args.nlist, niter=10, metric="ip", spherical=True, seed=1234)
+    xs = xt[: 256 * 256]
+    a = train.assign_ip(xs, cent)
+    t_coarse = time.time() - t0
+    indexes, secs = {}, {}
+    for m, nbits in arms:
+        t1 = time.time()
+        ix = rsb.IndexIVFPQ(args.d, args.nlist, m, nbits, device=device)
+        ix.nprobe = args.nprobe
+        ix.set_centroids(cent)
+        ix.set_codebook(train.train_pq(xs - cent[a], m, 1 << nbits, niter=25, seed=1234))
+        torch.cuda.synchronize()
+        indexes[(m, nbits)], secs[(m, nbits)] = ix, t_coarse + time.time() - t1
+    del xt, xs, a
+    first = next(iter(indexes.values()))
+    gt = {"D": None, "I": None, "pD": [], "pI": []}
+    t_gt = 0.0
+    for c in range((args.n + B.CHUNK_ROWS - 1) // B.CHUNK_ROWS):
+        rows = min(B.CHUNK_ROWS, args.n - c * B.CHUNK_ROWS)
+        t1 = time.time()
+        x = corpus.chunk(c, B.CHUNK_ROWS)[:rows]
+        D, I = rsb.knn_ip(gt_queries, x, args.k, id_offset=c * B.CHUNK_ROWS)
+        gt["pD"].append(D); gt["pI"].append(I)
+        if len(gt["pD"]) == 15:
+            B._fold_gt(gt, args.k)
+        lists = first.assign(x)
+        ids = torch.arange(c * B.CHUNK_ROWS, c * B.CHUNK_ROWS + rows, dtype=torch.int64, device=device)
+        torch.cuda.synchronize()
+        t_shared = time.time() - t1                   # corpus chunk + coarse assignment: charged to every arm
+        t_gt += t_shared
+        for key, ix in indexes.items():
+            t1 = time.time()
+            ix.add_preassigned(x, lists, ids)
+            secs[key] += t_shared + time.time() - t1
+        del x, lists, ids
+    for key, ix in indexes.items():
+        t1 = time.time()
+        ix.finalize()
+        torch.cuda.synchronize()
+        secs[key] += time.time() - t1
+    B._fold_gt(gt, args.k)
+    return indexes, corpus, gt["I"], secs
+
+
+def build_index(args, device, gt_queries):
+    """bench.py's index (--nbits 8), or the same build with 4-bit sub-quantizers."""
+    if args.nbits == 8:
+        return B.build_index(args, 0, 1, device, gt_queries=gt_queries)
+    indexes, corpus, gt_I, secs = build_arms(args, device, [(args.m, args.nbits)], gt_queries)
+    return indexes[(args.m, args.nbits)], corpus, None, gt_I, {"total_s": secs[(args.m, args.nbits)]}
+
+
+def arm_parity(index, xq, D, I, npq):
+    """Every (query, id, score) of the unrefined result re-scored in float64 from the exported codes."""
+    from oracle import pq4_oracle as P4
+    off, codes, ids = (t.cpu().numpy() for t in index.export_lists())
+    host = P4.host_ivfpq(index.get_centroids().cpu().numpy(), index.get_codebook().cpu().numpy(), off, codes, ids)
+    r = host.verify_pairs(xq[:npq].cpu().numpy(), D[:npq].cpu().numpy(), I[:npq].cpu().numpy(), rtol=1e-5, atol=2e-4)
+    r["oracle"] = "oracle/pq4_oracle.host_ivfpq (parity.HostIVFPQ on unpacked codes): <q, c_l + decode(code)> in float64"
+    r["ok"] = bool(r["rescore_out_of_tol"] == 0 and r["unknown_ids"] == 0)
+    return r
+
+
+def arms_main(args, device):
+    """IVF-PQ arms MxNBITS on one corpus, each unrefined and re-ranked from a shared fp16 and a shared sq8 store."""
+    import retrieval_scaling_b200 as rsb
+    from retrieval_scaling_b200 import synth
+    arms = [tuple(int(v) for v in s.lower().split("x")) for s in args.pq_arms.split(",")]
+    dtypes = ["float16", "sq8"]
+    need = sum(store_bytes(args, t) for t in dtypes) + sum(args.n * (m * nb // 8 + 8) for m, nb in arms) \
+        + 2 * B.CHUNK_ROWS * args.d * 4
+    free, _ = torch.cuda.mem_get_info(device)
+    if need > 0.9 * free:
+        raise SystemExit(f"the stores and the {len(arms)} indexes need ~{need} bytes, {free} are free on {device}")
+    k, kf = args.k, args.k_factor
+    kb = k * kf
+    probe = synth.Corpus(d=args.d, mode="gmm", n_centres=max(16, args.nlist // 4), device=device)
+    xq_all = probe.queries(args.nq)
+    del probe
+    n_gt = min(args.recall_queries, args.nq)
+    indexes, corpus, gt_I, build_s = build_arms(args, device, arms, xq_all[:n_gt].contiguous())
+    first = next(iter(indexes.values()))
+    stores = {t: rsb.IndexRefine(first, t, kf) for t in dtypes}
+    store_s = fill_stores(stores, corpus, args)
+    info = gpu_identity(device)
+    strip = lambda r: {kk: vv for kk, vv in r.items() if kk != "ground_truth"}   # noqa: E731
+    nqs = sorted({min(int(v), args.nq) for v in args.store_nq.split(",")}, reverse=True)
+    name = lambda key: f"PQ{key[0]}x{key[1]}"                                    # noqa: E731
+    blocks = {name(key): {"M": key[0], "nbits": key[1], "code_bytes": key[0] * key[1] // 8,
+                          "index_bytes": ix.index_bytes, "build_s": build_s[key], "per_nq": []}
+              for key, ix in indexes.items()}
+
+    def refined(ix, ref, xq):
+        Ib, _ = ix.search_ids(xq, kb)
+        return ref.rerank(xq, Ib, k)
+
+    for nq in nqs:
+        xq = xq_all[:nq].contiguous()
+        for key, ix in indexes.items():                 # arms alternated inside every batch size
+            blk = blocks[name(key)]
+            ms_u, (Iu, Du) = timed(lambda: ix.search_ids(xq, k), args.steps, args.warmup)
+            ix.set_profiling(True)
+            for _ in range(args.steps):
+                ix.search_ids(xq, k)
+            prof = ix.profile()
+            ix.set_profiling(False)
+            row = {"nq": nq, "qps_unrefined": nq / (ms_u / 1e3), "ms_per_step_unrefined": ms_u,
+                   "lut_ms": prof["lut_ms"], "scan_ms": prof["scan_ms"], "coarse_ms": prof["coarse_ms"]}
+            for t, ref in stores.items():
+                ms_r, (I, D) = timed(lambda: refined(ix, ref, xq), args.steps, args.warmup)
+                row[f"qps_refined_{t}"] = nq / (ms_r / 1e3)
+                row[f"ms_per_step_refined_{t}"] = ms_r
+                if nq == nqs[0]:
+                    ng = min(n_gt, nq)
+                    blk[f"recall_refined_{t}"] = strip(B.recall_block(I[:ng], gt_I[:ng], k))
+                    Ib, _ = ix.search_ids(xq, kb)
+                    Ir, Dr = ref.rerank(xq, Ib, k)
+                    blk[f"parity_refined_{t}"] = parity(ref, xq, Ib, Ir, Dr, k, min(args.parity_queries, nq))
+            if nq == nqs[0]:
+                ng = min(n_gt, nq)
+                blk["recall_unrefined"] = strip(B.recall_block(Iu[:ng], gt_I[:ng], k))
+                blk["recall_nq"] = ng
+                blk["parity_unrefined"] = arm_parity(ix, xq, Du, Iu, min(args.parity_queries, nq))
+            blk["per_nq"].append(row)
+    out = {"metric": f"IVF-PQ arms {args.pq_arms}: unrefined and exact re-ranking of k x {kf} candidates, "
+                     f"{args.n // 1_000_000}M x {args.d}",
+           "config": {**{kk: vv for kk, vv in B.make_config(args, 1).items() if kk not in ("M", "nbits")},
+                      "k_factor": kf, "k_base": kb},
+           "arms": blocks, "stores": {t: {"bytes": store_bytes(args, t), "build_s": store_s[t]} for t in dtypes},
+           **info, "refined_timing": "base search at k x k_factor, then the re-rank kernel (two calls per step)",
+           "recall_ground_truth": "exact fp32 inner-product search over the same corpus (librsb Flat kernels)",
+           "steps": args.steps, "warmup": args.warmup}
+    print(json.dumps(out), flush=True)
+    return 0
 
 
 def timed(fn, steps, warmup):
@@ -273,7 +433,7 @@ def tiered_main(args, device):
     xq_all = probe.queries(args.nq)
     del probe
     n_gt = min(args.recall_queries, args.nq)
-    index, corpus, _, gt_I, build = B.build_index(args, 0, 1, device, gt_queries=xq_all[:n_gt].contiguous())
+    index, corpus, _, gt_I, build = build_index(args, device, xq_all[:n_gt].contiguous())
 
     stores = {"tiered": rsb.IndexRefine(index, dtype, kf, device_rows=n_dev)}
     if args.compare_device:
@@ -361,7 +521,7 @@ def stores_main(args, device):
     xq_all = probe.queries(args.nq)
     del probe
     n_gt = min(args.recall_queries, args.nq)
-    index, corpus, _, gt_I, build = B.build_index(args, 0, 1, device, gt_queries=xq_all[:n_gt].contiguous())
+    index, corpus, _, gt_I, build = build_index(args, device, xq_all[:n_gt].contiguous())
     stores = {t: rsb.IndexRefine(index, t, kf) for t in dtypes}
     secs = fill_stores(stores, corpus, args)
     info = gpu_identity(device)
@@ -410,6 +570,8 @@ def main():
         raise SystemExit("bench_refine.py needs a CUDA device: the product path has no CPU fallback")
     device = torch.device("cuda", 0)
     torch.cuda.set_device(device)
+    if args.pq_arms:
+        return arms_main(args, device)
     if args.device_rows is not None:
         return tiered_main(args, device)
     if args.store_dtype != "float16" or args.compare_store is not None:
@@ -427,7 +589,7 @@ def main():
     xq = probe.queries(args.nq)
     del probe
     n_gt = min(args.recall_queries, args.nq)
-    index, corpus, _, gt_I, build = B.build_index(args, 0, 1, device, gt_queries=xq[:n_gt].contiguous())
+    index, corpus, _, gt_I, build = build_index(args, device, xq[:n_gt].contiguous())
 
     t0 = time.time()
     ref = rsb.IndexRefine(index, "float16", kf)
