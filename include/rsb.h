@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define RSB_VERSION 100 /* 0.1.0 */
+#define RSB_VERSION 200 /* 0.2.0 */
 
 enum {
     RSB_OK = 0,
@@ -174,84 +174,66 @@ int rsb_coarse(rsb_index_t* h, const float* q_dev, int nq, int nprobe, int64_t* 
 
 /* ---- exact re-ranking (faiss IndexRefine / IndexRefineFlat::search; the reference's unused re-score path
  *      src/indicies/ivf_pq.py:119-123 `get_knn_scores` against `self.embeds`) ------------------------------------
- * The re-rank store is caller-owned device memory [ntotal, d], row i = the vector of index id i, in fp32 or fp16
- * (16-byte aligned, d % 8 == 0).  Scores are <q, x_id> accumulated in fp32 from the decoded elements, in the same
- * order for both types (an fp16 store and an fp32 store of the same fp16-representable values agree bit for bit).  Rows are sorted by score descending, ties by ascending id; fewer than k valid candidates are
- * padded with id -1 / score -FLT_MAX; candidate ids -1 (and ids outside [0, ntotal)) are skipped.
- * k_base = k * k_factor <= 4096 (the scan's k limit); larger returns RSB_ERR_UNSUPPORTED.  ntotal <= 2^31. */
-enum { RSB_DTYPE_F32 = 0, RSB_DTYPE_F16 = 1, RSB_DTYPE_SQ8 = 2 /* re-rank store only: rsb_refine_sq8 below */ };
-size_t rsb_refine_workspace_bytes(int nq, int k_base, int k);
-/* re-rank given candidates cand_dev [nq, k_base] int64 (e.g. a search result at k_base) -> D_dev/I_dev [nq, k] */
-int rsb_refine(const float* q_dev, int nq, const void* store_dev, int store_dtype, int d, int64_t ntotal,
-               const int64_t* cand_dev, int k_base, int k, float* D_dev, int64_t* I_dev, void* ws_dev, size_t ws_bytes,
-               rsb_stream_t stream);
-/* IndexRefine::search on an IVFPQ handle: rsb_search at k_base = k * k_factor into the workspace, then rsb_refine */
-size_t rsb_search_refine_workspace_bytes(rsb_index_t* h, int nq, int k, int k_factor, int nprobe);
-int rsb_search_refine(rsb_index_t* h, const float* q_dev, int nq, int k, int k_factor, int nprobe, const void* store_dev,
-                      int store_dtype, int64_t ntotal, float* D_dev, int64_t* I_dev, void* ws_dev, size_t ws_bytes,
-                      rsb_stream_t stream);
-
-/* ---- tiered re-rank store: one logical [ntotal, d] store whose rows [0, n_dev) are device memory (store_dev) and
- *      rows [n_dev, ntotal) page-locked host memory mapped into the device address space (store_host points at row
- *      n_dev, not row 0).  n_dev = ntotal is the all-device store above; n_dev = 0 keeps every row on the host.
- * Results are bit-identical to rsb_refine / rsb_search_refine on an all-device store holding the same values.
- * Queries are processed in chunks of floor(staging_bytes / (k_base * d * elem_bytes)) (staging_bytes must hold at
- * least one query's worst case).  Within a chunk the host-tier candidates are de-duplicated on the device (radix sort
- * by id), every distinct host row crosses PCIe once into a staging buffer inside the workspace, and the re-rank reads
- * it from there; device-tier rows never cross PCIe.  Nothing synchronises the host.
- * host_rows_dev (device int64, may be NULL) is incremented by the number of distinct host rows gathered.
- * Every argument is checked before any launch: a host tier that is not page-locked and mapped (pageable memory, a
- * device pointer) returns RSB_ERR_INVALID. */
+ * The re-rank store is caller-owned, [ntotal, d], row i = the vector of index id i.  Scores are <q, x_id> accumulated
+ * in fp32 from the decoded elements, in the same order for every store dtype (an fp16 store and an fp32 store of the
+ * same fp16-representable values agree bit for bit).  Rows are sorted by score descending, ties by ascending id; fewer
+ * than k valid candidates are padded with id -1 / score -FLT_MAX; candidate ids -1 (and ids outside [0, ntotal)) are
+ * skipped.  k_base = k * k_factor <= 4096 (the scan's k limit); larger returns RSB_ERR_UNSUPPORTED.  ntotal <= 2^31.
+ *
+ * store_dtype (anything else: RSB_ERR_INVALID)
+ *   RSB_DTYPE_F32, RSB_DTYPE_F16   fp32 / fp16 rows, d % 8 == 0 (16-byte rows); sq_dev is ignored.
+ *   RSB_DTYPE_SQ8   faiss IndexRefine(base, IndexScalarQuantizer(d, QT_8bit)), factory string "...,Refine(SQ8)": one
+ *     uint8 code per element, d % 16 == 0 (whole 16-byte rows).  Scalar quantizer QT_8bit, RS_minmax, one range per
+ *     dimension; sq_dev (16-byte aligned) is [2, d] float32: vmin [d], then vdiff [d] (faiss' `sq.trained` layout).
+ *     Every operation below is a separately rounded fp32 operation:
+ *       train   vmin[j] = min over the rows of x[:, j], vdiff[j] = max - vmin[j]
+ *       encode  xi = vdiff != 0 ? (x - vmin) / vdiff : 0, clamped to [0, 1]; code = (int)(255.f * xi)  (rows outside the
+ *               trained range clamp; fp16 input is encoded from its exact fp32 value)
+ *       decode  x = vmin + ((code + 0.5f) / 255.f) * vdiff
+ *     The re-rank decodes every element and scores it as the fp32 store does (same lane order, same fmaf sequence), so
+ *     ids and scores are bit-identical to an fp32 store holding the decoded rows.
+ *
+ * Tiers: rows [0, n_dev) are device memory (store_dev, 16-byte aligned), rows [n_dev, ntotal) page-locked host memory
+ * mapped into the device address space (store_host points at row n_dev, not row 0; 16-byte aligned).  0 <= n_dev <=
+ * ntotal, else RSB_ERR_INVALID.
+ *   n_dev = ntotal   the all-device store: store_host and staging_bytes are ignored.
+ *   n_dev < ntotal   the tiered store (n_dev = 0 keeps every row on the host).  Results are bit-identical to the
+ *     all-device store holding the same values.  Queries are processed in chunks of floor(staging_bytes / (k_base * d *
+ *     elem_bytes)) (staging_bytes must hold at least one query's worst case).  Within a chunk the host-tier candidates
+ *     are de-duplicated on the device (radix sort by id), every distinct host row crosses PCIe once into a staging
+ *     buffer inside the workspace, and the re-rank reads it from there; device-tier rows never cross PCIe.  Nothing
+ *     synchronises the host.  host_rows_dev (device int64, may be NULL) is incremented by the number of distinct host
+ *     rows gathered.  A host tier that is not page-locked and mapped (pageable memory, a device pointer) returns
+ *     RSB_ERR_INVALID.
+ * Every argument is checked before any launch.  The workspace queries return 0 for arguments the call would refuse;
+ * they size the all-device store by nq, k_base and k alone, and the tiered store by its dtype and staging_bytes. */
+enum { RSB_DTYPE_F32 = 0, RSB_DTYPE_F16 = 1, RSB_DTYPE_SQ8 = 2 /* re-rank store only */ };
 int rsb_host_alloc(size_t bytes, void** out);   /* cudaHostAlloc(portable | mapped): exactly `bytes`, unlike torch's
                                                    pinned allocator, which rounds blocks up to a power of two */
 int rsb_host_free(void* p);
-size_t rsb_refine_tiered_workspace_bytes(int nq, int k_base, int k, int d, int store_dtype, size_t staging_bytes);
-int rsb_refine_tiered(const float* q_dev, int nq, const void* store_dev, int64_t n_dev, const void* store_host,
-                      int store_dtype, int d, int64_t ntotal, const int64_t* cand_dev, int k_base, int k, float* D_dev,
-                      int64_t* I_dev, void* ws_dev, size_t ws_bytes, size_t staging_bytes, int64_t* host_rows_dev,
-                      rsb_stream_t stream);
-/* workspace for either store dtype */
-size_t rsb_search_refine_tiered_workspace_bytes(rsb_index_t* h, int nq, int k, int k_factor, int nprobe,
-                                                size_t staging_bytes);
-int rsb_search_refine_tiered(rsb_index_t* h, const float* q_dev, int nq, int k, int k_factor, int nprobe,
-                             const void* store_dev, int64_t n_dev, const void* store_host, int store_dtype, int64_t ntotal,
-                             float* D_dev, int64_t* I_dev, void* ws_dev, size_t ws_bytes, size_t staging_bytes,
-                             int64_t* host_rows_dev, rsb_stream_t stream);
+size_t rsb_refine_workspace_bytes(int nq, int k_base, int k, int d, int store_dtype, int64_t n_dev, int64_t ntotal,
+                                  size_t staging_bytes);
+/* re-rank given candidates cand_dev [nq, k_base] int64 (e.g. a search result at k_base) -> D_dev/I_dev [nq, k] */
+int rsb_refine(const float* q_dev, int nq, const void* store_dev, int64_t n_dev, const void* store_host,
+               int store_dtype, const float* sq_dev, int d, int64_t ntotal, const int64_t* cand_dev, int k_base, int k,
+               float* D_dev, int64_t* I_dev, void* ws_dev, size_t ws_bytes, size_t staging_bytes,
+               int64_t* host_rows_dev, rsb_stream_t stream);
+/* IndexRefine::search on an IVFPQ handle: rsb_search at k_base = k * k_factor into the workspace, then rsb_refine */
+size_t rsb_search_refine_workspace_bytes(rsb_index_t* h, int nq, int k, int k_factor, int nprobe, int store_dtype,
+                                         int64_t n_dev, int64_t ntotal, size_t staging_bytes);
+int rsb_search_refine(rsb_index_t* h, const float* q_dev, int nq, int k, int k_factor, int nprobe,
+                      const void* store_dev, int64_t n_dev, const void* store_host, int store_dtype,
+                      const float* sq_dev, int64_t ntotal, float* D_dev, int64_t* I_dev, void* ws_dev,
+                      size_t ws_bytes, size_t staging_bytes, int64_t* host_rows_dev, rsb_stream_t stream);
 /* enable != 0: time the sort / gather / score stages of every later tiered chunk with CUDA events, on the device
  * current at the call (this waits for each chunk on the host: for measurement only).  ms_out (may be NULL) receives
  * the [3] milliseconds accumulated since the previous call, which resets them. */
 int rsb_refine_tiered_profile(int enable, double* ms_out);
-
-/* ---- SQ8 re-rank store: faiss IndexRefine(base, IndexScalarQuantizer(d, QT_8bit)), factory string "...,Refine(SQ8)" --
- *      (the same re-score path, src/indicies/ivf_pq.py:119-123 `get_knn_scores`, from one byte per element)
- * Scalar quantizer QT_8bit, RS_minmax, one range per dimension; sq_dev is [2, d] float32: vmin [d], then vdiff [d]
- * (faiss' `sq.trained` layout).  Every operation below is a separately rounded fp32 operation:
- *   train   vmin[j] = min over the rows of x[:, j], vdiff[j] = max - vmin[j]
- *   encode  xi = vdiff != 0 ? (x - vmin) / vdiff : 0, clamped to [0, 1]; code = (int)(255.f * xi)  (rows outside the
- *           trained range clamp; fp16 input is encoded from its exact fp32 value)
- *   decode  x = vmin + ((code + 0.5f) / 255.f) * vdiff
- * The re-rank decodes every element and scores it as the fp32 store does (same lane order, same fmaf sequence), so ids
- * and scores are bit-identical to rsb_refine / rsb_search_refine on an fp32 store holding the decoded rows.
- * x_dev [n, d] in x_dtype (RSB_DTYPE_F32 / RSB_DTYPE_F16); codes_dev [n, d] uint8.  rsb_sq8_train needs n >= 1. */
+/* Train / encode an SQ8 store (rules above): x_dev [n, d] in x_dtype (RSB_DTYPE_F32 / RSB_DTYPE_F16); codes_dev [n, d]
+ * uint8.  rsb_sq8_train needs n >= 1. */
 int rsb_sq8_train(const void* x_dev, int x_dtype, int64_t n, int d, float* sq_dev, rsb_stream_t stream);
 int rsb_sq8_encode(const void* x_dev, int x_dtype, int64_t n, int d, const float* sq_dev, uint8_t* codes_dev,
                    rsb_stream_t stream);
-/* rsb_refine_tiered / rsb_search_refine_tiered for an SQ8 store of codes: the store dtype is implied and sq_dev
- * (16-byte aligned) takes its place.  n_dev = ntotal is the all-device store (store_host unused); n_dev < ntotal keeps
- * rows [n_dev, ntotal) in mapped page-locked host memory, gathered as above at d bytes per row.  d % 16 == 0 (whole
- * 16-byte rows), else RSB_ERR_INVALID.  rsb_refine / rsb_search_refine / rsb_refine_tiered / rsb_search_refine_tiered
- * refuse RSB_DTYPE_SQ8 with RSB_ERR_INVALID: they have no trained range. */
-size_t rsb_refine_sq8_workspace_bytes(int nq, int k_base, int k, int d, size_t staging_bytes);
-int rsb_refine_sq8(const float* q_dev, int nq, const void* store_dev, int64_t n_dev, const void* store_host,
-                   const float* sq_dev, int d, int64_t ntotal, const int64_t* cand_dev, int k_base, int k, float* D_dev,
-                   int64_t* I_dev, void* ws_dev, size_t ws_bytes, size_t staging_bytes, int64_t* host_rows_dev,
-                   rsb_stream_t stream);
-size_t rsb_search_refine_sq8_workspace_bytes(rsb_index_t* h, int nq, int k, int k_factor, int nprobe,
-                                             size_t staging_bytes);
-int rsb_search_refine_sq8(rsb_index_t* h, const float* q_dev, int nq, int k, int k_factor, int nprobe,
-                          const void* store_dev, int64_t n_dev, const void* store_host, const float* sq_dev,
-                          int64_t ntotal, float* D_dev, int64_t* I_dev, void* ws_dev, size_t ws_bytes,
-                          size_t staging_bytes, int64_t* host_rows_dev, rsb_stream_t stream);
 
 /* ---- shard merge (src/search.py:357-367; api/serve_main_node.py:130-163) ---------------------------- */
 /* D_all_dev/I_all_dev [nshards, nq, k]: concat per query, sort by score desc (ties: lower shard, then lower

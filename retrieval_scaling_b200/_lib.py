@@ -58,29 +58,17 @@ SIGNATURES = [
     ("rsb_pq_accumulate_ksub", c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     ("rsb_peer_broadcast", c_int, [c_void_p, c_size_t, c_void_p, c_int, c_size_t, c_void_p]),
     ("rsb_coarse", c_int, [_H, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
-    ("rsb_refine_workspace_bytes", c_size_t, [c_int, c_int, c_int]),
-    ("rsb_refine", c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int64, c_void_p, c_int, c_int, c_void_p, c_void_p,
-                           c_void_p, c_size_t, c_void_p]),
-    ("rsb_search_refine_workspace_bytes", c_size_t, [_H, c_int, c_int, c_int, c_int]),
-    ("rsb_search_refine", c_int, [_H, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int64, c_void_p, c_void_p,
-                                  c_void_p, c_size_t, c_void_p]),
     ("rsb_host_alloc", c_int, [c_size_t, POINTER(c_void_p)]),
     ("rsb_host_free", c_int, [c_void_p]),
-    ("rsb_refine_tiered_workspace_bytes", c_size_t, [c_int, c_int, c_int, c_int, c_int, c_size_t]),
-    ("rsb_refine_tiered", c_int, [c_void_p, c_int, c_void_p, c_int64, c_void_p, c_int, c_int, c_int64, c_void_p, c_int,
-                                  c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_void_p, c_void_p]),
-    ("rsb_search_refine_tiered_workspace_bytes", c_size_t, [_H, c_int, c_int, c_int, c_int, c_size_t]),
-    ("rsb_search_refine_tiered", c_int, [_H, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_int,
-                                         c_int64, c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_void_p, c_void_p]),
+    ("rsb_refine_workspace_bytes", c_size_t, [c_int, c_int, c_int, c_int, c_int, c_int64, c_int64, c_size_t]),
+    ("rsb_refine", c_int, [c_void_p, c_int, c_void_p, c_int64, c_void_p, c_int, c_void_p, c_int, c_int64, c_void_p, c_int,
+                           c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_void_p, c_void_p]),
+    ("rsb_search_refine_workspace_bytes", c_size_t, [_H, c_int, c_int, c_int, c_int, c_int, c_int64, c_int64, c_size_t]),
+    ("rsb_search_refine", c_int, [_H, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_int, c_void_p,
+                                  c_int64, c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_void_p, c_void_p]),
     ("rsb_refine_tiered_profile", c_int, [c_int, POINTER(c_double)]),
     ("rsb_sq8_train", c_int, [c_void_p, c_int, c_int64, c_int, c_void_p, c_void_p]),
     ("rsb_sq8_encode", c_int, [c_void_p, c_int, c_int64, c_int, c_void_p, c_void_p, c_void_p]),
-    ("rsb_refine_sq8_workspace_bytes", c_size_t, [c_int, c_int, c_int, c_int, c_size_t]),
-    ("rsb_refine_sq8", c_int, [c_void_p, c_int, c_void_p, c_int64, c_void_p, c_void_p, c_int, c_int64, c_void_p, c_int,
-                               c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_void_p, c_void_p]),
-    ("rsb_search_refine_sq8_workspace_bytes", c_size_t, [_H, c_int, c_int, c_int, c_int, c_size_t]),
-    ("rsb_search_refine_sq8", c_int, [_H, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p,
-                                      c_int64, c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_void_p, c_void_p]),
     ("rsb_merge_topk", c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     ("rsb_merge_topk_peers", c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     ("rsb_merge_topk_peers_scatter", c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,

@@ -1081,109 +1081,8 @@ extern "C" int rsb_search_preassigned_shared(rsb_index_t* h, const float* q, int
 }
 
 // ---- exact re-ranking (faiss IndexRefine::search) -----------------------------------------------------------
-static int store_elem_bytes(int store_dtype) { return store_dtype == RSB_DTYPE_SQ8 ? 1 : store_dtype == RSB_DTYPE_F16 ? 2 : 4; }
-
-// store_rows: rows behind `store` (-1: all ntotal); a tiered store's device tier holds n_dev of them.
-// store_dtype RSB_DTYPE_SQ8 is accepted only from the SQ8 entry points (sq8 = true), which carry the trained range.
-static int refine_check(const void* store, int store_dtype, int d, int64_t ntotal, int k_base, int k, int64_t store_rows = -1,
-                        bool sq8 = false) {
-    if (store_dtype == RSB_DTYPE_SQ8 && !sq8)
-        return fail(RSB_ERR_INVALID, "an RSB_DTYPE_SQ8 store is decoded with its trained range: use rsb_refine_sq8 / "
-                                     "rsb_search_refine_sq8");
-    if (store_dtype != RSB_DTYPE_F32 && store_dtype != RSB_DTYPE_F16 && !sq8)
-        return fail(RSB_ERR_INVALID, "store_dtype must be RSB_DTYPE_F32 or RSB_DTYPE_F16, got %d", store_dtype);
-    if (k <= 0 || k_base < k) return fail(RSB_ERR_INVALID, "need 0 < k <= k_base, got k = %d, k_base = %d", k, k_base);
-    if (k_base > 4096) return fail(RSB_ERR_UNSUPPORTED, "k_base = k * k_factor = %d > 4096 is not supported", k_base);
-    if (ntotal < 0 || ntotal > ((int64_t)1 << 31)) return fail(RSB_ERR_INVALID, "store rows must be in [0, 2^31], got %lld", (long long)ntotal);
-    if (d <= 0 || d % 8) return fail(RSB_ERR_INVALID, "d = %d must be a positive multiple of 8 for the re-rank store", d);
-    if (sq8 && d % 16) return fail(RSB_ERR_INVALID, "d = %d must be a multiple of 16 for an SQ8 store (whole 16-byte rows)", d);
-    if ((store_rows < 0 ? ntotal : store_rows) > 0 && (!store || (reinterpret_cast<uintptr_t>(store) & 15)))
-        return fail(RSB_ERR_INVALID, "the re-rank store must be a 16-byte aligned device pointer");
-    return RSB_OK;
-}
-
-// sq: the SQ8 store's [2, d] (vmin, vdiff); null for fp16 / fp32
-static int refine_impl(const float* q, int nq, const void* store, int store_dtype, int d, int64_t ntotal, const int64_t* cand,
-                       int k_base, int k, float* D, int64_t* I, void* ws, size_t ws_bytes, cudaStream_t st,
-                       const float* sq = nullptr) {
-    const RefinePlan p = refine_plan(nq, k_base, k);
-    if (ws_bytes < p.ws_bytes) return fail(RSB_ERR_OOM, "workspace too small: need %zu bytes, got %zu", p.ws_bytes, ws_bytes);
-    if (launch_refine_rows(p, q, nq, store, store_elem_bytes(store_dtype), d, ntotal, cand, k_base, k, D, I, ws, st,
-                           nullptr, sq) != 0)
-        return fail(RSB_ERR_UNSUPPORTED, "d = %d with k_base = %d needs more shared memory than the re-rank kernel has", d, k_base);
-    CHECK_LAUNCH();
-    return RSB_OK;
-}
-
-extern "C" size_t rsb_refine_workspace_bytes(int nq, int k_base, int k) {
-    if (nq <= 0 || k <= 0 || k_base < k) return 0;
-    return refine_plan(nq, k_base, k).ws_bytes;
-}
-
-extern "C" int rsb_refine(const float* q, int nq, const void* store, int store_dtype, int d, int64_t ntotal,
-                          const int64_t* cand, int k_base, int k, float* D, int64_t* I, void* ws, size_t ws_bytes,
-                          rsb_stream_t stream) {
-    RSB_TRY(refine_check(store, store_dtype, d, ntotal, k_base, k));
-    if (nq < 0) return fail(RSB_ERR_INVALID, "bad nq = %d", nq);
-    if (nq == 0) return RSB_OK;
-    if (!q || !cand || !D || !I) return fail(RSB_ERR_INVALID, "null argument");
-    return refine_impl(q, nq, store, store_dtype, d, ntotal, cand, k_base, k, D, I, ws, ws_bytes, (cudaStream_t)stream);
-}
-
-// Queries are processed in batches of qb: base search at k_base into [qb, k_base] candidate buffers, then the re-rank.
-struct SearchRefinePlan {
-    int qb;
-    size_t search_ws, off_D, off_I, off_ref, total;
-};
-static SearchRefinePlan search_refine_plan(rsb_index* h, int nq, int k, int k_base, int nprobe) {
-    SearchRefinePlan p;
-    nq = std::max(nq, 1);
-    p.qb = std::min(nq, 16384);
-    const int last = nq % p.qb ? nq % p.qb : p.qb;     // the last batch may split its queries into more chunks
-    p.search_ws = align_up(rsb_workspace_bytes(h, p.qb, k_base, nprobe));
-    p.off_D = p.search_ws;
-    p.off_I = p.off_D + align_up((size_t)p.qb * k_base * 4);
-    p.off_ref = p.off_I + align_up((size_t)p.qb * k_base * 8);
-    p.total = p.off_ref + align_up(std::max(refine_plan(p.qb, k_base, k).ws_bytes, refine_plan(last, k_base, k).ws_bytes));
-    return p;
-}
-
-extern "C" size_t rsb_search_refine_workspace_bytes(rsb_index_t* h, int nq, int k, int k_factor, int nprobe) {
-    if (!h || k <= 0 || k_factor <= 0) return 0;
-    return search_refine_plan(h, nq, k, k * k_factor, nprobe).total;
-}
-
-extern "C" int rsb_search_refine(rsb_index_t* h, const float* q, int nq, int k, int k_factor, int nprobe, const void* store,
-                                 int store_dtype, int64_t ntotal, float* D, int64_t* I, void* ws, size_t ws_bytes,
-                                 rsb_stream_t stream) {
-    if (!h) return fail(RSB_ERR_INVALID, "null handle");
-    if (h->kind != RSB_IVFPQ) return fail(RSB_ERR_INVALID, "re-ranking is for IVFPQ indexes: Flat / IVFFlat scores are already exact");
-    if (k <= 0 || k_factor <= 0) return fail(RSB_ERR_INVALID, "bad k = %d / k_factor = %d", k, k_factor);
-    if ((int64_t)k * k_factor > 4096) return fail(RSB_ERR_UNSUPPORTED, "k * k_factor = %lld > 4096 is not supported", (long long)k * k_factor);
-    const int k_base = k * k_factor;
-    RSB_TRY(refine_check(store, store_dtype, h->d, ntotal, k_base, k));
-    if (ntotal != h->ntotal + h->n_staged)
-        return fail(RSB_ERR_INVALID, "the re-rank store has %lld rows, the index holds %lld vectors", (long long)ntotal,
-                    (long long)(h->ntotal + h->n_staged));
-    if (nq < 0) return fail(RSB_ERR_INVALID, "bad nq = %d", nq);
-    if (nq == 0) return RSB_OK;
-    if (!q || !D || !I) return fail(RSB_ERR_INVALID, "null argument");
-    const SearchRefinePlan p = search_refine_plan(h, nq, k, k_base, nprobe);
-    if (ws_bytes < p.total) return fail(RSB_ERR_OOM, "workspace too small: need %zu bytes, got %zu", p.total, ws_bytes);
-    unsigned char* w = static_cast<unsigned char*>(ws);
-    float* Db = reinterpret_cast<float*>(w + p.off_D);
-    int64_t* Ib = reinterpret_cast<int64_t*>(w + p.off_I);
-    for (int q0 = 0; q0 < nq; q0 += p.qb) {
-        const int nb = std::min(p.qb, nq - q0);
-        const float* qb = q + (size_t)q0 * h->d;
-        RSB_TRY(rsb_search(h, qb, nb, k_base, nprobe, Db, Ib, w, p.search_ws, stream));
-        RSB_TRY(refine_impl(qb, nb, store, store_dtype, h->d, ntotal, Ib, k_base, k, D + (size_t)q0 * k, I + (size_t)q0 * k,
-                            w + p.off_ref, p.total - p.off_ref, (cudaStream_t)stream));
-    }
-    return RSB_OK;
-}
-
-// ---- tiered re-rank store: rows [0, n_dev) in device memory, rows [n_dev, ntotal) in mapped page-locked host memory
+// The store [ntotal, d] in fp32, fp16 or SQ8 codes: rows [0, n_dev) in device memory, rows [n_dev, ntotal) in mapped
+// page-locked host memory (n_dev < ntotal: the tiered store).
 extern "C" int rsb_host_alloc(size_t bytes, void** out) {
     if (!out) return fail(RSB_ERR_INVALID, "out is NULL");
     *out = nullptr;
@@ -1197,31 +1096,53 @@ extern "C" int rsb_host_free(void* p) {
     return RSB_OK;
 }
 
-// Argument checks that need no CUDA call.
-static int tiered_check(const void* store_dev, int64_t n_dev, const void* store_host, int store_dtype, int d,
-                        int64_t ntotal, int k_base, int k, size_t staging_bytes, bool sq8 = false) {
+static bool misaligned16(const void* p) { return reinterpret_cast<uintptr_t>(p) & 15; }
+
+// The checks of the store that need no pointer (the workspace queries run these alone); *s gets its shape.
+static int store_shape(RefineStore* s, int store_dtype, int64_t n_dev, int64_t ntotal, int d, int k_base, int k,
+                       size_t staging_bytes) {
+    if (store_dtype != RSB_DTYPE_F32 && store_dtype != RSB_DTYPE_F16 && store_dtype != RSB_DTYPE_SQ8)
+        return fail(RSB_ERR_INVALID, "store_dtype must be RSB_DTYPE_F32, RSB_DTYPE_F16 or RSB_DTYPE_SQ8, got %d", store_dtype);
     if (n_dev < 0 || n_dev > ntotal)
         return fail(RSB_ERR_INVALID, "n_dev = %lld must be in [0, ntotal = %lld]", (long long)n_dev, (long long)ntotal);
-    RSB_TRY(refine_check(store_dev, store_dtype, d, ntotal, k_base, k, n_dev, sq8));
-    const size_t per_q = (size_t)k_base * d * store_elem_bytes(store_dtype);
-    if (staging_bytes < per_q)
+    if (k <= 0 || k_base < k) return fail(RSB_ERR_INVALID, "need 0 < k <= k_base, got k = %d, k_base = %d", k, k_base);
+    if (k_base > 4096) return fail(RSB_ERR_UNSUPPORTED, "k_base = k * k_factor = %d > 4096 is not supported", k_base);
+    if (ntotal > ((int64_t)1 << 31)) return fail(RSB_ERR_INVALID, "store rows must be in [0, 2^31], got %lld", (long long)ntotal);
+    if (d <= 0 || d % 8) return fail(RSB_ERR_INVALID, "d = %d must be a positive multiple of 8 for the re-rank store", d);
+    const bool sq8 = store_dtype == RSB_DTYPE_SQ8;
+    if (sq8 && d % 16) return fail(RSB_ERR_INVALID, "d = %d must be a multiple of 16 for an SQ8 store (whole 16-byte rows)", d);
+    const int eb = sq8 ? 1 : store_dtype == RSB_DTYPE_F16 ? 2 : 4;
+    const size_t per_q = (size_t)k_base * d * eb;
+    if (n_dev < ntotal && staging_bytes < per_q)
         return fail(RSB_ERR_INVALID, "staging_bytes = %zu is below one query's worst case (k_base * d * elem = %zu)",
                     staging_bytes, per_q);
-    if (n_dev < ntotal && (!store_host || (reinterpret_cast<uintptr_t>(store_host) & 15)))
+    *s = RefineStore{nullptr, n_dev, nullptr, eb, d, ntotal, nullptr};
+    return RSB_OK;
+}
+
+// Every check of the store that needs no CUDA call; *s gets the store, its host tier as the caller's pointer until
+// map_host_tier replaces it by the device alias.
+static int refine_store(RefineStore* s, const void* store_dev, int64_t n_dev, const void* store_host, int store_dtype,
+                        const float* sq, int d, int64_t ntotal, int k_base, int k, size_t staging_bytes) {
+    RSB_TRY(store_shape(s, store_dtype, n_dev, ntotal, d, k_base, k, staging_bytes));
+    if (n_dev > 0 && (!store_dev || misaligned16(store_dev)))
+        return fail(RSB_ERR_INVALID, "the re-rank store must be a 16-byte aligned device pointer");
+    if (n_dev < ntotal && (!store_host || misaligned16(store_host)))
         return fail(RSB_ERR_INVALID, "the host tier must be a 16-byte aligned page-locked host pointer");
-    return RSB_OK;
-}
-
-static int sq_check(const float* sq) {
-    if (!sq || (reinterpret_cast<uintptr_t>(sq) & 15))
+    if (store_dtype == RSB_DTYPE_SQ8 && (!sq || misaligned16(sq)))
         return fail(RSB_ERR_INVALID, "the SQ8 range sq_dev [2, d] must be a 16-byte aligned device pointer");
+    s->dev = store_dev;
+    s->host = n_dev < ntotal ? store_host : nullptr;
+    s->sq = store_dtype == RSB_DTYPE_SQ8 ? sq : nullptr;
     return RSB_OK;
 }
 
-// The host tier [first, first + bytes) must be page-locked and mapped: both ends are checked, and the kernels read it
-// through the device alias returned in *alias.  Pageable memory and device memory are refused.
-static int host_tier_alias(const void* first, size_t bytes, const void** alias) {
-    const unsigned char* p[2] = {static_cast<const unsigned char*>(first), static_cast<const unsigned char*>(first) + bytes - 1};
+// A tiered store's host tier must be page-locked and mapped: both ends are checked, and s->host becomes the device
+// alias the kernels read it through.  Pageable memory and device memory are refused.
+static int map_host_tier(RefineStore* s) {
+    if (s->n_dev == s->ntotal) return RSB_OK;
+    const size_t bytes = (size_t)(s->ntotal - s->n_dev) * s->d * s->elem_bytes;
+    const unsigned char* p[2] = {static_cast<const unsigned char*>(s->host), static_cast<const unsigned char*>(s->host) + bytes - 1};
     void* dp[2] = {nullptr, nullptr};
     for (int i = 0; i < 2; ++i) {
         cudaPointerAttributes a{};
@@ -1236,112 +1157,108 @@ static int host_tier_alias(const void* first, size_t bytes, const void** alias) 
     }
     if (static_cast<unsigned char*>(dp[1]) != static_cast<unsigned char*>(dp[0]) + bytes - 1)
         return fail(RSB_ERR_INVALID, "the host tier is not one mapped allocation");
-    *alias = dp[0];
+    s->host = dp[0];
     return RSB_OK;
 }
 
-// Both the workspace query and the call size the workspace for the larger of the fp16 and fp32 plans, so one query
-// serves either store dtype.  sq8: the SQ8 plan (1-byte elements) alone, for the SQ8 entry points.
-static size_t tiered_ws(int nq, int k_base, int k, int d, size_t staging_bytes, bool sq8 = false) {
-    if (sq8) {
-        const TieredPlan p = tiered_plan(nq, k_base, k, d, 1, staging_bytes);
-        return p.qc ? p.total : 0;
-    }
-    const TieredPlan a = tiered_plan(nq, k_base, k, d, 2, staging_bytes), b = tiered_plan(nq, k_base, k, d, 4, staging_bytes);
-    return std::max(a.qc ? a.total : 0, b.qc ? b.total : 0);
+// Workspace of one re-rank of nq queries: the plain kernel's for an all-device store, the tiered plan of the store's
+// element size otherwise (0: the tiered plan could not be sized).
+static size_t refine_ws(const RefineStore& s, int nq, int k_base, int k, size_t staging_bytes) {
+    if (s.n_dev == s.ntotal) return refine_plan(nq, k_base, k).ws_bytes;
+    const TieredPlan p = tiered_plan(nq, k_base, k, s.d, s.elem_bytes, staging_bytes);
+    return p.qc ? p.total : 0;
 }
 
-// Validated: the tiered re-rank of nq queries (all device rows: the plain kernel; no staging, no host rows).
-static int refine_tiered_impl(const float* q, int nq, const void* store_dev, int64_t n_dev, const void* host_alias,
-                              int store_dtype, int d, int64_t ntotal, const int64_t* cand, int k_base, int k, float* D,
-                              int64_t* I, void* ws, size_t ws_bytes, size_t staging_bytes, int64_t* host_rows,
-                              cudaStream_t st, const float* sq = nullptr) {
-    const int eb = store_elem_bytes(store_dtype);
-    if (n_dev == ntotal) return refine_impl(q, nq, store_dev, store_dtype, d, ntotal, cand, k_base, k, D, I, ws, ws_bytes, st, sq);
-    const TieredPlan p = tiered_plan(nq, k_base, k, d, eb, staging_bytes);
+// Validated: the re-rank of nq queries, by the plain kernel (all-device store) or the tiered launcher.
+static int refine_batch(const RefineStore& s, const float* q, int nq, const int64_t* cand, int k_base, int k, float* D,
+                        int64_t* I, void* ws, size_t ws_bytes, size_t staging_bytes, int64_t* host_rows, cudaStream_t st) {
+    const size_t need = refine_ws(s, nq, k_base, k, staging_bytes);
+    if (ws_bytes < need) return fail(RSB_ERR_OOM, "workspace too small: need %zu bytes, got %zu", need, ws_bytes);
+    if (s.n_dev == s.ntotal) {
+        if (launch_refine_rows(refine_plan(nq, k_base, k), q, nq, s, cand, k_base, k, D, I, ws, st) != 0)
+            return fail(RSB_ERR_UNSUPPORTED, "d = %d with k_base = %d needs more shared memory than the re-rank kernel has",
+                        s.d, k_base);
+        CHECK_LAUNCH();
+        return RSB_OK;
+    }
+    const TieredPlan p = tiered_plan(nq, k_base, k, s.d, s.elem_bytes, staging_bytes);
     if (!p.qc) return fail(RSB_ERR_CUDA, "could not size the tiered re-rank workspace: %s", cudaGetErrorString(cudaGetLastError()));
     if (!p.smem_ok)
-        return fail(RSB_ERR_UNSUPPORTED, "d = %d with k_base = %d needs more shared memory than the re-rank kernel has", d, k_base);
-    if (ws_bytes < p.total) return fail(RSB_ERR_OOM, "workspace too small: need %zu bytes, got %zu", p.total, ws_bytes);
-    const cudaError_t e = launch_refine_tiered(p, q, nq, store_dev, n_dev, host_alias, eb, d, ntotal, cand, k_base, k, D, I,
-                                               ws, reinterpret_cast<long long*>(host_rows), st, sq);
+        return fail(RSB_ERR_UNSUPPORTED, "d = %d with k_base = %d needs more shared memory than the re-rank kernel has", s.d, k_base);
+    const cudaError_t e = launch_refine_tiered(p, q, nq, s, cand, k_base, k, D, I, ws, reinterpret_cast<long long*>(host_rows), st);
     if (e != cudaSuccess) return fail(RSB_ERR_CUDA, "tiered re-rank: %s", cudaGetErrorString(e));
     return RSB_OK;
 }
 
-extern "C" size_t rsb_refine_tiered_workspace_bytes(int nq, int k_base, int k, int d, int store_dtype, size_t staging_bytes) {
-    if (nq <= 0 || k <= 0 || k_base < k || k_base > 4096 || d <= 0 || d % 8) return 0;
-    if (store_dtype != RSB_DTYPE_F32 && store_dtype != RSB_DTYPE_F16) return 0;
-    return std::max(refine_plan(nq, k_base, k).ws_bytes, tiered_ws(nq, k_base, k, d, staging_bytes));
+extern "C" size_t rsb_refine_workspace_bytes(int nq, int k_base, int k, int d, int store_dtype, int64_t n_dev,
+                                             int64_t ntotal, size_t staging_bytes) {
+    RefineStore s;
+    if (nq <= 0 || store_shape(&s, store_dtype, n_dev, ntotal, d, k_base, k, staging_bytes) != RSB_OK) return 0;
+    return refine_ws(s, nq, k_base, k, staging_bytes);
 }
 
-// rsb_refine_tiered and rsb_refine_sq8 (sq8 = true: store_dtype RSB_DTYPE_SQ8 with its range sq)
-static int refine_tiered_entry(const float* q, int nq, const void* store_dev, int64_t n_dev, const void* store_host,
-                               int store_dtype, int d, int64_t ntotal, const int64_t* cand, int k_base, int k, float* D,
-                               int64_t* I, void* ws, size_t ws_bytes, size_t staging_bytes, int64_t* host_rows,
-                               cudaStream_t stream, const float* sq, bool sq8) {
-    RSB_TRY(tiered_check(store_dev, n_dev, store_host, store_dtype, d, ntotal, k_base, k, staging_bytes, sq8));
-    if (sq8) RSB_TRY(sq_check(sq));
+extern "C" int rsb_refine(const float* q, int nq, const void* store_dev, int64_t n_dev, const void* store_host,
+                          int store_dtype, const float* sq, int d, int64_t ntotal, const int64_t* cand, int k_base, int k,
+                          float* D, int64_t* I, void* ws, size_t ws_bytes, size_t staging_bytes, int64_t* host_rows,
+                          rsb_stream_t stream) {
+    RefineStore s;
+    RSB_TRY(refine_store(&s, store_dev, n_dev, store_host, store_dtype, sq, d, ntotal, k_base, k, staging_bytes));
     if (nq < 0) return fail(RSB_ERR_INVALID, "bad nq = %d", nq);
     if (nq == 0) return RSB_OK;
     if (!q || !cand || !D || !I) return fail(RSB_ERR_INVALID, "null argument");
-    const void* alias = nullptr;
-    if (n_dev < ntotal)
-        RSB_TRY(host_tier_alias(store_host, (size_t)(ntotal - n_dev) * d * store_elem_bytes(store_dtype), &alias));
-    return refine_tiered_impl(q, nq, store_dev, n_dev, alias, store_dtype, d, ntotal, cand, k_base, k, D, I, ws, ws_bytes,
-                              staging_bytes, host_rows, stream, sq);
+    RSB_TRY(map_host_tier(&s));
+    return refine_batch(s, q, nq, cand, k_base, k, D, I, ws, ws_bytes, staging_bytes, host_rows, (cudaStream_t)stream);
 }
 
-extern "C" int rsb_refine_tiered(const float* q, int nq, const void* store_dev, int64_t n_dev, const void* store_host,
-                                 int store_dtype, int d, int64_t ntotal, const int64_t* cand, int k_base, int k, float* D,
-                                 int64_t* I, void* ws, size_t ws_bytes, size_t staging_bytes, int64_t* host_rows,
-                                 rsb_stream_t stream) {
-    return refine_tiered_entry(q, nq, store_dev, n_dev, store_host, store_dtype, d, ntotal, cand, k_base, k, D, I, ws,
-                               ws_bytes, staging_bytes, host_rows, (cudaStream_t)stream, nullptr, false);
+// Queries are processed in batches of qb: base search at k_base into [qb, k_base] candidate buffers, then the re-rank.
+struct SearchRefinePlan {
+    int qb;
+    size_t search_ws, off_D, off_I, off_ref, total;
+};
+static SearchRefinePlan search_refine_plan(rsb_index* h, const RefineStore& s, int nq, int k, int k_base, int nprobe,
+                                           size_t staging_bytes) {
+    SearchRefinePlan p;
+    nq = std::max(nq, 1);
+    p.qb = std::min(nq, 16384);
+    const int last = nq % p.qb ? nq % p.qb : p.qb;     // the last batch may split its queries into more chunks
+    p.search_ws = align_up(rsb_workspace_bytes(h, p.qb, k_base, nprobe));
+    p.off_D = p.search_ws;
+    p.off_I = p.off_D + align_up((size_t)p.qb * k_base * 4);
+    p.off_ref = p.off_I + align_up((size_t)p.qb * k_base * 8);
+    p.total = p.off_ref + align_up(std::max(refine_ws(s, p.qb, k_base, k, staging_bytes),
+                                            refine_ws(s, last, k_base, k, staging_bytes)));
+    return p;
 }
 
-static size_t search_refine_tiered_ws(rsb_index* h, int nq, int k, int k_base, int nprobe, size_t staging_bytes,
-                                      size_t* off_ref, bool sq8 = false) {
-    const SearchRefinePlan p = search_refine_plan(h, nq, k, k_base, nprobe);
-    const int n = std::max(nq, 1), last = n % p.qb ? n % p.qb : p.qb;
-    *off_ref = p.off_ref;
-    return p.total + std::max(tiered_ws(p.qb, k_base, k, h->d, staging_bytes, sq8),
-                              tiered_ws(last, k_base, k, h->d, staging_bytes, sq8));
-}
-
-extern "C" size_t rsb_search_refine_tiered_workspace_bytes(rsb_index_t* h, int nq, int k, int k_factor, int nprobe,
-                                                          size_t staging_bytes) {
+extern "C" size_t rsb_search_refine_workspace_bytes(rsb_index_t* h, int nq, int k, int k_factor, int nprobe,
+                                                    int store_dtype, int64_t n_dev, int64_t ntotal,
+                                                    size_t staging_bytes) {
     if (!h || k <= 0 || k_factor <= 0 || (int64_t)k * k_factor > 4096) return 0;
-    size_t off_ref = 0;
-    return search_refine_tiered_ws(h, nq, k, k * k_factor, nprobe, staging_bytes, &off_ref);
+    RefineStore s;
+    if (store_shape(&s, store_dtype, n_dev, ntotal, h->d, k * k_factor, k, staging_bytes) != RSB_OK) return 0;
+    return search_refine_plan(h, s, nq, k, k * k_factor, nprobe, staging_bytes).total;
 }
 
-// rsb_search_refine_tiered and rsb_search_refine_sq8 (sq8 = true: store_dtype RSB_DTYPE_SQ8 with its range sq)
-static int search_refine_tiered_entry(rsb_index_t* h, const float* q, int nq, int k, int k_factor, int nprobe,
-                                      const void* store_dev, int64_t n_dev, const void* store_host, int store_dtype,
-                                      int64_t ntotal, float* D, int64_t* I, void* ws, size_t ws_bytes,
-                                      size_t staging_bytes, int64_t* host_rows, rsb_stream_t stream, const float* sq,
-                                      bool sq8) {
+extern "C" int rsb_search_refine(rsb_index_t* h, const float* q, int nq, int k, int k_factor, int nprobe,
+                                 const void* store_dev, int64_t n_dev, const void* store_host, int store_dtype,
+                                 const float* sq, int64_t ntotal, float* D, int64_t* I, void* ws, size_t ws_bytes,
+                                 size_t staging_bytes, int64_t* host_rows, rsb_stream_t stream) {
     if (!h) return fail(RSB_ERR_INVALID, "null handle");
     if (h->kind != RSB_IVFPQ) return fail(RSB_ERR_INVALID, "re-ranking is for IVFPQ indexes: Flat / IVFFlat scores are already exact");
     if (k <= 0 || k_factor <= 0) return fail(RSB_ERR_INVALID, "bad k = %d / k_factor = %d", k, k_factor);
     if ((int64_t)k * k_factor > 4096) return fail(RSB_ERR_UNSUPPORTED, "k * k_factor = %lld > 4096 is not supported", (long long)k * k_factor);
     const int k_base = k * k_factor;
-    RSB_TRY(tiered_check(store_dev, n_dev, store_host, store_dtype, h->d, ntotal, k_base, k, staging_bytes, sq8));
-    if (sq8) RSB_TRY(sq_check(sq));
+    RefineStore s;
+    RSB_TRY(refine_store(&s, store_dev, n_dev, store_host, store_dtype, sq, h->d, ntotal, k_base, k, staging_bytes));
     if (ntotal != h->ntotal + h->n_staged)
         return fail(RSB_ERR_INVALID, "the re-rank store has %lld rows, the index holds %lld vectors", (long long)ntotal,
                     (long long)(h->ntotal + h->n_staged));
     if (nq < 0) return fail(RSB_ERR_INVALID, "bad nq = %d", nq);
     if (nq == 0) return RSB_OK;
     if (!q || !D || !I) return fail(RSB_ERR_INVALID, "null argument");
-    const void* alias = nullptr;
-    if (n_dev < ntotal)
-        RSB_TRY(host_tier_alias(store_host, (size_t)(ntotal - n_dev) * h->d * store_elem_bytes(store_dtype), &alias));
-    size_t off_ref = 0;
-    const size_t total = search_refine_tiered_ws(h, nq, k, k_base, nprobe, staging_bytes, &off_ref, sq8);
-    if (ws_bytes < total) return fail(RSB_ERR_OOM, "workspace too small: need %zu bytes, got %zu", total, ws_bytes);
-    const SearchRefinePlan p = search_refine_plan(h, nq, k, k_base, nprobe);
+    RSB_TRY(map_host_tier(&s));
+    const SearchRefinePlan p = search_refine_plan(h, s, nq, k, k_base, nprobe, staging_bytes);
+    if (ws_bytes < p.total) return fail(RSB_ERR_OOM, "workspace too small: need %zu bytes, got %zu", p.total, ws_bytes);
     unsigned char* w = static_cast<unsigned char*>(ws);
     float* Db = reinterpret_cast<float*>(w + p.off_D);
     int64_t* Ib = reinterpret_cast<int64_t*>(w + p.off_I);
@@ -1349,19 +1266,10 @@ static int search_refine_tiered_entry(rsb_index_t* h, const float* q, int nq, in
         const int nb = std::min(p.qb, nq - q0);
         const float* qb = q + (size_t)q0 * h->d;
         RSB_TRY(rsb_search(h, qb, nb, k_base, nprobe, Db, Ib, w, p.search_ws, stream));
-        RSB_TRY(refine_tiered_impl(qb, nb, store_dev, n_dev, alias, store_dtype, h->d, ntotal, Ib, k_base, k,
-                                   D + (size_t)q0 * k, I + (size_t)q0 * k, w + off_ref, ws_bytes - off_ref, staging_bytes,
-                                   host_rows, (cudaStream_t)stream, sq));
+        RSB_TRY(refine_batch(s, qb, nb, Ib, k_base, k, D + (size_t)q0 * k, I + (size_t)q0 * k, w + p.off_ref,
+                             p.total - p.off_ref, staging_bytes, host_rows, (cudaStream_t)stream));
     }
     return RSB_OK;
-}
-
-extern "C" int rsb_search_refine_tiered(rsb_index_t* h, const float* q, int nq, int k, int k_factor, int nprobe,
-                                        const void* store_dev, int64_t n_dev, const void* store_host, int store_dtype,
-                                        int64_t ntotal, float* D, int64_t* I, void* ws, size_t ws_bytes,
-                                        size_t staging_bytes, int64_t* host_rows, rsb_stream_t stream) {
-    return search_refine_tiered_entry(h, q, nq, k, k_factor, nprobe, store_dev, n_dev, store_host, store_dtype, ntotal, D,
-                                      I, ws, ws_bytes, staging_bytes, host_rows, stream, nullptr, false);
 }
 
 extern "C" int rsb_refine_tiered_profile(int enable, double* ms_out) {
@@ -1394,34 +1302,6 @@ extern "C" int rsb_sq8_encode(const void* x, int x_dtype, int64_t n, int d, cons
     const cudaError_t e = launch_sq8_encode(x, x_dtype == RSB_DTYPE_F16, n, d, sq, codes, (cudaStream_t)stream);
     if (e != cudaSuccess) return fail(RSB_ERR_CUDA, "sq8 encode: %s", cudaGetErrorString(e));
     return RSB_OK;
-}
-
-extern "C" size_t rsb_refine_sq8_workspace_bytes(int nq, int k_base, int k, int d, size_t staging_bytes) {
-    if (nq <= 0 || k <= 0 || k_base < k || k_base > 4096 || d <= 0 || d % 16) return 0;
-    return std::max(refine_plan(nq, k_base, k).ws_bytes, tiered_ws(nq, k_base, k, d, staging_bytes, true));
-}
-
-extern "C" int rsb_refine_sq8(const float* q, int nq, const void* store_dev, int64_t n_dev, const void* store_host,
-                              const float* sq, int d, int64_t ntotal, const int64_t* cand, int k_base, int k, float* D,
-                              int64_t* I, void* ws, size_t ws_bytes, size_t staging_bytes, int64_t* host_rows,
-                              rsb_stream_t stream) {
-    return refine_tiered_entry(q, nq, store_dev, n_dev, store_host, RSB_DTYPE_SQ8, d, ntotal, cand, k_base, k, D, I, ws,
-                               ws_bytes, staging_bytes, host_rows, (cudaStream_t)stream, sq, true);
-}
-
-extern "C" size_t rsb_search_refine_sq8_workspace_bytes(rsb_index_t* h, int nq, int k, int k_factor, int nprobe,
-                                                       size_t staging_bytes) {
-    if (!h || k <= 0 || k_factor <= 0 || (int64_t)k * k_factor > 4096 || h->d % 16) return 0;
-    size_t off_ref = 0;
-    return search_refine_tiered_ws(h, nq, k, k * k_factor, nprobe, staging_bytes, &off_ref, true);
-}
-
-extern "C" int rsb_search_refine_sq8(rsb_index_t* h, const float* q, int nq, int k, int k_factor, int nprobe,
-                                     const void* store_dev, int64_t n_dev, const void* store_host, const float* sq,
-                                     int64_t ntotal, float* D, int64_t* I, void* ws, size_t ws_bytes, size_t staging_bytes,
-                                     int64_t* host_rows, rsb_stream_t stream) {
-    return search_refine_tiered_entry(h, q, nq, k, k_factor, nprobe, store_dev, n_dev, store_host, RSB_DTYPE_SQ8, ntotal, D,
-                                      I, ws, ws_bytes, staging_bytes, host_rows, stream, sq, true);
 }
 
 // ---- training steps (index.train) ---------------------------------------------------------------------------

@@ -76,18 +76,22 @@ struct RefinePlan {
 RefinePlan refine_plan(int nq, int k_base, int k);
 // P * 8 + d * 4 bytes of shared memory (SQ8, elem_bytes 1: + 2 * d * 4 for vmin / vdiff) <= 200 KB
 bool refine_smem_fits(const RefinePlan& p, int d, int elem_bytes);
-// tiered store: rows id >= n_dev are read from staging + slot[q * k_base + j] * d
-struct TierArgs {
+// The re-rank store [ntotal, d]: rows [0, n_dev) at dev (device memory), rows [n_dev, ntotal) at host (the device
+// alias of the mapped page-locked host tier; null when n_dev == ntotal).  elem_bytes 1 (SQ8 codes), 2 (fp16) or 4
+// (fp32).  sq: the SQ8 store's [2, d] fp32 (vmin, vdiff), 16-byte aligned (null for fp16 / fp32).
+struct RefineStore {
+    const void* dev;
     int64_t n_dev;
-    const void* staging;
-    const int* slot;      // [nq, k_base]
+    const void* host;
+    int elem_bytes;
+    int d;
+    int64_t ntotal;
+    const float* sq;
 };
-// X: store [ntotal, d], elem_bytes 1 (SQ8 codes), 2 (fp16) or 4 (fp32); cand [nq, k_base] ids (-1 = skip); sq: the SQ8
-// store's [2, d] fp32 (vmin, vdiff), 16-byte aligned (null for fp16 / fp32); returns <0 if the shared memory the kernel
-// needs does not fit (refine_smem_fits)
-int launch_refine_rows(const RefinePlan& p, const float* Q, int nq, const void* X, int elem_bytes, int d,
-                       int64_t ntotal, const int64_t* cand, int k_base, int k, float* D, int64_t* I, void* ws,
-                       cudaStream_t st, const TierArgs* tier = nullptr, const float* sq = nullptr);
+// All-device re-rank (s.n_dev == s.ntotal): cand [nq, k_base] ids (-1 = skip); returns <0 if the shared memory the
+// kernel needs does not fit (refine_smem_fits)
+int launch_refine_rows(const RefinePlan& p, const float* Q, int nq, const RefineStore& s, const int64_t* cand,
+                       int k_base, int k, float* D, int64_t* I, void* ws, cudaStream_t st);
 // Workspace of a tiered re-rank of nq queries: queries are processed qc at a time, qc = the queries whose worst case
 // (k_base * d * elem_bytes each) fits staging_bytes.  qc = 0: staging_bytes is below one query's worst case, or the
 // CUB temporary sizes could not be queried.
@@ -98,12 +102,10 @@ struct TieredPlan {
     size_t off_keys, off_keys2, off_vals, off_vals2, off_slot, off_uniq, off_count, off_cub, off_ref, off_stage, total;
 };
 TieredPlan tiered_plan(int nq, int k_base, int k, int d, int elem_bytes, size_t staging_bytes);
-// X_dev: rows [0, n_dev); X_host: device alias of the mapped host tier, rows [n_dev, ntotal) (n_dev < ntotal).
-// host_rows (nullable) += distinct host rows gathered.
-cudaError_t launch_refine_tiered(const TieredPlan& p, const float* Q, int nq, const void* X_dev, int64_t n_dev,
-                                 const void* X_host, int elem_bytes, int d, int64_t ntotal, const int64_t* cand,
+// Tiered re-rank (s.n_dev < s.ntotal).  host_rows (nullable) += distinct host rows gathered.
+cudaError_t launch_refine_tiered(const TieredPlan& p, const float* Q, int nq, const RefineStore& s, const int64_t* cand,
                                  int k_base, int k, float* D, int64_t* I, void* ws, long long* host_rows,
-                                 cudaStream_t st, const float* sq = nullptr);
+                                 cudaStream_t st);
 // SQ8 store (faiss ScalarQuantizer QT_8bit, RS_minmax, per dimension): x [n, d] fp32 (x_f16 = 0) or fp16 (x_f16 = 1);
 // sq [2, d] fp32 = (vmin, vdiff).  train: vmin = min over the rows, vdiff = max - vmin.  encode: codes [n, d] uint8.
 cudaError_t launch_sq8_train(const void* x, int x_f16, int64_t n, int d, float* sq, cudaStream_t st);

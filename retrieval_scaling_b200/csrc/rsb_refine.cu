@@ -199,45 +199,55 @@ static size_t refine_smem(const RefinePlan& p, int d, int elem_bytes) {
 }
 bool refine_smem_fits(const RefinePlan& p, int d, int elem_bytes) { return refine_smem(p, d, elem_bytes) <= 200 * 1024; }
 
+// tiered launch: rows id >= s.n_dev are read from staging + slot[q * k_base + j] * d
+struct TierArgs {
+    const void* staging;
+    const int* slot;      // [nq, k_base]
+};
+
 template <typename T, bool TIERED>
-static void launch_rows(const RefinePlan& p, dim3 grid, size_t smem, const float* Q, const void* X, int d, int64_t ntotal,
+static void launch_rows(const RefinePlan& p, dim3 grid, size_t smem, const float* Q, const RefineStore& s,
                         const int64_t* cand, int k_base, int k, int direct, float* D, int64_t* I, u64* keys, int* cnt,
-                        const TierArgs* tier, const float* sq, cudaStream_t st) {
+                        const TierArgs* tier, cudaStream_t st) {
     static PerDeviceSize configured;
     if (smem > 48 * 1024 && configured.raise(smem))
         cudaFuncSetAttribute(refine_rows_kernel<T, TIERED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     refine_rows_kernel<T, TIERED><<<grid, RF_THREADS, smem, st>>>(
-        Q, static_cast<const T*>(X), d, ntotal, cand, k_base, p.chunk, p.P, k, direct, D, I, keys, cnt,
-        TIERED ? tier->n_dev : ntotal, TIERED ? static_cast<const T*>(tier->staging) : nullptr,
-        TIERED ? tier->slot : nullptr, sq);
+        Q, static_cast<const T*>(s.dev), s.d, s.ntotal, cand, k_base, p.chunk, p.P, k, direct, D, I, keys, cnt,
+        s.n_dev, TIERED ? static_cast<const T*>(tier->staging) : nullptr, TIERED ? tier->slot : nullptr, s.sq);
 }
 
 template <typename T>
-static void launch_rows(const RefinePlan& p, dim3 grid, size_t smem, const float* Q, const void* X, int d, int64_t ntotal,
+static void launch_rows(const RefinePlan& p, dim3 grid, size_t smem, const float* Q, const RefineStore& s,
                         const int64_t* cand, int k_base, int k, int direct, float* D, int64_t* I, u64* keys, int* cnt,
-                        const TierArgs* tier, const float* sq, cudaStream_t st) {
-    if (tier) launch_rows<T, true>(p, grid, smem, Q, X, d, ntotal, cand, k_base, k, direct, D, I, keys, cnt, tier, sq, st);
-    else launch_rows<T, false>(p, grid, smem, Q, X, d, ntotal, cand, k_base, k, direct, D, I, keys, cnt, tier, sq, st);
+                        const TierArgs* tier, cudaStream_t st) {
+    if (tier) launch_rows<T, true>(p, grid, smem, Q, s, cand, k_base, k, direct, D, I, keys, cnt, tier, st);
+    else launch_rows<T, false>(p, grid, smem, Q, s, cand, k_base, k, direct, D, I, keys, cnt, tier, st);
 }
 
-int launch_refine_rows(const RefinePlan& p, const float* Q, int nq, const void* X, int elem_bytes, int d,
-                       int64_t ntotal, const int64_t* cand, int k_base, int k, float* D, int64_t* I, void* ws,
-                       cudaStream_t st, const TierArgs* tier, const float* sq) {
+// tier: null for the all-device store
+static int refine_rows(const RefinePlan& p, const float* Q, int nq, const RefineStore& s, const int64_t* cand,
+                       int k_base, int k, float* D, int64_t* I, void* ws, const TierArgs* tier, cudaStream_t st) {
     if (nq <= 0) return 0;
-    const size_t smem = refine_smem(p, d, elem_bytes);
-    if (!refine_smem_fits(p, d, elem_bytes)) return -1;
+    const size_t smem = refine_smem(p, s.d, s.elem_bytes);
+    if (!refine_smem_fits(p, s.d, s.elem_bytes)) return -1;
     const int direct = p.nchunks == 1;
     u64* keys = direct ? nullptr : static_cast<u64*>(ws);
     int* cnt = direct ? nullptr : reinterpret_cast<int*>(static_cast<unsigned char*>(ws) + (size_t)nq * p.nchunks * p.k_item * 8);
     dim3 grid(nq, p.nchunks);
-    if (elem_bytes == 1)
-        launch_rows<uint8_t>(p, grid, smem, Q, X, d, ntotal, cand, k_base, k, direct, D, I, keys, cnt, tier, sq, st);
-    else if (elem_bytes == 2)
-        launch_rows<__half>(p, grid, smem, Q, X, d, ntotal, cand, k_base, k, direct, D, I, keys, cnt, tier, sq, st);
+    if (s.elem_bytes == 1)
+        launch_rows<uint8_t>(p, grid, smem, Q, s, cand, k_base, k, direct, D, I, keys, cnt, tier, st);
+    else if (s.elem_bytes == 2)
+        launch_rows<__half>(p, grid, smem, Q, s, cand, k_base, k, direct, D, I, keys, cnt, tier, st);
     else
-        launch_rows<float>(p, grid, smem, Q, X, d, ntotal, cand, k_base, k, direct, D, I, keys, cnt, tier, sq, st);
+        launch_rows<float>(p, grid, smem, Q, s, cand, k_base, k, direct, D, I, keys, cnt, tier, st);
     if (!direct) launch_merge_items(keys, cnt, nq, p.nchunks, p.k_item, k, nullptr, 0, D, I, st);
     return 0;
+}
+
+int launch_refine_rows(const RefinePlan& p, const float* Q, int nq, const RefineStore& s, const int64_t* cand,
+                       int k_base, int k, float* D, int64_t* I, void* ws, cudaStream_t st) {
+    return refine_rows(p, Q, nq, s, cand, k_base, k, D, I, ws, nullptr, st);
 }
 
 // ---- tiered store: de-duplication of host-tier candidates, staged gather ------------------------------------------
@@ -368,10 +378,11 @@ int tiered_profile(int enable, double* ms3) {
     return 0;
 }
 
-cudaError_t launch_refine_tiered(const TieredPlan& p, const float* Q, int nq, const void* X_dev, int64_t n_dev,
-                                 const void* X_host, int elem_bytes, int d, int64_t ntotal, const int64_t* cand,
+cudaError_t launch_refine_tiered(const TieredPlan& p, const float* Q, int nq, const RefineStore& s, const int64_t* cand,
                                  int k_base, int k, float* D, int64_t* I, void* ws, long long* host_rows,
-                                 cudaStream_t st, const float* sq) {
+                                 cudaStream_t st) {
+    const int64_t n_dev = s.n_dev, ntotal = s.ntotal;
+    const int d = s.d;
     unsigned char* w = static_cast<unsigned char*>(ws);
     unsigned* keys = reinterpret_cast<unsigned*>(w + p.off_keys);
     unsigned* keys2 = reinterpret_cast<unsigned*>(w + p.off_keys2);
@@ -388,11 +399,11 @@ cudaError_t launch_refine_tiered(const TieredPlan& p, const float* Q, int nq, co
     while (bits < 32 && ((uint64_t)1 << bits) <= n_host) ++bits;     // n_host itself (the "not host" key) must fit
     uint4* staging = reinterpret_cast<uint4*>(w + p.off_stage);
     TierArgs tier;
-    tier.n_dev = n_dev;
     tier.staging = staging;
     tier.slot = slot;
     TierProfile& prof = g_tier_prof;
-    const size_t row_bytes = (size_t)d * elem_bytes;
+    const size_t row_bytes = (size_t)d * s.elem_bytes;
+    const uint4* host = static_cast<const uint4*>(s.host);
     for (int q0 = 0; q0 < nq; q0 += p.qc) {
         const int nc = std::min(p.qc, nq - q0);
         const int L = nc * k_base;
@@ -411,15 +422,15 @@ cudaError_t launch_refine_tiered(const TieredPlan& p, const float* Q, int nq, co
         if (prof.on) cudaEventRecord(prof.ev[1], st);
         const size_t words = (size_t)L * row_bytes / 16;
         const unsigned gb = (unsigned)((words + GH_THREADS * GH_U - 1) / (GH_THREADS * GH_U));
-        if (elem_bytes == 1)
-            gather_host_rows_kernel<uint8_t><<<gb, GH_THREADS, 0, st>>>(static_cast<const uint4*>(X_host), uniq, count, d, staging);
-        else if (elem_bytes == 2)
-            gather_host_rows_kernel<__half><<<gb, GH_THREADS, 0, st>>>(static_cast<const uint4*>(X_host), uniq, count, d, staging);
+        if (s.elem_bytes == 1)
+            gather_host_rows_kernel<uint8_t><<<gb, GH_THREADS, 0, st>>>(host, uniq, count, d, staging);
+        else if (s.elem_bytes == 2)
+            gather_host_rows_kernel<__half><<<gb, GH_THREADS, 0, st>>>(host, uniq, count, d, staging);
         else
-            gather_host_rows_kernel<float><<<gb, GH_THREADS, 0, st>>>(static_cast<const uint4*>(X_host), uniq, count, d, staging);
+            gather_host_rows_kernel<float><<<gb, GH_THREADS, 0, st>>>(host, uniq, count, d, staging);
         if (prof.on) cudaEventRecord(prof.ev[2], st);
-        if (launch_refine_rows(refine_plan(nc, k_base, k), Q + (size_t)q0 * d, nc, X_dev, elem_bytes, d, ntotal, cq,
-                               k_base, k, D + (size_t)q0 * k, I + (size_t)q0 * k, w + p.off_ref, st, &tier, sq) != 0)
+        if (refine_rows(refine_plan(nc, k_base, k), Q + (size_t)q0 * d, nc, s, cq, k_base, k, D + (size_t)q0 * k,
+                        I + (size_t)q0 * k, w + p.off_ref, &tier, st) != 0)
             return cudaErrorInvalidConfiguration;       // not reached: the caller checked p.smem_ok
         if (prof.on) {                                  // profiling only: waits for the chunk to read its events
             cudaEventRecord(prof.ev[3], st);

@@ -455,10 +455,10 @@ class IndexRefine:
     to a float32 store holding those rows.  d % 16 == 0.
 
     device_rows = n (an integer) makes the store tiered, for stores larger than device memory: rows [0, n) stay in
-    device memory and rows from n on go to page-locked, device-mapped host memory (rsb_search_refine_tiered).  Each
-    search gathers the distinct host rows its candidates need over PCIe, `staging_bytes` of queries' worst case at a
-    time; the results are bit-identical to an all-device store of the same values.  device_rows = None (default)
-    keeps every row on the device."""
+    device memory and rows from n on go to page-locked, device-mapped host memory.  Each search gathers the distinct
+    host rows its candidates need over PCIe, `staging_bytes` of queries' worst case at a time; the results are
+    bit-identical to an all-device store of the same values.  device_rows = None (default) keeps every row on the
+    device."""
 
     staging_bytes = 512 << 20           # tiered store: device staging buffer for the host rows of a chunk of queries
 
@@ -502,8 +502,6 @@ class IndexRefine:
         ids = torch.as_tensor(ids).to(device="cpu", dtype=torch.int64).reshape(-1)
         if ids.numel() and (int(ids.min()) < 0 or int(ids.max()) >= self._n):
             raise IndexError(f"store ids must be in [0, {self._n})")
-        if not self.tiered:
-            return self._store[ids.to(self.device)]
         out = torch.empty((ids.numel(), self.d), dtype=self._store.dtype, device=self.device)
         on_dev = ids < self.n_dev
         out[on_dev.to(self.device)] = self._store[ids[on_dev].to(self.device)]
@@ -634,13 +632,12 @@ class IndexRefine:
         self._n += n
         torch.cuda.current_stream(self.device).synchronize()     # x may be a temporary
 
-    def _tier_args(self):
-        """(device tier, n_dev, host tier pointer) of rsb_*_tiered."""
-        return _ptr(self._store), self.n_dev, _ptr(self.host_store)
-
-    def _sq_ptr(self):
-        self.sq_params                                              # ValueError if the quantizer is untrained
-        return _ptr(self._sq)
+    def _store_args(self):
+        """(device tier, n_dev, host tier, store dtype code, SQ8 range) of rsb_refine / rsb_search_refine.  A store
+        that is not tiered is all-device: n_dev = ntotal and an empty host tier."""
+        if self.store_dtype == "sq8":
+            self.sq_params                                          # ValueError if the quantizer is untrained
+        return _ptr(self._store), self.n_dev, _ptr(self.host_store), _REFINE_DTYPES[self.store_dtype][1], _ptr(self._sq)
 
     def search_ids(self, q, k: int, nprobe: Optional[int] = None, k_factor: Optional[int] = None,
                    host_rows: Optional[torch.Tensor] = None):
@@ -657,24 +654,12 @@ class IndexRefine:
             I = torch.empty((nq, k), dtype=torch.int64, device=self.device)
             if nq == 0:
                 return I, D
-            if self.store_dtype == "sq8":                   # all-device (n_dev = ntotal) or tiered: one entry point
-                sb = int(self.staging_bytes)
-                ws = self.base._workspace(self.L.rsb_search_refine_sq8_workspace_bytes(self.base._h, nq, k, kf, npb, sb))
-                _lib.check(self.L.rsb_search_refine_sq8(
-                    self.base._h, _ptr(q), nq, k, kf, npb, *self._tier_args(), self._sq_ptr(), self._n, _ptr(D), _ptr(I),
-                    _ptr(ws), ws.numel(), sb, _ptr(host_rows), _stream()))
-                return I, D
-            if self.tiered:
-                sb = int(self.staging_bytes)
-                ws = self.base._workspace(self.L.rsb_search_refine_tiered_workspace_bytes(self.base._h, nq, k, kf, npb, sb))
-                _lib.check(self.L.rsb_search_refine_tiered(
-                    self.base._h, _ptr(q), nq, k, kf, npb, *self._tier_args(), _STORE_DTYPES[self.store_dtype][1],
-                    self._n, _ptr(D), _ptr(I), _ptr(ws), ws.numel(), sb, _ptr(host_rows), _stream()))
-                return I, D
-            ws = self.base._workspace(self.L.rsb_search_refine_workspace_bytes(self.base._h, nq, k, kf, npb))
-            _lib.check(self.L.rsb_search_refine(self.base._h, _ptr(q), nq, k, kf, npb, _ptr(self._store),
-                                                _STORE_DTYPES[self.store_dtype][1], self._n, _ptr(D), _ptr(I), _ptr(ws),
-                                                ws.numel(), _stream()))
+            dev, n_dev, host, dt, sq = self._store_args()
+            sb = int(self.staging_bytes)
+            ws = self.base._workspace(self.L.rsb_search_refine_workspace_bytes(self.base._h, nq, k, kf, npb, dt, n_dev,
+                                                                               self._n, sb))
+            _lib.check(self.L.rsb_search_refine(self.base._h, _ptr(q), nq, k, kf, npb, dev, n_dev, host, dt, sq, self._n,
+                                                _ptr(D), _ptr(I), _ptr(ws), ws.numel(), sb, _ptr(host_rows), _stream()))
             return I, D
 
     def search(self, x, k: int):
@@ -686,33 +671,19 @@ class IndexRefine:
 
     def rerank(self, q: torch.Tensor, cand: torch.Tensor, k: int, staging_bytes: Optional[int] = None,
                host_rows: Optional[torch.Tensor] = None):
-        """The re-rank step alone (rsb_refine / rsb_refine_tiered): candidates cand [nq, k_base] int64 (-1 = none) ->
-        (ids, scores) [nq, k].  staging_bytes and host_rows apply to a tiered store (see search_ids)."""
+        """The re-rank step alone (rsb_refine): candidates cand [nq, k_base] int64 (-1 = none) -> (ids, scores)
+        [nq, k].  staging_bytes and host_rows apply to a tiered store (see search_ids)."""
         with torch.cuda.device(self.device):
             q = _dev_f32(q, self.device)
             cand = cand.to(device=self.device, dtype=torch.int64).contiguous()
             nq, k_base = cand.shape
             D = torch.empty((nq, int(k)), dtype=torch.float32, device=self.device)
             I = torch.empty((nq, int(k)), dtype=torch.int64, device=self.device)
-            if self.store_dtype == "sq8":
-                sb = int(self.staging_bytes if staging_bytes is None else staging_bytes)
-                ws = self.base._workspace(self.L.rsb_refine_sq8_workspace_bytes(nq, k_base, int(k), self.d, sb))
-                _lib.check(self.L.rsb_refine_sq8(_ptr(q), nq, *self._tier_args(), self._sq_ptr(), self.d, self._n,
-                                                 _ptr(cand), k_base, int(k), _ptr(D), _ptr(I), _ptr(ws), ws.numel(), sb,
-                                                 _ptr(host_rows), _stream()))
-                return I, D
-            if self.tiered:
-                sb = int(self.staging_bytes if staging_bytes is None else staging_bytes)
-                dt = _STORE_DTYPES[self.store_dtype][1]
-                ws = self.base._workspace(self.L.rsb_refine_tiered_workspace_bytes(nq, k_base, int(k), self.d, dt, sb))
-                _lib.check(self.L.rsb_refine_tiered(_ptr(q), nq, *self._tier_args(), dt, self.d, self._n, _ptr(cand),
-                                                    k_base, int(k), _ptr(D), _ptr(I), _ptr(ws), ws.numel(), sb,
-                                                    _ptr(host_rows), _stream()))
-                return I, D
-            ws = self.base._workspace(self.L.rsb_refine_workspace_bytes(nq, k_base, int(k)))
-            _lib.check(self.L.rsb_refine(_ptr(q), nq, _ptr(self._store), _STORE_DTYPES[self.store_dtype][1], self.d,
-                                         self._n, _ptr(cand), k_base, int(k), _ptr(D), _ptr(I), _ptr(ws), ws.numel(),
-                                         _stream()))
+            dev, n_dev, host, dt, sq = self._store_args()
+            sb = int(self.staging_bytes if staging_bytes is None else staging_bytes)
+            ws = self.base._workspace(self.L.rsb_refine_workspace_bytes(nq, k_base, int(k), self.d, dt, n_dev, self._n, sb))
+            _lib.check(self.L.rsb_refine(_ptr(q), nq, dev, n_dev, host, dt, sq, self.d, self._n, _ptr(cand), k_base,
+                                         int(k), _ptr(D), _ptr(I), _ptr(ws), ws.numel(), sb, _ptr(host_rows), _stream()))
             return I, D
 
 
@@ -730,13 +701,13 @@ MAGIC = "RSB1"
 
 def _to_faiss_parts(index: _IndexBase) -> dict:
     if isinstance(index, IndexRefine):
+        rows = torch.cat([index.device_store.cpu(), index.host_store])
         if index.store_dtype == "sq8":      # faiss IndexRefine with an IndexScalarQuantizer(QT_8bit) refine index
-            codes = torch.cat([index.device_store.cpu(), index.host_store]) if index.tiered else index.store.cpu()
             return {"kind": "Refine", "d": index.d, "ntotal": index.ntotal, "base": _to_faiss_parts(index.base),
-                    "sq": torch.stack(index.sq_params).cpu().numpy(), "codes": codes.numpy(),
+                    "sq": torch.stack(index.sq_params).cpu().numpy(), "codes": rows.numpy(),
                     "k_factor": float(index.k_factor)}
         # faiss IndexRefineFlat: an fp16 store is written upcast to fp32 (exact)
-        xb = torch.cat([index.device_store.float().cpu(), index.host_store.float()]) if index.tiered else index.store.float().cpu()
+        xb = rows.float()
         return {"kind": "Refine", "d": index.d, "ntotal": index.ntotal, "base": _to_faiss_parts(index.base),
                 "xb": xb.numpy(), "k_factor": float(index.k_factor)}
     off, payload, ids = index.export_lists()

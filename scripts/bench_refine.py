@@ -395,17 +395,17 @@ def tiered_profile(L, enable):
 
 
 def zero_copy_rerank(ref, q, Ib, k):
-    """The all-device kernel (rsb_refine) handed the mapped host tier directly (n_dev = 0): every candidate row crosses
-    PCIe once per query, no de-duplication, no staging."""
+    """The all-device kernel (rsb_refine with n_dev = ntotal) handed the mapped host tier of a --device-rows 0 store
+    directly as its device rows: every candidate row crosses PCIe once per query, no de-duplication, no staging."""
     from retrieval_scaling_b200 import _lib
     from retrieval_scaling_b200.index import _ptr, _stream
     nq, kb = Ib.shape
     D = torch.empty((nq, k), dtype=torch.float32, device=ref.device)
     I = torch.empty((nq, k), dtype=torch.int64, device=ref.device)
-    ws = ref.base._workspace(ref.L.rsb_refine_workspace_bytes(nq, kb, k))
     dt = _lib.RSB_DTYPE_F16 if ref.store_dtype == "float16" else _lib.RSB_DTYPE_F32
-    _lib.check(ref.L.rsb_refine(_ptr(q), nq, _ptr(ref.host_store), dt, ref.d, ref.ntotal, _ptr(Ib), kb, k,
-                                _ptr(D), _ptr(I), _ptr(ws), ws.numel(), _stream()))
+    ws = ref.base._workspace(ref.L.rsb_refine_workspace_bytes(nq, kb, k, ref.d, dt, ref.ntotal, ref.ntotal, 0))
+    _lib.check(ref.L.rsb_refine(_ptr(q), nq, _ptr(ref.host_store), ref.ntotal, None, dt, None, ref.d, ref.ntotal,
+                                _ptr(Ib), kb, k, _ptr(D), _ptr(I), _ptr(ws), ws.numel(), 0, None, _stream()))
     return I, D
 
 
@@ -475,7 +475,7 @@ def tiered_main(args, device):
             row["zero_copy_same_result"] = bool(torch.equal(Iz, Ir) and torch.equal(Dz, Dr))
         else:
             row["zero_copy_rerank_ms"] = ("not measured (needs --device-rows 0: rsb_refine reads one contiguous store)"
-                                          if dtype != "sq8" else "not measured (rsb_refine has no sq8 form)")
+                                          if dtype != "sq8" else "not measured (fp16 / fp32 stores only)")
         if "device" in stores:
             full = stores["device"]
             ms_dev, (Id, Dd) = timed(lambda: full.search_ids(xq, k), args.steps, args.warmup)

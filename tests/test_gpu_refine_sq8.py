@@ -1,8 +1,9 @@
-"""SQ8 re-rank store on the GPU (IndexRefine(store_dtype="sq8"), rsb_sq8_train / rsb_sq8_encode / rsb_refine_sq8 /
-rsb_search_refine_sq8): training and encoding equal to the CPU oracle bit for bit (every code occurs in every dimension,
-so the decode is checked exhaustively), results byte-identical to an fp32 store holding the decoded rows for the
-split-query and direct paths, k' up to 4096, padding and out-of-range candidates, every tier split, the oracle, the
-IxRF + IxSQ round trip, and the Indexer(cfg) integration with `refine_dtype=sq8`."""
+"""SQ8 re-rank store on the GPU (IndexRefine(store_dtype="sq8"), rsb_sq8_train / rsb_sq8_encode / rsb_refine /
+rsb_search_refine with RSB_DTYPE_SQ8): training and encoding equal to the CPU oracle bit for bit (every code occurs in
+every dimension, so the decode is checked exhaustively), results byte-identical to an fp32 store holding the decoded
+rows for the split-query and direct paths, k' up to 4096, padding and out-of-range candidates, every tier split, the
+all-device workspace, the oracle, the IxRF + IxSQ round trip, and the Indexer(cfg) integration with
+`refine_dtype=sq8`."""
 import os
 import sys
 
@@ -170,7 +171,7 @@ def test_oracle_parity():
     O.assert_topk_equivalent(D.cpu().numpy(), I.cpu().numpy(), Do, Io, score_of=score_of, rtol=1e-5, atol=1e-5)
 
 
-def test_existing_entry_points_refuse_sq8_before_any_launch():
+def test_sq8_store_without_range_is_refused_before_any_launch():
     from retrieval_scaling_b200 import _lib
     from retrieval_scaling_b200.index import _ptr, _stream
     L = _lib.lib()
@@ -180,15 +181,47 @@ def test_existing_entry_points_refuse_sq8_before_any_launch():
     D = torch.full((nq, k), 7.0, device="cuda")
     I = torch.full((nq, k), 7, dtype=torch.int64, device="cuda")
     ws = torch.empty(64 << 20, dtype=torch.uint8, device="cuda")
-    h, st = sq8.base._h, _stream()
-    rcs = [L.rsb_search_refine(h, _ptr(q), nq, k, kf, 8, _ptr(sq8._store), _lib.RSB_DTYPE_SQ8, N, _ptr(D), _ptr(I),
-                               _ptr(ws), ws.numel(), st),
-           L.rsb_search_refine_tiered(h, _ptr(q), nq, k, kf, 8, _ptr(sq8._store), N, None, _lib.RSB_DTYPE_SQ8, N, _ptr(D),
-                                      _ptr(I), _ptr(ws), ws.numel(), 1 << 20, None, st)]
+    h, st, SQ8 = sq8.base._h, _stream(), _lib.RSB_DTYPE_SQ8
+    # all-device, then tiered (the host tier pointer is never read: the range is checked first)
+    rcs = [L.rsb_search_refine(h, _ptr(q), nq, k, kf, 8, _ptr(sq8._store), N, None, SQ8, None, N, _ptr(D), _ptr(I),
+                               _ptr(ws), ws.numel(), 0, None, st),
+           L.rsb_search_refine(h, _ptr(q), nq, k, kf, 8, _ptr(sq8._store), N // 2, _ptr(sq8._store[N // 2:]), SQ8, None,
+                               N, _ptr(D), _ptr(I), _ptr(ws), ws.numel(), 1 << 20, None, st)]
     for rc in rcs:
-        assert rc == _lib.RSB_ERR_INVALID and b"rsb_refine_sq8" in L.rsb_last_error()
+        assert rc == _lib.RSB_ERR_INVALID and b"sq_dev" in L.rsb_last_error()
     torch.cuda.synchronize()
     assert (D == 7.0).all() and (I == 7).all()
+
+
+def _refine_plan_bytes(nq, k_base, k):
+    """The all-device re-rank's workspace restated: partial keys and counts when a query's candidates are split over
+    several CTAs (at least 256 candidates each, about four CTAs per SM in all)."""
+    sms = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+    nchunks = max(1, min(max(1, k_base // 256), (4 * sms + nq - 1) // nq))
+    chunk = (k_base + nchunks - 1) // nchunks
+    nchunks = (k_base + chunk - 1) // chunk
+    return nq * nchunks * (min(k, chunk) * 8 + 4) + 16 if nchunks > 1 else 0
+
+
+def test_all_device_workspace_holds_no_staging_buffer():
+    """n_dev = ntotal: the SQ8 and fp16 workspace queries agree, do not depend on staging_bytes, and equal the plain
+    re-rank's size (a staging buffer and its sort buffers are reserved for a tiered store only)."""
+    from retrieval_scaling_b200 import _lib
+    L = _lib.lib()
+    F16, SQ8 = _lib.RSB_DTYPE_F16, _lib.RSB_DTYPE_SQ8
+    al = lambda x: (x + 255) // 256 * 256                                  # noqa: E731
+    for d in (64, 768):
+        h = _base(d)._h
+        for nq, k, kf in ((1, 10, 8), (64, 100, 8), (10000, 100, 8)):
+            kb = k * kf
+            want_search = (al(L.rsb_workspace_bytes(h, nq, kb, 8)) + al(nq * kb * 4) + al(nq * kb * 8)
+                           + al(_refine_plan_bytes(nq, kb, k)))
+            for sb in (0, 1 << 20, 512 << 20):
+                for dt in (F16, SQ8):
+                    assert L.rsb_refine_workspace_bytes(nq, kb, k, d, dt, N, N, sb) == _refine_plan_bytes(nq, kb, k)
+                    assert L.rsb_search_refine_workspace_bytes(h, nq, k, kf, 8, dt, N, N, sb) == want_search
+        tiered = [L.rsb_search_refine_workspace_bytes(h, 10000, 100, 8, 8, SQ8, 0, N, sb) for sb in (1 << 20, 512 << 20)]
+        assert want_search < tiered[0] < tiered[1]                         # the tiered store sizes its staging buffer
 
 
 def test_write_read_round_trip(tmp_path):

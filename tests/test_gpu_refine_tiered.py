@@ -1,7 +1,7 @@
-"""Tiered re-rank store on the GPU (IndexRefine(device_rows=...), rsb_refine_tiered / rsb_search_refine_tiered): results
-byte-identical to the all-device store for every split of the rows, the host-row de-duplication counts, ragged query
-chunks, padding and out-of-range candidates, refusal of host tiers a kernel cannot read, parity with the CPU oracle,
-and the Indexer(cfg) integration with `refine_device_rows`."""
+"""Tiered re-rank store on the GPU (IndexRefine(device_rows=...), rsb_refine / rsb_search_refine with n_dev < ntotal):
+results byte-identical to the all-device store for every split of the rows, the host-row de-duplication counts, ragged
+query chunks, padding and out-of-range candidates, refusal of host tiers a kernel cannot read, parity with the CPU
+oracle, and the Indexer(cfg) integration with `refine_device_rows`."""
 import ctypes
 import os
 import sys
@@ -136,7 +136,7 @@ def test_straddling_padding_and_out_of_range_candidates():
         tier.rerank(q, cand, k, staging_bytes=_per_query(tier, kb) - 16)
 
 
-def test_unreadable_host_tiers_are_refused_before_any_launch():
+def test_rsb_refine_refuses_unreadable_host_tiers_before_any_launch():
     from retrieval_scaling_b200 import _lib
     from retrieval_scaling_b200.index import _ptr, _stream
     L = _lib.lib()
@@ -147,13 +147,13 @@ def test_unreadable_host_tiers_are_refused_before_any_launch():
     D = torch.full((nq, k), 7.0, device="cuda")
     I = torch.full((nq, k), 7, dtype=torch.int64, device="cuda")
     rows = torch.zeros(1, dtype=torch.int64, device="cuda")
-    ws = torch.empty(L.rsb_refine_tiered_workspace_bytes(nq, kb, k, d, _lib.RSB_DTYPE_F32, 1 << 20), dtype=torch.uint8,
+    ws = torch.empty(L.rsb_refine_workspace_bytes(nq, kb, k, d, _lib.RSB_DTYPE_F32, 0, N, 1 << 20), dtype=torch.uint8,
                      device="cuda")
     pageable = np.zeros((N, d), np.float32)
     device_mem = torch.zeros((N, d), device="cuda")
     for host in (ctypes.c_void_p(pageable.ctypes.data), _ptr(device_mem)):
-        rc = L.rsb_refine_tiered(_ptr(q), nq, None, 0, host, _lib.RSB_DTYPE_F32, d, N, _ptr(cand), kb, k, _ptr(D), _ptr(I),
-                                 _ptr(ws), ws.numel(), 1 << 20, _ptr(rows), _stream())
+        rc = L.rsb_refine(_ptr(q), nq, None, 0, host, _lib.RSB_DTYPE_F32, None, d, N, _ptr(cand), kb, k, _ptr(D), _ptr(I),
+                          _ptr(ws), ws.numel(), 1 << 20, _ptr(rows), _stream())
         assert rc == _lib.RSB_ERR_INVALID, L.rsb_last_error()
         assert b"host tier" in L.rsb_last_error()
     torch.cuda.synchronize()

@@ -114,16 +114,19 @@ def test_config_keys():
         Indexer.refine_options(cfg.datastore.index)
 
 
-def test_c_abi_argument_checks():
+def test_all_device_refine_argument_checks():
     L = _lib.lib()
     z = None
     # k * k_factor beyond the scan's 4096 limit: unsupported, reported, not a fault
-    assert L.rsb_refine(z, 1, z, _lib.RSB_DTYPE_F16, 768, 0, z, 4097, 10, z, z, z, 0, z) == _lib.RSB_ERR_UNSUPPORTED
+    # an all-device store (n_dev = ntotal): store_host, sq_dev and staging_bytes are ignored
+    def refine(dtype, d, k_base, k):
+        return L.rsb_refine(z, 1, z, 0, z, dtype, z, d, 0, z, k_base, k, z, z, z, 0, 0, z, z)
+    assert refine(_lib.RSB_DTYPE_F16, 768, 4097, 10) == _lib.RSB_ERR_UNSUPPORTED
     assert b"4096" in L.rsb_last_error()
-    assert L.rsb_refine(z, 1, z, 7, 768, 0, z, 100, 10, z, z, z, 0, z) == _lib.RSB_ERR_INVALID        # dtype
-    assert L.rsb_refine(z, 1, z, _lib.RSB_DTYPE_F32, 768, 0, z, 5, 10, z, z, z, 0, z) == _lib.RSB_ERR_INVALID  # k > k_base
-    assert L.rsb_refine(z, 1, z, _lib.RSB_DTYPE_F32, 36, 0, z, 50, 10, z, z, z, 0, z) == _lib.RSB_ERR_INVALID  # d % 8
-    assert L.rsb_search_refine(z, z, 1, 10, 4, 8, z, 0, 0, z, z, z, 0, z) == _lib.RSB_ERR_INVALID         # null handle
+    assert refine(7, 768, 100, 10) == _lib.RSB_ERR_INVALID                                        # dtype
+    assert refine(_lib.RSB_DTYPE_F32, 768, 5, 10) == _lib.RSB_ERR_INVALID                         # k > k_base
+    assert refine(_lib.RSB_DTYPE_F32, 36, 50, 10) == _lib.RSB_ERR_INVALID                         # d % 8
+    assert L.rsb_search_refine(z, z, 1, 10, 4, 8, z, 0, z, 0, z, 0, z, z, z, 0, 0, z, z) == _lib.RSB_ERR_INVALID  # null handle
 
 
 def test_faiss_cross_check():

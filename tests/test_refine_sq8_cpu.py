@@ -144,30 +144,30 @@ def test_config_key():
             Indexer.refine_options(cfg.datastore.index)
 
 
-def test_c_abi_argument_checks():
+def test_sq8_store_argument_checks():
     L = _lib.lib()
     z = None
     SQ8 = _lib.RSB_DTYPE_SQ8
     assert SQ8 == 2
-    # the fp16 / fp32 entry points refuse an SQ8 store, and name the entry point that takes its range
-    # (rsb_search_refine / rsb_search_refine_tiered check their handle first: tests/test_gpu_refine_sq8.py)
-    for rc in (L.rsb_refine(z, 1, z, SQ8, 768, 0, z, 100, 10, z, z, z, 0, z),
-               L.rsb_refine_tiered(z, 1, z, 0, z, SQ8, 768, 0, z, 100, 10, z, z, z, 0, 1 << 30, z, z)):
+    # an SQ8 store without its range is refused, naming sq_dev
+    # (rsb_search_refine checks its handle first: tests/test_gpu_refine_sq8.py)
+    for rc in (L.rsb_refine(z, 1, z, 0, z, SQ8, z, 768, 0, z, 100, 10, z, z, z, 0, 0, z, z),
+               L.rsb_refine(z, 1, z, 0, FAKE_HOST, SQ8, z, 768, 1000, z, 100, 10, z, z, z, 0, 1 << 30, z, z)):
         assert rc == _lib.RSB_ERR_INVALID
-        assert b"rsb_refine_sq8" in L.rsb_last_error()
-    assert L.rsb_refine_tiered_workspace_bytes(1, 100, 10, 768, SQ8, 1 << 30) == 0
-    # rsb_refine_sq8: d % 16, k' > 4096, null range, staging below one query's worst case, null handle
+        assert b"sq_dev" in L.rsb_last_error()
+    # d % 16, k' > 4096, null range, staging below one query's worst case, null handle
     sq = ctypes_ptr(16)
-    assert L.rsb_refine_sq8(z, 1, z, 0, z, sq, 40, 0, z, 100, 10, z, z, z, 0, 1 << 30, z, z) == _lib.RSB_ERR_INVALID
+    assert L.rsb_refine(z, 1, z, 0, z, SQ8, sq, 40, 0, z, 100, 10, z, z, z, 0, 1 << 30, z, z) == _lib.RSB_ERR_INVALID
     assert b"16" in L.rsb_last_error()
-    assert L.rsb_refine_sq8(z, 1, z, 0, z, sq, 768, 0, z, 4097, 10, z, z, z, 0, 1 << 30, z, z) == _lib.RSB_ERR_UNSUPPORTED
-    assert L.rsb_refine_sq8(z, 1, z, 0, z, z, 768, 0, z, 100, 10, z, z, z, 0, 1 << 30, z, z) == _lib.RSB_ERR_INVALID
+    assert L.rsb_refine(z, 1, z, 0, z, SQ8, sq, 768, 0, z, 4097, 10, z, z, z, 0, 1 << 30, z, z) == _lib.RSB_ERR_UNSUPPORTED
+    assert L.rsb_refine(z, 1, z, 0, z, SQ8, z, 768, 0, z, 100, 10, z, z, z, 0, 1 << 30, z, z) == _lib.RSB_ERR_INVALID
     assert b"sq_dev" in L.rsb_last_error()
-    assert L.rsb_refine_sq8(z, 1, z, 0, z, ctypes_ptr(8), 768, 0, z, 100, 10, z, z, z, 0, 1 << 30, z, z) == _lib.RSB_ERR_INVALID
-    assert L.rsb_refine_sq8(z, 1, z, 0, z, sq, 768, 0, z, 100, 10, z, z, z, 0, 100 * 768 - 1, z, z) == _lib.RSB_ERR_INVALID
+    assert L.rsb_refine(z, 1, z, 0, z, SQ8, ctypes_ptr(8), 768, 0, z, 100, 10, z, z, z, 0, 1 << 30, z, z) == _lib.RSB_ERR_INVALID
+    # staging is checked for a tiered store only (n_dev < ntotal)
+    assert L.rsb_refine(z, 1, z, 0, FAKE_HOST, SQ8, sq, 768, 1000, z, 100, 10, z, z, z, 0, 100 * 768 - 1, z, z) == _lib.RSB_ERR_INVALID
     assert b"staging_bytes" in L.rsb_last_error()
-    assert L.rsb_search_refine_sq8(z, z, 1, 10, 4, 8, z, 0, z, sq, 0, z, z, z, 0, 1 << 30, z, z) == _lib.RSB_ERR_INVALID
-    assert L.rsb_refine_sq8_workspace_bytes(1, 100, 10, 40, 1 << 30) == 0          # d % 16
+    assert L.rsb_search_refine(z, z, 1, 10, 4, 8, z, 0, z, SQ8, sq, 0, z, z, z, 0, 1 << 30, z, z) == _lib.RSB_ERR_INVALID
+    assert L.rsb_refine_workspace_bytes(1, 100, 10, 40, SQ8, 0, 0, 1 << 30) == 0          # d % 16
     # train / encode: dtype, n, d, null pointers
     assert L.rsb_sq8_train(z, 7, 10, 16, sq, z) == _lib.RSB_ERR_INVALID
     assert L.rsb_sq8_train(z, _lib.RSB_DTYPE_F32, 0, 16, sq, z) == _lib.RSB_ERR_INVALID
@@ -175,6 +175,9 @@ def test_c_abi_argument_checks():
     assert L.rsb_sq8_encode(sq, _lib.RSB_DTYPE_F16, 10, 0, sq, sq, z) == _lib.RSB_ERR_INVALID
     assert L.rsb_sq8_encode(sq, _lib.RSB_DTYPE_F32, 10, 16, z, sq, z) == _lib.RSB_ERR_INVALID
     assert L.rsb_sq8_encode(sq, _lib.RSB_DTYPE_F32, 10, 16, sq, z, z) == _lib.RSB_ERR_INVALID
+
+
+FAKE_HOST = 1 << 20            # a non-null, 16-byte aligned host tier address: never dereferenced by the checks above
 
 
 def ctypes_ptr(align):

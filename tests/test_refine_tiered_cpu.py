@@ -1,4 +1,4 @@
-"""Tiered re-rank store (rows past `refine_device_rows` in pinned host memory) without a GPU: the config key, the new
+"""Tiered re-rank store (rows past `refine_device_rows` in pinned host memory) without a GPU: the config key, the
 C-ABI symbols, and the argument checks that return before any CUDA call."""
 import ctypes
 import os
@@ -7,8 +7,8 @@ import pytest
 
 from retrieval_scaling_b200 import _lib
 
-NEW_SYMBOLS = ("rsb_host_alloc", "rsb_host_free", "rsb_refine_tiered_workspace_bytes", "rsb_refine_tiered",
-               "rsb_search_refine_tiered_workspace_bytes", "rsb_search_refine_tiered", "rsb_refine_tiered_profile")
+REFINE_SYMBOLS = ("rsb_host_alloc", "rsb_host_free", "rsb_refine_workspace_bytes", "rsb_refine",
+               "rsb_search_refine_workspace_bytes", "rsb_search_refine", "rsb_refine_tiered_profile")
 F16, F32 = _lib.RSB_DTYPE_F16, _lib.RSB_DTYPE_F32
 INVALID = _lib.RSB_ERR_INVALID
 FAKE_HOST = 1 << 20            # a non-null, 16-byte aligned address: never dereferenced by the checks tested here
@@ -45,21 +45,21 @@ def test_index_refine_device_rows_argument():
             _check_device_rows(bad)
 
 
-def test_new_symbols_are_exported_and_bound():
+def test_refine_symbols_are_exported_and_bound():
     L = _lib.lib()
     bound = {name for name, _, _ in _lib.SIGNATURES}
-    for name in NEW_SYMBOLS:
+    for name in REFINE_SYMBOLS:
         assert name in bound and hasattr(L, name)
 
 
 def _tiered(q=None, nq=1, store_dev=None, n_dev=0, store_host=FAKE_HOST, dtype=F16, d=768, ntotal=1000, cand=None,
             k_base=800, k=100, D=None, I=None, staging=800 * 768 * 2):
     L = _lib.lib()
-    return L.rsb_refine_tiered(q, nq, store_dev, n_dev, store_host, dtype, d, ntotal, cand, k_base, k, D, I, None, 0,
-                               staging, None, None)
+    return L.rsb_refine(q, nq, store_dev, n_dev, store_host, dtype, None, d, ntotal, cand, k_base, k, D, I, None, 0,
+                        staging, None, None)
 
 
-def test_argument_checks_before_any_cuda_call():
+def test_tiered_store_argument_checks_before_any_cuda_call():
     L = _lib.lib()
     assert _tiered(dtype=7) == INVALID and b"store_dtype" in L.rsb_last_error()
     for n_dev in (-1, 1001):
@@ -72,11 +72,11 @@ def test_argument_checks_before_any_cuda_call():
     assert _tiered(q=None) == INVALID and b"null" in L.rsb_last_error()            # queries / candidates / outputs
     assert _tiered(k_base=4097) == _lib.RSB_ERR_UNSUPPORTED
     assert _tiered(nq=0) == _lib.RSB_OK
-    assert L.rsb_search_refine_tiered(None, None, 1, 10, 4, 8, None, 0, FAKE_HOST, F16, 0, None, None, None, 0,
-                                      1 << 20, None, None) == INVALID            # null handle
-    assert L.rsb_refine_tiered_workspace_bytes(1, 800, 100, 768, 7, 1 << 30) == 0
-    assert L.rsb_refine_tiered_workspace_bytes(1, 10, 100, 768, F16, 1 << 30) == 0     # k > k_base
-    assert L.rsb_search_refine_tiered_workspace_bytes(None, 1, 10, 4, 8, 1 << 30) == 0
+    assert L.rsb_search_refine(None, None, 1, 10, 4, 8, None, 0, FAKE_HOST, F16, None, 0, None, None, None, 0,
+                               1 << 20, None, None) == INVALID                   # null handle
+    assert L.rsb_refine_workspace_bytes(1, 800, 100, 768, 7, 0, 1000, 1 << 30) == 0
+    assert L.rsb_refine_workspace_bytes(1, 10, 100, 768, F16, 0, 1000, 1 << 30) == 0     # k > k_base
+    assert L.rsb_search_refine_workspace_bytes(None, 1, 10, 4, 8, F16, 0, 1000, 1 << 30) == 0
 
 
 def test_host_alloc_arguments():
