@@ -29,14 +29,14 @@
 extern "C" {
 #endif
 
-#define RSB_VERSION 200 /* 0.2.0 */
+#define RSB_VERSION 300 /* 0.3.0 */
 
 enum {
     RSB_OK = 0,
     RSB_ERR_INVALID = -1,     /* bad argument                         -> ValueError          */
     RSB_ERR_CUDA = -2,        /* CUDA runtime / launch failure        -> RuntimeError        */
     RSB_ERR_STATE = -3,       /* e.g. search before train             -> RuntimeError        */
-    RSB_ERR_UNSUPPORTED = -4, /* e.g. nbits != 8                      -> NotImplementedError */
+    RSB_ERR_UNSUPPORTED = -4, /* e.g. nbits = 6                       -> NotImplementedError */
     RSB_ERR_OOM = -5          /* cudaMalloc failed / workspace small  -> MemoryError         */
 };
 
@@ -49,41 +49,39 @@ int rsb_version(void);
 const char* rsb_last_error(void);
 
 /* ---- construction -------------------------------------------------------------------------------- */
-/* faiss.IndexFlatIP(d)                                               <- src/indicies/flat.py:42        */
-int rsb_flat_create(int d, rsb_index_t** out);
-/* faiss.IndexIVFFlat(IndexFlatIP(d), d, nlist, METRIC_INNER_PRODUCT) <- src/indicies/ivf_flat.py:143-149 */
-int rsb_ivfflat_create(int d, int nlist, rsb_index_t** out);
+/* dtype: storage dtype of the vectors (enum RSB_DTYPE_* below; anything else: RSB_ERR_INVALID).
+ *   RSB_DTYPE_F32   fp32 rows.
+ *   RSB_DTYPE_F16   every row as fp16 -- the embedding task writes fp16 passage embeddings (src/embed.py:137-138)
+ *     and the reference upcasts them only on load (src/indicies/flat.py:86), so fp16 storage of them is lossless at
+ *     half the bytes.  faiss equivalent: IndexScalarQuantizer / IndexIVFScalarQuantizer(QT_fp16, METRIC_INNER_PRODUCT,
+ *     no residual).  Stored values are the fp16 rounding (to nearest even) of what is added; scores are exact fp32
+ *     inner products of the fp32 query with the decoded rows.  d % 8 == 0 (16-byte rows), else RSB_ERR_INVALID. */
+/* faiss.IndexFlatIP(d)                           <- src/indicies/flat.py:42, ric/conf/default.yaml `index_type: Flat`
+ * fp16 rows are scored on wgmma tensor cores from the fp16 rows themselves (scaled fp16 hi/lo query split, then an
+ * exact fp32 re-score) and need d % 64 == 0, else RSB_ERR_UNSUPPORTED.  Final scores equal the fp32 index's wherever
+ * both return the same id. */
+int rsb_flat_create(int d, int dtype, rsb_index_t** out);
+/* faiss.IndexIVFFlat(IndexFlatIP(d), d, nlist, METRIC_INNER_PRODUCT)
+ *                                                    <- src/indicies/ivf_flat.py:143-149, api/conf/ivf_flat.yaml
+ * With fp16 rows the list scan reads 2 bytes per element and adds in the fp32 scan's order: ids and scores are
+ * bit-identical to an fp32 index holding the same values. */
+int rsb_ivfflat_create(int d, int nlist, int dtype, rsb_index_t** out);
 /* faiss.IndexIVFPQ(IndexFlatIP(d), d, nlist, M, nbits, METRIC_INNER_PRODUCT)
  *                                                                    <- src/indicies/ivf_pq.py:146-152
- * Sub-quantizer counts: M = 16, 32 or 64 run the tuned ADC scan (K = M/16 lanes of a warp cooperate on one vector with
- * a bank-conflict-free look-up layout that exists for K in {1, 2, 4}: csrc/rsb_layout.h); any other multiple of 4 up to
- * 128 dividing d (e.g. 24 / 48 / 96 on d = 768, which faiss and the reference's n_subquantizers key accept) runs a
- * functionally complete generic path (natural code order, [m][256] tables, one thread per vector) -- correct, not tuned.
- * rsb_ivfpq_create takes nbits = 8 only (tables of 256 entries, one byte per code); any other nbits returns
- * RSB_ERR_UNSUPPORTED (-> NotImplementedError in Python), as do other M. */
+ * M must divide d, else RSB_ERR_INVALID.  nbits other than 8 / 4 (codes crossing bytes, tables beyond shared memory)
+ * returns RSB_ERR_UNSUPPORTED (-> NotImplementedError in Python).
+ *   nbits = 8   tables of 256 entries, one byte per code.  M = 16, 32 or 64 run the tuned ADC scan (K = M/16 lanes of a
+ *     warp cooperate on one vector with a bank-conflict-free look-up layout that exists for K in {1, 2, 4}:
+ *     csrc/rsb_layout.h); any other multiple of 4 up to 128 (e.g. 24 / 48 / 96 on d = 768, which faiss and the
+ *     reference's n_subquantizers key accept) runs a functionally complete generic path (natural code order, [m][256]
+ *     tables, one thread per vector) -- correct, not tuned.  Other M: RSB_ERR_UNSUPPORTED.
+ *   nbits = 4   codes are packed two per byte in faiss' order (PQEncoderGeneric, LSB first: byte b = c[2b] | c[2b+1] <<
+ *     4), so a vector holds Mb = M / 2 code bytes, and the index is scanned as an 8-bit index of Mb byte sub-quantizers
+ *     with the pair tables T'[b][j] = T[2b][j & 15] + T[2b+1][j >> 4]: M = 32 / 64 / 128 run the tuned scan (Mb = 16 /
+ *     32 / 64), any other M with M % 8 == 0 and M / 2 <= 128 the generic one; other M: RSB_ERR_INVALID.  Scores differ
+ *     from faiss' sequential sum over m by fp32 rounding only.  The codebook (rsb_set_pq_codebook /
+ *     rsb_get_pq_codebook) is [M, 16, d/M], and codes (rsb_add_codes, rsb_export_lists) are [n, M / 2] packed bytes. */
 int rsb_ivfpq_create(int d, int nlist, int M, int nbits, rsb_index_t** out);
-/* As rsb_ivfpq_create, with nbits = 8 (identical to it) or nbits = 4.  4-bit codes are packed two per byte in faiss'
- * order (PQEncoderGeneric, LSB first: byte b = c[2b] | c[2b+1] << 4), so a vector holds Mb = M / 2 code bytes, and the
- * index is scanned as an 8-bit index of Mb byte sub-quantizers with the pair tables T'[b][j] = T[2b][j & 15] +
- * T[2b+1][j >> 4]: M = 32 / 64 / 128 run the tuned scan (Mb = 16 / 32 / 64), any other M with M % 8 == 0, M / 2 <= 128
- * and d % M == 0 the generic one.  Scores differ from faiss' sequential sum over m by fp32 rounding only.
- * nbits other than 4 / 8 (codes crossing bytes, tables beyond shared memory) -> RSB_ERR_UNSUPPORTED; a 4-bit M outside
- * those shapes -> RSB_ERR_INVALID.  With nbits = 4 the codebook (rsb_set_pq_codebook / rsb_get_pq_codebook) is
- * [M, 16, d/M], and codes (rsb_add_codes, rsb_export_lists) are [n, M / 2] packed bytes. */
-int rsb_ivfpq_create_nbits(int d, int nlist, int M, int nbits, rsb_index_t** out);
-/* Storage dtype of the vectors (enum RSB_DTYPE_* below): RSB_DTYPE_F32 is rsb_flat_create / rsb_ivfflat_create;
- * RSB_DTYPE_F16 keeps every row as fp16 -- the embedding task writes fp16 passage embeddings (src/embed.py:137-138)
- * and the reference upcasts them only on load (src/indicies/flat.py:86), so fp16 storage of them is lossless at half
- * the bytes.  faiss equivalent: IndexScalarQuantizer / IndexIVFScalarQuantizer(QT_fp16, METRIC_INNER_PRODUCT, no
- * residual).  Stored values are the fp16 rounding (to nearest even) of what is added; scores are exact fp32 inner
- * products of the fp32 query with the decoded rows.  d % 8 == 0 (16-byte rows), else RSB_ERR_INVALID.
- *   Flat (<- src/indicies/flat.py:42, ric/conf/default.yaml `index_type: Flat`): scored on wgmma tensor cores from the
- *     fp16 rows themselves (scaled fp16 hi/lo query split, then an exact fp32 re-score), needs d % 64 == 0, else
- *     RSB_ERR_UNSUPPORTED.  Final scores equal the fp32 index's wherever both return the same id.
- *   IVF-Flat (<- src/indicies/ivf_flat.py:143-149, api/conf/ivf_flat.yaml): the list scan reads 2 bytes per element and
- *     adds in the fp32 scan's order: ids and scores are bit-identical to an fp32 index holding the same values. */
-int rsb_flat_create_dtype(int d, int dtype, rsb_index_t** out);
-int rsb_ivfflat_create_dtype(int d, int nlist, int dtype, rsb_index_t** out);
 int rsb_free(rsb_index_t* h);
 
 /* ---- trained state (what index.train() produces; ivf_flat.py:166, ivf_pq.py:170) ------------------ */
@@ -95,23 +93,18 @@ int rsb_get_centroids(rsb_index_t* h, float* out_dev, rsb_stream_t stream);
 int rsb_get_pq_codebook(rsb_index_t* h, float* out_dev, rsb_stream_t stream);
 
 /* ---- population (index.add(x): flat.py:58, ivf_flat.py:180, ivf_pq.py:185) ------------------------- */
-/* ids_dev may be NULL: ids are then sequential from ntotal (faiss behaviour).  IVF: list = argmax_c <x,c>
- * computed here in fp32; IVFPQ additionally encodes the residual.  ws_dev/ws_bytes: see rsb_add_workspace_bytes. */
+/* Rows x_dev [n, d] in x_dtype (RSB_DTYPE_F32 or RSB_DTYPE_F16, else RSB_ERR_INVALID), converted on the device to the
+ * index's storage dtype: the embedding pickles' fp16 rows (src/indicies/flat.py:58-59, ivf_flat.py:180) cross PCIe once
+ * at 2 bytes per element.  IVFPQ takes RSB_DTYPE_F32 only (RSB_ERR_UNSUPPORTED otherwise).  ids_dev may be NULL: ids
+ * are then sequential from ntotal (faiss behaviour).  IVF: list = argmax_c <x,c> computed here in fp32 (fp16 rows are
+ * assigned on their upcast, exact values, so the lists are those an fp32 index assigns); IVFPQ additionally encodes the
+ * residual.  ws_dev/ws_bytes: see rsb_add_workspace_bytes. */
 size_t rsb_add_workspace_bytes(rsb_index_t* h, int64_t n);
-int rsb_add(rsb_index_t* h, const float* x_dev, int64_t n, const int64_t* ids_dev,
-            void* ws_dev, size_t ws_bytes, rsb_stream_t stream);
+int rsb_add(rsb_index_t* h, const void* x_dev, int x_dtype, int64_t n, const int64_t* ids_dev, void* ws_dev,
+            size_t ws_bytes, rsb_stream_t stream);
 /* as rsb_add but the coarse assignment is supplied by the caller (int32 list id per row) */
-int rsb_add_preassigned(rsb_index_t* h, const float* x_dev, int64_t n, const int64_t* ids_dev,
+int rsb_add_preassigned(rsb_index_t* h, const void* x_dev, int x_dtype, int64_t n, const int64_t* ids_dev,
                         const int32_t* list_dev, rsb_stream_t stream);
-/* rsb_add / rsb_add_preassigned with rows x_dev [n, d] in x_dtype (RSB_DTYPE_F32 or RSB_DTYPE_F16): the embedding
- * pickles' fp16 rows (src/indicies/flat.py:58-59, ivf_flat.py:180) cross PCIe once at 2 bytes per element and are
- * converted on the device to the index's storage dtype.  IVF list assignment of fp16 rows runs the fp32 coarse
- * quantizer on the upcast (exact) values, so the lists are those an fp32 index assigns.  IVFPQ takes RSB_DTYPE_F32
- * only (RSB_ERR_UNSUPPORTED otherwise). */
-int rsb_add_typed(rsb_index_t* h, const void* x_dev, int x_dtype, int64_t n, const int64_t* ids_dev, void* ws_dev,
-                  size_t ws_bytes, rsb_stream_t stream);
-int rsb_add_preassigned_typed(rsb_index_t* h, const void* x_dev, int x_dtype, int64_t n, const int64_t* ids_dev,
-                              const int32_t* list_dev, rsb_stream_t stream);
 /* IVFPQ only: rows are already PQ codes [n, M * nbits / 8] uint8 (e.g. read from an existing index file) */
 int rsb_add_codes(rsb_index_t* h, const uint8_t* codes_dev, int64_t n, const int64_t* ids_dev,
                   const int32_t* list_dev, rsb_stream_t stream);
@@ -146,22 +139,22 @@ int rsb_search(rsb_index_t* h, const float* q_dev, int nq, int k, int nprobe,
                float* D_dev, int64_t* I_dev, void* ws_dev, size_t ws_bytes, rsb_stream_t stream);
 /* faiss IndexIVF::search_preassigned: as rsb_search, but the probed lists list_dev [nq, nprobe] int64 (-1 =
  * skip) and their coarse scores coarse_dis_dev [nq, nprobe] float32 (<q, c_list>, added to every PQ score of
- * that list; ignored by IVFFLAT) come from the caller instead of the coarse quantizer. */
+ * that list; ignored by IVFFLAT) come from the caller instead of the coarse quantizer.
+ * Thresholds: tau_local_dev = NULL (with tau_peers_dev = NULL, npeers = 0) keeps the per-query running top-k
+ * thresholds in the workspace.  Otherwise they are shared between GPUs (one process per GPU, datastore partitioned
+ * across the GPUs; replaces the reference's one-process-per-shard search, src/search.py:282-296) in caller-owned
+ * peer-mapped arrays: tau_local_dev [nq] uint32 is THIS GPU's array; tau_peers_dev is a DEVICE array of `npeers` base
+ * pointers, one per GPU of the job (the own entry is recognised and skipped).  Whenever the scan raises a threshold it
+ * also raises it on every peer (relaxed system-scope max reduction over NVLink), so every GPU filters with the best
+ * bound found anywhere; results are unchanged (a bound is always the k-th best score of real candidates of that query).
+ * The caller zeroes the arrays before the first search of a batch on ANY GPU and keeps the GPUs within one batch of
+ * each other (a cross-GPU barrier per batch, which the top-k combine provides).  An inconsistent set (npeers < 0,
+ * npeers > 0 without tau_peers_dev, or tau_peers_dev / npeers without tau_local_dev) returns RSB_ERR_INVALID before
+ * any launch. */
 int rsb_search_preassigned(rsb_index_t* h, const float* q_dev, int nq, int k, int nprobe,
                            const int64_t* list_dev, const float* coarse_dis_dev, float* D_dev, int64_t* I_dev,
-                           void* ws_dev, size_t ws_bytes, rsb_stream_t stream);
-/* Multi-GPU form of rsb_search_preassigned (one process per GPU, datastore partitioned across the GPUs; replaces the
- * reference's one-process-per-shard search, src/search.py:282-296): the per-query running top-k thresholds live in
- * caller-owned peer-mapped arrays.  tau_local_dev [nq] uint32 is THIS GPU's array; tau_peers_dev is a DEVICE array of
- * `npeers` base pointers, one per GPU of the job (the own entry is recognised and skipped).  Whenever the scan raises a
- * threshold it also raises it on every peer (relaxed system-scope max reduction over NVLink), so every GPU filters
- * with the best bound found anywhere; results are unchanged (a bound is always the k-th best score of real
- * candidates of that query).  The caller zeroes the arrays before the first search of a batch on ANY GPU and keeps
- * the GPUs within one batch of each other (a cross-GPU barrier per batch, which the top-k combine provides). */
-int rsb_search_preassigned_shared(rsb_index_t* h, const float* q_dev, int nq, int k, int nprobe,
-                                  const int64_t* list_dev, const float* coarse_dis_dev, float* D_dev, int64_t* I_dev,
-                                  void* ws_dev, size_t ws_bytes, uint32_t* tau_local_dev,
-                                  uint32_t* const* tau_peers_dev, int npeers, rsb_stream_t stream);
+                           void* ws_dev, size_t ws_bytes, uint32_t* tau_local_dev, uint32_t* const* tau_peers_dev,
+                           int npeers, rsb_stream_t stream);
 /* Copy `bytes` from src_dev to dst_ptrs_dev[p] + dst_offset_bytes for every p < npeers (peer-mapped destinations; P2P
  * stores over NVLink).  Used to publish a rank's slice of the coarse-quantizer tables to every GPU without NCCL.
  * 16-byte aligned pointers / sizes. */
@@ -268,20 +261,15 @@ int rsb_knn_ip(const float* q_dev, int nq, const float* x_dev, int64_t n, int d,
 /* sums_dev [k, d] += x[i], counts_dev [k] (float) += 1 for assign_dev[i] (int32, out-of-range ids are skipped) */
 int rsb_kmeans_accumulate(const float* x_dev, int64_t n, int d, const int32_t* assign_dev, int k, float* sums_dev,
                           float* counts_dev, rsb_stream_t stream);
-/* PQ k-means assignment step: codes_dev [n, M] = argmin_j || r[i, m-th slice] - codebook[m][j] ||^2 (ksub = 256) */
-int rsb_pq_assign(const float* r_dev, int64_t n, int d, int M, const float* codebook_dev, uint8_t* codes_dev,
+/* PQ k-means steps with ksub = 256 (nbits = 8) or ksub = 16 (nbits = 4) entries per sub-quantizer; other ksub ->
+ * RSB_ERR_UNSUPPORTED.  codebook_dev [M, ksub, d/M]; codes_dev [n, M], one code per byte (not packed).
+ * assignment: codes_dev[i, m] = argmin_j || r[i, m-th slice] - codebook[m][j] ||^2, the lowest j winning exact ties.
+ * update: sums_dev [M, ksub, d/M] += slices, counts_dev [M, ksub] (float) += 1.  Member sums are added in a fixed
+ * order, so training gives the same codebook on every run. */
+int rsb_pq_assign(const float* r_dev, int64_t n, int d, int M, int ksub, const float* codebook_dev, uint8_t* codes_dev,
                   rsb_stream_t stream);
-/* PQ k-means update step: sums_dev [M, 256, d/M] += slices, counts_dev [M, 256] (float) += 1 */
-int rsb_pq_accumulate(const float* r_dev, int64_t n, int d, int M, const uint8_t* codes_dev, float* sums_dev,
+int rsb_pq_accumulate(const float* r_dev, int64_t n, int d, int M, int ksub, const uint8_t* codes_dev, float* sums_dev,
                       float* counts_dev, rsb_stream_t stream);
-/* The same two steps for ksub = 256 (nbits = 8: rsb_pq_assign / rsb_pq_accumulate) or ksub = 16 (nbits = 4); other
- * ksub -> RSB_ERR_UNSUPPORTED.  codebook_dev [M, ksub, d/M]; codes_dev [n, M], one code per byte (not packed), the
- * nearest entry by L2 with the lowest index winning exact ties; sums_dev [M, ksub, d/M], counts_dev [M, ksub].  Member
- * sums are added in a fixed order, so training gives the same codebook on every run. */
-int rsb_pq_assign_ksub(const float* r_dev, int64_t n, int d, int M, int ksub, const float* codebook_dev,
-                       uint8_t* codes_dev, rsb_stream_t stream);
-int rsb_pq_accumulate_ksub(const float* r_dev, int64_t n, int d, int M, int ksub, const uint8_t* codes_dev,
-                           float* sums_dev, float* counts_dev, rsb_stream_t stream);
 
 /* ---- options -------------------------------------------------------------------------------------------- */
 enum {

@@ -24,22 +24,17 @@ _H = c_void_p
 SIGNATURES = [
     ("rsb_version", c_int, []),
     ("rsb_last_error", c_char_p, []),
-    ("rsb_flat_create", c_int, [c_int, POINTER(_H)]),
-    ("rsb_ivfflat_create", c_int, [c_int, c_int, POINTER(_H)]),
+    ("rsb_flat_create", c_int, [c_int, c_int, POINTER(_H)]),
+    ("rsb_ivfflat_create", c_int, [c_int, c_int, c_int, POINTER(_H)]),
     ("rsb_ivfpq_create", c_int, [c_int, c_int, c_int, c_int, POINTER(_H)]),
-    ("rsb_ivfpq_create_nbits", c_int, [c_int, c_int, c_int, c_int, POINTER(_H)]),
-    ("rsb_flat_create_dtype", c_int, [c_int, c_int, POINTER(_H)]),
-    ("rsb_ivfflat_create_dtype", c_int, [c_int, c_int, c_int, POINTER(_H)]),
     ("rsb_free", c_int, [_H]),
     ("rsb_set_centroids", c_int, [_H, c_void_p, c_void_p]),
     ("rsb_set_pq_codebook", c_int, [_H, c_void_p, c_void_p]),
     ("rsb_get_centroids", c_int, [_H, c_void_p, c_void_p]),
     ("rsb_get_pq_codebook", c_int, [_H, c_void_p, c_void_p]),
     ("rsb_add_workspace_bytes", c_size_t, [_H, c_int64]),
-    ("rsb_add", c_int, [_H, c_void_p, c_int64, c_void_p, c_void_p, c_size_t, c_void_p]),
-    ("rsb_add_preassigned", c_int, [_H, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
-    ("rsb_add_typed", c_int, [_H, c_void_p, c_int, c_int64, c_void_p, c_void_p, c_size_t, c_void_p]),
-    ("rsb_add_preassigned_typed", c_int, [_H, c_void_p, c_int, c_int64, c_void_p, c_void_p, c_void_p]),
+    ("rsb_add", c_int, [_H, c_void_p, c_int, c_int64, c_void_p, c_void_p, c_size_t, c_void_p]),
+    ("rsb_add_preassigned", c_int, [_H, c_void_p, c_int, c_int64, c_void_p, c_void_p, c_void_p]),
     ("rsb_add_codes", c_int, [_H, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
     ("rsb_finalize", c_int, [_H, c_void_p]),
     ("rsb_info", c_int, [_H, c_int, POINTER(c_int64)]),
@@ -48,14 +43,10 @@ SIGNATURES = [
     ("rsb_workspace_bytes", c_size_t, [_H, c_int, c_int, c_int]),
     ("rsb_search", c_int, [_H, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     ("rsb_search_preassigned", c_int, [_H, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
-                                       c_void_p, c_size_t, c_void_p]),
-    ("rsb_search_preassigned_shared", c_int, [_H, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
-                                              c_void_p, c_size_t, c_void_p, c_void_p, c_int, c_void_p]),
+                                       c_void_p, c_size_t, c_void_p, c_void_p, c_int, c_void_p]),
     ("rsb_kmeans_accumulate", c_int, [c_void_p, c_int64, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
-    ("rsb_pq_assign", c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p]),
-    ("rsb_pq_accumulate", c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
-    ("rsb_pq_assign_ksub", c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
-    ("rsb_pq_accumulate_ksub", c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    ("rsb_pq_assign", c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    ("rsb_pq_accumulate", c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     ("rsb_peer_broadcast", c_int, [c_void_p, c_size_t, c_void_p, c_int, c_size_t, c_void_p]),
     ("rsb_coarse", c_int, [_H, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     ("rsb_host_alloc", c_int, [c_size_t, POINTER(c_void_p)]),

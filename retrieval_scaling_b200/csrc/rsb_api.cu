@@ -119,7 +119,7 @@ static void free_layout(rsb_index* h) {
 extern "C" int rsb_version(void) { return RSB_VERSION; }
 extern "C" const char* rsb_last_error(void) { return g_err.c_str(); }
 
-static int create_common(int kind, int d, int nlist, int M, int nbits, rsb_index_t** out, int dtype = RSB_DTYPE_F32) {
+static int create_common(int kind, int d, int nlist, int M, int nbits, int dtype, rsb_index_t** out) {
     if (!out) return fail(RSB_ERR_INVALID, "out is NULL");
     *out = nullptr;
     if (d <= 0 || (d & 3)) return fail(RSB_ERR_INVALID, "dimension must be a positive multiple of 4, got %d", d);
@@ -149,24 +149,14 @@ static int create_common(int kind, int d, int nlist, int M, int nbits, rsb_index
     *out = h;
     return RSB_OK;
 }
-extern "C" int rsb_flat_create(int d, rsb_index_t** out) { return create_common(RSB_FLAT, d, 1, 0, 0, out); }
-extern "C" int rsb_ivfflat_create(int d, int nlist, rsb_index_t** out) {
-    return create_common(RSB_IVFFLAT, d, nlist, 0, 0, out);
+extern "C" int rsb_flat_create(int d, int dtype, rsb_index_t** out) {
+    return create_common(RSB_FLAT, d, 1, 0, 0, dtype, out);
 }
-extern "C" int rsb_flat_create_dtype(int d, int dtype, rsb_index_t** out) {
-    return create_common(RSB_FLAT, d, 1, 0, 0, out, dtype);
-}
-extern "C" int rsb_ivfflat_create_dtype(int d, int nlist, int dtype, rsb_index_t** out) {
-    return create_common(RSB_IVFFLAT, d, nlist, 0, 0, out, dtype);
+extern "C" int rsb_ivfflat_create(int d, int nlist, int dtype, rsb_index_t** out) {
+    return create_common(RSB_IVFFLAT, d, nlist, 0, 0, dtype, out);
 }
 extern "C" int rsb_ivfpq_create(int d, int nlist, int M, int nbits, rsb_index_t** out) {
-    if (out) *out = nullptr;
-    if (nbits != 8)
-        return fail(RSB_ERR_UNSUPPORTED, "rsb_ivfpq_create takes nbits = 8 only, got %d (4-bit codes: rsb_ivfpq_create_nbits)", nbits);
-    return create_common(RSB_IVFPQ, d, nlist, M, nbits, out);
-}
-extern "C" int rsb_ivfpq_create_nbits(int d, int nlist, int M, int nbits, rsb_index_t** out) {
-    return create_common(RSB_IVFPQ, d, nlist, M, nbits, out);
+    return create_common(RSB_IVFPQ, d, nlist, M, nbits, RSB_DTYPE_F32, out);
 }
 extern "C" int rsb_free(rsb_index_t* h) {
     if (!h) return RSB_OK;
@@ -452,20 +442,12 @@ static int add_impl(rsb_index* h, const void* x, int x_dtype, const uint8_t* cod
     return RSB_OK;
 }
 
-extern "C" int rsb_add(rsb_index_t* h, const float* x, int64_t n, const int64_t* ids, void* ws, size_t ws_bytes,
-                       rsb_stream_t stream) {
-    return add_impl(h, x, RSB_DTYPE_F32, nullptr, n, ids, nullptr, ws, ws_bytes, (cudaStream_t)stream);
-}
-extern "C" int rsb_add_typed(rsb_index_t* h, const void* x, int x_dtype, int64_t n, const int64_t* ids, void* ws,
-                             size_t ws_bytes, rsb_stream_t stream) {
+extern "C" int rsb_add(rsb_index_t* h, const void* x, int x_dtype, int64_t n, const int64_t* ids, void* ws,
+                       size_t ws_bytes, rsb_stream_t stream) {
     return add_impl(h, x, x_dtype, nullptr, n, ids, nullptr, ws, ws_bytes, (cudaStream_t)stream);
 }
-extern "C" int rsb_add_preassigned(rsb_index_t* h, const float* x, int64_t n, const int64_t* ids,
+extern "C" int rsb_add_preassigned(rsb_index_t* h, const void* x, int x_dtype, int64_t n, const int64_t* ids,
                                    const int32_t* list, rsb_stream_t stream) {
-    return rsb_add_preassigned_typed(h, x, RSB_DTYPE_F32, n, ids, list, stream);
-}
-extern "C" int rsb_add_preassigned_typed(rsb_index_t* h, const void* x, int x_dtype, int64_t n, const int64_t* ids,
-                                         const int32_t* list, rsb_stream_t stream) {
     if (h && h->kind == RSB_FLAT) return fail(RSB_ERR_INVALID, "a Flat index has no lists");
     if (!list) return fail(RSB_ERR_INVALID, "list_dev is NULL");
     return add_impl(h, x, x_dtype, nullptr, n, ids, list, nullptr, 0, (cudaStream_t)stream);
@@ -894,6 +876,15 @@ struct SharedTau {
     int npeers = 0;
 };
 
+// The IVFPQ look-up tables for queries q [nq, d], as the scan reads them (Mb byte sub-quantizers).  The search and
+// the rsb_pq_tables diagnostic both build them here, so the tables a test reads are the ones the scan reads.
+static void launch_pq_tables(const rsb_index* h, const float* q, int nq, float* lut, cudaStream_t st) {
+    if (h->nbits == 4) launch_pq_lut4(q, nq, h->d, h->M, h->codebook, lut, st);
+    else if (pq_interleaved_layout(h->M)) launch_pq_lut(q, nq, h->d, h->M, h->codebook_t, lut, st);
+    else launch_pq_lut_generic(q, nq, h->d, h->M, h->codebook, lut, st);
+}
+
+// shared: the multi-GPU threshold exchange, or nullptr for thresholds kept in the workspace
 static int search_impl(rsb_index_t* h, const float* q, int nq, int k, int nprobe, const int64_t* pre_lists,
                        const float* pre_dis, float* D, int64_t* I, void* ws, size_t ws_bytes, rsb_stream_t stream,
                        const SharedTau* shared = nullptr) {
@@ -993,7 +984,7 @@ static int search_impl(rsb_index_t* h, const float* q, int nq, int k, int nprobe
         // selections per GPU.  RSB_LOCAL_LEADS=1: a lead pair per query on every GPU (its best-ranked list that is
         // non-empty there), the single-GPU rule.
         static const bool local_leads = getenv("RSB_LOCAL_LEADS") != nullptr;
-        const int lead_mode = (shared && shared->local && shared->npeers > 1 && !local_leads) ? 1 : 0;
+        const int lead_mode = (shared && shared->npeers > 1 && !local_leads) ? 1 : 0;
         const bool paired = pq_paired_scan(h) && nb > 1;          // one query: no list is probed twice
         launch_pair_setup(cI, nb, p.nprobe, h->nlist, h->list_len, lpt_order ? h->list_rank : nullptr, pw, st, lead_mode,
                           paired);
@@ -1006,7 +997,7 @@ static int search_impl(rsb_index_t* h, const float* q, int nq, int k, int nprobe
         a.list_len = h->list_len; a.list_off = h->list_slot_off;
         a.tau = reinterpret_cast<unsigned*>(w + p.off_tau);
         a.tau_peers = nullptr; a.n_peers = 0; a.tau_external = 0;
-        if (shared && shared->local) {
+        if (shared) {
             if (nq > p.qb) return fail(RSB_ERR_UNSUPPORTED, "shared thresholds need the whole batch in one pass (nq = %d > %d)", nq, p.qb);
             a.tau = shared->local; a.tau_peers = shared->peers; a.n_peers = shared->npeers; a.tau_external = 1;
         }
@@ -1024,9 +1015,7 @@ static int search_impl(rsb_index_t* h, const float* q, int nq, int k, int nprobe
         if (h->kind == RSB_IVFPQ) {
             float* lut = reinterpret_cast<float*>(w + p.off_lut);
             // from here on the index is scanned as Mb byte sub-quantizers (Mb = M for 8-bit codes)
-            if (h->nbits == 4) launch_pq_lut4(qb, nb, h->d, h->M, h->codebook, lut, st);
-            else if (pq_interleaved_layout(h->M)) launch_pq_lut(qb, nb, h->d, h->M, h->codebook_t, lut, st);
-            else launch_pq_lut_generic(qb, nb, h->d, h->M, h->codebook, lut, st);
+            launch_pq_tables(h, qb, nb, lut, st);
             h->launches += 1;
             if (paired) {
                 launch_pq_lut_quant(lut, nb, h->Mb, reinterpret_cast<unsigned short*>(w + p.off_qlut),
@@ -1062,22 +1051,17 @@ extern "C" int rsb_search(rsb_index_t* h, const float* q, int nq, int k, int npr
 }
 extern "C" int rsb_search_preassigned(rsb_index_t* h, const float* q, int nq, int k, int nprobe,
                                       const int64_t* list_dev, const float* coarse_dis_dev, float* D, int64_t* I,
-                                      void* ws, size_t ws_bytes, rsb_stream_t stream) {
+                                      void* ws, size_t ws_bytes, uint32_t* tau_local_dev,
+                                      uint32_t* const* tau_peers_dev, int npeers, rsb_stream_t stream) {
     if (h && h->kind == RSB_FLAT) return fail(RSB_ERR_INVALID, "a Flat index has no lists");
     if (!list_dev || !coarse_dis_dev) return fail(RSB_ERR_INVALID, "null argument");
-    return search_impl(h, q, nq, k, nprobe, list_dev, coarse_dis_dev, D, I, ws, ws_bytes, stream);
-}
-
-extern "C" int rsb_search_preassigned_shared(rsb_index_t* h, const float* q, int nq, int k, int nprobe,
-                                             const int64_t* list_dev, const float* coarse_dis_dev, float* D, int64_t* I,
-                                             void* ws, size_t ws_bytes, uint32_t* tau_local_dev,
-                                             uint32_t* const* tau_peers_dev, int npeers, rsb_stream_t stream) {
-    if (h && h->kind == RSB_FLAT) return fail(RSB_ERR_INVALID, "a Flat index has no lists");
-    if (!list_dev || !coarse_dis_dev) return fail(RSB_ERR_INVALID, "null argument");
-    if (!tau_local_dev || npeers < 0 || (npeers > 0 && !tau_peers_dev)) return fail(RSB_ERR_INVALID, "bad threshold arrays");
+    if (npeers < 0 || (npeers > 0 && !tau_peers_dev) || (!tau_local_dev && (npeers != 0 || tau_peers_dev)))
+        return fail(RSB_ERR_INVALID, "inconsistent threshold arrays: tau_local_dev %s, tau_peers_dev %s, npeers = %d",
+                    tau_local_dev ? "set" : "NULL", tau_peers_dev ? "set" : "NULL", npeers);
     SharedTau sh;
     sh.local = tau_local_dev; sh.peers = tau_peers_dev; sh.npeers = npeers;
-    return search_impl(h, q, nq, k, nprobe, list_dev, coarse_dis_dev, D, I, ws, ws_bytes, stream, &sh);
+    return search_impl(h, q, nq, k, nprobe, list_dev, coarse_dis_dev, D, I, ws, ws_bytes, stream,
+                       tau_local_dev ? &sh : nullptr);
 }
 
 // ---- exact re-ranking (faiss IndexRefine::search) -----------------------------------------------------------
@@ -1313,16 +1297,8 @@ extern "C" int rsb_kmeans_accumulate(const float* x, int64_t n, int d, const int
     CHECK_LAUNCH();
     return RSB_OK;
 }
-extern "C" int rsb_pq_assign(const float* r, int64_t n, int d, int M, const float* codebook, uint8_t* codes,
+extern "C" int rsb_pq_assign(const float* r, int64_t n, int d, int M, int ksub, const float* codebook, uint8_t* codes,
                              rsb_stream_t stream) {
-    return rsb_pq_assign_ksub(r, n, d, M, 256, codebook, codes, stream);
-}
-extern "C" int rsb_pq_accumulate(const float* r, int64_t n, int d, int M, const uint8_t* codes, float* sums, float* counts,
-                                 rsb_stream_t stream) {
-    return rsb_pq_accumulate_ksub(r, n, d, M, 256, codes, sums, counts, stream);
-}
-extern "C" int rsb_pq_assign_ksub(const float* r, int64_t n, int d, int M, int ksub, const float* codebook, uint8_t* codes,
-                                  rsb_stream_t stream) {
     if (!r || !codebook || !codes || n < 0 || d <= 0 || M <= 0 || d % M) return fail(RSB_ERR_INVALID, "bad argument");
     if (ksub != 256 && ksub != 16) return fail(RSB_ERR_UNSUPPORTED, "ksub must be 256 or 16 (nbits 8 or 4), got %d", ksub);
     if (ksub == 16) launch_pq_encode4(r, n, d, nullptr, nullptr, codebook, M, false, codes, (cudaStream_t)stream);
@@ -1330,8 +1306,8 @@ extern "C" int rsb_pq_assign_ksub(const float* r, int64_t n, int d, int M, int k
     CHECK_LAUNCH();
     return RSB_OK;
 }
-extern "C" int rsb_pq_accumulate_ksub(const float* r, int64_t n, int d, int M, int ksub, const uint8_t* codes, float* sums,
-                                      float* counts, rsb_stream_t stream) {
+extern "C" int rsb_pq_accumulate(const float* r, int64_t n, int d, int M, int ksub, const uint8_t* codes, float* sums,
+                                 float* counts, rsb_stream_t stream) {
     if (!r || !codes || !sums || !counts || n < 0 || d <= 0 || M <= 0 || d % M) return fail(RSB_ERR_INVALID, "bad argument");
     if (ksub != 256 && ksub != 16) return fail(RSB_ERR_UNSUPPORTED, "ksub must be 256 or 16 (nbits 8 or 4), got %d", ksub);
     const cudaError_t e = launch_pq_accumulate(r, n, d, M, ksub, codes, sums, counts, (cudaStream_t)stream);
@@ -1440,10 +1416,7 @@ extern "C" int rsb_pq_tables(rsb_index_t* h, const float* q, int nq, float* lut,
     if (!h || h->kind != RSB_IVFPQ) return fail(RSB_ERR_INVALID, "rsb_pq_tables needs an IVFPQ index");
     if (nq < 0 || (nq > 0 && (!q || !lut))) return fail(RSB_ERR_INVALID, "null argument");
     if (!h->has_codebook) return fail(RSB_ERR_STATE, "index has no PQ codebook");
-    cudaStream_t st = (cudaStream_t)stream;
-    if (h->nbits == 4) launch_pq_lut4(q, nq, h->d, h->M, h->codebook, lut, st);
-    else if (pq_interleaved_layout(h->M)) launch_pq_lut(q, nq, h->d, h->M, h->codebook_t, lut, st);
-    else launch_pq_lut_generic(q, nq, h->d, h->M, h->codebook, lut, st);
+    launch_pq_tables(h, q, nq, lut, (cudaStream_t)stream);
     CHECK_LAUNCH();
     return RSB_OK;
 }

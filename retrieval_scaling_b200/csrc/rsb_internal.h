@@ -182,10 +182,11 @@ struct ScanArgs {
     const int* list_len;          // [nlist]
     const int64_t* list_off;      // [nlist] first slot of the list (IVFPQ: multiple of 32; IVFFLAT: CSR offset)
     unsigned* tau;                // [nq] running per-query threshold (ordered uint, zeroed by launcher)
-    // Multi-GPU threshold exchange (rsb_search_preassigned_shared): `tau` then points into THIS GPU's symmetric-memory
-    // threshold array (owned and zeroed by the caller) and every raise of tau[q] is also pushed to tau_peers[p][q] of
-    // the other GPUs with a fire-and-forget system-scope reduction over NVLink, so every GPU filters with the best
-    // k-th-best bound any GPU has found for that query.  Exact: a bound is always the k-th best of real candidates.
+    // Multi-GPU threshold exchange (rsb_search_preassigned with tau_local_dev set): `tau` then points into THIS GPU's
+    // symmetric-memory threshold array (owned and zeroed by the caller) and every raise of tau[q] is also pushed to
+    // tau_peers[p][q] of the other GPUs with a fire-and-forget system-scope reduction over NVLink, so every GPU filters
+    // with the best k-th-best bound any GPU has found for that query.  Exact: a bound is always the k-th best of real
+    // candidates.
     unsigned* const* tau_peers;   // device array of n_peers pointers (entries equal to `tau`'s base are skipped); or null
     int n_peers;
     int tau_external;             // 1: the caller owns and zeroes `tau`

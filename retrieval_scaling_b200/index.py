@@ -42,7 +42,7 @@ def _dev_f32(x, device) -> torch.Tensor:
 
 
 def _dev_rows(x, device) -> torch.Tensor:
-    """Vectors to add: fp16 tensors / arrays stay fp16 (they cross PCIe at 2 bytes per element; rsb_add_typed converts
+    """Vectors to add: fp16 tensors / arrays stay fp16 (they cross PCIe at 2 bytes per element; rsb_add converts
     them on the device), anything else becomes fp32 as in _dev_f32."""
     if isinstance(x, np.ndarray):
         x = torch.from_numpy(np.ascontiguousarray(x))
@@ -52,7 +52,7 @@ def _dev_rows(x, device) -> torch.Tensor:
     return x.to(device=device, dtype=dtype, non_blocking=True).contiguous()
 
 
-# storage dtypes of Flat / IVF-Flat vectors (rsb_*_create_dtype) and of IndexRefine's store
+# storage dtypes of Flat / IVF-Flat vectors (rsb_flat_create / rsb_ivfflat_create) and of IndexRefine's store
 _STORE_DTYPES = {"float16": (torch.float16, _lib.RSB_DTYPE_F16), "float32": (torch.float32, _lib.RSB_DTYPE_F32)}
 
 
@@ -151,11 +151,7 @@ class _IndexBase:
                 if idt.numel() != n:
                     raise ValueError("ids and x disagree on n")
             ws = self._workspace(self.L.rsb_add_workspace_bytes(self._h, n))
-            if x.dtype == torch.float16:
-                _lib.check(self.L.rsb_add_typed(self._h, _ptr(x), _lib.RSB_DTYPE_F16, n, _ptr(idt), _ptr(ws), ws.numel(),
-                                                _stream()))
-            else:
-                _lib.check(self.L.rsb_add(self._h, _ptr(x), n, _ptr(idt), _ptr(ws), ws.numel(), _stream()))
+            _lib.check(self.L.rsb_add(self._h, _ptr(x), _dtype_code(x), n, _ptr(idt), _ptr(ws), ws.numel(), _stream()))
             torch.cuda.current_stream().synchronize()  # x / idt may be temporaries
 
     def finalize(self) -> None:
@@ -234,10 +230,7 @@ class IndexFlatIP(_IndexBase):
         super().__init__(d, device)
         self.dtype = _check_dtype(dtype)
         with torch.cuda.device(self.device):
-            if self.dtype == "float32":
-                _lib.check(self.L.rsb_flat_create(self.d, ctypes.byref(self._h)))
-            else:
-                _lib.check(self.L.rsb_flat_create_dtype(self.d, _STORE_DTYPES[self.dtype][1], ctypes.byref(self._h)))
+            _lib.check(self.L.rsb_flat_create(self.d, _STORE_DTYPES[self.dtype][1], ctypes.byref(self._h)))
 
 
 class _IVFBase(_IndexBase):
@@ -275,7 +268,7 @@ class _IVFBase(_IndexBase):
         """faiss search_preassigned: probe exactly `lists` [nq, nprobe]; returns (ids, scores) CUDA tensors.
         `shared_tau = (tau_local uint32 [nq] tensor in peer-mapped memory, table of every GPU's array pointer (int64
         CUDA tensor), number of GPUs)`: thresholds are exchanged between the GPUs of a sharded datastore while they scan
-        (rsb_search_preassigned_shared); the caller zeroes the arrays and keeps the GPUs within one batch of each other."""
+        (rsb_search_preassigned); the caller zeroes the arrays and keeps the GPUs within one batch of each other."""
         with torch.cuda.device(self.device):
             q = _dev_f32(q, self.device)
             lt = torch.as_tensor(lists).to(device=self.device, dtype=torch.int64).contiguous()
@@ -287,14 +280,10 @@ class _IVFBase(_IndexBase):
                 D = torch.empty((nq, k), dtype=torch.float32, device=self.device)
                 I = torch.empty((nq, k), dtype=torch.int64, device=self.device)
             ws = self._workspace(self.L.rsb_workspace_bytes(self._h, nq, k, npb))
-            if shared_tau is not None:
-                tau_local, tau_tab, npeers = shared_tau
-                _lib.check(self.L.rsb_search_preassigned_shared(
-                    self._h, _ptr(q), nq, int(k), npb, _ptr(lt), _ptr(cd), _ptr(D), _ptr(I), _ptr(ws), ws.numel(),
-                    _ptr(tau_local), _ptr(tau_tab), int(npeers), _stream()))
-                return I, D
+            tau_local, tau_tab, npeers = (None, None, 0) if shared_tau is None else shared_tau
             _lib.check(self.L.rsb_search_preassigned(self._h, _ptr(q), nq, int(k), npb, _ptr(lt), _ptr(cd), _ptr(D),
-                                                     _ptr(I), _ptr(ws), ws.numel(), _stream()))
+                                                     _ptr(I), _ptr(ws), ws.numel(), _ptr(tau_local), _ptr(tau_tab),
+                                                     int(npeers), _stream()))
             return I, D
 
     def assign(self, x) -> torch.Tensor:
@@ -307,11 +296,7 @@ class _IVFBase(_IndexBase):
             n = x.shape[0]
             lt = torch.as_tensor(lists).to(device=self.device, dtype=torch.int32).contiguous()
             idt = None if ids is None else torch.as_tensor(ids).to(device=self.device, dtype=torch.int64).contiguous()
-            if x.dtype == torch.float16:
-                _lib.check(self.L.rsb_add_preassigned_typed(self._h, _ptr(x), _lib.RSB_DTYPE_F16, n, _ptr(idt), _ptr(lt),
-                                                            _stream()))
-            else:
-                _lib.check(self.L.rsb_add_preassigned(self._h, _ptr(x), n, _ptr(idt), _ptr(lt), _stream()))
+            _lib.check(self.L.rsb_add_preassigned(self._h, _ptr(x), _dtype_code(x), n, _ptr(idt), _ptr(lt), _stream()))
             torch.cuda.current_stream().synchronize()
 
     def list_sizes(self) -> torch.Tensor:
@@ -337,11 +322,8 @@ class IndexIVFFlat(_IVFBase):
         super().__init__(d, nlist, device)
         self.dtype = _check_dtype(dtype)
         with torch.cuda.device(self.device):
-            if self.dtype == "float32":
-                _lib.check(self.L.rsb_ivfflat_create(self.d, self.nlist, ctypes.byref(self._h)))
-            else:
-                _lib.check(self.L.rsb_ivfflat_create_dtype(self.d, self.nlist, _STORE_DTYPES[self.dtype][1],
-                                                           ctypes.byref(self._h)))
+            _lib.check(self.L.rsb_ivfflat_create(self.d, self.nlist, _STORE_DTYPES[self.dtype][1],
+                                                 ctypes.byref(self._h)))
 
     def train(self, x) -> None:
         with torch.cuda.device(self.device):
@@ -359,7 +341,7 @@ class IndexIVFPQ(_IVFBase):
         super().__init__(d, nlist, device)
         self.M, self.nbits = int(M), int(nbits)
         with torch.cuda.device(self.device):
-            _lib.check(self.L.rsb_ivfpq_create_nbits(self.d, self.nlist, self.M, self.nbits, ctypes.byref(self._h)))
+            _lib.check(self.L.rsb_ivfpq_create(self.d, self.nlist, self.M, self.nbits, ctypes.byref(self._h)))
 
     @property
     def code_size(self) -> int:

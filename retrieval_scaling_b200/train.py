@@ -10,8 +10,8 @@ on residuals of at most 256*ksub points.  Parity is defined *given* the trained 
 The Lloyd iterations are driven from here; the arithmetic of every step runs in librsb (`LibrsbOps`):
   assignment (coarse)  : the coarse quantizer itself -- fused 3xTF32 wgmma scorer + exact fp32 re-score (rsb_coarse on a
                          scratch handle holding the current centroids) -> fp32-exact argmax
-  assignment (PQ)      : rsb_pq_assign_ksub (the residual-encoding kernel without the residual step)
-  update               : rsb_kmeans_accumulate / rsb_pq_accumulate_ksub (member sums and counts)
+  assignment (PQ)      : rsb_pq_assign (the residual-encoding kernel without the residual step)
+  update               : rsb_kmeans_accumulate / rsb_pq_accumulate (member sums and counts)
 torch only divides sums by counts, normalises and re-seeds empty clusters (O(k d) element-wise work) and draws the
 random subsets.  There is no CPU path: `LibrsbOps` raises without CUDA; the CPU unit tests of the host logic pass
 their own numpy stand-in for the three operations (tests/test_train_cpu.py).
@@ -73,9 +73,9 @@ class LibrsbOps:
         M, ksub = cb.shape[0], cb.shape[1]
         codes = torch.empty(n, M, dtype=torch.uint8, device=r.device)
         with torch.cuda.device(r.device):
-            _lib.check(_lib.lib().rsb_pq_assign_ksub(ctypes.c_void_p(r.data_ptr()), n, d, M, ksub,
-                                                     ctypes.c_void_p(cb.contiguous().data_ptr()),
-                                                     ctypes.c_void_p(codes.data_ptr()), self._st()))
+            _lib.check(_lib.lib().rsb_pq_assign(ctypes.c_void_p(r.data_ptr()), n, d, M, ksub,
+                                                ctypes.c_void_p(cb.contiguous().data_ptr()),
+                                                ctypes.c_void_p(codes.data_ptr()), self._st()))
         return codes
 
     def pq_accumulate(self, r: torch.Tensor, codes: torch.Tensor, M: int, ksub: int):
@@ -84,9 +84,9 @@ class LibrsbOps:
         sums = torch.zeros(M, ksub, d // M, dtype=torch.float32, device=r.device)
         counts = torch.zeros(M, ksub, dtype=torch.float32, device=r.device)
         with torch.cuda.device(r.device):
-            _lib.check(_lib.lib().rsb_pq_accumulate_ksub(ctypes.c_void_p(r.data_ptr()), n, d, M, ksub,
-                                                         ctypes.c_void_p(codes.data_ptr()), ctypes.c_void_p(sums.data_ptr()),
-                                                         ctypes.c_void_p(counts.data_ptr()), self._st()))
+            _lib.check(_lib.lib().rsb_pq_accumulate(ctypes.c_void_p(r.data_ptr()), n, d, M, ksub,
+                                                    ctypes.c_void_p(codes.data_ptr()), ctypes.c_void_p(sums.data_ptr()),
+                                                    ctypes.c_void_p(counts.data_ptr()), self._st()))
         return sums, counts
 
 

@@ -13,7 +13,7 @@ from retrieval_scaling_b200 import _lib
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def test_header_ctypes_table_and_exports_agree():
+def test_header_ctypes_table_exports_and_version_300_agree():
     L = _lib.lib()
     header = open(os.path.join(ROOT, "include", "rsb.h")).read()
     header = re.sub(r"/\*.*?\*/", "", header, flags=re.S)
@@ -23,20 +23,30 @@ def test_header_ctypes_table_and_exports_agree():
     assert declared == bound, f"header vs ctypes table mismatch: {declared ^ bound}"
     for name in declared:
         assert hasattr(L, name), f"librsb.so does not export {name}"
-    assert L.rsb_version() == 200
+    assert L.rsb_version() == 300
 
 
-def test_errors_are_reported_not_fatal():
+def test_create_refusals_are_reported_not_fatal():
     L = _lib.lib()
     h = ctypes.c_void_p(0)
-    assert L.rsb_ivfpq_create(768, 16, 64, 4, ctypes.byref(h)) == _lib.RSB_ERR_UNSUPPORTED  # nbits != 8
+    assert L.rsb_ivfpq_create(768, 16, 64, 6, ctypes.byref(h)) == _lib.RSB_ERR_UNSUPPORTED  # nbits not 8 / 4
     assert b"nbits" in L.rsb_last_error()
     assert L.rsb_ivfpq_create(770, 16, 64, 8, ctypes.byref(h)) == _lib.RSB_ERR_INVALID      # d % 4, d % M
-    assert L.rsb_flat_create(-1, ctypes.byref(h)) == _lib.RSB_ERR_INVALID
+    assert L.rsb_flat_create(-1, _lib.RSB_DTYPE_F32, ctypes.byref(h)) == _lib.RSB_ERR_INVALID
     with pytest.raises(NotImplementedError):
         _lib.check(_lib.RSB_ERR_UNSUPPORTED)
     with pytest.raises(ValueError):
         _lib.check(_lib.RSB_ERR_INVALID)
+
+
+def test_search_preassigned_refuses_peers_without_local_thresholds():
+    """Shared thresholds start at this GPU's array: peers without tau_local_dev are refused before any launch."""
+    L = _lib.lib()
+    p = ctypes.c_void_p(16)          # never dereferenced: the arguments are refused first
+    assert L.rsb_search_preassigned(None, p, 1, 1, 1, p, p, p, p, p, 256, None, None, 2, None) == _lib.RSB_ERR_INVALID
+    assert b"threshold arrays" in L.rsb_last_error()
+    assert L.rsb_search_preassigned(None, p, 1, 1, 1, p, p, p, p, p, 256, None, p, 0, None) == _lib.RSB_ERR_INVALID
+    assert b"threshold arrays" in L.rsb_last_error()
 
 
 @pytest.mark.parametrize("M", [16, 32, 64])

@@ -40,21 +40,21 @@ def test_storage_dtype_is_refused_for_ivfpq_before_anything_is_built():
         Indexer(cfg)
 
 
-def test_c_abi_dtype_errors_are_reported():
+def test_dtype_arguments_of_create_and_add_are_checked():
     L = _lib.lib()
     h = ctypes.c_void_p(0)
     F16 = _lib.RSB_DTYPE_F16
     # fp16 Flat scores on wgmma with 64 fp16 per K step: d = 72 is a valid fp16 row size but has no scorer
-    assert L.rsb_flat_create_dtype(72, F16, ctypes.byref(h)) == _lib.RSB_ERR_UNSUPPORTED
+    assert L.rsb_flat_create(72, F16, ctypes.byref(h)) == _lib.RSB_ERR_UNSUPPORTED
     assert b"64" in L.rsb_last_error()
     with pytest.raises(NotImplementedError):
-        _lib.check(L.rsb_flat_create_dtype(72, F16, ctypes.byref(h)))
-    assert L.rsb_flat_create_dtype(68, F16, ctypes.byref(h)) == _lib.RSB_ERR_INVALID            # d % 8: 16-byte rows
-    assert L.rsb_ivfflat_create_dtype(68, 16, F16, ctypes.byref(h)) == _lib.RSB_ERR_INVALID
-    assert L.rsb_ivfflat_create_dtype(768, 16, 7, ctypes.byref(h)) == _lib.RSB_ERR_INVALID      # unknown dtype
-    assert L.rsb_flat_create_dtype(768, 7, ctypes.byref(h)) == _lib.RSB_ERR_INVALID
-    assert L.rsb_add_typed(None, None, F16, 1, None, None, 0, None) == _lib.RSB_ERR_INVALID      # null handle
-    assert L.rsb_add_preassigned_typed(None, None, F16, 1, None, None, None) == _lib.RSB_ERR_INVALID
+        _lib.check(L.rsb_flat_create(72, F16, ctypes.byref(h)))
+    assert L.rsb_flat_create(68, F16, ctypes.byref(h)) == _lib.RSB_ERR_INVALID            # d % 8: 16-byte rows
+    assert L.rsb_ivfflat_create(68, 16, F16, ctypes.byref(h)) == _lib.RSB_ERR_INVALID
+    assert L.rsb_ivfflat_create(768, 16, 7, ctypes.byref(h)) == _lib.RSB_ERR_INVALID      # unknown dtype
+    assert L.rsb_flat_create(768, 7, ctypes.byref(h)) == _lib.RSB_ERR_INVALID
+    assert L.rsb_add(None, None, F16, 1, None, None, 0, None) == _lib.RSB_ERR_INVALID      # null handle
+    assert L.rsb_add_preassigned(None, None, F16, 1, None, None, None) == _lib.RSB_ERR_INVALID
     assert not h.value
 
 

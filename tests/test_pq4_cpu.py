@@ -122,10 +122,10 @@ def test_pair_table_layout_positions(Mb):
 
 
 # ---- C-ABI ---------------------------------------------------------------------------------------------------------
-def _create(fn, d, nlist, M, nbits):
+def _create(d, nlist, M, nbits):
     L = _lib.lib()
     h = ctypes.c_void_p(0)
-    rc = getattr(L, fn)(d, nlist, M, nbits, ctypes.byref(h))
+    rc = L.rsb_ivfpq_create(d, nlist, M, nbits, ctypes.byref(h))
     if rc == _lib.RSB_OK:
         L.rsb_free(h)
     return rc, L.rsb_last_error()
@@ -135,8 +135,8 @@ ACCEPTED = (_lib.RSB_OK, _lib.RSB_ERR_OOM, _lib.RSB_ERR_CUDA)    # shape accepte
 
 
 @pytest.mark.parametrize("M", [16, 32, 48, 64, 96, 128, 256])
-def test_create_nbits_accepts_4bit_shapes(M):
-    rc, _ = _create("rsb_ivfpq_create_nbits", 768, 16, M, 4)
+def test_ivfpq_create_accepts_4bit_shapes(M):
+    rc, _ = _create(768, 16, M, 4)
     assert rc in ACCEPTED
 
 
@@ -146,28 +146,20 @@ def test_create_nbits_accepts_4bit_shapes(M):
     (768, 12, 4, _lib.RSB_ERR_INVALID, b"M % 8"),        # M % 8 != 0
     (768, 384, 4, _lib.RSB_ERR_INVALID, b"M / 2"),       # 192 code bytes > 128
     (768, 40, 4, _lib.RSB_ERR_INVALID, b"divisible"),    # d % M != 0
+    (768, 3, 8, _lib.RSB_ERR_UNSUPPORTED, b"n_subquantizers"),      # 8-bit M not a multiple of 4
+    (768, 256, 8, _lib.RSB_ERR_UNSUPPORTED, b"n_subquantizers"),    # 8-bit M > 128
 ])
-def test_create_nbits_refuses(d, M, nbits, want, word):
-    rc, msg = _create("rsb_ivfpq_create_nbits", d, 16, M, nbits)
+def test_ivfpq_create_refuses_bad_nbits_and_shapes(d, M, nbits, want, word):
+    rc, msg = _create(d, 16, M, nbits)
     assert rc == want and word in msg
 
 
-@pytest.mark.parametrize("d,M", [(768, 64), (768, 24), (768, 3), (770, 64), (768, 256)])
-def test_create_nbits_8_is_create(d, M):
-    assert _create("rsb_ivfpq_create_nbits", d, 16, M, 8)[0] == _create("rsb_ivfpq_create", d, 16, M, 8)[0]
-
-
-def test_create_still_refuses_4bit():
-    rc, msg = _create("rsb_ivfpq_create", 768, 16, 64, 4)
-    assert rc == _lib.RSB_ERR_UNSUPPORTED and b"nbits" in msg
-
-
-def test_ksub_entry_points_refuse_other_ksub():
+def test_pq_training_steps_refuse_other_ksub():
     L = _lib.lib()
     p = ctypes.c_void_p(16)          # never dereferenced: the arguments are refused first
-    assert L.rsb_pq_assign_ksub(p, 10, 64, 16, 32, p, p, None) == _lib.RSB_ERR_UNSUPPORTED
-    assert L.rsb_pq_accumulate_ksub(p, 10, 64, 16, 64, p, p, p, None) == _lib.RSB_ERR_UNSUPPORTED
-    assert L.rsb_pq_assign_ksub(p, 10, 64, 15, 16, p, p, None) == _lib.RSB_ERR_INVALID      # d % M
+    assert L.rsb_pq_assign(p, 10, 64, 16, 32, p, p, None) == _lib.RSB_ERR_UNSUPPORTED
+    assert L.rsb_pq_accumulate(p, 10, 64, 16, 64, p, p, p, None) == _lib.RSB_ERR_UNSUPPORTED
+    assert L.rsb_pq_assign(p, 10, 64, 15, 16, p, p, None) == _lib.RSB_ERR_INVALID      # d % M
     assert L.rsb_pq_lut_floats(None) == -1
 
 
