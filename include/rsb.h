@@ -64,7 +64,16 @@ int rsb_flat_create(int d, int dtype, rsb_index_t** out);
 /* faiss.IndexIVFFlat(IndexFlatIP(d), d, nlist, METRIC_INNER_PRODUCT)
  *                                                    <- src/indicies/ivf_flat.py:143-149, api/conf/ivf_flat.yaml
  * With fp16 rows the list scan reads 2 bytes per element and adds in the fp32 scan's order: ids and scores are
- * bit-identical to an fp32 index holding the same values. */
+ * bit-identical to an fp32 index holding the same values.
+ * dtype = RSB_DTYPE_SQ8: faiss.IndexIVFScalarQuantizer(IndexFlatIP(d), d, nlist, QT_8bit, METRIC_INNER_PRODUCT,
+ *   by_residual), factory string "IVFn,SQ8": one uint8 code per element, d % 16 == 0 (else RSB_ERR_INVALID), with the
+ *   train / encode / decode rules of the SQ8 re-rank store below.  The range [2, d] is set with rsb_set_sq_range before
+ *   anything is added (rsb_add / rsb_add_codes / rsb_search before it: RSB_ERR_STATE).  RSB_OPT_BY_RESIDUAL (default 0)
+ *   selects faiss' by_residual: rows are encoded as x - c_list (fp32 subtraction; fp16 rows widen exactly) and every
+ *   score of list l is fl32(coarse_dis + s), coarse_dis = <q, c_l> added once after s = <q, decode(code)> is complete.
+ *   The list scan loads one 4-byte word of codes per lane and step and decodes every element before the fp32 scan's
+ *   fmaf sequence, so s (and, without residuals, ids and scores) is bit-identical to an fp32 index holding the decoded
+ *   rows in the same lists. */
 int rsb_ivfflat_create(int d, int nlist, int dtype, rsb_index_t** out);
 /* faiss.IndexIVFPQ(IndexFlatIP(d), d, nlist, M, nbits, METRIC_INNER_PRODUCT)
  *                                                                    <- src/indicies/ivf_pq.py:146-152
@@ -105,7 +114,9 @@ int rsb_add(rsb_index_t* h, const void* x_dev, int x_dtype, int64_t n, const int
 /* as rsb_add but the coarse assignment is supplied by the caller (int32 list id per row) */
 int rsb_add_preassigned(rsb_index_t* h, const void* x_dev, int x_dtype, int64_t n, const int64_t* ids_dev,
                         const int32_t* list_dev, rsb_stream_t stream);
-/* IVFPQ only: rows are already PQ codes [n, M * nbits / 8] uint8 (e.g. read from an existing index file) */
+/* rows that are already codes (e.g. read from an existing index file): IVFPQ: PQ codes [n, M * nbits / 8] uint8;
+ * IVFFLAT with SQ8 storage: SQ8 codes [n, d] uint8 of the index's range (encoded by residual when RSB_OPT_BY_RESIDUAL
+ * is set).  Other indexes: RSB_ERR_INVALID. */
 int rsb_add_codes(rsb_index_t* h, const uint8_t* codes_dev, int64_t n, const int64_t* ids_dev,
                   const int32_t* list_dev, rsb_stream_t stream);
 /* Build the searchable layout (CSR inverted lists; PQ codes interleaved per 32 vectors).  Synchronises
@@ -119,15 +130,17 @@ enum {
     RSB_INFO_IS_TRAINED = 6,   /* index.is_trained */
     RSB_INFO_MAX_LIST_LEN = 7,
     RSB_INFO_INDEX_BYTES = 8,  /* device bytes held by the searchable layout */
-    RSB_INFO_DTYPE = 9         /* storage dtype of the vectors: RSB_DTYPE_F32 / RSB_DTYPE_F16 (IVFPQ: RSB_DTYPE_F32) */
+    RSB_INFO_DTYPE = 9,        /* storage dtype of the vectors: RSB_DTYPE_F32 / RSB_DTYPE_F16 / RSB_DTYPE_SQ8 (IVFPQ:
+                                  RSB_DTYPE_F32) */
+    RSB_INFO_BY_RESIDUAL = 10  /* 1 if an SQ8 IVFFLAT index encodes residuals (RSB_OPT_BY_RESIDUAL), else 0 */
 };
 int rsb_info(rsb_index_t* h, int what, int64_t* out);
 /* list sizes [nlist] int64 to a device buffer */
 int rsb_list_sizes(rsb_index_t* h, int64_t* sizes_dev, rsb_stream_t stream);
 /* Export the inverted lists in natural CSR order (insertion order inside each list), as the oracle and a
  * faiss file writer want them: offsets_dev [nlist+1] int64, payload_dev = uint8 codes [ntotal, M * nbits / 8] (IVFPQ)
- * or vectors [ntotal, d] in the storage dtype, float32 or fp16 (IVFFLAT / FLAT), ids_dev [ntotal] int64.  Any pointer
- * may be NULL. */
+ * or vectors [ntotal, d] in the storage dtype, float32 or fp16 (IVFFLAT / FLAT), or uint8 SQ8 codes [ntotal, d]
+ * (IVFFLAT with SQ8 storage), ids_dev [ntotal] int64.  Any pointer may be NULL. */
 int rsb_export_lists(rsb_index_t* h, int64_t* offsets_dev, void* payload_dev, int64_t* ids_dev,
                      rsb_stream_t stream);
 
@@ -138,8 +151,9 @@ size_t rsb_workspace_bytes(rsb_index_t* h, int nq, int k, int nprobe);
 int rsb_search(rsb_index_t* h, const float* q_dev, int nq, int k, int nprobe,
                float* D_dev, int64_t* I_dev, void* ws_dev, size_t ws_bytes, rsb_stream_t stream);
 /* faiss IndexIVF::search_preassigned: as rsb_search, but the probed lists list_dev [nq, nprobe] int64 (-1 =
- * skip) and their coarse scores coarse_dis_dev [nq, nprobe] float32 (<q, c_list>, added to every PQ score of
- * that list; ignored by IVFFLAT) come from the caller instead of the coarse quantizer.
+ * skip) and their coarse scores coarse_dis_dev [nq, nprobe] float32 (<q, c_list>, added to every score of that list
+ * by IVFPQ and by an SQ8 IVFFLAT index with RSB_OPT_BY_RESIDUAL; ignored by other IVFFLAT indexes) come from the
+ * caller instead of the coarse quantizer.
  * Thresholds: tau_local_dev = NULL (with tau_peers_dev = NULL, npeers = 0) keeps the per-query running top-k
  * thresholds in the workspace.  Otherwise they are shared between GPUs (one process per GPU, datastore partitioned
  * across the GPUs; replaces the reference's one-process-per-shard search, src/search.py:282-296) in caller-owned
@@ -200,7 +214,8 @@ int rsb_coarse(rsb_index_t* h, const float* q_dev, int nq, int nprobe, int64_t* 
  *     RSB_ERR_INVALID.
  * Every argument is checked before any launch.  The workspace queries return 0 for arguments the call would refuse;
  * they size the all-device store by nq, k_base and k alone, and the tiered store by its dtype and staging_bytes. */
-enum { RSB_DTYPE_F32 = 0, RSB_DTYPE_F16 = 1, RSB_DTYPE_SQ8 = 2 /* re-rank store only */ };
+/* RSB_DTYPE_SQ8: a re-rank store, or the storage of an IVFFLAT index (rsb_ivfflat_create); not a Flat index */
+enum { RSB_DTYPE_F32 = 0, RSB_DTYPE_F16 = 1, RSB_DTYPE_SQ8 = 2 };
 int rsb_host_alloc(size_t bytes, void** out);   /* cudaHostAlloc(portable | mapped): exactly `bytes`, unlike torch's
                                                    pinned allocator, which rounds blocks up to a power of two */
 int rsb_host_free(void* p);
@@ -227,6 +242,11 @@ int rsb_refine_tiered_profile(int enable, double* ms_out);
 int rsb_sq8_train(const void* x_dev, int x_dtype, int64_t n, int d, float* sq_dev, rsb_stream_t stream);
 int rsb_sq8_encode(const void* x_dev, int x_dtype, int64_t n, int d, const float* sq_dev, uint8_t* codes_dev,
                    rsb_stream_t stream);
+/* The range of an IVFFLAT index with SQ8 storage: sq_dev [2, d] float32 (vmin, then vdiff), copied.  Other handles:
+ * RSB_ERR_INVALID.  rsb_set_sq_range on a populated index and rsb_get_sq_range before a range is set: RSB_ERR_STATE.
+ * RSB_INFO_IS_TRAINED of such an index means centroids and range are both set. */
+int rsb_set_sq_range(rsb_index_t* h, const float* sq_dev, rsb_stream_t stream);
+int rsb_get_sq_range(rsb_index_t* h, float* out_dev, rsb_stream_t stream);
 
 /* ---- shard merge (src/search.py:357-367; api/serve_main_node.py:130-163) ---------------------------- */
 /* D_all_dev/I_all_dev [nshards, nq, k]: concat per query, sort by score desc (ties: lower shard, then lower
@@ -273,9 +293,12 @@ int rsb_pq_accumulate(const float* r_dev, int64_t n, int d, int M, int ksub, con
 
 /* ---- options -------------------------------------------------------------------------------------------- */
 enum {
-    RSB_OPT_COARSE_TENSOR = 0 /* 1 (default): coarse quantizer scores by 3xTF32 on wgmma tensor cores (fp32-equivalent
+    RSB_OPT_COARSE_TENSOR = 0,/* 1 (default): coarse quantizer scores by 3xTF32 on wgmma tensor cores (fp32-equivalent
                                  accuracy); 0: CUDA-core fp32 FMA tiles.  0 on an fp16 Flat index returns
                                  RSB_ERR_UNSUPPORTED: its rows are scored on tensor cores only */
+    RSB_OPT_BY_RESIDUAL = 1   /* SQ8 IVFFLAT only (RSB_ERR_INVALID on other handles), before anything is added
+                                 (RSB_ERR_STATE after): 1 encodes x - c_list and adds the coarse score (faiss by_residual,
+                                 the default of index_factory "IVFn,SQ8"); 0 (default) encodes x */
 };
 int rsb_set_option(rsb_index_t* h, int option, int64_t value);
 
@@ -287,7 +310,7 @@ enum {
     RSB_PROF_SCAN_MS = 3,   /* inverted-list scan kernel (the hot one)  */
     RSB_PROF_MERGE_MS = 4,  /* per-query top-k merge                    */
     RSB_PROF_SCAN_BYTES = 5,/* algorithmic bytes of the scan: sum over probed (q,list) pairs of len*row_bytes
-                               (IVF-Flat row_bytes = d * 4, or d * 2 with fp16 storage) */
+                               (IVF-Flat row_bytes = d * 4, d * 2 with fp16 storage, d with SQ8 storage) */
     RSB_PROF_PAIRS = 6,     /* number of valid (q,list) pairs            */
     RSB_PROF_LAUNCHES = 7,  /* kernels launched by the last search       */
     RSB_PROF_SCAN_PATH = 8, /* IVFPQ scan: 1 = literal-offset shared-memory look-ups, 2 = generic addressing */

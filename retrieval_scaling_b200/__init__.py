@@ -15,6 +15,6 @@ def _lazy():
 
 
 def __getattr__(name):
-    if name in ("IndexFlatIP", "IndexIVFFlat", "IndexIVFPQ", "IndexRefine", "read_index", "write_index", "merge_topk", "knn_ip"):
+    if name in ("IndexFlatIP", "IndexIVFFlat", "IndexIVFPQ", "IndexIVFScalarQuantizer", "IndexRefine", "read_index", "write_index", "merge_topk", "knn_ip"):
         return getattr(_lazy(), name)
     raise AttributeError(name)

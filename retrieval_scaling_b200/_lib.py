@@ -15,7 +15,8 @@ RSB_ERR_INVALID, RSB_ERR_CUDA, RSB_ERR_STATE, RSB_ERR_UNSUPPORTED, RSB_ERR_OOM =
 RSB_FLAT, RSB_IVFFLAT, RSB_IVFPQ = 0, 1, 2
 RSB_DTYPE_F32, RSB_DTYPE_F16, RSB_DTYPE_SQ8 = 0, 1, 2
 (INFO_KIND, INFO_D, INFO_NLIST, INFO_M, INFO_NBITS, INFO_NTOTAL, INFO_IS_TRAINED, INFO_MAX_LIST_LEN,
- INFO_INDEX_BYTES, INFO_DTYPE) = range(10)
+ INFO_INDEX_BYTES, INFO_DTYPE, INFO_BY_RESIDUAL) = range(11)
+OPT_COARSE_TENSOR, OPT_BY_RESIDUAL = 0, 1
 PROF_NAMES = ("coarse_ms", "setup_ms", "lut_ms", "scan_ms", "merge_ms", "scan_bytes", "pairs", "launches", "scan_path",
               "rescored")
 
@@ -60,6 +61,8 @@ SIGNATURES = [
     ("rsb_refine_tiered_profile", c_int, [c_int, POINTER(c_double)]),
     ("rsb_sq8_train", c_int, [c_void_p, c_int, c_int64, c_int, c_void_p, c_void_p]),
     ("rsb_sq8_encode", c_int, [c_void_p, c_int, c_int64, c_int, c_void_p, c_void_p, c_void_p]),
+    ("rsb_set_sq_range", c_int, [_H, c_void_p, c_void_p]),
+    ("rsb_get_sq_range", c_int, [_H, c_void_p, c_void_p]),
     ("rsb_merge_topk", c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     ("rsb_merge_topk_peers", c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     ("rsb_merge_topk_peers_scatter", c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,

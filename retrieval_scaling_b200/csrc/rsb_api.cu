@@ -61,7 +61,11 @@ struct rsb_index {
     // Mb = M * nbits / 8 code bytes per vector (layout, interleave, tables, scan, export).  nbits = 4 packs two codes
     // per byte and is scanned as an 8-bit index of Mb byte sub-quantizers (rsb_ivf.cu, pq_lut4_kernel).
     int kind = 0, d = 0, nlist = 0, M = 0, nbits = 0, dsub = 0, Mb = 0;
-    int dtype = RSB_DTYPE_F32;   // storage of FLAT / IVFFLAT rows: RSB_DTYPE_F32 or RSB_DTYPE_F16
+    int dtype = RSB_DTYPE_F32;   // storage of FLAT / IVFFLAT rows: RSB_DTYPE_F32, RSB_DTYPE_F16 or (IVFFLAT) RSB_DTYPE_SQ8
+    // IVFFLAT with RSB_DTYPE_SQ8 (faiss IndexIVFScalarQuantizer, QT_8bit): sq [2, d] = (vmin, vdiff); by_residual encodes
+    // x - c_list and adds the list's coarse score to every score of the list
+    float* sq = nullptr;
+    bool has_sq = false, by_residual = false;
     float* centroids = nullptr;
     float* codebook = nullptr;
     float* codebook_t = nullptr;
@@ -97,7 +101,7 @@ struct rsb_index {
     int ev_done = 0;
     unsigned long long* prof_dev = nullptr;  // [4]: scan elements, pairs, scan path flag, re-scored vectors
     long launches = 0;
-    int elem_bytes() const { return dtype == RSB_DTYPE_F16 ? 2 : 4; }
+    int elem_bytes() const { return dtype == RSB_DTYPE_SQ8 ? 1 : dtype == RSB_DTYPE_F16 ? 2 : 4; }
     size_t row_bytes() const { return kind == RSB_IVFPQ ? (size_t)Mb : (size_t)d * elem_bytes(); }
     int ksub() const { return 1 << nbits; }
 };
@@ -123,8 +127,11 @@ static int create_common(int kind, int d, int nlist, int M, int nbits, int dtype
     if (!out) return fail(RSB_ERR_INVALID, "out is NULL");
     *out = nullptr;
     if (d <= 0 || (d & 3)) return fail(RSB_ERR_INVALID, "dimension must be a positive multiple of 4, got %d", d);
-    if (dtype != RSB_DTYPE_F32 && dtype != RSB_DTYPE_F16)
-        return fail(RSB_ERR_INVALID, "dtype must be RSB_DTYPE_F32 or RSB_DTYPE_F16, got %d", dtype);
+    if (dtype != RSB_DTYPE_F32 && dtype != RSB_DTYPE_F16 && !(dtype == RSB_DTYPE_SQ8 && kind == RSB_IVFFLAT))
+        return fail(RSB_ERR_INVALID, "dtype must be RSB_DTYPE_F32 or RSB_DTYPE_F16%s, got %d",
+                    kind == RSB_IVFFLAT ? " or RSB_DTYPE_SQ8" : "", dtype);
+    if (dtype == RSB_DTYPE_SQ8 && d % 16)
+        return fail(RSB_ERR_INVALID, "SQ8 storage needs whole 16-byte rows: d = %d is not a multiple of 16", d);
     if (dtype == RSB_DTYPE_F16) {
         if (d % 8) return fail(RSB_ERR_INVALID, "fp16 storage needs 16-byte rows: d = %d is not a multiple of 8", d);
         if (kind == RSB_FLAT && d % 64)
@@ -162,7 +169,7 @@ extern "C" int rsb_free(rsb_index_t* h) {
     if (!h) return RSB_OK;
     for (auto& s : h->staging) free_segment(s);
     free_layout(h);
-    cudaFree(h->centroids); cudaFree(h->codebook); cudaFree(h->codebook_t); cudaFree(h->prof_dev);
+    cudaFree(h->centroids); cudaFree(h->codebook); cudaFree(h->codebook_t); cudaFree(h->prof_dev); cudaFree(h->sq);
     cudaFree(h->cent_hi); cudaFree(h->cent_lo);
     for (auto& set : h->evs) for (auto& e : set) if (e) cudaEventDestroy(e);
     delete h;
@@ -216,9 +223,28 @@ extern "C" int rsb_get_pq_codebook(rsb_index_t* h, float* out, rsb_stream_t stre
     return RSB_OK;
 }
 
+static bool is_sq8_ivf(const rsb_index* h) { return h->kind == RSB_IVFFLAT && h->dtype == RSB_DTYPE_SQ8; }
+extern "C" int rsb_set_sq_range(rsb_index_t* h, const float* sq, rsb_stream_t stream) {
+    if (!h || !sq) return fail(RSB_ERR_INVALID, "null argument");
+    if (!is_sq8_ivf(h)) return fail(RSB_ERR_INVALID, "only an IVFFLAT index with RSB_DTYPE_SQ8 storage has a scalar-quantizer range");
+    if (h->ntotal || h->n_staged) return fail(RSB_ERR_STATE, "cannot change the range of a populated index (its codes use it)");
+    const size_t bytes = (size_t)2 * h->d * 4;
+    if (!h->sq) CU(cudaMalloc(&h->sq, bytes));
+    CU(cudaMemcpyAsync(h->sq, sq, bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+    h->has_sq = true;
+    return RSB_OK;
+}
+extern "C" int rsb_get_sq_range(rsb_index_t* h, float* out, rsb_stream_t stream) {
+    if (!h || !out) return fail(RSB_ERR_INVALID, "null argument");
+    if (!is_sq8_ivf(h)) return fail(RSB_ERR_INVALID, "only an IVFFLAT index with RSB_DTYPE_SQ8 storage has a scalar-quantizer range");
+    if (!h->has_sq) return fail(RSB_ERR_STATE, "the scalar-quantizer range is not set");
+    CU(cudaMemcpyAsync(out, h->sq, (size_t)2 * h->d * 4, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+    return RSB_OK;
+}
+
 static bool is_trained(const rsb_index* h) {
     if (h->kind == RSB_FLAT) return true;
-    if (h->kind == RSB_IVFFLAT) return h->has_centroids;
+    if (h->kind == RSB_IVFFLAT) return h->has_centroids && (h->dtype != RSB_DTYPE_SQ8 || h->has_sq);
     return h->has_centroids && h->has_codebook;
 }
 
@@ -385,7 +411,9 @@ static int add_impl(rsb_index* h, const void* x, int x_dtype, const uint8_t* cod
     if (n < 0) return fail(RSB_ERR_INVALID, "n < 0");
     if (n == 0) return RSB_OK;
     if (!x && !codes_in) return fail(RSB_ERR_INVALID, "null data pointer");
-    if (!is_trained(h)) return fail(RSB_ERR_STATE, "index is not trained (set centroids%s first)", h->kind == RSB_IVFPQ ? " and PQ codebook" : "");
+    if (!is_trained(h))
+        return fail(RSB_ERR_STATE, "index is not trained (set centroids%s first)",
+                    h->kind == RSB_IVFPQ ? " and PQ codebook" : is_sq8_ivf(h) ? " and the SQ8 range" : "");
     // slots are 32-bit in the candidate keys (2^32) and rsb_finalize sorts (list, row) pairs with a 32-bit item count
     if (h->ntotal + h->n_staged + n >= ((int64_t)1 << 31) - 64 * (int64_t)h->nlist)
         return fail(RSB_ERR_UNSUPPORTED, "more than 2^31 vectors per index shard (shard the datastore across GPUs)");
@@ -417,10 +445,17 @@ static int add_impl(rsb_index* h, const void* x, int x_dtype, const uint8_t* cod
             if (rc != RSB_OK) return bail(rc);
         }
     }
-    if (h->kind == RSB_IVFPQ) {
+    if (codes_in) {     // IVFPQ codes or SQ8 codes, as stored
+        CUB_(cudaMalloc(&seg.payload, (size_t)n * h->row_bytes()));
+        CUB_(cudaMemcpyAsync(seg.payload, codes_in, (size_t)n * h->row_bytes(), cudaMemcpyDeviceToDevice, st));
+    } else if (is_sq8_ivf(h)) {
+        // encode on the device; by residual: x - c_list of the list just assigned (fp16 rows widen exactly)
+        CUB_(cudaMalloc(&seg.payload, (size_t)n * h->d));
+        CUB_(launch_sq8_encode(x, x_dtype == RSB_DTYPE_F16, n, h->d, h->sq, static_cast<uint8_t*>(seg.payload), st,
+                               h->by_residual ? seg.list : nullptr, h->centroids));
+    } else if (h->kind == RSB_IVFPQ) {
         CUB_(cudaMalloc(&seg.payload, (size_t)n * h->Mb));
-        if (codes_in) CUB_(cudaMemcpyAsync(seg.payload, codes_in, (size_t)n * h->Mb, cudaMemcpyDeviceToDevice, st));
-        else if (h->nbits == 4)
+        if (h->nbits == 4)
             launch_pq_encode4(static_cast<const float*>(x), n, h->d, seg.list, h->centroids, h->codebook, h->M, true,
                               static_cast<uint8_t*>(seg.payload), st);
         else launch_pq_encode(static_cast<const float*>(x), n, h->d, seg.list, h->centroids, h->codebook, h->M,
@@ -454,7 +489,8 @@ extern "C" int rsb_add_preassigned(rsb_index_t* h, const void* x, int x_dtype, i
 }
 extern "C" int rsb_add_codes(rsb_index_t* h, const uint8_t* codes, int64_t n, const int64_t* ids,
                              const int32_t* list, rsb_stream_t stream) {
-    if (!h || h->kind != RSB_IVFPQ) return fail(RSB_ERR_INVALID, "rsb_add_codes needs an IVFPQ index");
+    if (!h || (h->kind != RSB_IVFPQ && !is_sq8_ivf(h)))
+        return fail(RSB_ERR_INVALID, "rsb_add_codes needs an IVFPQ index or an IVFFLAT index with SQ8 storage");
     if (!list || !codes) return fail(RSB_ERR_INVALID, "null argument");
     return add_impl(h, nullptr, RSB_DTYPE_F32, codes, n, ids, list, nullptr, 0, (cudaStream_t)stream);
 }
@@ -660,6 +696,7 @@ extern "C" int rsb_info(rsb_index_t* h, int what, int64_t* out) {
         case RSB_INFO_MAX_LIST_LEN: *out = h->max_list_len; break;
         case RSB_INFO_INDEX_BYTES: *out = (int64_t)(h->payload_bytes + (size_t)h->nslots * 8); break;
         case RSB_INFO_DTYPE: *out = h->dtype; break;
+        case RSB_INFO_BY_RESIDUAL: *out = h->by_residual ? 1 : 0; break;
         default: return fail(RSB_ERR_INVALID, "unknown info key %d", what);
     }
     return RSB_OK;
@@ -1027,7 +1064,7 @@ static int search_impl(rsb_index_t* h, const float* q, int nq, int k, int nprobe
                 return fail(RSB_ERR_UNSUPPORTED, "no scan kernel for %d code bytes per vector", h->Mb);
         } else {
             if (prof) CU(cudaEventRecord(h->ev[3], st));
-            launch_ivfflat_scan(a, qb, h->payload, h->elem_bytes(), h->d, nb, st);
+            launch_ivfflat_scan(a, qb, h->payload, h->elem_bytes(), h->d, nb, st, h->sq, h->by_residual);
         }
         h->launches += paired ? 2 : 1;                 // paired work list: both scan variants, one returns at once
         if (prof) CU(cudaEventRecord(h->ev[4], st));
@@ -1371,6 +1408,10 @@ extern "C" int rsb_set_option(rsb_index_t* h, int option, int64_t value) {
             if (value == 0 && h->kind == RSB_FLAT && h->dtype == RSB_DTYPE_F16)
                 return fail(RSB_ERR_UNSUPPORTED, "an fp16 Flat index scores on tensor cores only (no CUDA-core fp16 path)");
             h->coarse_tensor = value != 0; h->flat_tensor = value != 0; return RSB_OK;
+        case RSB_OPT_BY_RESIDUAL:
+            if (!is_sq8_ivf(h)) return fail(RSB_ERR_INVALID, "RSB_OPT_BY_RESIDUAL applies to an IVFFLAT index with SQ8 storage only");
+            if (h->ntotal || h->n_staged) return fail(RSB_ERR_STATE, "by_residual cannot change once vectors are added");
+            h->by_residual = value != 0; return RSB_OK;
         default: return fail(RSB_ERR_INVALID, "unknown option %d", option);
     }
 }

@@ -23,6 +23,19 @@ __device__ __forceinline__ float4 load_row4(const __half* p) {
     return make_float4(a.x, a.y, b.x, b.y);
 }
 
+// SQ8 decode (faiss ScalarQuantizer QT_8bit, non-uniform): x = vmin + ((c + 0.5f) / 255.f) * vdiff for the code c in
+// byte `byte` of w, every operation a separately rounded fp32 op.  c + 0.5 is exact from the bits of 2^23 + c; the
+// quotient comes from a reciprocal multiply and one fma correction, which gives the correctly rounded (c + 0.5f) / 255.f
+// for each of the 256 codes (a plain reciprocal multiply differs for 191 of them).  __fmul_rn / __fadd_rn keep nvcc
+// from contracting the decode.  Used by the SQ8 re-rank store and the IVF-SQ8 list scan.
+__device__ __forceinline__ float sq8_decode(unsigned w, unsigned byte, float vmin, float vdiff) {
+    constexpr float inv = 1.f / 255.f;
+    const float a = __fadd_rn(__uint_as_float(__byte_perm(w, 0x4B000000u, 0x7440u | byte)), -8388607.5f);
+    const float t = __fmul_rn(a, inv);
+    const float u = __fmaf_rn(__fmaf_rn(-t, 255.f, a), inv, t);
+    return __fadd_rn(vmin, __fmul_rn(u, vdiff));
+}
+
 // ---- order-preserving float <-> uint mapping (larger float => larger uint) -------------------------------
 __device__ __forceinline__ unsigned ord_f32(float f) {
     unsigned u = __float_as_uint(f);

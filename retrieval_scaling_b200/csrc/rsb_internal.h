@@ -107,10 +107,11 @@ cudaError_t launch_refine_tiered(const TieredPlan& p, const float* Q, int nq, co
                                  int k_base, int k, float* D, int64_t* I, void* ws, long long* host_rows,
                                  cudaStream_t st);
 // SQ8 store (faiss ScalarQuantizer QT_8bit, RS_minmax, per dimension): x [n, d] fp32 (x_f16 = 0) or fp16 (x_f16 = 1);
-// sq [2, d] fp32 = (vmin, vdiff).  train: vmin = min over the rows, vdiff = max - vmin.  encode: codes [n, d] uint8.
+// sq [2, d] fp32 = (vmin, vdiff).  train: vmin = min over the rows, vdiff = max - vmin.  encode: codes [n, d] uint8;
+// with list [n] int32 and centroids [nlist, d] (IVF-SQ8 by residual) row i is encoded as x[i] - centroids[list[i]].
 cudaError_t launch_sq8_train(const void* x, int x_f16, int64_t n, int d, float* sq, cudaStream_t st);
 cudaError_t launch_sq8_encode(const void* x, int x_f16, int64_t n, int d, const float* sq, uint8_t* codes,
-                              cudaStream_t st);
+                              cudaStream_t st, const int32_t* list = nullptr, const float* centroids = nullptr);
 // enable != 0: time every later tiered chunk's sort / gather / score with events (synchronises per chunk).
 // ms3 (nullable) <- the milliseconds accumulated since the previous call, which resets them.
 int tiered_profile(int enable, double* ms3);
@@ -202,9 +203,11 @@ struct ScanArgs {
     u64* rescored;                // nullable: += vectors re-scored exactly after the quantised filter
 };
 
-// IVF-Flat: vecs [nslots, d] in CSR order, fp32 (elem_bytes 4) or fp16 (elem_bytes 2); queries [nq, d] fp32
+// IVF-Flat: vecs [nslots, d] in CSR order, fp32 (elem_bytes 4), fp16 (elem_bytes 2) or SQ8 codes (elem_bytes 1, with
+// sq [2, d] fp32 = (vmin, vdiff); by_residual: each score is a.coarse_scores[pair] + the score of the decoded codes);
+// queries [nq, d] fp32
 void launch_ivfflat_scan(const ScanArgs& a, const float* queries, const void* vecs, int elem_bytes, int d, int nq,
-                         cudaStream_t st);
+                         cudaStream_t st, const float* sq = nullptr, bool by_residual = false);
 
 // IVF-PQ
 void launch_pq_lut(const float* queries, int nq, int d, int M, const float* codebook_t, float* lut,

@@ -198,23 +198,34 @@ __device__ __forceinline__ void raise_tau(const ScanArgs& a, int q, unsigned v) 
 // fp32 FMA, a 5-shuffle transposing reduction; scores above the running threshold go to the block's candidate
 // buffer.  HBM/L2-bandwidth bound: 4*d bytes per scored vector (fp32 rows) or 2*d (fp16 rows: lane l loads the
 // 4 halves of elements 4l + 128j .. +3 with one 8-byte load and runs the fp32 kernel's fmaf sequence on them, so
-// scores are bit-identical to those of fp32 rows holding the same values).
+// scores are bit-identical to those of fp32 rows holding the same values), or d bytes (SQ8 codes, T = uint8_t: lane l
+// loads the 4 codes of elements 4l + 128j .. +3 with one 4-byte load, decodes each with sq8_decode from vmin / vdiff
+// staged in shared memory after the query, and runs the same fmaf sequence, so scores are bit-identical to those of
+// fp32 rows holding the decoded values; by_residual adds the list's coarse score once, after the reduction).
 // =============================================================================================================
 constexpr int FS_THREADS = 256;
 constexpr int FS_WARPS = FS_THREADS / 32;
 constexpr int FS_CHECK = 16;                             // iterations between capacity checks
 constexpr int FS_SLACK = FS_CHECK * FS_WARPS * 2;        // candidates appended between checks (256)
 
+// floats of shared memory before the candidate keys: the query [d], then (SQ8) vmin [d] and vdiff [d]
+template <typename T> constexpr int fs_smem_rows() { return sizeof(T) == 1 ? 3 : 1; }
+
 template <typename T>
-__global__ __launch_bounds__(FS_THREADS)
-void ivfflat_scan_kernel(ScanArgs a, const float* __restrict__ queries, const T* __restrict__ vecs, int d,
-                         int cap) {
+__device__ __forceinline__ void ivfflat_scan_body(ScanArgs a, const float* __restrict__ queries,
+                                                  const T* __restrict__ vecs, int d, int cap,
+                                                  const float* __restrict__ sq, int by_residual) {
+    constexpr bool SQ8 = sizeof(T) == 1;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float* qs = reinterpret_cast<float*>(smem_raw);
-    u64* keys = reinterpret_cast<u64*>(smem_raw + (((size_t)d * 4 + 15) & ~(size_t)15));
+    u64* keys = reinterpret_cast<u64*>(smem_raw + (((size_t)d * 4 * fs_smem_rows<T>() + 15) & ~(size_t)15));
     __shared__ int s_count, s_item;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int n_items = *a.n_items;
+    if constexpr (SQ8) {
+        for (int c = tid * 4; c < 2 * d; c += FS_THREADS * 4)
+            *reinterpret_cast<float4*>(qs + d + c) = *reinterpret_cast<const float4*>(sq + c);
+    }
     int cur_q = -1;
     for (;;) {
         __syncthreads();
@@ -234,6 +245,7 @@ void ivfflat_scan_kernel(ScanArgs a, const float* __restrict__ queries, const T*
         __syncthreads();
         const int len = a.list_len[list];
         const int64_t base = a.list_off[list];
+        [[maybe_unused]] const float coarse = SQ8 && by_residual ? a.coarse_scores[pair] : 0.f;
         const int n_iter = (len + 2 * FS_WARPS - 1) / (2 * FS_WARPS);
         for (int it = 0; it < n_iter; ++it) {
             const int v0 = (it * FS_WARPS + warp) * 2, v1 = v0 + 1;
@@ -243,8 +255,20 @@ void ivfflat_scan_kernel(ScanArgs a, const float* __restrict__ queries, const T*
             float a0 = 0.f, a1 = 0.f;
 #pragma unroll 6
             for (int c = lane * 4; c < d; c += 128) {
-                const float4 x0 = load_row4(p0 + c);
-                const float4 x1 = load_row4(p1 + c);
+                float4 x0, x1;
+                if constexpr (SQ8) {
+                    const unsigned w0 = __ldg(reinterpret_cast<const unsigned*>(p0 + c));
+                    const unsigned w1 = __ldg(reinterpret_cast<const unsigned*>(p1 + c));
+                    const float4 lo = *reinterpret_cast<const float4*>(qs + d + c);
+                    const float4 df = *reinterpret_cast<const float4*>(qs + 2 * d + c);
+                    x0 = make_float4(sq8_decode(w0, 0, lo.x, df.x), sq8_decode(w0, 1, lo.y, df.y),
+                                     sq8_decode(w0, 2, lo.z, df.z), sq8_decode(w0, 3, lo.w, df.w));
+                    x1 = make_float4(sq8_decode(w1, 0, lo.x, df.x), sq8_decode(w1, 1, lo.y, df.y),
+                                     sq8_decode(w1, 2, lo.z, df.z), sq8_decode(w1, 3, lo.w, df.w));
+                } else {
+                    x0 = load_row4(p0 + c);
+                    x1 = load_row4(p1 + c);
+                }
                 const float4 qv = *reinterpret_cast<const float4*>(qs + c);
                 a0 = fmaf(x0.x, qv.x, a0); a0 = fmaf(x0.y, qv.y, a0); a0 = fmaf(x0.z, qv.z, a0); a0 = fmaf(x0.w, qv.w, a0);
                 a1 = fmaf(x1.x, qv.x, a1); a1 = fmaf(x1.y, qv.y, a1); a1 = fmaf(x1.z, qv.z, a1); a1 = fmaf(x1.w, qv.w, a1);
@@ -257,6 +281,9 @@ void ivfflat_scan_kernel(ScanArgs a, const float* __restrict__ queries, const T*
             keep += __shfl_xor_sync(0xffffffffu, keep, 4);
             keep += __shfl_xor_sync(0xffffffffu, keep, 2);
             keep += __shfl_xor_sync(0xffffffffu, keep, 1);
+            if constexpr (SQ8) {
+                if (by_residual) keep = __fadd_rn(coarse, keep);     // faiss: coarse_dis + <q, decoded residual>
+            }
             const unsigned o = ord_f32(keep);
             const bool mine = (lane == 0 && ok0) || (lane == 16 && ok1);
             const unsigned slot = (unsigned)(base + ((lane & 16) ? v1 : v0));
@@ -277,29 +304,46 @@ void ivfflat_scan_kernel(ScanArgs a, const float* __restrict__ queries, const T*
     }
 }
 
+template <typename T>
+__global__ __launch_bounds__(FS_THREADS)
+void ivfflat_scan_kernel(ScanArgs a, const float* __restrict__ queries, const T* __restrict__ vecs, int d, int cap) {
+    ivfflat_scan_body<T>(a, queries, vecs, d, cap, nullptr, 0);
+}
+
+// SQ8 codes: sq [2, d] = (vmin, vdiff); by_residual != 0 adds a.coarse_scores[pair] to every score of the pair
+__global__ __launch_bounds__(FS_THREADS)
+void ivfflat_scan_sq8_kernel(ScanArgs a, const float* __restrict__ queries, const uint8_t* __restrict__ vecs, int d,
+                             int cap, const float* __restrict__ sq, int by_residual) {
+    ivfflat_scan_body<uint8_t>(a, queries, vecs, d, cap, sq, by_residual);
+}
+
 static int num_sms() { return device_num_sms(); }
 
-template <typename T>
-static void launch_ivfflat_scan_t(const ScanArgs& a, const float* queries, const T* vecs, int d, int npairs,
-                                  cudaStream_t st) {
+template <typename T, typename... Extra>
+static void launch_ivfflat_scan_t(void (*kernel)(ScanArgs, const float*, const T*, int, int, Extra...), const ScanArgs& a,
+                                  const float* queries, const T* vecs, int d, int npairs, cudaStream_t st, Extra... extra) {
     const int cap = cand_capacity(a.k, FS_SLACK);
-    const size_t smem = (((size_t)d * 4 + 15) & ~(size_t)15) + (size_t)cap * 8;
-    cudaFuncSetAttribute(ivfflat_scan_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    const size_t smem = (((size_t)d * 4 * fs_smem_rows<T>() + 15) & ~(size_t)15) + (size_t)cap * 8;
+    cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     int occ = 1;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, ivfflat_scan_kernel<T>, FS_THREADS, smem);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, FS_THREADS, smem);
     if (occ < 1) occ = 1;
     const int grid = min(npairs, num_sms() * occ);
-    ivfflat_scan_kernel<T><<<grid, FS_THREADS, smem, st>>>(a, queries, vecs, d, cap);
+    kernel<<<grid, FS_THREADS, smem, st>>>(a, queries, vecs, d, cap, extra...);
 }
 
 void launch_ivfflat_scan(const ScanArgs& a, const float* queries, const void* vecs, int elem_bytes, int d, int nq,
-                         cudaStream_t st) {
+                         cudaStream_t st, const float* sq, bool by_residual) {
     const int npairs = nq * a.nprobe;
     if (!a.tau_external) cudaMemsetAsync(a.tau, 0, (size_t)nq * 4, st);
     cudaMemsetAsync(a.out_cnt, 0, (size_t)npairs * 4, st);
     if (npairs == 0) return;
-    if (elem_bytes == 2) launch_ivfflat_scan_t(a, queries, static_cast<const __half*>(vecs), d, npairs, st);
-    else launch_ivfflat_scan_t(a, queries, static_cast<const float*>(vecs), d, npairs, st);
+    if (elem_bytes == 1)
+        launch_ivfflat_scan_t(ivfflat_scan_sq8_kernel, a, queries, static_cast<const uint8_t*>(vecs), d, npairs, st, sq,
+                              by_residual ? 1 : 0);
+    else if (elem_bytes == 2)
+        launch_ivfflat_scan_t(ivfflat_scan_kernel<__half>, a, queries, static_cast<const __half*>(vecs), d, npairs, st);
+    else launch_ivfflat_scan_t(ivfflat_scan_kernel<float>, a, queries, static_cast<const float*>(vecs), d, npairs, st);
 }
 
 // =============================================================================================================

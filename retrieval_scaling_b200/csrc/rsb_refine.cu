@@ -62,18 +62,7 @@ __device__ __forceinline__ float dot8(const uint4 (&v)[1], const float* qs, floa
     return acc;
 }
 
-// SQ8 decode (faiss ScalarQuantizer QT_8bit, non-uniform): x = vmin + ((c + 0.5f) / 255.f) * vdiff, every operation a
-// separately rounded fp32 op.  c + 0.5 is exact from the bits of 2^23 + c; the quotient comes from a reciprocal
-// multiply and one fma correction, which gives the correctly rounded (c + 0.5f) / 255.f for each of the 256 codes
-// (a plain reciprocal multiply differs for 191 of them).  __fmul_rn / __fadd_rn keep nvcc from contracting the decode.
-__device__ __forceinline__ float sq8_decode(unsigned w, unsigned byte, float vmin, float vdiff) {
-    constexpr float inv = 1.f / 255.f;
-    const float a = __fadd_rn(__uint_as_float(__byte_perm(w, 0x4B000000u, 0x7440u | byte)), -8388607.5f);
-    const float t = __fmul_rn(a, inv);
-    const float u = __fmaf_rn(__fmaf_rn(-t, 255.f, a), inv, t);
-    return __fadd_rn(vmin, __fmul_rn(u, vdiff));
-}
-
+// SQ8 codes: sq8_decode (rsb_common.cuh) per element, then the same fmaf.
 __device__ __forceinline__ float dot8(const uint2 (&v)[1], const float* qs, float acc, uint8_t, const float* sq,
                                       int sq_d) {
 #pragma unroll
@@ -486,15 +475,19 @@ __global__ void sq8_finish_kernel(float* __restrict__ sq, int d) {
     sq[d + j] = __fsub_rn(vmax, vmin);
 }
 
-// code = (int)(255.f * clamp((x - vmin) / vdiff, 0, 1)), 0 where vdiff == 0; separately rounded fp32 ops
+// code = (int)(255.f * clamp((x - vmin) / vdiff, 0, 1)), 0 where vdiff == 0; separately rounded fp32 ops.
+// list != null (IVF-SQ8 by residual): x is first replaced by the fp32 residual x - centroids[list[row]].
 template <typename T>
 __global__ __launch_bounds__(SQ_THREADS)
 void sq8_encode_kernel(const T* __restrict__ x, size_t total, int d, const float* __restrict__ sq,
-                       uint8_t* __restrict__ codes) {
+                       uint8_t* __restrict__ codes, const int32_t* __restrict__ list,
+                       const float* __restrict__ centroids) {
     for (size_t i = (size_t)blockIdx.x * SQ_THREADS + threadIdx.x; i < total; i += (size_t)gridDim.x * SQ_THREADS) {
         const int j = (int)(i % d);
         const float vmin = sq[j], vdiff = sq[d + j];
-        float xi = vdiff != 0.f ? __fdiv_rn(__fsub_rn(to_f32(x[i]), vmin), vdiff) : 0.f;
+        float v = to_f32(x[i]);
+        if (list) v = __fsub_rn(v, centroids[(size_t)list[i / d] * d + j]);
+        float xi = vdiff != 0.f ? __fdiv_rn(__fsub_rn(v, vmin), vdiff) : 0.f;
         xi = xi < 0.f ? 0.f : (xi > 1.f ? 1.f : xi);
         codes[i] = (uint8_t)(int)__fmul_rn(255.f, xi);
     }
@@ -512,11 +505,15 @@ cudaError_t launch_sq8_train(const void* x, int x_f16, int64_t n, int d, float* 
 }
 
 cudaError_t launch_sq8_encode(const void* x, int x_f16, int64_t n, int d, const float* sq, uint8_t* codes,
-                              cudaStream_t st) {
+                              cudaStream_t st, const int32_t* list, const float* centroids) {
     const size_t total = (size_t)n * d;
     const unsigned blocks = (unsigned)std::min<size_t>((total + SQ_THREADS - 1) / SQ_THREADS, 132 * 64);
-    if (x_f16) sq8_encode_kernel<__half><<<blocks, SQ_THREADS, 0, st>>>(static_cast<const __half*>(x), total, d, sq, codes);
-    else sq8_encode_kernel<float><<<blocks, SQ_THREADS, 0, st>>>(static_cast<const float*>(x), total, d, sq, codes);
+    if (x_f16)
+        sq8_encode_kernel<__half><<<blocks, SQ_THREADS, 0, st>>>(static_cast<const __half*>(x), total, d, sq, codes, list,
+                                                                 centroids);
+    else
+        sq8_encode_kernel<float><<<blocks, SQ_THREADS, 0, st>>>(static_cast<const float*>(x), total, d, sq, codes, list,
+                                                                centroids);
     return cudaPeekAtLastError();
 }
 

@@ -3,6 +3,7 @@ persists with `faiss.write_index` / loads with `faiss.read_index` (`src/indicies
 `ivf_flat.py:71,167,185`, `ivf_pq.py:75,171,190`):
 
     "IxFI"  IndexFlatIP            "IwFl"  IndexIVFFlat (quantizer IndexFlatIP)      "IwPQ"  IndexIVFPQ (by_residual)
+    "IwSq"  IndexIVFScalarQuantizer (QT_8bit; index_factory "IVFn,SQ8"), also read in its older "IwSQ" form
     "IxRF"  IndexRefineFlat (IVF-PQ base + exact re-rank vectors; faiss IndexRefine with an IndexFlat refine index), or
             IndexRefine with an "IxSQ" IndexScalarQuantizer refine index of qtype QT_8bit (`Refine(SQ8)`)
 
@@ -26,6 +27,10 @@ faiss build.  Layout (little endian):
                    (write_ScalarQuantizer + the codes vector; only qtype QT_8bit = 0 is supported, whose trained vector
                    is [2, d] = vmin then vdiff and code_size = d; rangestat only steers training and is written as
                    RS_minmax = 0)
+  IwSq           : ivf header | ScalarQuantizer: qtype i32 | rangestat i32 | rangestat_arg f32 | d u64 | code_size u64
+                   | trained (u64 n | float32[n]) | code_size u64 | by_residual u8 | inverted lists (code_size = d)
+                   (index_write.cpp: write_ScalarQuantizer has no codes vector, unlike IxSQ; the codes live in the lists.
+                   index_read.cpp reads "IwSQ" the same way without the by_residual byte, and sets by_residual = true)
 """
 from __future__ import annotations
 
@@ -83,6 +88,18 @@ def _read_flat(f: BinaryIO, hdr: Dict) -> Dict:
     if n != hdr["ntotal"] * hdr["d"]:
         raise ValueError(f"flat index payload has {n} floats, expected {hdr['ntotal']} x {hdr['d']}")
     return {"kind": "Flat", **hdr, "xb": xb.reshape(hdr["ntotal"], hdr["d"])}
+
+
+def _read_scalar_quantizer(f: BinaryIO, d_expected: int) -> np.ndarray:
+    """read_ScalarQuantizer of a QT_8bit quantizer -> its trained range [2, d] (vmin, vdiff)."""
+    qtype, _rangestat, _rangestat_arg = _rd(f, "i"), _rd(f, "i"), _rd(f, "f")
+    d, code_size = _rd(f, "Q"), _rd(f, "Q")
+    trained = _rd_array(f, np.float32, _rd(f, "Q"))
+    if qtype != QT_8BIT:
+        raise NotImplementedError(f"ScalarQuantizer qtype {qtype}: only QT_8bit (0) is supported")
+    if d != d_expected or code_size != d or trained.size != 2 * d:
+        raise ValueError("ScalarQuantizer: d, code_size or trained disagree with the index header")
+    return trained.reshape(2, d)
 
 
 def _read_sq(f: BinaryIO, hdr: Dict) -> Dict:
@@ -175,6 +192,15 @@ def read_faiss(f) -> Dict:
         if cs != h["d"] * 4:
             raise ValueError("IVFFlat code_size mismatch")
         return {"kind": "IVFFlat", **h, "offsets": offsets, "vectors": codes.view(np.float32).reshape(-1, h["d"]), "ids": ids}
+    if tag in ("IwSq", "IwSQ"):
+        h = _read_ivf_header(f)
+        sq = _read_scalar_quantizer(f, h["d"])
+        code_size = _rd(f, "Q")
+        by_residual = bool(_rd(f, "B")) if tag == "IwSq" else True
+        cs, offsets, codes, ids = _read_invlists(f, h["nlist"])
+        if code_size != h["d"] or cs != code_size:
+            raise ValueError("IVF-SQ8: code_size disagrees with d")
+        return {"kind": "IVFSQ", **h, "by_residual": by_residual, "sq": sq, "offsets": offsets, "codes": codes, "ids": ids}
     if tag == "IwPQ":
         h = _read_ivf_header(f)
         by_residual = bool(_rd(f, "B"))
@@ -202,7 +228,7 @@ def read_faiss(f) -> Dict:
         if refine["kind"] == "SQ":          # SQ8 store: codes [ntotal, d] uint8 + sq [2, d] (vmin, vdiff), no "xb"
             return {"kind": "Refine", **hdr, "base": base, "sq": refine["sq"], "codes": refine["codes"], "k_factor": k_factor}
         return {"kind": "Refine", **hdr, "base": base, "xb": refine["xb"], "k_factor": k_factor}
-    raise NotImplementedError(f"faiss index type {tag!r} is not supported (Flat / IVFFlat / IVFPQ / RefineFlat only)")
+    raise NotImplementedError(f"faiss index type {tag!r} is not supported (Flat / IVFFlat / IVF-SQ8 / IVFPQ / RefineFlat only)")
 
 
 # ----------------------------------------------------------------------------------------------------------
@@ -245,6 +271,19 @@ def _write_sq(f: BinaryIO, sq: np.ndarray, codes: np.ndarray):
     f.write(codes.tobytes())
 
 
+def _write_scalar_quantizer(f: BinaryIO, sq: np.ndarray):
+    """write_ScalarQuantizer of a QT_8bit quantizer with the trained range sq [2, d]."""
+    sq = np.ascontiguousarray(sq, dtype=np.float32)
+    d = sq.shape[1]
+    _wr(f, "i", QT_8BIT)
+    _wr(f, "i", RS_MINMAX)
+    _wr(f, "f", 0.0)
+    _wr(f, "Q", d)
+    _wr(f, "Q", d)                            # code_size: one byte per element
+    _wr(f, "Q", sq.size)
+    f.write(sq.tobytes())
+
+
 def _write_invlists(f: BinaryIO, nlist: int, code_size: int, offsets: np.ndarray, codes: np.ndarray, ids: np.ndarray):
     _wr(f, "I", fourcc("ilar"))
     _wr(f, "Q", nlist)
@@ -279,7 +318,7 @@ def _write_ivf_header(f: BinaryIO, tag: str, d: int, ntotal: int, nlist: int, np
 
 
 def write_faiss(f, parts: Dict) -> None:
-    """Inverse of read_faiss: `parts` as returned by it (kind = Flat | IVFFlat | IVFPQ)."""
+    """Inverse of read_faiss: `parts` as returned by it (kind = Flat | IVFFlat | IVFSQ | IVFPQ | Refine)."""
     if isinstance(f, (str, bytes)):
         with open(f, "wb") as fh:
             return write_faiss(fh, parts)
@@ -291,6 +330,13 @@ def write_faiss(f, parts: Dict) -> None:
         _write_ivf_header(f, "IwFl", d, len(parts["ids"]), parts["centroids"].shape[0], parts.get("nprobe", 1), parts["centroids"])
         _write_invlists(f, parts["centroids"].shape[0], d * 4, parts["offsets"],
                         np.ascontiguousarray(parts["vectors"], dtype=np.float32), parts["ids"])
+    elif kind == "IVFSQ":
+        d = parts["centroids"].shape[1]
+        _write_ivf_header(f, "IwSq", d, len(parts["ids"]), parts["centroids"].shape[0], parts.get("nprobe", 1), parts["centroids"])
+        _write_scalar_quantizer(f, parts["sq"])
+        _wr(f, "Q", d)                        # code_size
+        _wr(f, "B", 1 if parts.get("by_residual", True) else 0)
+        _write_invlists(f, parts["centroids"].shape[0], d, parts["offsets"], parts["codes"], parts["ids"])
     elif kind == "IVFPQ":
         d = parts["centroids"].shape[1]
         M, ksub, dsub = parts["codebook"].shape
@@ -323,4 +369,4 @@ def is_faiss_file(path: str) -> bool:
             tag = f.read(4).decode("ascii", "replace")
     except OSError:
         return False
-    return tag in ("IxFI", "IxF2", "IxFl", "IwFl", "IwPQ", "IxRF")
+    return tag in ("IxFI", "IxF2", "IxFl", "IwFl", "IwPQ", "IwSq", "IwSQ", "IxRF")

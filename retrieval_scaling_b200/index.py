@@ -56,7 +56,8 @@ def _dev_rows(x, device) -> torch.Tensor:
 _STORE_DTYPES = {"float16": (torch.float16, _lib.RSB_DTYPE_F16), "float32": (torch.float32, _lib.RSB_DTYPE_F32)}
 
 
-# IndexRefine's store: the storage dtypes, plus "sq8" (uint8 codes of a trained scalar quantizer)
+# IndexRefine's store and IndexIVFScalarQuantizer's lists: the storage dtypes, plus "sq8" (uint8 codes of a trained
+# scalar quantizer)
 _REFINE_DTYPES = {**_STORE_DTYPES, "sq8": (torch.uint8, _lib.RSB_DTYPE_SQ8)}
 
 
@@ -211,7 +212,7 @@ class _IndexBase:
                 code_size = self._info(_lib.INFO_M) * self._info(_lib.INFO_NBITS) // 8
                 payload = torch.empty((n, code_size), dtype=torch.uint8, device=self.device)
             else:
-                payload = torch.empty((n, self.d), dtype=_STORE_DTYPES[self.dtype][0], device=self.device)
+                payload = torch.empty((n, self.d), dtype=_REFINE_DTYPES[self.dtype][0], device=self.device)
             ids = torch.empty(n, dtype=torch.int64, device=self.device)
             _lib.check(self.L.rsb_export_lists(self._h, _ptr(off), _ptr(payload), _ptr(ids), _stream()))
             torch.cuda.current_stream().synchronize()
@@ -382,6 +383,92 @@ class IndexIVFPQ(_IVFBase):
             lt = torch.as_tensor(lists).to(device=self.device, dtype=torch.int32).contiguous()
             idt = None if ids is None else torch.as_tensor(ids).to(device=self.device, dtype=torch.int64).contiguous()
             _lib.check(self.L.rsb_add_codes(self._h, _ptr(ct), n, _ptr(idt), _ptr(lt), _stream()))
+            torch.cuda.current_stream().synchronize()
+
+
+class IndexIVFScalarQuantizer(_IVFBase):
+    """faiss.IndexIVFScalarQuantizer(IndexFlatIP(d), d, nlist, QT_8bit, METRIC_INNER_PRODUCT, by_residual), the index
+    index_factory(d, "IVFn,SQ8") builds: inverted lists of one uint8 code per element (a quarter of the fp32 bytes), with
+    one (vmin, vdiff) range per dimension (RS_minmax).  d % 16 == 0.
+
+    by_residual=True (faiss' default) encodes x - c_list and scores a vector of list l as fl32(<q, c_l> + s); False
+    encodes x and scores s.  s = <q, decode(code)> is accumulated in the fp32 IVF-Flat scan's order from the decoded
+    elements vmin + ((c + 0.5f) / 255.f) * vdiff, so it is bit-identical to an fp32 IndexIVFFlat holding the decoded
+    rows in the same lists.  train(x) trains the coarse quantizer (as IndexIVFFlat.train) and then the range on the rows
+    or on their residuals against the lists add() would assign; train_sq(x) trains the range alone."""
+    kind = _lib.RSB_IVFFLAT
+    dtype = "sq8"
+    qtype = "QT_8bit"                   # the only scalar-quantizer type implemented
+    _TRAIN_CHUNK = 65536                # rows per coarse assignment while the residuals are formed
+
+    def __init__(self, d: int, nlist: int, by_residual: bool = True, device=None):
+        super().__init__(d, nlist, device)
+        with torch.cuda.device(self.device):
+            _lib.check(self.L.rsb_ivfflat_create(self.d, self.nlist, _lib.RSB_DTYPE_SQ8, ctypes.byref(self._h)))
+        self.set_option(_lib.OPT_BY_RESIDUAL, 1 if by_residual else 0)
+
+    @property
+    def by_residual(self) -> bool:
+        return bool(self._info(_lib.INFO_BY_RESIDUAL))
+
+    @property
+    def code_size(self) -> int:
+        return self.d
+
+    @property
+    def sq_params(self) -> Tuple[torch.Tensor, torch.Tensor]:
+        """The range (vmin [d], vdiff [d]) float32 device tensors."""
+        with torch.cuda.device(self.device):
+            out = torch.empty((2, self.d), dtype=torch.float32, device=self.device)
+            _lib.check(self.L.rsb_get_sq_range(self._h, _ptr(out), _stream()))
+            return out[0], out[1]
+
+    @sq_params.setter
+    def sq_params(self, sq) -> None:
+        """(vmin, vdiff) or a [2, d] array, used exactly as given (e.g. read from a file); only before anything is
+        added."""
+        with torch.cuda.device(self.device):
+            if isinstance(sq, (tuple, list)):
+                sq = torch.stack([_dev_f32(t, self.device).reshape(-1) for t in sq])
+            sq = _dev_f32(sq, self.device)
+            if tuple(sq.shape) != (2, self.d):
+                raise ValueError(f"the SQ8 range must be [2, {self.d}] (vmin, vdiff), got {tuple(sq.shape)}")
+            _lib.check(self.L.rsb_set_sq_range(self._h, _ptr(sq), _stream()))
+            torch.cuda.current_stream().synchronize()
+
+    def train(self, x) -> None:
+        with torch.cuda.device(self.device):
+            x = _dev_rows(x, self.device)
+            self._train_coarse(x.float())
+            self.train_sq(x)
+
+    def train_sq(self, x) -> None:
+        """Trains the range alone (per-dimension min / max, rsb_sq8_train) on the rows x [n, d] (fp16 or fp32) or, by
+        residual, on x - c_list with the lists of the coarse quantizer (nprobe = 1, the assignment add() makes)."""
+        with torch.cuda.device(self.device):
+            x = _dev_rows(x, self.device)
+            if x.dim() != 2 or x.shape[1] != self.d or x.shape[0] == 0:
+                raise ValueError(f"expected [n >= 1, {self.d}] training vectors, got {tuple(x.shape)}")
+            if self.by_residual:
+                c = self.get_centroids()
+                r = torch.empty(x.shape, dtype=torch.float32, device=self.device)
+                for a in range(0, x.shape[0], self._TRAIN_CHUNK):
+                    xc = x[a:a + self._TRAIN_CHUNK].float()             # fp16 rows widen exactly
+                    torch.sub(xc, c[self.assign(xc).long()], out=r[a:a + self._TRAIN_CHUNK])
+                x = r
+            sq = torch.empty((2, self.d), dtype=torch.float32, device=self.device)
+            _lib.check(self.L.rsb_sq8_train(_ptr(x), _dtype_code(x), x.shape[0], self.d, _ptr(sq), _stream()))
+            self.sq_params = sq
+
+    def add_codes(self, codes, lists, ids=None) -> None:
+        """Adds SQ8 codes [n, d] uint8 of this index's range (residual codes when by_residual) to the given lists."""
+        with torch.cuda.device(self.device):
+            ct = torch.as_tensor(codes).to(device=self.device, dtype=torch.uint8).contiguous()
+            if ct.dim() != 2 or ct.shape[1] != self.d:
+                raise ValueError(f"codes must be [n, {self.d}] uint8 (one byte per element), got {tuple(ct.shape)}")
+            lt = torch.as_tensor(lists).to(device=self.device, dtype=torch.int32).contiguous()
+            idt = None if ids is None else torch.as_tensor(ids).to(device=self.device, dtype=torch.int64).contiguous()
+            _lib.check(self.L.rsb_add_codes(self._h, _ptr(ct), ct.shape[0], _ptr(idt), _ptr(lt), _stream()))
             torch.cuda.current_stream().synchronize()
 
 
@@ -701,16 +788,31 @@ def _to_faiss_parts(index: _IndexBase) -> dict:
             raise ValueError("faiss IndexFlatIP has no id map: only sequential ids can be written in faiss format")
         return {"kind": "Flat", "xb": payload, "metric": 0}
     parts = {"centroids": index.get_centroids().cpu().numpy(), "offsets": off, "ids": ids, "nprobe": int(index.nprobe)}
+    if isinstance(index, IndexIVFScalarQuantizer):
+        return {"kind": "IVFSQ", "codes": payload, "sq": torch.stack(index.sq_params).cpu().numpy(),
+                "by_residual": index.by_residual, **parts}
     if index.kind == _lib.RSB_IVFFLAT:
         return {"kind": "IVFFlat", "vectors": payload, **parts}
     return {"kind": "IVFPQ", "codes": payload, "codebook": index.get_codebook().cpu().numpy(), **parts}
+
+
+def _check_sq8_storage(file_is_sq8: bool, storage_dtype: Optional[str]) -> None:
+    """storage_dtype "sq8" reads SQ8 files only, and an SQ8 file reads as sq8 only: turning float vectors into codes (or
+    back) would need a trained range, which reading does not do."""
+    if file_is_sq8 and storage_dtype not in (None, "sq8"):
+        raise ValueError(f"the index holds 8-bit scalar-quantizer codes (IVF-SQ8): its storage is sq8, not {storage_dtype}")
+    if not file_is_sq8 and storage_dtype == "sq8":
+        raise ValueError("storage_dtype sq8 reads IVF-SQ8 indexes only; this index holds float vectors (converting it "
+                         "would need a trained scalar quantizer: build an IndexIVFScalarQuantizer instead)")
 
 
 def _from_faiss_parts(p: dict, device=None, refine_dtype: Optional[str] = None,
                       storage_dtype: Optional[str] = None) -> _IndexBase:
     if p.get("metric", 0) != 0 or p.get("quantizer_metric", 0) != 0:
         raise NotImplementedError("only METRIC_INNER_PRODUCT indexes are supported (the reference builds IP indexes only)")
-    if storage_dtype is not None:
+    if p["kind"] == "IVFSQ" or storage_dtype == "sq8":
+        _check_sq8_storage(p["kind"] == "IVFSQ", storage_dtype)
+    elif storage_dtype is not None:
         _check_dtype(storage_dtype, "storage_dtype")
         if p["kind"] not in ("Flat", "IVFFlat"):
             raise ValueError(f"storage_dtype applies to Flat and IVFFlat indexes, not {p['kind']}")
@@ -752,7 +854,13 @@ def _from_faiss_parts(p: dict, device=None, refine_dtype: Optional[str] = None,
         return index
     nlist = p["nlist"]
     lists = np.repeat(np.arange(nlist, dtype=np.int32), np.diff(p["offsets"]))
-    if p["kind"] == "IVFFlat":
+    if p["kind"] == "IVFSQ":         # codes and range load as stored
+        index = IndexIVFScalarQuantizer(p["d"], nlist, by_residual=bool(p["by_residual"]), device=device)
+        index.set_centroids(p["centroids"])
+        index.sq_params = p["sq"]
+        if len(p["ids"]):
+            index.add_codes(p["codes"], lists, p["ids"])
+    elif p["kind"] == "IVFFlat":
         xb = _as_storage(p["vectors"], dtype, "the IVFFlat index's vectors") if len(p["ids"]) else None
         index = IndexIVFFlat(p["d"], nlist, device, dtype=dtype)
         index.set_centroids(p["centroids"])
@@ -794,6 +902,12 @@ def write_index(index: _IndexBase, path: str, fmt: Optional[str] = None) -> None
     blob = {"magic": MAGIC, "kind": int(index.kind), "d": index.d, "nprobe": int(index.nprobe)}
     if index.dtype != "float32":
         blob["dtype"] = index.dtype                      # the payload below is kept as stored
+    if isinstance(index, IndexIVFScalarQuantizer):
+        blob["by_residual"] = index.by_residual
+        try:
+            blob["sq"] = torch.stack(index.sq_params).cpu().numpy()
+        except _lib.RsbError:
+            pass
     if isinstance(index, _IVFBase):
         blob["nlist"] = index.nlist
         try:
@@ -823,7 +937,9 @@ def read_index(path: str, device=None, refine_dtype: Optional[str] = None,
     file (IxRF) `refine_dtype` picks the store: "float32" (default) or "float16", which is accepted only when every
     stored value round-trips through fp16 (ValueError otherwise).  An IxRF file whose refine index is an 8-bit scalar
     quantizer (IxSQ, QT_8bit) loads as an sq8 store (refine_dtype None or "sq8"; float16 / float32 raise ValueError).  `storage_dtype` does the same for the vectors of a
-    Flat / IVFFlat index (IxFI / IwFl / RSB1); None keeps the file's dtype (fp32 for faiss files)."""
+    Flat / IVFFlat index (IxFI / IwFl / RSB1); None keeps the file's dtype (fp32 for faiss files).  An IVF-SQ8 index
+    (IwSq / IwSQ, or RSB1 with dtype sq8) loads as an IndexIVFScalarQuantizer with its codes and range as stored
+    (storage_dtype None or "sq8"); "sq8" on a float index and float16 / float32 on an SQ8 index raise ValueError."""
     from . import faiss_io
     if faiss_io.is_faiss_file(path):
         return _from_faiss_parts(faiss_io.read_faiss(path), device, refine_dtype, storage_dtype)
@@ -832,7 +948,9 @@ def read_index(path: str, device=None, refine_dtype: Optional[str] = None,
     if not isinstance(blob, dict) or blob.get("magic") != MAGIC:
         raise ValueError(f"{path} is not an RSB1 index file")
     kind = blob["kind"]
-    if storage_dtype is not None:
+    if blob.get("dtype") == "sq8" or storage_dtype == "sq8":
+        _check_sq8_storage(blob.get("dtype") == "sq8", storage_dtype)
+    elif storage_dtype is not None:
         _check_dtype(storage_dtype, "storage_dtype")
         if kind not in (_lib.RSB_FLAT, _lib.RSB_IVFFLAT):
             raise ValueError("storage_dtype applies to Flat and IVFFlat indexes only")
@@ -841,6 +959,8 @@ def read_index(path: str, device=None, refine_dtype: Optional[str] = None,
         blob["payload"] = _as_storage(blob["payload"], dtype, f"{path}: the index vectors")
     if kind == _lib.RSB_FLAT:
         index = IndexFlatIP(blob["d"], device, dtype=dtype)
+    elif kind == _lib.RSB_IVFFLAT and dtype == "sq8":
+        index = IndexIVFScalarQuantizer(blob["d"], blob["nlist"], by_residual=bool(blob["by_residual"]), device=device)
     elif kind == _lib.RSB_IVFFLAT:
         index = IndexIVFFlat(blob["d"], blob["nlist"], device, dtype=dtype)
     elif kind == _lib.RSB_IVFPQ:
@@ -852,6 +972,8 @@ def read_index(path: str, device=None, refine_dtype: Optional[str] = None,
         index.set_centroids(blob["centroids"])
     if "codebook" in blob:
         index.set_codebook(blob["codebook"])
+    if "sq" in blob:
+        index.sq_params = blob["sq"]
     if "payload" in blob:
         ids = blob["ids"]
         if kind == _lib.RSB_FLAT:
@@ -859,7 +981,7 @@ def read_index(path: str, device=None, refine_dtype: Optional[str] = None,
         else:
             off = blob["offsets"]
             lists = np.repeat(np.arange(len(off) - 1, dtype=np.int32), np.diff(off))
-            if kind == _lib.RSB_IVFPQ:
+            if kind == _lib.RSB_IVFPQ or dtype == "sq8":
                 index.add_codes(blob["payload"], lists, ids)
             else:
                 index.add_preassigned(blob["payload"], lists, ids)

@@ -61,16 +61,21 @@ class Indexer(object):
 
     @staticmethod
     def storage_dtype(index_cfg):
-        """Optional key `storage_dtype` (float32 | float16; absent: None, today's fp32 path) -> the dtype Flat and IVFFlat
-        indexes store their vectors in.  IVFPQ stores codes, so the key is refused there."""
+        """Optional key `storage_dtype` (float32 | float16 | sq8; absent: None, today's fp32 path) -> the dtype Flat and
+        IVFFlat indexes store their vectors in.  sq8 (IVFFlat only) builds faiss' "IVFn,SQ8": an IndexIVFScalarQuantizer
+        with 8-bit codes of the residuals.  IVFPQ stores codes, so the key is refused there."""
         dtype = index_cfg.get("storage_dtype", None)
         if dtype is None:
             return None
-        if dtype not in ("float16", "float32"):
-            raise ValueError(f"datastore.index.storage_dtype must be float16 or float32, got {dtype!r}")
+        if dtype not in ("float16", "float32", "sq8"):
+            raise ValueError(f"datastore.index.storage_dtype must be float16 or float32 (IVFFlat also takes sq8), "
+                             f"got {dtype!r}")
         if index_cfg.index_type not in ("Flat", "IVFFlat"):
             raise ValueError(f"datastore.index.storage_dtype applies to Flat and IVFFlat indexes; {index_cfg.index_type} "
                              f"stores PQ codes")
+        if dtype == "sq8" and index_cfg.index_type != "IVFFlat":
+            raise ValueError(f"datastore.index.storage_dtype sq8 applies to IVFFlat indexes only (IVF-SQ8); "
+                             f"{index_cfg.index_type} takes float16 or float32")
         return dtype
 
     def __init__(self, cfg, index_shard_ids=None):

@@ -1,6 +1,6 @@
 """IVFFlatIndexer -- inverted file over raw fp32 vectors, inner product (reference
 `src/indicies/ivf_flat.py:35-227`: IndexIVFFlat(IndexFlatIP(d), d, ncentroids, METRIC_INNER_PRODUCT),
-`index.nprobe = probe`)."""
+`index.nprobe = probe`).  storage_dtype "sq8" builds faiss' IVFn,SQ8 (IndexIVFScalarQuantizer, by_residual) instead."""
 from __future__ import annotations
 
 from .. import index as rsb_index
@@ -22,4 +22,6 @@ class IVFFlatIndexer(BaseIndexer):
                          sample_train_size=sample_train_size, probe=probe, storage_dtype=storage_dtype)
 
     def _new_index(self):
+        if self.storage_dtype == "sq8":         # faiss index_factory(d, "IVFn,SQ8")
+            return rsb_index.IndexIVFScalarQuantizer(self.dimension, self.ncentroids, by_residual=True)
         return rsb_index.IndexIVFFlat(self.dimension, self.ncentroids, dtype=self.storage_dtype or "float32")

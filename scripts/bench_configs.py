@@ -3,6 +3,7 @@
   C1  Flat, 100k x 768 iid fp32, 1k queries, top-10
   C2  IVF-Flat nlist=4096 nprobe=64, 10M x 768 synthetic gmm, top-100  (30.7 GB of fp32 vectors on the GPU)
   c1_large  Flat 768-d past the 8 GB limit of the 3xTF32 split, fp16 storage (tensor cores) vs fp32 (CUDA cores)
+  c2_sq8    C2 as fp16 IVF-Flat and as IVF-SQ8 with / without residuals (run only when named)
 Every config measures fp16 storage and fp32 storage of the same (fp16-representable) values; the card name and power
 limit are part of each JSON object.  C1 alternates the arms in one loop; C2 and c1_large build one index at a time
 (the two do not fit on one 80 GB card together) and compare the results of a query sample afterwards.
@@ -205,6 +206,85 @@ def c2_both(**kw):
     return {"config": "C2 fp16 vs fp32 storage", "fp16": a, "fp32": b, "fp16_fp32_bit_identical": True}
 
 
+def c2_sq8(n=10_000_000, nlist=4096, nprobe=64, k=100, nq_parity=256):
+    """C2's corpus (10M x 768 gmm, nlist 4096, nprobe 64, top-100) as fp16 IVF-Flat and as IVF-SQ8 with and without
+    residuals (IndexIVFScalarQuantizer), one index at a time, all built from the same fp16 rows and centroids; the SQ8
+    range is trained on the centroid-training sample.  Per arm: index GB, QPS, scan ms, algorithmic scan GB/s (bytes the
+    scan must read: list length x row bytes, 1536 for fp16, 768 for SQ8), and the overlap of the top-100 with the fp16
+    arm's top-100 for the same 2048 queries (recall@100 against fp16 IVF-Flat).  SQ8 arms: tie-aware parity with the
+    IVF-SQ8 oracle (tests/ivfsq8_oracle.py) on nq_parity queries, every returned score re-scored in float64."""
+    import gc
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from ivfsq8_oracle import ivfsq8_search
+    from oracle import ann_oracle as O
+    from oracle.sq8_oracle import sq8_decode
+    d = 768
+    corpus = synth.Corpus(d=d, mode="gmm", n_centres=nlist // 4, device="cuda")
+    sample = corpus.train_sample(nlist * 64)
+    cent = train.kmeans(sample, nlist, niter=10, metric="ip", spherical=True)
+    xq_all = corpus.queries(10_000)[:2048].contiguous()
+    out = {"config": f"C2 IVF-Flat fp16 vs IVF-SQ8, nlist={nlist} nprobe={nprobe}, {n} x {d} gmm, top-{k}", **card()}
+    ref_I = None
+    for arm in ("fp16_ivfflat", "sq8_by_residual", "sq8_no_residual"):
+        t0 = time.time()
+        if arm == "fp16_ivfflat":
+            index = rsb.IndexIVFFlat(d, nlist, dtype="float16")
+            index.set_centroids(cent)
+        else:
+            index = rsb.IndexIVFScalarQuantizer(d, nlist, by_residual=arm == "sq8_by_residual")
+            index.set_centroids(cent)
+            index.train_sq(sample.half())
+        for c in range(n // 1_000_000):
+            x = corpus.chunk(c).half()
+            index.add(x, torch.arange(c * 1_000_000, (c + 1) * 1_000_000, device="cuda"))
+            del x
+        index.finalize()
+        index.nprobe = nprobe
+        index.set_profiling(True)
+        res = {"index_gb": index.index_bytes / 1e9, "build_s": time.time() - t0}
+        for nq in (1, 64, 2048):
+            xq = xq_all[:nq]
+            ms = timed(lambda: index.search_ids(xq, k), steps=5, warmup=2)
+            p = index.profile()
+            res[f"nq_{nq}"] = {"ms": ms, "queries_per_s": nq / ms * 1e3, "scan_ms": p["scan_ms"],
+                               "scan_algorithmic_gbs": p["scan_bytes"] / p["scan_ms"] / 1e6 if p["scan_ms"] > 0 else None}
+        I = index.search_ids(xq_all, k)[0].cpu().numpy()
+        if ref_I is None:
+            ref_I = I
+        res["recall_at_100_vs_fp16_ivfflat"] = O.recall_at_k(I, ref_I)
+        if arm != "fp16_ivfflat":
+            xq = xq_all[:nq_parity]
+            Ig, Dg = (t.cpu().numpy() for t in index.search_ids(xq, k))
+            lists, coarse = (t.cpu().numpy() for t in index.coarse(xq, nprobe))
+            off, codes, ids = (t.cpu().numpy() for t in index.export_lists())
+            sq = torch.stack(index.sq_params).cpu().numpy()
+            xq_np, cent_np = xq.cpu().numpy(), cent.cpu().numpy()
+            t0 = time.perf_counter()
+            Dr, Ir = ivfsq8_search(xq_np, cent_np, sq, off, codes, ids, nprobe, k, index.by_residual, lists=lists,
+                                   coarse_dis=coarse)
+            res["cpu_oracle_queries_per_s"] = nq_parity / (time.perf_counter() - t0)
+            row_of = np.empty(int(ids.max()) + 1, dtype=np.int64)
+            row_of[ids] = np.arange(ids.shape[0])
+            list_of = np.repeat(np.arange(nlist), np.diff(off))
+
+            def score_of(qi, id_):       # float64: <q, c_list> (by residual) + <q, decoded row>
+                r = row_of[np.atleast_1d(id_)]
+                x = sq8_decode(codes[r], sq).astype(np.float64)
+                if index.by_residual:
+                    x = x + cent_np[list_of[r]].astype(np.float64)
+                return (x @ xq_np[qi].astype(np.float64)).squeeze()
+            O.assert_topk_equivalent(Dg, Ig, Dr, Ir, score_of=score_of, rtol=1e-5, atol=1e-4)
+            s64 = np.stack([score_of(qi, Ig[qi]) for qi in range(nq_parity)])
+            res["parity"] = {"queries": nq_parity, "ids_equal_frac": float((Ig == Ir).mean()),
+                             "rescore_max_abs_err": float(np.abs(s64 - Dg).max())}
+            del codes
+        out[arm] = res
+        del index
+        gc.collect()
+        torch.cuda.empty_cache()
+    return out
+
+
 if __name__ == "__main__":
     which = sys.argv[1:] or ["c1", "c2", "c1_large"]
     if "c1" in which:
@@ -213,3 +293,5 @@ if __name__ == "__main__":
         print(json.dumps(c2_both()), flush=True)
     if "c1_large" in which:
         print(json.dumps(c1_large()), flush=True)
+    if "c2_sq8" in which:
+        print(json.dumps(c2_sq8()), flush=True)
