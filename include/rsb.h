@@ -132,7 +132,10 @@ enum {
     RSB_INFO_INDEX_BYTES = 8,  /* device bytes held by the searchable layout */
     RSB_INFO_DTYPE = 9,        /* storage dtype of the vectors: RSB_DTYPE_F32 / RSB_DTYPE_F16 / RSB_DTYPE_SQ8 (IVFPQ:
                                   RSB_DTYPE_F32) */
-    RSB_INFO_BY_RESIDUAL = 10  /* 1 if an SQ8 IVFFLAT index encodes residuals (RSB_OPT_BY_RESIDUAL), else 0 */
+    RSB_INFO_BY_RESIDUAL = 10, /* 1 if an SQ8 IVFFLAT index encodes residuals (RSB_OPT_BY_RESIDUAL), else 0 */
+    RSB_INFO_HOST_BYTES = 11,  /* page-locked host bytes held by a tiered Flat index's host tier (0 on other handles) */
+    RSB_INFO_DEVICE_ROWS = 12  /* rows held in device memory: min(device_rows, ntotal) on a tiered Flat index, else
+                                  ntotal */
 };
 int rsb_info(rsb_index_t* h, int what, int64_t* out);
 /* list sizes [nlist] int64 to a device buffer */
@@ -143,9 +146,16 @@ int rsb_list_sizes(rsb_index_t* h, int64_t* sizes_dev, rsb_stream_t stream);
  * (IVFFLAT with SQ8 storage), ids_dev [ntotal] int64.  Any pointer may be NULL. */
 int rsb_export_lists(rsb_index_t* h, int64_t* offsets_dev, void* payload_dev, int64_t* ids_dev,
                      rsb_stream_t stream);
+/* Rows [r0, r0 + n) of a FLAT index in its storage dtype ([n, d]), copied from whichever tier holds them to dst, which
+ * may be device memory or host memory (pageable or pinned).  Lets a caller export a tiered index larger than device
+ * memory one range at a time.  Pending adds are finalised first.  Other handles, or a range outside [0, ntotal):
+ * RSB_ERR_INVALID. */
+int rsb_export_rows(rsb_index_t* h, int64_t r0, int64_t n, void* dst, rsb_stream_t stream);
 
 /* ---- search (index.search(x, k) + index.nprobe: flat.py:139, ivf_flat.py:73,225, ivf_pq.py:76,230) --- */
-/* covers the fp16 Flat index's scaled query split (2 x [nq, d] fp16 + [nq] fp32 per query batch) */
+/* covers the fp16 Flat index's scaled query split (2 x [nq, d] fp16 + [nq] fp32 per query batch), and on a tiered Flat
+ * index two staging buffers of RSB_OPT_STAGING_BYTES each (fewer when the host tier is smaller), so a search allocates
+ * nothing */
 size_t rsb_workspace_bytes(rsb_index_t* h, int nq, int k, int nprobe);
 /* q_dev [nq, d] float32; D_dev [nq, k] float32; I_dev [nq, k] int64.  nprobe ignored for FLAT. */
 int rsb_search(rsb_index_t* h, const float* q_dev, int nq, int k, int nprobe,
@@ -296,9 +306,28 @@ enum {
     RSB_OPT_COARSE_TENSOR = 0,/* 1 (default): coarse quantizer scores by 3xTF32 on wgmma tensor cores (fp32-equivalent
                                  accuracy); 0: CUDA-core fp32 FMA tiles.  0 on an fp16 Flat index returns
                                  RSB_ERR_UNSUPPORTED: its rows are scored on tensor cores only */
-    RSB_OPT_BY_RESIDUAL = 1   /* SQ8 IVFFLAT only (RSB_ERR_INVALID on other handles), before anything is added
+    RSB_OPT_BY_RESIDUAL = 1,  /* SQ8 IVFFLAT only (RSB_ERR_INVALID on other handles), before anything is added
                                  (RSB_ERR_STATE after): 1 encodes x - c_list and adds the coarse score (faiss by_residual,
                                  the default of index_factory "IVFn,SQ8"); 0 (default) encodes x */
+    RSB_OPT_DEVICE_ROWS = 2,  /* tiered Flat index, for datastores larger than device memory.  FLAT with RSB_DTYPE_F16 only
+                                 (RSB_ERR_INVALID on other handles, fp32 Flat included), before anything is added
+                                 (RSB_ERR_STATE after), value >= 0.  Rows [0, value) are kept in device memory (allocated
+                                 once, at `value` rows, by the first add), rows from `value` on in page-locked host
+                                 blocks the handle owns, one of exactly the bytes needed per add; no row is ever held
+                                 twice.  rsb_add then also takes x in host memory (pageable or pinned): rows bound for
+                                 the host tier are copied host to host (fp32 rows rounded to nearest even there), rows
+                                 bound for the device tier cross PCIe once.
+                                 rsb_search keeps its signature and semantics.  Per query batch a copy stream owned by
+                                 the handle copies consecutive host chunks (RSB_OPT_STAGING_BYTES each) into two staging
+                                 buffers of the workspace on the copy engine, while the device tier and then each
+                                 resident chunk are scored: the fp16 candidate path of the all-device index over the
+                                 piece's rows, the exact fp32 re-score of its candidates, and a merge into the running
+                                 top-k (ties: the lower row).  Events order the reuse of the buffers and the copy stream
+                                 is joined back to `stream`; nothing synchronises the host.  Scores are bit-equal to the
+                                 all-device index wherever both return the same id.  While ntotal <= value the search is
+                                 the all-device one. */
+    RSB_OPT_STAGING_BYTES = 3 /* tiered Flat: bytes of one staging buffer (the search holds two), value >= d * 2 (one
+                                 row); default 256 MiB.  FLAT with RSB_DTYPE_F16 only, at any time */
 };
 int rsb_set_option(rsb_index_t* h, int option, int64_t value);
 

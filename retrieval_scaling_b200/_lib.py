@@ -15,8 +15,8 @@ RSB_ERR_INVALID, RSB_ERR_CUDA, RSB_ERR_STATE, RSB_ERR_UNSUPPORTED, RSB_ERR_OOM =
 RSB_FLAT, RSB_IVFFLAT, RSB_IVFPQ = 0, 1, 2
 RSB_DTYPE_F32, RSB_DTYPE_F16, RSB_DTYPE_SQ8 = 0, 1, 2
 (INFO_KIND, INFO_D, INFO_NLIST, INFO_M, INFO_NBITS, INFO_NTOTAL, INFO_IS_TRAINED, INFO_MAX_LIST_LEN,
- INFO_INDEX_BYTES, INFO_DTYPE, INFO_BY_RESIDUAL) = range(11)
-OPT_COARSE_TENSOR, OPT_BY_RESIDUAL = 0, 1
+ INFO_INDEX_BYTES, INFO_DTYPE, INFO_BY_RESIDUAL, INFO_HOST_BYTES, INFO_DEVICE_ROWS) = range(13)
+OPT_COARSE_TENSOR, OPT_BY_RESIDUAL, OPT_DEVICE_ROWS, OPT_STAGING_BYTES = 0, 1, 2, 3
 PROF_NAMES = ("coarse_ms", "setup_ms", "lut_ms", "scan_ms", "merge_ms", "scan_bytes", "pairs", "launches", "scan_path",
               "rescored")
 
@@ -41,6 +41,7 @@ SIGNATURES = [
     ("rsb_info", c_int, [_H, c_int, POINTER(c_int64)]),
     ("rsb_list_sizes", c_int, [_H, c_void_p, c_void_p]),
     ("rsb_export_lists", c_int, [_H, c_void_p, c_void_p, c_void_p, c_void_p]),
+    ("rsb_export_rows", c_int, [_H, c_int64, c_int64, c_void_p, c_void_p]),
     ("rsb_workspace_bytes", c_size_t, [_H, c_int, c_int, c_int]),
     ("rsb_search", c_int, [_H, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     ("rsb_search_preassigned", c_int, [_H, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,

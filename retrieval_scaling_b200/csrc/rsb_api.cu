@@ -56,6 +56,13 @@ struct Segment {
     int64_t n = 0;
 };
 
+// A page-locked host block of a tiered Flat index: rows [r0, r0 + n) of the index, exactly n * row_bytes bytes
+struct HostBlock {
+    void* p = nullptr;
+    int64_t r0 = 0, n = 0;
+};
+static const size_t kDefaultStagingBytes = (size_t)256 << 20;   // RSB_OPT_STAGING_BYTES default (per buffer)
+
 struct rsb_index {
     // IVFPQ: M sub-quantizers of nbits bits each (faiss' values: codebook, encoding, training, rsb_info) and
     // Mb = M * nbits / 8 code bytes per vector (layout, interleave, tables, scan, export).  nbits = 4 packs two codes
@@ -90,6 +97,19 @@ struct rsb_index {
     int64_t* list_slot_off = nullptr;  // [nlist + 1]
     int64_t* list_nat_off = nullptr;   // [nlist + 1]
     int max_list_len = 0;
+
+    // tiered Flat (RSB_OPT_DEVICE_ROWS, fp16 only): rows [0, dev_rows) live in `payload` (allocated once, at dev_rows
+    // rows, by the first add, and filled in place), rows [dev_rows, n_rows) in host_blocks (one per add, in row order).
+    // Only the ids go through the staging segments.  Search streams the host blocks through two staging buffers of the
+    // workspace on copy_st.
+    int64_t dev_rows = -1;                 // -1: not tiered
+    int64_t n_rows = 0;                    // rows held by the tiers (ntotal + n_staged)
+    std::vector<HostBlock> host_blocks;
+    size_t host_bytes = 0;
+    size_t staging_bytes = kDefaultStagingBytes;
+    cudaStream_t copy_st = nullptr;
+    cudaEvent_t stage_ready[2] = {}, stage_free[2] = {}, copy_start = nullptr, copy_done = nullptr;
+    bool tiered() const { return dev_rows >= 0; }
 
     // profiling
     bool prof = false;
@@ -172,6 +192,13 @@ extern "C" int rsb_free(rsb_index_t* h) {
     cudaFree(h->centroids); cudaFree(h->codebook); cudaFree(h->codebook_t); cudaFree(h->prof_dev); cudaFree(h->sq);
     cudaFree(h->cent_hi); cudaFree(h->cent_lo);
     for (auto& set : h->evs) for (auto& e : set) if (e) cudaEventDestroy(e);
+    if (h->copy_st) {   // a search in flight may still copy from the host blocks
+        cudaStreamSynchronize(h->copy_st);
+        cudaStreamDestroy(h->copy_st);
+    }
+    for (cudaEvent_t e : {h->stage_ready[0], h->stage_ready[1], h->stage_free[0], h->stage_free[1], h->copy_start, h->copy_done})
+        if (e) cudaEventDestroy(e);
+    for (auto& b : h->host_blocks) cudaFreeHost(b.p);
     delete h;
     return RSB_OK;
 }
@@ -399,6 +426,118 @@ static int stage_common(rsb_index* h, Segment& seg, const int64_t* ids, int64_t 
     return RSB_OK;
 }
 
+// fp32 -> fp16 on the host, rounded to nearest even like launch_f32_to_f16 (nan becomes a quiet nan): fp32 rows of a
+// tiered Flat index that land in its host tier are converted where they are
+static uint16_t f32_to_f16_host(float v) {
+    uint32_t f;
+    memcpy(&f, &v, 4);
+    const uint32_t sign = (f >> 16) & 0x8000u;
+    f &= 0x7fffffffu;
+    uint32_t o;
+    if (f >= 0x47800000u) {                      // |v| >= 65536, inf or nan
+        o = f > 0x7f800000u ? 0x7e00u : 0x7c00u;
+    } else if (f < 0x38800000u) {                // |v| < 2^-14: an fp16 subnormal or zero
+        float a, s;                              // adding 0.5f rounds (to nearest even) at the subnormal step 2^-24
+        memcpy(&a, &f, 4);
+        s = a + 0.5f;
+        uint32_t su;
+        memcpy(&su, &s, 4);
+        o = su - 0x3f000000u;
+    } else {                                     // rebias the exponent (-112 << 23), round to nearest even
+        o = (f + 0xc8000fffu + ((f >> 13) & 1u)) >> 13;
+    }
+    return (uint16_t)(sign | o);
+}
+
+// tiered Flat: rows [pos, pos + n) go to the device tier up to dev_rows and to one new page-locked host block after
+// it.  x is device or host memory (pageable or pinned); host rows bound for the host tier are copied (or converted)
+// host to host.  Only the ids are staged for rsb_finalize.
+static int add_tiered(rsb_index* h, const void* x, int x_dtype, int64_t n, const int64_t* ids, cudaStream_t st) {
+    cudaPointerAttributes attr;
+    if (cudaPointerGetAttributes(&attr, x) != cudaSuccess) {
+        cudaGetLastError();
+        attr.type = cudaMemoryTypeUnregistered;
+    }
+    const bool x_dev = attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged;
+    const bool f32 = x_dtype == RSB_DTYPE_F32;
+    const int d = h->d;
+    const size_t rb = h->row_bytes(), xrb = (size_t)d * (f32 ? 4 : 2);
+    const int64_t pos = h->n_rows;
+    const int64_t n_to_dev = std::max<int64_t>(0, std::min<int64_t>(n, h->dev_rows - pos));
+    const int64_t n_host = n - n_to_dev;
+    const uint8_t* xb = static_cast<const uint8_t*>(x);
+    if (n_to_dev && !h->payload) {   // the device tier, once, at its full size
+        CU(cudaMalloc(&h->payload, (size_t)h->dev_rows * rb));
+        h->payload_bytes = (size_t)h->dev_rows * rb;
+    }
+    HostBlock blk;
+    if (n_host) {
+        blk.r0 = pos + n_to_dev;
+        blk.n = n_host;
+        CU(cudaHostAlloc(&blk.p, (size_t)n_host * rb, cudaHostAllocPortable));
+    }
+    const int64_t conv_rows = std::max<int64_t>(1, ((int64_t)16 << 20) / (int64_t)rb);   // 16 MB conversion steps
+    std::vector<uint16_t> hbuf;
+    void* dbuf = nullptr;
+    auto run = [&]() -> int {
+        // device tier
+        uint8_t* dst = h->payload + (size_t)pos * rb;
+        if (n_to_dev && !f32) CU(cudaMemcpyAsync(dst, xb, (size_t)n_to_dev * rb, cudaMemcpyDefault, st));
+        else if (n_to_dev && x_dev) launch_f32_to_f16(static_cast<const float*>(x), (size_t)n_to_dev * d, dst, st);
+        else if (n_to_dev) {
+            hbuf.resize((size_t)std::min(n_to_dev, conv_rows) * d);
+            for (int64_t r = 0; r < n_to_dev; r += conv_rows) {
+                const int64_t m = std::min(conv_rows, n_to_dev - r);
+                const float* src = reinterpret_cast<const float*>(xb + (size_t)r * xrb);
+                for (size_t i = 0; i < (size_t)m * d; ++i) hbuf[i] = f32_to_f16_host(src[i]);
+                // from pageable memory: returns once hbuf has been consumed
+                CU(cudaMemcpyAsync(dst + (size_t)r * rb, hbuf.data(), (size_t)m * rb, cudaMemcpyHostToDevice, st));
+            }
+        }
+        if (!n_host) return RSB_OK;
+        // host tier
+        const uint8_t* src0 = xb + (size_t)n_to_dev * xrb;
+        uint8_t* hdst = static_cast<uint8_t*>(blk.p);
+        if (!f32 && x_dev) CU(cudaMemcpyAsync(hdst, src0, (size_t)n_host * rb, cudaMemcpyDeviceToHost, st));
+        else if (!f32) memcpy(hdst, src0, (size_t)n_host * rb);
+        else if (!x_dev) {
+            const float* src = reinterpret_cast<const float*>(src0);
+            uint16_t* out = static_cast<uint16_t*>(blk.p);
+            for (size_t i = 0; i < (size_t)n_host * d; ++i) out[i] = f32_to_f16_host(src[i]);
+        } else {   // fp32 rows on the device: converted there, 16 MB of fp16 at a time
+            const int64_t step = std::min(conv_rows, n_host);
+            CU(cudaMalloc(&dbuf, (size_t)step * rb));
+            for (int64_t r = 0; r < n_host; r += step) {
+                const int64_t m = std::min(step, n_host - r);
+                launch_f32_to_f16(reinterpret_cast<const float*>(src0 + (size_t)r * xrb), (size_t)m * d, dbuf, st);
+                CU(cudaMemcpyAsync(hdst + (size_t)r * rb, dbuf, (size_t)m * rb, cudaMemcpyDeviceToHost, st));
+            }
+            CU(cudaStreamSynchronize(st));
+        }
+        return RSB_OK;
+    };
+    int rc = run();
+    cudaFree(dbuf);
+    Segment seg;
+    if (rc == RSB_OK) rc = stage_common(h, seg, ids, n, st);
+    if (rc == RSB_OK && cudaPeekAtLastError() != cudaSuccess)
+        rc = fail(RSB_ERR_CUDA, "tiered add: %s", cudaGetErrorString(cudaGetLastError()));
+    if (rc != RSB_OK) {
+        cudaStreamSynchronize(st);
+        free_segment(seg);
+        cudaFreeHost(blk.p);
+        return rc;
+    }
+    if (n_host) {
+        h->host_blocks.push_back(blk);
+        h->host_bytes += (size_t)n_host * rb;
+    }
+    h->staging.push_back(seg);
+    h->n_staged += n;
+    h->n_rows += n;
+    return RSB_OK;
+}
+
 // x: [n, d] in x_dtype (RSB_DTYPE_F32 / RSB_DTYPE_F16); stored in the handle's dtype (fp32 -> fp16 rounds to nearest
 // even, fp16 -> fp32 is exact).  IVF list assignment runs on fp32 values (fp16 input is upcast 16384 rows at a time).
 static int add_impl(rsb_index* h, const void* x, int x_dtype, const uint8_t* codes_in, int64_t n, const int64_t* ids,
@@ -417,6 +556,7 @@ static int add_impl(rsb_index* h, const void* x, int x_dtype, const uint8_t* cod
     // slots are 32-bit in the candidate keys (2^32) and rsb_finalize sorts (list, row) pairs with a 32-bit item count
     if (h->ntotal + h->n_staged + n >= ((int64_t)1 << 31) - 64 * (int64_t)h->nlist)
         return fail(RSB_ERR_UNSUPPORTED, "more than 2^31 vectors per index shard (shard the datastore across GPUs)");
+    if (h->tiered()) return add_tiered(h, x, x_dtype, n, ids, st);
     Segment seg;
     int rc = stage_common(h, seg, ids, n, st);
     if (rc != RSB_OK) { free_segment(seg); return rc; }
@@ -531,10 +671,36 @@ static int layout_to_segment(rsb_index* h, cudaStream_t st) {
     return RSB_OK;
 }
 
+// tiered Flat: the rows are already in place; only the staged ids are appended to the id array
+static int finalize_tiered(rsb_index* h, cudaStream_t st) {
+    const int64_t n = h->ntotal + h->n_staged;
+    int64_t* ids = nullptr;
+    CU(cudaMalloc(&ids, (size_t)n * 8));
+    cudaError_t e = h->ntotal ? cudaMemcpyAsync(ids, h->ids_slots, (size_t)h->ntotal * 8, cudaMemcpyDeviceToDevice, st)
+                              : cudaSuccess;
+    int64_t o = h->ntotal;
+    for (const Segment& s : h->staging) {
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ids + o, s.ids, (size_t)s.n * 8, cudaMemcpyDeviceToDevice, st);
+        o += s.n;
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) {
+        cudaFree(ids);
+        return fail(RSB_ERR_CUDA, "tiered finalize: %s", cudaGetErrorString(e));
+    }
+    for (auto& s : h->staging) free_segment(s);
+    h->staging.clear(); h->n_staged = 0;
+    cudaFree(h->ids_slots);
+    h->ids_slots = ids;
+    h->ntotal = n; h->nslots = n; h->max_list_len = (int)std::min<int64_t>(n, 0x7fffffff);
+    return RSB_OK;
+}
+
 extern "C" int rsb_finalize(rsb_index_t* h, rsb_stream_t stream) {
     if (!h) return fail(RSB_ERR_INVALID, "null handle");
     cudaStream_t st = (cudaStream_t)stream;
     if (h->staging.empty()) return RSB_OK;
+    if (h->tiered()) return finalize_tiered(h, st);
     if (h->ntotal > 0) RSB_TRY(layout_to_segment(h, st));
     else free_layout(h);
     const int64_t n = h->n_staged;
@@ -697,6 +863,10 @@ extern "C" int rsb_info(rsb_index_t* h, int what, int64_t* out) {
         case RSB_INFO_INDEX_BYTES: *out = (int64_t)(h->payload_bytes + (size_t)h->nslots * 8); break;
         case RSB_INFO_DTYPE: *out = h->dtype; break;
         case RSB_INFO_BY_RESIDUAL: *out = h->by_residual ? 1 : 0; break;
+        case RSB_INFO_HOST_BYTES: *out = (int64_t)h->host_bytes; break;
+        case RSB_INFO_DEVICE_ROWS:
+            *out = h->tiered() ? std::min(h->dev_rows, h->ntotal + h->n_staged) : h->ntotal + h->n_staged;
+            break;
         default: return fail(RSB_ERR_INVALID, "unknown info key %d", what);
     }
     return RSB_OK;
@@ -717,6 +887,22 @@ extern "C" int rsb_list_sizes(rsb_index_t* h, int64_t* sizes, rsb_stream_t strea
     return RSB_OK;
 }
 
+// rows [r0, r0 + n) of a finalised Flat index, from whichever tier holds them, to dst (device or host memory)
+static int flat_copy_rows(rsb_index* h, int64_t r0, int64_t n, void* dst, cudaStream_t st) {
+    const size_t rb = h->row_bytes();
+    uint8_t* out = static_cast<uint8_t*>(dst);
+    const int64_t n_dev = h->tiered() ? std::min(h->dev_rows, h->ntotal) : h->ntotal;
+    if (r0 < n_dev && n > 0)
+        CU(cudaMemcpyAsync(out, h->payload + (size_t)r0 * rb, (size_t)std::min(n, n_dev - r0) * rb, cudaMemcpyDefault, st));
+    for (const HostBlock& b : h->host_blocks) {
+        const int64_t a = std::max(r0, b.r0), e = std::min(r0 + n, b.r0 + b.n);
+        if (a < e)
+            CU(cudaMemcpyAsync(out + (size_t)(a - r0) * rb, static_cast<const uint8_t*>(b.p) + (size_t)(a - b.r0) * rb,
+                               (size_t)(e - a) * rb, cudaMemcpyDefault, st));
+    }
+    return RSB_OK;
+}
+
 static int export_impl(rsb_index* h, int64_t* offsets, void* payload, int64_t* ids, cudaStream_t st) {
     if (h->kind == RSB_FLAT) {
         if (offsets) {
@@ -724,7 +910,8 @@ static int export_impl(rsb_index* h, int64_t* offsets, void* payload, int64_t* i
             CU(cudaMemcpyAsync(offsets, o, 16, cudaMemcpyHostToDevice, st));
             CU(cudaStreamSynchronize(st));
         }
-        if (payload && h->ntotal) CU(cudaMemcpyAsync(payload, h->payload, (size_t)h->ntotal * h->row_bytes(), cudaMemcpyDeviceToDevice, st));
+        if (payload && h->ntotal && h->tiered()) RSB_TRY(flat_copy_rows(h, 0, h->ntotal, payload, st));
+        else if (payload && h->ntotal) CU(cudaMemcpyAsync(payload, h->payload, (size_t)h->ntotal * h->row_bytes(), cudaMemcpyDeviceToDevice, st));
         if (ids && h->ntotal) CU(cudaMemcpyAsync(ids, h->ids_slots, (size_t)h->ntotal * 8, cudaMemcpyDeviceToDevice, st));
         return RSB_OK;
     }
@@ -752,6 +939,18 @@ extern "C" int rsb_export_lists(rsb_index_t* h, int64_t* offsets, void* payload,
     if (!h) return fail(RSB_ERR_INVALID, "null handle");
     if (!h->staging.empty()) RSB_TRY(rsb_finalize(h, stream));
     return export_impl(h, offsets, payload, ids, (cudaStream_t)stream);
+}
+
+extern "C" int rsb_export_rows(rsb_index_t* h, int64_t r0, int64_t n, void* dst, rsb_stream_t stream) {
+    if (!h) return fail(RSB_ERR_INVALID, "null handle");
+    if (h->kind != RSB_FLAT) return fail(RSB_ERR_INVALID, "rsb_export_rows reads the rows of a Flat index");
+    if (!h->staging.empty()) RSB_TRY(rsb_finalize(h, stream));
+    if (r0 < 0 || n < 0 || r0 + n > h->ntotal)
+        return fail(RSB_ERR_INVALID, "rows [%lld, %lld) are outside [0, %lld)", (long long)r0, (long long)(r0 + n),
+                    (long long)h->ntotal);
+    if (n == 0) return RSB_OK;
+    if (!dst) return fail(RSB_ERR_INVALID, "dst is NULL");
+    return flat_copy_rows(h, r0, n, dst, (cudaStream_t)stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -828,9 +1027,135 @@ static FlatPlan flat_plan(const rsb_index* h, int nq, int k) {
     return p;
 }
 
+// Tiered Flat search (rows past dev_rows in host memory).  The rows are scored in pieces: the device tier in place,
+// then the host tier in chunks of chunk_rows, copied by copy_st into two staging buffers while the previous piece is
+// scored.  Each piece runs the fp16 candidate path (kc = min(k + 8, 4096, rows) candidates) and the exact fp32
+// re-score of its own rows, and is merged into the running top-k (ties: the earlier piece, i.e. the lower row).
+struct TieredFlatPlan {
+    int qb, kc;
+    int64_t n_dev, chunk_rows, nchunks;
+    size_t knn_bytes, off_qsplit, off_D2, off_I2, off_mD, off_mI, off_stage[2], total;
+};
+static bool flat_is_streamed(const rsb_index* h) { return h->tiered() && h->n_rows > h->dev_rows; }
+static TieredFlatPlan tiered_flat_plan(const rsb_index* h, int nq, int k) {
+    TieredFlatPlan p;
+    const size_t rb = h->row_bytes();
+    p.n_dev = std::min(h->dev_rows, h->n_rows);
+    const int64_t n_host = h->n_rows - p.n_dev;
+    p.chunk_rows = std::max<int64_t>(1, std::min<int64_t>((int64_t)(h->staging_bytes / rb), n_host));
+    p.nchunks = (n_host + p.chunk_rows - 1) / p.chunk_rows;
+    p.kc = std::min(k + 8, 4096);
+    const int64_t rows = std::max<int64_t>({p.n_dev, p.chunk_rows, 1});
+    const KnnPlan kp = knn_plan(nq, rows, p.kc);
+    p.qb = kp.qb;
+    p.knn_bytes = kp.total;
+    if (nq % p.qb) p.knn_bytes = std::max(p.knn_bytes, knn_plan(nq % p.qb, rows, p.kc).total);   // the last batch
+    size_t o = align_up(p.knn_bytes);
+    p.off_qsplit = o; o += align_up((size_t)2 * p.qb * h->d * 4);
+    p.off_D2 = o;     o += align_up((size_t)p.qb * p.kc * 4);
+    p.off_I2 = o;     o += align_up((size_t)p.qb * p.kc * 8);
+    p.off_mD = o;     o += align_up((size_t)2 * p.qb * k * 4);   // merge input [2, nb, k]: running top-k, new piece
+    p.off_mI = o;     o += align_up((size_t)2 * p.qb * k * 8);
+    for (int b = 0; b < 2; ++b) {
+        p.off_stage[b] = o;
+        o += align_up((size_t)p.chunk_rows * rb);
+    }
+    p.total = o;
+    return p;
+}
+
+static int search_flat_tiered(rsb_index* h, const float* q, int nq, int k, float* D, int64_t* I, void* ws,
+                              size_t ws_bytes, cudaStream_t st) {
+    const TieredFlatPlan p = tiered_flat_plan(h, nq, k);
+    if (ws_bytes < p.total) return fail(RSB_ERR_OOM, "workspace too small: need %zu bytes, got %zu", p.total, ws_bytes);
+    const size_t rb = h->row_bytes();
+    unsigned char* w = static_cast<unsigned char*>(ws);
+    TensorOperands tc;   // [qb, d] fp16 hi, [qb, d] fp16 lo, [qb] fp32 inverse scales
+    tc.xh = tc.xl = nullptr;
+    tc.f16 = true;
+    tc.qh = reinterpret_cast<float*>(w + p.off_qsplit);
+    tc.ql = reinterpret_cast<float*>(reinterpret_cast<uint16_t*>(tc.qh) + (size_t)p.qb * h->d);
+    tc.qinv = reinterpret_cast<float*>(reinterpret_cast<uint16_t*>(tc.qh) + (size_t)2 * p.qb * h->d);
+    float* D2 = reinterpret_cast<float*>(w + p.off_D2);
+    int64_t* I2 = reinterpret_cast<int64_t*>(w + p.off_I2);
+    float* mD = reinterpret_cast<float*>(w + p.off_mD);
+    int64_t* mI = reinterpret_cast<int64_t*>(w + p.off_mI);
+    uint8_t* stage[2] = {w + p.off_stage[0], w + p.off_stage[1]};
+
+    // rows X [rows, d] = index rows [r0, r0 + rows) -> exact top-k of nb queries
+    auto score_piece = [&](const float* qb, int nb, const void* X, int64_t rows, int64_t r0, float* Do, int64_t* Io) -> int {
+        const int kc = (int)std::min<int64_t>(rows, p.kc);
+        RSB_TRY(knn_ip_device(h, qb, nb, X, rows, h->d, kc, nullptr, 0, D2, I2, w, p.knn_bytes, st, &tc));
+        if (launch_refine_exact(qb, nb, X, 2, h->d, I2, kc, k, Do, Io, h->ids_slots + r0, st) != 0)
+            return fail(RSB_ERR_UNSUPPORTED, "k = %d is too large for the re-score kernel", k);
+        h->launches += 1;
+        return RSB_OK;
+    };
+    // H2D copy of host chunk c into staging buffer c % 2 on the copy engine (copy_st), from the blocks it overlaps
+    auto copy_chunk = [&](int64_t c) -> int {
+        const int64_t r0 = p.n_dev + c * p.chunk_rows, r1 = std::min(h->ntotal, r0 + p.chunk_rows);
+        auto b = std::partition_point(h->host_blocks.begin(), h->host_blocks.end(),
+                                      [&](const HostBlock& blk) { return blk.r0 + blk.n <= r0; });
+        for (; b != h->host_blocks.end() && b->r0 < r1; ++b) {
+            const int64_t a = std::max(r0, b->r0), e = std::min(r1, b->r0 + b->n);
+            CU(cudaMemcpyAsync(stage[c & 1] + (size_t)(a - r0) * rb, static_cast<const uint8_t*>(b->p) + (size_t)(a - b->r0) * rb,
+                               (size_t)(e - a) * rb, cudaMemcpyHostToDevice, h->copy_st));
+        }
+        CU(cudaEventRecord(h->stage_ready[c & 1], h->copy_st));
+        return RSB_OK;
+    };
+
+    const int64_t pieces = (p.n_dev > 0 ? 1 : 0) + p.nchunks;
+    for (int q0 = 0; q0 < nq; q0 += p.qb) {
+        const int nb = std::min(p.qb, nq - q0);
+        const float* qb = q + (size_t)q0 * h->d;
+        float* Dq = D + (size_t)q0 * k;
+        int64_t* Iq = I + (size_t)q0 * k;
+        int64_t done = 0;
+        // piece `done` writes the final result (a single piece), the running slot (first piece) or the new-piece slot
+        auto outD = [&]() { return pieces == 1 ? Dq : mD + (done ? (size_t)nb * k : 0); };
+        auto outI = [&]() { return pieces == 1 ? Iq : mI + (done ? (size_t)nb * k : 0); };
+        auto merge = [&]() -> int {
+            if (done++ == 0) return RSB_OK;
+            if (launch_merge_shards(mD, mI, 2, nb, k, k, Dq, Iq, st) != 0)
+                return fail(RSB_ERR_UNSUPPORTED, "k = %d is too large for the merge kernel", k);
+            h->launches += 1;
+            if (done < pieces) {   // the merged top-k is the running slot of the next merge
+                CU(cudaMemcpyAsync(mD, Dq, (size_t)nb * k * 4, cudaMemcpyDeviceToDevice, st));
+                CU(cudaMemcpyAsync(mI, Iq, (size_t)nb * k * 8, cudaMemcpyDeviceToDevice, st));
+            }
+            return RSB_OK;
+        };
+        // copies start after everything the caller enqueued before (adds, the previous batch's use of the buffers)
+        CU(cudaEventRecord(h->copy_start, st));
+        CU(cudaStreamWaitEvent(h->copy_st, h->copy_start, 0));
+        for (int64_t c = 0; c < std::min<int64_t>(2, p.nchunks); ++c) RSB_TRY(copy_chunk(c));
+        if (p.n_dev > 0) {   // the device tier, in place, while the first chunks cross PCIe
+            RSB_TRY(score_piece(qb, nb, h->payload, p.n_dev, 0, outD(), outI()));
+            RSB_TRY(merge());
+        }
+        for (int64_t c = 0; c < p.nchunks; ++c) {
+            const int64_t r0 = p.n_dev + c * p.chunk_rows;
+            CU(cudaStreamWaitEvent(st, h->stage_ready[c & 1], 0));
+            RSB_TRY(score_piece(qb, nb, stage[c & 1], std::min(p.chunk_rows, h->ntotal - r0), r0, outD(), outI()));
+            CU(cudaEventRecord(h->stage_free[c & 1], st));
+            if (c + 2 < p.nchunks) {
+                CU(cudaStreamWaitEvent(h->copy_st, h->stage_free[c & 1], 0));
+                RSB_TRY(copy_chunk(c + 2));
+            }
+            RSB_TRY(merge());
+        }
+    }
+    CU(cudaEventRecord(h->copy_done, h->copy_st));   // join the copy stream back to the caller's
+    CU(cudaStreamWaitEvent(st, h->copy_done, 0));
+    CHECK_LAUNCH();
+    return RSB_OK;
+}
+
 extern "C" size_t rsb_workspace_bytes(rsb_index_t* h, int nq, int k, int nprobe) {
     if (!h) return 0;
     nq = std::max(nq, 1); k = std::max(k, 1);
+    if (h->kind == RSB_FLAT && flat_is_streamed(h)) return tiered_flat_plan(h, nq, k).total;
     if (h->kind == RSB_FLAT) {
         // pending adds are finalised by the search itself, which may switch the tensor path on: size for both
         const size_t plain = knn_plan(nq, std::max<int64_t>(h->ntotal + h->n_staged, 1), k).total;
@@ -939,7 +1264,9 @@ static int search_impl(rsb_index_t* h, const float* q, int nq, int k, int nprobe
     if (h->kind == RSB_FLAT) {
         if (h->prof) CU(cudaEventRecord(h->ev[0], st));
         const FlatPlan fp = flat_plan(h, nq, k);
-        if (fp.tensor && h->ntotal > 0) {
+        if (flat_is_streamed(h)) {
+            RSB_TRY(search_flat_tiered(h, q, nq, k, D, I, ws, ws_bytes, st));
+        } else if (fp.tensor && h->ntotal > 0) {
             // tensor-core candidates (k + 8 per query; 3xTF32 on wgmma, or the scaled fp16 query split against fp16
             // rows), then exact fp32 re-score -> top-k
             if (ws_bytes < fp.total) return fail(RSB_ERR_OOM, "workspace too small: need %zu bytes, got %zu", fp.total, ws_bytes);
@@ -1412,6 +1739,30 @@ extern "C" int rsb_set_option(rsb_index_t* h, int option, int64_t value) {
             if (!is_sq8_ivf(h)) return fail(RSB_ERR_INVALID, "RSB_OPT_BY_RESIDUAL applies to an IVFFLAT index with SQ8 storage only");
             if (h->ntotal || h->n_staged) return fail(RSB_ERR_STATE, "by_residual cannot change once vectors are added");
             h->by_residual = value != 0; return RSB_OK;
+        case RSB_OPT_DEVICE_ROWS:
+            if (h->kind != RSB_FLAT)
+                return fail(RSB_ERR_INVALID, "RSB_OPT_DEVICE_ROWS applies to a Flat index with fp16 storage (RSB_DTYPE_F16) only");
+            if (h->dtype != RSB_DTYPE_F16)
+                return fail(RSB_ERR_INVALID, "a tiered Flat index stores fp16 rows: create it with RSB_DTYPE_F16 (an fp32 Flat "
+                                             "index stays in device memory)");
+            if (h->ntotal || h->n_staged) return fail(RSB_ERR_STATE, "device_rows cannot change once vectors are added");
+            if (value < 0) return fail(RSB_ERR_INVALID, "device_rows must be >= 0, got %lld", (long long)value);
+            if (!h->copy_st) {   // on the device current now, which holds the index
+                CU(cudaStreamCreateWithFlags(&h->copy_st, cudaStreamNonBlocking));
+                for (cudaEvent_t* e : {&h->stage_ready[0], &h->stage_ready[1], &h->stage_free[0], &h->stage_free[1],
+                                       &h->copy_start, &h->copy_done})
+                    CU(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+            }
+            h->dev_rows = value;
+            return RSB_OK;
+        case RSB_OPT_STAGING_BYTES:
+            if (h->kind != RSB_FLAT || h->dtype != RSB_DTYPE_F16)
+                return fail(RSB_ERR_INVALID, "RSB_OPT_STAGING_BYTES applies to a Flat index with fp16 storage (RSB_DTYPE_F16) only");
+            if (value < (int64_t)h->row_bytes())
+                return fail(RSB_ERR_INVALID, "a staging buffer must hold one row (%zu bytes), got %lld", h->row_bytes(),
+                            (long long)value);
+            h->staging_bytes = (size_t)value;
+            return RSB_OK;
         default: return fail(RSB_ERR_INVALID, "unknown option %d", option);
     }
 }

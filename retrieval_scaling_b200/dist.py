@@ -170,7 +170,10 @@ class ShardedSearcher:
                  search_fn: Optional[Callable] = None, merge_fn: Optional[Callable] = None,
                  shard_coarse: bool = True, fused_gather: bool = True, sliced_merge: bool = True,
                  share_tau: bool = True, peer_coarse: bool = True):
-        from .index import IndexIVFScalarQuantizer, IndexRefine
+        from .index import IndexFlatIP, IndexIVFScalarQuantizer, IndexRefine
+        if isinstance(index, IndexFlatIP) and index.tiered:
+            raise NotImplementedError("ShardedSearcher does not search a tiered Flat index (rows in host memory): search "
+                                      "it per shard group (search.GroupSearcher) or with index.search on one GPU")
         if isinstance(index, IndexIVFScalarQuantizer) and int(world) > 1:
             raise NotImplementedError("ShardedSearcher over several GPUs is implemented for IVF-Flat and nbits = 8 IVF-PQ "
                                       "indexes, not IVF-SQ8.  Search it per shard group (search.GroupSearcher) or on one GPU")

@@ -255,6 +255,38 @@ def _write_flat(f: BinaryIO, xb: np.ndarray, metric: int = METRIC_INNER_PRODUCT)
     f.write(xb.tobytes())
 
 
+def write_flat_rows(f: BinaryIO, d: int, ntotal: int, row_chunks) -> None:
+    """IxFI from consecutive row chunks (arrays [m, d], written as float32): the bytes _write_flat writes for their
+    concatenation, without holding it, so an index larger than host memory is written one chunk at a time."""
+    _write_header(f, "IxFI", d, ntotal, True, METRIC_INNER_PRODUCT)
+    _wr(f, "Q", ntotal * d)
+    rows = 0
+    for c in row_chunks:
+        c = np.ascontiguousarray(c, dtype=np.float32)
+        f.write(c.tobytes())
+        rows += c.shape[0]
+    if rows != ntotal:
+        raise ValueError(f"wrote {rows} rows of a {ntotal}-row flat index")
+
+
+def flat_rows_memmap(path: str):
+    """(d, ntotal, rows) of an IxFI file, rows = a read-only float32 np.memmap [ntotal, d] over its payload: a flat
+    index can be loaded chunk by chunk without reading the file into memory."""
+    with open(path, "rb") as f:
+        tag = _fourcc_str(_rd(f, "I"))
+        if tag != "IxFI":
+            raise ValueError(f"{path} is not a faiss IndexFlatIP file (IxFI), it is {tag!r}")
+        hdr = _read_header(f)
+        n = _rd(f, "Q")
+        if n != hdr["ntotal"] * hdr["d"]:
+            raise ValueError(f"flat index payload has {n} floats, expected {hdr['ntotal']} x {hdr['d']}")
+        offset = f.tell()
+    if hdr["ntotal"] == 0:
+        return hdr["d"], 0, np.zeros((0, hdr["d"]), np.float32)
+    return hdr["d"], hdr["ntotal"], np.memmap(path, dtype=np.float32, mode="r", offset=offset,
+                                              shape=(hdr["ntotal"], hdr["d"]))
+
+
 def _write_sq(f: BinaryIO, sq: np.ndarray, codes: np.ndarray):
     sq = np.ascontiguousarray(sq, dtype=np.float32)
     codes = np.ascontiguousarray(codes, dtype=np.uint8)

@@ -224,14 +224,88 @@ class IndexFlatIP(_IndexBase):
 
     dtype="float16" stores the vectors as fp16 (faiss IndexScalarQuantizer(QT_fp16, METRIC_INNER_PRODUCT)): half the
     bytes, scored on tensor cores from the fp16 rows at any size that fits (d % 64 == 0, else NotImplementedError),
-    with exact fp32 final scores.  Lossless for the fp16 embeddings the embedding task writes."""
+    with exact fp32 final scores.  Lossless for the fp16 embeddings the embedding task writes.
+
+    device_rows = n (an integer; float16 only) makes the index tiered, for datastores larger than device memory: rows
+    [0, n) stay in device memory and rows from n on go to page-locked host memory the index owns.  Each search streams
+    the host rows through two device staging buffers of `staging_bytes` each (None: the library's 256 MiB) while the
+    tensor cores score; the ids are tie-equivalent and the scores bit-equal (where the ids agree) to the all-device
+    index, and with n >= ntotal the search is the all-device one.  add() of host rows (numpy, CPU tensors) copies the
+    rows bound for the host tier host to host."""
     kind = _lib.RSB_FLAT
 
-    def __init__(self, d: int, device=None, dtype: str = "float32"):
+    def __init__(self, d: int, device=None, dtype: str = "float32", device_rows: Optional[int] = None,
+                 staging_bytes: Optional[int] = None):
+        dtype, device_rows = _check_dtype(dtype), _check_device_rows(device_rows)   # before any device allocation
+        if device_rows is not None and dtype != "float16":
+            raise ValueError(f"device_rows (a tiered Flat index) needs dtype='float16'; a {dtype} Flat index stays in "
+                             f"device memory")
         super().__init__(d, device)
-        self.dtype = _check_dtype(dtype)
+        self.dtype, self.device_rows = dtype, device_rows
         with torch.cuda.device(self.device):
             _lib.check(self.L.rsb_flat_create(self.d, _STORE_DTYPES[self.dtype][1], ctypes.byref(self._h)))
+            if self.device_rows is not None:
+                self.set_option(_lib.OPT_DEVICE_ROWS, self.device_rows)
+                if staging_bytes is not None:
+                    self.set_option(_lib.OPT_STAGING_BYTES, int(staging_bytes))
+
+    @property
+    def tiered(self) -> bool:
+        return self.device_rows is not None
+
+    @property
+    def n_dev(self) -> int:
+        """Rows held in device memory (ntotal unless tiered)."""
+        return self._info(_lib.INFO_DEVICE_ROWS)
+
+    @property
+    def host_bytes(self) -> int:
+        """Page-locked host bytes of the host tier (0 unless tiered)."""
+        return self._info(_lib.INFO_HOST_BYTES)
+
+    def add(self, x, ids=None) -> None:
+        if not self.tiered:
+            return super().add(x, ids)
+        # tiered: host rows are handed over where they are (the library copies host-tier rows host to host)
+        if isinstance(x, np.ndarray):
+            x = torch.from_numpy(np.ascontiguousarray(x if x.dtype in (np.float16, np.float32) else x.astype(np.float32)))
+        x = torch.as_tensor(x)
+        if x.dtype not in (torch.float16, torch.float32):
+            x = x.float()
+        x = x.contiguous()
+        if x.dim() != 2 or x.shape[1] != self.d:
+            raise ValueError(f"expected [n, {self.d}] vectors, got {tuple(x.shape)}")
+        with torch.cuda.device(self.device):
+            if x.is_cuda and x.device != self.device:
+                x = x.to(self.device)
+            idt = None
+            if ids is not None:
+                idt = torch.as_tensor(ids).to(device=self.device, dtype=torch.int64).contiguous()
+                if idt.numel() != x.shape[0]:
+                    raise ValueError("ids and x disagree on n")
+            _lib.check(self.L.rsb_add(self._h, _ptr(x), _dtype_code(x), x.shape[0], _ptr(idt), None, 0, _stream()))
+            torch.cuda.current_stream().synchronize()  # x / idt may be temporaries
+
+    def export_rows(self, r0: int, n: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Rows [r0, r0 + n) in the storage dtype, from whichever tier holds them, into `out` (a contiguous [n, d] CPU
+        or CUDA tensor; default: a new CPU tensor)."""
+        if out is None:
+            out = torch.empty((int(n), self.d), dtype=_STORE_DTYPES[self.dtype][0])
+        if tuple(out.shape) != (int(n), self.d) or out.dtype != _STORE_DTYPES[self.dtype][0] or not out.is_contiguous():
+            raise ValueError(f"out must be a contiguous [{n}, {self.d}] {self.dtype} tensor")
+        with torch.cuda.device(self.device):
+            _lib.check(self.L.rsb_export_rows(self._h, int(r0), int(n), _ptr(out), _stream()))
+            torch.cuda.current_stream().synchronize()
+        return out
+
+    def export_ids(self) -> torch.Tensor:
+        """The ids of rows [0, ntotal) (a CUDA int64 tensor)."""
+        with torch.cuda.device(self.device):
+            self.finalize()
+            ids = torch.empty(self.ntotal, dtype=torch.int64, device=self.device)
+            _lib.check(self.L.rsb_export_lists(self._h, None, None, _ptr(ids), _stream()))
+            torch.cuda.current_stream().synchronize()
+        return ids
 
 
 class _IVFBase(_IndexBase):
@@ -879,11 +953,75 @@ def _from_faiss_parts(p: dict, device=None, refine_dtype: Optional[str] = None,
     return index
 
 
+_ROW_CHUNK_BYTES = 64 << 20     # tiered Flat persistence: rows moved per step between the tiers and the file
+
+
+def _write_flat_tiered(index: "IndexFlatIP", path: str, fmt: str) -> None:
+    """A tiered Flat index written in row ranges (rsb_export_rows): the same bytes as the all-device index of the same
+    rows, with host memory bounded by one chunk (faiss) beyond the tiers."""
+    from . import faiss_io
+    n, d = index.ntotal, index.d
+    step = max(1, _ROW_CHUNK_BYTES // (4 * d))
+    ids = index.export_ids()
+    if fmt == "faiss" and not torch.equal(ids, torch.arange(n, dtype=torch.int64, device=ids.device)):
+        import warnings
+        warnings.warn(f"{path}: faiss IndexFlatIP has no id map: only sequential ids can be written in faiss format; "
+                      f"writing the RSB1 container instead")
+        fmt = "rsb1"
+    tmp = path + ".tmp"
+    if fmt == "faiss":       # fp16 rows upcast to fp32 (exact), as _to_faiss_parts writes them
+        chunks = (index.export_rows(r0, min(step, n - r0)).float().numpy() for r0 in range(0, n, step))
+        with open(tmp, "wb") as f:
+            faiss_io.write_flat_rows(f, d, n, chunks)
+    else:
+        blob = {"magic": MAGIC, "kind": int(index.kind), "d": d, "nprobe": int(index.nprobe), "dtype": index.dtype}
+        if n > 0:
+            payload = np.empty((n, d), dtype=np.float16)
+            index.export_rows(0, n, out=torch.from_numpy(payload))
+            blob["offsets"] = np.array([0, n], dtype=np.int64)
+            blob["payload"] = payload
+            blob["ids"] = ids.cpu().numpy()
+        with open(tmp, "wb") as f:
+            pickle.dump(blob, f, protocol=4)
+    os.replace(tmp, path)
+
+
+def _read_flat_tiered(path: str, device, storage_dtype: Optional[str], device_rows: int) -> "IndexFlatIP":
+    """A Flat index file (IxFI or RSB1) into a tiered IndexFlatIP, filled a chunk at a time from a memory map of the
+    faiss payload (RSB1: from the unpickled payload)."""
+    from . import faiss_io
+    if storage_dtype != "float16":
+        raise ValueError(f"device_rows (a tiered Flat index) needs storage_dtype='float16', got {storage_dtype!r}")
+    ids = None
+    if faiss_io.is_faiss_file(path):
+        d, n, rows = faiss_io.flat_rows_memmap(path)
+    else:
+        with open(path, "rb") as f:
+            blob = pickle.load(f)
+        if not isinstance(blob, dict) or blob.get("magic") != MAGIC:
+            raise ValueError(f"{path} is not an RSB1 index file")
+        if blob["kind"] != _lib.RSB_FLAT:
+            raise ValueError("device_rows applies to Flat indexes only")
+        d = blob["d"]
+        rows = blob.get("payload", np.zeros((0, d), np.float16))
+        ids = blob.get("ids")
+        n = rows.shape[0]
+    index = IndexFlatIP(d, device, dtype="float16", device_rows=device_rows)
+    step = max(1, _ROW_CHUNK_BYTES // (4 * d))
+    for r0 in range(0, n, step):
+        chunk = _as_storage(np.asarray(rows[r0:r0 + step]), "float16", f"{path}: the Flat index's vectors")
+        index.add(chunk, None if ids is None else ids[r0:r0 + step])
+    index.finalize()
+    return index
+
+
 def write_index(index: _IndexBase, path: str, fmt: Optional[str] = None) -> None:
     """fmt "faiss" (default; env RSB_INDEX_FORMAT overrides: faiss 1.8 binary layout, see faiss_io.py) or "rsb1"."""
     fmt = (fmt or os.environ.get("RSB_INDEX_FORMAT", "faiss")).lower()
     if fmt not in ("faiss", "rsb1"):
         raise ValueError(f"unknown index file format {fmt!r} (faiss | rsb1)")
+    if isinstance(index, IndexFlatIP) and index.tiered:
+        return _write_flat_tiered(index, path, fmt)
     if isinstance(index, IndexRefine) and fmt != "faiss":
         raise ValueError("an IndexRefine is written in faiss' IndexRefineFlat layout only (fmt='faiss')")
     if fmt == "faiss":
@@ -932,15 +1070,20 @@ def write_index(index: _IndexBase, path: str, fmt: Optional[str] = None) -> None
 
 
 def read_index(path: str, device=None, refine_dtype: Optional[str] = None,
-               storage_dtype: Optional[str] = None) -> _IndexBase:
+               storage_dtype: Optional[str] = None, device_rows: Optional[int] = None) -> _IndexBase:
     """Loads an RSB1 container or a faiss binary index file (auto-detected by its fourcc).  For an IndexRefineFlat
     file (IxRF) `refine_dtype` picks the store: "float32" (default) or "float16", which is accepted only when every
     stored value round-trips through fp16 (ValueError otherwise).  An IxRF file whose refine index is an 8-bit scalar
     quantizer (IxSQ, QT_8bit) loads as an sq8 store (refine_dtype None or "sq8"; float16 / float32 raise ValueError).  `storage_dtype` does the same for the vectors of a
     Flat / IVFFlat index (IxFI / IwFl / RSB1); None keeps the file's dtype (fp32 for faiss files).  An IVF-SQ8 index
     (IwSq / IwSQ, or RSB1 with dtype sq8) loads as an IndexIVFScalarQuantizer with its codes and range as stored
-    (storage_dtype None or "sq8"); "sq8" on a float index and float16 / float32 on an SQ8 index raise ValueError."""
+    (storage_dtype None or "sq8"); "sq8" on a float index and float16 / float32 on an SQ8 index raise ValueError.
+    device_rows = n loads a Flat index (IxFI or RSB1) as a tiered IndexFlatIP (storage_dtype "float16" only, else
+    ValueError), filling the tiers a chunk at a time from a memory map of the faiss payload."""
     from . import faiss_io
+    device_rows = _check_device_rows(device_rows)
+    if device_rows is not None:
+        return _read_flat_tiered(path, device, storage_dtype, device_rows)
     if faiss_io.is_faiss_file(path):
         return _from_faiss_parts(faiss_io.read_faiss(path), device, refine_dtype, storage_dtype)
     with open(path, "rb") as f:

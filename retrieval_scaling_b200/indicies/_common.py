@@ -77,7 +77,8 @@ class BaseIndexer:
     index_kind = "Flat"
 
     def __init__(self, embed_paths, index_path, meta_file, passage_dir=None, pos_map_save_path=None,
-                 dimension=768, trained_index_path=None, sample_train_size=1000000, probe=1, storage_dtype=None):
+                 dimension=768, trained_index_path=None, sample_train_size=1000000, probe=1, storage_dtype=None,
+                 device_rows=None):
         self.embed_paths = list(embed_paths) if embed_paths is not None else []
         self.index_path, self.meta_file = index_path, meta_file
         self.trained_index_path = trained_index_path
@@ -86,10 +87,12 @@ class BaseIndexer:
         self.cuda = True   # informational: unlike the reference (`self.cuda = False`), search runs on the GPU
         # datastore.index.storage_dtype (Flat / IVFFlat): None = fp32 vectors, the reference's upcast-on-load path
         self.storage_dtype = storage_dtype
+        # datastore.index.device_rows (Flat, float16): None = every row in device memory, else a tiered index
+        self.device_rows = device_rows
 
         if os.path.exists(index_path) and os.path.exists(meta_file):
             print("Loading index...")
-            self.index = rsb_index.read_index(index_path, storage_dtype=storage_dtype)
+            self.index = rsb_index.read_index(index_path, storage_dtype=storage_dtype, device_rows=device_rows)
             self.index_id_to_db_id = DbIdMap.load(meta_file)
         else:
             self.index_id_to_db_id = DbIdMap()

@@ -78,12 +78,29 @@ class Indexer(object):
                              f"{index_cfg.index_type} takes float16 or float32")
         return dtype
 
+    @staticmethod
+    def device_rows(index_cfg):
+        """Optional key `device_rows` (absent: None, every row in device memory): an integer >= 0; Flat rows from that
+        position on are kept in pinned host memory and streamed to the GPU by each search (index.IndexFlatIP(
+        device_rows=...)).  Needs index_type Flat with storage_dtype float16."""
+        rows = index_cfg.get("device_rows", None)
+        if rows is None:
+            return None
+        if isinstance(rows, bool) or not isinstance(rows, int) or rows < 0:
+            raise ValueError(f"datastore.index.device_rows must be an integer >= 0, got {rows!r}")
+        if index_cfg.index_type != "Flat" or index_cfg.get("storage_dtype", None) != "float16":
+            raise ValueError(f"datastore.index.device_rows splits a Flat index between device and host memory: it needs "
+                             f"index_type Flat and storage_dtype float16 (got {index_cfg.index_type}, "
+                             f"{index_cfg.get('storage_dtype', None)})")
+        return rows
+
     def __init__(self, cfg, index_shard_ids=None):
         self.cfg = cfg
         self.args = cfg.datastore.index
         self.index_type = self.args.index_type
         self.refine_options(self.args)
         storage_dtype = self.storage_dtype(self.args)
+        device_rows = self.device_rows(self.args)
 
         passage_dir = self.cfg.datastore.embedding.passages_dir
         paths = self.artefact_paths(cfg, index_shard_ids)
@@ -99,7 +116,7 @@ class Indexer(object):
                 if os.path.exists(p):
                     os.remove(p)
         if self.index_type == "Flat":
-            self.datastore = FlatIndexer(storage_dtype=storage_dtype, **common)
+            self.datastore = FlatIndexer(storage_dtype=storage_dtype, device_rows=device_rows, **common)
         elif self.index_type == "IVFFlat":
             self.datastore = IVFFlatIndexer(trained_index_path=index_path + ".trained", sample_train_size=a.sample_train_size,
                                             prev_index_path=None, ncentroids=a.ncentroids, probe=a.probe,
