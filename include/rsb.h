@@ -120,8 +120,37 @@ int rsb_add_preassigned(rsb_index_t* h, const void* x_dev, int x_dtype, int64_t 
 int rsb_add_codes(rsb_index_t* h, const uint8_t* codes_dev, int64_t n, const int64_t* ids_dev,
                   const int32_t* list_dev, rsb_stream_t stream);
 /* Build the searchable layout (CSR inverted lists; PQ codes interleaved per 32 vectors).  Synchronises
- * `stream`.  rsb_search calls it implicitly when adds are pending. */
+ * `stream`.  rsb_search calls it implicitly when adds are pending.  No-op on an index with reserved lists. */
 int rsb_finalize(rsb_index_t* h, rsb_stream_t stream);
+/* Tiered IVFFLAT index (any storage dtype), for datastores larger than device memory: the list sizes are given up
+ * front and the lists are split by id between device memory and page-locked host memory.
+ *   sizes_host [nlist] int64 (host memory) fixes the CSR offsets.  L_dev = the largest list count whose rows fit
+ *   device_rows: lists [0, L_dev) keep their rows in device memory (allocated once, here), lists [L_dev, nlist) in one
+ *   page-locked block the handle owns, of exactly the bytes those lists need.  Ids, centroids, the SQ8 range and the
+ *   list tables stay in device memory (8 bytes of ids per vector).  staging_bytes is the size of one of the two staging
+ *   buffers a search copies host lists into (0: 256 MiB; raised to the largest host list, lowered to the host tier).
+ *   Synchronises `stream`.
+ * Refusals: an IVFPQ or FLAT handle, negative sizes or device_rows: RSB_ERR_INVALID; an untrained handle, a second
+ * reservation, or rows already added: RSB_ERR_STATE.
+ * After it, rsb_add / rsb_add_preassigned / rsb_add_codes place every row in its final slot: the batch is assigned (and
+ * SQ8-encoded) on the device as before, stably sorted by list (insertion order inside a list is kept), device-tier rows
+ * are scattered in place and host-tier rows copied device to host, one copy per run of consecutive slots; each add
+ * synchronises `stream`.  A batch that would overflow a list's reservation is refused whole with RSB_ERR_STATE.
+ * rsb_search, rsb_export_lists and rsb_export_rows before every reserved row has arrived return RSB_ERR_STATE (the
+ * message gives both counts).  rsb_list_sizes reports the reserved sizes.
+ * rsb_search / rsb_search_preassigned keep their signatures.  Per query batch: the coarse step; a kernel flags the host
+ * lists the batch probes and the [nlist] flags are copied to the host; the device lists are scanned in place, enqueued
+ * before the host waits for the flags (the one host synchronisation per batch: only the host can drive the copy
+ * engine); then the probed host lists are packed in list order into chunks of at most one staging buffer, copied by a
+ * copy stream the handle owns into two staging buffers of the workspace and scanned chunk by chunk.  Every (query,
+ * list) pair is scanned once, by the all-device scan kernel on the same bytes; all pieces share the batch's top-k
+ * thresholds and one merge gives the result, so ids and scores equal those of the all-device index of the same lists
+ * (up to the order of exact score ties at the k-th place).  Shared thresholds (rsb_search_preassigned with
+ * tau_local_dev) return RSB_ERR_UNSUPPORTED.
+ * RSB_INFO_DEVICE_ROWS: the rows of lists [0, L_dev) (<= device_rows); RSB_INFO_HOST_BYTES: the host tier;
+ * RSB_INFO_INDEX_BYTES: device bytes, as for every index.  Without a reservation nothing changes. */
+int rsb_reserve_lists(rsb_index_t* h, const int64_t* sizes_host, int64_t device_rows, size_t staging_bytes,
+                      rsb_stream_t stream);
 
 /* ---- introspection --------------------------------------------------------------------------------- */
 enum {
@@ -133,9 +162,10 @@ enum {
     RSB_INFO_DTYPE = 9,        /* storage dtype of the vectors: RSB_DTYPE_F32 / RSB_DTYPE_F16 / RSB_DTYPE_SQ8 (IVFPQ:
                                   RSB_DTYPE_F32) */
     RSB_INFO_BY_RESIDUAL = 10, /* 1 if an SQ8 IVFFLAT index encodes residuals (RSB_OPT_BY_RESIDUAL), else 0 */
-    RSB_INFO_HOST_BYTES = 11,  /* page-locked host bytes held by a tiered Flat index's host tier (0 on other handles) */
-    RSB_INFO_DEVICE_ROWS = 12  /* rows held in device memory: min(device_rows, ntotal) on a tiered Flat index, else
-                                  ntotal */
+    RSB_INFO_HOST_BYTES = 11,  /* page-locked host bytes held by the host tier of a tiered Flat index or of an IVFFLAT
+                                  index with reserved lists (0 on other handles) */
+    RSB_INFO_DEVICE_ROWS = 12  /* rows held in device memory: min(device_rows, ntotal) on a tiered Flat index, the rows of
+                                  lists [0, L_dev) on an IVFFLAT index with reserved lists, else ntotal */
 };
 int rsb_info(rsb_index_t* h, int what, int64_t* out);
 /* list sizes [nlist] int64 to a device buffer */
@@ -146,10 +176,11 @@ int rsb_list_sizes(rsb_index_t* h, int64_t* sizes_dev, rsb_stream_t stream);
  * (IVFFLAT with SQ8 storage), ids_dev [ntotal] int64.  Any pointer may be NULL. */
 int rsb_export_lists(rsb_index_t* h, int64_t* offsets_dev, void* payload_dev, int64_t* ids_dev,
                      rsb_stream_t stream);
-/* Rows [r0, r0 + n) of a FLAT index in its storage dtype ([n, d]), copied from whichever tier holds them to dst, which
- * may be device memory or host memory (pageable or pinned).  Lets a caller export a tiered index larger than device
- * memory one range at a time.  Pending adds are finalised first.  Other handles, or a range outside [0, ntotal):
- * RSB_ERR_INVALID. */
+/* Rows [r0, r0 + n) of a FLAT index, or CSR rows [r0, r0 + n) of an IVFFLAT index (the natural order of
+ * rsb_export_lists), in the storage dtype ([n, d]; SQ8: uint8 codes), copied from whichever tier holds them to dst,
+ * which may be device memory or host memory (pageable or pinned).  Lets a caller export a tiered index larger than
+ * device memory one range at a time.  Pending adds are finalised first.  IVFPQ handles, or a range outside
+ * [0, ntotal): RSB_ERR_INVALID; an IVFFLAT index whose reserved rows have not all arrived: RSB_ERR_STATE. */
 int rsb_export_rows(rsb_index_t* h, int64_t r0, int64_t n, void* dst, rsb_stream_t stream);
 
 /* ---- search (index.search(x, k) + index.nprobe: flat.py:139, ivf_flat.py:73,225, ivf_pq.py:76,230) --- */

@@ -42,6 +42,7 @@ SIGNATURES = [
     ("rsb_list_sizes", c_int, [_H, c_void_p, c_void_p]),
     ("rsb_export_lists", c_int, [_H, c_void_p, c_void_p, c_void_p, c_void_p]),
     ("rsb_export_rows", c_int, [_H, c_int64, c_int64, c_void_p, c_void_p]),
+    ("rsb_reserve_lists", c_int, [_H, c_void_p, c_int64, c_size_t, c_void_p]),
     ("rsb_workspace_bytes", c_size_t, [_H, c_int, c_int, c_int]),
     ("rsb_search", c_int, [_H, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     ("rsb_search_preassigned", c_int, [_H, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,

@@ -111,6 +111,26 @@ struct rsb_index {
     cudaEvent_t stage_ready[2] = {}, stage_free[2] = {}, copy_start = nullptr, copy_done = nullptr;
     bool tiered() const { return dev_rows >= 0; }
 
+    // tiered IVFFLAT (rsb_reserve_lists): the CSR layout is fixed up front from the reserved list sizes.  The rows of
+    // lists [0, l_dev) (slots [0, ivf_dev_rows)) live in `payload`, those of lists [l_dev, nlist) in ivf_host (page-
+    // locked, one block of exactly the bytes needed, slot s at row s - ivf_dev_rows).  Ids, list tables, centroids and
+    // the SQ8 range stay on the device.  rsb_add / rsb_add_preassigned / rsb_add_codes place every row in its final
+    // slot; ntotal counts the rows placed so far (nslots the rows reserved).  host_bytes / copy_st / the stage events
+    // are shared with the tiered Flat index.
+    bool ivf_reserved = false;
+    int l_dev = 0;
+    int64_t ivf_dev_rows = 0;
+    uint8_t* ivf_host = nullptr;
+    std::vector<int> ivf_len;              // [nlist] reserved sizes
+    std::vector<int64_t> ivf_off;          // [nlist + 1] CSR offsets
+    std::vector<int64_t> ivf_fill;         // [nlist] rows placed so far
+    int* dev_len = nullptr;                // [nlist] device: list_len on lists [0, l_dev), 0 elsewhere
+    size_t ivf_stage_bytes = 0;            // one staging buffer of the search (>= the largest host list)
+    unsigned char* tier_pinned = nullptr;  // page-locked: the per-batch table the search copies to the device
+                                           // (stage_off int64 [nlist], chunk_of int32 [nlist]), then probed flags [nlist]
+    cudaEvent_t flags_ready = nullptr;
+    bool ivf_streamed() const { return ivf_reserved && ivf_dev_rows < nslots; }
+
     // profiling
     bool prof = false;
     // ring of event sets: one set per profiled search since the last rsb_get_profile (which averages them), so a
@@ -132,6 +152,7 @@ static void free_segment(Segment& s) {
 }
 static void free_layout(rsb_index* h) {
     cudaFree(h->payload); cudaFree(h->ids_slots); cudaFree(h->list_len); cudaFree(h->list_rank);
+    cudaFree(h->dev_len); h->dev_len = nullptr;
     cudaFree(h->flat_hi); cudaFree(h->flat_lo);
     h->flat_hi = nullptr; h->flat_lo = nullptr; h->list_rank = nullptr;
     cudaFree(h->list_slot_off); cudaFree(h->list_nat_off);
@@ -199,6 +220,9 @@ extern "C" int rsb_free(rsb_index_t* h) {
     for (cudaEvent_t e : {h->stage_ready[0], h->stage_ready[1], h->stage_free[0], h->stage_free[1], h->copy_start, h->copy_done})
         if (e) cudaEventDestroy(e);
     for (auto& b : h->host_blocks) cudaFreeHost(b.p);
+    if (h->ivf_host) cudaFreeHost(h->ivf_host);
+    if (h->tier_pinned) cudaFreeHost(h->tier_pinned);
+    if (h->flags_ready) cudaEventDestroy(h->flags_ready);
     delete h;
     return RSB_OK;
 }
@@ -209,7 +233,8 @@ extern "C" int rsb_free(rsb_index_t* h) {
 extern "C" int rsb_set_centroids(rsb_index_t* h, const float* c, rsb_stream_t stream) {
     if (!h || !c) return fail(RSB_ERR_INVALID, "null argument");
     if (h->kind == RSB_FLAT) return fail(RSB_ERR_INVALID, "a Flat index has no centroids");
-    if (h->ntotal || h->n_staged) return fail(RSB_ERR_STATE, "cannot change centroids of a populated index");
+    if (h->ntotal || h->n_staged || h->ivf_reserved)
+        return fail(RSB_ERR_STATE, "cannot change centroids of a populated (or reserved) index");
     cudaStream_t st = (cudaStream_t)stream;
     const size_t bytes = (size_t)h->nlist * h->d * 4;
     if (!h->centroids) CU(cudaMalloc(&h->centroids, bytes));
@@ -254,7 +279,8 @@ static bool is_sq8_ivf(const rsb_index* h) { return h->kind == RSB_IVFFLAT && h-
 extern "C" int rsb_set_sq_range(rsb_index_t* h, const float* sq, rsb_stream_t stream) {
     if (!h || !sq) return fail(RSB_ERR_INVALID, "null argument");
     if (!is_sq8_ivf(h)) return fail(RSB_ERR_INVALID, "only an IVFFLAT index with RSB_DTYPE_SQ8 storage has a scalar-quantizer range");
-    if (h->ntotal || h->n_staged) return fail(RSB_ERR_STATE, "cannot change the range of a populated index (its codes use it)");
+    if (h->ntotal || h->n_staged || h->ivf_reserved)
+        return fail(RSB_ERR_STATE, "cannot change the range of a populated (or reserved) index (its codes use it)");
     const size_t bytes = (size_t)2 * h->d * 4;
     if (!h->sq) CU(cudaMalloc(&h->sq, bytes));
     CU(cudaMemcpyAsync(h->sq, sq, bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
@@ -401,6 +427,16 @@ extern "C" int rsb_knn_ip(const float* q, int nq, const float* x, int64_t n, int
     return knn_ip_device(nullptr, q, nq, x, n, d, k, nullptr, id_offset, D, I, ws, ws_bytes, (cudaStream_t)stream);
 }
 
+// the copy stream and stage events of a tiered index, on the device current now (which holds the index)
+static int ensure_copy_stream(rsb_index* h) {
+    if (h->copy_st) return RSB_OK;
+    CU(cudaStreamCreateWithFlags(&h->copy_st, cudaStreamNonBlocking));
+    for (cudaEvent_t* e : {&h->stage_ready[0], &h->stage_ready[1], &h->stage_free[0], &h->stage_free[1], &h->copy_start,
+                           &h->copy_done})
+        CU(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+    return RSB_OK;
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // population
 // ---------------------------------------------------------------------------------------------------------
@@ -540,6 +576,8 @@ static int add_tiered(rsb_index* h, const void* x, int x_dtype, int64_t n, const
 
 // x: [n, d] in x_dtype (RSB_DTYPE_F32 / RSB_DTYPE_F16); stored in the handle's dtype (fp32 -> fp16 rounds to nearest
 // even, fp16 -> fp32 is exact).  IVF list assignment runs on fp32 values (fp16 input is upcast 16384 rows at a time).
+static int place_segment(rsb_index* h, const Segment& seg, cudaStream_t st);
+
 static int add_impl(rsb_index* h, const void* x, int x_dtype, const uint8_t* codes_in, int64_t n, const int64_t* ids,
                     const int32_t* list_in, void* ws, size_t ws_bytes, cudaStream_t st) {
     if (!h) return fail(RSB_ERR_INVALID, "null handle");
@@ -557,6 +595,7 @@ static int add_impl(rsb_index* h, const void* x, int x_dtype, const uint8_t* cod
     if (h->ntotal + h->n_staged + n >= ((int64_t)1 << 31) - 64 * (int64_t)h->nlist)
         return fail(RSB_ERR_UNSUPPORTED, "more than 2^31 vectors per index shard (shard the datastore across GPUs)");
     if (h->tiered()) return add_tiered(h, x, x_dtype, n, ids, st);
+    const int64_t next_id0 = h->next_id;
     Segment seg;
     int rc = stage_common(h, seg, ids, n, st);
     if (rc != RSB_OK) { free_segment(seg); return rc; }
@@ -612,6 +651,13 @@ static int add_impl(rsb_index* h, const void* x, int x_dtype, const uint8_t* cod
     }
     CUB_(cudaPeekAtLastError());
 #undef CUB_
+    if (h->ivf_reserved) {   // the rows go to their final slots now; the segment was only the encoded batch
+        rc = place_segment(h, seg, st);
+        cudaStreamSynchronize(st);
+        free_segment(seg);
+        if (rc != RSB_OK) h->next_id = next_id0;
+        return rc;
+    }
     h->staging.push_back(seg);
     h->n_staged += n;
     return RSB_OK;
@@ -633,6 +679,195 @@ extern "C" int rsb_add_codes(rsb_index_t* h, const uint8_t* codes, int64_t n, co
         return fail(RSB_ERR_INVALID, "rsb_add_codes needs an IVFPQ index or an IVFFLAT index with SQ8 storage");
     if (!list || !codes) return fail(RSB_ERR_INVALID, "null argument");
     return add_impl(h, nullptr, RSB_DTYPE_F32, codes, n, ids, list, nullptr, 0, (cudaStream_t)stream);
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// tiered IVFFLAT: reserve the lists, then place every added row in its final slot
+// ---------------------------------------------------------------------------------------------------------
+extern "C" int rsb_reserve_lists(rsb_index_t* h, const int64_t* sizes, int64_t device_rows, size_t staging_bytes,
+                                 rsb_stream_t stream) {
+    if (!h) return fail(RSB_ERR_INVALID, "null handle");
+    if (h->kind != RSB_IVFFLAT)
+        return fail(RSB_ERR_INVALID, "rsb_reserve_lists splits the lists of an IVFFLAT index (any dtype), not an %s index",
+                    h->kind == RSB_IVFPQ ? "IVFPQ" : "FLAT");
+    if (!sizes) return fail(RSB_ERR_INVALID, "sizes is NULL");
+    if (device_rows < 0) return fail(RSB_ERR_INVALID, "device_rows must be >= 0, got %lld", (long long)device_rows);
+    const int nlist = h->nlist;
+    std::vector<int> len(nlist);
+    std::vector<int64_t> off(nlist + 1, 0);
+    for (int l = 0; l < nlist; ++l) {
+        if (sizes[l] < 0) return fail(RSB_ERR_INVALID, "list %d has a negative size %lld", l, (long long)sizes[l]);
+        if (sizes[l] >= ((int64_t)1 << 31) || off[l] + sizes[l] >= ((int64_t)1 << 31) - 64 * (int64_t)nlist)
+            return fail(RSB_ERR_UNSUPPORTED, "more than 2^31 vectors per index shard (shard the datastore across GPUs)");
+        len[l] = (int)sizes[l];
+        off[l + 1] = off[l] + sizes[l];
+    }
+    if (!is_trained(h))
+        return fail(RSB_ERR_STATE, "index is not trained (set centroids%s first)", is_sq8_ivf(h) ? " and the SQ8 range" : "");
+    if (h->ivf_reserved) return fail(RSB_ERR_STATE, "the lists are already reserved (one reservation per index)");
+    if (h->ntotal || h->n_staged) return fail(RSB_ERR_STATE, "rows were already added: reserve the lists of an empty index");
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t rb = h->row_bytes();
+    const int64_t total = off[nlist];
+    int l_dev = 0;                                  // the largest list count whose rows fit device_rows
+    while (l_dev < nlist && off[l_dev + 1] <= device_rows) ++l_dev;
+    const int64_t dev_rows = off[l_dev], host_rows = total - dev_rows;
+    int max_len = 0, max_host = 0;
+    for (int l = 0; l < nlist; ++l) {
+        max_len = std::max(max_len, len[l]);
+        if (l >= l_dev) max_host = std::max(max_host, len[l]);
+    }
+    // a staging buffer holds at least the largest host list, and never more than the whole host tier
+    size_t stage = staging_bytes ? staging_bytes : kDefaultStagingBytes;
+    stage = std::min(std::max(stage, (size_t)max_host * rb), (size_t)host_rows * rb);
+    std::vector<int> dlen(nlist), by_len(nlist), rank_of(nlist);
+    for (int l = 0; l < nlist; ++l) { dlen[l] = l < l_dev ? len[l] : 0; by_len[l] = l; }
+    std::stable_sort(by_len.begin(), by_len.end(), [&](int a, int b) { return len[a] > len[b]; });
+    for (int i = 0; i < nlist; ++i) rank_of[by_len[i]] = i;
+
+    auto undo = [&](int rc) {
+        cudaStreamSynchronize(st);
+        free_layout(h);
+        if (h->ivf_host) cudaFreeHost(h->ivf_host);
+        if (h->tier_pinned) cudaFreeHost(h->tier_pinned);
+        h->ivf_host = nullptr; h->tier_pinned = nullptr;
+        return rc;
+    };
+#define CUR(expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) return undo(fail(e__ == cudaErrorMemoryAllocation ? RSB_ERR_OOM : RSB_ERR_CUDA, "%s: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__)); } while (0)
+    free_layout(h);
+    CUR(cudaMalloc(&h->list_len, (size_t)nlist * 4));
+    CUR(cudaMalloc(&h->dev_len, (size_t)nlist * 4));
+    CUR(cudaMalloc(&h->list_rank, (size_t)nlist * 4));
+    CUR(cudaMalloc(&h->list_nat_off, (size_t)(nlist + 1) * 8));
+    CUR(cudaMalloc(&h->list_slot_off, (size_t)(nlist + 1) * 8));
+    CUR(cudaMemcpyAsync(h->list_len, len.data(), (size_t)nlist * 4, cudaMemcpyHostToDevice, st));
+    CUR(cudaMemcpyAsync(h->dev_len, dlen.data(), (size_t)nlist * 4, cudaMemcpyHostToDevice, st));
+    CUR(cudaMemcpyAsync(h->list_rank, rank_of.data(), (size_t)nlist * 4, cudaMemcpyHostToDevice, st));
+    CUR(cudaMemcpyAsync(h->list_nat_off, off.data(), (size_t)(nlist + 1) * 8, cudaMemcpyHostToDevice, st));
+    CUR(cudaMemcpyAsync(h->list_slot_off, off.data(), (size_t)(nlist + 1) * 8, cudaMemcpyHostToDevice, st));
+    CUR(cudaMalloc(&h->payload, std::max<size_t>((size_t)dev_rows * rb, 256)));     // the device tier, once
+    CUR(cudaMalloc(&h->ids_slots, std::max<size_t>((size_t)total * 8, 256)));
+    launch_fill_i64(h->ids_slots, total, -1, st);
+    CUR(cudaPeekAtLastError());
+    if (host_rows) CUR(cudaHostAlloc((void**)&h->ivf_host, (size_t)host_rows * rb, cudaHostAllocPortable));
+    CUR(cudaHostAlloc((void**)&h->tier_pinned, (size_t)nlist * 13, cudaHostAllocPortable));
+    if (ensure_copy_stream(h) != RSB_OK) return undo(RSB_ERR_CUDA);
+    if (!h->flags_ready) CUR(cudaEventCreateWithFlags(&h->flags_ready, cudaEventDisableTiming));
+    CUR(cudaStreamSynchronize(st));
+#undef CUR
+    h->ivf_reserved = true;
+    h->l_dev = l_dev;
+    h->ivf_dev_rows = dev_rows;
+    h->ivf_len = len; h->ivf_off = off; h->ivf_fill.assign(nlist, 0);
+    h->ivf_stage_bytes = stage;
+    h->host_bytes = (size_t)host_rows * rb;
+    h->payload_bytes = (size_t)dev_rows * rb;
+    h->nslots = total; h->ntotal = 0; h->max_list_len = max_len;
+    return RSB_OK;
+}
+
+// rsb_search / rsb_export_* of a reserved index: every reserved row must have arrived
+static int ivf_check_complete(const rsb_index* h) {
+    if (h->ivf_reserved && h->ntotal < h->nslots)
+        return fail(RSB_ERR_STATE, "%lld of the %lld reserved rows have been added: add the rest first",
+                    (long long)h->ntotal, (long long)h->nslots);
+    return RSB_OK;
+}
+
+// One add batch of a reserved index (seg: ids, lists, rows in the storage dtype, on the device): refused whole when a
+// list would overflow its reservation; else stably sorted by list (insertion order inside a list is kept), device-tier
+// rows scattered to list_slot_off[l] + fill[l] + rank, host-tier rows gathered in list order and copied device to host,
+// one copy per run of consecutive slots.  Synchronises st.
+static int place_segment(rsb_index* h, const Segment& seg, cudaStream_t st) {
+    const int64_t n = seg.n;
+    const int nlist = h->nlist;
+    const size_t rb = h->row_bytes();
+    int* hist = nullptr;
+    int32_t* sorted_list = nullptr;
+    int64_t *src_idx = nullptr, *sorted_src = nullptr, *tabs = nullptr;
+    uint8_t* host_stage = nullptr;
+    void* cub_tmp = nullptr;
+    auto cleanup = [&](int rc) {
+        cudaStreamSynchronize(st);
+        cudaFree(hist); cudaFree(sorted_list); cudaFree(src_idx); cudaFree(sorted_src); cudaFree(tabs);
+        cudaFree(host_stage); cudaFree(cub_tmp);
+        return rc;
+    };
+#define CUP(expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) return cleanup(fail(e__ == cudaErrorMemoryAllocation ? RSB_ERR_OOM : RSB_ERR_CUDA, "%s: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__)); } while (0)
+    CUP(cudaMalloc(&hist, (size_t)nlist * 4));
+    CUP(cudaMemsetAsync(hist, 0, (size_t)nlist * 4, st));
+    launch_list_hist(seg.list, n, nlist, hist, st);
+    std::vector<int> cnt(nlist);
+    CUP(cudaMemcpyAsync(cnt.data(), hist, (size_t)nlist * 4, cudaMemcpyDeviceToHost, st));
+    CUP(cudaStreamSynchronize(st));
+    int64_t in_range = 0;
+    for (int l = 0; l < nlist; ++l) in_range += cnt[l];
+    if (in_range != n)
+        return cleanup(fail(RSB_ERR_INVALID, "list ids out of range [0, %d): %lld of %lld rows assigned", nlist,
+                            (long long)in_range, (long long)n));
+    for (int l = 0; l < nlist; ++l)
+        if (h->ivf_fill[l] + cnt[l] > h->ivf_len[l])
+            return cleanup(fail(RSB_ERR_STATE, "the batch adds %d rows to list %d, which holds %lld of its %d reserved rows: "
+                                "nothing of the batch was added", cnt[l], l, (long long)h->ivf_fill[l], h->ivf_len[l]));
+    // batch_start [nlist] (first sorted row of list l in the batch), dst_base [nlist] (its slot)
+    std::vector<int64_t> tab(2 * (size_t)nlist);
+    int64_t acc = 0;
+    for (int l = 0; l < nlist; ++l) {
+        tab[l] = acc;
+        tab[nlist + l] = h->ivf_off[l] + h->ivf_fill[l];
+        acc += cnt[l];
+    }
+    const int64_t host_begin = h->l_dev < nlist ? tab[h->l_dev] : n;
+    CUP(cudaMalloc(&tabs, (size_t)2 * nlist * 8));
+    CUP(cudaMemcpyAsync(tabs, tab.data(), (size_t)2 * nlist * 8, cudaMemcpyHostToDevice, st));
+    CUP(cudaMalloc(&sorted_list, (size_t)n * 4));
+    CUP(cudaMalloc(&src_idx, (size_t)n * 8));
+    CUP(cudaMalloc(&sorted_src, (size_t)n * 8));
+    launch_iota_i64(src_idx, n, 0, st);
+    int bits = 1;
+    while ((1 << bits) < nlist) ++bits;
+    size_t tmp_bytes = 0;
+    CUP(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, seg.list, sorted_list, src_idx, sorted_src, n, 0, bits, st));
+    CUP(cudaMalloc(&cub_tmp, tmp_bytes));
+    CUP(cub::DeviceRadixSort::SortPairs(cub_tmp, tmp_bytes, seg.list, sorted_list, src_idx, sorted_src, n, 0, bits, st));
+    if (n > host_begin) CUP(cudaMalloc(&host_stage, (size_t)(n - host_begin) * rb));
+    launch_ivf_place_rows(sorted_list, sorted_src, n, tabs, tabs + nlist, h->l_dev, host_begin, seg.payload, seg.ids,
+                          (int)rb, h->payload, host_stage, h->ids_slots, st);
+    CUP(cudaPeekAtLastError());
+    // host-tier rows: one device-to-host copy per run of slots that are consecutive in both buffers
+    for (int l = h->l_dev; l < nlist;) {
+        if (!cnt[l]) { ++l; continue; }
+        const int64_t s0 = tab[l] - host_begin, d0 = tab[nlist + l] - h->ivf_dev_rows;
+        int64_t rows = cnt[l];
+        int e = l + 1;
+        for (; e < nlist; ++e) {
+            if (!cnt[e]) continue;
+            if (tab[e] - host_begin != s0 + rows || tab[nlist + e] - h->ivf_dev_rows != d0 + rows) break;
+            rows += cnt[e];
+        }
+        CUP(cudaMemcpyAsync(h->ivf_host + (size_t)d0 * rb, host_stage + (size_t)s0 * rb, (size_t)rows * rb,
+                            cudaMemcpyDeviceToHost, st));
+        l = e;
+    }
+    CUP(cudaStreamSynchronize(st));
+#undef CUP
+    for (int l = 0; l < nlist; ++l) h->ivf_fill[l] += cnt[l];
+    h->ntotal += n;
+    return cleanup(RSB_OK);
+}
+
+// slots [r0, r0 + n) of a reserved IVFFLAT index, from whichever tier holds them, to dst (device or host memory)
+static int ivf_copy_rows(rsb_index* h, int64_t r0, int64_t n, void* dst, cudaStream_t st) {
+    const size_t rb = h->row_bytes();
+    uint8_t* out = static_cast<uint8_t*>(dst);
+    const int64_t nd = h->ivf_dev_rows;
+    if (r0 < nd && n > 0)
+        CU(cudaMemcpyAsync(out, h->payload + (size_t)r0 * rb, (size_t)std::min(n, nd - r0) * rb, cudaMemcpyDefault, st));
+    const int64_t a = std::max(r0, nd), e = r0 + n;
+    if (a < e)
+        CU(cudaMemcpyAsync(out + (size_t)(a - r0) * rb, h->ivf_host + (size_t)(a - nd) * rb, (size_t)(e - a) * rb,
+                           cudaMemcpyDefault, st));
+    return RSB_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -865,7 +1100,8 @@ extern "C" int rsb_info(rsb_index_t* h, int what, int64_t* out) {
         case RSB_INFO_BY_RESIDUAL: *out = h->by_residual ? 1 : 0; break;
         case RSB_INFO_HOST_BYTES: *out = (int64_t)h->host_bytes; break;
         case RSB_INFO_DEVICE_ROWS:
-            *out = h->tiered() ? std::min(h->dev_rows, h->ntotal + h->n_staged) : h->ntotal + h->n_staged;
+            *out = h->tiered() ? std::min(h->dev_rows, h->ntotal + h->n_staged)
+                   : h->ivf_reserved ? h->ivf_dev_rows : h->ntotal + h->n_staged;
             break;
         default: return fail(RSB_ERR_INVALID, "unknown info key %d", what);
     }
@@ -921,6 +1157,11 @@ static int export_impl(rsb_index* h, int64_t* offsets, void* payload, int64_t* i
     }
     if (offsets) CU(cudaMemcpyAsync(offsets, h->list_nat_off, (size_t)(h->nlist + 1) * 8, cudaMemcpyDeviceToDevice, st));
     if (h->ntotal == 0) return RSB_OK;
+    if (h->ivf_reserved) {   // CSR slots are the natural order; rows from either tier, to device or host memory
+        if (payload) RSB_TRY(ivf_copy_rows(h, 0, h->ntotal, payload, st));
+        if (ids) CU(cudaMemcpyAsync(ids, h->ids_slots, (size_t)h->ntotal * 8, cudaMemcpyDefault, st));
+        return RSB_OK;
+    }
     if (h->kind == RSB_IVFPQ) {
         if (payload && pq_interleaved_layout(h->Mb))
             launch_pq_deinterleave(h->payload, h->list_nat_off, h->list_slot_off, h->list_len, h->nlist, h->Mb, static_cast<uint8_t*>(payload), st);
@@ -938,18 +1179,27 @@ static int export_impl(rsb_index* h, int64_t* offsets, void* payload, int64_t* i
 extern "C" int rsb_export_lists(rsb_index_t* h, int64_t* offsets, void* payload, int64_t* ids, rsb_stream_t stream) {
     if (!h) return fail(RSB_ERR_INVALID, "null handle");
     if (!h->staging.empty()) RSB_TRY(rsb_finalize(h, stream));
+    RSB_TRY(ivf_check_complete(h));
     return export_impl(h, offsets, payload, ids, (cudaStream_t)stream);
 }
 
 extern "C" int rsb_export_rows(rsb_index_t* h, int64_t r0, int64_t n, void* dst, rsb_stream_t stream) {
     if (!h) return fail(RSB_ERR_INVALID, "null handle");
-    if (h->kind != RSB_FLAT) return fail(RSB_ERR_INVALID, "rsb_export_rows reads the rows of a Flat index");
+    if (h->kind == RSB_IVFPQ)
+        return fail(RSB_ERR_INVALID, "rsb_export_rows reads the rows of a Flat or IVFFLAT index, not IVFPQ codes");
     if (!h->staging.empty()) RSB_TRY(rsb_finalize(h, stream));
+    RSB_TRY(ivf_check_complete(h));
     if (r0 < 0 || n < 0 || r0 + n > h->ntotal)
         return fail(RSB_ERR_INVALID, "rows [%lld, %lld) are outside [0, %lld)", (long long)r0, (long long)(r0 + n),
                     (long long)h->ntotal);
     if (n == 0) return RSB_OK;
     if (!dst) return fail(RSB_ERR_INVALID, "dst is NULL");
+    if (h->kind == RSB_IVFFLAT && h->ivf_reserved) return ivf_copy_rows(h, r0, n, dst, (cudaStream_t)stream);
+    if (h->kind == RSB_IVFFLAT) {   // the all-device CSR rows
+        CU(cudaMemcpyAsync(dst, h->payload + (size_t)r0 * h->row_bytes(), (size_t)n * h->row_bytes(), cudaMemcpyDefault,
+                           (cudaStream_t)stream));
+        return RSB_OK;
+    }
     return flat_copy_rows(h, r0, n, dst, (cudaStream_t)stream);
 }
 
@@ -1152,6 +1402,27 @@ static int search_flat_tiered(rsb_index* h, const float* q, int nq, int k, float
     return RSB_OK;
 }
 
+// Tiered IVFFLAT search (lists past l_dev in host memory): the search plan's workspace, then the probed-list flags
+// [nlist], one piece's masked list_len [nlist] int32 and staging offsets [nlist] int64, the per-batch table (stage_off
+// [nlist] int64, chunk_of [nlist] int32) and two staging buffers of ivf_stage_bytes.
+struct IvfTierPlan {
+    size_t off_flags, off_plen, off_pdata, off_table, off_stage[2], total;
+};
+static IvfTierPlan ivf_tier_plan(const rsb_index* h, size_t base) {
+    IvfTierPlan t;
+    size_t o = align_up(base);
+    t.off_flags = o; o += align_up((size_t)h->nlist);
+    t.off_plen = o;  o += align_up((size_t)h->nlist * 4);
+    t.off_pdata = o; o += align_up((size_t)h->nlist * 8);
+    t.off_table = o; o += align_up((size_t)h->nlist * 12);
+    for (int b = 0; b < 2; ++b) {
+        t.off_stage[b] = o;
+        o += align_up(h->ivf_stage_bytes);
+    }
+    t.total = o;
+    return t;
+}
+
 extern "C" size_t rsb_workspace_bytes(rsb_index_t* h, int nq, int k, int nprobe) {
     if (!h) return 0;
     nq = std::max(nq, 1); k = std::max(k, 1);
@@ -1165,6 +1436,7 @@ extern "C" size_t rsb_workspace_bytes(rsb_index_t* h, int nq, int k, int nprobe)
                             align_up((size_t)kp.qb * kc * 8);
         return std::max(plain, tens);
     }
+    if (h->ivf_streamed()) return ivf_tier_plan(h, search_plan(h, nq, k, nprobe).total).total;
     return search_plan(h, nq, k, nprobe).total;
 }
 
@@ -1246,6 +1518,127 @@ static void launch_pq_tables(const rsb_index* h, const float* q, int nq, float* 
     else launch_pq_lut_generic(q, nq, h->d, h->M, h->codebook, lut, st);
 }
 
+// Tiered IVFFLAT search, per query batch:
+//   1. the coarse step (or the caller's lists), then the probed host lists are flagged on the device and the [nlist]
+//      flags copied to page-locked memory;
+//   2. the device lists are scanned in place (list_len masked to lists [0, l_dev)), enqueued before the host waits;
+//   3. the host waits for the flags -- the one host synchronisation per batch, by design: only the host can drive the
+//      copy engine -- and packs the probed host lists, in list order, into chunks of at most one staging buffer
+//      (adjacent lists coalesced into one copy).  copy_st copies chunk c into staging buffer c % 2 (stage_ready /
+//      stage_free events, as in search_flat_tiered) while the caller's stream scans chunk c - 1; a small kernel
+//      derives each chunk's masked list_len and staging offsets from one per-batch table, copied by copy_st ahead of
+//      the chunks;
+//   4. every piece shares the batch's thresholds tau and writes disjoint (query, probe) slots of out_keys / out_cnt,
+//      so one merge_items gives the result, as in the all-device search.
+// The pinned flags / table are rewritten only after the host has waited for this batch's flags, which the caller's
+// stream orders after every use of them by the previous batch.
+static int search_ivf_tiered(rsb_index* h, const float* q, int nq, int k, const SearchPlan& p, const IvfTierPlan& t,
+                             const int64_t* pre_lists, const float* pre_dis, float* D, int64_t* I, unsigned char* w,
+                             cudaStream_t st) {
+    const int nlist = h->nlist;
+    const size_t rb = h->row_bytes();
+    const int64_t stage_rows = (int64_t)(h->ivf_stage_bytes / rb);
+    unsigned char* dflags = w + t.off_flags;
+    int* plen = reinterpret_cast<int*>(w + t.off_plen);
+    int64_t* pdata = reinterpret_cast<int64_t*>(w + t.off_pdata);
+    int64_t* dtab = reinterpret_cast<int64_t*>(w + t.off_table);
+    uint8_t* stage[2] = {w + t.off_stage[0], w + t.off_stage[1]};
+    int64_t* stage_off = reinterpret_cast<int64_t*>(h->tier_pinned);
+    int* chunk_of = reinterpret_cast<int*>(stage_off + nlist);
+    unsigned char* hflags = h->tier_pinned + (size_t)nlist * 12;
+    struct Run { int chunk; int64_t host_row, stage_row, rows; };
+    std::vector<Run> runs;
+    auto copy_chunk = [&](int c) -> int {
+        for (const Run& r : runs)
+            if (r.chunk == c)
+                CU(cudaMemcpyAsync(stage[c & 1] + (size_t)r.stage_row * rb, h->ivf_host + (size_t)r.host_row * rb,
+                                   (size_t)r.rows * rb, cudaMemcpyHostToDevice, h->copy_st));
+        CU(cudaEventRecord(h->stage_ready[c & 1], h->copy_st));
+        return RSB_OK;
+    };
+    for (int q0 = 0; q0 < nq; q0 += p.qb) {
+        const int nb = std::min(p.qb, nq - q0);
+        const float* qb = q + (size_t)q0 * h->d;
+        if (pre_lists) {
+            CU(cudaMemcpyAsync(w + p.off_cI, pre_lists + (size_t)q0 * p.nprobe, (size_t)nb * p.nprobe * 8, cudaMemcpyDeviceToDevice, st));
+            CU(cudaMemcpyAsync(w + p.off_cD, pre_dis + (size_t)q0 * p.nprobe, (size_t)nb * p.nprobe * 4, cudaMemcpyDeviceToDevice, st));
+        } else {
+            RSB_TRY(coarse_impl(h, qb, nb, p, w, st));
+        }
+        const int64_t* cI = reinterpret_cast<const int64_t*>(w + p.off_cI);
+        ScanArgs a;
+        a.coarse_ids = cI; a.coarse_scores = reinterpret_cast<const float*>(w + p.off_cD); a.nprobe = p.nprobe;
+        a.list_off = h->list_slot_off;
+        a.tau = reinterpret_cast<unsigned*>(w + p.off_tau);
+        a.tau_peers = nullptr; a.n_peers = 0; a.tau_external = 0;
+        a.k = k;
+        a.out_keys = reinterpret_cast<u64*>(w + p.off_keys);
+        a.out_cnt = reinterpret_cast<int*>(w + p.off_cnt);
+        a.dbg_flag = reinterpret_cast<unsigned*>(h->prof_dev + 2);
+        a.items = nullptr; a.qlut = nullptr; a.quant = nullptr; a.rescored = nullptr;
+        // the pieces of this batch share tau and out_cnt: zeroed once, here
+        CU(cudaMemsetAsync(a.tau, 0, (size_t)nb * 4, st));
+        CU(cudaMemsetAsync(a.out_cnt, 0, (size_t)nb * p.nprobe * 4, st));
+        launch_ivf_probed_flags(cI, nb * p.nprobe, nlist, h->l_dev, h->list_len, dflags, st);
+        CU(cudaMemcpyAsync(hflags, dflags, (size_t)nlist, cudaMemcpyDeviceToHost, st));
+        CU(cudaEventRecord(h->flags_ready, st));
+        // copies of this batch may start now: the previous batch's scans of the staging buffers are done by then
+        CU(cudaEventRecord(h->copy_start, st));
+        CU(cudaStreamWaitEvent(h->copy_st, h->copy_start, 0));
+        static const bool lpt_env = getenv("RSB_LIST_ORDER_LPT") != nullptr;
+        const bool lpt_order = lpt_env || ((long)nb * p.nprobe < 64L * 3 * device_num_sms());
+        PairWork pw = carve_pair_work(w + p.off_pair, nb, p.nprobe, nlist);
+        a.order = pw.order; a.n_items = pw.n_items; a.item_counter = pw.item_counter; a.n_pairs = pw.n_pairs;
+        auto scan_piece = [&](const int* len, const void* vecs, const int64_t* data) {
+            launch_pair_setup(cI, nb, p.nprobe, nlist, len, lpt_order ? h->list_rank : nullptr, pw, st, 0, false);
+            a.list_len = len;
+            launch_ivfflat_scan(a, qb, vecs, data, h->elem_bytes(), h->d, nb, st, h->sq, h->by_residual);
+            h->launches += 4;
+        };
+        if (h->ivf_dev_rows > 0) scan_piece(h->dev_len, h->payload, h->list_slot_off);   // the device lists, in place
+        CU(cudaEventSynchronize(h->flags_ready));
+        runs.clear();
+        int nchunks = 0;
+        int64_t used = stage_rows;
+        for (int l = 0; l < nlist; ++l) { chunk_of[l] = -1; stage_off[l] = 0; }
+        for (int l = h->l_dev; l < nlist; ++l) {
+            if (!hflags[l]) continue;
+            const int64_t len = h->ivf_len[l], host_row = h->ivf_off[l] - h->ivf_dev_rows;
+            if (used + len > stage_rows) { ++nchunks; used = 0; }
+            chunk_of[l] = nchunks - 1;
+            stage_off[l] = used;
+            Run* last = runs.empty() ? nullptr : &runs.back();
+            if (last && last->chunk == nchunks - 1 && last->host_row + last->rows == host_row) last->rows += len;
+            else runs.push_back(Run{nchunks - 1, host_row, used, len});
+            used += len;
+        }
+        if (nchunks > 0) {
+            // on the copy stream, ahead of the chunks: an H2D on `st` would queue behind the device-piece scan and
+            // hold up the chunk copies behind it on the copy engine.  st reads it after waiting for stage_ready.
+            CU(cudaMemcpyAsync(dtab, stage_off, (size_t)nlist * 12, cudaMemcpyHostToDevice, h->copy_st));
+            for (int c = 0; c < std::min(2, nchunks); ++c) RSB_TRY(copy_chunk(c));
+            for (int c = 0; c < nchunks; ++c) {
+                CU(cudaStreamWaitEvent(st, h->stage_ready[c & 1], 0));
+                launch_ivf_piece_tables(h->list_len, dtab, reinterpret_cast<const int*>(dtab + nlist), nlist, c, plen,
+                                        pdata, st);
+                scan_piece(plen, stage[c & 1], pdata);
+                CU(cudaEventRecord(h->stage_free[c & 1], st));
+                if (c + 2 < nchunks) {
+                    CU(cudaStreamWaitEvent(h->copy_st, h->stage_free[c & 1], 0));
+                    RSB_TRY(copy_chunk(c + 2));
+                }
+            }
+        }
+        launch_merge_items(a.out_keys, a.out_cnt, nb, p.nprobe, k, k, h->ids_slots, 0, D + (size_t)q0 * k,
+                           I + (size_t)q0 * k, st);
+        h->launches += 3;
+        CHECK_LAUNCH();
+    }
+    CU(cudaEventRecord(h->copy_done, h->copy_st));   // join the copy stream back to the caller's
+    CU(cudaStreamWaitEvent(st, h->copy_done, 0));
+    return RSB_OK;
+}
+
 // shared: the multi-GPU threshold exchange, or nullptr for thresholds kept in the workspace
 static int search_impl(rsb_index_t* h, const float* q, int nq, int k, int nprobe, const int64_t* pre_lists,
                        const float* pre_dis, float* D, int64_t* I, void* ws, size_t ws_bytes, rsb_stream_t stream,
@@ -1305,6 +1698,10 @@ static int search_impl(rsb_index_t* h, const float* q, int nq, int k, int nprobe
     }
 
     if (nprobe <= 0) return fail(RSB_ERR_INVALID, "nprobe must be > 0, got %d", nprobe);
+    RSB_TRY(ivf_check_complete(h));
+    if (h->ivf_reserved && shared)
+        return fail(RSB_ERR_UNSUPPORTED, "shared thresholds (a multi-GPU partition) are not implemented for an IVFFLAT "
+                                         "index with reserved, tiered lists");
     const SearchPlan p = search_plan(h, nq, k, nprobe);
     if (ws_bytes < p.total) return fail(RSB_ERR_OOM, "workspace too small: need %zu bytes, got %zu", p.total, ws_bytes);
     unsigned char* w = static_cast<unsigned char*>(ws);
@@ -1316,6 +1713,19 @@ static int search_impl(rsb_index_t* h, const float* q, int nq, int k, int nprobe
         CU(cudaMemcpyAsync(D, dpad.data(), dpad.size() * 4, cudaMemcpyHostToDevice, st));
         CU(cudaMemcpyAsync(I, ipad.data(), ipad.size() * 8, cudaMemcpyHostToDevice, st));
         CU(cudaStreamSynchronize(st));
+        return RSB_OK;
+    }
+    if (h->ivf_streamed()) {
+        const IvfTierPlan t = ivf_tier_plan(h, p.total);
+        if (pre_lists && p.nprobe != nprobe)
+            return fail(RSB_ERR_INVALID, "preassigned nprobe %d exceeds nlist %d", nprobe, h->nlist);
+        if (ws_bytes < t.total) return fail(RSB_ERR_OOM, "workspace too small: need %zu bytes, got %zu", t.total, ws_bytes);
+        if (h->prof) CU(cudaEventRecord(h->ev[0], st));
+        RSB_TRY(search_ivf_tiered(h, q, nq, k, p, t, pre_lists, pre_dis, D, I, w, st));
+        if (h->prof) {
+            for (int i = 1; i < 6; ++i) CU(cudaEventRecord(h->ev[i], st));
+            h->ev_done++;
+        }
         return RSB_OK;
     }
 
@@ -1391,7 +1801,9 @@ static int search_impl(rsb_index_t* h, const float* q, int nq, int k, int nprobe
                 return fail(RSB_ERR_UNSUPPORTED, "no scan kernel for %d code bytes per vector", h->Mb);
         } else {
             if (prof) CU(cudaEventRecord(h->ev[3], st));
-            launch_ivfflat_scan(a, qb, h->payload, h->elem_bytes(), h->d, nb, st, h->sq, h->by_residual);
+            if (!a.tau_external) CU(cudaMemsetAsync(a.tau, 0, (size_t)nb * 4, st));
+            CU(cudaMemsetAsync(a.out_cnt, 0, (size_t)nb * p.nprobe * 4, st));
+            launch_ivfflat_scan(a, qb, h->payload, h->list_slot_off, h->elem_bytes(), h->d, nb, st, h->sq, h->by_residual);
         }
         h->launches += paired ? 2 : 1;                 // paired work list: both scan variants, one returns at once
         if (prof) CU(cudaEventRecord(h->ev[4], st));
@@ -1737,7 +2149,8 @@ extern "C" int rsb_set_option(rsb_index_t* h, int option, int64_t value) {
             h->coarse_tensor = value != 0; h->flat_tensor = value != 0; return RSB_OK;
         case RSB_OPT_BY_RESIDUAL:
             if (!is_sq8_ivf(h)) return fail(RSB_ERR_INVALID, "RSB_OPT_BY_RESIDUAL applies to an IVFFLAT index with SQ8 storage only");
-            if (h->ntotal || h->n_staged) return fail(RSB_ERR_STATE, "by_residual cannot change once vectors are added");
+            if (h->ntotal || h->n_staged || h->ivf_reserved)
+                return fail(RSB_ERR_STATE, "by_residual cannot change once vectors are added (or lists reserved)");
             h->by_residual = value != 0; return RSB_OK;
         case RSB_OPT_DEVICE_ROWS:
             if (h->kind != RSB_FLAT)
@@ -1747,12 +2160,7 @@ extern "C" int rsb_set_option(rsb_index_t* h, int option, int64_t value) {
                                              "index stays in device memory)");
             if (h->ntotal || h->n_staged) return fail(RSB_ERR_STATE, "device_rows cannot change once vectors are added");
             if (value < 0) return fail(RSB_ERR_INVALID, "device_rows must be >= 0, got %lld", (long long)value);
-            if (!h->copy_st) {   // on the device current now, which holds the index
-                CU(cudaStreamCreateWithFlags(&h->copy_st, cudaStreamNonBlocking));
-                for (cudaEvent_t* e : {&h->stage_ready[0], &h->stage_ready[1], &h->stage_free[0], &h->stage_free[1],
-                                       &h->copy_start, &h->copy_done})
-                    CU(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
-            }
+            RSB_TRY(ensure_copy_stream(h));
             h->dev_rows = value;
             return RSB_OK;
         case RSB_OPT_STAGING_BYTES:

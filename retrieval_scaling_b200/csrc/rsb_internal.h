@@ -203,11 +203,26 @@ struct ScanArgs {
     u64* rescored;                // nullable: += vectors re-scored exactly after the quantised filter
 };
 
-// IVF-Flat: vecs [nslots, d] in CSR order, fp32 (elem_bytes 4), fp16 (elem_bytes 2) or SQ8 codes (elem_bytes 1, with
-// sq [2, d] fp32 = (vmin, vdiff); by_residual: each score is a.coarse_scores[pair] + the score of the decoded codes);
-// queries [nq, d] fp32
-void launch_ivfflat_scan(const ScanArgs& a, const float* queries, const void* vecs, int elem_bytes, int d, int nq,
-                         cudaStream_t st, const float* sq = nullptr, bool by_residual = false);
+// IVF-Flat: rows of d elements, fp32 (elem_bytes 4), fp16 (elem_bytes 2) or SQ8 codes (elem_bytes 1, with sq [2, d]
+// fp32 = (vmin, vdiff); by_residual: each score is a.coarse_scores[pair] + the score of the decoded codes); queries
+// [nq, d] fp32.  The rows of list l are vecs[list_data[l] + v] (the all-device index: list_data = a.list_off, vecs in
+// CSR order); candidate slots are a.list_off[l] + v.  The caller zeroes a.tau (unless external) and a.out_cnt before
+// the first scan of a query batch: several scans of one batch (the pieces of a tiered index) share them.
+void launch_ivfflat_scan(const ScanArgs& a, const float* queries, const void* vecs, const int64_t* list_data,
+                         int elem_bytes, int d, int nq, cudaStream_t st, const float* sq = nullptr,
+                         bool by_residual = false);
+// Tiered IVF-Flat (rsb_reserve_lists; lists [0, l_dev) in device memory, the rest in page-locked host memory).
+// flags [nlist] <- 1 for the host lists (l >= l_dev, non-empty) that a valid pair of coarse_ids [npairs] probes, else 0
+void launch_ivf_probed_flags(const int64_t* coarse_ids, int npairs, int nlist, int l_dev, const int* list_len,
+                             unsigned char* flags, cudaStream_t st);
+// a host piece: len_out[l] = list_len[l] and data_out[l] = stage_off[l] where chunk_of[l] == chunk, else 0
+void launch_ivf_piece_tables(const int* list_len, const int64_t* stage_off, const int* chunk_of, int nlist, int chunk,
+                             int* len_out, int64_t* data_out, cudaStream_t st);
+// placement of a batch sorted by list (stable): see ivf_place_rows_kernel in rsb_ivf.cu.  row_bytes % 16 == 0
+void launch_ivf_place_rows(const int32_t* sorted_list, const int64_t* sorted_src, int64_t n, const int64_t* batch_start,
+                           const int64_t* dst_base, int l_dev, int64_t host_begin, const void* src_rows,
+                           const int64_t* src_ids, int row_bytes, void* dev_rows, void* host_stage, int64_t* ids_slots,
+                           cudaStream_t st);
 
 // IVF-PQ
 void launch_pq_lut(const float* queries, int nq, int d, int M, const float* codebook_t, float* lut,

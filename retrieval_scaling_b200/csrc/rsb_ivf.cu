@@ -202,6 +202,9 @@ __device__ __forceinline__ void raise_tau(const ScanArgs& a, int q, unsigned v) 
 // loads the 4 codes of elements 4l + 128j .. +3 with one 4-byte load, decodes each with sq8_decode from vmin / vdiff
 // staged in shared memory after the query, and runs the same fmaf sequence, so scores are bit-identical to those of
 // fp32 rows holding the decoded values; by_residual adds the list's coarse score once, after the reduction).
+// The rows of list l start at row list_data[l] of `vecs`; the candidate slot (the id lookup) stays a.list_off[l] + v.
+// The all-device search passes list_data = a.list_off; a tiered index scans a staging buffer of host lists with their
+// staging offsets (launch_ivf_piece_tables).
 // =============================================================================================================
 constexpr int FS_THREADS = 256;
 constexpr int FS_WARPS = FS_THREADS / 32;
@@ -214,6 +217,7 @@ template <typename T> constexpr int fs_smem_rows() { return sizeof(T) == 1 ? 3 :
 template <typename T>
 __device__ __forceinline__ void ivfflat_scan_body(ScanArgs a, const float* __restrict__ queries,
                                                   const T* __restrict__ vecs, int d, int cap,
+                                                  const int64_t* __restrict__ list_data,
                                                   const float* __restrict__ sq, int by_residual) {
     constexpr bool SQ8 = sizeof(T) == 1;
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -245,13 +249,14 @@ __device__ __forceinline__ void ivfflat_scan_body(ScanArgs a, const float* __res
         __syncthreads();
         const int len = a.list_len[list];
         const int64_t base = a.list_off[list];
+        const int64_t dbase = list_data[list];
         [[maybe_unused]] const float coarse = SQ8 && by_residual ? a.coarse_scores[pair] : 0.f;
         const int n_iter = (len + 2 * FS_WARPS - 1) / (2 * FS_WARPS);
         for (int it = 0; it < n_iter; ++it) {
             const int v0 = (it * FS_WARPS + warp) * 2, v1 = v0 + 1;
             const bool ok0 = v0 < len, ok1 = v1 < len;
-            const T* p0 = vecs + (size_t)(base + (ok0 ? v0 : 0)) * d;
-            const T* p1 = vecs + (size_t)(base + (ok1 ? v1 : 0)) * d;
+            const T* p0 = vecs + (size_t)(dbase + (ok0 ? v0 : 0)) * d;
+            const T* p1 = vecs + (size_t)(dbase + (ok1 ? v1 : 0)) * d;
             float a0 = 0.f, a1 = 0.f;
 #pragma unroll 6
             for (int c = lane * 4; c < d; c += 128) {
@@ -306,22 +311,24 @@ __device__ __forceinline__ void ivfflat_scan_body(ScanArgs a, const float* __res
 
 template <typename T>
 __global__ __launch_bounds__(FS_THREADS)
-void ivfflat_scan_kernel(ScanArgs a, const float* __restrict__ queries, const T* __restrict__ vecs, int d, int cap) {
-    ivfflat_scan_body<T>(a, queries, vecs, d, cap, nullptr, 0);
+void ivfflat_scan_kernel(ScanArgs a, const float* __restrict__ queries, const T* __restrict__ vecs, int d, int cap,
+                         const int64_t* __restrict__ list_data) {
+    ivfflat_scan_body<T>(a, queries, vecs, d, cap, list_data, nullptr, 0);
 }
 
 // SQ8 codes: sq [2, d] = (vmin, vdiff); by_residual != 0 adds a.coarse_scores[pair] to every score of the pair
 __global__ __launch_bounds__(FS_THREADS)
 void ivfflat_scan_sq8_kernel(ScanArgs a, const float* __restrict__ queries, const uint8_t* __restrict__ vecs, int d,
-                             int cap, const float* __restrict__ sq, int by_residual) {
-    ivfflat_scan_body<uint8_t>(a, queries, vecs, d, cap, sq, by_residual);
+                             int cap, const int64_t* __restrict__ list_data, const float* __restrict__ sq, int by_residual) {
+    ivfflat_scan_body<uint8_t>(a, queries, vecs, d, cap, list_data, sq, by_residual);
 }
 
 static int num_sms() { return device_num_sms(); }
 
 template <typename T, typename... Extra>
-static void launch_ivfflat_scan_t(void (*kernel)(ScanArgs, const float*, const T*, int, int, Extra...), const ScanArgs& a,
-                                  const float* queries, const T* vecs, int d, int npairs, cudaStream_t st, Extra... extra) {
+static void launch_ivfflat_scan_t(void (*kernel)(ScanArgs, const float*, const T*, int, int, const int64_t*, Extra...),
+                                  const ScanArgs& a, const float* queries, const T* vecs, int d, int npairs,
+                                  const int64_t* list_data, cudaStream_t st, Extra... extra) {
     const int cap = cand_capacity(a.k, FS_SLACK);
     const size_t smem = (((size_t)d * 4 * fs_smem_rows<T>() + 15) & ~(size_t)15) + (size_t)cap * 8;
     cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -329,21 +336,89 @@ static void launch_ivfflat_scan_t(void (*kernel)(ScanArgs, const float*, const T
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, FS_THREADS, smem);
     if (occ < 1) occ = 1;
     const int grid = min(npairs, num_sms() * occ);
-    kernel<<<grid, FS_THREADS, smem, st>>>(a, queries, vecs, d, cap, extra...);
+    kernel<<<grid, FS_THREADS, smem, st>>>(a, queries, vecs, d, cap, list_data, extra...);
 }
 
-void launch_ivfflat_scan(const ScanArgs& a, const float* queries, const void* vecs, int elem_bytes, int d, int nq,
-                         cudaStream_t st, const float* sq, bool by_residual) {
+void launch_ivfflat_scan(const ScanArgs& a, const float* queries, const void* vecs, const int64_t* list_data,
+                         int elem_bytes, int d, int nq, cudaStream_t st, const float* sq, bool by_residual) {
     const int npairs = nq * a.nprobe;
-    if (!a.tau_external) cudaMemsetAsync(a.tau, 0, (size_t)nq * 4, st);
-    cudaMemsetAsync(a.out_cnt, 0, (size_t)npairs * 4, st);
     if (npairs == 0) return;
     if (elem_bytes == 1)
-        launch_ivfflat_scan_t(ivfflat_scan_sq8_kernel, a, queries, static_cast<const uint8_t*>(vecs), d, npairs, st, sq,
-                              by_residual ? 1 : 0);
+        launch_ivfflat_scan_t(ivfflat_scan_sq8_kernel, a, queries, static_cast<const uint8_t*>(vecs), d, npairs,
+                              list_data, st, sq, by_residual ? 1 : 0);
     else if (elem_bytes == 2)
-        launch_ivfflat_scan_t(ivfflat_scan_kernel<__half>, a, queries, static_cast<const __half*>(vecs), d, npairs, st);
-    else launch_ivfflat_scan_t(ivfflat_scan_kernel<float>, a, queries, static_cast<const float*>(vecs), d, npairs, st);
+        launch_ivfflat_scan_t(ivfflat_scan_kernel<__half>, a, queries, static_cast<const __half*>(vecs), d, npairs,
+                              list_data, st);
+    else launch_ivfflat_scan_t(ivfflat_scan_kernel<float>, a, queries, static_cast<const float*>(vecs), d, npairs,
+                               list_data, st);
+}
+
+// ---- tiered IVF-Flat (rsb_reserve_lists) -------------------------------------------------------------------
+// flags[l] = 1 for every list l >= l_dev that a valid pair of the batch probes (flags zeroed by the caller)
+__global__ void ivf_probed_flags_kernel(const int64_t* __restrict__ coarse_ids, int npairs, int nlist, int l_dev,
+                                        const int* __restrict__ list_len, unsigned char* __restrict__ flags) {
+    for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < npairs; p += gridDim.x * blockDim.x) {
+        const int64_t l = coarse_ids[p];
+        if (l >= l_dev && l < nlist && list_len[l] > 0) flags[l] = 1;
+    }
+}
+void launch_ivf_probed_flags(const int64_t* coarse_ids, int npairs, int nlist, int l_dev, const int* list_len,
+                             unsigned char* flags, cudaStream_t st) {
+    cudaMemsetAsync(flags, 0, (size_t)nlist, st);
+    if (npairs <= 0) return;
+    ivf_probed_flags_kernel<<<std::min(1024, (npairs + 255) / 256), 256, 0, st>>>(coarse_ids, npairs, nlist, l_dev,
+                                                                                  list_len, flags);
+}
+
+// piece `chunk` of the host lists: list_len masked to the lists copied into that chunk, their staging row offsets
+__global__ void ivf_piece_tables_kernel(const int* __restrict__ list_len, const int64_t* __restrict__ stage_off,
+                                        const int* __restrict__ chunk_of, int nlist, int chunk, int* __restrict__ len_out,
+                                        int64_t* __restrict__ data_out) {
+    for (int l = blockIdx.x * blockDim.x + threadIdx.x; l < nlist; l += gridDim.x * blockDim.x) {
+        const bool in = chunk_of[l] == chunk;
+        len_out[l] = in ? list_len[l] : 0;
+        data_out[l] = in ? stage_off[l] : 0;
+    }
+}
+void launch_ivf_piece_tables(const int* list_len, const int64_t* stage_off, const int* chunk_of, int nlist, int chunk,
+                             int* len_out, int64_t* data_out, cudaStream_t st) {
+    ivf_piece_tables_kernel<<<(nlist + 255) / 256, 256, 0, st>>>(list_len, stage_off, chunk_of, nlist, chunk, len_out,
+                                                                  data_out);
+}
+
+// Build of a reserved index: the i-th row of the batch in list order (sorted_src[i], list sorted_list[i]) goes to slot
+// dst_base[l] + (i - batch_start[l]).  Its id goes to ids_slots[slot]; its row to dev_rows[slot] when the slot is in the
+// device tier (l < l_dev), else to host_stage[i - host_begin] (the batch's host-tier rows, in list order, for the
+// copies to the host tier).  row_bytes % 16 == 0.
+__global__ void ivf_place_rows_kernel(const int32_t* __restrict__ sorted_list, const int64_t* __restrict__ sorted_src,
+                                      int64_t n, const int64_t* __restrict__ batch_start,
+                                      const int64_t* __restrict__ dst_base, int l_dev, int64_t host_begin,
+                                      const uint4* __restrict__ src_rows, const int64_t* __restrict__ src_ids,
+                                      int row_words, uint4* __restrict__ dev_rows, uint4* __restrict__ host_stage,
+                                      int64_t* __restrict__ ids_slots) {
+    const int64_t total = n * row_words;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t i = e / row_words;
+        const int w = (int)(e - i * row_words);
+        const int l = sorted_list[i];
+        const int64_t src = sorted_src[i];
+        const int64_t slot = dst_base[l] + (i - batch_start[l]);
+        if (w == 0) ids_slots[slot] = src_ids[src];
+        const uint4 v = src_rows[src * row_words + w];
+        if (l < l_dev) dev_rows[slot * row_words + w] = v;
+        else host_stage[(i - host_begin) * row_words + w] = v;
+    }
+}
+void launch_ivf_place_rows(const int32_t* sorted_list, const int64_t* sorted_src, int64_t n, const int64_t* batch_start,
+                           const int64_t* dst_base, int l_dev, int64_t host_begin, const void* src_rows,
+                           const int64_t* src_ids, int row_bytes, void* dev_rows, void* host_stage, int64_t* ids_slots,
+                           cudaStream_t st) {
+    if (n <= 0) return;
+    const int w = row_bytes / 16;
+    const int64_t total = n * w;
+    ivf_place_rows_kernel<<<(int)std::min<int64_t>(8192, (total + 255) / 256), 256, 0, st>>>(
+        sorted_list, sorted_src, n, batch_start, dst_base, l_dev, host_begin, static_cast<const uint4*>(src_rows),
+        src_ids, w, static_cast<uint4*>(dev_rows), static_cast<uint4*>(host_stage), ids_slots);
 }
 
 // =============================================================================================================

@@ -170,7 +170,11 @@ class ShardedSearcher:
                  search_fn: Optional[Callable] = None, merge_fn: Optional[Callable] = None,
                  shard_coarse: bool = True, fused_gather: bool = True, sliced_merge: bool = True,
                  share_tau: bool = True, peer_coarse: bool = True):
-        from .index import IndexFlatIP, IndexIVFScalarQuantizer, IndexRefine
+        from .index import IndexFlatIP, IndexIVFScalarQuantizer, IndexRefine, _IVFBase
+        if isinstance(index, _IVFBase) and index.tiered:
+            raise NotImplementedError("ShardedSearcher does not search a tiered IVF index (list_device_rows: lists in host "
+                                      "memory): search it per shard group (search.GroupSearcher) or with index.search "
+                                      "on one GPU")
         if isinstance(index, IndexFlatIP) and index.tiered:
             raise NotImplementedError("ShardedSearcher does not search a tiered Flat index (rows in host memory): search "
                                       "it per shard group (search.GroupSearcher) or with index.search on one GPU")

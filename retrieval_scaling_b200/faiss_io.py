@@ -151,6 +151,65 @@ def _read_invlists(f: BinaryIO, nlist_expected: int, tag_bytes: bytes = None):
     return code_size, offsets, codes, ids
 
 
+def ivf_lists_memmap(path: str):
+    """An IwFl / IwSq file without its payload: (meta, offsets [nlist + 1], read_lists), where meta holds the parts of
+    read_faiss except the codes / vectors and ids, and read_lists(l0, l1) -> (codes uint8 [rows, code_size], ids int64
+    [rows]) of lists [l0, l1), read from a memory map of the file: an index larger than host memory is loaded list
+    range by list range."""
+    with open(path, "rb") as f:
+        tag = _fourcc_str(_rd(f, "I"))
+        if tag not in ("IwFl", "IwSq", "IwSQ"):
+            raise ValueError(f"{path} is not a faiss IVF-Flat (IwFl) or IVF-SQ8 (IwSq) file, it is {tag!r}")
+        h = _read_ivf_header(f)
+        if tag == "IwFl":
+            peek = f.read(4)
+            if peek not in (b"ilar", b"il00"):           # the redundant code_size of early files (see read_faiss)
+                f.read(4)
+            else:
+                f.seek(-4, 1)
+            meta, code_size = {"kind": "IVFFlat", **h}, h["d"] * 4
+        else:
+            sq = _read_scalar_quantizer(f, h["d"])
+            code_size = _rd(f, "Q")
+            by_residual = bool(_rd(f, "B")) if tag == "IwSq" else True
+            meta = {"kind": "IVFSQ", **h, "by_residual": by_residual, "sq": sq}
+        tag = _fourcc_str(_rd(f, "I"))
+        if tag != "ilar":
+            raise NotImplementedError(f"inverted-list container {tag!r} is not supported (only ArrayInvertedLists 'ilar')")
+        nlist, cs = _rd(f, "Q"), _rd(f, "Q")
+        if nlist != h["nlist"] or cs != code_size:
+            raise ValueError("inverted lists disagree with the IVF header on nlist or code_size")
+        ltype = _fourcc_str(_rd(f, "I"))
+        sizes = np.zeros(nlist, dtype=np.int64)
+        n = _rd(f, "Q")
+        if ltype == "full":
+            sizes[:] = _rd_array(f, np.uint64, n).astype(np.int64)
+        elif ltype == "sprs":
+            pairs = _rd_array(f, np.uint64, n).astype(np.int64).reshape(-1, 2)
+            sizes[pairs[:, 0]] = pairs[:, 1]
+        else:
+            raise NotImplementedError(f"inverted-list size encoding {ltype!r}")
+        start = f.tell()
+    offsets = np.zeros(nlist + 1, dtype=np.int64)
+    np.cumsum(sizes, out=offsets[1:])
+    pos = start + offsets[:-1] * (code_size + 8)        # list l: codes [size, code_size], then ids [size]
+    mm = np.memmap(path, dtype=np.uint8, mode="r") if offsets[-1] else None
+
+    def read_lists(l0: int, l1: int):
+        rows = int(offsets[l1] - offsets[l0])
+        codes = np.empty((rows, code_size), dtype=np.uint8)
+        ids = np.empty(rows, dtype=np.int64)
+        for l in range(l0, l1):
+            s, a = int(sizes[l]), int(offsets[l] - offsets[l0])
+            if s:
+                p = int(pos[l])
+                codes[a:a + s] = mm[p:p + s * code_size].reshape(s, code_size)
+                ids[a:a + s] = mm[p + s * code_size:p + s * (code_size + 8)].view(np.int64)
+        return codes, ids
+
+    return meta, offsets, read_lists
+
+
 def _read_ivf_header(f: BinaryIO) -> Dict:
     hdr = _read_header(f)
     nlist = _rd(f, "Q")
@@ -338,6 +397,64 @@ def _write_invlists(f: BinaryIO, nlist: int, code_size: int, offsets: np.ndarray
         if b > a:
             f.write(codes[a:b].tobytes())
             f.write(ids[a:b].tobytes())
+
+
+def _write_invlists_head(f: BinaryIO, nlist: int, code_size: int, offsets: np.ndarray) -> None:
+    _wr(f, "I", fourcc("ilar"))
+    _wr(f, "Q", nlist)
+    _wr(f, "Q", code_size)
+    sizes = np.diff(offsets).astype(np.uint64)
+    nonzero = np.nonzero(sizes)[0]
+    if len(nonzero) > nlist // 2:
+        _wr(f, "I", fourcc("full"))
+        _wr(f, "Q", nlist)
+        f.write(sizes.tobytes())
+    else:                                     # faiss writes the sparse form when few lists are populated
+        _wr(f, "I", fourcc("sprs"))
+        pairs = np.stack([nonzero.astype(np.uint64), sizes[nonzero]], axis=1)
+        _wr(f, "Q", pairs.size)
+        f.write(np.ascontiguousarray(pairs).tobytes())
+
+
+def _write_ivf_prefix(f: BinaryIO, parts: Dict, ntotal: int) -> int:
+    """Everything of an IVFFlat / IVFSQ file before its inverted lists; returns the code size."""
+    c = parts["centroids"]
+    d, nlist = c.shape[1], c.shape[0]
+    if parts["kind"] == "IVFFlat":
+        _write_ivf_header(f, "IwFl", d, ntotal, nlist, parts.get("nprobe", 1), c)
+        return d * 4
+    _write_ivf_header(f, "IwSq", d, ntotal, nlist, parts.get("nprobe", 1), c)
+    _write_scalar_quantizer(f, parts["sq"])
+    _wr(f, "Q", d)                            # code_size
+    _wr(f, "B", 1 if parts.get("by_residual", True) else 0)
+    return d
+
+
+def write_ivf_streamed(f: BinaryIO, parts: Dict, offsets: np.ndarray, ids: np.ndarray, rows, step_rows: int) -> None:
+    """An IVFFlat / IVFSQ file (parts without the vectors / codes) whose CSR rows come from rows(r0, r1) -> [r1 - r0,
+    d] float32 (IVFFlat) or uint8 codes (IVFSQ), called for list ranges of about step_rows rows: the bytes write_faiss
+    writes for the whole arrays, holding one range at a time."""
+    nlist = parts["centroids"].shape[0]
+    offsets = np.asarray(offsets, dtype=np.int64)
+    ids = np.ascontiguousarray(ids, dtype=np.int64)
+    code_size = _write_ivf_prefix(f, parts, len(ids))
+    _write_invlists_head(f, nlist, code_size, offsets)
+    l0 = 0
+    while l0 < nlist:
+        l1 = min(nlist, max(int(np.searchsorted(offsets, offsets[l0] + max(1, step_rows), side="right")) - 1, l0 + 1))
+        r0, r1 = int(offsets[l0]), int(offsets[l1])
+        if r1 > r0:
+            x = rows(r0, r1)
+            x = np.ascontiguousarray(x, dtype=np.float32 if parts["kind"] == "IVFFlat" else np.uint8)
+            if x.shape[0] != r1 - r0:
+                raise ValueError(f"rows({r0}, {r1}) returned {x.shape[0]} rows")
+            x = x.view(np.uint8).reshape(r1 - r0, code_size)
+            for l in range(l0, l1):
+                a, b = int(offsets[l]), int(offsets[l + 1])
+                if b > a:
+                    f.write(x[a - r0:b - r0].tobytes())
+                    f.write(ids[a:b].tobytes())
+        l0 = l1
 
 
 def _write_ivf_header(f: BinaryIO, tag: str, d: int, ntotal: int, nlist: int, nprobe: int, centroids: np.ndarray):

@@ -308,10 +308,90 @@ class IndexFlatIP(_IndexBase):
         return ids
 
 
+def _check_rows_arg(v, name: str) -> Optional[int]:
+    if v is None:
+        return None
+    if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) or v < 0:
+        raise ValueError(f"{name} must be None or an integer >= 0, got {v!r}")
+    return int(v)
+
+
 class _IVFBase(_IndexBase):
+    # tiered IVF-Flat / IVF-SQ8 (list_device_rows set): lists are split by id between device memory and page-locked host
+    # memory, which needs the list sizes before the first add (reserve_lists)
+    list_device_rows: Optional[int] = None
+    staging_bytes: Optional[int] = None
+
     def __init__(self, d, nlist, device=None):
         super().__init__(d, device)
         self.nlist = int(nlist)
+        self._reserved = False
+
+    @staticmethod
+    def _tier_args(list_device_rows, staging_bytes):
+        """Checks list_device_rows / staging_bytes before any device allocation."""
+        return _check_rows_arg(list_device_rows, "list_device_rows"), _check_rows_arg(staging_bytes, "staging_bytes")
+
+    @property
+    def tiered(self) -> bool:
+        return self.list_device_rows is not None
+
+    @property
+    def n_dev(self) -> int:
+        """Rows held in device memory: those of lists [0, L_dev) once the lists are reserved, else ntotal."""
+        return self._info(_lib.INFO_DEVICE_ROWS)
+
+    @property
+    def host_bytes(self) -> int:
+        """Page-locked host bytes of the host lists (0 unless tiered and reserved)."""
+        return self._info(_lib.INFO_HOST_BYTES)
+
+    def reserve_lists(self, sizes) -> None:
+        """Fixes the list sizes [nlist] of a tiered index before anything is added (rsb_reserve_lists): lists [0, L_dev)
+        -- the most that fit list_device_rows rows -- get their rows in device memory, the others in page-locked host
+        memory.  Every later add places its rows in their final slots; the index is searchable once every reserved row
+        has been added."""
+        if not self.tiered:
+            raise ValueError("reserve_lists splits the lists of a tiered index: construct it with list_device_rows")
+        sz = np.ascontiguousarray(np.asarray(sizes.cpu() if isinstance(sizes, torch.Tensor) else sizes), dtype=np.int64)
+        if sz.shape != (self.nlist,):
+            raise ValueError(f"sizes must be [{self.nlist}] (one size per list), got {sz.shape}")
+        with torch.cuda.device(self.device):
+            _lib.check(self.L.rsb_reserve_lists(self._h, sz.ctypes.data_as(ctypes.c_void_p), self.list_device_rows,
+                                                int(self.staging_bytes or 0), _stream()))
+        self._reserved = True
+
+    def _check_reserved(self) -> None:
+        if self.tiered and not self._reserved:
+            raise ValueError("a tiered IVF index (list_device_rows) places every row in its final slot: call "
+                             "reserve_lists(sizes) with the list sizes (e.g. counted from assign()) before adding")
+
+    def add(self, x, ids=None) -> None:
+        self._check_reserved()
+        return super().add(x, ids)
+
+    def export_rows(self, r0: int, n: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """CSR rows [r0, r0 + n) (the natural order of export_lists) in the storage dtype, from whichever tier holds
+        them, into `out` (a contiguous [n, d] CPU or CUDA tensor; default: a new CPU tensor)."""
+        dt = _REFINE_DTYPES[self.dtype][0]
+        if out is None:
+            out = torch.empty((int(n), self.d), dtype=dt)
+        if tuple(out.shape) != (int(n), self.d) or out.dtype != dt or not out.is_contiguous():
+            raise ValueError(f"out must be a contiguous [{n}, {self.d}] {self.dtype} tensor")
+        with torch.cuda.device(self.device):
+            _lib.check(self.L.rsb_export_rows(self._h, int(r0), int(n), _ptr(out), _stream()))
+            torch.cuda.current_stream().synchronize()
+        return out
+
+    def export_ids_host(self) -> np.ndarray:
+        """The ids of CSR rows [0, ntotal) as a host int64 array."""
+        with torch.cuda.device(self.device):
+            self.finalize()
+            n = self.ntotal
+            ids = torch.empty(n, dtype=torch.int64, device=self.device if not self._reserved else "cpu")
+            _lib.check(self.L.rsb_export_lists(self._h, None, None, _ptr(ids), _stream()))
+            torch.cuda.current_stream().synchronize()
+        return ids.cpu().numpy()
 
     # trained state ------------------------------------------------------------------------------------------
     def set_centroids(self, c) -> None:
@@ -366,6 +446,7 @@ class _IVFBase(_IndexBase):
         return lists[:, 0].to(torch.int32)
 
     def add_preassigned(self, x, lists, ids=None) -> None:
+        self._check_reserved()
         with torch.cuda.device(self.device):
             x = _dev_f32(x, self.device) if self.kind == _lib.RSB_IVFPQ else _dev_rows(x, self.device)
             n = x.shape[0]
@@ -390,12 +471,22 @@ class IndexIVFFlat(_IVFBase):
     """faiss.IndexIVFFlat(IndexFlatIP(d), d, nlist, METRIC_INNER_PRODUCT)  (src/indicies/ivf_flat.py:143-149).
 
     dtype="float16" stores the vectors as fp16 (faiss IndexIVFScalarQuantizer(QT_fp16, by_residual=False)): the list
-    scan reads half the bytes, and ids and scores are bit-identical to an fp32 index holding the same values."""
+    scan reads half the bytes, and ids and scores are bit-identical to an fp32 index holding the same values.
+
+    list_device_rows = R (an integer) makes the index tiered by list, for datastores larger than device memory: after
+    reserve_lists(sizes), lists [0, L_dev) -- the most whose rows fit R -- keep their rows in device memory and the
+    others in page-locked host memory the index owns.  A search scans the device lists in place and copies only the
+    probed host lists through two device staging buffers of `staging_bytes` each (None: the library's 256 MiB); ids and
+    scores equal those of the all-device index of the same lists.  add / add_preassigned need the reservation first."""
     kind = _lib.RSB_IVFFLAT
 
-    def __init__(self, d: int, nlist: int, device=None, dtype: str = "float32"):
+    def __init__(self, d: int, nlist: int, device=None, dtype: str = "float32", list_device_rows: Optional[int] = None,
+                 staging_bytes: Optional[int] = None):
+        dtype = _check_dtype(dtype)
+        tier = self._tier_args(list_device_rows, staging_bytes)        # before any device allocation
         super().__init__(d, nlist, device)
-        self.dtype = _check_dtype(dtype)
+        self.list_device_rows, self.staging_bytes = tier
+        self.dtype = dtype
         with torch.cuda.device(self.device):
             _lib.check(self.L.rsb_ivfflat_create(self.d, self.nlist, _STORE_DTYPES[self.dtype][1],
                                                  ctypes.byref(self._h)))
@@ -469,14 +560,18 @@ class IndexIVFScalarQuantizer(_IVFBase):
     encodes x and scores s.  s = <q, decode(code)> is accumulated in the fp32 IVF-Flat scan's order from the decoded
     elements vmin + ((c + 0.5f) / 255.f) * vdiff, so it is bit-identical to an fp32 IndexIVFFlat holding the decoded
     rows in the same lists.  train(x) trains the coarse quantizer (as IndexIVFFlat.train) and then the range on the rows
-    or on their residuals against the lists add() would assign; train_sq(x) trains the range alone."""
+    or on their residuals against the lists add() would assign; train_sq(x) trains the range alone.
+    list_device_rows / staging_bytes tier the lists between device and host memory as in IndexIVFFlat."""
     kind = _lib.RSB_IVFFLAT
     dtype = "sq8"
     qtype = "QT_8bit"                   # the only scalar-quantizer type implemented
     _TRAIN_CHUNK = 65536                # rows per coarse assignment while the residuals are formed
 
-    def __init__(self, d: int, nlist: int, by_residual: bool = True, device=None):
+    def __init__(self, d: int, nlist: int, by_residual: bool = True, device=None,
+                 list_device_rows: Optional[int] = None, staging_bytes: Optional[int] = None):
+        tier = self._tier_args(list_device_rows, staging_bytes)        # before any device allocation
         super().__init__(d, nlist, device)
+        self.list_device_rows, self.staging_bytes = tier
         with torch.cuda.device(self.device):
             _lib.check(self.L.rsb_ivfflat_create(self.d, self.nlist, _lib.RSB_DTYPE_SQ8, ctypes.byref(self._h)))
         self.set_option(_lib.OPT_BY_RESIDUAL, 1 if by_residual else 0)
@@ -536,6 +631,7 @@ class IndexIVFScalarQuantizer(_IVFBase):
 
     def add_codes(self, codes, lists, ids=None) -> None:
         """Adds SQ8 codes [n, d] uint8 of this index's range (residual codes when by_residual) to the given lists."""
+        self._check_reserved()
         with torch.cuda.device(self.device):
             ct = torch.as_tensor(codes).to(device=self.device, dtype=torch.uint8).contiguous()
             if ct.dim() != 2 or ct.shape[1] != self.d:
@@ -1015,6 +1111,80 @@ def _read_flat_tiered(path: str, device, storage_dtype: Optional[str], device_ro
     return index
 
 
+def _write_ivf_tiered(index: "_IVFBase", path: str, fmt: str) -> None:
+    """A tiered IVF-Flat / IVF-SQ8 index written list range by list range (rsb_export_rows): the bytes the all-device
+    index of the same lists writes (fp16 rows upcast to fp32 a range at a time), with host memory bounded by the ids and
+    one range beyond the tiers."""
+    from . import faiss_io
+    if fmt != "faiss":
+        raise NotImplementedError("a tiered IVF index (list_device_rows) is written in the faiss format (IwFl / IwSq) "
+                                  "only, not the RSB1 container")
+    sizes = index.list_sizes().cpu().numpy()
+    off = np.zeros(index.nlist + 1, dtype=np.int64)
+    np.cumsum(sizes, out=off[1:])
+    ids = index.export_ids_host() if off[-1] else np.zeros(0, np.int64)
+    parts = {"centroids": index.get_centroids().cpu().numpy(), "nprobe": int(index.nprobe)}
+    if isinstance(index, IndexIVFScalarQuantizer):
+        parts.update(kind="IVFSQ", sq=torch.stack(index.sq_params).cpu().numpy(), by_residual=index.by_residual)
+    else:
+        parts.update(kind="IVFFlat")
+
+    def rows(r0: int, r1: int) -> np.ndarray:
+        x = index.export_rows(r0, r1 - r0).numpy()
+        return x.astype(np.float32) if x.dtype == np.float16 else x
+
+    tmp = path + ".tmp"
+    with open(tmp, "wb") as f:
+        faiss_io.write_ivf_streamed(f, parts, off, ids, rows, _ROW_CHUNK_BYTES // (4 * index.d))
+    os.replace(tmp, path)
+
+
+def _read_ivf_tiered(path: str, device, storage_dtype: Optional[str], list_device_rows: int,
+                     staging_bytes: Optional[int] = None) -> "_IVFBase":
+    """An IwFl / IwSq file into a tiered index: the list sizes are read first and reserved, then the lists are added
+    a range at a time from a memory map of the payload, with their ids and within-list order."""
+    from . import faiss_io
+    if not faiss_io.is_faiss_file(path):
+        raise NotImplementedError("list_device_rows reads IVF-Flat / IVF-SQ8 indexes in the faiss format (IwFl / IwSq); "
+                                  "an RSB1 container cannot be read into a tiered index")
+    meta, off, read_lists = faiss_io.ivf_lists_memmap(path)
+    if meta["metric"] != 0 or meta.get("quantizer_metric", 0) != 0:
+        raise NotImplementedError("only METRIC_INNER_PRODUCT indexes are supported (the reference builds IP indexes only)")
+    nlist, d = meta["nlist"], meta["d"]
+    if meta["kind"] == "IVFSQ":
+        _check_sq8_storage(True, storage_dtype)
+        index = IndexIVFScalarQuantizer(d, nlist, by_residual=bool(meta["by_residual"]), device=device,
+                                        list_device_rows=list_device_rows, staging_bytes=staging_bytes)
+        index.set_centroids(meta["centroids"])
+        index.sq_params = meta["sq"]
+    else:
+        _check_sq8_storage(False, storage_dtype)
+        dtype = _check_dtype(storage_dtype or "float32", "storage_dtype")
+        index = IndexIVFFlat(d, nlist, device, dtype=dtype, list_device_rows=list_device_rows,
+                             staging_bytes=staging_bytes)
+        index.set_centroids(meta["centroids"])
+    index.nprobe = int(meta.get("nprobe", 1))
+    sizes = np.diff(off)
+    if off[-1] == 0:                 # nothing to place: the index stays unreserved, as a freshly trained one
+        return index
+    index.reserve_lists(sizes)
+    step = max(1, _ROW_CHUNK_BYTES // (4 * d))
+    l0 = 0
+    while l0 < nlist:                # list ranges of about `step` rows (one list when a list is longer)
+        l1 = int(np.searchsorted(off, off[l0] + step, side="right")) - 1
+        l1 = min(nlist, max(l1, l0 + 1))
+        if off[l1] > off[l0]:
+            codes, ids = read_lists(l0, l1)
+            lists = np.repeat(np.arange(l0, l1, dtype=np.int32), sizes[l0:l1])
+            if meta["kind"] == "IVFSQ":
+                index.add_codes(codes, lists, ids)
+            else:
+                xb = _as_storage(codes.view(np.float32).reshape(-1, d), index.dtype, f"{path}: the IVFFlat index's vectors")
+                index.add_preassigned(xb, lists, ids)
+        l0 = l1
+    return index
+
+
 def write_index(index: _IndexBase, path: str, fmt: Optional[str] = None) -> None:
     """fmt "faiss" (default; env RSB_INDEX_FORMAT overrides: faiss 1.8 binary layout, see faiss_io.py) or "rsb1"."""
     fmt = (fmt or os.environ.get("RSB_INDEX_FORMAT", "faiss")).lower()
@@ -1022,6 +1192,8 @@ def write_index(index: _IndexBase, path: str, fmt: Optional[str] = None) -> None
         raise ValueError(f"unknown index file format {fmt!r} (faiss | rsb1)")
     if isinstance(index, IndexFlatIP) and index.tiered:
         return _write_flat_tiered(index, path, fmt)
+    if isinstance(index, _IVFBase) and index.tiered:
+        return _write_ivf_tiered(index, path, fmt)
     if isinstance(index, IndexRefine) and fmt != "faiss":
         raise ValueError("an IndexRefine is written in faiss' IndexRefineFlat layout only (fmt='faiss')")
     if fmt == "faiss":
@@ -1070,7 +1242,8 @@ def write_index(index: _IndexBase, path: str, fmt: Optional[str] = None) -> None
 
 
 def read_index(path: str, device=None, refine_dtype: Optional[str] = None,
-               storage_dtype: Optional[str] = None, device_rows: Optional[int] = None) -> _IndexBase:
+               storage_dtype: Optional[str] = None, device_rows: Optional[int] = None,
+               list_device_rows: Optional[int] = None) -> _IndexBase:
     """Loads an RSB1 container or a faiss binary index file (auto-detected by its fourcc).  For an IndexRefineFlat
     file (IxRF) `refine_dtype` picks the store: "float32" (default) or "float16", which is accepted only when every
     stored value round-trips through fp16 (ValueError otherwise).  An IxRF file whose refine index is an 8-bit scalar
@@ -1079,9 +1252,17 @@ def read_index(path: str, device=None, refine_dtype: Optional[str] = None,
     (IwSq / IwSQ, or RSB1 with dtype sq8) loads as an IndexIVFScalarQuantizer with its codes and range as stored
     (storage_dtype None or "sq8"); "sq8" on a float index and float16 / float32 on an SQ8 index raise ValueError.
     device_rows = n loads a Flat index (IxFI or RSB1) as a tiered IndexFlatIP (storage_dtype "float16" only, else
-    ValueError), filling the tiers a chunk at a time from a memory map of the faiss payload."""
+    ValueError), filling the tiers a chunk at a time from a memory map of the faiss payload.
+    list_device_rows = R loads an IVF-Flat or IVF-SQ8 index (IwFl / IwSq) as a tiered index (see IndexIVFFlat): the list
+    sizes are reserved first, then the lists are filled from a memory map of the payload; RSB1 files raise
+    NotImplementedError."""
     from . import faiss_io
     device_rows = _check_device_rows(device_rows)
+    list_device_rows = _check_rows_arg(list_device_rows, "list_device_rows")
+    if list_device_rows is not None:
+        if device_rows is not None:
+            raise ValueError("device_rows tiers a Flat index, list_device_rows an IVF index: give one of them")
+        return _read_ivf_tiered(path, device, storage_dtype, list_device_rows)
     if device_rows is not None:
         return _read_flat_tiered(path, device, storage_dtype, device_rows)
     if faiss_io.is_faiss_file(path):

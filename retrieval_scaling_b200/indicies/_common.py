@@ -78,7 +78,7 @@ class BaseIndexer:
 
     def __init__(self, embed_paths, index_path, meta_file, passage_dir=None, pos_map_save_path=None,
                  dimension=768, trained_index_path=None, sample_train_size=1000000, probe=1, storage_dtype=None,
-                 device_rows=None):
+                 device_rows=None, list_device_rows=None):
         self.embed_paths = list(embed_paths) if embed_paths is not None else []
         self.index_path, self.meta_file = index_path, meta_file
         self.trained_index_path = trained_index_path
@@ -89,17 +89,20 @@ class BaseIndexer:
         self.storage_dtype = storage_dtype
         # datastore.index.device_rows (Flat, float16): None = every row in device memory, else a tiered index
         self.device_rows = device_rows
+        # datastore.index.list_device_rows (IVFFlat): None = every list in device memory, else a tiered IVF index
+        self.list_device_rows = list_device_rows
+        tier = {} if list_device_rows is None else {"list_device_rows": list_device_rows}
 
         if os.path.exists(index_path) and os.path.exists(meta_file):
             print("Loading index...")
-            self.index = rsb_index.read_index(index_path, storage_dtype=storage_dtype, device_rows=device_rows)
+            self.index = rsb_index.read_index(index_path, storage_dtype=storage_dtype, device_rows=device_rows, **tier)
             self.index_id_to_db_id = DbIdMap.load(meta_file)
         else:
             self.index_id_to_db_id = DbIdMap()
             self.index = self._new_index()
             if not self.index.is_trained:
                 if trained_index_path and os.path.exists(trained_index_path):
-                    self.index = rsb_index.read_index(trained_index_path, storage_dtype=storage_dtype)
+                    self.index = rsb_index.read_index(trained_index_path, storage_dtype=storage_dtype, **tier)
                 else:
                     print("Training index...")
                     self._sample_and_train_index()
@@ -132,12 +135,40 @@ class BaseIndexer:
 
     def _add_keys(self) -> None:
         t0 = time.time()
+        if self.list_device_rows is not None:
+            return self._add_keys_tiered(t0)
         for i, p in enumerate(self.embed_paths):
             shard_id = iu.shard_id_of_embedding_path(p)
             emb = self._load_shard_for_add(p)
             self.index.add(emb)
             self.index_id_to_db_id.extend_shard(shard_id, emb.shape[0])
             print("Added %d / %d shards, (%d min)" % (i + 1, len(self.embed_paths), (time.time() - t0) / 60))
+        self._save(t0)
+
+    def _add_keys_tiered(self, t0: float) -> None:
+        """A tiered IVF index places every row in its final slot, so it learns its list sizes first: pass 1 assigns
+        each shard (the int32 lists stay on the host), then reserve_lists; pass 2 reloads each shard and adds it with
+        its kept lists."""
+        kept = []
+        sizes = np.zeros(self.index.nlist, dtype=np.int64)
+        for p in self.embed_paths:
+            emb = self._load_shard_for_add(p)
+            lists = np.concatenate([self.index.assign(emb[a:a + 65536]).cpu().numpy()
+                                    for a in range(0, emb.shape[0], 65536)]) if emb.shape[0] else np.zeros(0, np.int32)
+            sizes += np.bincount(lists, minlength=self.index.nlist)
+            kept.append(lists)
+        self.index.reserve_lists(sizes)
+        print("Reserved %d lists, %d rows in device memory (%d min)" % (self.index.nlist, self.index.n_dev,
+                                                                        (time.time() - t0) / 60))
+        for i, (p, lists) in enumerate(zip(self.embed_paths, kept)):
+            shard_id = iu.shard_id_of_embedding_path(p)
+            emb = self._load_shard_for_add(p)
+            self.index.add_preassigned(emb, lists)
+            self.index_id_to_db_id.extend_shard(shard_id, emb.shape[0])
+            print("Added %d / %d shards, (%d min)" % (i + 1, len(self.embed_paths), (time.time() - t0) / 60))
+        self._save(t0)
+
+    def _save(self, t0: float) -> None:
         self.index.finalize()
         os.makedirs(os.path.dirname(self.index_path) or ".", exist_ok=True)
         rsb_index.write_index(self.index, self.index_path)

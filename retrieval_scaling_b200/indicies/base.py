@@ -94,6 +94,22 @@ class Indexer(object):
                              f"{index_cfg.get('storage_dtype', None)})")
         return rows
 
+    @staticmethod
+    def list_device_rows(index_cfg):
+        """Optional key `list_device_rows` (absent: None, every list in device memory): an integer >= 0; an IVFFlat index
+        (any storage_dtype) keeps the rows of its first lists -- as many as fit that many rows -- in device memory and the
+        others in pinned host memory, copying only the probed host lists at search time (index.IndexIVFFlat(
+        list_device_rows=...)).  Needs index_type IVFFlat."""
+        rows = index_cfg.get("list_device_rows", None)
+        if rows is None:
+            return None
+        if isinstance(rows, bool) or not isinstance(rows, int) or rows < 0:
+            raise ValueError(f"datastore.index.list_device_rows must be an integer >= 0, got {rows!r}")
+        if index_cfg.index_type != "IVFFlat":
+            raise ValueError(f"datastore.index.list_device_rows splits the inverted lists of an IVFFlat index between "
+                             f"device and host memory: it needs index_type IVFFlat (got {index_cfg.index_type})")
+        return rows
+
     def __init__(self, cfg, index_shard_ids=None):
         self.cfg = cfg
         self.args = cfg.datastore.index
@@ -101,6 +117,7 @@ class Indexer(object):
         self.refine_options(self.args)
         storage_dtype = self.storage_dtype(self.args)
         device_rows = self.device_rows(self.args)
+        list_device_rows = self.list_device_rows(self.args)
 
         passage_dir = self.cfg.datastore.embedding.passages_dir
         paths = self.artefact_paths(cfg, index_shard_ids)
@@ -120,7 +137,7 @@ class Indexer(object):
         elif self.index_type == "IVFFlat":
             self.datastore = IVFFlatIndexer(trained_index_path=index_path + ".trained", sample_train_size=a.sample_train_size,
                                             prev_index_path=None, ncentroids=a.ncentroids, probe=a.probe,
-                                            storage_dtype=storage_dtype, **common)
+                                            storage_dtype=storage_dtype, list_device_rows=list_device_rows, **common)
         elif self.index_type == "IVFPQ":
             k_factor, refine_dtype = self.refine_options(a)
             self.datastore = IVFPQIndexer(trained_index_path=index_path + ".trained", sample_train_size=a.sample_train_size,
