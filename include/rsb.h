@@ -389,17 +389,37 @@ typedef struct rsb_bert rsb_bert_t;
 const char* rsb_bert_last_error(void);
 int rsb_bert_create(int hidden, int layers, int heads, int intermediate, int vocab, int max_pos, int type_vocab,
                     float ln_eps, rsb_bert_t** out);
+/* A T5 encoder behind the same handle: the transformer of a sentence-transformers model such as GTR-T5
+ * (`SentenceTransformer(name).encode(...)`, src/search.py:49-61 and :244-246, src/embed.py:25-40 and :130).  HF
+ * T5EncoderModel in fp16: d_model 768, 12 heads of 64 (d_kv 64), feed_forward_proj "relu" with d_ff % 128 == 0, any
+ * layer count, vocabulary and bucket count; anything else is RSB_ERR_UNSUPPORTED.  max_distance is the config's
+ * relative_attention_max_distance: the buckets themselves are uploaded as a table (rsb_bert_load).  The clamp of HF
+ * T5Block in fp16 is restated with the condition taken over the real tokens of the batch (HF's covers pad positions
+ * too).  Free with rsb_bert_free. */
+int rsb_t5_create(int layers, int d_ff, int vocab, int num_buckets, int max_distance, float eps, rsb_bert_t** out);
 int rsb_bert_free(rsb_bert_t* h);
-/* name = HF BertModel state_dict key (e.g. "encoder.layer.3.attention.self.query.weight"); data fp16, copied */
+/* name = HF BertModel state_dict key (e.g. "encoder.layer.3.attention.self.query.weight"); data fp16, copied.
+ * T5 handles take HF T5EncoderModel keys instead: "shared.weight" or "encoder.embed_tokens.weight" (tied),
+ * "encoder.block.N.layer.0.SelfAttention.{q,k,v,o}.weight", "encoder.block.N.layer.{0,1}.layer_norm.weight",
+ * "encoder.block.N.layer.1.DenseReluDense.{wi,wo}.weight", "encoder.final_layer_norm.weight",
+ * "encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight" ([num_buckets, 12], serves every layer) and
+ * "relative_position_bucket": int32 [1023], the bucket of relative position r = key - query = -511..511 at index
+ * r + 511, from HF's `_relative_position_bucket` (bidirectional) on the host; every entry must lie in
+ * [0, num_buckets) (RSB_ERR_INVALID otherwise).  Both architectures take the sentence-transformers Dense head
+ * "dense.weight" [768, 768] and "dense.bias" [768] (zero unless loaded). */
 int rsb_bert_load(rsb_bert_t* h, const char* name, const void* f16_dev, int64_t n_elements, rsb_stream_t stream);
 size_t rsb_bert_workspace_bytes(rsb_bert_t* h, int total_tokens);
-/* pooling: 0 = mean over tokens (Contriever), 1 = CLS row.  out_f16_dev [B, 768] fp16 */
+/* pooling: RSB_POOL_MEAN (0) = mean over tokens (Contriever), RSB_POOL_CLS (1) = CLS row, optionally OR-ed with the
+ * sentence-transformers head bits: RSB_POOL_DENSE (fp16 Linear 768 -> 768 on the pooled rows; RSB_ERR_STATE if
+ * dense.weight was not loaded) and RSB_POOL_NORMALIZE (x / max(||x||_2, 1e-12), after the Dense layer).  A T5 handle
+ * returns RSB_ERR_STATE until both of its bias tables are loaded.  out_f16_dev [B, 768] fp16 */
+enum { RSB_POOL_MEAN = 0, RSB_POOL_CLS = 1, RSB_POOL_DENSE = 2, RSB_POOL_NORMALIZE = 4 };
 int rsb_bert_forward(rsb_bert_t* h, const int32_t* input_ids_dev, const int32_t* token_type_ids_dev,
                      const int32_t* cu_seqlens_dev, int B, int T, int max_seqlen, int pooling, void* out_f16_dev,
                      void* ws_dev, size_t ws_bytes, rsb_stream_t stream);
 int64_t rsb_bert_launches(rsb_bert_t* h);
-/* the encoder's tensor-core GEMM on its own: C[M,N] = A[M,K] . W[N,K]^T + bias (epilogue 0), GELU (1) or
- * + residual (2); all fp16 row-major device pointers, N % 128 == 0, K % 64 == 0 */
+/* the encoder's tensor-core GEMM on its own: C[M,N] = A[M,K] . W[N,K]^T + bias (epilogue 0), GELU (1),
+ * + residual (2) or ReLU (3); all fp16 row-major device pointers, N % 128 == 0, K % 64 == 0 */
 int rsb_gemm_f16(const void* A_dev, const void* W_dev, const void* bias_dev, const void* residual_dev, void* C_dev,
                  int M, int N, int K, int epilogue, rsb_stream_t stream);
 

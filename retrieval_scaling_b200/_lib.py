@@ -17,6 +17,7 @@ RSB_DTYPE_F32, RSB_DTYPE_F16, RSB_DTYPE_SQ8 = 0, 1, 2
 (INFO_KIND, INFO_D, INFO_NLIST, INFO_M, INFO_NBITS, INFO_NTOTAL, INFO_IS_TRAINED, INFO_MAX_LIST_LEN,
  INFO_INDEX_BYTES, INFO_DTYPE, INFO_BY_RESIDUAL, INFO_HOST_BYTES, INFO_DEVICE_ROWS) = range(13)
 OPT_COARSE_TENSOR, OPT_BY_RESIDUAL, OPT_DEVICE_ROWS, OPT_STAGING_BYTES = 0, 1, 2, 3
+POOL_MEAN, POOL_CLS, POOL_DENSE, POOL_NORMALIZE = 0, 1, 2, 4
 PROF_NAMES = ("coarse_ms", "setup_ms", "lut_ms", "scan_ms", "merge_ms", "scan_bytes", "pairs", "launches", "scan_path",
               "rescored")
 
@@ -77,6 +78,7 @@ SIGNATURES = [
     ("rsb_get_profile", c_int, [_H, POINTER(c_double), c_int]),
     ("rsb_bert_last_error", c_char_p, []),
     ("rsb_bert_create", c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, POINTER(_H)]),
+    ("rsb_t5_create", c_int, [c_int, c_int, c_int, c_int, c_int, c_float, POINTER(_H)]),
     ("rsb_bert_free", c_int, [_H]),
     ("rsb_bert_load", c_int, [_H, c_char_p, c_void_p, c_int64, c_void_p]),
     ("rsb_bert_workspace_bytes", c_size_t, [_H, c_int]),

@@ -11,6 +11,12 @@
 //                        (collect_long_kernel lists those sequences once per forward)
 //   layernorm_rows_kernel  LayerNorm over 768 (fp32 statistics), persistent warps with the next row prefetched
 //   pool_kernel          masked mean over the valid tokens (all tokens of an un-padded sequence) or CLS row
+//
+// The same handle runs a T5 encoder (rsb_t5_create; sentence-transformers' GTR-T5, reference src/search.py:49-61 and
+// src/embed.py:25-40): embed_gather_kernel, then per pre-norm block layernorm_rows_kernel<true> (RMS norm + HF's fp16
+// clamp), the GEMMs with zero biases and the ReLU / inf-flagging residual epilogues, and the T5 form of both attention
+// kernels (relative-position bias, no scaling).  Either architecture can end in the sentence-transformers head:
+// pool_kernel -> Dense on gemm_tn_kernel -> l2normalize_rows_kernel.
 #include "../../include/rsb.h"
 
 #include "rsb_internal.h"
@@ -42,7 +48,9 @@ constexpr int G_TILE_BYTES = 128 * G_BK * 2;                            // 16 KB
 constexpr int G_STAGE_BYTES = 2 * G_TILE_BYTES;                         // A and B tiles
 constexpr int G_SMEM = G_STAGES * G_STAGE_BYTES + 1024 /*align*/ + 256; // ring + barriers
 
-enum { EPI_BIAS = 0, EPI_BIAS_GELU = 1, EPI_BIAS_RESIDUAL = 2 };
+// EPI_BIAS_RELU: T5's DenseReluDense (wi -> ReLU).  EPI_BIAS_RESIDUAL_INF: the T5 residual add, which also raises
+// *inf_flag when it writes +-inf -- the condition of HF T5Block's fp16 clamp, read by the next RMS norm.
+enum { EPI_BIAS = 0, EPI_BIAS_GELU = 1, EPI_BIAS_RESIDUAL = 2, EPI_BIAS_RELU = 3, EPI_BIAS_RESIDUAL_INF = 4 };
 
 #ifdef RSB_EXACT_ERF
 // HF BERT's "gelu" with CUDA's erff (-DRSB_EXACT_ERF; the default is the restatement gelu_erf_pair below)
@@ -107,7 +115,7 @@ template <int EPI>
 __global__ __launch_bounds__(G_THREADS, 1)
 void gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                     __half* __restrict__ C, const __half* __restrict__ bias, const __half* __restrict__ residual,
-                    int M, int N, int K, int m_rev) {
+                    int M, int N, int K, int m_rev, int* __restrict__ inf_flag) {
     extern __shared__ unsigned char smem_dyn[];
     // 1024-byte alignment required by the 128B swizzle atom
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
@@ -175,6 +183,7 @@ void gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     float2 bj[16];
 #pragma unroll
     for (int j = 0; j < 16; ++j) bj[j] = __half22float2(*reinterpret_cast<const __half2*>(bias + c_lo + 8 * j));
+    bool wrote_inf = false;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
         const int row = r_lo + 8 * h;
@@ -185,11 +194,14 @@ void gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         for (int j = 0; j < 16; ++j) {
             float x0 = __fadd_rn(acc[4 * j + 2 * h], bj[j].x), x1 = __fadd_rn(acc[4 * j + 2 * h + 1], bj[j].y);
             if (EPI == EPI_BIAS_GELU) f2unpack(gelu_erf_pair(f2pack(x0, x1)), x0, x1);
+            if (EPI == EPI_BIAS_RELU) { x0 = x0 < 0.f ? 0.f : x0; x1 = x1 < 0.f ? 0.f : x1; }   // NaN passes, as torch.relu
             __half2 o = __floats2half2_rn(x0, x1);
-            if (EPI == EPI_BIAS_RESIDUAL) o = __hadd2(o, *reinterpret_cast<const __half2*>(res + 8 * j));
+            if (EPI == EPI_BIAS_RESIDUAL || EPI == EPI_BIAS_RESIDUAL_INF) o = __hadd2(o, *reinterpret_cast<const __half2*>(res + 8 * j));
+            if (EPI == EPI_BIAS_RESIDUAL_INF) wrote_inf |= __hisinf(__low2half(o)) != 0 || __hisinf(__high2half(o)) != 0;
             *reinterpret_cast<__half2*>(dst + 8 * j) = o;
         }
     }
+    if (EPI == EPI_BIAS_RESIDUAL_INF && wrote_inf) *inf_flag = 1;   // every writer stores the same value
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -281,9 +293,18 @@ __global__ void layernorm_kernel(const __half* __restrict__ in, int T, const __h
 // row already requested while it reduces and stores the current one.  Inside a forward (clock lowered by the power
 // cap after a GEMM) a warp that loads, reduces and stores one row and exits is bound by its own latency chain, not by
 // HBM; the one-row-per-warp kernel was slower there than in isolation (RSB_BERT_PROFILE).  Same arithmetic, same order of operations per row (RSB_LN_V1=1: the first form, A/B).
+//
+// RMS = true is T5LayerNorm in fp16: fp32 x rsqrt(mean(x^2) + eps), rounded to half, times the half weight (beta is
+// unused).  It first applies HF T5Block's fp16 clamp to its input: when *clamp_flag is set (a residual add of the
+// previous GEMM wrote +-inf anywhere in the batch) every row is clamped to +-(65504 - 1000) -- rounded to half, that
+// is +-64512 -- and the clamped row is written back to the residual stream `in` before it is normalised.  Without the
+// flag the clamp to +-65504 leaves the finite rows unchanged.  The kernel boundary is the batch-wide barrier that
+// HF's `torch.isinf(hidden_states).any()` implies.
+template <bool RMS>
 __global__ __launch_bounds__(256, 3)
 void layernorm_rows_kernel(const __half* __restrict__ in, int T, const __half* __restrict__ gamma,
-                           const __half* __restrict__ beta, float eps, __half* __restrict__ out) {
+                           const __half* __restrict__ beta, float eps, __half* __restrict__ out,
+                           const int* __restrict__ clamp_flag) {
     const int lane = threadIdx.x & 31;
     const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
     if (gw >= T) return;
@@ -310,6 +331,41 @@ void layernorm_rows_kernel(const __half* __restrict__ in, int T, const __half* _
                 x[c * 8 + e * 2 + 1] = f.y;
             }
         }
+        if constexpr (RMS) {
+            if (clamp_flag && *clamp_flag) {
+#pragma unroll
+                for (int c = 0; c < 3; ++c) {
+                    uint4 cv;
+                    __half2* c2 = reinterpret_cast<__half2*>(&cv);
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                        float& a = x[c * 8 + e * 2];
+                        float& b = x[c * 8 + e * 2 + 1];
+                        a = a > 64504.f ? 64504.f : (a < -64504.f ? -64504.f : a);   // NaN passes, as torch.clamp
+                        b = b > 64504.f ? 64504.f : (b < -64504.f ? -64504.f : b);
+                        c2[e] = __floats2half2_rn(a, b);
+                        a = __low2float(c2[e]);
+                        b = __high2float(c2[e]);
+                    }
+                    *reinterpret_cast<uint4*>(const_cast<__half*>(in) + (size_t)t * HID + c * 256 + lane * 8) = cv;
+                }
+            }
+#pragma unroll
+            for (int i = 0; i < 24; ++i) s = fmaf(x[i], x[i], s);
+            for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+            const float rstd = rsqrtf(s * (1.f / HID) + eps);
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                const uint4 gv = *reinterpret_cast<const uint4*>(gamma + c * 256 + lane * 8);
+                const __half2* g2 = reinterpret_cast<const __half2*>(&gv);
+                uint4 ov;
+                __half2* o2 = reinterpret_cast<__half2*>(&ov);
+#pragma unroll
+                for (int e = 0; e < 4; ++e)
+                    o2[e] = __hmul2(__floats2half2_rn(x[c * 8 + e * 2] * rstd, x[c * 8 + e * 2 + 1] * rstd), g2[e]);
+                *reinterpret_cast<uint4*>(out + (size_t)t * HID + c * 256 + lane * 8) = ov;
+            }
+        } else {
 #pragma unroll
         for (int i = 0; i < 24; ++i) s += x[i];
         for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
@@ -335,9 +391,65 @@ void layernorm_rows_kernel(const __half* __restrict__ in, int T, const __half* _
             }
             *reinterpret_cast<uint4*>(out + (size_t)t * HID + c * 256 + lane * 8) = ov;
         }
+        }
 #pragma unroll
         for (int c = 0; c < 3; ++c) cur[c] = nxt[c];
     }
+}
+
+// T5 embedding (modeling_t5.py T5Stack: embed_tokens only, not scaled, no position embedding): one warp per token
+__global__ void embed_gather_kernel(const int* __restrict__ input_ids, int T, const __half* __restrict__ word, int vocab,
+                                    __half* __restrict__ out) {
+    const int lane = threadIdx.x & 31;
+    const int t = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (t >= T) return;
+    int id = input_ids[t];
+    id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+        *reinterpret_cast<uint4*>(out + (size_t)t * HID + c * 256 + lane * 8) =
+            *reinterpret_cast<const uint4*>(word + (size_t)id * HID + c * 256 + lane * 8);
+}
+
+// sentence-transformers Normalize on a half tensor (torch.nn.functional.normalize): x / max(||x||_2, 1e-12), the norm
+// accumulated in fp32 and rounded to half, the quotient rounded to half.  One warp per row, in place.
+__global__ void l2normalize_rows_kernel(__half* __restrict__ x, int B) {
+    const int lane = threadIdx.x & 31;
+    const int b = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (b >= B) return;
+    float v[24];
+    load_row24(x + (size_t)b * HID, lane, v, false);
+    float s = 0.f;
+#pragma unroll
+    for (int i = 0; i < 24; ++i) s = fmaf(v[i], v[i], s);
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    const float d = fmaxf(__half2float(__float2half_rn(sqrtf(s))), 1e-12f);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        uint4 ov;
+        __half2* o2 = reinterpret_cast<__half2*>(&ov);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) o2[e] = __floats2half2_rn(__fdiv_rn(v[c * 8 + e * 2], d), __fdiv_rn(v[c * 8 + e * 2 + 1], d));
+        *reinterpret_cast<uint4*>(x + (size_t)b * HID + c * 256 + lane * 8) = ov;
+    }
+}
+
+// T5 relative-position bias per head and relative position r = key - query in [-511, 511]: relb[h][r + 511] =
+// weight[bucket[r + 511]][h], with the bucket of every r computed on the host by HF's fp32 expression
+// (T5Attention._relative_position_bucket).  Run once when both tables have been loaded.
+constexpr int T5_REL = 1023;
+__global__ void t5_bias_expand_kernel(const int* __restrict__ bucket, const __half* __restrict__ weight, int heads,
+                                      float* __restrict__ relb) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= heads * T5_REL) return;
+    const int h = i / T5_REL, k = i % T5_REL;
+    relb[i] = __half2float(weight[bucket[k] * heads + h]);
+}
+
+// T5 attention score (modeling_t5.py T5Attention, fp16): scores = fp16(q.k) with no 1/sqrt(d) scaling, then
+// scores = fp16(scores + bias), the sum taken in fp32 as torch does for two half tensors
+__device__ __forceinline__ float t5_score(float qk, float bias) {
+    return __half2float(__float2half_rn(__half2float(__float2half_rn(qk)) + bias));
 }
 
 constexpr int ATT_HD = 64, ATT_PADH = 72, ATT_MAXS = 512;
@@ -360,10 +472,13 @@ __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
 }
 
 constexpr int ATT32_WARP_BYTES = 3 * 32 * ATT_PADH * 2;      // Q, K, V tiles of one (sequence, head)
+constexpr int ATT32_T5_BIAS_BYTES = 64 * 4;                   // T5: the head's bias for r = -31..31, per warp
 
+// T5 = true: T5 attention (t5_score, scale 1) with the head's relative-position bias from relb (t5_bias_expand_kernel)
+template <bool T5>
 __global__ __launch_bounds__(128)
 void attention_mma32_kernel(const __half* __restrict__ qkv, const int* __restrict__ cu_seqlens, __half* __restrict__ ctx,
-                            float scale, int heads, int B, int rev) {
+                            float scale, int heads, int B, int rev, const float* __restrict__ relb) {
     extern __shared__ __align__(16) unsigned char att32_smem[];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     // blocks run last sequence first: the QKV tensor (188 MB at 41k tokens) is larger than the L2 and the GEMM wrote its
@@ -379,6 +494,12 @@ void attention_mma32_kernel(const __half* __restrict__ qkv, const int* __restric
     typedef __half (*Tile)[ATT_PADH];
     Tile Qs = reinterpret_cast<Tile>(att32_smem + wib * ATT32_WARP_BYTES);
     Tile Ks = Qs + 32, Vs = Qs + 64;
+    float* bsm = nullptr;                               // T5: bsm[r + 31] = bias of relative position r
+    if constexpr (T5) {
+        bsm = reinterpret_cast<float*>(att32_smem + 4 * ATT32_WARP_BYTES) + wib * 64;
+        bsm[lane] = relb[h * T5_REL + 511 - 31 + lane];
+        if (lane < 31) bsm[32 + lane] = relb[h * T5_REL + 511 + 1 + lane];
+    }
 
     // (A persistent variant that prefetched the next item's tiles with cp.async into a second buffer was slower: the
     // double buffer halves the resident warps and the kernel is bound by the dependent-instruction latency of each warp.)
@@ -456,7 +577,9 @@ void attention_mma32_kernel(const __half* __restrict__ qkv, const int* __restric
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
                     const int col = nt * 8 + 2 * t + (e & 1);
-                    const float s = col < S ? sacc[mt][nt][e] : -INFINITY;
+                    float s;
+                    if constexpr (T5) s = col < S ? t5_score(sacc[mt][nt][e], bsm[col - (mt * 16 + g + (e >> 1) * 8) + 31]) : -INFINITY;
+                    else s = col < S ? sacc[mt][nt][e] : -INFINITY;
                     sacc[mt][nt][e] = s;
                     if (e < 2) mx0 = fmaxf(mx0, s); else mx1 = fmaxf(mx1, s);
                 }
@@ -542,12 +665,18 @@ __global__ void collect_long_kernel(const int* __restrict__ cu_seqlens, int B, i
 // maximum / sum, output rescaled when the maximum moves), O += P V with V^T fragments through ldmatrix.trans.
 // Same arithmetic as attention_mma32_kernel for a single key block.
 // ---------------------------------------------------------------------------------------------------------
+template <bool T5>
 __global__ __launch_bounds__(128)
 void attention_flash_kernel(const __half* __restrict__ qkv, const int* __restrict__ cu_seqlens, __half* __restrict__ ctx,
                             float scale, const int* __restrict__ long_list, const int* __restrict__ long_count, int heads,
-                            int nqb) {
+                            int nqb, const float* __restrict__ relb) {
     __shared__ __align__(16) __half Ks[32][ATT_PADH];
     __shared__ __align__(16) __half Vs[32][ATT_PADH];
+    float* Bs = nullptr;                                 // T5: Bs[r + 511] = bias of relative position r for this item's head
+    if constexpr (T5) {
+        __shared__ float t5_bias[T5_REL];
+        Bs = t5_bias;
+    }
     // work items (long sequence, head, block of 128 queries) in a grid-stride loop over the list that collect_long_kernel
     // wrote once for this forward.  A batch of queries holds one or two sequences beyond 32 tokens: walking all
     // B x heads x nqb candidates every layer would keep the side stream busy and slow the short-sequence kernel it
@@ -564,6 +693,9 @@ void attention_flash_kernel(const __half* __restrict__ qkv, const int* __restric
     const int qw = q0 + wib * 32;                        // first query row of this warp
     const bool active = qw < S;                          // warp-uniform; idle warps still stage K / V and hit the barriers
     const __half* base = qkv + (size_t)t0 * (3 * HID) + h * ATT_HD;
+    if constexpr (T5) {                                  // visible after the first barrier of the key loop
+        for (int i = threadIdx.x; i < T5_REL; i += 128) Bs[i] = relb[h * T5_REL + i];
+    }
 
     uint32_t qa[4][2][4];
 #pragma unroll
@@ -636,7 +768,9 @@ void attention_flash_kernel(const __half* __restrict__ qkv, const int* __restric
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
                     const int col = kb * 32 + nt * 8 + 2 * t + (e & 1);
-                    const float sv = col < S ? sacc[mt][nt][e] * scale : -INFINITY;
+                    float sv;
+                    if constexpr (T5) sv = col < S ? t5_score(sacc[mt][nt][e], Bs[col - (qw + mt * 16 + g + (e >> 1) * 8) + 511]) : -INFINITY;
+                    else sv = col < S ? sacc[mt][nt][e] * scale : -INFINITY;
                     sacc[mt][nt][e] = sv;
                     if (e < 2) mx0 = fmaxf(mx0, sv); else mx1 = fmaxf(mx1, sv);
                 }
@@ -756,6 +890,17 @@ struct rsb_bert {
     float eps = 1e-12f;
     __half *word = nullptr, *pos = nullptr, *type = nullptr, *emb_g = nullptr, *emb_b = nullptr;
     std::vector<Layer> L;
+    // T5 encoder (rsb_t5_create): pre-norm blocks, RMS norms ln1_g / ln2_g, no biases (the Linear biases stay zero)
+    bool t5 = false;
+    int num_buckets = 0, max_distance = 0;
+    int* bucket = nullptr;                               // [T5_REL] bucket of r = -511..511
+    __half* rel_w = nullptr;                             // [num_buckets, heads] relative_attention_bias.weight
+    float* relb = nullptr;                               // [heads, T5_REL] expanded by t5_bias_expand_kernel
+    bool bucket_loaded = false, rel_w_loaded = false;
+    __half* final_g = nullptr;                           // encoder.final_layer_norm.weight
+    // sentence-transformers Dense head (both architectures): 768 -> 768, bias zero unless loaded
+    Linear dense;
+    bool dense_loaded = false;
     long launches = 0;
     // the two attention kernels of a layer work on disjoint sequences (<= 32 tokens / longer): the long-sequence one runs
     // on a side stream so that it overlaps the other instead of adding its latency to every layer
@@ -781,7 +926,8 @@ void free_linear(Linear& l) { cudaFree(l.w); cudaFree(l.b); }
 // m_rev: visit the row tiles last-to-first.  The FFN intermediate (251 MB at 41k tokens) is twice the L2: FFN2 starts with the
 // rows FFN1 wrote last, which are still cached (RSB_NO_SNAKE=1 disables, A/B).
 template <int EPI>
-int launch_gemm(const __half* A, int M, const Linear& lin, __half* C, const __half* residual, cudaStream_t st, bool m_rev = false) {
+int launch_gemm(const __half* A, int M, const Linear& lin, __half* C, const __half* residual, cudaStream_t st, bool m_rev = false,
+                int* inf_flag = nullptr) {
     CUtensorMap tmA;
     if (!lin.map_ok || !make_map(&tmA, A, (uint64_t)M, (uint64_t)lin.K, G_BM)) return RSB_ERR_CUDA;
     static rsb::PerDeviceFlag configured;                    // attributes are per (function, device)
@@ -789,7 +935,7 @@ int launch_gemm(const __half* A, int M, const Linear& lin, __half* C, const __ha
     static const bool no_snake = getenv("RSB_NO_SNAKE") != nullptr;
     dim3 grid(lin.N / G_BN, (M + G_BM - 1) / G_BM);              // consecutive CTAs share one row tile of A
     gemm_tn_kernel<EPI><<<grid, G_THREADS, G_SMEM, st>>>(tmA, lin.map, C, lin.b, residual, M, lin.N, lin.K,
-                                                         (m_rev && !no_snake) ? 1 : 0);
+                                                         (m_rev && !no_snake) ? 1 : 0, inf_flag);
     return RSB_OK;
 }
 
@@ -813,6 +959,7 @@ extern "C" int rsb_bert_create(int hidden, int layers, int heads, int inter, int
     ok &= cudaMalloc(&h->type, (size_t)std::max(type_vocab, 2) * hidden * 2) == cudaSuccess;
     ok &= cudaMalloc(&h->emb_g, hidden * 2) == cudaSuccess;
     ok &= cudaMalloc(&h->emb_b, hidden * 2) == cudaSuccess;
+    ok &= alloc_linear(h->dense, hidden, hidden) == RSB_OK;
     if (ok) cudaMemset(h->type, 0, (size_t)std::max(type_vocab, 2) * hidden * 2);
     h->L.resize(layers);
     for (auto& l : h->L) {
@@ -830,9 +977,36 @@ extern "C" int rsb_bert_create(int hidden, int layers, int heads, int inter, int
     return RSB_OK;
 }
 
+// Replaces `SentenceTransformer(name)`'s T5 module (src/search.py:49-61, src/embed.py:25-40): HF T5EncoderModel with
+// d_model 768, 12 heads of 64 and a ReLU feed-forward of d_ff.
+extern "C" int rsb_t5_create(int layers, int d_ff, int vocab, int num_buckets, int max_distance, float eps,
+                             rsb_bert_t** out) {
+    if (!out) return bfail(RSB_ERR_INVALID, "out is NULL");
+    *out = nullptr;
+    if (layers <= 0 || d_ff <= 0 || d_ff % G_BN || vocab <= 0 || num_buckets < 2 || max_distance <= 0)
+        return bfail(RSB_ERR_UNSUPPORTED, "only T5 encoders with d_model 768, 12 heads of 64 and a ReLU feed-forward of a "
+                                          "multiple of 128 are implemented%s (got d_ff %ld)", "", (long)d_ff);
+    rsb_bert_t* h = nullptr;
+    const int rc = rsb_bert_create(768, layers, 12, d_ff, vocab, ATT_MAXS, 1, eps, &h);
+    if (rc != RSB_OK) return rc;
+    h->t5 = true;
+    h->num_buckets = num_buckets;
+    h->max_distance = max_distance;
+    bool ok = true;
+    ok &= cudaMalloc(&h->bucket, T5_REL * sizeof(int)) == cudaSuccess;
+    ok &= cudaMalloc(&h->rel_w, (size_t)num_buckets * h->heads * 2) == cudaSuccess;
+    ok &= cudaMalloc(&h->relb, (size_t)h->heads * T5_REL * sizeof(float)) == cudaSuccess;
+    ok &= cudaMalloc(&h->final_g, h->hidden * 2) == cudaSuccess;
+    if (!ok) { rsb_bert_free(h); return bfail(RSB_ERR_OOM, "allocating encoder weights failed"); }
+    *out = h;
+    return RSB_OK;
+}
+
 extern "C" int rsb_bert_free(rsb_bert_t* h) {
     if (!h) return RSB_OK;
     cudaFree(h->word); cudaFree(h->pos); cudaFree(h->type); cudaFree(h->emb_g); cudaFree(h->emb_b);
+    cudaFree(h->bucket); cudaFree(h->rel_w); cudaFree(h->relb); cudaFree(h->final_g);
+    free_linear(h->dense);
     if (h->side) cudaStreamDestroy(h->side);
     if (h->ev_fork) cudaEventDestroy(h->ev_fork);
     if (h->ev_join) cudaEventDestroy(h->ev_join);
@@ -843,6 +1017,57 @@ extern "C" int rsb_bert_free(rsb_bert_t* h) {
     }
     delete h;
     return RSB_OK;
+}
+
+// HF T5EncoderModel keys.  relative_position_bucket is int32 [1023]: the bucket of r = key - query = -511..511.
+template <class Put>
+static int t5_load(rsb_bert* h, const std::string& s, const void* dev_ptr, int64_t n, cudaStream_t st, Put put) {
+    const int H = h->hidden;
+    auto expand = [&]() -> int {                         // once both bias tables are present
+        if (h->bucket_loaded && h->rel_w_loaded) {
+            t5_bias_expand_kernel<<<(h->heads * T5_REL + 255) / 256, 256, 0, st>>>(h->bucket, h->rel_w, h->heads, h->relb);
+            if (cudaPeekAtLastError() != cudaSuccess) return bfail(RSB_ERR_CUDA, "bias table expansion failed");
+        }
+        return RSB_OK;
+    };
+    if (s == "shared.weight" || s == "encoder.embed_tokens.weight") return put(h->word, (int64_t)h->vocab * H);
+    if (s == "encoder.final_layer_norm.weight") return put(h->final_g, H);
+    if (s == "relative_position_bucket") {
+        if (n != T5_REL) return bfail(RSB_ERR_INVALID, "relative_position_bucket needs 1023 int32 entries%s (got %ld)", "", (long)n);
+        std::vector<int> hb(T5_REL);
+        if (cudaMemcpyAsync(hb.data(), dev_ptr, T5_REL * sizeof(int), cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+            cudaStreamSynchronize(st) != cudaSuccess)
+            return bfail(RSB_ERR_CUDA, "copy of relative_position_bucket failed");
+        for (int v : hb)
+            if (v < 0 || v >= h->num_buckets) return bfail(RSB_ERR_INVALID, "relative_position_bucket entry %s%ld is outside [0, num_buckets)", "", (long)v);
+        if (cudaMemcpyAsync(h->bucket, hb.data(), T5_REL * sizeof(int), cudaMemcpyHostToDevice, st) != cudaSuccess ||
+            cudaStreamSynchronize(st) != cudaSuccess)
+            return bfail(RSB_ERR_CUDA, "copy of relative_position_bucket failed");
+        h->bucket_loaded = true;
+        return expand();
+    }
+    int li = -1;
+    char rest[128] = {0};
+    if (sscanf(s.c_str(), "encoder.block.%d.%127s", &li, rest) == 2 && li >= 0 && li < h->layers) {
+        Layer& l = h->L[li];
+        std::string r(rest);
+        const int64_t HH = (int64_t)H * H;
+        if (r == "layer.0.SelfAttention.q.weight") return put(l.qkv.w, HH);
+        if (r == "layer.0.SelfAttention.k.weight") return put(l.qkv.w + HH, HH);
+        if (r == "layer.0.SelfAttention.v.weight") return put(l.qkv.w + 2 * HH, HH);
+        if (r == "layer.0.SelfAttention.o.weight") return put(l.attn_out.w, HH);
+        if (r == "layer.0.layer_norm.weight") return put(l.ln1_g, H);
+        if (r == "layer.1.DenseReluDense.wi.weight") return put(l.ffn1.w, (int64_t)h->inter * H);
+        if (r == "layer.1.DenseReluDense.wo.weight") return put(l.ffn2.w, (int64_t)h->inter * H);
+        if (r == "layer.1.layer_norm.weight") return put(l.ln2_g, H);
+        if (li == 0 && r == "layer.0.SelfAttention.relative_attention_bias.weight") {   // layer 0's table serves every layer
+            const int rc = put(h->rel_w, (int64_t)h->num_buckets * h->heads);
+            if (rc != RSB_OK) return rc;
+            h->rel_w_loaded = true;
+            return expand();
+        }
+    }
+    return bfail(RSB_ERR_INVALID, "unknown weight name %s", s.c_str());
 }
 
 // name = HF BertModel state_dict key (SURVEY.md App. B), data = fp16 device pointer, n = element count.
@@ -856,6 +1081,13 @@ extern "C" int rsb_bert_load(rsb_bert_t* h, const char* name, const void* dev_pt
                    ? RSB_OK : bfail(RSB_ERR_CUDA, "copy of %s failed", name);
     };
     std::string s(name);
+    if (s == "dense.weight") {
+        const int rc = put(h->dense.w, (int64_t)H * H);
+        if (rc == RSB_OK) h->dense_loaded = true;
+        return rc;
+    }
+    if (s == "dense.bias") return put(h->dense.b, H);
+    if (h->t5) return t5_load(h, s, dev_ptr, n, st, put);
     if (s == "embeddings.word_embeddings.weight") return put(h->word, (int64_t)h->vocab * H);
     if (s == "embeddings.position_embeddings.weight") return put(h->pos, (int64_t)h->max_pos * H);
     if (s == "embeddings.token_type_embeddings.weight") return put(h->type, (int64_t)h->type_vocab * H);
@@ -887,21 +1119,22 @@ extern "C" int rsb_bert_load(rsb_bert_t* h, const char* name, const void* dev_pt
     return bfail(RSB_ERR_INVALID, "unknown weight name %s", name);
 }
 
-static size_t bert_ws_layout(const rsb_bert* h, int T, size_t off[6]) {
+static size_t bert_ws_layout(const rsb_bert* h, int T, size_t off[7]) {
     auto al = [](size_t x) { return (x + 1023) / 1024 * 1024; };   // TMA global addresses: 16 B is enough; keep 1 KB
     const size_t Tp = (size_t)((T + 127) / 128 * 128);
     size_t o = 0;
-    off[0] = o; o += al(Tp * h->hidden * 2);        // H
+    off[0] = o; o += al(Tp * h->hidden * 2);        // H (T5: the RMS-normed rows)
     off[1] = o; o += al(Tp * 3 * h->hidden * 2);    // QKV
-    off[2] = o; o += al(Tp * h->hidden * 2);        // CTX
-    off[3] = o; o += al(Tp * h->hidden * 2);        // TMP (pre-LN sums)
+    off[2] = o; o += al(Tp * h->hidden * 2);        // CTX (after the last layer: the pooled rows the Dense head reads)
+    off[3] = o; o += al(Tp * h->hidden * 2);        // TMP (pre-LN sums; T5: the residual stream)
     off[4] = o; o += al(Tp * h->inter * 2);         // FFN intermediate
-    off[5] = o;
+    off[5] = o; if (h->t5) o += al((size_t)2 * h->layers * sizeof(int));   // T5: one clamp flag per residual add
+    off[6] = o;
     return o;
 }
 extern "C" size_t rsb_bert_workspace_bytes(rsb_bert_t* h, int total_tokens) {
     if (!h) return 0;
-    size_t off[6];
+    size_t off[7];
     return bert_ws_layout(h, std::max(total_tokens, 1), off);
 }
 
@@ -911,9 +1144,13 @@ extern "C" int rsb_bert_forward(rsb_bert_t* h, const int32_t* input_ids, const i
                                 void* ws, size_t ws_bytes, rsb_stream_t stream) {
     if (!h || !input_ids || !cu_seqlens || !out_f16) return bfail(RSB_ERR_INVALID, "null argument");
     if (B <= 0 || T <= 0) return bfail(RSB_ERR_INVALID, "empty batch");
+    if (pooling & ~(RSB_POOL_CLS | RSB_POOL_DENSE | RSB_POOL_NORMALIZE)) return bfail(RSB_ERR_INVALID, "unknown pooling bits%s %ld", "", (long)pooling);
+    if ((pooling & RSB_POOL_DENSE) && !h->dense_loaded) return bfail(RSB_ERR_STATE, "pooling asks for the Dense head but dense.weight was not loaded");
+    if (h->t5 && !(h->bucket_loaded && h->rel_w_loaded))
+        return bfail(RSB_ERR_STATE, "T5 forward before relative_position_bucket and the relative_attention_bias weight were loaded");
     if (max_seqlen > ATT_MAXS || max_seqlen > h->max_pos)
         return bfail(RSB_ERR_UNSUPPORTED, "sequence longer than %s%ld tokens", "", (long)std::min(ATT_MAXS, h->max_pos));
-    size_t off[6];
+    size_t off[7];
     const size_t need = bert_ws_layout(h, T, off);
     if (ws_bytes < need) return bfail(RSB_ERR_OOM, "encoder workspace too small (%s need %ld bytes)", "", (long)need);
     cudaStream_t st = (cudaStream_t)stream;
@@ -923,16 +1160,25 @@ extern "C" int rsb_bert_forward(rsb_bert_t* h, const int32_t* input_ids, const i
     __half* CTX = reinterpret_cast<__half*>(w + off[2]);
     __half* TMP = reinterpret_cast<__half*>(w + off[3]);
     __half* FF = reinterpret_cast<__half*>(w + off[4]);
+    int* flags = reinterpret_cast<int*>(w + off[5]);
     h->launches = 0;
 
     const int rows_per_block = 8;   // 256 threads = 8 warps = 8 rows
     const int ln_grid = (T + rows_per_block - 1) / rows_per_block;
-    embed_ln_kernel<<<ln_grid, 256, 0, st>>>(input_ids, token_type_ids, cu_seqlens, B, T, h->word, h->pos, h->type,
-                                             h->emb_g, h->emb_b, h->eps, h->vocab, h->max_pos, Hs);
+    if (h->t5) {
+        embed_gather_kernel<<<ln_grid, 256, 0, st>>>(input_ids, T, h->word, h->vocab, TMP);
+        cudaMemsetAsync(flags, 0, (size_t)2 * h->layers * sizeof(int), st);
+    } else {
+        embed_ln_kernel<<<ln_grid, 256, 0, st>>>(input_ids, token_type_ids, cu_seqlens, B, T, h->word, h->pos, h->type,
+                                                 h->emb_g, h->emb_b, h->eps, h->vocab, h->max_pos, Hs);
+    }
     h->launches++;
     static rsb::PerDeviceFlag att_configured;
-    if (att_configured.first())
-        cudaFuncSetAttribute(attention_mma32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * ATT32_WARP_BYTES);
+    if (att_configured.first()) {
+        cudaFuncSetAttribute(attention_mma32_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * ATT32_WARP_BYTES);
+        cudaFuncSetAttribute(attention_mma32_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             4 * (ATT32_WARP_BYTES + ATT32_T5_BIAS_BYTES));
+    }
     if (!h->side) {
         cudaStreamCreateWithFlags(&h->side, cudaStreamNonBlocking);
         cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming);
@@ -955,76 +1201,129 @@ extern "C" int rsb_bert_forward(rsb_bert_t* h, const int32_t* input_ids, const i
     const int ln_rows_grid = std::min(ln_grid, 3 * rsb::device_num_sms());   // 24 warps per SM, ~12 rows per warp at 41k tokens
     auto launch_ln = [&](const __half* x, const __half* g, const __half* b) {
         if (ln_v1) layernorm_kernel<<<ln_grid, 256, 0, st>>>(x, T, g, b, h->eps, Hs);
-        else layernorm_rows_kernel<<<ln_rows_grid, 256, 0, st>>>(x, T, g, b, h->eps, Hs);
+        else layernorm_rows_kernel<false><<<ln_rows_grid, 256, 0, st>>>(x, T, g, b, h->eps, Hs, nullptr);
+    };
+    // T5: Hs = rms(X) after the clamp that `flag` (the previous residual add's) calls for
+    auto launch_rms = [&](__half* x, const __half* g, const int* flag) {
+        layernorm_rows_kernel<true><<<ln_rows_grid, 256, 0, st>>>(x, T, g, nullptr, h->eps, Hs, flag);
     };
     auto launch_attention = [&](const __half* qkv_p, __half* ctx_p) {
         // sequences of <= 32 tokens (queries): warp-per-(sequence, head) tensor-core kernel; longer ones (passages, the odd
         // long query): flash-style kernel on a side stream -- the two work on disjoint sequences of the same buffers
+        const float scale = h->t5 ? 1.f : 0.125f;
         if (have_long) {
             cudaEventRecord(h->ev_fork, st);
             cudaStreamWaitEvent(h->side, h->ev_fork, 0);
             const int nqb = (max_seqlen + 127) / 128;
             const long items = (long)B * h->heads * nqb;
             const int fgrid = (int)std::min<long>(items, 2L * rsb::device_num_sms());   // 194 registers: two resident blocks per SM
-            attention_flash_kernel<<<fgrid, 128, 0, h->side>>>(qkv_p, cu_seqlens, ctx_p, 0.125f, h->long_list, h->long_list + h->long_cap,
-                                                               h->heads, nqb);
+            if (h->t5)
+                attention_flash_kernel<true><<<fgrid, 128, 0, h->side>>>(qkv_p, cu_seqlens, ctx_p, scale, h->long_list,
+                                                                         h->long_list + h->long_cap, h->heads, nqb, h->relb);
+            else
+                attention_flash_kernel<false><<<fgrid, 128, 0, h->side>>>(qkv_p, cu_seqlens, ctx_p, scale, h->long_list,
+                                                                          h->long_list + h->long_cap, h->heads, nqb, nullptr);
             cudaEventRecord(h->ev_join, h->side);
             h->launches++;
         }
         const int nwarps = B * h->heads;
         static const bool no_snake = getenv("RSB_NO_SNAKE") != nullptr;
-        attention_mma32_kernel<<<(nwarps + 3) / 4, 128, 4 * ATT32_WARP_BYTES, st>>>(qkv_p, cu_seqlens, ctx_p, 0.125f, h->heads, B,
-                                                                                   no_snake ? 0 : 1);
+        if (h->t5)
+            attention_mma32_kernel<true><<<(nwarps + 3) / 4, 128, 4 * (ATT32_WARP_BYTES + ATT32_T5_BIAS_BYTES), st>>>(
+                qkv_p, cu_seqlens, ctx_p, scale, h->heads, B, no_snake ? 0 : 1, h->relb);
+        else
+            attention_mma32_kernel<false><<<(nwarps + 3) / 4, 128, 4 * ATT32_WARP_BYTES, st>>>(
+                qkv_p, cu_seqlens, ctx_p, scale, h->heads, B, no_snake ? 0 : 1, nullptr);
         h->launches++;
         if (have_long) cudaStreamWaitEvent(st, h->ev_join, 0);   // join before the attention-output GEMM
     };
     // RSB_BERT_PROFILE=1 (diagnostic): CUDA events between the kernels of the forward, summed per kernel kind over the
     // layers and printed to stderr after each forward -- per-kernel times INSIDE a back-to-back run (ncu's are isolated,
-    // cold-cache and at other clocks).  Synchronises the stream; never set in a timed run.
+    // cold-cache and at other clocks).  Synchronises the stream; never set in a timed run.  The interval that ends at
+    // mark(kind) is counted as `kind`; ln1 / ln2 are the RMS norms before the attention / feed-forward on T5.
     static const bool prof = getenv("RSB_BERT_PROFILE") != nullptr;
     enum { P_QKV, P_ATT, P_AO, P_LN1, P_FFN1, P_FFN2, P_LN2, P_KINDS };
     std::vector<cudaEvent_t> pev;
-    auto mark = [&]() {
+    std::vector<int> pkind;
+    auto mark = [&](int kind) {
         if (!prof) return;
         cudaEvent_t e;
         cudaEventCreate(&e);
         cudaEventRecord(e, st);
         pev.push_back(e);
+        pkind.push_back(kind);
     };
-    mark();
+    const char* gemm_fail = "tensor map encode failed";
+    mark(-1);
     for (int li = 0; li < h->layers; ++li) {
         Layer& l = h->L[li];
-        if (launch_gemm<EPI_BIAS>(Hs, T, l.qkv, QKV, nullptr, st) != RSB_OK) return bfail(RSB_ERR_CUDA, "tensor map encode failed");
-        mark();
-        launch_attention(QKV, CTX);
-        mark();
-        if (launch_gemm<EPI_BIAS_RESIDUAL>(CTX, T, l.attn_out, TMP, Hs, st) != RSB_OK) return bfail(RSB_ERR_CUDA, "tensor map encode failed");
-        mark();
-        launch_ln(TMP, l.ln1_g, l.ln1_b);
-        mark();
-        if (launch_gemm<EPI_BIAS_GELU>(Hs, T, l.ffn1, FF, nullptr, st) != RSB_OK) return bfail(RSB_ERR_CUDA, "tensor map encode failed");
-        mark();
-        if (launch_gemm<EPI_BIAS_RESIDUAL>(FF, T, l.ffn2, TMP, Hs, st, true) != RSB_OK) return bfail(RSB_ERR_CUDA, "tensor map encode failed");
-        mark();
-        launch_ln(TMP, l.ln2_g, l.ln2_b);
-        mark();
+        if (h->t5) {
+            // pre-norm T5 block on the residual stream X = TMP:  X += o(attn(rms(X))), clamp;  X += wo(relu(wi(rms(X)))), clamp
+            // (the clamps are applied by the RMS norm that reads the add's flag)
+            launch_rms(TMP, l.ln1_g, li > 0 ? flags + 2 * li - 1 : nullptr);
+            mark(P_LN1);
+            if (launch_gemm<EPI_BIAS>(Hs, T, l.qkv, QKV, nullptr, st) != RSB_OK) return bfail(RSB_ERR_CUDA, gemm_fail);
+            mark(P_QKV);
+            launch_attention(QKV, CTX);
+            mark(P_ATT);
+            if (launch_gemm<EPI_BIAS_RESIDUAL_INF>(CTX, T, l.attn_out, TMP, TMP, st, false, flags + 2 * li) != RSB_OK)
+                return bfail(RSB_ERR_CUDA, gemm_fail);
+            mark(P_AO);
+            launch_rms(TMP, l.ln2_g, flags + 2 * li);
+            mark(P_LN2);
+            if (launch_gemm<EPI_BIAS_RELU>(Hs, T, l.ffn1, FF, nullptr, st) != RSB_OK) return bfail(RSB_ERR_CUDA, gemm_fail);
+            mark(P_FFN1);
+            if (launch_gemm<EPI_BIAS_RESIDUAL_INF>(FF, T, l.ffn2, TMP, TMP, st, true, flags + 2 * li + 1) != RSB_OK)
+                return bfail(RSB_ERR_CUDA, gemm_fail);
+            mark(P_FFN2);
+        } else {
+            if (launch_gemm<EPI_BIAS>(Hs, T, l.qkv, QKV, nullptr, st) != RSB_OK) return bfail(RSB_ERR_CUDA, gemm_fail);
+            mark(P_QKV);
+            launch_attention(QKV, CTX);
+            mark(P_ATT);
+            if (launch_gemm<EPI_BIAS_RESIDUAL>(CTX, T, l.attn_out, TMP, Hs, st) != RSB_OK) return bfail(RSB_ERR_CUDA, gemm_fail);
+            mark(P_AO);
+            launch_ln(TMP, l.ln1_g, l.ln1_b);
+            mark(P_LN1);
+            if (launch_gemm<EPI_BIAS_GELU>(Hs, T, l.ffn1, FF, nullptr, st) != RSB_OK) return bfail(RSB_ERR_CUDA, gemm_fail);
+            mark(P_FFN1);
+            if (launch_gemm<EPI_BIAS_RESIDUAL>(FF, T, l.ffn2, TMP, Hs, st, true) != RSB_OK) return bfail(RSB_ERR_CUDA, gemm_fail);
+            mark(P_FFN2);
+            launch_ln(TMP, l.ln2_g, l.ln2_b);
+            mark(P_LN2);
+        }
         h->launches += 6;   // + the attention launch(es), counted in launch_attention
     }
-    pool_kernel<<<B, 256, 0, st>>>(Hs, cu_seqlens, pooling, static_cast<__half*>(out_f16));
+    if (h->t5) {                                         // the last feed-forward's clamp, then final_layer_norm
+        launch_rms(TMP, h->final_g, flags + 2 * h->layers - 1);
+        h->launches++;
+    }
+    // sentence-transformers head: Pooling -> Dense (768 x 768 on the tensor-core GEMM, M = B) -> Normalize
+    __half* out = static_cast<__half*>(out_f16);
+    __half* pooled = (pooling & RSB_POOL_DENSE) ? CTX : out;
+    pool_kernel<<<B, 256, 0, st>>>(Hs, cu_seqlens, pooling & RSB_POOL_CLS, pooled);
     h->launches++;
+    if (pooling & RSB_POOL_DENSE) {
+        if (launch_gemm<EPI_BIAS>(CTX, B, h->dense, out, nullptr, st) != RSB_OK) return bfail(RSB_ERR_CUDA, gemm_fail);
+        h->launches++;
+    }
+    if (pooling & RSB_POOL_NORMALIZE) {
+        l2normalize_rows_kernel<<<(B + 7) / 8, 256, 0, st>>>(out, B);
+        h->launches++;
+    }
     if (prof) {
         cudaStreamSynchronize(st);
         float sum[P_KINDS] = {};
         for (size_t i = 0; i + 1 < pev.size(); ++i) {
             float ms = 0.f;
             cudaEventElapsedTime(&ms, pev[i], pev[i + 1]);
-            sum[i % P_KINDS] += ms;
+            sum[pkind[i + 1]] += ms;
         }
         for (cudaEvent_t e : pev) cudaEventDestroy(e);
         const float L = (float)h->layers * 1e-3f;
-        fprintf(stderr, "[rsb_bert profile] T=%d us/layer: qkv %.1f attn %.1f attn_out %.1f ln1 %.1f ffn1 %.1f ffn2 %.1f ln2 %.1f  (sum %.1f)\n", T,
-                sum[P_QKV] / L, sum[P_ATT] / L, sum[P_AO] / L, sum[P_LN1] / L, sum[P_FFN1] / L, sum[P_FFN2] / L, sum[P_LN2] / L,
-                (sum[0] + sum[1] + sum[2] + sum[3] + sum[4] + sum[5] + sum[6]) / L);
+        fprintf(stderr, "[rsb_%s profile] T=%d us/layer: qkv %.1f attn %.1f attn_out %.1f ln1 %.1f ffn1 %.1f ffn2 %.1f ln2 %.1f  (sum %.1f)\n",
+                h->t5 ? "t5" : "bert", T, sum[P_QKV] / L, sum[P_ATT] / L, sum[P_AO] / L, sum[P_LN1] / L, sum[P_FFN1] / L,
+                sum[P_FFN2] / L, sum[P_LN2] / L, (sum[0] + sum[1] + sum[2] + sum[3] + sum[4] + sum[5] + sum[6]) / L);
     }
     cudaError_t e = cudaPeekAtLastError();
     if (e != cudaSuccess) return bfail(RSB_ERR_CUDA, "encoder launch failed: %s", cudaGetErrorString(e));
@@ -1034,6 +1333,7 @@ extern "C" int rsb_bert_forward(rsb_bert_t* h, const int32_t* input_ids, const i
 extern "C" int64_t rsb_bert_launches(rsb_bert_t* h) { return h ? h->launches : 0; }
 
 // plain GEMM entry (tests / roofline of the tensor-core kernel): C[M,N] = A[M,K] W[N,K]^T + bias, epilogue as above
+// (0 bias, 1 GELU, 2 residual, 3 ReLU)
 extern "C" int rsb_gemm_f16(const void* A, const void* W, const void* bias, const void* residual, void* C, int M, int N,
                             int K, int epilogue, rsb_stream_t stream) {
     if (!A || !W || !bias || !C) return bfail(RSB_ERR_INVALID, "null argument");
@@ -1048,6 +1348,7 @@ extern "C" int rsb_gemm_f16(const void* A, const void* W, const void* bias, cons
     if (epilogue == EPI_BIAS) rc = launch_gemm<EPI_BIAS>((const __half*)A, M, lin, (__half*)C, nullptr, st);
     else if (epilogue == EPI_BIAS_GELU) rc = launch_gemm<EPI_BIAS_GELU>((const __half*)A, M, lin, (__half*)C, nullptr, st);
     else if (epilogue == EPI_BIAS_RESIDUAL) rc = launch_gemm<EPI_BIAS_RESIDUAL>((const __half*)A, M, lin, (__half*)C, (const __half*)residual, st);
+    else if (epilogue == EPI_BIAS_RELU) rc = launch_gemm<EPI_BIAS_RELU>((const __half*)A, M, lin, (__half*)C, nullptr, st);
     else return bfail(RSB_ERR_INVALID, "unknown epilogue");
     if (rc != RSB_OK) return bfail(RSB_ERR_CUDA, "tensor map encode failed");
     cudaError_t e = cudaPeekAtLastError();

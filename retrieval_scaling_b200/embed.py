@@ -6,9 +6,10 @@ passage shards into the `(ids, embeddings)` pickles the indexers read:
     {passages_dir}/raw_passages-{shard}-of-{num_shards}.jsonl   ->   {embedding_dir}/{prefix}_{shard:02d}.pkl
 
 What is NOT here: chunking raw corpora into passages (`src/data.py::fast_load_jsonl_shard`, CPU text processing,
-SURVEY.md §2 out of scope) -- a missing passage shard raises with that explanation -- and the non-BERT encoder
-families (sentence-transformers, e5, Qwen3, drama, GritLM), which raise `AttributeError` like the reference does for
-unknown names (`src/embed.py:131-133`).
+SURVEY.md §2 out of scope) -- a missing passage shard raises with that explanation -- and the decoder-LLM encoder
+families (Qwen3, drama, GritLM), which raise `AttributeError` like the reference does for unknown names
+(`src/embed.py:131-133`).  Sentence-transformers models (GTR-T5, e5-base) run through
+`encoder.SentenceTransformerEncoder` (reference `src/embed.py:25-40,130`).
 """
 from __future__ import annotations
 
@@ -42,7 +43,9 @@ def embed_passages(args, passages: Iterable[dict], model, tokenizer) -> Tuple[li
     `passage_maxlength` tokens; Contriever checkpoints mean-pool inside the model, other HF BERT checkpoints take the
     CLS row (reference :66-79)."""
     name = str(args.model_name_or_path)
-    if any(t in name for t in _UNSUPPORTED):
+    from .encoder import SentenceTransformerEncoder, is_sentence_transformers_name
+    st = isinstance(model, SentenceTransformerEncoder) and is_sentence_transformers_name(name)
+    if not st and any(t in name for t in _UNSUPPORTED):
         raise AttributeError(f"{name}: this encoder family is out of scope of the GPU hot path "
                              f"(BERT-architecture Contriever / dragon checkpoints only)")
     from . import search as _search                      # device is resolved there (tests patch it)
@@ -54,9 +57,12 @@ def embed_passages(args, passages: Iterable[dict], model, tokenizer) -> Tuple[li
     batch_ids, batch_text = [], []
 
     def flush():
-        enc = _tokenize(tokenizer, batch_text, max_len)
-        enc = {k: v.to(_search.device) for k, v in enc.items()}
-        out = model(**enc)
+        if st:                               # the model's own tokenisation and max_seq_length (reference :25-40)
+            out = model.encode_batch(batch_text)
+        else:
+            enc = _tokenize(tokenizer, batch_text, max_len)
+            enc = {k: v.to(_search.device) for k, v in enc.items()}
+            out = model(**enc)
         if "contriever" not in name and hasattr(out, "last_hidden_state"):
             out = out.last_hidden_state[:, 0, :]
         out = out if out.dtype == torch.float16 else out.float()
@@ -118,6 +124,8 @@ def load_passage_shard(args, shard_id: int) -> List[dict]:
 def load_passage_encoder(args):
     name = str(args.model_name_or_path)
     from . import encoder as enc
+    if enc.is_sentence_transformers_name(name) and not ("contriever" in name or "dragon" in name):
+        return enc.load_sentence_transformer(name), None  # reference :130: SentenceTransformer(name), no tokenizer
     if any(t in name for t in _UNSUPPORTED) or not ("contriever" in name or "dragon" in name):
         print(f"{name} is not supported!")
         raise AttributeError(name)

@@ -7,6 +7,11 @@
 The forward pass is librsb's `rsb_bert_forward` (wgmma tensor-core GEMMs fed by TMA with fused bias / GELU /
 residual epilogues, fused embedding+LayerNorm, shared-memory attention, mean / CLS pooling) on the un-padded
 token stream.  No CPU / eager-PyTorch fallback: constructing the model without CUDA raises.
+
+The same library runs the sentence-transformers retrievers the reference loads with `SentenceTransformer(name)`
+(`src/search.py:49-61`, `src/embed.py:25-40`): `load_sentence_transformer(path)` reads the model directory into a
+`SentenceTransformerEncoder` whose transformer is a T5 encoder (`B200T5Encoder`, GTR-T5) or a BERT-base model
+(`B200Contriever`, e5-base), with the Pooling -> Dense -> Normalize head run by `rsb_bert_forward` as well.
 """
 from __future__ import annotations
 
@@ -46,24 +51,31 @@ class B200Contriever:
     # so the batch composition does not change any sequence's output; 2048 is where the GEMMs fill the GPU.
     encode_group = 2048
 
-    def __init__(self, config=None, pooling: str = "average", device=None):
+    def __init__(self, config=None, pooling: str = "average", device=None, dense: bool = False, normalize: bool = False):
+        """`dense` / `normalize` add the sentence-transformers head after the pooling: a 768 x 768 Linear
+        (`dense.weight`, optional `dense.bias`) and L2 normalisation."""
         if not torch.cuda.is_available():
-            raise RuntimeError("B200Contriever needs a CUDA device (sm_90a): there is no CPU path")
+            raise RuntimeError(f"{type(self).__name__} needs a CUDA device (sm_90a): there is no CPU path")
         if pooling not in ("average", "cls"):
             raise ValueError(f"unknown pooling {pooling!r}")
         self.L = _lib.lib()
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        self.config = {k: _cfg_get(config or {}, k) for k in BERT_BASE}
-        self.pooling = pooling
+        self.pooling, self.dense, self.normalize = pooling, bool(dense), bool(normalize)
+        self._pool_flags = ((_lib.POOL_MEAN if pooling == "average" else _lib.POOL_CLS)
+                            | (_lib.POOL_DENSE if dense else 0) | (_lib.POOL_NORMALIZE if normalize else 0))
         self._h = ctypes.c_void_p(0)
-        c = self.config
-        with torch.cuda.device(self.device):
-            rc = self.L.rsb_bert_create(c["hidden_size"], c["num_hidden_layers"], c["num_attention_heads"],
-                                        c["intermediate_size"], c["vocab_size"], c["max_position_embeddings"],
-                                        c["type_vocab_size"], ctypes.c_float(c["layer_norm_eps"]), ctypes.byref(self._h))
-        self._check(rc)
         self._ws: Optional[torch.Tensor] = None
         self.loaded = set()
+        with torch.cuda.device(self.device):
+            self._create(config)
+
+    def _create(self, config):
+        self.config = {k: _cfg_get(config or {}, k) for k in BERT_BASE}
+        c = self.config
+        rc = self.L.rsb_bert_create(c["hidden_size"], c["num_hidden_layers"], c["num_attention_heads"],
+                                    c["intermediate_size"], c["vocab_size"], c["max_position_embeddings"],
+                                    c["type_vocab_size"], ctypes.c_float(c["layer_norm_eps"]), ctypes.byref(self._h))
+        self._check(rc)
 
     def _check(self, rc):
         if rc == _lib.RSB_OK:
@@ -84,6 +96,8 @@ class B200Contriever:
                 self._h = ctypes.c_void_p(0)
         except Exception:
             pass
+
+    _ALIASES: Dict[str, str] = {}
 
     # -- nn.Module-like surface used by the reference -----------------------------------------------------------
     def eval(self):
@@ -113,7 +127,7 @@ class B200Contriever:
                     unexpected.append(name)
                     continue
                 self._check(rc)
-                self.loaded.add(name)
+                self.loaded.add(self._ALIASES.get(name, name))
             torch.cuda.current_stream().synchronize()
         if strict and unexpected:
             raise KeyError(f"unexpected keys in state_dict: {unexpected[:5]}")
@@ -131,7 +145,7 @@ class B200Contriever:
             self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
         tt = ctypes.c_void_p(token_types.data_ptr()) if token_types is not None else ctypes.c_void_p(0)
         rc = self.L.rsb_bert_forward(self._h, ctypes.c_void_p(ids.data_ptr()), tt, ctypes.c_void_p(cu_seqlens.data_ptr()),
-                                     B, T, int(max_seqlen), 0 if self.pooling == "average" else 1,
+                                     B, T, int(max_seqlen), self._pool_flags,
                                      ctypes.c_void_p(out.data_ptr()), ctypes.c_void_p(self._ws.data_ptr()),
                                      self._ws.numel(), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
         self._check(rc)
@@ -156,7 +170,7 @@ class B200Contriever:
     forward = __call__
 
     def expected_keys(self):
-        return expected_keys(self.config["num_hidden_layers"])
+        return expected_keys(self.config["num_hidden_layers"]) + (["dense.weight"] if self.dense else [])
 
     def missing_keys(self):
         return [k for k in self.expected_keys() if k not in self.loaded]
@@ -270,3 +284,264 @@ def load_retriever(model_path: str, tokenizer_name: Optional[str] = None, poolin
     model.load_state_dict(sd, strict=False)
     model.require_all_weights(model_path)
     return model, tokenizer, model_id
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# T5 encoder (GTR-T5) and the sentence-transformers model directory
+# ----------------------------------------------------------------------------------------------------------------
+T5_BASE = dict(num_layers=12, d_ff=3072, vocab_size=32128, relative_attention_num_buckets=32,
+               relative_attention_max_distance=128, layer_norm_epsilon=1e-6)
+T5_MAX_REL = 511            # relative positions -511..511 cover every pair of a 512-token sequence
+
+
+def t5_bucket_table(num_buckets: int, max_distance: int) -> torch.Tensor:
+    """int32 [1023]: the bucket of relative position r = key - query at index r + 511.  HF T5Attention's
+    `_relative_position_bucket` (bidirectional encoder), with its fp32 log expression evaluated once on the host so
+    that the device never rounds a logarithm differently."""
+    import math
+    r = torch.arange(-T5_MAX_REL, T5_MAX_REL + 1, dtype=torch.long)
+    nb = num_buckets // 2
+    buckets = (r > 0).to(torch.long) * nb
+    a = torch.abs(r)
+    max_exact = nb // 2
+    large = max_exact + (torch.log(a.float() / max_exact) / math.log(max_distance / max_exact)
+                         * (nb - max_exact)).to(torch.long)
+    large = torch.min(large, torch.full_like(large, nb - 1))
+    return (buckets + torch.where(a < max_exact, a, large)).to(torch.int32)
+
+
+def t5_expected_keys(num_layers: int):
+    """Every weight the T5 forward reads (HF T5EncoderModel names)."""
+    keys = ["shared.weight", "encoder.final_layer_norm.weight",
+            "encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight"]
+    for i in range(num_layers):
+        p = f"encoder.block.{i}.layer."
+        keys += [p + f"0.SelfAttention.{m}.weight" for m in "qkvo"]
+        keys += [p + "0.layer_norm.weight", p + "1.DenseReluDense.wi.weight", p + "1.DenseReluDense.wo.weight",
+                 p + "1.layer_norm.weight"]
+    return keys
+
+
+def _t5_config(config) -> dict:
+    """The T5 geometry the kernels run (d_model 768, 12 heads of 64, ReLU feed-forward), or AttributeError."""
+    get = (lambda k, d=None: config.get(k, d)) if isinstance(config, dict) else (lambda k, d=None: getattr(config, k, d))
+    geom = dict(d_model=get("d_model", 768), num_heads=get("num_heads", 12), d_kv=get("d_kv", 64),
+                feed_forward_proj=get("feed_forward_proj", "relu"))
+    if geom != dict(d_model=768, num_heads=12, d_kv=64, feed_forward_proj="relu"):
+        raise AttributeError(f"unsupported T5 geometry {geom}: only d_model 768, 12 heads of 64 and "
+                             f"feed_forward_proj 'relu' (T5 v1.0, GTR-T5-base) run on the GPU path")
+    return {k: get(k, T5_BASE[k]) for k in T5_BASE}
+
+
+class B200T5Encoder(B200Contriever):
+    """HF `T5EncoderModel` (fp16, d_model 768, 12 heads of 64, ReLU feed-forward) + mean / first-token pooling and the
+    optional sentence-transformers Dense / Normalize head, on librsb (`rsb_t5_create`).  Same call surface as
+    `B200Contriever`; `token_type_ids` are ignored.  The relative-position bucket table is uploaded at construction."""
+
+    _ALIASES = {"encoder.embed_tokens.weight": "shared.weight"}     # tied embeddings: either name loads them
+
+    def _create(self, config):
+        self.config = dict(_t5_config(config or {}), hidden_size=768)     # hidden_size: the output width
+        c = self.config
+        rc = self.L.rsb_t5_create(c["num_layers"], c["d_ff"], c["vocab_size"], c["relative_attention_num_buckets"],
+                                  c["relative_attention_max_distance"], ctypes.c_float(c["layer_norm_epsilon"]),
+                                  ctypes.byref(self._h))
+        self._check(rc)
+        table = t5_bucket_table(c["relative_attention_num_buckets"], c["relative_attention_max_distance"]).to(self.device)
+        rc = self.L.rsb_bert_load(self._h, b"relative_position_bucket", ctypes.c_void_p(table.data_ptr()), table.numel(),
+                                  ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
+        self._check(rc)
+
+    def expected_keys(self):
+        return t5_expected_keys(self.config["num_layers"]) + (["dense.weight"] if self.dense else [])
+
+    def require_all_weights(self, source: str = "state_dict"):
+        missing = self.missing_keys()
+        if missing:
+            raise KeyError(f"{source}: {len(missing)} of {len(self.expected_keys())} T5 encoder weights were not found "
+                           f"(first missing: {missing[:4]}); keys must follow HF T5EncoderModel naming")
+
+
+def random_t5_state_dict(config=None, seed: int = 0, device="cpu", head: bool = True) -> Dict[str, torch.Tensor]:
+    """Seeded random-init T5 encoder weights with HF T5EncoderModel names, plus the sentence-transformers Dense
+    head (`dense.weight`, `dense.bias`) when `head` (benchmarks run without pretrained checkpoints)."""
+    c = _t5_config(config or {})
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    H, F = 768, c["d_ff"]
+
+    def n(*shape, std):
+        return (torch.randn(*shape, generator=g) * std).to(device)
+
+    sd = {"shared.weight": n(c["vocab_size"], H, std=0.5),
+          "encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight":
+              n(c["relative_attention_num_buckets"], 12, std=0.5)}
+    for i in range(c["num_layers"]):
+        p = f"encoder.block.{i}.layer."
+        sd[p + "0.SelfAttention.q.weight"] = n(H, H, std=0.02)
+        for m in "kvo":
+            sd[p + f"0.SelfAttention.{m}.weight"] = n(H, H, std=0.04)
+        sd[p + "0.layer_norm.weight"] = 1.0 + n(H, std=0.1)
+        sd[p + "1.DenseReluDense.wi.weight"] = n(F, H, std=0.04)
+        sd[p + "1.DenseReluDense.wo.weight"] = n(H, F, std=0.02)
+        sd[p + "1.layer_norm.weight"] = 1.0 + n(H, std=0.1)
+    sd["encoder.final_layer_norm.weight"] = 1.0 + n(H, std=0.1)
+    if head:
+        sd["dense.weight"] = n(H, H, std=0.04)
+        sd["dense.bias"] = n(H, std=0.02)
+    return sd
+
+
+_ST_MODULE = "sentence_transformers.models."
+_OTHER_FAMILIES = ("Qwen3", "drama", "ReasonIR", "GRIT")
+
+
+def is_sentence_transformers_name(name: str) -> bool:
+    """The reference's name dispatch (`src/search.py:49,244`, `src/embed.py:25,130`) for the family this project
+    runs: "sentence-transformers" or "e5" in the name; Qwen3 and the other decoder-LLM embedders are not run here."""
+    return ("sentence-transformers" in name or "e5" in name) and not any(t in name for t in _OTHER_FAMILIES)
+
+
+class SentenceTransformerEncoder:
+    """A sentence-transformers model (`SentenceTransformer(path)`, reference `src/search.py:244-246`) on the GPU:
+    host tokenisation as its Transformer module does it (strip, optional lower-casing, truncation to
+    `max_seq_length`), then one `rsb_bert_forward` that runs the transformer, the pooling and the head."""
+
+    def __init__(self, model: B200Contriever, tokenizer, max_seq_length: int, do_lower_case: bool, path: str = ""):
+        self.model, self.tokenizer = model, tokenizer
+        self.max_seq_length, self.do_lower_case, self.path = int(max_seq_length), bool(do_lower_case), path
+
+    @property
+    def encode_group(self) -> int:
+        return self.model.encode_group
+
+    def eval(self):
+        return self
+
+    def half(self):
+        return self
+
+    def to(self, *a, **k):
+        return self
+
+    def encode_batch(self, texts) -> torch.Tensor:
+        """list[str] -> fp16 [n, 768] on the device."""
+        texts = [str(t).strip() for t in texts]
+        if self.do_lower_case:
+            texts = [t.lower() for t in texts]
+        enc = self.tokenizer(texts, return_tensors="pt", max_length=self.max_seq_length, padding=True, truncation=True)
+        return self.model(input_ids=enc["input_ids"], attention_mask=enc["attention_mask"],
+                          token_type_ids=enc.get("token_type_ids"))
+
+
+def _read_json(path: str) -> dict:
+    import json
+    with open(path) as f:
+        return json.load(f)
+
+
+def _read_weights(directory: str) -> Dict[str, torch.Tensor]:
+    import os
+    st = os.path.join(directory, "model.safetensors")
+    if os.path.exists(st):
+        from safetensors.torch import load_file
+        return load_file(st)
+    pt = os.path.join(directory, "pytorch_model.bin")
+    if os.path.exists(pt):
+        return torch.load(pt, map_location="cpu", weights_only=True)
+    raise AttributeError(f"{directory}: neither model.safetensors nor pytorch_model.bin is present")
+
+
+def _resolve_model_dir(path: str) -> str:
+    import os
+    if os.path.isdir(path):
+        return path
+    try:
+        from huggingface_hub import snapshot_download
+        return snapshot_download(path, local_files_only=True)
+    except Exception as e:  # noqa: BLE001 -- any failure means the files are not available locally
+        raise FileNotFoundError(f"{path}: not a local directory and not in the Hugging Face cache ({e})") from e
+
+
+def read_sentence_transformer(path: str) -> dict:
+    """Validates a sentence-transformers directory against what the GPU path runs and returns its description:
+    {"dir", "arch" ("t5" | "bert"), "config", "max_seq_length", "do_lower_case", "pooling" ("average" | "cls"),
+    "dense" (None or {"in_features", "out_features", "bias", "dir"}), "normalize"}.  Pure host code; anything it
+    does not support raises AttributeError naming it."""
+    import os
+    root = _resolve_model_dir(path)
+    mpath = os.path.join(root, "modules.json")
+    if not os.path.exists(mpath):
+        raise AttributeError(f"{path}: modules.json not found, not a sentence-transformers directory")
+    mods = sorted(_read_json(mpath), key=lambda m: int(m.get("idx", 0)))
+    kinds = [str(m.get("type", "")).replace(_ST_MODULE, "") for m in mods]
+    if kinds[:2] != ["Transformer", "Pooling"] or kinds[2:] not in ([], ["Dense"], ["Normalize"], ["Dense", "Normalize"]):
+        raise AttributeError(f"{path}: unsupported module stack {kinds}; supported: Transformer, Pooling, "
+                             f"optionally Dense, optionally Normalize")
+    mdir = [os.path.join(root, m.get("path", "")) for m in mods]
+    # 1. Transformer
+    sbc = os.path.join(mdir[0], "sentence_bert_config.json")
+    st_cfg = _read_json(sbc) if os.path.exists(sbc) else {}
+    max_len = int(st_cfg.get("max_seq_length") or 512)
+    if max_len > 512:
+        raise AttributeError(f"{path}: max_seq_length {max_len} > 512 is not supported")
+    cfg = _read_json(os.path.join(mdir[0], "config.json"))
+    arch = cfg.get("model_type")
+    if arch == "t5":
+        _t5_config(cfg)
+    elif arch == "bert":
+        geom = {k: cfg.get(k) for k in ("hidden_size", "num_attention_heads", "hidden_act")}
+        if geom != dict(hidden_size=768, num_attention_heads=12, hidden_act="gelu") or int(cfg.get("intermediate_size", 0)) % 128:
+            raise AttributeError(f"{path}: unsupported BERT geometry {geom}: only BERT-base (hidden 768, 12 heads, "
+                                 f"GELU) runs on the GPU path")
+    else:
+        raise AttributeError(f"{path}: transformer model_type {arch!r} is not supported (T5 encoder or BERT-base only)")
+    # 2. Pooling
+    pc = _read_json(os.path.join(mdir[1], "config.json"))
+    modes = sorted(k for k, v in pc.items() if k.startswith("pooling_mode_") and v)
+    if modes == ["pooling_mode_mean_tokens"]:
+        pooling = "average"
+    elif modes == ["pooling_mode_cls_token"]:
+        pooling = "cls"
+    else:
+        raise AttributeError(f"{path}: unsupported pooling modes {modes}; exactly one of pooling_mode_mean_tokens "
+                             f"or pooling_mode_cls_token")
+    if int(pc.get("word_embedding_dimension", 768)) != 768:
+        raise AttributeError(f"{path}: pooling dimension {pc.get('word_embedding_dimension')} is not 768")
+    # 3. Dense
+    dense = None
+    if "Dense" in kinds:
+        i = kinds.index("Dense")
+        dc = _read_json(os.path.join(mdir[i], "config.json"))
+        act = str(dc.get("activation_function", "torch.nn.modules.linear.Identity"))
+        if (int(dc.get("in_features", 0)), int(dc.get("out_features", 0))) != (768, 768):
+            raise AttributeError(f"{path}: Dense {dc.get('in_features')} -> {dc.get('out_features')} is not supported "
+                                 f"(768 -> 768 only)")
+        if not act.endswith("Identity"):
+            raise AttributeError(f"{path}: Dense activation {act} is not supported (Identity only)")
+        dense = dict(in_features=768, out_features=768, bias=bool(dc.get("bias", True)), dir=mdir[i])
+    return dict(dir=mdir[0], arch=arch, config=cfg, max_seq_length=max_len,
+                do_lower_case=bool(st_cfg.get("do_lower_case", False)), pooling=pooling, dense=dense,
+                normalize="Normalize" in kinds)
+
+
+def load_sentence_transformer(path: str, device=None) -> SentenceTransformerEncoder:
+    """`SentenceTransformer(path)` for the supported stacks (see `read_sentence_transformer`): weights and tokenizer
+    from the local directory or the Hugging Face cache (no download)."""
+    import transformers
+    d = read_sentence_transformer(path)
+    sd = _read_weights(d["dir"])
+    if d["dense"] is not None:
+        hw = _read_weights(d["dense"]["dir"])
+        sd["dense.weight"] = hw["linear.weight"]
+        if d["dense"]["bias"]:
+            sd["dense.bias"] = hw["linear.bias"]
+    cls = B200T5Encoder if d["arch"] == "t5" else B200Contriever
+    if d["arch"] == "bert":
+        sd = strip_wrapper_prefix(sd)
+    else:
+        sd = {k: v for k, v in sd.items() if not k.startswith("decoder.") and not k.startswith("lm_head.")}
+    model = cls(d["config"], d["pooling"], device=device, dense=d["dense"] is not None, normalize=d["normalize"])
+    model.load_state_dict(sd, strict=False)
+    model.require_all_weights(path)
+    tokenizer = transformers.AutoTokenizer.from_pretrained(d["dir"], local_files_only=True)
+    return SentenceTransformerEncoder(model, tokenizer, d["max_seq_length"], d["do_lower_case"], path)

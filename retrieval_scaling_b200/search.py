@@ -41,10 +41,15 @@ def _tokenize(tokenizer, texts: List[str], max_length: int):
 def embed_queries(args, queries, model, tokenizer, model_name_or_path):
     """list[str] -> np.ndarray [nq, d].  Batches of `per_gpu_batch_size`, pad-to-longest, truncate to
     `question_maxlength`; Contriever models mean-pool inside the model, other HF BERT checkpoints (dragon*)
-    take the CLS row (`output.last_hidden_state[:, 0, :]`, reference :93-94)."""
-    if any(t in model_name_or_path for t in ("sentence-transformers", "e5", "Qwen3", "drama", "ReasonIR", "GRIT")):
+    take the CLS row (`output.last_hidden_state[:, 0, :]`, reference :93-94).  A sentence-transformers model
+    (`encoder.SentenceTransformerEncoder`, reference :49-61) tokenises with its own `max_seq_length` and returns its
+    pooled (and Dense / Normalize) rows."""
+    from .encoder import SentenceTransformerEncoder, is_sentence_transformers_name
+    st = isinstance(model, SentenceTransformerEncoder) and is_sentence_transformers_name(model_name_or_path)
+    if not st and any(t in model_name_or_path for t in ("sentence-transformers", "e5", "Qwen3", "drama", "ReasonIR", "GRIT")):
         raise AttributeError(f"{model_name_or_path}: this encoder family is out of scope of the GPU hot path "
-                             f"(BERT-architecture Contriever / dragon checkpoints only)")
+                             f"(BERT-architecture Contriever / dragon checkpoints and sentence-transformers T5 / "
+                             f"BERT-base models loaded with encoder.load_sentence_transformer only)")
     if hasattr(model, "eval"):
         model.eval()
     embeddings, batch = [], []
@@ -65,9 +70,12 @@ def embed_queries(args, queries, model, tokenizer, model_name_or_path):
                 q = _normalize_text(q)
             batch.append(q)
             if len(batch) == group or k == len(queries) - 1:
-                enc = _tokenize(tokenizer, batch, int(args.question_maxlength))
-                enc = {kk: vv.to(device) for kk, vv in enc.items()}
-                out = model(**enc)
+                if st:
+                    out = model.encode_batch(batch)
+                else:
+                    enc = _tokenize(tokenizer, batch, int(args.question_maxlength))
+                    enc = {kk: vv.to(device) for kk, vv in enc.items()}
+                    out = model(**enc)
                 if "contriever" not in model_name_or_path and hasattr(out, "last_hidden_state"):
                     out = out.last_hidden_state[:, 0, :]
                 embeddings.append(out)
@@ -175,6 +183,8 @@ def load_query_encoder(cfg):
                                                  pooling="average" if "contriever" in name else "cls",
                                                  fp16=not cfg.datastore.index.get("no_fp16", False))
         return model, tokenizer
+    if enc.is_sentence_transformers_name(name):         # reference :244-246: SentenceTransformer(name), no tokenizer
+        return enc.load_sentence_transformer(name), None
     print(f"{name} is not supported!")
     raise AttributeError(name)
 
