@@ -412,14 +412,28 @@ size_t rsb_bert_workspace_bytes(rsb_bert_t* h, int total_tokens);
 /* pooling: RSB_POOL_MEAN (0) = mean over tokens (Contriever), RSB_POOL_CLS (1) = CLS row, optionally OR-ed with the
  * sentence-transformers head bits: RSB_POOL_DENSE (fp16 Linear 768 -> 768 on the pooled rows; RSB_ERR_STATE if
  * dense.weight was not loaded) and RSB_POOL_NORMALIZE (x / max(||x||_2, 1e-12), after the Dense layer).  A T5 handle
- * returns RSB_ERR_STATE until both of its bias tables are loaded.  out_f16_dev [B, 768] fp16 */
-enum { RSB_POOL_MEAN = 0, RSB_POOL_CLS = 1, RSB_POOL_DENSE = 2, RSB_POOL_NORMALIZE = 4 };
+ * returns RSB_ERR_STATE until both of its bias tables are loaded.  out_f16_dev [B, 768] fp16.
+ * Diagnostic, not used on the product path: RSB_POOL_TOKENS (alone; with any other bit RSB_ERR_INVALID) skips the
+ * pooling and writes the final hidden states [T, 768] fp16 to out_f16_dev (BERT: after the last LayerNorm; T5: after
+ * final_layer_norm), so that tests can compare every token row with a reference. */
+enum { RSB_POOL_MEAN = 0, RSB_POOL_CLS = 1, RSB_POOL_DENSE = 2, RSB_POOL_NORMALIZE = 4, RSB_POOL_TOKENS = 8 };
 int rsb_bert_forward(rsb_bert_t* h, const int32_t* input_ids_dev, const int32_t* token_type_ids_dev,
                      const int32_t* cu_seqlens_dev, int B, int T, int max_seqlen, int pooling, void* out_f16_dev,
                      void* ws_dev, size_t ws_bytes, rsb_stream_t stream);
 int64_t rsb_bert_launches(rsb_bert_t* h);
+/* Diagnostic, not used on the product path: one attention step of rsb_bert_forward on a caller's tensors, through
+ * the forward's own dispatch (the list of sequences longer than 32 tokens, the flash kernel on the handle's side
+ * stream, the kernel for sequences of <= 32 tokens on `stream`, the join).  qkv_dev [T, 2304] fp16 holds each token's
+ * Q | K | V (12 heads of 64 each), ctx_dev [T, 768] fp16 receives softmax(scores) V per sequence and head; rows of
+ * zero-length sequences and rows past cu_seqlens[B] are not written.  BERT handles score q.k / 8; T5 handles score
+ * fp16(fp16(q.k) + bias[key - query]) from the loaded bias tables (RSB_ERR_STATE until both are loaded).
+ * max_seqlen > 512 or above the handle's max_pos: RSB_ERR_UNSUPPORTED. */
+int rsb_bert_attention(rsb_bert_t* h, const void* qkv_dev, const int32_t* cu_seqlens_dev, int B, int T, int max_seqlen,
+                       void* ctx_dev, rsb_stream_t stream);
 /* the encoder's tensor-core GEMM on its own: C[M,N] = A[M,K] . W[N,K]^T + bias (epilogue 0), GELU (1),
- * + residual (2) or ReLU (3); all fp16 row-major device pointers, N % 128 == 0, K % 64 == 0 */
+ * + residual (2) or ReLU (3); all fp16 row-major device pointers, N % 128 == 0, K % 64 == 0.  OR-ing
+ * RSB_GEMM_REVERSED into the epilogue visits the 128-row tiles last-to-first, the order of the forward's FFN2. */
+enum { RSB_GEMM_REVERSED = 256 };
 int rsb_gemm_f16(const void* A_dev, const void* W_dev, const void* bias_dev, const void* residual_dev, void* C_dev,
                  int M, int N, int K, int epilogue, rsb_stream_t stream);
 

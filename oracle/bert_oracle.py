@@ -49,9 +49,15 @@ def seeded_state_dict(config: dict, seed: int) -> Dict[str, torch.Tensor]:
     return sd
 
 
-def bert_forward(sd: Dict[str, torch.Tensor], config: dict, input_ids, attention_mask, token_type_ids=None,
-                 pooling: str = "average", dtype=torch.float32):
-    """Returns [B, hidden] in `dtype` (float32 = exact restatement; float16 on CUDA mirrors `.half()`)."""
+def attention(q, k, v, add_mask, head_dim: int):
+    """HF BertSelfAttention core on [B, heads, S, hd] tensors: softmax(q k^T / sqrt(hd) + add_mask) v."""
+    att = torch.softmax((q @ k.transpose(-1, -2)) / math.sqrt(head_dim) + add_mask, dim=-1)
+    return att @ v
+
+
+def bert_hidden(sd: Dict[str, torch.Tensor], config: dict, input_ids, attention_mask, token_type_ids=None,
+                dtype=torch.float32):
+    """last_hidden_state [B, S, hidden] of HF BertModel in `dtype` (pad positions not zeroed)."""
     dev = input_ids.device
     w = {k: v.to(device=dev, dtype=dtype) for k, v in sd.items()}
     B, S = input_ids.shape
@@ -71,13 +77,20 @@ def bert_forward(sd: Dict[str, torch.Tensor], config: dict, input_ids, attention
         q = lin("attention.self.query", x).view(B, S, nh, hd).transpose(1, 2)
         k = lin("attention.self.key", x).view(B, S, nh, hd).transpose(1, 2)
         v = lin("attention.self.value", x).view(B, S, nh, hd).transpose(1, 2)
-        att = torch.softmax((q @ k.transpose(-1, -2)) / math.sqrt(hd) + add_mask, dim=-1)
-        ctx = (att @ v).transpose(1, 2).reshape(B, S, H)
+        ctx = attention(q, k, v, add_mask, hd).transpose(1, 2).reshape(B, S, H)
         x = F.layer_norm(lin("attention.output.dense", ctx) + x, (H,), w[p + "attention.output.LayerNorm.weight"],
                          w[p + "attention.output.LayerNorm.bias"], eps)
         ff = F.gelu(lin("intermediate.dense", x))           # exact erf GELU (hidden_act="gelu")
         x = F.layer_norm(lin("output.dense", ff) + x, (H,), w[p + "output.LayerNorm.weight"],
                          w[p + "output.LayerNorm.bias"], eps)
+    return x
+
+
+def bert_forward(sd: Dict[str, torch.Tensor], config: dict, input_ids, attention_mask, token_type_ids=None,
+                 pooling: str = "average", dtype=torch.float32):
+    """Returns [B, hidden] in `dtype` (float32 = exact restatement; float16 on CUDA mirrors `.half()`)."""
+    x = bert_hidden(sd, config, input_ids, attention_mask, token_type_ids, dtype)
+    mask = attention_mask.bool()
     last = x.masked_fill(~mask[..., None], 0.0)              # contriever.py:46
     if pooling == "average":
         return last.sum(dim=1) / attention_mask.sum(dim=1)[..., None].to(dtype)   # contriever.py:49

@@ -88,6 +88,15 @@ def _clamp(x):
     return torch.clamp(x, min=-c, max=c)
 
 
+def attention(q, k, v, position_bias):
+    """HF T5Attention core on [B, heads, S, d_kv] tensors: scores = q k^T (no scaling) + position_bias (the relative
+    bias plus the key mask), softmax in fp32 and cast back, times v."""
+    scores = torch.matmul(q, k.transpose(3, 2))
+    scores += position_bias
+    att = torch.softmax(scores.float(), dim=-1).type_as(scores)
+    return torch.matmul(att, v)
+
+
 def t5_hidden(sd: Dict[str, torch.Tensor], config: dict, input_ids, attention_mask, dtype=torch.float32):
     """last_hidden_state [B, S, 768] of T5EncoderModel in `dtype` (float32 = exact restatement; float16 on CUDA
     mirrors `.half()`)."""
@@ -106,10 +115,7 @@ def t5_hidden(sd: Dict[str, torch.Tensor], config: dict, input_ids, attention_ma
         p = f"encoder.block.{i}.layer."
         h = _rms(x, w[p + "0.layer_norm.weight"], eps)
         q, k, v = (F.linear(h, w[p + f"0.SelfAttention.{m}.weight"]).view(B, S, nh, hd).transpose(1, 2) for m in "qkv")
-        scores = torch.matmul(q, k.transpose(3, 2))
-        scores += position_bias
-        att = torch.softmax(scores.float(), dim=-1).type_as(scores)
-        ctx = torch.matmul(att, v).transpose(1, 2).reshape(B, S, nh * hd)
+        ctx = attention(q, k, v, position_bias).transpose(1, 2).reshape(B, S, nh * hd)
         x = _clamp(x + F.linear(ctx, w[p + "0.SelfAttention.o.weight"]))
         h = _rms(x, w[p + "1.layer_norm.weight"], eps)
         x = _clamp(x + F.linear(F.relu(F.linear(h, w[p + "1.DenseReluDense.wi.weight"])),

@@ -18,6 +18,8 @@ RSB_DTYPE_F32, RSB_DTYPE_F16, RSB_DTYPE_SQ8 = 0, 1, 2
  INFO_INDEX_BYTES, INFO_DTYPE, INFO_BY_RESIDUAL, INFO_HOST_BYTES, INFO_DEVICE_ROWS) = range(13)
 OPT_COARSE_TENSOR, OPT_BY_RESIDUAL, OPT_DEVICE_ROWS, OPT_STAGING_BYTES = 0, 1, 2, 3
 POOL_MEAN, POOL_CLS, POOL_DENSE, POOL_NORMALIZE = 0, 1, 2, 4
+POOL_TOKENS = 8                  # diagnostic: the final hidden states [T, 768] instead of a pooled row per sequence
+GEMM_REVERSED = 256              # rsb_gemm_f16 epilogue bit: row tiles last-to-first (the forward's FFN2 order)
 PROF_NAMES = ("coarse_ms", "setup_ms", "lut_ms", "scan_ms", "merge_ms", "scan_bytes", "pairs", "launches", "scan_path",
               "rescored")
 
@@ -85,6 +87,7 @@ SIGNATURES = [
     ("rsb_bert_forward", c_int, [_H, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                                  c_size_t, c_void_p]),
     ("rsb_bert_launches", c_int64, [_H]),
+    ("rsb_bert_attention", c_int, [_H, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),   # diagnostic
     ("rsb_gemm_f16", c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     ("rsb_debug_smem_base", c_int, []),
     ("rsb_pq_lut_floats", c_int, [_H]),

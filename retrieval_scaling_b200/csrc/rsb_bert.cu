@@ -939,6 +939,71 @@ int launch_gemm(const __half* A, int M, const Linear& lin, __half* C, const __ha
     return RSB_OK;
 }
 
+// Per-forward set-up of the attention step: the kernels' shared-memory attributes, the side stream and its events, and
+// -- when max_seqlen > 32 -- the list of sequences the flash kernel takes (collect_long_kernel), built once and read by
+// every layer's launch_attention.
+int prepare_attention(rsb_bert* h, const int* cu_seqlens, int B, int max_seqlen, cudaStream_t st) {
+    static rsb::PerDeviceFlag att_configured;
+    if (att_configured.first()) {
+        cudaFuncSetAttribute(attention_mma32_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * ATT32_WARP_BYTES);
+        cudaFuncSetAttribute(attention_mma32_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             4 * (ATT32_WARP_BYTES + ATT32_T5_BIAS_BYTES));
+    }
+    if (!h->side) {
+        cudaStreamCreateWithFlags(&h->side, cudaStreamNonBlocking);
+        cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming);
+        cudaEventCreateWithFlags(&h->ev_join, cudaEventDisableTiming);
+    }
+    if (max_seqlen > 32) {                               // list of the sequences the flash kernel has to take, once per forward
+        if (h->long_cap < B) {
+            cudaFree(h->long_list);
+            h->long_list = nullptr;
+            h->long_cap = 0;
+            if (cudaMalloc(&h->long_list, ((size_t)B + 1) * sizeof(int)) != cudaSuccess) return bfail(RSB_ERR_OOM, "long-sequence list");
+            h->long_cap = B;
+        }
+        cudaMemsetAsync(h->long_list + h->long_cap, 0, sizeof(int), st);          // the count lives behind the list
+        collect_long_kernel<<<(B + 255) / 256, 256, 0, st>>>(cu_seqlens, B, 32, h->long_list, h->long_list + h->long_cap);
+        h->launches++;
+    }
+    return RSB_OK;
+}
+
+// One attention step, ctx [T, 768] from qkv [T, 2304], after prepare_attention with the same cu_seqlens / B / max_seqlen.
+// Sequences of <= 32 tokens (queries): warp-per-(sequence, head) tensor-core kernel; longer ones (passages, the odd long
+// query): flash-style kernel on a side stream -- the two work on disjoint sequences of the same buffers -- joined
+// before the caller's next launch on st.
+void launch_attention(rsb_bert* h, const __half* qkv_p, const int* cu_seqlens, int B, int max_seqlen, __half* ctx_p,
+                      cudaStream_t st) {
+    const float scale = h->t5 ? 1.f : 0.125f;
+    const bool have_long = max_seqlen > 32;
+    if (have_long) {
+        cudaEventRecord(h->ev_fork, st);
+        cudaStreamWaitEvent(h->side, h->ev_fork, 0);
+        const int nqb = (max_seqlen + 127) / 128;
+        const long items = (long)B * h->heads * nqb;
+        const int fgrid = (int)std::min<long>(items, 2L * rsb::device_num_sms());   // 194 registers: two resident blocks per SM
+        if (h->t5)
+            attention_flash_kernel<true><<<fgrid, 128, 0, h->side>>>(qkv_p, cu_seqlens, ctx_p, scale, h->long_list,
+                                                                     h->long_list + h->long_cap, h->heads, nqb, h->relb);
+        else
+            attention_flash_kernel<false><<<fgrid, 128, 0, h->side>>>(qkv_p, cu_seqlens, ctx_p, scale, h->long_list,
+                                                                      h->long_list + h->long_cap, h->heads, nqb, nullptr);
+        cudaEventRecord(h->ev_join, h->side);
+        h->launches++;
+    }
+    const int nwarps = B * h->heads;
+    static const bool no_snake = getenv("RSB_NO_SNAKE") != nullptr;
+    if (h->t5)
+        attention_mma32_kernel<true><<<(nwarps + 3) / 4, 128, 4 * (ATT32_WARP_BYTES + ATT32_T5_BIAS_BYTES), st>>>(
+            qkv_p, cu_seqlens, ctx_p, scale, h->heads, B, no_snake ? 0 : 1, h->relb);
+    else
+        attention_mma32_kernel<false><<<(nwarps + 3) / 4, 128, 4 * ATT32_WARP_BYTES, st>>>(
+            qkv_p, cu_seqlens, ctx_p, scale, h->heads, B, no_snake ? 0 : 1, nullptr);
+    h->launches++;
+    if (have_long) cudaStreamWaitEvent(st, h->ev_join, 0);   // join before the attention-output GEMM
+}
+
 }  // namespace
 
 extern "C" const char* rsb_bert_last_error(void) { return g_berr.c_str(); }
@@ -1144,7 +1209,9 @@ extern "C" int rsb_bert_forward(rsb_bert_t* h, const int32_t* input_ids, const i
                                 void* ws, size_t ws_bytes, rsb_stream_t stream) {
     if (!h || !input_ids || !cu_seqlens || !out_f16) return bfail(RSB_ERR_INVALID, "null argument");
     if (B <= 0 || T <= 0) return bfail(RSB_ERR_INVALID, "empty batch");
-    if (pooling & ~(RSB_POOL_CLS | RSB_POOL_DENSE | RSB_POOL_NORMALIZE)) return bfail(RSB_ERR_INVALID, "unknown pooling bits%s %ld", "", (long)pooling);
+    if (pooling & ~(RSB_POOL_CLS | RSB_POOL_DENSE | RSB_POOL_NORMALIZE | RSB_POOL_TOKENS)) return bfail(RSB_ERR_INVALID, "unknown pooling bits%s %ld", "", (long)pooling);
+    if ((pooling & RSB_POOL_TOKENS) && pooling != RSB_POOL_TOKENS)
+        return bfail(RSB_ERR_INVALID, "RSB_POOL_TOKENS cannot be combined with other pooling bits%s (got %ld)", "", (long)pooling);
     if ((pooling & RSB_POOL_DENSE) && !h->dense_loaded) return bfail(RSB_ERR_STATE, "pooling asks for the Dense head but dense.weight was not loaded");
     if (h->t5 && !(h->bucket_loaded && h->rel_w_loaded))
         return bfail(RSB_ERR_STATE, "T5 forward before relative_position_bucket and the relative_attention_bias weight were loaded");
@@ -1173,30 +1240,8 @@ extern "C" int rsb_bert_forward(rsb_bert_t* h, const int32_t* input_ids, const i
                                                  h->emb_g, h->emb_b, h->eps, h->vocab, h->max_pos, Hs);
     }
     h->launches++;
-    static rsb::PerDeviceFlag att_configured;
-    if (att_configured.first()) {
-        cudaFuncSetAttribute(attention_mma32_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * ATT32_WARP_BYTES);
-        cudaFuncSetAttribute(attention_mma32_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             4 * (ATT32_WARP_BYTES + ATT32_T5_BIAS_BYTES));
-    }
-    if (!h->side) {
-        cudaStreamCreateWithFlags(&h->side, cudaStreamNonBlocking);
-        cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming);
-        cudaEventCreateWithFlags(&h->ev_join, cudaEventDisableTiming);
-    }
-    const bool have_long = max_seqlen > 32;
-    if (have_long) {                                     // list of the sequences the flash kernel has to take, once per forward
-        if (h->long_cap < B) {
-            cudaFree(h->long_list);
-            h->long_list = nullptr;
-            h->long_cap = 0;
-            if (cudaMalloc(&h->long_list, ((size_t)B + 1) * sizeof(int)) != cudaSuccess) return bfail(RSB_ERR_OOM, "long-sequence list");
-            h->long_cap = B;
-        }
-        cudaMemsetAsync(h->long_list + h->long_cap, 0, sizeof(int), st);          // the count lives behind the list
-        collect_long_kernel<<<(B + 255) / 256, 256, 0, st>>>(cu_seqlens, B, 32, h->long_list, h->long_list + h->long_cap);
-        h->launches++;
-    }
+    const int prc = prepare_attention(h, cu_seqlens, B, max_seqlen, st);
+    if (prc != RSB_OK) return prc;
     static const bool ln_v1 = getenv("RSB_LN_V1") != nullptr;
     const int ln_rows_grid = std::min(ln_grid, 3 * rsb::device_num_sms());   // 24 warps per SM, ~12 rows per warp at 41k tokens
     auto launch_ln = [&](const __half* x, const __half* g, const __half* b) {
@@ -1206,36 +1251,6 @@ extern "C" int rsb_bert_forward(rsb_bert_t* h, const int32_t* input_ids, const i
     // T5: Hs = rms(X) after the clamp that `flag` (the previous residual add's) calls for
     auto launch_rms = [&](__half* x, const __half* g, const int* flag) {
         layernorm_rows_kernel<true><<<ln_rows_grid, 256, 0, st>>>(x, T, g, nullptr, h->eps, Hs, flag);
-    };
-    auto launch_attention = [&](const __half* qkv_p, __half* ctx_p) {
-        // sequences of <= 32 tokens (queries): warp-per-(sequence, head) tensor-core kernel; longer ones (passages, the odd
-        // long query): flash-style kernel on a side stream -- the two work on disjoint sequences of the same buffers
-        const float scale = h->t5 ? 1.f : 0.125f;
-        if (have_long) {
-            cudaEventRecord(h->ev_fork, st);
-            cudaStreamWaitEvent(h->side, h->ev_fork, 0);
-            const int nqb = (max_seqlen + 127) / 128;
-            const long items = (long)B * h->heads * nqb;
-            const int fgrid = (int)std::min<long>(items, 2L * rsb::device_num_sms());   // 194 registers: two resident blocks per SM
-            if (h->t5)
-                attention_flash_kernel<true><<<fgrid, 128, 0, h->side>>>(qkv_p, cu_seqlens, ctx_p, scale, h->long_list,
-                                                                         h->long_list + h->long_cap, h->heads, nqb, h->relb);
-            else
-                attention_flash_kernel<false><<<fgrid, 128, 0, h->side>>>(qkv_p, cu_seqlens, ctx_p, scale, h->long_list,
-                                                                          h->long_list + h->long_cap, h->heads, nqb, nullptr);
-            cudaEventRecord(h->ev_join, h->side);
-            h->launches++;
-        }
-        const int nwarps = B * h->heads;
-        static const bool no_snake = getenv("RSB_NO_SNAKE") != nullptr;
-        if (h->t5)
-            attention_mma32_kernel<true><<<(nwarps + 3) / 4, 128, 4 * (ATT32_WARP_BYTES + ATT32_T5_BIAS_BYTES), st>>>(
-                qkv_p, cu_seqlens, ctx_p, scale, h->heads, B, no_snake ? 0 : 1, h->relb);
-        else
-            attention_mma32_kernel<false><<<(nwarps + 3) / 4, 128, 4 * ATT32_WARP_BYTES, st>>>(
-                qkv_p, cu_seqlens, ctx_p, scale, h->heads, B, no_snake ? 0 : 1, nullptr);
-        h->launches++;
-        if (have_long) cudaStreamWaitEvent(st, h->ev_join, 0);   // join before the attention-output GEMM
     };
     // RSB_BERT_PROFILE=1 (diagnostic): CUDA events between the kernels of the forward, summed per kernel kind over the
     // layers and printed to stderr after each forward -- per-kernel times INSIDE a back-to-back run (ncu's are isolated,
@@ -1264,7 +1279,7 @@ extern "C" int rsb_bert_forward(rsb_bert_t* h, const int32_t* input_ids, const i
             mark(P_LN1);
             if (launch_gemm<EPI_BIAS>(Hs, T, l.qkv, QKV, nullptr, st) != RSB_OK) return bfail(RSB_ERR_CUDA, gemm_fail);
             mark(P_QKV);
-            launch_attention(QKV, CTX);
+            launch_attention(h, QKV, cu_seqlens, B, max_seqlen, CTX, st);
             mark(P_ATT);
             if (launch_gemm<EPI_BIAS_RESIDUAL_INF>(CTX, T, l.attn_out, TMP, TMP, st, false, flags + 2 * li) != RSB_OK)
                 return bfail(RSB_ERR_CUDA, gemm_fail);
@@ -1279,7 +1294,7 @@ extern "C" int rsb_bert_forward(rsb_bert_t* h, const int32_t* input_ids, const i
         } else {
             if (launch_gemm<EPI_BIAS>(Hs, T, l.qkv, QKV, nullptr, st) != RSB_OK) return bfail(RSB_ERR_CUDA, gemm_fail);
             mark(P_QKV);
-            launch_attention(QKV, CTX);
+            launch_attention(h, QKV, cu_seqlens, B, max_seqlen, CTX, st);
             mark(P_ATT);
             if (launch_gemm<EPI_BIAS_RESIDUAL>(CTX, T, l.attn_out, TMP, Hs, st) != RSB_OK) return bfail(RSB_ERR_CUDA, gemm_fail);
             mark(P_AO);
@@ -1300,9 +1315,13 @@ extern "C" int rsb_bert_forward(rsb_bert_t* h, const int32_t* input_ids, const i
     }
     // sentence-transformers head: Pooling -> Dense (768 x 768 on the tensor-core GEMM, M = B) -> Normalize
     __half* out = static_cast<__half*>(out_f16);
-    __half* pooled = (pooling & RSB_POOL_DENSE) ? CTX : out;
-    pool_kernel<<<B, 256, 0, st>>>(Hs, cu_seqlens, pooling & RSB_POOL_CLS, pooled);
-    h->launches++;
+    if (pooling == RSB_POOL_TOKENS) {                    // diagnostic: the final hidden states themselves, [T, 768], no head
+        cudaMemcpyAsync(out, Hs, (size_t)T * h->hidden * 2, cudaMemcpyDeviceToDevice, st);
+    } else {
+        __half* pooled = (pooling & RSB_POOL_DENSE) ? CTX : out;
+        pool_kernel<<<B, 256, 0, st>>>(Hs, cu_seqlens, pooling & RSB_POOL_CLS, pooled);
+        h->launches++;
+    }
     if (pooling & RSB_POOL_DENSE) {
         if (launch_gemm<EPI_BIAS>(CTX, B, h->dense, out, nullptr, st) != RSB_OK) return bfail(RSB_ERR_CUDA, gemm_fail);
         h->launches++;
@@ -1332,12 +1351,33 @@ extern "C" int rsb_bert_forward(rsb_bert_t* h, const int32_t* input_ids, const i
 
 extern "C" int64_t rsb_bert_launches(rsb_bert_t* h) { return h ? h->launches : 0; }
 
+// diagnostic: one attention step of the forward on a caller's QKV, through the forward's own dispatch
+extern "C" int rsb_bert_attention(rsb_bert_t* h, const void* qkv, const int32_t* cu_seqlens, int B, int T, int max_seqlen,
+                                  void* ctx, rsb_stream_t stream) {
+    if (!h || !qkv || !cu_seqlens || !ctx) return bfail(RSB_ERR_INVALID, "null argument");
+    if (B <= 0 || T <= 0) return bfail(RSB_ERR_INVALID, "empty batch");
+    if (h->t5 && !(h->bucket_loaded && h->rel_w_loaded))
+        return bfail(RSB_ERR_STATE, "T5 attention before relative_position_bucket and the relative_attention_bias weight were loaded");
+    if (max_seqlen > ATT_MAXS || max_seqlen > h->max_pos)
+        return bfail(RSB_ERR_UNSUPPORTED, "sequence longer than %s%ld tokens", "", (long)std::min(ATT_MAXS, h->max_pos));
+    cudaStream_t st = (cudaStream_t)stream;
+    h->launches = 0;
+    const int rc = prepare_attention(h, cu_seqlens, B, max_seqlen, st);
+    if (rc != RSB_OK) return rc;
+    launch_attention(h, static_cast<const __half*>(qkv), cu_seqlens, B, max_seqlen, static_cast<__half*>(ctx), st);
+    cudaError_t e = cudaPeekAtLastError();
+    if (e != cudaSuccess) return bfail(RSB_ERR_CUDA, "attention launch failed: %s", cudaGetErrorString(e));
+    return RSB_OK;
+}
+
 // plain GEMM entry (tests / roofline of the tensor-core kernel): C[M,N] = A[M,K] W[N,K]^T + bias, epilogue as above
-// (0 bias, 1 GELU, 2 residual, 3 ReLU)
+// (0 bias, 1 GELU, 2 residual, 3 ReLU), OR-ed with RSB_GEMM_REVERSED to visit the row tiles last-to-first as FFN2 does
 extern "C" int rsb_gemm_f16(const void* A, const void* W, const void* bias, const void* residual, void* C, int M, int N,
                             int K, int epilogue, rsb_stream_t stream) {
     if (!A || !W || !bias || !C) return bfail(RSB_ERR_INVALID, "null argument");
     if (M <= 0 || N % G_BN || K % G_BK || N <= 0 || K <= 0) return bfail(RSB_ERR_INVALID, "need N %% 128 == 0 and K %% 64 == 0");
+    const bool m_rev = (epilogue & RSB_GEMM_REVERSED) != 0;
+    epilogue &= ~RSB_GEMM_REVERSED;
     if (epilogue == EPI_BIAS_RESIDUAL && !residual) return bfail(RSB_ERR_INVALID, "residual is NULL");
     Linear lin;
     lin.w = (__half*)W; lin.b = (__half*)bias; lin.N = N; lin.K = K;
@@ -1345,10 +1385,10 @@ extern "C" int rsb_gemm_f16(const void* A, const void* W, const void* bias, cons
     if (!lin.map_ok) return bfail(RSB_ERR_CUDA, "tensor map encode failed");
     cudaStream_t st = (cudaStream_t)stream;
     int rc;
-    if (epilogue == EPI_BIAS) rc = launch_gemm<EPI_BIAS>((const __half*)A, M, lin, (__half*)C, nullptr, st);
-    else if (epilogue == EPI_BIAS_GELU) rc = launch_gemm<EPI_BIAS_GELU>((const __half*)A, M, lin, (__half*)C, nullptr, st);
-    else if (epilogue == EPI_BIAS_RESIDUAL) rc = launch_gemm<EPI_BIAS_RESIDUAL>((const __half*)A, M, lin, (__half*)C, (const __half*)residual, st);
-    else if (epilogue == EPI_BIAS_RELU) rc = launch_gemm<EPI_BIAS_RELU>((const __half*)A, M, lin, (__half*)C, nullptr, st);
+    if (epilogue == EPI_BIAS) rc = launch_gemm<EPI_BIAS>((const __half*)A, M, lin, (__half*)C, nullptr, st, m_rev);
+    else if (epilogue == EPI_BIAS_GELU) rc = launch_gemm<EPI_BIAS_GELU>((const __half*)A, M, lin, (__half*)C, nullptr, st, m_rev);
+    else if (epilogue == EPI_BIAS_RESIDUAL) rc = launch_gemm<EPI_BIAS_RESIDUAL>((const __half*)A, M, lin, (__half*)C, (const __half*)residual, st, m_rev);
+    else if (epilogue == EPI_BIAS_RELU) rc = launch_gemm<EPI_BIAS_RELU>((const __half*)A, M, lin, (__half*)C, nullptr, st, m_rev);
     else return bfail(RSB_ERR_INVALID, "unknown epilogue");
     if (rc != RSB_OK) return bfail(RSB_ERR_CUDA, "tensor map encode failed");
     cudaError_t e = cudaPeekAtLastError();

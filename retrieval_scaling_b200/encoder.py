@@ -135,39 +135,54 @@ class B200Contriever:
 
     # -- forward ------------------------------------------------------------------------------------------------
     def forward_varlen(self, ids: torch.Tensor, cu_seqlens: torch.Tensor, max_seqlen: int,
-                       token_types: Optional[torch.Tensor] = None, total_tokens: Optional[int] = None) -> torch.Tensor:
+                       token_types: Optional[torch.Tensor] = None, total_tokens: Optional[int] = None,
+                       pool_flags: Optional[int] = None) -> torch.Tensor:
+        """[B, 768] fp16 with the model's pooling and head, or [T, 768] with pool_flags=_lib.POOL_TOKENS."""
         B = cu_seqlens.numel() - 1
         T = int(ids.numel()) if total_tokens is None else int(total_tokens)
-        out = torch.empty((B, self.config["hidden_size"]), dtype=torch.float16, device=self.device)
+        flags = self._pool_flags if pool_flags is None else int(pool_flags)
+        rows = T if flags == _lib.POOL_TOKENS else B
+        out = torch.empty((rows, self.config["hidden_size"]), dtype=torch.float16, device=self.device)
         need = self.L.rsb_bert_workspace_bytes(self._h, T)
         if self._ws is None or self._ws.numel() < need:
             self._ws = None
             self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
         tt = ctypes.c_void_p(token_types.data_ptr()) if token_types is not None else ctypes.c_void_p(0)
         rc = self.L.rsb_bert_forward(self._h, ctypes.c_void_p(ids.data_ptr()), tt, ctypes.c_void_p(cu_seqlens.data_ptr()),
-                                     B, T, int(max_seqlen), self._pool_flags,
+                                     B, T, int(max_seqlen), flags,
                                      ctypes.c_void_p(out.data_ptr()), ctypes.c_void_p(self._ws.data_ptr()),
                                      self._ws.numel(), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
         self._check(rc)
         return out
 
+    def _unpad(self, input_ids, attention_mask, token_type_ids):
+        input_ids = input_ids.to(self.device)
+        Bsz, S = input_ids.shape
+        if attention_mask is None:
+            attention_mask = torch.ones_like(input_ids)
+        mask = attention_mask.to(self.device).bool()
+        lens = mask.sum(dim=1, dtype=torch.int32)
+        cu = torch.zeros(Bsz + 1, dtype=torch.int32, device=self.device)
+        cu[1:] = torch.cumsum(lens, 0)
+        ids = input_ids[mask].to(torch.int32).contiguous()               # right-padded batches: order is preserved
+        tts = None
+        if token_type_ids is not None:
+            tts = token_type_ids.to(self.device)[mask].to(torch.int32).contiguous()
+        return ids, cu, S, tts
+
     def __call__(self, input_ids=None, attention_mask=None, token_type_ids=None, **_unused) -> torch.Tensor:
         with torch.cuda.device(self.device):
-            input_ids = input_ids.to(self.device)
-            Bsz, S = input_ids.shape
-            if attention_mask is None:
-                attention_mask = torch.ones_like(input_ids)
-            mask = attention_mask.to(self.device).bool()
-            lens = mask.sum(dim=1, dtype=torch.int32)
-            cu = torch.zeros(Bsz + 1, dtype=torch.int32, device=self.device)
-            cu[1:] = torch.cumsum(lens, 0)
-            ids = input_ids[mask].to(torch.int32).contiguous()           # right-padded batches: order is preserved
-            tts = None
-            if token_type_ids is not None:
-                tts = token_type_ids.to(self.device)[mask].to(torch.int32).contiguous()
+            ids, cu, S, tts = self._unpad(input_ids, attention_mask, token_type_ids)
             return self.forward_varlen(ids, cu, S, tts)
 
     forward = __call__
+
+    def hidden_states(self, input_ids=None, attention_mask=None, token_type_ids=None):
+        """Diagnostic (tests): the final hidden states of the real tokens, before any pooling -- BERT after the last
+        LayerNorm, T5 after final_layer_norm -- as ([T, 768] fp16 rows in batch order, cu_seqlens [B + 1] int32)."""
+        with torch.cuda.device(self.device):
+            ids, cu, S, tts = self._unpad(input_ids, attention_mask, token_type_ids)
+            return self.forward_varlen(ids, cu, S, tts, pool_flags=_lib.POOL_TOKENS), cu
 
     def expected_keys(self):
         return expected_keys(self.config["num_hidden_layers"]) + (["dense.weight"] if self.dense else [])
