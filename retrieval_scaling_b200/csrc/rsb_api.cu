@@ -12,6 +12,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <string>
 #include <vector>
 
@@ -56,12 +57,30 @@ struct Segment {
     int64_t n = 0;
 };
 
-// A page-locked host block of a tiered Flat index: rows [r0, r0 + n) of the index, exactly n * row_bytes bytes
+// A page-locked host block of a tiered index: rows [r0, r0 + n) of the index, exactly n * row_bytes bytes
 struct HostBlock {
     void* p = nullptr;
     int64_t r0 = 0, n = 0;
 };
 static const size_t kDefaultStagingBytes = (size_t)256 << 20;   // RSB_OPT_STAGING_BYTES default (per buffer)
+
+// The split of a tiered index between device and page-locked host memory: rows [0, dev_rows) live in the handle's
+// `payload`, rows [dev_rows, rows) in `blocks`.  A tiered Flat index (RSB_OPT_DEVICE_ROWS, fp16 only) allocates the
+// device tier once, at dev_rows rows, and adds one block per add; a reserved IVFFLAT index (rsb_reserve_lists) counts
+// CSR slots, with dev_rows the slots of lists [0, l_dev) and one block for the other lists.  Search streams the host
+// rows through two staging buffers of the workspace on copy_st (StagePipe).
+struct HostTier {
+    int64_t dev_rows = -1;                 // -1: not tiered
+    int64_t rows = 0;                      // Flat: rows added (ntotal + n_staged); IVFFLAT: slots reserved
+    std::vector<HostBlock> blocks;         // in row order
+    // one staging buffer of the search: Flat: as requested (clamped per search); IVFFLAT: clamped at reservation to
+    // [largest host list, host tier], in bytes that need not be whole rows
+    size_t staging_bytes = kDefaultStagingBytes;
+    cudaStream_t copy_st = nullptr;
+    cudaEvent_t stage_ready[2] = {}, stage_free[2] = {}, copy_start = nullptr, copy_done = nullptr, flags_ready = nullptr;
+    unsigned char* pinned = nullptr;       // IVFFLAT, page-locked: the per-batch table the search copies to the device
+                                           // (stage_off int64 [nlist], chunk_of int32 [nlist]), then probed flags [nlist]
+};
 
 struct rsb_index {
     // IVFPQ: M sub-quantizers of nbits bits each (faiss' values: codebook, encoding, training, rsb_info) and
@@ -98,38 +117,21 @@ struct rsb_index {
     int64_t* list_nat_off = nullptr;   // [nlist + 1]
     int max_list_len = 0;
 
-    // tiered Flat (RSB_OPT_DEVICE_ROWS, fp16 only): rows [0, dev_rows) live in `payload` (allocated once, at dev_rows
-    // rows, by the first add, and filled in place), rows [dev_rows, n_rows) in host_blocks (one per add, in row order).
-    // Only the ids go through the staging segments.  Search streams the host blocks through two staging buffers of the
-    // workspace on copy_st.
-    int64_t dev_rows = -1;                 // -1: not tiered
-    int64_t n_rows = 0;                    // rows held by the tiers (ntotal + n_staged)
-    std::vector<HostBlock> host_blocks;
-    size_t host_bytes = 0;
-    size_t staging_bytes = kDefaultStagingBytes;
-    cudaStream_t copy_st = nullptr;
-    cudaEvent_t stage_ready[2] = {}, stage_free[2] = {}, copy_start = nullptr, copy_done = nullptr;
-    bool tiered() const { return dev_rows >= 0; }
-
-    // tiered IVFFLAT (rsb_reserve_lists): the CSR layout is fixed up front from the reserved list sizes.  The rows of
-    // lists [0, l_dev) (slots [0, ivf_dev_rows)) live in `payload`, those of lists [l_dev, nlist) in ivf_host (page-
-    // locked, one block of exactly the bytes needed, slot s at row s - ivf_dev_rows).  Ids, list tables, centroids and
-    // the SQ8 range stay on the device.  rsb_add / rsb_add_preassigned / rsb_add_codes place every row in its final
-    // slot; ntotal counts the rows placed so far (nslots the rows reserved).  host_bytes / copy_st / the stage events
-    // are shared with the tiered Flat index.
-    bool ivf_reserved = false;
+    // tiered Flat: only the ids go through the staging segments.  Reserved IVFFLAT: the CSR layout is fixed up front
+    // from the reserved list sizes; ids, list tables, centroids and the SQ8 range stay on the device.  rsb_add /
+    // rsb_add_preassigned / rsb_add_codes place every row in its final slot; ntotal counts the rows placed so far
+    // (nslots the rows reserved).
+    HostTier tier;
     int l_dev = 0;
-    int64_t ivf_dev_rows = 0;
-    uint8_t* ivf_host = nullptr;
     std::vector<int> ivf_len;              // [nlist] reserved sizes
     std::vector<int64_t> ivf_off;          // [nlist + 1] CSR offsets
     std::vector<int64_t> ivf_fill;         // [nlist] rows placed so far
     int* dev_len = nullptr;                // [nlist] device: list_len on lists [0, l_dev), 0 elsewhere
-    size_t ivf_stage_bytes = 0;            // one staging buffer of the search (>= the largest host list)
-    unsigned char* tier_pinned = nullptr;  // page-locked: the per-batch table the search copies to the device
-                                           // (stage_off int64 [nlist], chunk_of int32 [nlist]), then probed flags [nlist]
-    cudaEvent_t flags_ready = nullptr;
-    bool ivf_streamed() const { return ivf_reserved && ivf_dev_rows < nslots; }
+    bool tiered() const { return tier.dev_rows >= 0; }
+    bool ivf_reserved() const { return kind == RSB_IVFFLAT && tiered(); }
+    // rows in device memory (RSB_INFO_DEVICE_ROWS) and in the host tier
+    int64_t device_rows() const { return tiered() ? std::min(tier.dev_rows, tier.rows) : ntotal + n_staged; }
+    int64_t host_rows() const { return tiered() ? tier.rows - device_rows() : 0; }
 
     // profiling
     bool prof = false;
@@ -159,6 +161,18 @@ static void free_layout(rsb_index* h) {
     h->payload = nullptr; h->ids_slots = nullptr; h->list_len = nullptr;
     h->list_slot_off = nullptr; h->list_nat_off = nullptr;
     h->ntotal = 0; h->nslots = 0; h->payload_bytes = 0; h->max_list_len = 0;
+}
+static void free_tier(HostTier& t) {
+    if (t.copy_st) {   // a search in flight may still copy from the host blocks
+        cudaStreamSynchronize(t.copy_st);
+        cudaStreamDestroy(t.copy_st);
+    }
+    for (cudaEvent_t e : {t.stage_ready[0], t.stage_ready[1], t.stage_free[0], t.stage_free[1], t.copy_start, t.copy_done,
+                          t.flags_ready})
+        if (e) cudaEventDestroy(e);
+    for (auto& b : t.blocks) if (b.p) cudaFreeHost(b.p);
+    if (t.pinned) cudaFreeHost(t.pinned);
+    t = HostTier();
 }
 
 extern "C" int rsb_version(void) { return RSB_VERSION; }
@@ -213,16 +227,7 @@ extern "C" int rsb_free(rsb_index_t* h) {
     cudaFree(h->centroids); cudaFree(h->codebook); cudaFree(h->codebook_t); cudaFree(h->prof_dev); cudaFree(h->sq);
     cudaFree(h->cent_hi); cudaFree(h->cent_lo);
     for (auto& set : h->evs) for (auto& e : set) if (e) cudaEventDestroy(e);
-    if (h->copy_st) {   // a search in flight may still copy from the host blocks
-        cudaStreamSynchronize(h->copy_st);
-        cudaStreamDestroy(h->copy_st);
-    }
-    for (cudaEvent_t e : {h->stage_ready[0], h->stage_ready[1], h->stage_free[0], h->stage_free[1], h->copy_start, h->copy_done})
-        if (e) cudaEventDestroy(e);
-    for (auto& b : h->host_blocks) cudaFreeHost(b.p);
-    if (h->ivf_host) cudaFreeHost(h->ivf_host);
-    if (h->tier_pinned) cudaFreeHost(h->tier_pinned);
-    if (h->flags_ready) cudaEventDestroy(h->flags_ready);
+    free_tier(h->tier);
     delete h;
     return RSB_OK;
 }
@@ -233,7 +238,7 @@ extern "C" int rsb_free(rsb_index_t* h) {
 extern "C" int rsb_set_centroids(rsb_index_t* h, const float* c, rsb_stream_t stream) {
     if (!h || !c) return fail(RSB_ERR_INVALID, "null argument");
     if (h->kind == RSB_FLAT) return fail(RSB_ERR_INVALID, "a Flat index has no centroids");
-    if (h->ntotal || h->n_staged || h->ivf_reserved)
+    if (h->ntotal || h->n_staged || h->ivf_reserved())
         return fail(RSB_ERR_STATE, "cannot change centroids of a populated (or reserved) index");
     cudaStream_t st = (cudaStream_t)stream;
     const size_t bytes = (size_t)h->nlist * h->d * 4;
@@ -279,7 +284,7 @@ static bool is_sq8_ivf(const rsb_index* h) { return h->kind == RSB_IVFFLAT && h-
 extern "C" int rsb_set_sq_range(rsb_index_t* h, const float* sq, rsb_stream_t stream) {
     if (!h || !sq) return fail(RSB_ERR_INVALID, "null argument");
     if (!is_sq8_ivf(h)) return fail(RSB_ERR_INVALID, "only an IVFFLAT index with RSB_DTYPE_SQ8 storage has a scalar-quantizer range");
-    if (h->ntotal || h->n_staged || h->ivf_reserved)
+    if (h->ntotal || h->n_staged || h->ivf_reserved())
         return fail(RSB_ERR_STATE, "cannot change the range of a populated (or reserved) index (its codes use it)");
     const size_t bytes = (size_t)2 * h->d * 4;
     if (!h->sq) CU(cudaMalloc(&h->sq, bytes));
@@ -428,13 +433,19 @@ extern "C" int rsb_knn_ip(const float* q, int nq, const float* x, int64_t n, int
 }
 
 // the copy stream and stage events of a tiered index, on the device current now (which holds the index)
-static int ensure_copy_stream(rsb_index* h) {
-    if (h->copy_st) return RSB_OK;
-    CU(cudaStreamCreateWithFlags(&h->copy_st, cudaStreamNonBlocking));
-    for (cudaEvent_t* e : {&h->stage_ready[0], &h->stage_ready[1], &h->stage_free[0], &h->stage_free[1], &h->copy_start,
-                           &h->copy_done})
+static int ensure_copy_stream(HostTier& t) {
+    if (t.copy_st) return RSB_OK;
+    CU(cudaStreamCreateWithFlags(&t.copy_st, cudaStreamNonBlocking));
+    for (cudaEvent_t* e : {&t.stage_ready[0], &t.stage_ready[1], &t.stage_free[0], &t.stage_free[1], &t.copy_start,
+                           &t.copy_done, &t.flags_ready})
         CU(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
     return RSB_OK;
+}
+
+// bytes of one staging buffer of a tiered search: the requested size, but at least min_rows rows and at most the host
+// tier's host_rows (min_rows <= host_rows)
+static size_t staging_size(size_t requested, size_t rb, int64_t min_rows, int64_t host_rows) {
+    return std::min(std::max(requested, (size_t)min_rows * rb), (size_t)host_rows * rb);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -498,13 +509,13 @@ static int add_tiered(rsb_index* h, const void* x, int x_dtype, int64_t n, const
     const bool f32 = x_dtype == RSB_DTYPE_F32;
     const int d = h->d;
     const size_t rb = h->row_bytes(), xrb = (size_t)d * (f32 ? 4 : 2);
-    const int64_t pos = h->n_rows;
-    const int64_t n_to_dev = std::max<int64_t>(0, std::min<int64_t>(n, h->dev_rows - pos));
+    const int64_t pos = h->tier.rows;
+    const int64_t n_to_dev = std::max<int64_t>(0, std::min<int64_t>(n, h->tier.dev_rows - pos));
     const int64_t n_host = n - n_to_dev;
     const uint8_t* xb = static_cast<const uint8_t*>(x);
     if (n_to_dev && !h->payload) {   // the device tier, once, at its full size
-        CU(cudaMalloc(&h->payload, (size_t)h->dev_rows * rb));
-        h->payload_bytes = (size_t)h->dev_rows * rb;
+        CU(cudaMalloc(&h->payload, (size_t)h->tier.dev_rows * rb));
+        h->payload_bytes = (size_t)h->tier.dev_rows * rb;
     }
     HostBlock blk;
     if (n_host) {
@@ -564,13 +575,10 @@ static int add_tiered(rsb_index* h, const void* x, int x_dtype, int64_t n, const
         cudaFreeHost(blk.p);
         return rc;
     }
-    if (n_host) {
-        h->host_blocks.push_back(blk);
-        h->host_bytes += (size_t)n_host * rb;
-    }
+    if (n_host) h->tier.blocks.push_back(blk);
     h->staging.push_back(seg);
     h->n_staged += n;
-    h->n_rows += n;
+    h->tier.rows += n;
     return RSB_OK;
 }
 
@@ -594,7 +602,7 @@ static int add_impl(rsb_index* h, const void* x, int x_dtype, const uint8_t* cod
     // slots are 32-bit in the candidate keys (2^32) and rsb_finalize sorts (list, row) pairs with a 32-bit item count
     if (h->ntotal + h->n_staged + n >= ((int64_t)1 << 31) - 64 * (int64_t)h->nlist)
         return fail(RSB_ERR_UNSUPPORTED, "more than 2^31 vectors per index shard (shard the datastore across GPUs)");
-    if (h->tiered()) return add_tiered(h, x, x_dtype, n, ids, st);
+    if (h->kind == RSB_FLAT && h->tiered()) return add_tiered(h, x, x_dtype, n, ids, st);
     const int64_t next_id0 = h->next_id;
     Segment seg;
     int rc = stage_common(h, seg, ids, n, st);
@@ -651,7 +659,7 @@ static int add_impl(rsb_index* h, const void* x, int x_dtype, const uint8_t* cod
     }
     CUB_(cudaPeekAtLastError());
 #undef CUB_
-    if (h->ivf_reserved) {   // the rows go to their final slots now; the segment was only the encoded batch
+    if (h->ivf_reserved()) {   // the rows go to their final slots now; the segment was only the encoded batch
         rc = place_segment(h, seg, st);
         cudaStreamSynchronize(st);
         free_segment(seg);
@@ -704,7 +712,7 @@ extern "C" int rsb_reserve_lists(rsb_index_t* h, const int64_t* sizes, int64_t d
     }
     if (!is_trained(h))
         return fail(RSB_ERR_STATE, "index is not trained (set centroids%s first)", is_sq8_ivf(h) ? " and the SQ8 range" : "");
-    if (h->ivf_reserved) return fail(RSB_ERR_STATE, "the lists are already reserved (one reservation per index)");
+    if (h->ivf_reserved()) return fail(RSB_ERR_STATE, "the lists are already reserved (one reservation per index)");
     if (h->ntotal || h->n_staged) return fail(RSB_ERR_STATE, "rows were already added: reserve the lists of an empty index");
     cudaStream_t st = (cudaStream_t)stream;
     const size_t rb = h->row_bytes();
@@ -717,9 +725,6 @@ extern "C" int rsb_reserve_lists(rsb_index_t* h, const int64_t* sizes, int64_t d
         max_len = std::max(max_len, len[l]);
         if (l >= l_dev) max_host = std::max(max_host, len[l]);
     }
-    // a staging buffer holds at least the largest host list, and never more than the whole host tier
-    size_t stage = staging_bytes ? staging_bytes : kDefaultStagingBytes;
-    stage = std::min(std::max(stage, (size_t)max_host * rb), (size_t)host_rows * rb);
     std::vector<int> dlen(nlist), by_len(nlist), rank_of(nlist);
     for (int l = 0; l < nlist; ++l) { dlen[l] = l < l_dev ? len[l] : 0; by_len[l] = l; }
     std::stable_sort(by_len.begin(), by_len.end(), [&](int a, int b) { return len[a] > len[b]; });
@@ -728,9 +733,7 @@ extern "C" int rsb_reserve_lists(rsb_index_t* h, const int64_t* sizes, int64_t d
     auto undo = [&](int rc) {
         cudaStreamSynchronize(st);
         free_layout(h);
-        if (h->ivf_host) cudaFreeHost(h->ivf_host);
-        if (h->tier_pinned) cudaFreeHost(h->tier_pinned);
-        h->ivf_host = nullptr; h->tier_pinned = nullptr;
+        free_tier(h->tier);
         return rc;
     };
 #define CUR(expr) do { cudaError_t e__ = (expr); if (e__ != cudaSuccess) return undo(fail(e__ == cudaErrorMemoryAllocation ? RSB_ERR_OOM : RSB_ERR_CUDA, "%s: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__)); } while (0)
@@ -749,18 +752,19 @@ extern "C" int rsb_reserve_lists(rsb_index_t* h, const int64_t* sizes, int64_t d
     CUR(cudaMalloc(&h->ids_slots, std::max<size_t>((size_t)total * 8, 256)));
     launch_fill_i64(h->ids_slots, total, -1, st);
     CUR(cudaPeekAtLastError());
-    if (host_rows) CUR(cudaHostAlloc((void**)&h->ivf_host, (size_t)host_rows * rb, cudaHostAllocPortable));
-    CUR(cudaHostAlloc((void**)&h->tier_pinned, (size_t)nlist * 13, cudaHostAllocPortable));
-    if (ensure_copy_stream(h) != RSB_OK) return undo(RSB_ERR_CUDA);
-    if (!h->flags_ready) CUR(cudaEventCreateWithFlags(&h->flags_ready, cudaEventDisableTiming));
+    if (host_rows) {
+        h->tier.blocks.push_back(HostBlock{nullptr, dev_rows, host_rows});
+        CUR(cudaHostAlloc(&h->tier.blocks[0].p, (size_t)host_rows * rb, cudaHostAllocPortable));
+    }
+    CUR(cudaHostAlloc((void**)&h->tier.pinned, (size_t)nlist * 13, cudaHostAllocPortable));
+    if (ensure_copy_stream(h->tier) != RSB_OK) return undo(RSB_ERR_CUDA);
     CUR(cudaStreamSynchronize(st));
 #undef CUR
-    h->ivf_reserved = true;
+    h->tier.dev_rows = dev_rows;
+    h->tier.rows = total;
+    h->tier.staging_bytes = staging_size(staging_bytes ? staging_bytes : kDefaultStagingBytes, rb, max_host, host_rows);
     h->l_dev = l_dev;
-    h->ivf_dev_rows = dev_rows;
     h->ivf_len = len; h->ivf_off = off; h->ivf_fill.assign(nlist, 0);
-    h->ivf_stage_bytes = stage;
-    h->host_bytes = (size_t)host_rows * rb;
     h->payload_bytes = (size_t)dev_rows * rb;
     h->nslots = total; h->ntotal = 0; h->max_list_len = max_len;
     return RSB_OK;
@@ -768,7 +772,7 @@ extern "C" int rsb_reserve_lists(rsb_index_t* h, const int64_t* sizes, int64_t d
 
 // rsb_search / rsb_export_* of a reserved index: every reserved row must have arrived
 static int ivf_check_complete(const rsb_index* h) {
-    if (h->ivf_reserved && h->ntotal < h->nslots)
+    if (h->ivf_reserved() && h->ntotal < h->nslots)
         return fail(RSB_ERR_STATE, "%lld of the %lld reserved rows have been added: add the rest first",
                     (long long)h->ntotal, (long long)h->nslots);
     return RSB_OK;
@@ -837,15 +841,16 @@ static int place_segment(rsb_index* h, const Segment& seg, cudaStream_t st) {
     // host-tier rows: one device-to-host copy per run of slots that are consecutive in both buffers
     for (int l = h->l_dev; l < nlist;) {
         if (!cnt[l]) { ++l; continue; }
-        const int64_t s0 = tab[l] - host_begin, d0 = tab[nlist + l] - h->ivf_dev_rows;
+        const HostBlock& hb = h->tier.blocks[0];
+        const int64_t s0 = tab[l] - host_begin, d0 = tab[nlist + l] - hb.r0;
         int64_t rows = cnt[l];
         int e = l + 1;
         for (; e < nlist; ++e) {
             if (!cnt[e]) continue;
-            if (tab[e] - host_begin != s0 + rows || tab[nlist + e] - h->ivf_dev_rows != d0 + rows) break;
+            if (tab[e] - host_begin != s0 + rows || tab[nlist + e] - hb.r0 != d0 + rows) break;
             rows += cnt[e];
         }
-        CUP(cudaMemcpyAsync(h->ivf_host + (size_t)d0 * rb, host_stage + (size_t)s0 * rb, (size_t)rows * rb,
+        CUP(cudaMemcpyAsync(static_cast<uint8_t*>(hb.p) + (size_t)d0 * rb, host_stage + (size_t)s0 * rb, (size_t)rows * rb,
                             cudaMemcpyDeviceToHost, st));
         l = e;
     }
@@ -856,17 +861,21 @@ static int place_segment(rsb_index* h, const Segment& seg, cudaStream_t st) {
     return cleanup(RSB_OK);
 }
 
-// slots [r0, r0 + n) of a reserved IVFFLAT index, from whichever tier holds them, to dst (device or host memory)
-static int ivf_copy_rows(rsb_index* h, int64_t r0, int64_t n, void* dst, cudaStream_t st) {
+// rows [r0, r0 + n) of a Flat or IVFFLAT index (IVFFLAT: CSR slots), from whichever tier holds them, to dst (device
+// or host memory): one copy for the device rows and one per host block the range overlaps
+static int tier_copy_rows(rsb_index* h, int64_t r0, int64_t n, void* dst, cudaStream_t st) {
     const size_t rb = h->row_bytes();
     uint8_t* out = static_cast<uint8_t*>(dst);
-    const int64_t nd = h->ivf_dev_rows;
-    if (r0 < nd && n > 0)
-        CU(cudaMemcpyAsync(out, h->payload + (size_t)r0 * rb, (size_t)std::min(n, nd - r0) * rb, cudaMemcpyDefault, st));
-    const int64_t a = std::max(r0, nd), e = r0 + n;
-    if (a < e)
-        CU(cudaMemcpyAsync(out + (size_t)(a - r0) * rb, h->ivf_host + (size_t)(a - nd) * rb, (size_t)(e - a) * rb,
-                           cudaMemcpyDefault, st));
+    const int64_t n_dev = h->device_rows(), r1 = r0 + n;
+    if (r0 < n_dev && n > 0)
+        CU(cudaMemcpyAsync(out, h->payload + (size_t)r0 * rb, (size_t)std::min(n, n_dev - r0) * rb, cudaMemcpyDefault, st));
+    const std::vector<HostBlock>& blocks = h->tier.blocks;
+    auto b = std::partition_point(blocks.begin(), blocks.end(), [&](const HostBlock& blk) { return blk.r0 + blk.n <= r0; });
+    for (; b != blocks.end() && b->r0 < r1; ++b) {
+        const int64_t a = std::max(r0, b->r0), e = std::min(r1, b->r0 + b->n);
+        CU(cudaMemcpyAsync(out + (size_t)(a - r0) * rb, static_cast<const uint8_t*>(b->p) + (size_t)(a - b->r0) * rb,
+                           (size_t)(e - a) * rb, cudaMemcpyDefault, st));
+    }
     return RSB_OK;
 }
 
@@ -1098,11 +1107,8 @@ extern "C" int rsb_info(rsb_index_t* h, int what, int64_t* out) {
         case RSB_INFO_INDEX_BYTES: *out = (int64_t)(h->payload_bytes + (size_t)h->nslots * 8); break;
         case RSB_INFO_DTYPE: *out = h->dtype; break;
         case RSB_INFO_BY_RESIDUAL: *out = h->by_residual ? 1 : 0; break;
-        case RSB_INFO_HOST_BYTES: *out = (int64_t)h->host_bytes; break;
-        case RSB_INFO_DEVICE_ROWS:
-            *out = h->tiered() ? std::min(h->dev_rows, h->ntotal + h->n_staged)
-                   : h->ivf_reserved ? h->ivf_dev_rows : h->ntotal + h->n_staged;
-            break;
+        case RSB_INFO_HOST_BYTES: *out = h->host_rows() * (int64_t)h->row_bytes(); break;
+        case RSB_INFO_DEVICE_ROWS: *out = h->device_rows(); break;
         default: return fail(RSB_ERR_INVALID, "unknown info key %d", what);
     }
     return RSB_OK;
@@ -1123,22 +1129,6 @@ extern "C" int rsb_list_sizes(rsb_index_t* h, int64_t* sizes, rsb_stream_t strea
     return RSB_OK;
 }
 
-// rows [r0, r0 + n) of a finalised Flat index, from whichever tier holds them, to dst (device or host memory)
-static int flat_copy_rows(rsb_index* h, int64_t r0, int64_t n, void* dst, cudaStream_t st) {
-    const size_t rb = h->row_bytes();
-    uint8_t* out = static_cast<uint8_t*>(dst);
-    const int64_t n_dev = h->tiered() ? std::min(h->dev_rows, h->ntotal) : h->ntotal;
-    if (r0 < n_dev && n > 0)
-        CU(cudaMemcpyAsync(out, h->payload + (size_t)r0 * rb, (size_t)std::min(n, n_dev - r0) * rb, cudaMemcpyDefault, st));
-    for (const HostBlock& b : h->host_blocks) {
-        const int64_t a = std::max(r0, b.r0), e = std::min(r0 + n, b.r0 + b.n);
-        if (a < e)
-            CU(cudaMemcpyAsync(out + (size_t)(a - r0) * rb, static_cast<const uint8_t*>(b.p) + (size_t)(a - b.r0) * rb,
-                               (size_t)(e - a) * rb, cudaMemcpyDefault, st));
-    }
-    return RSB_OK;
-}
-
 static int export_impl(rsb_index* h, int64_t* offsets, void* payload, int64_t* ids, cudaStream_t st) {
     if (h->kind == RSB_FLAT) {
         if (offsets) {
@@ -1146,22 +1136,13 @@ static int export_impl(rsb_index* h, int64_t* offsets, void* payload, int64_t* i
             CU(cudaMemcpyAsync(offsets, o, 16, cudaMemcpyHostToDevice, st));
             CU(cudaStreamSynchronize(st));
         }
-        if (payload && h->ntotal && h->tiered()) RSB_TRY(flat_copy_rows(h, 0, h->ntotal, payload, st));
-        else if (payload && h->ntotal) CU(cudaMemcpyAsync(payload, h->payload, (size_t)h->ntotal * h->row_bytes(), cudaMemcpyDeviceToDevice, st));
-        if (ids && h->ntotal) CU(cudaMemcpyAsync(ids, h->ids_slots, (size_t)h->ntotal * 8, cudaMemcpyDeviceToDevice, st));
-        return RSB_OK;
-    }
-    if (!h->list_nat_off) {
+    } else if (!h->list_nat_off) {
         if (offsets) CU(cudaMemsetAsync(offsets, 0, (size_t)(h->nlist + 1) * 8, st));
         return RSB_OK;
+    } else if (offsets) {
+        CU(cudaMemcpyAsync(offsets, h->list_nat_off, (size_t)(h->nlist + 1) * 8, cudaMemcpyDeviceToDevice, st));
     }
-    if (offsets) CU(cudaMemcpyAsync(offsets, h->list_nat_off, (size_t)(h->nlist + 1) * 8, cudaMemcpyDeviceToDevice, st));
     if (h->ntotal == 0) return RSB_OK;
-    if (h->ivf_reserved) {   // CSR slots are the natural order; rows from either tier, to device or host memory
-        if (payload) RSB_TRY(ivf_copy_rows(h, 0, h->ntotal, payload, st));
-        if (ids) CU(cudaMemcpyAsync(ids, h->ids_slots, (size_t)h->ntotal * 8, cudaMemcpyDefault, st));
-        return RSB_OK;
-    }
     if (h->kind == RSB_IVFPQ) {
         if (payload && pq_interleaved_layout(h->Mb))
             launch_pq_deinterleave(h->payload, h->list_nat_off, h->list_slot_off, h->list_len, h->nlist, h->Mb, static_cast<uint8_t*>(payload), st);
@@ -1169,10 +1150,11 @@ static int export_impl(rsb_index* h, int64_t* offsets, void* payload, int64_t* i
             launch_compact_slots_rows(h->payload, h->list_nat_off, h->list_slot_off, h->nlist, h->Mb, static_cast<uint8_t*>(payload), st);
         if (ids) launch_compact_slots_i64(h->ids_slots, h->list_nat_off, h->list_slot_off, h->list_len, h->nlist, ids, st);
         CHECK_LAUNCH();
-    } else {
-        if (payload) CU(cudaMemcpyAsync(payload, h->payload, (size_t)h->ntotal * h->row_bytes(), cudaMemcpyDeviceToDevice, st));
-        if (ids) CU(cudaMemcpyAsync(ids, h->ids_slots, (size_t)h->ntotal * 8, cudaMemcpyDeviceToDevice, st));
+        return RSB_OK;
     }
+    // Flat and IVFFLAT slots are the natural order; rows from either tier, to device or host memory
+    if (payload) RSB_TRY(tier_copy_rows(h, 0, h->ntotal, payload, st));
+    if (ids) CU(cudaMemcpyAsync(ids, h->ids_slots, (size_t)h->ntotal * 8, cudaMemcpyDefault, st));
     return RSB_OK;
 }
 
@@ -1194,13 +1176,7 @@ extern "C" int rsb_export_rows(rsb_index_t* h, int64_t r0, int64_t n, void* dst,
                     (long long)h->ntotal);
     if (n == 0) return RSB_OK;
     if (!dst) return fail(RSB_ERR_INVALID, "dst is NULL");
-    if (h->kind == RSB_IVFFLAT && h->ivf_reserved) return ivf_copy_rows(h, r0, n, dst, (cudaStream_t)stream);
-    if (h->kind == RSB_IVFFLAT) {   // the all-device CSR rows
-        CU(cudaMemcpyAsync(dst, h->payload + (size_t)r0 * h->row_bytes(), (size_t)n * h->row_bytes(), cudaMemcpyDefault,
-                           (cudaStream_t)stream));
-        return RSB_OK;
-    }
-    return flat_copy_rows(h, r0, n, dst, (cudaStream_t)stream);
+    return tier_copy_rows(h, r0, n, dst, (cudaStream_t)stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -1277,22 +1253,76 @@ static FlatPlan flat_plan(const rsb_index* h, int nq, int k) {
     return p;
 }
 
+// The staging pipeline of both tiered searches: host chunk c is copied by the tier's copy stream into staging buffer
+// c % 2 while the caller's stream scores chunk c - 1.  Per query batch the caller runs begin, prefetch, then
+// acquire / score / release for every chunk; end joins the copy stream back to the caller's stream after the last
+// batch.  `copy(c, buf)` enqueues chunk c's copies into buf on tier.copy_st.
+struct StagePipe {
+    HostTier& t;
+    uint8_t* buf[2];
+    std::function<int(int64_t, uint8_t*)> copy;
+    int64_t nchunks = 0;
+
+    uint8_t* buffer(int64_t c) const { return buf[c & 1]; }
+    // copies of this batch start after everything enqueued on st before (adds, the previous batch's use of the buffers)
+    int begin(cudaStream_t st) {
+        CU(cudaEventRecord(t.copy_start, st));
+        CU(cudaStreamWaitEvent(t.copy_st, t.copy_start, 0));
+        return RSB_OK;
+    }
+    int fill(int64_t c) {
+        RSB_TRY(copy(c, buffer(c)));
+        CU(cudaEventRecord(t.stage_ready[c & 1], t.copy_st));
+        return RSB_OK;
+    }
+    int prefetch(int64_t n) {
+        nchunks = n;
+        for (int64_t c = 0; c < std::min<int64_t>(2, n); ++c) RSB_TRY(fill(c));
+        return RSB_OK;
+    }
+    int acquire(int64_t c, cudaStream_t st) {
+        CU(cudaStreamWaitEvent(st, t.stage_ready[c & 1], 0));
+        return RSB_OK;
+    }
+    // chunk c's buffer is free once st has scored it: it takes chunk c + 2
+    int release(int64_t c, cudaStream_t st) {
+        CU(cudaEventRecord(t.stage_free[c & 1], st));
+        if (c + 2 < nchunks) {
+            CU(cudaStreamWaitEvent(t.copy_st, t.stage_free[c & 1], 0));
+            RSB_TRY(fill(c + 2));
+        }
+        return RSB_OK;
+    }
+    int end(cudaStream_t st) {
+        CU(cudaEventRecord(t.copy_done, t.copy_st));
+        CU(cudaStreamWaitEvent(st, t.copy_done, 0));
+        return RSB_OK;
+    }
+};
+// two staging buffers of `bytes` each from workspace offset o; returns the offset after them
+static size_t plan_staging(size_t o, size_t bytes, size_t off_stage[2]) {
+    for (int b = 0; b < 2; ++b) {
+        off_stage[b] = o;
+        o += align_up(bytes);
+    }
+    return o;
+}
+
 // Tiered Flat search (rows past dev_rows in host memory).  The rows are scored in pieces: the device tier in place,
-// then the host tier in chunks of chunk_rows, copied by copy_st into two staging buffers while the previous piece is
-// scored.  Each piece runs the fp16 candidate path (kc = min(k + 8, 4096, rows) candidates) and the exact fp32
-// re-score of its own rows, and is merged into the running top-k (ties: the earlier piece, i.e. the lower row).
+// then the host tier in chunks of chunk_rows, staged by StagePipe while the previous piece is scored.  Each piece
+// runs the fp16 candidate path (kc = min(k + 8, 4096, rows) candidates) and the exact fp32 re-score of its own rows,
+// and is merged into the running top-k (ties: the earlier piece, i.e. the lower row).
 struct TieredFlatPlan {
     int qb, kc;
     int64_t n_dev, chunk_rows, nchunks;
     size_t knn_bytes, off_qsplit, off_D2, off_I2, off_mD, off_mI, off_stage[2], total;
 };
-static bool flat_is_streamed(const rsb_index* h) { return h->tiered() && h->n_rows > h->dev_rows; }
 static TieredFlatPlan tiered_flat_plan(const rsb_index* h, int nq, int k) {
     TieredFlatPlan p;
     const size_t rb = h->row_bytes();
-    p.n_dev = std::min(h->dev_rows, h->n_rows);
-    const int64_t n_host = h->n_rows - p.n_dev;
-    p.chunk_rows = std::max<int64_t>(1, std::min<int64_t>((int64_t)(h->staging_bytes / rb), n_host));
+    p.n_dev = h->device_rows();
+    const int64_t n_host = h->host_rows();
+    p.chunk_rows = (int64_t)(staging_size(h->tier.staging_bytes, rb, 1, n_host) / rb);
     p.nchunks = (n_host + p.chunk_rows - 1) / p.chunk_rows;
     p.kc = std::min(k + 8, 4096);
     const int64_t rows = std::max<int64_t>({p.n_dev, p.chunk_rows, 1});
@@ -1306,11 +1336,7 @@ static TieredFlatPlan tiered_flat_plan(const rsb_index* h, int nq, int k) {
     p.off_I2 = o;     o += align_up((size_t)p.qb * p.kc * 8);
     p.off_mD = o;     o += align_up((size_t)2 * p.qb * k * 4);   // merge input [2, nb, k]: running top-k, new piece
     p.off_mI = o;     o += align_up((size_t)2 * p.qb * k * 8);
-    for (int b = 0; b < 2; ++b) {
-        p.off_stage[b] = o;
-        o += align_up((size_t)p.chunk_rows * rb);
-    }
-    p.total = o;
+    p.total = plan_staging(o, (size_t)p.chunk_rows * rb, p.off_stage);
     return p;
 }
 
@@ -1318,7 +1344,6 @@ static int search_flat_tiered(rsb_index* h, const float* q, int nq, int k, float
                               size_t ws_bytes, cudaStream_t st) {
     const TieredFlatPlan p = tiered_flat_plan(h, nq, k);
     if (ws_bytes < p.total) return fail(RSB_ERR_OOM, "workspace too small: need %zu bytes, got %zu", p.total, ws_bytes);
-    const size_t rb = h->row_bytes();
     unsigned char* w = static_cast<unsigned char*>(ws);
     TensorOperands tc;   // [qb, d] fp16 hi, [qb, d] fp16 lo, [qb] fp32 inverse scales
     tc.xh = tc.xl = nullptr;
@@ -1330,7 +1355,10 @@ static int search_flat_tiered(rsb_index* h, const float* q, int nq, int k, float
     int64_t* I2 = reinterpret_cast<int64_t*>(w + p.off_I2);
     float* mD = reinterpret_cast<float*>(w + p.off_mD);
     int64_t* mI = reinterpret_cast<int64_t*>(w + p.off_mI);
-    uint8_t* stage[2] = {w + p.off_stage[0], w + p.off_stage[1]};
+    StagePipe pipe{h->tier, {w + p.off_stage[0], w + p.off_stage[1]}, [&](int64_t c, uint8_t* buf) -> int {
+        const int64_t r0 = p.n_dev + c * p.chunk_rows;
+        return tier_copy_rows(h, r0, std::min(p.chunk_rows, h->ntotal - r0), buf, h->tier.copy_st);
+    }};
 
     // rows X [rows, d] = index rows [r0, r0 + rows) -> exact top-k of nb queries
     auto score_piece = [&](const float* qb, int nb, const void* X, int64_t rows, int64_t r0, float* Do, int64_t* Io) -> int {
@@ -1341,20 +1369,6 @@ static int search_flat_tiered(rsb_index* h, const float* q, int nq, int k, float
         h->launches += 1;
         return RSB_OK;
     };
-    // H2D copy of host chunk c into staging buffer c % 2 on the copy engine (copy_st), from the blocks it overlaps
-    auto copy_chunk = [&](int64_t c) -> int {
-        const int64_t r0 = p.n_dev + c * p.chunk_rows, r1 = std::min(h->ntotal, r0 + p.chunk_rows);
-        auto b = std::partition_point(h->host_blocks.begin(), h->host_blocks.end(),
-                                      [&](const HostBlock& blk) { return blk.r0 + blk.n <= r0; });
-        for (; b != h->host_blocks.end() && b->r0 < r1; ++b) {
-            const int64_t a = std::max(r0, b->r0), e = std::min(r1, b->r0 + b->n);
-            CU(cudaMemcpyAsync(stage[c & 1] + (size_t)(a - r0) * rb, static_cast<const uint8_t*>(b->p) + (size_t)(a - b->r0) * rb,
-                               (size_t)(e - a) * rb, cudaMemcpyHostToDevice, h->copy_st));
-        }
-        CU(cudaEventRecord(h->stage_ready[c & 1], h->copy_st));
-        return RSB_OK;
-    };
-
     const int64_t pieces = (p.n_dev > 0 ? 1 : 0) + p.nchunks;
     for (int q0 = 0; q0 < nq; q0 += p.qb) {
         const int nb = std::min(p.qb, nq - q0);
@@ -1376,35 +1390,28 @@ static int search_flat_tiered(rsb_index* h, const float* q, int nq, int k, float
             }
             return RSB_OK;
         };
-        // copies start after everything the caller enqueued before (adds, the previous batch's use of the buffers)
-        CU(cudaEventRecord(h->copy_start, st));
-        CU(cudaStreamWaitEvent(h->copy_st, h->copy_start, 0));
-        for (int64_t c = 0; c < std::min<int64_t>(2, p.nchunks); ++c) RSB_TRY(copy_chunk(c));
+        RSB_TRY(pipe.begin(st));
+        RSB_TRY(pipe.prefetch(p.nchunks));
         if (p.n_dev > 0) {   // the device tier, in place, while the first chunks cross PCIe
             RSB_TRY(score_piece(qb, nb, h->payload, p.n_dev, 0, outD(), outI()));
             RSB_TRY(merge());
         }
         for (int64_t c = 0; c < p.nchunks; ++c) {
             const int64_t r0 = p.n_dev + c * p.chunk_rows;
-            CU(cudaStreamWaitEvent(st, h->stage_ready[c & 1], 0));
-            RSB_TRY(score_piece(qb, nb, stage[c & 1], std::min(p.chunk_rows, h->ntotal - r0), r0, outD(), outI()));
-            CU(cudaEventRecord(h->stage_free[c & 1], st));
-            if (c + 2 < p.nchunks) {
-                CU(cudaStreamWaitEvent(h->copy_st, h->stage_free[c & 1], 0));
-                RSB_TRY(copy_chunk(c + 2));
-            }
+            RSB_TRY(pipe.acquire(c, st));
+            RSB_TRY(score_piece(qb, nb, pipe.buffer(c), std::min(p.chunk_rows, h->ntotal - r0), r0, outD(), outI()));
+            RSB_TRY(pipe.release(c, st));
             RSB_TRY(merge());
         }
     }
-    CU(cudaEventRecord(h->copy_done, h->copy_st));   // join the copy stream back to the caller's
-    CU(cudaStreamWaitEvent(st, h->copy_done, 0));
+    RSB_TRY(pipe.end(st));
     CHECK_LAUNCH();
     return RSB_OK;
 }
 
 // Tiered IVFFLAT search (lists past l_dev in host memory): the search plan's workspace, then the probed-list flags
 // [nlist], one piece's masked list_len [nlist] int32 and staging offsets [nlist] int64, the per-batch table (stage_off
-// [nlist] int64, chunk_of [nlist] int32) and two staging buffers of ivf_stage_bytes.
+// [nlist] int64, chunk_of [nlist] int32) and two staging buffers of tier.staging_bytes.
 struct IvfTierPlan {
     size_t off_flags, off_plen, off_pdata, off_table, off_stage[2], total;
 };
@@ -1415,18 +1422,14 @@ static IvfTierPlan ivf_tier_plan(const rsb_index* h, size_t base) {
     t.off_plen = o;  o += align_up((size_t)h->nlist * 4);
     t.off_pdata = o; o += align_up((size_t)h->nlist * 8);
     t.off_table = o; o += align_up((size_t)h->nlist * 12);
-    for (int b = 0; b < 2; ++b) {
-        t.off_stage[b] = o;
-        o += align_up(h->ivf_stage_bytes);
-    }
-    t.total = o;
+    t.total = plan_staging(o, h->tier.staging_bytes, t.off_stage);
     return t;
 }
 
 extern "C" size_t rsb_workspace_bytes(rsb_index_t* h, int nq, int k, int nprobe) {
     if (!h) return 0;
     nq = std::max(nq, 1); k = std::max(k, 1);
-    if (h->kind == RSB_FLAT && flat_is_streamed(h)) return tiered_flat_plan(h, nq, k).total;
+    if (h->kind == RSB_FLAT && h->host_rows() > 0) return tiered_flat_plan(h, nq, k).total;
     if (h->kind == RSB_FLAT) {
         // pending adds are finalised by the search itself, which may switch the tensor path on: size for both
         const size_t plain = knn_plan(nq, std::max<int64_t>(h->ntotal + h->n_staged, 1), k).total;
@@ -1436,7 +1439,7 @@ extern "C" size_t rsb_workspace_bytes(rsb_index_t* h, int nq, int k, int nprobe)
                             align_up((size_t)kp.qb * kc * 8);
         return std::max(plain, tens);
     }
-    if (h->ivf_streamed()) return ivf_tier_plan(h, search_plan(h, nq, k, nprobe).total).total;
+    if (h->host_rows() > 0) return ivf_tier_plan(h, search_plan(h, nq, k, nprobe).total).total;
     return search_plan(h, nq, k, nprobe).total;
 }
 
@@ -1524,10 +1527,9 @@ static void launch_pq_tables(const rsb_index* h, const float* q, int nq, float* 
 //   2. the device lists are scanned in place (list_len masked to lists [0, l_dev)), enqueued before the host waits;
 //   3. the host waits for the flags -- the one host synchronisation per batch, by design: only the host can drive the
 //      copy engine -- and packs the probed host lists, in list order, into chunks of at most one staging buffer
-//      (adjacent lists coalesced into one copy).  copy_st copies chunk c into staging buffer c % 2 (stage_ready /
-//      stage_free events, as in search_flat_tiered) while the caller's stream scans chunk c - 1; a small kernel
-//      derives each chunk's masked list_len and staging offsets from one per-batch table, copied by copy_st ahead of
-//      the chunks;
+//      (adjacent lists coalesced into one copy).  StagePipe copies chunk c into staging buffer c % 2 while the caller's
+//      stream scans chunk c - 1, as in search_flat_tiered; a small kernel derives each chunk's masked list_len and
+//      staging offsets from one per-batch table, copied by copy_st ahead of the chunks;
 //   4. every piece shares the batch's thresholds tau and writes disjoint (query, probe) slots of out_keys / out_cnt,
 //      so one merge_items gives the result, as in the all-device search.
 // The pinned flags / table are rewritten only after the host has waited for this batch's flags, which the caller's
@@ -1537,25 +1539,21 @@ static int search_ivf_tiered(rsb_index* h, const float* q, int nq, int k, const 
                              cudaStream_t st) {
     const int nlist = h->nlist;
     const size_t rb = h->row_bytes();
-    const int64_t stage_rows = (int64_t)(h->ivf_stage_bytes / rb);
+    const int64_t stage_rows = (int64_t)(h->tier.staging_bytes / rb);
     unsigned char* dflags = w + t.off_flags;
     int* plen = reinterpret_cast<int*>(w + t.off_plen);
     int64_t* pdata = reinterpret_cast<int64_t*>(w + t.off_pdata);
     int64_t* dtab = reinterpret_cast<int64_t*>(w + t.off_table);
-    uint8_t* stage[2] = {w + t.off_stage[0], w + t.off_stage[1]};
-    int64_t* stage_off = reinterpret_cast<int64_t*>(h->tier_pinned);
+    int64_t* stage_off = reinterpret_cast<int64_t*>(h->tier.pinned);
     int* chunk_of = reinterpret_cast<int*>(stage_off + nlist);
-    unsigned char* hflags = h->tier_pinned + (size_t)nlist * 12;
-    struct Run { int chunk; int64_t host_row, stage_row, rows; };
+    unsigned char* hflags = h->tier.pinned + (size_t)nlist * 12;
+    struct Run { int64_t chunk, slot, stage_row, rows; };
     std::vector<Run> runs;
-    auto copy_chunk = [&](int c) -> int {
+    StagePipe pipe{h->tier, {w + t.off_stage[0], w + t.off_stage[1]}, [&](int64_t c, uint8_t* buf) -> int {
         for (const Run& r : runs)
-            if (r.chunk == c)
-                CU(cudaMemcpyAsync(stage[c & 1] + (size_t)r.stage_row * rb, h->ivf_host + (size_t)r.host_row * rb,
-                                   (size_t)r.rows * rb, cudaMemcpyHostToDevice, h->copy_st));
-        CU(cudaEventRecord(h->stage_ready[c & 1], h->copy_st));
+            if (r.chunk == c) RSB_TRY(tier_copy_rows(h, r.slot, r.rows, buf + (size_t)r.stage_row * rb, h->tier.copy_st));
         return RSB_OK;
-    };
+    }};
     for (int q0 = 0; q0 < nq; q0 += p.qb) {
         const int nb = std::min(p.qb, nq - q0);
         const float* qb = q + (size_t)q0 * h->d;
@@ -1581,10 +1579,8 @@ static int search_ivf_tiered(rsb_index* h, const float* q, int nq, int k, const 
         CU(cudaMemsetAsync(a.out_cnt, 0, (size_t)nb * p.nprobe * 4, st));
         launch_ivf_probed_flags(cI, nb * p.nprobe, nlist, h->l_dev, h->list_len, dflags, st);
         CU(cudaMemcpyAsync(hflags, dflags, (size_t)nlist, cudaMemcpyDeviceToHost, st));
-        CU(cudaEventRecord(h->flags_ready, st));
-        // copies of this batch may start now: the previous batch's scans of the staging buffers are done by then
-        CU(cudaEventRecord(h->copy_start, st));
-        CU(cudaStreamWaitEvent(h->copy_st, h->copy_start, 0));
+        CU(cudaEventRecord(h->tier.flags_ready, st));
+        RSB_TRY(pipe.begin(st));
         static const bool lpt_env = getenv("RSB_LIST_ORDER_LPT") != nullptr;
         const bool lpt_order = lpt_env || ((long)nb * p.nprobe < 64L * 3 * device_num_sms());
         PairWork pw = carve_pair_work(w + p.off_pair, nb, p.nprobe, nlist);
@@ -1595,38 +1591,34 @@ static int search_ivf_tiered(rsb_index* h, const float* q, int nq, int k, const 
             launch_ivfflat_scan(a, qb, vecs, data, h->elem_bytes(), h->d, nb, st, h->sq, h->by_residual);
             h->launches += 4;
         };
-        if (h->ivf_dev_rows > 0) scan_piece(h->dev_len, h->payload, h->list_slot_off);   // the device lists, in place
-        CU(cudaEventSynchronize(h->flags_ready));
+        if (h->tier.dev_rows > 0) scan_piece(h->dev_len, h->payload, h->list_slot_off);   // the device lists, in place
+        CU(cudaEventSynchronize(h->tier.flags_ready));
         runs.clear();
         int nchunks = 0;
         int64_t used = stage_rows;
         for (int l = 0; l < nlist; ++l) { chunk_of[l] = -1; stage_off[l] = 0; }
         for (int l = h->l_dev; l < nlist; ++l) {
             if (!hflags[l]) continue;
-            const int64_t len = h->ivf_len[l], host_row = h->ivf_off[l] - h->ivf_dev_rows;
+            const int64_t len = h->ivf_len[l], slot = h->ivf_off[l];
             if (used + len > stage_rows) { ++nchunks; used = 0; }
             chunk_of[l] = nchunks - 1;
             stage_off[l] = used;
             Run* last = runs.empty() ? nullptr : &runs.back();
-            if (last && last->chunk == nchunks - 1 && last->host_row + last->rows == host_row) last->rows += len;
-            else runs.push_back(Run{nchunks - 1, host_row, used, len});
+            if (last && last->chunk == nchunks - 1 && last->slot + last->rows == slot) last->rows += len;
+            else runs.push_back(Run{nchunks - 1, slot, used, len});
             used += len;
         }
         if (nchunks > 0) {
             // on the copy stream, ahead of the chunks: an H2D on `st` would queue behind the device-piece scan and
             // hold up the chunk copies behind it on the copy engine.  st reads it after waiting for stage_ready.
-            CU(cudaMemcpyAsync(dtab, stage_off, (size_t)nlist * 12, cudaMemcpyHostToDevice, h->copy_st));
-            for (int c = 0; c < std::min(2, nchunks); ++c) RSB_TRY(copy_chunk(c));
+            CU(cudaMemcpyAsync(dtab, stage_off, (size_t)nlist * 12, cudaMemcpyHostToDevice, h->tier.copy_st));
+            RSB_TRY(pipe.prefetch(nchunks));
             for (int c = 0; c < nchunks; ++c) {
-                CU(cudaStreamWaitEvent(st, h->stage_ready[c & 1], 0));
+                RSB_TRY(pipe.acquire(c, st));
                 launch_ivf_piece_tables(h->list_len, dtab, reinterpret_cast<const int*>(dtab + nlist), nlist, c, plen,
                                         pdata, st);
-                scan_piece(plen, stage[c & 1], pdata);
-                CU(cudaEventRecord(h->stage_free[c & 1], st));
-                if (c + 2 < nchunks) {
-                    CU(cudaStreamWaitEvent(h->copy_st, h->stage_free[c & 1], 0));
-                    RSB_TRY(copy_chunk(c + 2));
-                }
+                scan_piece(plen, pipe.buffer(c), pdata);
+                RSB_TRY(pipe.release(c, st));
             }
         }
         launch_merge_items(a.out_keys, a.out_cnt, nb, p.nprobe, k, k, h->ids_slots, 0, D + (size_t)q0 * k,
@@ -1634,9 +1626,7 @@ static int search_ivf_tiered(rsb_index* h, const float* q, int nq, int k, const 
         h->launches += 3;
         CHECK_LAUNCH();
     }
-    CU(cudaEventRecord(h->copy_done, h->copy_st));   // join the copy stream back to the caller's
-    CU(cudaStreamWaitEvent(st, h->copy_done, 0));
-    return RSB_OK;
+    return pipe.end(st);
 }
 
 // shared: the multi-GPU threshold exchange, or nullptr for thresholds kept in the workspace
@@ -1657,7 +1647,7 @@ static int search_impl(rsb_index_t* h, const float* q, int nq, int k, int nprobe
     if (h->kind == RSB_FLAT) {
         if (h->prof) CU(cudaEventRecord(h->ev[0], st));
         const FlatPlan fp = flat_plan(h, nq, k);
-        if (flat_is_streamed(h)) {
+        if (h->host_rows() > 0) {
             RSB_TRY(search_flat_tiered(h, q, nq, k, D, I, ws, ws_bytes, st));
         } else if (fp.tensor && h->ntotal > 0) {
             // tensor-core candidates (k + 8 per query; 3xTF32 on wgmma, or the scaled fp16 query split against fp16
@@ -1699,7 +1689,7 @@ static int search_impl(rsb_index_t* h, const float* q, int nq, int k, int nprobe
 
     if (nprobe <= 0) return fail(RSB_ERR_INVALID, "nprobe must be > 0, got %d", nprobe);
     RSB_TRY(ivf_check_complete(h));
-    if (h->ivf_reserved && shared)
+    if (h->ivf_reserved() && shared)
         return fail(RSB_ERR_UNSUPPORTED, "shared thresholds (a multi-GPU partition) are not implemented for an IVFFLAT "
                                          "index with reserved, tiered lists");
     const SearchPlan p = search_plan(h, nq, k, nprobe);
@@ -1715,7 +1705,7 @@ static int search_impl(rsb_index_t* h, const float* q, int nq, int k, int nprobe
         CU(cudaStreamSynchronize(st));
         return RSB_OK;
     }
-    if (h->ivf_streamed()) {
+    if (h->host_rows() > 0) {
         const IvfTierPlan t = ivf_tier_plan(h, p.total);
         if (pre_lists && p.nprobe != nprobe)
             return fail(RSB_ERR_INVALID, "preassigned nprobe %d exceeds nlist %d", nprobe, h->nlist);
@@ -2149,7 +2139,7 @@ extern "C" int rsb_set_option(rsb_index_t* h, int option, int64_t value) {
             h->coarse_tensor = value != 0; h->flat_tensor = value != 0; return RSB_OK;
         case RSB_OPT_BY_RESIDUAL:
             if (!is_sq8_ivf(h)) return fail(RSB_ERR_INVALID, "RSB_OPT_BY_RESIDUAL applies to an IVFFLAT index with SQ8 storage only");
-            if (h->ntotal || h->n_staged || h->ivf_reserved)
+            if (h->ntotal || h->n_staged || h->ivf_reserved())
                 return fail(RSB_ERR_STATE, "by_residual cannot change once vectors are added (or lists reserved)");
             h->by_residual = value != 0; return RSB_OK;
         case RSB_OPT_DEVICE_ROWS:
@@ -2160,8 +2150,8 @@ extern "C" int rsb_set_option(rsb_index_t* h, int option, int64_t value) {
                                              "index stays in device memory)");
             if (h->ntotal || h->n_staged) return fail(RSB_ERR_STATE, "device_rows cannot change once vectors are added");
             if (value < 0) return fail(RSB_ERR_INVALID, "device_rows must be >= 0, got %lld", (long long)value);
-            RSB_TRY(ensure_copy_stream(h));
-            h->dev_rows = value;
+            RSB_TRY(ensure_copy_stream(h->tier));
+            h->tier.dev_rows = value;
             return RSB_OK;
         case RSB_OPT_STAGING_BYTES:
             if (h->kind != RSB_FLAT || h->dtype != RSB_DTYPE_F16)
@@ -2169,7 +2159,7 @@ extern "C" int rsb_set_option(rsb_index_t* h, int option, int64_t value) {
             if (value < (int64_t)h->row_bytes())
                 return fail(RSB_ERR_INVALID, "a staging buffer must hold one row (%zu bytes), got %lld", h->row_bytes(),
                             (long long)value);
-            h->staging_bytes = (size_t)value;
+            h->tier.staging_bytes = (size_t)value;
             return RSB_OK;
         default: return fail(RSB_ERR_INVALID, "unknown option %d", option);
     }

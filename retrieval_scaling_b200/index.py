@@ -71,6 +71,19 @@ def _check_dtype(dtype: str, what: str = "dtype") -> str:
     return dtype
 
 
+def _check_rows_arg(v, name: str) -> Optional[int]:
+    if v is None:
+        return None
+    if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) or v < 0:
+        raise ValueError(f"{name} must be None or an integer >= 0, got {v!r}")
+    return int(v)
+
+
+def _check_device_rows(device_rows) -> Optional[int]:
+    """The device_rows argument of IndexFlatIP, IndexRefine and read_index."""
+    return _check_rows_arg(device_rows, "device_rows")
+
+
 def _as_storage(x: np.ndarray, dtype: str, what: str) -> np.ndarray:
     """Host vectors for an index that stores `dtype`: an fp16 index accepts only values that round-trip through fp16."""
     if dtype != "float16" or x.dtype == np.float16:
@@ -128,6 +141,17 @@ class _IndexBase:
     @property
     def index_bytes(self) -> int:
         return self._info(_lib.INFO_INDEX_BYTES)
+
+    @property
+    def n_dev(self) -> int:
+        """Rows held in device memory: ntotal unless tiered (a tiered IVF index: those of lists [0, L_dev) once the
+        lists are reserved)."""
+        return self._info(_lib.INFO_DEVICE_ROWS)
+
+    @property
+    def host_bytes(self) -> int:
+        """Page-locked host bytes of the host tier (0 unless tiered)."""
+        return self._info(_lib.INFO_HOST_BYTES)
 
     def _workspace(self, nbytes: int) -> torch.Tensor:
         nbytes = max(int(nbytes), 256)
@@ -202,6 +226,20 @@ class _IndexBase:
         return {n: float(buf[i]) for i, n in enumerate(_lib.PROF_NAMES)}
 
     # -- export (natural CSR order: what the oracle and a faiss file writer consume) --------------------------
+    def export_rows(self, r0: int, n: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Rows [r0, r0 + n) of a Flat or IVF-Flat / IVF-SQ8 index (IVF: CSR rows, the natural order of export_lists)
+        in the storage dtype, from whichever tier holds them, into `out` (a contiguous [n, d] CPU or CUDA tensor;
+        default: a new CPU tensor)."""
+        dt = _REFINE_DTYPES[self.dtype][0]
+        if out is None:
+            out = torch.empty((int(n), self.d), dtype=dt)
+        if tuple(out.shape) != (int(n), self.d) or out.dtype != dt or not out.is_contiguous():
+            raise ValueError(f"out must be a contiguous [{n}, {self.d}] {self.dtype} tensor")
+        with torch.cuda.device(self.device):
+            _lib.check(self.L.rsb_export_rows(self._h, int(r0), int(n), _ptr(out), _stream()))
+            torch.cuda.current_stream().synchronize()
+        return out
+
     def export_lists(self):
         with torch.cuda.device(self.device):
             self.finalize()
@@ -253,16 +291,6 @@ class IndexFlatIP(_IndexBase):
     def tiered(self) -> bool:
         return self.device_rows is not None
 
-    @property
-    def n_dev(self) -> int:
-        """Rows held in device memory (ntotal unless tiered)."""
-        return self._info(_lib.INFO_DEVICE_ROWS)
-
-    @property
-    def host_bytes(self) -> int:
-        """Page-locked host bytes of the host tier (0 unless tiered)."""
-        return self._info(_lib.INFO_HOST_BYTES)
-
     def add(self, x, ids=None) -> None:
         if not self.tiered:
             return super().add(x, ids)
@@ -286,18 +314,6 @@ class IndexFlatIP(_IndexBase):
             _lib.check(self.L.rsb_add(self._h, _ptr(x), _dtype_code(x), x.shape[0], _ptr(idt), None, 0, _stream()))
             torch.cuda.current_stream().synchronize()  # x / idt may be temporaries
 
-    def export_rows(self, r0: int, n: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """Rows [r0, r0 + n) in the storage dtype, from whichever tier holds them, into `out` (a contiguous [n, d] CPU
-        or CUDA tensor; default: a new CPU tensor)."""
-        if out is None:
-            out = torch.empty((int(n), self.d), dtype=_STORE_DTYPES[self.dtype][0])
-        if tuple(out.shape) != (int(n), self.d) or out.dtype != _STORE_DTYPES[self.dtype][0] or not out.is_contiguous():
-            raise ValueError(f"out must be a contiguous [{n}, {self.d}] {self.dtype} tensor")
-        with torch.cuda.device(self.device):
-            _lib.check(self.L.rsb_export_rows(self._h, int(r0), int(n), _ptr(out), _stream()))
-            torch.cuda.current_stream().synchronize()
-        return out
-
     def export_ids(self) -> torch.Tensor:
         """The ids of rows [0, ntotal) (a CUDA int64 tensor)."""
         with torch.cuda.device(self.device):
@@ -306,14 +322,6 @@ class IndexFlatIP(_IndexBase):
             _lib.check(self.L.rsb_export_lists(self._h, None, None, _ptr(ids), _stream()))
             torch.cuda.current_stream().synchronize()
         return ids
-
-
-def _check_rows_arg(v, name: str) -> Optional[int]:
-    if v is None:
-        return None
-    if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) or v < 0:
-        raise ValueError(f"{name} must be None or an integer >= 0, got {v!r}")
-    return int(v)
 
 
 class _IVFBase(_IndexBase):
@@ -335,16 +343,6 @@ class _IVFBase(_IndexBase):
     @property
     def tiered(self) -> bool:
         return self.list_device_rows is not None
-
-    @property
-    def n_dev(self) -> int:
-        """Rows held in device memory: those of lists [0, L_dev) once the lists are reserved, else ntotal."""
-        return self._info(_lib.INFO_DEVICE_ROWS)
-
-    @property
-    def host_bytes(self) -> int:
-        """Page-locked host bytes of the host lists (0 unless tiered and reserved)."""
-        return self._info(_lib.INFO_HOST_BYTES)
 
     def reserve_lists(self, sizes) -> None:
         """Fixes the list sizes [nlist] of a tiered index before anything is added (rsb_reserve_lists): lists [0, L_dev)
@@ -369,19 +367,6 @@ class _IVFBase(_IndexBase):
     def add(self, x, ids=None) -> None:
         self._check_reserved()
         return super().add(x, ids)
-
-    def export_rows(self, r0: int, n: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """CSR rows [r0, r0 + n) (the natural order of export_lists) in the storage dtype, from whichever tier holds
-        them, into `out` (a contiguous [n, d] CPU or CUDA tensor; default: a new CPU tensor)."""
-        dt = _REFINE_DTYPES[self.dtype][0]
-        if out is None:
-            out = torch.empty((int(n), self.d), dtype=dt)
-        if tuple(out.shape) != (int(n), self.d) or out.dtype != dt or not out.is_contiguous():
-            raise ValueError(f"out must be a contiguous [{n}, {self.d}] {self.dtype} tensor")
-        with torch.cuda.device(self.device):
-            _lib.check(self.L.rsb_export_rows(self._h, int(r0), int(n), _ptr(out), _stream()))
-            torch.cuda.current_stream().synchronize()
-        return out
 
     def export_ids_host(self) -> np.ndarray:
         """The ids of CSR rows [0, ntotal) as a host int64 array."""
@@ -668,14 +653,6 @@ def _pinned_rows(L, rows: int, d: int, dtype: torch.dtype, device) -> torch.Tens
     buf = (ctypes.c_char * nbytes).from_address(p.value)
     buf._owner = _PinnedOwner(L, p.value, device)
     return torch.frombuffer(buf, dtype=dtype).view(int(rows), d)
-
-
-def _check_device_rows(device_rows) -> Optional[int]:
-    if device_rows is None:
-        return None
-    if isinstance(device_rows, (bool, np.bool_)) or not isinstance(device_rows, (int, np.integer)) or device_rows < 0:
-        raise ValueError(f"device_rows must be None or an integer >= 0, got {device_rows!r}")
-    return int(device_rows)
 
 
 class IndexRefine:

@@ -47,14 +47,20 @@ class Indexer(object):
         return k_factor, dtype
 
     @staticmethod
+    def _rows_key(index_cfg, key):
+        """Optional key `key`: None when absent, else an integer >= 0 (ValueError naming the key otherwise)."""
+        rows = index_cfg.get(key, None)
+        if rows is not None and (isinstance(rows, bool) or not isinstance(rows, int) or rows < 0):
+            raise ValueError(f"datastore.index.{key} must be an integer >= 0, got {rows!r}")
+        return rows
+
+    @staticmethod
     def refine_device_rows(index_cfg):
         """Optional key `refine_device_rows` (absent: None, every store row in device memory): an integer >= 0; store rows
         from that id on are kept in pinned host memory (index.IndexRefine(device_rows=...)).  Needs refine_k_factor > 0."""
-        rows = index_cfg.get("refine_device_rows", None)
+        rows = Indexer._rows_key(index_cfg, "refine_device_rows")
         if rows is None:
             return None
-        if isinstance(rows, bool) or not isinstance(rows, int) or rows < 0:
-            raise ValueError(f"datastore.index.refine_device_rows must be an integer >= 0, got {rows!r}")
         if not int(index_cfg.get("refine_k_factor", 0) or 0) > 0:
             raise ValueError("datastore.index.refine_device_rows splits the re-rank store: it needs refine_k_factor > 0")
         return rows
@@ -83,11 +89,9 @@ class Indexer(object):
         """Optional key `device_rows` (absent: None, every row in device memory): an integer >= 0; Flat rows from that
         position on are kept in pinned host memory and streamed to the GPU by each search (index.IndexFlatIP(
         device_rows=...)).  Needs index_type Flat with storage_dtype float16."""
-        rows = index_cfg.get("device_rows", None)
+        rows = Indexer._rows_key(index_cfg, "device_rows")
         if rows is None:
             return None
-        if isinstance(rows, bool) or not isinstance(rows, int) or rows < 0:
-            raise ValueError(f"datastore.index.device_rows must be an integer >= 0, got {rows!r}")
         if index_cfg.index_type != "Flat" or index_cfg.get("storage_dtype", None) != "float16":
             raise ValueError(f"datastore.index.device_rows splits a Flat index between device and host memory: it needs "
                              f"index_type Flat and storage_dtype float16 (got {index_cfg.index_type}, "
@@ -100,11 +104,9 @@ class Indexer(object):
         (any storage_dtype) keeps the rows of its first lists -- as many as fit that many rows -- in device memory and the
         others in pinned host memory, copying only the probed host lists at search time (index.IndexIVFFlat(
         list_device_rows=...)).  Needs index_type IVFFlat."""
-        rows = index_cfg.get("list_device_rows", None)
+        rows = Indexer._rows_key(index_cfg, "list_device_rows")
         if rows is None:
             return None
-        if isinstance(rows, bool) or not isinstance(rows, int) or rows < 0:
-            raise ValueError(f"datastore.index.list_device_rows must be an integer >= 0, got {rows!r}")
         if index_cfg.index_type != "IVFFlat":
             raise ValueError(f"datastore.index.list_device_rows splits the inverted lists of an IVFFlat index between "
                              f"device and host memory: it needs index_type IVFFlat (got {index_cfg.index_type})")
