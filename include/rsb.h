@@ -397,6 +397,21 @@ int rsb_bert_create(int hidden, int layers, int heads, int intermediate, int voc
  * T5Block in fp16 is restated with the condition taken over the real tokens of the batch (HF's covers pad positions
  * too).  Free with rsb_bert_free. */
 int rsb_t5_create(int layers, int d_ff, int vocab, int num_buckets, int max_distance, float eps, rsb_bert_t** out);
+/* A RoBERTa encoder behind the same handle: HF RobertaModel as `AutoModel.from_pretrained(name)` builds it for the
+ * DRAGON-RoBERTa query and context encoders, with the CLS row taken (src/search.py:241-243 and :93-94, src/embed.py:
+ * 123-126 and :74-78).  BERT-base layers (hidden 768, 12 heads, erf GELU; intermediate % 128 == 0, RSB_ERR_UNSUPPORTED
+ * otherwise) with RoBERTa's positions: a token with id padding_idx gets position padding_idx, every other token
+ * padding_idx + the number of ids != padding_idx from the start of its sequence up to and including itself
+ * (modeling_roberta.py create_position_ids_from_input_ids), so a pad id inside a sequence is not counted.
+ * padding_idx must leave at least one position below max_pos (RSB_ERR_INVALID); type_vocab 1 or 2
+ * (RSB_ERR_UNSUPPORTED otherwise).  The handle then takes rsb_bert_load with HF RobertaModel keys, which are
+ * BertModel's ("embeddings.token_type_embeddings.weight" is [type_vocab, 768]; pooler.* is not loaded), and runs
+ * rsb_bert_forward / rsb_bert_attention.  rsb_bert_forward on it returns RSB_ERR_UNSUPPORTED before any launch when
+ * padding_idx + max_seqlen >= max_pos (a position would pass the table; with roberta-base's 514 rows and padding_idx 1
+ * every sequence of <= 512 tokens fits), and RSB_ERR_INVALID when token_type_ids_dev holds a value outside
+ * [0, type_vocab) (it reads them back to the host to check; NULL means all zero).  Free with rsb_bert_free. */
+int rsb_roberta_create(int layers, int intermediate, int vocab, int max_pos, int type_vocab, float ln_eps,
+                       int padding_idx, rsb_bert_t** out);
 int rsb_bert_free(rsb_bert_t* h);
 /* name = HF BertModel state_dict key (e.g. "encoder.layer.3.attention.self.query.weight"); data fp16, copied.
  * T5 handles take HF T5EncoderModel keys instead: "shared.weight" or "encoder.embed_tokens.weight" (tied),

@@ -81,6 +81,7 @@ SIGNATURES = [
     ("rsb_bert_last_error", c_char_p, []),
     ("rsb_bert_create", c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, POINTER(_H)]),
     ("rsb_t5_create", c_int, [c_int, c_int, c_int, c_int, c_int, c_float, POINTER(_H)]),
+    ("rsb_roberta_create", c_int, [c_int, c_int, c_int, c_int, c_int, c_float, c_int, POINTER(_H)]),
     ("rsb_bert_free", c_int, [_H]),
     ("rsb_bert_load", c_int, [_H, c_char_p, c_void_p, c_int64, c_void_p]),
     ("rsb_bert_workspace_bytes", c_size_t, [_H, c_int]),

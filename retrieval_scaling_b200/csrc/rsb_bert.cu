@@ -2,6 +2,7 @@
 // called from src/search.py:83-96 with the model in fp16) on variable-length (un-padded) token streams.
 //
 //   embed_ln_kernel      word + position + token-type gather, LayerNorm(eps)                    -> H  [T,768]  f16
+//                        (<true>: RoBERTa positions, padding_idx + count of non-pad ids, for rsb_roberta_create)
 //   gemm_tn_kernel       Y = X . W^T (+bias [+GELU | +residual]) on the Hopper tensor cores: TMA (cp.async.bulk.tensor,
 //                        128B swizzle) -> shared-memory ring -> wgmma.mma_async f16 (fp32 accumulate in registers) ->
 //                        epilogue from the registers.  Warp-specialised producer / consumer warpgroups synchronised
@@ -254,11 +255,28 @@ __device__ __forceinline__ void load_row24(const __half* row, int lane, float (&
     }
 }
 
+// RoBERTa position of the token at offset p of the sequence starting at seq (modeling_roberta.py
+// create_position_ids_from_input_ids): padding_idx for a pad id, otherwise padding_idx + the number of non-pad ids in
+// seq[0..p].  Called by the whole warp (p is warp-uniform): 32 ids per ballot, ceil((p + 1) / 32) coalesced loads.
+__device__ __forceinline__ int roberta_position(const int* __restrict__ seq, int p, int id, int padding_idx, int lane) {
+    if (id == padding_idx) return padding_idx;
+    int n = 0;
+    for (int j0 = 0; j0 <= p; j0 += 32) {
+        const int j = j0 + lane;
+        n += __popc(__ballot_sync(0xffffffffu, j <= p && seq[j] != padding_idx));
+    }
+    return padding_idx + n;
+}
+
+// ROBERTA = false: BERT, position = offset in the sequence.  ROBERTA = true: roberta_position (the host has refused any
+// sequence whose positions would pass max_pos).  In both forms the position is clamped to the table, which only
+// matters for a caller that passes a max_seqlen below its longest sequence.
+template <bool ROBERTA>
 __global__ void embed_ln_kernel(const int* __restrict__ input_ids, const int* __restrict__ type_ids,
                                 const int* __restrict__ cu_seqlens, int B, int T, const __half* __restrict__ word,
                                 const __half* __restrict__ pos, const __half* __restrict__ type,
                                 const __half* __restrict__ gamma, const __half* __restrict__ beta, float eps,
-                                int vocab, int max_pos, __half* __restrict__ out) {
+                                int vocab, int max_pos, __half* __restrict__ out, int padding_idx) {
     const int lane = threadIdx.x & 31;
     const int t = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (t >= T) return;
@@ -268,6 +286,7 @@ __global__ void embed_ln_kernel(const int* __restrict__ input_ids, const int* __
         if (cu_seqlens[mid] <= t) lo = mid; else hi = mid;
     }
     int p = t - cu_seqlens[lo];
+    if constexpr (ROBERTA) p = roberta_position(input_ids + cu_seqlens[lo], p, input_ids[t], padding_idx, lane);
     p = p < max_pos ? p : max_pos - 1;
     int id = input_ids[t];
     id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
@@ -888,6 +907,7 @@ struct Layer {
 struct rsb_bert {
     int hidden = 768, layers = 12, heads = 12, inter = 3072, vocab = 30522, max_pos = 512, type_vocab = 2;
     float eps = 1e-12f;
+    int padding_idx = -1;                                // >= 0: a RoBERTa handle (rsb_roberta_create), its position rule
     __half *word = nullptr, *pos = nullptr, *type = nullptr, *emb_g = nullptr, *emb_b = nullptr;
     std::vector<Layer> L;
     // T5 encoder (rsb_t5_create): pre-norm blocks, RMS norms ln1_g / ln2_g, no biases (the Linear biases stay zero)
@@ -1067,6 +1087,25 @@ extern "C" int rsb_t5_create(int layers, int d_ff, int vocab, int num_buckets, i
     return RSB_OK;
 }
 
+// Replaces `AutoModel.from_pretrained(name)` + `last_hidden_state[:, 0, :]` for RoBERTa checkpoints such as
+// DRAGON-RoBERTa's query and context encoders (src/search.py:241-243 and :93-94, src/embed.py:123-126 and :74-78):
+// HF RobertaModel = BERT-base layers behind RoBERTa's embedding positions.
+extern "C" int rsb_roberta_create(int layers, int inter, int vocab, int max_pos, int type_vocab, float ln_eps,
+                                  int padding_idx, rsb_bert_t** out) {
+    if (!out) return bfail(RSB_ERR_INVALID, "out is NULL");
+    *out = nullptr;
+    if (padding_idx < 0 || padding_idx + 2 > max_pos)
+        return bfail(RSB_ERR_INVALID, "padding_idx %s%ld leaves no position for a token below max_pos", "", (long)padding_idx);
+    if (type_vocab != 1 && type_vocab != 2)
+        return bfail(RSB_ERR_UNSUPPORTED, "RoBERTa with type_vocab_size %s%ld: only 1 or 2 are implemented", "", (long)type_vocab);
+    rsb_bert_t* h = nullptr;
+    const int rc = rsb_bert_create(768, layers, 12, inter, vocab, max_pos, type_vocab, ln_eps, &h);
+    if (rc != RSB_OK) return rc;
+    h->padding_idx = padding_idx;
+    *out = h;
+    return RSB_OK;
+}
+
 extern "C" int rsb_bert_free(rsb_bert_t* h) {
     if (!h) return RSB_OK;
     cudaFree(h->word); cudaFree(h->pos); cudaFree(h->type); cudaFree(h->emb_g); cudaFree(h->emb_b);
@@ -1217,10 +1256,23 @@ extern "C" int rsb_bert_forward(rsb_bert_t* h, const int32_t* input_ids, const i
         return bfail(RSB_ERR_STATE, "T5 forward before relative_position_bucket and the relative_attention_bias weight were loaded");
     if (max_seqlen > ATT_MAXS || max_seqlen > h->max_pos)
         return bfail(RSB_ERR_UNSUPPORTED, "sequence longer than %s%ld tokens", "", (long)std::min(ATT_MAXS, h->max_pos));
+    const bool roberta = h->padding_idx >= 0;
+    if (roberta && h->padding_idx + max_seqlen >= h->max_pos)    // the last token's position is at most padding_idx + S
+        return bfail(RSB_ERR_UNSUPPORTED, "RoBERTa positions of a %s%ld-token sequence pass max_position_embeddings",
+                     "", (long)max_seqlen);
     size_t off[7];
     const size_t need = bert_ws_layout(h, T, off);
     if (ws_bytes < need) return bfail(RSB_ERR_OOM, "encoder workspace too small (%s need %ld bytes)", "", (long)need);
     cudaStream_t st = (cudaStream_t)stream;
+    if (roberta && token_type_ids) {                     // HF raises on a token type outside the table: refuse, not clamp
+        std::vector<int32_t> tt(T);
+        if (cudaMemcpyAsync(tt.data(), token_type_ids, (size_t)T * sizeof(int32_t), cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+            cudaStreamSynchronize(st) != cudaSuccess)
+            return bfail(RSB_ERR_CUDA, "copy of token_type_ids failed");
+        for (int32_t v : tt)
+            if (v < 0 || v >= h->type_vocab)
+                return bfail(RSB_ERR_INVALID, "token type %s%ld is outside this RoBERTa handle's type_vocab_size", "", (long)v);
+    }
     unsigned char* w = static_cast<unsigned char*>(ws);
     __half* Hs = reinterpret_cast<__half*>(w + off[0]);
     __half* QKV = reinterpret_cast<__half*>(w + off[1]);
@@ -1235,9 +1287,12 @@ extern "C" int rsb_bert_forward(rsb_bert_t* h, const int32_t* input_ids, const i
     if (h->t5) {
         embed_gather_kernel<<<ln_grid, 256, 0, st>>>(input_ids, T, h->word, h->vocab, TMP);
         cudaMemsetAsync(flags, 0, (size_t)2 * h->layers * sizeof(int), st);
+    } else if (roberta) {
+        embed_ln_kernel<true><<<ln_grid, 256, 0, st>>>(input_ids, token_type_ids, cu_seqlens, B, T, h->word, h->pos, h->type,
+                                                       h->emb_g, h->emb_b, h->eps, h->vocab, h->max_pos, Hs, h->padding_idx);
     } else {
-        embed_ln_kernel<<<ln_grid, 256, 0, st>>>(input_ids, token_type_ids, cu_seqlens, B, T, h->word, h->pos, h->type,
-                                                 h->emb_g, h->emb_b, h->eps, h->vocab, h->max_pos, Hs);
+        embed_ln_kernel<false><<<ln_grid, 256, 0, st>>>(input_ids, token_type_ids, cu_seqlens, B, T, h->word, h->pos, h->type,
+                                                        h->emb_g, h->emb_b, h->eps, h->vocab, h->max_pos, Hs, -1);
     }
     h->launches++;
     const int prc = prepare_attention(h, cu_seqlens, B, max_seqlen, st);

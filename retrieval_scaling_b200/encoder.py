@@ -6,7 +6,9 @@
 
 The forward pass is librsb's `rsb_bert_forward` (wgmma tensor-core GEMMs fed by TMA with fused bias / GELU /
 residual epilogues, fused embedding+LayerNorm, shared-memory attention, mean / CLS pooling) on the un-padded
-token stream.  No CPU / eager-PyTorch fallback: constructing the model without CUDA raises.
+token stream.  No CPU / eager-PyTorch fallback: constructing the model without CUDA raises.  An HF checkpoint whose
+`model_type` is "roberta" (DRAGON-RoBERTa's query and context encoders) loads as `B200Roberta`: the same layers behind
+RoBERTa's embedding positions (`rsb_roberta_create`).
 
 The same library runs the sentence-transformers retrievers the reference loads with `SentenceTransformer(name)`
 (`src/search.py:49-61`, `src/embed.py:25-40`): `load_sentence_transformer(path)` reads the model directory into a
@@ -233,7 +235,7 @@ def random_state_dict(config=None, seed: int = 0, device="cpu") -> Dict[str, tor
 
 
 def strip_wrapper_prefix(sd: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
-    """Checkpoint key names -> HF BertModel key names.
+    """Checkpoint key names -> HF BertModel key names (RobertaModel uses the same names, behind 'roberta.').
 
     The reference (`contriever.py:121-125`) keeps the keys containing 'encoder_q.' (MoCo wrapper: query tower) or else
     'encoder.' (in-batch wrapper) and removes that substring with `str.replace` -- which removes EVERY occurrence, so
@@ -245,8 +247,9 @@ def strip_wrapper_prefix(sd: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]
         return {k[len("encoder_q."):]: v for k, v in sd.items() if k.startswith("encoder_q.")}
     if any(k.startswith("encoder.embeddings.") or k.startswith("encoder.encoder.") for k in keys):
         return {k[len("encoder."):]: v for k, v in sd.items() if k.startswith("encoder.")}
-    if any(k.startswith("bert.") for k in keys):
-        return {k[len("bert."):]: v for k, v in sd.items() if k.startswith("bert.")}
+    for prefix in ("bert.", "roberta."):
+        if any(k.startswith(prefix) for k in keys):
+            return {k[len(prefix):]: v for k, v in sd.items() if k.startswith(prefix)}
     return dict(sd)
 
 
@@ -277,8 +280,11 @@ def read_retriever_files(model_path: str, tokenizer_name: Optional[str] = None):
         tokenizer = load_hf(transformers.AutoTokenizer, tokenizer_name or model_path)
         hf = load_hf(transformers.AutoModel, model_path)
         sd = strip_wrapper_prefix(hf.state_dict())
-    if getattr(cfg, "model_type", "bert") != "bert":
-        raise AttributeError(f"{model_path}: only BERT-architecture encoders run on the GPU path")
+    model_type = getattr(cfg, "model_type", "bert")
+    if model_type == "roberta":
+        _roberta_config(cfg)
+    elif model_type != "bert":
+        raise AttributeError(f"{model_path}: only BERT-architecture encoders (BERT, RoBERTa-base) run on the GPU path")
     return sd, cfg, tokenizer, model_id
 
 
@@ -295,10 +301,54 @@ def load_retriever(model_path: str, tokenizer_name: Optional[str] = None, poolin
         import warnings
         warnings.warn("no_fp16 / fp16=False was requested, but the encoder computes in fp16 with fp32 accumulation "
                       "only (the reference's default path, src/search.py:257-258); continuing in fp16")
-    model = B200Contriever(cfg, pooling)
+    cls = B200Roberta if getattr(cfg, "model_type", "bert") == "roberta" else B200Contriever
+    model = cls(cfg, pooling)
     model.load_state_dict(sd, strict=False)
     model.require_all_weights(model_path)
     return model, tokenizer, model_id
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# RoBERTa-base (DRAGON-RoBERTa's query and context encoders)
+# ----------------------------------------------------------------------------------------------------------------
+ROBERTA_BASE = dict(BERT_BASE, vocab_size=50265, max_position_embeddings=514, type_vocab_size=1, layer_norm_eps=1e-5,
+                    pad_token_id=1)
+
+
+def _roberta_config(config) -> dict:
+    """The RoBERTa geometry the kernels run (hidden 768, 12 heads, erf GELU), or AttributeError."""
+    get = (lambda k, d=None: config.get(k, d)) if isinstance(config, dict) else (lambda k, d=None: getattr(config, k, d))
+    geom = dict(hidden_size=get("hidden_size", 768), num_attention_heads=get("num_attention_heads", 12),
+                hidden_act=get("hidden_act", "gelu"))
+    if geom != dict(hidden_size=768, num_attention_heads=12, hidden_act="gelu"):
+        raise AttributeError(f"unsupported RoBERTa geometry {geom}: only RoBERTa-base (hidden 768, 12 heads, GELU) "
+                             f"runs on the GPU path")
+    c = {k: get(k, ROBERTA_BASE[k]) for k in ROBERTA_BASE}
+    if c["pad_token_id"] is None:
+        raise AttributeError("RoBERTa config without pad_token_id: its positions are counted from padding_idx")
+    return c
+
+
+class B200Roberta(B200Contriever):
+    """HF `RobertaModel` (RoBERTa-base geometry) + CLS row or mean pooling on librsb (`rsb_roberta_create`): the BERT
+    layers behind RoBERTa's positions, padding_idx + the count of non-pad ids up to each token.  Same call surface
+    and HF key names as `B200Contriever`; token_type_ids other than 0 on a type_vocab_size 1 model raise ValueError,
+    as HF raises on them."""
+
+    def _create(self, config):
+        self.config = _roberta_config(config or {})
+        c = self.config
+        rc = self.L.rsb_roberta_create(c["num_hidden_layers"], c["intermediate_size"], c["vocab_size"],
+                                       c["max_position_embeddings"], c["type_vocab_size"],
+                                       ctypes.c_float(c["layer_norm_eps"]), int(c["pad_token_id"]), ctypes.byref(self._h))
+        self._check(rc)
+
+    def require_all_weights(self, source: str = "state_dict"):
+        missing = self.missing_keys()
+        if missing:
+            raise KeyError(f"{source}: {len(missing)} of {len(self.expected_keys())} RoBERTa encoder weights were not "
+                           f"found (first missing: {missing[:4]}); keys must follow HF RobertaModel naming after the "
+                           f"'roberta.' prefix stripping")
 
 
 # ----------------------------------------------------------------------------------------------------------------

@@ -1,6 +1,7 @@
 """T5 encoder (GTR-T5 geometry: 12 layers, d_model 768, 12 heads of 64, d_ff 3072, with the sentence-transformers
-Dense + Normalize head) against the BERT-base forward (Contriever, mean pooling) on the same token streams, in one
-process, the two alternated.
+Dense + Normalize head) and RoBERTa-base (DRAGON-RoBERTa geometry: 12 layers, vocabulary 50265, 514 positions, CLS
+row) against the BERT-base forward (Contriever, mean pooling), in one process, the three alternated.  RoBERTa runs on
+the BERT arm's token streams themselves (ids 3 .. 30521, valid and never the pad id 1 in its vocabulary).
 
 Workloads (seeded weights, random token ids; only the lengths matter to the kernels):
   q64 / q2048   10 000 queries whose token counts are drawn from tests/golden/nq_open_token_lengths.npy (NQ-open
@@ -9,7 +10,7 @@ Workloads (seeded weights, random token ids; only the lengths matter to the kern
   p256 / p512   512 passages of 256 and of 512 tokens (the passage side at its reference batch size)
 
 Per workload: median ms over `--steps` alternated repetitions of the whole workload, and TFLOP/s of its Linear-layer
-work: 169.9 MFLOP per token for both models (2 x (4 x 768^2 + 2 x 768 x 3072) x 12 layers; T5 only drops the biases).
+work: 169.9 MFLOP per token for all three models (2 x (4 x 768^2 + 2 x 768 x 3072) x 12 layers; T5 only drops the biases).
 Attention and the head are not counted.  The card's name and power limit are read in the same run.
 
     python scripts/bench_encoder_st.py --steps 5 --warmup 2 [--out results.json]
@@ -75,14 +76,17 @@ def main():
     a = ap.parse_args()
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
-    from retrieval_scaling_b200.encoder import (BERT_BASE, T5_BASE, B200Contriever, B200T5Encoder, random_state_dict,
-                                                random_t5_state_dict)
+    from retrieval_scaling_b200.encoder import (BERT_BASE, ROBERTA_BASE, T5_BASE, B200Contriever, B200Roberta,
+                                                B200T5Encoder, random_state_dict, random_t5_state_dict)
     t5 = B200T5Encoder(T5_BASE, "average", dense=True, normalize=True)
     t5.load_state_dict(random_t5_state_dict(T5_BASE, 0))
     t5.require_all_weights("bench")
     bert = B200Contriever(BERT_BASE, "average")
     bert.load_state_dict(random_state_dict(BERT_BASE, 0))
-    models = {"t5": t5, "bert": bert}
+    roberta = B200Roberta(ROBERTA_BASE, "cls")
+    roberta.load_state_dict(random_state_dict(ROBERTA_BASE, 0))
+    roberta.require_all_weights("bench")
+    models = {"t5": t5, "bert": bert, "roberta": roberta}
     vocab = {"t5": T5_BASE["vocab_size"], "bert": BERT_BASE["vocab_size"]}
     ident = gpu_identity(dev)
     rng = np.random.default_rng(0)
@@ -91,7 +95,8 @@ def main():
         if a.only and name not in a.only.split(","):
             continue
         seed = int(rng.integers(1 << 30))
-        fwd = {m: batches(lens, group, vocab[m], np.random.default_rng(seed), dev) for m in models}
+        fwd = {m: batches(lens, group, vocab[m], np.random.default_rng(seed), dev) for m in vocab}
+        fwd["roberta"] = fwd["bert"]
         tokens = int(lens.sum())
         if a.profile:
             for m in models:
@@ -118,6 +123,7 @@ def main():
             line[m] = {"ms": round(med, 3), "ms_min": round(min(ms[m]), 3), "ms_max": round(max(ms[m]), 3),
                        "linear_tflops": round(LINEAR_FLOP_PER_TOKEN * tokens / (med * 1e-3) / 1e12, 1)}
         line["t5_over_bert"] = round(line["t5"]["ms"] / line["bert"]["ms"], 3)
+        line["roberta_over_bert"] = round(line["roberta"]["ms"] / line["bert"]["ms"], 3)
         print(json.dumps(line), flush=True)
         results.append(line)
     if a.out and results:
