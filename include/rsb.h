@@ -452,6 +452,33 @@ enum { RSB_GEMM_REVERSED = 256 };
 int rsb_gemm_f16(const void* A_dev, const void* W_dev, const void* bias_dev, const void* residual_dev, void* C_dev,
                  int M, int N, int K, int epilogue, rsb_stream_t stream);
 
+/* ---- MinHash de-duplication of retrieved passages ----------------------------------------------------------------
+ * Replaces utils/deduplication.py's `remove_duplicates_with_minhash` (datasketch MinHash(num_perm=128) and
+ * MinHashLSH(threshold=0.8)) run by src/search.py:471-479 on the merged multi-source results.  Errors of these entries
+ * are reported by rsb_dedup_last_error().
+ * rsb_minhash_signatures: texts are the UTF-8 slices text_dev[text_off_dev[t] .. text_off_dev[t+1]) of one buffer of
+ * total_bytes < 2^31 bytes, each valid UTF-8 on its own.  Words are split on the code points of Python's str.isspace()
+ * (`text.split()`); shingle i of a text is words i..i+12 joined by single spaces, hashed as datasketch's sha1_hash32
+ * (first 4 bytes of SHA-1, little-endian).  sig_dev [n_texts, 128] uint32 receives, per permutation j, the minimum over
+ * the shingles of ((h * a_j + b_j) mod 2^64) mod (2^61 - 1) & 0xffffffff (2^32 - 1 without shingles); perm_a_dev /
+ * perm_b_dev uint64 [128] are MinHash.permutations.  n_words_dev [n_texts] int32 receives the word counts.  ws_dev holds
+ * rsb_minhash_workspace_bytes(total_bytes) bytes. */
+const char* rsb_dedup_last_error(void);
+size_t rsb_minhash_workspace_bytes(int64_t total_bytes);
+int rsb_minhash_signatures(const uint8_t* text_dev, const int64_t* text_off_dev, int n_texts, int64_t total_bytes,
+                           const uint64_t* perm_a_dev, const uint64_t* perm_b_dev, uint32_t* sig_dev, int32_t* n_words_dev,
+                           void* ws_dev, size_t ws_bytes, rsb_stream_t stream);
+/* rsb_minhash_dedup: the slots of group g are rows group_off_dev[g] .. group_off_dev[g+1]) of sig_dev [*, 128] (16-byte
+ * aligned) and n_words_dev.  keep_dev[s] = 1 unless slot s has fewer than 13 words, or some earlier slot of its group
+ * shares all `rows` values of one of the `bands` bands [k * rows, (k + 1) * rows) with it and more than max_equal of
+ * the 128 values (MinHashLSH candidate with jaccard > threshold; 0.8 -> bands 9, rows 13, max_equal 102).
+ * bands * rows <= 128. */
+int rsb_minhash_dedup(const uint32_t* sig_dev, const int32_t* n_words_dev, const int32_t* group_off_dev, int n_groups,
+                      int bands, int rows, int max_equal, uint8_t* keep_dev, rsb_stream_t stream);
+/* host function, no GPU: mask[q] = 1 iff byte q of the valid UTF-8 bytes[0, n) belongs to a character on which the
+ * signatures' word split splits (lets host-side tests pin the whitespace set against Python's str.isspace()) */
+int rsb_utf8_space_mask(const uint8_t* bytes, int64_t n, uint8_t* mask);
+
 /* diagnostic: shared-window address at which dynamic shared memory starts (the scan kernel folds it into LDS) */
 int rsb_debug_smem_base(void);
 /* diagnostic: the fp32 look-up tables an IVFPQ search builds for queries q_dev [nq, d], as the scan reads them:

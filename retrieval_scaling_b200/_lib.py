@@ -90,6 +90,12 @@ SIGNATURES = [
     ("rsb_bert_launches", c_int64, [_H]),
     ("rsb_bert_attention", c_int, [_H, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),   # diagnostic
     ("rsb_gemm_f16", c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    ("rsb_dedup_last_error", c_char_p, []),
+    ("rsb_minhash_workspace_bytes", c_size_t, [c_int64]),
+    ("rsb_minhash_signatures", c_int, [c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,
+                                       c_void_p, c_size_t, c_void_p]),
+    ("rsb_minhash_dedup", c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    ("rsb_utf8_space_mask", c_int, [c_void_p, c_int64, c_void_p]),
     ("rsb_debug_smem_base", c_int, []),
     ("rsb_pq_lut_floats", c_int, [_H]),
     ("rsb_pq_tables", c_int, [_H, c_void_p, c_int, c_void_p, c_void_p]),

@@ -8,8 +8,10 @@
 
 Same function names, argument meaning, output file scheme and resume/overwrite behaviour, so the lm-eval
 harness fork consumes the JSONL unchanged (`ctxs[i]["retrieval text"]`, `"retrieval score"` as str).
-Out of scope here (SURVEY §2 #8): BM25 search, multi-domain merge + MinHash dedup + rerank (CPU text
-post-processing): `search_topk` raises NotImplementedError for `model.sparse_retriever`.
+Multi-source merge with MinHash de-duplication and coin-flip subsampling (:386-546) is
+`post_hoc_merge_topk_multi_domain`, its de-duplication on the GPU (`dedup.py`).  Out of scope (SURVEY §2 #8): BM25
+search (`search_topk` raises NotImplementedError for `model.sparse_retriever`) and the answer-based re-ranking of
+the multi-source merge (`rerank_method`).
 """
 from __future__ import annotations
 
@@ -18,6 +20,8 @@ import json
 import logging
 import os
 import pickle as pkl
+import random
+import re
 from typing import List
 
 import numpy as np
@@ -386,8 +390,8 @@ def search_dense_topk(cfg):
             os.makedirs(os.path.dirname(output_path), exist_ok=True)
             safe_write_jsonl(copied, output_path)
     if eval_args.search.get("merge_multi_source_results", False) and eval_args.search.get("topk_subsample_p", None):
-        raise NotImplementedError("multi-domain merge / dedup / rerank is CPU text post-processing outside the hot path")
-    if eval_args.search.get("merge_multi_index_results", True):
+        post_hoc_merge_topk_multi_domain(cfg)
+    elif eval_args.search.get("merge_multi_index_results", True):
         post_hoc_merge_topk(cfg)
 
 
@@ -418,6 +422,140 @@ def post_hoc_merge_topk(cfg):
         ex["ctxs"] = merge_ctxs(lists, n_docs)
     os.makedirs(os.path.dirname(output_path), exist_ok=True)
     safe_write_jsonl(merged, output_path)
+
+
+# ----------------------------------------------------------------------------------------------------------
+# multi-source merge + MinHash de-duplication + coin-flip subsampling (reference src/search.py:377-566)
+# ----------------------------------------------------------------------------------------------------------
+DATASTORE_DOMAIN = re.compile(r"/([^/]+)_datastore")
+
+
+def merged_before_dedup_path(base_merged_path: str) -> str:
+    """Where the merged, not yet de-duplicated results go (reference :395).  The reference takes
+    `basename.strip('dedup_')`: str.strip removes any of the characters 'd', 'e', 'u', 'p', '_' from both ends of the
+    name, not the prefix "dedup_".  'dedup_merged.jsonl' gives 'merged.jsonl', but 'dedup_dev.jsonl' gives 'v.jsonl'
+    and 'pubmed' gives 'bm'.  Kept as is, so that existing merged files are found under their names."""
+    return os.path.join(os.path.dirname(base_merged_path), os.path.basename(base_merged_path).strip("dedup_"))
+
+
+def subsample_by_coin_flip(items, probability):
+    return [item for item in items if random.random() < probability]
+
+
+def additional_remove_short_chunk(ctxs):
+    """Drops passages of 12 or fewer space-separated pieces (`split(' ')`, unlike the de-duplication's `split()`)."""
+    return [ctx for ctx in ctxs if len(ctx["retrieval text"].split(" ")) > 12]
+
+
+def merge_multi_domain(paths_to_merge: List[str], n_docs: int) -> list:
+    """The per-source result files, merged query by query (reference :414-461): the passages of a source without a
+    "source" field are tagged with the domain of its path (`.../<domain>_datastore...`), the lists concatenated in file
+    order, stably sorted on "retrieval score" descending and cut to n_docs.  The sort compares the stored values as
+    they are: the result files hold scores as strings, so the order is the strings' lexicographic order."""
+    merged = []
+    for domain_idx, path in enumerate(paths_to_merge):
+        print(f"Adding {path}")
+        matches = DATASTORE_DOMAIN.findall(path)
+        ds_domain = matches[0] if matches else None
+        rows = []
+        with open(path) as f:
+            for line in f:
+                try:
+                    ex = json.loads(line)
+                except Exception:  # noqa: BLE001 -- the reference reports the file and raises AttributeError
+                    print(f"Line read error when reading {path}")
+                    raise AttributeError
+                if not ex["ctxs"] or ex["ctxs"][0] is None:
+                    ctxs = []
+                else:
+                    if "source" not in ex["ctxs"][0].keys() or not ex["ctxs"][0]["source"]:
+                        for ctx in ex["ctxs"]:
+                            ctx["source"] = ds_domain
+                    ctxs = ex["ctxs"]
+                ex["ctxs"] = ctxs
+                rows.append(ex)
+        if domain_idx == 0:
+            merged = rows
+            continue
+        for id_, (_, ex) in enumerate(zip(merged, rows)):
+            assert merged[id_]["raw_query"] == ex["raw_query"]
+            merged[id_]["ctxs"].extend(ex["ctxs"])
+            if merged[id_]["ctxs"] and merged[id_]["ctxs"][0] is not None:
+                merged[id_]["ctxs"] = sorted(merged[id_]["ctxs"], key=lambda x: x["retrieval score"], reverse=True)[:n_docs]
+                assert len(merged[id_]["ctxs"]) == n_docs
+            else:
+                assert id_ == 0 or id_ == 983      # the reference's allowance for queries without passages
+    return merged
+
+
+def _read_jsonl_strict(path):
+    with open(path) as f:
+        return [json.loads(line) for line in f]
+
+
+def post_hoc_merge_topk_multi_domain(cfg, deduplicate=None):
+    """Merge the results of several sources (`evaluation.search.paths_to_merge`, a text file with one result file per
+    line), de-duplicate them on the GPU, subsample each query's passages with probability `topk_subsample_p` and write
+    `full_subsampled_{p}_{seed}_{basename(merged_path)}` next to `merged_path` (reference :386-546).
+
+    Files: the merged results go to `merged_before_dedup_path(merged_path)` and are read back from there when that file
+    exists; the de-duplicated results go to `merged_path`, and with `use_saved_dedup_data` an existing `merged_path` is
+    read instead of merging and de-duplicating again.  `deduplicate(examples)` (in place) defaults to
+    `dedup.deduplicate`.  Returns the output path."""
+    s = cfg.evaluation.search
+    if s.get("rerank_method", None):
+        raise NotImplementedError(f"rerank_method={s.rerank_method}: re-ranking (lexical / inclusion / unigram_f1) "
+                                  f"needs the task answer files and is not implemented")
+    if deduplicate is None:
+        from .dedup import deduplicate
+    base_merged_path = s.merged_path
+    merged_path = merged_before_dedup_path(base_merged_path)
+    use_saved = s.get("use_saved_dedup_data", False)
+
+    if not os.path.exists(base_merged_path) or not use_saved:
+        if not os.path.exists(merged_path):
+            paths_to_merge = []
+            with open(s.paths_to_merge) as f:
+                for line in f:
+                    path = line.strip()
+                    paths_to_merge.append(path)
+                    assert os.path.exists(path), f"{path}"
+            print(f"Merging files:\n{paths_to_merge}")
+            merged_data = merge_multi_domain(paths_to_merge, s.n_docs)
+            if os.path.dirname(merged_path):    # the reference writes here before creating the directory (and fails)
+                os.makedirs(os.path.dirname(merged_path), exist_ok=True)
+            safe_write_jsonl(merged_data, merged_path)
+        else:
+            merged_data = _read_jsonl_strict(merged_path)
+        deduplicate(merged_data)
+
+    if os.path.exists(base_merged_path) and use_saved:
+        merged_data = _read_jsonl_strict(base_merged_path)
+    else:
+        if os.path.dirname(base_merged_path):
+            os.makedirs(os.path.dirname(base_merged_path), exist_ok=True)
+        safe_write_jsonl(merged_data, base_merged_path)
+
+    p = s.topk_subsample_p
+    seed = s.get("subsample_seed", 1000)
+    if p < 1:                                   # the draws of random.random() after random.seed(seed), query by query
+        random.seed(seed)
+        for ex in merged_data:
+            ex["ctxs"] = subsample_by_coin_flip(ex["ctxs"], p)
+    for ex in merged_data:
+        ex["ctxs"] = additional_remove_short_chunk(ex["ctxs"])
+    no_enough_data_count = 0
+    for ex in merged_data:
+        if len(ex["ctxs"]) < 3:
+            no_enough_data_count += 1
+            print(f"WARNING: the subsampled documents only have {len(ex['ctxs'])} left!")
+    output_path = os.path.join(os.path.dirname(base_merged_path),
+                               f"full_subsampled_{str(p)}_{seed}_{os.path.basename(base_merged_path)}")
+    if os.path.dirname(output_path):
+        os.makedirs(os.path.dirname(output_path), exist_ok=True)
+    safe_write_jsonl(merged_data, output_path)
+    print(f"Saved merged results to {output_path} with {no_enough_data_count} documents having less than 5 documents.")
+    return output_path
 
 
 def search_topk(cfg):

@@ -5,9 +5,10 @@
 
 Hydra / OmegaConf are replaced by `retrieval_scaling_b200.config` (same YAML files, same dotted overrides).
 Task switches: tasks.datastore.embedding (already-chunked passage shards -> embedding pickles, SURVEY §8f-4),
-tasks.datastore.index (build or load the index), tasks.eval.search (query -> top-k, the hot path).
-tasks.eval.merge_search and tasks.eval.inference belong to subsystems that are out of scope of the GPU hot path
-(SURVEY.md §2) and raise NotImplementedError.
+tasks.datastore.index (build or load the index), tasks.eval.search (query -> top-k, the hot path),
+tasks.eval.merge_search (multi-source merge, MinHash de-duplication on the GPU and subsampling, reference :31-33).
+tasks.eval.inference belongs to a subsystem that is out of scope of the GPU hot path (SURVEY.md §2) and raises
+NotImplementedError.
 """
 import logging
 import os
@@ -59,7 +60,9 @@ def main(cfg) -> None:
         search_topk(cfg)
 
     if cfg.tasks.eval.get("merge_search", False):
-        raise NotImplementedError("multi-domain merge is CPU text post-processing outside the hot path")
+        logging.info("\n\n************** Post Merging Searched Results from Multiple Domains ***********")
+        from retrieval_scaling_b200.search import post_hoc_merge_topk_multi_domain
+        post_hoc_merge_topk_multi_domain(cfg)
     if cfg.tasks.eval.get("inference", False):
         raise NotImplementedError("reader-LM perplexity evaluation is downstream of retrieval (out of scope)")
 
