@@ -452,6 +452,32 @@ enum { RSB_GEMM_REVERSED = 256 };
 int rsb_gemm_f16(const void* A_dev, const void* W_dev, const void* bias_dev, const void* residual_dev, void* C_dev,
                  int M, int N, int K, int epilogue, rsb_stream_t stream);
 
+/* ---- reader LM for perplexity evaluation: HF LlamaForCausalLM, prefill only, fp16 ----------------------------------
+ * Replaces the reader of the reference's perplexity loop (src/evaluate_perplexity.py:98-108 loads it, :126-134 runs
+ * `lm(input_ids, labels=labels)` one window at a time).  Errors of these entries are reported by rsb_llm_last_error().
+ * rsb_llm_create: head_dim 128 (hidden == 128 * heads), heads % kv_heads == 0, intermediate % 128 == 0, SiLU MLP, no
+ * biases, default RoPE (inv_freq = 1 / rope_theta ** (2i / 128) in fp32); anything else RSB_ERR_UNSUPPORTED, non-positive
+ * sizes RSB_ERR_INVALID, both before any CUDA call.  Any vocabulary size: the LM head is padded to a multiple of 128
+ * rows that never enter the log-sum-exp.  tied = 1 (tie_word_embeddings): the LM head is model.embed_tokens.weight. */
+typedef struct rsb_llm rsb_llm_t;
+const char* rsb_llm_last_error(void);
+int rsb_llm_create(int layers, int hidden, int heads, int kv_heads, int intermediate, int vocab, int max_pos,
+                   float rope_theta, float rms_eps, int tied, rsb_llm_t** out);
+/* name = HF LlamaForCausalLM state_dict key: "model.embed_tokens.weight", "model.norm.weight", "lm_head.weight"
+ * (untied; accepted and ignored when tied) and "model.layers.N.{self_attn.{q,k,v,o}_proj, mlp.{gate,up,down}_proj,
+ * input_layernorm, post_attention_layernorm}.weight"; data fp16 on the device, copied. */
+int rsb_llm_load(rsb_llm_t* h, const char* name, const void* f16_dev, int64_t n_elements, rsb_stream_t stream);
+size_t rsb_llm_workspace_bytes(rsb_llm_t* h, int total_tokens, int label_tokens);
+/* B packed sequences: ids_dev / labels_dev [T] int32 (label -100 = ignored), cu_seqlens_dev [B+1] int32 (0 .. T), every
+ * sequence <= max_seqlen <= max_pos tokens (RSB_ERR_UNSUPPORTED past max_pos).  Positions restart at 0 in every
+ * sequence.  nll_out_dev [T] fp32: at position t that is not the first of its sequence and whose label is not -100,
+ * logsumexp(logits of t - 1) - logit[labels[t]] (HF's shifted causal-LM loss per token), 0 elsewhere.  label_tokens of
+ * rsb_llm_workspace_bytes counts those positions.  Ids outside [0, vocab), labels that are neither -100 nor an id and
+ * malformed offsets are RSB_ERR_INVALID before any launch; RSB_ERR_STATE until every weight is loaded. */
+int rsb_llm_nll(rsb_llm_t* h, const int32_t* ids_dev, const int32_t* cu_seqlens_dev, int B, int T, int max_seqlen,
+                const int32_t* labels_dev, float* nll_out_dev, void* ws_dev, size_t ws_bytes, rsb_stream_t stream);
+int rsb_llm_free(rsb_llm_t* h);
+
 /* ---- MinHash de-duplication of retrieved passages ----------------------------------------------------------------
  * Replaces utils/deduplication.py's `remove_duplicates_with_minhash` (datasketch MinHash(num_perm=128) and
  * MinHashLSH(threshold=0.8)) run by src/search.py:471-479 on the merged multi-source results.  Errors of these entries

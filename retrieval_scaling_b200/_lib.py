@@ -90,6 +90,12 @@ SIGNATURES = [
     ("rsb_bert_launches", c_int64, [_H]),
     ("rsb_bert_attention", c_int, [_H, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),   # diagnostic
     ("rsb_gemm_f16", c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    ("rsb_llm_last_error", c_char_p, []),
+    ("rsb_llm_create", c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_int, POINTER(_H)]),
+    ("rsb_llm_load", c_int, [_H, c_char_p, c_void_p, c_int64, c_void_p]),
+    ("rsb_llm_workspace_bytes", c_size_t, [_H, c_int, c_int]),
+    ("rsb_llm_nll", c_int, [_H, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    ("rsb_llm_free", c_int, [_H]),
     ("rsb_dedup_last_error", c_char_p, []),
     ("rsb_minhash_workspace_bytes", c_size_t, [c_int64]),
     ("rsb_minhash_signatures", c_int, [c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,

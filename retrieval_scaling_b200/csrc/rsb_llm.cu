@@ -1,0 +1,605 @@
+// rsb_llm.cu -- reader-LM forward for perplexity evaluation: HF LlamaForCausalLM (Llama-2 MHA, Llama-3 GQA) in fp16,
+// prefill only, over packed un-padded sequences, ending in the per-token negative log-likelihood of the labels.
+// Replaces the reader call of the reference's perplexity loop (src/evaluate_perplexity.py:126-134: `lm(input_ids,
+// labels=labels)` one window at a time, HF in bf16).  No KV cache, no generation.
+//
+//   embed_rows_kernel        X[t] = embed_tokens[ids[t]]
+//   rms_rows_kernel          LlamaRMSNorm in HF's order: fp32 x * rsqrt(mean(x^2) + eps), rounded to half, times the half
+//                            weight; the final norm runs on the gathered label rows only
+//   rsb_gemm_f16             every linear layer on the encoder's TMA + wgmma kernel (gemm_tn_kernel, rsb_bert.cu): fused
+//                            q|k|v and gate|up weights, residual adds through its residual epilogue with a zero bias
+//   rope_kernel              HF rotate_half RoPE on the Q and K heads of the fused QKV rows; positions restart at 0 in
+//                            every packed sequence
+//   attention_causal_kernel  causal flash attention, head_dim 128, GQA, mma.sync.m16n8k16 with fp32 running max / sum;
+//                            key blocks above the diagonal are never visited
+//   swiglu_kernel            act = fp16(fp16(silu(gate)) * up), HF LlamaMLP's order
+//   nll_rows_kernel          fp32 logsumexp over the real vocabulary (pad rows of the LM head excluded) - logit[label]
+#include "../../include/rsb.h"
+
+#include "rsb_internal.h"
+
+#include <cuda_fp16.h>
+
+#include <algorithm>
+#include <cmath>
+#include <cstdarg>
+#include <cstdio>
+#include <set>
+#include <string>
+#include <vector>
+
+namespace {
+
+constexpr int HD = 128;                      // head_dim of every supported reader
+constexpr int AQ = 64, AK = 64, APAD = HD + 8;   // attention: 64 queries per block (16 per warp), key blocks of 64
+constexpr size_t LOGIT_BYTES = 256u << 20;   // bound of the logits workspace of one LM-head chunk
+
+__device__ __forceinline__ float block_sum(float v, float* red) {
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+    __syncthreads();
+    if (lane == 0) red[warp] = v;
+    __syncthreads();
+    float s = 0.f;
+    for (int i = 0; i < nw; ++i) s += red[i];
+    return s;
+}
+
+// one block per token; hidden % 8 == 0
+__global__ void embed_rows_kernel(const int* __restrict__ ids, const __half* __restrict__ embed, int hidden,
+                                  __half* __restrict__ X) {
+    const int t = blockIdx.x;
+    const uint4* src = reinterpret_cast<const uint4*>(embed + (size_t)ids[t] * hidden);
+    uint4* dst = reinterpret_cast<uint4*>(X + (size_t)t * hidden);
+    for (int i = threadIdx.x; i < hidden / 8; i += blockDim.x) dst[i] = src[i];
+}
+
+// LlamaRMSNorm (modeling_llama.py): h = x.float(); h *= rsqrt(mean(h^2) + eps); weight * h.half().  One block per
+// output row i, input row rows ? rows[i] : i.
+__global__ __launch_bounds__(256)
+void rms_rows_kernel(const __half* __restrict__ in, const int* __restrict__ rows, int hidden,
+                     const __half* __restrict__ w, float eps, __half* __restrict__ out) {
+    __shared__ float red[8];
+    const int i = blockIdx.x;
+    const int r = rows ? rows[i] : i;
+    const uint4* x = reinterpret_cast<const uint4*>(in + (size_t)r * hidden);
+    float s = 0.f;
+    for (int c = threadIdx.x; c < hidden / 8; c += blockDim.x) {
+        const uint4 v = x[c];
+        const __half2* h2 = reinterpret_cast<const __half2*>(&v);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const float2 f = __half22float2(h2[e]);
+            s = fmaf(f.x, f.x, s);
+            s = fmaf(f.y, f.y, s);
+        }
+    }
+    const float rstd = rsqrtf(block_sum(s, red) / (float)hidden + eps);
+    const uint4* wv = reinterpret_cast<const uint4*>(w);
+    uint4* o = reinterpret_cast<uint4*>(out + (size_t)i * hidden);
+    for (int c = threadIdx.x; c < hidden / 8; c += blockDim.x) {
+        const uint4 v = x[c], g = wv[c];
+        const __half2* h2 = reinterpret_cast<const __half2*>(&v);
+        const __half2* g2 = reinterpret_cast<const __half2*>(&g);
+        uint4 ov;
+        __half2* o2 = reinterpret_cast<__half2*>(&ov);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const float2 f = __half22float2(h2[e]);
+            o2[e] = __hmul2(g2[e], __floats2half2_rn(f.x * rstd, f.y * rstd));
+        }
+        o[c] = ov;
+    }
+}
+
+// HF apply_rotary_pos_emb on the Q heads and K heads (contiguous at the start of each QKV row, ld halves apart):
+// x_embed = x * cos + rotate_half(x) * sin in fp16, cos / sin = fp16(cos / sin(fp32(inv_freq[i] * pos))).  Each fp16
+// product and sum is one fp32 operation rounded to half, as torch computes half tensors.  One block per token.
+__global__ void rope_kernel(__half* __restrict__ qkv, const int* __restrict__ cu_seqlens, int B, int ld, int rot_heads,
+                            const float* __restrict__ inv_freq) {
+    const int t = blockIdx.x;
+    int lo = 0, hi = B;                          // sequence b with cu[b] <= t < cu[b+1]
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (cu_seqlens[mid] <= t) lo = mid; else hi = mid;
+    }
+    const float pos = (float)(t - cu_seqlens[lo]);
+    __half* row = qkv + (size_t)t * ld;
+    for (int p = threadIdx.x; p < rot_heads * (HD / 2); p += blockDim.x) {
+        const int i = p % (HD / 2);
+        __half* x = row + (p / (HD / 2)) * HD;
+        const float f = inv_freq[i] * pos;
+        const float c = __half2float(__float2half_rn(cosf(f))), s = __half2float(__float2half_rn(sinf(f)));
+        const float x1 = __half2float(x[i]), x2 = __half2float(x[i + HD / 2]);
+        const float a1 = __half2float(__float2half_rn(x1 * c)), b1 = __half2float(__float2half_rn(-x2 * s));
+        const float a2 = __half2float(__float2half_rn(x2 * c)), b2 = __half2float(__float2half_rn(x1 * s));
+        x[i] = __float2half_rn(a1 + b1);
+        x[i + HD / 2] = __float2half_rn(a2 + b2);
+    }
+}
+
+__device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+}
+__device__ __forceinline__ uint32_t half2_bits(float lo, float hi) {
+    const __half2 h = __floats2half2_rn(lo, hi);
+    return *reinterpret_cast<const uint32_t*>(&h);
+}
+__device__ __forceinline__ uint32_t ld32(const __half* p) { return *reinterpret_cast<const uint32_t*>(p); }
+
+// Causal attention of one (sequence, query block of 64, head): blockIdx.x = item (b, qb) from the host's list, heaviest
+// query blocks first; blockIdx.y = query head h, which reads KV head h / (heads / kv_heads).  4 warps, 16 query rows each
+// with their Q fragments in registers; key blocks 0..qb (every later one is fully masked) are staged in shared memory
+// by the whole block.  S = Q K^T and O += P V on mma.sync.m16n8k16 with fp32 accumulators; online softmax in the log2
+// domain with fp32 running maximum and sum, P rounded to half for the P V product.  Inside the diagonal block a warp
+// skips the key tiles of 8 that lie entirely above its last row.
+__global__ __launch_bounds__(128)
+void attention_causal_kernel(const __half* __restrict__ qkv, const int* __restrict__ cu_seqlens,
+                             const int2* __restrict__ items, __half* __restrict__ ctx, int heads, int kv_heads,
+                             float scale_log2) {
+    __shared__ __align__(16) __half Ks[AK][APAD];
+    __shared__ __align__(16) __half Vs[AK][APAD];
+    const int2 it = items[blockIdx.x];
+    const int b = it.x, qb = it.y, h = blockIdx.y, kvh = h / (heads / kv_heads);
+    const int hid = heads * HD, ld = hid + 2 * kv_heads * HD;
+    const int t0 = cu_seqlens[b], S = cu_seqlens[b + 1] - t0;
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
+    const int qw = qb * AQ + wib * 16;           // first query row of this warp
+    const bool active = qw < S;                  // warp-uniform; idle warps still stage K / V and meet the barriers
+    const __half* qbase = qkv + (size_t)t0 * ld + h * HD;
+    const __half* kbase = qkv + (size_t)t0 * ld + hid + kvh * HD;
+    const __half* vbase = kbase + kv_heads * HD;
+    const int r0 = qw + g, r1 = r0 + 8;
+
+    uint32_t qa[8][4];
+#pragma unroll
+    for (int ks = 0; ks < 8; ++ks) {
+        const int c = ks * 16 + 2 * t;
+        qa[ks][0] = r0 < S ? ld32(qbase + (size_t)r0 * ld + c) : 0u;
+        qa[ks][1] = r1 < S ? ld32(qbase + (size_t)r1 * ld + c) : 0u;
+        qa[ks][2] = r0 < S ? ld32(qbase + (size_t)r0 * ld + c + 8) : 0u;
+        qa[ks][3] = r1 < S ? ld32(qbase + (size_t)r1 * ld + c + 8) : 0u;
+    }
+    float o[16][4];
+#pragma unroll
+    for (int nt = 0; nt < 16; ++nt)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) o[nt][e] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};   // l_run: per-lane partial sums
+
+    for (int kb = 0; kb <= qb; ++kb) {
+        __syncthreads();                         // the previous key block has been consumed by every warp
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {            // 64 rows x 16 uint4 of K and of V
+            const int idx = threadIdx.x + 128 * i, j = idx >> 4, c = idx & 15;
+            const int key = kb * AK + j;
+            uint4 kv = make_uint4(0, 0, 0, 0), vv = kv;
+            if (key < S) {
+                kv = *reinterpret_cast<const uint4*>(kbase + (size_t)key * ld + c * 8);
+                vv = *reinterpret_cast<const uint4*>(vbase + (size_t)key * ld + c * 8);
+            }
+            *reinterpret_cast<uint4*>(&Ks[j][c * 8]) = kv;
+            *reinterpret_cast<uint4*>(&Vs[j][c * 8]) = vv;
+        }
+        __syncthreads();
+        if (!active) continue;
+        // key tiles of 8 holding at least one key <= this warp's last row (all 8 below the diagonal block)
+        const int nvt = kb < qb ? 8 : min(8, (qw + 15 - kb * AK) / 8 + 1);
+        float sacc[8][4];
+#pragma unroll
+        for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) sacc[nt][e] = 0.f;
+#pragma unroll
+        for (int ks = 0; ks < 8; ++ks)
+#pragma unroll
+            for (int nt = 0; nt < 8; ++nt) {
+                if (nt < nvt) {
+                    const int j = nt * 8 + g, c = ks * 16 + 2 * t;
+                    const uint32_t kf[2] = {ld32(&Ks[j][c]), ld32(&Ks[j][c + 8])};
+                    mma16816(sacc[nt], qa[ks], kf);
+                }
+            }
+        float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+        for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const int key = kb * AK + nt * 8 + 2 * t + (e & 1), row = (e < 2) ? r0 : r1;
+                const float sv = (nt < nvt && key <= row && key < S) ? sacc[nt][e] * scale_log2 : -INFINITY;
+                sacc[nt][e] = sv;
+                mx[e >> 1] = fmaxf(mx[e >> 1], sv);
+            }
+        float corr[2], mref[2];
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+            mx[hr] = fmaxf(mx[hr], __shfl_xor_sync(0xffffffffu, mx[hr], 1));
+            mx[hr] = fmaxf(mx[hr], __shfl_xor_sync(0xffffffffu, mx[hr], 2));
+            const float mn = fmaxf(m_run[hr], mx[hr]);
+            mref[hr] = mn == -INFINITY ? 0.f : mn;   // a row without any valid key so far keeps probability 0
+            corr[hr] = exp2f(m_run[hr] - mref[hr]);
+            m_run[hr] = mn;
+        }
+        float sum[2] = {0.f, 0.f};
+#pragma unroll
+        for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const float p = exp2f(sacc[nt][e] - mref[e >> 1]);   // 2^-inf = 0
+                sacc[nt][e] = p;
+                sum[e >> 1] += p;
+            }
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) l_run[hr] = l_run[hr] * corr[hr] + sum[hr];
+#pragma unroll
+        for (int nt = 0; nt < 16; ++nt) {
+            o[nt][0] *= corr[0]; o[nt][1] *= corr[0];
+            o[nt][2] *= corr[1]; o[nt][3] *= corr[1];
+        }
+        uint32_t pa[4][4];
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+            pa[kk][0] = half2_bits(sacc[2 * kk][0], sacc[2 * kk][1]);
+            pa[kk][1] = half2_bits(sacc[2 * kk][2], sacc[2 * kk][3]);
+            pa[kk][2] = half2_bits(sacc[2 * kk + 1][0], sacc[2 * kk + 1][1]);
+            pa[kk][3] = half2_bits(sacc[2 * kk + 1][2], sacc[2 * kk + 1][3]);
+        }
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+            if (kk * 2 < nvt) {                  // a 16-key step whose keys are all masked adds nothing
+#pragma unroll
+                for (int nt = 0; nt < 16; ++nt) {
+                    uint32_t vb[2];
+                    const uint32_t addr = (uint32_t)__cvta_generic_to_shared(&Vs[kk * 16 + (lane & 15)][nt * 8]);
+                    asm volatile("ldmatrix.sync.aligned.m8n8.x2.trans.shared.b16 {%0,%1}, [%2];"
+                                 : "=r"(vb[0]), "=r"(vb[1]) : "r"(addr));
+                    mma16816(o[nt], pa[kk], vb);
+                }
+            }
+        }
+    }
+    if (!active) return;
+    float inv[2];
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+        float l = l_run[hr];
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        inv[hr] = l > 0.f ? 1.f / l : 0.f;
+    }
+#pragma unroll
+    for (int nt = 0; nt < 16; ++nt) {
+        const int col = h * HD + nt * 8 + 2 * t;
+        if (r0 < S) *reinterpret_cast<__half2*>(ctx + (size_t)(t0 + r0) * hid + col) = __floats2half2_rn(o[nt][0] * inv[0], o[nt][1] * inv[0]);
+        if (r1 < S) *reinterpret_cast<__half2*>(ctx + (size_t)(t0 + r1) * hid + col) = __floats2half2_rn(o[nt][2] * inv[1], o[nt][3] * inv[1]);
+    }
+}
+
+// act[t, j] = fp16(fp16(silu(gate[t, j])) * up[t, j]) with gu = [gate | up] rows of 2 * inter; silu as torch computes it
+// on half, x / (1 + exp(-x)) in fp32 rounded to half.  8 elements per thread.
+__global__ void swiglu_kernel(const __half* __restrict__ gu, long long n8, int inter, __half* __restrict__ act) {
+    const int per_row = inter / 8;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n8; i += (long long)gridDim.x * blockDim.x) {
+        const long long t = i / per_row;
+        const int c = (int)(i % per_row) * 8;
+        const uint4 gv = *reinterpret_cast<const uint4*>(gu + t * 2 * inter + c);
+        const uint4 uv = *reinterpret_cast<const uint4*>(gu + t * 2 * inter + inter + c);
+        const __half2* g2 = reinterpret_cast<const __half2*>(&gv);
+        const __half2* u2 = reinterpret_cast<const __half2*>(&uv);
+        uint4 ov;
+        __half2* o2 = reinterpret_cast<__half2*>(&ov);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const float2 x = __half22float2(g2[e]);
+            const __half2 s = __floats2half2_rn(__fdiv_rn(x.x, 1.f + expf(-x.x)), __fdiv_rn(x.y, 1.f + expf(-x.y)));
+            const float2 sf = __half22float2(s), uf = __half22float2(u2[e]);
+            o2[e] = __floats2half2_rn(sf.x * uf.x, sf.y * uf.y);
+        }
+        *reinterpret_cast<uint4*>(act + t * inter + c) = ov;
+    }
+}
+
+__device__ __forceinline__ void lse_merge(float& m, float& s, float m2, float s2) {
+    const float mn = fmaxf(m, m2);
+    if (mn == -INFINITY) return;
+    s = s * expf(m - mn) + s2 * expf(m2 - mn);
+    m = mn;
+}
+
+// nll_out[out_idx[i]] = logsumexp(logits[i, 0:vocab]) - logits[i, label[i]] in fp32; columns vocab..ld-1 are the LM
+// head's pad rows and never enter the sum.  One block per row, one pass with a running (max, sum) per thread.
+__global__ __launch_bounds__(256)
+void nll_rows_kernel(const __half* __restrict__ logits, int vocab, int ld, const int* __restrict__ labels,
+                     const int* __restrict__ out_idx, float* __restrict__ nll_out) {
+    __shared__ float rm[8], rs[8];
+    const int i = blockIdx.x;
+    const __half* row = logits + (size_t)i * ld;
+    float m = -INFINITY, s = 0.f;
+    for (int c = threadIdx.x * 8; c < vocab; c += blockDim.x * 8) {
+        const uint4 v = *reinterpret_cast<const uint4*>(row + c);
+        const __half* hv = reinterpret_cast<const __half*>(&v);
+        float x[8], mx = -INFINITY;
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+            x[e] = c + e < vocab ? __half2float(hv[e]) : -INFINITY;
+            mx = fmaxf(mx, x[e]);
+        }
+        const float mn = fmaxf(m, mx);
+        float acc = s * expf(m - mn);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) acc += expf(x[e] - mn);
+        m = mn;
+        s = acc;
+    }
+    for (int off = 16; off > 0; off >>= 1)
+        lse_merge(m, s, __shfl_xor_sync(0xffffffffu, m, off), __shfl_xor_sync(0xffffffffu, s, off));
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (lane == 0) { rm[warp] = m; rs[warp] = s; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float M = rm[0], Sm = rs[0];
+        for (int w = 1; w < (int)(blockDim.x >> 5); ++w) lse_merge(M, Sm, rm[w], rs[w]);
+        nll_out[out_idx[i]] = (M + logf(Sm)) - __half2float(row[labels[i]]);
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// host side
+// ---------------------------------------------------------------------------------------------------------
+thread_local std::string g_lerr;
+int lfail(int code, const char* fmt, ...) {
+    char buf[512];
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(buf, sizeof buf, fmt, ap);
+    va_end(ap);
+    g_lerr = buf;
+    return code;
+}
+
+struct LlmLayer {
+    __half *wqkv = nullptr, *wo = nullptr, *wgu = nullptr, *wdown = nullptr, *ln1 = nullptr, *ln2 = nullptr;
+};
+
+}  // namespace
+
+struct rsb_llm {
+    int layers = 0, hidden = 0, heads = 0, kv_heads = 0, inter = 0, vocab = 0, vocab_pad = 0, max_pos = 0;
+    float rope_theta = 0.f, eps = 0.f;
+    bool tied = false;
+    __half *embed = nullptr, *lm_head = nullptr, *final_g = nullptr, *zero_bias = nullptr;
+    float* inv_freq = nullptr;
+    std::vector<LlmLayer> L;
+    std::set<std::string> loaded;                // required weights loaded so far
+    int qkv_n() const { return (heads + 2 * kv_heads) * HD; }
+    size_t required() const { return 2 + 9 * (size_t)layers + (tied ? 0 : 1); }
+    int chunk_rows() const { return (int)std::max<size_t>(128, LOGIT_BYTES / ((size_t)vocab_pad * 2) / 128 * 128); }
+};
+
+namespace {
+
+int gemm(const __half* A, int M, const __half* W, int N, int K, const __half* bias, const __half* residual, __half* C,
+         int epi, cudaStream_t st) {
+    const int rc = rsb_gemm_f16(A, W, bias, residual, C, M, N, K, epi, st);
+    return rc == RSB_OK ? RSB_OK : lfail(rc, "linear layer (%s)", rsb_bert_last_error());
+}
+
+// workspace: X, normed rows, QKV, attention output, gate|up, SwiGLU output, one chunk of logits, the label tables and
+// the attention work list.  Label tables: logit row, label and output index per scored token.
+size_t llm_ws_layout(const rsb_llm* h, size_t T, size_t nl, size_t off[10]) {
+    auto al = [](size_t x) { return (x + 1023) / 1024 * 1024; };
+    const size_t chunk = std::min<size_t>(std::max<size_t>(nl, 1), (size_t)h->chunk_rows());
+    size_t o = 0;
+    off[0] = o; o += al(T * h->hidden * 2);                 // X (residual stream)
+    off[1] = o; o += al(T * h->hidden * 2);                 // normed rows
+    off[2] = o; o += al(T * (size_t)h->qkv_n() * 2);        // QKV
+    off[3] = o; o += al(T * h->hidden * 2);                 // attention output
+    off[4] = o; o += al(T * 2 * (size_t)h->inter * 2);      // gate | up
+    off[5] = o; o += al(T * (size_t)h->inter * 2);          // SwiGLU output
+    off[6] = o; o += al(chunk * (size_t)h->vocab_pad * 2);  // logits of one chunk of label rows
+    off[7] = o; o += al(3 * std::max<size_t>(nl, 1) * sizeof(int));   // rows | labels | out_idx
+    off[8] = o; o += al(T * sizeof(int2));                  // attention items (b, query block)
+    off[9] = o;
+    return o;
+}
+
+}  // namespace
+
+extern "C" const char* rsb_llm_last_error(void) { return g_lerr.c_str(); }
+
+// Replaces `AutoModelForCausalLM.from_pretrained(cfg.model.lm_model, torch_dtype=torch.bfloat16)` for Llama readers
+// (src/evaluate_perplexity.py:98-108).  Every refusal comes before any CUDA call.
+extern "C" int rsb_llm_create(int layers, int hidden, int heads, int kv_heads, int intermediate, int vocab, int max_pos,
+                              float rope_theta, float rms_eps, int tied, rsb_llm_t** out) {
+    if (!out) return lfail(RSB_ERR_INVALID, "out is NULL");
+    *out = nullptr;
+    if (layers <= 0 || vocab <= 0 || max_pos <= 0 || !(rope_theta > 0.f) || !(rms_eps > 0.f) || (tied != 0 && tied != 1))
+        return lfail(RSB_ERR_INVALID, "layers, vocab, max_pos, rope_theta and rms_eps must be positive, tied 0 or 1");
+    if (heads <= 0 || hidden != heads * HD)
+        return lfail(RSB_ERR_UNSUPPORTED, "only head_dim 128 is implemented (hidden %ld != 128 x heads)", (long)hidden);
+    if (kv_heads <= 0 || heads % kv_heads)
+        return lfail(RSB_ERR_UNSUPPORTED, "num_attention_heads must be a multiple of num_key_value_heads (got %ld kv heads)", (long)kv_heads);
+    if (intermediate <= 0 || intermediate % 128)
+        return lfail(RSB_ERR_UNSUPPORTED, "intermediate_size %ld is not a multiple of 128", (long)intermediate);
+    rsb_llm* h = new rsb_llm();
+    h->layers = layers; h->hidden = hidden; h->heads = heads; h->kv_heads = kv_heads; h->inter = intermediate;
+    h->vocab = vocab; h->vocab_pad = (vocab + 127) / 128 * 128; h->max_pos = max_pos;
+    h->rope_theta = rope_theta; h->eps = rms_eps; h->tied = tied != 0;
+    const size_t H = hidden, V = h->vocab_pad;
+    const size_t zb = std::max({(size_t)h->qkv_n(), 2 * (size_t)intermediate, V, H});
+    bool ok = true;
+    ok &= cudaMalloc(&h->embed, (size_t)vocab * H * 2) == cudaSuccess;
+    ok &= cudaMalloc(&h->lm_head, V * H * 2) == cudaSuccess;
+    ok &= cudaMalloc(&h->final_g, H * 2) == cudaSuccess;
+    ok &= cudaMalloc(&h->zero_bias, zb * 2) == cudaSuccess;
+    ok &= cudaMalloc(&h->inv_freq, HD / 2 * sizeof(float)) == cudaSuccess;
+    h->L.resize(layers);
+    for (auto& l : h->L) {
+        ok &= cudaMalloc(&l.wqkv, (size_t)h->qkv_n() * H * 2) == cudaSuccess;
+        ok &= cudaMalloc(&l.wo, H * H * 2) == cudaSuccess;
+        ok &= cudaMalloc(&l.wgu, 2 * (size_t)intermediate * H * 2) == cudaSuccess;
+        ok &= cudaMalloc(&l.wdown, (size_t)intermediate * H * 2) == cudaSuccess;
+        ok &= cudaMalloc(&l.ln1, H * 2) == cudaSuccess;
+        ok &= cudaMalloc(&l.ln2, H * 2) == cudaSuccess;
+    }
+    if (!ok) { rsb_llm_free(h); return lfail(RSB_ERR_OOM, "allocating reader weights failed"); }
+    // LlamaRotaryEmbedding: inv_freq = 1 / theta ** (arange(0, 128, 2).float() / 128), in fp32
+    float inv[HD / 2];
+    for (int i = 0; i < HD / 2; ++i) inv[i] = 1.f / powf(rope_theta, (float)(2 * i) / (float)HD);
+    ok &= cudaMemcpy(h->inv_freq, inv, sizeof inv, cudaMemcpyHostToDevice) == cudaSuccess;
+    ok &= cudaMemset(h->zero_bias, 0, zb * 2) == cudaSuccess;
+    ok &= cudaMemset(h->lm_head, 0, V * H * 2) == cudaSuccess;   // pad rows stay zero (and outside the sum)
+    if (!ok) { rsb_llm_free(h); return lfail(RSB_ERR_CUDA, "initialising the reader failed"); }
+    *out = h;
+    return RSB_OK;
+}
+
+extern "C" int rsb_llm_free(rsb_llm_t* h) {
+    if (!h) return RSB_OK;
+    cudaFree(h->embed); cudaFree(h->lm_head); cudaFree(h->final_g); cudaFree(h->zero_bias); cudaFree(h->inv_freq);
+    for (auto& l : h->L) {
+        cudaFree(l.wqkv); cudaFree(l.wo); cudaFree(l.wgu); cudaFree(l.wdown); cudaFree(l.ln1); cudaFree(l.ln2);
+    }
+    delete h;
+    return RSB_OK;
+}
+
+// name = HF LlamaForCausalLM state_dict key, data fp16 on the device, copied (src/evaluate_perplexity.py:98-108 loads
+// the same checkpoint).  q|k|v and gate|up land in one fused weight each.
+extern "C" int rsb_llm_load(rsb_llm_t* h, const char* name, const void* f16_dev, int64_t n, rsb_stream_t stream) {
+    if (!h || !name || !f16_dev) return lfail(RSB_ERR_INVALID, "null argument");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int64_t H = h->hidden, KV = (int64_t)h->kv_heads * HD, I = h->inter;
+    const std::string s(name);
+    auto put = [&](__half* dst, int64_t expect) -> int {
+        if (n != expect) return lfail(RSB_ERR_INVALID, "weight %s has the wrong size (%ld elements)", name, (long)n);
+        if (cudaMemcpyAsync(dst, f16_dev, (size_t)n * 2, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
+            return lfail(RSB_ERR_CUDA, "copy of %s failed", name);
+        if (!(h->tied && s == "lm_head.weight")) h->loaded.insert(s);
+        return RSB_OK;
+    };
+    if (s == "model.embed_tokens.weight") {
+        const int rc = put(h->embed, (int64_t)h->vocab * H);
+        if (rc != RSB_OK || !h->tied) return rc;
+        return put(h->lm_head, (int64_t)h->vocab * H);
+    }
+    if (s == "lm_head.weight") return put(h->lm_head, (int64_t)h->vocab * H);
+    if (s == "model.norm.weight") return put(h->final_g, H);
+    int li = -1;
+    char rest[128] = {0};
+    if (sscanf(name, "model.layers.%d.%127s", &li, rest) == 2 && li >= 0 && li < h->layers) {
+        LlmLayer& l = h->L[li];
+        const std::string r(rest);
+        if (r == "self_attn.q_proj.weight") return put(l.wqkv, H * H);
+        if (r == "self_attn.k_proj.weight") return put(l.wqkv + H * H, KV * H);
+        if (r == "self_attn.v_proj.weight") return put(l.wqkv + (H + KV) * H, KV * H);
+        if (r == "self_attn.o_proj.weight") return put(l.wo, H * H);
+        if (r == "mlp.gate_proj.weight") return put(l.wgu, I * H);
+        if (r == "mlp.up_proj.weight") return put(l.wgu + I * H, I * H);
+        if (r == "mlp.down_proj.weight") return put(l.wdown, I * H);
+        if (r == "input_layernorm.weight") return put(l.ln1, H);
+        if (r == "post_attention_layernorm.weight") return put(l.ln2, H);
+    }
+    return lfail(RSB_ERR_INVALID, "unknown weight name %s", name);
+}
+
+extern "C" size_t rsb_llm_workspace_bytes(rsb_llm_t* h, int total_tokens, int label_tokens) {
+    if (!h || total_tokens < 0 || label_tokens < 0) return 0;
+    size_t off[10];
+    return llm_ws_layout(h, (size_t)std::max(total_tokens, 1), (size_t)label_tokens, off);
+}
+
+// The reader forward and loss of src/evaluate_perplexity.py:126-134 (`lm(input_ids, labels=labels)` per window) over B
+// packed windows.  ids / labels [T] int32 and cu_seqlens [B+1] int32 on the device; nll_out [T] fp32 receives, at
+// every position t that is not the first of its sequence and whose label is not -100, -log p(labels[t] | ids of the
+// sequence before t), and 0 elsewhere.  The ids, labels and offsets are read back and checked before any launch.
+extern "C" int rsb_llm_nll(rsb_llm_t* h, const int32_t* ids, const int32_t* cu_seqlens, int B, int T, int max_seqlen,
+                           const int32_t* labels, float* nll_out, void* ws, size_t ws_bytes, rsb_stream_t stream) {
+    if (!h || !ids || !cu_seqlens || !labels || !nll_out || !ws) return lfail(RSB_ERR_INVALID, "null argument");
+    if (B <= 0 || T <= 0) return lfail(RSB_ERR_INVALID, "empty batch");
+    if (max_seqlen > h->max_pos)
+        return lfail(RSB_ERR_UNSUPPORTED, "sequence longer than max_position_embeddings (%ld)", (long)h->max_pos);
+    if (h->loaded.size() != h->required())
+        return lfail(RSB_ERR_STATE, "%ld reader weights are not loaded", (long)(h->required() - h->loaded.size()));
+    cudaStream_t st = (cudaStream_t)stream;
+    std::vector<int32_t> cu(B + 1), hid(T), lab(T);
+    if (cudaMemcpyAsync(cu.data(), cu_seqlens, cu.size() * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+        cudaMemcpyAsync(hid.data(), ids, (size_t)T * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+        cudaMemcpyAsync(lab.data(), labels, (size_t)T * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+        cudaStreamSynchronize(st) != cudaSuccess)
+        return lfail(RSB_ERR_CUDA, "reading back the batch failed");
+    if (cu[0] != 0 || cu[B] != T) return lfail(RSB_ERR_INVALID, "cu_seqlens must run from 0 to T (T = %ld)", (long)T);
+    std::vector<int32_t> rows, labs, outi;
+    std::vector<int2> items;
+    for (int b = 0; b < B; ++b) {
+        const int S = cu[b + 1] - cu[b];
+        if (S < 0) return lfail(RSB_ERR_INVALID, "cu_seqlens decreases at sequence %ld", (long)b);
+        if (S > max_seqlen) return lfail(RSB_ERR_INVALID, "a sequence of %ld tokens is longer than max_seqlen", (long)S);
+        for (int q = 0; q * AQ < S; ++q) items.push_back(make_int2(b, q));
+        for (int t = cu[b] + 1; t < cu[b + 1]; ++t)
+            if (lab[t] != -100) { rows.push_back(t - 1); labs.push_back(lab[t]); outi.push_back(t); }
+    }
+    for (int t = 0; t < T; ++t) {
+        if (hid[t] < 0 || hid[t] >= h->vocab) return lfail(RSB_ERR_INVALID, "token id %ld is outside the vocabulary", (long)hid[t]);
+        if (lab[t] != -100 && (lab[t] < 0 || lab[t] >= h->vocab))
+            return lfail(RSB_ERR_INVALID, "label %ld is neither -100 nor a token id", (long)lab[t]);
+    }
+    // heaviest query blocks first: block q of a sequence visits q + 1 key blocks
+    std::stable_sort(items.begin(), items.end(), [](const int2& a, const int2& b) { return a.y > b.y; });
+    const int nl = (int)rows.size();
+    size_t off[10];
+    const size_t need = llm_ws_layout(h, (size_t)T, (size_t)nl, off);
+    if (ws_bytes < need) return lfail(RSB_ERR_OOM, "reader workspace too small (need %ld bytes)", (long)need);
+    unsigned char* w = static_cast<unsigned char*>(ws);
+    __half* X = reinterpret_cast<__half*>(w + off[0]);
+    __half* Hn = reinterpret_cast<__half*>(w + off[1]);
+    __half* QKV = reinterpret_cast<__half*>(w + off[2]);
+    __half* CTX = reinterpret_cast<__half*>(w + off[3]);
+    __half* GU = reinterpret_cast<__half*>(w + off[4]);
+    __half* ACT = reinterpret_cast<__half*>(w + off[5]);
+    __half* LOG = reinterpret_cast<__half*>(w + off[6]);
+    int* d_rows = reinterpret_cast<int*>(w + off[7]);
+    int* d_labs = d_rows + nl;
+    int* d_outi = d_labs + nl;
+    int2* d_items = reinterpret_cast<int2*>(w + off[8]);
+    if (nl > 0 && (cudaMemcpyAsync(d_rows, rows.data(), (size_t)nl * 4, cudaMemcpyHostToDevice, st) != cudaSuccess ||
+                   cudaMemcpyAsync(d_labs, labs.data(), (size_t)nl * 4, cudaMemcpyHostToDevice, st) != cudaSuccess ||
+                   cudaMemcpyAsync(d_outi, outi.data(), (size_t)nl * 4, cudaMemcpyHostToDevice, st) != cudaSuccess))
+        return lfail(RSB_ERR_CUDA, "uploading the label rows failed");
+    if (cudaMemcpyAsync(d_items, items.data(), items.size() * sizeof(int2), cudaMemcpyHostToDevice, st) != cudaSuccess ||
+        cudaMemsetAsync(nll_out, 0, (size_t)T * sizeof(float), st) != cudaSuccess)
+        return lfail(RSB_ERR_CUDA, "uploading the attention work list failed");
+
+    const int Hd = h->hidden, NQKV = h->qkv_n(), I = h->inter;
+    const float scale_log2 = 1.4426950408889634f / sqrtf((float)HD);   // 1/sqrt(128) in the log2 domain
+    const long long n8 = (long long)T * I / 8;
+    const int sw_grid = (int)std::min<long long>((n8 + 255) / 256, 8LL * rsb::device_num_sms());
+    embed_rows_kernel<<<T, 128, 0, st>>>(ids, h->embed, Hd, X);
+    int rc;
+    for (int li = 0; li < h->layers; ++li) {
+        const LlmLayer& l = h->L[li];
+        rms_rows_kernel<<<T, 256, 0, st>>>(X, nullptr, Hd, l.ln1, h->eps, Hn);
+        if ((rc = gemm(Hn, T, l.wqkv, NQKV, Hd, h->zero_bias, nullptr, QKV, 0, st)) != RSB_OK) return rc;
+        rope_kernel<<<T, 256, 0, st>>>(QKV, cu_seqlens, B, NQKV, h->heads + h->kv_heads, h->inv_freq);
+        attention_causal_kernel<<<dim3((unsigned)items.size(), h->heads), 128, 0, st>>>(QKV, cu_seqlens, d_items, CTX,
+                                                                                        h->heads, h->kv_heads, scale_log2);
+        if ((rc = gemm(CTX, T, l.wo, Hd, Hd, h->zero_bias, X, X, 2, st)) != RSB_OK) return rc;
+        rms_rows_kernel<<<T, 256, 0, st>>>(X, nullptr, Hd, l.ln2, h->eps, Hn);
+        if ((rc = gemm(Hn, T, l.wgu, 2 * I, Hd, h->zero_bias, nullptr, GU, 0, st)) != RSB_OK) return rc;
+        swiglu_kernel<<<sw_grid, 256, 0, st>>>(GU, n8, I, ACT);
+        if ((rc = gemm(ACT, T, l.wdown, Hd, I, h->zero_bias, X, X, 2 | RSB_GEMM_REVERSED, st)) != RSB_OK) return rc;
+    }
+    // final norm and LM head on the label rows only, in chunks that bound the logits workspace
+    const int chunk = h->chunk_rows();
+    for (int c0 = 0; c0 < nl; c0 += chunk) {
+        const int n = std::min(chunk, nl - c0);
+        rms_rows_kernel<<<n, 256, 0, st>>>(X, d_rows + c0, Hd, h->final_g, h->eps, Hn);
+        if ((rc = gemm(Hn, n, h->lm_head, h->vocab_pad, Hd, h->zero_bias, nullptr, LOG, 0, st)) != RSB_OK) return rc;
+        nll_rows_kernel<<<n, 256, 0, st>>>(LOG, h->vocab, h->vocab_pad, d_labs + c0, d_outi + c0, nll_out);
+    }
+    const cudaError_t e = cudaPeekAtLastError();
+    if (e != cudaSuccess) return lfail(RSB_ERR_CUDA, "reader launch failed: %s", cudaGetErrorString(e));
+    return RSB_OK;
+}

@@ -1,0 +1,268 @@
+"""GPU reader LM for perplexity evaluation: HF `LlamaForCausalLM` (Llama-2 MHA, Llama-3 GQA) in fp16 on librsb.
+
+The reference loads its reader with `AutoModelForCausalLM.from_pretrained(cfg.model.lm_model, torch_dtype=bfloat16)`
+and calls `lm(input_ids, labels=labels)` one window at a time (`src/evaluate_perplexity.py:98-134`).  Here
+
+    model = load_reader(path)                                   # local directory or HF cache, no download
+    nll = model.nll([ids_0, ids_1, ...], [labels_0, ...])       # per-token NLL, many windows per forward
+    losses = model.loss([ids_0, ...], [labels_0, ...])          # HF's per-window mean loss
+
+runs `rsb_llm_nll`: a prefill-only forward over packed, un-padded windows whose LM head runs only on the rows whose
+next token is a label.  No CPU / eager-PyTorch fallback: constructing the model without CUDA raises.  A checkpoint the
+kernels do not run (another `model_type` such as GPT-NeoX / Pythia, another head_dim, RoPE scaling, biases, ...) raises
+AttributeError naming the field before any weight is read or device memory is allocated.
+"""
+from __future__ import annotations
+
+import ctypes
+import json
+import math
+import os
+from typing import Dict, List, Optional, Sequence
+
+import torch
+
+from . import _lib
+
+IGNORE = -100
+
+
+def _get(cfg, key, default=None):
+    if isinstance(cfg, dict):
+        return cfg.get(key, default)
+    return getattr(cfg, key, default)
+
+
+def llama_geometry(cfg) -> dict:
+    """The reader geometry the kernels run, from an HF config (dict or object), or AttributeError naming the field."""
+    mt = _get(cfg, "model_type")
+    if mt != "llama":
+        why = (" (GPT-NeoX / Pythia needs head_dim-256 attention, partial rotary and a parallel residual)"
+               if mt == "gpt_neox" else "")
+        raise AttributeError(f"model_type {mt!r}: only 'llama' readers run on the GPU path{why}")
+    hidden, heads = _get(cfg, "hidden_size"), _get(cfg, "num_attention_heads")
+    kv = _get(cfg, "num_key_value_heads") or heads
+    head_dim = _get(cfg, "head_dim") or (hidden // heads if hidden and heads else None)
+    if head_dim != 128 or hidden != heads * 128:
+        raise AttributeError(f"head_dim {head_dim} (hidden_size {hidden}, num_attention_heads {heads}): only head_dim "
+                             f"128 with hidden_size = 128 x num_attention_heads is implemented")
+    if heads % kv:
+        raise AttributeError(f"num_key_value_heads {kv} does not divide num_attention_heads {heads}")
+    if _get(cfg, "hidden_act", "silu") != "silu":
+        raise AttributeError(f"hidden_act {_get(cfg, 'hidden_act')!r}: only 'silu' is implemented")
+    inter = _get(cfg, "intermediate_size")
+    if hidden % 128 or not inter or inter % 128:
+        raise AttributeError(f"hidden_size {hidden} / intermediate_size {inter}: both must be multiples of 128")
+    for key in ("attention_bias", "mlp_bias"):
+        if _get(cfg, key, False):
+            raise AttributeError(f"{key} is set: only bias-free Llama layers are implemented")
+    theta = _get(cfg, "rope_theta")
+    rp = _get(cfg, "rope_parameters")
+    if isinstance(rp, dict):                     # transformers >= 5 folds rope_theta / rope_scaling into rope_parameters
+        if rp.get("rope_type", "default") != "default":
+            raise AttributeError(f"rope_parameters {rp}: only the default RoPE is implemented (rope_scaling null)")
+        theta = rp.get("rope_theta", theta)
+    if _get(cfg, "rope_scaling") is not None and not (isinstance(rp, dict) and _get(cfg, "rope_scaling") == rp):
+        raise AttributeError(f"rope_scaling {_get(cfg, 'rope_scaling')}: only rope_scaling null is implemented")
+    vocab = _get(cfg, "vocab_size")
+    if not vocab or vocab <= 0:
+        raise AttributeError(f"vocab_size {vocab} is not a positive size")
+    return dict(num_hidden_layers=_get(cfg, "num_hidden_layers"), hidden_size=hidden, num_attention_heads=heads,
+                num_key_value_heads=kv, intermediate_size=inter, vocab_size=vocab,
+                max_position_embeddings=_get(cfg, "max_position_embeddings", 2048),
+                rope_theta=float(theta if theta is not None else 10000.0),
+                rms_norm_eps=float(_get(cfg, "rms_norm_eps", 1e-6)),
+                tie_word_embeddings=bool(_get(cfg, "tie_word_embeddings", False)))
+
+
+def expected_keys(geom: dict) -> List[str]:
+    """Every weight the forward reads (HF LlamaForCausalLM names)."""
+    keys = ["model.embed_tokens.weight", "model.norm.weight"]
+    if not geom["tie_word_embeddings"]:
+        keys.append("lm_head.weight")
+    for i in range(geom["num_hidden_layers"]):
+        keys += [f"model.layers.{i}.{n}.weight" for n in (
+            "self_attn.q_proj", "self_attn.k_proj", "self_attn.v_proj", "self_attn.o_proj", "mlp.gate_proj",
+            "mlp.up_proj", "mlp.down_proj", "input_layernorm", "post_attention_layernorm")]
+    return keys
+
+
+def scored_positions(labels: Sequence[int]) -> List[int]:
+    """Positions whose label enters HF's shifted loss: every position after the first whose label is not -100."""
+    return [t for t in range(1, len(labels)) if labels[t] != IGNORE]
+
+
+class B200Llama:
+    """An HF LlamaForCausalLM reader on librsb (`rsb_llm_*`)."""
+
+    # tokens per forward that `nll` packs: the GEMMs fill the GPU well before this, and the activations of a
+    # Llama-3-8B forward stay near 3 GB
+    token_budget = 16384
+
+    def __init__(self, config, device=None):
+        self.geom = llama_geometry(config)
+        if not torch.cuda.is_available():
+            raise RuntimeError("B200Llama needs a CUDA device (sm_90a): there is no CPU path")
+        self.L = _lib.lib()
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        self._h = ctypes.c_void_p(0)
+        self._ws: Optional[torch.Tensor] = None
+        self.loaded = set()
+        g = self.geom
+        with torch.cuda.device(self.device):
+            self._check(self.L.rsb_llm_create(
+                g["num_hidden_layers"], g["hidden_size"], g["num_attention_heads"], g["num_key_value_heads"],
+                g["intermediate_size"], g["vocab_size"], g["max_position_embeddings"], ctypes.c_float(g["rope_theta"]),
+                ctypes.c_float(g["rms_norm_eps"]), int(g["tie_word_embeddings"]), ctypes.byref(self._h)))
+
+    def _check(self, rc):
+        if rc == _lib.RSB_OK:
+            return
+        msg = self.L.rsb_llm_last_error().decode("utf-8", "replace")
+        if rc == _lib.RSB_ERR_INVALID:
+            raise ValueError(msg)
+        if rc == _lib.RSB_ERR_UNSUPPORTED:
+            raise NotImplementedError(msg)
+        if rc == _lib.RSB_ERR_OOM:
+            raise MemoryError(msg)
+        raise _lib.RsbError(f"librsb reader error {rc}: {msg}")
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None) and self._h.value:
+                self.L.rsb_llm_free(self._h)
+                self._h = ctypes.c_void_p(0)
+        except Exception:
+            pass
+
+    @property
+    def max_position_embeddings(self) -> int:
+        return self.geom["max_position_embeddings"]
+
+    def load_weight(self, name: str, t: torch.Tensor) -> bool:
+        """Uploads one HF weight in fp16; False for a name the reader does not use.  A weight that does not stay
+        finite in fp16 (a bf16 value beyond 65504) is refused."""
+        if name.endswith("rotary_emb.inv_freq"):
+            return False
+        w = t.detach().to(device=self.device, dtype=torch.float16).contiguous()
+        if not bool(torch.isfinite(w).all()):
+            raise ValueError(f"weight {name} does not stay finite in fp16")
+        stream = ctypes.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        rc = self.L.rsb_llm_load(self._h, name.encode(), ctypes.c_void_p(w.data_ptr()), w.numel(), stream)
+        if rc == _lib.RSB_ERR_INVALID and b"unknown weight" in self.L.rsb_llm_last_error():
+            return False
+        self._check(rc)
+        torch.cuda.current_stream(self.device).synchronize()
+        self.loaded.add(name)
+        return True
+
+    def load_state_dict(self, sd: Dict[str, torch.Tensor], strict: bool = True):
+        with torch.cuda.device(self.device):
+            unexpected = [n for n, t in sd.items() if not self.load_weight(n, t) and not n.endswith("rotary_emb.inv_freq")]
+        if strict and unexpected:
+            raise KeyError(f"unexpected keys in state_dict: {unexpected[:5]}")
+        if strict:
+            self.require_all_weights()
+        return unexpected
+
+    def missing_keys(self):
+        return [k for k in expected_keys(self.geom) if k not in self.loaded]
+
+    def require_all_weights(self, source: str = "state_dict"):
+        missing = self.missing_keys()
+        if missing:
+            raise KeyError(f"{source} lacks {len(missing)} reader weights, e.g. {missing[:3]}")
+
+    # -- forward ------------------------------------------------------------------------------------------------
+    def _nll_packed(self, ids: Sequence[Sequence[int]], labels: Sequence[Sequence[int]]) -> List[torch.Tensor]:
+        lens = [len(x) for x in ids]
+        T = sum(lens)
+        n_label = sum(len(scored_positions(lb)) for lb in labels)
+        cu = [0]
+        for n in lens:
+            cu.append(cu[-1] + n)
+        dev = self.device
+        flat_ids = torch.tensor([v for x in ids for v in x], dtype=torch.int32, device=dev)
+        flat_lab = torch.tensor([v for x in labels for v in x], dtype=torch.int32, device=dev)
+        cu_t = torch.tensor(cu, dtype=torch.int32, device=dev)
+        out = torch.empty(T, dtype=torch.float32, device=dev)
+        need = self.L.rsb_llm_workspace_bytes(self._h, T, n_label)
+        if self._ws is None or self._ws.numel() < need:
+            self._ws = None
+            self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev):
+            rc = self.L.rsb_llm_nll(self._h, ctypes.c_void_p(flat_ids.data_ptr()), ctypes.c_void_p(cu_t.data_ptr()),
+                                    len(lens), T, max(lens), ctypes.c_void_p(flat_lab.data_ptr()),
+                                    ctypes.c_void_p(out.data_ptr()), ctypes.c_void_p(self._ws.data_ptr()),
+                                    self._ws.numel(), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+        self._check(rc)
+        host = out.cpu()
+        if not bool(torch.isfinite(host).all()):
+            raise FloatingPointError("non-finite per-token NLL: the fp16 activations overflowed (|x| > 65504); this "
+                                     "checkpoint needs a bf16 or fp32 residual stream")
+        return [host[cu[i]:cu[i + 1]].clone() for i in range(len(lens))]
+
+    def nll(self, input_ids_list, labels_list, max_tokens: Optional[int] = None) -> List[torch.Tensor]:
+        """Per-token NLL of each window, fp32 [len(ids)] on the host: position t holds -log p(labels[t] | ids[:t])
+        where t > 0 and labels[t] != -100, 0 elsewhere.  Consecutive windows are packed into one forward up to
+        `max_tokens` (default `token_budget`); the kernels treat every window on its own, so the values are the
+        same as one call per window."""
+        ids = [[int(v) for v in x] for x in input_ids_list]
+        labels = [[int(v) for v in x] for x in labels_list]
+        if len(ids) != len(labels) or any(len(a) != len(b) for a, b in zip(ids, labels)):
+            raise ValueError("every window needs one label per token")
+        if any(len(x) == 0 for x in ids):
+            raise ValueError("empty window")
+        budget = self.token_budget if max_tokens is None else int(max_tokens)
+        out: List[torch.Tensor] = []
+        i = 0
+        while i < len(ids):
+            j, tokens = i, 0
+            while j < len(ids) and (j == i or tokens + len(ids[j]) <= budget):
+                tokens += len(ids[j])
+                j += 1
+            out += self._nll_packed(ids[i:j], labels[i:j])
+            i = j
+        return out
+
+    def loss(self, input_ids_list, labels_list, max_tokens: Optional[int] = None) -> List[float]:
+        """`lm(input_ids, labels=labels).loss` per window: the mean NLL over the scored positions, NaN for a window
+        without any (HF's mean over zero tokens)."""
+        res = []
+        for nll, lb in zip(self.nll(input_ids_list, labels_list, max_tokens), labels_list):
+            pos = scored_positions([int(v) for v in lb])
+            res.append(float(nll[pos].double().sum() / len(pos)) if pos else math.nan)
+        return res
+
+
+def _shard_files(directory: str) -> List[str]:
+    index = os.path.join(directory, "model.safetensors.index.json")
+    if os.path.exists(index):
+        with open(index) as f:
+            files = sorted(set(json.load(f)["weight_map"].values()))
+        return [os.path.join(directory, fn) for fn in files]
+    single = os.path.join(directory, "model.safetensors")
+    if os.path.exists(single):
+        return [single]
+    raise FileNotFoundError(f"{directory}: neither model.safetensors nor model.safetensors.index.json is present")
+
+
+def load_reader(path: str, device=None) -> B200Llama:
+    """The reader of `cfg.model.lm_model` from a local directory or the Hugging Face cache (never downloaded), with
+    single-file or sharded safetensors weights; bf16 / fp32 weights are converted to fp16."""
+    from safetensors import safe_open
+
+    from .encoder import _resolve_model_dir
+    directory = _resolve_model_dir(path)
+    with open(os.path.join(directory, "config.json")) as f:
+        cfg = json.load(f)
+    llama_geometry(cfg)                          # refuses before any weight is read or device memory allocated
+    files = _shard_files(directory)
+    model = B200Llama(cfg, device=device)
+    with torch.cuda.device(model.device):
+        for fn in files:
+            with safe_open(fn, framework="pt") as f:
+                for name in f.keys():
+                    model.load_weight(name, f.get_tensor(name))
+    model.require_all_weights(directory)
+    return model

@@ -159,8 +159,9 @@ def load_jsonl(path):
 
 
 def load_eval_data(cfg):
-    """Eval-data adapter (reference `src/data.py:271-318`).  `lm-eval`: query = ex['query'].  The perplexity
-    task needs the reader LM's tokenizer (network / HF cache) and is loaded lazily only when asked for."""
+    """Eval-data adapter (reference `src/data.py:271-318`).  `lm-eval`: query = ex['query'].  `perplexity`: windows
+    of ex['text'] in the tokens of `model.lm_model` (`perplexity.prepare_ppl_eval_data`); its tokenizer is read from a
+    local directory or the HF cache only when this task asks for it."""
     path = cfg.evaluation.data.eval_data
     task = cfg.tasks.eval.task_name
     if not path.endswith(".jsonl"):
@@ -170,9 +171,12 @@ def load_eval_data(cfg):
         for ex in data:
             ex["raw_query"] = ex["query"]
         return data
-    if task == "perplexity":
-        raise NotImplementedError("perplexity eval-data windowing (src/data.py:332-366) is outside the retrieval "
-                                  "hot path; run with tasks.eval.task_name=lm-eval")
+    if task == "perplexity":                     # windows of the eval text in the reader's tokens (src/data.py:283-295)
+        from .perplexity import load_lm_tokenizer, prepare_ppl_eval_data
+        d = cfg.evaluation.data
+        return prepare_ppl_eval_data(data, load_lm_tokenizer(cfg.model.lm_model), d.get("max_eval_data_seq_length", 1024),
+                                     d.get("eval_stride", 512), d.get("merge", True), d.get("num_eval_samples", None),
+                                     d.get("seed", 310))
     raise AttributeError(task)
 
 

@@ -6,9 +6,9 @@
 Hydra / OmegaConf are replaced by `retrieval_scaling_b200.config` (same YAML files, same dotted overrides).
 Task switches: tasks.datastore.embedding (already-chunked passage shards -> embedding pickles, SURVEY §8f-4),
 tasks.datastore.index (build or load the index), tasks.eval.search (query -> top-k, the hot path),
-tasks.eval.merge_search (multi-source merge, MinHash de-duplication on the GPU and subsampling, reference :31-33).
-tasks.eval.inference belongs to a subsystem that is out of scope of the GPU hot path (SURVEY.md §2) and raises
-NotImplementedError.
+tasks.eval.merge_search (multi-source merge, MinHash de-duplication on the GPU and subsampling, reference :31-33),
+tasks.eval.inference (task_name perplexity: reader-LM perplexity with concate_k retrieved documents prepended, the
+Llama reader on the GPU, reference :35-38; perplexity_calibration and lm-eval raise NotImplementedError).
 """
 import logging
 import os
@@ -64,7 +64,10 @@ def main(cfg) -> None:
         from retrieval_scaling_b200.search import post_hoc_merge_topk_multi_domain
         post_hoc_merge_topk_multi_domain(cfg)
     if cfg.tasks.eval.get("inference", False):
-        raise NotImplementedError("reader-LM perplexity evaluation is downstream of retrieval (out of scope)")
+        logging.info("\n\n************** Running Perplexity Evaluation ***********")
+        from retrieval_scaling_b200.perplexity import evaluate_perplexity, log_results_separately
+        outputs = evaluate_perplexity(cfg)     # reference :36-39; perplexity_calibration / lm-eval: NotImplementedError
+        log_results_separately(cfg, outputs)
 
 
 if __name__ == "__main__":
