@@ -4,10 +4,10 @@
 // is ~2^-22 relative) accumulated in fp32 registers.  Used for the IVF coarse quantizer (the IndexFlatIP the reference
 // builds at src/indicies/ivf_flat.py:142, ivf_pq.py:145).
 //
-// Same pipeline as the encoder GEMM (rsb_bert.cu): 128 x 128 output tile per CTA, TMA tensor loads (128B swizzle,
-// 32 fp32 = one swizzle row per K step) -> 3-stage shared-memory ring of {Ah, Al, Bh, Bl} tiles filled by one
-// producer thread -> two consumer warpgroups, each issuing 12 wgmma.m64n128k8.tf32 per stage (4 K-slices x 3
-// products) on its 64 rows -> epilogue from the accumulator registers.
+// 128 x 128 output tiles, TMA tensor loads (128B swizzle, 32 fp32 = one swizzle row per K step) -> 3-stage
+// shared-memory ring of {Ah, Al, Bh, Bl} tiles filled by one producer thread -> two consumer warpgroups that take the
+// tiles of a persistent CTA in turn, each issuing 24 wgmma.m64n128k8.tf32 per stage (4 K-slices x 3 products x 2
+// row halves) -> epilogue from the accumulator registers while the other warpgroup runs the next tile's MMAs.
 //
 // fp16 form (F16 = true; Flat indexes with fp16 storage): B is the database as stored (fp16 rows, exact), so no split
 // copy of it exists.  Each query row is scaled by a power of two s that puts its largest |element| in [2^14, 2^15)
@@ -19,6 +19,7 @@
 #include "rsb_internal.h"
 #include "rsb_tc.cuh"
 
+#include <algorithm>
 #include <math.h>
 #include <stdlib.h>
 
@@ -31,8 +32,6 @@ constexpr int T_THREADS = 384;                                // warpgroup 0: TM
 constexpr int T_TILE_BYTES = 128 * T_BK * 4;                  // 16 KB
 constexpr int T_STAGE_BYTES = 4 * T_TILE_BYTES;               // Ah, Al, Bh, Bl (fp16 form: Ah, Al, B)
 constexpr int T_SMEM = T_STAGES * T_STAGE_BYTES + 1024 + 256;
-constexpr int T_LDS = T_BN + 1;                               // row stride of the fused epilogue's staged tile (floats)
-static_assert(T_BM * T_LDS * 4 + T_BM * 9 * 8 <= T_STAGES * T_STAGE_BYTES, "staged tile must fit in the ring");
 
 __global__ void split_tf32_kernel(const float* __restrict__ x, size_t n, float* __restrict__ hi, float* __restrict__ lo) {
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
@@ -82,204 +81,264 @@ void launch_split_f16(const float* q, int M, int K, void* hi, void* lo, float* i
     split_f16_kernel<<<M, 128, 0, st>>>(q, K, static_cast<__half*>(hi), static_cast<__half*>(lo), inv);
 }
 
-// FUSED = false: the 128 x 128 score tile goes to C.  FUSED = true: the score tile never goes to HBM.  Every row of
-// the tile keeps its 9 largest scores (sorted insertion in column order, strict comparisons => ties keep the lower
-// column); the top 8 are emitted as candidates (64 B per row per 128-column tile) together with the 9th as a bound:
-// an element the filter dropped is <= the 9th largest of its tile, so if the kc-th best CANDIDATE of a row is
-// strictly greater than the maximum of these bounds over the row, no dropped element can belong to the row's top kc
-// -- select_cands_kernel checks exactly that and flags the (rare) rows for which it fails; those are re-done
-// exhaustively in fp32 by exact_rows_kernel.  The result is therefore the exact top-kc of the 3xTF32 scores without
-// writing and re-reading nq x nlist x 4 bytes.
+// Persistent, warp-specialised: every CTA walks the tiles blockIdx.x, blockIdx.x + gridDim.x, ... of tile_coords' order.
+// Warpgroup 0 (one thread) streams the {A, B} k-blocks of all of them through the ring without draining it between
+// tiles; consumer warpgroups 1 and 2 take the CTA's tiles in turn (ping-pong) and each computes a whole 128 x 128 tile
+// (two m64n128 accumulators), so one warpgroup's epilogue runs while the other one's MMAs keep the tensor cores busy.
+// The k-blocks of consecutive tiles pass through the ring in order, so warpgroup w starts waiting on the stages of its
+// tile only once the other warpgroup has seen every stage of the previous tile filled (mdone): a stage's full barrier
+// is then never more than one phase behind the parity waited for.
+//
+// FUSED = false: the score tile goes to C.  FUSED = true: the score tile never goes to HBM.  Every row of the tile
+// keeps its 9 largest scores in the total order (score descending, column ascending) -- the order a sequential strict
+// insertion in column order realises; the top 8 are emitted as candidates (64 B per row per 128-column tile) together
+// with the 9th as a bound: an element the filter dropped is <= the 9th largest of its tile, so if the kc-th best
+// CANDIDATE of a row is strictly greater than the maximum of these bounds over the row, no dropped element can belong
+// to the row's top kc -- select_cands_kernel checks exactly that and flags the (rare) rows for which it fails; those
+// are re-done exhaustively in fp32 by exact_rows_kernel.  The result is therefore the exact top-kc of the 3xTF32
+// scores without writing and re-reading nq x nlist x 4 bytes.
 // F16: fp16 operands (tmBl unused), scores multiplied by inv[row] before either epilogue.
+
+// tile t -> (query tile, column tile): bands of `band` query tiles; inside a band the query tile runs fastest, so the
+// CTAs in flight share a few column tiles and the band's query operand stays L2-resident while it sweeps all columns
+__device__ __forceinline__ void tile_coords(int t, int tiles_m, int tiles_n, int band, int& tm, int& tn) {
+    const int per_band = band * tiles_n;
+    const int b = t / per_band;
+    const int rows = min(band, tiles_m - b * band);
+    const int local = t - b * per_band;
+    tm = b * band + local % rows;
+    tn = local / rows;
+}
+
+// sorted insertion, strict comparisons: fed in ascending column order, ties keep the lower column
+__device__ __forceinline__ void top9_push(float (&v)[9], int (&c)[9], float x, int col) {
+    if (x > v[8]) {
+        v[8] = x; c[8] = col;
+#pragma unroll
+        for (int i = 8; i > 0; --i) {
+            if (v[i] > v[i - 1]) {
+                const float tv = v[i]; v[i] = v[i - 1]; v[i - 1] = tv;
+                const int tc = c[i]; c[i] = c[i - 1]; c[i - 1] = tc;
+            }
+        }
+    }
+}
+// (x, cx) ranks before (y, cy): higher score, or the same score and the lower column; empty entries (-inf, -1) last
+__device__ __forceinline__ bool top9_before(float x, int cx, float y, int cy) {
+    return x > y || (x == y && (unsigned)cx < (unsigned)cy);
+}
+// merge the list of lane ^ off into this lane's: both lanes end with the top 9 of the union in the total order
+__device__ __forceinline__ void top9_merge(float (&v)[9], int (&c)[9], int off) {
+    float pv[9];
+    int pc[9];
+#pragma unroll
+    for (int i = 0; i < 9; ++i) {
+        pv[i] = __shfl_xor_sync(0xffffffffu, v[i], off);
+        pc[i] = __shfl_xor_sync(0xffffffffu, c[i], off);
+    }
+#pragma unroll
+    for (int k = 0; k < 9; ++k) {
+        if (top9_before(pv[k], pc[k], v[8], c[8])) {
+            v[8] = pv[k]; c[8] = pc[k];
+#pragma unroll
+            for (int i = 8; i > 0; --i) {
+                if (top9_before(v[i], c[i], v[i - 1], c[i - 1])) {
+                    const float tv = v[i]; v[i] = v[i - 1]; v[i - 1] = tv;
+                    const int tc = c[i]; c[i] = c[i - 1]; c[i - 1] = tc;
+                }
+            }
+        }
+    }
+}
+
 template <bool F16, bool FUSED>
 __global__ __launch_bounds__(T_THREADS, 1)
 void gemm_ip_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
                        const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl,
                        const float* __restrict__ inv, float* __restrict__ C, int ldc, u64* __restrict__ cand,
-                       unsigned* __restrict__ xbound, int M, int N, int K, unsigned col_base, int m_fastest) {
+                       unsigned* __restrict__ xbound, int M, int N, int K, unsigned col_base, int band) {
     constexpr int BK = F16 ? T_BK16 : T_BK;                   // K elements per stage: one 128-byte swizzle row
     constexpr int STAGE_TX = (F16 ? 3 : 4) * T_TILE_BYTES;
     extern __shared__ unsigned char smem_dyn[];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + T_STAGES * T_STAGE_BYTES);
     uint64_t* empty = full + T_STAGES;
+    uint64_t* mdone = empty + T_STAGES;                       // [w]: warpgroup w has seen all stages of its tile filled
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
-    int tm = blockIdx.y, tn = blockIdx.x;
-    const int nhalf = 2 * ((N + 255) / 256);                  // 128-column candidate items per row (FUSED)
-    if (FUSED) {
-        // tile order: m fastest = consecutive tiles share one B (centroid) tile and sweep the query tiles, which stay
-        // L2-resident -- n fastest re-reads the whole centroid matrix per query tile
-        const int tiles_m = (M + T_BM - 1) / T_BM;
-        tm = m_fastest ? (int)blockIdx.x % tiles_m : (int)blockIdx.x / nhalf;
-        tn = m_fastest ? (int)blockIdx.x / tiles_m : (int)blockIdx.x % nhalf;
-    }
-    const int m0 = tm * T_BM, n0 = tn * T_BN;
+    const int tiles_m = (M + T_BM - 1) / T_BM, tiles_n = (N + T_BN - 1) / T_BN;
+    const int ntiles = tiles_m * tiles_n;
     const int nk = K / BK;
-    if (FUSED && n0 >= N) {                                   // the empty second half of a 256-column group: no candidates
-        const int row = m0 + (int)threadIdx.x;
-        if (threadIdx.x < T_BM && row < M) {
-            const size_t item = (size_t)row * nhalf + (size_t)tn;
-            ulonglong2* dst = reinterpret_cast<ulonglong2*>(cand + item * 8);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) dst[i] = make_ulonglong2(0ull, 0ull);
-            xbound[item] = 0u;
-        }
-        return;
-    }
 
     if (threadIdx.x == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmAh)) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmAl)) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmBh)) : "memory");
         if (!F16) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmBl)) : "memory");
-        for (int s = 0; s < T_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }   // 8 consumer warps
+        for (int s = 0; s < T_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 4); }   // 4 warps of one consumer
+        mbar_init(&mdone[0], 1);
+        mbar_init(&mdone[1], 1);
         fence_barrier_init();
     }
     __syncthreads();
 
     if (wg == 0) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
         if (threadIdx.x == 0) {
-            for (int kb = 0; kb < nk; ++kb) {
-                const int s = kb % T_STAGES;
-                mbar_wait(&empty[s], ((kb / T_STAGES) & 1) ^ 1);   // the first pass over the ring falls through
-                unsigned char* base = smem + s * T_STAGE_BYTES;
-                mbar_expect_tx(&full[s], STAGE_TX);
-                tma_load_2d(base + 0 * T_TILE_BYTES, &tmAh, &full[s], kb * BK, m0);   // rows past M / N read as zero
-                tma_load_2d(base + 1 * T_TILE_BYTES, &tmAl, &full[s], kb * BK, m0);
-                tma_load_2d(base + 2 * T_TILE_BYTES, &tmBh, &full[s], kb * BK, n0);
-                if (!F16) tma_load_2d(base + 3 * T_TILE_BYTES, &tmBl, &full[s], kb * BK, n0);
-            }
-        }
-        return;
-    }
-
-    const int cw = wg - 1;                                    // consumer warpgroup: tile rows 64 cw .. 64 cw + 63
-    float acc[64];
-#pragma unroll
-    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-    for (int kb = 0; kb < nk; ++kb) {
-        const int s = kb % T_STAGES;
-        mbar_wait(&full[s], (kb / T_STAGES) & 1);
-        const uint32_t base = smem_u32(smem + s * T_STAGE_BYTES);
-        const uint64_t ah = make_sw128_kmajor_desc(base + cw * 64 * 128);
-        const uint64_t al = make_sw128_kmajor_desc(base + T_TILE_BYTES + cw * 64 * 128);
-        const uint64_t bh = make_sw128_kmajor_desc(base + 2 * T_TILE_BYTES);
-        const uint64_t bl = make_sw128_kmajor_desc(base + 3 * T_TILE_BYTES);
-        acc_fence(acc);
-        wgmma_fence();
-        if (F16) {
-#pragma unroll
-            for (int k4 = 0; k4 < T_BK16 / 16; ++k4) {        // K = 16 fp16 = 32 bytes: +2 in the (addr >> 4) field
-                const uint64_t o = (uint64_t)(k4 * 2);
-                wgmma_f16_n128(acc, al + o, bh + o);          // the small term first, then the dominant hi.B product
-                wgmma_f16_n128(acc, ah + o, bh + o);
-            }
-        } else {
-#pragma unroll
-            for (int k4 = 0; k4 < T_BK / 8; ++k4) {           // K = 8 tf32 = 32 bytes: +2 in the (addr >> 4) field
-                const uint64_t o = (uint64_t)(k4 * 2);
-                wgmma_tf32_n128(acc, al + o, bh + o);         // small terms first, the dominant Ah.Bh product last
-                wgmma_tf32_n128(acc, ah + o, bl + o);
-                wgmma_tf32_n128(acc, ah + o, bh + o);
-            }
-        }
-        wgmma_commit();
-        acc_fence(acc);
-        wgmma_wait<1>();                                      // the previous k-block's MMAs have retired: free its stage
-        if (kb > 0) {
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&empty[(kb - 1) % T_STAGES]);
-        }
-    }
-    wgmma_wait<0>();
-    acc_fence(acc);
-
-    const int r_lo = cw * 64 + (warp & 3) * 16 + (lane >> 2);   // tile row of acc[4 j + c]; acc[4 j + 2 + c]: r_lo + 8
-    const int c_lo = 2 * (lane & 3);                            // tile column of acc[4 j]: 8 j + c_lo
-    if (F16) {                                                  // undo the per-row query scale (a power of two: exact)
-        const float s0 = m0 + r_lo < M ? inv[m0 + r_lo] : 0.f;
-        const float s1 = m0 + r_lo + 8 < M ? inv[m0 + r_lo + 8] : 0.f;
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-            acc[4 * j] *= s0; acc[4 * j + 1] *= s0;
-            acc[4 * j + 2] *= s1; acc[4 * j + 3] *= s1;
-        }
-    }
-    if (!FUSED) {
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int row = m0 + r_lo + 8 * h;
-            if (row >= M) continue;
-            float* dst = C + (size_t)row * ldc + n0;
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-                const int col = 8 * j + c_lo;
-                if (n0 + col + 1 < N) *reinterpret_cast<float2*>(dst + col) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-                else if (n0 + col < N) dst[col] = acc[4 * j + 2 * h];
-            }
-        }
-        return;
-    }
-
-    // fused epilogue: both consumer warpgroups are done with the ring -> stage the 128 x 128 tile there.  Every row is
-    // split between the warpgroups: each selects the 9 largest scores of its 64 columns in column order, then the
-    // second half's list (sorted, ties in column order) goes through the same strict-comparison insertion into the
-    // first half's -- the result is exactly that of one sequential pass over the 128 columns.
-    named_sync(1, 256);
-    float* S = reinterpret_cast<float*>(smem);
-#pragma unroll
-    for (int j = 0; j < 16; ++j)
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            S[(r_lo + 8 * h) * T_LDS + 8 * j + c_lo] = acc[4 * j + 2 * h];
-            S[(r_lo + 8 * h) * T_LDS + 8 * j + c_lo + 1] = acc[4 * j + 2 * h + 1];
-        }
-    named_sync(1, 256);
-    const int r = (int)threadIdx.x & 127;                     // tile row
-    const int half = cw;                                      // columns 64 half .. 64 half + 63
-    const int row = m0 + r;
-    float v[9];
-    int c[9];
-#pragma unroll
-    for (int i = 0; i < 9; ++i) { v[i] = -INFINITY; c[i] = -1; }
-    auto insert = [&](float x, int col) {
-        if (x > v[8]) {
-            v[8] = x; c[8] = col;
-#pragma unroll
-            for (int i = 8; i > 0; --i) {
-                if (v[i] > v[i - 1]) {
-                    const float tv = v[i]; v[i] = v[i - 1]; v[i - 1] = tv;
-                    const int tc = c[i]; c[i] = c[i - 1]; c[i - 1] = tc;
+            int g = 0;                                        // k-block counter over all tiles of this CTA
+            for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
+                int tm, tn;
+                tile_coords(t, tiles_m, tiles_n, band, tm, tn);
+                for (int kb = 0; kb < nk; ++kb, ++g) {
+                    const int s = g % T_STAGES;
+                    mbar_wait(&empty[s], ((g / T_STAGES) & 1) ^ 1);   // the first pass over the ring falls through
+                    unsigned char* base = smem + s * T_STAGE_BYTES;
+                    mbar_expect_tx(&full[s], STAGE_TX);
+                    tma_load_2d(base + 0 * T_TILE_BYTES, &tmAh, &full[s], kb * BK, tm * T_BM);   // rows past M / N read as zero
+                    tma_load_2d(base + 1 * T_TILE_BYTES, &tmAl, &full[s], kb * BK, tm * T_BM);
+                    tma_load_2d(base + 2 * T_TILE_BYTES, &tmBh, &full[s], kb * BK, tn * T_BN);
+                    if (!F16) tma_load_2d(base + 3 * T_TILE_BYTES, &tmBl, &full[s], kb * BK, tn * T_BN);
                 }
             }
         }
-    };
-    const float* srow = S + r * T_LDS;
-    const int ncol = N - n0 < T_BN ? N - n0 : T_BN;
-    const int e1 = ncol < 64 * (half + 1) ? ncol : 64 * (half + 1);
-#pragma unroll 4
-    for (int e = 64 * half; e < e1; ++e) insert(srow[e], n0 + e);
-    float* hv = S + T_BM * T_LDS;                             // second half's lists: [128][9] scores, [128][9] columns
-    int* hc = reinterpret_cast<int*>(hv + T_BM * 9);
-    if (half == 1) {
-#pragma unroll
-        for (int i = 0; i < 9; ++i) { hv[r * 9 + i] = v[i]; hc[r * 9 + i] = c[i]; }
+        return;
     }
-    named_sync(1, 256);
-    if (half == 1 || row >= M) return;
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+
+    const int cw = wg - 1;                                    // consumer warpgroup: local tiles cw, cw + 2, ...
+    const int r_lo = (warp & 3) * 16 + (lane >> 2);           // rows of acc[h][4 j + c]: 64 h + r_lo; acc[h][4 j + 2 + c]: + 8
+    const int c_lo = 2 * (lane & 3);                          // column of acc[h][4 j + c]: 8 j + c_lo + c
+    float acc[2][64];
+    for (int i = cw;; i += 2) {
+        const int t = blockIdx.x + i * gridDim.x;
+        if (t >= ntiles) break;
+        int tm, tn;
+        tile_coords(t, tiles_m, tiles_n, band, tm, tn);
+        const int m0 = tm * T_BM, n0 = tn * T_BN;
 #pragma unroll
-    for (int i = 0; i < 9; ++i) insert(hv[r * 9 + i], hc[r * 9 + i]);
-    const size_t item = (size_t)row * nhalf + (size_t)tn;
-    u64 keys[8];
+        for (int e = 0; e < 64; ++e) { acc[0][e] = 0.f; acc[1][e] = 0.f; }
+        if (i > 0) mbar_wait(&mdone[(i - 1) & 1], ((i - 1) >> 1) & 1);
+        int g = i * nk;
+        for (int kb = 0; kb < nk; ++kb, ++g) {
+            const int s = g % T_STAGES;
+            mbar_wait(&full[s], (g / T_STAGES) & 1);
+            const uint32_t base = smem_u32(smem + s * T_STAGE_BYTES);
+            const uint64_t ah = make_sw128_kmajor_desc(base);
+            const uint64_t al = make_sw128_kmajor_desc(base + T_TILE_BYTES);
+            const uint64_t bh = make_sw128_kmajor_desc(base + 2 * T_TILE_BYTES);
+            const uint64_t bl = make_sw128_kmajor_desc(base + 3 * T_TILE_BYTES);
+            constexpr uint64_t LOWER = (64 * 128) >> 4;       // rows 64..127: 64 swizzle rows further in the A tiles
+            acc_fence(acc[0]);
+            acc_fence(acc[1]);
+            wgmma_fence();
+            // per output element, per K slice: the small term(s) first, the dominant hi product last
+            if (F16) {
 #pragma unroll
-    for (int i = 0; i < 8; ++i)
-        keys[i] = c[i] >= 0 ? ((static_cast<u64>(ord_f32(v[i])) << 32) | static_cast<u64>(0xFFFFFFFFu - (col_base + (unsigned)c[i])))
-                            : 0ull;
-    ulonglong2* dst = reinterpret_cast<ulonglong2*>(cand + item * 8);
+                for (int k4 = 0; k4 < T_BK16 / 16; ++k4) {    // K = 16 fp16 = 32 bytes: +2 in the (addr >> 4) field
+                    const uint64_t o = (uint64_t)(k4 * 2);
+                    wgmma_f16_n128(acc[0], al + o, bh + o);
+                    wgmma_f16_n128(acc[1], al + LOWER + o, bh + o);
+                    wgmma_f16_n128(acc[0], ah + o, bh + o);
+                    wgmma_f16_n128(acc[1], ah + LOWER + o, bh + o);
+                }
+            } else {
 #pragma unroll
-    for (int i = 0; i < 4; ++i) dst[i] = make_ulonglong2(keys[2 * i], keys[2 * i + 1]);
-    xbound[item] = c[8] >= 0 ? ord_f32(v[8]) : 0u;
+                for (int k4 = 0; k4 < T_BK / 8; ++k4) {       // K = 8 tf32 = 32 bytes: +2 in the (addr >> 4) field
+                    const uint64_t o = (uint64_t)(k4 * 2);
+                    wgmma_tf32_n128(acc[0], al + o, bh + o);
+                    wgmma_tf32_n128(acc[1], al + LOWER + o, bh + o);
+                    wgmma_tf32_n128(acc[0], ah + o, bl + o);
+                    wgmma_tf32_n128(acc[1], ah + LOWER + o, bl + o);
+                    wgmma_tf32_n128(acc[0], ah + o, bh + o);
+                    wgmma_tf32_n128(acc[1], ah + LOWER + o, bh + o);
+                }
+            }
+            wgmma_commit();
+            acc_fence(acc[0]);
+            acc_fence(acc[1]);
+            wgmma_wait<1>();                                  // the previous k-block's MMAs have retired: free its stage
+            if (kb > 0) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty[(g - 1) % T_STAGES]);
+            }
+        }
+        if (threadIdx.x % 128 == 0) mbar_arrive(&mdone[cw]);  // the other warpgroup may start on the next tile's stages
+        wgmma_wait<0>();
+        acc_fence(acc[0]);
+        acc_fence(acc[1]);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[(g - 1) % T_STAGES]);
+
+        if (!FUSED) {
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int row = m0 + 64 * hh + r_lo + 8 * h;
+                    if (row >= M) continue;
+                    const float s = F16 ? inv[row] : 1.f;     // undo the per-row query scale (a power of two: exact)
+                    float* dst = C + (size_t)row * ldc + n0;
+#pragma unroll
+                    for (int j = 0; j < 16; ++j) {
+                        const int col = 8 * j + c_lo;
+                        float x0 = acc[hh][4 * j + 2 * h], x1 = acc[hh][4 * j + 2 * h + 1];
+                        if (F16) { x0 *= s; x1 *= s; }
+                        if (n0 + col + 1 < N) *reinterpret_cast<float2*>(dst + col) = make_float2(x0, x1);
+                        else if (n0 + col < N) dst[col] = x0;
+                    }
+                }
+            continue;
+        }
+
+        // fused epilogue, straight from the accumulators: a row of the tile lives in the 4 lanes of a quad (lane & 3),
+        // 32 columns each.  Each lane keeps its columns' top 9 (fed in column order), then two butterfly merges give
+        // every lane of the quad the row's top 9 of the total order -- the same 9 as one sequential pass over the row.
+        const int nhalf = 2 * ((N + 255) / 256);              // 128-column candidate items per row
+        const int q = lane & 3;
+        const int nrows = m0 + 64 < M ? 4 : 2;               // tile rows 64..127 hold no query: skip them
+#pragma unroll 1
+        for (int rr = 0; rr < nrows; ++rr) {                  // tile row 64 (rr >> 1) + r_lo + 8 (rr & 1)
+            const int hh = rr >> 1, h = rr & 1;
+            const int row = m0 + 64 * hh + r_lo + 8 * h;
+            const float s = F16 ? (row < M ? inv[row] : 0.f) : 1.f;
+            float v[9];
+            int c[9];
+#pragma unroll
+            for (int e = 0; e < 9; ++e) { v[e] = -INFINITY; c[e] = -1; }
+#pragma unroll
+            for (int j = 0; j < 16; ++j)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const float a0 = h ? acc[0][4 * j + 2 + e] : acc[0][4 * j + e];
+                    const float a1 = h ? acc[1][4 * j + 2 + e] : acc[1][4 * j + e];
+                    float x = hh ? a1 : a0;
+                    if (F16) x *= s;
+                    const int col = 8 * j + c_lo + e;
+                    if (n0 + col < N) top9_push(v, c, x, n0 + col);
+                }
+            top9_merge(v, c, 1);
+            top9_merge(v, c, 2);
+            if (row >= M) continue;
+            u64 k0 = 0ull, k1 = 0ull;                         // this lane writes candidates 2 q, 2 q + 1
+#pragma unroll
+            for (int e = 0; e < 4; ++e)
+                if (q == e) {
+                    k0 = c[2 * e] >= 0 ? ((static_cast<u64>(ord_f32(v[2 * e])) << 32) |
+                                          static_cast<u64>(0xFFFFFFFFu - (col_base + (unsigned)c[2 * e])))
+                                       : 0ull;
+                    k1 = c[2 * e + 1] >= 0 ? ((static_cast<u64>(ord_f32(v[2 * e + 1])) << 32) |
+                                              static_cast<u64>(0xFFFFFFFFu - (col_base + (unsigned)c[2 * e + 1])))
+                                           : 0ull;
+                }
+            const size_t item = (size_t)row * nhalf + (size_t)tn;
+            reinterpret_cast<ulonglong2*>(cand + item * 8)[q] = make_ulonglong2(k0, k1);
+            if (q == 0) xbound[item] = c[8] >= 0 ? ord_f32(v[8]) : 0u;
+            if (tn + 1 < nhalf && tn + 1 == tiles_n) {        // the empty second half of the last 256-column group
+                reinterpret_cast<ulonglong2*>(cand + (item + 1) * 8)[q] = make_ulonglong2(0ull, 0ull);
+                if (q == 0) xbound[item + 1] = 0u;
+            }
+        }
+    }
 }
 
 static bool make_maps(CUtensorMap (&m)[4], const float* Ah, const float* Al, int M, const float* Bh, const float* Bl, int N, int K) {
@@ -290,27 +349,38 @@ static bool make_maps(CUtensorMap (&m)[4], const float* Ah, const float* Al, int
 // candidates kept per row per call: 8 per 128-column tile, counted in pairs of tiles (256 columns)
 size_t fused_cand_per_row(int N) { return (size_t)((N + 255) / 256) * 2 * 8; }
 
-template <bool F16>
-static void launch_gemm_topt(const CUtensorMap (&m)[4], const float* inv, int M, int N, int K, unsigned col_base, u64* cand,
-                             unsigned* xbound, cudaStream_t st) {
-    static PerDeviceSize configured;
-    if (configured.raise(T_SMEM))
-        cudaFuncSetAttribute(gemm_ip_tc_kernel<F16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, T_SMEM);
-    const int ntiles = ((M + T_BM - 1) / T_BM) * (int)(fused_cand_per_row(N) / 8);
-    static const int m_fastest = getenv("RSB_COARSE_N_FASTEST") ? 0 : 1;
-    gemm_ip_tc_kernel<F16, true><<<ntiles, T_THREADS, T_SMEM, st>>>(m[0], m[1], m[2], m[3], inv, nullptr, 0, cand, xbound,
-                                                                    M, N, K, col_base, m_fastest);
+static int device_l2_bytes() {
+    static int l2[64] = {};
+    int& b = l2[current_device_slot()];
+    if (!b) {
+        int dev = 0;
+        cudaGetDevice(&dev);
+        cudaDeviceGetAttribute(&b, cudaDevAttrL2CacheSize, dev);
+        if (b <= 0) b = 50 << 20;
+    }
+    return b;
 }
 
-template <bool F16>
-static void launch_gemm_scores(const CUtensorMap (&m)[4], const float* inv, int M, int N, int K, float* C, int ldc,
-                               cudaStream_t st) {
+// query tiles per band of the tile order: the band's hi + lo query operand takes about a third of L2, which leaves
+// room for the column tiles in flight (the CTAs of one wave share them) and for what else the stream keeps there
+static int tile_band(int M, int K, int elem_bytes) {
+    const int tiles_m = (M + T_BM - 1) / T_BM;
+    const size_t a_tile = (size_t)T_BM * K * elem_bytes * 2;
+    const size_t band = (size_t)device_l2_bytes() / 3 / a_tile;
+    return (int)std::max<size_t>(1, std::min<size_t>(band, (size_t)tiles_m));
+}
+
+// FUSED: cand / xbound (C unused); else C (cand / xbound unused)
+template <bool F16, bool FUSED>
+static void launch_gemm(const CUtensorMap (&m)[4], const float* inv, int M, int N, int K, float* C, int ldc,
+                        unsigned col_base, u64* cand, unsigned* xbound, cudaStream_t st) {
     static PerDeviceSize configured;
     if (configured.raise(T_SMEM))
-        cudaFuncSetAttribute(gemm_ip_tc_kernel<F16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, T_SMEM);
-    dim3 grid((N + T_BN - 1) / T_BN, (M + T_BM - 1) / T_BM);
-    gemm_ip_tc_kernel<F16, false><<<grid, T_THREADS, T_SMEM, st>>>(m[0], m[1], m[2], m[3], inv, C, ldc, nullptr, nullptr,
-                                                                   M, N, K, 0u, 0);
+        cudaFuncSetAttribute(gemm_ip_tc_kernel<F16, FUSED>, cudaFuncAttributeMaxDynamicSharedMemorySize, T_SMEM);
+    const int ntiles = ((M + T_BM - 1) / T_BM) * ((N + T_BN - 1) / T_BN);
+    const int grid = std::min(ntiles, device_num_sms());     // one CTA per SM (shared memory), persistent
+    gemm_ip_tc_kernel<F16, FUSED><<<grid, T_THREADS, T_SMEM, st>>>(m[0], m[1], m[2], m[3], inv, C, ldc, cand, xbound, M, N,
+                                                                   K, col_base, tile_band(M, K, F16 ? 2 : 4));
 }
 
 // Ah/Al [M,K], Bh/Bl [N,K] fp32 (already split).  cand [M, fused_cand_per_row(N)] u64 keys (score order high word,
@@ -322,7 +392,7 @@ bool launch_gemm_tf32x3_topt(const float* Ah, const float* Al, int M, const floa
     if (K % T_BK) return false;
     CUtensorMap m[4];
     if (!make_maps(m, Ah, Al, M, Bh, Bl, N, K)) return false;
-    launch_gemm_topt<false>(m, nullptr, M, N, K, col_base, cand, xbound, st);
+    launch_gemm<false, true>(m, nullptr, M, N, K, nullptr, 0, col_base, cand, xbound, st);
     return true;
 }
 
@@ -336,7 +406,7 @@ bool launch_gemm_tf32x3(const float* Ah, const float* Al, int M, const float* Bh
     if (K % T_BK) return false;
     CUtensorMap m[4];
     if (!make_maps(m, Ah, Al, M, Bh, Bl, N, K)) return false;
-    launch_gemm_scores<false>(m, nullptr, M, N, K, C, ldc, st);
+    launch_gemm<false, false>(m, nullptr, M, N, K, C, ldc, 0u, nullptr, nullptr, st);
     return true;
 }
 
@@ -356,7 +426,7 @@ bool launch_gemm_f16x2(const void* Ah, const void* Al, const float* inv, int M, 
     if (K % T_BK16) return false;
     CUtensorMap m[4];
     if (!make_maps_f16(m, Ah, Al, M, B, N, K)) return false;
-    launch_gemm_scores<true>(m, inv, M, N, K, C, ldc, st);
+    launch_gemm<true, false>(m, inv, M, N, K, C, ldc, 0u, nullptr, nullptr, st);
     return true;
 }
 
@@ -366,7 +436,7 @@ bool launch_gemm_f16x2_topt(const void* Ah, const void* Al, const float* inv, in
     if (K % T_BK16) return false;
     CUtensorMap m[4];
     if (!make_maps_f16(m, Ah, Al, M, B, N, K)) return false;
-    launch_gemm_topt<true>(m, inv, M, N, K, col_base, cand, xbound, st);
+    launch_gemm<true, true>(m, inv, M, N, K, nullptr, 0, col_base, cand, xbound, st);
     return true;
 }
 
