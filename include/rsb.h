@@ -447,7 +447,10 @@ int rsb_bert_attention(rsb_bert_t* h, const void* qkv_dev, const int32_t* cu_seq
                        void* ctx_dev, rsb_stream_t stream);
 /* the encoder's tensor-core GEMM on its own: C[M,N] = A[M,K] . W[N,K]^T + bias (epilogue 0), GELU (1),
  * + residual (2) or ReLU (3); all fp16 row-major device pointers, N % 128 == 0, K % 64 == 0.  OR-ing
- * RSB_GEMM_REVERSED into the epilogue visits the 128-row tiles last-to-first, the order of the forward's FFN2. */
+ * RSB_GEMM_REVERSED into the epilogue visits the 128-row tiles last-to-first, the order of the forward's FFN2.
+ * C_dev may be residual_dev itself (the residual add in place, as the reader's o_proj and down_proj run it): each
+ * element's residual is loaded by the thread that stores that element, before the store.  A_dev and W_dev must not
+ * overlap C_dev. */
 enum { RSB_GEMM_REVERSED = 256 };
 int rsb_gemm_f16(const void* A_dev, const void* W_dev, const void* bias_dev, const void* residual_dev, void* C_dev,
                  int M, int N, int K, int epilogue, rsb_stream_t stream);
@@ -477,6 +480,20 @@ size_t rsb_llm_workspace_bytes(rsb_llm_t* h, int total_tokens, int label_tokens)
 int rsb_llm_nll(rsb_llm_t* h, const int32_t* ids_dev, const int32_t* cu_seqlens_dev, int B, int T, int max_seqlen,
                 const int32_t* labels_dev, float* nll_out_dev, void* ws_dev, size_t ws_bytes, rsb_stream_t stream);
 int rsb_llm_free(rsb_llm_t* h);
+/* Diagnostic, not used on the product path: one attention step of rsb_llm_nll on a caller's tensors, with the forward's
+ * own work list.  qkv_dev [T, (heads + 2 kv_heads) 128] fp16 holds each token's Q | K | V heads; RoPE is applied to its
+ * Q and K heads in place (positions restart at 0 in every window), then ctx_dev [T, heads 128] fp16 receives causal
+ * softmax(q k^T / sqrt(128)) v per window and query head h, which reads KV head h / (heads / kv_heads).  Windows may be
+ * empty and cu_seqlens_dev [B+1] may end below T: rows of empty windows and rows at or past cu_seqlens[B] are neither
+ * rotated nor written.  The offset refusals of rsb_llm_nll apply (RSB_ERR_INVALID / RSB_ERR_UNSUPPORTED before any
+ * launch); no weight needs to be loaded. */
+int rsb_llm_attention(rsb_llm_t* h, void* qkv_dev, const int32_t* cu_seqlens_dev, int B, int T, int max_seqlen,
+                      void* ctx_dev, rsb_stream_t stream);
+/* Diagnostic, not used on the product path: the residual stream after the last decoder layer of rsb_llm_nll's forward,
+ * before the final norm, out_dev [T, hidden] fp16.  The refusals of rsb_llm_nll apply; the workspace is
+ * rsb_llm_workspace_bytes(h, T, 0). */
+int rsb_llm_hidden_states(rsb_llm_t* h, const int32_t* ids_dev, const int32_t* cu_seqlens_dev, int B, int T,
+                          int max_seqlen, void* out_dev, void* ws_dev, size_t ws_bytes, rsb_stream_t stream);
 
 /* ---- MinHash de-duplication of retrieved passages ----------------------------------------------------------------
  * Replaces utils/deduplication.py's `remove_duplicates_with_minhash` (datasketch MinHash(num_perm=128) and

@@ -96,6 +96,9 @@ SIGNATURES = [
     ("rsb_llm_workspace_bytes", c_size_t, [_H, c_int, c_int]),
     ("rsb_llm_nll", c_int, [_H, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     ("rsb_llm_free", c_int, [_H]),
+    ("rsb_llm_attention", c_int, [_H, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),   # diagnostic
+    ("rsb_llm_hidden_states", c_int, [_H, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t,
+                                      c_void_p]),                                                   # diagnostic
     ("rsb_dedup_last_error", c_char_p, []),
     ("rsb_minhash_workspace_bytes", c_size_t, [c_int64]),
     ("rsb_minhash_signatures", c_int, [c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,

@@ -511,6 +511,104 @@ extern "C" size_t rsb_llm_workspace_bytes(rsb_llm_t* h, int total_tokens, int la
     return llm_ws_layout(h, (size_t)std::max(total_tokens, 1), (size_t)label_tokens, off);
 }
 
+namespace {
+
+// Checks offsets read back from the device: 0 = cu[0] <= cu[1] <= ... <= cu[B] <= T, every window <= max_seqlen tokens.
+int check_offsets(const std::vector<int32_t>& cu, int B, int T, int max_seqlen) {
+    if (cu[0] != 0 || cu[B] > T) return lfail(RSB_ERR_INVALID, "cu_seqlens must run from 0 to at most T (T = %ld)", (long)T);
+    for (int b = 0; b < B; ++b) {
+        const int S = cu[b + 1] - cu[b];
+        if (S < 0) return lfail(RSB_ERR_INVALID, "cu_seqlens decreases at sequence %ld", (long)b);
+        if (S > max_seqlen) return lfail(RSB_ERR_INVALID, "a sequence of %ld tokens is longer than max_seqlen", (long)S);
+    }
+    return RSB_OK;
+}
+
+// The attention work list: one item (sequence b, query block q) per 64 queries of every window, heaviest query blocks
+// first (block q of a sequence visits q + 1 key blocks), uploaded to d_items (room for cu[B] items).
+int upload_attention_items(const std::vector<int32_t>& cu, int B, int2* d_items, cudaStream_t st, int* n_items) {
+    std::vector<int2> items;
+    for (int b = 0; b < B; ++b)
+        for (int q = 0; q * AQ < cu[b + 1] - cu[b]; ++q) items.push_back(make_int2(b, q));
+    std::stable_sort(items.begin(), items.end(), [](const int2& a, const int2& b) { return a.y > b.y; });
+    *n_items = (int)items.size();
+    if (!items.empty() &&
+        cudaMemcpyAsync(d_items, items.data(), items.size() * sizeof(int2), cudaMemcpyHostToDevice, st) != cudaSuccess)
+        return lfail(RSB_ERR_CUDA, "uploading the attention work list failed");
+    return RSB_OK;
+}
+
+// One attention step on the fused QKV rows [n_tok, qkv_n] of a batch whose windows end at n_tok = cu[B]: RoPE on the
+// Q and K heads in place, then causal attention into CTX [n_tok, hidden].
+void attention_step(const rsb_llm* h, __half* QKV, const int32_t* cu_seqlens, int B, int n_tok, const int2* d_items,
+                    int n_items, __half* CTX, cudaStream_t st) {
+    if (n_tok == 0 || n_items == 0) return;
+    const float scale_log2 = 1.4426950408889634f / sqrtf((float)HD);   // 1/sqrt(128) in the log2 domain
+    rope_kernel<<<n_tok, 256, 0, st>>>(QKV, cu_seqlens, B, h->qkv_n(), h->heads + h->kv_heads, h->inv_freq);
+    attention_causal_kernel<<<dim3((unsigned)n_items, h->heads), 128, 0, st>>>(QKV, cu_seqlens, d_items, CTX, h->heads,
+                                                                               h->kv_heads, scale_log2);
+}
+
+// Refusals shared by rsb_llm_nll and rsb_llm_hidden_states, then the read-back of the offsets and ids (and labels).
+int check_forward(rsb_llm* h, const int32_t* ids, const int32_t* cu_seqlens, const int32_t* labels, int B, int T,
+                  int max_seqlen, cudaStream_t st, std::vector<int32_t>& cu, std::vector<int32_t>& lab) {
+    if (B <= 0 || T <= 0) return lfail(RSB_ERR_INVALID, "empty batch");
+    if (max_seqlen > h->max_pos)
+        return lfail(RSB_ERR_UNSUPPORTED, "sequence longer than max_position_embeddings (%ld)", (long)h->max_pos);
+    if (h->loaded.size() != h->required())
+        return lfail(RSB_ERR_STATE, "%ld reader weights are not loaded", (long)(h->required() - h->loaded.size()));
+    std::vector<int32_t> hid(T);
+    cu.assign(B + 1, 0);
+    lab.assign(labels ? T : 0, 0);
+    if (cudaMemcpyAsync(cu.data(), cu_seqlens, cu.size() * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+        cudaMemcpyAsync(hid.data(), ids, (size_t)T * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+        (labels && cudaMemcpyAsync(lab.data(), labels, (size_t)T * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess) ||
+        cudaStreamSynchronize(st) != cudaSuccess)
+        return lfail(RSB_ERR_CUDA, "reading back the batch failed");
+    if (cu[0] != 0 || cu[B] != T) return lfail(RSB_ERR_INVALID, "cu_seqlens must run from 0 to T (T = %ld)", (long)T);
+    const int rc = check_offsets(cu, B, T, max_seqlen);
+    if (rc != RSB_OK) return rc;
+    for (int t = 0; t < T; ++t) {
+        if (hid[t] < 0 || hid[t] >= h->vocab) return lfail(RSB_ERR_INVALID, "token id %ld is outside the vocabulary", (long)hid[t]);
+        if (labels && lab[t] != -100 && (lab[t] < 0 || lab[t] >= h->vocab))
+            return lfail(RSB_ERR_INVALID, "label %ld is neither -100 nor a token id", (long)lab[t]);
+    }
+    return RSB_OK;
+}
+
+// The decoder layers: X (workspace slot 0) ends as the residual stream after the last layer, before the final norm.
+int trunk(rsb_llm* h, const int32_t* ids, const int32_t* cu_seqlens, int B, int T, const std::vector<int32_t>& cu,
+          unsigned char* w, const size_t off[10], cudaStream_t st) {
+    __half* X = reinterpret_cast<__half*>(w + off[0]);
+    __half* Hn = reinterpret_cast<__half*>(w + off[1]);
+    __half* QKV = reinterpret_cast<__half*>(w + off[2]);
+    __half* CTX = reinterpret_cast<__half*>(w + off[3]);
+    __half* GU = reinterpret_cast<__half*>(w + off[4]);
+    __half* ACT = reinterpret_cast<__half*>(w + off[5]);
+    int2* d_items = reinterpret_cast<int2*>(w + off[8]);
+    int n_items, rc;
+    if ((rc = upload_attention_items(cu, B, d_items, st, &n_items)) != RSB_OK) return rc;
+
+    const int Hd = h->hidden, NQKV = h->qkv_n(), I = h->inter;
+    const long long n8 = (long long)T * I / 8;
+    const int sw_grid = (int)std::min<long long>((n8 + 255) / 256, 8LL * rsb::device_num_sms());
+    embed_rows_kernel<<<T, 128, 0, st>>>(ids, h->embed, Hd, X);
+    for (int li = 0; li < h->layers; ++li) {
+        const LlmLayer& l = h->L[li];
+        rms_rows_kernel<<<T, 256, 0, st>>>(X, nullptr, Hd, l.ln1, h->eps, Hn);
+        if ((rc = gemm(Hn, T, l.wqkv, NQKV, Hd, h->zero_bias, nullptr, QKV, 0, st)) != RSB_OK) return rc;
+        attention_step(h, QKV, cu_seqlens, B, T, d_items, n_items, CTX, st);
+        if ((rc = gemm(CTX, T, l.wo, Hd, Hd, h->zero_bias, X, X, 2, st)) != RSB_OK) return rc;
+        rms_rows_kernel<<<T, 256, 0, st>>>(X, nullptr, Hd, l.ln2, h->eps, Hn);
+        if ((rc = gemm(Hn, T, l.wgu, 2 * I, Hd, h->zero_bias, nullptr, GU, 0, st)) != RSB_OK) return rc;
+        swiglu_kernel<<<sw_grid, 256, 0, st>>>(GU, n8, I, ACT);
+        if ((rc = gemm(ACT, T, l.wdown, Hd, I, h->zero_bias, X, X, 2 | RSB_GEMM_REVERSED, st)) != RSB_OK) return rc;
+    }
+    return RSB_OK;
+}
+
+}  // namespace
+
 // The reader forward and loss of src/evaluate_perplexity.py:126-134 (`lm(input_ids, labels=labels)` per window) over B
 // packed windows.  ids / labels [T] int32 and cu_seqlens [B+1] int32 on the device; nll_out [T] fp32 receives, at
 // every position t that is not the first of its sequence and whose label is not -100, -log p(labels[t] | ids of the
@@ -518,36 +616,14 @@ extern "C" size_t rsb_llm_workspace_bytes(rsb_llm_t* h, int total_tokens, int la
 extern "C" int rsb_llm_nll(rsb_llm_t* h, const int32_t* ids, const int32_t* cu_seqlens, int B, int T, int max_seqlen,
                            const int32_t* labels, float* nll_out, void* ws, size_t ws_bytes, rsb_stream_t stream) {
     if (!h || !ids || !cu_seqlens || !labels || !nll_out || !ws) return lfail(RSB_ERR_INVALID, "null argument");
-    if (B <= 0 || T <= 0) return lfail(RSB_ERR_INVALID, "empty batch");
-    if (max_seqlen > h->max_pos)
-        return lfail(RSB_ERR_UNSUPPORTED, "sequence longer than max_position_embeddings (%ld)", (long)h->max_pos);
-    if (h->loaded.size() != h->required())
-        return lfail(RSB_ERR_STATE, "%ld reader weights are not loaded", (long)(h->required() - h->loaded.size()));
     cudaStream_t st = (cudaStream_t)stream;
-    std::vector<int32_t> cu(B + 1), hid(T), lab(T);
-    if (cudaMemcpyAsync(cu.data(), cu_seqlens, cu.size() * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-        cudaMemcpyAsync(hid.data(), ids, (size_t)T * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-        cudaMemcpyAsync(lab.data(), labels, (size_t)T * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-        cudaStreamSynchronize(st) != cudaSuccess)
-        return lfail(RSB_ERR_CUDA, "reading back the batch failed");
-    if (cu[0] != 0 || cu[B] != T) return lfail(RSB_ERR_INVALID, "cu_seqlens must run from 0 to T (T = %ld)", (long)T);
+    std::vector<int32_t> cu, lab;
+    int rc = check_forward(h, ids, cu_seqlens, labels, B, T, max_seqlen, st, cu, lab);
+    if (rc != RSB_OK) return rc;
     std::vector<int32_t> rows, labs, outi;
-    std::vector<int2> items;
-    for (int b = 0; b < B; ++b) {
-        const int S = cu[b + 1] - cu[b];
-        if (S < 0) return lfail(RSB_ERR_INVALID, "cu_seqlens decreases at sequence %ld", (long)b);
-        if (S > max_seqlen) return lfail(RSB_ERR_INVALID, "a sequence of %ld tokens is longer than max_seqlen", (long)S);
-        for (int q = 0; q * AQ < S; ++q) items.push_back(make_int2(b, q));
+    for (int b = 0; b < B; ++b)
         for (int t = cu[b] + 1; t < cu[b + 1]; ++t)
             if (lab[t] != -100) { rows.push_back(t - 1); labs.push_back(lab[t]); outi.push_back(t); }
-    }
-    for (int t = 0; t < T; ++t) {
-        if (hid[t] < 0 || hid[t] >= h->vocab) return lfail(RSB_ERR_INVALID, "token id %ld is outside the vocabulary", (long)hid[t]);
-        if (lab[t] != -100 && (lab[t] < 0 || lab[t] >= h->vocab))
-            return lfail(RSB_ERR_INVALID, "label %ld is neither -100 nor a token id", (long)lab[t]);
-    }
-    // heaviest query blocks first: block q of a sequence visits q + 1 key blocks
-    std::stable_sort(items.begin(), items.end(), [](const int2& a, const int2& b) { return a.y > b.y; });
     const int nl = (int)rows.size();
     size_t off[10];
     const size_t need = llm_ws_layout(h, (size_t)T, (size_t)nl, off);
@@ -555,44 +631,19 @@ extern "C" int rsb_llm_nll(rsb_llm_t* h, const int32_t* ids, const int32_t* cu_s
     unsigned char* w = static_cast<unsigned char*>(ws);
     __half* X = reinterpret_cast<__half*>(w + off[0]);
     __half* Hn = reinterpret_cast<__half*>(w + off[1]);
-    __half* QKV = reinterpret_cast<__half*>(w + off[2]);
-    __half* CTX = reinterpret_cast<__half*>(w + off[3]);
-    __half* GU = reinterpret_cast<__half*>(w + off[4]);
-    __half* ACT = reinterpret_cast<__half*>(w + off[5]);
     __half* LOG = reinterpret_cast<__half*>(w + off[6]);
     int* d_rows = reinterpret_cast<int*>(w + off[7]);
     int* d_labs = d_rows + nl;
     int* d_outi = d_labs + nl;
-    int2* d_items = reinterpret_cast<int2*>(w + off[8]);
     if (nl > 0 && (cudaMemcpyAsync(d_rows, rows.data(), (size_t)nl * 4, cudaMemcpyHostToDevice, st) != cudaSuccess ||
                    cudaMemcpyAsync(d_labs, labs.data(), (size_t)nl * 4, cudaMemcpyHostToDevice, st) != cudaSuccess ||
                    cudaMemcpyAsync(d_outi, outi.data(), (size_t)nl * 4, cudaMemcpyHostToDevice, st) != cudaSuccess))
         return lfail(RSB_ERR_CUDA, "uploading the label rows failed");
-    if (cudaMemcpyAsync(d_items, items.data(), items.size() * sizeof(int2), cudaMemcpyHostToDevice, st) != cudaSuccess ||
-        cudaMemsetAsync(nll_out, 0, (size_t)T * sizeof(float), st) != cudaSuccess)
-        return lfail(RSB_ERR_CUDA, "uploading the attention work list failed");
-
-    const int Hd = h->hidden, NQKV = h->qkv_n(), I = h->inter;
-    const float scale_log2 = 1.4426950408889634f / sqrtf((float)HD);   // 1/sqrt(128) in the log2 domain
-    const long long n8 = (long long)T * I / 8;
-    const int sw_grid = (int)std::min<long long>((n8 + 255) / 256, 8LL * rsb::device_num_sms());
-    embed_rows_kernel<<<T, 128, 0, st>>>(ids, h->embed, Hd, X);
-    int rc;
-    for (int li = 0; li < h->layers; ++li) {
-        const LlmLayer& l = h->L[li];
-        rms_rows_kernel<<<T, 256, 0, st>>>(X, nullptr, Hd, l.ln1, h->eps, Hn);
-        if ((rc = gemm(Hn, T, l.wqkv, NQKV, Hd, h->zero_bias, nullptr, QKV, 0, st)) != RSB_OK) return rc;
-        rope_kernel<<<T, 256, 0, st>>>(QKV, cu_seqlens, B, NQKV, h->heads + h->kv_heads, h->inv_freq);
-        attention_causal_kernel<<<dim3((unsigned)items.size(), h->heads), 128, 0, st>>>(QKV, cu_seqlens, d_items, CTX,
-                                                                                        h->heads, h->kv_heads, scale_log2);
-        if ((rc = gemm(CTX, T, l.wo, Hd, Hd, h->zero_bias, X, X, 2, st)) != RSB_OK) return rc;
-        rms_rows_kernel<<<T, 256, 0, st>>>(X, nullptr, Hd, l.ln2, h->eps, Hn);
-        if ((rc = gemm(Hn, T, l.wgu, 2 * I, Hd, h->zero_bias, nullptr, GU, 0, st)) != RSB_OK) return rc;
-        swiglu_kernel<<<sw_grid, 256, 0, st>>>(GU, n8, I, ACT);
-        if ((rc = gemm(ACT, T, l.wdown, Hd, I, h->zero_bias, X, X, 2 | RSB_GEMM_REVERSED, st)) != RSB_OK) return rc;
-    }
+    if (cudaMemsetAsync(nll_out, 0, (size_t)T * sizeof(float), st) != cudaSuccess)
+        return lfail(RSB_ERR_CUDA, "clearing nll_out failed");
+    if ((rc = trunk(h, ids, cu_seqlens, B, T, cu, w, off, st)) != RSB_OK) return rc;
     // final norm and LM head on the label rows only, in chunks that bound the logits workspace
-    const int chunk = h->chunk_rows();
+    const int Hd = h->hidden, chunk = h->chunk_rows();
     for (int c0 = 0; c0 < nl; c0 += chunk) {
         const int n = std::min(chunk, nl - c0);
         rms_rows_kernel<<<n, 256, 0, st>>>(X, d_rows + c0, Hd, h->final_g, h->eps, Hn);
@@ -601,5 +652,53 @@ extern "C" int rsb_llm_nll(rsb_llm_t* h, const int32_t* ids, const int32_t* cu_s
     }
     const cudaError_t e = cudaPeekAtLastError();
     if (e != cudaSuccess) return lfail(RSB_ERR_CUDA, "reader launch failed: %s", cudaGetErrorString(e));
+    return RSB_OK;
+}
+
+// Diagnostic: the residual stream after the last layer (before the final norm) of the same forward, [T, hidden] fp16.
+extern "C" int rsb_llm_hidden_states(rsb_llm_t* h, const int32_t* ids, const int32_t* cu_seqlens, int B, int T,
+                                     int max_seqlen, void* out, void* ws, size_t ws_bytes, rsb_stream_t stream) {
+    if (!h || !ids || !cu_seqlens || !out || !ws) return lfail(RSB_ERR_INVALID, "null argument");
+    cudaStream_t st = (cudaStream_t)stream;
+    std::vector<int32_t> cu, lab;
+    int rc = check_forward(h, ids, cu_seqlens, nullptr, B, T, max_seqlen, st, cu, lab);
+    if (rc != RSB_OK) return rc;
+    size_t off[10];
+    const size_t need = llm_ws_layout(h, (size_t)T, 0, off);
+    if (ws_bytes < need) return lfail(RSB_ERR_OOM, "reader workspace too small (need %ld bytes)", (long)need);
+    unsigned char* w = static_cast<unsigned char*>(ws);
+    if ((rc = trunk(h, ids, cu_seqlens, B, T, cu, w, off, st)) != RSB_OK) return rc;
+    if (cudaMemcpyAsync(out, w + off[0], (size_t)T * h->hidden * 2, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
+        return lfail(RSB_ERR_CUDA, "copying the hidden states failed");
+    const cudaError_t e = cudaPeekAtLastError();
+    if (e != cudaSuccess) return lfail(RSB_ERR_CUDA, "reader launch failed: %s", cudaGetErrorString(e));
+    return RSB_OK;
+}
+
+// Diagnostic: one attention step of the forward on a caller's fused QKV rows [T, (heads + 2 kv_heads) 128] fp16.
+extern "C" int rsb_llm_attention(rsb_llm_t* h, void* qkv, const int32_t* cu_seqlens, int B, int T, int max_seqlen,
+                                 void* ctx, rsb_stream_t stream) {
+    if (!h || !qkv || !cu_seqlens || !ctx) return lfail(RSB_ERR_INVALID, "null argument");
+    if (B <= 0 || T <= 0) return lfail(RSB_ERR_INVALID, "empty batch");
+    if (max_seqlen > h->max_pos)
+        return lfail(RSB_ERR_UNSUPPORTED, "sequence longer than max_position_embeddings (%ld)", (long)h->max_pos);
+    cudaStream_t st = (cudaStream_t)stream;
+    std::vector<int32_t> cu(B + 1);
+    if (cudaMemcpyAsync(cu.data(), cu_seqlens, cu.size() * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+        cudaStreamSynchronize(st) != cudaSuccess)
+        return lfail(RSB_ERR_CUDA, "reading back cu_seqlens failed");
+    int rc = check_offsets(cu, B, T, max_seqlen);
+    if (rc != RSB_OK) return rc;
+    int2* d_items = nullptr;
+    if (cu[B] > 0 && cudaMallocAsync(&d_items, (size_t)cu[B] * sizeof(int2), st) != cudaSuccess)
+        return lfail(RSB_ERR_OOM, "allocating the attention work list failed");
+    int n_items = 0;
+    rc = upload_attention_items(cu, B, d_items, st, &n_items);
+    if (rc == RSB_OK)
+        attention_step(h, static_cast<__half*>(qkv), cu_seqlens, B, cu[B], d_items, n_items, static_cast<__half*>(ctx), st);
+    if (d_items) cudaFreeAsync(d_items, st);
+    if (rc != RSB_OK) return rc;
+    const cudaError_t e = cudaPeekAtLastError();
+    if (e != cudaSuccess) return lfail(RSB_ERR_CUDA, "attention launch failed: %s", cudaGetErrorString(e));
     return RSB_OK;
 }

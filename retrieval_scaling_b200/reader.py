@@ -225,6 +225,33 @@ class B200Llama:
             i = j
         return out
 
+    # -- diagnostics (rsb_llm_attention / rsb_llm_hidden_states), not used by nll / loss ----------------------------
+    def attention(self, qkv: torch.Tensor, cu_seqlens: torch.Tensor, max_seqlen: int, ctx: torch.Tensor):
+        """One attention step of the forward: RoPE in place on the Q / K heads of qkv [T, (heads + 2 kv_heads) 128]
+        fp16, then causal attention into ctx [T, hidden] fp16 for the windows of cu_seqlens (int32 [B + 1], empty
+        windows allowed, may end below T).  Rows outside the windows are left as they are."""
+        with torch.cuda.device(self.device):
+            rc = self.L.rsb_llm_attention(self._h, ctypes.c_void_p(qkv.data_ptr()), ctypes.c_void_p(cu_seqlens.data_ptr()),
+                                          cu_seqlens.numel() - 1, qkv.shape[0], int(max_seqlen),
+                                          ctypes.c_void_p(ctx.data_ptr()),
+                                          ctypes.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
+        self._check(rc)
+
+    def hidden_states(self, ids: torch.Tensor, cu_seqlens: torch.Tensor, max_seqlen: int) -> torch.Tensor:
+        """The residual stream after the last layer, before the final norm: [T, hidden] fp16 for the packed int32 ids
+        [T] and cu_seqlens [B + 1] on the device."""
+        T = ids.numel()
+        out = torch.empty((T, self.geom["hidden_size"]), dtype=torch.float16, device=self.device)
+        ws = torch.empty(self.L.rsb_llm_workspace_bytes(self._h, T, 0), dtype=torch.uint8, device=self.device)
+        with torch.cuda.device(self.device):
+            rc = self.L.rsb_llm_hidden_states(self._h, ctypes.c_void_p(ids.data_ptr()),
+                                              ctypes.c_void_p(cu_seqlens.data_ptr()), cu_seqlens.numel() - 1, T,
+                                              int(max_seqlen), ctypes.c_void_p(out.data_ptr()),
+                                              ctypes.c_void_p(ws.data_ptr()), ws.numel(),
+                                              ctypes.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
+        self._check(rc)
+        return out
+
     def loss(self, input_ids_list, labels_list, max_tokens: Optional[int] = None) -> List[float]:
         """`lm(input_ids, labels=labels).loss` per window: the mean NLL over the scored positions, NaN for a window
         without any (HF's mean over zero tokens)."""

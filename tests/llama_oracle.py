@@ -24,16 +24,18 @@ def _rotate_half(x):
     return torch.cat((-x[..., h:], x[..., :h]), dim=-1)
 
 
-def token_nll(sd, cfg, ids) -> np.ndarray:
-    """nll[t] = -log p(ids[t] | ids[:t]) in fp64 for one window, 0 at t = 0."""
-    W = {k: v.double() for k, v in sd.items()}
+def hidden_rows(sd, cfg, ids, device="cpu"):
+    """[x_0, x_1, ..., x_L] float64 [S, hidden] on `device` for one window: the embedding rows and the residual stream
+    after each decoder layer (x_L is the input of the final norm)."""
+    W = {k: v.to(device=device, dtype=torch.float64) for k, v in sd.items()}
     H, nh, nkv = cfg["hidden_size"], cfg["num_attention_heads"], cfg["num_key_value_heads"]
     eps, d = cfg["rms_norm_eps"], 128
-    ids = torch.as_tensor(np.asarray(ids), dtype=torch.long)
+    ids = torch.as_tensor(np.asarray(ids), dtype=torch.long, device=device)
     S = len(ids)
     x = W["model.embed_tokens.weight"][ids]
-    cos, sin = rope_tables(S, cfg["rope_theta"])
-    mask = torch.full((S, S), -torch.inf, dtype=torch.float64).triu(1)
+    cos, sin = (t.to(device) for t in rope_tables(S, cfg["rope_theta"]))
+    mask = torch.full((S, S), -torch.inf, dtype=torch.float64, device=device).triu(1)
+    out = [x]
     for i in range(cfg["num_hidden_layers"]):
         p = f"model.layers.{i}."
         h = _rms(x, W[p + "input_layernorm.weight"], eps)
@@ -49,12 +51,22 @@ def token_nll(sd, cfg, ids) -> np.ndarray:
         h = _rms(x, W[p + "post_attention_layernorm.weight"], eps)
         g = h @ W[p + "mlp.gate_proj.weight"].T
         x = x + (torch.nn.functional.silu(g) * (h @ W[p + "mlp.up_proj.weight"].T)) @ W[p + "mlp.down_proj.weight"].T
-    x = _rms(x, W["model.norm.weight"], eps)
-    head = W["model.embed_tokens.weight"] if cfg.get("tie_word_embeddings") else W["lm_head.weight"]
-    lp = torch.log_softmax(x @ head.T, dim=-1)
+        out.append(x)
+    return out
+
+
+def token_nll(sd, cfg, ids, device="cpu") -> np.ndarray:
+    """nll[t] = -log p(ids[t] | ids[:t]) in fp64 for one window, 0 at t = 0; the forward runs on `device`."""
+    x = hidden_rows(sd, cfg, ids, device)[-1]
+    eps = cfg["rms_norm_eps"]
+    x = _rms(x, sd["model.norm.weight"].to(device=device, dtype=torch.float64), eps)
+    head = sd["model.embed_tokens.weight"] if cfg.get("tie_word_embeddings") else sd["lm_head.weight"]
+    lp = torch.log_softmax(x @ head.to(device=device, dtype=torch.float64).T, dim=-1)
+    ids = torch.as_tensor(np.asarray(ids), dtype=torch.long, device=device)
+    S = len(ids)
     out = np.zeros(S, np.float64)
     if S > 1:
-        out[1:] = (-lp[:-1].gather(1, ids[1:, None]).squeeze(1)).numpy()
+        out[1:] = (-lp[:-1].gather(1, ids[1:, None]).squeeze(1)).cpu().numpy()
     return out
 
 

@@ -219,9 +219,16 @@ def test_attention_refusals_that_need_a_handle():
 # ---------------------------------------------------------------------------------------------------------------
 GEMM_M = [1, 2, 63, 64, 65, 127, 128, 129, 255, 256, 257, 4097, 41000, 262144]
 GEMM_NK = [(2304, 768), (768, 768), (3072, 768), (768, 3072), (128, 64), (128, 128), (2304, 3072), (3072, 64)]
+# the reader's (N, K) at Llama-2-7B / Llama-3-8B / Llama-2-13B width, each at a small or partial M: q|k|v (MHA, GQA
+# 32:8), gate|up, down, LM head (Llama-2, Llama-3)
+READER_NK = [(12288, 4096), (6144, 4096), (22016, 4096), (28672, 4096), (27648, 5120), (4096, 11008), (4096, 14336),
+             (5120, 13824), (32000, 4096), (128256, 4096)]
+READER_M = [1, 65, 129, 7, 200, 255, 1, 63, 129, 130]
 
 
 def _gemm_nk(i, M):
+    if i >= len(GEMM_M):
+        return READER_NK[i - len(GEMM_M)]
     if M == 262144:
         return 768, 3072                                    # FFN2 of 512 passages x 512 tokens
     if M == 41000:
@@ -229,17 +236,19 @@ def _gemm_nk(i, M):
     return GEMM_NK[i % len(GEMM_NK)]
 
 
-@pytest.mark.parametrize("i,M", list(enumerate(GEMM_M)))
+@pytest.mark.parametrize("i,M", list(enumerate(GEMM_M)) + [(len(GEMM_M) + j, M) for j, M in enumerate(READER_M)])
 def test_gemm_per_element_bound(i, M):
     """rsb_gemm_f16 for epilogues bias / GELU / residual / ReLU, each in both row-tile orders (RSB_GEMM_REVERSED is the
-    order FFN2 runs in), against fp64 of the same fp16 operands, per element:
+    order FFN2 runs in), and the residual epilogue in place (C == residual, as the reader's o_proj and down_proj run it)
+    in both orders, against fp64 of the same fp16 operands, per element:
         pre = A W^T + bias (fp64); e = 2 K 2^-24 (|A| |W|^T) + 2^-24 |pre|   (fp32 accumulation with truncation, the
                                                                           fp32 bias add)
         bias / ReLU:  |out - f(pre)| <= e + 1/2 ulp(f(pre) + e)
         GELU:         |out - gelu(pre)| <= 1.13 e + 1.5 ulp(gelu(pre) + 1.13 e)   (|gelu'| <= 1.13; the kernel's
                                                                           restated GELU is within 1 ulp of erf's)
         residual:     |out - (pre + r)| <= e + 1/2 ulp(pre + e) + 1/2 ulp(pre + r + 2e)   (rounded, then added in half)
-    Large M is compared in row chunks.  The comparison must reject the reference shifted by one row."""
+    The encoder's shapes and the reader's (N, K) at small and partial M.  Large M is compared in row chunks, the fp64
+    product once per chunk for every epilogue.  The comparison must reject the reference shifted by one row."""
     from retrieval_scaling_b200 import _lib
     N, K = _gemm_nk(i, M)
     g = torch.Generator(device="cuda").manual_seed(1000 + i)
@@ -247,44 +256,57 @@ def test_gemm_per_element_bound(i, M):
     W = (torch.randn(N, K, generator=g, device="cuda") * (1.0 / K ** 0.5)).half()
     b = (torch.randn(N, generator=g, device="cuda") * 0.1).half()
     R = (torch.randn(M, N, generator=g, device="cuda") * 0.5).half()
-    C = torch.empty((M, N), dtype=torch.float16, device="cuda")
-    chunk = max(1, (1 << 26) // max(N, K))
-    worst = 0.0
-    for epi in (0, 1, 2, 3):
+    outs = {}
+    for epi in (0, 1, 2, 3, "in_place"):
         for rev in (0, _lib.GEMM_REVERSED):
-            C.fill_(float("nan"))
+            if epi == "in_place":
+                C = R.clone()
+                res = C
+            else:
+                C = torch.full((M, N), float("nan"), dtype=torch.float16, device="cuda")
+                res = R
             rc = _L().rsb_gemm_f16(ctypes.c_void_p(A.data_ptr()), ctypes.c_void_p(W.data_ptr()), ctypes.c_void_p(b.data_ptr()),
-                                   ctypes.c_void_p(R.data_ptr()), ctypes.c_void_p(C.data_ptr()), M, N, K, epi | rev, _stream())
+                                   ctypes.c_void_p(res.data_ptr()), ctypes.c_void_p(C.data_ptr()), M, N, K,
+                                   (2 if epi == "in_place" else epi) | rev, _stream())
             assert rc == 0, _L().rsb_bert_last_error()
-            torch.cuda.synchronize()
-            Wd, bd = W.double(), b.double()
-            shifted_ok = True
-            for r0 in range(0, M, chunk):
-                r1 = min(M, r0 + chunk)
-                Ad = A[r0:r1].double()
-                pre = Ad @ Wd.T + bd
-                e = 2 * K * 2.0 ** -24 * (Ad.abs() @ Wd.abs().T) + 2.0 ** -24 * pre.abs()
-                if epi == 0:
-                    ref, bnd = pre, e + 0.5 * _ulp16(pre.abs() + e)
-                elif epi == 3:
-                    ref = pre.clamp_min(0)
-                    bnd = e + 0.5 * _ulp16(ref + e)
-                elif epi == 1:
-                    ref = F.gelu(pre)
-                    bnd = 1.13 * e + 1.5 * _ulp16(ref.abs() + 1.13 * e)
-                else:
-                    ref = pre + R[r0:r1].double()
-                    bnd = e + 0.5 * _ulp16(pre.abs() + e) + 0.5 * _ulp16(ref.abs() + 2 * e)
+            outs[(epi, rev)] = C
+    torch.cuda.synchronize()
+    chunk = max(1, (1 << 26) // max(N, K))
+    Wd, bd = W.double(), b.double()
+    Wa = Wd.abs()
+    worst = {}
+    shifted_ok = {key: True for key in outs}
+    for r0 in range(0, M, chunk):
+        r1 = min(M, r0 + chunk)
+        Ad = A[r0:r1].double()
+        pre = Ad @ Wd.T + bd
+        e = 2 * K * 2.0 ** -24 * (Ad.abs() @ Wa.T) + 2.0 ** -24 * pre.abs()
+        for epi in (0, 1, 2, 3):
+            if epi == 0:
+                ref, bnd = pre, e + 0.5 * _ulp16(pre.abs() + e)
+            elif epi == 3:
+                ref = pre.clamp_min(0)
+                bnd = e + 0.5 * _ulp16(ref + e)
+            elif epi == 1:
+                ref = F.gelu(pre)
+                bnd = 1.13 * e + 1.5 * _ulp16(ref.abs() + 1.13 * e)
+            else:
+                ref = pre + R[r0:r1].double()
+                bnd = e + 0.5 * _ulp16(pre.abs() + e) + 0.5 * _ulp16(ref.abs() + 2 * e)
+            for key, C in outs.items():
+                if (2 if key[0] == "in_place" else key[0]) != epi:
+                    continue
                 out = C[r0:r1].double()
-                err = (out - ref).abs()
-                assert torch.isfinite(out).all(), (epi, rev, r0)
-                ratio = (err / bnd).max().item()
-                worst = max(worst, ratio)
-                assert ratio <= 1.0, (M, N, K, epi, rev, r0, ratio)
+                assert torch.isfinite(out).all(), (key, r0)
+                ratio = ((out - ref).abs() / bnd).max().item()
+                worst[key[0]] = max(worst.get(key[0], 0.0), ratio)
+                assert ratio <= 1.0, (M, N, K, key, r0, ratio)
                 if r1 - r0 >= 2:
-                    shifted_ok &= bool(((out[1:] - ref[:-1]).abs() <= bnd[1:]).all().item())
-            if M >= 2:
-                _must_fail("reference shifted by one row", shifted_ok)
+                    shifted_ok[key] &= bool(((out[1:] - ref[:-1]).abs() <= bnd[1:]).all().item())
+    if M >= 2:
+        for key, ok in shifted_ok.items():
+            _must_fail(f"reference shifted by one row {key}", ok)
+    worst = max(worst.values())
     print(f"[gemm M={M} N={N} K={K}] max |err| / bound = {worst:.3f}")
 
 

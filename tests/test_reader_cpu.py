@@ -167,5 +167,8 @@ def test_llm_abi_refusals_need_no_device():
     p = ctypes.c_void_p(16)              # never dereferenced: the arguments are refused first
     assert L.rsb_llm_nll(None, p, p, 1, 1, 1, p, p, p, 1 << 20, None) == _lib.RSB_ERR_INVALID
     assert L.rsb_llm_load(None, b"model.norm.weight", p, 512, None) == _lib.RSB_ERR_INVALID
+    assert L.rsb_llm_attention(None, p, p, 1, 1, 1, p, None) == _lib.RSB_ERR_INVALID
+    assert L.rsb_llm_hidden_states(None, p, p, 1, 1, 1, p, p, 1 << 20, None) == _lib.RSB_ERR_INVALID
+    assert b"null" in L.rsb_llm_last_error()
     assert L.rsb_llm_workspace_bytes(None, 10, 10) == 0
     assert L.rsb_llm_free(None) == _lib.RSB_OK
