@@ -466,6 +466,26 @@ typedef struct rsb_llm rsb_llm_t;
 const char* rsb_llm_last_error(void);
 int rsb_llm_create(int layers, int hidden, int heads, int kv_heads, int intermediate, int vocab, int max_pos,
                    float rope_theta, float rms_eps, int tied, rsb_llm_t** out);
+/* GPT-NeoX readers (HF GPTNeoXForCausalLM: Pythia), a second constructor for the same handle type: heads = kv heads,
+ * head_dim = hidden / heads in {64, 80, 128, 256} (else RSB_ERR_UNSUPPORTED naming head_dim), hidden <= 8192 (the
+ * LayerNorm kernel's widest row, else RSB_ERR_UNSUPPORTED naming hidden; Pythia-12B has 5120), rotary_dims = HF's
+ * rotary_ndims, even and in [2, head_dim] (rotary_dims <= 0 or > head_dim RSB_ERR_INVALID, odd RSB_ERR_UNSUPPORTED),
+ * inv_freq = 1 / rotary_base ** (2i / rotary_dims) in fp32, intermediate % 128 == 0 (else RSB_ERR_UNSUPPORTED),
+ * non-positive sizes RSB_ERR_INVALID; all before any CUDA call.  The forward is HF's in fp16: LayerNorm (fp32 mean and
+ * biased variance, one rounding) with bias, query_key_value with bias, partial rotary on dims [0, rotary_dims) of each
+ * Q / K head, causal attention scaled by head_dim^-0.5, dense with bias, dense_h_to_4h -> GELU -> dense_4h_to_h with
+ * biases, the parallel residual x = fp16(fp16(mlp(ln2(x)) + attn(ln1(x))) + x), final_layer_norm and an untied,
+ * bias-free embed_out over any vocabulary size.  rsb_llm_load, _workspace_bytes, _nll, _hidden_states, _attention and
+ * _free take both kinds of handle; on a GPT-NeoX handle
+ *   rsb_llm_load takes "gpt_neox.embed_in.weight", "embed_out.weight", "gpt_neox.final_layer_norm.{weight,bias}" and
+ *     "gpt_neox.layers.N.{input_layernorm, post_attention_layernorm, attention.query_key_value, attention.dense,
+ *     mlp.dense_h_to_4h, mlp.dense_4h_to_h}.{weight,bias}".  query_key_value's per-head interleaved rows
+ *     (q_h | k_h | v_h for each head h) are stored as [Q heads | K heads | V heads];
+ *   rsb_llm_hidden_states returns the residual stream before final_layer_norm;
+ *   rsb_llm_attention takes qkv rows in that permuted [Q heads | K heads | V heads] layout, [T, 3 hidden], rotates the
+ *     first rotary_dims of each Q / K head (the other dims are left bit-identical) and scales by head_dim^-0.5. */
+int rsb_llm_create_neox(int layers, int hidden, int heads, int intermediate, int vocab, int max_pos, int rotary_dims,
+                        float rotary_base, float ln_eps, rsb_llm_t** out);
 /* name = HF LlamaForCausalLM state_dict key: "model.embed_tokens.weight", "model.norm.weight", "lm_head.weight"
  * (untied; accepted and ignored when tied) and "model.layers.N.{self_attn.{q,k,v,o}_proj, mlp.{gate,up,down}_proj,
  * input_layernorm, post_attention_layernorm}.weight"; data fp16 on the device, copied. */
@@ -494,6 +514,17 @@ int rsb_llm_attention(rsb_llm_t* h, void* qkv_dev, const int32_t* cu_seqlens_dev
  * rsb_llm_workspace_bytes(h, T, 0). */
 int rsb_llm_hidden_states(rsb_llm_t* h, const int32_t* ids_dev, const int32_t* cu_seqlens_dev, int B, int T,
                           int max_seqlen, void* out_dev, void* ws_dev, size_t ws_bytes, rsb_stream_t stream);
+/* Diagnostic, not used on the product path: the GPT-NeoX LayerNorm step of rsb_llm_nll's forward on a caller's fp16 rows
+ * of `hidden` elements.  Output row i reads input row r = rows_dev ? rows_dev[i] : i of x_dev, i < n_rows.
+ *   add_dev != NULL: first x[r] = fp16(x[r] + add[r]) (the parallel residual's last sum), written back to x_dev.
+ *   w1_dev != NULL: out1[i] = fp16((x[r] - mean) * rsqrt(var + eps) * w1 + b1), mean and biased variance in fp32, one
+ *   rounding (torch's fp16 LayerNorm); w2_dev != NULL (only with w1_dev): out2[i] likewise with w2 / b2, from the same
+ *   statistics.  Neither: only the add.
+ * hidden must be a multiple of 8 and at most 8192 (RSB_ERR_UNSUPPORTED, also the largest hidden rsb_llm_create_neox
+ * accepts); a missing bias or output RSB_ERR_INVALID; both before any launch.  No handle is needed. */
+int rsb_llm_layernorm(int hidden, float eps, void* x_dev, const void* add_dev, const int32_t* rows_dev, int n_rows,
+                      const void* w1_dev, const void* b1_dev, const void* w2_dev, const void* b2_dev, void* out1_dev,
+                      void* out2_dev, rsb_stream_t stream);
 
 /* ---- MinHash de-duplication of retrieved passages ----------------------------------------------------------------
  * Replaces utils/deduplication.py's `remove_duplicates_with_minhash` (datasketch MinHash(num_perm=128) and

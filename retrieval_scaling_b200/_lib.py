@@ -92,6 +92,7 @@ SIGNATURES = [
     ("rsb_gemm_f16", c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     ("rsb_llm_last_error", c_char_p, []),
     ("rsb_llm_create", c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_int, POINTER(_H)]),
+    ("rsb_llm_create_neox", c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_float, POINTER(_H)]),
     ("rsb_llm_load", c_int, [_H, c_char_p, c_void_p, c_int64, c_void_p]),
     ("rsb_llm_workspace_bytes", c_size_t, [_H, c_int, c_int]),
     ("rsb_llm_nll", c_int, [_H, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
@@ -99,6 +100,8 @@ SIGNATURES = [
     ("rsb_llm_attention", c_int, [_H, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),   # diagnostic
     ("rsb_llm_hidden_states", c_int, [_H, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t,
                                       c_void_p]),                                                   # diagnostic
+    ("rsb_llm_layernorm", c_int, [c_int, c_float, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
+                                  c_void_p, c_void_p, c_void_p, c_void_p]),                          # diagnostic
     ("rsb_dedup_last_error", c_char_p, []),
     ("rsb_minhash_workspace_bytes", c_size_t, [c_int64]),
     ("rsb_minhash_signatures", c_int, [c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,

@@ -1,5 +1,6 @@
-// rsb_llm.cu -- reader-LM forward for perplexity evaluation: HF LlamaForCausalLM (Llama-2 MHA, Llama-3 GQA) in fp16,
-// prefill only, over packed un-padded sequences, ending in the per-token negative log-likelihood of the labels.
+// rsb_llm.cu -- reader-LM forward for perplexity evaluation: HF LlamaForCausalLM (Llama-2 MHA, Llama-3 GQA) and
+// GPTNeoXForCausalLM (Pythia; rsb_llm_create_neox) in fp16, prefill only, over packed un-padded sequences, ending in
+// the per-token negative log-likelihood of the labels.
 // Replaces the reader call of the reference's perplexity loop (src/evaluate_perplexity.py:126-134: `lm(input_ids,
 // labels=labels)` one window at a time, HF in bf16).  No KV cache, no generation.
 //
@@ -10,7 +11,9 @@
 //                            q|k|v and gate|up weights, residual adds through its residual epilogue with a zero bias
 //   rope_kernel              HF rotate_half RoPE on the Q and K heads of the fused QKV rows; positions restart at 0 in
 //                            every packed sequence
-//   attention_causal_kernel  causal flash attention, head_dim 128, GQA, mma.sync.m16n8k16 with fp32 running max / sum;
+//   ln_rows_kernel           GPT-NeoX: torch's fp16 LayerNorm, with the parallel residual's last add and both norms fused
+//   rope_partial_kernel      GPT-NeoX: rotate_half on the first rotary_dims of each Q / K head
+//   attention_causal_kernel  causal flash attention, head_dim 64 / 80 / 128 / 256, GQA, mma.sync.m16n8k16 with fp32 running max / sum;
 //                            key blocks above the diagonal are never visited
 //   swiglu_kernel            act = fp16(fp16(silu(gate)) * up), HF LlamaMLP's order
 //   nll_rows_kernel          fp32 logsumexp over the real vocabulary (pad rows of the LM head excluded) - logit[label]
@@ -30,8 +33,8 @@
 
 namespace {
 
-constexpr int HD = 128;                      // head_dim of every supported reader
-constexpr int AQ = 64, AK = 64, APAD = HD + 8;   // attention: 64 queries per block (16 per warp), key blocks of 64
+constexpr int HD = 128;                      // head_dim of every Llama reader
+constexpr int AQ = 64, AK = 64;              // attention: 64 queries per block (16 per warp), key blocks of 64
 constexpr size_t LOGIT_BYTES = 256u << 20;   // bound of the logits workspace of one LM-head chunk
 
 __device__ __forceinline__ float block_sum(float v, float* red) {
@@ -118,6 +121,115 @@ __global__ void rope_kernel(__half* __restrict__ qkv, const int* __restrict__ cu
     }
 }
 
+// GPT-NeoX partial rotary (modeling_gpt_neox.py apply_rotary_pos_emb): rotate_half on dims [0, rot) of every Q and K
+// head (head_dim hd apart, Q heads then K heads at the start of each QKV row), in rope_kernel's fp16 order; dims
+// [rot, hd) are neither read nor written.  One block per token.
+__global__ void rope_partial_kernel(__half* __restrict__ qkv, const int* __restrict__ cu_seqlens, int B, int ld,
+                                    int rot_heads, int hd, int rot, const float* __restrict__ inv_freq) {
+    const int t = blockIdx.x;
+    int lo = 0, hi = B;
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (cu_seqlens[mid] <= t) lo = mid; else hi = mid;
+    }
+    const float pos = (float)(t - cu_seqlens[lo]);
+    const int half_rot = rot >> 1;
+    __half* row = qkv + (size_t)t * ld;
+    for (int p = threadIdx.x; p < rot_heads * half_rot; p += blockDim.x) {
+        const int i = p % half_rot;
+        __half* x = row + (p / half_rot) * hd;
+        const float f = inv_freq[i] * pos;
+        const float c = __half2float(__float2half_rn(cosf(f))), s = __half2float(__float2half_rn(sinf(f)));
+        const float x1 = __half2float(x[i]), x2 = __half2float(x[i + half_rot]);
+        const float a1 = __half2float(__float2half_rn(x1 * c)), b1 = __half2float(__float2half_rn(-x2 * s));
+        const float a2 = __half2float(__float2half_rn(x2 * c)), b2 = __half2float(__float2half_rn(x1 * s));
+        x[i] = __float2half_rn(a1 + b1);
+        x[i + half_rot] = __float2half_rn(a2 + b2);
+    }
+}
+
+// torch's fp16 nn.LayerNorm, once or twice on the same row: mean and biased variance in fp32 (two passes over the row
+// held in registers), y = fp16((x - mean) * rsqrt(var + eps) * w + b) with one rounding.  One block of 256 threads per
+// output row i, input row r = rows ? rows[i] : i; hidden % 8 == 0 and hidden <= 8192.
+//   add != nullptr: first X[r] = fp16(X[r] + add[r]) (the parallel residual's last sum, HF's order), written back.
+//   w1 != nullptr: out1[i] = LN(X[r]; w1, b1); w2 != nullptr: out2[i] = LN(X[r]; w2, b2) from the same statistics.
+constexpr int LN_THREADS = 256, LN_VEC = 4;   // up to 4 x 8 halves per thread
+constexpr int LN_MAX_HIDDEN = LN_THREADS * LN_VEC * 8;   // 8192: the widest row ln_rows_kernel holds
+__global__ __launch_bounds__(LN_THREADS)
+void ln_rows_kernel(__half* __restrict__ X, const __half* __restrict__ add, const int* __restrict__ rows, int hidden,
+                    const __half* __restrict__ w1, const __half* __restrict__ b1, const __half* __restrict__ w2,
+                    const __half* __restrict__ b2, float eps, __half* __restrict__ out1, __half* __restrict__ out2) {
+    __shared__ float red[LN_THREADS / 32];
+    const int i = blockIdx.x;
+    const int r = rows ? rows[i] : i;
+    const int n8 = hidden / 8;
+    uint4* x = reinterpret_cast<uint4*>(X + (size_t)r * hidden);
+    uint4 v[LN_VEC];
+    float s = 0.f;
+#pragma unroll
+    for (int k = 0; k < LN_VEC; ++k) {
+        const int c = threadIdx.x + k * LN_THREADS;
+        v[k] = make_uint4(0, 0, 0, 0);
+        if (c < n8) {
+            v[k] = x[c];
+            if (add) {
+                const uint4 a = reinterpret_cast<const uint4*>(add + (size_t)r * hidden)[c];
+                __half2* h2 = reinterpret_cast<__half2*>(&v[k]);
+                const __half2* a2 = reinterpret_cast<const __half2*>(&a);
+#pragma unroll
+                for (int e = 0; e < 4; ++e) h2[e] = __hadd2(h2[e], a2[e]);
+                x[c] = v[k];
+            }
+            const __half2* h2 = reinterpret_cast<const __half2*>(&v[k]);
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const float2 f = __half22float2(h2[e]);
+                s += f.x + f.y;
+            }
+        }
+    }
+    if (!w1 && !w2) return;
+    const float mean = block_sum(s, red) / (float)hidden;
+    float q = 0.f;
+#pragma unroll
+    for (int k = 0; k < LN_VEC; ++k) {
+        if (threadIdx.x + k * LN_THREADS < n8) {
+            const __half2* h2 = reinterpret_cast<const __half2*>(&v[k]);
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const float2 f = __half22float2(h2[e]);
+                const float d0 = f.x - mean, d1 = f.y - mean;
+                q = fmaf(d0, d0, q);
+                q = fmaf(d1, d1, q);
+            }
+        }
+    }
+    const float rstd = rsqrtf(block_sum(q, red) / (float)hidden + eps);
+    for (int n = 0; n < 2; ++n) {
+        const __half* w = n ? w2 : w1;
+        const __half* b = n ? b2 : b1;
+        if (!w) continue;
+        uint4* o = reinterpret_cast<uint4*>((n ? out2 : out1) + (size_t)i * hidden);
+#pragma unroll
+        for (int k = 0; k < LN_VEC; ++k) {
+            const int c = threadIdx.x + k * LN_THREADS;
+            if (c >= n8) continue;
+            const uint4 g = reinterpret_cast<const uint4*>(w)[c], bb = reinterpret_cast<const uint4*>(b)[c];
+            const __half2* h2 = reinterpret_cast<const __half2*>(&v[k]);
+            const __half2* g2 = reinterpret_cast<const __half2*>(&g);
+            const __half2* bb2 = reinterpret_cast<const __half2*>(&bb);
+            uint4 ov;
+            __half2* o2 = reinterpret_cast<__half2*>(&ov);
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const float2 f = __half22float2(h2[e]), gf = __half22float2(g2[e]), bf = __half22float2(bb2[e]);
+                o2[e] = __floats2half2_rn(fmaf((f.x - mean) * rstd, gf.x, bf.x), fmaf((f.y - mean) * rstd, gf.y, bf.y));
+            }
+            o[c] = ov;
+        }
+    }
+}
+
 __device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
     asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
                  : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
@@ -129,42 +241,79 @@ __device__ __forceinline__ uint32_t half2_bits(float lo, float hi) {
 }
 __device__ __forceinline__ uint32_t ld32(const __half* p) { return *reinterpret_cast<const uint32_t*>(p); }
 
-// Causal attention of one (sequence, query block of 64, head): blockIdx.x = item (b, qb) from the host's list, heaviest
-// query blocks first; blockIdx.y = query head h, which reads KV head h / (heads / kv_heads).  4 warps, 16 query rows each
-// with their Q fragments in registers; key blocks 0..qb (every later one is fully masked) are staged in shared memory
-// by the whole block.  S = Q K^T and O += P V on mma.sync.m16n8k16 with fp32 accumulators; online softmax in the log2
-// domain with fp32 running maximum and sum, P rounded to half for the P V product.  Inside the diagonal block a warp
-// skips the key tiles of 8 that lie entirely above its last row.
+// Row of 16-byte element idx >= 0 of a tile with n such elements per row: a shift when n is a power of two.
+template <int n>
+__device__ __forceinline__ int tile_row(int idx) {
+    if constexpr ((n & (n - 1)) == 0) return idx >> (31 - __builtin_clz(n));
+    else return (int)((unsigned)idx / n);
+}
+
+// Shared tile `which` (0 = K, 1 = V, 2 = Q) of 64 rows of D halves, padded by 8 halves per row against bank conflicts.
+template <int D, int which>
+__device__ __forceinline__ __half (&attention_tile())[AK][D + 8] {
+    if constexpr (D > 128) {
+        extern __shared__ __align__(16) unsigned char attn_dyn[];
+        return *reinterpret_cast<__half (*)[AK][D + 8]>(attn_dyn + which * sizeof(__half[AK][D + 8]));
+    } else {
+        __shared__ __align__(16) __half tile[AK][D + 8];
+        return tile;
+    }
+}
+
+// Causal attention of one (sequence, query block of 64, head) at head_dim D: blockIdx.x = item (b, qb) from the host's
+// list, heaviest query blocks first; blockIdx.y = query head h, which reads KV head h / (heads / kv_heads).  4 warps,
+// 16 query rows each; key blocks 0..qb (every later one is fully masked) are staged in shared memory by the whole block.
+// S = Q K^T and O += P V on mma.sync.m16n8k16 with fp32 accumulators; online softmax in the log2 domain with fp32
+// running maximum and sum, P rounded to half for the P V product.  Inside the diagonal block a warp skips the key tiles
+// of 8 that lie entirely above its last row.
+// D <= 128: Q fragments in registers, K / V tiles in static shared memory (34.8 KB at D = 128).  D = 256: the 16 x 256
+// fp32 output alone is 128 registers per thread, so Q is staged once in shared memory and its fragments are loaded
+// with ldmatrix per 16-column step; Q, K and V tiles (3 x 33.8 KB) are dynamic shared memory.
+template <int D>
 __global__ __launch_bounds__(128)
 void attention_causal_kernel(const __half* __restrict__ qkv, const int* __restrict__ cu_seqlens,
                              const int2* __restrict__ items, __half* __restrict__ ctx, int heads, int kv_heads,
                              float scale_log2) {
-    __shared__ __align__(16) __half Ks[AK][APAD];
-    __shared__ __align__(16) __half Vs[AK][APAD];
+    constexpr int PAD = D + 8, KS = D / 16, NT = D / 8;
+    constexpr bool QSMEM = D > 128;
+    constexpr int KT = QSMEM ? 32 : AK, NKT = KT / 8;   // keys per softmax step; its key tiles of 8
+    auto& Ks = attention_tile<D, 0>();
+    auto& Vs = attention_tile<D, 1>();
+    auto& Qs = attention_tile<D, 2>();           // D > 128 only
     const int2 it = items[blockIdx.x];
     const int b = it.x, qb = it.y, h = blockIdx.y, kvh = h / (heads / kv_heads);
-    const int hid = heads * HD, ld = hid + 2 * kv_heads * HD;
+    const int hid = heads * D, ld = hid + 2 * kv_heads * D;
     const int t0 = cu_seqlens[b], S = cu_seqlens[b + 1] - t0;
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
     const int qw = qb * AQ + wib * 16;           // first query row of this warp
     const bool active = qw < S;                  // warp-uniform; idle warps still stage K / V and meet the barriers
-    const __half* qbase = qkv + (size_t)t0 * ld + h * HD;
-    const __half* kbase = qkv + (size_t)t0 * ld + hid + kvh * HD;
-    const __half* vbase = kbase + kv_heads * HD;
+    const __half* qbase = qkv + (size_t)t0 * ld + h * D;
+    const __half* kbase = qkv + (size_t)t0 * ld + hid + kvh * D;
+    const __half* vbase = kbase + kv_heads * D;
     const int r0 = qw + g, r1 = r0 + 8;
 
-    uint32_t qa[8][4];
+    uint32_t qa[QSMEM ? 1 : KS][4];
+    if constexpr (QSMEM) {
 #pragma unroll
-    for (int ks = 0; ks < 8; ++ks) {
-        const int c = ks * 16 + 2 * t;
-        qa[ks][0] = r0 < S ? ld32(qbase + (size_t)r0 * ld + c) : 0u;
-        qa[ks][1] = r1 < S ? ld32(qbase + (size_t)r1 * ld + c) : 0u;
-        qa[ks][2] = r0 < S ? ld32(qbase + (size_t)r0 * ld + c + 8) : 0u;
-        qa[ks][3] = r1 < S ? ld32(qbase + (size_t)r1 * ld + c + 8) : 0u;
+        for (int i = 0; i < AQ * NT / 128; ++i) {   // 64 query rows, zero past the window (read by the first barrier)
+            const int idx = threadIdx.x + 128 * i, j = tile_row<NT>(idx), c = idx - j * NT;
+            const int q = qb * AQ + j;
+            *reinterpret_cast<uint4*>(&Qs[j][c * 8]) =
+                q < S ? *reinterpret_cast<const uint4*>(qbase + (size_t)q * ld + c * 8) : make_uint4(0, 0, 0, 0);
+        }
+    } else {
+#pragma unroll
+        for (int ks = 0; ks < KS; ++ks) {
+            const int c = ks * 16 + 2 * t;
+            qa[ks][0] = r0 < S ? ld32(qbase + (size_t)r0 * ld + c) : 0u;
+            qa[ks][1] = r1 < S ? ld32(qbase + (size_t)r1 * ld + c) : 0u;
+            qa[ks][2] = r0 < S ? ld32(qbase + (size_t)r0 * ld + c + 8) : 0u;
+            qa[ks][3] = r1 < S ? ld32(qbase + (size_t)r1 * ld + c + 8) : 0u;
+        }
     }
-    float o[16][4];
+    float o[NT][4];
 #pragma unroll
-    for (int nt = 0; nt < 16; ++nt)
+    for (int nt = 0; nt < NT; ++nt)
 #pragma unroll
         for (int e = 0; e < 4; ++e) o[nt][e] = 0.f;
     float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};   // l_run: per-lane partial sums
@@ -172,8 +321,8 @@ void attention_causal_kernel(const __half* __restrict__ qkv, const int* __restri
     for (int kb = 0; kb <= qb; ++kb) {
         __syncthreads();                         // the previous key block has been consumed by every warp
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {            // 64 rows x 16 uint4 of K and of V
-            const int idx = threadIdx.x + 128 * i, j = idx >> 4, c = idx & 15;
+        for (int i = 0; i < AK * NT / 128; ++i) {   // 64 rows x D / 8 uint4 of K and of V
+            const int idx = threadIdx.x + 128 * i, j = tile_row<NT>(idx), c = idx - j * NT;
             const int key = kb * AK + j;
             uint4 kv = make_uint4(0, 0, 0, 0), vv = kv;
             if (key < S) {
@@ -185,29 +334,44 @@ void attention_causal_kernel(const __half* __restrict__ qkv, const int* __restri
         }
         __syncthreads();
         if (!active) continue;
-        // key tiles of 8 holding at least one key <= this warp's last row (all 8 below the diagonal block)
-        const int nvt = kb < qb ? 8 : min(8, (qw + 15 - kb * AK) / 8 + 1);
-        float sacc[8][4];
 #pragma unroll
-        for (int nt = 0; nt < 8; ++nt)
+        for (int sb = 0; sb < AK / KT; ++sb) {   // key steps of KT within the staged block
+        const int k0 = kb * AK + sb * KT;        // first key of this step
+        // key tiles of 8 holding at least one key <= this warp's last row (all of them below the diagonal block)
+        int nvt;
+        if constexpr (KT == AK) {
+            nvt = kb < qb ? 8 : min(8, (qw + 15 - k0) / 8 + 1);
+        } else {
+            nvt = kb < qb ? NKT : (qw + 15 < k0 ? 0 : min(NKT, (qw + 15 - k0) / 8 + 1));
+            if (nvt == 0) continue;              // warp-uniform: every key of the step is above this warp's rows
+        }
+        float sacc[NKT][4];
+#pragma unroll
+        for (int nt = 0; nt < NKT; ++nt)
 #pragma unroll
             for (int e = 0; e < 4; ++e) sacc[nt][e] = 0.f;
 #pragma unroll
-        for (int ks = 0; ks < 8; ++ks)
+        for (int ks = 0; ks < KS; ++ks) {
+            if constexpr (QSMEM) {
+                const uint32_t addr = (uint32_t)__cvta_generic_to_shared(&Qs[wib * 16 + (lane & 15)][ks * 16 + (lane >> 4) * 8]);
+                asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
+                             : "=r"(qa[0][0]), "=r"(qa[0][1]), "=r"(qa[0][2]), "=r"(qa[0][3]) : "r"(addr));
+            }
 #pragma unroll
-            for (int nt = 0; nt < 8; ++nt) {
+            for (int nt = 0; nt < NKT; ++nt) {
                 if (nt < nvt) {
-                    const int j = nt * 8 + g, c = ks * 16 + 2 * t;
+                    const int j = sb * KT + nt * 8 + g, c = ks * 16 + 2 * t;
                     const uint32_t kf[2] = {ld32(&Ks[j][c]), ld32(&Ks[j][c + 8])};
-                    mma16816(sacc[nt], qa[ks], kf);
+                    mma16816(sacc[nt], qa[QSMEM ? 0 : ks], kf);
                 }
             }
+        }
         float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-        for (int nt = 0; nt < 8; ++nt)
+        for (int nt = 0; nt < NKT; ++nt)
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
-                const int key = kb * AK + nt * 8 + 2 * t + (e & 1), row = (e < 2) ? r0 : r1;
+                const int key = k0 + nt * 8 + 2 * t + (e & 1), row = (e < 2) ? r0 : r1;
                 const float sv = (nt < nvt && key <= row && key < S) ? sacc[nt][e] * scale_log2 : -INFINITY;
                 sacc[nt][e] = sv;
                 mx[e >> 1] = fmaxf(mx[e >> 1], sv);
@@ -224,7 +388,7 @@ void attention_causal_kernel(const __half* __restrict__ qkv, const int* __restri
         }
         float sum[2] = {0.f, 0.f};
 #pragma unroll
-        for (int nt = 0; nt < 8; ++nt)
+        for (int nt = 0; nt < NKT; ++nt)
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
                 const float p = exp2f(sacc[nt][e] - mref[e >> 1]);   // 2^-inf = 0
@@ -234,30 +398,31 @@ void attention_causal_kernel(const __half* __restrict__ qkv, const int* __restri
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) l_run[hr] = l_run[hr] * corr[hr] + sum[hr];
 #pragma unroll
-        for (int nt = 0; nt < 16; ++nt) {
+        for (int nt = 0; nt < NT; ++nt) {
             o[nt][0] *= corr[0]; o[nt][1] *= corr[0];
             o[nt][2] *= corr[1]; o[nt][3] *= corr[1];
         }
-        uint32_t pa[4][4];
+        uint32_t pa[NKT / 2][4];
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
+        for (int kk = 0; kk < NKT / 2; ++kk) {
             pa[kk][0] = half2_bits(sacc[2 * kk][0], sacc[2 * kk][1]);
             pa[kk][1] = half2_bits(sacc[2 * kk][2], sacc[2 * kk][3]);
             pa[kk][2] = half2_bits(sacc[2 * kk + 1][0], sacc[2 * kk + 1][1]);
             pa[kk][3] = half2_bits(sacc[2 * kk + 1][2], sacc[2 * kk + 1][3]);
         }
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
+        for (int kk = 0; kk < NKT / 2; ++kk) {
             if (kk * 2 < nvt) {                  // a 16-key step whose keys are all masked adds nothing
 #pragma unroll
-                for (int nt = 0; nt < 16; ++nt) {
+                for (int nt = 0; nt < NT; ++nt) {
                     uint32_t vb[2];
-                    const uint32_t addr = (uint32_t)__cvta_generic_to_shared(&Vs[kk * 16 + (lane & 15)][nt * 8]);
+                    const uint32_t addr = (uint32_t)__cvta_generic_to_shared(&Vs[sb * KT + kk * 16 + (lane & 15)][nt * 8]);
                     asm volatile("ldmatrix.sync.aligned.m8n8.x2.trans.shared.b16 {%0,%1}, [%2];"
                                  : "=r"(vb[0]), "=r"(vb[1]) : "r"(addr));
                     mma16816(o[nt], pa[kk], vb);
                 }
             }
+        }
         }
     }
     if (!active) return;
@@ -270,12 +435,13 @@ void attention_causal_kernel(const __half* __restrict__ qkv, const int* __restri
         inv[hr] = l > 0.f ? 1.f / l : 0.f;
     }
 #pragma unroll
-    for (int nt = 0; nt < 16; ++nt) {
-        const int col = h * HD + nt * 8 + 2 * t;
+    for (int nt = 0; nt < NT; ++nt) {
+        const int col = h * D + nt * 8 + 2 * t;
         if (r0 < S) *reinterpret_cast<__half2*>(ctx + (size_t)(t0 + r0) * hid + col) = __floats2half2_rn(o[nt][0] * inv[0], o[nt][1] * inv[0]);
         if (r1 < S) *reinterpret_cast<__half2*>(ctx + (size_t)(t0 + r1) * hid + col) = __floats2half2_rn(o[nt][2] * inv[1], o[nt][3] * inv[1]);
     }
 }
+constexpr size_t attention_dyn_smem(int D) { return D > 128 ? 3 * (size_t)AK * (D + 8) * sizeof(__half) : 0; }
 
 // act[t, j] = fp16(fp16(silu(gate[t, j])) * up[t, j]) with gu = [gate | up] rows of 2 * inter; silu as torch computes it
 // on half, x / (1 + exp(-x)) in fp32 rounded to half.  8 elements per thread.
@@ -359,22 +525,26 @@ int lfail(int code, const char* fmt, ...) {
     return code;
 }
 
+// Llama: wgu = gate | up, no biases.  GPT-NeoX: wgu = dense_h_to_4h, wdown = dense_4h_to_h, wqkv = query_key_value
+// with its rows permuted to [Q heads | K heads | V heads], and the biases and LayerNorm biases below.
 struct LlmLayer {
     __half *wqkv = nullptr, *wo = nullptr, *wgu = nullptr, *wdown = nullptr, *ln1 = nullptr, *ln2 = nullptr;
+    __half *bqkv = nullptr, *bo = nullptr, *bgu = nullptr, *bdown = nullptr, *ln1b = nullptr, *ln2b = nullptr;
 };
 
 }  // namespace
 
 struct rsb_llm {
     int layers = 0, hidden = 0, heads = 0, kv_heads = 0, inter = 0, vocab = 0, vocab_pad = 0, max_pos = 0;
+    int head_dim = HD, rot = HD;                 // rot: rotated dims of each Q / K head (GPT-NeoX rotary_ndims)
     float rope_theta = 0.f, eps = 0.f;
-    bool tied = false;
-    __half *embed = nullptr, *lm_head = nullptr, *final_g = nullptr, *zero_bias = nullptr;
+    bool tied = false, neox = false;
+    __half *embed = nullptr, *lm_head = nullptr, *final_g = nullptr, *final_b = nullptr, *zero_bias = nullptr;
     float* inv_freq = nullptr;
     std::vector<LlmLayer> L;
     std::set<std::string> loaded;                // required weights loaded so far
-    int qkv_n() const { return (heads + 2 * kv_heads) * HD; }
-    size_t required() const { return 2 + 9 * (size_t)layers + (tied ? 0 : 1); }
+    int qkv_n() const { return (heads + 2 * kv_heads) * head_dim; }
+    size_t required() const { return neox ? 4 + 12 * (size_t)layers : 2 + 9 * (size_t)layers + (tied ? 0 : 1); }
     int chunk_rows() const { return (int)std::max<size_t>(128, LOGIT_BYTES / ((size_t)vocab_pad * 2) / 128 * 128); }
 };
 
@@ -387,17 +557,19 @@ int gemm(const __half* A, int M, const __half* W, int N, int K, const __half* bi
 }
 
 // workspace: X, normed rows, QKV, attention output, gate|up, SwiGLU output, one chunk of logits, the label tables and
-// the attention work list.  Label tables: logit row, label and output index per scored token.
+// the attention work list.  Label tables: logit row, label and output index per scored token.  GPT-NeoX: slot 1 holds
+// both normed rows (ln1 | ln2), slot 4 the dense_h_to_4h output and slot 5 the attention block's output, to which the
+// MLP output is added in place.
 size_t llm_ws_layout(const rsb_llm* h, size_t T, size_t nl, size_t off[10]) {
     auto al = [](size_t x) { return (x + 1023) / 1024 * 1024; };
     const size_t chunk = std::min<size_t>(std::max<size_t>(nl, 1), (size_t)h->chunk_rows());
     size_t o = 0;
     off[0] = o; o += al(T * h->hidden * 2);                 // X (residual stream)
-    off[1] = o; o += al(T * h->hidden * 2);                 // normed rows
+    off[1] = o; o += al((h->neox ? 2 : 1) * T * h->hidden * 2);           // normed rows
     off[2] = o; o += al(T * (size_t)h->qkv_n() * 2);        // QKV
     off[3] = o; o += al(T * h->hidden * 2);                 // attention output
-    off[4] = o; o += al(T * 2 * (size_t)h->inter * 2);      // gate | up
-    off[5] = o; o += al(T * (size_t)h->inter * 2);          // SwiGLU output
+    off[4] = o; o += al((h->neox ? 1 : 2) * T * (size_t)h->inter * 2);    // gate | up
+    off[5] = o; o += al(T * (size_t)(h->neox ? h->hidden : h->inter) * 2);   // SwiGLU output
     off[6] = o; o += al(chunk * (size_t)h->vocab_pad * 2);  // logits of one chunk of label rows
     off[7] = o; o += al(3 * std::max<size_t>(nl, 1) * sizeof(int));   // rows | labels | out_idx
     off[8] = o; o += al(T * sizeof(int2));                  // attention items (b, query block)
@@ -456,11 +628,74 @@ extern "C" int rsb_llm_create(int layers, int hidden, int heads, int kv_heads, i
     return RSB_OK;
 }
 
+// Replaces the same call for GPT-NeoX readers (Pythia, the reference's default lm_model): LayerNorm with biases,
+// per-head interleaved query_key_value with biases, partial rotary on rotary_dims of each head, exact-GELU MLP, the
+// parallel residual and an untied embed_out.  Every refusal comes before any CUDA call.
+extern "C" int rsb_llm_create_neox(int layers, int hidden, int heads, int intermediate, int vocab, int max_pos,
+                                   int rotary_dims, float rotary_base, float ln_eps, rsb_llm_t** out) {
+    if (!out) return lfail(RSB_ERR_INVALID, "out is NULL");
+    *out = nullptr;
+    if (layers <= 0 || hidden <= 0 || heads <= 0 || intermediate <= 0 || vocab <= 0 || max_pos <= 0 ||
+        !(rotary_base > 0.f) || !(ln_eps > 0.f))
+        return lfail(RSB_ERR_INVALID, "layers, hidden, heads, intermediate, vocab, max_pos, rotary_base and ln_eps must be positive");
+    const int hd = hidden / heads;
+    if (hidden % heads || (hd != 64 && hd != 80 && hd != 128 && hd != 256))
+        return lfail(RSB_ERR_UNSUPPORTED, "head_dim %ld (hidden %ld / heads %ld): only head_dim 64, 80, 128 and 256 are "
+                     "implemented", (long)(hidden % heads ? -1 : hd), (long)hidden, (long)heads);
+    if (rotary_dims <= 0 || rotary_dims > hd)
+        return lfail(RSB_ERR_INVALID, "rotary_dims %ld is not in [1, head_dim %ld]", (long)rotary_dims, (long)hd);
+    if (rotary_dims % 2)
+        return lfail(RSB_ERR_UNSUPPORTED, "rotary_dims %ld is odd", (long)rotary_dims);
+    if (hidden > LN_MAX_HIDDEN)
+        return lfail(RSB_ERR_UNSUPPORTED, "hidden %ld: the LayerNorm kernel holds rows of at most %ld", (long)hidden,
+                     (long)LN_MAX_HIDDEN);
+    if (intermediate % 128)
+        return lfail(RSB_ERR_UNSUPPORTED, "intermediate_size %ld is not a multiple of 128", (long)intermediate);
+    rsb_llm* h = new rsb_llm();
+    h->neox = true;
+    h->layers = layers; h->hidden = hidden; h->heads = heads; h->kv_heads = heads; h->inter = intermediate;
+    h->head_dim = hd; h->rot = rotary_dims;
+    h->vocab = vocab; h->vocab_pad = (vocab + 127) / 128 * 128; h->max_pos = max_pos;
+    h->rope_theta = rotary_base; h->eps = ln_eps;
+    const size_t H = hidden, V = h->vocab_pad, I = intermediate;
+    bool ok = true;
+    ok &= cudaMalloc(&h->embed, (size_t)vocab * H * 2) == cudaSuccess;
+    ok &= cudaMalloc(&h->lm_head, V * H * 2) == cudaSuccess;
+    ok &= cudaMalloc(&h->final_g, H * 2) == cudaSuccess;
+    ok &= cudaMalloc(&h->final_b, H * 2) == cudaSuccess;
+    ok &= cudaMalloc(&h->zero_bias, V * 2) == cudaSuccess;            // the LM head's (embed_out has no bias)
+    ok &= cudaMalloc(&h->inv_freq, rotary_dims / 2 * sizeof(float)) == cudaSuccess;
+    h->L.resize(layers);
+    for (auto& l : h->L) {
+        ok &= cudaMalloc(&l.wqkv, 3 * H * H * 2) == cudaSuccess;
+        ok &= cudaMalloc(&l.wo, H * H * 2) == cudaSuccess;
+        ok &= cudaMalloc(&l.wgu, I * H * 2) == cudaSuccess;
+        ok &= cudaMalloc(&l.wdown, I * H * 2) == cudaSuccess;
+        ok &= cudaMalloc(&l.bqkv, 3 * H * 2) == cudaSuccess;
+        ok &= cudaMalloc(&l.bo, H * 2) == cudaSuccess;
+        ok &= cudaMalloc(&l.bgu, I * 2) == cudaSuccess;
+        ok &= cudaMalloc(&l.bdown, H * 2) == cudaSuccess;
+        for (__half** p : {&l.ln1, &l.ln1b, &l.ln2, &l.ln2b}) ok &= cudaMalloc(p, H * 2) == cudaSuccess;
+    }
+    if (!ok) { rsb_llm_free(h); return lfail(RSB_ERR_OOM, "allocating reader weights failed"); }
+    // GPTNeoXRotaryEmbedding: inv_freq = 1 / base ** (arange(0, rot, 2).float() / rot), in fp32
+    std::vector<float> inv(rotary_dims / 2);
+    for (int i = 0; i < rotary_dims / 2; ++i) inv[i] = 1.f / powf(rotary_base, (float)(2 * i) / (float)rotary_dims);
+    ok &= cudaMemcpy(h->inv_freq, inv.data(), inv.size() * sizeof(float), cudaMemcpyHostToDevice) == cudaSuccess;
+    ok &= cudaMemset(h->zero_bias, 0, V * 2) == cudaSuccess;
+    ok &= cudaMemset(h->lm_head, 0, V * H * 2) == cudaSuccess;   // pad rows stay zero (and outside the sum)
+    if (!ok) { rsb_llm_free(h); return lfail(RSB_ERR_CUDA, "initialising the reader failed"); }
+    *out = h;
+    return RSB_OK;
+}
+
 extern "C" int rsb_llm_free(rsb_llm_t* h) {
     if (!h) return RSB_OK;
-    cudaFree(h->embed); cudaFree(h->lm_head); cudaFree(h->final_g); cudaFree(h->zero_bias); cudaFree(h->inv_freq);
+    cudaFree(h->embed); cudaFree(h->lm_head); cudaFree(h->final_g); cudaFree(h->final_b); cudaFree(h->zero_bias);
+    cudaFree(h->inv_freq);
     for (auto& l : h->L) {
         cudaFree(l.wqkv); cudaFree(l.wo); cudaFree(l.wgu); cudaFree(l.wdown); cudaFree(l.ln1); cudaFree(l.ln2);
+        cudaFree(l.bqkv); cudaFree(l.bo); cudaFree(l.bgu); cudaFree(l.bdown); cudaFree(l.ln1b); cudaFree(l.ln2b);
     }
     delete h;
     return RSB_OK;
@@ -468,9 +703,62 @@ extern "C" int rsb_llm_free(rsb_llm_t* h) {
 
 // name = HF LlamaForCausalLM state_dict key, data fp16 on the device, copied (src/evaluate_perplexity.py:98-108 loads
 // the same checkpoint).  q|k|v and gate|up land in one fused weight each.
+namespace {
+
+// GPTNeoXForCausalLM state_dict keys.  query_key_value's rows are [heads, 3, head_dim] (q_h | k_h | v_h per head); they
+// land as [Q heads | K heads | V heads], one strided copy per part, so the forward reads the Llama layout.
+int load_neox(rsb_llm* h, const char* name, const void* src, int64_t n, cudaStream_t st) {
+    const int64_t H = h->hidden, I = h->inter;
+    const std::string s(name);
+    auto copied = [&](cudaError_t e) -> int {
+        if (e != cudaSuccess) return lfail(RSB_ERR_CUDA, "copy of %s failed", name);
+        h->loaded.insert(s);
+        return RSB_OK;
+    };
+    auto put = [&](__half* dst, int64_t expect) -> int {
+        if (n != expect) return lfail(RSB_ERR_INVALID, "weight %s has the wrong size (%ld elements)", name, (long)n);
+        return copied(cudaMemcpyAsync(dst, src, (size_t)n * 2, cudaMemcpyDeviceToDevice, st));
+    };
+    auto put_qkv = [&](__half* dst, int64_t per_row) -> int {      // per_row = H (weight) or 1 (bias)
+        if (n != 3 * H * per_row) return lfail(RSB_ERR_INVALID, "weight %s has the wrong size (%ld elements)", name, (long)n);
+        const size_t part = (size_t)h->head_dim * per_row * 2;      // bytes of one head's q (or k or v) rows
+        cudaError_t e = cudaSuccess;
+        for (int p = 0; p < 3 && e == cudaSuccess; ++p)
+            e = cudaMemcpy2DAsync(dst + p * H * per_row, part, static_cast<const char*>(src) + p * part, 3 * part, part,
+                                  h->heads, cudaMemcpyDeviceToDevice, st);
+        return copied(e);
+    };
+    if (s == "gpt_neox.embed_in.weight") return put(h->embed, (int64_t)h->vocab * H);
+    if (s == "embed_out.weight") return put(h->lm_head, (int64_t)h->vocab * H);
+    if (s == "gpt_neox.final_layer_norm.weight") return put(h->final_g, H);
+    if (s == "gpt_neox.final_layer_norm.bias") return put(h->final_b, H);
+    int li = -1;
+    char rest[128] = {0};
+    if (sscanf(name, "gpt_neox.layers.%d.%127s", &li, rest) == 2 && li >= 0 && li < h->layers) {
+        LlmLayer& l = h->L[li];
+        const std::string r(rest);
+        if (r == "input_layernorm.weight") return put(l.ln1, H);
+        if (r == "input_layernorm.bias") return put(l.ln1b, H);
+        if (r == "post_attention_layernorm.weight") return put(l.ln2, H);
+        if (r == "post_attention_layernorm.bias") return put(l.ln2b, H);
+        if (r == "attention.query_key_value.weight") return put_qkv(l.wqkv, H);
+        if (r == "attention.query_key_value.bias") return put_qkv(l.bqkv, 1);
+        if (r == "attention.dense.weight") return put(l.wo, H * H);
+        if (r == "attention.dense.bias") return put(l.bo, H);
+        if (r == "mlp.dense_h_to_4h.weight") return put(l.wgu, I * H);
+        if (r == "mlp.dense_h_to_4h.bias") return put(l.bgu, I);
+        if (r == "mlp.dense_4h_to_h.weight") return put(l.wdown, H * I);
+        if (r == "mlp.dense_4h_to_h.bias") return put(l.bdown, H);
+    }
+    return lfail(RSB_ERR_INVALID, "unknown weight name %s", name);
+}
+
+}  // namespace
+
 extern "C" int rsb_llm_load(rsb_llm_t* h, const char* name, const void* f16_dev, int64_t n, rsb_stream_t stream) {
     if (!h || !name || !f16_dev) return lfail(RSB_ERR_INVALID, "null argument");
     cudaStream_t st = (cudaStream_t)stream;
+    if (h->neox) return load_neox(h, name, f16_dev, n, st);
     const int64_t H = h->hidden, KV = (int64_t)h->kv_heads * HD, I = h->inter;
     const std::string s(name);
     auto put = [&](__half* dst, int64_t expect) -> int {
@@ -543,10 +831,25 @@ int upload_attention_items(const std::vector<int32_t>& cu, int B, int2* d_items,
 void attention_step(const rsb_llm* h, __half* QKV, const int32_t* cu_seqlens, int B, int n_tok, const int2* d_items,
                     int n_items, __half* CTX, cudaStream_t st) {
     if (n_tok == 0 || n_items == 0) return;
-    const float scale_log2 = 1.4426950408889634f / sqrtf((float)HD);   // 1/sqrt(128) in the log2 domain
-    rope_kernel<<<n_tok, 256, 0, st>>>(QKV, cu_seqlens, B, h->qkv_n(), h->heads + h->kv_heads, h->inv_freq);
-    attention_causal_kernel<<<dim3((unsigned)n_items, h->heads), 128, 0, st>>>(QKV, cu_seqlens, d_items, CTX, h->heads,
-                                                                               h->kv_heads, scale_log2);
+    const float scale_log2 = 1.4426950408889634f / sqrtf((float)h->head_dim);   // 1/sqrt(head_dim) in the log2 domain
+    if (h->neox)
+        rope_partial_kernel<<<n_tok, 256, 0, st>>>(QKV, cu_seqlens, B, h->qkv_n(), h->heads + h->kv_heads, h->head_dim,
+                                                   h->rot, h->inv_freq);
+    else
+        rope_kernel<<<n_tok, 256, 0, st>>>(QKV, cu_seqlens, B, h->qkv_n(), h->heads + h->kv_heads, h->inv_freq);
+    const dim3 grid((unsigned)n_items, h->heads);
+    switch (h->head_dim) {
+        case 64: attention_causal_kernel<64><<<grid, 128, 0, st>>>(QKV, cu_seqlens, d_items, CTX, h->heads, h->kv_heads, scale_log2); break;
+        case 80: attention_causal_kernel<80><<<grid, 128, 0, st>>>(QKV, cu_seqlens, d_items, CTX, h->heads, h->kv_heads, scale_log2); break;
+        case 128: attention_causal_kernel<128><<<grid, 128, 0, st>>>(QKV, cu_seqlens, d_items, CTX, h->heads, h->kv_heads, scale_log2); break;
+        default: {
+            constexpr size_t smem = attention_dyn_smem(256);
+            static rsb::PerDeviceFlag configured;            // attributes are per (function, device)
+            if (configured.first())
+                cudaFuncSetAttribute(attention_causal_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            attention_causal_kernel<256><<<grid, 128, smem, st>>>(QKV, cu_seqlens, d_items, CTX, h->heads, h->kv_heads, scale_log2);
+        }
+    }
 }
 
 // Refusals shared by rsb_llm_nll and rsb_llm_hidden_states, then the read-back of the offsets and ids (and labels).
@@ -576,35 +879,85 @@ int check_forward(rsb_llm* h, const int32_t* ids, const int32_t* cu_seqlens, con
     return RSB_OK;
 }
 
+// Workspace slots of one forward (llm_ws_layout) and its attention work list.
+struct Fwd {
+    __half *X, *Hn, *QKV, *CTX, *GU, *ACT;
+    const int32_t* cu_seqlens;
+    int B, T, n_items;
+    const int2* d_items;
+};
+
+// LlamaDecoderLayer x layers: x += o_proj(attn(rms1(x))); x += down(swiglu(gate|up(rms2(x)))).
+int llama_layers(rsb_llm* h, const Fwd& f, cudaStream_t st) {
+    const int Hd = h->hidden, NQKV = h->qkv_n(), I = h->inter, T = f.T;
+    const long long n8 = (long long)T * I / 8;
+    const int sw_grid = (int)std::min<long long>((n8 + 255) / 256, 8LL * rsb::device_num_sms());
+    int rc;
+    for (int li = 0; li < h->layers; ++li) {
+        const LlmLayer& l = h->L[li];
+        rms_rows_kernel<<<T, 256, 0, st>>>(f.X, nullptr, Hd, l.ln1, h->eps, f.Hn);
+        if ((rc = gemm(f.Hn, T, l.wqkv, NQKV, Hd, h->zero_bias, nullptr, f.QKV, 0, st)) != RSB_OK) return rc;
+        attention_step(h, f.QKV, f.cu_seqlens, f.B, T, f.d_items, f.n_items, f.CTX, st);
+        if ((rc = gemm(f.CTX, T, l.wo, Hd, Hd, h->zero_bias, f.X, f.X, 2, st)) != RSB_OK) return rc;
+        rms_rows_kernel<<<T, 256, 0, st>>>(f.X, nullptr, Hd, l.ln2, h->eps, f.Hn);
+        if ((rc = gemm(f.Hn, T, l.wgu, 2 * I, Hd, h->zero_bias, nullptr, f.GU, 0, st)) != RSB_OK) return rc;
+        swiglu_kernel<<<sw_grid, 256, 0, st>>>(f.GU, n8, I, f.ACT);
+        if ((rc = gemm(f.ACT, T, l.wdown, Hd, I, h->zero_bias, f.X, f.X, 2 | RSB_GEMM_REVERSED, st)) != RSB_OK) return rc;
+    }
+    return RSB_OK;
+}
+
+// GPTNeoXLayer x layers with the parallel residual: x = fp16(fp16(mlp(ln2(x)) + attn(ln1(x))) + x).  The MLP's last
+// GEMM adds the attention block's output A in its residual epilogue (A = fp16(mlp + attn), in place); the next
+// ln_rows_kernel adds A to x, writes x back and normalises it twice, for the next layer's ln1 and ln2.
+int neox_layers(rsb_llm* h, const Fwd& f, cudaStream_t st) {
+    const int Hd = h->hidden, NQKV = h->qkv_n(), I = h->inter, T = f.T;
+    __half *N1 = f.Hn, *N2 = f.Hn + (size_t)T * Hd, *FF = f.GU, *A = f.ACT;
+    int rc;
+    ln_rows_kernel<<<T, LN_THREADS, 0, st>>>(f.X, nullptr, nullptr, Hd, h->L[0].ln1, h->L[0].ln1b, h->L[0].ln2,
+                                             h->L[0].ln2b, h->eps, N1, N2);
+    for (int li = 0; li < h->layers; ++li) {
+        const LlmLayer& l = h->L[li];
+        if ((rc = gemm(N1, T, l.wqkv, NQKV, Hd, l.bqkv, nullptr, f.QKV, 0, st)) != RSB_OK) return rc;
+        attention_step(h, f.QKV, f.cu_seqlens, f.B, T, f.d_items, f.n_items, f.CTX, st);
+        if ((rc = gemm(f.CTX, T, l.wo, Hd, Hd, l.bo, nullptr, A, 0, st)) != RSB_OK) return rc;
+        if ((rc = gemm(N2, T, l.wgu, I, Hd, l.bgu, nullptr, FF, 1, st)) != RSB_OK) return rc;
+        if ((rc = gemm(FF, T, l.wdown, Hd, I, l.bdown, A, A, 2 | RSB_GEMM_REVERSED, st)) != RSB_OK) return rc;
+        const LlmLayer* nx = li + 1 < h->layers ? &h->L[li + 1] : nullptr;   // the last layer only adds
+        ln_rows_kernel<<<T, LN_THREADS, 0, st>>>(f.X, A, nullptr, Hd, nx ? nx->ln1 : nullptr, nx ? nx->ln1b : nullptr,
+                                                 nx ? nx->ln2 : nullptr, nx ? nx->ln2b : nullptr, h->eps, N1, N2);
+    }
+    return RSB_OK;
+}
+
 // The decoder layers: X (workspace slot 0) ends as the residual stream after the last layer, before the final norm.
 int trunk(rsb_llm* h, const int32_t* ids, const int32_t* cu_seqlens, int B, int T, const std::vector<int32_t>& cu,
           unsigned char* w, const size_t off[10], cudaStream_t st) {
-    __half* X = reinterpret_cast<__half*>(w + off[0]);
-    __half* Hn = reinterpret_cast<__half*>(w + off[1]);
-    __half* QKV = reinterpret_cast<__half*>(w + off[2]);
-    __half* CTX = reinterpret_cast<__half*>(w + off[3]);
-    __half* GU = reinterpret_cast<__half*>(w + off[4]);
-    __half* ACT = reinterpret_cast<__half*>(w + off[5]);
+    Fwd f;
+    f.X = reinterpret_cast<__half*>(w + off[0]);
+    f.Hn = reinterpret_cast<__half*>(w + off[1]);
+    f.QKV = reinterpret_cast<__half*>(w + off[2]);
+    f.CTX = reinterpret_cast<__half*>(w + off[3]);
+    f.GU = reinterpret_cast<__half*>(w + off[4]);
+    f.ACT = reinterpret_cast<__half*>(w + off[5]);
+    f.cu_seqlens = cu_seqlens;
+    f.B = B;
+    f.T = T;
     int2* d_items = reinterpret_cast<int2*>(w + off[8]);
-    int n_items, rc;
-    if ((rc = upload_attention_items(cu, B, d_items, st, &n_items)) != RSB_OK) return rc;
+    f.d_items = d_items;
+    int rc;
+    if ((rc = upload_attention_items(cu, B, d_items, st, &f.n_items)) != RSB_OK) return rc;
+    embed_rows_kernel<<<T, 128, 0, st>>>(ids, h->embed, h->hidden, f.X);
+    return h->neox ? neox_layers(h, f, st) : llama_layers(h, f, st);
+}
 
-    const int Hd = h->hidden, NQKV = h->qkv_n(), I = h->inter;
-    const long long n8 = (long long)T * I / 8;
-    const int sw_grid = (int)std::min<long long>((n8 + 255) / 256, 8LL * rsb::device_num_sms());
-    embed_rows_kernel<<<T, 128, 0, st>>>(ids, h->embed, Hd, X);
-    for (int li = 0; li < h->layers; ++li) {
-        const LlmLayer& l = h->L[li];
-        rms_rows_kernel<<<T, 256, 0, st>>>(X, nullptr, Hd, l.ln1, h->eps, Hn);
-        if ((rc = gemm(Hn, T, l.wqkv, NQKV, Hd, h->zero_bias, nullptr, QKV, 0, st)) != RSB_OK) return rc;
-        attention_step(h, QKV, cu_seqlens, B, T, d_items, n_items, CTX, st);
-        if ((rc = gemm(CTX, T, l.wo, Hd, Hd, h->zero_bias, X, X, 2, st)) != RSB_OK) return rc;
-        rms_rows_kernel<<<T, 256, 0, st>>>(X, nullptr, Hd, l.ln2, h->eps, Hn);
-        if ((rc = gemm(Hn, T, l.wgu, 2 * I, Hd, h->zero_bias, nullptr, GU, 0, st)) != RSB_OK) return rc;
-        swiglu_kernel<<<sw_grid, 256, 0, st>>>(GU, n8, I, ACT);
-        if ((rc = gemm(ACT, T, l.wdown, Hd, I, h->zero_bias, X, X, 2 | RSB_GEMM_REVERSED, st)) != RSB_OK) return rc;
-    }
-    return RSB_OK;
+// The final norm of the label rows X[rows[i]] into out[i], i < n.
+void final_norm(const rsb_llm* h, const __half* X, const int* rows, int n, __half* out, cudaStream_t st) {
+    if (h->neox)
+        ln_rows_kernel<<<n, LN_THREADS, 0, st>>>(const_cast<__half*>(X), nullptr, rows, h->hidden, h->final_g, h->final_b,
+                                                 nullptr, nullptr, h->eps, out, nullptr);
+    else
+        rms_rows_kernel<<<n, 256, 0, st>>>(X, rows, h->hidden, h->final_g, h->eps, out);
 }
 
 }  // namespace
@@ -646,7 +999,7 @@ extern "C" int rsb_llm_nll(rsb_llm_t* h, const int32_t* ids, const int32_t* cu_s
     const int Hd = h->hidden, chunk = h->chunk_rows();
     for (int c0 = 0; c0 < nl; c0 += chunk) {
         const int n = std::min(chunk, nl - c0);
-        rms_rows_kernel<<<n, 256, 0, st>>>(X, d_rows + c0, Hd, h->final_g, h->eps, Hn);
+        final_norm(h, X, d_rows + c0, n, Hn, st);
         if ((rc = gemm(Hn, n, h->lm_head, h->vocab_pad, Hd, h->zero_bias, nullptr, LOG, 0, st)) != RSB_OK) return rc;
         nll_rows_kernel<<<n, 256, 0, st>>>(LOG, h->vocab, h->vocab_pad, d_labs + c0, d_outi + c0, nll_out);
     }
@@ -675,7 +1028,8 @@ extern "C" int rsb_llm_hidden_states(rsb_llm_t* h, const int32_t* ids, const int
     return RSB_OK;
 }
 
-// Diagnostic: one attention step of the forward on a caller's fused QKV rows [T, (heads + 2 kv_heads) 128] fp16.
+// Diagnostic: one attention step of the forward on a caller's fused QKV rows [T, (heads + 2 kv_heads) head_dim] fp16
+// (GPT-NeoX: [Q heads | K heads | V heads], as rsb_llm_load permutes query_key_value).
 extern "C" int rsb_llm_attention(rsb_llm_t* h, void* qkv, const int32_t* cu_seqlens, int B, int T, int max_seqlen,
                                  void* ctx, rsb_stream_t stream) {
     if (!h || !qkv || !cu_seqlens || !ctx) return lfail(RSB_ERR_INVALID, "null argument");
@@ -700,5 +1054,25 @@ extern "C" int rsb_llm_attention(rsb_llm_t* h, void* qkv, const int32_t* cu_seql
     if (rc != RSB_OK) return rc;
     const cudaError_t e = cudaPeekAtLastError();
     if (e != cudaSuccess) return lfail(RSB_ERR_CUDA, "attention launch failed: %s", cudaGetErrorString(e));
+    return RSB_OK;
+}
+
+// Diagnostic: ln_rows_kernel, the GPT-NeoX LayerNorm step of the forward, on a caller's rows (rsb.h).
+extern "C" int rsb_llm_layernorm(int hidden, float eps, void* x, const void* add, const int32_t* rows, int n_rows,
+                                 const void* w1, const void* b1, const void* w2, const void* b2, void* out1, void* out2,
+                                 rsb_stream_t stream) {
+    if (!x || (w1 && (!b1 || !out1)) || (w2 && (!b2 || !out2)) || (!w1 && w2))
+        return lfail(RSB_ERR_INVALID, "null argument (x, or a norm's bias or output, or w2 without w1)");
+    if (n_rows < 0 || !(eps > 0.f)) return lfail(RSB_ERR_INVALID, "n_rows must be >= 0 and eps positive");
+    if (hidden <= 0 || hidden % 8 || hidden > LN_MAX_HIDDEN)
+        return lfail(RSB_ERR_UNSUPPORTED, "hidden %ld: the LayerNorm kernel takes multiples of 8 up to %ld", (long)hidden,
+                     (long)LN_MAX_HIDDEN);
+    if (n_rows == 0) return RSB_OK;
+    auto h16 = [](const void* p) { return static_cast<const __half*>(p); };
+    ln_rows_kernel<<<n_rows, LN_THREADS, 0, (cudaStream_t)stream>>>(
+        static_cast<__half*>(x), h16(add), rows, hidden, h16(w1), h16(b1), h16(w2), h16(b2), eps,
+        static_cast<__half*>(out1), static_cast<__half*>(out2));
+    const cudaError_t e = cudaPeekAtLastError();
+    if (e != cudaSuccess) return lfail(RSB_ERR_CUDA, "layernorm launch failed: %s", cudaGetErrorString(e));
     return RSB_OK;
 }

@@ -195,7 +195,8 @@ def build_doc_prompts(eval_data, args) -> Tuple[List[str], List[str], int]:
 
 def reader_inputs(tokenizer, context: str, answer: str, max_len: int, pad_token: int) -> Tuple[List[int], List[int]]:
     """(input_ids, labels) of one window as the reference builds them (evaluate_perplexity.py:121-132)."""
-    ctx = tokenizer(context, truncation=False)["input_ids"]    # both tokenisations add BOS: the answer's BOS is scored
+    # a tokenizer that adds BOS (Llama) adds it to both: the answer's BOS is scored; Pythia's adds none
+    ctx = tokenizer(context, truncation=False)["input_ids"]
     ans = tokenizer(answer, truncation=False)["input_ids"]
     ids = list(ctx) + list(ans)
     labels = [IGNORE] * len(ctx) + list(ans)

@@ -1,4 +1,5 @@
-"""GPU reader LM for perplexity evaluation: HF `LlamaForCausalLM` (Llama-2 MHA, Llama-3 GQA) in fp16 on librsb.
+"""GPU reader LM for perplexity evaluation in fp16 on librsb: HF `LlamaForCausalLM` (Llama-2 MHA, Llama-3 GQA) and
+HF `GPTNeoXForCausalLM` (the Pythia suite, whose pythia-1b is the reference's default `model.lm_model`).
 
 The reference loads its reader with `AutoModelForCausalLM.from_pretrained(cfg.model.lm_model, torch_dtype=bfloat16)`
 and calls `lm(input_ids, labels=labels)` one window at a time (`src/evaluate_perplexity.py:98-134`).  Here
@@ -8,9 +9,10 @@ and calls `lm(input_ids, labels=labels)` one window at a time (`src/evaluate_per
     losses = model.loss([ids_0, ...], [labels_0, ...])          # HF's per-window mean loss
 
 runs `rsb_llm_nll`: a prefill-only forward over packed, un-padded windows whose LM head runs only on the rows whose
-next token is a label.  No CPU / eager-PyTorch fallback: constructing the model without CUDA raises.  A checkpoint the
-kernels do not run (another `model_type` such as GPT-NeoX / Pythia, another head_dim, RoPE scaling, biases, ...) raises
-AttributeError naming the field before any weight is read or device memory is allocated.
+next token is a label.  `load_reader` picks `B200Llama` or `B200NeoX` from the config's `model_type`.  No CPU /
+eager-PyTorch fallback: constructing the model without CUDA raises.  A checkpoint the kernels do not run (another
+`model_type`, another head_dim, RoPE scaling, a sequential residual, ...) raises AttributeError naming the field before
+any weight is read or device memory is allocated.
 """
 from __future__ import annotations
 
@@ -75,6 +77,72 @@ def llama_geometry(cfg) -> dict:
                 tie_word_embeddings=bool(_get(cfg, "tie_word_embeddings", False)))
 
 
+NEOX_HEAD_DIMS = (64, 80, 128, 256)
+NEOX_MAX_HIDDEN = 8192                           # ln_rows_kernel's widest row
+
+
+def neox_geometry(cfg) -> dict:
+    """The GPT-NeoX reader geometry the kernels run, from an HF config in the Hub's form (`rotary_pct`,
+    `rotary_emb_base`) or transformers 5's (`rope_parameters`), or AttributeError naming the field."""
+    mt = _get(cfg, "model_type")
+
+    def refuse(msg):
+        raise AttributeError(f"model_type {mt!r}: {msg}")
+    if mt != "gpt_neox":
+        refuse("only 'gpt_neox' readers run on this path")
+    act = _get(cfg, "hidden_act", "gelu")
+    if act != "gelu":
+        refuse(f"hidden_act {act!r}: only the exact-erf 'gelu' is implemented")
+    hidden, heads = _get(cfg, "hidden_size"), _get(cfg, "num_attention_heads")
+    if not hidden or not heads or hidden <= 0 or heads <= 0 or hidden % heads:
+        refuse(f"hidden_size {hidden} is not a multiple of num_attention_heads {heads}")
+    head_dim = hidden // heads
+    if head_dim not in NEOX_HEAD_DIMS:
+        refuse(f"head_dim {head_dim} (hidden_size {hidden} / num_attention_heads {heads}): only head_dim "
+               f"{', '.join(map(str, NEOX_HEAD_DIMS))} is implemented")
+    if hidden > NEOX_MAX_HIDDEN:
+        refuse(f"hidden_size {hidden}: the LayerNorm kernel holds rows of at most {NEOX_MAX_HIDDEN} (Pythia-12B: 5120)")
+    inter = _get(cfg, "intermediate_size")
+    if hidden % 128 or not inter or inter % 128:
+        refuse(f"hidden_size {hidden} / intermediate_size {inter}: both must be multiples of 128")
+    pct, base = _get(cfg, "rotary_pct", 0.25), _get(cfg, "rotary_emb_base", 10000.0)
+    rp = _get(cfg, "rope_parameters")
+    if isinstance(rp, dict):                     # transformers >= 5: rope_parameters carries the factor and the base
+        if rp.get("rope_type", "default") != "default":
+            refuse(f"rope_parameters {rp}: only the default RoPE is implemented")
+        pct, base = rp.get("partial_rotary_factor", pct), rp.get("rope_theta", base)
+    if _get(cfg, "rope_scaling") is not None and not (isinstance(rp, dict) and _get(cfg, "rope_scaling") == rp):
+        refuse(f"rope_scaling {_get(cfg, 'rope_scaling')}: only rope_scaling null is implemented")
+    rot = int(head_dim * pct)
+    if rot <= 0 or rot % 2 or rot > head_dim:
+        refuse(f"rotary_ndims {rot} (rotary_pct {pct} x head_dim {head_dim}) must be even and in [2, head_dim]")
+    if not (base and base > 0):
+        refuse(f"rotary_emb_base {base} is not positive")
+    for key, want in (("use_parallel_residual", True), ("attention_bias", True), ("tie_word_embeddings", False)):
+        if bool(_get(cfg, key, want)) != want:
+            refuse(f"{key} {_get(cfg, key)}: only {key} {want} (every Pythia model) is implemented")
+    vocab = _get(cfg, "vocab_size")
+    if not vocab or vocab <= 0:
+        refuse(f"vocab_size {vocab} is not a positive size")
+    layers = _get(cfg, "num_hidden_layers")
+    if not layers or layers <= 0:
+        refuse(f"num_hidden_layers {layers} is not a positive size")
+    return dict(num_hidden_layers=layers, hidden_size=hidden, num_attention_heads=heads, head_dim=head_dim,
+                intermediate_size=inter, vocab_size=vocab, max_position_embeddings=_get(cfg, "max_position_embeddings", 2048),
+                rotary_ndims=rot, rotary_emb_base=float(base), layer_norm_eps=float(_get(cfg, "layer_norm_eps", 1e-5)))
+
+
+def neox_expected_keys(geom: dict) -> List[str]:
+    """Every weight the GPT-NeoX forward reads (HF GPTNeoXForCausalLM names)."""
+    keys = ["gpt_neox.embed_in.weight", "gpt_neox.final_layer_norm.weight", "gpt_neox.final_layer_norm.bias",
+            "embed_out.weight"]
+    for i in range(geom["num_hidden_layers"]):
+        keys += [f"gpt_neox.layers.{i}.{n}.{p}" for n in (
+            "input_layernorm", "post_attention_layernorm", "attention.query_key_value", "attention.dense",
+            "mlp.dense_h_to_4h", "mlp.dense_4h_to_h") for p in ("weight", "bias")]
+    return keys
+
+
 def expected_keys(geom: dict) -> List[str]:
     """Every weight the forward reads (HF LlamaForCausalLM names)."""
     keys = ["model.embed_tokens.weight", "model.norm.weight"]
@@ -92,28 +160,26 @@ def scored_positions(labels: Sequence[int]) -> List[int]:
     return [t for t in range(1, len(labels)) if labels[t] != IGNORE]
 
 
-class B200Llama:
-    """An HF LlamaForCausalLM reader on librsb (`rsb_llm_*`)."""
+class _Reader:
+    """A causal-LM reader on librsb (`rsb_llm_*`): everything but the geometry and the constructor call."""
 
     # tokens per forward that `nll` packs: the GEMMs fill the GPU well before this, and the activations of a
     # Llama-3-8B forward stay near 3 GB
     token_budget = 16384
+    # non-weight buffers of HF checkpoints, skipped by name before any conversion
+    _buffers = ("rotary_emb.inv_freq",)
 
     def __init__(self, config, device=None):
-        self.geom = llama_geometry(config)
+        self.geom = self._geometry(config)
         if not torch.cuda.is_available():
-            raise RuntimeError("B200Llama needs a CUDA device (sm_90a): there is no CPU path")
+            raise RuntimeError(f"{type(self).__name__} needs a CUDA device (sm_90a): there is no CPU path")
         self.L = _lib.lib()
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         self._h = ctypes.c_void_p(0)
         self._ws: Optional[torch.Tensor] = None
         self.loaded = set()
-        g = self.geom
         with torch.cuda.device(self.device):
-            self._check(self.L.rsb_llm_create(
-                g["num_hidden_layers"], g["hidden_size"], g["num_attention_heads"], g["num_key_value_heads"],
-                g["intermediate_size"], g["vocab_size"], g["max_position_embeddings"], ctypes.c_float(g["rope_theta"]),
-                ctypes.c_float(g["rms_norm_eps"]), int(g["tie_word_embeddings"]), ctypes.byref(self._h)))
+            self._check(self._create(self.geom))
 
     def _check(self, rc):
         if rc == _lib.RSB_OK:
@@ -142,7 +208,7 @@ class B200Llama:
     def load_weight(self, name: str, t: torch.Tensor) -> bool:
         """Uploads one HF weight in fp16; False for a name the reader does not use.  A weight that does not stay
         finite in fp16 (a bf16 value beyond 65504) is refused."""
-        if name.endswith("rotary_emb.inv_freq"):
+        if name.endswith(self._buffers):
             return False
         w = t.detach().to(device=self.device, dtype=torch.float16).contiguous()
         if not bool(torch.isfinite(w).all()):
@@ -158,7 +224,7 @@ class B200Llama:
 
     def load_state_dict(self, sd: Dict[str, torch.Tensor], strict: bool = True):
         with torch.cuda.device(self.device):
-            unexpected = [n for n, t in sd.items() if not self.load_weight(n, t) and not n.endswith("rotary_emb.inv_freq")]
+            unexpected = [n for n, t in sd.items() if not self.load_weight(n, t) and not n.endswith(self._buffers)]
         if strict and unexpected:
             raise KeyError(f"unexpected keys in state_dict: {unexpected[:5]}")
         if strict:
@@ -166,7 +232,7 @@ class B200Llama:
         return unexpected
 
     def missing_keys(self):
-        return [k for k in expected_keys(self.geom) if k not in self.loaded]
+        return [k for k in self._expected_keys(self.geom) if k not in self.loaded]
 
     def require_all_weights(self, source: str = "state_dict"):
         missing = self.missing_keys()
@@ -227,9 +293,10 @@ class B200Llama:
 
     # -- diagnostics (rsb_llm_attention / rsb_llm_hidden_states), not used by nll / loss ----------------------------
     def attention(self, qkv: torch.Tensor, cu_seqlens: torch.Tensor, max_seqlen: int, ctx: torch.Tensor):
-        """One attention step of the forward: RoPE in place on the Q / K heads of qkv [T, (heads + 2 kv_heads) 128]
-        fp16, then causal attention into ctx [T, hidden] fp16 for the windows of cu_seqlens (int32 [B + 1], empty
-        windows allowed, may end below T).  Rows outside the windows are left as they are."""
+        """One attention step of the forward: RoPE in place on the Q / K heads of qkv [T, (heads + 2 kv_heads)
+        head_dim] fp16 (GPT-NeoX: [Q heads | K heads | V heads], only the first rotary_ndims of each head rotated),
+        then causal attention into ctx [T, hidden] fp16 for the windows of cu_seqlens (int32 [B + 1], empty windows
+        allowed, may end below T).  Rows outside the windows are left as they are."""
         with torch.cuda.device(self.device):
             rc = self.L.rsb_llm_attention(self._h, ctypes.c_void_p(qkv.data_ptr()), ctypes.c_void_p(cu_seqlens.data_ptr()),
                                           cu_seqlens.numel() - 1, qkv.shape[0], int(max_seqlen),
@@ -262,6 +329,37 @@ class B200Llama:
         return res
 
 
+class B200Llama(_Reader):
+    """An HF LlamaForCausalLM reader on librsb (`rsb_llm_*`)."""
+
+    _geometry = staticmethod(llama_geometry)
+    _expected_keys = staticmethod(expected_keys)
+
+    def _create(self, g):
+        return self.L.rsb_llm_create(
+            g["num_hidden_layers"], g["hidden_size"], g["num_attention_heads"], g["num_key_value_heads"],
+            g["intermediate_size"], g["vocab_size"], g["max_position_embeddings"], ctypes.c_float(g["rope_theta"]),
+            ctypes.c_float(g["rms_norm_eps"]), int(g["tie_word_embeddings"]), ctypes.byref(self._h))
+
+
+class B200NeoX(_Reader):
+    """An HF GPTNeoXForCausalLM reader (Pythia) on librsb (`rsb_llm_create_neox`, then the same `rsb_llm_*`)."""
+
+    _geometry = staticmethod(neox_geometry)
+    _expected_keys = staticmethod(neox_expected_keys)
+    # older checkpoints also carry the causal mask (a 2048 x 2048 bool) and the masked-score constant
+    _buffers = ("rotary_emb.inv_freq", ".attention.bias", ".attention.masked_bias")
+
+    def _create(self, g):
+        return self.L.rsb_llm_create_neox(
+            g["num_hidden_layers"], g["hidden_size"], g["num_attention_heads"], g["intermediate_size"],
+            g["vocab_size"], g["max_position_embeddings"], g["rotary_ndims"], ctypes.c_float(g["rotary_emb_base"]),
+            ctypes.c_float(g["layer_norm_eps"]), ctypes.byref(self._h))
+
+
+READERS = {"llama": (llama_geometry, B200Llama), "gpt_neox": (neox_geometry, B200NeoX)}
+
+
 def _shard_files(directory: str) -> List[str]:
     index = os.path.join(directory, "model.safetensors.index.json")
     if os.path.exists(index):
@@ -271,25 +369,45 @@ def _shard_files(directory: str) -> List[str]:
     single = os.path.join(directory, "model.safetensors")
     if os.path.exists(single):
         return [single]
-    raise FileNotFoundError(f"{directory}: neither model.safetensors nor model.safetensors.index.json is present")
+    # PyTorch pickles, as the Pythia suite publishes its intermediate-step revisions
+    index = os.path.join(directory, "pytorch_model.bin.index.json")
+    if os.path.exists(index):
+        with open(index) as f:
+            files = sorted(set(json.load(f)["weight_map"].values()))
+        return [os.path.join(directory, fn) for fn in files]
+    single = os.path.join(directory, "pytorch_model.bin")
+    if os.path.exists(single):
+        return [single]
+    raise FileNotFoundError(f"{directory}: neither model.safetensors nor model.safetensors.index.json is present "
+                            f"(nor pytorch_model.bin / pytorch_model.bin.index.json)")
 
 
-def load_reader(path: str, device=None) -> B200Llama:
-    """The reader of `cfg.model.lm_model` from a local directory or the Hugging Face cache (never downloaded), with
-    single-file or sharded safetensors weights; bf16 / fp32 weights are converted to fp16."""
-    from safetensors import safe_open
+def _tensors(fn: str):
+    """(name, tensor) of one weight file, safetensors or a PyTorch pickle (read with weights_only=True)."""
+    if fn.endswith(".safetensors"):
+        from safetensors import safe_open
+        with safe_open(fn, framework="pt") as f:
+            for name in f.keys():
+                yield name, f.get_tensor(name)
+    else:
+        yield from torch.load(fn, weights_only=True, map_location="cpu").items()
 
+
+def load_reader(path: str, device=None):
+    """The reader of `cfg.model.lm_model` from a local directory or the Hugging Face cache (never downloaded):
+    `B200Llama` for model_type 'llama', `B200NeoX` for 'gpt_neox'.  Single-file or sharded safetensors weights, or
+    PyTorch `pytorch_model.bin` files when no safetensors file is present; bf16 / fp32 weights are converted to fp16."""
     from .encoder import _resolve_model_dir
     directory = _resolve_model_dir(path)
     with open(os.path.join(directory, "config.json")) as f:
         cfg = json.load(f)
-    llama_geometry(cfg)                          # refuses before any weight is read or device memory allocated
+    geometry, cls = READERS.get(cfg.get("model_type"), READERS["llama"])
+    geometry(cfg)                                # refuses before any weight is read or device memory allocated
     files = _shard_files(directory)
-    model = B200Llama(cfg, device=device)
+    model = cls(cfg, device=device)
     with torch.cuda.device(model.device):
         for fn in files:
-            with safe_open(fn, framework="pt") as f:
-                for name in f.keys():
-                    model.load_weight(name, f.get_tensor(name))
+            for name, t in _tensors(fn):
+                model.load_weight(name, t)
     model.require_all_weights(directory)
     return model

@@ -4,6 +4,7 @@ sdpa attention, the reference's reader path minus flash-attn-2 (src/evaluate_per
 and the same windows.
 
 Seeded weights with the full-depth geometry of Llama-2-7B (MHA, vocab 32000) and Llama-3-8B (GQA 4:1, vocab 128256),
+or of Pythia-1B (head_dim 256), Pythia-1.4B and Pythia-6.9B (GPT-NeoX: librsb's B200NeoX against HF GPTNeoXForCausalLM),
 generated on the device.  --windows windows of --context context tokens (retrieved documents + query, label -100)
 followed by --answer answer tokens (the labels), as the reference builds them with concate_k documents in front of a
 1024-token evaluation chunk.  Timed with CUDA events after --warmup passes, --repeats passes per model, the median
@@ -33,11 +34,59 @@ GEOMETRY = {
                       num_key_value_heads=8, intermediate_size=14336, vocab_size=128256, max_position_embeddings=8192,
                       rope_theta=500000.0, rms_norm_eps=1e-5, hidden_act="silu", tie_word_embeddings=False),
 }
+_PYTHIA = dict(model_type="gpt_neox", max_position_embeddings=2048, rotary_pct=0.25, rotary_emb_base=10000,
+               layer_norm_eps=1e-5, hidden_act="gelu", use_parallel_residual=True, tie_word_embeddings=False)
+GEOMETRY.update({
+    "pythia-1b": dict(_PYTHIA, num_hidden_layers=16, hidden_size=2048, num_attention_heads=8, intermediate_size=8192,
+                      vocab_size=50304),
+    "pythia-1.4b": dict(_PYTHIA, num_hidden_layers=24, hidden_size=2048, num_attention_heads=16, intermediate_size=8192,
+                        vocab_size=50304),
+    "pythia-6.9b": dict(_PYTHIA, num_hidden_layers=32, hidden_size=4096, num_attention_heads=32,
+                        intermediate_size=16384, vocab_size=50432),
+})
 PEAK_TFLOPS = 989.0
+
+
+def neox(cfg):
+    return cfg["model_type"] == "gpt_neox"
+
+
+def head_dim(cfg):
+    return cfg["hidden_size"] // cfg["num_attention_heads"]
+
+
+def kv_heads(cfg):
+    return cfg.get("num_key_value_heads", cfg["num_attention_heads"])
+
+
+def neox_weights(cfg, seed=0):
+    """GPTNeoXForCausalLM (name, fp16 tensor on the device) in HF order, regenerated from the seed for each path."""
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    H, I, V = cfg["hidden_size"], cfg["intermediate_size"], cfg["vocab_size"]
+
+    def n(*shape, std):
+        return torch.randn(*shape, generator=g, device="cuda", dtype=torch.float16) * std
+
+    yield "gpt_neox.embed_in.weight", n(V, H, std=1.0)
+    for i in range(cfg["num_hidden_layers"]):
+        p = f"gpt_neox.layers.{i}."
+        for ln in ("input_layernorm", "post_attention_layernorm"):
+            yield p + ln + ".weight", 1.0 + n(H, std=0.05)
+            yield p + ln + ".bias", n(H, std=0.05)
+        for name, shape, fan in (("attention.query_key_value", (3 * H, H), H), ("attention.dense", (H, H), H),
+                                 ("mlp.dense_h_to_4h", (I, H), H), ("mlp.dense_4h_to_h", (H, I), I)):
+            yield p + name + ".weight", n(*shape, std=fan ** -0.5)
+            yield p + name + ".bias", n(shape[0], std=0.02)
+    yield "gpt_neox.final_layer_norm.weight", 1.0 + n(H, std=0.05)
+    yield "gpt_neox.final_layer_norm.bias", n(H, std=0.05)
+    yield "embed_out.weight", n(V, H, std=2.0 * H ** -0.5)
 
 
 def weights(cfg, seed=0):
     """(name, fp16 tensor on the device) in HF order, regenerated from the seed for each path."""
+    if neox(cfg):
+        yield from neox_weights(cfg, seed)
+        return
     g = torch.Generator(device="cuda").manual_seed(seed)
     H, I, V = cfg["hidden_size"], cfg["intermediate_size"], cfg["vocab_size"]
     KV = cfg["num_key_value_heads"] * 128
@@ -69,10 +118,11 @@ def windows(cfg, n, context, answer, seed=1):
 def model_flops(cfg, context, answer):
     """FLOPs of one window: linear layers on every token, causal attention, LM head on the label rows."""
     H, I, L = cfg["hidden_size"], cfg["intermediate_size"], cfg["num_hidden_layers"]
-    KV = cfg["num_key_value_heads"] * 128
+    KV = kv_heads(cfg) * head_dim(cfg)
     S = context + answer
-    lin = 2 * S * L * (H * (H + 2 * KV) + H * H + 3 * H * I)
-    att = 2 * 2 * L * cfg["num_attention_heads"] * 128 * S * (S + 1) // 2
+    mlp = (2 if neox(cfg) else 3) * H * I            # GELU MLP: two matrices; SwiGLU: three
+    lin = 2 * S * L * (H * (H + 2 * KV) + H * H + mlp)
+    att = 2 * 2 * L * cfg["num_attention_heads"] * head_dim(cfg) * S * (S + 1) // 2
     head = 2 * answer * H * cfg["vocab_size"]
     return lin + att + head
 
@@ -109,8 +159,8 @@ def kernel_table(fn, n_windows):
 
 
 def bench_rsb(cfg, ids, labels, args):
-    from retrieval_scaling_b200.reader import B200Llama
-    m = B200Llama(cfg)
+    from retrieval_scaling_b200.reader import B200Llama, B200NeoX
+    m = (B200NeoX if neox(cfg) else B200Llama)(cfg)
     for name, w in weights(cfg):
         m.load_weight(name, w)
         del w
@@ -129,10 +179,10 @@ def bench_rsb(cfg, ids, labels, args):
 def bench_hf(cfg, ids, labels, args):
     import transformers
     kw = {k: v for k, v in cfg.items() if k != "model_type"}
-    hc = transformers.LlamaConfig(**kw)
+    hc = (transformers.GPTNeoXConfig if neox(cfg) else transformers.LlamaConfig)(**kw)
     hc._attn_implementation = "sdpa"
     with torch.device("meta"):
-        lm = transformers.LlamaForCausalLM(hc)
+        lm = (transformers.GPTNeoXForCausalLM if neox(cfg) else transformers.LlamaForCausalLM)(hc)
     lm = lm.to_empty(device="cuda").to(torch.bfloat16).eval()
     params = dict(lm.named_parameters())
     with torch.no_grad():
