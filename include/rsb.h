@@ -486,6 +486,32 @@ int rsb_llm_create(int layers, int hidden, int heads, int kv_heads, int intermed
  *     first rotary_dims of each Q / K head (the other dims are left bit-identical) and scales by head_dim^-0.5. */
 int rsb_llm_create_neox(int layers, int hidden, int heads, int intermediate, int vocab, int max_pos, int rotary_dims,
                         float rotary_base, float ln_eps, rsb_llm_t** out);
+/* OLMo readers, a third constructor for the same handle type: version 1 = HF OlmoForCausalLM (OLMo-1B/7B-hf, OLMo-1.7),
+ * version 2 = Olmo2ForCausalLM (OLMo-2).  The geometry rules of rsb_llm_create apply (head_dim 128 with hidden == 128 *
+ * heads, heads % kv_heads == 0, intermediate % 128 == 0: else RSB_ERR_UNSUPPORTED; non-positive sizes, rope_theta or eps
+ * RSB_ERR_INVALID), and also: version other than 1 or 2 RSB_ERR_INVALID; clip_qkv negative, infinite or NaN, or non-zero
+ * with version 2, RSB_ERR_INVALID; version 1 with hidden > 8192 (the LayerNorm kernel's widest row) RSB_ERR_UNSUPPORTED.
+ * All before any CUDA call.  The forward is HF's in fp16, a Llama layer (SwiGLU, no biases, default RoPE with
+ * inv_freq = 1 / rope_theta ** (2i / 128) in fp32, causal GQA attention scaled by 128^-0.5) except:
+ *   RoPE keeps cos / sin in fp32: x * cos + rotate_half(x) * sin is evaluated in fp32 and rounded to half once;
+ *   version 1: both pre-norms and the final norm are OlmoLayerNorm, without weight or bias: fp16 of the fp32
+ *     (x - mean) * rsqrt(biased var + eps), one rounding; eps is 1e-5 in HF (no config field).  clip_qkv > 0 clamps every
+ *     q, k and v projection element to [-clip_qkv, clip_qkv] before RoPE; 0 = none (HF clip_qkv null);
+ *   version 2: no pre-norms.  x = fp16(x + post_attention_layernorm(o_proj(attn(x)))), then x = fp16(x +
+ *     post_feedforward_layernorm(mlp(x))).  Every norm is Olmo2RMSNorm, fp16(w * (x * rsqrt(mean(x^2) + eps))) with the
+ *     weight multiply in fp32 and one rounding; q_norm normalises the whole q projection (hidden wide) and k_norm the
+ *     whole k projection (kv_heads * 128 wide), before RoPE; the final model.norm is one too.  eps = rms_norm_eps.
+ * tied = 1 (tie_word_embeddings): the LM head is model.embed_tokens.weight.  rsb_llm_load, _workspace_bytes, _nll,
+ * _hidden_states, _attention and _free take OLMo handles; on them
+ *   rsb_llm_load takes "model.embed_tokens.weight", "lm_head.weight" (untied; accepted and ignored when tied) and
+ *     "model.layers.N.{self_attn.{q,k,v,o}_proj, mlp.{gate,up,down}_proj}.weight"; version 2 also "model.norm.weight" and
+ *     "model.layers.N.{self_attn.q_norm, self_attn.k_norm, post_attention_layernorm, post_feedforward_layernorm}.weight".
+ *     Version 1 has no norm weights: a norm name is an unknown weight (RSB_ERR_INVALID);
+ *   rsb_llm_hidden_states returns the residual stream before the final norm;
+ *   rsb_llm_attention runs layer 0's prologue in place of RoPE: the clip_qkv clamp of q, k and v (version 1), or q_norm /
+ *     k_norm (version 2; RSB_ERR_STATE until layer 0's q_norm and k_norm are loaded), then the fp32-cos / sin RoPE. */
+int rsb_llm_create_olmo(int version, int layers, int hidden, int heads, int kv_heads, int intermediate, int vocab,
+                        int max_pos, float rope_theta, float eps, float clip_qkv, int tied, rsb_llm_t** out);
 /* name = HF LlamaForCausalLM state_dict key: "model.embed_tokens.weight", "model.norm.weight", "lm_head.weight"
  * (untied; accepted and ignored when tied) and "model.layers.N.{self_attn.{q,k,v,o}_proj, mlp.{gate,up,down}_proj,
  * input_layernorm, post_attention_layernorm}.weight"; data fp16 on the device, copied. */
@@ -525,6 +551,16 @@ int rsb_llm_hidden_states(rsb_llm_t* h, const int32_t* ids_dev, const int32_t* c
 int rsb_llm_layernorm(int hidden, float eps, void* x_dev, const void* add_dev, const int32_t* rows_dev, int n_rows,
                       const void* w1_dev, const void* b1_dev, const void* w2_dev, const void* b2_dev, void* out1_dev,
                       void* out2_dev, rsb_stream_t stream);
+/* Diagnostic, not used on the product path: the OLMo-2 norm step of rsb_llm_nll's forward on a caller's fp16 rows of
+ * `hidden` elements, with Olmo2RMSNorm norm(v) = fp16(w * (v * rsqrt(mean(v^2) + eps))) (fp32 statistics, the weight
+ * multiply in fp32, one rounding).  Row i reads row r = rows_dev ? rows_dev[i] : i, i < n_rows.
+ *   a_dev != NULL: x[r] = fp16(x[r] + norm(a[r])) in place (the post-norm residual add); out_dev is not written.
+ *   a_dev == NULL: out[i] = norm(x[r]) (the final norm); x_dev is read only.
+ * A null x_dev or w_dev, or a null out_dev without a_dev, RSB_ERR_INVALID; hidden not a positive multiple of 8
+ * RSB_ERR_UNSUPPORTED; both before any launch.  No handle is needed. (OLMo's LayerNorm is rsb_llm_layernorm with unit
+ * w1 and zero b1.) */
+int rsb_llm_olmo2_norm(int hidden, float eps, void* x_dev, const void* a_dev, const int32_t* rows_dev, int n_rows,
+                       const void* w_dev, void* out_dev, rsb_stream_t stream);
 
 /* ---- MinHash de-duplication of retrieved passages ----------------------------------------------------------------
  * Replaces utils/deduplication.py's `remove_duplicates_with_minhash` (datasketch MinHash(num_perm=128) and

@@ -102,6 +102,10 @@ SIGNATURES = [
                                       c_void_p]),                                                   # diagnostic
     ("rsb_llm_layernorm", c_int, [c_int, c_float, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
                                   c_void_p, c_void_p, c_void_p, c_void_p]),                          # diagnostic
+    ("rsb_llm_create_olmo", c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_float,
+                                    c_int, POINTER(_H)]),
+    ("rsb_llm_olmo2_norm", c_int, [c_int, c_float, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
+                                   c_void_p]),                                                       # diagnostic
     ("rsb_dedup_last_error", c_char_p, []),
     ("rsb_minhash_workspace_bytes", c_size_t, [c_int64]),
     ("rsb_minhash_signatures", c_int, [c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,

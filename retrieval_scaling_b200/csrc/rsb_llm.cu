@@ -1,6 +1,6 @@
-// rsb_llm.cu -- reader-LM forward for perplexity evaluation: HF LlamaForCausalLM (Llama-2 MHA, Llama-3 GQA) and
-// GPTNeoXForCausalLM (Pythia; rsb_llm_create_neox) in fp16, prefill only, over packed un-padded sequences, ending in
-// the per-token negative log-likelihood of the labels.
+// rsb_llm.cu -- reader-LM forward for perplexity evaluation: HF LlamaForCausalLM (Llama-2 MHA, Llama-3 GQA),
+// GPTNeoXForCausalLM (Pythia; rsb_llm_create_neox) and OlmoForCausalLM / Olmo2ForCausalLM (rsb_llm_create_olmo) in
+// fp16, prefill only, over packed un-padded sequences, ending in the per-token negative log-likelihood of the labels.
 // Replaces the reader call of the reference's perplexity loop (src/evaluate_perplexity.py:126-134: `lm(input_ids,
 // labels=labels)` one window at a time, HF in bf16).  No KV cache, no generation.
 //
@@ -13,6 +13,8 @@
 //                            every packed sequence
 //   ln_rows_kernel           GPT-NeoX: torch's fp16 LayerNorm, with the parallel residual's last add and both norms fused
 //   rope_partial_kernel      GPT-NeoX: rotate_half on the first rotary_dims of each Q / K head
+//   olmo_qkv_kernel          OLMo / OLMo-2: clip_qkv clamp or whole-projection QK RMSNorm, then RoPE with fp32 cos / sin
+//   rms_post_kernel          OLMo-2: Olmo2RMSNorm (weight multiply in fp32) fused with the post-norm residual add
 //   attention_causal_kernel  causal flash attention, head_dim 64 / 80 / 128 / 256, GQA, mma.sync.m16n8k16 with fp32 running max / sum;
 //                            key blocks above the diagonal are never visited
 //   swiglu_kernel            act = fp16(fp16(silu(gate)) * up), HF LlamaMLP's order
@@ -226,6 +228,118 @@ void ln_rows_kernel(__half* __restrict__ X, const __half* __restrict__ add, cons
                 o2[e] = __floats2half2_rn(fmaf((f.x - mean) * rstd, gf.x, bf.x), fmaf((f.y - mean) * rstd, gf.y, bf.y));
             }
             o[c] = ov;
+        }
+    }
+}
+
+// OLMo / OLMo-2 attention prologue on the fused QKV rows ([Q heads | K heads | V heads], 128 wide), HF's order.  One
+// block per token; positions restart at 0 in every packed sequence.
+//   clip > 0 (OLMo clip_qkv): every Q, K and V element is clamped to [-clip, clip] (in fp32, rounded to half).
+//   qn != nullptr (OLMo-2 q_norm / k_norm): Q = fp16(qn * (Q * rsqrt(mean(Q^2) + eps))) over the whole Q projection
+//   (heads x 128 wide, not per head), K likewise with kn over kv_heads x 128: fp32 statistics, the weight multiply in
+//   fp32, one rounding, which RoPE then reads.
+//   RoPE: OlmoRotaryEmbedding / Olmo2RotaryEmbedding keep cos / sin in fp32, so x * cos + rotate_half(x) * sin is
+//   evaluated in fp32 (each product and the sum one fp32 rounding, as torch promotes) and rounded to half once.
+__global__ __launch_bounds__(256)
+void olmo_qkv_kernel(__half* __restrict__ qkv, const int* __restrict__ cu_seqlens, int B, int heads, int kv_heads,
+                     const float* __restrict__ inv_freq, float clip, const __half* __restrict__ qn,
+                     const __half* __restrict__ kn, float eps) {
+    __shared__ float red[8];
+    const int t = blockIdx.x;
+    int lo = 0, hi = B;
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (cu_seqlens[mid] <= t) lo = mid; else hi = mid;
+    }
+    const float pos = (float)(t - cu_seqlens[lo]);
+    const int nq = heads * HD, nk = kv_heads * HD;
+    __half* row = qkv + (size_t)t * (nq + 2 * nk);
+    float rq = 1.f, rk = 1.f;
+    if (qn) {
+        float sq = 0.f, sk = 0.f;
+        const uint4* v = reinterpret_cast<const uint4*>(row);
+        for (int c = threadIdx.x; c < (nq + nk) / 8; c += blockDim.x) {
+            const uint4 u = v[c];
+            const __half2* h2 = reinterpret_cast<const __half2*>(&u);
+            float s = 0.f;
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const float2 f = __half22float2(h2[e]);
+                s = fmaf(f.x, f.x, s);
+                s = fmaf(f.y, f.y, s);
+            }
+            if (c < nq / 8) sq += s; else sk += s;
+        }
+        rq = rsqrtf(block_sum(sq, red) / (float)nq + eps);   // every read of the row precedes block_sum's barriers
+        rk = rsqrtf(block_sum(sk, red) / (float)nk + eps);
+    }
+    auto clamped = [clip](float x) { return __half2float(__float2half_rn(fminf(fmaxf(x, -clip), clip))); };
+    for (int p = threadIdx.x; p < (heads + kv_heads) * (HD / 2); p += blockDim.x) {
+        const int hh = p / (HD / 2), i = p % (HD / 2);
+        __half* x = row + hh * HD;
+        float x1 = __half2float(x[i]), x2 = __half2float(x[i + HD / 2]);
+        if (clip > 0.f) { x1 = clamped(x1); x2 = clamped(x2); }
+        if (qn) {
+            const bool q = hh < heads;
+            const __half* w = q ? qn + hh * HD : kn + (hh - heads) * HD;
+            const float r = q ? rq : rk;
+            x1 = __half2float(__float2half_rn(__fmul_rn(__half2float(w[i]), __fmul_rn(x1, r))));
+            x2 = __half2float(__float2half_rn(__fmul_rn(__half2float(w[i + HD / 2]), __fmul_rn(x2, r))));
+        }
+        const float f = inv_freq[i] * pos;
+        const float c = cosf(f), s = sinf(f);
+        x[i] = __float2half_rn(__fadd_rn(__fmul_rn(x1, c), __fmul_rn(-x2, s)));
+        x[i + HD / 2] = __float2half_rn(__fadd_rn(__fmul_rn(x2, c), __fmul_rn(x1, s)));
+    }
+    if (clip > 0.f)
+        for (int e = threadIdx.x; e < nk; e += blockDim.x) row[nq + nk + e] = __float2half_rn(clamped(__half2float(row[nq + nk + e])));
+}
+
+// Olmo2RMSNorm: fp16(w * (x * rsqrt(mean(x^2) + eps))) with fp32 statistics, the weight multiply in fp32 and one
+// rounding (LlamaRMSNorm rounds to half before the weight).  One block per output row i, input row r = rows ? rows[i] : i.
+//   A != nullptr: X[r] = fp16(X[r] + norm(A[r])), OLMo-2's post-norm residual add, in place; out is not written.
+//   A == nullptr: out[i] = norm(X[r]), the final norm on the label rows.
+__global__ __launch_bounds__(256)
+void rms_post_kernel(__half* __restrict__ X, const __half* __restrict__ A, const int* __restrict__ rows, int hidden,
+                     const __half* __restrict__ w, float eps, __half* __restrict__ out) {
+    __shared__ float red[8];
+    const int i = blockIdx.x;
+    const int r = rows ? rows[i] : i;
+    const uint4* a = reinterpret_cast<const uint4*>((A ? A : X) + (size_t)r * hidden);
+    float s = 0.f;
+    for (int c = threadIdx.x; c < hidden / 8; c += blockDim.x) {
+        const uint4 v = a[c];
+        const __half2* h2 = reinterpret_cast<const __half2*>(&v);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const float2 f = __half22float2(h2[e]);
+            s = fmaf(f.x, f.x, s);
+            s = fmaf(f.y, f.y, s);
+        }
+    }
+    const float rstd = rsqrtf(block_sum(s, red) / (float)hidden + eps);
+    const uint4* wv = reinterpret_cast<const uint4*>(w);
+    uint4* x = reinterpret_cast<uint4*>(X + (size_t)r * hidden);
+    uint4* o = reinterpret_cast<uint4*>(out + (size_t)i * hidden);
+    for (int c = threadIdx.x; c < hidden / 8; c += blockDim.x) {
+        const uint4 v = a[c], g = wv[c];
+        const __half2* h2 = reinterpret_cast<const __half2*>(&v);
+        const __half2* g2 = reinterpret_cast<const __half2*>(&g);
+        uint4 nv;
+        __half2* n2 = reinterpret_cast<__half2*>(&nv);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const float2 f = __half22float2(h2[e]), gf = __half22float2(g2[e]);
+            n2[e] = __floats2half2_rn(__fmul_rn(gf.x, __fmul_rn(f.x, rstd)), __fmul_rn(gf.y, __fmul_rn(f.y, rstd)));
+        }
+        if (A) {
+            uint4 xv = x[c];
+            __half2* x2 = reinterpret_cast<__half2*>(&xv);
+#pragma unroll
+            for (int e = 0; e < 4; ++e) x2[e] = __hadd2(x2[e], n2[e]);
+            x[c] = xv;
+        } else {
+            o[c] = nv;
         }
     }
 }
@@ -526,10 +640,12 @@ int lfail(int code, const char* fmt, ...) {
 }
 
 // Llama: wgu = gate | up, no biases.  GPT-NeoX: wgu = dense_h_to_4h, wdown = dense_4h_to_h, wqkv = query_key_value
-// with its rows permuted to [Q heads | K heads | V heads], and the biases and LayerNorm biases below.
+// with its rows permuted to [Q heads | K heads | V heads], and the biases and LayerNorm biases below.  OLMo-2: ln1 / ln2
+// = post_attention_layernorm / post_feedforward_layernorm, qn / kn = self_attn.q_norm / k_norm.
 struct LlmLayer {
     __half *wqkv = nullptr, *wo = nullptr, *wgu = nullptr, *wdown = nullptr, *ln1 = nullptr, *ln2 = nullptr;
     __half *bqkv = nullptr, *bo = nullptr, *bgu = nullptr, *bdown = nullptr, *ln1b = nullptr, *ln2b = nullptr;
+    __half *qn = nullptr, *kn = nullptr;
 };
 
 }  // namespace
@@ -537,14 +653,22 @@ struct LlmLayer {
 struct rsb_llm {
     int layers = 0, hidden = 0, heads = 0, kv_heads = 0, inter = 0, vocab = 0, vocab_pad = 0, max_pos = 0;
     int head_dim = HD, rot = HD;                 // rot: rotated dims of each Q / K head (GPT-NeoX rotary_ndims)
-    float rope_theta = 0.f, eps = 0.f;
+    int olmo = 0;                                // 1 = OLMo, 2 = OLMo-2 (rsb_llm_create_olmo), 0 otherwise
+    float rope_theta = 0.f, eps = 0.f, clip = 0.f;   // clip: OLMo clip_qkv, 0 = none
     bool tied = false, neox = false;
+    // OLMo: final_g holds ones, the unit scale with which ln_rows_kernel (and zero_bias as its shift) is OlmoLayerNorm
     __half *embed = nullptr, *lm_head = nullptr, *final_g = nullptr, *final_b = nullptr, *zero_bias = nullptr;
     float* inv_freq = nullptr;
     std::vector<LlmLayer> L;
     std::set<std::string> loaded;                // required weights loaded so far
     int qkv_n() const { return (heads + 2 * kv_heads) * head_dim; }
-    size_t required() const { return neox ? 4 + 12 * (size_t)layers : 2 + 9 * (size_t)layers + (tied ? 0 : 1); }
+    size_t required() const {
+        const size_t head = tied ? 0 : 1;
+        if (neox) return 4 + 12 * (size_t)layers;
+        if (olmo == 1) return 1 + 7 * (size_t)layers + head;
+        if (olmo == 2) return 2 + 11 * (size_t)layers + head;
+        return 2 + 9 * (size_t)layers + head;
+    }
     int chunk_rows() const { return (int)std::max<size_t>(128, LOGIT_BYTES / ((size_t)vocab_pad * 2) / 128 * 128); }
 };
 
@@ -689,6 +813,44 @@ extern "C" int rsb_llm_create_neox(int layers, int hidden, int heads, int interm
     return RSB_OK;
 }
 
+// Replaces the same call for OLMo (version 1, OlmoForCausalLM) and OLMo-2 (version 2, Olmo2ForCausalLM) readers: the
+// Llama handle with OLMo's norms, clip_qkv, QK-norm and fp32 rotary.  Every refusal comes before any CUDA call
+// (rsb_llm_create's included).
+extern "C" int rsb_llm_create_olmo(int version, int layers, int hidden, int heads, int kv_heads, int intermediate,
+                                   int vocab, int max_pos, float rope_theta, float eps, float clip_qkv, int tied,
+                                   rsb_llm_t** out) {
+    if (!out) return lfail(RSB_ERR_INVALID, "out is NULL");
+    *out = nullptr;
+    if (version != 1 && version != 2)
+        return lfail(RSB_ERR_INVALID, "version %ld is neither 1 (OLMo) nor 2 (OLMo-2)", (long)version);
+    if (!(clip_qkv >= 0.f) || std::isinf(clip_qkv) || (version == 2 && clip_qkv != 0.f))
+        return lfail(RSB_ERR_INVALID, "clip_qkv must be finite and >= 0 (0 = none), and 0 for OLMo-2");
+    if (version == 1 && hidden > LN_MAX_HIDDEN)
+        return lfail(RSB_ERR_UNSUPPORTED, "hidden %ld: the LayerNorm kernel holds rows of at most %ld", (long)hidden,
+                     (long)LN_MAX_HIDDEN);
+    int rc = rsb_llm_create(layers, hidden, heads, kv_heads, intermediate, vocab, max_pos, rope_theta, eps, tied, out);
+    if (rc != RSB_OK) return rc;
+    rsb_llm* h = *out;
+    h->olmo = version;
+    h->clip = clip_qkv;
+    bool ok = true;
+    if (version == 1) {
+        const std::vector<__half> ones(hidden, __float2half(1.f));
+        ok = cudaMemcpy(h->final_g, ones.data(), (size_t)hidden * 2, cudaMemcpyHostToDevice) == cudaSuccess;
+    } else {
+        for (auto& l : h->L) {
+            ok &= cudaMalloc(&l.qn, (size_t)hidden * 2) == cudaSuccess;
+            ok &= cudaMalloc(&l.kn, (size_t)kv_heads * HD * 2) == cudaSuccess;
+        }
+    }
+    if (!ok) {
+        rsb_llm_free(h);
+        *out = nullptr;
+        return lfail(RSB_ERR_OOM, "allocating reader weights failed");
+    }
+    return RSB_OK;
+}
+
 extern "C" int rsb_llm_free(rsb_llm_t* h) {
     if (!h) return RSB_OK;
     cudaFree(h->embed); cudaFree(h->lm_head); cudaFree(h->final_g); cudaFree(h->final_b); cudaFree(h->zero_bias);
@@ -696,6 +858,7 @@ extern "C" int rsb_llm_free(rsb_llm_t* h) {
     for (auto& l : h->L) {
         cudaFree(l.wqkv); cudaFree(l.wo); cudaFree(l.wgu); cudaFree(l.wdown); cudaFree(l.ln1); cudaFree(l.ln2);
         cudaFree(l.bqkv); cudaFree(l.bo); cudaFree(l.bgu); cudaFree(l.bdown); cudaFree(l.ln1b); cudaFree(l.ln2b);
+        cudaFree(l.qn); cudaFree(l.kn);
     }
     delete h;
     return RSB_OK;
@@ -774,7 +937,7 @@ extern "C" int rsb_llm_load(rsb_llm_t* h, const char* name, const void* f16_dev,
         return put(h->lm_head, (int64_t)h->vocab * H);
     }
     if (s == "lm_head.weight") return put(h->lm_head, (int64_t)h->vocab * H);
-    if (s == "model.norm.weight") return put(h->final_g, H);
+    if (s == "model.norm.weight" && h->olmo != 1) return put(h->final_g, H);   // OlmoLayerNorm has no weight
     int li = -1;
     char rest[128] = {0};
     if (sscanf(name, "model.layers.%d.%127s", &li, rest) == 2 && li >= 0 && li < h->layers) {
@@ -787,8 +950,15 @@ extern "C" int rsb_llm_load(rsb_llm_t* h, const char* name, const void* f16_dev,
         if (r == "mlp.gate_proj.weight") return put(l.wgu, I * H);
         if (r == "mlp.up_proj.weight") return put(l.wgu + I * H, I * H);
         if (r == "mlp.down_proj.weight") return put(l.wdown, I * H);
-        if (r == "input_layernorm.weight") return put(l.ln1, H);
-        if (r == "post_attention_layernorm.weight") return put(l.ln2, H);
+        if (h->olmo == 0) {
+            if (r == "input_layernorm.weight") return put(l.ln1, H);
+            if (r == "post_attention_layernorm.weight") return put(l.ln2, H);
+        } else if (h->olmo == 2) {
+            if (r == "post_attention_layernorm.weight") return put(l.ln1, H);
+            if (r == "post_feedforward_layernorm.weight") return put(l.ln2, H);
+            if (r == "self_attn.q_norm.weight") return put(l.qn, H);
+            if (r == "self_attn.k_norm.weight") return put(l.kn, KV);
+        }
     }
     return lfail(RSB_ERR_INVALID, "unknown weight name %s", name);
 }
@@ -826,15 +996,19 @@ int upload_attention_items(const std::vector<int32_t>& cu, int B, int2* d_items,
     return RSB_OK;
 }
 
-// One attention step on the fused QKV rows [n_tok, qkv_n] of a batch whose windows end at n_tok = cu[B]: RoPE on the
-// Q and K heads in place, then causal attention into CTX [n_tok, hidden].
-void attention_step(const rsb_llm* h, __half* QKV, const int32_t* cu_seqlens, int B, int n_tok, const int2* d_items,
-                    int n_items, __half* CTX, cudaStream_t st) {
+// One attention step of layer l on the fused QKV rows [n_tok, qkv_n] of a batch whose windows end at n_tok = cu[B]:
+// RoPE on the Q and K heads in place (OLMo: the clip / QK-norm prologue and fp32 RoPE), then causal attention into CTX
+// [n_tok, hidden].
+void attention_step(const rsb_llm* h, const LlmLayer& l, __half* QKV, const int32_t* cu_seqlens, int B, int n_tok,
+                    const int2* d_items, int n_items, __half* CTX, cudaStream_t st) {
     if (n_tok == 0 || n_items == 0) return;
     const float scale_log2 = 1.4426950408889634f / sqrtf((float)h->head_dim);   // 1/sqrt(head_dim) in the log2 domain
     if (h->neox)
         rope_partial_kernel<<<n_tok, 256, 0, st>>>(QKV, cu_seqlens, B, h->qkv_n(), h->heads + h->kv_heads, h->head_dim,
                                                    h->rot, h->inv_freq);
+    else if (h->olmo)
+        olmo_qkv_kernel<<<n_tok, 256, 0, st>>>(QKV, cu_seqlens, B, h->heads, h->kv_heads, h->inv_freq, h->clip,
+                                               h->olmo == 2 ? l.qn : nullptr, l.kn, h->eps);
     else
         rope_kernel<<<n_tok, 256, 0, st>>>(QKV, cu_seqlens, B, h->qkv_n(), h->heads + h->kv_heads, h->inv_freq);
     const dim3 grid((unsigned)n_items, h->heads);
@@ -897,12 +1071,51 @@ int llama_layers(rsb_llm* h, const Fwd& f, cudaStream_t st) {
         const LlmLayer& l = h->L[li];
         rms_rows_kernel<<<T, 256, 0, st>>>(f.X, nullptr, Hd, l.ln1, h->eps, f.Hn);
         if ((rc = gemm(f.Hn, T, l.wqkv, NQKV, Hd, h->zero_bias, nullptr, f.QKV, 0, st)) != RSB_OK) return rc;
-        attention_step(h, f.QKV, f.cu_seqlens, f.B, T, f.d_items, f.n_items, f.CTX, st);
+        attention_step(h, l, f.QKV, f.cu_seqlens, f.B, T, f.d_items, f.n_items, f.CTX, st);
         if ((rc = gemm(f.CTX, T, l.wo, Hd, Hd, h->zero_bias, f.X, f.X, 2, st)) != RSB_OK) return rc;
         rms_rows_kernel<<<T, 256, 0, st>>>(f.X, nullptr, Hd, l.ln2, h->eps, f.Hn);
         if ((rc = gemm(f.Hn, T, l.wgu, 2 * I, Hd, h->zero_bias, nullptr, f.GU, 0, st)) != RSB_OK) return rc;
         swiglu_kernel<<<sw_grid, 256, 0, st>>>(f.GU, n8, I, f.ACT);
         if ((rc = gemm(f.ACT, T, l.wdown, Hd, I, h->zero_bias, f.X, f.X, 2 | RSB_GEMM_REVERSED, st)) != RSB_OK) return rc;
+    }
+    return RSB_OK;
+}
+
+// OlmoDecoderLayer x layers: Llama's sequence with OlmoLayerNorm (ln_rows_kernel with unit scale and zero shift) as
+// both pre-norms.  Olmo2DecoderLayer x layers: no pre-norms; x = fp16(x + post_attention_layernorm(o_proj(attn(x)))),
+// then x = fp16(x + post_feedforward_layernorm(down(swiglu(gate|up(x))))).  A norm sits between each projection and
+// its add, so o_proj and down_proj write slot 1 (free without pre-norms) and rms_post_kernel adds the normed rows to x.
+int olmo_layers(rsb_llm* h, const Fwd& f, cudaStream_t st) {
+    const int Hd = h->hidden, NQKV = h->qkv_n(), I = h->inter, T = f.T;
+    const long long n8 = (long long)T * I / 8;
+    const int sw_grid = (int)std::min<long long>((n8 + 255) / 256, 8LL * rsb::device_num_sms());
+    const bool v2 = h->olmo == 2;
+    const __half* in = v2 ? f.X : f.Hn;          // what q|k|v and gate|up read
+    auto olmo_ln = [&]() {
+        ln_rows_kernel<<<T, LN_THREADS, 0, st>>>(f.X, nullptr, nullptr, Hd, h->final_g, h->zero_bias, nullptr, nullptr,
+                                                 h->eps, f.Hn, nullptr);
+    };
+    int rc;
+    for (int li = 0; li < h->layers; ++li) {
+        const LlmLayer& l = h->L[li];
+        if (!v2) olmo_ln();
+        if ((rc = gemm(in, T, l.wqkv, NQKV, Hd, h->zero_bias, nullptr, f.QKV, 0, st)) != RSB_OK) return rc;
+        attention_step(h, l, f.QKV, f.cu_seqlens, f.B, T, f.d_items, f.n_items, f.CTX, st);
+        if (v2) {
+            if ((rc = gemm(f.CTX, T, l.wo, Hd, Hd, h->zero_bias, nullptr, f.Hn, 0, st)) != RSB_OK) return rc;
+            rms_post_kernel<<<T, 256, 0, st>>>(f.X, f.Hn, nullptr, Hd, l.ln1, h->eps, nullptr);
+        } else {
+            if ((rc = gemm(f.CTX, T, l.wo, Hd, Hd, h->zero_bias, f.X, f.X, 2, st)) != RSB_OK) return rc;
+            olmo_ln();
+        }
+        if ((rc = gemm(in, T, l.wgu, 2 * I, Hd, h->zero_bias, nullptr, f.GU, 0, st)) != RSB_OK) return rc;
+        swiglu_kernel<<<sw_grid, 256, 0, st>>>(f.GU, n8, I, f.ACT);
+        if (v2) {
+            if ((rc = gemm(f.ACT, T, l.wdown, Hd, I, h->zero_bias, nullptr, f.Hn, 0, st)) != RSB_OK) return rc;
+            rms_post_kernel<<<T, 256, 0, st>>>(f.X, f.Hn, nullptr, Hd, l.ln2, h->eps, nullptr);
+        } else if ((rc = gemm(f.ACT, T, l.wdown, Hd, I, h->zero_bias, f.X, f.X, 2 | RSB_GEMM_REVERSED, st)) != RSB_OK) {
+            return rc;
+        }
     }
     return RSB_OK;
 }
@@ -919,7 +1132,7 @@ int neox_layers(rsb_llm* h, const Fwd& f, cudaStream_t st) {
     for (int li = 0; li < h->layers; ++li) {
         const LlmLayer& l = h->L[li];
         if ((rc = gemm(N1, T, l.wqkv, NQKV, Hd, l.bqkv, nullptr, f.QKV, 0, st)) != RSB_OK) return rc;
-        attention_step(h, f.QKV, f.cu_seqlens, f.B, T, f.d_items, f.n_items, f.CTX, st);
+        attention_step(h, l, f.QKV, f.cu_seqlens, f.B, T, f.d_items, f.n_items, f.CTX, st);
         if ((rc = gemm(f.CTX, T, l.wo, Hd, Hd, l.bo, nullptr, A, 0, st)) != RSB_OK) return rc;
         if ((rc = gemm(N2, T, l.wgu, I, Hd, l.bgu, nullptr, FF, 1, st)) != RSB_OK) return rc;
         if ((rc = gemm(FF, T, l.wdown, Hd, I, l.bdown, A, A, 2 | RSB_GEMM_REVERSED, st)) != RSB_OK) return rc;
@@ -948,14 +1161,17 @@ int trunk(rsb_llm* h, const int32_t* ids, const int32_t* cu_seqlens, int B, int 
     int rc;
     if ((rc = upload_attention_items(cu, B, d_items, st, &f.n_items)) != RSB_OK) return rc;
     embed_rows_kernel<<<T, 128, 0, st>>>(ids, h->embed, h->hidden, f.X);
-    return h->neox ? neox_layers(h, f, st) : llama_layers(h, f, st);
+    if (h->neox) return neox_layers(h, f, st);
+    return h->olmo ? olmo_layers(h, f, st) : llama_layers(h, f, st);
 }
 
 // The final norm of the label rows X[rows[i]] into out[i], i < n.
 void final_norm(const rsb_llm* h, const __half* X, const int* rows, int n, __half* out, cudaStream_t st) {
-    if (h->neox)
-        ln_rows_kernel<<<n, LN_THREADS, 0, st>>>(const_cast<__half*>(X), nullptr, rows, h->hidden, h->final_g, h->final_b,
-                                                 nullptr, nullptr, h->eps, out, nullptr);
+    if (h->neox || h->olmo == 1)                 // OLMo: unit scale (final_g) and zero shift
+        ln_rows_kernel<<<n, LN_THREADS, 0, st>>>(const_cast<__half*>(X), nullptr, rows, h->hidden, h->final_g,
+                                                 h->neox ? h->final_b : h->zero_bias, nullptr, nullptr, h->eps, out, nullptr);
+    else if (h->olmo == 2)
+        rms_post_kernel<<<n, 256, 0, st>>>(const_cast<__half*>(X), nullptr, rows, h->hidden, h->final_g, h->eps, out);
     else
         rms_rows_kernel<<<n, 256, 0, st>>>(X, rows, h->hidden, h->final_g, h->eps, out);
 }
@@ -1036,6 +1252,9 @@ extern "C" int rsb_llm_attention(rsb_llm_t* h, void* qkv, const int32_t* cu_seql
     if (B <= 0 || T <= 0) return lfail(RSB_ERR_INVALID, "empty batch");
     if (max_seqlen > h->max_pos)
         return lfail(RSB_ERR_UNSUPPORTED, "sequence longer than max_position_embeddings (%ld)", (long)h->max_pos);
+    if (h->olmo == 2 && !(h->loaded.count("model.layers.0.self_attn.q_norm.weight") &&
+                          h->loaded.count("model.layers.0.self_attn.k_norm.weight")))
+        return lfail(RSB_ERR_STATE, "layer 0's self_attn.q_norm / k_norm weights are not loaded");
     cudaStream_t st = (cudaStream_t)stream;
     std::vector<int32_t> cu(B + 1);
     if (cudaMemcpyAsync(cu.data(), cu_seqlens, cu.size() * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
@@ -1049,7 +1268,8 @@ extern "C" int rsb_llm_attention(rsb_llm_t* h, void* qkv, const int32_t* cu_seql
     int n_items = 0;
     rc = upload_attention_items(cu, B, d_items, st, &n_items);
     if (rc == RSB_OK)
-        attention_step(h, static_cast<__half*>(qkv), cu_seqlens, B, cu[B], d_items, n_items, static_cast<__half*>(ctx), st);
+        attention_step(h, h->L[0], static_cast<__half*>(qkv), cu_seqlens, B, cu[B], d_items, n_items,
+                       static_cast<__half*>(ctx), st);
     if (d_items) cudaFreeAsync(d_items, st);
     if (rc != RSB_OK) return rc;
     const cudaError_t e = cudaPeekAtLastError();
@@ -1074,5 +1294,21 @@ extern "C" int rsb_llm_layernorm(int hidden, float eps, void* x, const void* add
         static_cast<__half*>(out1), static_cast<__half*>(out2));
     const cudaError_t e = cudaPeekAtLastError();
     if (e != cudaSuccess) return lfail(RSB_ERR_CUDA, "layernorm launch failed: %s", cudaGetErrorString(e));
+    return RSB_OK;
+}
+
+// Diagnostic: rms_post_kernel, OLMo-2's post-norm residual add and final norm, on a caller's rows (rsb.h).
+extern "C" int rsb_llm_olmo2_norm(int hidden, float eps, void* x, const void* a, const int32_t* rows, int n_rows,
+                                  const void* w, void* out, rsb_stream_t stream) {
+    if (!x || !w || (!a && !out)) return lfail(RSB_ERR_INVALID, "null argument (x, w, or out without a)");
+    if (n_rows < 0 || !(eps > 0.f)) return lfail(RSB_ERR_INVALID, "n_rows must be >= 0 and eps positive");
+    if (hidden <= 0 || hidden % 8)
+        return lfail(RSB_ERR_UNSUPPORTED, "hidden %ld: the RMSNorm kernel takes positive multiples of 8", (long)hidden);
+    if (n_rows == 0) return RSB_OK;
+    rms_post_kernel<<<n_rows, 256, 0, (cudaStream_t)stream>>>(static_cast<__half*>(x), static_cast<const __half*>(a),
+                                                              rows, hidden, static_cast<const __half*>(w), eps,
+                                                              static_cast<__half*>(out));
+    const cudaError_t e = cudaPeekAtLastError();
+    if (e != cudaSuccess) return lfail(RSB_ERR_CUDA, "rmsnorm launch failed: %s", cudaGetErrorString(e));
     return RSB_OK;
 }

@@ -1,5 +1,6 @@
-"""GPU reader LM for perplexity evaluation in fp16 on librsb: HF `LlamaForCausalLM` (Llama-2 MHA, Llama-3 GQA) and
-HF `GPTNeoXForCausalLM` (the Pythia suite, whose pythia-1b is the reference's default `model.lm_model`).
+"""GPU reader LM for perplexity evaluation in fp16 on librsb: HF `LlamaForCausalLM` (Llama-2 MHA, Llama-3 GQA),
+HF `GPTNeoXForCausalLM` (the Pythia suite, whose pythia-1b is the reference's default `model.lm_model`) and HF
+`OlmoForCausalLM` / `Olmo2ForCausalLM` (OLMo, OLMo-1.7 and OLMo-2).
 
 The reference loads its reader with `AutoModelForCausalLM.from_pretrained(cfg.model.lm_model, torch_dtype=bfloat16)`
 and calls `lm(input_ids, labels=labels)` one window at a time (`src/evaluate_perplexity.py:98-134`).  Here
@@ -9,7 +10,7 @@ and calls `lm(input_ids, labels=labels)` one window at a time (`src/evaluate_per
     losses = model.loss([ids_0, ...], [labels_0, ...])          # HF's per-window mean loss
 
 runs `rsb_llm_nll`: a prefill-only forward over packed, un-padded windows whose LM head runs only on the rows whose
-next token is a label.  `load_reader` picks `B200Llama` or `B200NeoX` from the config's `model_type`.  No CPU /
+next token is a label.  `load_reader` picks `B200Llama`, `B200NeoX` or `B200Olmo` from the config's `model_type`.  No CPU /
 eager-PyTorch fallback: constructing the model without CUDA raises.  A checkpoint the kernels do not run (another
 `model_type`, another head_dim, RoPE scaling, a sequential residual, ...) raises AttributeError naming the field before
 any weight is read or device memory is allocated.
@@ -140,6 +141,81 @@ def neox_expected_keys(geom: dict) -> List[str]:
         keys += [f"gpt_neox.layers.{i}.{n}.{p}" for n in (
             "input_layernorm", "post_attention_layernorm", "attention.query_key_value", "attention.dense",
             "mlp.dense_h_to_4h", "mlp.dense_4h_to_h") for p in ("weight", "bias")]
+    return keys
+
+
+OLMO_MAX_HIDDEN = 8192                           # OLMo's LayerNorm runs on ln_rows_kernel
+
+
+def olmo_geometry(cfg) -> dict:
+    """The OLMo (`model_type` 'olmo', version 1) or OLMo-2 ('olmo2', version 2) reader geometry the kernels run, from an
+    HF config in either the `rope_theta` or transformers 5's `rope_parameters` form, or AttributeError naming the
+    field.  The non-HF 'hf_olmo' repos and 'olmo3' are other model_types and are refused by `load_reader`."""
+    mt = _get(cfg, "model_type")
+
+    def refuse(msg):
+        raise AttributeError(f"model_type {mt!r}: {msg}")
+    if mt not in ("olmo", "olmo2"):
+        refuse("only 'olmo' and 'olmo2' readers run on this path")
+    act = _get(cfg, "hidden_act", "silu")
+    if act != "silu":
+        refuse(f"hidden_act {act!r}: only 'silu' is implemented")
+    if _get(cfg, "attention_bias", False):
+        refuse("attention_bias is set: only bias-free attention is implemented")
+    hidden, heads = _get(cfg, "hidden_size"), _get(cfg, "num_attention_heads")
+    kv = _get(cfg, "num_key_value_heads") or heads
+    head_dim = _get(cfg, "head_dim") or (hidden // heads if hidden and heads else None)
+    if head_dim != 128 or not heads or hidden != heads * 128:
+        refuse(f"head_dim {head_dim} (hidden_size {hidden}, num_attention_heads {heads}): only head_dim 128 with "
+               f"hidden_size = 128 x num_attention_heads is implemented")
+    if kv <= 0 or heads % kv:
+        refuse(f"num_key_value_heads {kv} does not divide num_attention_heads {heads}")
+    inter = _get(cfg, "intermediate_size")
+    if not inter or inter <= 0 or inter % 128:
+        refuse(f"intermediate_size {inter}: must be a positive multiple of 128 (hidden_size {hidden} is)")
+    if mt == "olmo" and hidden > OLMO_MAX_HIDDEN:
+        refuse(f"hidden_size {hidden}: the LayerNorm kernel holds rows of at most {OLMO_MAX_HIDDEN}")
+    theta = _get(cfg, "rope_theta")
+    rp = _get(cfg, "rope_parameters")
+    if isinstance(rp, dict):                     # transformers >= 5 folds rope_theta / rope_scaling into rope_parameters
+        if rp.get("rope_type", "default") != "default":
+            refuse(f"rope_parameters {rp}: only the default RoPE is implemented (rope_scaling null)")
+        theta = rp.get("rope_theta", theta)
+    if _get(cfg, "rope_scaling") is not None and not (isinstance(rp, dict) and _get(cfg, "rope_scaling") == rp):
+        refuse(f"rope_scaling {_get(cfg, 'rope_scaling')}: only rope_scaling null is implemented")
+    theta = float(theta if theta is not None else 10000.0)
+    if not theta > 0:
+        refuse(f"rope_theta {theta} is not positive")
+    clip = _get(cfg, "clip_qkv") if mt == "olmo" else None   # Olmo2ForCausalLM never reads clip_qkv
+    if clip is not None and not clip > 0:
+        refuse(f"clip_qkv {clip}: must be null or positive")
+    vocab = _get(cfg, "vocab_size")
+    if not vocab or vocab <= 0:
+        refuse(f"vocab_size {vocab} is not a positive size")
+    layers = _get(cfg, "num_hidden_layers")
+    if not layers or layers <= 0:
+        refuse(f"num_hidden_layers {layers} is not a positive size")
+    # OlmoLayerNorm's eps is 1e-5 in the model code; OLMo-2 reads rms_norm_eps
+    eps = 1e-5 if mt == "olmo" else float(_get(cfg, "rms_norm_eps", 1e-5))
+    return dict(version=1 if mt == "olmo" else 2, num_hidden_layers=layers, hidden_size=hidden,
+                num_attention_heads=heads, num_key_value_heads=kv, intermediate_size=inter, vocab_size=vocab,
+                max_position_embeddings=_get(cfg, "max_position_embeddings", 2048), rope_theta=theta, eps=eps,
+                clip_qkv=float(clip or 0.0), tie_word_embeddings=bool(_get(cfg, "tie_word_embeddings", False)))
+
+
+def olmo_expected_keys(geom: dict) -> List[str]:
+    """Every weight the OLMo / OLMo-2 forward reads (HF OlmoForCausalLM / Olmo2ForCausalLM names); OLMo has no norm
+    weights."""
+    v2 = geom["version"] == 2
+    keys = ["model.embed_tokens.weight"] + (["model.norm.weight"] if v2 else [])
+    if not geom["tie_word_embeddings"]:
+        keys.append("lm_head.weight")
+    names = ["self_attn.q_proj", "self_attn.k_proj", "self_attn.v_proj", "self_attn.o_proj", "mlp.gate_proj",
+             "mlp.up_proj", "mlp.down_proj"]
+    if v2:
+        names += ["self_attn.q_norm", "self_attn.k_norm", "post_attention_layernorm", "post_feedforward_layernorm"]
+    for i in range(geom["num_hidden_layers"]):
+        keys += [f"model.layers.{i}.{n}.weight" for n in names]
     return keys
 
 
@@ -357,7 +433,23 @@ class B200NeoX(_Reader):
             ctypes.c_float(g["layer_norm_eps"]), ctypes.byref(self._h))
 
 
-READERS = {"llama": (llama_geometry, B200Llama), "gpt_neox": (neox_geometry, B200NeoX)}
+class B200Olmo(_Reader):
+    """An HF OlmoForCausalLM / Olmo2ForCausalLM reader on librsb (`rsb_llm_create_olmo`, then the same `rsb_llm_*`).
+    Diagnostics: `attention` runs layer 0's clip_qkv / QK-norm prologue in place of RoPE, then the same attention."""
+
+    _geometry = staticmethod(olmo_geometry)
+    _expected_keys = staticmethod(olmo_expected_keys)
+
+    def _create(self, g):
+        return self.L.rsb_llm_create_olmo(
+            g["version"], g["num_hidden_layers"], g["hidden_size"], g["num_attention_heads"],
+            g["num_key_value_heads"], g["intermediate_size"], g["vocab_size"], g["max_position_embeddings"],
+            ctypes.c_float(g["rope_theta"]), ctypes.c_float(g["eps"]), ctypes.c_float(g["clip_qkv"]),
+            int(g["tie_word_embeddings"]), ctypes.byref(self._h))
+
+
+READERS = {"llama": (llama_geometry, B200Llama), "gpt_neox": (neox_geometry, B200NeoX),
+           "olmo": (olmo_geometry, B200Olmo), "olmo2": (olmo_geometry, B200Olmo)}
 
 
 def _shard_files(directory: str) -> List[str]:
@@ -395,7 +487,7 @@ def _tensors(fn: str):
 
 def load_reader(path: str, device=None):
     """The reader of `cfg.model.lm_model` from a local directory or the Hugging Face cache (never downloaded):
-    `B200Llama` for model_type 'llama', `B200NeoX` for 'gpt_neox'.  Single-file or sharded safetensors weights, or
+    `B200Llama` for model_type 'llama', `B200NeoX` for 'gpt_neox', `B200Olmo` for 'olmo' and 'olmo2'.  Single-file or sharded safetensors weights, or
     PyTorch `pytorch_model.bin` files when no safetensors file is present; bf16 / fp32 weights are converted to fp16."""
     from .encoder import _resolve_model_dir
     directory = _resolve_model_dir(path)

@@ -5,7 +5,8 @@ and the same windows.
 
 Seeded weights with the full-depth geometry of Llama-2-7B (MHA, vocab 32000) and Llama-3-8B (GQA 4:1, vocab 128256),
 or of Pythia-1B (head_dim 256), Pythia-1.4B and Pythia-6.9B (GPT-NeoX: librsb's B200NeoX against HF GPTNeoXForCausalLM),
-generated on the device.  --windows windows of --context context tokens (retrieved documents + query, label -100)
+or of OLMo-1B (tied head), OLMo-7B-0424 (clip_qkv 8) and OLMo-2-7B (librsb's B200Olmo against HF OlmoForCausalLM /
+Olmo2ForCausalLM), generated on the device.  --windows windows of --context context tokens (retrieved documents + query, label -100)
 followed by --answer answer tokens (the labels), as the reference builds them with concate_k documents in front of a
 1024-token evaluation chunk.  Timed with CUDA events after --warmup passes, --repeats passes per model, the median
 reported.  Per-kernel times come from a separate torch.profiler pass.  Achieved TFLOP/s counts the model's FLOPs with
@@ -43,6 +44,19 @@ GEOMETRY.update({
                         vocab_size=50304),
     "pythia-6.9b": dict(_PYTHIA, num_hidden_layers=32, hidden_size=4096, num_attention_heads=32,
                         intermediate_size=16384, vocab_size=50432),
+})
+_OLMO = dict(hidden_act="silu", attention_bias=False, rope_theta=10000.0, max_position_embeddings=2048,
+             tie_word_embeddings=False)
+GEOMETRY.update({
+    "olmo-1b": dict(_OLMO, model_type="olmo", num_hidden_layers=16, hidden_size=2048, num_attention_heads=16,
+                    num_key_value_heads=16, intermediate_size=8192, vocab_size=50304, clip_qkv=None,
+                    tie_word_embeddings=True),
+    "olmo-7b": dict(_OLMO, model_type="olmo", num_hidden_layers=32, hidden_size=4096, num_attention_heads=32,
+                    num_key_value_heads=32, intermediate_size=11008, vocab_size=50304, clip_qkv=8.0,
+                    max_position_embeddings=4096),
+    "olmo2-7b": dict(_OLMO, model_type="olmo2", num_hidden_layers=32, hidden_size=4096, num_attention_heads=32,
+                     num_key_value_heads=32, intermediate_size=11008, vocab_size=100352, rope_theta=500000.0,
+                     rms_norm_eps=1e-6, max_position_embeddings=4096),
 })
 PEAK_TFLOPS = 989.0
 
@@ -83,28 +97,35 @@ def neox_weights(cfg, seed=0):
 
 
 def weights(cfg, seed=0):
-    """(name, fp16 tensor on the device) in HF order, regenerated from the seed for each path."""
+    """(name, fp16 tensor on the device) in HF order, regenerated from the seed for each path.  Llama, OLMo (no norm
+    weights) and OLMo-2 (post-norms and QK-norms) share the projections."""
     if neox(cfg):
         yield from neox_weights(cfg, seed)
         return
     g = torch.Generator(device="cuda").manual_seed(seed)
     H, I, V = cfg["hidden_size"], cfg["intermediate_size"], cfg["vocab_size"]
     KV = cfg["num_key_value_heads"] * 128
+    mt, tied = cfg["model_type"], cfg["tie_word_embeddings"]
 
     def n(*shape, std):
         return torch.randn(*shape, generator=g, device="cuda", dtype=torch.float16) * std
 
-    yield "model.embed_tokens.weight", n(V, H, std=1.0)
+    yield "model.embed_tokens.weight", n(V, H, std=2.0 * H ** -0.5 if tied else 1.0)
     for i in range(cfg["num_hidden_layers"]):
         p = f"model.layers.{i}."
         for name, shape, fan in (("self_attn.q_proj", (H, H), H), ("self_attn.k_proj", (KV, H), H),
                                  ("self_attn.v_proj", (KV, H), H), ("self_attn.o_proj", (H, H), H),
                                  ("mlp.gate_proj", (I, H), H), ("mlp.up_proj", (I, H), H), ("mlp.down_proj", (H, I), I)):
             yield p + name + ".weight", n(*shape, std=fan ** -0.5)
-        yield p + "input_layernorm.weight", 1.0 + n(H, std=0.05)
-        yield p + "post_attention_layernorm.weight", 1.0 + n(H, std=0.05)
-    yield "model.norm.weight", 1.0 + n(H, std=0.05)
-    yield "lm_head.weight", n(V, H, std=2.0 * H ** -0.5)
+        norms = {"llama": (("input_layernorm", H), ("post_attention_layernorm", H)), "olmo": (),
+                 "olmo2": (("self_attn.q_norm", H), ("self_attn.k_norm", KV), ("post_attention_layernorm", H),
+                           ("post_feedforward_layernorm", H))}[mt]
+        for name, width in norms:
+            yield p + name + ".weight", 1.0 + n(width, std=0.05)
+    if mt != "olmo":
+        yield "model.norm.weight", 1.0 + n(H, std=0.05)
+    if not tied:
+        yield "lm_head.weight", n(V, H, std=2.0 * H ** -0.5)
 
 
 def windows(cfg, n, context, answer, seed=1):
@@ -159,8 +180,8 @@ def kernel_table(fn, n_windows):
 
 
 def bench_rsb(cfg, ids, labels, args):
-    from retrieval_scaling_b200.reader import B200Llama, B200NeoX
-    m = (B200NeoX if neox(cfg) else B200Llama)(cfg)
+    from retrieval_scaling_b200.reader import READERS
+    m = READERS[cfg["model_type"]][1](cfg)
     for name, w in weights(cfg):
         m.load_weight(name, w)
         del w
@@ -179,11 +200,16 @@ def bench_rsb(cfg, ids, labels, args):
 def bench_hf(cfg, ids, labels, args):
     import transformers
     kw = {k: v for k, v in cfg.items() if k != "model_type"}
-    hc = (transformers.GPTNeoXConfig if neox(cfg) else transformers.LlamaConfig)(**kw)
+    conf, cls = {"llama": (transformers.LlamaConfig, transformers.LlamaForCausalLM),
+                 "gpt_neox": (transformers.GPTNeoXConfig, transformers.GPTNeoXForCausalLM),
+                 "olmo": (transformers.OlmoConfig, transformers.OlmoForCausalLM),
+                 "olmo2": (transformers.Olmo2Config, transformers.Olmo2ForCausalLM)}[cfg["model_type"]]
+    hc = conf(**kw)
     hc._attn_implementation = "sdpa"
     with torch.device("meta"):
-        lm = (transformers.GPTNeoXForCausalLM if neox(cfg) else transformers.LlamaForCausalLM)(hc)
+        lm = cls(hc)
     lm = lm.to_empty(device="cuda").to(torch.bfloat16).eval()
+    lm.tie_weights()                             # to_empty gives a tied head storage of its own: share it again
     params = dict(lm.named_parameters())
     with torch.no_grad():
         for name, w in weights(cfg):
