@@ -256,7 +256,8 @@ int rsb_coarse(rsb_index_t* h, const float* q_dev, int nq, int nprobe, int64_t* 
  * Every argument is checked before any launch.  The workspace queries return 0 for arguments the call would refuse;
  * they size the all-device store by nq, k_base and k alone, and the tiered store by its dtype and staging_bytes. */
 /* RSB_DTYPE_SQ8: a re-rank store, or the storage of an IVFFLAT index (rsb_ivfflat_create); not a Flat index */
-enum { RSB_DTYPE_F32 = 0, RSB_DTYPE_F16 = 1, RSB_DTYPE_SQ8 = 2 };
+/* RSB_DTYPE_BF16: readers only (rsb_llm_set_dtype); every index and re-rank store creator refuses it (RSB_ERR_INVALID) */
+enum { RSB_DTYPE_F32 = 0, RSB_DTYPE_F16 = 1, RSB_DTYPE_SQ8 = 2, RSB_DTYPE_BF16 = 3 };
 int rsb_host_alloc(size_t bytes, void** out);   /* cudaHostAlloc(portable | mapped): exactly `bytes`, unlike torch's
                                                    pinned allocator, which rounds blocks up to a power of two */
 int rsb_host_free(void* p);
@@ -455,7 +456,7 @@ enum { RSB_GEMM_REVERSED = 256 };
 int rsb_gemm_f16(const void* A_dev, const void* W_dev, const void* bias_dev, const void* residual_dev, void* C_dev,
                  int M, int N, int K, int epilogue, rsb_stream_t stream);
 
-/* ---- reader LM for perplexity evaluation: HF LlamaForCausalLM, prefill only, fp16 ----------------------------------
+/* ---- reader LM for perplexity evaluation: HF LlamaForCausalLM, prefill only, fp16 or bf16 --------------------------
  * Replaces the reader of the reference's perplexity loop (src/evaluate_perplexity.py:98-108 loads it, :126-134 runs
  * `lm(input_ids, labels=labels)` one window at a time).  Errors of these entries are reported by rsb_llm_last_error().
  * rsb_llm_create: head_dim 128 (hidden == 128 * heads), heads % kv_heads == 0, intermediate % 128 == 0, SiLU MLP, no
@@ -512,9 +513,19 @@ int rsb_llm_create_neox(int layers, int hidden, int heads, int intermediate, int
  *     k_norm (version 2; RSB_ERR_STATE until layer 0's q_norm and k_norm are loaded), then the fp32-cos / sin RoPE. */
 int rsb_llm_create_olmo(int version, int layers, int hidden, int heads, int kv_heads, int intermediate, int vocab,
                         int max_pos, float rope_theta, float eps, float clip_qkv, int tied, rsb_llm_t** out);
+/* The element type of a handle's weights and activations, for every constructor: RSB_DTYPE_F16 (the default) or
+ * RSB_DTYPE_BF16, the reference's reader dtype; any other value RSB_ERR_INVALID, and RSB_ERR_STATE once rsb_llm_load has
+ * been called.  In bf16 the forward is HF's bf16 forward: every point where the fp16 forward rounds to fp16 (each GEMM
+ * output, norm output, RoPE product and sum, attention's P before P V, SwiGLU / GELU output, residual add, the logits)
+ * rounds to bf16 instead, with the same fp32 arithmetic in between; OLMo's fp32 cos / sin RoPE rounds once, to bf16, and
+ * clip_qkv acts as the bf16 clamp (the clamped value is the bound rounded to bf16).  The NLL is the fp32 log-sum-exp of
+ * the bf16 logits, as transformers' logits.float() after a bf16 lm_head.  rsb_llm_load, rsb_llm_attention and
+ * rsb_llm_hidden_states then take and return bf16. */
+int rsb_llm_set_dtype(rsb_llm_t* h, int dtype);
 /* name = HF LlamaForCausalLM state_dict key: "model.embed_tokens.weight", "model.norm.weight", "lm_head.weight"
  * (untied; accepted and ignored when tied) and "model.layers.N.{self_attn.{q,k,v,o}_proj, mlp.{gate,up,down}_proj,
- * input_layernorm, post_attention_layernorm}.weight"; data fp16 on the device, copied. */
+ * input_layernorm, post_attention_layernorm}.weight"; data on the device in the handle's dtype (fp16 unless
+ * rsb_llm_set_dtype chose bf16), copied. */
 int rsb_llm_load(rsb_llm_t* h, const char* name, const void* f16_dev, int64_t n_elements, rsb_stream_t stream);
 size_t rsb_llm_workspace_bytes(rsb_llm_t* h, int total_tokens, int label_tokens);
 /* B packed sequences: ids_dev / labels_dev [T] int32 (label -100 = ignored), cu_seqlens_dev [B+1] int32 (0 .. T), every
@@ -527,8 +538,9 @@ int rsb_llm_nll(rsb_llm_t* h, const int32_t* ids_dev, const int32_t* cu_seqlens_
                 const int32_t* labels_dev, float* nll_out_dev, void* ws_dev, size_t ws_bytes, rsb_stream_t stream);
 int rsb_llm_free(rsb_llm_t* h);
 /* Diagnostic, not used on the product path: one attention step of rsb_llm_nll on a caller's tensors, with the forward's
- * own work list.  qkv_dev [T, (heads + 2 kv_heads) 128] fp16 holds each token's Q | K | V heads; RoPE is applied to its
- * Q and K heads in place (positions restart at 0 in every window), then ctx_dev [T, heads 128] fp16 receives causal
+ * own work list.  qkv_dev [T, (heads + 2 kv_heads) 128] in the handle's dtype (fp16 or bf16) holds each token's Q | K |
+ * V heads; RoPE is applied to its Q and K heads in place (positions restart at 0 in every window), then ctx_dev
+ * [T, heads 128] in the same dtype receives causal
  * softmax(q k^T / sqrt(128)) v per window and query head h, which reads KV head h / (heads / kv_heads).  Windows may be
  * empty and cu_seqlens_dev [B+1] may end below T: rows of empty windows and rows at or past cu_seqlens[B] are neither
  * rotated nor written.  The offset refusals of rsb_llm_nll apply (RSB_ERR_INVALID / RSB_ERR_UNSUPPORTED before any
@@ -536,7 +548,7 @@ int rsb_llm_free(rsb_llm_t* h);
 int rsb_llm_attention(rsb_llm_t* h, void* qkv_dev, const int32_t* cu_seqlens_dev, int B, int T, int max_seqlen,
                       void* ctx_dev, rsb_stream_t stream);
 /* Diagnostic, not used on the product path: the residual stream after the last decoder layer of rsb_llm_nll's forward,
- * before the final norm, out_dev [T, hidden] fp16.  The refusals of rsb_llm_nll apply; the workspace is
+ * before the final norm, out_dev [T, hidden] in the handle's dtype.  The refusals of rsb_llm_nll apply; the workspace is
  * rsb_llm_workspace_bytes(h, T, 0). */
 int rsb_llm_hidden_states(rsb_llm_t* h, const int32_t* ids_dev, const int32_t* cu_seqlens_dev, int B, int T,
                           int max_seqlen, void* out_dev, void* ws_dev, size_t ws_bytes, rsb_stream_t stream);

@@ -13,7 +13,7 @@ LIB_PATH = os.environ.get("RSB_LIBRARY") or os.path.join(_HERE, "librsb.so")
 RSB_OK = 0
 RSB_ERR_INVALID, RSB_ERR_CUDA, RSB_ERR_STATE, RSB_ERR_UNSUPPORTED, RSB_ERR_OOM = -1, -2, -3, -4, -5
 RSB_FLAT, RSB_IVFFLAT, RSB_IVFPQ = 0, 1, 2
-RSB_DTYPE_F32, RSB_DTYPE_F16, RSB_DTYPE_SQ8 = 0, 1, 2
+RSB_DTYPE_F32, RSB_DTYPE_F16, RSB_DTYPE_SQ8, RSB_DTYPE_BF16 = 0, 1, 2, 3   # BF16: readers only
 (INFO_KIND, INFO_D, INFO_NLIST, INFO_M, INFO_NBITS, INFO_NTOTAL, INFO_IS_TRAINED, INFO_MAX_LIST_LEN,
  INFO_INDEX_BYTES, INFO_DTYPE, INFO_BY_RESIDUAL, INFO_HOST_BYTES, INFO_DEVICE_ROWS) = range(13)
 OPT_COARSE_TENSOR, OPT_BY_RESIDUAL, OPT_DEVICE_ROWS, OPT_STAGING_BYTES = 0, 1, 2, 3
@@ -104,6 +104,7 @@ SIGNATURES = [
                                   c_void_p, c_void_p, c_void_p, c_void_p]),                          # diagnostic
     ("rsb_llm_create_olmo", c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_float,
                                     c_int, POINTER(_H)]),
+    ("rsb_llm_set_dtype", c_int, [_H, c_int]),
     ("rsb_llm_olmo2_norm", c_int, [c_int, c_float, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
                                    c_void_p]),                                                       # diagnostic
     ("rsb_dedup_last_error", c_char_p, []),

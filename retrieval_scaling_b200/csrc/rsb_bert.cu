@@ -20,6 +20,7 @@
 // pool_kernel -> Dense on gemm_tn_kernel -> l2normalize_rows_kernel.
 #include "../../include/rsb.h"
 
+#include "rsb_dtype.cuh"
 #include "rsb_internal.h"
 #include "rsb_tc.cuh"
 
@@ -31,6 +32,7 @@
 #include <cstring>
 #include <map>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 namespace {
@@ -112,11 +114,15 @@ __device__ __forceinline__ unsigned long long gelu_erf_pair(unsigned long long X
 #endif
 }
 
-template <int EPI>
+// T = __half (every epilogue) or __nv_bfloat16 (EPI_BIAS / _GELU / _RESIDUAL, the reader's): A, B, bias, residual and
+// C in T, fp32 accumulation, the epilogue rounding to T where the fp16 one rounds to half.
+template <int EPI, typename T = __half>
 __global__ __launch_bounds__(G_THREADS, 1)
 void gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                    __half* __restrict__ C, const __half* __restrict__ bias, const __half* __restrict__ residual,
+                    T* __restrict__ C, const T* __restrict__ bias, const T* __restrict__ residual,
                     int M, int N, int K, int m_rev, int* __restrict__ inf_flag) {
+    static_assert(std::is_same<T, __half>::value || EPI == EPI_BIAS || EPI == EPI_BIAS_GELU || EPI == EPI_BIAS_RESIDUAL,
+                  "bf16 epilogues: bias, GELU and residual only");
     extern __shared__ unsigned char smem_dyn[];
     // 1024-byte alignment required by the 128B swizzle atom
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
@@ -164,7 +170,10 @@ void gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         wgmma_fence();
 #pragma unroll
         for (int k4 = 0; k4 < G_BK / 16; ++k4)   // advance 16 K-elements = 32 bytes inside the swizzle row: +2 in the (addr >> 4) field
-            wgmma_f16_n128(acc, adesc + (uint64_t)(k4 * 2), bdesc + (uint64_t)(k4 * 2));
+            if constexpr (std::is_same<T, __half>::value)
+                wgmma_f16_n128(acc, adesc + (uint64_t)(k4 * 2), bdesc + (uint64_t)(k4 * 2));
+            else
+                wgmma_bf16_n128(acc, adesc + (uint64_t)(k4 * 2), bdesc + (uint64_t)(k4 * 2));
         wgmma_commit();
         acc_fence(acc);
         wgmma_wait<1>();                                      // the previous k-block's MMAs have retired: free its stage
@@ -183,23 +192,23 @@ void gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     const int c_lo = n0 + 2 * (lane & 3);
     float2 bj[16];
 #pragma unroll
-    for (int j = 0; j < 16; ++j) bj[j] = __half22float2(*reinterpret_cast<const __half2*>(bias + c_lo + 8 * j));
+    for (int j = 0; j < 16; ++j) bj[j] = rsbdt::to_f2(*reinterpret_cast<const rsbdt::pair_t<T>*>(bias + c_lo + 8 * j));
     bool wrote_inf = false;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
         const int row = r_lo + 8 * h;
         if (row >= M) continue;
-        __half* dst = C + (size_t)row * N + c_lo;
-        const __half* res = residual + (size_t)row * N + c_lo;
+        T* dst = C + (size_t)row * N + c_lo;
+        const T* res = residual + (size_t)row * N + c_lo;
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
             float x0 = __fadd_rn(acc[4 * j + 2 * h], bj[j].x), x1 = __fadd_rn(acc[4 * j + 2 * h + 1], bj[j].y);
             if (EPI == EPI_BIAS_GELU) f2unpack(gelu_erf_pair(f2pack(x0, x1)), x0, x1);
             if (EPI == EPI_BIAS_RELU) { x0 = x0 < 0.f ? 0.f : x0; x1 = x1 < 0.f ? 0.f : x1; }   // NaN passes, as torch.relu
-            __half2 o = __floats2half2_rn(x0, x1);
-            if (EPI == EPI_BIAS_RESIDUAL || EPI == EPI_BIAS_RESIDUAL_INF) o = __hadd2(o, *reinterpret_cast<const __half2*>(res + 8 * j));
-            if (EPI == EPI_BIAS_RESIDUAL_INF) wrote_inf |= __hisinf(__low2half(o)) != 0 || __hisinf(__high2half(o)) != 0;
-            *reinterpret_cast<__half2*>(dst + 8 * j) = o;
+            rsbdt::pair_t<T> o = rsbdt::from_f2<T>(x0, x1);
+            if (EPI == EPI_BIAS_RESIDUAL || EPI == EPI_BIAS_RESIDUAL_INF) o = __hadd2(o, *reinterpret_cast<const rsbdt::pair_t<T>*>(res + 8 * j));
+            if constexpr (EPI == EPI_BIAS_RESIDUAL_INF) wrote_inf |= __hisinf(__low2half(o)) != 0 || __hisinf(__high2half(o)) != 0;
+            *reinterpret_cast<rsbdt::pair_t<T>*>(dst + 8 * j) = o;
         }
     }
     if (EPI == EPI_BIAS_RESIDUAL_INF && wrote_inf) *inf_flag = 1;   // every writer stores the same value
@@ -885,8 +894,8 @@ int bfail(int code, const char* fmt, const char* a = "", long b = 0) {
     return code;
 }
 
-bool make_map(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows) {
-    return rsbtc::make_map_2d(m, base, rows, cols, box_rows, 2);
+bool make_map(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows, bool bf16 = false) {
+    return rsbtc::make_map_2d(m, base, rows, cols, box_rows, 2, bf16);
 }
 
 struct Linear {
@@ -945,17 +954,20 @@ void free_linear(Linear& l) { cudaFree(l.w); cudaFree(l.b); }
 
 // m_rev: visit the row tiles last-to-first.  The FFN intermediate (251 MB at 41k tokens) is twice the L2: FFN2 starts with the
 // rows FFN1 wrote last, which are still cached (RSB_NO_SNAKE=1 disables, A/B).
-template <int EPI>
-int launch_gemm(const __half* A, int M, const Linear& lin, __half* C, const __half* residual, cudaStream_t st, bool m_rev = false,
+// T = __nv_bfloat16: lin.w / lin.b hold bf16 and lin.map is a BFLOAT16 map.
+template <int EPI, typename T = __half>
+int launch_gemm(const T* A, int M, const Linear& lin, typename std::common_type<T>::type* C,
+                const typename std::common_type<T>::type* residual, cudaStream_t st, bool m_rev = false,
                 int* inf_flag = nullptr) {
+    constexpr bool bf16 = std::is_same<T, __nv_bfloat16>::value;
     CUtensorMap tmA;
-    if (!lin.map_ok || !make_map(&tmA, A, (uint64_t)M, (uint64_t)lin.K, G_BM)) return RSB_ERR_CUDA;
+    if (!lin.map_ok || !make_map(&tmA, A, (uint64_t)M, (uint64_t)lin.K, G_BM, bf16)) return RSB_ERR_CUDA;
     static rsb::PerDeviceFlag configured;                    // attributes are per (function, device)
-    if (configured.first()) cudaFuncSetAttribute(gemm_tn_kernel<EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, G_SMEM);
+    if (configured.first()) cudaFuncSetAttribute(gemm_tn_kernel<EPI, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, G_SMEM);
     static const bool no_snake = getenv("RSB_NO_SNAKE") != nullptr;
     dim3 grid(lin.N / G_BN, (M + G_BM - 1) / G_BM);              // consecutive CTAs share one row tile of A
-    gemm_tn_kernel<EPI><<<grid, G_THREADS, G_SMEM, st>>>(tmA, lin.map, C, lin.b, residual, M, lin.N, lin.K,
-                                                         (m_rev && !no_snake) ? 1 : 0, inf_flag);
+    gemm_tn_kernel<EPI, T><<<grid, G_THREADS, G_SMEM, st>>>(tmA, lin.map, C, reinterpret_cast<const T*>(lin.b), residual,
+                                                            M, lin.N, lin.K, (m_rev && !no_snake) ? 1 : 0, inf_flag);
     return RSB_OK;
 }
 
@@ -1427,8 +1439,13 @@ extern "C" int rsb_bert_attention(rsb_bert_t* h, const void* qkv, const int32_t*
 
 // plain GEMM entry (tests / roofline of the tensor-core kernel): C[M,N] = A[M,K] W[N,K]^T + bias, epilogue as above
 // (0 bias, 1 GELU, 2 residual, 3 ReLU), OR-ed with RSB_GEMM_REVERSED to visit the row tiles last-to-first as FFN2 does
-extern "C" int rsb_gemm_f16(const void* A, const void* W, const void* bias, const void* residual, void* C, int M, int N,
-                            int K, int epilogue, rsb_stream_t stream) {
+namespace {
+
+// rsb_gemm_f16's checks and launch for element type T; bf16 has no ReLU epilogue (only the encoder uses it).
+template <typename T>
+int gemm_entry(const void* A, const void* W, const void* bias, const void* residual, void* C, int M, int N, int K,
+               int epilogue, cudaStream_t st) {
+    constexpr bool bf16 = std::is_same<T, __nv_bfloat16>::value;
     if (!A || !W || !bias || !C) return bfail(RSB_ERR_INVALID, "null argument");
     if (M <= 0 || N % G_BN || K % G_BK || N <= 0 || K <= 0) return bfail(RSB_ERR_INVALID, "need N %% 128 == 0 and K %% 64 == 0");
     const bool m_rev = (epilogue & RSB_GEMM_REVERSED) != 0;
@@ -1436,17 +1453,34 @@ extern "C" int rsb_gemm_f16(const void* A, const void* W, const void* bias, cons
     if (epilogue == EPI_BIAS_RESIDUAL && !residual) return bfail(RSB_ERR_INVALID, "residual is NULL");
     Linear lin;
     lin.w = (__half*)W; lin.b = (__half*)bias; lin.N = N; lin.K = K;
-    lin.map_ok = make_map(&lin.map, W, N, K, G_BN);
+    lin.map_ok = make_map(&lin.map, W, N, K, G_BN, bf16);
     if (!lin.map_ok) return bfail(RSB_ERR_CUDA, "tensor map encode failed");
-    cudaStream_t st = (cudaStream_t)stream;
+    const T* a = static_cast<const T*>(A);
+    T* c = static_cast<T*>(C);
     int rc;
-    if (epilogue == EPI_BIAS) rc = launch_gemm<EPI_BIAS>((const __half*)A, M, lin, (__half*)C, nullptr, st, m_rev);
-    else if (epilogue == EPI_BIAS_GELU) rc = launch_gemm<EPI_BIAS_GELU>((const __half*)A, M, lin, (__half*)C, nullptr, st, m_rev);
-    else if (epilogue == EPI_BIAS_RESIDUAL) rc = launch_gemm<EPI_BIAS_RESIDUAL>((const __half*)A, M, lin, (__half*)C, (const __half*)residual, st, m_rev);
-    else if (epilogue == EPI_BIAS_RELU) rc = launch_gemm<EPI_BIAS_RELU>((const __half*)A, M, lin, (__half*)C, nullptr, st, m_rev);
-    else return bfail(RSB_ERR_INVALID, "unknown epilogue");
+    if (epilogue == EPI_BIAS) rc = launch_gemm<EPI_BIAS, T>(a, M, lin, c, nullptr, st, m_rev);
+    else if (epilogue == EPI_BIAS_GELU) rc = launch_gemm<EPI_BIAS_GELU, T>(a, M, lin, c, nullptr, st, m_rev);
+    else if (epilogue == EPI_BIAS_RESIDUAL) rc = launch_gemm<EPI_BIAS_RESIDUAL, T>(a, M, lin, c, static_cast<const T*>(residual), st, m_rev);
+    else if constexpr (!bf16) {
+        if (epilogue == EPI_BIAS_RELU) rc = launch_gemm<EPI_BIAS_RELU>(a, M, lin, c, nullptr, st, m_rev);
+        else return bfail(RSB_ERR_INVALID, "unknown epilogue");
+    } else {
+        return bfail(RSB_ERR_INVALID, "unknown epilogue (bf16: 0 bias, 1 GELU, 2 residual)");
+    }
     if (rc != RSB_OK) return bfail(RSB_ERR_CUDA, "tensor map encode failed");
     cudaError_t e = cudaPeekAtLastError();
     if (e != cudaSuccess) return bfail(RSB_ERR_CUDA, "gemm launch failed: %s", cudaGetErrorString(e));
     return RSB_OK;
+}
+
+}  // namespace
+
+extern "C" int rsb_gemm_f16(const void* A, const void* W, const void* bias, const void* residual, void* C, int M, int N,
+                            int K, int epilogue, rsb_stream_t stream) {
+    return gemm_entry<__half>(A, W, bias, residual, C, M, N, K, epilogue, (cudaStream_t)stream);
+}
+
+int rsb::gemm_bf16(const void* A, const void* W, const void* bias, const void* residual, void* C, int M, int N, int K,
+                   int epilogue, cudaStream_t stream) {
+    return gemm_entry<__nv_bfloat16>(A, W, bias, residual, C, M, N, K, epilogue, stream);
 }

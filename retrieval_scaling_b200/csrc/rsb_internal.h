@@ -48,6 +48,12 @@ inline int device_num_sms() {
     return n;
 }
 
+// ---- rsb_bert.cu ----------------------------------------------------------------------------------------
+// rsb_gemm_f16 (rsb.h) on bf16 A, W, bias, residual and C, for the reader in bf16: epilogue 0 (bias), 1 (bias + GELU)
+// or 2 (bias + residual), OR-ed with RSB_GEMM_REVERSED; the same checks and errors (rsb_bert_last_error).
+int gemm_bf16(const void* A, const void* W, const void* bias, const void* residual, void* C, int M, int N, int K,
+              int epilogue, cudaStream_t stream);
+
 // ---- rsb_dense.cu ---------------------------------------------------------------------------------------
 void launch_sgemm_nt(const float* A, int M, const float* B, int N, int K, float* C, int ldc, cudaStream_t st);
 void launch_select_rows(const float* S, int nrows, int ncols, int ld, unsigned col_base, int k, int nsplit,

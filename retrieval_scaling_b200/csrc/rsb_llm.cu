@@ -1,6 +1,8 @@
 // rsb_llm.cu -- reader-LM forward for perplexity evaluation: HF LlamaForCausalLM (Llama-2 MHA, Llama-3 GQA),
 // GPTNeoXForCausalLM (Pythia; rsb_llm_create_neox) and OlmoForCausalLM / Olmo2ForCausalLM (rsb_llm_create_olmo) in
-// fp16, prefill only, over packed un-padded sequences, ending in the per-token negative log-likelihood of the labels.
+// fp16 or bf16 (rsb_llm_set_dtype; every kernel is a template on its element type and rounds to it where HF's forward
+// in that dtype rounds), prefill only, over packed un-padded sequences, ending in the per-token negative
+// log-likelihood of the labels.
 // Replaces the reader call of the reference's perplexity loop (src/evaluate_perplexity.py:126-134: `lm(input_ids,
 // labels=labels)` one window at a time, HF in bf16).  No KV cache, no generation.
 //
@@ -23,7 +25,7 @@
 
 #include "rsb_internal.h"
 
-#include <cuda_fp16.h>
+#include "rsb_dtype.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -31,9 +33,12 @@
 #include <cstdio>
 #include <set>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 namespace {
+
+using namespace rsbdt;
 
 constexpr int HD = 128;                      // head_dim of every Llama reader
 constexpr int AQ = 64, AK = 64;              // attention: 64 queries per block (16 per warp), key blocks of 64
@@ -51,8 +56,9 @@ __device__ __forceinline__ float block_sum(float v, float* red) {
 }
 
 // one block per token; hidden % 8 == 0
-__global__ void embed_rows_kernel(const int* __restrict__ ids, const __half* __restrict__ embed, int hidden,
-                                  __half* __restrict__ X) {
+template <typename T>
+__global__ void embed_rows_kernel(const int* __restrict__ ids, const T* __restrict__ embed, int hidden,
+                                  T* __restrict__ X) {
     const int t = blockIdx.x;
     const uint4* src = reinterpret_cast<const uint4*>(embed + (size_t)ids[t] * hidden);
     uint4* dst = reinterpret_cast<uint4*>(X + (size_t)t * hidden);
@@ -61,9 +67,10 @@ __global__ void embed_rows_kernel(const int* __restrict__ ids, const __half* __r
 
 // LlamaRMSNorm (modeling_llama.py): h = x.float(); h *= rsqrt(mean(h^2) + eps); weight * h.half().  One block per
 // output row i, input row rows ? rows[i] : i.
+template <typename T>
 __global__ __launch_bounds__(256)
-void rms_rows_kernel(const __half* __restrict__ in, const int* __restrict__ rows, int hidden,
-                     const __half* __restrict__ w, float eps, __half* __restrict__ out) {
+void rms_rows_kernel(const T* __restrict__ in, const int* __restrict__ rows, int hidden,
+                     const T* __restrict__ w, float eps, T* __restrict__ out) {
     __shared__ float red[8];
     const int i = blockIdx.x;
     const int r = rows ? rows[i] : i;
@@ -71,10 +78,10 @@ void rms_rows_kernel(const __half* __restrict__ in, const int* __restrict__ rows
     float s = 0.f;
     for (int c = threadIdx.x; c < hidden / 8; c += blockDim.x) {
         const uint4 v = x[c];
-        const __half2* h2 = reinterpret_cast<const __half2*>(&v);
+        const pair_t<T>* h2 = reinterpret_cast<const pair_t<T>*>(&v);
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-            const float2 f = __half22float2(h2[e]);
+            const float2 f = to_f2(h2[e]);
             s = fmaf(f.x, f.x, s);
             s = fmaf(f.y, f.y, s);
         }
@@ -84,14 +91,14 @@ void rms_rows_kernel(const __half* __restrict__ in, const int* __restrict__ rows
     uint4* o = reinterpret_cast<uint4*>(out + (size_t)i * hidden);
     for (int c = threadIdx.x; c < hidden / 8; c += blockDim.x) {
         const uint4 v = x[c], g = wv[c];
-        const __half2* h2 = reinterpret_cast<const __half2*>(&v);
-        const __half2* g2 = reinterpret_cast<const __half2*>(&g);
+        const pair_t<T>* h2 = reinterpret_cast<const pair_t<T>*>(&v);
+        const pair_t<T>* g2 = reinterpret_cast<const pair_t<T>*>(&g);
         uint4 ov;
-        __half2* o2 = reinterpret_cast<__half2*>(&ov);
+        pair_t<T>* o2 = reinterpret_cast<pair_t<T>*>(&ov);
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-            const float2 f = __half22float2(h2[e]);
-            o2[e] = __hmul2(g2[e], __floats2half2_rn(f.x * rstd, f.y * rstd));
+            const float2 f = to_f2(h2[e]);
+            o2[e] = __hmul2(g2[e], from_f2<T>(f.x * rstd, f.y * rstd));
         }
         o[c] = ov;
     }
@@ -100,7 +107,8 @@ void rms_rows_kernel(const __half* __restrict__ in, const int* __restrict__ rows
 // HF apply_rotary_pos_emb on the Q heads and K heads (contiguous at the start of each QKV row, ld halves apart):
 // x_embed = x * cos + rotate_half(x) * sin in fp16, cos / sin = fp16(cos / sin(fp32(inv_freq[i] * pos))).  Each fp16
 // product and sum is one fp32 operation rounded to half, as torch computes half tensors.  One block per token.
-__global__ void rope_kernel(__half* __restrict__ qkv, const int* __restrict__ cu_seqlens, int B, int ld, int rot_heads,
+template <typename T>
+__global__ void rope_kernel(T* __restrict__ qkv, const int* __restrict__ cu_seqlens, int B, int ld, int rot_heads,
                             const float* __restrict__ inv_freq) {
     const int t = blockIdx.x;
     int lo = 0, hi = B;                          // sequence b with cu[b] <= t < cu[b+1]
@@ -109,24 +117,25 @@ __global__ void rope_kernel(__half* __restrict__ qkv, const int* __restrict__ cu
         if (cu_seqlens[mid] <= t) lo = mid; else hi = mid;
     }
     const float pos = (float)(t - cu_seqlens[lo]);
-    __half* row = qkv + (size_t)t * ld;
+    T* row = qkv + (size_t)t * ld;
     for (int p = threadIdx.x; p < rot_heads * (HD / 2); p += blockDim.x) {
         const int i = p % (HD / 2);
-        __half* x = row + (p / (HD / 2)) * HD;
+        T* x = row + (p / (HD / 2)) * HD;
         const float f = inv_freq[i] * pos;
-        const float c = __half2float(__float2half_rn(cosf(f))), s = __half2float(__float2half_rn(sinf(f)));
-        const float x1 = __half2float(x[i]), x2 = __half2float(x[i + HD / 2]);
-        const float a1 = __half2float(__float2half_rn(x1 * c)), b1 = __half2float(__float2half_rn(-x2 * s));
-        const float a2 = __half2float(__float2half_rn(x2 * c)), b2 = __half2float(__float2half_rn(x1 * s));
-        x[i] = __float2half_rn(a1 + b1);
-        x[i + HD / 2] = __float2half_rn(a2 + b2);
+        const float c = to_f(from_f<T>(cosf(f))), s = to_f(from_f<T>(sinf(f)));
+        const float x1 = to_f(x[i]), x2 = to_f(x[i + HD / 2]);
+        const float a1 = to_f(from_f<T>(x1 * c)), b1 = to_f(from_f<T>(-x2 * s));
+        const float a2 = to_f(from_f<T>(x2 * c)), b2 = to_f(from_f<T>(x1 * s));
+        x[i] = from_f<T>(a1 + b1);
+        x[i + HD / 2] = from_f<T>(a2 + b2);
     }
 }
 
 // GPT-NeoX partial rotary (modeling_gpt_neox.py apply_rotary_pos_emb): rotate_half on dims [0, rot) of every Q and K
 // head (head_dim hd apart, Q heads then K heads at the start of each QKV row), in rope_kernel's fp16 order; dims
 // [rot, hd) are neither read nor written.  One block per token.
-__global__ void rope_partial_kernel(__half* __restrict__ qkv, const int* __restrict__ cu_seqlens, int B, int ld,
+template <typename T>
+__global__ void rope_partial_kernel(T* __restrict__ qkv, const int* __restrict__ cu_seqlens, int B, int ld,
                                     int rot_heads, int hd, int rot, const float* __restrict__ inv_freq) {
     const int t = blockIdx.x;
     int lo = 0, hi = B;
@@ -136,17 +145,17 @@ __global__ void rope_partial_kernel(__half* __restrict__ qkv, const int* __restr
     }
     const float pos = (float)(t - cu_seqlens[lo]);
     const int half_rot = rot >> 1;
-    __half* row = qkv + (size_t)t * ld;
+    T* row = qkv + (size_t)t * ld;
     for (int p = threadIdx.x; p < rot_heads * half_rot; p += blockDim.x) {
         const int i = p % half_rot;
-        __half* x = row + (p / half_rot) * hd;
+        T* x = row + (p / half_rot) * hd;
         const float f = inv_freq[i] * pos;
-        const float c = __half2float(__float2half_rn(cosf(f))), s = __half2float(__float2half_rn(sinf(f)));
-        const float x1 = __half2float(x[i]), x2 = __half2float(x[i + half_rot]);
-        const float a1 = __half2float(__float2half_rn(x1 * c)), b1 = __half2float(__float2half_rn(-x2 * s));
-        const float a2 = __half2float(__float2half_rn(x2 * c)), b2 = __half2float(__float2half_rn(x1 * s));
-        x[i] = __float2half_rn(a1 + b1);
-        x[i + half_rot] = __float2half_rn(a2 + b2);
+        const float c = to_f(from_f<T>(cosf(f))), s = to_f(from_f<T>(sinf(f)));
+        const float x1 = to_f(x[i]), x2 = to_f(x[i + half_rot]);
+        const float a1 = to_f(from_f<T>(x1 * c)), b1 = to_f(from_f<T>(-x2 * s));
+        const float a2 = to_f(from_f<T>(x2 * c)), b2 = to_f(from_f<T>(x1 * s));
+        x[i] = from_f<T>(a1 + b1);
+        x[i + half_rot] = from_f<T>(a2 + b2);
     }
 }
 
@@ -157,10 +166,11 @@ __global__ void rope_partial_kernel(__half* __restrict__ qkv, const int* __restr
 //   w1 != nullptr: out1[i] = LN(X[r]; w1, b1); w2 != nullptr: out2[i] = LN(X[r]; w2, b2) from the same statistics.
 constexpr int LN_THREADS = 256, LN_VEC = 4;   // up to 4 x 8 halves per thread
 constexpr int LN_MAX_HIDDEN = LN_THREADS * LN_VEC * 8;   // 8192: the widest row ln_rows_kernel holds
+template <typename T>
 __global__ __launch_bounds__(LN_THREADS)
-void ln_rows_kernel(__half* __restrict__ X, const __half* __restrict__ add, const int* __restrict__ rows, int hidden,
-                    const __half* __restrict__ w1, const __half* __restrict__ b1, const __half* __restrict__ w2,
-                    const __half* __restrict__ b2, float eps, __half* __restrict__ out1, __half* __restrict__ out2) {
+void ln_rows_kernel(T* __restrict__ X, const T* __restrict__ add, const int* __restrict__ rows, int hidden,
+                    const T* __restrict__ w1, const T* __restrict__ b1, const T* __restrict__ w2,
+                    const T* __restrict__ b2, float eps, T* __restrict__ out1, T* __restrict__ out2) {
     __shared__ float red[LN_THREADS / 32];
     const int i = blockIdx.x;
     const int r = rows ? rows[i] : i;
@@ -176,16 +186,16 @@ void ln_rows_kernel(__half* __restrict__ X, const __half* __restrict__ add, cons
             v[k] = x[c];
             if (add) {
                 const uint4 a = reinterpret_cast<const uint4*>(add + (size_t)r * hidden)[c];
-                __half2* h2 = reinterpret_cast<__half2*>(&v[k]);
-                const __half2* a2 = reinterpret_cast<const __half2*>(&a);
+                pair_t<T>* h2 = reinterpret_cast<pair_t<T>*>(&v[k]);
+                const pair_t<T>* a2 = reinterpret_cast<const pair_t<T>*>(&a);
 #pragma unroll
                 for (int e = 0; e < 4; ++e) h2[e] = __hadd2(h2[e], a2[e]);
                 x[c] = v[k];
             }
-            const __half2* h2 = reinterpret_cast<const __half2*>(&v[k]);
+            const pair_t<T>* h2 = reinterpret_cast<const pair_t<T>*>(&v[k]);
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
-                const float2 f = __half22float2(h2[e]);
+                const float2 f = to_f2(h2[e]);
                 s += f.x + f.y;
             }
         }
@@ -196,10 +206,10 @@ void ln_rows_kernel(__half* __restrict__ X, const __half* __restrict__ add, cons
 #pragma unroll
     for (int k = 0; k < LN_VEC; ++k) {
         if (threadIdx.x + k * LN_THREADS < n8) {
-            const __half2* h2 = reinterpret_cast<const __half2*>(&v[k]);
+            const pair_t<T>* h2 = reinterpret_cast<const pair_t<T>*>(&v[k]);
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
-                const float2 f = __half22float2(h2[e]);
+                const float2 f = to_f2(h2[e]);
                 const float d0 = f.x - mean, d1 = f.y - mean;
                 q = fmaf(d0, d0, q);
                 q = fmaf(d1, d1, q);
@@ -208,8 +218,8 @@ void ln_rows_kernel(__half* __restrict__ X, const __half* __restrict__ add, cons
     }
     const float rstd = rsqrtf(block_sum(q, red) / (float)hidden + eps);
     for (int n = 0; n < 2; ++n) {
-        const __half* w = n ? w2 : w1;
-        const __half* b = n ? b2 : b1;
+        const T* w = n ? w2 : w1;
+        const T* b = n ? b2 : b1;
         if (!w) continue;
         uint4* o = reinterpret_cast<uint4*>((n ? out2 : out1) + (size_t)i * hidden);
 #pragma unroll
@@ -217,15 +227,15 @@ void ln_rows_kernel(__half* __restrict__ X, const __half* __restrict__ add, cons
             const int c = threadIdx.x + k * LN_THREADS;
             if (c >= n8) continue;
             const uint4 g = reinterpret_cast<const uint4*>(w)[c], bb = reinterpret_cast<const uint4*>(b)[c];
-            const __half2* h2 = reinterpret_cast<const __half2*>(&v[k]);
-            const __half2* g2 = reinterpret_cast<const __half2*>(&g);
-            const __half2* bb2 = reinterpret_cast<const __half2*>(&bb);
+            const pair_t<T>* h2 = reinterpret_cast<const pair_t<T>*>(&v[k]);
+            const pair_t<T>* g2 = reinterpret_cast<const pair_t<T>*>(&g);
+            const pair_t<T>* bb2 = reinterpret_cast<const pair_t<T>*>(&bb);
             uint4 ov;
-            __half2* o2 = reinterpret_cast<__half2*>(&ov);
+            pair_t<T>* o2 = reinterpret_cast<pair_t<T>*>(&ov);
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
-                const float2 f = __half22float2(h2[e]), gf = __half22float2(g2[e]), bf = __half22float2(bb2[e]);
-                o2[e] = __floats2half2_rn(fmaf((f.x - mean) * rstd, gf.x, bf.x), fmaf((f.y - mean) * rstd, gf.y, bf.y));
+                const float2 f = to_f2(h2[e]), gf = to_f2(g2[e]), bf = to_f2(bb2[e]);
+                o2[e] = from_f2<T>(fmaf((f.x - mean) * rstd, gf.x, bf.x), fmaf((f.y - mean) * rstd, gf.y, bf.y));
             }
             o[c] = ov;
         }
@@ -240,10 +250,11 @@ void ln_rows_kernel(__half* __restrict__ X, const __half* __restrict__ add, cons
 //   fp32, one rounding, which RoPE then reads.
 //   RoPE: OlmoRotaryEmbedding / Olmo2RotaryEmbedding keep cos / sin in fp32, so x * cos + rotate_half(x) * sin is
 //   evaluated in fp32 (each product and the sum one fp32 rounding, as torch promotes) and rounded to half once.
+template <typename T>
 __global__ __launch_bounds__(256)
-void olmo_qkv_kernel(__half* __restrict__ qkv, const int* __restrict__ cu_seqlens, int B, int heads, int kv_heads,
-                     const float* __restrict__ inv_freq, float clip, const __half* __restrict__ qn,
-                     const __half* __restrict__ kn, float eps) {
+void olmo_qkv_kernel(T* __restrict__ qkv, const int* __restrict__ cu_seqlens, int B, int heads, int kv_heads,
+                     const float* __restrict__ inv_freq, float clip, const T* __restrict__ qn,
+                     const T* __restrict__ kn, float eps) {
     __shared__ float red[8];
     const int t = blockIdx.x;
     int lo = 0, hi = B;
@@ -253,18 +264,18 @@ void olmo_qkv_kernel(__half* __restrict__ qkv, const int* __restrict__ cu_seqlen
     }
     const float pos = (float)(t - cu_seqlens[lo]);
     const int nq = heads * HD, nk = kv_heads * HD;
-    __half* row = qkv + (size_t)t * (nq + 2 * nk);
+    T* row = qkv + (size_t)t * (nq + 2 * nk);
     float rq = 1.f, rk = 1.f;
     if (qn) {
         float sq = 0.f, sk = 0.f;
         const uint4* v = reinterpret_cast<const uint4*>(row);
         for (int c = threadIdx.x; c < (nq + nk) / 8; c += blockDim.x) {
             const uint4 u = v[c];
-            const __half2* h2 = reinterpret_cast<const __half2*>(&u);
+            const pair_t<T>* h2 = reinterpret_cast<const pair_t<T>*>(&u);
             float s = 0.f;
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
-                const float2 f = __half22float2(h2[e]);
+                const float2 f = to_f2(h2[e]);
                 s = fmaf(f.x, f.x, s);
                 s = fmaf(f.y, f.y, s);
             }
@@ -273,35 +284,36 @@ void olmo_qkv_kernel(__half* __restrict__ qkv, const int* __restrict__ cu_seqlen
         rq = rsqrtf(block_sum(sq, red) / (float)nq + eps);   // every read of the row precedes block_sum's barriers
         rk = rsqrtf(block_sum(sk, red) / (float)nk + eps);
     }
-    auto clamped = [clip](float x) { return __half2float(__float2half_rn(fminf(fmaxf(x, -clip), clip))); };
+    auto clamped = [clip](float x) { return to_f(from_f<T>(fminf(fmaxf(x, -clip), clip))); };
     for (int p = threadIdx.x; p < (heads + kv_heads) * (HD / 2); p += blockDim.x) {
         const int hh = p / (HD / 2), i = p % (HD / 2);
-        __half* x = row + hh * HD;
-        float x1 = __half2float(x[i]), x2 = __half2float(x[i + HD / 2]);
+        T* x = row + hh * HD;
+        float x1 = to_f(x[i]), x2 = to_f(x[i + HD / 2]);
         if (clip > 0.f) { x1 = clamped(x1); x2 = clamped(x2); }
         if (qn) {
             const bool q = hh < heads;
-            const __half* w = q ? qn + hh * HD : kn + (hh - heads) * HD;
+            const T* w = q ? qn + hh * HD : kn + (hh - heads) * HD;
             const float r = q ? rq : rk;
-            x1 = __half2float(__float2half_rn(__fmul_rn(__half2float(w[i]), __fmul_rn(x1, r))));
-            x2 = __half2float(__float2half_rn(__fmul_rn(__half2float(w[i + HD / 2]), __fmul_rn(x2, r))));
+            x1 = to_f(from_f<T>(__fmul_rn(to_f(w[i]), __fmul_rn(x1, r))));
+            x2 = to_f(from_f<T>(__fmul_rn(to_f(w[i + HD / 2]), __fmul_rn(x2, r))));
         }
         const float f = inv_freq[i] * pos;
         const float c = cosf(f), s = sinf(f);
-        x[i] = __float2half_rn(__fadd_rn(__fmul_rn(x1, c), __fmul_rn(-x2, s)));
-        x[i + HD / 2] = __float2half_rn(__fadd_rn(__fmul_rn(x2, c), __fmul_rn(x1, s)));
+        x[i] = from_f<T>(__fadd_rn(__fmul_rn(x1, c), __fmul_rn(-x2, s)));
+        x[i + HD / 2] = from_f<T>(__fadd_rn(__fmul_rn(x2, c), __fmul_rn(x1, s)));
     }
     if (clip > 0.f)
-        for (int e = threadIdx.x; e < nk; e += blockDim.x) row[nq + nk + e] = __float2half_rn(clamped(__half2float(row[nq + nk + e])));
+        for (int e = threadIdx.x; e < nk; e += blockDim.x) row[nq + nk + e] = from_f<T>(clamped(to_f(row[nq + nk + e])));
 }
 
 // Olmo2RMSNorm: fp16(w * (x * rsqrt(mean(x^2) + eps))) with fp32 statistics, the weight multiply in fp32 and one
 // rounding (LlamaRMSNorm rounds to half before the weight).  One block per output row i, input row r = rows ? rows[i] : i.
 //   A != nullptr: X[r] = fp16(X[r] + norm(A[r])), OLMo-2's post-norm residual add, in place; out is not written.
 //   A == nullptr: out[i] = norm(X[r]), the final norm on the label rows.
+template <typename T>
 __global__ __launch_bounds__(256)
-void rms_post_kernel(__half* __restrict__ X, const __half* __restrict__ A, const int* __restrict__ rows, int hidden,
-                     const __half* __restrict__ w, float eps, __half* __restrict__ out) {
+void rms_post_kernel(T* __restrict__ X, const T* __restrict__ A, const int* __restrict__ rows, int hidden,
+                     const T* __restrict__ w, float eps, T* __restrict__ out) {
     __shared__ float red[8];
     const int i = blockIdx.x;
     const int r = rows ? rows[i] : i;
@@ -309,10 +321,10 @@ void rms_post_kernel(__half* __restrict__ X, const __half* __restrict__ A, const
     float s = 0.f;
     for (int c = threadIdx.x; c < hidden / 8; c += blockDim.x) {
         const uint4 v = a[c];
-        const __half2* h2 = reinterpret_cast<const __half2*>(&v);
+        const pair_t<T>* h2 = reinterpret_cast<const pair_t<T>*>(&v);
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-            const float2 f = __half22float2(h2[e]);
+            const float2 f = to_f2(h2[e]);
             s = fmaf(f.x, f.x, s);
             s = fmaf(f.y, f.y, s);
         }
@@ -323,18 +335,18 @@ void rms_post_kernel(__half* __restrict__ X, const __half* __restrict__ A, const
     uint4* o = reinterpret_cast<uint4*>(out + (size_t)i * hidden);
     for (int c = threadIdx.x; c < hidden / 8; c += blockDim.x) {
         const uint4 v = a[c], g = wv[c];
-        const __half2* h2 = reinterpret_cast<const __half2*>(&v);
-        const __half2* g2 = reinterpret_cast<const __half2*>(&g);
+        const pair_t<T>* h2 = reinterpret_cast<const pair_t<T>*>(&v);
+        const pair_t<T>* g2 = reinterpret_cast<const pair_t<T>*>(&g);
         uint4 nv;
-        __half2* n2 = reinterpret_cast<__half2*>(&nv);
+        pair_t<T>* n2 = reinterpret_cast<pair_t<T>*>(&nv);
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-            const float2 f = __half22float2(h2[e]), gf = __half22float2(g2[e]);
-            n2[e] = __floats2half2_rn(__fmul_rn(gf.x, __fmul_rn(f.x, rstd)), __fmul_rn(gf.y, __fmul_rn(f.y, rstd)));
+            const float2 f = to_f2(h2[e]), gf = to_f2(g2[e]);
+            n2[e] = from_f2<T>(__fmul_rn(gf.x, __fmul_rn(f.x, rstd)), __fmul_rn(gf.y, __fmul_rn(f.y, rstd)));
         }
         if (A) {
             uint4 xv = x[c];
-            __half2* x2 = reinterpret_cast<__half2*>(&xv);
+            pair_t<T>* x2 = reinterpret_cast<pair_t<T>*>(&xv);
 #pragma unroll
             for (int e = 0; e < 4; ++e) x2[e] = __hadd2(x2[e], n2[e]);
             x[c] = xv;
@@ -344,16 +356,19 @@ void rms_post_kernel(__half* __restrict__ X, const __half* __restrict__ A, const
     }
 }
 
+template <typename T>
 __device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+    if constexpr (std::is_same<T, __half>::value)
+        asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                     : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+                     : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+    else
+        asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                     : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+                     : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
 }
-__device__ __forceinline__ uint32_t half2_bits(float lo, float hi) {
-    const __half2 h = __floats2half2_rn(lo, hi);
-    return *reinterpret_cast<const uint32_t*>(&h);
-}
-__device__ __forceinline__ uint32_t ld32(const __half* p) { return *reinterpret_cast<const uint32_t*>(p); }
+template <typename T>
+__device__ __forceinline__ uint32_t ld32(const T* p) { return *reinterpret_cast<const uint32_t*>(p); }
 
 // Row of 16-byte element idx >= 0 of a tile with n such elements per row: a shift when n is a power of two.
 template <int n>
@@ -363,13 +378,13 @@ __device__ __forceinline__ int tile_row(int idx) {
 }
 
 // Shared tile `which` (0 = K, 1 = V, 2 = Q) of 64 rows of D halves, padded by 8 halves per row against bank conflicts.
-template <int D, int which>
-__device__ __forceinline__ __half (&attention_tile())[AK][D + 8] {
+template <int D, int which, typename T>
+__device__ __forceinline__ T (&attention_tile())[AK][D + 8] {
     if constexpr (D > 128) {
         extern __shared__ __align__(16) unsigned char attn_dyn[];
-        return *reinterpret_cast<__half (*)[AK][D + 8]>(attn_dyn + which * sizeof(__half[AK][D + 8]));
+        return *reinterpret_cast<T (*)[AK][D + 8]>(attn_dyn + which * sizeof(T[AK][D + 8]));
     } else {
-        __shared__ __align__(16) __half tile[AK][D + 8];
+        __shared__ __align__(16) T tile[AK][D + 8];
         return tile;
     }
 }
@@ -383,17 +398,17 @@ __device__ __forceinline__ __half (&attention_tile())[AK][D + 8] {
 // D <= 128: Q fragments in registers, K / V tiles in static shared memory (34.8 KB at D = 128).  D = 256: the 16 x 256
 // fp32 output alone is 128 registers per thread, so Q is staged once in shared memory and its fragments are loaded
 // with ldmatrix per 16-column step; Q, K and V tiles (3 x 33.8 KB) are dynamic shared memory.
-template <int D>
+template <int D, typename T>
 __global__ __launch_bounds__(128)
-void attention_causal_kernel(const __half* __restrict__ qkv, const int* __restrict__ cu_seqlens,
-                             const int2* __restrict__ items, __half* __restrict__ ctx, int heads, int kv_heads,
+void attention_causal_kernel(const T* __restrict__ qkv, const int* __restrict__ cu_seqlens,
+                             const int2* __restrict__ items, T* __restrict__ ctx, int heads, int kv_heads,
                              float scale_log2) {
     constexpr int PAD = D + 8, KS = D / 16, NT = D / 8;
     constexpr bool QSMEM = D > 128;
     constexpr int KT = QSMEM ? 32 : AK, NKT = KT / 8;   // keys per softmax step; its key tiles of 8
-    auto& Ks = attention_tile<D, 0>();
-    auto& Vs = attention_tile<D, 1>();
-    auto& Qs = attention_tile<D, 2>();           // D > 128 only
+    auto& Ks = attention_tile<D, 0, T>();
+    auto& Vs = attention_tile<D, 1, T>();
+    auto& Qs = attention_tile<D, 2, T>();           // D > 128 only
     const int2 it = items[blockIdx.x];
     const int b = it.x, qb = it.y, h = blockIdx.y, kvh = h / (heads / kv_heads);
     const int hid = heads * D, ld = hid + 2 * kv_heads * D;
@@ -401,9 +416,9 @@ void attention_causal_kernel(const __half* __restrict__ qkv, const int* __restri
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
     const int qw = qb * AQ + wib * 16;           // first query row of this warp
     const bool active = qw < S;                  // warp-uniform; idle warps still stage K / V and meet the barriers
-    const __half* qbase = qkv + (size_t)t0 * ld + h * D;
-    const __half* kbase = qkv + (size_t)t0 * ld + hid + kvh * D;
-    const __half* vbase = kbase + kv_heads * D;
+    const T* qbase = qkv + (size_t)t0 * ld + h * D;
+    const T* kbase = qkv + (size_t)t0 * ld + hid + kvh * D;
+    const T* vbase = kbase + kv_heads * D;
     const int r0 = qw + g, r1 = r0 + 8;
 
     uint32_t qa[QSMEM ? 1 : KS][4];
@@ -476,7 +491,7 @@ void attention_causal_kernel(const __half* __restrict__ qkv, const int* __restri
                 if (nt < nvt) {
                     const int j = sb * KT + nt * 8 + g, c = ks * 16 + 2 * t;
                     const uint32_t kf[2] = {ld32(&Ks[j][c]), ld32(&Ks[j][c + 8])};
-                    mma16816(sacc[nt], qa[QSMEM ? 0 : ks], kf);
+                    mma16816<T>(sacc[nt], qa[QSMEM ? 0 : ks], kf);
                 }
             }
         }
@@ -519,10 +534,10 @@ void attention_causal_kernel(const __half* __restrict__ qkv, const int* __restri
         uint32_t pa[NKT / 2][4];
 #pragma unroll
         for (int kk = 0; kk < NKT / 2; ++kk) {
-            pa[kk][0] = half2_bits(sacc[2 * kk][0], sacc[2 * kk][1]);
-            pa[kk][1] = half2_bits(sacc[2 * kk][2], sacc[2 * kk][3]);
-            pa[kk][2] = half2_bits(sacc[2 * kk + 1][0], sacc[2 * kk + 1][1]);
-            pa[kk][3] = half2_bits(sacc[2 * kk + 1][2], sacc[2 * kk + 1][3]);
+            pa[kk][0] = pair_bits<T>(sacc[2 * kk][0], sacc[2 * kk][1]);
+            pa[kk][1] = pair_bits<T>(sacc[2 * kk][2], sacc[2 * kk][3]);
+            pa[kk][2] = pair_bits<T>(sacc[2 * kk + 1][0], sacc[2 * kk + 1][1]);
+            pa[kk][3] = pair_bits<T>(sacc[2 * kk + 1][2], sacc[2 * kk + 1][3]);
         }
 #pragma unroll
         for (int kk = 0; kk < NKT / 2; ++kk) {
@@ -533,7 +548,7 @@ void attention_causal_kernel(const __half* __restrict__ qkv, const int* __restri
                     const uint32_t addr = (uint32_t)__cvta_generic_to_shared(&Vs[sb * KT + kk * 16 + (lane & 15)][nt * 8]);
                     asm volatile("ldmatrix.sync.aligned.m8n8.x2.trans.shared.b16 {%0,%1}, [%2];"
                                  : "=r"(vb[0]), "=r"(vb[1]) : "r"(addr));
-                    mma16816(o[nt], pa[kk], vb);
+                    mma16816<T>(o[nt], pa[kk], vb);
                 }
             }
         }
@@ -551,31 +566,32 @@ void attention_causal_kernel(const __half* __restrict__ qkv, const int* __restri
 #pragma unroll
     for (int nt = 0; nt < NT; ++nt) {
         const int col = h * D + nt * 8 + 2 * t;
-        if (r0 < S) *reinterpret_cast<__half2*>(ctx + (size_t)(t0 + r0) * hid + col) = __floats2half2_rn(o[nt][0] * inv[0], o[nt][1] * inv[0]);
-        if (r1 < S) *reinterpret_cast<__half2*>(ctx + (size_t)(t0 + r1) * hid + col) = __floats2half2_rn(o[nt][2] * inv[1], o[nt][3] * inv[1]);
+        if (r0 < S) *reinterpret_cast<pair_t<T>*>(ctx + (size_t)(t0 + r0) * hid + col) = from_f2<T>(o[nt][0] * inv[0], o[nt][1] * inv[0]);
+        if (r1 < S) *reinterpret_cast<pair_t<T>*>(ctx + (size_t)(t0 + r1) * hid + col) = from_f2<T>(o[nt][2] * inv[1], o[nt][3] * inv[1]);
     }
 }
-constexpr size_t attention_dyn_smem(int D) { return D > 128 ? 3 * (size_t)AK * (D + 8) * sizeof(__half) : 0; }
+constexpr size_t attention_dyn_smem(int D) { return D > 128 ? 3 * (size_t)AK * (D + 8) * sizeof(__half) : 0; }   // 2-byte elements in both dtypes
 
 // act[t, j] = fp16(fp16(silu(gate[t, j])) * up[t, j]) with gu = [gate | up] rows of 2 * inter; silu as torch computes it
 // on half, x / (1 + exp(-x)) in fp32 rounded to half.  8 elements per thread.
-__global__ void swiglu_kernel(const __half* __restrict__ gu, long long n8, int inter, __half* __restrict__ act) {
+template <typename T>
+__global__ void swiglu_kernel(const T* __restrict__ gu, long long n8, int inter, T* __restrict__ act) {
     const int per_row = inter / 8;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n8; i += (long long)gridDim.x * blockDim.x) {
         const long long t = i / per_row;
         const int c = (int)(i % per_row) * 8;
         const uint4 gv = *reinterpret_cast<const uint4*>(gu + t * 2 * inter + c);
         const uint4 uv = *reinterpret_cast<const uint4*>(gu + t * 2 * inter + inter + c);
-        const __half2* g2 = reinterpret_cast<const __half2*>(&gv);
-        const __half2* u2 = reinterpret_cast<const __half2*>(&uv);
+        const pair_t<T>* g2 = reinterpret_cast<const pair_t<T>*>(&gv);
+        const pair_t<T>* u2 = reinterpret_cast<const pair_t<T>*>(&uv);
         uint4 ov;
-        __half2* o2 = reinterpret_cast<__half2*>(&ov);
+        pair_t<T>* o2 = reinterpret_cast<pair_t<T>*>(&ov);
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-            const float2 x = __half22float2(g2[e]);
-            const __half2 s = __floats2half2_rn(__fdiv_rn(x.x, 1.f + expf(-x.x)), __fdiv_rn(x.y, 1.f + expf(-x.y)));
-            const float2 sf = __half22float2(s), uf = __half22float2(u2[e]);
-            o2[e] = __floats2half2_rn(sf.x * uf.x, sf.y * uf.y);
+            const float2 x = to_f2(g2[e]);
+            const pair_t<T> s = from_f2<T>(__fdiv_rn(x.x, 1.f + expf(-x.x)), __fdiv_rn(x.y, 1.f + expf(-x.y)));
+            const float2 sf = to_f2(s), uf = to_f2(u2[e]);
+            o2[e] = from_f2<T>(sf.x * uf.x, sf.y * uf.y);
         }
         *reinterpret_cast<uint4*>(act + t * inter + c) = ov;
     }
@@ -590,20 +606,21 @@ __device__ __forceinline__ void lse_merge(float& m, float& s, float m2, float s2
 
 // nll_out[out_idx[i]] = logsumexp(logits[i, 0:vocab]) - logits[i, label[i]] in fp32; columns vocab..ld-1 are the LM
 // head's pad rows and never enter the sum.  One block per row, one pass with a running (max, sum) per thread.
+template <typename T>
 __global__ __launch_bounds__(256)
-void nll_rows_kernel(const __half* __restrict__ logits, int vocab, int ld, const int* __restrict__ labels,
+void nll_rows_kernel(const T* __restrict__ logits, int vocab, int ld, const int* __restrict__ labels,
                      const int* __restrict__ out_idx, float* __restrict__ nll_out) {
     __shared__ float rm[8], rs[8];
     const int i = blockIdx.x;
-    const __half* row = logits + (size_t)i * ld;
+    const T* row = logits + (size_t)i * ld;
     float m = -INFINITY, s = 0.f;
     for (int c = threadIdx.x * 8; c < vocab; c += blockDim.x * 8) {
         const uint4 v = *reinterpret_cast<const uint4*>(row + c);
-        const __half* hv = reinterpret_cast<const __half*>(&v);
+        const T* hv = reinterpret_cast<const T*>(&v);
         float x[8], mx = -INFINITY;
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
-            x[e] = c + e < vocab ? __half2float(hv[e]) : -INFINITY;
+            x[e] = c + e < vocab ? to_f(hv[e]) : -INFINITY;
             mx = fmaxf(mx, x[e]);
         }
         const float mn = fmaxf(m, mx);
@@ -621,7 +638,7 @@ void nll_rows_kernel(const __half* __restrict__ logits, int vocab, int ld, const
     if (threadIdx.x == 0) {
         float M = rm[0], Sm = rs[0];
         for (int w = 1; w < (int)(blockDim.x >> 5); ++w) lse_merge(M, Sm, rm[w], rs[w]);
-        nll_out[out_idx[i]] = (M + logf(Sm)) - __half2float(row[labels[i]]);
+        nll_out[out_idx[i]] = (M + logf(Sm)) - to_f(row[labels[i]]);
     }
 }
 
@@ -656,6 +673,9 @@ struct rsb_llm {
     int olmo = 0;                                // 1 = OLMo, 2 = OLMo-2 (rsb_llm_create_olmo), 0 otherwise
     float rope_theta = 0.f, eps = 0.f, clip = 0.f;   // clip: OLMo clip_qkv, 0 = none
     bool tied = false, neox = false;
+    bool bf16 = false;                           // element type of weights and activations (rsb_llm_set_dtype)
+    bool load_called = false;                    // rsb_llm_load has been called: the dtype is fixed
+    // Device buffers of 2-byte elements, fp16 or bf16 by the handle's dtype; every zero fill means 0 in both.
     // OLMo: final_g holds ones, the unit scale with which ln_rows_kernel (and zero_bias as its shift) is OlmoLayerNorm
     __half *embed = nullptr, *lm_head = nullptr, *final_g = nullptr, *final_b = nullptr, *zero_bias = nullptr;
     float* inv_freq = nullptr;
@@ -674,9 +694,19 @@ struct rsb_llm {
 
 namespace {
 
-int gemm(const __half* A, int M, const __half* W, int N, int K, const __half* bias, const __half* residual, __half* C,
+// A weight or bias buffer of the handle as element type E (the buffers are allocated as __half, 2 bytes either way).
+template <typename E> const E* as(const __half* p) { return reinterpret_cast<const E*>(p); }
+
+// f(E()) for the handle's element type E
+template <class F> int with_dtype(const rsb_llm* h, F&& f) { return h->bf16 ? f(__nv_bfloat16()) : f(__half()); }
+
+template <typename E> using same_t = typename std::common_type<E>::type;   // E, not deduced from this argument
+
+template <typename E>
+int gemm(const E* A, int M, const __half* W, int N, int K, const __half* bias, const same_t<E>* residual, same_t<E>* C,
          int epi, cudaStream_t st) {
-    const int rc = rsb_gemm_f16(A, W, bias, residual, C, M, N, K, epi, st);
+    const int rc = std::is_same<E, __half>::value ? rsb_gemm_f16(A, W, bias, residual, C, M, N, K, epi, st)
+                                                  : rsb::gemm_bf16(A, W, bias, residual, C, M, N, K, epi, st);
     return rc == RSB_OK ? RSB_OK : lfail(rc, "linear layer (%s)", rsb_bert_last_error());
 }
 
@@ -851,6 +881,23 @@ extern "C" int rsb_llm_create_olmo(int version, int layers, int hidden, int head
     return RSB_OK;
 }
 
+// The element type of the handle's weights and activations: RSB_DTYPE_F16 (the default) or RSB_DTYPE_BF16, before the
+// first rsb_llm_load.  OLMo's unit LayerNorm scale is rewritten in the new type.
+extern "C" int rsb_llm_set_dtype(rsb_llm_t* h, int dtype) {
+    if (!h) return lfail(RSB_ERR_INVALID, "null argument");
+    if (dtype != RSB_DTYPE_F16 && dtype != RSB_DTYPE_BF16)
+        return lfail(RSB_ERR_INVALID, "dtype %ld is neither RSB_DTYPE_F16 nor RSB_DTYPE_BF16", (long)dtype);
+    if (h->load_called) return lfail(RSB_ERR_STATE, "the dtype is fixed once rsb_llm_load has been called");
+    h->bf16 = dtype == RSB_DTYPE_BF16;
+    if (h->olmo == 1) {
+        const uint16_t one = h->bf16 ? 0x3F80 : 0x3C00;   // 1.0 in bf16 / fp16
+        const std::vector<uint16_t> ones(h->hidden, one);
+        if (cudaMemcpy(h->final_g, ones.data(), (size_t)h->hidden * 2, cudaMemcpyHostToDevice) != cudaSuccess)
+            return lfail(RSB_ERR_CUDA, "writing the OLMo LayerNorm scale failed");
+    }
+    return RSB_OK;
+}
+
 extern "C" int rsb_llm_free(rsb_llm_t* h) {
     if (!h) return RSB_OK;
     cudaFree(h->embed); cudaFree(h->lm_head); cudaFree(h->final_g); cudaFree(h->final_b); cudaFree(h->zero_bias);
@@ -920,6 +967,7 @@ int load_neox(rsb_llm* h, const char* name, const void* src, int64_t n, cudaStre
 
 extern "C" int rsb_llm_load(rsb_llm_t* h, const char* name, const void* f16_dev, int64_t n, rsb_stream_t stream) {
     if (!h || !name || !f16_dev) return lfail(RSB_ERR_INVALID, "null argument");
+    h->load_called = true;
     cudaStream_t st = (cudaStream_t)stream;
     if (h->neox) return load_neox(h, name, f16_dev, n, st);
     const int64_t H = h->hidden, KV = (int64_t)h->kv_heads * HD, I = h->inter;
@@ -999,29 +1047,30 @@ int upload_attention_items(const std::vector<int32_t>& cu, int B, int2* d_items,
 // One attention step of layer l on the fused QKV rows [n_tok, qkv_n] of a batch whose windows end at n_tok = cu[B]:
 // RoPE on the Q and K heads in place (OLMo: the clip / QK-norm prologue and fp32 RoPE), then causal attention into CTX
 // [n_tok, hidden].
-void attention_step(const rsb_llm* h, const LlmLayer& l, __half* QKV, const int32_t* cu_seqlens, int B, int n_tok,
-                    const int2* d_items, int n_items, __half* CTX, cudaStream_t st) {
+template <typename E>
+void attention_step(const rsb_llm* h, const LlmLayer& l, E* QKV, const int32_t* cu_seqlens, int B, int n_tok,
+                    const int2* d_items, int n_items, E* CTX, cudaStream_t st) {
     if (n_tok == 0 || n_items == 0) return;
     const float scale_log2 = 1.4426950408889634f / sqrtf((float)h->head_dim);   // 1/sqrt(head_dim) in the log2 domain
     if (h->neox)
-        rope_partial_kernel<<<n_tok, 256, 0, st>>>(QKV, cu_seqlens, B, h->qkv_n(), h->heads + h->kv_heads, h->head_dim,
+        rope_partial_kernel<E><<<n_tok, 256, 0, st>>>(QKV, cu_seqlens, B, h->qkv_n(), h->heads + h->kv_heads, h->head_dim,
                                                    h->rot, h->inv_freq);
     else if (h->olmo)
-        olmo_qkv_kernel<<<n_tok, 256, 0, st>>>(QKV, cu_seqlens, B, h->heads, h->kv_heads, h->inv_freq, h->clip,
-                                               h->olmo == 2 ? l.qn : nullptr, l.kn, h->eps);
+        olmo_qkv_kernel<E><<<n_tok, 256, 0, st>>>(QKV, cu_seqlens, B, h->heads, h->kv_heads, h->inv_freq, h->clip,
+                                                  h->olmo == 2 ? as<E>(l.qn) : nullptr, as<E>(l.kn), h->eps);
     else
-        rope_kernel<<<n_tok, 256, 0, st>>>(QKV, cu_seqlens, B, h->qkv_n(), h->heads + h->kv_heads, h->inv_freq);
+        rope_kernel<E><<<n_tok, 256, 0, st>>>(QKV, cu_seqlens, B, h->qkv_n(), h->heads + h->kv_heads, h->inv_freq);
     const dim3 grid((unsigned)n_items, h->heads);
     switch (h->head_dim) {
-        case 64: attention_causal_kernel<64><<<grid, 128, 0, st>>>(QKV, cu_seqlens, d_items, CTX, h->heads, h->kv_heads, scale_log2); break;
-        case 80: attention_causal_kernel<80><<<grid, 128, 0, st>>>(QKV, cu_seqlens, d_items, CTX, h->heads, h->kv_heads, scale_log2); break;
-        case 128: attention_causal_kernel<128><<<grid, 128, 0, st>>>(QKV, cu_seqlens, d_items, CTX, h->heads, h->kv_heads, scale_log2); break;
+        case 64: attention_causal_kernel<64, E><<<grid, 128, 0, st>>>(QKV, cu_seqlens, d_items, CTX, h->heads, h->kv_heads, scale_log2); break;
+        case 80: attention_causal_kernel<80, E><<<grid, 128, 0, st>>>(QKV, cu_seqlens, d_items, CTX, h->heads, h->kv_heads, scale_log2); break;
+        case 128: attention_causal_kernel<128, E><<<grid, 128, 0, st>>>(QKV, cu_seqlens, d_items, CTX, h->heads, h->kv_heads, scale_log2); break;
         default: {
             constexpr size_t smem = attention_dyn_smem(256);
             static rsb::PerDeviceFlag configured;            // attributes are per (function, device)
             if (configured.first())
-                cudaFuncSetAttribute(attention_causal_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            attention_causal_kernel<256><<<grid, 128, smem, st>>>(QKV, cu_seqlens, d_items, CTX, h->heads, h->kv_heads, scale_log2);
+                cudaFuncSetAttribute(attention_causal_kernel<256, E>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            attention_causal_kernel<256, E><<<grid, 128, smem, st>>>(QKV, cu_seqlens, d_items, CTX, h->heads, h->kv_heads, scale_log2);
         }
     }
 }
@@ -1054,28 +1103,30 @@ int check_forward(rsb_llm* h, const int32_t* ids, const int32_t* cu_seqlens, con
 }
 
 // Workspace slots of one forward (llm_ws_layout) and its attention work list.
+template <typename E>
 struct Fwd {
-    __half *X, *Hn, *QKV, *CTX, *GU, *ACT;
+    E *X, *Hn, *QKV, *CTX, *GU, *ACT;
     const int32_t* cu_seqlens;
     int B, T, n_items;
     const int2* d_items;
 };
 
 // LlamaDecoderLayer x layers: x += o_proj(attn(rms1(x))); x += down(swiglu(gate|up(rms2(x)))).
-int llama_layers(rsb_llm* h, const Fwd& f, cudaStream_t st) {
+template <typename E>
+int llama_layers(rsb_llm* h, const Fwd<E>& f, cudaStream_t st) {
     const int Hd = h->hidden, NQKV = h->qkv_n(), I = h->inter, T = f.T;
     const long long n8 = (long long)T * I / 8;
     const int sw_grid = (int)std::min<long long>((n8 + 255) / 256, 8LL * rsb::device_num_sms());
     int rc;
     for (int li = 0; li < h->layers; ++li) {
         const LlmLayer& l = h->L[li];
-        rms_rows_kernel<<<T, 256, 0, st>>>(f.X, nullptr, Hd, l.ln1, h->eps, f.Hn);
+        rms_rows_kernel<E><<<T, 256, 0, st>>>(f.X, nullptr, Hd, as<E>(l.ln1), h->eps, f.Hn);
         if ((rc = gemm(f.Hn, T, l.wqkv, NQKV, Hd, h->zero_bias, nullptr, f.QKV, 0, st)) != RSB_OK) return rc;
         attention_step(h, l, f.QKV, f.cu_seqlens, f.B, T, f.d_items, f.n_items, f.CTX, st);
         if ((rc = gemm(f.CTX, T, l.wo, Hd, Hd, h->zero_bias, f.X, f.X, 2, st)) != RSB_OK) return rc;
-        rms_rows_kernel<<<T, 256, 0, st>>>(f.X, nullptr, Hd, l.ln2, h->eps, f.Hn);
+        rms_rows_kernel<E><<<T, 256, 0, st>>>(f.X, nullptr, Hd, as<E>(l.ln2), h->eps, f.Hn);
         if ((rc = gemm(f.Hn, T, l.wgu, 2 * I, Hd, h->zero_bias, nullptr, f.GU, 0, st)) != RSB_OK) return rc;
-        swiglu_kernel<<<sw_grid, 256, 0, st>>>(f.GU, n8, I, f.ACT);
+        swiglu_kernel<E><<<sw_grid, 256, 0, st>>>(f.GU, n8, I, f.ACT);
         if ((rc = gemm(f.ACT, T, l.wdown, Hd, I, h->zero_bias, f.X, f.X, 2 | RSB_GEMM_REVERSED, st)) != RSB_OK) return rc;
     }
     return RSB_OK;
@@ -1085,15 +1136,16 @@ int llama_layers(rsb_llm* h, const Fwd& f, cudaStream_t st) {
 // both pre-norms.  Olmo2DecoderLayer x layers: no pre-norms; x = fp16(x + post_attention_layernorm(o_proj(attn(x)))),
 // then x = fp16(x + post_feedforward_layernorm(down(swiglu(gate|up(x))))).  A norm sits between each projection and
 // its add, so o_proj and down_proj write slot 1 (free without pre-norms) and rms_post_kernel adds the normed rows to x.
-int olmo_layers(rsb_llm* h, const Fwd& f, cudaStream_t st) {
+template <typename E>
+int olmo_layers(rsb_llm* h, const Fwd<E>& f, cudaStream_t st) {
     const int Hd = h->hidden, NQKV = h->qkv_n(), I = h->inter, T = f.T;
     const long long n8 = (long long)T * I / 8;
     const int sw_grid = (int)std::min<long long>((n8 + 255) / 256, 8LL * rsb::device_num_sms());
     const bool v2 = h->olmo == 2;
-    const __half* in = v2 ? f.X : f.Hn;          // what q|k|v and gate|up read
+    const E* in = v2 ? f.X : f.Hn;               // what q|k|v and gate|up read
     auto olmo_ln = [&]() {
-        ln_rows_kernel<<<T, LN_THREADS, 0, st>>>(f.X, nullptr, nullptr, Hd, h->final_g, h->zero_bias, nullptr, nullptr,
-                                                 h->eps, f.Hn, nullptr);
+        ln_rows_kernel<E><<<T, LN_THREADS, 0, st>>>(f.X, nullptr, nullptr, Hd, as<E>(h->final_g), as<E>(h->zero_bias),
+                                                    nullptr, nullptr, h->eps, f.Hn, nullptr);
     };
     int rc;
     for (int li = 0; li < h->layers; ++li) {
@@ -1103,16 +1155,16 @@ int olmo_layers(rsb_llm* h, const Fwd& f, cudaStream_t st) {
         attention_step(h, l, f.QKV, f.cu_seqlens, f.B, T, f.d_items, f.n_items, f.CTX, st);
         if (v2) {
             if ((rc = gemm(f.CTX, T, l.wo, Hd, Hd, h->zero_bias, nullptr, f.Hn, 0, st)) != RSB_OK) return rc;
-            rms_post_kernel<<<T, 256, 0, st>>>(f.X, f.Hn, nullptr, Hd, l.ln1, h->eps, nullptr);
+            rms_post_kernel<E><<<T, 256, 0, st>>>(f.X, f.Hn, nullptr, Hd, as<E>(l.ln1), h->eps, nullptr);
         } else {
             if ((rc = gemm(f.CTX, T, l.wo, Hd, Hd, h->zero_bias, f.X, f.X, 2, st)) != RSB_OK) return rc;
             olmo_ln();
         }
         if ((rc = gemm(in, T, l.wgu, 2 * I, Hd, h->zero_bias, nullptr, f.GU, 0, st)) != RSB_OK) return rc;
-        swiglu_kernel<<<sw_grid, 256, 0, st>>>(f.GU, n8, I, f.ACT);
+        swiglu_kernel<E><<<sw_grid, 256, 0, st>>>(f.GU, n8, I, f.ACT);
         if (v2) {
             if ((rc = gemm(f.ACT, T, l.wdown, Hd, I, h->zero_bias, nullptr, f.Hn, 0, st)) != RSB_OK) return rc;
-            rms_post_kernel<<<T, 256, 0, st>>>(f.X, f.Hn, nullptr, Hd, l.ln2, h->eps, nullptr);
+            rms_post_kernel<E><<<T, 256, 0, st>>>(f.X, f.Hn, nullptr, Hd, as<E>(l.ln2), h->eps, nullptr);
         } else if ((rc = gemm(f.ACT, T, l.wdown, Hd, I, h->zero_bias, f.X, f.X, 2 | RSB_GEMM_REVERSED, st)) != RSB_OK) {
             return rc;
         }
@@ -1123,12 +1175,14 @@ int olmo_layers(rsb_llm* h, const Fwd& f, cudaStream_t st) {
 // GPTNeoXLayer x layers with the parallel residual: x = fp16(fp16(mlp(ln2(x)) + attn(ln1(x))) + x).  The MLP's last
 // GEMM adds the attention block's output A in its residual epilogue (A = fp16(mlp + attn), in place); the next
 // ln_rows_kernel adds A to x, writes x back and normalises it twice, for the next layer's ln1 and ln2.
-int neox_layers(rsb_llm* h, const Fwd& f, cudaStream_t st) {
+template <typename E>
+int neox_layers(rsb_llm* h, const Fwd<E>& f, cudaStream_t st) {
     const int Hd = h->hidden, NQKV = h->qkv_n(), I = h->inter, T = f.T;
-    __half *N1 = f.Hn, *N2 = f.Hn + (size_t)T * Hd, *FF = f.GU, *A = f.ACT;
+    E *N1 = f.Hn, *N2 = f.Hn + (size_t)T * Hd, *FF = f.GU, *A = f.ACT;
+    const LlmLayer& l0 = h->L[0];
     int rc;
-    ln_rows_kernel<<<T, LN_THREADS, 0, st>>>(f.X, nullptr, nullptr, Hd, h->L[0].ln1, h->L[0].ln1b, h->L[0].ln2,
-                                             h->L[0].ln2b, h->eps, N1, N2);
+    ln_rows_kernel<E><<<T, LN_THREADS, 0, st>>>(f.X, nullptr, nullptr, Hd, as<E>(l0.ln1), as<E>(l0.ln1b), as<E>(l0.ln2),
+                                                as<E>(l0.ln2b), h->eps, N1, N2);
     for (int li = 0; li < h->layers; ++li) {
         const LlmLayer& l = h->L[li];
         if ((rc = gemm(N1, T, l.wqkv, NQKV, Hd, l.bqkv, nullptr, f.QKV, 0, st)) != RSB_OK) return rc;
@@ -1137,22 +1191,24 @@ int neox_layers(rsb_llm* h, const Fwd& f, cudaStream_t st) {
         if ((rc = gemm(N2, T, l.wgu, I, Hd, l.bgu, nullptr, FF, 1, st)) != RSB_OK) return rc;
         if ((rc = gemm(FF, T, l.wdown, Hd, I, l.bdown, A, A, 2 | RSB_GEMM_REVERSED, st)) != RSB_OK) return rc;
         const LlmLayer* nx = li + 1 < h->layers ? &h->L[li + 1] : nullptr;   // the last layer only adds
-        ln_rows_kernel<<<T, LN_THREADS, 0, st>>>(f.X, A, nullptr, Hd, nx ? nx->ln1 : nullptr, nx ? nx->ln1b : nullptr,
-                                                 nx ? nx->ln2 : nullptr, nx ? nx->ln2b : nullptr, h->eps, N1, N2);
+        ln_rows_kernel<E><<<T, LN_THREADS, 0, st>>>(f.X, A, nullptr, Hd, nx ? as<E>(nx->ln1) : nullptr,
+                                                    nx ? as<E>(nx->ln1b) : nullptr, nx ? as<E>(nx->ln2) : nullptr,
+                                                    nx ? as<E>(nx->ln2b) : nullptr, h->eps, N1, N2);
     }
     return RSB_OK;
 }
 
 // The decoder layers: X (workspace slot 0) ends as the residual stream after the last layer, before the final norm.
+template <typename E>
 int trunk(rsb_llm* h, const int32_t* ids, const int32_t* cu_seqlens, int B, int T, const std::vector<int32_t>& cu,
           unsigned char* w, const size_t off[10], cudaStream_t st) {
-    Fwd f;
-    f.X = reinterpret_cast<__half*>(w + off[0]);
-    f.Hn = reinterpret_cast<__half*>(w + off[1]);
-    f.QKV = reinterpret_cast<__half*>(w + off[2]);
-    f.CTX = reinterpret_cast<__half*>(w + off[3]);
-    f.GU = reinterpret_cast<__half*>(w + off[4]);
-    f.ACT = reinterpret_cast<__half*>(w + off[5]);
+    Fwd<E> f;
+    f.X = reinterpret_cast<E*>(w + off[0]);
+    f.Hn = reinterpret_cast<E*>(w + off[1]);
+    f.QKV = reinterpret_cast<E*>(w + off[2]);
+    f.CTX = reinterpret_cast<E*>(w + off[3]);
+    f.GU = reinterpret_cast<E*>(w + off[4]);
+    f.ACT = reinterpret_cast<E*>(w + off[5]);
     f.cu_seqlens = cu_seqlens;
     f.B = B;
     f.T = T;
@@ -1160,20 +1216,22 @@ int trunk(rsb_llm* h, const int32_t* ids, const int32_t* cu_seqlens, int B, int 
     f.d_items = d_items;
     int rc;
     if ((rc = upload_attention_items(cu, B, d_items, st, &f.n_items)) != RSB_OK) return rc;
-    embed_rows_kernel<<<T, 128, 0, st>>>(ids, h->embed, h->hidden, f.X);
+    embed_rows_kernel<E><<<T, 128, 0, st>>>(ids, as<E>(h->embed), h->hidden, f.X);
     if (h->neox) return neox_layers(h, f, st);
     return h->olmo ? olmo_layers(h, f, st) : llama_layers(h, f, st);
 }
 
 // The final norm of the label rows X[rows[i]] into out[i], i < n.
-void final_norm(const rsb_llm* h, const __half* X, const int* rows, int n, __half* out, cudaStream_t st) {
+template <typename E>
+void final_norm(const rsb_llm* h, const E* X, const int* rows, int n, E* out, cudaStream_t st) {
     if (h->neox || h->olmo == 1)                 // OLMo: unit scale (final_g) and zero shift
-        ln_rows_kernel<<<n, LN_THREADS, 0, st>>>(const_cast<__half*>(X), nullptr, rows, h->hidden, h->final_g,
-                                                 h->neox ? h->final_b : h->zero_bias, nullptr, nullptr, h->eps, out, nullptr);
+        ln_rows_kernel<E><<<n, LN_THREADS, 0, st>>>(const_cast<E*>(X), nullptr, rows, h->hidden, as<E>(h->final_g),
+                                                    as<E>(h->neox ? h->final_b : h->zero_bias), nullptr, nullptr, h->eps,
+                                                    out, nullptr);
     else if (h->olmo == 2)
-        rms_post_kernel<<<n, 256, 0, st>>>(const_cast<__half*>(X), nullptr, rows, h->hidden, h->final_g, h->eps, out);
+        rms_post_kernel<E><<<n, 256, 0, st>>>(const_cast<E*>(X), nullptr, rows, h->hidden, as<E>(h->final_g), h->eps, out);
     else
-        rms_rows_kernel<<<n, 256, 0, st>>>(X, rows, h->hidden, h->final_g, h->eps, out);
+        rms_rows_kernel<E><<<n, 256, 0, st>>>(X, rows, h->hidden, as<E>(h->final_g), h->eps, out);
 }
 
 }  // namespace
@@ -1198,9 +1256,6 @@ extern "C" int rsb_llm_nll(rsb_llm_t* h, const int32_t* ids, const int32_t* cu_s
     const size_t need = llm_ws_layout(h, (size_t)T, (size_t)nl, off);
     if (ws_bytes < need) return lfail(RSB_ERR_OOM, "reader workspace too small (need %ld bytes)", (long)need);
     unsigned char* w = static_cast<unsigned char*>(ws);
-    __half* X = reinterpret_cast<__half*>(w + off[0]);
-    __half* Hn = reinterpret_cast<__half*>(w + off[1]);
-    __half* LOG = reinterpret_cast<__half*>(w + off[6]);
     int* d_rows = reinterpret_cast<int*>(w + off[7]);
     int* d_labs = d_rows + nl;
     int* d_outi = d_labs + nl;
@@ -1210,21 +1265,32 @@ extern "C" int rsb_llm_nll(rsb_llm_t* h, const int32_t* ids, const int32_t* cu_s
         return lfail(RSB_ERR_CUDA, "uploading the label rows failed");
     if (cudaMemsetAsync(nll_out, 0, (size_t)T * sizeof(float), st) != cudaSuccess)
         return lfail(RSB_ERR_CUDA, "clearing nll_out failed");
-    if ((rc = trunk(h, ids, cu_seqlens, B, T, cu, w, off, st)) != RSB_OK) return rc;
-    // final norm and LM head on the label rows only, in chunks that bound the logits workspace
-    const int Hd = h->hidden, chunk = h->chunk_rows();
-    for (int c0 = 0; c0 < nl; c0 += chunk) {
-        const int n = std::min(chunk, nl - c0);
-        final_norm(h, X, d_rows + c0, n, Hn, st);
-        if ((rc = gemm(Hn, n, h->lm_head, h->vocab_pad, Hd, h->zero_bias, nullptr, LOG, 0, st)) != RSB_OK) return rc;
-        nll_rows_kernel<<<n, 256, 0, st>>>(LOG, h->vocab, h->vocab_pad, d_labs + c0, d_outi + c0, nll_out);
-    }
+    rc = with_dtype(h, [&](auto tag) -> int {
+        using E = decltype(tag);
+        int rc = trunk<E>(h, ids, cu_seqlens, B, T, cu, w, off, st);
+        if (rc != RSB_OK) return rc;
+        // final norm and LM head on the label rows only, in chunks that bound the logits workspace; the logits are in
+        // the handle's dtype and nll_rows_kernel takes their fp32 log-sum-exp (transformers' logits.float())
+        E* X = reinterpret_cast<E*>(w + off[0]);
+        E* Hn = reinterpret_cast<E*>(w + off[1]);
+        E* LOG = reinterpret_cast<E*>(w + off[6]);
+        const int Hd = h->hidden, chunk = h->chunk_rows();
+        for (int c0 = 0; c0 < nl; c0 += chunk) {
+            const int n = std::min(chunk, nl - c0);
+            final_norm<E>(h, X, d_rows + c0, n, Hn, st);
+            if ((rc = gemm<E>(Hn, n, h->lm_head, h->vocab_pad, Hd, h->zero_bias, nullptr, LOG, 0, st)) != RSB_OK) return rc;
+            nll_rows_kernel<E><<<n, 256, 0, st>>>(LOG, h->vocab, h->vocab_pad, d_labs + c0, d_outi + c0, nll_out);
+        }
+        return RSB_OK;
+    });
+    if (rc != RSB_OK) return rc;
     const cudaError_t e = cudaPeekAtLastError();
     if (e != cudaSuccess) return lfail(RSB_ERR_CUDA, "reader launch failed: %s", cudaGetErrorString(e));
     return RSB_OK;
 }
 
-// Diagnostic: the residual stream after the last layer (before the final norm) of the same forward, [T, hidden] fp16.
+// Diagnostic: the residual stream after the last layer (before the final norm) of the same forward, [T, hidden] in the
+// handle's dtype.
 extern "C" int rsb_llm_hidden_states(rsb_llm_t* h, const int32_t* ids, const int32_t* cu_seqlens, int B, int T,
                                      int max_seqlen, void* out, void* ws, size_t ws_bytes, rsb_stream_t stream) {
     if (!h || !ids || !cu_seqlens || !out || !ws) return lfail(RSB_ERR_INVALID, "null argument");
@@ -1236,7 +1302,8 @@ extern "C" int rsb_llm_hidden_states(rsb_llm_t* h, const int32_t* ids, const int
     const size_t need = llm_ws_layout(h, (size_t)T, 0, off);
     if (ws_bytes < need) return lfail(RSB_ERR_OOM, "reader workspace too small (need %ld bytes)", (long)need);
     unsigned char* w = static_cast<unsigned char*>(ws);
-    if ((rc = trunk(h, ids, cu_seqlens, B, T, cu, w, off, st)) != RSB_OK) return rc;
+    rc = with_dtype(h, [&](auto tag) -> int { return trunk<decltype(tag)>(h, ids, cu_seqlens, B, T, cu, w, off, st); });
+    if (rc != RSB_OK) return rc;
     if (cudaMemcpyAsync(out, w + off[0], (size_t)T * h->hidden * 2, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
         return lfail(RSB_ERR_CUDA, "copying the hidden states failed");
     const cudaError_t e = cudaPeekAtLastError();
@@ -1244,8 +1311,8 @@ extern "C" int rsb_llm_hidden_states(rsb_llm_t* h, const int32_t* ids, const int
     return RSB_OK;
 }
 
-// Diagnostic: one attention step of the forward on a caller's fused QKV rows [T, (heads + 2 kv_heads) head_dim] fp16
-// (GPT-NeoX: [Q heads | K heads | V heads], as rsb_llm_load permutes query_key_value).
+// Diagnostic: one attention step of the forward on a caller's fused QKV rows [T, (heads + 2 kv_heads) head_dim] in the
+// handle's dtype (GPT-NeoX: [Q heads | K heads | V heads], as rsb_llm_load permutes query_key_value).
 extern "C" int rsb_llm_attention(rsb_llm_t* h, void* qkv, const int32_t* cu_seqlens, int B, int T, int max_seqlen,
                                  void* ctx, rsb_stream_t stream) {
     if (!h || !qkv || !cu_seqlens || !ctx) return lfail(RSB_ERR_INVALID, "null argument");
@@ -1268,8 +1335,12 @@ extern "C" int rsb_llm_attention(rsb_llm_t* h, void* qkv, const int32_t* cu_seql
     int n_items = 0;
     rc = upload_attention_items(cu, B, d_items, st, &n_items);
     if (rc == RSB_OK)
-        attention_step(h, h->L[0], static_cast<__half*>(qkv), cu_seqlens, B, cu[B], d_items, n_items,
-                       static_cast<__half*>(ctx), st);
+        with_dtype(h, [&](auto tag) -> int {
+            using E = decltype(tag);
+            attention_step<E>(h, h->L[0], static_cast<E*>(qkv), cu_seqlens, B, cu[B], d_items, n_items,
+                              static_cast<E*>(ctx), st);
+            return RSB_OK;
+        });
     if (d_items) cudaFreeAsync(d_items, st);
     if (rc != RSB_OK) return rc;
     const cudaError_t e = cudaPeekAtLastError();
@@ -1289,7 +1360,7 @@ extern "C" int rsb_llm_layernorm(int hidden, float eps, void* x, const void* add
                      (long)LN_MAX_HIDDEN);
     if (n_rows == 0) return RSB_OK;
     auto h16 = [](const void* p) { return static_cast<const __half*>(p); };
-    ln_rows_kernel<<<n_rows, LN_THREADS, 0, (cudaStream_t)stream>>>(
+    ln_rows_kernel<__half><<<n_rows, LN_THREADS, 0, (cudaStream_t)stream>>>(
         static_cast<__half*>(x), h16(add), rows, hidden, h16(w1), h16(b1), h16(w2), h16(b2), eps,
         static_cast<__half*>(out1), static_cast<__half*>(out2));
     const cudaError_t e = cudaPeekAtLastError();
@@ -1305,7 +1376,7 @@ extern "C" int rsb_llm_olmo2_norm(int hidden, float eps, void* x, const void* a,
     if (hidden <= 0 || hidden % 8)
         return lfail(RSB_ERR_UNSUPPORTED, "hidden %ld: the RMSNorm kernel takes positive multiples of 8", (long)hidden);
     if (n_rows == 0) return RSB_OK;
-    rms_post_kernel<<<n_rows, 256, 0, (cudaStream_t)stream>>>(static_cast<__half*>(x), static_cast<const __half*>(a),
+    rms_post_kernel<__half><<<n_rows, 256, 0, (cudaStream_t)stream>>>(static_cast<__half*>(x), static_cast<const __half*>(a),
                                                               rows, hidden, static_cast<const __half*>(w), eps,
                                                               static_cast<__half*>(out));
     const cudaError_t e = cudaPeekAtLastError();

@@ -1,5 +1,5 @@
 // rsb_tc.cuh -- thin inline-PTX wrappers for the Hopper (sm_90a) tensor-core path shared by the encoder GEMM
-// (rsb_bert.cu, f16) and the coarse-quantizer GEMM (rsb_tf32.cu, tf32): mbarrier, TMA tensor loads, warpgroup
+// (rsb_bert.cu, f16 / bf16) and the coarse-quantizer GEMM (rsb_tf32.cu, tf32): mbarrier, TMA tensor loads, warpgroup
 // MMAs (wgmma.mma_async) and the K-major 128B-swizzle shared-memory descriptor.
 #ifndef RSB_TC_CUH_
 #define RSB_TC_CUH_
@@ -72,6 +72,13 @@ __device__ __forceinline__ void wgmma_f16_n128(float (&d)[64], uint64_t adesc, u
                  : RSB_WG_OUT64(d)
                  : "l"(adesc), "l"(bdesc), "r"(1));
 }
+// K = 16 bf16 elements (32 bytes of each operand row)
+__device__ __forceinline__ void wgmma_bf16_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " RSB_WG_D64 ", %64, %65, p, 1, 1, 0, 0;\n}\n"
+                 : RSB_WG_OUT64(d)
+                 : "l"(adesc), "l"(bdesc), "r"(1));
+}
 // K = 8 tf32 elements (32 bytes of each operand row)
 __device__ __forceinline__ void wgmma_tf32_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
     asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
@@ -116,16 +123,20 @@ inline EncodeTiledFn get_encode() {
     }
     return fn;
 }
-// row-major [rows, cols] matrix of 2-byte (f16) or 4-byte (f32) elements; box = one 128-byte swizzle row of columns
-// x box_rows; rows beyond `rows` read as zero
-inline bool make_map_2d(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows, int elem_bytes) {
+// row-major [rows, cols] matrix of 2-byte (f16, or bf16 with bf16 set) or 4-byte (f32) elements; box = one 128-byte
+// swizzle row of columns x box_rows; rows beyond `rows` read as zero
+inline bool make_map_2d(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows, int elem_bytes,
+                        bool bf16 = false) {
     EncodeTiledFn enc = get_encode();
     if (!enc) return false;
     const cuuint64_t dims[2] = {cols, rows};
     const cuuint64_t strides[1] = {cols * (uint64_t)elem_bytes};
     const cuuint32_t box[2] = {(cuuint32_t)(128 / elem_bytes), box_rows};
     const cuuint32_t estr[2] = {1, 1};
-    return enc(m, elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
+    const CUtensorMapDataType dt = elem_bytes == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                   : bf16         ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                                  : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+    return enc(m, dt, 2,
                const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;

@@ -270,6 +270,12 @@ def evaluate_perplexity(cfg, model=None, tokenizer=None) -> PplEvalOutput:
         raise NotImplementedError("perplexity_calibration (src/evaluate_perplexity.py:220-297) is not implemented")
     if task != "perplexity":
         raise NotImplementedError(f"inference for task_name {task!r} is not implemented (lm-eval runs in its harness)")
+    from .reader import reader_dtype
+    lm_dtype = (cfg.get("model") or {}).get("lm_dtype", None)
+    try:
+        dtype = reader_dtype("float16" if lm_dtype is None else lm_dtype)
+    except ValueError as e:
+        raise ValueError(f"model.lm_dtype: {e}") from None
     args = cfg.evaluation
     if args.get("concate_k", 0):
         s = args.get("search") or {}
@@ -286,7 +292,7 @@ def evaluate_perplexity(cfg, model=None, tokenizer=None) -> PplEvalOutput:
     tokenizer = tokenizer or load_lm_tokenizer(cfg.model.lm_model)
     if model is None:
         from .reader import load_reader
-        model = load_reader(cfg.model.lm_model)
+        model = load_reader(cfg.model.lm_model, dtype=dtype)
     pad = lm_pad_token_id(tokenizer)
     pairs = [reader_inputs(tokenizer, c, a, model.max_position_embeddings, pad) for c, a in zip(contexts, answers)]
     losses = model.loss([p[0] for p in pairs], [p[1] for p in pairs])

@@ -1,4 +1,4 @@
-"""GPU reader LM for perplexity evaluation in fp16 on librsb: HF `LlamaForCausalLM` (Llama-2 MHA, Llama-3 GQA),
+"""GPU reader LM for perplexity evaluation in fp16 (the default) or bf16 on librsb: HF `LlamaForCausalLM` (Llama-2 MHA, Llama-3 GQA),
 HF `GPTNeoXForCausalLM` (the Pythia suite, whose pythia-1b is the reference's default `model.lm_model`) and HF
 `OlmoForCausalLM` / `Olmo2ForCausalLM` (OLMo, OLMo-1.7 and OLMo-2).
 
@@ -6,6 +6,7 @@ The reference loads its reader with `AutoModelForCausalLM.from_pretrained(cfg.mo
 and calls `lm(input_ids, labels=labels)` one window at a time (`src/evaluate_perplexity.py:98-134`).  Here
 
     model = load_reader(path)                                   # local directory or HF cache, no download
+    model = load_reader(path, dtype=torch.bfloat16)             # the reference's reader dtype
     nll = model.nll([ids_0, ids_1, ...], [labels_0, ...])       # per-token NLL, many windows per forward
     losses = model.loss([ids_0, ...], [labels_0, ...])          # HF's per-window mean loss
 
@@ -231,6 +232,19 @@ def expected_keys(geom: dict) -> List[str]:
     return keys
 
 
+READER_DTYPES = {torch.float16: "float16", torch.bfloat16: "bfloat16"}
+
+
+def reader_dtype(dtype) -> torch.dtype:
+    """torch.float16 or torch.bfloat16 from either torch dtype or its name ('float16', 'bfloat16'); ValueError
+    otherwise."""
+    for t, name in READER_DTYPES.items():
+        if (isinstance(dtype, torch.dtype) and dtype == t) or (isinstance(dtype, str) and dtype == name):
+            return t
+    raise ValueError(f"reader dtype {dtype!r}: only torch.float16 / 'float16' and torch.bfloat16 / 'bfloat16' are "
+                     f"implemented")
+
+
 def scored_positions(labels: Sequence[int]) -> List[int]:
     """Positions whose label enters HF's shifted loss: every position after the first whose label is not -100."""
     return [t for t in range(1, len(labels)) if labels[t] != IGNORE]
@@ -245,7 +259,8 @@ class _Reader:
     # non-weight buffers of HF checkpoints, skipped by name before any conversion
     _buffers = ("rotary_emb.inv_freq",)
 
-    def __init__(self, config, device=None):
+    def __init__(self, config, device=None, dtype=torch.float16):
+        self.dtype = reader_dtype(dtype)
         self.geom = self._geometry(config)
         if not torch.cuda.is_available():
             raise RuntimeError(f"{type(self).__name__} needs a CUDA device (sm_90a): there is no CPU path")
@@ -256,6 +271,8 @@ class _Reader:
         self.loaded = set()
         with torch.cuda.device(self.device):
             self._check(self._create(self.geom))
+            if self.dtype == torch.bfloat16:
+                self._check(self.L.rsb_llm_set_dtype(self._h, _lib.RSB_DTYPE_BF16))
 
     def _check(self, rc):
         if rc == _lib.RSB_OK:
@@ -282,13 +299,14 @@ class _Reader:
         return self.geom["max_position_embeddings"]
 
     def load_weight(self, name: str, t: torch.Tensor) -> bool:
-        """Uploads one HF weight in fp16; False for a name the reader does not use.  A weight that does not stay
-        finite in fp16 (a bf16 value beyond 65504) is refused."""
+        """Uploads one HF weight in the reader's dtype (round to nearest even, as `from_pretrained(torch_dtype=...)`
+        converts); False for a name the reader does not use.  A weight that does not stay finite in that dtype (in
+        fp16, a bf16 value beyond 65504) is refused."""
         if name.endswith(self._buffers):
             return False
-        w = t.detach().to(device=self.device, dtype=torch.float16).contiguous()
+        w = t.detach().to(device=self.device, dtype=self.dtype).contiguous()
         if not bool(torch.isfinite(w).all()):
-            raise ValueError(f"weight {name} does not stay finite in fp16")
+            raise ValueError(f"weight {name} does not stay finite in {READER_DTYPES[self.dtype]}")
         stream = ctypes.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
         rc = self.L.rsb_llm_load(self._h, name.encode(), ctypes.c_void_p(w.data_ptr()), w.numel(), stream)
         if rc == _lib.RSB_ERR_INVALID and b"unknown weight" in self.L.rsb_llm_last_error():
@@ -340,8 +358,12 @@ class _Reader:
         self._check(rc)
         host = out.cpu()
         if not bool(torch.isfinite(host).all()):
-            raise FloatingPointError("non-finite per-token NLL: the fp16 activations overflowed (|x| > 65504); this "
-                                     "checkpoint needs a bf16 or fp32 residual stream")
+            if self.dtype == torch.float16:
+                raise FloatingPointError("non-finite per-token NLL: the fp16 activations overflowed (|x| > 65504); "
+                                         "this checkpoint needs a bf16 reader (load_reader(..., dtype=torch.bfloat16), "
+                                         "model.lm_dtype=bfloat16)")
+            raise FloatingPointError("non-finite per-token NLL: the bf16 activations overflowed (|x| > 3.39e38) or the "
+                                     "checkpoint's weights produce NaN")
         return [host[cu[i]:cu[i + 1]].clone() for i in range(len(lens))]
 
     def nll(self, input_ids_list, labels_list, max_tokens: Optional[int] = None) -> List[torch.Tensor]:
@@ -370,9 +392,12 @@ class _Reader:
     # -- diagnostics (rsb_llm_attention / rsb_llm_hidden_states), not used by nll / loss ----------------------------
     def attention(self, qkv: torch.Tensor, cu_seqlens: torch.Tensor, max_seqlen: int, ctx: torch.Tensor):
         """One attention step of the forward: RoPE in place on the Q / K heads of qkv [T, (heads + 2 kv_heads)
-        head_dim] fp16 (GPT-NeoX: [Q heads | K heads | V heads], only the first rotary_ndims of each head rotated),
-        then causal attention into ctx [T, hidden] fp16 for the windows of cu_seqlens (int32 [B + 1], empty windows
-        allowed, may end below T).  Rows outside the windows are left as they are."""
+        head_dim] in the reader's dtype (GPT-NeoX: [Q heads | K heads | V heads], only the first rotary_ndims of each
+        head rotated), then causal attention into ctx [T, hidden] of the same dtype for the windows of cu_seqlens
+        (int32 [B + 1], empty windows allowed, may end below T).  Rows outside the windows are left as they are."""
+        for what, t in (("qkv", qkv), ("ctx", ctx)):
+            if t.dtype != self.dtype:
+                raise ValueError(f"{what} is {t.dtype}; this reader runs in {self.dtype}")
         with torch.cuda.device(self.device):
             rc = self.L.rsb_llm_attention(self._h, ctypes.c_void_p(qkv.data_ptr()), ctypes.c_void_p(cu_seqlens.data_ptr()),
                                           cu_seqlens.numel() - 1, qkv.shape[0], int(max_seqlen),
@@ -381,10 +406,10 @@ class _Reader:
         self._check(rc)
 
     def hidden_states(self, ids: torch.Tensor, cu_seqlens: torch.Tensor, max_seqlen: int) -> torch.Tensor:
-        """The residual stream after the last layer, before the final norm: [T, hidden] fp16 for the packed int32 ids
-        [T] and cu_seqlens [B + 1] on the device."""
+        """The residual stream after the last layer, before the final norm: [T, hidden] in the reader's dtype for the
+        packed int32 ids [T] and cu_seqlens [B + 1] on the device."""
         T = ids.numel()
-        out = torch.empty((T, self.geom["hidden_size"]), dtype=torch.float16, device=self.device)
+        out = torch.empty((T, self.geom["hidden_size"]), dtype=self.dtype, device=self.device)
         ws = torch.empty(self.L.rsb_llm_workspace_bytes(self._h, T, 0), dtype=torch.uint8, device=self.device)
         with torch.cuda.device(self.device):
             rc = self.L.rsb_llm_hidden_states(self._h, ctypes.c_void_p(ids.data_ptr()),
@@ -485,10 +510,13 @@ def _tensors(fn: str):
         yield from torch.load(fn, weights_only=True, map_location="cpu").items()
 
 
-def load_reader(path: str, device=None):
+def load_reader(path: str, device=None, dtype=torch.float16):
     """The reader of `cfg.model.lm_model` from a local directory or the Hugging Face cache (never downloaded):
     `B200Llama` for model_type 'llama', `B200NeoX` for 'gpt_neox', `B200Olmo` for 'olmo' and 'olmo2'.  Single-file or sharded safetensors weights, or
-    PyTorch `pytorch_model.bin` files when no safetensors file is present; bf16 / fp32 weights are converted to fp16."""
+    PyTorch `pytorch_model.bin` files when no safetensors file is present, converted to `dtype`: torch.float16 (the
+    default) or torch.bfloat16 (the reference's reader dtype; also 'float16' / 'bfloat16').  Any other dtype raises
+    ValueError before any file is read."""
+    dtype = reader_dtype(dtype)
     from .encoder import _resolve_model_dir
     directory = _resolve_model_dir(path)
     with open(os.path.join(directory, "config.json")) as f:
@@ -496,7 +524,7 @@ def load_reader(path: str, device=None):
     geometry, cls = READERS.get(cfg.get("model_type"), READERS["llama"])
     geometry(cfg)                                # refuses before any weight is read or device memory allocated
     files = _shard_files(directory)
-    model = cls(cfg, device=device)
+    model = cls(cfg, device=device, dtype=dtype)
     with torch.cuda.device(model.device):
         for fn in files:
             for name, t in _tensors(fn):

@@ -179,9 +179,9 @@ def kernel_table(fn, n_windows):
     return dict(sorted(tab.items(), key=lambda kv: -kv[1])[:16])
 
 
-def bench_rsb(cfg, ids, labels, args):
+def bench_rsb(cfg, ids, labels, args, dtype="float16"):
     from retrieval_scaling_b200.reader import READERS
-    m = READERS[cfg["model_type"]][1](cfg)
+    m = READERS[cfg["model_type"]][1](cfg, dtype=dtype)
     for name, w in weights(cfg):
         m.load_weight(name, w)
         del w
@@ -243,9 +243,15 @@ def main():
     ap.add_argument("--token-budget", type=int, default=16384)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--repeats", type=int, default=5)
+    ap.add_argument("--dtype", default="float16",
+                    help="librsb reader dtypes, comma-separated: float16 (reported as 'rsb') and / or bfloat16 "
+                         "('rsb_bf16'); every run is timed against the same HF bf16 sdpa arm")
     ap.add_argument("--no-hf", action="store_true")
     ap.add_argument("--out", default=None, help="also write the result as JSON here")
     args = ap.parse_args()
+    dtypes = args.dtype.split(",")
+    if not dtypes or any(d not in ("float16", "bfloat16") for d in dtypes):
+        raise SystemExit(f"--dtype {args.dtype!r}: float16 and / or bfloat16")
     if not torch.cuda.is_available():
         raise SystemExit("bench_reader.py measures the GPU path: no CUDA device")
     smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
@@ -256,19 +262,24 @@ def main():
         ids, labels = windows(cfg, args.windows, args.context, args.answer)
         tokens = ids.numel()
         flops = model_flops(cfg, args.context, args.answer) * args.windows
-        ms, kernels, l_rsb = bench_rsb(cfg, ids, labels, args)
-        med = statistics.median(ms)
-        r = {"rsb": {"ms_runs": [round(x, 2) for x in ms], "ms_per_sample": round(med / args.windows, 3),
-                     "tokens_per_s": round(tokens / med * 1e3), "tflops": round(flops / med / 1e9, 1),
-                     "share_of_peak": round(flops / med / 1e9 / PEAK_TFLOPS, 3), "kernels_ms_per_sample": kernels,
-                     "loss_first_windows": [round(x, 4) for x in l_rsb]}}
+        r, meds = {}, {}
+        for dt in dtypes:
+            ms, kernels, l_rsb = bench_rsb(cfg, ids, labels, args, dt)
+            med = meds[dt] = statistics.median(ms)
+            r["rsb" if dt == "float16" else "rsb_bf16"] = {
+                "ms_runs": [round(x, 2) for x in ms], "ms_per_sample": round(med / args.windows, 3),
+                "tokens_per_s": round(tokens / med * 1e3), "tflops": round(flops / med / 1e9, 1),
+                "share_of_peak": round(flops / med / 1e9 / PEAK_TFLOPS, 3), "kernels_ms_per_sample": kernels,
+                "loss_first_windows": [round(x, 4) for x in l_rsb]}
         if not args.no_hf:
             ms_h, l_hf = bench_hf(cfg, ids, labels, args)
             med_h = statistics.median(ms_h)
             r["hf_bf16_sdpa"] = {"ms_runs": [round(x, 2) for x in ms_h], "ms_per_sample": round(med_h / args.windows, 3),
                                  "tokens_per_s": round(tokens / med_h * 1e3), "tflops": round(flops / med_h / 1e9, 1),
                                  "loss_first_windows": [round(x, 4) for x in l_hf]}
-            r["speedup"] = round(med_h / med, 2)
+            for dt, key in (("float16", "speedup"), ("bfloat16", "speedup_bf16")):
+                if dt in meds:
+                    r[key] = round(med_h / meds[dt], 2)
         result["models"][name] = r
         print(json.dumps({name: r}), flush=True)
     if args.out:
