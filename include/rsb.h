@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define RSB_VERSION 300 /* 0.3.0 */
+#define RSB_VERSION 301 /* 0.3.1 */
 
 enum {
     RSB_OK = 0,
@@ -256,7 +256,7 @@ int rsb_coarse(rsb_index_t* h, const float* q_dev, int nq, int nprobe, int64_t* 
  * Every argument is checked before any launch.  The workspace queries return 0 for arguments the call would refuse;
  * they size the all-device store by nq, k_base and k alone, and the tiered store by its dtype and staging_bytes. */
 /* RSB_DTYPE_SQ8: a re-rank store, or the storage of an IVFFLAT index (rsb_ivfflat_create); not a Flat index */
-/* RSB_DTYPE_BF16: readers only (rsb_llm_set_dtype); every index and re-rank store creator refuses it (RSB_ERR_INVALID) */
+/* RSB_DTYPE_BF16: readers only (rsb_llm_create); every index and re-rank store creator refuses it (RSB_ERR_INVALID) */
 enum { RSB_DTYPE_F32 = 0, RSB_DTYPE_F16 = 1, RSB_DTYPE_SQ8 = 2, RSB_DTYPE_BF16 = 3 };
 int rsb_host_alloc(size_t bytes, void** out);   /* cudaHostAlloc(portable | mapped): exactly `bytes`, unlike torch's
                                                    pinned allocator, which rounds blocks up to a power of two */
@@ -456,76 +456,64 @@ enum { RSB_GEMM_REVERSED = 256 };
 int rsb_gemm_f16(const void* A_dev, const void* W_dev, const void* bias_dev, const void* residual_dev, void* C_dev,
                  int M, int N, int K, int epilogue, rsb_stream_t stream);
 
-/* ---- reader LM for perplexity evaluation: HF LlamaForCausalLM, prefill only, fp16 or bf16 --------------------------
+/* ---- reader LM for perplexity evaluation: HF causal LMs, prefill only, fp16 or bf16 ---------------------------------
  * Replaces the reader of the reference's perplexity loop (src/evaluate_perplexity.py:98-108 loads it, :126-134 runs
  * `lm(input_ids, labels=labels)` one window at a time).  Errors of these entries are reported by rsb_llm_last_error().
- * rsb_llm_create: head_dim 128 (hidden == 128 * heads), heads % kv_heads == 0, intermediate % 128 == 0, SiLU MLP, no
- * biases, default RoPE (inv_freq = 1 / rope_theta ** (2i / 128) in fp32); anything else RSB_ERR_UNSUPPORTED, non-positive
- * sizes RSB_ERR_INVALID, both before any CUDA call.  Any vocabulary size: the LM head is padded to a multiple of 128
- * rows that never enter the log-sum-exp.  tied = 1 (tie_word_embeddings): the LM head is model.embed_tokens.weight. */
-typedef struct rsb_llm rsb_llm_t;
-const char* rsb_llm_last_error(void);
-int rsb_llm_create(int layers, int hidden, int heads, int kv_heads, int intermediate, int vocab, int max_pos,
-                   float rope_theta, float rms_eps, int tied, rsb_llm_t** out);
-/* GPT-NeoX readers (HF GPTNeoXForCausalLM: Pythia), a second constructor for the same handle type: heads = kv heads,
- * head_dim = hidden / heads in {64, 80, 128, 256} (else RSB_ERR_UNSUPPORTED naming head_dim), hidden <= 8192 (the
- * LayerNorm kernel's widest row, else RSB_ERR_UNSUPPORTED naming hidden; Pythia-12B has 5120), rotary_dims = HF's
- * rotary_ndims, even and in [2, head_dim] (rotary_dims <= 0 or > head_dim RSB_ERR_INVALID, odd RSB_ERR_UNSUPPORTED),
- * inv_freq = 1 / rotary_base ** (2i / rotary_dims) in fp32, intermediate % 128 == 0 (else RSB_ERR_UNSUPPORTED),
- * non-positive sizes RSB_ERR_INVALID; all before any CUDA call.  The forward is HF's in fp16: LayerNorm (fp32 mean and
- * biased variance, one rounding) with bias, query_key_value with bias, partial rotary on dims [0, rotary_dims) of each
- * Q / K head, causal attention scaled by head_dim^-0.5, dense with bias, dense_h_to_4h -> GELU -> dense_4h_to_h with
- * biases, the parallel residual x = fp16(fp16(mlp(ln2(x)) + attn(ln1(x))) + x), final_layer_norm and an untied,
- * bias-free embed_out over any vocabulary size.  rsb_llm_load, _workspace_bytes, _nll, _hidden_states, _attention and
- * _free take both kinds of handle; on a GPT-NeoX handle
- *   rsb_llm_load takes "gpt_neox.embed_in.weight", "embed_out.weight", "gpt_neox.final_layer_norm.{weight,bias}" and
- *     "gpt_neox.layers.N.{input_layernorm, post_attention_layernorm, attention.query_key_value, attention.dense,
- *     mlp.dense_h_to_4h, mlp.dense_4h_to_h}.{weight,bias}".  query_key_value's per-head interleaved rows
- *     (q_h | k_h | v_h for each head h) are stored as [Q heads | K heads | V heads];
- *   rsb_llm_hidden_states returns the residual stream before final_layer_norm;
- *   rsb_llm_attention takes qkv rows in that permuted [Q heads | K heads | V heads] layout, [T, 3 hidden], rotates the
- *     first rotary_dims of each Q / K head (the other dims are left bit-identical) and scales by head_dim^-0.5. */
-int rsb_llm_create_neox(int layers, int hidden, int heads, int intermediate, int vocab, int max_pos, int rotary_dims,
-                        float rotary_base, float ln_eps, rsb_llm_t** out);
-/* OLMo readers, a third constructor for the same handle type: version 1 = HF OlmoForCausalLM (OLMo-1B/7B-hf, OLMo-1.7),
- * version 2 = Olmo2ForCausalLM (OLMo-2).  The geometry rules of rsb_llm_create apply (head_dim 128 with hidden == 128 *
- * heads, heads % kv_heads == 0, intermediate % 128 == 0: else RSB_ERR_UNSUPPORTED; non-positive sizes, rope_theta or eps
- * RSB_ERR_INVALID), and also: version other than 1 or 2 RSB_ERR_INVALID; clip_qkv negative, infinite or NaN, or non-zero
- * with version 2, RSB_ERR_INVALID; version 1 with hidden > 8192 (the LayerNorm kernel's widest row) RSB_ERR_UNSUPPORTED.
- * All before any CUDA call.  The forward is HF's in fp16, a Llama layer (SwiGLU, no biases, default RoPE with
- * inv_freq = 1 / rope_theta ** (2i / 128) in fp32, causal GQA attention scaled by 128^-0.5) except:
- *   RoPE keeps cos / sin in fp32: x * cos + rotate_half(x) * sin is evaluated in fp32 and rounded to half once;
- *   version 1: both pre-norms and the final norm are OlmoLayerNorm, without weight or bias: fp16 of the fp32
- *     (x - mean) * rsqrt(biased var + eps), one rounding; eps is 1e-5 in HF (no config field).  clip_qkv > 0 clamps every
- *     q, k and v projection element to [-clip_qkv, clip_qkv] before RoPE; 0 = none (HF clip_qkv null);
- *   version 2: no pre-norms.  x = fp16(x + post_attention_layernorm(o_proj(attn(x)))), then x = fp16(x +
- *     post_feedforward_layernorm(mlp(x))).  Every norm is Olmo2RMSNorm, fp16(w * (x * rsqrt(mean(x^2) + eps))) with the
- *     weight multiply in fp32 and one rounding; q_norm normalises the whole q projection (hidden wide) and k_norm the
- *     whole k projection (kv_heads * 128 wide), before RoPE; the final model.norm is one too.  eps = rms_norm_eps.
- * tied = 1 (tie_word_embeddings): the LM head is model.embed_tokens.weight.  rsb_llm_load, _workspace_bytes, _nll,
- * _hidden_states, _attention and _free take OLMo handles; on them
- *   rsb_llm_load takes "model.embed_tokens.weight", "lm_head.weight" (untied; accepted and ignored when tied) and
- *     "model.layers.N.{self_attn.{q,k,v,o}_proj, mlp.{gate,up,down}_proj}.weight"; version 2 also "model.norm.weight" and
- *     "model.layers.N.{self_attn.q_norm, self_attn.k_norm, post_attention_layernorm, post_feedforward_layernorm}.weight".
- *     Version 1 has no norm weights: a norm name is an unknown weight (RSB_ERR_INVALID);
- *   rsb_llm_hidden_states returns the residual stream before the final norm;
- *   rsb_llm_attention runs layer 0's prologue in place of RoPE: the clip_qkv clamp of q, k and v (version 1), or q_norm /
- *     k_norm (version 2; RSB_ERR_STATE until layer 0's q_norm and k_norm are loaded), then the fp32-cos / sin RoPE. */
-int rsb_llm_create_olmo(int version, int layers, int hidden, int heads, int kv_heads, int intermediate, int vocab,
-                        int max_pos, float rope_theta, float eps, float clip_qkv, int tied, rsb_llm_t** out);
-/* The element type of a handle's weights and activations, for every constructor: RSB_DTYPE_F16 (the default) or
- * RSB_DTYPE_BF16, the reference's reader dtype; any other value RSB_ERR_INVALID, and RSB_ERR_STATE once rsb_llm_load has
- * been called.  In bf16 the forward is HF's bf16 forward: every point where the fp16 forward rounds to fp16 (each GEMM
+ * rsb_llm_create makes a reader of one family.  Every refusal below comes before any CUDA call, and the error names the
+ * field.  For every family: family not one of RSB_LLM_*, or dtype neither RSB_DTYPE_F16 nor RSB_DTYPE_BF16,
+ * RSB_ERR_INVALID; non-positive layers, vocab, max_pos, rope_theta or eps, or tied not 0 / 1, RSB_ERR_INVALID; clip_qkv
+ * negative, infinite or NaN, or non-zero for any family but RSB_LLM_OLMO, RSB_ERR_INVALID; intermediate % 128 != 0
+ * RSB_ERR_UNSUPPORTED.  Any vocabulary size: the LM head is padded to a multiple of 128 rows that never enter the
+ * log-sum-exp.  tied = 1 (tie_word_embeddings): the LM head is the embedding; an untied "lm_head.weight" is accepted
+ * and ignored.  inv_freq = 1 / rope_theta ** (2i / rotary_dims) in fp32.
+ *   RSB_LLM_LLAMA, HF LlamaForCausalLM: head_dim 128 (hidden == 128 * heads), heads % kv_heads == 0 (else
+ *     RSB_ERR_UNSUPPORTED), rotary_dims = 128 (else RSB_ERR_INVALID), eps = rms_norm_eps.  SiLU MLP, no biases,
+ *     LlamaRMSNorm, default RoPE.  Weights: "model.embed_tokens.weight", "model.norm.weight", "lm_head.weight" and
+ *     "model.layers.N.{self_attn.{q,k,v,o}_proj, mlp.{gate,up,down}_proj, input_layernorm,
+ *     post_attention_layernorm}.weight".
+ *   RSB_LLM_NEOX, HF GPTNeoXForCausalLM (Pythia): kv_heads == heads and tied = 0 (else RSB_ERR_UNSUPPORTED); hidden,
+ *     heads and intermediate positive (else RSB_ERR_INVALID); head_dim = hidden / heads in {64, 80, 128, 256} (else
+ *     RSB_ERR_UNSUPPORTED naming head_dim); hidden <= 8192 (the LayerNorm kernel's widest row, else RSB_ERR_UNSUPPORTED
+ *     naming hidden; Pythia-12B has 5120); rotary_dims = HF's rotary_ndims, even and in [2, head_dim] (rotary_dims <= 0
+ *     or > head_dim RSB_ERR_INVALID, odd RSB_ERR_UNSUPPORTED); rope_theta = rotary_emb_base, eps = layer_norm_eps.
+ *     The forward is HF's: LayerNorm (fp32 mean and biased variance, one rounding) with bias, query_key_value with
+ *     bias, partial rotary on dims [0, rotary_dims) of each Q / K head, causal attention scaled by head_dim^-0.5, dense
+ *     with bias, dense_h_to_4h -> GELU -> dense_4h_to_h with biases, the parallel residual x = fp16(fp16(mlp(ln2(x)) +
+ *     attn(ln1(x))) + x), final_layer_norm and a bias-free embed_out.  Weights: "gpt_neox.embed_in.weight",
+ *     "embed_out.weight", "gpt_neox.final_layer_norm.{weight,bias}" and "gpt_neox.layers.N.{input_layernorm,
+ *     post_attention_layernorm, attention.query_key_value, attention.dense, mlp.dense_h_to_4h,
+ *     mlp.dense_4h_to_h}.{weight,bias}".  query_key_value's per-head interleaved rows (q_h | k_h | v_h for each head h)
+ *     are stored as [Q heads | K heads | V heads].
+ *   RSB_LLM_OLMO (HF OlmoForCausalLM: OLMo-1B/7B-hf, OLMo-1.7) and RSB_LLM_OLMO2 (Olmo2ForCausalLM): the Llama rules
+ *     (head_dim 128, heads % kv_heads == 0, rotary_dims = 128), and OLMo with hidden > 8192 (the LayerNorm kernel's
+ *     widest row) RSB_ERR_UNSUPPORTED.  The forward is a Llama layer (SwiGLU, no biases, causal GQA attention scaled by
+ *     128^-0.5) except:
+ *     RoPE keeps cos / sin in fp32: x * cos + rotate_half(x) * sin is evaluated in fp32 and rounded to half once;
+ *     OLMo: both pre-norms and the final norm are OlmoLayerNorm, without weight or bias: fp16 of the fp32 (x - mean) *
+ *       rsqrt(biased var + eps), one rounding; eps is 1e-5 in HF (no config field).  clip_qkv > 0 clamps every q, k and
+ *       v projection element to [-clip_qkv, clip_qkv] before RoPE; 0 = none (HF clip_qkv null);
+ *     OLMo-2: no pre-norms.  x = fp16(x + post_attention_layernorm(o_proj(attn(x)))), then x = fp16(x +
+ *       post_feedforward_layernorm(mlp(x))).  Every norm is Olmo2RMSNorm, fp16(w * (x * rsqrt(mean(x^2) + eps))) with the
+ *       weight multiply in fp32 and one rounding; q_norm normalises the whole q projection (hidden wide) and k_norm the
+ *       whole k projection (kv_heads * 128 wide), before RoPE; the final model.norm is one too.  eps = rms_norm_eps.
+ *     Weights: "model.embed_tokens.weight", "lm_head.weight" and "model.layers.N.{self_attn.{q,k,v,o}_proj,
+ *     mlp.{gate,up,down}_proj}.weight"; OLMo-2 also "model.norm.weight" and "model.layers.N.{self_attn.q_norm,
+ *     self_attn.k_norm, post_attention_layernorm, post_feedforward_layernorm}.weight".  OLMo has no norm weights: a
+ *     norm name is an unknown weight (RSB_ERR_INVALID).
+ * dtype is the element type of the handle's weights and activations: RSB_DTYPE_F16, or RSB_DTYPE_BF16, the reference's
+ * reader dtype.  In bf16 the forward is HF's bf16 forward: every point where the fp16 forward rounds to fp16 (each GEMM
  * output, norm output, RoPE product and sum, attention's P before P V, SwiGLU / GELU output, residual add, the logits)
  * rounds to bf16 instead, with the same fp32 arithmetic in between; OLMo's fp32 cos / sin RoPE rounds once, to bf16, and
  * clip_qkv acts as the bf16 clamp (the clamped value is the bound rounded to bf16).  The NLL is the fp32 log-sum-exp of
  * the bf16 logits, as transformers' logits.float() after a bf16 lm_head.  rsb_llm_load, rsb_llm_attention and
- * rsb_llm_hidden_states then take and return bf16. */
-int rsb_llm_set_dtype(rsb_llm_t* h, int dtype);
-/* name = HF LlamaForCausalLM state_dict key: "model.embed_tokens.weight", "model.norm.weight", "lm_head.weight"
- * (untied; accepted and ignored when tied) and "model.layers.N.{self_attn.{q,k,v,o}_proj, mlp.{gate,up,down}_proj,
- * input_layernorm, post_attention_layernorm}.weight"; data on the device in the handle's dtype (fp16 unless
- * rsb_llm_set_dtype chose bf16), copied. */
+ * rsb_llm_hidden_states take and return the handle's dtype. */
+typedef struct rsb_llm rsb_llm_t;
+enum { RSB_LLM_LLAMA = 0, RSB_LLM_NEOX = 1, RSB_LLM_OLMO = 2, RSB_LLM_OLMO2 = 3 };
+const char* rsb_llm_last_error(void);
+int rsb_llm_create(int family, int dtype, int layers, int hidden, int heads, int kv_heads, int intermediate, int vocab,
+                   int max_pos, int rotary_dims, float rope_theta, float eps, float clip_qkv, int tied, rsb_llm_t** out);
+/* name = an HF state-dict key of the handle's family (above), data on the device in the handle's dtype, copied; any
+ * other name RSB_ERR_INVALID ("unknown weight name"). */
 int rsb_llm_load(rsb_llm_t* h, const char* name, const void* f16_dev, int64_t n_elements, rsb_stream_t stream);
 size_t rsb_llm_workspace_bytes(rsb_llm_t* h, int total_tokens, int label_tokens);
 /* B packed sequences: ids_dev / labels_dev [T] int32 (label -100 = ignored), cu_seqlens_dev [B+1] int32 (0 .. T), every
@@ -538,13 +526,16 @@ int rsb_llm_nll(rsb_llm_t* h, const int32_t* ids_dev, const int32_t* cu_seqlens_
                 const int32_t* labels_dev, float* nll_out_dev, void* ws_dev, size_t ws_bytes, rsb_stream_t stream);
 int rsb_llm_free(rsb_llm_t* h);
 /* Diagnostic, not used on the product path: one attention step of rsb_llm_nll on a caller's tensors, with the forward's
- * own work list.  qkv_dev [T, (heads + 2 kv_heads) 128] in the handle's dtype (fp16 or bf16) holds each token's Q | K |
- * V heads; RoPE is applied to its Q and K heads in place (positions restart at 0 in every window), then ctx_dev
- * [T, heads 128] in the same dtype receives causal
- * softmax(q k^T / sqrt(128)) v per window and query head h, which reads KV head h / (heads / kv_heads).  Windows may be
- * empty and cu_seqlens_dev [B+1] may end below T: rows of empty windows and rows at or past cu_seqlens[B] are neither
- * rotated nor written.  The offset refusals of rsb_llm_nll apply (RSB_ERR_INVALID / RSB_ERR_UNSUPPORTED before any
- * launch); no weight needs to be loaded. */
+ * own work list.  qkv_dev [T, (heads + 2 kv_heads) head_dim] in the handle's dtype (fp16 or bf16) holds each token's
+ * Q | K | V heads (GPT-NeoX: the permuted [Q heads | K heads | V heads] layout rsb_llm_load stores); RoPE is applied to
+ * its Q and K heads in place (positions restart at 0 in every window; GPT-NeoX rotates the first rotary_dims of each
+ * head and leaves the other dims bit-identical), then ctx_dev [T, heads head_dim] in the same dtype receives causal
+ * softmax(q k^T / sqrt(head_dim)) v per window and query head h, which reads KV head h / (heads / kv_heads).  OLMo and
+ * OLMo-2 run layer 0's prologue in place of RoPE: the clip_qkv clamp of q, k and v (OLMo), or q_norm / k_norm (OLMo-2;
+ * RSB_ERR_STATE until layer 0's q_norm and k_norm are loaded), then the fp32-cos / sin RoPE.  Windows may be empty and
+ * cu_seqlens_dev [B+1] may end below T: rows of empty windows and rows at or past cu_seqlens[B] are neither rotated nor
+ * written.  The offset refusals of rsb_llm_nll apply (RSB_ERR_INVALID / RSB_ERR_UNSUPPORTED before any launch); no
+ * other weight needs to be loaded. */
 int rsb_llm_attention(rsb_llm_t* h, void* qkv_dev, const int32_t* cu_seqlens_dev, int B, int T, int max_seqlen,
                       void* ctx_dev, rsb_stream_t stream);
 /* Diagnostic, not used on the product path: the residual stream after the last decoder layer of rsb_llm_nll's forward,
@@ -558,7 +549,7 @@ int rsb_llm_hidden_states(rsb_llm_t* h, const int32_t* ids_dev, const int32_t* c
  *   w1_dev != NULL: out1[i] = fp16((x[r] - mean) * rsqrt(var + eps) * w1 + b1), mean and biased variance in fp32, one
  *   rounding (torch's fp16 LayerNorm); w2_dev != NULL (only with w1_dev): out2[i] likewise with w2 / b2, from the same
  *   statistics.  Neither: only the add.
- * hidden must be a multiple of 8 and at most 8192 (RSB_ERR_UNSUPPORTED, also the largest hidden rsb_llm_create_neox
+ * hidden must be a multiple of 8 and at most 8192 (RSB_ERR_UNSUPPORTED, also the largest GPT-NeoX hidden rsb_llm_create
  * accepts); a missing bias or output RSB_ERR_INVALID; both before any launch.  No handle is needed. */
 int rsb_llm_layernorm(int hidden, float eps, void* x_dev, const void* add_dev, const int32_t* rows_dev, int n_rows,
                       const void* w1_dev, const void* b1_dev, const void* w2_dev, const void* b2_dev, void* out1_dev,

@@ -14,6 +14,7 @@ RSB_OK = 0
 RSB_ERR_INVALID, RSB_ERR_CUDA, RSB_ERR_STATE, RSB_ERR_UNSUPPORTED, RSB_ERR_OOM = -1, -2, -3, -4, -5
 RSB_FLAT, RSB_IVFFLAT, RSB_IVFPQ = 0, 1, 2
 RSB_DTYPE_F32, RSB_DTYPE_F16, RSB_DTYPE_SQ8, RSB_DTYPE_BF16 = 0, 1, 2, 3   # BF16: readers only
+RSB_LLM_LLAMA, RSB_LLM_NEOX, RSB_LLM_OLMO, RSB_LLM_OLMO2 = 0, 1, 2, 3          # rsb_llm_create's reader families
 (INFO_KIND, INFO_D, INFO_NLIST, INFO_M, INFO_NBITS, INFO_NTOTAL, INFO_IS_TRAINED, INFO_MAX_LIST_LEN,
  INFO_INDEX_BYTES, INFO_DTYPE, INFO_BY_RESIDUAL, INFO_HOST_BYTES, INFO_DEVICE_ROWS) = range(13)
 OPT_COARSE_TENSOR, OPT_BY_RESIDUAL, OPT_DEVICE_ROWS, OPT_STAGING_BYTES = 0, 1, 2, 3
@@ -91,8 +92,8 @@ SIGNATURES = [
     ("rsb_bert_attention", c_int, [_H, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),   # diagnostic
     ("rsb_gemm_f16", c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     ("rsb_llm_last_error", c_char_p, []),
-    ("rsb_llm_create", c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_int, POINTER(_H)]),
-    ("rsb_llm_create_neox", c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_float, POINTER(_H)]),
+    ("rsb_llm_create", c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_float,
+                               c_float, c_int, POINTER(_H)]),
     ("rsb_llm_load", c_int, [_H, c_char_p, c_void_p, c_int64, c_void_p]),
     ("rsb_llm_workspace_bytes", c_size_t, [_H, c_int, c_int]),
     ("rsb_llm_nll", c_int, [_H, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
@@ -102,9 +103,6 @@ SIGNATURES = [
                                       c_void_p]),                                                   # diagnostic
     ("rsb_llm_layernorm", c_int, [c_int, c_float, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
                                   c_void_p, c_void_p, c_void_p, c_void_p]),                          # diagnostic
-    ("rsb_llm_create_olmo", c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_float,
-                                    c_int, POINTER(_H)]),
-    ("rsb_llm_set_dtype", c_int, [_H, c_int]),
     ("rsb_llm_olmo2_norm", c_int, [c_int, c_float, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
                                    c_void_p]),                                                       # diagnostic
     ("rsb_dedup_last_error", c_char_p, []),

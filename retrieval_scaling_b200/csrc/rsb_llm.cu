@@ -1,22 +1,19 @@
 // rsb_llm.cu -- reader-LM forward for perplexity evaluation: HF LlamaForCausalLM (Llama-2 MHA, Llama-3 GQA),
-// GPTNeoXForCausalLM (Pythia; rsb_llm_create_neox) and OlmoForCausalLM / Olmo2ForCausalLM (rsb_llm_create_olmo) in
-// fp16 or bf16 (rsb_llm_set_dtype; every kernel is a template on its element type and rounds to it where HF's forward
-// in that dtype rounds), prefill only, over packed un-padded sequences, ending in the per-token negative
-// log-likelihood of the labels.
+// GPTNeoXForCausalLM (Pythia) and OlmoForCausalLM / Olmo2ForCausalLM, chosen by rsb_llm_create's family, in fp16 or
+// bf16 (every kernel is a template on its element type and rounds to it where HF's forward in that dtype rounds),
+// prefill only, over packed un-padded sequences, ending in the per-token negative log-likelihood of the labels.
 // Replaces the reader call of the reference's perplexity loop (src/evaluate_perplexity.py:126-134: `lm(input_ids,
 // labels=labels)` one window at a time, HF in bf16).  No KV cache, no generation.
 //
 //   embed_rows_kernel        X[t] = embed_tokens[ids[t]]
-//   rms_rows_kernel          LlamaRMSNorm in HF's order: fp32 x * rsqrt(mean(x^2) + eps), rounded to half, times the half
-//                            weight; the final norm runs on the gathered label rows only
+//   rms_rows_kernel          LlamaRMSNorm (the weight multiply in half) or Olmo2RMSNorm (in fp32), optionally fused with
+//                            OLMo-2's post-norm residual add; the final norm runs on the gathered label rows only
 //   rsb_gemm_f16             every linear layer on the encoder's TMA + wgmma kernel (gemm_tn_kernel, rsb_bert.cu): fused
 //                            q|k|v and gate|up weights, residual adds through its residual epilogue with a zero bias
-//   rope_kernel              HF rotate_half RoPE on the Q and K heads of the fused QKV rows; positions restart at 0 in
-//                            every packed sequence
+//   rope_kernel              HF rotate_half RoPE on the first rotary_dims of each Q and K head of the fused QKV rows (all
+//                            128 for Llama); positions restart at 0 in every packed sequence
 //   ln_rows_kernel           GPT-NeoX: torch's fp16 LayerNorm, with the parallel residual's last add and both norms fused
-//   rope_partial_kernel      GPT-NeoX: rotate_half on the first rotary_dims of each Q / K head
 //   olmo_qkv_kernel          OLMo / OLMo-2: clip_qkv clamp or whole-projection QK RMSNorm, then RoPE with fp32 cos / sin
-//   rms_post_kernel          OLMo-2: Olmo2RMSNorm (weight multiply in fp32) fused with the post-norm residual add
 //   attention_causal_kernel  causal flash attention, head_dim 64 / 80 / 128 / 256, GQA, mma.sync.m16n8k16 with fp32 running max / sum;
 //                            key blocks above the diagonal are never visited
 //   swiglu_kernel            act = fp16(fp16(silu(gate)) * up), HF LlamaMLP's order
@@ -31,6 +28,7 @@
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
+#include <map>
 #include <set>
 #include <string>
 #include <type_traits>
@@ -65,19 +63,23 @@ __global__ void embed_rows_kernel(const int* __restrict__ ids, const T* __restri
     for (int i = threadIdx.x; i < hidden / 8; i += blockDim.x) dst[i] = src[i];
 }
 
-// LlamaRMSNorm (modeling_llama.py): h = x.float(); h *= rsqrt(mean(h^2) + eps); weight * h.half().  One block per
-// output row i, input row rows ? rows[i] : i.
-template <typename T>
+// RMSNorm with fp32 statistics, rstd = rsqrt(mean(v^2) + eps), in one of HF's two rounding orders.  One block per
+// output row i, input row r = rows ? rows[i] : i.
+//   OLMO2 = false, LlamaRMSNorm (modeling_llama.py): weight * fp16(v * rstd), the weight multiply in half.
+//   OLMO2 = true, Olmo2RMSNorm: fp16(w * (v * rstd)), the weight multiply in fp32 and one rounding.
+//   A != nullptr: X[r] = fp16(X[r] + norm(A[r])), OLMo-2's post-norm residual add, in place; out is not written.
+//   A == nullptr: out[i] = norm(X[r]).
+template <typename T, bool OLMO2>
 __global__ __launch_bounds__(256)
-void rms_rows_kernel(const T* __restrict__ in, const int* __restrict__ rows, int hidden,
+void rms_rows_kernel(T* __restrict__ X, const T* __restrict__ A, const int* __restrict__ rows, int hidden,
                      const T* __restrict__ w, float eps, T* __restrict__ out) {
     __shared__ float red[8];
     const int i = blockIdx.x;
     const int r = rows ? rows[i] : i;
-    const uint4* x = reinterpret_cast<const uint4*>(in + (size_t)r * hidden);
+    const uint4* a = reinterpret_cast<const uint4*>((A ? A : X) + (size_t)r * hidden);
     float s = 0.f;
     for (int c = threadIdx.x; c < hidden / 8; c += blockDim.x) {
-        const uint4 v = x[c];
+        const uint4 v = a[c];
         const pair_t<T>* h2 = reinterpret_cast<const pair_t<T>*>(&v);
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
@@ -88,67 +90,64 @@ void rms_rows_kernel(const T* __restrict__ in, const int* __restrict__ rows, int
     }
     const float rstd = rsqrtf(block_sum(s, red) / (float)hidden + eps);
     const uint4* wv = reinterpret_cast<const uint4*>(w);
+    uint4* x = reinterpret_cast<uint4*>(X + (size_t)r * hidden);
     uint4* o = reinterpret_cast<uint4*>(out + (size_t)i * hidden);
     for (int c = threadIdx.x; c < hidden / 8; c += blockDim.x) {
-        const uint4 v = x[c], g = wv[c];
+        const uint4 v = a[c], g = wv[c];
         const pair_t<T>* h2 = reinterpret_cast<const pair_t<T>*>(&v);
         const pair_t<T>* g2 = reinterpret_cast<const pair_t<T>*>(&g);
-        uint4 ov;
-        pair_t<T>* o2 = reinterpret_cast<pair_t<T>*>(&ov);
+        uint4 nv;
+        pair_t<T>* n2 = reinterpret_cast<pair_t<T>*>(&nv);
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
             const float2 f = to_f2(h2[e]);
-            o2[e] = __hmul2(g2[e], from_f2<T>(f.x * rstd, f.y * rstd));
+            if constexpr (OLMO2) {
+                const float2 gf = to_f2(g2[e]);
+                n2[e] = from_f2<T>(__fmul_rn(gf.x, __fmul_rn(f.x, rstd)), __fmul_rn(gf.y, __fmul_rn(f.y, rstd)));
+            } else {
+                n2[e] = __hmul2(g2[e], from_f2<T>(f.x * rstd, f.y * rstd));
+            }
         }
-        o[c] = ov;
+        if (A) {
+            uint4 xv = x[c];
+            pair_t<T>* x2 = reinterpret_cast<pair_t<T>*>(&xv);
+#pragma unroll
+            for (int e = 0; e < 4; ++e) x2[e] = __hadd2(x2[e], n2[e]);
+            x[c] = xv;
+        } else {
+            o[c] = nv;
+        }
     }
 }
 
-// HF apply_rotary_pos_emb on the Q heads and K heads (contiguous at the start of each QKV row, ld halves apart):
-// x_embed = x * cos + rotate_half(x) * sin in fp16, cos / sin = fp16(cos / sin(fp32(inv_freq[i] * pos))).  Each fp16
-// product and sum is one fp32 operation rounded to half, as torch computes half tensors.  One block per token.
-template <typename T>
-__global__ void rope_kernel(T* __restrict__ qkv, const int* __restrict__ cu_seqlens, int B, int ld, int rot_heads,
-                            const float* __restrict__ inv_freq) {
-    const int t = blockIdx.x;
-    int lo = 0, hi = B;                          // sequence b with cu[b] <= t < cu[b+1]
-    while (hi - lo > 1) {
-        const int mid = (lo + hi) >> 1;
-        if (cu_seqlens[mid] <= t) lo = mid; else hi = mid;
-    }
-    const float pos = (float)(t - cu_seqlens[lo]);
-    T* row = qkv + (size_t)t * ld;
-    for (int p = threadIdx.x; p < rot_heads * (HD / 2); p += blockDim.x) {
-        const int i = p % (HD / 2);
-        T* x = row + (p / (HD / 2)) * HD;
-        const float f = inv_freq[i] * pos;
-        const float c = to_f(from_f<T>(cosf(f))), s = to_f(from_f<T>(sinf(f)));
-        const float x1 = to_f(x[i]), x2 = to_f(x[i + HD / 2]);
-        const float a1 = to_f(from_f<T>(x1 * c)), b1 = to_f(from_f<T>(-x2 * s));
-        const float a2 = to_f(from_f<T>(x2 * c)), b2 = to_f(from_f<T>(x1 * s));
-        x[i] = from_f<T>(a1 + b1);
-        x[i + HD / 2] = from_f<T>(a2 + b2);
-    }
-}
-
-// GPT-NeoX partial rotary (modeling_gpt_neox.py apply_rotary_pos_emb): rotate_half on dims [0, rot) of every Q and K
-// head (head_dim hd apart, Q heads then K heads at the start of each QKV row), in rope_kernel's fp16 order; dims
-// [rot, hd) are neither read nor written.  One block per token.
-template <typename T>
-__global__ void rope_partial_kernel(T* __restrict__ qkv, const int* __restrict__ cu_seqlens, int B, int ld,
-                                    int rot_heads, int hd, int rot, const float* __restrict__ inv_freq) {
-    const int t = blockIdx.x;
+// Position of token t in its packed sequence: t - cu[b] for the sequence b with cu[b] <= t < cu[b+1].
+__device__ __forceinline__ int seq_position(const int* __restrict__ cu_seqlens, int B, int t) {
     int lo = 0, hi = B;
     while (hi - lo > 1) {
         const int mid = (lo + hi) >> 1;
         if (cu_seqlens[mid] <= t) lo = mid; else hi = mid;
     }
-    const float pos = (float)(t - cu_seqlens[lo]);
+    return t - cu_seqlens[lo];
+}
+
+// HF apply_rotary_pos_emb (modeling_llama.py, modeling_gpt_neox.py): rotate_half on dims [0, rot) of every Q and K
+// head (head_dim hd apart, Q heads then K heads at the start of each QKV row, ld halves apart); dims [rot, hd) are
+// neither read nor written (GPT-NeoX partial rotary; Llama has rot = hd = 128).  x_embed = x * cos + rotate_half(x) *
+// sin in fp16, cos / sin = fp16(cos / sin(fp32(inv_freq[i] * pos))).  Each fp16 product and sum is one fp32 operation
+// rounded to half, as torch computes half tensors.  One block per token.
+template <typename T>
+__global__ void rope_kernel(T* __restrict__ qkv, const int* __restrict__ cu_seqlens, int B, int ld, int rot_heads,
+                            int hd, int rot, const float* __restrict__ inv_freq) {
+    const int t = blockIdx.x;
+    const float pos = (float)seq_position(cu_seqlens, B, t);
     const int half_rot = rot >> 1;
     T* row = qkv + (size_t)t * ld;
-    for (int p = threadIdx.x; p < rot_heads * half_rot; p += blockDim.x) {
-        const int i = p % half_rot;
-        T* x = row + (p / half_rot) * hd;
+    // pair p = head hh, dim i: advanced by blockDim.x pairs per step without a division in the loop
+    const int dh = blockDim.x / half_rot, di = blockDim.x % half_rot;
+    int hh = threadIdx.x / half_rot, i = threadIdx.x % half_rot;
+    for (int p = threadIdx.x; p < rot_heads * half_rot; p += blockDim.x, hh += dh, i += di) {
+        if (i >= half_rot) { i -= half_rot; ++hh; }
+        T* x = row + hh * hd;
         const float f = inv_freq[i] * pos;
         const float c = to_f(from_f<T>(cosf(f))), s = to_f(from_f<T>(sinf(f)));
         const float x1 = to_f(x[i]), x2 = to_f(x[i + half_rot]);
@@ -257,12 +256,7 @@ void olmo_qkv_kernel(T* __restrict__ qkv, const int* __restrict__ cu_seqlens, in
                      const T* __restrict__ kn, float eps) {
     __shared__ float red[8];
     const int t = blockIdx.x;
-    int lo = 0, hi = B;
-    while (hi - lo > 1) {
-        const int mid = (lo + hi) >> 1;
-        if (cu_seqlens[mid] <= t) lo = mid; else hi = mid;
-    }
-    const float pos = (float)(t - cu_seqlens[lo]);
+    const float pos = (float)seq_position(cu_seqlens, B, t);
     const int nq = heads * HD, nk = kv_heads * HD;
     T* row = qkv + (size_t)t * (nq + 2 * nk);
     float rq = 1.f, rk = 1.f;
@@ -304,56 +298,6 @@ void olmo_qkv_kernel(T* __restrict__ qkv, const int* __restrict__ cu_seqlens, in
     }
     if (clip > 0.f)
         for (int e = threadIdx.x; e < nk; e += blockDim.x) row[nq + nk + e] = from_f<T>(clamped(to_f(row[nq + nk + e])));
-}
-
-// Olmo2RMSNorm: fp16(w * (x * rsqrt(mean(x^2) + eps))) with fp32 statistics, the weight multiply in fp32 and one
-// rounding (LlamaRMSNorm rounds to half before the weight).  One block per output row i, input row r = rows ? rows[i] : i.
-//   A != nullptr: X[r] = fp16(X[r] + norm(A[r])), OLMo-2's post-norm residual add, in place; out is not written.
-//   A == nullptr: out[i] = norm(X[r]), the final norm on the label rows.
-template <typename T>
-__global__ __launch_bounds__(256)
-void rms_post_kernel(T* __restrict__ X, const T* __restrict__ A, const int* __restrict__ rows, int hidden,
-                     const T* __restrict__ w, float eps, T* __restrict__ out) {
-    __shared__ float red[8];
-    const int i = blockIdx.x;
-    const int r = rows ? rows[i] : i;
-    const uint4* a = reinterpret_cast<const uint4*>((A ? A : X) + (size_t)r * hidden);
-    float s = 0.f;
-    for (int c = threadIdx.x; c < hidden / 8; c += blockDim.x) {
-        const uint4 v = a[c];
-        const pair_t<T>* h2 = reinterpret_cast<const pair_t<T>*>(&v);
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            const float2 f = to_f2(h2[e]);
-            s = fmaf(f.x, f.x, s);
-            s = fmaf(f.y, f.y, s);
-        }
-    }
-    const float rstd = rsqrtf(block_sum(s, red) / (float)hidden + eps);
-    const uint4* wv = reinterpret_cast<const uint4*>(w);
-    uint4* x = reinterpret_cast<uint4*>(X + (size_t)r * hidden);
-    uint4* o = reinterpret_cast<uint4*>(out + (size_t)i * hidden);
-    for (int c = threadIdx.x; c < hidden / 8; c += blockDim.x) {
-        const uint4 v = a[c], g = wv[c];
-        const pair_t<T>* h2 = reinterpret_cast<const pair_t<T>*>(&v);
-        const pair_t<T>* g2 = reinterpret_cast<const pair_t<T>*>(&g);
-        uint4 nv;
-        pair_t<T>* n2 = reinterpret_cast<pair_t<T>*>(&nv);
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            const float2 f = to_f2(h2[e]), gf = to_f2(g2[e]);
-            n2[e] = from_f2<T>(__fmul_rn(gf.x, __fmul_rn(f.x, rstd)), __fmul_rn(gf.y, __fmul_rn(f.y, rstd)));
-        }
-        if (A) {
-            uint4 xv = x[c];
-            pair_t<T>* x2 = reinterpret_cast<pair_t<T>*>(&xv);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) x2[e] = __hadd2(x2[e], n2[e]);
-            x[c] = xv;
-        } else {
-            o[c] = nv;
-        }
-    }
 }
 
 template <typename T>
@@ -665,29 +609,41 @@ struct LlmLayer {
     __half *qn = nullptr, *kn = nullptr;
 };
 
+// How rsb_llm_load copies a weight to its destination.
+enum class Copy {
+    plain,
+    neox_qkv,    // GPT-NeoX query_key_value weight or bias: per-head q_h | k_h | v_h rows to [Q heads | K heads | V heads]
+    tied,        // the embedding of a tied handle: embed and lm_head
+};
+
+// Destination of one HF state-dict name.
+struct Weight {
+    __half* dst;
+    int64_t n;                                   // elements
+    Copy copy;
+    bool counted;                                // required; a tied handle's lm_head.weight is accepted, copied, not counted
+};
+
 }  // namespace
 
 struct rsb_llm {
+    int family = RSB_LLM_LLAMA, dtype = RSB_DTYPE_F16;   // dtype: element type of weights and activations
     int layers = 0, hidden = 0, heads = 0, kv_heads = 0, inter = 0, vocab = 0, vocab_pad = 0, max_pos = 0;
     int head_dim = HD, rot = HD;                 // rot: rotated dims of each Q / K head (GPT-NeoX rotary_ndims)
-    int olmo = 0;                                // 1 = OLMo, 2 = OLMo-2 (rsb_llm_create_olmo), 0 otherwise
-    float rope_theta = 0.f, eps = 0.f, clip = 0.f;   // clip: OLMo clip_qkv, 0 = none
-    bool tied = false, neox = false;
-    bool bf16 = false;                           // element type of weights and activations (rsb_llm_set_dtype)
-    bool load_called = false;                    // rsb_llm_load has been called: the dtype is fixed
+    float eps = 0.f, clip = 0.f;                 // clip: OLMo clip_qkv, 0 = none
+    bool tied = false;
     // Device buffers of 2-byte elements, fp16 or bf16 by the handle's dtype; every zero fill means 0 in both.
     // OLMo: final_g holds ones, the unit scale with which ln_rows_kernel (and zero_bias as its shift) is OlmoLayerNorm
     __half *embed = nullptr, *lm_head = nullptr, *final_g = nullptr, *final_b = nullptr, *zero_bias = nullptr;
     float* inv_freq = nullptr;
     std::vector<LlmLayer> L;
+    // The only place the C side knows HF weight names: every name rsb_llm_load takes, with its destination.
+    std::map<std::string, Weight> weights;
+    std::vector<void*> owned;                    // every device allocation of the handle
     std::set<std::string> loaded;                // required weights loaded so far
     int qkv_n() const { return (heads + 2 * kv_heads) * head_dim; }
     size_t required() const {
-        const size_t head = tied ? 0 : 1;
-        if (neox) return 4 + 12 * (size_t)layers;
-        if (olmo == 1) return 1 + 7 * (size_t)layers + head;
-        if (olmo == 2) return 2 + 11 * (size_t)layers + head;
-        return 2 + 9 * (size_t)layers + head;
+        return std::count_if(weights.begin(), weights.end(), [](const auto& w) { return w.second.counted; });
     }
     int chunk_rows() const { return (int)std::max<size_t>(128, LOGIT_BYTES / ((size_t)vocab_pad * 2) / 128 * 128); }
 };
@@ -698,7 +654,9 @@ namespace {
 template <typename E> const E* as(const __half* p) { return reinterpret_cast<const E*>(p); }
 
 // f(E()) for the handle's element type E
-template <class F> int with_dtype(const rsb_llm* h, F&& f) { return h->bf16 ? f(__nv_bfloat16()) : f(__half()); }
+template <class F> int with_dtype(const rsb_llm* h, F&& f) {
+    return h->dtype == RSB_DTYPE_BF16 ? f(__nv_bfloat16()) : f(__half());
+}
 
 template <typename E> using same_t = typename std::common_type<E>::type;   // E, not deduced from this argument
 
@@ -716,14 +674,15 @@ int gemm(const E* A, int M, const __half* W, int N, int K, const __half* bias, c
 // MLP output is added in place.
 size_t llm_ws_layout(const rsb_llm* h, size_t T, size_t nl, size_t off[10]) {
     auto al = [](size_t x) { return (x + 1023) / 1024 * 1024; };
+    const bool neox = h->family == RSB_LLM_NEOX;
     const size_t chunk = std::min<size_t>(std::max<size_t>(nl, 1), (size_t)h->chunk_rows());
     size_t o = 0;
     off[0] = o; o += al(T * h->hidden * 2);                 // X (residual stream)
-    off[1] = o; o += al((h->neox ? 2 : 1) * T * h->hidden * 2);           // normed rows
+    off[1] = o; o += al((neox ? 2 : 1) * T * h->hidden * 2);           // normed rows
     off[2] = o; o += al(T * (size_t)h->qkv_n() * 2);        // QKV
     off[3] = o; o += al(T * h->hidden * 2);                 // attention output
-    off[4] = o; o += al((h->neox ? 1 : 2) * T * (size_t)h->inter * 2);    // gate | up
-    off[5] = o; o += al(T * (size_t)(h->neox ? h->hidden : h->inter) * 2);   // SwiGLU output
+    off[4] = o; o += al((neox ? 1 : 2) * T * (size_t)h->inter * 2);    // gate | up
+    off[5] = o; o += al(T * (size_t)(neox ? h->hidden : h->inter) * 2);   // SwiGLU output
     off[6] = o; o += al(chunk * (size_t)h->vocab_pad * 2);  // logits of one chunk of label rows
     off[7] = o; o += al(3 * std::max<size_t>(nl, 1) * sizeof(int));   // rows | labels | out_idx
     off[8] = o; o += al(T * sizeof(int2));                  // attention items (b, query block)
@@ -731,284 +690,209 @@ size_t llm_ws_layout(const rsb_llm* h, size_t T, size_t nl, size_t off[10]) {
     return o;
 }
 
+// Allocates a handle's device buffers and registers weight names against them; ok turns false on a failed cudaMalloc.
+struct WeightTable {
+    rsb_llm* h;
+    bool ok = true;
+    template <typename P = __half>
+    P* alloc(size_t n) {
+        void* p = nullptr;
+        if (cudaMalloc(&p, n * sizeof(P)) != cudaSuccess) { ok = false; return nullptr; }
+        h->owned.push_back(p);
+        return static_cast<P*>(p);
+    }
+    void add(const std::string& name, __half* dst, int64_t n, Copy copy = Copy::plain, bool counted = true) {
+        h->weights[name] = Weight{dst, n, copy, counted};
+    }
+    __half* weight(const std::string& name, int64_t n, Copy copy = Copy::plain) {   // a buffer of its own
+        __half* p = alloc(n);
+        add(name, p, n, copy);
+        return p;
+    }
+};
+
+// LlamaForCausalLM, OlmoForCausalLM and Olmo2ForCausalLM names; q|k|v and gate|up land in one fused weight each.
+// Llama: input_layernorm / post_attention_layernorm are ln1 / ln2.  OLMo: no norm weights (OlmoLayerNorm has none).
+// OLMo-2: post_attention_layernorm / post_feedforward_layernorm are ln1 / ln2, and q_norm / k_norm.
+void llama_weights(WeightTable& t) {
+    rsb_llm* h = t.h;
+    const int64_t H = h->hidden, KV = (int64_t)h->kv_heads * HD, I = h->inter, V = h->vocab;
+    t.add("model.embed_tokens.weight", h->embed, V * H, h->tied ? Copy::tied : Copy::plain);
+    t.add("lm_head.weight", h->lm_head, V * H, Copy::plain, !h->tied);
+    if (h->family != RSB_LLM_OLMO) t.add("model.norm.weight", h->final_g, H);
+    for (int li = 0; li < h->layers; ++li) {
+        LlmLayer& l = h->L[li];
+        const std::string p = "model.layers." + std::to_string(li) + ".";
+        l.wqkv = t.alloc((H + 2 * KV) * H);
+        t.add(p + "self_attn.q_proj.weight", l.wqkv, H * H);
+        t.add(p + "self_attn.k_proj.weight", l.wqkv + H * H, KV * H);
+        t.add(p + "self_attn.v_proj.weight", l.wqkv + (H + KV) * H, KV * H);
+        l.wo = t.weight(p + "self_attn.o_proj.weight", H * H);
+        l.wgu = t.alloc(2 * I * H);
+        t.add(p + "mlp.gate_proj.weight", l.wgu, I * H);
+        t.add(p + "mlp.up_proj.weight", l.wgu + I * H, I * H);
+        l.wdown = t.weight(p + "mlp.down_proj.weight", I * H);
+        if (h->family == RSB_LLM_LLAMA) {
+            l.ln1 = t.weight(p + "input_layernorm.weight", H);
+            l.ln2 = t.weight(p + "post_attention_layernorm.weight", H);
+        } else if (h->family == RSB_LLM_OLMO2) {
+            l.ln1 = t.weight(p + "post_attention_layernorm.weight", H);
+            l.ln2 = t.weight(p + "post_feedforward_layernorm.weight", H);
+            l.qn = t.weight(p + "self_attn.q_norm.weight", H);
+            l.kn = t.weight(p + "self_attn.k_norm.weight", KV);
+        }
+    }
+}
+
+// GPTNeoXForCausalLM names.  query_key_value's rows are [heads, 3, head_dim] (q_h | k_h | v_h per head); they land as
+// [Q heads | K heads | V heads], so the forward reads the Llama layout.
+void neox_weights(WeightTable& t) {
+    rsb_llm* h = t.h;
+    const int64_t H = h->hidden, I = h->inter, V = h->vocab;
+    t.add("gpt_neox.embed_in.weight", h->embed, V * H);
+    t.add("embed_out.weight", h->lm_head, V * H);
+    t.add("gpt_neox.final_layer_norm.weight", h->final_g, H);
+    h->final_b = t.weight("gpt_neox.final_layer_norm.bias", H);
+    for (int li = 0; li < h->layers; ++li) {
+        LlmLayer& l = h->L[li];
+        const std::string p = "gpt_neox.layers." + std::to_string(li) + ".";
+        l.ln1 = t.weight(p + "input_layernorm.weight", H);
+        l.ln1b = t.weight(p + "input_layernorm.bias", H);
+        l.ln2 = t.weight(p + "post_attention_layernorm.weight", H);
+        l.ln2b = t.weight(p + "post_attention_layernorm.bias", H);
+        l.wqkv = t.weight(p + "attention.query_key_value.weight", 3 * H * H, Copy::neox_qkv);
+        l.bqkv = t.weight(p + "attention.query_key_value.bias", 3 * H, Copy::neox_qkv);
+        l.wo = t.weight(p + "attention.dense.weight", H * H);
+        l.bo = t.weight(p + "attention.dense.bias", H);
+        l.wgu = t.weight(p + "mlp.dense_h_to_4h.weight", I * H);
+        l.bgu = t.weight(p + "mlp.dense_h_to_4h.bias", I);
+        l.wdown = t.weight(p + "mlp.dense_4h_to_h.weight", H * I);
+        l.bdown = t.weight(p + "mlp.dense_4h_to_h.bias", H);
+    }
+}
+
+// The refusals of rsb_llm_create (rsb.h), before any CUDA call.
+int check_create(int family, int dtype, int layers, int hidden, int heads, int kv_heads, int intermediate, int vocab,
+                 int max_pos, int rotary_dims, float rope_theta, float eps, float clip_qkv, int tied) {
+    if (family < RSB_LLM_LLAMA || family > RSB_LLM_OLMO2)
+        return lfail(RSB_ERR_INVALID, "family %ld is none of RSB_LLM_LLAMA, _NEOX, _OLMO and _OLMO2", (long)family);
+    if (dtype != RSB_DTYPE_F16 && dtype != RSB_DTYPE_BF16)
+        return lfail(RSB_ERR_INVALID, "dtype %ld is neither RSB_DTYPE_F16 nor RSB_DTYPE_BF16", (long)dtype);
+    const bool neox = family == RSB_LLM_NEOX;
+    if (layers <= 0 || vocab <= 0 || max_pos <= 0 || !(rope_theta > 0.f) || !(eps > 0.f) || (tied != 0 && tied != 1) ||
+        (neox && (hidden <= 0 || heads <= 0 || intermediate <= 0)))
+        return lfail(RSB_ERR_INVALID, "layers, vocab, max_pos, rope_theta (GPT-NeoX rotary_base), eps (rms_eps, ln_eps) "
+                     "and, for GPT-NeoX, hidden, heads and intermediate must be positive, tied 0 or 1");
+    if (!(clip_qkv >= 0.f) || std::isinf(clip_qkv) || (family != RSB_LLM_OLMO && clip_qkv != 0.f))
+        return lfail(RSB_ERR_INVALID, "clip_qkv must be finite and >= 0 (0 = none), and 0 for every family but OLMo");
+    if (neox) {
+        if (kv_heads != heads)
+            return lfail(RSB_ERR_UNSUPPORTED, "kv_heads %ld != heads %ld: GPT-NeoX has no grouped KV heads",
+                         (long)kv_heads, (long)heads);
+        if (tied) return lfail(RSB_ERR_UNSUPPORTED, "tied: GPT-NeoX readers have an untied embed_out");
+        const int hd = hidden / heads;
+        if (hidden % heads || (hd != 64 && hd != 80 && hd != 128 && hd != 256))
+            return lfail(RSB_ERR_UNSUPPORTED, "head_dim %ld (hidden %ld / heads %ld): only head_dim 64, 80, 128 and 256 "
+                         "are implemented", (long)(hidden % heads ? -1 : hd), (long)hidden, (long)heads);
+        if (rotary_dims <= 0 || rotary_dims > hd)
+            return lfail(RSB_ERR_INVALID, "rotary_dims %ld is not in [1, head_dim %ld]", (long)rotary_dims, (long)hd);
+        if (rotary_dims % 2) return lfail(RSB_ERR_UNSUPPORTED, "rotary_dims %ld is odd", (long)rotary_dims);
+    } else {
+        if (heads <= 0 || hidden != heads * HD)
+            return lfail(RSB_ERR_UNSUPPORTED, "only head_dim 128 is implemented (hidden %ld != 128 x heads)", (long)hidden);
+        if (kv_heads <= 0 || heads % kv_heads)
+            return lfail(RSB_ERR_UNSUPPORTED, "num_attention_heads must be a multiple of num_key_value_heads (got %ld kv "
+                         "heads)", (long)kv_heads);
+        if (rotary_dims != HD)
+            return lfail(RSB_ERR_INVALID, "rotary_dims %ld: only GPT-NeoX rotates part of a head (rotary_dims = head_dim "
+                         "128)", (long)rotary_dims);
+    }
+    if ((neox || family == RSB_LLM_OLMO) && hidden > LN_MAX_HIDDEN)
+        return lfail(RSB_ERR_UNSUPPORTED, "hidden %ld: the LayerNorm kernel holds rows of at most %ld", (long)hidden,
+                     (long)LN_MAX_HIDDEN);
+    if (intermediate <= 0 || intermediate % 128)
+        return lfail(RSB_ERR_UNSUPPORTED, "intermediate_size %ld is not a multiple of 128", (long)intermediate);
+    return RSB_OK;
+}
+
 }  // namespace
 
 extern "C" const char* rsb_llm_last_error(void) { return g_lerr.c_str(); }
 
-// Replaces `AutoModelForCausalLM.from_pretrained(cfg.model.lm_model, torch_dtype=torch.bfloat16)` for Llama readers
+// Replaces `AutoModelForCausalLM.from_pretrained(cfg.model.lm_model, torch_dtype=torch.bfloat16)`
 // (src/evaluate_perplexity.py:98-108).  Every refusal comes before any CUDA call.
-extern "C" int rsb_llm_create(int layers, int hidden, int heads, int kv_heads, int intermediate, int vocab, int max_pos,
-                              float rope_theta, float rms_eps, int tied, rsb_llm_t** out) {
+extern "C" int rsb_llm_create(int family, int dtype, int layers, int hidden, int heads, int kv_heads, int intermediate,
+                              int vocab, int max_pos, int rotary_dims, float rope_theta, float eps, float clip_qkv,
+                              int tied, rsb_llm_t** out) {
     if (!out) return lfail(RSB_ERR_INVALID, "out is NULL");
     *out = nullptr;
-    if (layers <= 0 || vocab <= 0 || max_pos <= 0 || !(rope_theta > 0.f) || !(rms_eps > 0.f) || (tied != 0 && tied != 1))
-        return lfail(RSB_ERR_INVALID, "layers, vocab, max_pos, rope_theta and rms_eps must be positive, tied 0 or 1");
-    if (heads <= 0 || hidden != heads * HD)
-        return lfail(RSB_ERR_UNSUPPORTED, "only head_dim 128 is implemented (hidden %ld != 128 x heads)", (long)hidden);
-    if (kv_heads <= 0 || heads % kv_heads)
-        return lfail(RSB_ERR_UNSUPPORTED, "num_attention_heads must be a multiple of num_key_value_heads (got %ld kv heads)", (long)kv_heads);
-    if (intermediate <= 0 || intermediate % 128)
-        return lfail(RSB_ERR_UNSUPPORTED, "intermediate_size %ld is not a multiple of 128", (long)intermediate);
+    const int rc = check_create(family, dtype, layers, hidden, heads, kv_heads, intermediate, vocab, max_pos,
+                                rotary_dims, rope_theta, eps, clip_qkv, tied);
+    if (rc != RSB_OK) return rc;
     rsb_llm* h = new rsb_llm();
+    h->family = family; h->dtype = dtype;
     h->layers = layers; h->hidden = hidden; h->heads = heads; h->kv_heads = kv_heads; h->inter = intermediate;
+    h->head_dim = hidden / heads; h->rot = rotary_dims;
     h->vocab = vocab; h->vocab_pad = (vocab + 127) / 128 * 128; h->max_pos = max_pos;
-    h->rope_theta = rope_theta; h->eps = rms_eps; h->tied = tied != 0;
+    h->eps = eps; h->clip = clip_qkv; h->tied = tied != 0;
     const size_t H = hidden, V = h->vocab_pad;
     const size_t zb = std::max({(size_t)h->qkv_n(), 2 * (size_t)intermediate, V, H});
-    bool ok = true;
-    ok &= cudaMalloc(&h->embed, (size_t)vocab * H * 2) == cudaSuccess;
-    ok &= cudaMalloc(&h->lm_head, V * H * 2) == cudaSuccess;
-    ok &= cudaMalloc(&h->final_g, H * 2) == cudaSuccess;
-    ok &= cudaMalloc(&h->zero_bias, zb * 2) == cudaSuccess;
-    ok &= cudaMalloc(&h->inv_freq, HD / 2 * sizeof(float)) == cudaSuccess;
+    WeightTable t{h};
+    h->embed = t.alloc((size_t)vocab * H);
+    h->lm_head = t.alloc(V * H);
+    h->final_g = t.alloc(H);
+    h->zero_bias = t.alloc(zb);
+    h->inv_freq = t.alloc<float>(rotary_dims / 2);
     h->L.resize(layers);
-    for (auto& l : h->L) {
-        ok &= cudaMalloc(&l.wqkv, (size_t)h->qkv_n() * H * 2) == cudaSuccess;
-        ok &= cudaMalloc(&l.wo, H * H * 2) == cudaSuccess;
-        ok &= cudaMalloc(&l.wgu, 2 * (size_t)intermediate * H * 2) == cudaSuccess;
-        ok &= cudaMalloc(&l.wdown, (size_t)intermediate * H * 2) == cudaSuccess;
-        ok &= cudaMalloc(&l.ln1, H * 2) == cudaSuccess;
-        ok &= cudaMalloc(&l.ln2, H * 2) == cudaSuccess;
-    }
-    if (!ok) { rsb_llm_free(h); return lfail(RSB_ERR_OOM, "allocating reader weights failed"); }
-    // LlamaRotaryEmbedding: inv_freq = 1 / theta ** (arange(0, 128, 2).float() / 128), in fp32
-    float inv[HD / 2];
-    for (int i = 0; i < HD / 2; ++i) inv[i] = 1.f / powf(rope_theta, (float)(2 * i) / (float)HD);
-    ok &= cudaMemcpy(h->inv_freq, inv, sizeof inv, cudaMemcpyHostToDevice) == cudaSuccess;
+    if (family == RSB_LLM_NEOX) neox_weights(t); else llama_weights(t);
+    if (!t.ok) { rsb_llm_free(h); return lfail(RSB_ERR_OOM, "allocating reader weights failed"); }
+    // LlamaRotaryEmbedding / GPTNeoXRotaryEmbedding: inv_freq = 1 / theta ** (arange(0, rot, 2).float() / rot), in fp32
+    std::vector<float> inv(rotary_dims / 2);
+    for (int i = 0; i < rotary_dims / 2; ++i) inv[i] = 1.f / powf(rope_theta, (float)(2 * i) / (float)rotary_dims);
+    bool ok = cudaMemcpy(h->inv_freq, inv.data(), inv.size() * sizeof(float), cudaMemcpyHostToDevice) == cudaSuccess;
     ok &= cudaMemset(h->zero_bias, 0, zb * 2) == cudaSuccess;
     ok &= cudaMemset(h->lm_head, 0, V * H * 2) == cudaSuccess;   // pad rows stay zero (and outside the sum)
+    if (family == RSB_LLM_OLMO) {
+        const std::vector<uint16_t> ones(H, dtype == RSB_DTYPE_BF16 ? 0x3F80 : 0x3C00);   // 1.0 in bf16 / fp16
+        ok &= cudaMemcpy(h->final_g, ones.data(), H * 2, cudaMemcpyHostToDevice) == cudaSuccess;
+    }
     if (!ok) { rsb_llm_free(h); return lfail(RSB_ERR_CUDA, "initialising the reader failed"); }
     *out = h;
-    return RSB_OK;
-}
-
-// Replaces the same call for GPT-NeoX readers (Pythia, the reference's default lm_model): LayerNorm with biases,
-// per-head interleaved query_key_value with biases, partial rotary on rotary_dims of each head, exact-GELU MLP, the
-// parallel residual and an untied embed_out.  Every refusal comes before any CUDA call.
-extern "C" int rsb_llm_create_neox(int layers, int hidden, int heads, int intermediate, int vocab, int max_pos,
-                                   int rotary_dims, float rotary_base, float ln_eps, rsb_llm_t** out) {
-    if (!out) return lfail(RSB_ERR_INVALID, "out is NULL");
-    *out = nullptr;
-    if (layers <= 0 || hidden <= 0 || heads <= 0 || intermediate <= 0 || vocab <= 0 || max_pos <= 0 ||
-        !(rotary_base > 0.f) || !(ln_eps > 0.f))
-        return lfail(RSB_ERR_INVALID, "layers, hidden, heads, intermediate, vocab, max_pos, rotary_base and ln_eps must be positive");
-    const int hd = hidden / heads;
-    if (hidden % heads || (hd != 64 && hd != 80 && hd != 128 && hd != 256))
-        return lfail(RSB_ERR_UNSUPPORTED, "head_dim %ld (hidden %ld / heads %ld): only head_dim 64, 80, 128 and 256 are "
-                     "implemented", (long)(hidden % heads ? -1 : hd), (long)hidden, (long)heads);
-    if (rotary_dims <= 0 || rotary_dims > hd)
-        return lfail(RSB_ERR_INVALID, "rotary_dims %ld is not in [1, head_dim %ld]", (long)rotary_dims, (long)hd);
-    if (rotary_dims % 2)
-        return lfail(RSB_ERR_UNSUPPORTED, "rotary_dims %ld is odd", (long)rotary_dims);
-    if (hidden > LN_MAX_HIDDEN)
-        return lfail(RSB_ERR_UNSUPPORTED, "hidden %ld: the LayerNorm kernel holds rows of at most %ld", (long)hidden,
-                     (long)LN_MAX_HIDDEN);
-    if (intermediate % 128)
-        return lfail(RSB_ERR_UNSUPPORTED, "intermediate_size %ld is not a multiple of 128", (long)intermediate);
-    rsb_llm* h = new rsb_llm();
-    h->neox = true;
-    h->layers = layers; h->hidden = hidden; h->heads = heads; h->kv_heads = heads; h->inter = intermediate;
-    h->head_dim = hd; h->rot = rotary_dims;
-    h->vocab = vocab; h->vocab_pad = (vocab + 127) / 128 * 128; h->max_pos = max_pos;
-    h->rope_theta = rotary_base; h->eps = ln_eps;
-    const size_t H = hidden, V = h->vocab_pad, I = intermediate;
-    bool ok = true;
-    ok &= cudaMalloc(&h->embed, (size_t)vocab * H * 2) == cudaSuccess;
-    ok &= cudaMalloc(&h->lm_head, V * H * 2) == cudaSuccess;
-    ok &= cudaMalloc(&h->final_g, H * 2) == cudaSuccess;
-    ok &= cudaMalloc(&h->final_b, H * 2) == cudaSuccess;
-    ok &= cudaMalloc(&h->zero_bias, V * 2) == cudaSuccess;            // the LM head's (embed_out has no bias)
-    ok &= cudaMalloc(&h->inv_freq, rotary_dims / 2 * sizeof(float)) == cudaSuccess;
-    h->L.resize(layers);
-    for (auto& l : h->L) {
-        ok &= cudaMalloc(&l.wqkv, 3 * H * H * 2) == cudaSuccess;
-        ok &= cudaMalloc(&l.wo, H * H * 2) == cudaSuccess;
-        ok &= cudaMalloc(&l.wgu, I * H * 2) == cudaSuccess;
-        ok &= cudaMalloc(&l.wdown, I * H * 2) == cudaSuccess;
-        ok &= cudaMalloc(&l.bqkv, 3 * H * 2) == cudaSuccess;
-        ok &= cudaMalloc(&l.bo, H * 2) == cudaSuccess;
-        ok &= cudaMalloc(&l.bgu, I * 2) == cudaSuccess;
-        ok &= cudaMalloc(&l.bdown, H * 2) == cudaSuccess;
-        for (__half** p : {&l.ln1, &l.ln1b, &l.ln2, &l.ln2b}) ok &= cudaMalloc(p, H * 2) == cudaSuccess;
-    }
-    if (!ok) { rsb_llm_free(h); return lfail(RSB_ERR_OOM, "allocating reader weights failed"); }
-    // GPTNeoXRotaryEmbedding: inv_freq = 1 / base ** (arange(0, rot, 2).float() / rot), in fp32
-    std::vector<float> inv(rotary_dims / 2);
-    for (int i = 0; i < rotary_dims / 2; ++i) inv[i] = 1.f / powf(rotary_base, (float)(2 * i) / (float)rotary_dims);
-    ok &= cudaMemcpy(h->inv_freq, inv.data(), inv.size() * sizeof(float), cudaMemcpyHostToDevice) == cudaSuccess;
-    ok &= cudaMemset(h->zero_bias, 0, V * 2) == cudaSuccess;
-    ok &= cudaMemset(h->lm_head, 0, V * H * 2) == cudaSuccess;   // pad rows stay zero (and outside the sum)
-    if (!ok) { rsb_llm_free(h); return lfail(RSB_ERR_CUDA, "initialising the reader failed"); }
-    *out = h;
-    return RSB_OK;
-}
-
-// Replaces the same call for OLMo (version 1, OlmoForCausalLM) and OLMo-2 (version 2, Olmo2ForCausalLM) readers: the
-// Llama handle with OLMo's norms, clip_qkv, QK-norm and fp32 rotary.  Every refusal comes before any CUDA call
-// (rsb_llm_create's included).
-extern "C" int rsb_llm_create_olmo(int version, int layers, int hidden, int heads, int kv_heads, int intermediate,
-                                   int vocab, int max_pos, float rope_theta, float eps, float clip_qkv, int tied,
-                                   rsb_llm_t** out) {
-    if (!out) return lfail(RSB_ERR_INVALID, "out is NULL");
-    *out = nullptr;
-    if (version != 1 && version != 2)
-        return lfail(RSB_ERR_INVALID, "version %ld is neither 1 (OLMo) nor 2 (OLMo-2)", (long)version);
-    if (!(clip_qkv >= 0.f) || std::isinf(clip_qkv) || (version == 2 && clip_qkv != 0.f))
-        return lfail(RSB_ERR_INVALID, "clip_qkv must be finite and >= 0 (0 = none), and 0 for OLMo-2");
-    if (version == 1 && hidden > LN_MAX_HIDDEN)
-        return lfail(RSB_ERR_UNSUPPORTED, "hidden %ld: the LayerNorm kernel holds rows of at most %ld", (long)hidden,
-                     (long)LN_MAX_HIDDEN);
-    int rc = rsb_llm_create(layers, hidden, heads, kv_heads, intermediate, vocab, max_pos, rope_theta, eps, tied, out);
-    if (rc != RSB_OK) return rc;
-    rsb_llm* h = *out;
-    h->olmo = version;
-    h->clip = clip_qkv;
-    bool ok = true;
-    if (version == 1) {
-        const std::vector<__half> ones(hidden, __float2half(1.f));
-        ok = cudaMemcpy(h->final_g, ones.data(), (size_t)hidden * 2, cudaMemcpyHostToDevice) == cudaSuccess;
-    } else {
-        for (auto& l : h->L) {
-            ok &= cudaMalloc(&l.qn, (size_t)hidden * 2) == cudaSuccess;
-            ok &= cudaMalloc(&l.kn, (size_t)kv_heads * HD * 2) == cudaSuccess;
-        }
-    }
-    if (!ok) {
-        rsb_llm_free(h);
-        *out = nullptr;
-        return lfail(RSB_ERR_OOM, "allocating reader weights failed");
-    }
-    return RSB_OK;
-}
-
-// The element type of the handle's weights and activations: RSB_DTYPE_F16 (the default) or RSB_DTYPE_BF16, before the
-// first rsb_llm_load.  OLMo's unit LayerNorm scale is rewritten in the new type.
-extern "C" int rsb_llm_set_dtype(rsb_llm_t* h, int dtype) {
-    if (!h) return lfail(RSB_ERR_INVALID, "null argument");
-    if (dtype != RSB_DTYPE_F16 && dtype != RSB_DTYPE_BF16)
-        return lfail(RSB_ERR_INVALID, "dtype %ld is neither RSB_DTYPE_F16 nor RSB_DTYPE_BF16", (long)dtype);
-    if (h->load_called) return lfail(RSB_ERR_STATE, "the dtype is fixed once rsb_llm_load has been called");
-    h->bf16 = dtype == RSB_DTYPE_BF16;
-    if (h->olmo == 1) {
-        const uint16_t one = h->bf16 ? 0x3F80 : 0x3C00;   // 1.0 in bf16 / fp16
-        const std::vector<uint16_t> ones(h->hidden, one);
-        if (cudaMemcpy(h->final_g, ones.data(), (size_t)h->hidden * 2, cudaMemcpyHostToDevice) != cudaSuccess)
-            return lfail(RSB_ERR_CUDA, "writing the OLMo LayerNorm scale failed");
-    }
     return RSB_OK;
 }
 
 extern "C" int rsb_llm_free(rsb_llm_t* h) {
     if (!h) return RSB_OK;
-    cudaFree(h->embed); cudaFree(h->lm_head); cudaFree(h->final_g); cudaFree(h->final_b); cudaFree(h->zero_bias);
-    cudaFree(h->inv_freq);
-    for (auto& l : h->L) {
-        cudaFree(l.wqkv); cudaFree(l.wo); cudaFree(l.wgu); cudaFree(l.wdown); cudaFree(l.ln1); cudaFree(l.ln2);
-        cudaFree(l.bqkv); cudaFree(l.bo); cudaFree(l.bgu); cudaFree(l.bdown); cudaFree(l.ln1b); cudaFree(l.ln2b);
-        cudaFree(l.qn); cudaFree(l.kn);
-    }
+    for (void* p : h->owned) cudaFree(p);
     delete h;
     return RSB_OK;
 }
 
-// name = HF LlamaForCausalLM state_dict key, data fp16 on the device, copied (src/evaluate_perplexity.py:98-108 loads
-// the same checkpoint).  q|k|v and gate|up land in one fused weight each.
-namespace {
-
-// GPTNeoXForCausalLM state_dict keys.  query_key_value's rows are [heads, 3, head_dim] (q_h | k_h | v_h per head); they
-// land as [Q heads | K heads | V heads], one strided copy per part, so the forward reads the Llama layout.
-int load_neox(rsb_llm* h, const char* name, const void* src, int64_t n, cudaStream_t st) {
-    const int64_t H = h->hidden, I = h->inter;
-    const std::string s(name);
-    auto copied = [&](cudaError_t e) -> int {
-        if (e != cudaSuccess) return lfail(RSB_ERR_CUDA, "copy of %s failed", name);
-        h->loaded.insert(s);
-        return RSB_OK;
-    };
-    auto put = [&](__half* dst, int64_t expect) -> int {
-        if (n != expect) return lfail(RSB_ERR_INVALID, "weight %s has the wrong size (%ld elements)", name, (long)n);
-        return copied(cudaMemcpyAsync(dst, src, (size_t)n * 2, cudaMemcpyDeviceToDevice, st));
-    };
-    auto put_qkv = [&](__half* dst, int64_t per_row) -> int {      // per_row = H (weight) or 1 (bias)
-        if (n != 3 * H * per_row) return lfail(RSB_ERR_INVALID, "weight %s has the wrong size (%ld elements)", name, (long)n);
-        const size_t part = (size_t)h->head_dim * per_row * 2;      // bytes of one head's q (or k or v) rows
-        cudaError_t e = cudaSuccess;
-        for (int p = 0; p < 3 && e == cudaSuccess; ++p)
-            e = cudaMemcpy2DAsync(dst + p * H * per_row, part, static_cast<const char*>(src) + p * part, 3 * part, part,
-                                  h->heads, cudaMemcpyDeviceToDevice, st);
-        return copied(e);
-    };
-    if (s == "gpt_neox.embed_in.weight") return put(h->embed, (int64_t)h->vocab * H);
-    if (s == "embed_out.weight") return put(h->lm_head, (int64_t)h->vocab * H);
-    if (s == "gpt_neox.final_layer_norm.weight") return put(h->final_g, H);
-    if (s == "gpt_neox.final_layer_norm.bias") return put(h->final_b, H);
-    int li = -1;
-    char rest[128] = {0};
-    if (sscanf(name, "gpt_neox.layers.%d.%127s", &li, rest) == 2 && li >= 0 && li < h->layers) {
-        LlmLayer& l = h->L[li];
-        const std::string r(rest);
-        if (r == "input_layernorm.weight") return put(l.ln1, H);
-        if (r == "input_layernorm.bias") return put(l.ln1b, H);
-        if (r == "post_attention_layernorm.weight") return put(l.ln2, H);
-        if (r == "post_attention_layernorm.bias") return put(l.ln2b, H);
-        if (r == "attention.query_key_value.weight") return put_qkv(l.wqkv, H);
-        if (r == "attention.query_key_value.bias") return put_qkv(l.bqkv, 1);
-        if (r == "attention.dense.weight") return put(l.wo, H * H);
-        if (r == "attention.dense.bias") return put(l.bo, H);
-        if (r == "mlp.dense_h_to_4h.weight") return put(l.wgu, I * H);
-        if (r == "mlp.dense_h_to_4h.bias") return put(l.bgu, I);
-        if (r == "mlp.dense_4h_to_h.weight") return put(l.wdown, H * I);
-        if (r == "mlp.dense_4h_to_h.bias") return put(l.bdown, H);
-    }
-    return lfail(RSB_ERR_INVALID, "unknown weight name %s", name);
-}
-
-}  // namespace
-
+// name = an HF state-dict key of the handle's family (rsb.h), data on the device in the handle's dtype, copied
+// (src/evaluate_perplexity.py:98-108 loads the same checkpoint).
 extern "C" int rsb_llm_load(rsb_llm_t* h, const char* name, const void* f16_dev, int64_t n, rsb_stream_t stream) {
     if (!h || !name || !f16_dev) return lfail(RSB_ERR_INVALID, "null argument");
-    h->load_called = true;
+    const auto it = h->weights.find(name);
+    if (it == h->weights.end()) return lfail(RSB_ERR_INVALID, "unknown weight name %s", name);
+    const Weight& w = it->second;
+    if (n != w.n) return lfail(RSB_ERR_INVALID, "weight %s has the wrong size (%ld elements)", name, (long)n);
     cudaStream_t st = (cudaStream_t)stream;
-    if (h->neox) return load_neox(h, name, f16_dev, n, st);
-    const int64_t H = h->hidden, KV = (int64_t)h->kv_heads * HD, I = h->inter;
-    const std::string s(name);
-    auto put = [&](__half* dst, int64_t expect) -> int {
-        if (n != expect) return lfail(RSB_ERR_INVALID, "weight %s has the wrong size (%ld elements)", name, (long)n);
-        if (cudaMemcpyAsync(dst, f16_dev, (size_t)n * 2, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
-            return lfail(RSB_ERR_CUDA, "copy of %s failed", name);
-        if (!(h->tied && s == "lm_head.weight")) h->loaded.insert(s);
-        return RSB_OK;
-    };
-    if (s == "model.embed_tokens.weight") {
-        const int rc = put(h->embed, (int64_t)h->vocab * H);
-        if (rc != RSB_OK || !h->tied) return rc;
-        return put(h->lm_head, (int64_t)h->vocab * H);
+    cudaError_t e;
+    if (w.copy == Copy::neox_qkv) {              // one strided copy per part
+        const int64_t H = h->hidden, per_row = n / (3 * H);   // H (weight) or 1 (bias)
+        const size_t part = (size_t)h->head_dim * per_row * 2;     // bytes of one head's q (or k or v) rows
+        e = cudaSuccess;
+        for (int p = 0; p < 3 && e == cudaSuccess; ++p)
+            e = cudaMemcpy2DAsync(w.dst + p * H * per_row, part, static_cast<const char*>(f16_dev) + p * part, 3 * part,
+                                  part, h->heads, cudaMemcpyDeviceToDevice, st);
+    } else {
+        e = cudaMemcpyAsync(w.dst, f16_dev, (size_t)n * 2, cudaMemcpyDeviceToDevice, st);
+        if (e == cudaSuccess && w.copy == Copy::tied)
+            e = cudaMemcpyAsync(h->lm_head, f16_dev, (size_t)n * 2, cudaMemcpyDeviceToDevice, st);
     }
-    if (s == "lm_head.weight") return put(h->lm_head, (int64_t)h->vocab * H);
-    if (s == "model.norm.weight" && h->olmo != 1) return put(h->final_g, H);   // OlmoLayerNorm has no weight
-    int li = -1;
-    char rest[128] = {0};
-    if (sscanf(name, "model.layers.%d.%127s", &li, rest) == 2 && li >= 0 && li < h->layers) {
-        LlmLayer& l = h->L[li];
-        const std::string r(rest);
-        if (r == "self_attn.q_proj.weight") return put(l.wqkv, H * H);
-        if (r == "self_attn.k_proj.weight") return put(l.wqkv + H * H, KV * H);
-        if (r == "self_attn.v_proj.weight") return put(l.wqkv + (H + KV) * H, KV * H);
-        if (r == "self_attn.o_proj.weight") return put(l.wo, H * H);
-        if (r == "mlp.gate_proj.weight") return put(l.wgu, I * H);
-        if (r == "mlp.up_proj.weight") return put(l.wgu + I * H, I * H);
-        if (r == "mlp.down_proj.weight") return put(l.wdown, I * H);
-        if (h->olmo == 0) {
-            if (r == "input_layernorm.weight") return put(l.ln1, H);
-            if (r == "post_attention_layernorm.weight") return put(l.ln2, H);
-        } else if (h->olmo == 2) {
-            if (r == "post_attention_layernorm.weight") return put(l.ln1, H);
-            if (r == "post_feedforward_layernorm.weight") return put(l.ln2, H);
-            if (r == "self_attn.q_norm.weight") return put(l.qn, H);
-            if (r == "self_attn.k_norm.weight") return put(l.kn, KV);
-        }
-    }
-    return lfail(RSB_ERR_INVALID, "unknown weight name %s", name);
+    if (e != cudaSuccess) return lfail(RSB_ERR_CUDA, "copy of %s failed", name);
+    if (w.counted) h->loaded.insert(name);
+    return RSB_OK;
 }
 
 extern "C" size_t rsb_llm_workspace_bytes(rsb_llm_t* h, int total_tokens, int label_tokens) {
@@ -1052,14 +936,12 @@ void attention_step(const rsb_llm* h, const LlmLayer& l, E* QKV, const int32_t* 
                     const int2* d_items, int n_items, E* CTX, cudaStream_t st) {
     if (n_tok == 0 || n_items == 0) return;
     const float scale_log2 = 1.4426950408889634f / sqrtf((float)h->head_dim);   // 1/sqrt(head_dim) in the log2 domain
-    if (h->neox)
-        rope_partial_kernel<E><<<n_tok, 256, 0, st>>>(QKV, cu_seqlens, B, h->qkv_n(), h->heads + h->kv_heads, h->head_dim,
-                                                   h->rot, h->inv_freq);
-    else if (h->olmo)
+    if (h->family == RSB_LLM_OLMO || h->family == RSB_LLM_OLMO2)
         olmo_qkv_kernel<E><<<n_tok, 256, 0, st>>>(QKV, cu_seqlens, B, h->heads, h->kv_heads, h->inv_freq, h->clip,
-                                                  h->olmo == 2 ? as<E>(l.qn) : nullptr, as<E>(l.kn), h->eps);
+                                                  as<E>(l.qn), as<E>(l.kn), h->eps);
     else
-        rope_kernel<E><<<n_tok, 256, 0, st>>>(QKV, cu_seqlens, B, h->qkv_n(), h->heads + h->kv_heads, h->inv_freq);
+        rope_kernel<E><<<n_tok, 256, 0, st>>>(QKV, cu_seqlens, B, h->qkv_n(), h->heads + h->kv_heads, h->head_dim, h->rot,
+                                              h->inv_freq);
     const dim3 grid((unsigned)n_items, h->heads);
     switch (h->head_dim) {
         case 64: attention_causal_kernel<64, E><<<grid, 128, 0, st>>>(QKV, cu_seqlens, d_items, CTX, h->heads, h->kv_heads, scale_log2); break;
@@ -1111,63 +993,44 @@ struct Fwd {
     const int2* d_items;
 };
 
-// LlamaDecoderLayer x layers: x += o_proj(attn(rms1(x))); x += down(swiglu(gate|up(rms2(x)))).
+// The sequential-residual decoder layers, x layers.  LlamaDecoderLayer: x += o_proj(attn(rms1(x))); x +=
+// down(swiglu(gate|up(rms2(x)))).  OlmoDecoderLayer: the same with OlmoLayerNorm (ln_rows_kernel with unit scale and
+// zero shift) as both pre-norms.  Olmo2DecoderLayer: no pre-norms; x = fp16(x +
+// post_attention_layernorm(o_proj(attn(x)))), then x = fp16(x + post_feedforward_layernorm(down(swiglu(gate|up(x))))).
+// A norm sits between each projection and its add, so o_proj and down_proj write slot 1 (free without pre-norms) and
+// rms_rows_kernel adds the normed rows to x.
 template <typename E>
-int llama_layers(rsb_llm* h, const Fwd<E>& f, cudaStream_t st) {
+int sequential_layers(rsb_llm* h, const Fwd<E>& f, cudaStream_t st) {
     const int Hd = h->hidden, NQKV = h->qkv_n(), I = h->inter, T = f.T;
     const long long n8 = (long long)T * I / 8;
     const int sw_grid = (int)std::min<long long>((n8 + 255) / 256, 8LL * rsb::device_num_sms());
-    int rc;
-    for (int li = 0; li < h->layers; ++li) {
-        const LlmLayer& l = h->L[li];
-        rms_rows_kernel<E><<<T, 256, 0, st>>>(f.X, nullptr, Hd, as<E>(l.ln1), h->eps, f.Hn);
-        if ((rc = gemm(f.Hn, T, l.wqkv, NQKV, Hd, h->zero_bias, nullptr, f.QKV, 0, st)) != RSB_OK) return rc;
-        attention_step(h, l, f.QKV, f.cu_seqlens, f.B, T, f.d_items, f.n_items, f.CTX, st);
-        if ((rc = gemm(f.CTX, T, l.wo, Hd, Hd, h->zero_bias, f.X, f.X, 2, st)) != RSB_OK) return rc;
-        rms_rows_kernel<E><<<T, 256, 0, st>>>(f.X, nullptr, Hd, as<E>(l.ln2), h->eps, f.Hn);
-        if ((rc = gemm(f.Hn, T, l.wgu, 2 * I, Hd, h->zero_bias, nullptr, f.GU, 0, st)) != RSB_OK) return rc;
-        swiglu_kernel<E><<<sw_grid, 256, 0, st>>>(f.GU, n8, I, f.ACT);
-        if ((rc = gemm(f.ACT, T, l.wdown, Hd, I, h->zero_bias, f.X, f.X, 2 | RSB_GEMM_REVERSED, st)) != RSB_OK) return rc;
-    }
-    return RSB_OK;
-}
-
-// OlmoDecoderLayer x layers: Llama's sequence with OlmoLayerNorm (ln_rows_kernel with unit scale and zero shift) as
-// both pre-norms.  Olmo2DecoderLayer x layers: no pre-norms; x = fp16(x + post_attention_layernorm(o_proj(attn(x)))),
-// then x = fp16(x + post_feedforward_layernorm(down(swiglu(gate|up(x))))).  A norm sits between each projection and
-// its add, so o_proj and down_proj write slot 1 (free without pre-norms) and rms_post_kernel adds the normed rows to x.
-template <typename E>
-int olmo_layers(rsb_llm* h, const Fwd<E>& f, cudaStream_t st) {
-    const int Hd = h->hidden, NQKV = h->qkv_n(), I = h->inter, T = f.T;
-    const long long n8 = (long long)T * I / 8;
-    const int sw_grid = (int)std::min<long long>((n8 + 255) / 256, 8LL * rsb::device_num_sms());
-    const bool v2 = h->olmo == 2;
+    const bool v2 = h->family == RSB_LLM_OLMO2;
     const E* in = v2 ? f.X : f.Hn;               // what q|k|v and gate|up read
-    auto olmo_ln = [&]() {
-        ln_rows_kernel<E><<<T, LN_THREADS, 0, st>>>(f.X, nullptr, nullptr, Hd, as<E>(h->final_g), as<E>(h->zero_bias),
-                                                    nullptr, nullptr, h->eps, f.Hn, nullptr);
+    auto pre_norm = [&](const __half* w) {       // w: the Llama norm's weight
+        if (h->family == RSB_LLM_LLAMA)
+            rms_rows_kernel<E, false><<<T, 256, 0, st>>>(f.X, nullptr, nullptr, Hd, as<E>(w), h->eps, f.Hn);
+        else if (h->family == RSB_LLM_OLMO)
+            ln_rows_kernel<E><<<T, LN_THREADS, 0, st>>>(f.X, nullptr, nullptr, Hd, as<E>(h->final_g), as<E>(h->zero_bias),
+                                                        nullptr, nullptr, h->eps, f.Hn, nullptr);
+    };
+    // x += A W^T, or for OLMo-2 x = fp16(x + norm(A W^T)) with the post-norm weight w
+    auto residual = [&](const E* A, const __half* W, int K, int epi, const __half* w) -> int {
+        if (!v2) return gemm(A, T, W, Hd, K, h->zero_bias, f.X, f.X, 2 | epi, st);
+        const int rc = gemm(A, T, W, Hd, K, h->zero_bias, nullptr, f.Hn, 0, st);
+        if (rc == RSB_OK) rms_rows_kernel<E, true><<<T, 256, 0, st>>>(f.X, f.Hn, nullptr, Hd, as<E>(w), h->eps, nullptr);
+        return rc;
     };
     int rc;
     for (int li = 0; li < h->layers; ++li) {
         const LlmLayer& l = h->L[li];
-        if (!v2) olmo_ln();
+        pre_norm(l.ln1);
         if ((rc = gemm(in, T, l.wqkv, NQKV, Hd, h->zero_bias, nullptr, f.QKV, 0, st)) != RSB_OK) return rc;
         attention_step(h, l, f.QKV, f.cu_seqlens, f.B, T, f.d_items, f.n_items, f.CTX, st);
-        if (v2) {
-            if ((rc = gemm(f.CTX, T, l.wo, Hd, Hd, h->zero_bias, nullptr, f.Hn, 0, st)) != RSB_OK) return rc;
-            rms_post_kernel<E><<<T, 256, 0, st>>>(f.X, f.Hn, nullptr, Hd, as<E>(l.ln1), h->eps, nullptr);
-        } else {
-            if ((rc = gemm(f.CTX, T, l.wo, Hd, Hd, h->zero_bias, f.X, f.X, 2, st)) != RSB_OK) return rc;
-            olmo_ln();
-        }
+        if ((rc = residual(f.CTX, l.wo, Hd, 0, l.ln1)) != RSB_OK) return rc;
+        pre_norm(l.ln2);
         if ((rc = gemm(in, T, l.wgu, 2 * I, Hd, h->zero_bias, nullptr, f.GU, 0, st)) != RSB_OK) return rc;
         swiglu_kernel<E><<<sw_grid, 256, 0, st>>>(f.GU, n8, I, f.ACT);
-        if (v2) {
-            if ((rc = gemm(f.ACT, T, l.wdown, Hd, I, h->zero_bias, nullptr, f.Hn, 0, st)) != RSB_OK) return rc;
-            rms_post_kernel<E><<<T, 256, 0, st>>>(f.X, f.Hn, nullptr, Hd, as<E>(l.ln2), h->eps, nullptr);
-        } else if ((rc = gemm(f.ACT, T, l.wdown, Hd, I, h->zero_bias, f.X, f.X, 2 | RSB_GEMM_REVERSED, st)) != RSB_OK) {
-            return rc;
-        }
+        if ((rc = residual(f.ACT, l.wdown, I, RSB_GEMM_REVERSED, l.ln2)) != RSB_OK) return rc;
     }
     return RSB_OK;
 }
@@ -1217,21 +1080,23 @@ int trunk(rsb_llm* h, const int32_t* ids, const int32_t* cu_seqlens, int B, int 
     int rc;
     if ((rc = upload_attention_items(cu, B, d_items, st, &f.n_items)) != RSB_OK) return rc;
     embed_rows_kernel<E><<<T, 128, 0, st>>>(ids, as<E>(h->embed), h->hidden, f.X);
-    if (h->neox) return neox_layers(h, f, st);
-    return h->olmo ? olmo_layers(h, f, st) : llama_layers(h, f, st);
+    return h->family == RSB_LLM_NEOX ? neox_layers(h, f, st) : sequential_layers(h, f, st);
 }
 
 // The final norm of the label rows X[rows[i]] into out[i], i < n.
 template <typename E>
 void final_norm(const rsb_llm* h, const E* X, const int* rows, int n, E* out, cudaStream_t st) {
-    if (h->neox || h->olmo == 1)                 // OLMo: unit scale (final_g) and zero shift
+    const bool neox = h->family == RSB_LLM_NEOX;
+    if (neox || h->family == RSB_LLM_OLMO)       // OLMo: unit scale (final_g) and zero shift
         ln_rows_kernel<E><<<n, LN_THREADS, 0, st>>>(const_cast<E*>(X), nullptr, rows, h->hidden, as<E>(h->final_g),
-                                                    as<E>(h->neox ? h->final_b : h->zero_bias), nullptr, nullptr, h->eps,
+                                                    as<E>(neox ? h->final_b : h->zero_bias), nullptr, nullptr, h->eps,
                                                     out, nullptr);
-    else if (h->olmo == 2)
-        rms_post_kernel<E><<<n, 256, 0, st>>>(const_cast<E*>(X), nullptr, rows, h->hidden, as<E>(h->final_g), h->eps, out);
+    else if (h->family == RSB_LLM_OLMO2)
+        rms_rows_kernel<E, true><<<n, 256, 0, st>>>(const_cast<E*>(X), nullptr, rows, h->hidden, as<E>(h->final_g), h->eps,
+                                                    out);
     else
-        rms_rows_kernel<E><<<n, 256, 0, st>>>(X, rows, h->hidden, as<E>(h->final_g), h->eps, out);
+        rms_rows_kernel<E, false><<<n, 256, 0, st>>>(const_cast<E*>(X), nullptr, rows, h->hidden, as<E>(h->final_g),
+                                                     h->eps, out);
 }
 
 }  // namespace
@@ -1319,7 +1184,7 @@ extern "C" int rsb_llm_attention(rsb_llm_t* h, void* qkv, const int32_t* cu_seql
     if (B <= 0 || T <= 0) return lfail(RSB_ERR_INVALID, "empty batch");
     if (max_seqlen > h->max_pos)
         return lfail(RSB_ERR_UNSUPPORTED, "sequence longer than max_position_embeddings (%ld)", (long)h->max_pos);
-    if (h->olmo == 2 && !(h->loaded.count("model.layers.0.self_attn.q_norm.weight") &&
+    if (h->family == RSB_LLM_OLMO2 && !(h->loaded.count("model.layers.0.self_attn.q_norm.weight") &&
                           h->loaded.count("model.layers.0.self_attn.k_norm.weight")))
         return lfail(RSB_ERR_STATE, "layer 0's self_attn.q_norm / k_norm weights are not loaded");
     cudaStream_t st = (cudaStream_t)stream;
@@ -1368,7 +1233,7 @@ extern "C" int rsb_llm_layernorm(int hidden, float eps, void* x, const void* add
     return RSB_OK;
 }
 
-// Diagnostic: rms_post_kernel, OLMo-2's post-norm residual add and final norm, on a caller's rows (rsb.h).
+// Diagnostic: rms_rows_kernel in OLMo-2's order, the post-norm residual add and final norm, on a caller's rows (rsb.h).
 extern "C" int rsb_llm_olmo2_norm(int hidden, float eps, void* x, const void* a, const int32_t* rows, int n_rows,
                                   const void* w, void* out, rsb_stream_t stream) {
     if (!x || !w || (!a && !out)) return lfail(RSB_ERR_INVALID, "null argument (x, w, or out without a)");
@@ -1376,9 +1241,9 @@ extern "C" int rsb_llm_olmo2_norm(int hidden, float eps, void* x, const void* a,
     if (hidden <= 0 || hidden % 8)
         return lfail(RSB_ERR_UNSUPPORTED, "hidden %ld: the RMSNorm kernel takes positive multiples of 8", (long)hidden);
     if (n_rows == 0) return RSB_OK;
-    rms_post_kernel<__half><<<n_rows, 256, 0, (cudaStream_t)stream>>>(static_cast<__half*>(x), static_cast<const __half*>(a),
-                                                              rows, hidden, static_cast<const __half*>(w), eps,
-                                                              static_cast<__half*>(out));
+    rms_rows_kernel<__half, true><<<n_rows, 256, 0, (cudaStream_t)stream>>>(
+        static_cast<__half*>(x), static_cast<const __half*>(a), rows, hidden, static_cast<const __half*>(w), eps,
+        static_cast<__half*>(out));
     const cudaError_t e = cudaPeekAtLastError();
     if (e != cudaSuccess) return lfail(RSB_ERR_CUDA, "rmsnorm launch failed: %s", cudaGetErrorString(e));
     return RSB_OK;

@@ -37,6 +37,31 @@ def _get(cfg, key, default=None):
     return getattr(cfg, key, default)
 
 
+def _refuse(msg):
+    raise AttributeError(msg)
+
+
+def _rope_parameters(cfg, refuse, **fields):
+    """`fields` (rope_parameters key -> value read outside it) as the config gives them: transformers >= 5 folds them
+    and rope_scaling into rope_parameters.  Anything but the default RoPE is refused."""
+    rp = _get(cfg, "rope_parameters")
+    if isinstance(rp, dict):
+        if rp.get("rope_type", "default") != "default":
+            refuse(f"rope_parameters {rp}: only the default RoPE is implemented (rope_scaling null)")
+        fields = {k: rp.get(k, v) for k, v in fields.items()}
+    if _get(cfg, "rope_scaling") is not None and not (isinstance(rp, dict) and _get(cfg, "rope_scaling") == rp):
+        refuse(f"rope_scaling {_get(cfg, 'rope_scaling')}: only rope_scaling null is implemented")
+    return fields
+
+
+def _positive_sizes(cfg, refuse, *keys):
+    """The values of `keys`, each refused unless a positive size."""
+    for key in keys:
+        if not _get(cfg, key) or _get(cfg, key) <= 0:
+            refuse(f"{key} {_get(cfg, key)} is not a positive size")
+    return [_get(cfg, key) for key in keys]
+
+
 def llama_geometry(cfg) -> dict:
     """The reader geometry the kernels run, from an HF config (dict or object), or AttributeError naming the field."""
     mt = _get(cfg, "model_type")
@@ -60,17 +85,8 @@ def llama_geometry(cfg) -> dict:
     for key in ("attention_bias", "mlp_bias"):
         if _get(cfg, key, False):
             raise AttributeError(f"{key} is set: only bias-free Llama layers are implemented")
-    theta = _get(cfg, "rope_theta")
-    rp = _get(cfg, "rope_parameters")
-    if isinstance(rp, dict):                     # transformers >= 5 folds rope_theta / rope_scaling into rope_parameters
-        if rp.get("rope_type", "default") != "default":
-            raise AttributeError(f"rope_parameters {rp}: only the default RoPE is implemented (rope_scaling null)")
-        theta = rp.get("rope_theta", theta)
-    if _get(cfg, "rope_scaling") is not None and not (isinstance(rp, dict) and _get(cfg, "rope_scaling") == rp):
-        raise AttributeError(f"rope_scaling {_get(cfg, 'rope_scaling')}: only rope_scaling null is implemented")
-    vocab = _get(cfg, "vocab_size")
-    if not vocab or vocab <= 0:
-        raise AttributeError(f"vocab_size {vocab} is not a positive size")
+    theta = _rope_parameters(cfg, _refuse, rope_theta=_get(cfg, "rope_theta"))["rope_theta"]
+    vocab, = _positive_sizes(cfg, _refuse, "vocab_size")
     return dict(num_hidden_layers=_get(cfg, "num_hidden_layers"), hidden_size=hidden, num_attention_heads=heads,
                 num_key_value_heads=kv, intermediate_size=inter, vocab_size=vocab,
                 max_position_embeddings=_get(cfg, "max_position_embeddings", 2048),
@@ -107,14 +123,9 @@ def neox_geometry(cfg) -> dict:
     inter = _get(cfg, "intermediate_size")
     if hidden % 128 or not inter or inter % 128:
         refuse(f"hidden_size {hidden} / intermediate_size {inter}: both must be multiples of 128")
-    pct, base = _get(cfg, "rotary_pct", 0.25), _get(cfg, "rotary_emb_base", 10000.0)
-    rp = _get(cfg, "rope_parameters")
-    if isinstance(rp, dict):                     # transformers >= 5: rope_parameters carries the factor and the base
-        if rp.get("rope_type", "default") != "default":
-            refuse(f"rope_parameters {rp}: only the default RoPE is implemented")
-        pct, base = rp.get("partial_rotary_factor", pct), rp.get("rope_theta", base)
-    if _get(cfg, "rope_scaling") is not None and not (isinstance(rp, dict) and _get(cfg, "rope_scaling") == rp):
-        refuse(f"rope_scaling {_get(cfg, 'rope_scaling')}: only rope_scaling null is implemented")
+    rope = _rope_parameters(cfg, refuse, partial_rotary_factor=_get(cfg, "rotary_pct", 0.25),
+                            rope_theta=_get(cfg, "rotary_emb_base", 10000.0))
+    pct, base = rope["partial_rotary_factor"], rope["rope_theta"]
     rot = int(head_dim * pct)
     if rot <= 0 or rot % 2 or rot > head_dim:
         refuse(f"rotary_ndims {rot} (rotary_pct {pct} x head_dim {head_dim}) must be even and in [2, head_dim]")
@@ -123,12 +134,7 @@ def neox_geometry(cfg) -> dict:
     for key, want in (("use_parallel_residual", True), ("attention_bias", True), ("tie_word_embeddings", False)):
         if bool(_get(cfg, key, want)) != want:
             refuse(f"{key} {_get(cfg, key)}: only {key} {want} (every Pythia model) is implemented")
-    vocab = _get(cfg, "vocab_size")
-    if not vocab or vocab <= 0:
-        refuse(f"vocab_size {vocab} is not a positive size")
-    layers = _get(cfg, "num_hidden_layers")
-    if not layers or layers <= 0:
-        refuse(f"num_hidden_layers {layers} is not a positive size")
+    vocab, layers = _positive_sizes(cfg, refuse, "vocab_size", "num_hidden_layers")
     return dict(num_hidden_layers=layers, hidden_size=hidden, num_attention_heads=heads, head_dim=head_dim,
                 intermediate_size=inter, vocab_size=vocab, max_position_embeddings=_get(cfg, "max_position_embeddings", 2048),
                 rotary_ndims=rot, rotary_emb_base=float(base), layer_norm_eps=float(_get(cfg, "layer_norm_eps", 1e-5)))
@@ -176,26 +182,14 @@ def olmo_geometry(cfg) -> dict:
         refuse(f"intermediate_size {inter}: must be a positive multiple of 128 (hidden_size {hidden} is)")
     if mt == "olmo" and hidden > OLMO_MAX_HIDDEN:
         refuse(f"hidden_size {hidden}: the LayerNorm kernel holds rows of at most {OLMO_MAX_HIDDEN}")
-    theta = _get(cfg, "rope_theta")
-    rp = _get(cfg, "rope_parameters")
-    if isinstance(rp, dict):                     # transformers >= 5 folds rope_theta / rope_scaling into rope_parameters
-        if rp.get("rope_type", "default") != "default":
-            refuse(f"rope_parameters {rp}: only the default RoPE is implemented (rope_scaling null)")
-        theta = rp.get("rope_theta", theta)
-    if _get(cfg, "rope_scaling") is not None and not (isinstance(rp, dict) and _get(cfg, "rope_scaling") == rp):
-        refuse(f"rope_scaling {_get(cfg, 'rope_scaling')}: only rope_scaling null is implemented")
+    theta = _rope_parameters(cfg, refuse, rope_theta=_get(cfg, "rope_theta"))["rope_theta"]
     theta = float(theta if theta is not None else 10000.0)
     if not theta > 0:
         refuse(f"rope_theta {theta} is not positive")
     clip = _get(cfg, "clip_qkv") if mt == "olmo" else None   # Olmo2ForCausalLM never reads clip_qkv
     if clip is not None and not clip > 0:
         refuse(f"clip_qkv {clip}: must be null or positive")
-    vocab = _get(cfg, "vocab_size")
-    if not vocab or vocab <= 0:
-        refuse(f"vocab_size {vocab} is not a positive size")
-    layers = _get(cfg, "num_hidden_layers")
-    if not layers or layers <= 0:
-        refuse(f"num_hidden_layers {layers} is not a positive size")
+    vocab, layers = _positive_sizes(cfg, refuse, "vocab_size", "num_hidden_layers")
     # OlmoLayerNorm's eps is 1e-5 in the model code; OLMo-2 reads rms_norm_eps
     eps = 1e-5 if mt == "olmo" else float(_get(cfg, "rms_norm_eps", 1e-5))
     return dict(version=1 if mt == "olmo" else 2, num_hidden_layers=layers, hidden_size=hidden,
@@ -251,7 +245,7 @@ def scored_positions(labels: Sequence[int]) -> List[int]:
 
 
 class _Reader:
-    """A causal-LM reader on librsb (`rsb_llm_*`): everything but the geometry and the constructor call."""
+    """A causal-LM reader on librsb (`rsb_llm_*`): everything but the geometry and the constructor's arguments."""
 
     # tokens per forward that `nll` packs: the GEMMs fill the GPU well before this, and the activations of a
     # Llama-3-8B forward stay near 3 GB
@@ -271,8 +265,10 @@ class _Reader:
         self.loaded = set()
         with torch.cuda.device(self.device):
             self._check(self._create(self.geom))
-            if self.dtype == torch.bfloat16:
-                self._check(self.L.rsb_llm_set_dtype(self._h, _lib.RSB_DTYPE_BF16))
+
+    def _create(self, g):
+        dtype = _lib.RSB_DTYPE_BF16 if self.dtype == torch.bfloat16 else _lib.RSB_DTYPE_F16
+        return self.L.rsb_llm_create(self.family, dtype, *self._create_args(g), ctypes.byref(self._h))
 
     def _check(self, rc):
         if rc == _lib.RSB_OK:
@@ -435,42 +431,44 @@ class B200Llama(_Reader):
 
     _geometry = staticmethod(llama_geometry)
     _expected_keys = staticmethod(expected_keys)
+    family = _lib.RSB_LLM_LLAMA
 
-    def _create(self, g):
-        return self.L.rsb_llm_create(
-            g["num_hidden_layers"], g["hidden_size"], g["num_attention_heads"], g["num_key_value_heads"],
-            g["intermediate_size"], g["vocab_size"], g["max_position_embeddings"], ctypes.c_float(g["rope_theta"]),
-            ctypes.c_float(g["rms_norm_eps"]), int(g["tie_word_embeddings"]), ctypes.byref(self._h))
+    def _create_args(self, g):                   # rsb_llm_create's arguments after family and dtype
+        return (g["num_hidden_layers"], g["hidden_size"], g["num_attention_heads"], g["num_key_value_heads"],
+                g["intermediate_size"], g["vocab_size"], g["max_position_embeddings"], 128, g["rope_theta"],
+                g["rms_norm_eps"], 0.0, int(g["tie_word_embeddings"]))
 
 
 class B200NeoX(_Reader):
-    """An HF GPTNeoXForCausalLM reader (Pythia) on librsb (`rsb_llm_create_neox`, then the same `rsb_llm_*`)."""
+    """An HF GPTNeoXForCausalLM reader (Pythia) on librsb (`rsb_llm_*`)."""
 
     _geometry = staticmethod(neox_geometry)
     _expected_keys = staticmethod(neox_expected_keys)
+    family = _lib.RSB_LLM_NEOX
     # older checkpoints also carry the causal mask (a 2048 x 2048 bool) and the masked-score constant
     _buffers = ("rotary_emb.inv_freq", ".attention.bias", ".attention.masked_bias")
 
-    def _create(self, g):
-        return self.L.rsb_llm_create_neox(
-            g["num_hidden_layers"], g["hidden_size"], g["num_attention_heads"], g["intermediate_size"],
-            g["vocab_size"], g["max_position_embeddings"], g["rotary_ndims"], ctypes.c_float(g["rotary_emb_base"]),
-            ctypes.c_float(g["layer_norm_eps"]), ctypes.byref(self._h))
+    def _create_args(self, g):
+        return (g["num_hidden_layers"], g["hidden_size"], g["num_attention_heads"], g["num_attention_heads"],
+                g["intermediate_size"], g["vocab_size"], g["max_position_embeddings"], g["rotary_ndims"],
+                g["rotary_emb_base"], g["layer_norm_eps"], 0.0, 0)
 
 
 class B200Olmo(_Reader):
-    """An HF OlmoForCausalLM / Olmo2ForCausalLM reader on librsb (`rsb_llm_create_olmo`, then the same `rsb_llm_*`).
-    Diagnostics: `attention` runs layer 0's clip_qkv / QK-norm prologue in place of RoPE, then the same attention."""
+    """An HF OlmoForCausalLM / Olmo2ForCausalLM reader on librsb (`rsb_llm_*`).  Diagnostics: `attention` runs layer
+    0's clip_qkv / QK-norm prologue in place of RoPE, then the same attention."""
 
     _geometry = staticmethod(olmo_geometry)
     _expected_keys = staticmethod(olmo_expected_keys)
 
-    def _create(self, g):
-        return self.L.rsb_llm_create_olmo(
-            g["version"], g["num_hidden_layers"], g["hidden_size"], g["num_attention_heads"],
-            g["num_key_value_heads"], g["intermediate_size"], g["vocab_size"], g["max_position_embeddings"],
-            ctypes.c_float(g["rope_theta"]), ctypes.c_float(g["eps"]), ctypes.c_float(g["clip_qkv"]),
-            int(g["tie_word_embeddings"]), ctypes.byref(self._h))
+    @property
+    def family(self):
+        return _lib.RSB_LLM_OLMO if self.geom["version"] == 1 else _lib.RSB_LLM_OLMO2
+
+    def _create_args(self, g):
+        return (g["num_hidden_layers"], g["hidden_size"], g["num_attention_heads"], g["num_key_value_heads"],
+                g["intermediate_size"], g["vocab_size"], g["max_position_embeddings"], 128, g["rope_theta"], g["eps"],
+                g["clip_qkv"], int(g["tie_word_embeddings"]))
 
 
 READERS = {"llama": (llama_geometry, B200Llama), "gpt_neox": (neox_geometry, B200NeoX),

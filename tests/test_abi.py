@@ -13,7 +13,7 @@ from retrieval_scaling_b200 import _lib
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def test_header_ctypes_table_exports_and_version_300_agree():
+def test_header_ctypes_table_exports_and_version_301_agree():
     L = _lib.lib()
     header = open(os.path.join(ROOT, "include", "rsb.h")).read()
     header = re.sub(r"/\*.*?\*/", "", header, flags=re.S)
@@ -23,7 +23,7 @@ def test_header_ctypes_table_exports_and_version_300_agree():
     assert declared == bound, f"header vs ctypes table mismatch: {declared ^ bound}"
     for name in declared:
         assert hasattr(L, name), f"librsb.so does not export {name}"
-    assert L.rsb_version() == 300
+    assert L.rsb_version() == 301
 
 
 def test_create_refusals_are_reported_not_fatal():

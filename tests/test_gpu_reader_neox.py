@@ -1,4 +1,4 @@
-"""GPU checks of the GPT-NeoX reader (rsb_llm_create_neox, then rsb_llm_*): per-token NLL against the committed fp64
+"""GPU checks of the GPT-NeoX reader (rsb_llm_create, then rsb_llm_*): per-token NLL against the committed fp64
 golden held to HF bf16's own error, label masks, packing and determinism, partial RoPE bit for bit, causal attention
 per element at head_dim 64 / 80 / 128 / 256, production widths against transformers, pickle loading and the overflow
 check.  Every per-element comparison also has to reject a deliberately wrong reference."""

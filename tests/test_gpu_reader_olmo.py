@@ -1,4 +1,4 @@
-"""GPU checks of the OLMo / OLMo-2 reader (rsb_llm_create_olmo, then rsb_llm_*): per-token NLL against the committed
+"""GPU checks of the OLMo / OLMo-2 reader (rsb_llm_create, then rsb_llm_*): per-token NLL against the committed
 fp64 golden held to HF bf16's own error, packing and determinism, the attention prologue (clip_qkv clamp, whole-
 projection QK-norm, fp32-cos / sin RoPE) per element, the two norms per element, production widths against
 transformers, the refusals, the overflow check and `main_ric.py` end to end.  Every per-element comparison also has

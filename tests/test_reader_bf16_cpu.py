@@ -1,6 +1,7 @@
 """bf16 readers, host side: the dtype argument of `load_reader` / `_Reader` and the `model.lm_dtype` key, each refused
-before any weight file is opened or device memory allocated; `rsb_llm_set_dtype`'s refusals without a handle; the index
-creators' refusal of RSB_DTYPE_BF16; and `main_ric.py`'s plumbing of `+model.lm_dtype=bfloat16` to `load_reader`."""
+before any weight file is opened or device memory allocated; `rsb_llm_create`'s dtype refusals before any CUDA call;
+the index creators' refusal of RSB_DTYPE_BF16; and `main_ric.py`'s plumbing of `+model.lm_dtype=bfloat16` to
+`load_reader`."""
 import ctypes
 import importlib.util
 import json
@@ -69,9 +70,15 @@ def test_reader_constructor_refuses_a_dtype_first(monkeypatch, cls, cfg):
         cls(dict(cfg, model_type="bert"), dtype="float64")
 
 
-def test_set_dtype_refusals_without_a_handle():
+def test_create_dtype_refusals_before_any_cuda_call():
     L = _lib.lib()
-    assert L.rsb_llm_set_dtype(None, _lib.RSB_DTYPE_BF16) == _lib.RSB_ERR_INVALID
+    h = ctypes.c_void_p(0)
+    geometry = (2, 512, 4, 1, 1024, 1000, 4096, 128, ctypes.c_float(1e4), ctypes.c_float(1e-5), ctypes.c_float(0.0), 0)
+    for dtype in (7, _lib.RSB_DTYPE_F32):
+        for out in (None, ctypes.byref(h)):
+            assert L.rsb_llm_create(_lib.RSB_LLM_LLAMA, dtype, *geometry, out) == _lib.RSB_ERR_INVALID
+        assert b"dtype" in L.rsb_llm_last_error()
+        assert h.value is None
     assert _lib.RSB_DTYPE_BF16 == 3
 
 

@@ -145,20 +145,25 @@ def test_llm_abi_refusals_need_no_device():
     header = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "rsb.h")).read(), flags=re.S)
     decl = re.search(r"int\s+rsb_llm_create\s*\(([^)]*)\)", header).group(1)
     assert [p.split()[-1] for p in decl.split(",")][:-1] == [
-        "layers", "hidden", "heads", "kv_heads", "intermediate", "vocab", "max_pos", "rope_theta", "rms_eps", "tied"]
+        "family", "dtype", "layers", "hidden", "heads", "kv_heads", "intermediate", "vocab", "max_pos", "rotary_dims",
+        "rope_theta", "eps", "clip_qkv", "tied"]
     L = _lib.lib()
     h = ctypes.c_void_p(0)
     f = ctypes.c_float
-    ok = (2, 512, 4, 1, 1024, 1000, 4096, f(1e4), f(1e-5), 0)
+    LL, z = (_lib.RSB_LLM_LLAMA, _lib.RSB_DTYPE_F16), f(0.0)
+    ok = (*LL, 2, 512, 4, 1, 1024, 1000, 4096, 128, f(1e4), f(1e-5), z, 0)
     assert L.rsb_llm_create(*ok, None) == _lib.RSB_ERR_INVALID
     bad = [
-        ((2, 512, 8, 1, 1024, 1000, 4096, f(1e4), f(1e-5), 0), _lib.RSB_ERR_UNSUPPORTED, b"head_dim"),      # head_dim 64
-        ((2, 512, 4, 3, 1024, 1000, 4096, f(1e4), f(1e-5), 0), _lib.RSB_ERR_UNSUPPORTED, b"num_key_value_heads"),
-        ((2, 512, 4, 1, 1000, 1000, 4096, f(1e4), f(1e-5), 0), _lib.RSB_ERR_UNSUPPORTED, b"intermediate_size"),
-        ((0, 512, 4, 1, 1024, 1000, 4096, f(1e4), f(1e-5), 0), _lib.RSB_ERR_INVALID, b"positive"),
-        ((2, 512, 4, 1, 1024, 0, 4096, f(1e4), f(1e-5), 0), _lib.RSB_ERR_INVALID, b"positive"),
-        ((2, 512, 4, 1, 1024, 1000, 4096, f(0.0), f(1e-5), 0), _lib.RSB_ERR_INVALID, b"rope_theta"),
-        ((2, 512, 4, 1, 1024, 1000, 4096, f(1e4), f(1e-5), 2), _lib.RSB_ERR_INVALID, b"tied"),
+        ((*LL, 2, 512, 8, 1, 1024, 1000, 4096, 128, f(1e4), f(1e-5), z, 0), _lib.RSB_ERR_UNSUPPORTED, b"head_dim"),   # 64
+        ((*LL, 2, 512, 4, 3, 1024, 1000, 4096, 128, f(1e4), f(1e-5), z, 0), _lib.RSB_ERR_UNSUPPORTED, b"num_key_value_heads"),
+        ((*LL, 2, 512, 4, 1, 1000, 1000, 4096, 128, f(1e4), f(1e-5), z, 0), _lib.RSB_ERR_UNSUPPORTED, b"intermediate_size"),
+        ((*LL, 0, 512, 4, 1, 1024, 1000, 4096, 128, f(1e4), f(1e-5), z, 0), _lib.RSB_ERR_INVALID, b"positive"),
+        ((*LL, 2, 512, 4, 1, 1024, 0, 4096, 128, f(1e4), f(1e-5), z, 0), _lib.RSB_ERR_INVALID, b"positive"),
+        ((*LL, 2, 512, 4, 1, 1024, 1000, 4096, 128, f(0.0), f(1e-5), z, 0), _lib.RSB_ERR_INVALID, b"rope_theta"),
+        ((*LL, 2, 512, 4, 1, 1024, 1000, 4096, 128, f(1e4), f(1e-5), z, 2), _lib.RSB_ERR_INVALID, b"tied"),
+        # combinations only the one constructor can express
+        ((*LL, 2, 512, 4, 1, 1024, 1000, 4096, 64, f(1e4), f(1e-5), z, 0), _lib.RSB_ERR_INVALID, b"rotary_dims"),
+        ((*LL, 2, 512, 4, 1, 1024, 1000, 4096, 128, f(1e4), f(1e-5), f(8.0), 0), _lib.RSB_ERR_INVALID, b"clip_qkv"),
     ]
     for args, rc, msg in bad:
         assert L.rsb_llm_create(*args, ctypes.byref(h)) == rc, args

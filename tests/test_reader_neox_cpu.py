@@ -148,30 +148,37 @@ def test_neox_abi_refusals_need_no_device():
     import re
     from retrieval_scaling_b200 import _lib
     header = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "rsb.h")).read(), flags=re.S)
-    decl = re.search(r"int\s+rsb_llm_create_neox\s*\(([^)]*)\)", header).group(1)
+    decl = re.search(r"int\s+rsb_llm_create\s*\(([^)]*)\)", header).group(1)
     assert [p.split()[-1] for p in decl.split(",")][:-1] == [
-        "layers", "hidden", "heads", "intermediate", "vocab", "max_pos", "rotary_dims", "rotary_base", "ln_eps"]
+        "family", "dtype", "layers", "hidden", "heads", "kv_heads", "intermediate", "vocab", "max_pos", "rotary_dims",
+        "rope_theta", "eps", "clip_qkv", "tied"]
     L = _lib.lib()
     h = ctypes.c_void_p(0)
     f = ctypes.c_float
-    assert L.rsb_llm_create_neox(2, 512, 2, 2048, 1000, 2048, 64, f(1e4), f(1e-5), None) == _lib.RSB_ERR_INVALID
+    NX, z = (_lib.RSB_LLM_NEOX, _lib.RSB_DTYPE_F16), f(0.0)
+    ok = (*NX, 2, 512, 2, 2, 2048, 1000, 2048, 64, f(1e4), f(1e-5), z, 0)
+    assert L.rsb_llm_create(*ok, None) == _lib.RSB_ERR_INVALID
     bad = [
-        ((2, 6144, 64, 24576, 1000, 2048, 24, f(1e4), f(1e-5)), _lib.RSB_ERR_UNSUPPORTED, b"head_dim"),   # 96
-        ((2, 512, 3, 2048, 1000, 2048, 64, f(1e4), f(1e-5)), _lib.RSB_ERR_UNSUPPORTED, b"head_dim"),
-        ((2, 512, 1, 2048, 1000, 2048, 64, f(1e4), f(1e-5)), _lib.RSB_ERR_UNSUPPORTED, b"head_dim"),     # 512
-        ((2, 512, 2, 2048, 1000, 2048, 63, f(1e4), f(1e-5)), _lib.RSB_ERR_UNSUPPORTED, b"rotary"),
-        ((2, 512, 2, 2048, 1000, 2048, 0, f(1e4), f(1e-5)), _lib.RSB_ERR_INVALID, b"rotary"),
-        ((2, 512, 2, 2048, 1000, 2048, 258, f(1e4), f(1e-5)), _lib.RSB_ERR_INVALID, b"rotary"),
-        ((2, 512, 2, 2000, 1000, 2048, 64, f(1e4), f(1e-5)), _lib.RSB_ERR_UNSUPPORTED, b"intermediate"),
-        ((2, 10240, 40, 40960, 1000, 2048, 64, f(1e4), f(1e-5)), _lib.RSB_ERR_UNSUPPORTED, b"hidden"),
-        ((2, 10240, 80, 40960, 1000, 2048, 32, f(1e4), f(1e-5)), _lib.RSB_ERR_UNSUPPORTED, b"hidden"),
-        ((0, 512, 2, 2048, 1000, 2048, 64, f(1e4), f(1e-5)), _lib.RSB_ERR_INVALID, b"positive"),
-        ((2, 512, 2, 2048, 0, 2048, 64, f(1e4), f(1e-5)), _lib.RSB_ERR_INVALID, b"positive"),
-        ((2, 512, 2, 2048, 1000, 2048, 64, f(0.0), f(1e-5)), _lib.RSB_ERR_INVALID, b"rotary_base"),
-        ((2, 512, 2, 2048, 1000, 2048, 64, f(1e4), f(0.0)), _lib.RSB_ERR_INVALID, b"ln_eps"),
+        ((*NX, 2, 6144, 64, 64, 24576, 1000, 2048, 24, f(1e4), f(1e-5), z, 0), _lib.RSB_ERR_UNSUPPORTED, b"head_dim"),   # 96
+        ((*NX, 2, 512, 3, 3, 2048, 1000, 2048, 64, f(1e4), f(1e-5), z, 0), _lib.RSB_ERR_UNSUPPORTED, b"head_dim"),
+        ((*NX, 2, 512, 1, 1, 2048, 1000, 2048, 64, f(1e4), f(1e-5), z, 0), _lib.RSB_ERR_UNSUPPORTED, b"head_dim"),     # 512
+        ((*NX, 2, 512, 2, 2, 2048, 1000, 2048, 63, f(1e4), f(1e-5), z, 0), _lib.RSB_ERR_UNSUPPORTED, b"rotary"),
+        ((*NX, 2, 512, 2, 2, 2048, 1000, 2048, 0, f(1e4), f(1e-5), z, 0), _lib.RSB_ERR_INVALID, b"rotary"),
+        ((*NX, 2, 512, 2, 2, 2048, 1000, 2048, 258, f(1e4), f(1e-5), z, 0), _lib.RSB_ERR_INVALID, b"rotary"),
+        ((*NX, 2, 512, 2, 2, 2000, 1000, 2048, 64, f(1e4), f(1e-5), z, 0), _lib.RSB_ERR_UNSUPPORTED, b"intermediate"),
+        ((*NX, 2, 10240, 40, 40, 40960, 1000, 2048, 64, f(1e4), f(1e-5), z, 0), _lib.RSB_ERR_UNSUPPORTED, b"hidden"),
+        ((*NX, 2, 10240, 80, 80, 40960, 1000, 2048, 32, f(1e4), f(1e-5), z, 0), _lib.RSB_ERR_UNSUPPORTED, b"hidden"),
+        ((*NX, 0, 512, 2, 2, 2048, 1000, 2048, 64, f(1e4), f(1e-5), z, 0), _lib.RSB_ERR_INVALID, b"positive"),
+        ((*NX, 2, 512, 2, 2, 2048, 0, 2048, 64, f(1e4), f(1e-5), z, 0), _lib.RSB_ERR_INVALID, b"positive"),
+        ((*NX, 2, 512, 2, 2, 2048, 1000, 2048, 64, f(0.0), f(1e-5), z, 0), _lib.RSB_ERR_INVALID, b"rotary_base"),
+        ((*NX, 2, 512, 2, 2, 2048, 1000, 2048, 64, f(1e4), f(0.0), z, 0), _lib.RSB_ERR_INVALID, b"ln_eps"),
+        # combinations only the one constructor can express
+        ((*NX, 2, 512, 2, 1, 2048, 1000, 2048, 64, f(1e4), f(1e-5), z, 0), _lib.RSB_ERR_UNSUPPORTED, b"kv_heads"),
+        ((*ok[:-1], 1), _lib.RSB_ERR_UNSUPPORTED, b"tied"),
+        ((*ok[:-2], f(8.0), 0), _lib.RSB_ERR_INVALID, b"clip_qkv"),
     ]
     for args, rc, msg in bad:
-        assert L.rsb_llm_create_neox(*args, ctypes.byref(h)) == rc, args
+        assert L.rsb_llm_create(*args, ctypes.byref(h)) == rc, args
         assert msg in L.rsb_llm_last_error(), (args, L.rsb_llm_last_error())
         assert h.value is None
     # the LayerNorm diagnostic: refused before any launch (the pointers are never dereferenced)

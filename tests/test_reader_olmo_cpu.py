@@ -165,33 +165,39 @@ def test_olmo_abi_refusals_need_no_device():
     import re
     from retrieval_scaling_b200 import _lib
     header = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "rsb.h")).read(), flags=re.S)
-    decl = re.search(r"int\s+rsb_llm_create_olmo\s*\(([^)]*)\)", header).group(1)
+    decl = re.search(r"int\s+rsb_llm_create\s*\(([^)]*)\)", header).group(1)
     assert [p.split()[-1] for p in decl.split(",")][:-1] == [
-        "version", "layers", "hidden", "heads", "kv_heads", "intermediate", "vocab", "max_pos", "rope_theta", "eps",
-        "clip_qkv", "tied"]
+        "family", "dtype", "layers", "hidden", "heads", "kv_heads", "intermediate", "vocab", "max_pos", "rotary_dims",
+        "rope_theta", "eps", "clip_qkv", "tied"]
     L = _lib.lib()
     h = ctypes.c_void_p(0)
     f = ctypes.c_float
-    ok = (2, 4096, 32, 32, 11008, 50304, 2048, f(1e4), f(1e-5))
-    assert L.rsb_llm_create_olmo(1, *ok, f(0.0), 0, None) == _lib.RSB_ERR_INVALID
+    F16 = _lib.RSB_DTYPE_F16
+    O1, O2 = (_lib.RSB_LLM_OLMO, F16), (_lib.RSB_LLM_OLMO2, F16)
+    ok = (2, 4096, 32, 32, 11008, 50304, 2048, 128, f(1e4), f(1e-5))
+    assert L.rsb_llm_create(*O1, *ok, f(0.0), 0, None) == _lib.RSB_ERR_INVALID
     bad = [
-        ((0, *ok, f(0.0), 0), _lib.RSB_ERR_INVALID, b"version"),
-        ((3, *ok, f(0.0), 0), _lib.RSB_ERR_INVALID, b"version"),
-        ((1, *ok, f(-1.0), 0), _lib.RSB_ERR_INVALID, b"clip_qkv"),
-        ((1, *ok, f(float("nan")), 0), _lib.RSB_ERR_INVALID, b"clip_qkv"),
-        ((1, *ok, f(float("inf")), 0), _lib.RSB_ERR_INVALID, b"clip_qkv"),
-        ((2, *ok, f(8.0), 0), _lib.RSB_ERR_INVALID, b"clip_qkv"),
-        ((1, 2, 10240, 80, 80, 11008, 50304, 2048, f(1e4), f(1e-5), f(0.0), 0), _lib.RSB_ERR_UNSUPPORTED, b"hidden"),
-        ((2, 2, 4000, 32, 32, 11008, 50304, 2048, f(1e4), f(1e-5), f(0.0), 0), _lib.RSB_ERR_UNSUPPORTED, b"head_dim"),
-        ((2, 2, 4096, 32, 3, 11008, 50304, 2048, f(1e4), f(1e-5), f(0.0), 0), _lib.RSB_ERR_UNSUPPORTED, b"num_key_value_heads"),
-        ((1, 2, 4096, 32, 32, 11000, 50304, 2048, f(1e4), f(1e-5), f(0.0), 0), _lib.RSB_ERR_UNSUPPORTED, b"intermediate"),
-        ((1, 0, 4096, 32, 32, 11008, 50304, 2048, f(1e4), f(1e-5), f(0.0), 0), _lib.RSB_ERR_INVALID, b"positive"),
-        ((2, 2, 4096, 32, 32, 11008, 0, 2048, f(1e4), f(1e-5), f(0.0), 0), _lib.RSB_ERR_INVALID, b"positive"),
-        ((2, *ok[:-1], f(0.0), f(0.0), 0), _lib.RSB_ERR_INVALID, b"positive"),
-        ((1, *ok, f(0.0), 2), _lib.RSB_ERR_INVALID, b"tied"),
+        ((-1, F16, *ok, f(0.0), 0), _lib.RSB_ERR_INVALID, b"family"),
+        ((4, F16, *ok, f(0.0), 0), _lib.RSB_ERR_INVALID, b"family"),
+        ((*O1, *ok, f(-1.0), 0), _lib.RSB_ERR_INVALID, b"clip_qkv"),
+        ((*O1, *ok, f(float("nan")), 0), _lib.RSB_ERR_INVALID, b"clip_qkv"),
+        ((*O1, *ok, f(float("inf")), 0), _lib.RSB_ERR_INVALID, b"clip_qkv"),
+        ((*O2, *ok, f(8.0), 0), _lib.RSB_ERR_INVALID, b"clip_qkv"),
+        ((*O1, 2, 10240, 80, 80, 11008, 50304, 2048, 128, f(1e4), f(1e-5), f(0.0), 0), _lib.RSB_ERR_UNSUPPORTED, b"hidden"),
+        ((*O2, 2, 4000, 32, 32, 11008, 50304, 2048, 128, f(1e4), f(1e-5), f(0.0), 0), _lib.RSB_ERR_UNSUPPORTED, b"head_dim"),
+        ((*O2, 2, 4096, 32, 3, 11008, 50304, 2048, 128, f(1e4), f(1e-5), f(0.0), 0), _lib.RSB_ERR_UNSUPPORTED,
+         b"num_key_value_heads"),
+        ((*O1, 2, 4096, 32, 32, 11000, 50304, 2048, 128, f(1e4), f(1e-5), f(0.0), 0), _lib.RSB_ERR_UNSUPPORTED,
+         b"intermediate"),
+        ((*O1, 0, 4096, 32, 32, 11008, 50304, 2048, 128, f(1e4), f(1e-5), f(0.0), 0), _lib.RSB_ERR_INVALID, b"positive"),
+        ((*O2, 2, 4096, 32, 32, 11008, 0, 2048, 128, f(1e4), f(1e-5), f(0.0), 0), _lib.RSB_ERR_INVALID, b"positive"),
+        ((*O2, *ok[:-1], f(0.0), f(0.0), 0), _lib.RSB_ERR_INVALID, b"positive"),
+        ((*O1, *ok, f(0.0), 2), _lib.RSB_ERR_INVALID, b"tied"),
+        # combinations only the one constructor can express
+        ((*O2, 2, 4096, 32, 32, 11008, 50304, 2048, 64, f(1e4), f(1e-5), f(0.0), 0), _lib.RSB_ERR_INVALID, b"rotary_dims"),
     ]
     for args, rc, msg in bad:
-        assert L.rsb_llm_create_olmo(*args, ctypes.byref(h)) == rc, args
+        assert L.rsb_llm_create(*args, ctypes.byref(h)) == rc, args
         assert msg in L.rsb_llm_last_error(), (args, L.rsb_llm_last_error())
         assert h.value is None
     # the OLMo-2 norm diagnostic: refused before any launch (the pointers are never dereferenced)
