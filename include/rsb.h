@@ -335,9 +335,10 @@ int rsb_pq_accumulate(const float* r_dev, int64_t n, int d, int M, int ksub, con
 
 /* ---- options -------------------------------------------------------------------------------------------- */
 enum {
-    RSB_OPT_COARSE_TENSOR = 0,/* 1 (default): coarse quantizer scores by 3xTF32 on wgmma tensor cores (fp32-equivalent
-                                 accuracy); 0: CUDA-core fp32 FMA tiles.  0 on an fp16 Flat index returns
-                                 RSB_ERR_UNSUPPORTED: its rows are scored on tensor cores only */
+    RSB_OPT_COARSE_TENSOR = 0,/* 1 (default): wgmma tensor-core candidates re-scored exactly in fp32 (coarse quantizer:
+                                 fp16 hi/lo split of queries and centroids; fp32 Flat: 3xTF32); 0: CUDA-core fp32
+                                 FMA tiles.  0 on an fp16 Flat index returns RSB_ERR_UNSUPPORTED: its rows are
+                                 scored on tensor cores only */
     RSB_OPT_BY_RESIDUAL = 1,  /* SQ8 IVFFLAT only (RSB_ERR_INVALID on other handles), before anything is added
                                  (RSB_ERR_STATE after): 1 encodes x - c_list and adds the coarse score (faiss by_residual,
                                  the default of index_factory "IVFn,SQ8"); 0 (default) encodes x */

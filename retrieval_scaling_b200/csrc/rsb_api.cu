@@ -95,7 +95,10 @@ struct rsb_index {
     float* centroids = nullptr;
     float* codebook = nullptr;
     float* codebook_t = nullptr;
-    float *cent_hi = nullptr, *cent_lo = nullptr;   // tf32 hi/lo split of the centroids (tensor-core coarse scan)
+    // fp16 hi/lo split of the centroids and their inverse row scales (launch_split_f16): the B operand of the
+    // tensor-core coarse scan, [nlist, d] fp16 each and [nlist] fp32
+    uint16_t *cent_hi = nullptr, *cent_lo = nullptr;
+    float* cent_inv = nullptr;
     bool coarse_tensor = true;
     float *flat_hi = nullptr, *flat_lo = nullptr;   // FLAT: tf32 hi/lo split of the database rows
     bool flat_tensor = true;
@@ -225,7 +228,7 @@ extern "C" int rsb_free(rsb_index_t* h) {
     for (auto& s : h->staging) free_segment(s);
     free_layout(h);
     cudaFree(h->centroids); cudaFree(h->codebook); cudaFree(h->codebook_t); cudaFree(h->prof_dev); cudaFree(h->sq);
-    cudaFree(h->cent_hi); cudaFree(h->cent_lo);
+    cudaFree(h->cent_hi); cudaFree(h->cent_lo); cudaFree(h->cent_inv);
     for (auto& set : h->evs) for (auto& e : set) if (e) cudaEventDestroy(e);
     free_tier(h->tier);
     delete h;
@@ -244,9 +247,10 @@ extern "C" int rsb_set_centroids(rsb_index_t* h, const float* c, rsb_stream_t st
     const size_t bytes = (size_t)h->nlist * h->d * 4;
     if (!h->centroids) CU(cudaMalloc(&h->centroids, bytes));
     CU(cudaMemcpyAsync(h->centroids, c, bytes, cudaMemcpyDeviceToDevice, st));
-    if (!h->cent_hi) CU(cudaMalloc(&h->cent_hi, bytes));
-    if (!h->cent_lo) CU(cudaMalloc(&h->cent_lo, bytes));
-    launch_split_tf32(h->centroids, (size_t)h->nlist * h->d, h->cent_hi, h->cent_lo, st);
+    if (!h->cent_hi) CU(cudaMalloc(&h->cent_hi, bytes / 2));
+    if (!h->cent_lo) CU(cudaMalloc(&h->cent_lo, bytes / 2));
+    if (!h->cent_inv) CU(cudaMalloc(&h->cent_inv, (size_t)h->nlist * 4));
+    launch_split_f16(h->centroids, h->nlist, h->d, h->cent_hi, h->cent_lo, h->cent_inv, st);
     CHECK_LAUNCH();
     h->has_centroids = true;
     return RSB_OK;
@@ -339,16 +343,19 @@ static KnnPlan knn_plan(int nq, int64_t n, int k) {
     return p;
 }
 
-// optional tensor-core operands: database rows pre-split into tf32 hi/lo parts + scratch for the split queries.
-// f16: the database rows x are fp16 and are the B operand themselves (xh / xl unused); qh / ql hold the scaled fp16
-// query split and qinv [min(nq, qb)] the inverse scales (launch_split_f16).
+// optional tensor-core operands: database rows pre-split into hi/lo parts + scratch for the split queries.
+//   tf32 (f16 false, xinv null): xh / xl the tf32 split of fp32 rows, qh / ql the tf32 query split;
+//   f16: the database rows x are fp16 and are the B operand themselves (xh / xl unused);
+//   xinv set: xh / xl the scaled fp16 split of fp32 rows and xinv [n] their inverse scales (launch_split_f16).
+// In both fp16 forms qh / ql hold the scaled fp16 query split and qinv [min(nq, qb)] the inverse scales.
 struct TensorOperands {
-    const float* xh;
-    const float* xl;
+    const void* xh;
+    const void* xl;
     float* qh;   // [min(nq, qb), d]
     float* ql;
     bool f16 = false;
     float* qinv = nullptr;
+    const float* xinv = nullptr;
 };
 
 // x: [n, d] fp32 rows, or fp16 rows when tc->f16
@@ -363,16 +370,26 @@ static int knn_ip_device(rsb_index* h, const float* q, int nq, const void* x, in
     float* S = reinterpret_cast<float*>(w + p.off_S);
     u64* keys = reinterpret_cast<u64*>(w + p.off_keys);
     int* cnt = reinterpret_cast<int*>(w + p.off_cnt);
-    const bool f16 = tc && tc->f16;
+    const bool f16 = tc && tc->f16;                   // fp16 rows
+    const bool h16 = tc && (tc->f16 || tc->xinv);     // fp16 operands on wgmma
     const int eb = f16 ? 2 : 4;
     const unsigned char* xb8 = static_cast<const unsigned char*>(x);
+    // the B operand of columns [c0, c0 + cols)
+    auto bh = [&](int64_t c0) -> const void* {
+        return f16 ? xb8 + (size_t)c0 * d * 2
+                   : static_cast<const unsigned char*>(tc->xh) + (size_t)c0 * d * (tc->xinv ? 2 : 4);
+    };
+    auto bl = [&](int64_t c0) -> const void* {
+        return f16 ? nullptr : static_cast<const unsigned char*>(tc->xl) + (size_t)c0 * d * (tc->xinv ? 2 : 4);
+    };
+    auto binv = [&](int64_t c0) -> const float* { return tc->xinv ? tc->xinv + c0 : nullptr; };
     for (int q0 = 0; q0 < nq; q0 += p.qb) {
         const int nb = std::min(p.qb, nq - q0);
         if (n == 0) {
             CU(cudaMemsetAsync(cnt, 0, (size_t)nb * p.items * 4, st));
         }
         if (tc && n > 0) {
-            if (f16) launch_split_f16(q + (size_t)q0 * d, nb, d, tc->qh, tc->ql, tc->qinv, st);
+            if (h16) launch_split_f16(q + (size_t)q0 * d, nb, d, tc->qh, tc->ql, tc->qinv, st);
             else launch_split_tf32(q + (size_t)q0 * d, (size_t)nb * d, tc->qh, tc->ql, st);
             if (h) h->launches += 1;
         }
@@ -392,10 +409,10 @@ static int knn_ip_device(rsb_index* h, const float* q, int nq, const void* x, in
                     unsigned* xb = reinterpret_cast<unsigned*>(w + p.off_S + align_up((size_t)nb * ncand * 8));
                     unsigned char* flags = w + p.off_S + align_up((size_t)nb * ncand * 8) + align_up((size_t)nb * nx * 4);
                     const bool scored =
-                        f16 ? launch_gemm_f16x2_topt(tc->qh, tc->ql, tc->qinv, nb, xb8 + (size_t)c0 * d * eb, cols, d, (unsigned)c0,
-                                                     cand, xb, st)
-                            : launch_gemm_tf32x3_topt(tc->qh, tc->ql, nb, tc->xh + (size_t)c0 * d, tc->xl + (size_t)c0 * d, cols,
-                                                      d, (unsigned)c0, cand, xb, st);
+                        h16 ? launch_gemm_f16_topt(tc->qh, tc->ql, tc->qinv, nb, bh(c0), bl(c0), binv(c0), cols, d,
+                                                   (unsigned)c0, cand, xb, st)
+                            : launch_gemm_tf32x3_topt(tc->qh, tc->ql, nb, static_cast<const float*>(bh(c0)),
+                                                      static_cast<const float*>(bl(c0)), cols, d, (unsigned)c0, cand, xb, st);
                     if (scored && launch_select_cands(cand, nb, (int)ncand, xb, (int)nx, k, keys, cnt, p.items, c, flags, st) == 0) {
                         launch_exact_rows(q + (size_t)q0 * d, nb, xb8 + (size_t)c0 * d * eb, eb, cols, d, (unsigned)c0, flags, k,
                                           keys, cnt, p.items, c, st);
@@ -404,12 +421,12 @@ static int knn_ip_device(rsb_index* h, const float* q, int nq, const void* x, in
                     }
                 }
             }
-            if (f16)  // fp16 rows: hi/lo query split on wgmma; there is no CUDA-core fp16 path
-                on_tensor = launch_gemm_f16x2(tc->qh, tc->ql, tc->qinv, nb, xb8 + (size_t)c0 * d * eb, cols, d, S, p.chunk, st);
+            if (h16)  // fp16 hi/lo query split on wgmma; there is no CUDA-core fp16 path
+                on_tensor = launch_gemm_f16(tc->qh, tc->ql, tc->qinv, nb, bh(c0), bl(c0), binv(c0), cols, d, S, p.chunk, st);
             else if (tc)  // 3xTF32 on wgmma (fp32-equivalent accuracy); CUDA-core fp32 tiles otherwise
-                on_tensor = launch_gemm_tf32x3(tc->qh, tc->ql, nb, tc->xh + (size_t)c0 * d, tc->xl + (size_t)c0 * d, cols, d,
-                                               S, p.chunk, st);
-            if (f16 && !on_tensor) return fail(RSB_ERR_CUDA, "the fp16 tensor-core scorer could not be set up (tensor map encoding failed)");
+                on_tensor = launch_gemm_tf32x3(tc->qh, tc->ql, nb, static_cast<const float*>(bh(c0)),
+                                               static_cast<const float*>(bl(c0)), cols, d, S, p.chunk, st);
+            if (h16 && !on_tensor) return fail(RSB_ERR_CUDA, "the fp16 tensor-core scorer could not be set up (tensor map encoding failed)");
             if (!on_tensor)
                 launch_sgemm_nt(q + (size_t)q0 * d, nb, static_cast<const float*>(x) + (size_t)c0 * d, cols, d, S, p.chunk, st);
             launch_select_rows(S, nb, cols, p.chunk, (unsigned)c0, k, p.nsplit, keys, cnt, p.items, c * p.nsplit, st);
@@ -1449,9 +1466,11 @@ static int coarse_impl(rsb_index* h, const float* q, int nq, const SearchPlan& p
     TensorOperands tc;
     const bool use_tc = h->coarse_tensor && h->cent_hi && h->cent_lo && (h->d % 32 == 0) && tf32_path_available();
     if (use_tc) {
-        tc.xh = h->cent_hi; tc.xl = h->cent_lo;
+        // [qb, d] fp16 hi, [qb, d] fp16 lo, [qb] fp32 inverse scales
+        tc.xh = h->cent_hi; tc.xl = h->cent_lo; tc.xinv = h->cent_inv;
         tc.qh = reinterpret_cast<float*>(w + p.off_qsplit);
-        tc.ql = tc.qh + (size_t)p.qb * h->d;
+        tc.ql = reinterpret_cast<float*>(reinterpret_cast<uint16_t*>(tc.qh) + (size_t)p.qb * h->d);
+        tc.qinv = reinterpret_cast<float*>(reinterpret_cast<uint16_t*>(tc.qh) + (size_t)2 * p.qb * h->d);
     }
     if (!use_tc)
         return knn_ip_device(h, q, nq, h->centroids, h->nlist, h->d, p.nprobe, nullptr, 0, cD, cI, w + p.off_coarse_ws,

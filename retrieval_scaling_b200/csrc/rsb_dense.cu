@@ -2,9 +2,10 @@
 // src/indicies/flat.py:139 and the IVF coarse quantizer inside ivf_flat.py:225 / ivf_pq.py:230) and the top-k
 // machinery shared by every index type.
 //
-//   sgemm_nt_kernel      S[nq, n] = Q[nq, d] . X[n, d]^T   fp32 FMA tiles on the CUDA cores (used when d % 32 != 0, for
-//                        rsb_add's list assignment, or when RSB_OPT_COARSE_TENSOR = 0; the default scorer is the
-//                        3xTF32 wgmma GEMM of rsb_tf32.cu followed by refine_exact_kernel below)
+//   sgemm_nt_kernel      S[nq, n] = Q[nq, d] . X[n, d]^T   fp32 FMA tiles on the CUDA cores (used when d % 32 != 0,
+//                        or when RSB_OPT_COARSE_TENSOR = 0; the default scorers are the wgmma GEMMs of rsb_tf32.cu --
+//                        fp16 hi/lo for the coarse quantizer, 3xTF32 for fp32 Flat rows -- followed by
+//                        refine_exact_kernel below)
 //   select_rows_kernel   per (row, column-split): thread-maxima prefilter + threshold-filtered candidate buffer
 //                        -> top-k keys
 //   merge_items_kernel   per query: merge the per-item key lists -> D (f32), I (i64)
@@ -252,7 +253,7 @@ void launch_select_rows(const float* S, int nrows, int ncols, int ld, unsigned c
 }
 
 // =============================================================================================================
-// Back end of the fused scorer (rsb_tf32.cu: gemm_tf32x3_topt_kernel).  One block per row: top-kc of the row's
+// Back end of the fused scorer (rsb_tf32.cu: gemm_ip_tc_kernel<F16, true>).  One block per row: top-kc of the row's
 // candidate keys (8 per 128-column half tile) with the thread-maxima prefilter, then the exactness check:
 // a dropped element is <= the largest "9th best of a half tile" X of the row, so the result is the row's true
 // top-kc iff the kc-th best candidate is strictly greater than X (or nothing was dropped: X == 0).  Rows that fail

@@ -139,15 +139,18 @@ void launch_exact_rows(const float* Q, int nrows, const void* X, int elem_bytes,
                        const unsigned char* flags, int kc, u64* out_keys, int* out_cnt, int items_per_row, int item,
                        cudaStream_t st);
 
-// ---- rsb_tf32.cu, fp16 form (Flat with fp16 storage): the database rows are the fp16 B operand as stored ------
-// queries [M, K] fp32 -> per row a power-of-two scale s (largest |element| * s in [2^14, 2^15)), hi = fp16(q s),
-// lo = fp16(q s - hi), inv = 1 / s
+// ---- rsb_tf32.cu, fp16 forms: Flat with fp16 storage (the database rows are the fp16 B operand as stored) and the
+// IVF coarse quantizer (the centroids split once, as the queries are) ------
+// rows [M, K] fp32 -> per row a power-of-two scale s (largest |element| * s in [2^14, 2^15)), hi = fp16(x s),
+// lo = fp16(x s - hi), inv = 1 / s
 void launch_split_f16(const float* q, int M, int K, void* hi, void* lo, float* inv, cudaStream_t st);
-// as launch_gemm_tf32x3 / _topt with S = (hi + lo) . B^T * inv[row]; B [N, K] fp16; K % 64 == 0
-bool launch_gemm_f16x2(const void* Ah, const void* Al, const float* inv, int M, const void* B, int N, int K, float* C,
-                       int ldc, cudaStream_t st);
-bool launch_gemm_f16x2_topt(const void* Ah, const void* Al, const float* inv, int M, const void* B, int N, int K,
-                            unsigned col_base, u64* cand, unsigned* xbound, cudaStream_t st);
+// as launch_gemm_tf32x3 / _topt with S = (Ah + Al) . B^T * inv[row] * inv_b[col]: B [N, K] fp16 rows as stored
+// (Bl = inv_b = nullptr, K % 64 == 0), or Bh + Bl with inv_b [N] from launch_split_f16 (K % 8 == 0)
+bool launch_gemm_f16(const void* Ah, const void* Al, const float* inv, int M, const void* Bh, const void* Bl,
+                     const float* inv_b, int N, int K, float* C, int ldc, cudaStream_t st);
+bool launch_gemm_f16_topt(const void* Ah, const void* Al, const float* inv, int M, const void* Bh, const void* Bl,
+                          const float* inv_b, int N, int K, unsigned col_base, u64* cand, unsigned* xbound,
+                          cudaStream_t st);
 
 // ---- rsb_ivf.cu -----------------------------------------------------------------------------------------
 // (query, list) work list, sorted by list so that concurrently running blocks share inverted lists in L2.

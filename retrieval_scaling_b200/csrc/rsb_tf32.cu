@@ -1,20 +1,39 @@
 // rsb_tf32.cu -- fp32-accurate inner-product scores on the Hopper tensor cores: S[M,N] = A[M,K] . B[N,K]^T with
 // A, B fp32, computed as the error-compensated 3xTF32 product
 //        A.B ~= Ah.Bh + Ah.Bl + Al.Bh        (x = xh + xl, xh = tf32(x), xl = tf32(x - xh); the dropped Al.Bl term
-// is ~2^-22 relative) accumulated in fp32 registers.  Used for the IVF coarse quantizer (the IndexFlatIP the reference
-// builds at src/indicies/ivf_flat.py:142, ivf_pq.py:145).
+// is ~2^-22 relative) accumulated in fp32 registers.  Used for Flat search over fp32 rows.
 //
 // 128 x 128 output tiles, TMA tensor loads (128B swizzle, 32 fp32 = one swizzle row per K step) -> 3-stage
 // shared-memory ring of {Ah, Al, Bh, Bl} tiles filled by one producer thread -> two consumer warpgroups that take the
 // tiles of a persistent CTA in turn, each issuing 24 wgmma.m64n128k8.tf32 per stage (4 K-slices x 3 products x 2
 // row halves) -> epilogue from the accumulator registers while the other warpgroup runs the next tile's MMAs.
 //
-// fp16 form (F16 = true; Flat indexes with fp16 storage): B is the database as stored (fp16 rows, exact), so no split
-// copy of it exists.  Each query row is scaled by a power of two s that puts its largest |element| in [2^14, 2^15)
-// (exact), and split into fp16 hi = fp16(q s), lo = fp16(q s - hi): 22 significant bits, as many as the 3xTF32 query
-// split; there is no lo.lo term because B is exact.  Per stage two wgmma.m64n128k16.f16 per 16-wide K-slice (lo.B,
-// then hi.B) share the B tile, 64 fp16 = one swizzle row per K step; the epilogue multiplies by 1 / s.  Both forms
-// share the mainloop ring and the epilogues below (score tile, or the fused top-8 candidate + bound filter).
+// fp16 forms (F16 = true).  Each row of an fp32 operand is scaled by a power of two s that puts its largest
+// |element| in [2^14, 2^15) (exact), and split into fp16 hi = fp16(x s), lo = fp16(x s - hi) (split_f16_kernel).
+// 64 fp16 = one swizzle row per K step, so a stage carries twice the K of the tf32 form in the same 64 KB.
+//  * B exact (Flat indexes with fp16 storage): B is the database as stored, so no split copy of it exists; per
+//    16-wide K-slice two wgmma.m64n128k16.f16 (lo.B, then hi.B) share the B tile; the epilogue multiplies by
+//    inv_a[row] = 1 / s.
+//  * B split (the IVF coarse quantizer: queries against the centroids, split once when the index gets them): per
+//    16-wide K-slice three wgmma.m64n128k16.f16 in 3xTF32's order, Al.Bh, Ah.Bl, Ah.Bh; the epilogue multiplies by
+//    inv_b[col], then inv_a[row] (powers of two: exact unless a product leaves the normal fp32 range).
+//    Error per product a b, in scaled units (a = x s of one operand row, b of the other), u = 2^-11 the fp16 unit
+//    round-off, d = 2^-25 half the fp16 subnormal spacing: a = Ah + Al + ea with
+//      |Al| <= u (1 + u) |a| + d,  |ea| <= u^2 |a| + d      (|a - Ah| <= u |a|; Al rounds that remainder to 11
+//                                                             significant bits, or to the subnormal grid below 2^-14)
+//      a b - (Ah Bh + Ah Bl + Al Bh) = Al Bl + a eb + ea b - ea eb
+//      |a b - (Ah Bh + Ah Bl + Al Bh)| <= (3 u^2 + 2 u^3 + 2 u^4) |a b| + d (1 + u + 2 u^2) (|a| + |b|) + 2 d^2.
+//    The relative term is about 3 * 2^-22 (3xTF32: the same 3 u^2 with u = 2^-11); the absolute term is below 2^-39
+//    of the row maxima (each row's largest |a| is >= 2^14), so a lo that goes subnormal costs nothing measurable.
+//    Each fp16 product is exact in fp32; the accumulators add them in the 3xTF32 form's order.
+//    tests/test_coarse_f16_split_cpu.py restates the split and this bound in fp64.
+//    Exactness: the coarse stage keeps the top kc = nprobe + 8 of these scores (the fused filter below is exact with
+//    respect to them) and re-scores the kc candidates in fp32 (refine_exact_kernel).  A column of the exact top
+//    nprobe can only be missed if kc columns score at least as high in S~, so with eps the largest score error of the
+//    row (the bound above summed over K, plus the fp32 accumulation) at least 8 columns outside the exact top nprobe
+//    come within 2 eps of it: the result is the exact fp32 top nprobe unless the exact scores at ranks
+//    nprobe and nprobe + 8 lie within 2 eps -- the same boundary caveat as the 3xTF32 form.
+// All forms share the mainloop ring and the epilogues below (score tile, or the fused top-8 candidate + bound filter).
 #include "rsb_common.cuh"
 #include "rsb_internal.h"
 #include "rsb_tc.cuh"
@@ -22,6 +41,7 @@
 #include <algorithm>
 #include <math.h>
 #include <stdlib.h>
+#include <type_traits>
 
 namespace rsb {
 
@@ -97,7 +117,8 @@ void launch_split_f16(const float* q, int M, int K, void* hi, void* lo, float* i
 // to the row's top kc -- select_cands_kernel checks exactly that and flags the (rare) rows for which it fails; those
 // are re-done exhaustively in fp32 by exact_rows_kernel.  The result is therefore the exact top-kc of the 3xTF32
 // scores without writing and re-reading nq x nlist x 4 bytes.
-// F16: fp16 operands (tmBl unused), scores multiplied by inv[row] before either epilogue.
+// F16: fp16 operands, scores multiplied by inv_b[col] (B split; tmBl unused when inv_b is null) and inv_a[row] before
+// either epilogue.
 
 // tile t -> (query tile, column tile): bands of `band` query tiles; inside a band the query tile runs fastest, so the
 // CTAs in flight share a few column tiles and the band's query operand stays L2-resident while it sweeps all columns
@@ -110,22 +131,29 @@ __device__ __forceinline__ void tile_coords(int t, int tiles_m, int tiles_n, int
     tn = local / rows;
 }
 
-// sorted insertion, strict comparisons: fed in ascending column order, ties keep the lower column
-__device__ __forceinline__ void top9_push(float (&v)[9], int (&c)[9], float x, int col) {
-    if (x > v[8]) {
-        v[8] = x; c[8] = col;
-#pragma unroll
-        for (int i = 8; i > 0; --i) {
-            if (v[i] > v[i - 1]) {
-                const float tv = v[i]; v[i] = v[i - 1]; v[i - 1] = tv;
-                const int tc = c[i]; c[i] = c[i - 1]; c[i - 1] = tc;
-            }
-        }
-    }
-}
 // (x, cx) ranks before (y, cy): higher score, or the same score and the lower column; empty entries (-inf, -1) last
 __device__ __forceinline__ bool top9_before(float x, int cx, float y, int cy) {
     return x > y || (x == y && (unsigned)cx < (unsigned)cy);
+}
+// Insert (x, cx) into the sorted list where it ranks before entry i (p[i]), dropping the last entry; nothing changes
+// if it ranks before none.  The list is sorted, so p is false up to the insertion point and true from there on, and
+// every entry takes its new value from the old list alone: a branch-free step whose 9 lanes are independent, instead
+// of a chain of 8 dependent compare-and-swaps.  The epilogue of a 128 x 128 tile runs 4 x 32 of these per lane plus
+// the merges, and with one warp per scheduler their latency is not hidden.
+// COL_ORDER: fed in ascending column order, so (x, cx) ranks before entry i iff x > v[i] (strict: ties keep the
+// lower column, the one already in the list).
+template <bool COL_ORDER>
+__device__ __forceinline__ void top9_insert(float (&v)[9], int (&c)[9], float x, int cx) {
+    bool p[9];
+#pragma unroll
+    for (int i = 0; i < 9; ++i) p[i] = COL_ORDER ? x > v[i] : top9_before(x, cx, v[i], c[i]);
+#pragma unroll
+    for (int i = 8; i > 0; --i) {                             // descending: v[i - 1] is still the old entry
+        v[i] = p[i - 1] ? v[i - 1] : p[i] ? x : v[i];
+        c[i] = p[i - 1] ? c[i - 1] : p[i] ? cx : c[i];
+    }
+    v[0] = p[0] ? x : v[0];
+    c[0] = p[0] ? cx : c[0];
 }
 // merge the list of lane ^ off into this lane's: both lanes end with the top 9 of the union in the total order
 __device__ __forceinline__ void top9_merge(float (&v)[9], int (&c)[9], int off) {
@@ -137,28 +165,19 @@ __device__ __forceinline__ void top9_merge(float (&v)[9], int (&c)[9], int off) 
         pc[i] = __shfl_xor_sync(0xffffffffu, c[i], off);
     }
 #pragma unroll
-    for (int k = 0; k < 9; ++k) {
-        if (top9_before(pv[k], pc[k], v[8], c[8])) {
-            v[8] = pv[k]; c[8] = pc[k];
-#pragma unroll
-            for (int i = 8; i > 0; --i) {
-                if (top9_before(v[i], c[i], v[i - 1], c[i - 1])) {
-                    const float tv = v[i]; v[i] = v[i - 1]; v[i - 1] = tv;
-                    const int tc = c[i]; c[i] = c[i - 1]; c[i - 1] = tc;
-                }
-            }
-        }
-    }
+    for (int k = 0; k < 9; ++k) top9_insert<false>(v, c, pv[k], pc[k]);
 }
 
 template <bool F16, bool FUSED>
 __global__ __launch_bounds__(T_THREADS, 1)
 void gemm_ip_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
                        const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl,
-                       const float* __restrict__ inv, float* __restrict__ C, int ldc, u64* __restrict__ cand,
-                       unsigned* __restrict__ xbound, int M, int N, int K, unsigned col_base, int band) {
+                       const float* __restrict__ inv, const float* __restrict__ inv_b, float* __restrict__ C, int ldc,
+                       u64* __restrict__ cand, unsigned* __restrict__ xbound, int M, int N, int K, unsigned col_base,
+                       int band) {
     constexpr int BK = F16 ? T_BK16 : T_BK;                   // K elements per stage: one 128-byte swizzle row
-    constexpr int STAGE_TX = (F16 ? 3 : 4) * T_TILE_BYTES;
+    const bool b_split = !F16 || inv_b != nullptr;            // B has a lo part (uniform over the grid)
+    const int stage_tx = (b_split ? 4 : 3) * T_TILE_BYTES;
     extern __shared__ unsigned char smem_dyn[];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + T_STAGES * T_STAGE_BYTES);
@@ -168,13 +187,13 @@ void gemm_ip_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_co
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
     const int tiles_m = (M + T_BM - 1) / T_BM, tiles_n = (N + T_BN - 1) / T_BN;
     const int ntiles = tiles_m * tiles_n;
-    const int nk = K / BK;
+    const int nk = (K + BK - 1) / BK;                         // columns past K read as zero
 
     if (threadIdx.x == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmAh)) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmAl)) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmBh)) : "memory");
-        if (!F16) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmBl)) : "memory");
+        if (b_split) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmBl)) : "memory");
         for (int s = 0; s < T_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 4); }   // 4 warps of one consumer
         mbar_init(&mdone[0], 1);
         mbar_init(&mdone[1], 1);
@@ -193,11 +212,11 @@ void gemm_ip_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_co
                     const int s = g % T_STAGES;
                     mbar_wait(&empty[s], ((g / T_STAGES) & 1) ^ 1);   // the first pass over the ring falls through
                     unsigned char* base = smem + s * T_STAGE_BYTES;
-                    mbar_expect_tx(&full[s], STAGE_TX);
+                    mbar_expect_tx(&full[s], stage_tx);
                     tma_load_2d(base + 0 * T_TILE_BYTES, &tmAh, &full[s], kb * BK, tm * T_BM);   // rows past M / N read as zero
                     tma_load_2d(base + 1 * T_TILE_BYTES, &tmAl, &full[s], kb * BK, tm * T_BM);
                     tma_load_2d(base + 2 * T_TILE_BYTES, &tmBh, &full[s], kb * BK, tn * T_BN);
-                    if (!F16) tma_load_2d(base + 3 * T_TILE_BYTES, &tmBl, &full[s], kb * BK, tn * T_BN);
+                    if (b_split) tma_load_2d(base + 3 * T_TILE_BYTES, &tmBl, &full[s], kb * BK, tn * T_BN);
                 }
             }
         }
@@ -219,55 +238,86 @@ void gemm_ip_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_co
         for (int e = 0; e < 64; ++e) { acc[0][e] = 0.f; acc[1][e] = 0.f; }
         if (i > 0) mbar_wait(&mdone[(i - 1) & 1], ((i - 1) >> 1) & 1);
         int g = i * nk;
-        for (int kb = 0; kb < nk; ++kb, ++g) {
-            const int s = g % T_STAGES;
-            mbar_wait(&full[s], (g / T_STAGES) & 1);
-            const uint32_t base = smem_u32(smem + s * T_STAGE_BYTES);
-            const uint64_t ah = make_sw128_kmajor_desc(base);
-            const uint64_t al = make_sw128_kmajor_desc(base + T_TILE_BYTES);
-            const uint64_t bh = make_sw128_kmajor_desc(base + 2 * T_TILE_BYTES);
-            const uint64_t bl = make_sw128_kmajor_desc(base + 3 * T_TILE_BYTES);
-            constexpr uint64_t LOWER = (64 * 128) >> 4;       // rows 64..127: 64 swizzle rows further in the A tiles
-            acc_fence(acc[0]);
-            acc_fence(acc[1]);
-            wgmma_fence();
-            // per output element, per K slice: the small term(s) first, the dominant hi product last
-            if (F16) {
+        // one copy of the k-loop per B form, so that no branch sits between the MMAs of a stage
+        auto mainloop = [&](auto split) {
+            constexpr bool SPLIT = decltype(split)::value;
+            for (int kb = 0; kb < nk; ++kb, ++g) {
+                const int s = g % T_STAGES;
+                mbar_wait(&full[s], (g / T_STAGES) & 1);
+                const uint32_t base = smem_u32(smem + s * T_STAGE_BYTES);
+                const uint64_t ah = make_sw128_kmajor_desc(base);
+                const uint64_t al = make_sw128_kmajor_desc(base + T_TILE_BYTES);
+                const uint64_t bh = make_sw128_kmajor_desc(base + 2 * T_TILE_BYTES);
+                const uint64_t bl = make_sw128_kmajor_desc(base + 3 * T_TILE_BYTES);
+                constexpr uint64_t LOWER = (64 * 128) >> 4;   // rows 64..127: 64 swizzle rows further in the A tiles
+                acc_fence(acc[0]);
+                acc_fence(acc[1]);
+                wgmma_fence();
+                // per output element, per K slice: the small term(s) first, the dominant hi product last
+                if constexpr (F16 && SPLIT) {
 #pragma unroll
-                for (int k4 = 0; k4 < T_BK16 / 16; ++k4) {    // K = 16 fp16 = 32 bytes: +2 in the (addr >> 4) field
-                    const uint64_t o = (uint64_t)(k4 * 2);
-                    wgmma_f16_n128(acc[0], al + o, bh + o);
-                    wgmma_f16_n128(acc[1], al + LOWER + o, bh + o);
-                    wgmma_f16_n128(acc[0], ah + o, bh + o);
-                    wgmma_f16_n128(acc[1], ah + LOWER + o, bh + o);
+                    for (int k4 = 0; k4 < T_BK16 / 16; ++k4) {  // K = 16 fp16 = 32 bytes: +2 in the (addr >> 4) field
+                        const uint64_t o = (uint64_t)(k4 * 2);
+                        wgmma_f16_n128(acc[0], al + o, bh + o);
+                        wgmma_f16_n128(acc[1], al + LOWER + o, bh + o);
+                        wgmma_f16_n128(acc[0], ah + o, bl + o);
+                        wgmma_f16_n128(acc[1], ah + LOWER + o, bl + o);
+                        wgmma_f16_n128(acc[0], ah + o, bh + o);
+                        wgmma_f16_n128(acc[1], ah + LOWER + o, bh + o);
+                    }
+                } else if constexpr (F16) {
+#pragma unroll
+                    for (int k4 = 0; k4 < T_BK16 / 16; ++k4) {
+                        const uint64_t o = (uint64_t)(k4 * 2);
+                        wgmma_f16_n128(acc[0], al + o, bh + o);
+                        wgmma_f16_n128(acc[1], al + LOWER + o, bh + o);
+                        wgmma_f16_n128(acc[0], ah + o, bh + o);
+                        wgmma_f16_n128(acc[1], ah + LOWER + o, bh + o);
+                    }
+                } else {
+#pragma unroll
+                    for (int k4 = 0; k4 < T_BK / 8; ++k4) {     // K = 8 tf32 = 32 bytes: +2 in the (addr >> 4) field
+                        const uint64_t o = (uint64_t)(k4 * 2);
+                        wgmma_tf32_n128(acc[0], al + o, bh + o);
+                        wgmma_tf32_n128(acc[1], al + LOWER + o, bh + o);
+                        wgmma_tf32_n128(acc[0], ah + o, bl + o);
+                        wgmma_tf32_n128(acc[1], ah + LOWER + o, bl + o);
+                        wgmma_tf32_n128(acc[0], ah + o, bh + o);
+                        wgmma_tf32_n128(acc[1], ah + LOWER + o, bh + o);
+                    }
                 }
-            } else {
-#pragma unroll
-                for (int k4 = 0; k4 < T_BK / 8; ++k4) {       // K = 8 tf32 = 32 bytes: +2 in the (addr >> 4) field
-                    const uint64_t o = (uint64_t)(k4 * 2);
-                    wgmma_tf32_n128(acc[0], al + o, bh + o);
-                    wgmma_tf32_n128(acc[1], al + LOWER + o, bh + o);
-                    wgmma_tf32_n128(acc[0], ah + o, bl + o);
-                    wgmma_tf32_n128(acc[1], ah + LOWER + o, bl + o);
-                    wgmma_tf32_n128(acc[0], ah + o, bh + o);
-                    wgmma_tf32_n128(acc[1], ah + LOWER + o, bh + o);
+                wgmma_commit();
+                acc_fence(acc[0]);
+                acc_fence(acc[1]);
+                wgmma_wait<1>();                              // the previous k-block's MMAs have retired: free its stage
+                if (kb > 0) {
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&empty[(g - 1) % T_STAGES]);
                 }
             }
-            wgmma_commit();
-            acc_fence(acc[0]);
-            acc_fence(acc[1]);
-            wgmma_wait<1>();                                  // the previous k-block's MMAs have retired: free its stage
-            if (kb > 0) {
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&empty[(g - 1) % T_STAGES]);
-            }
-        }
+        };
+        if (b_split) mainloop(std::true_type{});
+        else mainloop(std::false_type{});
         if (threadIdx.x % 128 == 0) mbar_arrive(&mdone[cw]);  // the other warpgroup may start on the next tile's stages
         wgmma_wait<0>();
         acc_fence(acc[0]);
         acc_fence(acc[1]);
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty[(g - 1) % T_STAGES]);
+        if (F16 && b_split) {                                 // undo the per-column scale (a power of two: exact)
+#pragma unroll
+            for (int j = 0; j < 16; ++j)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int col = n0 + 8 * j + c_lo + e;
+                    const float sb = col < N ? inv_b[col] : 0.f;
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        acc[0][4 * j + 2 * h + e] *= sb;
+                        acc[1][4 * j + 2 * h + e] *= sb;
+                    }
+                }
+        }
 
         if (!FUSED) {
 #pragma unroll
@@ -314,7 +364,7 @@ void gemm_ip_tc_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_co
                     float x = hh ? a1 : a0;
                     if (F16) x *= s;
                     const int col = 8 * j + c_lo + e;
-                    if (n0 + col < N) top9_push(v, c, x, n0 + col);
+                    if (n0 + col < N) top9_insert<true>(v, c, x, n0 + col);
                 }
             top9_merge(v, c, 1);
             top9_merge(v, c, 2);
@@ -372,15 +422,15 @@ static int tile_band(int M, int K, int elem_bytes) {
 
 // FUSED: cand / xbound (C unused); else C (cand / xbound unused)
 template <bool F16, bool FUSED>
-static void launch_gemm(const CUtensorMap (&m)[4], const float* inv, int M, int N, int K, float* C, int ldc,
-                        unsigned col_base, u64* cand, unsigned* xbound, cudaStream_t st) {
+static void launch_gemm(const CUtensorMap (&m)[4], const float* inv, const float* inv_b, int M, int N, int K, float* C,
+                        int ldc, unsigned col_base, u64* cand, unsigned* xbound, cudaStream_t st) {
     static PerDeviceSize configured;
     if (configured.raise(T_SMEM))
         cudaFuncSetAttribute(gemm_ip_tc_kernel<F16, FUSED>, cudaFuncAttributeMaxDynamicSharedMemorySize, T_SMEM);
     const int ntiles = ((M + T_BM - 1) / T_BM) * ((N + T_BN - 1) / T_BN);
     const int grid = std::min(ntiles, device_num_sms());     // one CTA per SM (shared memory), persistent
-    gemm_ip_tc_kernel<F16, FUSED><<<grid, T_THREADS, T_SMEM, st>>>(m[0], m[1], m[2], m[3], inv, C, ldc, cand, xbound, M, N,
-                                                                   K, col_base, tile_band(M, K, F16 ? 2 : 4));
+    gemm_ip_tc_kernel<F16, FUSED><<<grid, T_THREADS, T_SMEM, st>>>(m[0], m[1], m[2], m[3], inv, inv_b, C, ldc, cand, xbound,
+                                                                   M, N, K, col_base, tile_band(M, K, F16 ? 2 : 4));
 }
 
 // Ah/Al [M,K], Bh/Bl [N,K] fp32 (already split).  cand [M, fused_cand_per_row(N)] u64 keys (score order high word,
@@ -392,7 +442,7 @@ bool launch_gemm_tf32x3_topt(const float* Ah, const float* Al, int M, const floa
     if (K % T_BK) return false;
     CUtensorMap m[4];
     if (!make_maps(m, Ah, Al, M, Bh, Bl, N, K)) return false;
-    launch_gemm<false, true>(m, nullptr, M, N, K, nullptr, 0, col_base, cand, xbound, st);
+    launch_gemm<false, true>(m, nullptr, nullptr, M, N, K, nullptr, 0, col_base, cand, xbound, st);
     return true;
 }
 
@@ -406,37 +456,43 @@ bool launch_gemm_tf32x3(const float* Ah, const float* Al, int M, const float* Bh
     if (K % T_BK) return false;
     CUtensorMap m[4];
     if (!make_maps(m, Ah, Al, M, Bh, Bl, N, K)) return false;
-    launch_gemm<false, false>(m, nullptr, M, N, K, C, ldc, 0u, nullptr, nullptr, st);
+    launch_gemm<false, false>(m, nullptr, nullptr, M, N, K, C, ldc, 0u, nullptr, nullptr, st);
     return true;
 }
 
-// Ah/Al [M,K] fp16 (launch_split_f16), inv [M], B [N,K] fp16 rows as stored.  K % 64 == 0.  Returns false if the
-// tensor maps cannot be encoded; there is no CUDA-core fp16 path to fall back to (the caller reports an error).
-static bool make_maps_f16(CUtensorMap (&m)[4], const void* Ah, const void* Al, int M, const void* B, int N, int K) {
+// Ah/Al [M,K] fp16 (launch_split_f16), inv [M].  B [N,K] fp16: the rows as stored (Bl and inv_b null), or Bh/Bl and
+// inv_b [N] of launch_split_f16.  K % 8 == 0 (16-byte rows; a partial last K step reads zeros).  Returns false if
+// the tensor maps cannot be encoded; there is no CUDA-core fp16 path to fall back to (the caller reports an error).
+static bool make_maps_f16(CUtensorMap (&m)[4], const void* Ah, const void* Al, int M, const void* Bh, const void* Bl,
+                          int N, int K) {
     if (!(make_map_2d(&m[0], Ah, (uint64_t)M, (uint64_t)K, T_BM, 2) && make_map_2d(&m[1], Al, (uint64_t)M, (uint64_t)K, T_BM, 2) &&
-          make_map_2d(&m[2], B, (uint64_t)N, (uint64_t)K, T_BN, 2)))
+          make_map_2d(&m[2], Bh, (uint64_t)N, (uint64_t)K, T_BN, 2)))
         return false;
-    m[3] = m[2];                                              // unused by the fp16 kernel
+    if (!Bl) {
+        m[3] = m[2];                                          // unused by the kernel
+        return true;
+    }
+    return make_map_2d(&m[3], Bl, (uint64_t)N, (uint64_t)K, T_BN, 2);
+}
+
+bool launch_gemm_f16(const void* Ah, const void* Al, const float* inv, int M, const void* Bh, const void* Bl,
+                     const float* inv_b, int N, int K, float* C, int ldc, cudaStream_t st) {
+    if (M <= 0 || N <= 0) return true;
+    if (K % 8 || (!Bl && K % T_BK16) || !Bl != !inv_b) return false;
+    CUtensorMap m[4];
+    if (!make_maps_f16(m, Ah, Al, M, Bh, Bl, N, K)) return false;
+    launch_gemm<true, false>(m, inv, inv_b, M, N, K, C, ldc, 0u, nullptr, nullptr, st);
     return true;
 }
 
-bool launch_gemm_f16x2(const void* Ah, const void* Al, const float* inv, int M, const void* B, int N, int K, float* C,
-                       int ldc, cudaStream_t st) {
+bool launch_gemm_f16_topt(const void* Ah, const void* Al, const float* inv, int M, const void* Bh, const void* Bl,
+                          const float* inv_b, int N, int K, unsigned col_base, u64* cand, unsigned* xbound,
+                          cudaStream_t st) {
     if (M <= 0 || N <= 0) return true;
-    if (K % T_BK16) return false;
+    if (K % 8 || (!Bl && K % T_BK16) || !Bl != !inv_b) return false;
     CUtensorMap m[4];
-    if (!make_maps_f16(m, Ah, Al, M, B, N, K)) return false;
-    launch_gemm<true, false>(m, inv, M, N, K, C, ldc, 0u, nullptr, nullptr, st);
-    return true;
-}
-
-bool launch_gemm_f16x2_topt(const void* Ah, const void* Al, const float* inv, int M, const void* B, int N, int K,
-                            unsigned col_base, u64* cand, unsigned* xbound, cudaStream_t st) {
-    if (M <= 0 || N <= 0) return true;
-    if (K % T_BK16) return false;
-    CUtensorMap m[4];
-    if (!make_maps_f16(m, Ah, Al, M, B, N, K)) return false;
-    launch_gemm<true, true>(m, inv, M, N, K, nullptr, 0, col_base, cand, xbound, st);
+    if (!make_maps_f16(m, Ah, Al, M, Bh, Bl, N, K)) return false;
+    launch_gemm<true, true>(m, inv, inv_b, M, N, K, nullptr, 0, col_base, cand, xbound, st);
     return true;
 }
 

@@ -8,7 +8,7 @@ product through the IndexFlatIP quantizer); PQ sub-quantizers: L2 k-means, ksub=
 on residuals of at most 256*ksub points.  Parity is defined *given* the trained centroids / codebooks (SURVEY §8a row a10).
 
 The Lloyd iterations are driven from here; the arithmetic of every step runs in librsb (`LibrsbOps`):
-  assignment (coarse)  : the coarse quantizer itself -- fused 3xTF32 wgmma scorer + exact fp32 re-score (rsb_coarse on a
+  assignment (coarse)  : the coarse quantizer itself -- fused fp16 hi/lo wgmma scorer + exact fp32 re-score (rsb_coarse on a
                          scratch handle holding the current centroids) -> fp32-exact argmax
   assignment (PQ)      : rsb_pq_assign (the residual-encoding kernel without the residual step)
   update               : rsb_kmeans_accumulate / rsb_pq_accumulate (member sums and counts)

@@ -1,14 +1,14 @@
-"""Times the IVF coarse stage (rsb_coarse: query split, 3xTF32 fused scorer, select_cands, exact_rows, refine_exact)
+"""Times the IVF coarse stage (rsb_coarse: query split, fp16 hi/lo fused scorer, select_cands, exact_rows, refine_exact)
 at bench.py's geometry: nlist 16384, d 768, nprobe 32, for nq in {1, 1250, 10000} (1250 = the per-GPU share of 10k
 queries at 8 GPUs).
 
     python scripts/bench_coarse.py [--steps 20] [--warmup 5] [--out DIR]
 
 Stage time: CUDA events around `steps` back-to-back calls.  Per-kernel split: torch.profiler in a separate run (CUDA
-activities), kernel time summed per kernel name.  For the GEMM it also prints the achieved TFLOP/s of TF32 tensor
-work (3 products) against the 495 TFLOP/s data-sheet figure, and the operand bytes the tile schedule implies: DRAM
-(each band of query tiles once, the centroid operand once per band) and L2 -> SM (every tile loads its hi + lo query
-and centroid tiles)."""
+activities), kernel time summed per kernel name.  For the GEMM it also prints the achieved TFLOP/s of fp16 tensor
+work (3 products) against the 989 TFLOP/s dense fp16 data-sheet figure, and the operand bytes the tile schedule
+implies (2-byte hi + lo operands): DRAM (each band of query tiles once, the centroid operand once per band) and
+L2 -> SM (every tile loads its hi + lo query and centroid tiles)."""
 import argparse
 import json
 import os
@@ -21,17 +21,17 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import retrieval_scaling_b200 as r  # noqa: E402
 
-TF32_PEAK = 495e12
-KERNELS = ("split_tf32_kernel", "gemm_ip_tc_kernel", "select_cands_kernel", "exact_rows_kernel", "refine_exact_kernel")
+F16_PEAK = 989e12
+KERNELS = ("split_f16_kernel", "gemm_ip_tc_kernel", "select_cands_kernel", "exact_rows_kernel", "refine_exact_kernel")
 
 
 def schedule_bytes(nq, nlist, d, l2_bytes):
     """Operand bytes of one fused pass under the kernel's tile order (tile_band in rsb_tf32.cu)."""
     tiles_m, tiles_n = -(-nq // 128), -(-nlist // 128)
-    a_tile = 128 * d * 4 * 2                                  # hi + lo
+    a_tile = 128 * d * 2 * 2                                  # fp16 hi + lo
     band = max(1, min(l2_bytes // 3 // a_tile, tiles_m))
     bands = -(-tiles_m // band)
-    dram = nq * d * 8 + bands * nlist * d * 8
+    dram = nq * d * 4 + bands * nlist * d * 4
     l2_to_sm = tiles_m * tiles_n * 2 * a_tile
     return band, dram, l2_to_sm
 
@@ -86,7 +86,7 @@ def main():
         gemm_ms = split.get("gemm_ip_tc_kernel", float("nan"))
         flop = 3 * 2 * nq * a.nlist * a.d
         row = {"nq": nq, "stage_ms": round(stage_ms, 4), "kernel_ms": {k: round(v, 4) for k, v in split.items()},
-               "gemm_tflops": round(flop / (gemm_ms * 1e-3) / 1e12, 1), "gemm_share_of_tf32_peak": round(flop / TF32_PEAK / (gemm_ms * 1e-3), 3),
+               "gemm_tflops": round(flop / (gemm_ms * 1e-3) / 1e12, 1), "gemm_share_of_f16_peak": round(flop / F16_PEAK / (gemm_ms * 1e-3), 3),
                "band_query_tiles": band, "dram_operand_mb": round(dram / 1e6, 1), "l2_to_sm_operand_gb": round(l2sm / 1e9, 2)}
         out["runs"].append(row)
         print(json.dumps(row), flush=True)
