@@ -593,6 +593,25 @@ int rsb_minhash_dedup(const uint32_t* sig_dev, const int32_t* n_words_dev, const
  * signatures' word split splits (lets host-side tests pin the whitespace set against Python's str.isspace()) */
 int rsb_utf8_space_mask(const uint8_t* bytes, int64_t n, uint8_t* mask);
 
+/* ---- BM25 search (the reference's sparse retriever) ----------------------------------------------------------------
+ * Replaces src/search.py:763-807's pyserini LuceneSearcher.search (Lucene 9 BM25Similarity, k1 = 0.9, b = 0.4) over
+ * a term-major posting index; retrieval_scaling_b200/bm25.py builds the index and analyzes the queries.  Stateless:
+ * the caller owns every array.  Errors of these entries are reported by rsb_bm25_last_error().
+ * rsb_bm25_search: the postings of term t are post_dev[term_off_dev[t] .. term_off_dev[t+1]), each an 8-byte pair
+ * (int32 document number, fp32 x = 1f + (float) tf * cache[norm(doc)]) sorted by document, post_dev 8-byte aligned.
+ * Query q's clauses are q_off_dev[q] .. q_off_dev[q+1]) of q_term_dev (term ids, strictly ascending, each < the number
+ * of terms) and q_w_dev (fp32 clause weights count * idf).  Score of document d = the fp32 sum, in ascending term id,
+ * of w - w / x over the clauses whose term has a posting for d, each operation rounded on its own.  D_dev [nq, k]
+ * fp32 and I_dev [nq, k] int64 receive the hits (score > 0) best first, ties to the lower document number, then
+ * -FLT_MAX and -1.  ws_dev holds rsb_bm25_workspace_bytes(n_docs, nq, k) bytes.  n_docs < 2^31; k > 4096
+ * RSB_ERR_UNSUPPORTED; both before any launch.  q_term_dev / q_w_dev may be null when no query has a clause, and
+ * post_dev when no term has a posting (zero-length arrays); term_off_dev and q_off_dev are always read. */
+const char* rsb_bm25_last_error(void);
+size_t rsb_bm25_workspace_bytes(int64_t n_docs, int nq, int k);
+int rsb_bm25_search(const int64_t* term_off_dev, const int32_t* post_dev, int64_t n_docs, const int32_t* q_off_dev,
+                    const int32_t* q_term_dev, const float* q_w_dev, int nq, int k, float* D_dev, int64_t* I_dev,
+                    void* ws_dev, size_t ws_bytes, rsb_stream_t stream);
+
 /* diagnostic: shared-window address at which dynamic shared memory starts (the scan kernel folds it into LDS) */
 int rsb_debug_smem_base(void);
 /* diagnostic: the fp32 look-up tables an IVFPQ search builds for queries q_dev [nq, d], as the scan reads them:

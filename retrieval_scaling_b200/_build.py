@@ -18,7 +18,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "_obj")
 LIB = os.path.join(HERE, "librsb.so")
 SOURCES = ["rsb_dense.cu", "rsb_ivf.cu", "rsb_api.cu", "rsb_bert.cu", "rsb_tf32.cu", "rsb_refine.cu", "rsb_dedup.cu",
-           "rsb_llm.cu"]
+           "rsb_llm.cu", "rsb_bm25.cu"]
 NVCC_FLAGS = [
     "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v",

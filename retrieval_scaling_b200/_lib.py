@@ -111,6 +111,10 @@ SIGNATURES = [
                                        c_void_p, c_size_t, c_void_p]),
     ("rsb_minhash_dedup", c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     ("rsb_utf8_space_mask", c_int, [c_void_p, c_int64, c_void_p]),
+    ("rsb_bm25_last_error", c_char_p, []),
+    ("rsb_bm25_workspace_bytes", c_size_t, [c_int64, c_int, c_int]),
+    ("rsb_bm25_search", c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p,
+                                c_void_p, c_void_p, c_size_t, c_void_p]),
     ("rsb_debug_smem_base", c_int, []),
     ("rsb_pq_lut_floats", c_int, [_H]),
     ("rsb_pq_tables", c_int, [_H, c_void_p, c_int, c_void_p, c_void_p]),

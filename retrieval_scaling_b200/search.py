@@ -9,9 +9,13 @@
 Same function names, argument meaning, output file scheme and resume/overwrite behaviour, so the lm-eval
 harness fork consumes the JSONL unchanged (`ctxs[i]["retrieval text"]`, `"retrieval score"` as str).
 Multi-source merge with MinHash de-duplication and coin-flip subsampling (:386-546) is
-`post_hoc_merge_topk_multi_domain`, its de-duplication on the GPU (`dedup.py`).  Out of scope (SURVEY §2 #8): BM25
-search (`search_topk` raises NotImplementedError for `model.sparse_retriever`) and the answer-based re-ranking of
-the multi-source merge (`rerank_method`).
+`post_hoc_merge_topk_multi_domain`, its de-duplication on the GPU (`dedup.py`).
+
+    search_topk(cfg) -> search_sparse_topk(cfg)   with model.sparse_retriever=bm25   (:763-807, :827-829)
+      load eval data -> BM25Index.load(rsb_index/) -> analyze + score on the GPU (`bm25.py`, `rsb_bm25.cu`)
+      passages by (shard, line) -> safe_write_jsonl, "retrieval score" as a JSON number as the reference writes it
+
+Out of scope (SURVEY §2 #8): the answer-based re-ranking of the multi-source merge (`rerank_method`).
 """
 from __future__ import annotations
 
@@ -562,7 +566,61 @@ def post_hoc_merge_topk_multi_domain(cfg, deduplicate=None):
     return output_path
 
 
+# ----------------------------------------------------------------------------------------------------------
+# BM25 (reference src/search.py:763-807): one index over every passage of the listed shards, on one GPU
+# ----------------------------------------------------------------------------------------------------------
+def check_sparse_retriever(cfg):
+    """`model.sparse_retriever`: None (dense) or "bm25"; anything else raises NotImplementedError naming it.  BM25
+    runs one index on one GPU: under torchrun with more than one process it raises NotImplementedError."""
+    name = cfg.model.get("sparse_retriever", None)
+    if name and name != "bm25":
+        raise NotImplementedError(f"model.sparse_retriever={name}: only bm25 is implemented")
+    if name and _dist_state()[1] > 1:
+        raise NotImplementedError("model.sparse_retriever=bm25 searches one index on one GPU; run it without torchrun")
+    return name
+
+
+def search_sparse_topk(cfg):
+    """BM25 top-n_docs for every eval example, written to get_search_output_path(cfg, flattened shard ids):
+    ctxs = [{"retrieval text", "retrieval score" (a JSON number, as the reference writes it)}] best first, [None] for
+    an empty raw_query, [] for a query without hits."""
+    from . import bm25
+    from .indicies import index_utils as iu
+    eval_args = cfg.evaluation
+    shard_ids = bm25.flat_shard_ids(cfg)
+    output_path = get_search_output_path(cfg, shard_ids)
+    if os.path.exists(output_path) and not eval_args.search.get("overwrite", False):
+        logging.info(f"All search results for {cfg.datastore.index.index_shard_ids} exist, skipping searching.")
+        return
+    data = load_eval_data(cfg)
+    logging.info(f"Searching for {len(data)} total evaluation samples...")
+    path = bm25.index_dir(cfg, shard_ids)
+    if not os.path.exists(os.path.join(path, "meta.json")):
+        raise FileNotFoundError(f"The BM25 index does not exist, build it first (tasks.datastore.index=true)\n"
+                                f"Missing: {path}")
+    n_docs = int(eval_args.search.n_docs)
+    bm25.check_k(n_docs)
+    index = bm25.BM25Index.load(path, device=device)
+    valid = [i for i, ex in enumerate(data) if ex["raw_query"]]
+    D, I = index.search([data[i]["raw_query"] for i in valid], n_docs)
+    hit = I >= 0
+    passages_dir = cfg.datastore.embedding.passages_dir
+    pos_map = iu.get_passage_pos_ids(passages_dir, os.path.join(os.path.dirname(path), "passage_pos_id_map.pkl"))
+    records = iu.fetch_passages(pos_map, index.db_ids(I[hit]))
+    it = 0
+    for ex in data:
+        ex["ctxs"] = [None]
+    for row, i in enumerate(valid):
+        nh = int(hit[row].sum())
+        data[i]["ctxs"] = [{"retrieval text": rec["text"], "retrieval score": float(s)}
+                           for rec, s in zip(records[it:it + nh], D[row, :nh])]
+        it += nh
+    os.makedirs(os.path.dirname(output_path), exist_ok=True)
+    safe_write_jsonl(data, output_path)
+
+
 def search_topk(cfg):
-    if cfg.model.get("sparse_retriever", None):
-        raise NotImplementedError("BM25 / pyserini search is outside the GPU hot path (SURVEY §2 #10)")
-    search_dense_topk(cfg)
+    if check_sparse_retriever(cfg):
+        search_sparse_topk(cfg)
+    else:
+        search_dense_topk(cfg)

@@ -5,7 +5,8 @@
 
 Hydra / OmegaConf are replaced by `retrieval_scaling_b200.config` (same YAML files, same dotted overrides).
 Task switches: tasks.datastore.embedding (already-chunked passage shards -> embedding pickles, SURVEY §8f-4),
-tasks.datastore.index (build or load the index), tasks.eval.search (query -> top-k, the hot path),
+tasks.datastore.index (build or load the index; with model.sparse_retriever=bm25 the BM25 index of every listed shard
+under {passages_dir}/bm25/{ids}/rsb_index), tasks.eval.search (query -> top-k, the hot path; dense, or BM25 on the GPU),
 tasks.eval.merge_search (multi-source merge, MinHash de-duplication on the GPU and subsampling, reference :31-33),
 tasks.eval.inference (task_name perplexity: reader-LM perplexity with concate_k retrieved documents prepended, the
 Llama reader on the GPU, reference :35-38; perplexity_calibration and lm-eval raise NotImplementedError).
@@ -51,8 +52,13 @@ def main(cfg) -> None:
 
     if cfg.tasks.datastore.get("index", False):
         logging.info("\n\n************** Indexing ***********")
-        from retrieval_scaling_b200.indicies.base import Indexer
-        Indexer(cfg)   # reference src/index.py:46-57: constructing the Indexer builds / loads the index
+        from retrieval_scaling_b200.search import check_sparse_retriever
+        if check_sparse_retriever(cfg):
+            from retrieval_scaling_b200 import bm25
+            bm25.build_index(cfg)   # reference src/index.py:164-207: one BM25 index over every listed shard
+        else:
+            from retrieval_scaling_b200.indicies.base import Indexer
+            Indexer(cfg)   # reference src/index.py:46-57: constructing the Indexer builds / loads the index
 
     if cfg.tasks.eval.get("search", False):
         logging.info("\n\n************** Running Search ***********")
