@@ -457,7 +457,7 @@ enum { RSB_GEMM_REVERSED = 256 };
 int rsb_gemm_f16(const void* A_dev, const void* W_dev, const void* bias_dev, const void* residual_dev, void* C_dev,
                  int M, int N, int K, int epilogue, rsb_stream_t stream);
 
-/* ---- reader LM for perplexity evaluation: HF causal LMs, prefill only, fp16 or bf16 ---------------------------------
+/* ---- reader LM for perplexity evaluation and greedy generation: HF causal LMs, fp16 or bf16 -------------------------
  * Replaces the reader of the reference's perplexity loop (src/evaluate_perplexity.py:98-108 loads it, :126-134 runs
  * `lm(input_ids, labels=labels)` one window at a time).  Errors of these entries are reported by rsb_llm_last_error().
  * rsb_llm_create makes a reader of one family.  Every refusal below comes before any CUDA call, and the error names the
@@ -526,6 +526,26 @@ size_t rsb_llm_workspace_bytes(rsb_llm_t* h, int total_tokens, int label_tokens)
 int rsb_llm_nll(rsb_llm_t* h, const int32_t* ids_dev, const int32_t* cu_seqlens_dev, int B, int T, int max_seqlen,
                 const int32_t* labels_dev, float* nll_out_dev, void* ws_dev, size_t ws_bytes, rsb_stream_t stream);
 int rsb_llm_free(rsb_llm_t* h);
+/* Greedy generation (HF `model.generate(do_sample=False, num_beams=1)`) from B packed contexts: ids_dev [T] and
+ * cu_seqlens_dev [B+1] as rsb_llm_nll, every context non-empty and at most max_seqlen tokens, and max_seqlen +
+ * max_new_tokens <= max_pos.  A prefill over the contexts fills a KV cache in the workspace (K after RoPE, OLMo after
+ * clip_qkv / QK-norm, and V, in the handle's dtype, one contiguous run of positions per sequence and KV head) and
+ * chooses each sequence's first token; then each decode step runs one row per sequence still running through the same
+ * layers, at explicit positions, with split-KV attention over its cache.  The choice is the argmax of the logits over the
+ * real vocabulary compared in fp32, the lowest id on ties (torch.argmax).  A sequence ends after emitting an id of
+ * eos_ids (host array of n_eos >= 0 ids; the id is part of its output) or after max_new_tokens ids; the call returns
+ * when every sequence has ended.  out_tokens_dev [B, max_new_tokens] int32 receives the ids (-1 past the end),
+ * out_lens_dev [B] int32 the number of ids, and out_logprob_dev [B, max_new_tokens] fp32 (may be NULL) the fp32
+ * log-softmax of each chosen id (0 past the end).  A sequence's ids do not depend on the other sequences of the call.
+ * Any heads / kv_heads group runs; a group wider than 16 query heads reads its cache once per 16 heads.
+ * One read-back of the chosen ids per step.  Before any launch: max_seqlen + max_new_tokens > max_pos
+ * RSB_ERR_UNSUPPORTED; an empty context, ids outside [0, vocab), malformed offsets, max_new_tokens <= 0 or n_eos < 0
+ * RSB_ERR_INVALID; a workspace below rsb_llm_generate_workspace_bytes(h, B, T, max_seqlen, max_new_tokens)
+ * RSB_ERR_OOM; RSB_ERR_STATE until every weight is loaded. */
+size_t rsb_llm_generate_workspace_bytes(rsb_llm_t* h, int B, int T, int max_seqlen, int max_new_tokens);
+int rsb_llm_generate(rsb_llm_t* h, const int32_t* ids_dev, const int32_t* cu_seqlens_dev, int B, int T, int max_seqlen,
+                     int max_new_tokens, const int32_t* eos_ids, int n_eos, int32_t* out_tokens_dev,
+                     int32_t* out_lens_dev, float* out_logprob_dev, void* ws_dev, size_t ws_bytes, rsb_stream_t stream);
 /* Diagnostic, not used on the product path: one attention step of rsb_llm_nll on a caller's tensors, with the forward's
  * own work list.  qkv_dev [T, (heads + 2 kv_heads) head_dim] in the handle's dtype (fp16 or bf16) holds each token's
  * Q | K | V heads (GPT-NeoX: the permuted [Q heads | K heads | V heads] layout rsb_llm_load stores); RoPE is applied to

@@ -1,9 +1,9 @@
 // rsb_llm.cu -- reader-LM forward for perplexity evaluation: HF LlamaForCausalLM (Llama-2 MHA, Llama-3 GQA),
 // GPTNeoXForCausalLM (Pythia) and OlmoForCausalLM / Olmo2ForCausalLM, chosen by rsb_llm_create's family, in fp16 or
 // bf16 (every kernel is a template on its element type and rounds to it where HF's forward in that dtype rounds),
-// prefill only, over packed un-padded sequences, ending in the per-token negative log-likelihood of the labels.
-// Replaces the reader call of the reference's perplexity loop (src/evaluate_perplexity.py:126-134: `lm(input_ids,
-// labels=labels)` one window at a time, HF in bf16).  No KV cache, no generation.
+// over packed un-padded sequences: a prefill ending in the per-token negative log-likelihood of the labels, which
+// replaces the reader call of the reference's perplexity loop (src/evaluate_perplexity.py:126-134: `lm(input_ids,
+// labels=labels)` one window at a time, HF in bf16), and greedy generation with a KV cache (rsb_llm_generate).
 //
 //   embed_rows_kernel        X[t] = embed_tokens[ids[t]]
 //   rms_rows_kernel          LlamaRMSNorm (the weight multiply in half) or Olmo2RMSNorm (in fp32), optionally fused with
@@ -18,6 +18,11 @@
 //                            key blocks above the diagonal are never visited
 //   swiglu_kernel            act = fp16(fp16(silu(gate)) * up), HF LlamaMLP's order
 //   nll_rows_kernel          fp32 logsumexp over the real vocabulary (pad rows of the LM head excluded) - logit[label]
+// Generation adds:
+//   kv_store_kernel          K (after RoPE) and V of each row into the KV cache, in the prefill and in every decode step
+//   decode_attention_kernel  split-KV attention of one query row per sequence over its cache, all query heads of a KV
+//                            head in one mma tile; decode_combine_kernel merges the chunks
+//   greedy_rows_kernel       fp32 argmax over the real vocabulary (lowest id on ties) and its log-softmax
 #include "../../include/rsb.h"
 
 #include "rsb_internal.h"
@@ -25,6 +30,7 @@
 #include "rsb_dtype.cuh"
 
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -120,26 +126,32 @@ void rms_rows_kernel(T* __restrict__ X, const T* __restrict__ A, const int* __re
     }
 }
 
-// Position of token t in its packed sequence: t - cu[b] for the sequence b with cu[b] <= t < cu[b+1].
-__device__ __forceinline__ int seq_position(const int* __restrict__ cu_seqlens, int B, int t) {
+// The packed sequence b of token t: cu[b] <= t < cu[b+1].
+__device__ __forceinline__ int seq_index(const int* __restrict__ cu_seqlens, int B, int t) {
     int lo = 0, hi = B;
     while (hi - lo > 1) {
         const int mid = (lo + hi) >> 1;
         if (cu_seqlens[mid] <= t) lo = mid; else hi = mid;
     }
-    return t - cu_seqlens[lo];
+    return lo;
+}
+
+// Position of row t: pos[t] when the caller gives explicit positions (a decode step, one row per sequence), else its
+// position in its packed sequence, t - cu[b].
+__device__ __forceinline__ int seq_position(const int* __restrict__ cu_seqlens, int B, const int* __restrict__ pos, int t) {
+    return pos ? pos[t] : t - cu_seqlens[seq_index(cu_seqlens, B, t)];
 }
 
 // HF apply_rotary_pos_emb (modeling_llama.py, modeling_gpt_neox.py): rotate_half on dims [0, rot) of every Q and K
 // head (head_dim hd apart, Q heads then K heads at the start of each QKV row, ld halves apart); dims [rot, hd) are
 // neither read nor written (GPT-NeoX partial rotary; Llama has rot = hd = 128).  x_embed = x * cos + rotate_half(x) *
 // sin in fp16, cos / sin = fp16(cos / sin(fp32(inv_freq[i] * pos))).  Each fp16 product and sum is one fp32 operation
-// rounded to half, as torch computes half tensors.  One block per token.
+// rounded to half, as torch computes half tensors.  One block per token; positions as seq_position.
 template <typename T>
-__global__ void rope_kernel(T* __restrict__ qkv, const int* __restrict__ cu_seqlens, int B, int ld, int rot_heads,
-                            int hd, int rot, const float* __restrict__ inv_freq) {
+__global__ void rope_kernel(T* __restrict__ qkv, const int* __restrict__ cu_seqlens, int B, const int* __restrict__ positions,
+                            int ld, int rot_heads, int hd, int rot, const float* __restrict__ inv_freq) {
     const int t = blockIdx.x;
-    const float pos = (float)seq_position(cu_seqlens, B, t);
+    const float pos = (float)seq_position(cu_seqlens, B, positions, t);
     const int half_rot = rot >> 1;
     T* row = qkv + (size_t)t * ld;
     // pair p = head hh, dim i: advanced by blockDim.x pairs per step without a division in the loop
@@ -242,7 +254,7 @@ void ln_rows_kernel(T* __restrict__ X, const T* __restrict__ add, const int* __r
 }
 
 // OLMo / OLMo-2 attention prologue on the fused QKV rows ([Q heads | K heads | V heads], 128 wide), HF's order.  One
-// block per token; positions restart at 0 in every packed sequence.
+// block per token; positions as seq_position (restarting at 0 in every packed sequence, or explicit).
 //   clip > 0 (OLMo clip_qkv): every Q, K and V element is clamped to [-clip, clip] (in fp32, rounded to half).
 //   qn != nullptr (OLMo-2 q_norm / k_norm): Q = fp16(qn * (Q * rsqrt(mean(Q^2) + eps))) over the whole Q projection
 //   (heads x 128 wide, not per head), K likewise with kn over kv_heads x 128: fp32 statistics, the weight multiply in
@@ -251,12 +263,12 @@ void ln_rows_kernel(T* __restrict__ X, const T* __restrict__ add, const int* __r
 //   evaluated in fp32 (each product and the sum one fp32 rounding, as torch promotes) and rounded to half once.
 template <typename T>
 __global__ __launch_bounds__(256)
-void olmo_qkv_kernel(T* __restrict__ qkv, const int* __restrict__ cu_seqlens, int B, int heads, int kv_heads,
-                     const float* __restrict__ inv_freq, float clip, const T* __restrict__ qn,
+void olmo_qkv_kernel(T* __restrict__ qkv, const int* __restrict__ cu_seqlens, int B, const int* __restrict__ positions,
+                     int heads, int kv_heads, const float* __restrict__ inv_freq, float clip, const T* __restrict__ qn,
                      const T* __restrict__ kn, float eps) {
     __shared__ float red[8];
     const int t = blockIdx.x;
-    const float pos = (float)seq_position(cu_seqlens, B, t);
+    const float pos = (float)seq_position(cu_seqlens, B, positions, t);
     const int nq = heads * HD, nk = kv_heads * HD;
     T* row = qkv + (size_t)t * (nq + 2 * nk);
     float rq = 1.f, rk = 1.f;
@@ -516,6 +528,189 @@ void attention_causal_kernel(const T* __restrict__ qkv, const int* __restrict__ 
 }
 constexpr size_t attention_dyn_smem(int D) { return D > 128 ? 3 * (size_t)AK * (D + 8) * sizeof(__half) : 0; }   // 2-byte elements in both dtypes
 
+// KV cache of a generate call, per layer [slots][kv_heads][cap][head_dim] for K and again for V: one (sequence, KV head)
+// is a contiguous run of positions.  Row t of the fused QKV rows goes to slot b, position p: in a prefill (slot ==
+// nullptr) b is its packed sequence and p its position there, in a decode step b = slot[t] and p = pos[t].  K is stored
+// after RoPE (OLMo: after clip_qkv and QK-norm), the values the attention kernels read.  One block per row.
+template <typename T>
+__global__ void kv_store_kernel(const T* __restrict__ qkv, const int* __restrict__ cu_seqlens, int B,
+                                const int* __restrict__ slot, const int* __restrict__ pos, int heads, int kv_heads,
+                                int hd, int cap, T* __restrict__ kc, T* __restrict__ vc) {
+    const int t = blockIdx.x;
+    const int b = slot ? slot[t] : seq_index(cu_seqlens, B, t);
+    const int p = seq_position(cu_seqlens, B, pos, t);
+    const int ld = (heads + 2 * kv_heads) * hd, n8 = hd / 8;
+    const uint4* k = reinterpret_cast<const uint4*>(qkv + (size_t)t * ld + heads * hd);
+    const uint4* v = k + kv_heads * n8;
+    for (int e = threadIdx.x; e < kv_heads * n8; e += blockDim.x) {
+        const int kvh = e / n8, c = e - kvh * n8;
+        const size_t dst = (((size_t)b * kv_heads + kvh) * cap + p) * n8 + c;
+        reinterpret_cast<uint4*>(kc)[dst] = k[e];
+        reinterpret_cast<uint4*>(vc)[dst] = v[e];
+    }
+}
+
+// Split-KV decode attention (flash-decoding).  Row i (one query token per live sequence) attends to positions
+// [0, pos[i]] of its cache slot.  The positions are cut into chunks of DCH; warp w of block (x, y, i) takes chunk c =
+// 4x + w and, as the rows of one 16-row mma tile, query heads 16 gt .. 16 gt + 15 of the G = heads / kv_heads that read
+// KV head kvh, with y = kvh * ceil(G / 16) + gt.  For G <= 16 (every GQA reader released so far) one tile holds the
+// whole group, so every cached byte is read once per step; a larger group (multi-query attention) reads it once per
+// tile.  Chunk boundaries depend on the position only, never on the batch, so a
+// sequence's result is the same in any batch.  Per chunk the warp stages Q (once) and 16 keys of K and V at a time in
+// its own shared memory, computes S = Q K^T and O += P V on mma.sync.m16n8k16 with fp32 accumulators, online softmax
+// in the log2 domain with fp32 running max and sum, P rounded to the dtype for P V (the prefill kernel's numerics).
+// It writes the unnormalised O [D] and (max, sum) of every query head to part; decode_combine_kernel merges them.
+constexpr int DCH = 64;                          // positions per chunk
+constexpr int DEC_WARPS = 4;
+template <int D> constexpr size_t decode_smem() { return (size_t)DEC_WARPS * 3 * 16 * (D + 8) * sizeof(__half); }
+
+template <int D, typename T>
+__global__ __launch_bounds__(32 * DEC_WARPS)
+void decode_attention_kernel(const T* __restrict__ qkv, const T* __restrict__ kc, const T* __restrict__ vc,
+                             const int* __restrict__ slot, const int* __restrict__ pos, int heads, int kv_heads, int cap,
+                             int chunks, float scale_log2, float* __restrict__ part_o, float2* __restrict__ part_ml) {
+    constexpr int PAD = D + 8, KS = D / 16, NT = D / 8, N8 = D / 8;
+    extern __shared__ __align__(16) unsigned char dec_smem[];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
+    const int G = heads / kv_heads, gtiles = (G + 15) / 16, ld = (heads + 2 * kv_heads) * D;
+    const int c = blockIdx.x * DEC_WARPS + w, kvh = blockIdx.y / gtiles, g0 = (blockIdx.y - kvh * gtiles) * 16;
+    const int i = blockIdx.z, nq = min(16, G - g0);   // query heads kvh * G + g0 .. + nq - 1
+    const int L = pos[i] + 1, k_begin = c * DCH;
+    if (k_begin >= L) return;                    // warp-uniform; no block-wide barrier below
+    T (*Qs)[PAD] = reinterpret_cast<T (*)[PAD]>(dec_smem + (size_t)w * 3 * 16 * PAD * sizeof(T));
+    T (*Ks)[PAD] = Qs + 16;
+    T (*Vs)[PAD] = Qs + 32;
+    const T* q = qkv + (size_t)i * ld + ((size_t)kvh * G + g0) * D;
+    const size_t base = ((size_t)slot[i] * kv_heads + kvh) * cap * D;
+    const T* kb = kc + base;
+    const T* vb = vc + base;
+    for (int e = lane; e < 16 * N8; e += 32) {   // the tile's query heads; rows >= nq are zero
+        const int r = e / N8, cc = e - r * N8;
+        *reinterpret_cast<uint4*>(&Qs[r][cc * 8]) =
+            r < nq ? reinterpret_cast<const uint4*>(q + (size_t)r * D)[cc] : make_uint4(0, 0, 0, 0);
+    }
+    float o[NT][4];
+#pragma unroll
+    for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) o[nt][e] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+    const int k_end = min(L, k_begin + DCH);
+    for (int k0 = k_begin; k0 < k_end; k0 += 16) {
+        __syncwarp();                            // the previous step's tiles (and the Q rows) are in place / consumed
+        for (int e = lane; e < 16 * N8; e += 32) {   // keys past the row's length are zero, never stale cache
+            const int r = e / N8, cc = e - r * N8, key = k0 + r;
+            uint4 kv = make_uint4(0, 0, 0, 0), vv = kv;
+            if (key < k_end) {
+                kv = reinterpret_cast<const uint4*>(kb + (size_t)key * D)[cc];
+                vv = reinterpret_cast<const uint4*>(vb + (size_t)key * D)[cc];
+            }
+            *reinterpret_cast<uint4*>(&Ks[r][cc * 8]) = kv;
+            *reinterpret_cast<uint4*>(&Vs[r][cc * 8]) = vv;
+        }
+        __syncwarp();
+        float sacc[2][4];
+#pragma unroll
+        for (int nt = 0; nt < 2; ++nt)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) sacc[nt][e] = 0.f;
+#pragma unroll
+        for (int ks = 0; ks < KS; ++ks) {
+            uint32_t qa[4];
+            const uint32_t addr = (uint32_t)__cvta_generic_to_shared(&Qs[lane & 15][ks * 16 + (lane >> 4) * 8]);
+            asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
+                         : "=r"(qa[0]), "=r"(qa[1]), "=r"(qa[2]), "=r"(qa[3]) : "r"(addr));
+#pragma unroll
+            for (int nt = 0; nt < 2; ++nt) {
+                const int j = nt * 8 + g, cc = ks * 16 + 2 * t;
+                const uint32_t kf[2] = {ld32(&Ks[j][cc]), ld32(&Ks[j][cc + 8])};
+                mma16816<T>(sacc[nt], qa, kf);
+            }
+        }
+        float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+        for (int nt = 0; nt < 2; ++nt)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const int key = k0 + nt * 8 + 2 * t + (e & 1);
+                const float sv = key < k_end ? sacc[nt][e] * scale_log2 : -INFINITY;
+                sacc[nt][e] = sv;
+                mx[e >> 1] = fmaxf(mx[e >> 1], sv);
+            }
+        float corr[2], mref[2];
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+            mx[hr] = fmaxf(mx[hr], __shfl_xor_sync(0xffffffffu, mx[hr], 1));
+            mx[hr] = fmaxf(mx[hr], __shfl_xor_sync(0xffffffffu, mx[hr], 2));
+            const float mn = fmaxf(m_run[hr], mx[hr]);   // finite: key k0 < k_end is valid in every step
+            mref[hr] = mn;
+            corr[hr] = exp2f(m_run[hr] - mref[hr]);
+            m_run[hr] = mn;
+        }
+        float sum[2] = {0.f, 0.f};
+#pragma unroll
+        for (int nt = 0; nt < 2; ++nt)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const float p = exp2f(sacc[nt][e] - mref[e >> 1]);
+                sacc[nt][e] = p;
+                sum[e >> 1] += p;
+            }
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) l_run[hr] = l_run[hr] * corr[hr] + sum[hr];
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt) {
+            o[nt][0] *= corr[0]; o[nt][1] *= corr[0];
+            o[nt][2] *= corr[1]; o[nt][3] *= corr[1];
+        }
+        const uint32_t pa[4] = {pair_bits<T>(sacc[0][0], sacc[0][1]), pair_bits<T>(sacc[0][2], sacc[0][3]),
+                                pair_bits<T>(sacc[1][0], sacc[1][1]), pair_bits<T>(sacc[1][2], sacc[1][3])};
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt) {
+            uint32_t vf[2];
+            const uint32_t addr = (uint32_t)__cvta_generic_to_shared(&Vs[lane & 15][nt * 8]);
+            asm volatile("ldmatrix.sync.aligned.m8n8.x2.trans.shared.b16 {%0,%1}, [%2];" : "=r"(vf[0]), "=r"(vf[1]) : "r"(addr));
+            mma16816<T>(o[nt], pa, vf);
+        }
+    }
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+        l_run[hr] += __shfl_xor_sync(0xffffffffu, l_run[hr], 1);
+        l_run[hr] += __shfl_xor_sync(0xffffffffu, l_run[hr], 2);
+    }
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+        const int r = g + 8 * hr;                // query head kvh * G + g0 + r
+        if (r >= nq) continue;
+        const size_t idx = ((size_t)i * heads + kvh * G + g0 + r) * chunks + c;
+        float* po = part_o + idx * D;
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt)
+            *reinterpret_cast<float2*>(po + nt * 8 + 2 * t) = make_float2(o[nt][2 * hr], o[nt][2 * hr + 1]);
+        if (t == 0) part_ml[idx] = make_float2(m_run[hr], l_run[hr]);
+    }
+}
+
+// ctx[i, h] = sum_c 2^(m_c - M) O_c / sum_c 2^(m_c - M) l_c over the chunks of row i in chunk order, rounded to the
+// dtype once.  Block (h, i), one thread per element of the head.
+template <typename T>
+__global__ void decode_combine_kernel(const float* __restrict__ part_o, const float2* __restrict__ part_ml,
+                                      const int* __restrict__ pos, int heads, int D, int chunks, T* __restrict__ ctx) {
+    const int h = blockIdx.x, i = blockIdx.y, d = threadIdx.x;
+    const int n = (pos[i] + DCH) / DCH;          // chunks holding positions 0 .. pos[i]
+    const size_t base = ((size_t)i * heads + h) * chunks;
+    float M = -INFINITY;
+    for (int c = 0; c < n; ++c) M = fmaxf(M, part_ml[base + c].x);
+    float num = 0.f, den = 0.f;
+    for (int c = 0; c < n; ++c) {
+        const float2 ml = part_ml[base + c];
+        const float s = exp2f(ml.x - M);
+        num = fmaf(s, part_o[(base + c) * D + d], num);
+        den = fmaf(s, ml.y, den);
+    }
+    ctx[((size_t)i * heads + h) * D + d] = from_f<T>(num / den);
+}
+
 // act[t, j] = fp16(fp16(silu(gate[t, j])) * up[t, j]) with gu = [gate | up] rows of 2 * inter; silu as torch computes it
 // on half, x / (1 + exp(-x)) in fp32 rounded to half.  8 elements per thread.
 template <typename T>
@@ -583,6 +778,63 @@ void nll_rows_kernel(const T* __restrict__ logits, int vocab, int ld, const int*
         float M = rm[0], Sm = rs[0];
         for (int w = 1; w < (int)(blockDim.x >> 5); ++w) lse_merge(M, Sm, rm[w], rs[w]);
         nll_out[out_idx[i]] = (M + logf(Sm)) - to_f(row[labels[i]]);
+    }
+}
+
+// Greedy choice of row i: the argmax over logits[i, 0:vocab] compared in fp32, the lowest index on ties (torch.argmax);
+// the LM head's pad columns vocab..ld-1 never compete.  Writes the id to next[i] and out_tokens[s, step], and its fp32
+// log-softmax logit - logsumexp (nll_rows_kernel's sum) to out_lp[s, step] when out_lp is given, with s = slot ? slot[i]
+// : base + i.  One block per row.
+template <typename T>
+__global__ __launch_bounds__(256)
+void greedy_rows_kernel(const T* __restrict__ logits, int vocab, int ld, const int* __restrict__ slot, int base,
+                        int step, int max_new, int* __restrict__ next, int* __restrict__ out_tokens,
+                        float* __restrict__ out_lp) {
+    __shared__ float rm[8], rs[8], rv[8];
+    __shared__ int ri[8];
+    const int i = blockIdx.x;
+    const T* row = logits + (size_t)i * ld;
+    float m = -INFINITY, s = 0.f, bv = -INFINITY;
+    int bi = INT_MAX;
+    for (int c = threadIdx.x * 8; c < vocab; c += blockDim.x * 8) {
+        const uint4 v = *reinterpret_cast<const uint4*>(row + c);
+        const T* hv = reinterpret_cast<const T*>(&v);
+        float x[8], mx = -INFINITY;
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+            x[e] = c + e < vocab ? to_f(hv[e]) : -INFINITY;
+            mx = fmaxf(mx, x[e]);
+            if (c + e < vocab && (x[e] > bv || (x[e] == bv && c + e < bi))) { bv = x[e]; bi = c + e; }
+        }
+        const float mn = fmaxf(m, mx);
+        float acc = s * expf(m - mn);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) acc += expf(x[e] - mn);
+        m = mn;
+        s = acc;
+    }
+    auto better = [](float v, int k, float bv, int bk) { return v > bv || (v == bv && k < bk); };
+    for (int off = 16; off > 0; off >>= 1) {
+        lse_merge(m, s, __shfl_xor_sync(0xffffffffu, m, off), __shfl_xor_sync(0xffffffffu, s, off));
+        const float ov = __shfl_xor_sync(0xffffffffu, bv, off);
+        const int oi = __shfl_xor_sync(0xffffffffu, bi, off);
+        if (better(ov, oi, bv, bi)) { bv = ov; bi = oi; }
+    }
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (lane == 0) { rm[warp] = m; rs[warp] = s; rv[warp] = bv; ri[warp] = bi; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float M = rm[0], Sm = rs[0], V = rv[0];
+        int I = ri[0];
+        for (int w = 1; w < (int)(blockDim.x >> 5); ++w) {
+            lse_merge(M, Sm, rm[w], rs[w]);
+            if (better(rv[w], ri[w], V, I)) { V = rv[w]; I = ri[w]; }
+        }
+        if (I >= vocab) I = 0;                   // every logit NaN: the log-probability below is NaN as well
+        const size_t o = (size_t)(slot ? slot[i] : base + i) * max_new + step;
+        next[i] = I;
+        out_tokens[o] = I;
+        if (out_lp) out_lp[o] = V - (M + logf(Sm));
     }
 }
 
@@ -928,20 +1180,68 @@ int upload_attention_items(const std::vector<int32_t>& cu, int B, int2* d_items,
     return RSB_OK;
 }
 
-// One attention step of layer l on the fused QKV rows [n_tok, qkv_n] of a batch whose windows end at n_tok = cu[B]:
-// RoPE on the Q and K heads in place (OLMo: the clip / QK-norm prologue and fp32 RoPE), then causal attention into CTX
-// [n_tok, hidden].
+// The KV cache of a generate call (kv_store_kernel's layout) and, in a decode step, where each row goes.
 template <typename E>
-void attention_step(const rsb_llm* h, const LlmLayer& l, E* QKV, const int32_t* cu_seqlens, int B, int n_tok,
-                    const int2* d_items, int n_items, E* CTX, cudaStream_t st) {
-    if (n_tok == 0 || n_items == 0) return;
+struct KvCache {
+    E *k, *v;                                    // [layers][slots][kv_heads][cap][head_dim] each
+    int slots, cap;
+    const int *slot = nullptr, *pos = nullptr;   // decode step: cache slot and position of each row; prefill: nullptr
+    float* part_o = nullptr;                     // decode step: split-KV partials of decode_attention_kernel
+    float2* part_ml = nullptr;
+    int chunks = 0;                              // decode step: DCH-position chunks of the longest row
+    size_t layer_elems(const rsb_llm* h) const { return (size_t)slots * h->kv_heads * cap * h->head_dim; }
+};
+
+template <int D, typename E>
+void launch_decode_attention(const rsb_llm* h, const E* QKV, const E* kc, const E* vc, const KvCache<E>& kv, int n_rows,
+                             float scale_log2, cudaStream_t st) {
+    constexpr size_t smem = decode_smem<D>();
+    static rsb::PerDeviceFlag configured;        // attributes are per (function, device)
+    if (configured.first())
+        cudaFuncSetAttribute(decode_attention_kernel<D, E>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    const int gtiles = (h->heads / h->kv_heads + 15) / 16;   // 16-row query-head tiles per KV head
+    const dim3 grid((unsigned)((kv.chunks + DEC_WARPS - 1) / DEC_WARPS), h->kv_heads * gtiles, n_rows);
+    decode_attention_kernel<D, E><<<grid, 32 * DEC_WARPS, smem, st>>>(QKV, kc, vc, kv.slot, kv.pos, h->heads, h->kv_heads,
+                                                                      kv.cap, kv.chunks, scale_log2, kv.part_o, kv.part_ml);
+}
+
+// One attention step of layer li on the fused QKV rows [n_tok, qkv_n]: RoPE on the Q and K heads in place (OLMo: the
+// clip / QK-norm prologue and fp32 RoPE), then attention into CTX [n_tok, hidden].
+//   kv == nullptr or a prefill (kv->pos == nullptr): rows are the packed windows of cu_seqlens, n_tok = cu[B], with
+//   positions restarting at 0 in each; causal attention.  With kv, K and V also go to the cache, slot b for window b.
+//   A decode step (kv->pos): row i is one token of cache slot kv->slot[i] at position kv->pos[i]; its K and V are
+//   appended there and it attends to positions 0 .. pos[i] of the slot (split-KV).
+template <typename E>
+void attention_step(const rsb_llm* h, int li, E* QKV, const int32_t* cu_seqlens, int B, int n_tok,
+                    const int2* d_items, int n_items, E* CTX, const KvCache<E>* kv, cudaStream_t st) {
+    const bool decode = kv && kv->pos;
+    if (n_tok == 0 || (!decode && n_items == 0)) return;
+    const LlmLayer& l = h->L[li];
+    const int* pos = decode ? kv->pos : nullptr;
     const float scale_log2 = 1.4426950408889634f / sqrtf((float)h->head_dim);   // 1/sqrt(head_dim) in the log2 domain
     if (h->family == RSB_LLM_OLMO || h->family == RSB_LLM_OLMO2)
-        olmo_qkv_kernel<E><<<n_tok, 256, 0, st>>>(QKV, cu_seqlens, B, h->heads, h->kv_heads, h->inv_freq, h->clip,
+        olmo_qkv_kernel<E><<<n_tok, 256, 0, st>>>(QKV, cu_seqlens, B, pos, h->heads, h->kv_heads, h->inv_freq, h->clip,
                                                   as<E>(l.qn), as<E>(l.kn), h->eps);
     else
-        rope_kernel<E><<<n_tok, 256, 0, st>>>(QKV, cu_seqlens, B, h->qkv_n(), h->heads + h->kv_heads, h->head_dim, h->rot,
-                                              h->inv_freq);
+        rope_kernel<E><<<n_tok, 256, 0, st>>>(QKV, cu_seqlens, B, pos, h->qkv_n(), h->heads + h->kv_heads, h->head_dim,
+                                              h->rot, h->inv_freq);
+    if (kv) {
+        E* kc = kv->k + (size_t)li * kv->layer_elems(h);
+        E* vc = kv->v + (size_t)li * kv->layer_elems(h);
+        kv_store_kernel<E><<<n_tok, 128, 0, st>>>(QKV, cu_seqlens, B, kv->slot, pos, h->heads, h->kv_heads, h->head_dim,
+                                                  kv->cap, kc, vc);
+        if (decode) {
+            switch (h->head_dim) {
+                case 64: launch_decode_attention<64>(h, QKV, kc, vc, *kv, n_tok, scale_log2, st); break;
+                case 80: launch_decode_attention<80>(h, QKV, kc, vc, *kv, n_tok, scale_log2, st); break;
+                case 128: launch_decode_attention<128>(h, QKV, kc, vc, *kv, n_tok, scale_log2, st); break;
+                default: launch_decode_attention<256>(h, QKV, kc, vc, *kv, n_tok, scale_log2, st);
+            }
+            decode_combine_kernel<E><<<dim3(h->heads, n_tok), h->head_dim, 0, st>>>(kv->part_o, kv->part_ml, pos, h->heads,
+                                                                                  h->head_dim, kv->chunks, CTX);
+            return;
+        }
+    }
     const dim3 grid((unsigned)n_items, h->heads);
     switch (h->head_dim) {
         case 64: attention_causal_kernel<64, E><<<grid, 128, 0, st>>>(QKV, cu_seqlens, d_items, CTX, h->heads, h->kv_heads, scale_log2); break;
@@ -984,13 +1284,14 @@ int check_forward(rsb_llm* h, const int32_t* ids, const int32_t* cu_seqlens, con
     return RSB_OK;
 }
 
-// Workspace slots of one forward (llm_ws_layout) and its attention work list.
+// Workspace slots of one forward (llm_ws_layout), its attention work list and, in rsb_llm_generate, the KV cache.
 template <typename E>
 struct Fwd {
     E *X, *Hn, *QKV, *CTX, *GU, *ACT;
     const int32_t* cu_seqlens;
     int B, T, n_items;
     const int2* d_items;
+    const KvCache<E>* kv = nullptr;
 };
 
 // The sequential-residual decoder layers, x layers.  LlamaDecoderLayer: x += o_proj(attn(rms1(x))); x +=
@@ -1025,7 +1326,7 @@ int sequential_layers(rsb_llm* h, const Fwd<E>& f, cudaStream_t st) {
         const LlmLayer& l = h->L[li];
         pre_norm(l.ln1);
         if ((rc = gemm(in, T, l.wqkv, NQKV, Hd, h->zero_bias, nullptr, f.QKV, 0, st)) != RSB_OK) return rc;
-        attention_step(h, l, f.QKV, f.cu_seqlens, f.B, T, f.d_items, f.n_items, f.CTX, st);
+        attention_step(h, li, f.QKV, f.cu_seqlens, f.B, T, f.d_items, f.n_items, f.CTX, f.kv, st);
         if ((rc = residual(f.CTX, l.wo, Hd, 0, l.ln1)) != RSB_OK) return rc;
         pre_norm(l.ln2);
         if ((rc = gemm(in, T, l.wgu, 2 * I, Hd, h->zero_bias, nullptr, f.GU, 0, st)) != RSB_OK) return rc;
@@ -1049,7 +1350,7 @@ int neox_layers(rsb_llm* h, const Fwd<E>& f, cudaStream_t st) {
     for (int li = 0; li < h->layers; ++li) {
         const LlmLayer& l = h->L[li];
         if ((rc = gemm(N1, T, l.wqkv, NQKV, Hd, l.bqkv, nullptr, f.QKV, 0, st)) != RSB_OK) return rc;
-        attention_step(h, l, f.QKV, f.cu_seqlens, f.B, T, f.d_items, f.n_items, f.CTX, st);
+        attention_step(h, li, f.QKV, f.cu_seqlens, f.B, T, f.d_items, f.n_items, f.CTX, f.kv, st);
         if ((rc = gemm(f.CTX, T, l.wo, Hd, Hd, l.bo, nullptr, A, 0, st)) != RSB_OK) return rc;
         if ((rc = gemm(N2, T, l.wgu, I, Hd, l.bgu, nullptr, FF, 1, st)) != RSB_OK) return rc;
         if ((rc = gemm(FF, T, l.wdown, Hd, I, l.bdown, A, A, 2 | RSB_GEMM_REVERSED, st)) != RSB_OK) return rc;
@@ -1062,9 +1363,10 @@ int neox_layers(rsb_llm* h, const Fwd<E>& f, cudaStream_t st) {
 }
 
 // The decoder layers: X (workspace slot 0) ends as the residual stream after the last layer, before the final norm.
+// Packed windows (cu, cu_seqlens), or with kv->pos one row per live sequence of a decode step (cu_seqlens unused).
 template <typename E>
 int trunk(rsb_llm* h, const int32_t* ids, const int32_t* cu_seqlens, int B, int T, const std::vector<int32_t>& cu,
-          unsigned char* w, const size_t off[10], cudaStream_t st) {
+          unsigned char* w, const size_t off[10], cudaStream_t st, const KvCache<E>* kv = nullptr) {
     Fwd<E> f;
     f.X = reinterpret_cast<E*>(w + off[0]);
     f.Hn = reinterpret_cast<E*>(w + off[1]);
@@ -1075,10 +1377,12 @@ int trunk(rsb_llm* h, const int32_t* ids, const int32_t* cu_seqlens, int B, int 
     f.cu_seqlens = cu_seqlens;
     f.B = B;
     f.T = T;
+    f.kv = kv;
     int2* d_items = reinterpret_cast<int2*>(w + off[8]);
     f.d_items = d_items;
+    f.n_items = 0;
     int rc;
-    if ((rc = upload_attention_items(cu, B, d_items, st, &f.n_items)) != RSB_OK) return rc;
+    if (!(kv && kv->pos) && (rc = upload_attention_items(cu, B, d_items, st, &f.n_items)) != RSB_OK) return rc;
     embed_rows_kernel<E><<<T, 128, 0, st>>>(ids, as<E>(h->embed), h->hidden, f.X);
     return h->family == RSB_LLM_NEOX ? neox_layers(h, f, st) : sequential_layers(h, f, st);
 }
@@ -1176,6 +1480,146 @@ extern "C" int rsb_llm_hidden_states(rsb_llm_t* h, const int32_t* ids, const int
     return RSB_OK;
 }
 
+namespace {
+
+// rsb_llm_generate's workspace: the forward's slots for the T context tokens with B label rows (every decode step runs
+// at most B rows through the same slots), then the KV cache, the split-KV partials and four int tables of B entries
+// (slot, position, id and chosen id of each decode row).  The cache holds max_seqlen + max_new_tokens - 1 positions per
+// slot: the last chosen token is never fed back.
+struct GenLayout {
+    size_t off[10], k, v, part_o, part_ml, ints, total;
+    int cap, chunks;
+};
+GenLayout gen_layout(const rsb_llm* h, size_t B, size_t T, int max_seqlen, int max_new_tokens) {
+    auto al = [](size_t x) { return (x + 1023) / 1024 * 1024; };
+    GenLayout g;
+    size_t o = llm_ws_layout(h, T, B, g.off);
+    g.cap = max_seqlen + max_new_tokens - 1;
+    g.chunks = (g.cap + DCH - 1) / DCH;
+    const size_t kv_bytes = (size_t)h->layers * B * h->kv_heads * (size_t)g.cap * h->head_dim * 2;
+    const size_t parts = B * h->heads * (size_t)g.chunks;
+    g.k = o; o += al(kv_bytes);
+    g.v = o; o += al(kv_bytes);
+    g.part_o = o; o += al(parts * h->head_dim * sizeof(float));
+    g.part_ml = o; o += al(parts * sizeof(float2));
+    g.ints = o; o += al(4 * B * sizeof(int));
+    g.total = o;
+    return g;
+}
+
+}  // namespace
+
+extern "C" size_t rsb_llm_generate_workspace_bytes(rsb_llm_t* h, int B, int T, int max_seqlen, int max_new_tokens) {
+    if (!h || B <= 0 || T <= 0 || max_seqlen <= 0 || max_new_tokens <= 0) return 0;
+    return gen_layout(h, (size_t)B, (size_t)T, max_seqlen, max_new_tokens).total;
+}
+
+// Greedy decoding of HF `model.generate(do_sample=False, num_beams=1)` from B packed contexts (rsb.h): a prefill over
+// the contexts that fills the KV cache and chooses each sequence's first token, then one decode step per token for the
+// sequences still running, through the same layer loops at M = live rows.  One read-back of the chosen ids per step.
+extern "C" int rsb_llm_generate(rsb_llm_t* h, const int32_t* ids, const int32_t* cu_seqlens, int B, int T, int max_seqlen,
+                                int max_new_tokens, const int32_t* eos_ids, int n_eos, int32_t* out_tokens,
+                                int32_t* out_lens, float* out_logprob, void* ws, size_t ws_bytes, rsb_stream_t stream) {
+    if (!h || !ids || !cu_seqlens || !out_tokens || !out_lens || !ws || (n_eos > 0 && !eos_ids))
+        return lfail(RSB_ERR_INVALID, "null argument");
+    if (max_new_tokens <= 0 || n_eos < 0) return lfail(RSB_ERR_INVALID, "max_new_tokens must be positive and n_eos >= 0");
+    if ((long long)max_seqlen + max_new_tokens > h->max_pos)
+        return lfail(RSB_ERR_UNSUPPORTED, "a context of %ld tokens plus %ld new tokens is longer than "
+                     "max_position_embeddings (%ld)", (long)max_seqlen, (long)max_new_tokens, (long)h->max_pos);
+    cudaStream_t st = (cudaStream_t)stream;
+    std::vector<int32_t> cu, lab;
+    int rc = check_forward(h, ids, cu_seqlens, nullptr, B, T, max_seqlen, st, cu, lab);
+    if (rc != RSB_OK) return rc;
+    for (int b = 0; b < B; ++b)
+        if (cu[b + 1] == cu[b]) return lfail(RSB_ERR_INVALID, "context %ld is empty", (long)b);
+    const GenLayout g = gen_layout(h, (size_t)B, (size_t)T, max_seqlen, max_new_tokens);
+    if (ws_bytes < g.total) return lfail(RSB_ERR_OOM, "generate workspace too small (need %ld bytes)", (long)g.total);
+    unsigned char* w = static_cast<unsigned char*>(ws);
+    int* d_rows = reinterpret_cast<int*>(w + g.off[7]);
+    int* d_ints = reinterpret_cast<int*>(w + g.ints);   // slot | pos | ids of n decode rows, then next at 3B
+    int* d_next = d_ints + 3 * (size_t)B;
+    std::vector<int32_t> ctx(B), rows(B);
+    for (int b = 0; b < B; ++b) { ctx[b] = cu[b + 1] - cu[b]; rows[b] = cu[b + 1] - 1; }
+    const size_t n_out = (size_t)B * max_new_tokens;
+    if (cudaMemcpyAsync(d_rows, rows.data(), (size_t)B * 4, cudaMemcpyHostToDevice, st) != cudaSuccess ||
+        cudaMemsetAsync(out_tokens, 0xFF, n_out * 4, st) != cudaSuccess ||
+        (out_logprob && cudaMemsetAsync(out_logprob, 0, n_out * 4, st) != cudaSuccess))
+        return lfail(RSB_ERR_CUDA, "initialising the generate buffers failed");
+    const std::vector<int32_t> eos(eos_ids, eos_ids + std::max(n_eos, 0));
+    auto ends = [&](int tok, int len) { return len == max_new_tokens || std::find(eos.begin(), eos.end(), tok) != eos.end(); };
+    std::vector<int32_t> tok(B), lens(B, 0), next(B), host(3 * (size_t)B), live;
+    rc = with_dtype(h, [&](auto tag) -> int {
+        using E = decltype(tag);
+        KvCache<E> kv;
+        kv.k = reinterpret_cast<E*>(w + g.k);
+        kv.v = reinterpret_cast<E*>(w + g.v);
+        kv.slots = B;
+        kv.cap = g.cap;
+        E* X = reinterpret_cast<E*>(w + g.off[0]);
+        E* Hn = reinterpret_cast<E*>(w + g.off[1]);
+        E* LOG = reinterpret_cast<E*>(w + g.off[6]);
+        const int Hd = h->hidden, chunk = h->chunk_rows();
+        // final norm, LM head and greedy choice of n rows (X rows[i], or X row i), read back into next
+        auto choose = [&](const int* d_r, int n, const int* slot, int step) -> int {
+            int rc;
+            for (int c0 = 0; c0 < n; c0 += chunk) {
+                const int m = std::min(chunk, n - c0);
+                final_norm<E>(h, d_r ? X : X + (size_t)c0 * Hd, d_r ? d_r + c0 : nullptr, m, Hn, st);
+                if ((rc = gemm<E>(Hn, m, h->lm_head, h->vocab_pad, Hd, h->zero_bias, nullptr, LOG, 0, st)) != RSB_OK) return rc;
+                greedy_rows_kernel<E><<<m, 256, 0, st>>>(LOG, h->vocab, h->vocab_pad, slot ? slot + c0 : nullptr, c0, step,
+                                                         max_new_tokens, d_next + c0, out_tokens, out_logprob);
+            }
+            if (cudaMemcpyAsync(next.data(), d_next, (size_t)n * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+                cudaStreamSynchronize(st) != cudaSuccess)
+                return lfail(RSB_ERR_CUDA, "generate step failed: %s", cudaGetErrorString(cudaGetLastError()));
+            return RSB_OK;
+        };
+        int rc = trunk<E>(h, ids, cu_seqlens, B, T, cu, w, g.off, st, &kv);
+        if (rc != RSB_OK || (rc = choose(d_rows, B, nullptr, 0)) != RSB_OK) return rc;
+        for (int b = 0; b < B; ++b) {
+            tok[b] = next[b];
+            lens[b] = 1;
+            if (!ends(tok[b], 1)) live.push_back(b);
+        }
+        for (int step = 1; step < max_new_tokens && !live.empty(); ++step) {
+            const int n = (int)live.size();
+            int max_p = 0;
+            for (int i = 0; i < n; ++i) {
+                const int b = live[i];
+                host[i] = b;
+                host[n + i] = ctx[b] + step - 1;   // the token chosen at step - 1 sits right after the previous one
+                host[2 * n + i] = tok[b];
+                max_p = std::max(max_p, host[n + i]);
+            }
+            if (cudaMemcpyAsync(d_ints, host.data(), (size_t)3 * n * 4, cudaMemcpyHostToDevice, st) != cudaSuccess)
+                return lfail(RSB_ERR_CUDA, "uploading the decode rows failed");
+            kv.slot = d_ints;
+            kv.pos = d_ints + n;
+            kv.chunks = max_p / DCH + 1;
+            kv.part_o = reinterpret_cast<float*>(w + g.part_o);
+            kv.part_ml = reinterpret_cast<float2*>(w + g.part_ml);
+            if ((rc = trunk<E>(h, d_ints + 2 * n, nullptr, n, n, cu, w, g.off, st, &kv)) != RSB_OK) return rc;
+            if ((rc = choose(nullptr, n, d_ints, step)) != RSB_OK) return rc;
+            std::vector<int32_t> still;
+            for (int i = 0; i < n; ++i) {
+                const int b = live[i];
+                tok[b] = next[i];
+                lens[b] = step + 1;
+                if (!ends(tok[b], step + 1)) still.push_back(b);
+            }
+            live.swap(still);
+        }
+        return RSB_OK;
+    });
+    if (rc != RSB_OK) return rc;
+    if (cudaMemcpyAsync(out_lens, lens.data(), (size_t)B * 4, cudaMemcpyHostToDevice, st) != cudaSuccess ||
+        cudaStreamSynchronize(st) != cudaSuccess)
+        return lfail(RSB_ERR_CUDA, "writing out_lens failed");
+    const cudaError_t e = cudaPeekAtLastError();
+    if (e != cudaSuccess) return lfail(RSB_ERR_CUDA, "generate launch failed: %s", cudaGetErrorString(e));
+    return RSB_OK;
+}
+
 // Diagnostic: one attention step of the forward on a caller's fused QKV rows [T, (heads + 2 kv_heads) head_dim] in the
 // handle's dtype (GPT-NeoX: [Q heads | K heads | V heads], as rsb_llm_load permutes query_key_value).
 extern "C" int rsb_llm_attention(rsb_llm_t* h, void* qkv, const int32_t* cu_seqlens, int B, int T, int max_seqlen,
@@ -1202,8 +1646,8 @@ extern "C" int rsb_llm_attention(rsb_llm_t* h, void* qkv, const int32_t* cu_seql
     if (rc == RSB_OK)
         with_dtype(h, [&](auto tag) -> int {
             using E = decltype(tag);
-            attention_step<E>(h, h->L[0], static_cast<E*>(qkv), cu_seqlens, B, cu[B], d_items, n_items,
-                              static_cast<E*>(ctx), st);
+            attention_step<E>(h, 0, static_cast<E*>(qkv), cu_seqlens, B, cu[B], d_items, n_items,
+                              static_cast<E*>(ctx), nullptr, st);
             return RSB_OK;
         });
     if (d_items) cudaFreeAsync(d_items, st);

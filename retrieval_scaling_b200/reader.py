@@ -9,6 +9,7 @@ and calls `lm(input_ids, labels=labels)` one window at a time (`src/evaluate_per
     model = load_reader(path, dtype=torch.bfloat16)             # the reference's reader dtype
     nll = model.nll([ids_0, ids_1, ...], [labels_0, ...])       # per-token NLL, many windows per forward
     losses = model.loss([ids_0, ...], [labels_0, ...])          # HF's per-window mean loss
+    new_ids = model.generate([prompt_0, ...], 256, eos_ids)      # greedy decoding with a KV cache (rsb_llm_generate)
 
 runs `rsb_llm_nll`: a prefill-only forward over packed, un-padded windows whose LM head runs only on the rows whose
 next token is a label.  `load_reader` picks `B200Llama`, `B200NeoX` or `B200Olmo` from the config's `model_type`.  No CPU /
@@ -24,6 +25,7 @@ import math
 import os
 from typing import Dict, List, Optional, Sequence
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -384,6 +386,74 @@ class _Reader:
             out += self._nll_packed(ids[i:j], labels[i:j])
             i = j
         return out
+
+    # -- greedy generation (rsb_llm_generate) ---------------------------------------------------------------------
+    # share of the free device memory one generate call's workspace (KV cache, activations, partials) may take
+    generate_memory_share = 0.8
+
+    def _generate_batch(self, prompts, max_new: int, eos: List[int]):
+        lens = [len(p) for p in prompts]
+        B, T = len(prompts), sum(lens)
+        dev = self.device
+        ids = torch.tensor([v for p in prompts for v in p], dtype=torch.int32, device=dev)
+        cu = torch.tensor([0] + list(np.cumsum(lens)), dtype=torch.int32, device=dev)
+        toks = torch.empty((B, max_new), dtype=torch.int32, device=dev)
+        out_lens = torch.empty(B, dtype=torch.int32, device=dev)
+        lp = torch.empty((B, max_new), dtype=torch.float32, device=dev)
+        ws = torch.empty(self.L.rsb_llm_generate_workspace_bytes(self._h, B, T, max(lens), max_new), dtype=torch.uint8,
+                         device=dev)
+        eos_arr = (ctypes.c_int32 * max(len(eos), 1))(*eos)
+        with torch.cuda.device(dev):
+            rc = self.L.rsb_llm_generate(self._h, ctypes.c_void_p(ids.data_ptr()), ctypes.c_void_p(cu.data_ptr()), B, T,
+                                         max(lens), max_new, eos_arr, len(eos), ctypes.c_void_p(toks.data_ptr()),
+                                         ctypes.c_void_p(out_lens.data_ptr()), ctypes.c_void_p(lp.data_ptr()),
+                                         ctypes.c_void_p(ws.data_ptr()), ws.numel(),
+                                         ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+        self._check(rc)
+        n = out_lens.cpu().tolist()
+        toks, lp = toks.cpu(), lp.cpu()
+        out = [(toks[b, :n[b]].tolist(), lp[b, :n[b]].clone()) for b in range(B)]
+        if not all(bool(torch.isfinite(x).all()) for _, x in out):
+            raise FloatingPointError(f"non-finite logits while generating: the {READER_DTYPES[self.dtype]} activations "
+                                     f"overflowed or the checkpoint's weights produce NaN"
+                                     + (" (a bf16 reader may evaluate it)" if self.dtype == torch.float16 else ""))
+        return out
+
+    def generate(self, prompt_ids, max_new_tokens: int, eos_token_ids=(), return_logprobs: bool = False):
+        """Greedy continuation of every prompt (HF `generate(do_sample=False)` with `eos_token_id=eos_token_ids`): per
+        prompt, in input order, the new ids, ending after the first id of `eos_token_ids` (included) or after
+        `max_new_tokens` ids.  With return_logprobs, also each id's fp32 log-softmax (a float32 tensor per prompt).
+        Prompts run longest first, as many per call as the workspace (KV cache included) fits in
+        `generate_memory_share` of the free device memory; a prompt's ids do not depend on the others.  Raises
+        FloatingPointError on non-finite logits; a prompt plus max_new_tokens past max_position_embeddings raises
+        NotImplementedError."""
+        prompts = [[int(v) for v in p] for p in prompt_ids]
+        max_new = int(max_new_tokens)
+        if max_new <= 0:
+            raise ValueError(f"max_new_tokens {max_new_tokens} must be positive")
+        if any(len(p) == 0 for p in prompts):
+            raise ValueError("empty prompt")
+        eos = [int(eos_token_ids)] if isinstance(eos_token_ids, int) else [int(e) for e in (eos_token_ids or ())]
+        order = sorted(range(len(prompts)), key=lambda i: -len(prompts[i]))
+        with torch.cuda.device(self.device):
+            free = torch.cuda.mem_get_info(self.device)[0] + torch.cuda.memory_reserved(self.device) \
+                - torch.cuda.memory_allocated(self.device)
+        budget = self.generate_memory_share * free
+        res: List = [None] * len(prompts)
+        i = 0
+        while i < len(order):
+            j, T = i + 1, len(prompts[order[i]])
+            longest = T
+            while j < len(order) and self.L.rsb_llm_generate_workspace_bytes(
+                    self._h, j + 1 - i, T + len(prompts[order[j]]), longest, max_new) <= budget:
+                T += len(prompts[order[j]])
+                j += 1
+            for k, r in zip(order[i:j], self._generate_batch([prompts[k] for k in order[i:j]], max_new, eos)):
+                res[k] = r
+            i = j
+        if return_logprobs:
+            return [r[0] for r in res], [r[1] for r in res]
+        return [r[0] for r in res]
 
     # -- diagnostics (rsb_llm_attention / rsb_llm_hidden_states), not used by nll / loss ----------------------------
     def attention(self, qkv: torch.Tensor, cu_seqlens: torch.Tensor, max_seqlen: int, ctx: torch.Tensor):

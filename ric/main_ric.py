@@ -9,7 +9,8 @@ tasks.datastore.index (build or load the index; with model.sparse_retriever=bm25
 under {passages_dir}/bm25/{ids}/rsb_index), tasks.eval.search (query -> top-k, the hot path; dense, or BM25 on the GPU),
 tasks.eval.merge_search (multi-source merge, MinHash de-duplication on the GPU and subsampling, reference :31-33),
 tasks.eval.inference (task_name perplexity: reader-LM perplexity with concate_k retrieved documents prepended, the
-Llama reader on the GPU, reference :35-38; perplexity_calibration and lm-eval raise NotImplementedError).
+Llama reader on the GPU, reference :35-38; task_name lm-eval: retrieval-augmented QA with greedy generation on the GPU
+reader, the lm-eval fork's generate_until; perplexity_calibration raises NotImplementedError).
 """
 import logging
 import os
@@ -69,10 +70,15 @@ def main(cfg) -> None:
         logging.info("\n\n************** Post Merging Searched Results from Multiple Domains ***********")
         from retrieval_scaling_b200.search import post_hoc_merge_topk_multi_domain
         post_hoc_merge_topk_multi_domain(cfg)
-    if cfg.tasks.eval.get("inference", False):
+    if cfg.tasks.eval.get("inference", False) and cfg.tasks.eval.get("task_name", "perplexity") == "lm-eval":
+        logging.info("\n\n************** Running Retrieval-Augmented QA ***********")
+        from retrieval_scaling_b200 import rag_qa
+        outputs = rag_qa.evaluate_lm_eval(cfg)   # the lm-eval fork's generate_until with --retrieval_file
+        rag_qa.log_results_separately(cfg, outputs)
+    elif cfg.tasks.eval.get("inference", False):
         logging.info("\n\n************** Running Perplexity Evaluation ***********")
         from retrieval_scaling_b200.perplexity import evaluate_perplexity, log_results_separately
-        outputs = evaluate_perplexity(cfg)     # reference :36-39; perplexity_calibration / lm-eval: NotImplementedError
+        outputs = evaluate_perplexity(cfg)     # reference :36-39; perplexity_calibration: NotImplementedError
         log_results_separately(cfg, outputs)
 
 
