@@ -559,6 +559,27 @@ int rsb_llm_generate(rsb_llm_t* h, const int32_t* ids_dev, const int32_t* cu_seq
  * other weight needs to be loaded. */
 int rsb_llm_attention(rsb_llm_t* h, void* qkv_dev, const int32_t* cu_seqlens_dev, int B, int T, int max_seqlen,
                       void* ctx_dev, rsb_stream_t stream);
+/* Diagnostic, not used on the product path: one decode step of rsb_llm_generate's attention (layer 0's prologue) on
+ * caller-owned buffers.  qkv_dev [n_rows, (heads + 2 kv_heads) head_dim] in the handle's dtype holds one token per
+ * row; row i belongs to cache slot slot_dev[i] at position pos_dev[i] (int32 on the device).  Its Q and K heads are
+ * rotated in place at that position (OLMo / OLMo-2: the clip_qkv clamp or QK-norm first, as rsb_llm_attention), its K
+ * and V go to k_cache_dev / v_cache_dev [slots][kv_heads][cap][head_dim] (one layer of the generate KV cache) at
+ * (slot, :, pos), and ctx_dev [n_rows, heads head_dim] receives softmax(q k^T / sqrt(head_dim)) v over positions
+ * 0 .. pos of the slot, query head h reading KV head h / (heads / kv_heads), through the split-KV kernels.  No other
+ * cache element is written.  Before any launch: a null pointer, n_rows, slots or cap <= 0, or a buffer that is not
+ * 16-byte aligned RSB_ERR_INVALID; then slot_dev and pos_dev are read back: a slot outside [0, slots), two rows on one
+ * slot, or a position outside [0, cap) RSB_ERR_INVALID, a position >= max_pos RSB_ERR_UNSUPPORTED; OLMo-2 without
+ * layer 0's q_norm / k_norm RSB_ERR_STATE.  No other weight needs to be loaded. */
+int rsb_llm_decode_attention(rsb_llm_t* h, void* qkv_dev, const int32_t* slot_dev, const int32_t* pos_dev, int n_rows,
+                             void* k_cache_dev, void* v_cache_dev, int slots, int cap, void* ctx_dev,
+                             rsb_stream_t stream);
+/* Diagnostic, not used on the product path: rsb_llm_generate's greedy choice on caller logits.  logits_dev [n_rows, ld]
+ * in dtype (RSB_DTYPE_F16 or RSB_DTYPE_BF16); columns [vocab, ld) are padding and never chosen nor summed.  ids_dev
+ * [n_rows] int32 receives the argmax over [0, vocab) compared in fp32, the lowest id on ties, and logprob_dev [n_rows]
+ * fp32 its log-softmax.  Before any launch: another dtype, a null pointer, vocab <= 0, ld < vocab, ld % 8 != 0,
+ * n_rows < 0 or logits_dev not 16-byte aligned RSB_ERR_INVALID.  No handle is needed. */
+int rsb_llm_greedy(int dtype, const void* logits_dev, int vocab, int ld, int n_rows, int32_t* ids_dev,
+                   float* logprob_dev, rsb_stream_t stream);
 /* Diagnostic, not used on the product path: the residual stream after the last decoder layer of rsb_llm_nll's forward,
  * before the final norm, out_dev [T, hidden] in the handle's dtype.  The refusals of rsb_llm_nll apply; the workspace is
  * rsb_llm_workspace_bytes(h, T, 0). */

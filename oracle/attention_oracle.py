@@ -17,11 +17,12 @@ fp32 accumulation, the softmax in fp32 with hardware exp2, rounds the probabilit
 output to fp16 (see `attention` for the terms).  The keyword arguments `scale`, `rel_sign`, `head_shift` and
 `drop_last_key` build deliberately wrong references, used by the tests to show that their comparisons discriminate.
 
-Reader (`rope_f16`, `causal_attention`): the step `rsb_llm_attention` takes, on fused rows [T, (heads + 2 kv_heads) 128]
-of Q | K | V heads with head_dim 128.  `rope_f16` restates HF apply_rotary_pos_emb in fp16 (positions restart in every
-window); `causal_attention` is causal softmax(q k^T / sqrt(128)) v per window in fp64 with grouped-query heads (query
-head h reads KV head h // (heads / kv_heads), HF's repeat_kv) and a per-element bound of the same terms as the encoder's.
-Both run on torch tensors on any device, so that the reference of production-width cases runs where the kernel does.
+Reader (`rope_f16`, `causal_attention`): the step `rsb_llm_attention` takes, on fused rows [T, (heads + 2 kv_heads) D]
+of Q | K | V heads.  `rope_f16` restates HF apply_rotary_pos_emb in fp16 at head_dim 128 (positions restart in every
+window); `causal_attention` is causal softmax(q k^T / sqrt(D)) v per window in fp64 at any head_dim D, with grouped-query
+heads (query head h reads KV head h // (heads / kv_heads), HF's repeat_kv) and a per-element bound of the same terms as
+the encoder's for fp16 or bf16 rows.  A decode step (`rsb_llm_decode_attention`) at position p is the last row of a
+window of p + 1 positions.  Both run on torch tensors on any device, so that the reference of production-width cases runs where the kernel does.
 """
 from __future__ import annotations
 
@@ -138,11 +139,8 @@ def attention(qkv, cu_seqlens, form: str = "bert", bias=None, *, scale: float = 
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# reader: RoPE and causal grouped-query attention, head_dim 128
+# reader: RoPE (head_dim 128) and causal grouped-query attention (any head_dim, fp16 or bf16)
 # ---------------------------------------------------------------------------------------------------------------
-LLAMA_HEAD_DIM = 128
-
-
 def window_positions(cu_seqlens, T: int) -> np.ndarray:
     """int64 [T]: the position of every row inside its window (0 at every window start); rows at or past cu[-1] get
     -1."""
@@ -160,6 +158,12 @@ def _r16(x):
 def _ulp16_t(x):
     e = torch.floor(torch.log2(x.abs().clamp_min(2.0 ** -14)))
     return torch.exp2(e.clamp_min(-14) - 10)
+
+
+def _ulpb_t(x):
+    """Spacing of bf16 at |x|."""
+    e = torch.floor(torch.log2(x.abs().clamp_min(2.0 ** -126)))
+    return torch.exp2(e.clamp_min(-126) - 7)
 
 
 def rope_f16(x, pos, theta: float, *, pairing: str = "half", angles: str = "fp32", cs_shift=(0, 0)):
@@ -210,39 +214,53 @@ def rope_f16(x, pos, theta: float, *, pairing: str = "half", angles: str = "fp32
 
 
 def causal_attention(qkv, cu_seqlens, heads: int, kv_heads: int, *, kv_map: str = "grouped", mask_shift: int = 0,
-                     drop_key=None, with_bound: bool = False, budget: int = 1 << 25):
-    """ctx [cu[-1], heads 128] float64 on qkv's device (rows of empty windows stay 0), or (ctx, bound) with
-    `with_bound`, for fused rows qkv [>= cu[-1], (heads + 2 kv_heads) 128] fp16 whose Q / K heads are already rotated.
-    Per window and query head h: ctx = softmax(q k^T / sqrt(128) over the keys j <= i) v with K / V of head
-    h // (heads / kv_heads).
+                     drop_key=None, scale=None, last_row_only: bool = False, with_bound: bool = False,
+                     budget: int = 1 << 25):
+    """ctx [cu[-1], heads D] float64 on qkv's device (rows of empty windows stay 0), or (ctx, bound) with
+    `with_bound`, for fused rows qkv [>= cu[-1], (heads + 2 kv_heads) D] whose Q / K heads are already rotated; the
+    head_dim D is qkv.shape[1] / (heads + 2 kv_heads), any of the readers' 64, 80, 128 and 256.  Per window and query
+    head h: ctx = softmax(q k^T / sqrt(D) over the keys j <= i) v with K / V of head h // (heads / kv_heads).
+    last_row_only: only the last row of each window is computed (the others stay 0), which is a decode row at position
+    S - 1 attending to positions 0 .. S - 1.
 
     bound[t, c] is the largest |kernel - ctx| of a kernel that scores in fp32 (mma.sync accumulation), runs the softmax in
-    fp32 with hardware exp2, rounds the probabilities to fp16 before P.V and its output to fp16; the terms are those of
-    `attention` with head_dim 128 and S_vis = i + 1 visible keys:
-      (2^-11 + (S_vis + 32) 2^-24) E + S_vis 2^-25 vmax + 2 a (E + |ctx|) + 1/2 ulp_fp16,  E = sum_j p_j |v_j|,
-      a = 2^-20 + 2^-22 max|s| + S_vis 2^-24 + 128 2^-23 max_j |q|.|k_j| / sqrt(128).
+    fp32 with hardware exp2, rounds the probabilities to the dtype of qkv before P.V and its output to that dtype; the
+    terms are those of `attention` with S_vis = i + 1 visible keys and the dtype's unit roundoff u (fp16 2^-11, bf16
+    2^-8; any other dtype is taken as fp16):
+      (u + (S_vis + 32) 2^-24) E + S_vis tiny vmax + 2 a (E + |ctx|) + 1/2 ulp(ctx),  E = sum_j p_j |v_j|,
+      a = 2^-20 + 2^-22 max|s| + S_vis 2^-24 + D 2^-23 max_j |q|.|k_j| / sqrt(D),
+    with tiny the absolute rounding of a probability below the dtype's normal range (fp16 2^-25, bf16 2^-134).  A split-KV
+    decode kernel, which merges per-chunk (max, sum, output) in fp32, stays within the same terms: its sums are no deeper
+    than S_vis + 32 and its rescaling factors are exp2 of fp32 score differences.
 
-    Wrong forms for the tests: kv_map="interleaved" (KV head h % kv_heads), mask_shift=+1 / -1 (keys j <= i + 1 /
-    j <= i - 1 visible), drop_key=j (key j of every window removed)."""
-    D = LLAMA_HEAD_DIM
+    Wrong forms for the tests: kv_map="interleaved" (KV head h % kv_heads) or "next" (the neighbouring KV head,
+    h // (heads / kv_heads) + 1 mod kv_heads), mask_shift=+1 / -1 (keys j <= i + 1 / j <= i - 1 visible),
+    drop_key=j or a sequence of keys (removed from every window), scale=s in place of 1 / sqrt(D)."""
     dev = qkv.device
+    if qkv.shape[1] % (heads + 2 * kv_heads):
+        raise ValueError(f"qkv rows of {qkv.shape[1]} are not (heads + 2 kv_heads) head_dim")
+    D = qkv.shape[1] // (heads + 2 * kv_heads)
+    bf16 = qkv.dtype == torch.bfloat16
+    u, tiny = (2.0 ** -8, 2.0 ** -134) if bf16 else (2.0 ** -11, 2.0 ** -25)
     cu = np.asarray(cu_seqlens, dtype=np.int64)
     T = int(cu[-1])
     hid = heads * D
     out = torch.zeros((T, hid), dtype=torch.float64, device=dev)
     bnd = torch.zeros((T, hid), dtype=torch.float64, device=dev) if with_bound else None
     grp = heads // kv_heads
-    kvh = torch.arange(heads, device=dev) // grp if kv_map == "grouped" else torch.arange(heads, device=dev) % kv_heads
-    if kv_map not in ("grouped", "interleaved"):
+    hh = torch.arange(heads, device=dev)
+    kvh = {"grouped": hh // grp, "interleaved": hh % kv_heads, "next": (hh // grp + 1) % kv_heads}.get(kv_map)
+    if kvh is None:
         raise ValueError(kv_map)
-    scale = 1.0 / D ** 0.5
+    scale = 1.0 / D ** 0.5 if scale is None else float(scale)
+    dropped = None if drop_key is None else torch.as_tensor(np.atleast_1d(drop_key), device=dev)
     lens = np.diff(cu)
     for S in np.unique(lens):
         S = int(S)
         if S == 0:
             continue
         seqs = np.nonzero(lens == S)[0]
-        nwin = max(1, budget // (heads * S * max(S, D)))         # windows per step (scores and expanded K / V)
+        nwin = max(1, budget // (heads * S * max(S if not last_row_only else 1, D)))   # windows per step
         qc = S if heads * S * S <= budget else max(1, budget // (heads * S))
         for c0 in range(0, len(seqs), nwin):
             sel = seqs[c0:c0 + nwin]
@@ -253,15 +271,15 @@ def causal_attention(qkv, cu_seqlens, heads: int, kv_heads: int, *, kv_map: str 
             v = x[..., hid + kv_heads * D:].reshape(n, S, kv_heads, D).permute(0, 2, 1, 3)[:, kvh]
             q_all = x[..., :hid].reshape(n, S, heads, D).permute(0, 2, 1, 3)
             av = v.abs()
-            for q0 in range(0, S, qc):
+            for q0 in range(S - 1 if last_row_only else 0, S, qc):
                 q1 = min(S, q0 + qc)
                 q = q_all[:, :, q0:q1]
                 sc = (q @ k.transpose(-1, -2)) * scale                                       # [n, h, qc, S]
                 i = torch.arange(q0, q1, device=dev)[:, None]
                 j = torch.arange(S, device=dev)[None, :]
                 vis = j <= i + mask_shift
-                if drop_key is not None:
-                    vis = vis & (j != drop_key)
+                if dropped is not None:
+                    vis = vis & ~torch.isin(j, dropped)
                 sc = sc.masked_fill(~vis, -torch.inf)
                 m = sc.amax(-1, keepdim=True)
                 m = torch.where(torch.isfinite(m), m, torch.zeros_like(m))
@@ -277,7 +295,7 @@ def causal_attention(qkv, cu_seqlens, heads: int, kv_heads: int, *, kv_map: str 
                     qk = (q.abs() @ k.abs().transpose(-1, -2)).masked_fill(~vis, 0).amax(-1, keepdim=True)
                     smax = sc.abs().masked_fill(~vis, 0).amax(-1, keepdim=True)
                     a = 2.0 ** -20 + 2.0 ** -22 * smax + svis * 2.0 ** -24 + scale * D * 2.0 ** -23 * qk
-                    b = (2.0 ** -11 + (svis + 32) * 2.0 ** -24) * E + svis * 2.0 ** -25 * vmax + 2 * a * (E + o.abs())
-                    b = b + 0.5 * _ulp16_t(o.abs() + b)
+                    b = (u + (svis + 32) * 2.0 ** -24) * E + svis * tiny * vmax + 2 * a * (E + o.abs())
+                    b = b + 0.5 * (_ulpb_t(o.abs() + b) if bf16 else _ulp16_t(o.abs() + b))
                     bnd[rows[:, q0:q1]] = b.permute(0, 2, 1, 3).reshape(n, q1 - q0, hid)
     return (out, bnd) if with_bound else out

@@ -102,6 +102,9 @@ SIGNATURES = [
     ("rsb_llm_generate", c_int, [_H, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p,
                                  c_void_p, c_void_p, c_size_t, c_void_p]),
     ("rsb_llm_attention", c_int, [_H, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),   # diagnostic
+    ("rsb_llm_decode_attention", c_int, [_H, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int,
+                                         c_void_p, c_void_p]),                                      # diagnostic
+    ("rsb_llm_greedy", c_int, [c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),   # diagnostic
     ("rsb_llm_hidden_states", c_int, [_H, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t,
                                       c_void_p]),                                                   # diagnostic
     ("rsb_llm_layernorm", c_int, [c_int, c_float, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,

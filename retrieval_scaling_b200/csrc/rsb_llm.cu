@@ -763,6 +763,7 @@ void nll_rows_kernel(const T* __restrict__ logits, int vocab, int ld, const int*
             mx = fmaxf(mx, x[e]);
         }
         const float mn = fmaxf(m, mx);
+        if (mn == -INFINITY) continue;           // every logit so far -inf: nothing to add, and -inf - -inf is NaN
         float acc = s * expf(m - mn);
 #pragma unroll
         for (int e = 0; e < 8; ++e) acc += expf(x[e] - mn);
@@ -807,6 +808,7 @@ void greedy_rows_kernel(const T* __restrict__ logits, int vocab, int ld, const i
             if (c + e < vocab && (x[e] > bv || (x[e] == bv && c + e < bi))) { bv = x[e]; bi = c + e; }
         }
         const float mn = fmaxf(m, mx);
+        if (mn == -INFINITY) continue;           // every logit so far -inf: nothing to add, and -inf - -inf is NaN
         float acc = s * expf(m - mn);
 #pragma unroll
         for (int e = 0; e < 8; ++e) acc += expf(x[e] - mn);
@@ -1654,6 +1656,100 @@ extern "C" int rsb_llm_attention(rsb_llm_t* h, void* qkv, const int32_t* cu_seql
     if (rc != RSB_OK) return rc;
     const cudaError_t e = cudaPeekAtLastError();
     if (e != cudaSuccess) return lfail(RSB_ERR_CUDA, "attention launch failed: %s", cudaGetErrorString(e));
+    return RSB_OK;
+}
+
+// Diagnostic: one decode step of attention_step on caller-owned rows and one layer's KV cache (rsb.h).  The slots and
+// positions are read back and checked first, so every launch stays inside the caller's buffers.  The split-KV partials
+// are allocated here and filled with NaN bytes: a chunk read without having been written shows up in ctx.
+extern "C" int rsb_llm_decode_attention(rsb_llm_t* h, void* qkv, const int32_t* slot, const int32_t* pos, int n_rows,
+                                        void* k_cache, void* v_cache, int slots, int cap, void* ctx,
+                                        rsb_stream_t stream) {
+    if (!h || !qkv || !slot || !pos || !k_cache || !v_cache || !ctx) return lfail(RSB_ERR_INVALID, "null argument");
+    if (n_rows <= 0 || slots <= 0 || cap <= 0) return lfail(RSB_ERR_INVALID, "n_rows, slots and cap must be positive");
+    for (const void* p : {(const void*)qkv, (const void*)k_cache, (const void*)v_cache, (const void*)ctx})
+        if (reinterpret_cast<uintptr_t>(p) % 16)
+            return lfail(RSB_ERR_INVALID, "qkv, the caches and ctx must be 16-byte aligned");
+    if (h->family == RSB_LLM_OLMO2 && !(h->loaded.count("model.layers.0.self_attn.q_norm.weight") &&
+                                        h->loaded.count("model.layers.0.self_attn.k_norm.weight")))
+        return lfail(RSB_ERR_STATE, "layer 0's self_attn.q_norm / k_norm weights are not loaded");
+    cudaStream_t st = (cudaStream_t)stream;
+    std::vector<int32_t> hs(n_rows), hp(n_rows);
+    if (cudaMemcpyAsync(hs.data(), slot, (size_t)n_rows * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+        cudaMemcpyAsync(hp.data(), pos, (size_t)n_rows * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+        cudaStreamSynchronize(st) != cudaSuccess)
+        return lfail(RSB_ERR_CUDA, "reading back slot / pos failed");
+    std::vector<char> used(slots, 0);
+    int max_p = 0;
+    for (int i = 0; i < n_rows; ++i) {
+        if (hs[i] < 0 || hs[i] >= slots)
+            return lfail(RSB_ERR_INVALID, "slot %ld of row %ld is outside [0, slots = %ld)", (long)hs[i], (long)i, (long)slots);
+        if (used[hs[i]]) return lfail(RSB_ERR_INVALID, "two rows on slot %ld", (long)hs[i]);
+        used[hs[i]] = 1;
+        if (hp[i] < 0 || hp[i] >= cap)
+            return lfail(RSB_ERR_INVALID, "position %ld of row %ld is outside [0, cap = %ld)", (long)hp[i], (long)i, (long)cap);
+        if (hp[i] >= h->max_pos)
+            return lfail(RSB_ERR_UNSUPPORTED, "position %ld is past max_position_embeddings (%ld)", (long)hp[i],
+                         (long)h->max_pos);
+        max_p = std::max(max_p, hp[i]);
+    }
+    const int chunks = max_p / DCH + 1;
+    const size_t parts = (size_t)n_rows * h->heads * chunks;
+    float* part_o = nullptr;
+    float2* part_ml = nullptr;
+    if (cudaMallocAsync(&part_o, parts * h->head_dim * sizeof(float), st) != cudaSuccess ||
+        cudaMallocAsync(&part_ml, parts * sizeof(float2), st) != cudaSuccess) {
+        if (part_o) cudaFreeAsync(part_o, st);
+        return lfail(RSB_ERR_OOM, "allocating the split-KV partials failed");
+    }
+    int rc = RSB_OK;
+    if (cudaMemsetAsync(part_o, 0xFF, parts * h->head_dim * sizeof(float), st) != cudaSuccess ||
+        cudaMemsetAsync(part_ml, 0xFF, parts * sizeof(float2), st) != cudaSuccess)
+        rc = lfail(RSB_ERR_CUDA, "filling the split-KV partials failed");
+    if (rc == RSB_OK)
+        with_dtype(h, [&](auto tag) -> int {
+            using E = decltype(tag);
+            KvCache<E> kv;
+            kv.k = static_cast<E*>(k_cache);
+            kv.v = static_cast<E*>(v_cache);
+            kv.slots = slots;
+            kv.cap = cap;
+            kv.slot = slot;
+            kv.pos = pos;
+            kv.part_o = part_o;
+            kv.part_ml = part_ml;
+            kv.chunks = chunks;
+            attention_step<E>(h, 0, static_cast<E*>(qkv), nullptr, 0, n_rows, nullptr, 0, static_cast<E*>(ctx), &kv, st);
+            return RSB_OK;
+        });
+    cudaFreeAsync(part_o, st);
+    cudaFreeAsync(part_ml, st);
+    if (rc != RSB_OK) return rc;
+    const cudaError_t e = cudaPeekAtLastError();
+    if (e != cudaSuccess) return lfail(RSB_ERR_CUDA, "decode attention launch failed: %s", cudaGetErrorString(e));
+    return RSB_OK;
+}
+
+// Diagnostic: greedy_rows_kernel on a caller's logits (rsb.h).  next and out_tokens are both ids: with slot = nullptr,
+// base 0, step 0 and max_new 1, row i writes the same id to the same element through each.
+extern "C" int rsb_llm_greedy(int dtype, const void* logits, int vocab, int ld, int n_rows, int32_t* ids,
+                              float* logprob, rsb_stream_t stream) {
+    if (dtype != RSB_DTYPE_F16 && dtype != RSB_DTYPE_BF16)
+        return lfail(RSB_ERR_INVALID, "dtype %ld is neither RSB_DTYPE_F16 nor RSB_DTYPE_BF16", (long)dtype);
+    if (!logits || !ids || !logprob) return lfail(RSB_ERR_INVALID, "null argument");
+    if (vocab <= 0 || ld < vocab || ld % 8 || n_rows < 0)
+        return lfail(RSB_ERR_INVALID, "vocab must be positive, ld >= vocab and a multiple of 8, n_rows >= 0");
+    if (reinterpret_cast<uintptr_t>(logits) % 16) return lfail(RSB_ERR_INVALID, "logits must be 16-byte aligned");
+    if (n_rows == 0) return RSB_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (dtype == RSB_DTYPE_BF16)
+        greedy_rows_kernel<__nv_bfloat16><<<n_rows, 256, 0, st>>>(static_cast<const __nv_bfloat16*>(logits), vocab, ld,
+                                                                  nullptr, 0, 0, 1, ids, ids, logprob);
+    else
+        greedy_rows_kernel<__half><<<n_rows, 256, 0, st>>>(static_cast<const __half*>(logits), vocab, ld, nullptr, 0, 0,
+                                                           1, ids, ids, logprob);
+    const cudaError_t e = cudaPeekAtLastError();
+    if (e != cudaSuccess) return lfail(RSB_ERR_CUDA, "greedy launch failed: %s", cudaGetErrorString(e));
     return RSB_OK;
 }
 

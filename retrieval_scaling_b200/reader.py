@@ -471,6 +471,35 @@ class _Reader:
                                           ctypes.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
         self._check(rc)
 
+    def decode_attention(self, qkv: torch.Tensor, slot: torch.Tensor, pos: torch.Tensor, k_cache: torch.Tensor,
+                         v_cache: torch.Tensor, ctx: torch.Tensor):
+        """One decode step of generate's attention: row i of qkv [n, (heads + 2 kv_heads) head_dim] is rotated in place
+        at position pos[i] (int32 [n] on the device), its K and V are stored in k_cache / v_cache [slots, kv_heads, cap,
+        head_dim] at (slot[i], :, pos[i]), and ctx [n, hidden] receives its attention over positions 0 .. pos[i] of the
+        slot.  Every tensor in the reader's dtype but slot / pos."""
+        for what, t in (("qkv", qkv), ("k_cache", k_cache), ("v_cache", v_cache), ("ctx", ctx)):
+            if t.dtype != self.dtype:
+                raise ValueError(f"{what} is {t.dtype}; this reader runs in {self.dtype}")
+        g = self.geom
+        H, heads = g["hidden_size"], g["num_attention_heads"]
+        kv, d = g.get("num_key_value_heads", heads), H // heads
+        n = qkv.shape[0]
+        shapes = {"qkv": (qkv, (n, (heads + 2 * kv) * d)), "ctx": (ctx, (n, H)), "slot": (slot, (n,)), "pos": (pos, (n,)),
+                  "v_cache": (v_cache, tuple(k_cache.shape))}
+        if k_cache.dim() != 4 or tuple(k_cache.shape[1::2]) != (kv, d):
+            raise ValueError(f"k_cache is {tuple(k_cache.shape)}, not [slots, {kv}, cap, {d}]")
+        for what, (t, want) in shapes.items():
+            if tuple(t.shape) != want or not t.is_contiguous():
+                raise ValueError(f"{what} is {tuple(t.shape)}, not a contiguous {want}")
+        if slot.dtype != torch.int32 or pos.dtype != torch.int32:
+            raise ValueError("slot and pos must be int32")
+        p = lambda t: ctypes.c_void_p(t.data_ptr())   # noqa: E731
+        with torch.cuda.device(self.device):
+            rc = self.L.rsb_llm_decode_attention(self._h, p(qkv), p(slot), p(pos), qkv.shape[0], p(k_cache), p(v_cache),
+                                                 k_cache.shape[0], k_cache.shape[2], p(ctx),
+                                                 ctypes.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
+        self._check(rc)
+
     def hidden_states(self, ids: torch.Tensor, cu_seqlens: torch.Tensor, max_seqlen: int) -> torch.Tensor:
         """The residual stream after the last layer, before the final norm: [T, hidden] in the reader's dtype for the
         packed int32 ids [T] and cu_seqlens [B + 1] on the device."""

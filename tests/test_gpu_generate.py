@@ -120,18 +120,46 @@ def test_decode_against_prefill_and_oracle(name, dtype):
     assert compared >= 0.5 * steps
 
 
+# A one-layer Llama at hidden 128 whose LM head is cut into chunks of 128 rows: chunk_rows() = 256 MiB / (vocab_pad x 2
+# bytes), floored to 128 rows, is 128 at vocab_pad 2^20.  The vocabulary is not a multiple of 8.
+CHUNKED_HEAD = dict(hidden_size=128, num_attention_heads=1, num_key_value_heads=1, intermediate_size=128,
+                    num_hidden_layers=1, vocab_size=(1 << 20) - 99)
+
+
 @pytest.mark.parametrize("name, dtype", [("llama-gqa4", "fp16"), ("llama-gqa4", "bf16"), ("neox-d256", "fp16"),
-                                         ("olmo2", "bf16")])
+                                         ("olmo2", "bf16"), ("llama-chunked-head", "fp16")])
 def test_batch_invariance(name, dtype):
     """A sequence decoded alone and inside a batch of 37 mixed-length prompts gives bit-identical ids and
-    log-probabilities."""
-    m, cfg, _, _ = _reader(name, dtype)
+    log-probabilities.  llama-chunked-head: 300 prompts through an LM head of 128-row chunks, so the prefill and the
+    decode steps choose rows past the first chunk (choose()'s c0 > 0); EOS ids taken from a first run end a third of
+    the prompts at their first token and another third by their third, so the live rows drop from 300 to at most 200
+    and then to at most 100 (three chunks, two, one).  Every prompt alone gives the same ids and log-probabilities, and
+    the run with EOS ids is the run without them cut after each prompt's first EOS."""
+    if name == "llama-chunked-head":
+        m, cfg, _, _ = _reader("llama-gqa4", dtype, **CHUNKED_HEAD)
+        n, max_new, check = 300, 6, range(300)
+    else:
+        m, cfg, _, _ = _reader(name, dtype)
+        n, max_new, check = 37, 20, None
     rng = np.random.default_rng(5)
-    lens = rng.integers(1, 400, 37).tolist()
+    lens = rng.integers(1, 400, n).tolist()
     prompts = _prompts(cfg["vocab_size"], lens, 6)
-    toks, lps = m.generate(prompts, 20, [], return_logprobs=True)
-    for i in (0, 7, 19, 36, int(np.argmin(lens)), int(np.argmax(lens))):
-        t, lp = m.generate([prompts[i]], 20, [], return_logprobs=True)
+    toks, lps = m.generate(prompts, max_new, [], return_logprobs=True)
+    eos = []
+    if check is None:
+        check = (0, 7, 19, 36, int(np.argmin(lens)), int(np.argmax(lens)))
+    else:
+        eos = sorted({toks[i][0] for i in range(100)} | {toks[i][2] for i in range(100, 200)})
+        full_t, full_lp = toks, lps
+        toks, lps = m.generate(prompts, max_new, eos, return_logprobs=True)
+        for i in range(n):
+            cut = next((s + 1 for s, v in enumerate(full_t[i]) if v in eos), max_new)
+            assert toks[i] == full_t[i][:cut] and torch.equal(lps[i], full_lp[i][:cut]), i
+        live = [sum(len(t) > s for t in toks) for s in range(max_new)]   # rows of decode step s (s = 0: the prefill)
+        print(f"{name}: {len(set(v for t in full_t for v in t))} distinct ids in {n} x {max_new}; live rows per step {live}")
+        assert live[0] == n and live[1] > 128 and max(live[1:3]) <= 256 and live[3] <= 128 and live[4] > 0
+    for i in check:
+        t, lp = m.generate([prompts[i]], max_new, eos, return_logprobs=True)
         assert t[0] == toks[i] and torch.equal(lp[0], lps[i]), i
 
 

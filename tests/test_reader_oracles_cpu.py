@@ -2,7 +2,9 @@
 tests/test_gpu_reader_kernels.py compare the kernels with HF and not with a restatement of the kernels:
 
   oracle/attention_oracle.rope_f16          HF LlamaRotaryEmbedding + apply_rotary_pos_emb in fp16
-  oracle/attention_oracle.causal_attention  HF repeat_kv + eager_attention_forward in fp64, and tests/llama_oracle.py
+  oracle/attention_oracle.causal_attention  HF repeat_kv + eager_attention_forward in fp64, and tests/llama_oracle.py;
+                                            plain fp64 softmax attention at head_dim 64 / 80 / 128 / 256, fp16 and bf16
+  oracle/greedy_oracle.greedy               the lowest id on ties, pad columns ignored
   tests/llama_oracle.py                     per-layer hidden rows against transformers fp32, on an explicit device"""
 import os
 import sys
@@ -143,3 +145,69 @@ def test_oracle_hidden_rows_match_transformers_fp32(kv_heads):
     for i, g in enumerate(got):
         np.testing.assert_allclose(rows[i + 1].numpy(), g.numpy(), atol=1e-4, rtol=0)
     np.testing.assert_allclose(O.token_nll(sd, cfg, ids, device="cpu"), F.hf_token_nll(model, ids), atol=1e-4, rtol=0)
+
+
+def _plain_attention(qkv, S, heads, kv_heads, d):
+    """Causal softmax attention in fp64 written out directly: scores, mask, torch.softmax, weighted sum."""
+    x = qkv.double()
+    g = heads // kv_heads
+    q = x[:, :heads * d].reshape(S, heads, d).transpose(0, 1)
+    k = x[:, heads * d:(heads + kv_heads) * d].reshape(S, kv_heads, d).transpose(0, 1).repeat_interleave(g, 0)
+    v = x[:, (heads + kv_heads) * d:].reshape(S, kv_heads, d).transpose(0, 1).repeat_interleave(g, 0)
+    sc = (q @ k.transpose(1, 2)) / d ** 0.5
+    sc = sc.masked_fill(torch.ones(S, S, dtype=torch.bool).triu(1), -torch.inf)
+    return (torch.softmax(sc, -1) @ v).transpose(0, 1).reshape(S, heads * d)
+
+
+@pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
+@pytest.mark.parametrize("d", [64, 80, 128, 256])
+def test_causal_attention_at_every_head_dim(d, dtype):
+    """causal_attention at head_dim 64 / 80 / 128 / 256 (taken from the row width) in fp16 and bf16 rows equals plain
+    fp64 softmax attention to 1e-12; last_row_only gives the last row of every window and zeros elsewhere; the bound
+    carries the dtype's unit roundoff (bf16's is 8x fp16's on the P term); the wrong forms used by the decode tests (the
+    neighbouring KV head, a 1 / sqrt(d +- 8) scale, a run of keys dropped) differ from the reference."""
+    heads, kv = 4, 2
+    rng = np.random.default_rng(d)
+    lens = [1, 70, 0, 130]
+    cu = np.concatenate([[0], np.cumsum(lens)])
+    qkv = torch.from_numpy(rng.standard_normal((int(cu[-1]), (heads + 2 * kv) * d)) * 1.5).to(dtype)
+    ref, bnd = AO.causal_attention(qkv, cu, heads, kv, with_bound=True)
+    for b, S in enumerate(lens):
+        if S:
+            np.testing.assert_allclose(ref[cu[b]:cu[b + 1]].numpy(),
+                                       _plain_attention(qkv[cu[b]:cu[b + 1]], S, heads, kv, d).numpy(), atol=1e-12, rtol=0)
+    last, lbnd = AO.causal_attention(qkv, cu, heads, kv, last_row_only=True, with_bound=True)
+    ends = [int(cu[b + 1]) - 1 for b, S in enumerate(lens) if S]
+    assert torch.equal(last[ends], ref[ends]) and torch.equal(lbnd[ends], bnd[ends])
+    others = torch.ones(len(ref), dtype=torch.bool)
+    others[ends] = False
+    assert (last[others] == 0).all()
+    assert (bnd[ends] > 0).all()
+    other = AO.causal_attention(qkv.to(torch.bfloat16 if dtype == torch.float16 else torch.float16), cu, heads, kv,
+                                with_bound=True)[1]
+    assert ((bnd > other) == (dtype == torch.bfloat16))[ends].all()
+    for kw in (dict(kv_map="next"), dict(scale=(d + 8) ** -0.5), dict(scale=(d - 8) ** -0.5),
+               dict(drop_key=np.arange(64, 128))):
+        assert (AO.causal_attention(qkv, cu, heads, kv, **kw) - ref).abs().max() > 1e-3, kw
+
+
+def test_greedy_reference_tie_rule_and_pad():
+    """greedy_oracle.greedy: the lowest id among equal maxima (numpy's argmax), columns past the vocabulary ignored
+    whatever they hold, -inf entries weight 0, and the log-probability of equal logits -log(vocab)."""
+    from oracle import greedy_oracle as GO
+    V, ld = 1001, 1024
+    x = np.random.default_rng(0).standard_normal((6, ld)).astype(np.float32)
+    x[0, [5, 6, 900]] = 7.0                           # a three-way tie: id 5
+    x[1, [1000, 3]] = 7.0                             # the tie's lowest id comes second in memory order: 3
+    x[2, :] = 0.5                                     # all equal: id 0, -log(V)
+    x[3, V:] = np.nan                                 # pad columns never chosen nor summed
+    x[3, V - 1] = 7.0
+    x[4, V:] = np.inf
+    x[5, :V] = -np.inf                                # one finite logit
+    x[5, 17] = 2.0
+    ids, lp, bound = GO.greedy(x, V)
+    assert ids.tolist() == [5, 3, 0, V - 1, int(np.argmax(x[4, :V])), 17]
+    assert lp[2] == pytest.approx(-np.log(V), abs=1e-12) and lp[5] == 0.0
+    assert np.all(np.isfinite(lp)) and np.all(np.isfinite(bound)) and np.all(bound > 0) and np.all(bound < 1e-4)
+    want = x[3, :V].astype(np.float64)
+    assert lp[3] == pytest.approx(want[V - 1] - (want.max() + np.log(np.exp(want - want.max()).sum())), abs=1e-12)
