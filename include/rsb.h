@@ -546,6 +546,20 @@ size_t rsb_llm_generate_workspace_bytes(rsb_llm_t* h, int B, int T, int max_seql
 int rsb_llm_generate(rsb_llm_t* h, const int32_t* ids_dev, const int32_t* cu_seqlens_dev, int B, int T, int max_seqlen,
                      int max_new_tokens, const int32_t* eos_ids, int n_eos, int32_t* out_tokens_dev,
                      int32_t* out_lens_dev, float* out_logprob_dev, void* ws_dev, size_t ws_bytes, rsb_stream_t stream);
+/* Log-likelihood scoring of chosen tokens (multiple-choice evaluation): the forward of rsb_llm_nll over the same packed
+ * windows (ids_dev, cu_seqlens_dev, B, T, max_seqlen and their refusals), then for each target i < n_targets
+ * out_logprob_dev[i] = log_softmax(logits of packed row tgt_row_dev[i])[tgt_token_dev[i]] in fp32 (the logits of row t
+ * predict the token after t), bit for bit minus rsb_llm_nll's value for that (row, label), and out_greedy_dev[i] = 1
+ * when tgt_token_dev[i] is that row's argmax over [0, vocab) compared in fp32, lowest id on ties (rsb_llm_generate's
+ * choice), else 0.  Targets may repeat, share a row and come in any order; outputs are in target order.  The final
+ * norm and LM head run once per distinct row.  Before any launch and without writing an output: a row outside [0, T)
+ * or a token outside [0, vocab) RSB_ERR_INVALID, a workspace below rsb_llm_loglikelihood_workspace_bytes(h, T,
+ * n_targets) RSB_ERR_OOM. */
+size_t rsb_llm_loglikelihood_workspace_bytes(rsb_llm_t* h, int T, int n_targets);
+int rsb_llm_loglikelihood(rsb_llm_t* h, const int32_t* ids_dev, const int32_t* cu_seqlens_dev, int B, int T,
+                          int max_seqlen, const int32_t* tgt_row_dev, const int32_t* tgt_token_dev, int n_targets,
+                          float* out_logprob_dev, int32_t* out_greedy_dev, void* ws_dev, size_t ws_bytes,
+                          rsb_stream_t stream);
 /* Diagnostic, not used on the product path: one attention step of rsb_llm_nll on a caller's tensors, with the forward's
  * own work list.  qkv_dev [T, (heads + 2 kv_heads) head_dim] in the handle's dtype (fp16 or bf16) holds each token's
  * Q | K | V heads (GPT-NeoX: the permuted [Q heads | K heads | V heads] layout rsb_llm_load stores); RoPE is applied to

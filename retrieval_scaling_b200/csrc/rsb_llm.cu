@@ -23,6 +23,8 @@
 //   decode_attention_kernel  split-KV attention of one query row per sequence over its cache, all query heads of a KV
 //                            head in one mma tile; decode_combine_kernel merges the chunks
 //   greedy_rows_kernel       fp32 argmax over the real vocabulary (lowest id on ties) and its log-softmax
+// Multiple-choice scoring (rsb_llm_loglikelihood) adds:
+//   choice_rows_kernel       the same pass over each scored row, then the log-softmax and greedy flag of its targets
 #include "../../include/rsb.h"
 
 #include "rsb_internal.h"
@@ -782,19 +784,13 @@ void nll_rows_kernel(const T* __restrict__ logits, int vocab, int ld, const int*
     }
 }
 
-// Greedy choice of row i: the argmax over logits[i, 0:vocab] compared in fp32, the lowest index on ties (torch.argmax);
-// the LM head's pad columns vocab..ld-1 never compete.  Writes the id to next[i] and out_tokens[s, step], and its fp32
-// log-softmax logit - logsumexp (nll_rows_kernel's sum) to out_lp[s, step] when out_lp is given, with s = slot ? slot[i]
-// : base + i.  One block per row.
+// One block's single pass over row[0:vocab]: the fp32 logsumexp (nll_rows_kernel's sum) and the argmax compared in fp32,
+// the lowest index on ties (torch.argmax); the LM head's pad columns vocab.. never compete.  The results are valid in
+// thread 0 only.  blockDim.x <= 256.
 template <typename T>
-__global__ __launch_bounds__(256)
-void greedy_rows_kernel(const T* __restrict__ logits, int vocab, int ld, const int* __restrict__ slot, int base,
-                        int step, int max_new, int* __restrict__ next, int* __restrict__ out_tokens,
-                        float* __restrict__ out_lp) {
+__device__ __forceinline__ void row_lse_argmax(const T* __restrict__ row, int vocab, float& lse, float& best, int& arg) {
     __shared__ float rm[8], rs[8], rv[8];
     __shared__ int ri[8];
-    const int i = blockIdx.x;
-    const T* row = logits + (size_t)i * ld;
     float m = -INFINITY, s = 0.f, bv = -INFINITY;
     int bi = INT_MAX;
     for (int c = threadIdx.x * 8; c < vocab; c += blockDim.x * 8) {
@@ -832,11 +828,53 @@ void greedy_rows_kernel(const T* __restrict__ logits, int vocab, int ld, const i
             lse_merge(M, Sm, rm[w], rs[w]);
             if (better(rv[w], ri[w], V, I)) { V = rv[w]; I = ri[w]; }
         }
-        if (I >= vocab) I = 0;                   // every logit NaN: the log-probability below is NaN as well
+        if (I >= vocab) I = 0;                   // every logit NaN: the log-probability is NaN as well
+        lse = M + logf(Sm);
+        best = V;
+        arg = I;
+    }
+}
+
+// Greedy choice of row i (row_lse_argmax).  Writes the id to next[i] and out_tokens[s, step], and its fp32 log-softmax
+// logit - logsumexp to out_lp[s, step] when out_lp is given, with s = slot ? slot[i] : base + i.  One block per row.
+template <typename T>
+__global__ __launch_bounds__(256)
+void greedy_rows_kernel(const T* __restrict__ logits, int vocab, int ld, const int* __restrict__ slot, int base,
+                        int step, int max_new, int* __restrict__ next, int* __restrict__ out_tokens,
+                        float* __restrict__ out_lp) {
+    const int i = blockIdx.x;
+    float lse, V;
+    int I;
+    row_lse_argmax(logits + (size_t)i * ld, vocab, lse, V, I);
+    if (threadIdx.x == 0) {
         const size_t o = (size_t)(slot ? slot[i] : base + i) * max_new + step;
         next[i] = I;
         out_tokens[o] = I;
-        if (out_lp) out_lp[o] = V - (M + logf(Sm));
+        if (out_lp) out_lp[o] = V - lse;
+    }
+}
+
+// Scored choices of row i (row_lse_argmax): for each of its targets j in [ptr[i], ptr[i+1]), out_lp[out[j]] = fp32
+// logit[tok[j]] - logsumexp, bit for bit -nll_rows_kernel of the same (row, label), and out_greedy[out[j]] = 1 when
+// tok[j] is the row's argmax, else 0.  One block per distinct row; the targets are spread over the block.
+template <typename T>
+__global__ __launch_bounds__(256)
+void choice_rows_kernel(const T* __restrict__ logits, int vocab, int ld, const int* __restrict__ ptr,
+                        const int* __restrict__ tok, const int* __restrict__ out, float* __restrict__ out_lp,
+                        int* __restrict__ out_greedy) {
+    __shared__ float s_lse;
+    __shared__ int s_arg;
+    const int i = blockIdx.x;
+    const T* row = logits + (size_t)i * ld;
+    float lse, V;
+    int I;
+    row_lse_argmax(row, vocab, lse, V, I);
+    if (threadIdx.x == 0) { s_lse = lse; s_arg = I; }
+    __syncthreads();
+    for (int j = ptr[i] + threadIdx.x; j < ptr[i + 1]; j += blockDim.x) {
+        const int t = tok[j];
+        out_lp[out[j]] = to_f(row[t]) - s_lse;
+        out_greedy[out[j]] = t == s_arg;
     }
 }
 
@@ -1451,6 +1489,103 @@ extern "C" int rsb_llm_nll(rsb_llm_t* h, const int32_t* ids, const int32_t* cu_s
             final_norm<E>(h, X, d_rows + c0, n, Hn, st);
             if ((rc = gemm<E>(Hn, n, h->lm_head, h->vocab_pad, Hd, h->zero_bias, nullptr, LOG, 0, st)) != RSB_OK) return rc;
             nll_rows_kernel<E><<<n, 256, 0, st>>>(LOG, h->vocab, h->vocab_pad, d_labs + c0, d_outi + c0, nll_out);
+        }
+        return RSB_OK;
+    });
+    if (rc != RSB_OK) return rc;
+    const cudaError_t e = cudaPeekAtLastError();
+    if (e != cudaSuccess) return lfail(RSB_ERR_CUDA, "reader launch failed: %s", cudaGetErrorString(e));
+    return RSB_OK;
+}
+
+namespace {
+
+// rsb_llm_loglikelihood's workspace: the forward's slots for T tokens with up to min(n, T) scored rows, then the
+// target tables: distinct rows [R], CSR offsets [R + 1], and token and output index per target [n] each.
+size_t ll_layout(const rsb_llm* h, size_t T, size_t n, size_t off[10], size_t* tables) {
+    const size_t R = std::min(n, T);
+    *tables = llm_ws_layout(h, T, R, off);
+    return *tables + (2 * R + 1 + 2 * n) * sizeof(int);
+}
+
+}  // namespace
+
+extern "C" size_t rsb_llm_loglikelihood_workspace_bytes(rsb_llm_t* h, int T, int n_targets) {
+    if (!h || T <= 0 || n_targets < 0) return 0;
+    size_t off[10], tables;
+    return ll_layout(h, (size_t)T, (size_t)n_targets, off, &tables);
+}
+
+// The reader forward of rsb_llm_nll, scored at caller-chosen (row, token) pairs: out_logprob[i] = log_softmax(logits of
+// packed row tgt_row[i])[tgt_token[i]] in fp32 and out_greedy[i] = whether tgt_token[i] is that row's argmax.  The final
+// norm and LM head run once per distinct row.
+extern "C" int rsb_llm_loglikelihood(rsb_llm_t* h, const int32_t* ids, const int32_t* cu_seqlens, int B, int T,
+                                     int max_seqlen, const int32_t* tgt_row, const int32_t* tgt_token, int n_targets,
+                                     float* out_logprob, int32_t* out_greedy, void* ws, size_t ws_bytes,
+                                     rsb_stream_t stream) {
+    if (!h || !ids || !cu_seqlens || !ws || (n_targets > 0 && (!tgt_row || !tgt_token || !out_logprob || !out_greedy)))
+        return lfail(RSB_ERR_INVALID, "null argument");
+    if (n_targets < 0) return lfail(RSB_ERR_INVALID, "n_targets %ld is negative", (long)n_targets);
+    cudaStream_t st = (cudaStream_t)stream;
+    std::vector<int32_t> cu, lab;
+    int rc = check_forward(h, ids, cu_seqlens, nullptr, B, T, max_seqlen, st, cu, lab);
+    if (rc != RSB_OK) return rc;
+    const int n = n_targets;
+    std::vector<int32_t> row(n), tok(n);
+    if (n > 0 && (cudaMemcpyAsync(row.data(), tgt_row, (size_t)n * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+                  cudaMemcpyAsync(tok.data(), tgt_token, (size_t)n * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+                  cudaStreamSynchronize(st) != cudaSuccess))
+        return lfail(RSB_ERR_CUDA, "reading back the targets failed");
+    for (int i = 0; i < n; ++i) {
+        if (row[i] < 0 || row[i] >= T)
+            return lfail(RSB_ERR_INVALID, "target %ld: row %ld is outside [0, T = %ld)", (long)i, (long)row[i], (long)T);
+        if (tok[i] < 0 || tok[i] >= h->vocab)
+            return lfail(RSB_ERR_INVALID, "target %ld: token %ld is outside the vocabulary", (long)i, (long)tok[i]);
+    }
+    size_t off[10], tables;
+    const size_t need = ll_layout(h, (size_t)T, (size_t)n, off, &tables);
+    if (ws_bytes < need) return lfail(RSB_ERR_OOM, "reader workspace too small (need %ld bytes)", (long)need);
+    if (n == 0) return RSB_OK;
+    // targets sorted by row: distinct rows, and per row a CSR run of (token, output index)
+    std::vector<int32_t> order(n), rows, ptr{0}, stok(n), sout(n);
+    for (int i = 0; i < n; ++i) order[i] = i;
+    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return row[a] < row[b]; });
+    for (int j = 0; j < n; ++j) {
+        const int i = order[j];
+        if (rows.empty() || rows.back() != row[i]) {
+            if (!rows.empty()) ptr.push_back(j);
+            rows.push_back(row[i]);
+        }
+        stok[j] = tok[i];
+        sout[j] = i;
+    }
+    ptr.push_back(n);
+    const int R = (int)rows.size();
+    unsigned char* w = static_cast<unsigned char*>(ws);
+    int* d_rows = reinterpret_cast<int*>(w + tables);
+    int* d_ptr = d_rows + R;
+    int* d_tok = d_ptr + R + 1;
+    int* d_out = d_tok + n;
+    if (cudaMemcpyAsync(d_rows, rows.data(), (size_t)R * 4, cudaMemcpyHostToDevice, st) != cudaSuccess ||
+        cudaMemcpyAsync(d_ptr, ptr.data(), (size_t)(R + 1) * 4, cudaMemcpyHostToDevice, st) != cudaSuccess ||
+        cudaMemcpyAsync(d_tok, stok.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st) != cudaSuccess ||
+        cudaMemcpyAsync(d_out, sout.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st) != cudaSuccess)
+        return lfail(RSB_ERR_CUDA, "uploading the targets failed");
+    rc = with_dtype(h, [&](auto tag) -> int {
+        using E = decltype(tag);
+        int rc = trunk<E>(h, ids, cu_seqlens, B, T, cu, w, off, st);
+        if (rc != RSB_OK) return rc;
+        // final norm and LM head on the distinct rows only, in rsb_llm_nll's chunks
+        E* X = reinterpret_cast<E*>(w + off[0]);
+        E* Hn = reinterpret_cast<E*>(w + off[1]);
+        E* LOG = reinterpret_cast<E*>(w + off[6]);
+        const int Hd = h->hidden, chunk = h->chunk_rows();
+        for (int c0 = 0; c0 < R; c0 += chunk) {
+            const int m = std::min(chunk, R - c0);
+            final_norm<E>(h, X, d_rows + c0, m, Hn, st);
+            if ((rc = gemm<E>(Hn, m, h->lm_head, h->vocab_pad, Hd, h->zero_bias, nullptr, LOG, 0, st)) != RSB_OK) return rc;
+            choice_rows_kernel<E><<<m, 256, 0, st>>>(LOG, h->vocab, h->vocab_pad, d_ptr + c0, d_tok, d_out, out_logprob,
+                                                     out_greedy);
         }
         return RSB_OK;
     });

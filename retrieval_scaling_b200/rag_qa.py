@@ -231,9 +231,13 @@ def _load_jsonl(path: str) -> List[dict]:
 
 
 def evaluate_lm_eval(cfg, model=None, tokenizer=None, model_config: Optional[dict] = None) -> LmEvalOutput:
-    """`tasks.eval.inference` with task_name lm-eval: the fork's generate_until on evaluation.domain's task."""
+    """`tasks.eval.inference` with task_name lm-eval: the fork's generate_until on evaluation.domain's task, or its
+    multiple-choice log-likelihood scoring for MMLU and MedQA (`rag_mc`)."""
     if int(os.environ.get("WORLD_SIZE", "1")) > 1:
         raise NotImplementedError("lm-eval inference runs in one process (the reader is single-GPU)")
+    from . import rag_mc
+    if rag_mc.is_mc_task(cfg.evaluation.get("domain")):
+        return rag_mc.evaluate(cfg, model, tokenizer, model_config)
     settings = domain_settings(cfg.evaluation.get("domain"))
     args = _lm_eval_args(cfg)
     if not args["prompts_file"]:

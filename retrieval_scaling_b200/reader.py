@@ -10,6 +10,7 @@ and calls `lm(input_ids, labels=labels)` one window at a time (`src/evaluate_per
     nll = model.nll([ids_0, ids_1, ...], [labels_0, ...])       # per-token NLL, many windows per forward
     losses = model.loss([ids_0, ...], [labels_0, ...])          # HF's per-window mean loss
     new_ids = model.generate([prompt_0, ...], 256, eos_ids)      # greedy decoding with a KV cache (rsb_llm_generate)
+    ll = model.loglikelihood([(ctx_0, cont_0), ...], 2048)      # (log p(cont | ctx), is_greedy) (rsb_llm_loglikelihood)
 
 runs `rsb_llm_nll`: a prefill-only forward over packed, un-padded windows whose LM head runs only on the rows whose
 next token is a label.  `load_reader` picks `B200Llama`, `B200NeoX` or `B200Olmo` from the config's `model_type`.  No CPU /
@@ -23,7 +24,7 @@ import ctypes
 import json
 import math
 import os
-from typing import Dict, List, Optional, Sequence
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -356,13 +357,16 @@ class _Reader:
         self._check(rc)
         host = out.cpu()
         if not bool(torch.isfinite(host).all()):
-            if self.dtype == torch.float16:
-                raise FloatingPointError("non-finite per-token NLL: the fp16 activations overflowed (|x| > 65504); "
-                                         "this checkpoint needs a bf16 reader (load_reader(..., dtype=torch.bfloat16), "
-                                         "model.lm_dtype=bfloat16)")
-            raise FloatingPointError("non-finite per-token NLL: the bf16 activations overflowed (|x| > 3.39e38) or the "
-                                     "checkpoint's weights produce NaN")
+            raise self._overflow("per-token NLL")
         return [host[cu[i]:cu[i + 1]].clone() for i in range(len(lens))]
+
+    def _overflow(self, what: str) -> FloatingPointError:
+        if self.dtype == torch.float16:
+            return FloatingPointError(f"non-finite {what}: the fp16 activations overflowed (|x| > 65504); this "
+                                      f"checkpoint needs a bf16 reader (load_reader(..., dtype=torch.bfloat16), "
+                                      f"model.lm_dtype=bfloat16)")
+        return FloatingPointError(f"non-finite {what}: the bf16 activations overflowed (|x| > 3.39e38) or the "
+                                  f"checkpoint's weights produce NaN")
 
     def nll(self, input_ids_list, labels_list, max_tokens: Optional[int] = None) -> List[torch.Tensor]:
         """Per-token NLL of each window, fp32 [len(ids)] on the host: position t holds -log p(labels[t] | ids[:t])
@@ -386,6 +390,92 @@ class _Reader:
             out += self._nll_packed(ids[i:j], labels[i:j])
             i = j
         return out
+
+    # -- multiple-choice scoring (rsb_llm_loglikelihood) ----------------------------------------------------------
+    def _loglikelihood_packed(self, windows: Sequence[Sequence[int]], targets: Sequence[Sequence[Tuple[int, int]]]):
+        """fp32 log-probabilities and greedy flags (numpy, in target order) of the (row within its window, token)
+        targets of each window, one forward over the packed windows."""
+        lens = [len(w) for w in windows]
+        cu = [0] + np.cumsum(lens).tolist()
+        T = cu[-1]
+        rows = [cu[b] + r for b, ts in enumerate(targets) for r, _ in ts]
+        toks = [t for ts in targets for _, t in ts]
+        n = len(rows)
+        dev = self.device
+        i32 = lambda v: torch.tensor(v, dtype=torch.int32, device=dev)   # noqa: E731
+        flat_ids, cu_t, d_row, d_tok = i32([v for w in windows for v in w]), i32(cu), i32(rows), i32(toks)
+        lp = torch.empty(n, dtype=torch.float32, device=dev)
+        greedy = torch.empty(n, dtype=torch.int32, device=dev)
+        need = self.L.rsb_llm_loglikelihood_workspace_bytes(self._h, T, n)
+        if self._ws is None or self._ws.numel() < need:
+            self._ws = None
+            self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
+        p = lambda t: ctypes.c_void_p(t.data_ptr())   # noqa: E731
+        with torch.cuda.device(dev):
+            rc = self.L.rsb_llm_loglikelihood(self._h, p(flat_ids), p(cu_t), len(lens), T, max(lens), p(d_row), p(d_tok),
+                                              n, p(lp), p(greedy), p(self._ws), self._ws.numel(),
+                                              ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+        self._check(rc)
+        lp, greedy = lp.cpu().numpy(), greedy.cpu().numpy()
+        if not np.isfinite(lp).all():
+            raise self._overflow("log-likelihood")
+        return lp, greedy
+
+    def loglikelihood(self, requests, max_length: int, max_tokens: Optional[int] = None) -> List[Tuple[float, bool]]:
+        """(log p(continuation | context), is_greedy) per (context_ids, continuation_ids) request, in input order: the
+        lm-eval fork's HFLM._loglikelihood_tokens (lm_eval/models/huggingface.py:948-1162) for a causal LM.
+
+        The input window is (context + continuation)[-(max_length + 1):][:-1], and the continuation is scored on its
+        last len(continuation) rows (:1030-1046); the log-likelihood is the fp64 sum of the tokens' fp32 log-softmax
+        (:1106, :1147-1153), and is_greedy holds when every continuation token is its row's argmax (:1128, :1144).
+        Requests with identical windows share one forward, as the fork's group_by="contexts" cache shares the logits of
+        one-token continuations (:968-984), so an MMLU question costs one window for its four choices.  Windows run
+        longest first (:957-967), packed up to `max_tokens` (default `token_budget`) per forward.  An empty context or
+        continuation, or a continuation longer than max_length, raises ValueError; non-finite values raise
+        FloatingPointError."""
+        max_length = int(max_length)
+        windows: Dict[tuple, int] = {}
+        scored = []                              # per request: (window, first scored row, continuation)
+        for ctx, cont in requests:
+            ctx, cont = [int(v) for v in ctx], [int(v) for v in cont]
+            if not ctx:
+                raise ValueError("empty context: the harness scores an empty context after its prefix token (BOS, "
+                                 "else EOS)")
+            if not cont:
+                raise ValueError("empty continuation")
+            if len(cont) > max_length:
+                raise ValueError(f"a continuation of {len(cont)} tokens is longer than max_length {max_length}")
+            inp = tuple((ctx + cont)[-(max_length + 1):][:-1])
+            w = windows.setdefault(inp, len(windows))
+            scored.append((w, len(inp) - len(cont), cont))
+        wins = list(windows)
+        targets: List[List[Tuple[int, int]]] = [[] for _ in wins]
+        first: List[Tuple[int, int]] = []        # per request: (window, index of its first target in the window)
+        for w, r0, cont in scored:
+            first.append((w, len(targets[w])))
+            targets[w] += [(r0 + j, t) for j, t in enumerate(cont)]
+        order = sorted(range(len(wins)), key=lambda w: -len(wins[w]))
+        budget = self.token_budget if max_tokens is None else int(max_tokens)
+        lp: List = [None] * len(wins)
+        greedy: List = [None] * len(wins)
+        i = 0
+        while i < len(order):
+            j, tokens = i, 0
+            while j < len(order) and (j == i or tokens + len(wins[order[j]]) <= budget):
+                tokens += len(wins[order[j]])
+                j += 1
+            batch = order[i:j]
+            l_all, g_all = self._loglikelihood_packed([wins[w] for w in batch], [targets[w] for w in batch])
+            k = 0
+            for w in batch:
+                lp[w], greedy[w] = l_all[k:k + len(targets[w])], g_all[k:k + len(targets[w])]
+                k += len(targets[w])
+            i = j
+        res = []
+        for (w, t0), (_, _, cont) in zip(first, scored):
+            sl = slice(t0, t0 + len(cont))
+            res.append((float(lp[w][sl].astype(np.float64).sum()), bool(greedy[w][sl].all())))
+        return res
 
     # -- greedy generation (rsb_llm_generate) ---------------------------------------------------------------------
     # share of the free device memory one generate call's workspace (KV cache, activations, partials) may take

@@ -10,7 +10,8 @@ under {passages_dir}/bm25/{ids}/rsb_index), tasks.eval.search (query -> top-k, t
 tasks.eval.merge_search (multi-source merge, MinHash de-duplication on the GPU and subsampling, reference :31-33),
 tasks.eval.inference (task_name perplexity: reader-LM perplexity with concate_k retrieved documents prepended, the
 Llama reader on the GPU, reference :35-38; task_name lm-eval: retrieval-augmented QA with greedy generation on the GPU
-reader, the lm-eval fork's generate_until; perplexity_calibration raises NotImplementedError).
+reader, the lm-eval fork's generate_until, or for MMLU and MedQA its multiple-choice log-likelihood scoring;
+perplexity_calibration raises NotImplementedError).
 """
 import logging
 import os
